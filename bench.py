@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the KernelSHAP hot path: instances explained / second (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            our CUDA engine (N > 1: run under torchrun)
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   our CUDA engine (N > 1: run under torchrun)
   python bench.py --impl reference [...]                         the reference's CPU path on the host cores
 
 Workload (config[1] of BASELINE.json): Adult-shaped synthetic tabular data (the real pickles need the network),
@@ -12,6 +12,10 @@ A "step" explains the 2560 instances once.  ``value`` times steps with the input
 the engine's stream, L2 flushed between steps); ``e2e`` times the same step through the reference-facing plug-in
 (`KernelShap._explainer.get_explanation`, i.e. the dks_explain_host C-ABI call) from pinned HOST buffers, including
 the H2D copy of X and the D2H copy of the shap values.  One JSON line on stdout (rank 0).
+
+``--dump-outputs DIR`` writes what the last timed step computed -- the shap values [C, n, G] of this rank's instances,
+float64 -- to DIR/phi.npy, so that two builds can be compared output for output (the inputs are seeded: identical from
+run to run with the same arguments).
 """
 import argparse
 import json
@@ -36,7 +40,7 @@ if REPO not in sys.path:
 N_INSTANCES = 2560
 N_BACKGROUND = 100
 NSAMPLES = 2048
-METRIC = "instances explained/sec (bg=100, nsamples=2048) at 1/2/4/8 B200 vs ray CPU"
+METRIC = "instances explained/sec (bg=100, nsamples=2048) at 1/2/4/8 H100 vs ray CPU"
 try:                                               # BASELINE.json's metric string, verbatim
     with open(os.path.join(REPO, "BASELINE.json")) as _f:
         METRIC = json.load(_f).get("metric", METRIC)
@@ -58,7 +62,12 @@ def parse_args():
     ap.add_argument("--no-other-mode", action="store_true", help="skip the secondary leg (the other plan mode)")
     ap.add_argument("--no-other-configs", action="store_true", help="skip the bounded runs of BASELINE configs[2]-[4]")
     ap.add_argument("--cpu-sample", type=int, default=16, help="instances the CPU baseline explains")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the shap values of the last timed step to DIR/phi.npy (float64 [C, n, G])")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 def workload(rank=0):
@@ -139,6 +148,18 @@ def reference_config(cores, per_worker):
             "groups": 12, "plan": "per instance (MT19937 stream of each worker, like shap)",
             "parallelism": f"{cores} single-threaded worker processes x {per_worker} instances (the ray ActorPool of "
                            "distributed.py:125 without ray)", "kernel": "cpu-oracle"}
+
+
+def _power_limit_w(device):
+    """Enforced power limit of the GPU in watts (NVML), None where it cannot be read: part of every number measured."""
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        visible = os.environ.get("CUDA_VISIBLE_DEVICES")
+        index = int(visible.split(",")[device]) if visible and visible.split(",")[0].isdigit() else device
+        return pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(index)) / 1000.0
+    except Exception:
+        return None
 
 
 def usable_cores():
@@ -333,7 +354,7 @@ OTHER_CONFIGS = {
 }
 
 
-def measure_config(name, spec, flush, stream, steps=3, warmup=2):
+def measure_config(name, spec, flush, stream, steps, warmup=2):
     """Throughput of one of the other BASELINE.json configs at a bounded instance count on one GPU (shared plans): device
     resident (CUDA events, L2 flushed between steps), through the host API with l1_reg=False, and through the host API with
     the reference's DEFAULT kwargs (l1_reg='auto': LassoLarsIC feature selection on the device, csrc/dks_l1.cuh)."""
@@ -439,7 +460,7 @@ def run_ours(args):
     X_dev = torch.from_numpy(X).cuda()
     phi_dev = torch.empty((C, n, G), dtype=torch.float64, device="cuda")
     phi_all = torch.empty((world, C, n, G), dtype=torch.float64, device="cuda") if world > 1 else None
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")   # > 126 MB of L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")   # several times the 50 MB L2
     # N > 1: the all-gather of phi is the engine's own push over NVLink peer memory (each rank stores its block into every
     # peer's gathered buffer, then one cross-GPU barrier); NCCL all_gather_into_tensor if peer memory cannot be mapped
     gather, collective = None, "none"
@@ -447,8 +468,7 @@ def run_ours(args):
         collective = "nccl all_gather_into_tensor"
         # after the solve the engine's push kernel stores this rank's phi block into all peers' gathered buffers over NVLink peer
         # memory (128-bit coalesced stores) and the explain call ends with the engine's own flag exchange (signal + wait per
-        # peer).  Measured on an 8-GPU box (profiles/r2_bench_8gpu_d_*): 0.185 ms/step at N=8 against 0.200 with
-        # ncclAllGather and 0.210 with the stores issued from the fused kernel's epilogue (DKS_PUSH_IN_KERNEL=1).
+        # peer).  DKS_PUSH_IN_KERNEL=1 issues the stores from the fused kernel's epilogue instead.
         # DKS_BENCH_NCCL=1 forces NCCL, DKS_BENCH_SYMM_BARRIER=1 the symmetric-memory barrier instead of the flags.
         use_push = os.environ.get("DKS_BENCH_NCCL", "0") != "1"
         if use_push:
@@ -516,6 +536,9 @@ def run_ours(args):
         dist.barrier()
     clocks = sampler.stop()
     engine.check_status()
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "phi.npy"), phi_dev.cpu().numpy().astype(np.float64))
     launches = engine.kernel_launches() - launches0
     # per-kernel device time (CUDA events around the coalition stage): three extra steps with plain launches -- the replayed
     # graph of the timed region carries no timing nodes
@@ -593,7 +616,7 @@ def run_ours(args):
                      "clocks": {"sm_mhz": ck["sm_mhz"], "sm_max_mhz": ck["sm_max_mhz"], "reasons": ck["reasons"],
                                 "samples": ck["samples"]}}
 
-    # ---------------- the other plan mode (same timing rules), so that the driver's record holds both ----------------
+    # ---------------- the other plan mode (same timing rules), so that the record holds both ----------------
     other = None
     if world == 1 and not args.no_other_mode:
         other_mode = "per_instance" if args.plan_mode == "shared" else "shared"
@@ -605,7 +628,7 @@ def run_ours(args):
         other_configs = {}
         for cname, spec in OTHER_CONFIGS.items():
             try:
-                other_configs[cname] = measure_config(cname, spec, flush, stream)
+                other_configs[cname] = measure_config(cname, spec, flush, stream, args.steps)
             except Exception as exc:                                          # pragma: no cover
                 other_configs[cname] = {"error": repr(exc)[:300]}
 
@@ -620,44 +643,38 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
     alg_bytes = 4.0 * NSAMPLES * N_BACKGROUND * D * n            # SURVEY §8(d): B_alg = 4*S*N*D per instance
     k_ms = statistics.mean(kernel_ms) if kernel_ms else ms_per_step
     achieved = alg_bytes / (k_ms * 1e-3) / 1e9
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(REPO, "profiles", "roofline_traffic.json"))).get("dram_bytes_per_launch")
-    except Exception:
-        pass
     elems = float(NSAMPLES) * N_BACKGROUND * n                   # sigmoid evaluations per launch (T_alg)
-    sm_mhz = clocks.get("sm_mhz") or float(peaks.get("sm_max_mhz", 1965.0))
-    mufu_peak = 148 * 16 * sm_mhz * 1e6                          # MUFU ops/s at the observed clock (16 lanes/clk/SM, measured)
-    fused_names = "explain_shared_fused_kernel (shared-plan path: coalition sums + link + projection solve in one kernel; tcgen05 kernel on a side stream for partial varying sets)"
+    sm_mhz = clocks.get("sm_mhz") or float(peaks.get("sm_max_mhz", 1980.0))
+    props = torch.cuda.get_device_properties(local_rank)
+    n_sm = props.multi_processor_count
+    mufu_peak = n_sm * 16 * sm_mhz * 1e6                         # MUFU ops/s at the observed clock (16 lanes/clk/SM on sm_90)
+    fused_names = "explain_shared_fused_kernel (shared-plan path: coalition sums + link + projection solve in one kernel; tensor-core kernel on a side stream for partial varying sets)"
     kname, mufu_per_elem = {
         "auto": (fused_names, 0.5), "shared": (fused_names, 0.5),
-        "tcgen05": ("explain_tcgen05_kernel", 1.5), "simt": ("explain_simt_kernel", 2.0)}[engine.kernel]
+        "tcgen05": ("explain_wgmma_kernel", 1.5), "simt": ("explain_simt_kernel", 2.0)}[engine.kernel]
     if args.plan_mode == "per_instance" and engine.kernel != "simt":
-        kname, mufu_per_elem = "sample_plans_kernel + factor_plans_kernel + explain_tcgen05_kernel (per-instance plans)", 1.5
+        kname, mufu_per_elem = "sample_plans_kernel + factor_plans_kernel + explain_wgmma_kernel (per-instance plans)", 1.5
     mufu_ops = mufu_per_elem * elems / (k_ms * 1e-3)
     # The pipe that binds this stage is the MUFU (XU) pipe -- neither HBM nor the tensor pipe: `frac` is measured against
     # it.  The effective-HBM figure SURVEY §8(d) defines (bytes of the reference-shaped masked batch / kernel time) is kept
     # as a secondary field: the fused kernels never materialise that batch, so it exceeds the HBM peak by design.
     roofline = {"bound": "mufu", "achieved": mufu_ops / 1e9, "peak": mufu_peak / 1e9, "unit": "Gop/s (MUFU lane-ops)",
-                "frac": mufu_ops / mufu_peak, "traffic": traffic, "kernel": kname, "kernel_ms": k_ms,
-                "peak_source": "148 SMs x 16 MUFU lanes/clk (measured, profiles/r1_mufu_probe_b200.txt) x the SM clock sampled "
-                               "during the timed region",
+                "frac": mufu_ops / mufu_peak, "kernel": kname, "kernel_ms": k_ms,
+                "peak_source": f"{n_sm} SMs x 16 MUFU lanes/clk (sm_90 throughput table) x the SM clock sampled during the "
+                               "timed region",
                 "mufu_ops_per_elem": mufu_per_elem, "elems_per_launch": elems,
                 "effective_hbm": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                                   "peak_source": peak_src,
                                   "note": "algorithmic bytes of the masked batch (4*S*N*D per instance, SURVEY §8d) / kernel "
-                                          "time; an EFFECTIVE figure (> 1 expected): the batch is never materialised"},
-                "traffic_note": "dram__bytes_read + dram__bytes_write of the dominant kernel per launch, ncu --set full "
-                                "(profiles/roofline_traffic.json)"}
+                                          "time; an EFFECTIVE figure (> 1 expected): the batch is never materialised"}}
     if engine.kernel in ("auto", "shared") and args.plan_mode == "shared":
-        # 7 packed fp32 ops (FFMA2/FMUL2/FADD2: two lanes each, two issue cycles) per four sigmoids = 3.5 fp32 lane-ops per
-        # element against 128 lanes/clk/SM
-        fp32_peak = 148 * 128 * sm_mhz * 1e6
+        # 14 fp32 ops per four sigmoids = 3.5 fp32 lane-ops per element against 128 lanes/clk/SM
+        fp32_peak = n_sm * 128 * sm_mhz * 1e6
         roofline.update({"fp32_lane_ops_per_elem": 3.5, "fp32_pipe_frac": 3.5 * elems / (k_ms * 1e-3) / fp32_peak})
 
     line = {"metric": METRIC, "value": value, "unit": "instances/s", "n_gpus": world, "steps": args.steps,
@@ -670,7 +687,8 @@ def run_ours(args):
                     "api": "KernelShap._explainer.get_explanation -> dks_explain_host (pinned host X in, host phi out); N > 1: "
                            "DistributedExplainer under torchrun (phi stays on the device through the all-gather, one D2H)",
                     "timing": f"median of 5 blocks of {args.steps} calls, wall clock, max over ranks"},
-            "gpu_launches": int(launches), "step_ms_rank0": step_spread, "roofline": roofline}
+            "gpu_launches": int(launches), "step_ms_rank0": step_spread, "roofline": roofline,
+            "gpu": {"name": props.name, "sm_count": n_sm, "power_limit_w": _power_limit_w(local_rank)}}
     if sustained is not None:
         line["sustained"] = sustained
     if other is not None:

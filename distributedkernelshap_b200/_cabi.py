@@ -97,7 +97,7 @@ def load(build_if_needed=True):
     global _lib
     if _lib is not None:
         return _lib
-    path = os.environ.get("DKS_LIB", _build.LIB_PATH)     # DKS_LIB: tuning variants built by scripts/build_variants.sh
+    path = os.environ.get("DKS_LIB", _build.LIB_PATH)     # DKS_LIB: another build of the library (comparisons)
     if path == _build.LIB_PATH and build_if_needed and _build.is_stale() and _build.find_nvcc() is not None:
         _build.build_library()
     if not os.path.exists(path):

@@ -1,4 +1,4 @@
-"""Builds ``libdks.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_100a."""
+"""Builds ``libdks.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100)."""
 import os
 import shutil
 import subprocess
@@ -10,7 +10,7 @@ INCLUDE = os.path.join(REPO_ROOT, "include")
 LIB_PATH = os.path.join(PKG_DIR, "libdks.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
 ]

@@ -1,5 +1,5 @@
 // libdks.so -- host side of the C ABI declared in include/dks.h.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC (see build.py)
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC (see build.py)
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -235,7 +235,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     if (S_cap < 2) S_cap = 2;
     p.S_cap = S_cap;
 
-    if (ctx->dbg_i >= 0) {   // debug dump of one instance's accumulator tile (tcgen05 kernel only)
+    if (ctx->dbg_i >= 0) {   // debug dump of one instance's accumulator tile (tensor-core kernel only)
         int rows = S_cap, cols = dks::tc_npad(ctx->N);
         if (rows != ctx->dbg_rows || cols != ctx->dbg_cols) {
             TRY(dev_alloc(&ctx->dbg_T, (size_t)rows * cols));
@@ -327,7 +327,9 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             if (need > ctx->cap_acache) { TRY(dev_alloc(&ctx->d_acache, need)); ctx->cap_acache = need; ctx->epoch++; }
             sp.acache = ctx->d_acache;
         }
-        ctx->launches += dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->stream) - 1;
+        const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream);
+        if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
+        ctx->launches += nl - 1;
         dks::shared_path::WlsSharedParams wp;
         wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = ctx->C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link;
         wp.uniform_w = 1; wp.sums = ctx->d_sums; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink;
@@ -445,7 +447,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         kernel = dks::tc_supported(ctx, p) ? DKS_KERNEL_TCGEN05 : DKS_KERNEL_SIMT;
     if (kernel == DKS_KERNEL_TCGEN05) {
         if (!dks::tc_supported(ctx, p))
-            return fail(DKS_ERR_UNSUPPORTED, "tcgen05 kernel does not support this shape/head (N=%d G=%d act=%d)", ctx->N,
+            return fail(DKS_ERR_UNSUPPORTED, "tensor-core kernel does not support this shape/head (N=%d G=%d act=%d)", ctx->N,
                         ctx->G, ctx->act);
         TRY(dks::tc_launch(ctx, p, gstream));
     } else {
@@ -506,8 +508,8 @@ int dks_create(dks_ctx** out, int device) {
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10)
-        return fail(DKS_ERR_UNSUPPORTED, "dks_create: device %d is sm_%d%d; this library is built for sm_100a only", device,
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_create: device %d is sm_%d%d; this library is built for sm_90a only", device,
                     prop.major, prop.minor);
     dks_ctx* ctx = new dks_ctx();
     ctx->device = device;

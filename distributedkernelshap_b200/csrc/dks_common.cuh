@@ -1,4 +1,4 @@
-// Shared declarations of the B200 KernelSHAP engine (host context + device parameter blocks).
+// Shared declarations of the H100 KernelSHAP engine (host context + device parameter blocks).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -96,7 +96,7 @@ struct dks_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    int sm_count = 148;
+    int sm_count = 132;
     int max_smem_optin = 0;
 
     // problem definition
@@ -107,7 +107,7 @@ struct dks_ctx {
     int kernel_choice = DKS_KERNEL_AUTO;
     int nsamples_req = 0;
     bool uniform_w = true;      // background weights all equal
-    float* dbg_T = nullptr;     // debug dump of the tcgen05 score tile of instance dbg_i ([dbg_rows][dbg_cols])
+    float* dbg_T = nullptr;     // debug dump of the tensor-core score tile of instance dbg_i ([dbg_rows][dbg_cols])
     int dbg_i = -1, dbg_rows = 0, dbg_cols = 0;
     float* dbg_time = nullptr;  // [6][256] clock64 timeline of CTA 0 (debug kernel variant)
 

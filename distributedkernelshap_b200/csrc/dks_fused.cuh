@@ -1,6 +1,6 @@
 // Shared-plan fast path with the link and the projection solve FUSED into the coalition kernel.
 //
-// explain_shared_tmem_kernel (dks_shared.cuh) writes (sum p1, sum p0) per (instance, coalition) to a global buffer (42 MB
+// explain_shared_smem_kernel (dks_shared.cuh) writes (sum p1, sum p0) per (instance, coalition) to a global buffer (42 MB
 // on the Adult-shaped workload) that wls_pmat_kernel reads back.  Here the same warp that produced a row's sums finishes
 // the job: y = link(ey) - link(fnull) in place, then beta_k(i) = sum_s P[k][s] y(i, s) with P = inv(E^T W E) E^T W of the
 // shared plan (float64, the warp's 32 rows of it resident in shared memory).  The sum over s runs across the lanes of a warp
@@ -13,7 +13,8 @@
 // eliminated group, snaps |phi| < 1e-10 and writes phi for both classes (and, on a multi-GPU run, stores them into every
 // peer's gathered buffer over NVLink).  It also resets the accumulator and the counter, so the next launch needs no memset.
 //
-// NI = 1 or 2 instances share one pass over the warp's rows of tensor memory (one tcgen05.ld feeds both).
+// The warp's 32 rows of Dm (pair sums and pair products) sit in its slice of shared memory, as in
+// explain_shared_smem_kernel.  NI = 1 or 2 instances share one pass over them (one load feeds both).
 #pragma once
 
 #include "dks_shared.cuh"
@@ -83,23 +84,23 @@ __device__ __noinline__ void peer_push_finished(const double* __restrict__ phi, 
     }
 }
 
-inline size_t fused_smem_bytes(int warps, int kpad, int B) {
-    return (size_t)warps * 32 * kpad * sizeof(double) + (size_t)warps * 32 * (B + 1) * sizeof(double) +
-           DKS_LOGTAB_SIZE * sizeof(LogTabEntry);
+inline size_t fused_smem_bytes(int warps, int kpad, int B, int N) {
+    return (size_t)warps * dm_slice_bytes(N) + (size_t)warps * 32 * kpad * sizeof(double) +
+           (size_t)warps * 32 * (B + 1) * sizeof(double) + DKS_LOGTAB_SIZE * sizeof(LogTabEntry);
 }
 
-// NCT: background rows at compile time (0 = run-time p.N): with NCT the chunk loop unrolls completely (static tensor-memory
+// NCT: background rows at compile time (0 = run-time p.N): with NCT the chunk loop unrolls completely (static shared-memory
 // offsets, no loop control, the tail folded).  B (instances parked per warp) is a power of two.
 template <int NCT, int KPAD, int NWARPS, int NI>
-__global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(FusedParams p, int warps_used, int cstride) {
+__global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(FusedParams p, int warps_used) {
     extern __shared__ __align__(16) unsigned char fsm[];
-    __shared__ uint32_t s_tmem;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int B = p.B, ystride = B + 1;
-    double* sP = reinterpret_cast<double*>(fsm);                                 // [warps_used][32][KPAD]
+    const int nq = dm_quads(NCT ? NCT : p.N);
+    float4* sDm = reinterpret_cast<float4*>(fsm);                                // [warps_used][nq][32]
+    double* sP = reinterpret_cast<double*>(sDm + (size_t)warps_used * nq * 32);  // [warps_used][32][KPAD]
     double* sY = sP + (size_t)warps_used * 32 * KPAD;                            // [warps_used][32][B + 1]
     LogTabEntry* s_logtab = reinterpret_cast<LogTabEntry*>(sY + (size_t)warps_used * 32 * ystride);
-    if (warp == 0) tc::tmem_alloc(&s_tmem, 512);
     if (threadIdx.x >= 64 && threadIdx.x < 64 + DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x - 64);
 
     const int n_rg = p.S_pad / 32;                       // row groups
@@ -114,10 +115,7 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
         const double* src = p.pmat64 + (size_t)rg * 32 * KPAD;     // the warp's 32 rows are contiguous
         for (int idx = lane; idx < 32 * KPAD; idx += 32) sPw[idx] = src[idx];
     }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tbase = s_tmem;
 
     if (active) {
         constexpr int MAXCH = MAXN / 16;
@@ -127,9 +125,9 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
         const int nfull = N / 16, ntail = N - nfull * 16;
         const int nq_t = ntail >> 2, rem_t = ntail & 3;
         const int nch = nfull + (ntail > 0 ? 1 : 0);
-        const uint32_t taddr = tbase + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((warp >> 2) * cstride);
+        float4* sl = sDm + (size_t)warp * nq * 32;          // this warp's slice
         const double es = p.dme[s];
-        // ---- this warp's 32 rows of Dm into tensor memory: pair sums and pair products per quad of columns (0,2) (1,3)
+        // ---- this warp's 32 rows of Dm into its slice: pair sums and pair products per quad of columns (0,2) (1,3)
 #pragma unroll
         for (int c = 0; c < MAXCH; ++c) {
             if (c < nch) {
@@ -147,18 +145,9 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                         v[jj] = d0 + d2; v[jj + 1] = d1 + d3; v[jj + 2] = d0 * d2; v[jj + 3] = d1 * d3;
                     }
                 }
-                if (c < nfull) {
-                    tmem_st16(taddr + c * 16, v);
-                } else {
-                    // four columns at a time: the slice stride is N rounded up to 4 (a wider store would run into the next slice)
-                    if (ntail > 0) tmem_st4(taddr + c * 16 + 0, v[0], v[1], v[2], v[3]);
-                    if (ntail > 4) tmem_st4(taddr + c * 16 + 4, v[4], v[5], v[6], v[7]);
-                    if (ntail > 8) tmem_st4(taddr + c * 16 + 8, v[8], v[9], v[10], v[11]);
-                    if (ntail > 12) tmem_st4(taddr + c * 16 + 12, v[12], v[13], v[14], v[15]);
-                }
+                dm_st16(sl, c, nq, lane, v);
             }
         }
-        tmem_st_wait();
 
         const uint64_t zz = s < p.S ? p.z[s] : 0ull;
         const int ntab = (G + 3) / 4;                     // <= 4 (the host sends wider problems down the unfused path)
@@ -230,7 +219,7 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
         const double* xb2 = p.XT + (ntab > 2 ? 32 + (int)((zz >> 8) & 15ull) : 0);
         const double* xb3 = p.XT + (ntab > 3 ? 48 + (int)((zz >> 12) & 15ull) : 0);
         const int last_it = my_n > 0 ? my_n - 1 : 0;
-        // NI instances share one pass over the warp's rows of tensor memory: instance ordinals it .. it + NI - 1
+        // NI instances share one pass over the warp's rows of Dm: instance ordinals it .. it + NI - 1
         int i_nx[NI];
         double nx[NI][4];
 #pragma unroll
@@ -287,12 +276,11 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                     t1s[u] = t0s[u] = 0.f;
                 }
                 float v[2][16];
-                tc::tmem_ld16(taddr, v[0]);
+                dm_ld16(sl, 0, nq, lane, v[0]);
 #pragma unroll
                 for (int c = 0; c < MAXCH; ++c) {
                     if (c < nch) {
-                        tc::tmem_ld_wait(v[c & 1]);
-                        if (c + 1 < nch) tc::tmem_ld16(taddr + (c + 1) * 16, v[(c + 1) & 1]);
+                        if (c + 1 < nch) dm_ld16(sl, c + 1, nq, lane, v[(c + 1) & 1]);
 #pragma unroll
                         for (int u = 0; u < NI; ++u) {
                             if (c < nfull) chunk_sums<16>(v[c & 1], A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
@@ -330,9 +318,6 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
             }
         }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, 512);
 }
 
 // P in float64, one row of KPAD coefficients per coalition: pmat64[s][k] = w_s sum_l inv(A)[k][l] (z_sl - z_sL)
@@ -370,59 +355,66 @@ __global__ void plan_dvec64_kernel(const uint64_t* __restrict__ z, const double*
 
 inline int fused_kpad(int G) { return G - 1 <= 12 ? 12 : 16; }
 
-struct FusedConfig { int ni, warps, B, slices; size_t smem; };
+struct FusedConfig { int ni, warps, B; size_t smem; };
 
 // picks (warps per CTA, batch) for a shape; returns false when the fused kernel does not apply.
 // want_warps / want_B: 0 = default (tuning knobs, dks_set_option)
 inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, int want_ni, int want_warps, int want_B,
                          FusedConfig* cfg) {
     if (G < 2 || G > 16 || N > MAXN) return false;                        // at most four nibble tables, 15 coefficients
-    const int cstride = (N + 3) / 4 * 4, reach = (N + 15) / 16 * 16;
-    int slices = 5;
-    while (slices > 1 && (slices - 1) * cstride + reach > 512) --slices;
-    int warps = 4 * slices;
-    if (want_warps == 16 && warps > 16) warps = 16;
     const int kpad = fused_kpad(G);
-    int B = 16;                                    // measured best on B200 (a smaller staging tile leaves more L1 to the table loads)
+    // warps per CTA: as many as the shared memory holds (each brings its slice of Dm, its rows of P and its staging
+    // tile), at most 20.  B = 16 unless B = 8 buys more warps.
+    auto max_warps = [&](int b) {
+        int w = 20;
+        while (w > 0 && fused_smem_bytes(w, kpad, b, N) + 1024 > (size_t)max_smem) --w;
+        return w;
+    };
+    int B = 16;
     if (want_B == 32 || want_B == 8) B = want_B;
-    while (B > 8 && fused_smem_bytes(warps, kpad, B) + 1024 > (size_t)max_smem) B >>= 1;
-    if (fused_smem_bytes(warps, kpad, B) + 1024 > (size_t)max_smem) return false;
+    int warps = max_warps(B);
+    if (want_B == 0 && max_warps(8) > warps) { B = 8; warps = max_warps(8); }
+    if (want_warps > 0 && want_warps < warps) warps = want_warps;
+    if (warps < 1) return false;
     if ((long long)sm_count * warps < S_pad / 32) return false;          // every row group needs a warp
-    cfg->ni = (want_ni == 2 && fused_kpad(G) == 12) ? 2 : 1;          // two instances per tensor-memory pass (tuning knob)
-    cfg->warps = warps; cfg->B = B; cfg->slices = warps / 4;
-    cfg->smem = fused_smem_bytes(warps, kpad, B);
+    cfg->ni = (want_ni == 2 && fused_kpad(G) == 12) ? 2 : 1;          // two instances per pass over Dm (tuning knob)
+    cfg->warps = warps; cfg->B = B;
+    cfg->smem = fused_smem_bytes(warps, kpad, B, N);
     return true;
 }
 
 inline cudaError_t launch_explain_fused(const FusedParams& p, const FusedConfig& cfg, int grid, cudaStream_t stream) {
     const int kpad = fused_kpad(p.G);
-    const int cstride = (p.N + 3) / 4 * 4;
     cudaError_t err = cudaSuccess;
 #define DKS_FUSED_LAUNCH(NCT, KP, NW, NI)                                                                             \
     do {                                                                                                              \
         err = cudaFuncSetAttribute(explain_shared_fused_kernel<NCT, KP, NW, NI>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                    (int)cfg.smem);                                                                    \
         if (err == cudaSuccess)                                                                                       \
-            explain_shared_fused_kernel<NCT, KP, NW, NI><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.warps, cstride); \
+            explain_shared_fused_kernel<NCT, KP, NW, NI><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.warps);          \
     } while (0)
     // background sizes with a compile-time specialisation (the chunk loop unrolls completely); everything else takes the
-    // run-time version
-    const int nw = cfg.warps > 16 ? 20 : 16;
+    // run-time version.  Block size: the smallest of 12 / 16 / 20 warps that holds cfg.warps.
+    const int nw = cfg.warps > 16 ? 20 : (cfg.warps > 12 ? 16 : 12);
+#define DKS_FUSED_NW(NCT, KP, NI)                                                                                     \
+    do {                                                                                                              \
+        if (nw == 12) DKS_FUSED_LAUNCH(NCT, KP, 12, NI);                                                              \
+        else if (nw == 16) DKS_FUSED_LAUNCH(NCT, KP, 16, NI);                                                         \
+        else DKS_FUSED_LAUNCH(NCT, KP, 20, NI);                                                                       \
+    } while (0)
     if (kpad == 12 && cfg.ni == 2) {
-        if (p.N == 100 && nw == 20) DKS_FUSED_LAUNCH(100, 12, 20, 2);
-        else if (nw == 20) DKS_FUSED_LAUNCH(0, 12, 20, 2);
-        else DKS_FUSED_LAUNCH(0, 12, 16, 2);
+        if (p.N == 100) DKS_FUSED_NW(100, 12, 2);
+        else DKS_FUSED_NW(0, 12, 2);
     } else if (kpad == 12) {
-        if (p.N == 100 && nw == 20) DKS_FUSED_LAUNCH(100, 12, 20, 1);
-        else if (p.N == 128 && nw == 16) DKS_FUSED_LAUNCH(128, 12, 16, 1);
-        else if (p.N == 64 && nw == 20) DKS_FUSED_LAUNCH(64, 12, 20, 1);
-        else if (nw == 20) DKS_FUSED_LAUNCH(0, 12, 20, 1);
-        else DKS_FUSED_LAUNCH(0, 12, 16, 1);
+        if (p.N == 100) DKS_FUSED_NW(100, 12, 1);
+        else if (p.N == 128) DKS_FUSED_NW(128, 12, 1);
+        else if (p.N == 64) DKS_FUSED_NW(64, 12, 1);
+        else DKS_FUSED_NW(0, 12, 1);
     } else {
-        if (p.N == 100 && nw == 20) DKS_FUSED_LAUNCH(100, 16, 20, 1);
-        else if (nw == 20) DKS_FUSED_LAUNCH(0, 16, 20, 1);
-        else DKS_FUSED_LAUNCH(0, 16, 16, 1);
+        if (p.N == 100) DKS_FUSED_NW(100, 16, 1);
+        else DKS_FUSED_NW(0, 16, 1);
     }
+#undef DKS_FUSED_NW
 #undef DKS_FUSED_LAUNCH
     return err;
 }

@@ -1,4 +1,4 @@
-// Device code of the B200 KernelSHAP engine: fit kernels (K0), per-instance preparation, and the fused
+// Device code of the H100 KernelSHAP engine: fit kernels (K0), per-instance preparation, and the fused
 // coalition kernel (mask/impute + predict + background reduction + link + constrained WLS).
 //
 // Algebra used throughout (DESIGN.md §3): the model head sees linear scores, so a masked row's score is
@@ -176,14 +176,15 @@ __global__ void predict_kernel(const double* __restrict__ X, const double* __res
     for (int c = 0; c < C; ++c) out[(size_t)i * C + c] = o[c];
 }
 
-// Packed fp32 (sm_100 FFMA2/FMUL2/FADD2: two fp32 lanes per thread in one 64-bit register pair, one issue slot).
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) { f32x2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void f2_unpack(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { f32x2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+// Two fp32 lanes handled together.  Hopper has no packed fp32 instructions, so each lane is one scalar
+// round-to-nearest op (explicit intrinsics: no contraction, the same rounding per lane as a packed op).
+struct f32x2 { float lo, hi; };
+__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) { return f32x2{lo, hi}; }
+__device__ __forceinline__ void f2_unpack(f32x2 v, float& lo, float& hi) { lo = v.lo; hi = v.hi; }
+__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
 __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r;
+    return f32x2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)};
 }
 
 

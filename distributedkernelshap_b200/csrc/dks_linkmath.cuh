@@ -4,9 +4,8 @@
 
 namespace dks {
 
-// ---- cheap link arithmetic.  Measured on B200 (scripts/probes/fp64_probe.cu): DFMA/DADD 64 lanes/clk/SM, but
-// f32<->f64 conversions only ~16 (they share the XU pipe with MUFU) and a float64 division + log() is a ~110-instruction
-// dependent chain.  So the per-row log is evaluated in fp32 around a 64-entry table with two float64 ops at the end.
+// ---- cheap link arithmetic.  f32<->f64 conversions run at 16 lanes/clk/SM (they share the XU pipe with MUFU) and a
+// float64 division + log() is a ~110-instruction dependent chain.  So the per-row log is evaluated in fp32 around a 64-entry table with two float64 ops at the end.
 //
 // ln(a1) - ln(a0) for positive float32 sums.  a = 2^e * m, m in [1,2) = c_k (1 + r) with c_k = 1 + (k + 1/2)/64 the centre
 // of the k-th of 64 mantissa intervals, |r| <= 2^-7.  r = m/c_k - 1 is formed with a two-float reciprocal

@@ -6,20 +6,19 @@
 // so  2^t = A(i, s) * Dm(s, j)  with Dm = 2^d independent of the instance.  Dm (S x N floats, 0.8 MB for Adult) is
 // computed once per plan, row-normalised; a warp owns 32 coalition rows and streams the instances through them.  Two
 // elements share a reciprocal,  p1a + p1b = (2 + sm) / (1 + sm + q),  sm = A (Dma + Dmb),  q = A^2 (Dma Dmb),  so what the
-// kernel keeps per row are the pair sums and pair products of Dm -- in TENSOR MEMORY (explain_shared_tmem_kernel, the
+// kernel keeps per row are the pair sums and pair products of Dm -- in SHARED MEMORY (explain_shared_smem_kernel, the
 // default) or, in the first version kept for comparisons, the raw row in registers (explain_shared_kernel,
-// DKS_SHARED_DM=regs).  No GEMM, no EX2 per element: 3.5 packed-fp32 lane-ops + 0.5 MUFU.  Output: (sum p1, sum p0) per
+// DKS_SHARED_DM=regs).  No GEMM, no EX2 per element: 3.5 fp32 ops + 0.5 MUFU.  Output: (sum p1, sum p0) per
 // (instance, coalition); wls_pmat_kernel / wls_shared_kernel apply the link and solve with what the plan precomputed.
 // Instances with a partial varying set, per-instance plans and other heads go through the general kernels.
 #pragma once
 
 #include "dks_kernels.cuh"
-#include "dks_tc.cuh"
 
 namespace dks {
 namespace shared_path {
 
-constexpr int MAXN = 128;            // background rows per launch (a warp's slice of tensor memory / a lane's registers)
+constexpr int MAXN = 128;            // background rows per launch (a warp's slice of shared memory / a lane's registers)
 constexpr int WARPS_PER_CTA = 12;
 constexpr float U_CLAMP = 1.152921504606846976e18f;   // 2^60: (1 + ua)(1 + ub) stays finite in fp32
 
@@ -158,7 +157,7 @@ __device__ __forceinline__ void row_sums_packed(const float (&dm)[MAXN], float A
 }
 
 // one warp = 32 coalition rows (one per lane) x a strided subset of the instances
-// W = 64-bit words per coalition row (1: up to 64 groups, 2: up to 128; the tensor-memory version below also 16: up to 1024)
+// W = 64-bit words per coalition row (1: up to 64 groups, 2: up to 128; the shared-memory version below also 16: up to 1024)
 template <int NTAIL, int W>
 __global__ void __launch_bounds__(32 * WARPS_PER_CTA, 1) explain_shared_kernel(SharedParams p) {
     const int lane = threadIdx.x & 31;
@@ -225,34 +224,32 @@ __global__ void __launch_bounds__(32 * WARPS_PER_CTA, 1) explain_shared_kernel(S
     }
 }
 
-// ---- the same kernel with the Dm rows parked in TENSOR MEMORY ------------------------------------------------------
+// ---- the same kernel with the Dm rows parked in SHARED MEMORY ------------------------------------------------------
 // The register version above keeps a lane's row of Dm (up to 128 floats) in registers: 168 registers per thread, 12
-// warps per SM, and the kernel is latency bound.  TMEM (512 columns x 128 lanes x 32 bit per SM) is otherwise idle on this
-// path, so it holds the rows instead: warp w owns TMEM lanes 32*(w%4) .. +31 (the hardware's lane quarter of that warp)
-// and the column range (w/4)*cstride .. +N; it writes its 32 rows once (tcgen05.st) and re-reads them 16 columns at a time
-// (tcgen05.ld, next chunk in flight while the current one is consumed).  That frees ~100 registers per thread: 16 or 20
-// warps per SM instead of 12.
+// warps per SM, and the kernel is latency bound.  Here every warp parks its 32 rows in its own slice of shared memory
+// instead, one float4 per (quad of columns, lane): a lane reads back only what it wrote itself (no barrier), and the
+// 128-bit loads of one quad by a warp cover 512 consecutive bytes (no bank conflicts).  That frees ~100 registers per
+// thread; the number of warps per CTA follows from the shared memory a slice takes.
 constexpr int TM_MAX_WARPS = 20;
+__host__ __device__ inline int dm_quads(int N) { return (N + 3) / 4; }
+__host__ __device__ inline size_t dm_slice_bytes(int N) { return (size_t)dm_quads(N) * 32 * sizeof(float4); }
 
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-          "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])),
-          "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])),
-          "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])),
-          "r"(__float_as_uint(v[15]))
-        : "memory");
+// columns 16c .. 16c + 15 of this lane's row: quads 4c .. 4c + 3 of the slice, those below nq
+__device__ __forceinline__ void dm_st16(float4* sl, int c, int nq, int lane, const float (&v)[16]) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        if (4 * c + k < nq) sl[(4 * c + k) * 32 + lane] = make_float4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
 }
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, float v0, float v1, float v2, float v3) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(__float_as_uint(v0)),
-                 "r"(__float_as_uint(v1)), "r"(__float_as_uint(v2)), "r"(__float_as_uint(v3))
-                 : "memory");
+__device__ __forceinline__ void dm_ld16(const float4* sl, int c, int nq, int lane, float (&v)[16]) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float4 t = 4 * c + k < nq ? sl[(4 * c + k) * 32 + lane] : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[4 * k] = t.x; v[4 * k + 1] = t.y; v[4 * k + 2] = t.z; v[4 * k + 3] = t.w;
+    }
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// The same four sigmoids from what tensor memory holds for a quad of columns (0,2) (1,3): ds = (dm0 + dm2, dm1 + dm3) and
-// dq = (dm0 dm2, dm1 dm3), both independent of the instance:  sm = A ds,  q = A^2 dq.  7 packed ops + 2 MUFU per four
+// The same four sigmoids from what the slice holds for a quad of columns (0,2) (1,3): ds = (dm0 + dm2, dm1 + dm3) and
+// dq = (dm0 dm2, dm1 dm3), both independent of the instance:  sm = A ds,  q = A^2 dq.  14 fp32 ops + 2 MUFU per four
 // elements (A2 = (A, A), AA2 = (A^2, A^2), AA2x2 = 2 AA2).
 __device__ __forceinline__ void quad_acc_sq(f32x2 A2, f32x2 AA2, f32x2 AA2x2, f32x2 ds, f32x2 dq, f32x2 one2, f32x2 two2,
                                             f32x2& a1, f32x2& a0) {
@@ -283,14 +280,9 @@ __device__ __forceinline__ void chunk_sums(const float (&v)[16], float A, f32x2 
 }
 
 template <int NTAIL, int W>
-__global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_tmem_kernel(SharedParams p, int warps_used, int cstride) {
-    __shared__ uint32_t s_tmem;
+__global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_smem_kernel(SharedParams p, int warps_used) {
+    extern __shared__ float4 s_dm[];                      // [warps_used][dm_quads(N)][32]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (warp == 0) tc::tmem_alloc(&s_tmem, 512);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tbase = s_tmem;
 
     const int n_rg = p.S_pad / 32;                       // row groups
     const int total_warps = gridDim.x * warps_used;
@@ -303,8 +295,8 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_tmem_kern
         const int cnt = *p.count;
         const int N = p.N, G = p.G;
         const int nfull = N / 16;
-        // this warp's slice of tensor memory: its lane quarter, column range warp / 4
-        const uint32_t taddr = tbase + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)((warp >> 2) * cstride);
+        const int nq = dm_quads(N);
+        float4* sl = s_dm + (size_t)warp * nq * 32;      // this warp's slice
         const double es = p.dme[s];                      // exponent the row of Dm was normalised by (entries <= sqrt 2)
         for (int c = 0; c * 16 < N; ++c) {
             float v[16];
@@ -322,16 +314,8 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_tmem_kern
                     v[jj] = d0 + d2; v[jj + 1] = d1 + d3; v[jj + 2] = d0 * d2; v[jj + 3] = d1 * d3;
                 }
             }
-            if (c < nfull) {
-                tmem_st16(taddr + c * 16, v);
-            } else {
-                // the tail is written four columns at a time: the slice stride is N rounded up to 4, and a wider store
-                // would run into the next warp's slice
-#pragma unroll
-                for (int q = 0; q < (NTAIL + 3) / 4; ++q) tmem_st4(taddr + c * 16 + 4 * q, v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            }
+            dm_st16(sl, c, nq, lane, v);
         }
-        tmem_st_wait();
         // rows of one or two words stay in registers; sixteen-word rows (more than 128 groups) are re-read per instance
         constexpr int WR = W <= 2 ? W : 1;
         uint64_t zz[WR];
@@ -447,15 +431,13 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_tmem_kern
             // chunks of 16 columns, the next one in flight while this one is consumed
             float va[16], vb[16];
             const int nch = nfull + (NTAIL > 0 ? 1 : 0);
-            tc::tmem_ld16(taddr, va);
+            dm_ld16(sl, 0, nq, lane, va);
             for (int c = 0; c < nch; c += 2) {
-                tc::tmem_ld_wait(va);
-                if (c + 1 < nch) tc::tmem_ld16(taddr + (c + 1) * 16, vb);
+                if (c + 1 < nch) dm_ld16(sl, c + 1, nq, lane, vb);
                 if (c < nfull) chunk_sums<16>(va, A, A2, AA2, AA2x2, one2, two2, acc1, acc0, t1s, t0s);
                 else if (NTAIL > 0) chunk_sums<NTAIL>(va, A, A2, AA2, AA2x2, one2, two2, acc1, acc0, t1s, t0s);
                 if (c + 1 < nch) {
-                    tc::tmem_ld_wait(vb);
-                    if (c + 2 < nch) tc::tmem_ld16(taddr + (c + 2) * 16, va);
+                    if (c + 2 < nch) dm_ld16(sl, c + 2, nq, lane, va);
                     if (c + 1 < nfull) chunk_sums<16>(vb, A, A2, AA2, AA2x2, one2, two2, acc1, acc0, t1s, t0s);
                     else if (NTAIL > 0) chunk_sums<NTAIL>(vb, A, A2, AA2, AA2x2, one2, two2, acc1, acc0, t1s, t0s);
                 }
@@ -471,13 +453,10 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_tmem_kern
             }
         }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tbase, 512);
 }
 
-// 0: registers, 1: tensor memory (default); DKS_SHARED_DM=regs selects the register version for comparisons
-inline bool shared_dm_in_tmem() {
+// 0: registers, 1: shared memory (default); DKS_SHARED_DM=regs selects the register version for comparisons
+inline bool shared_dm_in_smem() {
     static int mode = -1;
     if (mode < 0) {
         const char* e = getenv("DKS_SHARED_DM");
@@ -486,28 +465,29 @@ inline bool shared_dm_in_tmem() {
     return mode == 1;
 }
 
-inline void launch_explain_shared_chunk(const SharedParams& p, int words, int grid, cudaStream_t stream) {
-    if (shared_dm_in_tmem() || words > 2) {                  // sixteen-word rows exist for the tensor-memory kernel only
-        // column stride of a warp's slice: N rounded up to 4.  Reads are whole 16-column chunks (the last one may look into
-        // the next slice, which is harmless), so the last slice must leave room for a full chunk: 5 slices up to N = 100,
-        // 4 up to N = 128
-        const int cstride = (p.N + 3) / 4 * 4;
-        const int reach = (p.N + 15) / 16 * 16;              // columns a slice's reads can touch
-        int slices = 5;
-        while (slices > 1 && (slices - 1) * cstride + reach > 512) --slices;
-        const int warps_used = 4 * slices;
+inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words, int grid, int max_smem, cudaStream_t stream) {
+    if (shared_dm_in_smem() || words > 2) {                  // sixteen-word rows exist for the shared-memory kernel only
+        const size_t slice = dm_slice_bytes(p.N);
+        int warps_used = (int)(((size_t)max_smem - 1024) / slice);
+        if (warps_used > TM_MAX_WARPS) warps_used = TM_MAX_WARPS;
+        const size_t smem = (size_t)warps_used * slice;
+        cudaError_t err = cudaSuccess;
         switch (p.N % 16) {
+#define DKS_CASE_W(T, W)                                                                                                  \
+    err = cudaFuncSetAttribute(explain_shared_smem_kernel<T, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+    if (err == cudaSuccess) explain_shared_smem_kernel<T, W><<<grid, 32 * TM_MAX_WARPS, smem, stream>>>(p, warps_used);
 #define DKS_CASE(T)                                                                                          \
     case T:                                                                                                  \
-        if (words == 1) explain_shared_tmem_kernel<T, 1><<<grid, 32 * TM_MAX_WARPS, 0, stream>>>(p, warps_used, cstride); \
-        else if (words == 2) explain_shared_tmem_kernel<T, 2><<<grid, 32 * TM_MAX_WARPS, 0, stream>>>(p, warps_used, cstride); \
-        else explain_shared_tmem_kernel<T, 16><<<grid, 32 * TM_MAX_WARPS, 0, stream>>>(p, warps_used, cstride);           \
+        if (words == 1) { DKS_CASE_W(T, 1) }                                                                 \
+        else if (words == 2) { DKS_CASE_W(T, 2) }                                                            \
+        else { DKS_CASE_W(T, 16) }                                                                           \
         break;
             DKS_CASE(0) DKS_CASE(1) DKS_CASE(2) DKS_CASE(3) DKS_CASE(4) DKS_CASE(5) DKS_CASE(6) DKS_CASE(7)
             DKS_CASE(8) DKS_CASE(9) DKS_CASE(10) DKS_CASE(11) DKS_CASE(12) DKS_CASE(13) DKS_CASE(14) DKS_CASE(15)
 #undef DKS_CASE
+#undef DKS_CASE_W
         }
-        return;
+        return err;
     }
 
     const int threads = 32 * WARPS_PER_CTA;
@@ -521,10 +501,12 @@ inline void launch_explain_shared_chunk(const SharedParams& p, int words, int gr
         DKS_CASE(8) DKS_CASE(9) DKS_CASE(10) DKS_CASE(11) DKS_CASE(12) DKS_CASE(13) DKS_CASE(14) DKS_CASE(15)
 #undef DKS_CASE
     }
+    return cudaSuccess;
 }
 
-// Backgrounds larger than MAXN rows go through in chunks of MAXN columns of Dm (one launch each, sums accumulated)
-inline int launch_explain_shared(SharedParams p, int words, int grid, cudaStream_t stream) {
+// Backgrounds larger than MAXN rows go through in chunks of MAXN columns of Dm (one launch each, sums accumulated).
+// Returns the number of launches (0 when one of them could not be configured).
+inline int launch_explain_shared(SharedParams p, int words, int grid, int max_smem, cudaStream_t stream) {
     const int N = p.N;
     const float* dm = p.DmT;
     int launches = 0;
@@ -534,7 +516,7 @@ inline int launch_explain_shared(SharedParams p, int words, int grid, cudaStream
         p.DmT = dm + (size_t)j0 * p.S_pad;
         p.accumulate = j0 > 0;
         p.acache_mode = use_cache ? (j0 == 0 ? 1 : 2) : 0;
-        launch_explain_shared_chunk(p, words, grid, stream);
+        if (launch_explain_shared_chunk(p, words, grid, max_smem, stream) != cudaSuccess) return 0;
     }
     return launches;
 }
@@ -685,8 +667,8 @@ __global__ void __launch_bounds__(THREADS) wls_pmat_kernel(WlsPmatParams p) {
 inline bool launch_wls_pmat(const WlsPmatParams& p, int n, int sm_count, int max_smem, cudaStream_t stream, cudaError_t* err) {
     const int kpad = wls_pmat_kpad(p.G);
     const size_t sm_d = wls_pmat_smem(p.G, p.S_pad, true), sm_f = wls_pmat_smem(p.G, p.S_pad, false);
-    // measured on B200 (Adult shape): float32 table, 2 CTAs of 256 threads per SM: 57 us; float64 table, 1 CTA of 512
-    // threads: 90 us.  DKS_PMAT=double selects the float64 variant for comparisons.
+    // float32 table, 2 CTAs of 256 threads per SM by default; DKS_PMAT=double selects the float64 variant (1 CTA of 512
+    // threads) for comparisons.
     static int want_double = -1;
     if (want_double < 0) { const char* e = getenv("DKS_PMAT"); want_double = (e && e[0] == 'd') ? 1 : 0; }
     const bool as_double = want_double && sm_d + 8192 <= (size_t)max_smem;

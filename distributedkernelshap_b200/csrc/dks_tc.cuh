@@ -1,61 +1,40 @@
-// Fused coalition kernel on tcgen05 / TMEM (sm_100a), binary-logistic head.
+// Fused coalition kernel on the Hopper tensor cores (wgmma, sm_90a), binary-logistic head.
 //
 // Per instance i and 128-coalition tile the masked-batch scores are one small dense contraction
 //     T[s][j] = sum_k Z[s][k] * Delta_i[j][k],      Delta_i[j][k] = scale*(XW_i[v_k] - BW[j][v_k]),  k < M
 //                                                   Delta_i[j][M] = scale*score_j   (Z[s][M] = 1)
 // (scale = -kappa*log2 e, so exp(-kappa*score) = 2^T).  Z is 0/1 and exact in bf16; Delta is split into three bf16
-// terms (hi/mid/lo, ~fp32-exact) and accumulated in fp32 in TMEM by three tcgen05.mma (M=128, N=Npad, K=16).
-// Warp roles of the persistent CTA (one per SM):
-//   warps 0-3   builders (one thread per tile row / background row): the instance's B operand (Delta splits) and each
-//               tile's A operand (Z bits expanded to bf16 through a 256-entry byte LUT, never read from HBM as a
-//               matrix) into shared memory, running up to four tiles ahead;
-//   warp 24     issuer: lane 0 waits for "A/B ready" and "accumulator free" and issues the three tcgen05.mma + commit;
-//   warps 4-19  epilogue, four groups of four warps = four TMEM accumulator buffers: tcgen05.ld the 128 x N scores,
-//               p1 = 1/(1+2^T), background-weighted sums (sum p1, sum p0) per coalition row -> shared memory;
-//   warps 20-23 WLS warpgroup, one instance behind (float64): y = link(ey) - link(fnull) per row folded into
-//               E^T W y, per-instance normal matrix when the plan is not shared, triangular solves, phi.
-// All hand-offs are mbarriers (tcgen05.commit for MMA completion); no __syncthreads in the steady state.
+// terms (hi/mid/lo, ~fp32-exact) and accumulated in fp32 registers by three wgmma (M=64, N=32, K=16) per 64-row half
+// and 32-column block of the tile.
+// Warpgroup roles of the persistent CTA (one per SM):
+//   warpgroup 0           builders (one thread per tile row / background row): the instance's B operand (Delta splits)
+//                         and each tile's A operand (Z bits expanded to bf16 through a 256-entry byte LUT, never read
+//                         from HBM as a matrix) into shared memory, running up to NBUF tiles ahead;
+//   warpgroups 1..N_CONS  consumers: tile g goes to consumer g % N_CONS, which issues the wgmma of each 64 x 32 block,
+//                         waits for them and turns the fp32 scores into p1 = 1/(1+2^T) and the background-weighted sums
+//                         (sum p1, sum p0) per coalition row -> link -> shared memory.  Four consumers keep enough
+//                         independent MUFU chains in flight per SM sub-partition while another consumer waits on wgmma;
+//   last warpgroup        WLS (float64), one instance behind: y = link(ey) - link(fnull) per row folded into E^T W y,
+//                         per-instance normal matrix when the plan is not shared, triangular solves, phi.
+// All hand-offs are mbarriers; no __syncthreads in the steady state.
 #pragma once
 
 #include <cuda_bf16.h>
 
-#include <cstdlib>
-
 #include "dks_kernels.cuh"
-
-// tuning switches (compile-time; the defaults are the measured best, see DESIGN.md)
-#ifndef DKS_TC_WARP_POLL
-#define DKS_TC_WARP_POLL 0      // 1: only lane 0 of a warp polls an mbarrier
-#endif
-#ifndef DKS_TC_WARP_ARRIVE
-#define DKS_TC_WARP_ARRIVE 0    // 1: one mbarrier arrival per warp instead of per thread
-#endif
-#ifndef DKS_TC_PREFETCH
-#define DKS_TC_PREFETCH 0       // 1: double-buffered tcgen05.ld and early accumulator release
-#endif
-#ifndef DKS_TC_EPI_WARPS
-#define DKS_TC_EPI_WARPS 16     // epilogue warps: 16 = four groups (one accumulator buffer each), 8 = two groups x two buffers
-#endif
-#ifndef DKS_TC_PINGPONG
-#define DKS_TC_PINGPONG 0       // 1: epilogue group pairs {0,1} / {2,3} alternate their compute phases (named barriers 3/4)
-#endif
-#ifndef DKS_TC_LOG_IN_WLS
-#define DKS_TC_LOG_IN_WLS 0     // 1: the epilogue hands (sum p1, sum p0) to the WLS warpgroup, which applies the link
-#endif
 
 namespace dks {
 namespace tc {
 
-constexpr int TILE_S = 128;      // coalitions per MMA tile (UMMA M)
+constexpr int TILE_S = 128;      // coalitions per A tile: two wgmma M = 64 halves
 constexpr int KP = 16;           // K per split: up to 15 varying groups + the constant column
 constexpr int NSPLIT = 3;        // bf16 hi/mid/lo
-constexpr int MAX_NPAD = 128;    // background rows per accumulator buffer (TMEM columns)
-constexpr int N_PROD_WARPS = 4, N_EPI_WARPS = DKS_TC_EPI_WARPS, N_WLS_WARPS = 4;
-constexpr int N_GROUPS = N_EPI_WARPS / 4;   // epilogue groups; group k drains the tiles with g % N_GROUPS == k
-constexpr int ISSUER_WARP = N_PROD_WARPS + N_EPI_WARPS + N_WLS_WARPS;   // one more warp: its lane 0 issues the MMAs
-constexpr int NTHREADS = 32 * (ISSUER_WARP + 1);
-constexpr int NBUF = 4;          // accumulator / A-tile buffers: two per epilogue group
-constexpr int TMEM_COLS = 512;   // four accumulator buffers of 128 fp32 columns
+constexpr int MAX_NPAD = 128;    // background rows of one instance's B operand
+constexpr int NBLK = 32;         // background columns per wgmma (N)
+constexpr int N_CONS = 4;        // consumer warpgroups
+constexpr int N_PROD_WARPS = 4, N_EPI_WARPS = 4 * N_CONS, N_WLS_WARPS = 4;
+constexpr int NTHREADS = 32 * (N_PROD_WARPS + N_EPI_WARPS + N_WLS_WARPS);
+constexpr int NBUF = 2 * N_CONS; // A-tile buffers: two per consumer
 constexpr float T_CLAMP = 60.f;  // 2^t is clamped at 2^60 so the product of two (1 + 2^t) stays finite in fp32
 constexpr uint32_t SPIN_LIMIT = 1u << 26;
 
@@ -91,25 +70,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* s
         }
     }
 }
-// one polling lane per warp (fewer SYNCS operations on the barrier); __syncwarp orders the other lanes behind it
-__device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity, int* status) {
-#if DKS_TC_WARP_POLL
-    if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity, status);
-    __syncwarp();
-#else
-    mbar_wait(bar, parity, status);
-#endif
-}
-// arrival of a whole warp: either every thread arrives, or lane 0 on behalf of the (synchronised) warp
-__device__ __forceinline__ void mbar_arrive_warp(uint64_t* bar) {
-#if DKS_TC_WARP_ARRIVE
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
-#else
-    mbar_arrive(bar);
-#endif
-}
-constexpr uint32_t ARRIVALS_PER_WARP = DKS_TC_WARP_ARRIVE ? 1u : 32u;
 // TMA bulk copy global -> shared (1-D, cp.async.bulk), completion counted in bytes on an mbarrier
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -121,78 +81,55 @@ __device__ __forceinline__ void tma_load_1d(void* dst_smem, const void* src_gmem
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
-    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
+// wgmma: the accumulator registers are in/out operands of every wrapper, so no access to them can be scheduled across
+// the fence, the MMAs or the wait
+__device__ __forceinline__ void wgmma_fence(float (&d)[16]) {
+    asm volatile("wgmma.fence.sync.aligned;"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+                   "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 :
                  : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, single CTA
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, M = 64, N = 32, K = 16, both operands K-major
+__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate)
         : "memory");
 }
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-#pragma unroll
-    for (int q = 0; q < 16; ++q) v[q] = __uint_as_float(r[q]);
-}
-// wait for outstanding tcgen05.ld; the registers are in/out operands so no consumer can be scheduled above the wait
-__device__ __forceinline__ void tmem_ld_wait(float (&v)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]),
-                   "+f"(v[9]), "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15])
+__device__ __forceinline__ void wgmma_commit_wait(float (&d)[16]) {
+    asm volatile("wgmma.commit_group.sync.aligned;\n\twgmma.wait_group.sync.aligned 0;"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+                   "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                  :
                  : "memory");
 }
 
-// shared-memory matrix descriptor, K-major, no swizzle (canonical layout ((8,m),(T,2)):((1T,SBO),(1,LBO)):
+// wgmma shared-memory matrix descriptor, K-major, no swizzle (canonical layout ((8,m),(T,2)):((1T,SBO),(1,LBO)):
 // 8x16-byte core matrices; LBO = bytes between the two K-adjacent core matrices of one K=16 step, SBO = bytes
-// between core matrices adjacent along M/N).  cute::UMMA::SmemDescriptor bit layout, version 1 (sm_100).
+// between core matrices adjacent along M/N).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
-}
-// cute::UMMA::InstrDescriptor for kind::f16: fp32 accumulate, bf16 A/B, both K-major, M = 128, N = n
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TILE_S >> 4) << 24);
 }
 
 // ---- shared memory carve-up ---------------------------------------------------------------------------------
+constexpr int NBARS = 2 * NBUF + 9;   // a_full[NBUF], a_empty[NBUF], b_full[2], b_empty[2], inst_full[2], inst_empty[2], plan_ready
+constexpr int BAR_BYTES = (NBARS * 8 + 127) / 128 * 128;
 struct Smem {
-    uint64_t* bars;      // [19]: tmem_full[4], tmem_empty[4], inst_full[2], inst_empty[2], a_full[4], b_full[2], plan_ready
-    uint32_t* tmem_ptr;  // [1]
+    uint64_t* bars;
     int* vi;             // [16] varying position -> group (producer group only)
     double* chol;        // [15*15]
     double* rhs;         // [16]
@@ -204,20 +141,19 @@ struct Smem {
     LogTabEntry* logtab; // [64] table of fast_log_ratio
     uint4* lut;          // [256] byte -> eight bf16 (1.0 / 0.0)
     unsigned char* A;    // [NBUF][128*KP*2]
-    unsigned char* B;    // [2][NSPLIT][Npad*KP*2]
+    unsigned char* B;    // [2][NSPLIT][Nb*KP*2]
 };
-__host__ __device__ inline size_t smem_bytes(int S_cap, int Npad) {
-    return 192 /*bars + tmem ptr*/ + 16 * sizeof(int) + (15 * 15 + 16 + N_WLS_WARPS * 16) * sizeof(double) +
+__host__ __device__ inline size_t smem_bytes(int S_cap, int Nb) {
+    return BAR_BYTES + 16 * sizeof(int) + (15 * 15 + 16 + N_WLS_WARPS * 16) * sizeof(double) +
            2 * (size_t)S_cap * sizeof(double) + 2 * ((size_t)S_cap + 2) * 8 + MAX_NPAD * sizeof(float) + DKS_LOGTAB_SIZE * 16 +
            256 * 16 + NBUF * (size_t)TILE_S * KP * 2 +
-           2 * NSPLIT * (size_t)Npad * KP * 2 + 64;
+           2 * NSPLIT * (size_t)Nb * KP * 2 + 192;
 }
-__device__ inline Smem carve(unsigned char* base, int S_cap, int Npad) {
+__device__ inline Smem carve(unsigned char* base, int S_cap) {
     Smem s;
     s.bars = reinterpret_cast<uint64_t*>(base);
-    s.tmem_ptr = reinterpret_cast<uint32_t*>(base + 168);
-    s.vi = reinterpret_cast<int*>(base + 192);
-    s.chol = reinterpret_cast<double*>(base + 192 + 16 * sizeof(int));
+    s.vi = reinterpret_cast<int*>(base + BAR_BYTES);
+    s.chol = reinterpret_cast<double*>(base + BAR_BYTES + 16 * sizeof(int));
     s.rhs = s.chol + 15 * 15;
     s.part = s.rhs + 16;
     s.ys = s.part + N_WLS_WARPS * 16;
@@ -230,7 +166,8 @@ __device__ inline Smem carve(unsigned char* base, int S_cap, int Npad) {
     p += 2 * plan_words * 8;
     s.logtab = reinterpret_cast<LogTabEntry*>(p);
     s.lut = reinterpret_cast<uint4*>(p + DKS_LOGTAB_SIZE * 16);
-    s.A = p + DKS_LOGTAB_SIZE * 16 + 256 * 16;
+    p += DKS_LOGTAB_SIZE * 16 + 256 * 16;
+    s.A = reinterpret_cast<unsigned char*>(((uintptr_t)p + 127) & ~(uintptr_t)127);   // MMA operands: 128-byte aligned
     s.B = s.A + NBUF * (size_t)TILE_S * KP * 2;
     return s;
 }
@@ -239,12 +176,11 @@ struct TcParams {
     ExplainParams p;
     const double* BW;      // [N][G] grouped background contributions, float64 (R == 1)
     const double* scores;  // [N]
-    int Npad;
-    int uniform_w;
+    int Nb;                // background rows of the B operand (N rounded up to NBLK)
+    int Npad;              // columns of the debug dump (N rounded up to 16)
     float* dbg_T;          // optional [S_cap][Npad] dump of the scores of instance dbg_i
     int dbg_i;
     float* dbg_time;       // optional [6][256] clock64 timeline of CTA 0 (debug kernel variant only)
-    int ablate;            // bring-up aid (env DKS_TC_ABLATE, bit mask): knocks out one pipeline stage for timing
 };
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
@@ -267,8 +203,6 @@ __device__ __forceinline__ int tiles_of(const ExplainParams& p, int i, int& M, i
 
 // p1 = 1/(1+2^t) and p0 = 2^t/(1+2^t) (no cancellation) summed over background rows.  Two elements share one
 // reciprocal: r = 1/((1+ua)(1+ub)), p1a = r(1+ub), p1b = r(1+ua)  -> 1.5 MUFU ops per element instead of 2.
-// UW: uniform background weights (plain sums).
-template <bool UW>
 __device__ __forceinline__ void consume_pair(float ta, float tb, float wa, float wb_, float& a1, float& a0) {
     ta = fminf(ta, T_CLAMP);
     tb = fminf(tb, T_CLAMP);
@@ -276,22 +210,15 @@ __device__ __forceinline__ void consume_pair(float ta, float tb, float wa, float
     const float da = 1.f + ua, db = 1.f + ub;
     const float r = rcp_approx(da * db);
     const float ra = r * db, rb = r * da;
-    if (UW) {
-        a1 += ra;
-        a1 += rb;
-        a0 = fmaf(ua, ra, a0);
-        a0 = fmaf(ub, rb, a0);
-    } else {
-        a1 = fmaf(wa, ra, a1);
-        a1 = fmaf(wb_, rb, a1);
-        a0 = fmaf(wa * ua, ra, a0);
-        a0 = fmaf(wb_ * ub, rb, a0);
-    }
+    a1 = fmaf(wa, ra, a1);
+    a1 = fmaf(wb_, rb, a1);
+    a0 = fmaf(wa * ua, ra, a0);
+    a0 = fmaf(wb_ * ub, rb, a0);
 }
 
-// Uniform background weights: four columns at a time in packed fp32 (FFMA2/FMUL2/FADD2).  With u = 2^t per column and
-// the columns paired (0,2), (1,3):  p1a + p1b = (2 + sm) / (1 + sm + q),  p0a + p0b = (sm + 2q) / (1 + sm + q),
-// sm = ua + ub, q = ua ub -- one reciprocal per pair, 8 packed ops + 4 clamps + 6 MUFU per four columns.
+// Uniform background weights: four columns at a time.  With u = 2^t per column and the columns paired (0,2), (1,3):
+// p1a + p1b = (2 + sm) / (1 + sm + q),  p0a + p0b = (sm + 2q) / (1 + sm + q),  sm = ua + ub, q = ua ub -- one
+// reciprocal per pair, 6 MUFU per four columns.
 __device__ __forceinline__ void consume_quad(float t0, float t1, float t2, float t3, f32x2& a1, f32x2& a0) {
     const f32x2 u = f2_pack(ex2_approx(fminf(t0, T_CLAMP)), ex2_approx(fminf(t1, T_CLAMP)));
     const f32x2 v = f2_pack(ex2_approx(fminf(t2, T_CLAMP)), ex2_approx(fminf(t3, T_CLAMP)));
@@ -305,64 +232,67 @@ __device__ __forceinline__ void consume_quad(float t0, float t1, float t2, float
     a0 = f2_fma(r, f2_fma(two2, q, sm), a0);
 }
 
+// One accumulator row of a 64 x 32 block: v[2jj], v[2jj+1] hold columns 8jj + cq and 8jj + cq + 1.  `wb` points at the
+// weight of column 0 of the block + cq; `full`: all 32 columns of the block are background rows, else `nleft` = background
+// rows from column cq of the block on.
 template <bool UW>
-__device__ __forceinline__ void consume16(const float (&v)[16], const float* __restrict__ wb, float& acc1, float& acc0) {
-    if (UW) {
-        f32x2 p1[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)}, p0[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)};
+__device__ __forceinline__ void consume_row(const float (&v)[8], const float* __restrict__ wb, bool full, int nleft,
+                                            float& acc1, float& acc0) {
+    if (full) {
+        if (UW) {
+            f32x2 p1[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)}, p0[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)};
+            consume_quad(v[0], v[1], v[2], v[3], p1[0], p0[0]);
+            consume_quad(v[4], v[5], v[6], v[7], p1[1], p0[1]);
+            float x0, x1, y0, y1;
+            f2_unpack(f2_add(p1[0], p1[1]), x0, x1);
+            f2_unpack(f2_add(p0[0], p0[1]), y0, y1);
+            acc1 += x0 + x1;
+            acc0 += y0 + y1;
+            return;
+        }
+        float a1[2] = {0.f, 0.f}, a0[2] = {0.f, 0.f};
 #pragma unroll
-        for (int jj = 0; jj < 16; jj += 4) consume_quad(v[jj], v[jj + 1], v[jj + 2], v[jj + 3], p1[(jj >> 2) & 1], p0[(jj >> 2) & 1]);
-        float x0, x1, y0, y1;
-        f2_unpack(f2_add(p1[0], p1[1]), x0, x1);
-        f2_unpack(f2_add(p0[0], p0[1]), y0, y1);
-        acc1 += x0 + x1;
-        acc0 += y0 + y1;
+        for (int jj = 0; jj < 4; ++jj) consume_pair(v[2 * jj], v[2 * jj + 1], wb[8 * jj], wb[8 * jj + 1], a1[jj & 1], a0[jj & 1]);
+        acc1 += a1[0] + a1[1];
+        acc0 += a0[0] + a0[1];
         return;
     }
-    float a1[2] = {0.f, 0.f}, a0[2] = {0.f, 0.f};
-#pragma unroll
-    for (int jj = 0; jj < 16; jj += 2)
-        consume_pair<UW>(v[jj], v[jj + 1], UW ? 1.f : wb[jj], UW ? 1.f : wb[jj + 1], a1[(jj >> 1) & 1], a0[(jj >> 1) & 1]);
-    acc1 += a1[0] + a1[1];
-    acc0 += a0[0] + a0[1];
-}
-
-// last, partially filled chunk: only the first n (< 16) columns are background rows; weights come from shared memory
-// (zero for the padding column that completes an odd pair)
-__device__ __forceinline__ void consume_tail(const float (&v)[16], const float* __restrict__ wb, int n, float& acc1,
-                                             float& acc0) {
+    // last, partially filled block: weights come from shared memory (zero for the padding column of an odd pair)
     float a1 = 0.f, a0 = 0.f;
 #pragma unroll
-    for (int jj = 0; jj < 16; jj += 2)
-        if (jj < n) consume_pair<false>(v[jj], v[jj + 1], wb[jj], wb[jj + 1], a1, a0);
+    for (int jj = 0; jj < 4; ++jj)
+        if (8 * jj < nleft) consume_pair(v[2 * jj], v[2 * jj + 1], wb[8 * jj], wb[8 * jj + 1], a1, a0);
     acc1 += a1;
     acc0 += a0;
 }
 
 template <bool UW, bool DBG>
-__global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams tp) {
+__global__ void __launch_bounds__(NTHREADS, 1) explain_wgmma_kernel(TcParams tp) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const ExplainParams& p = tp.p;
-    const int Npad = tp.Npad, N = p.N, G = p.G;
-    Smem sm = carve(smem_raw, p.S_cap, Npad);
-    uint64_t* tmem_full = sm.bars;
-    uint64_t* tmem_empty = sm.bars + NBUF;
-    uint64_t* inst_full = sm.bars + 2 * NBUF;
-    uint64_t* inst_empty = sm.bars + 2 * NBUF + 2;
-    uint64_t* a_full = sm.bars + 2 * NBUF + 4;
-    uint64_t* b_full = sm.bars + 3 * NBUF + 4;
-    uint64_t* plan_ready = sm.bars + 3 * NBUF + 6;
+    const int Nb = tp.Nb, N = p.N, G = p.G;
+    Smem sm = carve(smem_raw, p.S_cap);
+    uint64_t* a_full = sm.bars;
+    uint64_t* a_empty = sm.bars + NBUF;
+    uint64_t* b_full = sm.bars + 2 * NBUF;
+    uint64_t* b_empty = sm.bars + 2 * NBUF + 2;
+    uint64_t* inst_full = sm.bars + 2 * NBUF + 4;
+    uint64_t* inst_empty = sm.bars + 2 * NBUF + 6;
+    uint64_t* plan_ready = sm.bars + 2 * NBUF + 8;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const size_t slab = (size_t)p.n * G;
     const int ninst = dks_inst_count(p);
-    if ((int)blockIdx.x >= ninst) return;        // nothing for this CTA (before any TMEM allocation)
+    if ((int)blockIdx.x >= ninst) return;        // nothing for this CTA
 
+    constexpr int PROD_THREADS = 32 * N_PROD_WARPS, CONS_THREADS = 32 * N_EPI_WARPS, WLS_THREADS = 32 * N_WLS_WARPS;
     if (threadIdx.x == 0) {
-        // arrivals are per warp (lane 0 after __syncwarp), not per thread
-        for (int b = 0; b < NBUF; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 4 * ARRIVALS_PER_WARP); }
-        mbar_init(&inst_full[0], N_EPI_WARPS * ARRIVALS_PER_WARP); mbar_init(&inst_full[1], N_EPI_WARPS * ARRIVALS_PER_WARP);
-        mbar_init(&inst_empty[0], N_WLS_WARPS * ARRIVALS_PER_WARP); mbar_init(&inst_empty[1], N_WLS_WARPS * ARRIVALS_PER_WARP);
-        for (int b = 0; b < NBUF; ++b) mbar_init(&a_full[b], 32 * N_PROD_WARPS);
-        mbar_init(&b_full[0], 32 * N_PROD_WARPS); mbar_init(&b_full[1], 32 * N_PROD_WARPS);
+        for (int b = 0; b < NBUF; ++b) { mbar_init(&a_full[b], PROD_THREADS); mbar_init(&a_empty[b], 128); }
+        for (int b = 0; b < 2; ++b) {
+            mbar_init(&b_full[b], PROD_THREADS);
+            mbar_init(&b_empty[b], CONS_THREADS);
+            mbar_init(&inst_full[b], CONS_THREADS);
+            mbar_init(&inst_empty[b], WLS_THREADS);
+        }
         mbar_init(plan_ready, 1);
         fence_barrier_init();
     }
@@ -377,23 +307,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
         e.w = ((b & 64) ? 0x00003F80u : 0u) | ((b & 128) ? 0x3F800000u : 0u);
         sm.lut[b] = e;
     }
-    if (warp == 0) tmem_alloc(sm.tmem_ptr, TMEM_COLS);
-#if DKS_TC_PINGPONG
-    if (warp == 1) {   // total number of tiles this CTA will process (the ping-pong protocol needs whole rounds)
-        int cnt = 0;
-        for (int qi = blockIdx.x + lane * gridDim.x; qi < dks_inst_count(p); qi += 32 * gridDim.x) {
-            int M_, S_;
-            cnt += tiles_of(p, dks_inst_at(p, qi), M_, S_);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        if (lane == 0) sm.tmem_ptr[1] = (uint32_t)cnt;
-    }
-#endif
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *sm.tmem_ptr;
 
     // Stage the shared plan of this CTA's first instance (coalition words + weights) into shared memory with two TMA
     // bulk copies; builders and WLS warps read it from there instead of re-reading global memory every tile.
@@ -415,7 +329,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
         }
     }
 
-    const uint32_t a_bytes = TILE_S * KP * 2, b_split_bytes = (uint32_t)Npad * KP * 2;
+    const uint32_t a_bytes = TILE_S * KP * 2, b_split_bytes = (uint32_t)Nb * KP * 2;
     const long long t_start = clock64();
     auto stamp = [&](int ev, uint32_t g) {   // debug timeline: event ev of tile g of CTA 0, in cycles since start
         if (DBG && tp.dbg_time != nullptr && blockIdx.x == 0 && g < 256)
@@ -423,15 +337,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
     };
 
     if (warp < N_PROD_WARPS) {
-        // =================================== producer group / MMA issuer ===================================
+        // =================================== builders ===================================
         const int ptid = threadIdx.x;                 // 0..127: tile row (A) and background row (B) of this thread
-        constexpr int PROD_THREADS = 32 * N_PROD_WARPS;
-        const uint32_t idesc = make_idesc(Npad);
 
-        // B operand of instance i into slot `slot`: Delta splits, K-major core matrices [kc][j][8]; thread = row j
-        auto build_B = [&](int i, int M, int slot) {
+        // B operand of the instance with ordinal o into slot o & 1: Delta splits, K-major core matrices [kc][j][8];
+        // thread = row j.  The slot is free once the consumers are done with ordinal o - 2.
+        auto build_B = [&](int i, int M, int o) {
+            mbar_wait(&b_empty[o & 1], ((o >> 1) & 1) ^ 1, p.status);
             const uint64_t vm = p.vmask[i];
-            unsigned char* Bq = sm.B + (size_t)slot * NSPLIT * b_split_bytes;
+            unsigned char* Bq = sm.B + (size_t)(o & 1) * NSPLIT * b_split_bytes;
             named_bar_sync(2, PROD_THREADS);            // previous readers of sm.vi are done
             if (ptid < KP) {                            // thread k finds the k-th varying group
                 int cnt = 0, gsel = 0;
@@ -441,7 +355,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
             }
             named_bar_sync(2, PROD_THREADS);
             const int j = ptid;
-            if (j < Npad && !(tp.ablate & 32)) {
+            if (j < Nb) {
 #pragma unroll
                 for (int kc = 0; kc < 2; ++kc) {
                     float hi[8], mid[8], lo[8];
@@ -468,12 +382,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
                     wm.z = pack_bf16(mid[4], mid[5]); wm.w = pack_bf16(mid[6], mid[7]);
                     wl.x = pack_bf16(lo[0], lo[1]); wl.y = pack_bf16(lo[2], lo[3]);
                     wl.z = pack_bf16(lo[4], lo[5]); wl.w = pack_bf16(lo[6], lo[7]);
-                    const size_t off = (size_t)kc * Npad * 16 + (size_t)j * 16;
+                    const size_t off = (size_t)kc * Nb * 16 + (size_t)j * 16;
                     *reinterpret_cast<uint4*>(Bq + 0 * b_split_bytes + off) = wh;
                     *reinterpret_cast<uint4*>(Bq + 1 * b_split_bytes + off) = wm;
                     *reinterpret_cast<uint4*>(Bq + 2 * b_split_bytes + off) = wl;
                 }
             }
+            fence_proxy_async_smem();   // generic-proxy writes -> visible to the tensor core (async proxy)
+            mbar_arrive(&b_full[o & 1]);
         };
         auto next_work = [&](int qi, int& Mn) {   // next instance of this CTA that has tiles (-1: none)
             for (int q2 = qi + gridDim.x; q2 < ninst; q2 += gridDim.x) {
@@ -493,233 +409,135 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
             const int T = tiles_of(p, i, M, S);
             if (T == 0) continue;
             const uint64_t* zp = p.ext_z ? p.ext_z + (size_t)i * p.ext_stride : (M == staged_M ? sm.zs : p.plans[M].z);
-            if (built_for != i) {            // only the first instance; later ones are prefetched below
-                build_B(i, M, qb & 1);
-                fence_proxy_async_smem();
-                mbar_arrive(&b_full[qb & 1]);
-            }
-            const uint32_t g0 = g;
+            if (built_for != i) build_B(i, M, qb);    // only the first instance; later ones are prefetched below
             const int t_prefetch = T > NBUF - 1 ? NBUF - 1 : T - 1;   // after this tile: build the next instance's B
             for (int t = 0; t < T; ++t, ++g) {
                 const uint32_t buf = g % NBUF, u = g / NBUF;
                 const int s = t * TILE_S + ptid;
                 uint32_t zz = 0;
                 if (s < S) zz = (uint32_t)(zp[s] & 0xFFFFull) | (1u << M);       // constant column carries score_j
-                if (g >= NBUF) mbar_wait_warp(&tmem_full[buf], (u - 1) & 1, p.status); // A[buf] free (MMA g-NBUF done)
+                mbar_wait(&a_empty[buf], (u & 1) ^ 1, p.status);                 // consumer of tile g - NBUF is done
                 unsigned char* Ab = sm.A + (size_t)buf * a_bytes;
                 *reinterpret_cast<uint4*>(Ab + 0 * (TILE_S * 16) + ptid * 16) = sm.lut[zz & 0xFFu];
                 *reinterpret_cast<uint4*>(Ab + 1 * (TILE_S * 16) + ptid * 16) = sm.lut[(zz >> 8) & 0xFFu];
-                fence_proxy_async_smem();   // generic-proxy writes -> visible to the tensor core (async proxy)
+                fence_proxy_async_smem();
                 mbar_arrive(&a_full[buf]);
                 if (ptid == 0) stamp(0, g);                               // A tile ready
-                // prefetch: while this instance is in flight, build the next instance's B operand.  Its slot was last
-                // read by the previous instance; MMAs complete in order, so once this instance's first MMA has
-                // completed that slot is free.
+                // prefetch: while this instance is in flight, build the next instance's B operand
                 if (t == t_prefetch) {
                     int Mn;
                     int inext = next_work(qi, Mn);
                     if (inext >= 0) {
-                        mbar_wait_warp(&tmem_full[g0 % NBUF], (g0 / NBUF) & 1, p.status);
-                        build_B(inext, Mn, (qb + 1) & 1);
-                        fence_proxy_async_smem();
-                        mbar_arrive(&b_full[(qb + 1) & 1]);
+                        build_B(inext, Mn, qb + 1);
                         built_for = inext;
                     }
                 }
             }
             ++qb;
         }
-    } else if (warp == ISSUER_WARP) {
-        // =================================== MMA issuer (one thread) ===================================
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc(Npad);
-            uint64_t adesc[NBUF], bdesc[2][NSPLIT];
-#pragma unroll
-            for (int b = 0; b < NBUF; ++b) adesc[b] = make_smem_desc(smem_u32(sm.A + (size_t)b * a_bytes), TILE_S * 16, 128);
-#pragma unroll
-            for (int sl = 0; sl < 2; ++sl)
-#pragma unroll
-                for (int sp = 0; sp < NSPLIT; ++sp)
-                    bdesc[sl][sp] = make_smem_desc(smem_u32(sm.B + ((size_t)sl * NSPLIT + sp) * b_split_bytes), (uint32_t)Npad * 16, 128);
-            uint32_t g = 0;
-            int qb = 0;
-            for (int qi = blockIdx.x; qi < ninst; qi += gridDim.x) {
-                const int i = dks_inst_at(p, qi);
-                int M, S;
-                const int T = tiles_of(p, i, M, S);
-                if (T == 0) continue;
-                const int slot = qb & 1;
-                mbar_wait(&b_full[slot], (qb >> 1) & 1, p.status);      // B operand of this instance is in place
-                for (int t = 0; t < T; ++t, ++g) {
-                    const uint32_t buf = g % NBUF, u = g / NBUF;
-                    mbar_wait(&a_full[buf], u & 1, p.status);             // A tile in place
-                    mbar_wait(&tmem_empty[buf], (u & 1) ^ 1, p.status);   // epilogue drained this accumulator
-                    stamp(1, g);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + buf * 128;
-                    const int nsp = (tp.ablate & 2) ? 1 : NSPLIT;
-                    for (int sp = 0; sp < nsp; ++sp) {
-                        const uint64_t bd = slot ? bdesc[1][sp] : bdesc[0][sp];
-                        uint64_t ad = adesc[0];
-                        if (buf == 1) ad = adesc[1];
-                        if (buf == 2) ad = adesc[2];
-                        if (buf == 3) ad = adesc[3];
-                        umma_bf16(d_tmem, ad, bd, idesc, sp > 0 ? 1u : 0u);
-                    }
-                    umma_commit(&tmem_full[buf]);   // arrives when the MMAs have completed
-                    stamp(2, g);
-                }
-                ++qb;
-            }
-        }
     } else if (warp < N_PROD_WARPS + N_EPI_WARPS) {
-        // =================================== epilogue ===================================
-        // 16 warps = 4 groups x 4 warps; group g4 drains accumulator buffer g4 (tiles with g % 4 == g4).  Four
-        // epilogue warps share each SM sub-partition, enough independent MUFU chains in flight to keep its XU busy.
-        const int ew = warp - N_PROD_WARPS;           // 0..15
-        const int grp = ew >> 2;                      // accumulator buffer this group drains
-        const int quarter = warp & 3;                 // TMEM lanes 32*quarter .. +31 (hardware rule: warp id % 4)
-        const int row_in_tile = quarter * 32 + lane;
-        const int nfull = N / 16;                     // accumulator chunks of 16 columns without padding
-        const int ntail = N - nfull * 16;             // background rows in the last, partial chunk
-        const int nchunks = nfull + (ntail ? 1 : 0);
-        const uint32_t taddr0 = tmem_base + ((uint32_t)(quarter * 32) << 16);
+        // =================================== consumers ===================================
+        const int cw = warp - N_PROD_WARPS;           // 0..N_EPI_WARPS-1
+        const int cons = cw >> 2;                     // consumer warpgroup: tiles with g % N_CONS == cons
+        const int r_lo = 16 * (cw & 3) + (lane >> 2); // accumulator rows r_lo and r_lo + 8 of each 64-row half
+        const int cq = 2 * (lane & 3);                // accumulator columns 8jj + cq, 8jj + cq + 1 of each block
+        const int nblk = (N + NBLK - 1) / NBLK;
         const double lf1 = p.linkfnull[1], f1 = p.fnull[1];
         const float inv_n = 1.0f / (float)N;
+        const uint32_t a_base = smem_u32(sm.A), b_base = smem_u32(sm.B);
 
-#if DKS_TC_PINGPONG
-        static_assert(DKS_TC_PINGPONG == 0 || N_GROUPS == 4, "ping-pong needs four epilogue groups");
-        const int pair = grp >> 1;                   // pairs {0,1} and {2,3} alternate compute phases
-        constexpr int PP_THREADS = 2 * 256;          // both pairs take part in each barrier (sync + arrive)
-        if (pair == 1) named_bar_arrive(3, PP_THREADS);   // pair 0 computes first
-        int my_rounds = 0;
-#endif
         uint32_t g = 0;
-        int q = 0;
+        int q = 0, qb = 0;
         for (int qi = blockIdx.x; qi < ninst; qi += gridDim.x, ++q) {
             const int i = dks_inst_at(p, qi);
             int M, S;
             const int T = tiles_of(p, i, M, S);
             double* ys = sm.ys + (size_t)(q & 1) * p.S_cap;
             bool waited = false;
+            const int slot = qb & 1;
+            if (T > 0) mbar_wait(&b_full[slot], (qb >> 1) & 1, p.status);     // B operand of this instance is in place
             for (int t = 0; t < T; ++t, ++g) {
-                if ((int)(g % N_GROUPS) != grp) continue;
+                if ((int)(g % N_CONS) != cons) continue;
                 const uint32_t buf = g % NBUF, u = g / NBUF;
-                const uint32_t taddr = taddr0 + buf * 128;
-                const int s = t * TILE_S + row_in_tile;
-                if (quarter == 0 && lane == 0) stamp(3, g);               // epilogue group starts waiting
-                mbar_wait_warp(&tmem_full[buf], u & 1, p.status);
-#if DKS_TC_PINGPONG
-                named_bar_sync(3 + pair, PP_THREADS);                     // my pair's turn on the MUFU pipe
-                ++my_rounds;
-#endif
-                if (quarter == 0 && lane == 0) stamp(4, g);               // accumulator full seen
-                tc_fence_after();
-                float acc1 = 0.f, acc0 = 0.f;
-#if DKS_TC_PREFETCH
-                float va[16], vb[16];
-                auto release = [&]() {               // every chunk of this tile is in registers: free the accumulator
-                    tc_fence_before();
-                    mbar_arrive_warp(&tmem_empty[buf]);
-                };
-                if (tp.ablate & 8) {
+                if ((cw & 3) == 0 && lane == 0) stamp(3, g);              // consumer starts waiting
+                mbar_wait(&a_full[buf], u & 1, p.status);
+                if ((cw & 3) == 0 && lane == 0) stamp(4, g);              // A tile seen
+                float acc1[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, acc0[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [half][row]
 #pragma unroll
-                    for (int jj = 0; jj < 16; ++jj) { va[jj] = 0.01f * jj; vb[jj] = 0.02f * jj; }
-                } else {
-                    tmem_ld16(taddr, va);
-                    tmem_ld_wait(va);
-                }
-                if (nchunks == 1) release();
-                for (int c = 0; c < nchunks; c += 2) {
-                    const bool has_b = c + 1 < nchunks, has_next = c + 2 < nchunks;
-                    if (has_b && !(tp.ablate & 8)) tmem_ld16(taddr + (c + 1) * 16, vb);  // in flight during consume(va)
-                    if (DBG) {
-                        if (i == tp.dbg_i && s < p.S_cap)
-                            for (int jj = 0; jj < 16; ++jj) tp.dbg_T[(size_t)s * Npad + c * 16 + jj] = va[jj];
-                    }
-                    if (tp.ablate & 1) { acc1 += va[0]; acc0 += 1.f; }
-                    else if (c < nfull) consume16<UW>(va, sm.wb + c * 16, acc1, acc0);
-                    else consume_tail(va, sm.wb + c * 16, ntail, acc1, acc0);
-                    if (has_b) {
-                        if (!(tp.ablate & 8)) tmem_ld_wait(vb);
-                        if (!has_next) release();
-                        if (has_next && !(tp.ablate & 8)) tmem_ld16(taddr + (c + 2) * 16, va);
-                        if (DBG) {
-                            if (i == tp.dbg_i && s < p.S_cap)
-                                for (int jj = 0; jj < 16; ++jj) tp.dbg_T[(size_t)s * Npad + (c + 1) * 16 + jj] = vb[jj];
-                        }
-                        if (tp.ablate & 1) { acc1 += vb[0]; acc0 += 1.f; }
-                        else if (c + 1 < nfull) consume16<UW>(vb, sm.wb + (c + 1) * 16, acc1, acc0);
-                        else consume_tail(vb, sm.wb + (c + 1) * 16, ntail, acc1, acc0);
-                        if (has_next) {
-                            if (!(tp.ablate & 8)) tmem_ld_wait(va);
-                            if (c + 3 >= nchunks) release();     // va holds the last chunk
-                        }
-                    }
-                }
-#else
-                for (int c = 0; c < nchunks; ++c) {
-                    float v[16];
-                    if (tp.ablate & 8) {
+                for (int h = 0; h < 2; ++h) {
+                    const uint64_t ad = make_smem_desc(a_base + buf * a_bytes + h * 64 * 16, TILE_S * 16, 128);
+                    for (int c = 0; c < nblk; ++c) {
+                        float d[16];
 #pragma unroll
-                        for (int jj = 0; jj < 16; ++jj) v[jj] = 0.01f * (float)(jj + c);
-                    } else {
-                        tmem_ld16(taddr + c * 16, v);
-                        tmem_ld_wait(v);
+                        for (int e = 0; e < 16; ++e) d[e] = 0.f;
+                        wgmma_fence(d);
+#pragma unroll
+                        for (int sp = 0; sp < NSPLIT; ++sp) {
+                            const uint32_t baddr = b_base + ((uint32_t)slot * NSPLIT + sp) * b_split_bytes + c * NBLK * 16;
+                            wgmma_bf16_n32(d, ad, make_smem_desc(baddr, (uint32_t)Nb * 16, 128), sp > 0 ? 1u : 0u);
+                        }
+                        wgmma_commit_wait(d);
+                        if (DBG && i == tp.dbg_i) {
+#pragma unroll
+                            for (int e = 0; e < 16; ++e) {
+                                const int s = t * TILE_S + h * 64 + r_lo + ((e >> 1) & 1) * 8;
+                                const int col = c * NBLK + (e >> 2) * 8 + cq + (e & 1);
+                                if (s < p.S_cap && col < tp.Npad) tp.dbg_T[(size_t)s * tp.Npad + col] = d[e];
+                            }
+                        }
+                        const float va[8] = {d[0], d[1], d[4], d[5], d[8], d[9], d[12], d[13]};
+                        const float vb[8] = {d[2], d[3], d[6], d[7], d[10], d[11], d[14], d[15]};
+                        const int col0 = c * NBLK + cq;
+                        const bool full = (c + 1) * NBLK <= N;
+                        consume_row<UW>(va, sm.wb + col0, full, N - col0, acc1[h][0], acc0[h][0]);
+                        consume_row<UW>(vb, sm.wb + col0, full, N - col0, acc1[h][1], acc0[h][1]);
                     }
-                    if (DBG) {
-                        if (i == tp.dbg_i && s < p.S_cap)
-                            for (int jj = 0; jj < 16; ++jj) tp.dbg_T[(size_t)s * Npad + c * 16 + jj] = v[jj];
-                    }
-                    if (tp.ablate & 1) { acc1 += v[0]; acc0 += 1.f; }
-                    else if (c < nfull) consume16<UW>(v, sm.wb + c * 16, acc1, acc0);
-                    else consume_tail(v, sm.wb + c * 16, ntail, acc1, acc0);
                 }
-                tc_fence_before();
-                mbar_arrive_warp(&tmem_empty[buf]);  // accumulator buffer may be overwritten
-                if (quarter == 0 && lane == 0) stamp(5, g);               // accumulator drained
-#endif
-#if DKS_TC_PINGPONG
-                // hand the MUFU pipe to the other pair (pair 1's arrival after the very last round has no taker)
-                if (!(pair == 1 && my_rounds == ((int)sm.tmem_ptr[1] + N_GROUPS - 1) / N_GROUPS))
-                    named_bar_arrive(3 + (pair ^ 1), PP_THREADS);
-#endif
+                mbar_arrive(&a_empty[buf]);          // every wgmma reading A[buf] has completed
+                if ((cw & 3) == 0 && lane == 0) stamp(5, g);              // tile drained
+                // the four lanes of a quad hold the same rows: sum their column partials
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+                        for (int o = 1; o < 4; o <<= 1) {
+                            acc1[h][rr] += __shfl_xor_sync(0xffffffffu, acc1[h][rr], o);
+                            acc0[h][rr] += __shfl_xor_sync(0xffffffffu, acc0[h][rr], o);
+                        }
                 if (!waited) {   // the row buffer of ordinal q-2 must have been consumed by the WLS warps
-                    mbar_wait_warp(&inst_empty[q & 1], ((q >> 1) & 1) ^ 1, p.status);
+                    mbar_wait(&inst_empty[q & 1], ((q >> 1) & 1) ^ 1, p.status);
                     waited = true;
                 }
-                if (s < S && !(tp.ablate & 512)) {
-#if DKS_TC_LOG_IN_WLS
-                    reinterpret_cast<float2*>(ys)[s] = make_float2(acc1, acc0);   // link applied by the WLS warpgroup
-#else
-                    // link(ey) - link(fnull); with the logit link the normalisation of the sums cancels
-                    double y;
-                    if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(acc1, acc0, sm.logtab) - lf1;
-                    else y = (double)(UW ? acc1 * inv_n : acc1) - f1;
-                    ys[s] = y;
-#endif
+                if ((lane & 3) == 0) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int rr = 0; rr < 2; ++rr) {
+                            const int s = t * TILE_S + h * 64 + r_lo + rr * 8;
+                            if (s < S) {
+                                // link(ey) - link(fnull); with the logit link the normalisation of the sums cancels
+                                double y;
+                                if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(acc1[h][rr], acc0[h][rr], sm.logtab) - lf1;
+                                else y = (double)(UW ? acc1[h][rr] * inv_n : acc1[h][rr]) - f1;
+                                ys[s] = y;
+                            }
+                        }
                 }
             }
-            if (!waited) mbar_wait_warp(&inst_empty[q & 1], ((q >> 1) & 1) ^ 1, p.status);
-            mbar_arrive_warp(&inst_full[q & 1]);     // release-arrive: publishes the rows written by this warp
-        }
-#if DKS_TC_PINGPONG
-        {   // groups without a tile in the last (partial) round still take part in its barriers
-            const int rounds = ((int)sm.tmem_ptr[1] + N_GROUPS - 1) / N_GROUPS;
-            while (my_rounds < rounds) {
-                named_bar_sync(3 + pair, PP_THREADS);
-                ++my_rounds;
-                if (!(pair == 1 && my_rounds == rounds)) named_bar_arrive(3 + (pair ^ 1), PP_THREADS);
+            if (T > 0) {
+                mbar_arrive(&b_empty[slot]);
+                ++qb;
             }
+            if (!waited) mbar_wait(&inst_empty[q & 1], ((q >> 1) & 1) ^ 1, p.status);
+            mbar_arrive(&inst_full[q & 1]);          // release-arrive: publishes the rows written by this thread
         }
-#endif
     } else {
         // =================================== WLS warpgroup (float64) ===================================
-        // per row: y = link(ey) - link(fnull) from the (sum p1, sum p0) pair, folded into E^T W y; then the
-        // triangular solves and phi.  Runs one instance behind the epilogue.
+        // per row: y = link(ey) - link(fnull) folded into E^T W y; then the triangular solves and phi.  Runs one
+        // instance behind the consumers.
         const int ww = warp - (N_PROD_WARPS + N_EPI_WARPS);                  // 0..3
         const int wtid = threadIdx.x - 32 * (N_PROD_WARPS + N_EPI_WARPS);     // 0..127
-        constexpr int WLS_THREADS = 32 * N_WLS_WARPS;
         int cachedM = -1;
         bool have_inverse = false;
         int q = 0;
@@ -728,11 +546,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
             int M, S;
             const int T = tiles_of(p, i, M, S);
             const int C = p.C;
-            if (!(tp.ablate & 256))
-                for (int idx = wtid; idx < C * G; idx += WLS_THREADS)
-                    p.phi[(size_t)(idx / G) * slab + (size_t)i * G + idx % G] = 0.0;
+            for (int idx = wtid; idx < C * G; idx += WLS_THREADS)
+                p.phi[(size_t)(idx / G) * slab + (size_t)i * G + idx % G] = 0.0;
             if (T == 0) {
-                mbar_wait_warp(&inst_full[q & 1], (q >> 1) & 1, p.status);
+                mbar_wait(&inst_full[q & 1], (q >> 1) & 1, p.status);
                 if (M == 1) {
                     if (wtid < C) {
                         int gI = __ffsll((long long)p.vmask[i]) - 1;
@@ -744,14 +561,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
                     if (missing) { if (atomicCAS(&p.status[0], 0, DKS_ERR_PLAN_MISSING) == 0) p.status[1] = M; }
                     else { if (atomicCAS(&p.status[0], 0, DKS_ERR_INVALID) == 0) p.status[1] = i; }
                 }
-                mbar_arrive_warp(&inst_empty[q & 1]);
+                mbar_arrive(&inst_empty[q & 1]);
                 continue;
             }
             const int nA = M - 1, L = M - 1;
             const uint64_t* zp;
             const double* wp;
             // normal matrix / its Cholesky factor: shared plans bring a precomputed factor; per-instance plans are
-            // factored here, overlapping the epilogue of the same instance
+            // factored here, overlapping the consumers' work on the same instance
             if (p.ext_z == nullptr) {
                 zp = M == staged_M ? sm.zs : p.plans[M].z;
                 wp = M == staged_M ? sm.ws : p.plans[M].w;
@@ -782,23 +599,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
                 }
             }
             const double delta = p.dlink[(size_t)i * C + 1];
-            mbar_wait_warp(&inst_full[q & 1], (q >> 1) & 1, p.status);
+            mbar_wait(&inst_full[q & 1], (q >> 1) & 1, p.status);
             const double* ys = sm.ys + (size_t)(q & 1) * p.S_cap;
             long long Tk[KP - 1];                    // fixed-point partial sums of E^T W y (exact integer adds)
 #pragma unroll
             for (int k = 0; k < KP - 1; ++k) Tk[k] = 0;
-#if DKS_TC_LOG_IN_WLS
-            const double lf1 = p.linkfnull[1], f1 = p.fnull[1], inv_n = 1.0 / (double)N;
-#endif
-            for (int s = wtid; s < ((tp.ablate & 4) ? 0 : S); s += WLS_THREADS) {
-#if DKS_TC_LOG_IN_WLS
-                const float2 a = reinterpret_cast<const float2*>(ys)[s];
-                double y;
-                if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(a.x, a.y, sm.logtab) - lf1;
-                else y = (UW ? (double)a.x * inv_n : (double)a.x) - f1;
-#else
+            for (int s = wtid; s < S; s += WLS_THREADS) {
                 const double y = ys[s];
-#endif
                 const uint64_t zrow = zp[s];
                 const double wrow = wp[s];
                 // fold the row into E^T W y:  e_k = z_k - z_L = (z_L ? -1 : 1) * z'_k with z' = z_L ? ~z : z
@@ -813,7 +620,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
             long long* part_ll = reinterpret_cast<long long*>(sm.part);
 #pragma unroll
             for (int k = 0; k < KP - 1; ++k)
-                if (k < nA && !(tp.ablate & 128)) {
+                if (k < nA) {
                     const long long r = warp_sum_ll(Tk[k]);
                     if (lane == 0) part_ll[ww * 16 + k] = r;
                 }
@@ -827,7 +634,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
             if (have_inverse) {
                 // beta = inv(E^T W E) (E^T W y): one thread per coefficient, then phi (both classes) by warp 0
                 double beta = 0.0;
-                if (ww == 0 && lane < nA && !(tp.ablate & 64)) {
+                if (ww == 0 && lane < nA) {
                     for (int l = 0; l < nA; ++l) beta = fma(sm.chol[lane * nA + l], sm.rhs[l], beta);
                 }
                 if (ww == 0) {
@@ -859,25 +666,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_tcgen05_kernel(TcParams t
                 for (int k = 0; k < M; ++k) { double v = phi1[vi[k]]; phi0[vi[k]] = (v == 0.0) ? 0.0 : -v; }
             }
             named_bar_sync(1, WLS_THREADS);
-            mbar_arrive_warp(&inst_empty[q & 1]);
+            mbar_arrive(&inst_empty[q & 1]);
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 }  // namespace tc
 
 // ---- host glue --------------------------------------------------------------------------------------------------
 inline int tc_npad(int N) { return (N + 15) / 16 * 16; }
+inline int tc_nb(int N) { return (N + tc::NBLK - 1) / tc::NBLK * tc::NBLK; }
 
 inline bool tc_supported(const dks_ctx* ctx, const ExplainParams& p) {
     if (ctx->act != DKS_ACT_BINARY_LOGISTIC || ctx->R != 1) return false;
     if (ctx->G > tc::KP - 1) return false;            // M + constant column must fit one K = 16 step
-    if (ctx->N > tc::MAX_NPAD) return false;          // one accumulator buffer holds the whole background
-    if ((long long)tc::smem_bytes(p.S_cap, tc_npad(ctx->N)) > (long long)ctx->max_smem_optin) return false;
+    if (ctx->N > tc::MAX_NPAD) return false;          // one B operand holds the whole background
+    if ((long long)tc::smem_bytes(p.S_cap, tc_nb(ctx->N)) > (long long)ctx->max_smem_optin) return false;
     return true;
 }
 
@@ -886,18 +690,17 @@ inline int tc_launch(dks_ctx* ctx, const ExplainParams& p, cudaStream_t stream) 
     tp.p = p;
     tp.BW = ctx->d_BW;
     tp.scores = ctx->d_scores;
+    tp.Nb = tc_nb(ctx->N);
     tp.Npad = tc_npad(ctx->N);
-    tp.uniform_w = ctx->uniform_w ? 1 : 0;
     tp.dbg_T = ctx->dbg_T;
     tp.dbg_i = ctx->dbg_i;
     tp.dbg_time = ctx->dbg_time;
-    const char* ab = getenv("DKS_TC_ABLATE");
-    tp.ablate = ab ? atoi(ab) : 0;
-    size_t smem = tc::smem_bytes(p.S_cap, tp.Npad);
+    size_t smem = tc::smem_bytes(p.S_cap, tp.Nb);
     void (*kern)(tc::TcParams) = nullptr;
     const bool dbg = tp.dbg_T != nullptr && tp.dbg_i >= 0;
-    if (dbg) kern = tp.uniform_w ? tc::explain_tcgen05_kernel<true, true> : tc::explain_tcgen05_kernel<false, true>;
-    else kern = tp.uniform_w ? tc::explain_tcgen05_kernel<true, false> : tc::explain_tcgen05_kernel<false, false>;
+    const bool uw = ctx->uniform_w;
+    if (dbg) kern = uw ? tc::explain_wgmma_kernel<true, true> : tc::explain_wgmma_kernel<false, true>;
+    else kern = uw ? tc::explain_wgmma_kernel<true, false> : tc::explain_wgmma_kernel<false, false>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return DKS_ERR_CUDA;
     int grid = ctx->sm_count < p.n ? ctx->sm_count : p.n;

@@ -1,7 +1,7 @@
 // Solve stage of the shared-plan path for plans of more than 128 groups (sixteen 64-bit words per coalition row; configs[3]
 // of BASELINE.json read as 1024 singleton groups).
 //
-// The coalition stage is the shared-plan kernel of dks_shared.cuh (explain_shared_tmem_kernel<NTAIL, 16>): it leaves
+// The coalition stage is the shared-plan kernel of dks_shared.cuh (explain_shared_smem_kernel<NTAIL, 16>): it leaves
 // (sum p1, sum p0) per (instance, coalition).  The (M-1) x (M-1) normal matrix -- 8 MB at M = 1024 -- no longer fits shared
 // memory, and it does not have to: the plan is shared, so the projection P = inv(E^T W E) E^T W is formed ONCE on the host
 // in float64 (plan.py: projection(), np.linalg.inv like upstream's solve) and uploaded transposed, PT [S_pad][KP], with

@@ -5,7 +5,7 @@ In the reference that slot holds ``KernelExplainerWrapper`` (explainers/kernel_s
 ``.vector_out`` from it (kernel_shap.py:789-790, :880-887).  This class keeps that constructor shape
 ``(predictor, background_data, link=..., seed=...)`` and those members, and runs the per-instance hot path
 (varying groups -> coalition plan -> mask/impute -> predict -> background mean -> link -> constrained WLS) in
-CUDA through the C ABI of ``include/dks.h``.  No CPU fallback: without ``libdks.so`` and a B200 it raises.
+CUDA through the C ABI of ``include/dks.h``.  No CPU fallback: without ``libdks.so`` and an H100 it raises.
 """
 import ctypes as C
 import logging
@@ -548,7 +548,7 @@ class GpuKernelExplainer:
         return {"prepare": float(out[0]), "coalitions": float(out[1]), "total": float(out[2])}
 
     def debug_scores(self, X, instance, nsamples="auto"):
-        """Raw accumulator tile of the tcgen05 kernel for one instance: float32 [S_cap, Npad] of scaled masked scores
+        """Raw accumulator tile of the tensor-core kernel for one instance: float32 [S_cap, Npad] of scaled masked scores
         ``-kappa*log2(e) * score(s, j)`` (tests only)."""
         _cabi.check(self.lib.dks_debug_score_dump(self._ctx, int(instance)))
         try:
@@ -561,7 +561,7 @@ class GpuKernelExplainer:
         return buf[:rows.value * cols.value].reshape(rows.value, cols.value).copy()
 
     def debug_timeline(self, X, nsamples="auto"):
-        """clock64 timeline [6, 256] of CTA 0 of the tcgen05 kernel (see ``dks_debug_get_timeline``); tests/tuning only."""
+        """clock64 timeline [6, 256] of CTA 0 of the tensor-core kernel (see ``dks_debug_get_timeline``); tests/tuning only."""
         self.shap_values(X, nsamples=nsamples, l1_reg=False)          # plans uploaded, steady state
         _cabi.check(self.lib.dks_debug_score_dump(self._ctx, 0))
         try:

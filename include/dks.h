@@ -1,5 +1,5 @@
 /*
- * dks.h -- C ABI of the B200-native KernelSHAP engine (libdks.so).
+ * dks.h -- C ABI of the H100-native KernelSHAP engine (libdks.so).
  *
  * The reference (alexcoca/DistributedKernelShap) has no FFI: its hot path is reached through a Python
  * duck-typed slot, `KernelShap._explainer` (explainers/kernel_shap.py:774-788), whose object must offer
@@ -48,7 +48,7 @@ extern "C" {
 /* which fused kernel evaluates the coalitions */
 #define DKS_KERNEL_AUTO 0
 #define DKS_KERNEL_SIMT 1       /* CUDA-core kernel (all shapes) */
-#define DKS_KERNEL_TCGEN05 2    /* tensor-core kernel: Z tile x background tile on tcgen05/TMEM */
+#define DKS_KERNEL_TCGEN05 2    /* tensor-core kernel: Z tile x background tile on wgmma (the name is historical) */
 #define DKS_KERNEL_SHARED 3     /* shared-plan fast path for instances whose groups all vary (+ best general kernel
                                  * for the rest); DKS_KERNEL_AUTO picks it whenever it applies */
 
@@ -208,14 +208,14 @@ int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by th
  * coalition kernel, [2] total; synchronises. */
 int dks_last_timings(dks_ctx* ctx, float* ms3);
 
-/* ---- debugging aid for the tcgen05 kernel (tests only) ---------------------------------------------------
+/* ---- debugging aid for the tensor-core kernel (tests only) ---------------------------------------------------
  * dks_debug_score_dump(ctx, i): the next explains also write the raw accumulator tile of instance i (scaled masked
  * scores T[s][j], float32 [rows x cols]); i < 0 switches it off.  dks_debug_get_scores copies the dump to the host
  * (synchronises); rows/cols report its shape. */
 int dks_debug_score_dump(dks_ctx* ctx, int instance);
 int dks_debug_get_scores(dks_ctx* ctx, float* out_host, int max_floats, int* rows, int* cols);
 /* cycle timeline of CTA 0 recorded by the same debug run: float32 [6][256], event e of tile g at [e*256+g]
- * (0 A-tile ready, 1 accumulator free, 2 MMAs issued, 3 epilogue waits, 4 accumulator full, 5 accumulator drained) */
+ * (0 A tile ready, 3 consumer starts waiting for it, 4 A tile seen by the consumer, 5 tile drained; 1 and 2 unused) */
 int dks_debug_get_timeline(dks_ctx* ctx, float* out_host);
 
 #ifdef __cplusplus

@@ -25,7 +25,7 @@ def _engine(prob, link="logit", predict="predict_proba", **kw):
     return GpuKernelExplainer(getattr(prob["clf"], predict), dd, link=link, **kw)
 
 
-KERNELS = ["simt", "tcgen05", "auto"]      # auto = shared-plan fast path where it applies + tcgen05 for the rest
+KERNELS = ["simt", "tcgen05", "auto"]      # tcgen05 = the tensor-core (wgmma) kernel; auto = shared-plan fast path where it applies + it for the rest
 
 
 def _compare(got, want, tol=TOL):
