@@ -80,6 +80,7 @@ SIGNATURES = {
     "dks_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "dks_kernel_launches": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "dks_last_timings": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "dks_last_path": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "dks_debug_score_dump": (C.c_int, [C.c_void_p, C.c_int]),
     "dks_debug_get_timeline": (C.c_int, [C.c_void_p, C.c_void_p]),
     "dks_debug_get_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

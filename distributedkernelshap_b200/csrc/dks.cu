@@ -146,6 +146,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     REQUIRE(ctx->prepared, "dks_explain: call dks_prepare_* first");
     REQUIRE((ext_z == nullptr) == (ext_w == nullptr), "ext_zbits and ext_w must both be given or both be NULL");
     const int n = ctx->cur_n;
+    int32_t* path = ctx->last_path;                  // what this call launches (dks_last_path)
+    memset(path, 0, sizeof(ctx->last_path));
     const double* ext_chol = nullptr;
     const double* ext_ainv = nullptr;
     int ext_fstride = 0;
@@ -311,6 +313,9 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         }
         CUDA_TRY(dks::shared_path::launch_explain_fused(fp, fcfg, ctx->sm_count, ctx->stream));
         ctx->launches += 1;
+        path[DKS_PATH_SHARED] = DKS_SHARED_FUSED; path[DKS_PATH_CHUNKS] = 1; path[DKS_PATH_WARPS] = fcfg.warps;
+        path[DKS_PATH_GRID] = ctx->sm_count; path[DKS_PATH_FUSED_B] = fcfg.B; path[DKS_PATH_FUSED_NI] = fcfg.ni;
+        path[DKS_PATH_SOLVE] = DKS_SOLVE_FUSED;
         CUDA_TRY(cudaGetLastError());
         p.list = ctx->d_idx_other;
         p.count = ctx->d_counts + 1;
@@ -327,9 +332,12 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             if (need > ctx->cap_acache) { TRY(dev_alloc(&ctx->d_acache, need)); ctx->cap_acache = need; ctx->epoch++; }
             sp.acache = ctx->d_acache;
         }
-        const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream);
+        dks::shared_path::SharedLaunch sl;
+        const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &sl);
         if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
         ctx->launches += nl - 1;
+        path[DKS_PATH_SHARED] = sl.regs ? DKS_SHARED_REGS : DKS_SHARED_SMEM; path[DKS_PATH_CHUNKS] = sl.chunks;
+        path[DKS_PATH_WARPS] = sl.warps; path[DKS_PATH_GRID] = sl.grid;
         dks::shared_path::WlsSharedParams wp;
         wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = ctx->C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link;
         wp.uniform_w = 1; wp.sums = ctx->d_sums; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink;
@@ -376,6 +384,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             if (lgrid > ctx->sm_count * per_sm) lgrid = ctx->sm_count * per_sm;
             CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_lars_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm));
             dks::l1::l1_lars_kernel<<<lgrid, 32 * wpc, lsm, ctx->stream>>>(lp, wpc, stage_gram);
+            path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
         } else if (pg.W > 2) {
             // more than 128 groups: link, float64 product with the host-supplied projection, remainder (dks_wide.cuh)
             const size_t need_y = (size_t)n * S_pad, need_b = (size_t)n * pg.kpw;
@@ -389,6 +398,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             qp.y = ctx->d_yw; qp.beta = ctx->d_betaw; qp.phi = phi_dev;
             CUDA_TRY(dks::wide::launch_wide_solve(qp, n, ctx->sm_count, ctx->opt_wide_gemm, ctx->stream));
             ctx->launches += 2;                      // three launches; the common tail below counts one of them
+            path[DKS_PATH_SOLVE] = DKS_SOLVE_WIDE;
         } else if (pg.pmat != nullptr) {
             dks::shared_path::WlsPmatParams pp;
             pp.n = n; pp.N = ctx->N; pp.G = G; pp.C = ctx->C; pp.S = S; pp.S_pad = S_pad; pp.link = ctx->link; pp.uniform_w = 1;
@@ -399,6 +409,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             if (!dks::shared_path::launch_wls_pmat(pp, n, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &perr))
                 return fail(DKS_ERR_UNSUPPORTED, "projection solve does not fit shared memory");
             CUDA_TRY(perr);
+            path[DKS_PATH_SOLVE] = DKS_SOLVE_PMAT; path[DKS_PATH_PMAT_KPAD] = dks::shared_path::wls_pmat_kpad(G);
         } else {
             const size_t wsm = dks::shared_path::wls_shared_smem(G);
             int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 24 * 1024));
@@ -412,6 +423,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
                 CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
                 dks::shared_path::wls_shared_kernel<2><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
             }
+            path[DKS_PATH_SOLVE] = DKS_SOLVE_WLS_SHARED;
         }
         ctx->launches += 2;
         CUDA_TRY(cudaGetLastError());
@@ -422,6 +434,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         // instances with a partial varying set would need their own selection: reported, not computed
         dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 1;
+        path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(join());
         CUDA_TRY(record_ev(ctx, 3));
@@ -438,6 +451,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
                         "background weights, kernel 'auto' or 'shared', shared plan of M=%d uploaded)", G);
         dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 1;
+        path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(join());
         CUDA_TRY(record_ev(ctx, 3));
@@ -450,9 +464,21 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             return fail(DKS_ERR_UNSUPPORTED, "tensor-core kernel does not support this shape/head (N=%d G=%d act=%d)", ctx->N,
                         ctx->G, ctx->act);
         TRY(dks::tc_launch(ctx, p, gstream));
+        path[DKS_PATH_GENERAL] = DKS_GENERAL_TC;
     } else {
         const bool sfm = ctx->act == DKS_ACT_SOFTMAX;
         size_t smem = dks::simt_smem_bytes(S_cap, ctx->N, ctx->G, sfm ? ctx->R : 1, sfm ? ctx->C : 1);
+        if ((long long)smem > (long long)ctx->max_smem_optin && fast) {
+            // the shared-plan path took the instances whose groups all vary; the general kernel is sized for the largest
+            // plan set and cannot hold it.  The instances left for it (often none) are reported, not computed.
+            dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
+            ctx->launches += 1;
+            path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
+            CUDA_TRY(cudaGetLastError());
+            CUDA_TRY(join());
+            CUDA_TRY(record_ev(ctx, 3));
+            return DKS_OK;
+        }
         if ((long long)smem > (long long)ctx->max_smem_optin)
             return fail(DKS_ERR_UNSUPPORTED, "SIMT kernel needs %zu B of shared memory (> %d): N*G or nsamples too large",
                         smem, ctx->max_smem_optin);
@@ -464,6 +490,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if (grid > n) grid = n;
         dks::explain_simt_kernel<<<grid, 256, smem, gstream>>>(p);
         ctx->launches += 1;
+        path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT;
     }
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(join());
@@ -1370,6 +1397,12 @@ int dks_last_timings(dks_ctx* ctx, float* ms3) {
     CUDA_TRY(cudaEventElapsedTime(&ms3[0], ctx->ev[0], ctx->ev[1]));
     CUDA_TRY(cudaEventElapsedTime(&ms3[1], ctx->ev[2], ctx->ev[3]));
     CUDA_TRY(cudaEventElapsedTime(&ms3[2], ctx->ev[0], ctx->ev[3]));
+    return DKS_OK;
+}
+
+int dks_last_path(dks_ctx* ctx, int32_t* out, int n) {
+    REQUIRE(ctx && out && n >= 0, "dks_last_path: bad arguments");
+    for (int k = 0; k < n; ++k) out[k] = k < DKS_PATH_FIELDS ? ctx->last_path[k] : 0;
     return DKS_OK;
 }
 

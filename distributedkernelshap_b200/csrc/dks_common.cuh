@@ -229,6 +229,7 @@ struct dks_ctx {
     bool opt_graph_timing = false;   // keep the timing event records inside a captured graph (dks_last_timings after replays)
     bool timing_valid = false, last_was_graph = false;
     bool last_fused = false;                       // the last explain ran the fused shared-plan kernel
+    int32_t last_path[DKS_PATH_FIELDS] = {};       // what the last explain launched (dks_last_path), recorded while enqueuing
 
     // the general kernel for the instances the shared-plan path does not take runs on a side stream, next to the fused kernel
     // (it is usually empty: a serialised empty launch cost 6 us per step)

@@ -465,12 +465,30 @@ inline bool shared_dm_in_smem() {
     return mode == 1;
 }
 
-inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words, int grid, int max_smem, cudaStream_t stream) {
+// What the launches of the unfused coalition kernel used (reported by dks_last_path): the fewest warps per CTA and the
+// largest grid over the background chunks.
+struct SharedLaunch { int regs, warps, grid, chunks; };
+
+// CTAs for n_rg row groups at `warps` warps per CTA: at least one per SM, and enough that every row group has a warp (a
+// warp without a row group does nothing, so a grid of fewer warps than row groups would leave sums unwritten).  The
+// kernels need no co-resident CTAs: every warp works on its own rows, so the extra CTAs simply run in later waves.
+inline int shared_grid(int n_rg, int warps, int sm_count) {
+    const int need = (n_rg + warps - 1) / warps;
+    return need > sm_count ? need : sm_count;
+}
+
+inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words, int sm_count, int max_smem, cudaStream_t stream,
+                                               SharedLaunch* info) {
+    const int n_rg = p.S_pad / 32;
     if (shared_dm_in_smem() || words > 2) {                  // sixteen-word rows exist for the shared-memory kernel only
         const size_t slice = dm_slice_bytes(p.N);
         int warps_used = (int)(((size_t)max_smem - 1024) / slice);
         if (warps_used > TM_MAX_WARPS) warps_used = TM_MAX_WARPS;
         const size_t smem = (size_t)warps_used * slice;
+        const int grid = shared_grid(n_rg, warps_used, sm_count);
+        info->regs = 0;
+        if (info->warps == 0 || warps_used < info->warps) info->warps = warps_used;
+        if (grid > info->grid) info->grid = grid;
         cudaError_t err = cudaSuccess;
         switch (p.N % 16) {
 #define DKS_CASE_W(T, W)                                                                                                  \
@@ -491,6 +509,10 @@ inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words,
     }
 
     const int threads = 32 * WARPS_PER_CTA;
+    const int grid = shared_grid(n_rg, WARPS_PER_CTA, sm_count);
+    info->regs = 1;
+    info->warps = WARPS_PER_CTA;
+    if (grid > info->grid) info->grid = grid;
     switch (p.N % 16) {
 #define DKS_CASE(T)                                                             \
     case T:                                                                     \
@@ -506,18 +528,20 @@ inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words,
 
 // Backgrounds larger than MAXN rows go through in chunks of MAXN columns of Dm (one launch each, sums accumulated).
 // Returns the number of launches (0 when one of them could not be configured).
-inline int launch_explain_shared(SharedParams p, int words, int grid, int max_smem, cudaStream_t stream) {
+inline int launch_explain_shared(SharedParams p, int words, int sm_count, int max_smem, cudaStream_t stream, SharedLaunch* info) {
     const int N = p.N;
     const float* dm = p.DmT;
     int launches = 0;
+    info->grid = 0; info->warps = 0;
     const bool use_cache = words > 2 && p.acache != nullptr && N > MAXN;
     for (int j0 = 0; j0 < N; j0 += MAXN, ++launches) {
         p.N = N - j0 < MAXN ? N - j0 : MAXN;
         p.DmT = dm + (size_t)j0 * p.S_pad;
         p.accumulate = j0 > 0;
         p.acache_mode = use_cache ? (j0 == 0 ? 1 : 2) : 0;
-        if (launch_explain_shared_chunk(p, words, grid, max_smem, stream) != cudaSuccess) return 0;
+        if (launch_explain_shared_chunk(p, words, sm_count, max_smem, stream, info) != cudaSuccess) return 0;
     }
+    info->chunks = launches;
     return launches;
 }
 

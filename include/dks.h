@@ -204,6 +204,34 @@ int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
  * chunk's launch only (default 1).  Both give identical bits either way. */
 int dks_set_option(dks_ctx* ctx, const char* name, int value);
 int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by this ctx so far */
+/* Which kernels the last explain call launched (dks_explain_* / dks_run_dev), recorded on the host while the launch
+ * sequence is enqueued: a CUDA-graph replay keeps the record of the call it captured.  out[0 .. n) receives the first n
+ * of the DKS_PATH_FIELDS entries indexed by DKS_PATH_*; n may be smaller (older callers) or larger (zero-filled). */
+#define DKS_PATH_SHARED 0        /* shared-plan coalition kernel: DKS_SHARED_* */
+#define DKS_PATH_CHUNKS 1        /* background chunks (launches) of the unfused coalition kernel; 1 for the fused one */
+#define DKS_PATH_WARPS 2         /* warps per CTA the coalition kernel uses (the fewest over the chunks) */
+#define DKS_PATH_GRID 3          /* CTAs of the coalition kernel (the largest over the chunks) */
+#define DKS_PATH_FUSED_B 4       /* fused kernel: instances parked per warp before the turn-around */
+#define DKS_PATH_FUSED_NI 5      /* fused kernel: instances per pass over a warp's rows */
+#define DKS_PATH_SOLVE 6         /* DKS_SOLVE_* */
+#define DKS_PATH_PMAT_KPAD 7     /* projection solve (DKS_SOLVE_PMAT): coefficient rows of P, padded */
+#define DKS_PATH_GENERAL 8       /* DKS_GENERAL_*: the kernel of the instances the shared-plan path does not take */
+#define DKS_PATH_FIELDS 9
+#define DKS_SHARED_NONE 0
+#define DKS_SHARED_FUSED 1       /* explain_shared_fused_kernel: link + projection solve inside */
+#define DKS_SHARED_SMEM 2        /* explain_shared_smem_kernel (Dm rows in shared memory) */
+#define DKS_SHARED_REGS 3        /* explain_shared_kernel (Dm rows in registers; DKS_SHARED_DM=regs) */
+#define DKS_SOLVE_NONE 0
+#define DKS_SOLVE_FUSED 1
+#define DKS_SOLVE_PMAT 2         /* wls_pmat_kernel */
+#define DKS_SOLVE_WLS_SHARED 3   /* wls_shared_kernel */
+#define DKS_SOLVE_WIDE 4         /* more than 128 groups: float64 projection product (dks_wide.cuh) */
+#define DKS_SOLVE_L1 5           /* l1 feature selection + restricted WLS */
+#define DKS_GENERAL_NONE 0
+#define DKS_GENERAL_TC 1         /* explain_wgmma_kernel */
+#define DKS_GENERAL_SIMT 2       /* explain_simt_kernel */
+#define DKS_GENERAL_FLAGGED 3    /* not computed: instances left for it are reported as DKS_ERR_UNSUPPORTED */
+int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
 int dks_last_timings(dks_ctx* ctx, float* ms3);
