@@ -315,7 +315,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         ctx->launches += 1;
         path[DKS_PATH_SHARED] = DKS_SHARED_FUSED; path[DKS_PATH_CHUNKS] = 1; path[DKS_PATH_WARPS] = fcfg.warps;
         path[DKS_PATH_GRID] = ctx->sm_count; path[DKS_PATH_FUSED_B] = fcfg.B; path[DKS_PATH_FUSED_NI] = fcfg.ni;
-        path[DKS_PATH_SOLVE] = DKS_SOLVE_FUSED;
+        path[DKS_PATH_SOLVE] = DKS_SOLVE_FUSED; path[DKS_PATH_FUSED_CTA_WARPS] = fcfg.slices * fcfg.kw;
         CUDA_TRY(cudaGetLastError());
         p.list = ctx->d_idx_other;
         p.count = ctx->d_counts + 1;

@@ -6,15 +6,19 @@
 // shared plan (float64, the warp's 32 rows of it resident in shared memory).  The sum over s runs across the lanes of a warp
 // (lane = coalition row), so instead of shuffling per instance the warp parks y for a batch of B instances in shared
 // memory ([row][instance], conflict-free both ways) and then turns the tile around: lane = instance, loop over its 32
-// rows with P broadcast from shared memory -- 12 DFMA + 7 shared loads per (instance, row group) on the otherwise idle
-// FP64 pipe, no shuffles.  Each warp adds its partial beta to a per-instance accumulator in 2^-40 FIXED POINT with 64-bit
-// integer atomics (exact and order-independent: results are bit-reproducible whatever the scheduling), and the warp that
-// delivers the last of the S/32 partials of an instance (a per-instance counter) applies the delta term, back-fills the
-// eliminated group, snaps |phi| < 1e-10 and writes phi for both classes (and, on a multi-GPU run, stores them into every
-// peer's gathered buffer over NVLink).  It also resets the accumulator and the counter, so the next launch needs no memset.
+// rows with P broadcast from shared memory, four lanes per instance and KPAD / 4 coefficients per lane (every lane busy on
+// the otherwise idle FP64 pipe, no shuffles).  Each warp adds its partial beta to a per-instance accumulator in 2^-40 FIXED
+// POINT with relaxed 64-bit integer reductions (exact and order-independent: results are bit-reproducible whatever the
+// scheduling), then publishes the delivery with a release add on a per-instance counter; the warp that delivers the last of
+// the S/32 partials of an instance takes an acquire fence, applies the delta term, back-fills the eliminated group, snaps
+// |phi| < 1e-10 and writes phi for both classes (and, on a multi-GPU run, stores them into every peer's gathered buffer over
+// NVLink).  It also resets the accumulator and the counter, so the next launch needs no memset.
 //
-// The warp's 32 rows of Dm (pair sums and pair products) sit in its slice of shared memory, as in
-// explain_shared_smem_kernel.  NI = 1 or 2 instances share one pass over them (one load feeds both).
+// A CTA holds `slices` row groups: each slice is the group's 32 rows of Dm (pair sums and pair products, as in
+// explain_shared_smem_kernel) and of P.  kw warps share a slice and stream disjoint subsets of the instances through it,
+// each with its own staging tile.  kw = 1 is one slice per warp, which fits the most row groups into a CTA (the largest
+// plans); kw > 1 runs more warps per SM than slices of their own would fit.  NI = 1 or 2 instances share one pass over the
+// slice (one load feeds both).
 #pragma once
 
 #include "dks_shared.cuh"
@@ -84,53 +88,72 @@ __device__ __noinline__ void peer_push_finished(const double* __restrict__ phi, 
     }
 }
 
-inline size_t fused_smem_bytes(int warps, int kpad, int B, int N) {
-    return (size_t)warps * dm_slice_bytes(N) + (size_t)warps * 32 * kpad * sizeof(double) +
-           (size_t)warps * 32 * (B + 1) * sizeof(double) + DKS_LOGTAB_SIZE * sizeof(LogTabEntry);
+// every row group has delivered instance i: phi of both classes from its accumulator (read from L2), then the accumulator
+// and the counter reset for the next launch
+template <int KPAD>
+__device__ __forceinline__ void finish_instance(const FusedParams& p, int i, int nA, size_t slab) {
+    long long* acc = p.acc + (size_t)i * KPAD;
+    const double delta = p.dlink[(size_t)i * p.C + 1];
+    double sum = 0.0;
+    double* phi1 = p.phi + slab + (size_t)i * p.G;
+    double* phi0 = p.phi + (size_t)i * p.G;
+    for (int k = 0; k < nA; ++k) {
+        double val = from_fix(__ldcg(acc + k)) - delta * p.dvec[k];
+        sum += val;
+        if (fabs(val) < 1e-10) val = 0.0;
+        phi1[k] = val;
+        phi0[k] = (val == 0.0) ? 0.0 : -val;
+        acc[k] = 0;
+    }
+    double last = delta - sum;                  // the eliminated (last) group takes the remainder
+    if (fabs(last) < 1e-10) last = 0.0;
+    phi1[nA] = last;
+    phi0[nA] = (last == 0.0) ? 0.0 : -last;
+    p.done[i] = 0;
+}
+
+inline size_t fused_smem_bytes(int slices, int kw, int kpad, int B, int N) {
+    return (size_t)slices * dm_slice_bytes(N) + (size_t)slices * 32 * kpad * sizeof(double) +
+           (size_t)slices * kw * 32 * (B + 1) * sizeof(double) + DKS_LOGTAB_SIZE * sizeof(LogTabEntry);
 }
 
 // NCT: background rows at compile time (0 = run-time p.N): with NCT the chunk loop unrolls completely (static shared-memory
-// offsets, no loop control, the tail folded).  B (instances parked per warp) is a power of two.
+// offsets, no loop control, the tail folded).  B (instances parked per warp) is a power of two.  Warp w of a CTA works on
+// slice w / kw; warps from slices * kw on idle.
 template <int NCT, int KPAD, int NWARPS, int NI>
-__global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(FusedParams p, int warps_used) {
+__global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(FusedParams p, int slices, int kw) {
     extern __shared__ __align__(16) unsigned char fsm[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int slice = warp / kw, sub = warp - slice * kw;
     const int B = p.B, ystride = B + 1;
     const int nq = dm_quads(NCT ? NCT : p.N);
-    float4* sDm = reinterpret_cast<float4*>(fsm);                                // [warps_used][nq][32]
-    double* sP = reinterpret_cast<double*>(sDm + (size_t)warps_used * nq * 32);  // [warps_used][32][KPAD]
-    double* sY = sP + (size_t)warps_used * 32 * KPAD;                            // [warps_used][32][B + 1]
-    LogTabEntry* s_logtab = reinterpret_cast<LogTabEntry*>(sY + (size_t)warps_used * 32 * ystride);
+    float4* sDm = reinterpret_cast<float4*>(fsm);                                // [slices][nq][32]
+    double* sP = reinterpret_cast<double*>(sDm + (size_t)slices * nq * 32);      // [slices][32][KPAD]
+    double* sY = sP + (size_t)slices * 32 * KPAD;                                // [slices * kw][32][B + 1]
+    LogTabEntry* s_logtab = reinterpret_cast<LogTabEntry*>(sY + (size_t)slices * kw * 32 * ystride);
     if (threadIdx.x >= 64 && threadIdx.x < 64 + DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x - 64);
 
+    constexpr int MAXCH = MAXN / 16;
+    const int N = NCT ? NCT : p.N;
+    const int nfull = N / 16, ntail = N - nfull * 16;
+    const int nch = nfull + (ntail > 0 ? 1 : 0);
     const int n_rg = p.S_pad / 32;                       // row groups
-    const int total_warps = gridDim.x * warps_used;
-    const int nparts = total_warps / n_rg;               // replicas of every row group (>= 1: checked by the host)
-    const int gw = blockIdx.x * warps_used + warp;
-    const bool active = warp < warps_used && gw < nparts * n_rg;
-    const int rg = active ? gw % n_rg : 0, part = active ? gw / n_rg : 0;
-    double* sPw = sP + (size_t)warp * 32 * KPAD;
+    const int nparts = gridDim.x * slices / n_rg;        // replicas of every row group (>= 1: checked by the host)
+    const int gs = blockIdx.x * slices + slice;
+    const bool active = slice < slices && gs < nparts * n_rg;
+    const int rg = active ? gs % n_rg : 0, part = active ? gs / n_rg : 0;
+    const int s = rg * 32 + lane;
+    double* sPw = sP + (size_t)slice * 32 * KPAD;
     double* sYw = sY + (size_t)warp * 32 * ystride;
+    float4* sl = sDm + (size_t)slice * nq * 32;          // this warp's slice
     if (active) {
-        const double* src = p.pmat64 + (size_t)rg * 32 * KPAD;     // the warp's 32 rows are contiguous
-        for (int idx = lane; idx < 32 * KPAD; idx += 32) sPw[idx] = src[idx];
-    }
-    __syncthreads();
-
-    if (active) {
-        constexpr int MAXCH = MAXN / 16;
-        const int s = rg * 32 + lane;
-        const int cnt = *p.count;
-        const int N = NCT ? NCT : p.N, G = p.G, nA = G - 1;
-        const int nfull = N / 16, ntail = N - nfull * 16;
-        const int nq_t = ntail >> 2, rem_t = ntail & 3;
-        const int nch = nfull + (ntail > 0 ? 1 : 0);
-        float4* sl = sDm + (size_t)warp * nq * 32;          // this warp's slice
-        const double es = p.dme[s];
-        // ---- this warp's 32 rows of Dm into its slice: pair sums and pair products per quad of columns (0,2) (1,3)
+        // ---- the slice's 32 rows of P and of Dm, split over its kw warps; Dm as pair sums and pair products per quad of
+        // columns (0,2) (1,3)
+        const double* src = p.pmat64 + (size_t)rg * 32 * KPAD;     // the slice's 32 rows are contiguous
+        for (int idx = sub * 32 + lane; idx < 32 * KPAD; idx += 32 * kw) sPw[idx] = src[idx];
 #pragma unroll
         for (int c = 0; c < MAXCH; ++c) {
-            if (c < nch) {
+            if (c < nch && c % kw == sub) {
                 float v[16];
 #pragma unroll
                 for (int jj = 0; jj < 16; ++jj) {
@@ -148,65 +171,67 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                 dm_st16(sl, c, nq, lane, v);
             }
         }
+    }
+    __syncthreads();
 
+    if (active) {
+        const int cnt = *p.count;
+        const int G = p.G, nA = G - 1;
+        const int nq_t = ntail >> 2, rem_t = ntail & 3;
+        const double es = p.dme[s];
         const uint64_t zz = s < p.S ? p.z[s] : 0ull;
         const int ntab = (G + 3) / 4;                     // <= 4 (the host sends wider problems down the unfused path)
         const f32x2 one2 = f2_pack(1.f, 1.f), two2 = f2_pack(2.f, 2.f);
-        const double lf1 = p.linkfnull[1], f1 = p.fnull[1], inv_n = 1.0 / (double)N;
+        const double yf = p.link == DKS_LINK_LOGIT ? p.linkfnull[1] : p.fnull[1], inv_n = 1.0 / (double)N;   // link(fnull)
         const size_t slab = (size_t)p.n * G;
-        const int my_n = part < cnt ? (cnt - part + nparts - 1) / nparts : 0;     // instances this warp streams
+        // instances of this warp: ordinals first, first + stride, ... of the list (the part's instances dealt round-robin
+        // over the slice's kw warps)
+        const int first = part + sub * nparts, stride = nparts * kw;
+        const int my_n = first < cnt ? (cnt - first + stride - 1) / stride : 0;
         const bool row_ok = s < p.S;
         const int bmask = B - 1;
 
-        // ---- the turn-around: lane = instance of the batch, loop over the warp's 32 rows
+        // ---- the turn-around: four lanes per instance of the batch (eight instances per round), lane q of an instance owns
+        // coefficients q, q + 4, ...; each sums the warp's 32 rows in order sr = 0 .. 31
         auto flush = [&](int bstart, int bcount) {
-            int fin_i = -1;                 // instance this lane finished in this flush (its phi is complete in local memory)
-            if (lane < bcount) {
-                double beta[KPAD];
+            constexpr int KPL = KPAD / 4;
+            const int q = lane & 3;
+            for (int b0 = 0; b0 < bcount; b0 += 8) {
+                const int b = b0 + (lane >> 2);
+                const bool mine = b < bcount;
+                int i = 0;
+                int fin_i = -1;             // instance this lane finished in this round (its phi is complete in local memory)
+                if (mine) {
+                    double beta[KPL];
 #pragma unroll
-                for (int k = 0; k < KPAD; ++k) beta[k] = 0.0;
+                    for (int j = 0; j < KPL; ++j) beta[j] = 0.0;
 #pragma unroll 4
-                for (int sr = 0; sr < 32; ++sr) {
-                    const double y = sYw[sr * ystride + lane];
-                    const double2* pr = reinterpret_cast<const double2*>(sPw + sr * KPAD);
+                    for (int sr = 0; sr < 32; ++sr) {
+                        const double y = sYw[sr * ystride + b];
 #pragma unroll
-                    for (int k2 = 0; k2 < KPAD / 2; ++k2) {
-                        const double2 pp = pr[k2];
-                        beta[2 * k2] = fma(pp.x, y, beta[2 * k2]);
-                        beta[2 * k2 + 1] = fma(pp.y, y, beta[2 * k2 + 1]);
+                        for (int j = 0; j < KPL; ++j) beta[j] = fma(sPw[sr * KPAD + q + 4 * j], y, beta[j]);
+                    }
+                    i = p.list[first + (bstart + b) * stride];
+                    long long* acc = p.acc + (size_t)i * KPAD;
+#pragma unroll
+                    for (int j = 0; j < KPL; ++j)
+                        if (q + 4 * j < nA)
+                            asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(acc + q + 4 * j),
+                                         "l"((unsigned long long)to_fix(beta[j])) : "memory");
+                }
+                __syncwarp();               // the instance's four lanes have added: its first lane publishes the delivery
+                if (mine && q == 0) {
+                    int old;
+                    asm volatile("atom.release.gpu.global.add.s32 %0, [%1], 1;" : "=r"(old) : "l"(p.done + i) : "memory");
+                    if (old == n_rg - 1) {
+                        // every row group has delivered: finish the instance
+                        asm volatile("fence.acq_rel.gpu;" ::: "memory");
+                        finish_instance<KPAD>(p, i, nA, slab);
+                        fin_i = i;
                     }
                 }
-                const int i = p.list[part + (bstart + lane) * nparts];
-                long long* acc = p.acc + (size_t)i * KPAD;
-#pragma unroll
-                for (int k = 0; k < KPAD; ++k)
-                    if (k < nA) atomicAdd(reinterpret_cast<unsigned long long*>(acc + k), (unsigned long long)to_fix(beta[k]));
-                __threadfence();
-                const int old = atomicAdd(p.done + i, 1);
-                if (old == n_rg - 1) {
-                    // every row group has delivered: finish the instance
-                    __threadfence();
-                    const double delta = p.dlink[(size_t)i * p.C + 1];
-                    double sum = 0.0;
-                    double* phi1 = p.phi + slab + (size_t)i * G;
-                    double* phi0 = p.phi + (size_t)i * G;
-                    for (int k = 0; k < nA; ++k) {
-                        double val = from_fix(__ldcg(acc + k)) - delta * p.dvec[k];
-                        sum += val;
-                        if (fabs(val) < 1e-10) val = 0.0;
-                        phi1[k] = val;
-                        phi0[k] = (val == 0.0) ? 0.0 : -val;
-                        acc[k] = 0;
-                    }
-                    double last = delta - sum;                  // the eliminated (last) group takes the remainder
-                    if (fabs(last) < 1e-10) last = 0.0;
-                    phi1[nA] = last;
-                    phi0[nA] = (last == 0.0) ? 0.0 : -last;
-                    p.done[i] = 0;
-                    fin_i = i;
-                }
+                if (p.npeers > 0) peer_push_finished(p.phi, p.peer_phi, p.npeers, fin_i, lane, G, slab);     // multi-GPU only (kept out of line: no registers here)
             }
-            if (p.npeers > 0) peer_push_finished(p.phi, p.peer_phi, p.npeers, fin_i, lane, G, slab);     // multi-GPU only (kept out of line: no registers here)
         };
 
         // a(i, s) = sum over the row's nibbles of one table entry each; the entries of the NEXT instance are loaded one
@@ -225,10 +250,10 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
 #pragma unroll
         for (int u = 0; u < NI; ++u) {
             const int o0 = u < last_it ? u : last_it, o1 = NI + u < last_it ? NI + u : last_it;
-            i_nx[u] = my_n > 0 ? p.list[part + o1 * nparts] : 0;
+            i_nx[u] = my_n > 0 ? p.list[first + o1 * stride] : 0;
             nx[u][0] = nx[u][1] = nx[u][2] = nx[u][3] = 0.0;
             if (my_n > 0) {
-                const size_t o = (size_t)p.list[part + o0 * nparts] * xstride;
+                const size_t o = (size_t)p.list[first + o0 * stride] * xstride;
                 nx[u][0] = __ldg(xb0 + o); nx[u][1] = __ldg(xb1 + o); nx[u][2] = __ldg(xb2 + o); nx[u][3] = __ldg(xb3 + o);
             }
         }
@@ -243,7 +268,7 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                     const size_t o = (size_t)i_nx[u] * xstride;
                     nx[u][0] = __ldg(xb0 + o); nx[u][1] = __ldg(xb1 + o); nx[u][2] = __ldg(xb2 + o); nx[u][3] = __ldg(xb3 + o);
                     const int it2 = it + 2 * NI + u < last_it ? it + 2 * NI + u : last_it;
-                    i_nx[u] = p.list[part + it2 * nparts];
+                    i_nx[u] = p.list[first + it2 * stride];
                 }
                 // A = 2^a = 2^n 2^f, n = rint(a) through the 1.5 * 2^52 trick (no conversion instructions), |f| <= 1/2; the
                 // exponent is clamped to [-120, 120] (saturated scores; the clamped scalar path below takes A > 1e18)
@@ -303,8 +328,8 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                 if (it + u < my_n) {
                     double y = 0.0;
                     if (row_ok) {
-                        if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(s1[u], s0[u], s_logtab) - lf1;
-                        else y = (double)s1[u] * inv_n - f1;
+                        if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(s1[u], s0[u], s_logtab) - yf;
+                        else y = (double)s1[u] * inv_n - yf;
                     }
                     sYw[lane * ystride + ((it + u) & bmask)] = y;
                 }
@@ -355,19 +380,28 @@ __global__ void plan_dvec64_kernel(const uint64_t* __restrict__ z, const double*
 
 inline int fused_kpad(int G) { return G - 1 <= 12 ? 12 : 16; }
 
-struct FusedConfig { int ni, warps, B; size_t smem; };
+// slices: row groups per CTA; kw: warps per slice; warps: the slices a CTA holds at kw = 1 (the most row groups the fused
+// kernel covers per CTA: the fused / unfused boundary is S_pad / 32 <= sm_count * warps)
+struct FusedConfig { int ni, warps, slices, kw, B; size_t smem; };
 
-// picks (warps per CTA, batch) for a shape; returns false when the fused kernel does not apply.
-// want_warps / want_B: 0 = default (tuning knobs, dks_set_option)
+// warps per CTA with kw > 1.  24 warps of 32 lanes fill the SM's register file at 80 registers per thread, which the
+// kernel fits without spilling only with the background size compiled in (NCT = 100, or 128 with 12 coefficients) and one
+// instance per pass; the other shapes take at most 16 warps (up to 128 registers)
+inline int fused_max_cta_warps(int N, int kpad, int ni) {
+    return ni == 1 && (N == 100 || (N == 128 && kpad == 12)) ? 24 : 16;
+}
+
+// picks the layout (slices, warps per slice) and the batch for a shape; returns false when the fused kernel does not apply.
+// want_warps (warps per CTA) / want_B: 0 = default (tuning knobs, dks_set_option)
 inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, int want_ni, int want_warps, int want_B,
                          FusedConfig* cfg) {
     if (G < 2 || G > 16 || N > MAXN) return false;                        // at most four nibble tables, 15 coefficients
     const int kpad = fused_kpad(G);
-    // warps per CTA: as many as the shared memory holds (each brings its slice of Dm, its rows of P and its staging
-    // tile), at most 20.  B = 16 unless B = 8 buys more warps.
+    // kw = 1: as many slices as the shared memory holds (each brings its rows of Dm and P and one warp's staging tile), at
+    // most 20.  B = 16 unless B = 8 buys more warps.
     auto max_warps = [&](int b) {
         int w = 20;
-        while (w > 0 && fused_smem_bytes(w, kpad, b, N) + 1024 > (size_t)max_smem) --w;
+        while (w > 0 && fused_smem_bytes(w, 1, kpad, b, N) + 1024 > (size_t)max_smem) --w;
         return w;
     };
     int B = 16;
@@ -376,10 +410,23 @@ inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, in
     if (want_B == 0 && max_warps(8) > warps) { B = 8; warps = max_warps(8); }
     if (want_warps > 0 && want_warps < warps) warps = want_warps;
     if (warps < 1) return false;
-    if ((long long)sm_count * warps < S_pad / 32) return false;          // every row group needs a warp
-    cfg->ni = (want_ni == 2 && fused_kpad(G) == 12) ? 2 : 1;          // two instances per pass over Dm (tuning knob)
-    cfg->warps = warps; cfg->B = B;
-    cfg->smem = fused_smem_bytes(warps, kpad, B, N);
+    const int n_rg = S_pad / 32;
+    if ((long long)sm_count * warps < n_rg) return false;                // every row group needs a slice
+    const int ni = (want_ni == 2 && kpad == 12) ? 2 : 1;                // two instances per pass over Dm (tuning knob)
+    // kw > 1: R slices of floor(cap / R) warps each, where that keeps more warps streaming than kw = 1 does (replicas of
+    // every row group: floor(sm_count * R / n_rg); the slices beyond them idle)
+    auto busy = [&](int R, int K) { return (long long)K * ((long long)sm_count * R / n_rg) * n_rg; };
+    const int max_cta = fused_max_cta_warps(N, kpad, ni);
+    const int cap = want_warps > 0 && want_warps < max_cta ? want_warps : max_cta;
+    int slices = warps, kw = 1;
+    for (int R = 1; R <= warps && cap / R >= 2; ++R) {
+        const int K = cap / R;
+        if ((long long)sm_count * R < n_rg || fused_smem_bytes(R, K, kpad, B, N) + 1024 > (size_t)max_smem) continue;
+        if (busy(R, K) > busy(slices, kw)) { slices = R; kw = K; }
+    }
+    cfg->ni = ni;
+    cfg->warps = warps; cfg->slices = slices; cfg->kw = kw; cfg->B = B;
+    cfg->smem = fused_smem_bytes(slices, kw, kpad, B, N);
     return true;
 }
 
@@ -391,29 +438,37 @@ inline cudaError_t launch_explain_fused(const FusedParams& p, const FusedConfig&
         err = cudaFuncSetAttribute(explain_shared_fused_kernel<NCT, KP, NW, NI>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                    (int)cfg.smem);                                                                    \
         if (err == cudaSuccess)                                                                                       \
-            explain_shared_fused_kernel<NCT, KP, NW, NI><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.warps);          \
+            explain_shared_fused_kernel<NCT, KP, NW, NI><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.slices, cfg.kw); \
     } while (0)
     // background sizes with a compile-time specialisation (the chunk loop unrolls completely); everything else takes the
-    // run-time version.  Block size: the smallest of 12 / 16 / 20 warps that holds cfg.warps.
-    const int nw = cfg.warps > 16 ? 20 : (cfg.warps > 12 ? 16 : 12);
+    // run-time version.  Block size: the smallest of 12 / 16 / 20 / 24 warps that holds slices x kw (24 only where
+    // fused_max_cta_warps allows it).
+    const int cta_warps = cfg.slices * cfg.kw;
+    const int nw = cta_warps > 20 ? 24 : (cta_warps > 16 ? 20 : (cta_warps > 12 ? 16 : 12));
 #define DKS_FUSED_NW(NCT, KP, NI)                                                                                     \
     do {                                                                                                              \
         if (nw == 12) DKS_FUSED_LAUNCH(NCT, KP, 12, NI);                                                              \
         else if (nw == 16) DKS_FUSED_LAUNCH(NCT, KP, 16, NI);                                                         \
         else DKS_FUSED_LAUNCH(NCT, KP, 20, NI);                                                                       \
     } while (0)
+#define DKS_FUSED_NW24(NCT, KP, NI)                                                                                   \
+    do {                                                                                                              \
+        if (nw == 24) DKS_FUSED_LAUNCH(NCT, KP, 24, NI);                                                              \
+        else DKS_FUSED_NW(NCT, KP, NI);                                                                               \
+    } while (0)
     if (kpad == 12 && cfg.ni == 2) {
         if (p.N == 100) DKS_FUSED_NW(100, 12, 2);
         else DKS_FUSED_NW(0, 12, 2);
     } else if (kpad == 12) {
-        if (p.N == 100) DKS_FUSED_NW(100, 12, 1);
-        else if (p.N == 128) DKS_FUSED_NW(128, 12, 1);
+        if (p.N == 100) DKS_FUSED_NW24(100, 12, 1);
+        else if (p.N == 128) DKS_FUSED_NW24(128, 12, 1);
         else if (p.N == 64) DKS_FUSED_NW(64, 12, 1);
         else DKS_FUSED_NW(0, 12, 1);
     } else {
-        if (p.N == 100) DKS_FUSED_NW(100, 16, 1);
+        if (p.N == 100) DKS_FUSED_NW24(100, 16, 1);
         else DKS_FUSED_NW(0, 16, 1);
     }
+#undef DKS_FUSED_NW24
 #undef DKS_FUSED_NW
 #undef DKS_FUSED_LAUNCH
     return err;

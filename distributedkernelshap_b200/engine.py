@@ -557,15 +557,17 @@ class GpuKernelExplainer:
         """Which kernels the last explain call launched (``dks_last_path``), recorded when the call was enqueued (a
         replayed CUDA graph reports the call it captured): ``shared`` (shared-plan coalition kernel: 'none' | 'fused' |
         'smem' | 'regs'), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
-        ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``
-        and ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
-        are reported as unsupported, not computed)."""
-        out = np.zeros(9, dtype=np.int32)
+        ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
+        ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
+        are reported as unsupported, not computed) and ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
+        row-group slices at one warp each, or fewer slices shared by several warps each)."""
+        out = np.zeros(10, dtype=np.int32)
         _cabi.check(self.lib.dks_last_path(self._ctx, _cabi.ptr(out), len(out)))
         names = self._PATH_NAMES
         return {"shared": names["shared"][out[0]], "chunks": int(out[1]), "warps": int(out[2]), "grid": int(out[3]),
                 "fused_B": int(out[4]), "fused_NI": int(out[5]), "solve": names["solve"][out[6]],
-                "pmat_kpad": int(out[7]), "general": names["general"][out[8]]}
+                "pmat_kpad": int(out[7]), "general": names["general"][out[8]],
+                "cta_warps": int(out[9])}
 
     def debug_scores(self, X, instance, nsamples="auto"):
         """Raw accumulator tile of the tensor-core kernel for one instance: float32 [S_cap, Npad] of scaled masked scores

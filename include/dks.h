@@ -194,7 +194,8 @@ int dks_summarise_host(dks_ctx* ctx, int n, const int32_t* seg_offsets_host, int
 int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
 /* tuning knobs, all optional (defaults are the measured best): "fused" 0/1 -- link + projection solve inside the shared-plan
  * coalition kernel (default 1; 0 = separate (sum p1, sum p0) buffer + solve kernel); "fused_ni" 1/2 instances per pass over
- * a warp's rows; "fused_warps" 16/20 warps per CTA; "fused_batch" instances parked per warp before the turn-around;
+ * a warp's rows; "fused_warps" caps the warps per CTA (default: as many as fit, at most 24); "fused_batch" instances
+ * parked per warp before the turn-around;
  * "push_in_kernel" 0/1 -- multi-GPU: the fused kernel's epilogue stores phi into the peers' buffers itself instead of the
  * separate push kernel (default 0: measured slower, it stalls the finishing warps); "graph" 0/1 (CUDA-graph
  * replay of dks_run_dev); "graph_timing" 0/1 -- keep the timing event records inside the graph (default 0: a replayed graph
@@ -216,7 +217,10 @@ int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by th
 #define DKS_PATH_SOLVE 6         /* DKS_SOLVE_* */
 #define DKS_PATH_PMAT_KPAD 7     /* projection solve (DKS_SOLVE_PMAT): coefficient rows of P, padded */
 #define DKS_PATH_GENERAL 8       /* DKS_GENERAL_*: the kernel of the instances the shared-plan path does not take */
-#define DKS_PATH_FIELDS 9
+#define DKS_PATH_FUSED_CTA_WARPS 9 /* fused kernel: warps per CTA it runs.  DKS_PATH_WARPS is the row-group slices a CTA
+                                    * holds with one warp per slice (what decides fused or not); when fewer slices cover the
+                                    * plan, several warps share each slice and this is larger */
+#define DKS_PATH_FIELDS 10
 #define DKS_SHARED_NONE 0
 #define DKS_SHARED_FUSED 1       /* explain_shared_fused_kernel: link + projection solve inside */
 #define DKS_SHARED_SMEM 2        /* explain_shared_smem_kernel (Dm rows in shared memory) */
