@@ -255,10 +255,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     const int G = ctx->G;
     const PlanDev& pg = ctx->h_plans[G <= DKS_MAX_GROUPS ? G : 0];
     const bool fast = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
-                      ctx->act == DKS_ACT_BINARY_LOGISTIC && ctx->uniform_w && G >= 2 && pg.dmT != nullptr &&
+                      ctx->act == DKS_ACT_BINARY_LOGISTIC && G >= 2 && pg.dmT != nullptr &&
                       pg.S == dks_effective_S(G, ctx->nsamples_req) && (pg.W <= 2 || pg.ptw != nullptr);
     if (kernel == DKS_KERNEL_SHARED && !fast && ext_z == nullptr && pg.z != nullptr)
-        return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head and uniform background weights");
+        return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head");
+    // non-uniform background weights: the weighted instantiations of the shared-plan kernels (dks_shared.cuh)
+    const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn;
+    if (fast) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
     // the general kernel below (instances that are not on the shared-plan path) forks off here and joins at the end
     cudaStream_t gstream = ctx->stream;
     if (fast && ctx->side_stream != nullptr) {
@@ -280,12 +283,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if (pg.W > 2)
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
         if (!fast || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic head, uniform "
-                        "background weights) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic head) and the "
+                        "l1 tables of the M=%d plan (dks_set_l1_tables)", G);
     }
     const bool fused = fast && !l1 && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
                        dks::shared_path::fused_config(ctx->N, G, pg.S_pad, ctx->sm_count, ctx->max_smem_optin,
-                                                      ctx->opt_fused_ni, ctx->opt_fused_warps, ctx->opt_fused_B, &fcfg);
+                                                      ctx->opt_fused_ni, ctx->opt_fused_warps, ctx->opt_fused_B, &fcfg,
+                                                      wn != nullptr);
     ctx->last_fused = fused;
     if (fused) {
         // link + projection solve inside the coalition kernel: no (sum p1, sum p0) buffer, no separate solve launch
@@ -295,6 +299,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         fp.scale = ctx->scale; fp.DmT = pg.dmT; fp.dme = pg.dme; fp.z = pg.z; fp.XT = ctx->d_XT; fp.list = ctx->d_idx_full;
         fp.count = ctx->d_counts; fp.pmat64 = pg.pmat64; fp.dvec = pg.dvec64; fp.dlink = ctx->d_dlink;
         fp.linkfnull = ctx->d_linkfnull; fp.fnull = ctx->d_fnull; fp.acc = ctx->d_acc; fp.done = ctx->d_done; fp.phi = phi_dev;
+        fp.wn = wn;
         if (ctx->peer_world > 1 && ctx->push_in_kernel) {
             double* slabs[16];
             int np = 0;
@@ -326,7 +331,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         dks::shared_path::SharedParams sp;
         sp.n = n; sp.N = ctx->N; sp.G = G; sp.S = S; sp.S_pad = S_pad; sp.scale = ctx->scale;
         sp.DmT = pg.dmT; sp.dme = pg.dme; sp.z = pg.z; sp.XT = ctx->d_XT; sp.list = ctx->d_idx_full; sp.count = ctx->d_counts; sp.sums = ctx->d_sums; sp.accumulate = 0;
-        sp.acache = nullptr; sp.acache_mode = 0;
+        sp.acache = nullptr; sp.acache_mode = 0; sp.wn = wn;
         if (pg.W > 2 && ctx->opt_wide_acache && ctx->N > dks::shared_path::MAXN) {
             // sixteen-word rows, several background chunks: A(i, s) is computed by the first chunk's launch only
             if (need > ctx->cap_acache) { TRY(dev_alloc(&ctx->d_acache, need)); ctx->cap_acache = need; ctx->epoch++; }
@@ -447,8 +452,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
         }
         if (!fast)
-            return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, uniform "
-                        "background weights, kernel 'auto' or 'shared', shared plan of M=%d uploaded)", G);
+            return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, kernel "
+                        "'auto' or 'shared', shared plan of M=%d uploaded)", G);
         dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 1;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
@@ -579,7 +584,7 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
     dev_free(&ctx->d_fnull); dev_free(&ctx->d_linkfnull); dev_free(&ctx->d_BWs); dev_free(&ctx->d_bases);
-    dev_free(&ctx->d_wbf); dev_free(&ctx->d_plans); dev_free(&ctx->d_X); dev_free(&ctx->d_XW); dev_free(&ctx->d_XT);
+    dev_free(&ctx->d_wbf); dev_free(&ctx->d_wn); dev_free(&ctx->d_plans); dev_free(&ctx->d_X); dev_free(&ctx->d_XW); dev_free(&ctx->d_XT);
     dev_free(&ctx->d_vflag); dev_free(&ctx->d_vmask); dev_free(&ctx->d_M); dev_free(&ctx->d_dlink);
     dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_sums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
     dev_free(&ctx->d_status); ctx->d_hist = nullptr; ctx->d_counts = nullptr; dev_free(&ctx->d_yw); dev_free(&ctx->d_betaw); dev_free(&ctx->d_acache); dev_free(&ctx->d_phi); if (ctx->h_phi_pin) { cudaFreeHost(ctx->h_phi_pin); ctx->h_phi_pin = nullptr; } dev_free(&ctx->d_genz); dev_free(&ctx->d_genw); dev_free(&ctx->d_genchol); dev_free(&ctx->d_genainv); dev_free(&ctx->d_afix); dev_free(&ctx->d_sinfo); dev_free(&ctx->d_extz);
@@ -716,7 +721,14 @@ int dks_fit(dks_ctx* ctx) {
     TRY(dev_alloc(&ctx->d_BWs, (size_t)N * G * R));
     TRY(dev_alloc(&ctx->d_bases, (size_t)N * R));
     TRY(dev_alloc(&ctx->d_wbf, (size_t)N));
+    TRY(dev_alloc(&ctx->d_wn, (size_t)N));
     cudaStream_t st = ctx->stream;
+    {
+        // the weighted shared-plan kernels read w'_j = N w_j: their sums then have the magnitude of the uniform ones
+        std::vector<float> wn(N);
+        for (int j = 0; j < N; ++j) wn[j] = (float)((double)N * ctx->h_wbg[j]);
+        CUDA_TRY(cudaMemcpy(ctx->d_wn, wn.data(), sizeof(float) * N, cudaMemcpyHostToDevice));
+    }
     CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_W, ctx->h_W.data(), sizeof(double) * R * D, cudaMemcpyHostToDevice, st));

@@ -122,6 +122,7 @@ struct dks_ctx {
     int* d_colnan = nullptr;
     double *d_BW = nullptr, *d_scores = nullptr, *d_Bbar = nullptr, *d_fnull = nullptr, *d_linkfnull = nullptr;
     float *d_BWs = nullptr, *d_bases = nullptr, *d_wbf = nullptr;
+    float* d_wn = nullptr;      // [N] N w_j in float: the background weights the weighted shared-plan kernels read
     double scale = 1.0;
     std::vector<double> h_fnull, h_linkfnull;
 

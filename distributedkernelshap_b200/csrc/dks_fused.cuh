@@ -47,6 +47,7 @@ struct FusedParams {
     double* phi;             // [C][n][G]
     int npeers;              // multi-GPU push: phi of every finished instance also goes to these buffers ([C][n][G] each)
     double* const* peer_phi; // [npeers] device array of the peers' slab addresses (NULL on one GPU)
+    const float* wn;         // [N] weighted backgrounds: N w_j (the weighted instantiations only; dks_shared.cuh)
 };
 
 // one 16-column chunk whose valid columns are a run-time count: nq full quads (pair sums / products), then rem < 4 raw
@@ -112,26 +113,34 @@ __device__ __forceinline__ void finish_instance(const FusedParams& p, int i, int
     p.done[i] = 0;
 }
 
-inline size_t fused_smem_bytes(int slices, int kw, int kpad, int B, int N) {
-    return (size_t)slices * dm_slice_bytes(N) + (size_t)slices * 32 * kpad * sizeof(double) +
-           (size_t)slices * kw * 32 * (B + 1) * sizeof(double) + DKS_LOGTAB_SIZE * sizeof(LogTabEntry);
+// weighted: the weighted slice (twice the bytes) and the per-CTA W2 array of dks_shared.cuh
+inline size_t fused_smem_bytes(int slices, int kw, int kpad, int B, int N, bool weighted = false) {
+    return (size_t)slices * (weighted ? dm_slice_bytes_w(N) : dm_slice_bytes(N)) + (size_t)slices * 32 * kpad * sizeof(double) +
+           (size_t)slices * kw * 32 * (B + 1) * sizeof(double) + DKS_LOGTAB_SIZE * sizeof(LogTabEntry) +
+           (weighted ? sizeof(float2) * (size_t)dm_quads_w(N) : 0);
 }
 
 // NCT: background rows at compile time (0 = run-time p.N): with NCT the chunk loop unrolls completely (static shared-memory
 // offsets, no loop control, the tail folded).  B (instances parked per warp) is a power of two.  Warp w of a CTA works on
-// slice w / kw; warps from slices * kw on idle.
-template <int NCT, int KPAD, int NWARPS, int NI>
+// slice w / kw; warps from slices * kw on idle.  WT: weighted background (quad_acc_w, dks_shared.cuh).
+template <int NCT, int KPAD, int NWARPS, int NI, bool WT = false>
 __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(FusedParams p, int slices, int kw) {
     extern __shared__ __align__(16) unsigned char fsm[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int slice = warp / kw, sub = warp - slice * kw;
     const int B = p.B, ystride = B + 1;
     const int nq = dm_quads(NCT ? NCT : p.N);
-    float4* sDm = reinterpret_cast<float4*>(fsm);                                // [slices][nq][32]
-    double* sP = reinterpret_cast<double*>(sDm + (size_t)slices * nq * 32);      // [slices][32][KPAD]
+    const int nqw = dm_quads_w(NCT ? NCT : p.N);                                 // weighted: quads of the slice (even)
+    const int sq4 = WT ? 2 * nqw : nq;                                           // float4 per lane and slice
+    float4* sDm = reinterpret_cast<float4*>(fsm);                                // [slices][sq4][32]
+    double* sP = reinterpret_cast<double*>(sDm + (size_t)slices * sq4 * 32);     // [slices][32][KPAD]
     double* sY = sP + (size_t)slices * 32 * KPAD;                                // [slices * kw][32][B + 1]
     LogTabEntry* s_logtab = reinterpret_cast<LogTabEntry*>(sY + (size_t)slices * kw * 32 * ystride);
+    float2* sW2 = reinterpret_cast<float2*>(s_logtab + DKS_LOGTAB_SIZE);         // weighted: [nqw]
     if (threadIdx.x >= 64 && threadIdx.x < 64 + DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x - 64);
+    if constexpr (WT) {
+        for (int q = threadIdx.x; q < nqw; q += blockDim.x) sW2[q] = w2_quad(p.wn, NCT ? NCT : p.N, q);
+    }
 
     constexpr int MAXCH = MAXN / 16;
     const int N = NCT ? NCT : p.N;
@@ -145,15 +154,23 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
     const int s = rg * 32 + lane;
     double* sPw = sP + (size_t)slice * 32 * KPAD;
     double* sYw = sY + (size_t)warp * 32 * ystride;
-    float4* sl = sDm + (size_t)slice * nq * 32;          // this warp's slice
+    float4* sl = sDm + (size_t)slice * sq4 * 32;         // this warp's slice
     if (active) {
         // ---- the slice's 32 rows of P and of Dm, split over its kw warps; Dm as pair sums and pair products per quad of
         // columns (0,2) (1,3)
         const double* src = p.pmat64 + (size_t)rg * 32 * KPAD;     // the slice's 32 rows are contiguous
         for (int idx = sub * 32 + lane; idx < 32 * KPAD; idx += 32 * kw) sPw[idx] = src[idx];
+        if constexpr (WT) {
+            for (int q = sub; q < nqw; q += kw) {
+                float4 sq, xy;
+                dm_quad_w(p.DmT, p.wn, N, p.S_pad, s, q, sq, xy);
+                sl[(2 * q) * 32 + lane] = sq;
+                sl[(2 * q + 1) * 32 + lane] = xy;
+            }
+        }
 #pragma unroll
         for (int c = 0; c < MAXCH; ++c) {
-            if (c < nch && c % kw == sub) {
+            if (!WT && c < nch && c % kw == sub) {
                 float v[16];
 #pragma unroll
                 for (int jj = 0; jj < 16; ++jj) {
@@ -279,7 +296,44 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                 risky_l = risky_l || A[u] > 1.0e18f;
             }
             float s1[NI], s0[NI];
-            if (__any_sync(0xffffffffu, risky_l)) {
+            if constexpr (WT) {
+                if (__any_sync(0xffffffffu, risky_l)) {
+#pragma unroll
+                    for (int u = 0; u < NI; ++u) row_sums_clamped_w(p.DmT, p.wn, N, p.S_pad, s, A[u], s1[u], s0[u]);
+                } else {
+                    // every quad of the slice (all columns compiled in with NCT), two accumulator chains per instance
+                    f32x2 A2[NI], AA2[NI], acc1[NI][2], acc0[NI][2];
+#pragma unroll
+                    for (int u = 0; u < NI; ++u) {
+                        const float AA = A[u] * A[u];
+                        A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA);
+                        acc1[u][0] = acc1[u][1] = acc0[u][0] = acc0[u][1] = f2_pack(0.f, 0.f);
+                    }
+                    // quad q on accumulator chain h (a constant after unrolling: the accumulators stay in registers)
+                    auto quad = [&](int q, int h) {
+                        const float4 sq = sl[(2 * q) * 32 + lane], xy = sl[(2 * q + 1) * 32 + lane];
+                        const float2 w2 = sW2[q];
+#pragma unroll
+                        for (int u = 0; u < NI; ++u) quad_acc_w(A2[u], AA2[u], sq, xy, w2, one2, acc1[u][h], acc0[u][h]);
+                    };
+                    if (NCT) {
+#pragma unroll
+                        for (int q = 0; q < dm_quads(NCT); ++q) quad(q, q & 1);
+                    } else {
+                        // run-time N: the slice's even number of quads in pairs (a zero quad past an odd count adds 0)
+#pragma unroll 2
+                        for (int q = 0; q < nqw; q += 2) { quad(q, 0); quad(q + 1, 1); }
+                    }
+#pragma unroll
+                    for (int u = 0; u < NI; ++u) {
+                        float q0, q1, q2, q3;
+                        f2_unpack(f2_add(acc1[u][0], acc1[u][1]), q0, q1);
+                        f2_unpack(f2_add(acc0[u][0], acc0[u][1]), q2, q3);
+                        s1[u] = q0 + q1;
+                        s0[u] = q2 + q3;
+                    }
+                }
+            } else if (__any_sync(0xffffffffu, risky_l)) {
                 // A^2 would leave the fp32 range: clamped scalar path on the raw row from global memory (saturated scores)
 #pragma unroll
                 for (int u = 0; u < NI; ++u) {
@@ -387,21 +441,25 @@ struct FusedConfig { int ni, warps, slices, kw, B; size_t smem; };
 // warps per CTA with kw > 1.  24 warps of 32 lanes fill the SM's register file at 80 registers per thread, which the
 // kernel fits without spilling only with the background size compiled in (NCT = 100, or 128 with 12 coefficients) and one
 // instance per pass; the other shapes take at most 16 warps (up to 128 registers)
-inline int fused_max_cta_warps(int N, int kpad, int ni) {
+// Weighted backgrounds (one instance per pass only) take at most 20 warps with NCT = 100 / 128 and 16 elsewhere: at 24
+// warps (80 registers) the weighted kernel spills, at 20 (up to 102) it does not; their kw = 1 layouts hold at most 16
+// slices.
+inline int fused_max_cta_warps(int N, int kpad, int ni, bool weighted = false) {
+    if (weighted) return N == 100 || N == 128 ? 20 : 16;
     return ni == 1 && (N == 100 || (N == 128 && kpad == 12)) ? 24 : 16;
 }
 
 // picks the layout (slices, warps per slice) and the batch for a shape; returns false when the fused kernel does not apply.
 // want_warps (warps per CTA) / want_B: 0 = default (tuning knobs, dks_set_option)
 inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, int want_ni, int want_warps, int want_B,
-                         FusedConfig* cfg) {
+                         FusedConfig* cfg, bool weighted = false) {
     if (G < 2 || G > 16 || N > MAXN) return false;                        // at most four nibble tables, 15 coefficients
     const int kpad = fused_kpad(G);
     // kw = 1: as many slices as the shared memory holds (each brings its rows of Dm and P and one warp's staging tile), at
-    // most 20.  B = 16 unless B = 8 buys more warps.
+    // most 20 (weighted: 16).  B = 16 unless B = 8 buys more warps.
     auto max_warps = [&](int b) {
-        int w = 20;
-        while (w > 0 && fused_smem_bytes(w, 1, kpad, b, N) + 1024 > (size_t)max_smem) --w;
+        int w = weighted ? 16 : 20;
+        while (w > 0 && fused_smem_bytes(w, 1, kpad, b, N, weighted) + 1024 > (size_t)max_smem) --w;
         return w;
     };
     int B = 16;
@@ -412,21 +470,21 @@ inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, in
     if (warps < 1) return false;
     const int n_rg = S_pad / 32;
     if ((long long)sm_count * warps < n_rg) return false;                // every row group needs a slice
-    const int ni = (want_ni == 2 && kpad == 12) ? 2 : 1;                // two instances per pass over Dm (tuning knob)
+    const int ni = (want_ni == 2 && kpad == 12 && !weighted) ? 2 : 1;   // two instances per pass over Dm (tuning knob)
     // kw > 1: R slices of floor(cap / R) warps each, where that keeps more warps streaming than kw = 1 does (replicas of
     // every row group: floor(sm_count * R / n_rg); the slices beyond them idle)
     auto busy = [&](int R, int K) { return (long long)K * ((long long)sm_count * R / n_rg) * n_rg; };
-    const int max_cta = fused_max_cta_warps(N, kpad, ni);
+    const int max_cta = fused_max_cta_warps(N, kpad, ni, weighted);
     const int cap = want_warps > 0 && want_warps < max_cta ? want_warps : max_cta;
     int slices = warps, kw = 1;
     for (int R = 1; R <= warps && cap / R >= 2; ++R) {
         const int K = cap / R;
-        if ((long long)sm_count * R < n_rg || fused_smem_bytes(R, K, kpad, B, N) + 1024 > (size_t)max_smem) continue;
+        if ((long long)sm_count * R < n_rg || fused_smem_bytes(R, K, kpad, B, N, weighted) + 1024 > (size_t)max_smem) continue;
         if (busy(R, K) > busy(slices, kw)) { slices = R; kw = K; }
     }
     cfg->ni = ni;
     cfg->warps = warps; cfg->slices = slices; cfg->kw = kw; cfg->B = B;
-    cfg->smem = fused_smem_bytes(slices, kw, kpad, B, N);
+    cfg->smem = fused_smem_bytes(slices, kw, kpad, B, N, weighted);
     return true;
 }
 
@@ -444,6 +502,40 @@ inline cudaError_t launch_explain_fused(const FusedParams& p, const FusedConfig&
     // run-time version.  Block size: the smallest of 12 / 16 / 20 / 24 warps that holds slices x kw (24 only where
     // fused_max_cta_warps allows it).
     const int cta_warps = cfg.slices * cfg.kw;
+    if (p.wn != nullptr) {
+        // weighted background: one instance per pass, 12 / 16 / 20 warps (20 only where fused_max_cta_warps allows it)
+#define DKS_FUSED_LAUNCH_WT(NCT, KP, NW)                                                                              \
+    do {                                                                                                              \
+        err = cudaFuncSetAttribute(explain_shared_fused_kernel<NCT, KP, NW, 1, true>,                                 \
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smem);                       \
+        if (err == cudaSuccess)                                                                                       \
+            explain_shared_fused_kernel<NCT, KP, NW, 1, true><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.slices, cfg.kw); \
+    } while (0)
+#define DKS_FUSED_WT(NCT, KP)                                                                                         \
+    do {                                                                                                              \
+        if (cta_warps > 16) DKS_FUSED_LAUNCH_WT(NCT, KP, 20);                                                         \
+        else if (cta_warps > 12) DKS_FUSED_LAUNCH_WT(NCT, KP, 16);                                                    \
+        else DKS_FUSED_LAUNCH_WT(NCT, KP, 12);                                                                        \
+    } while (0)
+#define DKS_FUSED_WT16(NCT, KP)                                                                                       \
+    do {                                                                                                              \
+        if (cta_warps > 12) DKS_FUSED_LAUNCH_WT(NCT, KP, 16);                                                         \
+        else DKS_FUSED_LAUNCH_WT(NCT, KP, 12);                                                                        \
+    } while (0)
+        if (kpad == 12) {
+            if (p.N == 100) DKS_FUSED_WT(100, 12);
+            else if (p.N == 128) DKS_FUSED_WT(128, 12);
+            else DKS_FUSED_WT16(0, 12);
+        } else {
+            if (p.N == 100) DKS_FUSED_WT(100, 16);
+            else if (p.N == 128) DKS_FUSED_WT(128, 16);
+            else DKS_FUSED_WT16(0, 16);
+        }
+#undef DKS_FUSED_WT16
+#undef DKS_FUSED_WT
+#undef DKS_FUSED_LAUNCH_WT
+        return err;
+    }
     const int nw = cta_warps > 20 ? 24 : (cta_warps > 16 ? 20 : (cta_warps > 12 ? 16 : 12));
 #define DKS_FUSED_NW(NCT, KP, NI)                                                                                     \
     do {                                                                                                              \

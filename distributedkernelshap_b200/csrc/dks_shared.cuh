@@ -69,6 +69,7 @@ struct SharedParams {
     int accumulate;          // add to sums instead of overwriting them (second and later background chunks)
     float* acache;           // [n][S_pad] A(i, s) of sixteen-word rows, kept between the launches of the background chunks
     int acache_mode;         // 0: off, 1: this launch writes it (first chunk), 2: this launch reads it
+    const float* wn;         // [N] weighted backgrounds: N w_j with the w_j summing to 1 (the weighted kernels only)
 };
 
 // Two sigmoids with one reciprocal.  With ua = 2^ta, ub = 2^tb:  (1+ua)(1+ub) = 1 + sm + q,  sm = ua + ub, q = ua*ub
@@ -279,9 +280,77 @@ __device__ __forceinline__ void chunk_sums(const float (&v)[16], float A, f32x2 
     if (NV & 1) single_acc(A, v[NV - 1], t1s, t0s);
 }
 
-template <int NTAIL, int W>
+// ---- weighted backgrounds (k-means centroids, user weights) ----------------------------------------------------------
+// The kernels see w'_j = N w_j (the w_j sum to 1), so the weighted sums have the magnitude of the uniform ones and every
+// consumer (the logit link, the identity link's sum * (1 / N), the solves) is unchanged.  A pair (a, b) still shares one
+// reciprocal:  with ua = A Dma, ub = A Dmb, den = (1 + ua)(1 + ub) = 1 + A (Dma + Dmb) + A^2 Dma Dmb,
+//   wa p1a + wb p1b = (W2 + A X) / den                   X = wa Dmb + wb Dma
+//   wa p0a + wb p0b = (A Y + A^2 W2 Dma Dmb) / den       Y = wa Dma + wb Dmb,   W2 = wa + wb
+// X and Y are per row and column pair, W2 per column pair only.  The weighted slice holds two float4 per quad of columns
+// (0,2) (1,3) and lane: (ds, dq) as in the uniform slice, then (X, Y); W2 comes from a small per-CTA array (a broadcast
+// load).  Columns past N have Dm = 0 and weight 0 and contribute exactly nothing, so a partial last quad needs no tail
+// code.  p0 keeps its own sum (forming it as W - sum p1 would cancel at saturated scores).  The weighted slice holds an
+// even number of quads (a zero quad past an odd count), so that loops with a run-time trip count can take them in pairs,
+// each pair member on its own accumulator chain, with register-resident accumulators.
+__host__ __device__ inline int dm_quads_w(int N) { return (dm_quads(N) + 1) & ~1; }
+__host__ __device__ inline size_t dm_slice_bytes_w(int N) { return (size_t)dm_quads_w(N) * 2 * 32 * sizeof(float4); }
+
+// quad q of row s for the weighted slice, from the raw columns of Dm and their weights
+__device__ __forceinline__ void dm_quad_w(const float* __restrict__ DmT, const float* __restrict__ wn, int N, int S_pad, int s,
+                                          int q, float4& sq, float4& xy) {
+    float d[4], w[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int j = 4 * q + k;
+        d[k] = j < N ? DmT[(size_t)j * S_pad + s] : 0.f;
+        w[k] = j < N ? wn[j] : 0.f;
+    }
+    sq = make_float4(__fadd_rn(d[0], d[2]), __fadd_rn(d[1], d[3]), __fmul_rn(d[0], d[2]), __fmul_rn(d[1], d[3]));
+    xy = make_float4(__fadd_rn(__fmul_rn(w[0], d[2]), __fmul_rn(w[2], d[0])), __fadd_rn(__fmul_rn(w[1], d[3]), __fmul_rn(w[3], d[1])),
+                     __fadd_rn(__fmul_rn(w[0], d[0]), __fmul_rn(w[2], d[2])), __fadd_rn(__fmul_rn(w[1], d[1]), __fmul_rn(w[3], d[3])));
+}
+// W2 of quad q (zero past N)
+__device__ __forceinline__ float2 w2_quad(const float* __restrict__ wn, int N, int q) {
+    const int j = 4 * q;
+    const float w0 = j < N ? wn[j] : 0.f, w1 = j + 1 < N ? wn[j + 1] : 0.f;
+    const float w2 = j + 2 < N ? wn[j + 2] : 0.f, w3 = j + 3 < N ? wn[j + 3] : 0.f;
+    return make_float2(__fadd_rn(w0, w2), __fadd_rn(w1, w3));
+}
+
+// four weighted sigmoids, two reciprocals: 10 packed ops + 2 MUFU (the uniform quad_acc_sq: 7 + 2).  The A^2 W2 Dma Dmb
+// term is formed as (r q) W2: q = A^2 Dma Dmb reaches 2^121 below the clamped path's threshold (A <= 1e18, Dm <= sqrt 2)
+// and W2 is bounded only by the background size, so q W2 could pass the fp32 range, while r q = q / den < 1.
+__device__ __forceinline__ void quad_acc_w(f32x2 A2, f32x2 AA2, float4 sq, float4 xy, float2 w2, f32x2 one2, f32x2& a1,
+                                           f32x2& a0) {
+    const f32x2 W2 = f2_pack(w2.x, w2.y);
+    const f32x2 sm = f2_mul(A2, f2_pack(sq.x, sq.y));
+    const f32x2 q = f2_mul(AA2, f2_pack(sq.z, sq.w));
+    const f32x2 den = f2_add(f2_add(sm, one2), q);
+    float dlo, dhi;
+    f2_unpack(den, dlo, dhi);
+    const f32x2 r = f2_pack(rcp_approx(dlo), rcp_approx(dhi));
+    a1 = f2_fma(r, f2_fma(A2, f2_pack(xy.x, xy.y), W2), a1);
+    a0 = f2_fma(f2_mul(r, q), W2, f2_fma(r, f2_mul(A2, f2_pack(xy.z, xy.w)), a0));
+}
+
+// the clamped scalar path of a weighted row (A > 1e18: saturated scores), one element at a time from the raw row
+__device__ __forceinline__ void row_sums_clamped_w(const float* __restrict__ DmT, const float* __restrict__ wn, int N, int S_pad,
+                                                   int s, float A, float& s1, float& s0) {
+    float r1 = 0.f, r0 = 0.f;
+    for (int j = 0; j < N; ++j) {
+        const float w = wn[j];
+        const float ua = fminf(A * DmT[(size_t)j * S_pad + s], U_CLAMP);
+        const float r = rcp_approx(1.f + ua);
+        r1 = fmaf(w, r, r1);
+        r0 = fmaf(w * ua, r, r0);
+    }
+    s1 = r1; s0 = r0;
+}
+
+// WT: weighted background (the weighted slice and quad_acc_w above; NTAIL is unused and 0)
+template <int NTAIL, int W, bool WT = false>
 __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_smem_kernel(SharedParams p, int warps_used) {
-    extern __shared__ float4 s_dm[];                      // [warps_used][dm_quads(N)][32]
+    extern __shared__ float4 s_dm[];                      // [warps_used][dm_quads(N)][32]  (weighted: [warps_used][2 nqw][32])
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 
     const int n_rg = p.S_pad / 32;                       // row groups
@@ -289,6 +358,13 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_smem_kern
     const int nparts = total_warps / n_rg;               // replicas of every row group
     const int gw = blockIdx.x * warps_used + warp;
     const bool active = warp < warps_used && nparts > 0 && gw < nparts * n_rg;
+    float2* sW2 = nullptr;                               // weighted: [nqw] W2 per quad, after the slices
+    if constexpr (WT) {
+        const int nqw = dm_quads_w(p.N);
+        sW2 = reinterpret_cast<float2*>(s_dm + (size_t)warps_used * 2 * nqw * 32);
+        for (int q = threadIdx.x; q < nqw; q += blockDim.x) sW2[q] = w2_quad(p.wn, p.N, q);
+        __syncthreads();
+    }
     if (active) {
         const int rg = gw % n_rg, part = gw / n_rg;
         const int s = rg * 32 + lane;
@@ -296,9 +372,18 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_smem_kern
         const int N = p.N, G = p.G;
         const int nfull = N / 16;
         const int nq = dm_quads(N);
-        float4* sl = s_dm + (size_t)warp * nq * 32;      // this warp's slice
+        const int nqw = dm_quads_w(N);                  // weighted: quads of the slice (even)
+        float4* sl = s_dm + (size_t)warp * (WT ? 2 * nqw : nq) * 32;    // this warp's slice
         const double es = p.dme[s];                      // exponent the row of Dm was normalised by (entries <= sqrt 2)
-        for (int c = 0; c * 16 < N; ++c) {
+        if constexpr (WT) {
+            for (int q = 0; q < nqw; ++q) {
+                float4 sq, xy;
+                dm_quad_w(p.DmT, p.wn, N, p.S_pad, s, q, sq, xy);
+                sl[(2 * q) * 32 + lane] = sq;
+                sl[(2 * q + 1) * 32 + lane] = xy;
+            }
+        }
+        for (int c = 0; !WT && c * 16 < N; ++c) {
             float v[16];
 #pragma unroll
             for (int jj = 0; jj < 16; ++jj) {
@@ -411,6 +496,34 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_smem_kern
             // A^2 must stay finite in fp32 (the normalised entries are <= sqrt 2, so A bounds every u): rows beyond that
             // take the clamped scalar path on the raw row from global memory (rare: saturated scores)
             const bool risky = __any_sync(0xffffffffu, A > 1.0e18f);
+            if constexpr (WT) {
+                float s1, s0;
+                if (risky) {
+                    row_sums_clamped_w(p.DmT, p.wn, N, p.S_pad, s, A, s1, s0);
+                } else {
+                    const f32x2 A2 = f2_pack(A, A);
+                    const float AA = A * A;
+                    const f32x2 AA2 = f2_pack(AA, AA);
+                    f32x2 acc1[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)}, acc0[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)};
+#pragma unroll 2
+                    for (int q = 0; q < nqw; q += 2) {
+                        quad_acc_w(A2, AA2, sl[(2 * q) * 32 + lane], sl[(2 * q + 1) * 32 + lane], sW2[q], one2, acc1[0],
+                                   acc0[0]);
+                        quad_acc_w(A2, AA2, sl[(2 * q + 2) * 32 + lane], sl[(2 * q + 3) * 32 + lane], sW2[q + 1], one2,
+                                   acc1[1], acc0[1]);
+                    }
+                    float q0, q1, q2, q3;
+                    f2_unpack(f2_add(acc1[0], acc1[1]), q0, q1);
+                    f2_unpack(f2_add(acc0[0], acc0[1]), q2, q3);
+                    s1 = q0 + q1; s0 = q2 + q3;
+                }
+                if (s < p.S) {
+                    float2* dst = p.sums + (size_t)i * p.S_pad + s;
+                    if (p.accumulate) { const float2 o = *dst; s1 += o.x; s0 += o.y; }
+                    *dst = make_float2(s1, s0);
+                }
+                continue;
+            }
             if (risky) {
                 float r1 = 0.f, r0 = 0.f;
                 for (int j = 0; j + 1 < N; j += 2)
@@ -480,6 +593,26 @@ inline int shared_grid(int n_rg, int warps, int sm_count) {
 inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words, int sm_count, int max_smem, cudaStream_t stream,
                                                SharedLaunch* info) {
     const int n_rg = p.S_pad / 32;
+    if (p.wn != nullptr) {
+        // weighted background: the shared-memory kernel with the weighted slice (twice the bytes), W2 after the slices
+        const size_t slice = dm_slice_bytes_w(p.N), w2 = sizeof(float2) * (size_t)dm_quads_w(p.N);
+        int warps_used = (int)(((size_t)max_smem - 1024 - w2) / slice);
+        if (warps_used > TM_MAX_WARPS) warps_used = TM_MAX_WARPS;
+        const size_t smem = (size_t)warps_used * slice + w2;
+        const int grid = shared_grid(n_rg, warps_used, sm_count);
+        info->regs = 0;
+        if (info->warps == 0 || warps_used < info->warps) info->warps = warps_used;
+        if (grid > info->grid) info->grid = grid;
+        cudaError_t err = cudaSuccess;
+#define DKS_CASE_WT(W)                                                                                                        \
+    err = cudaFuncSetAttribute(explain_shared_smem_kernel<0, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+    if (err == cudaSuccess) explain_shared_smem_kernel<0, W, true><<<grid, 32 * TM_MAX_WARPS, smem, stream>>>(p, warps_used);
+        if (words == 1) { DKS_CASE_WT(1) }
+        else if (words == 2) { DKS_CASE_WT(2) }
+        else { DKS_CASE_WT(16) }
+#undef DKS_CASE_WT
+        return err;
+    }
     if (shared_dm_in_smem() || words > 2) {                  // sixteen-word rows exist for the shared-memory kernel only
         const size_t slice = dm_slice_bytes(p.N);
         int warps_used = (int)(((size_t)max_smem - 1024) / slice);
@@ -526,17 +659,20 @@ inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words,
     return cudaSuccess;
 }
 
-// Backgrounds larger than MAXN rows go through in chunks of MAXN columns of Dm (one launch each, sums accumulated).
-// Returns the number of launches (0 when one of them could not be configured).
+// Backgrounds larger than MAXN rows go through in chunks of MAXN columns of Dm (one launch each, sums accumulated; a
+// weighted chunk uses its own columns' weights).  Returns the number of launches (0 when one of them could not be
+// configured).
 inline int launch_explain_shared(SharedParams p, int words, int sm_count, int max_smem, cudaStream_t stream, SharedLaunch* info) {
     const int N = p.N;
     const float* dm = p.DmT;
+    const float* wn = p.wn;
     int launches = 0;
     info->grid = 0; info->warps = 0;
     const bool use_cache = words > 2 && p.acache != nullptr && N > MAXN;
     for (int j0 = 0; j0 < N; j0 += MAXN, ++launches) {
         p.N = N - j0 < MAXN ? N - j0 : MAXN;
         p.DmT = dm + (size_t)j0 * p.S_pad;
+        if (wn != nullptr) p.wn = wn + j0;
         p.accumulate = j0 > 0;
         p.acache_mode = use_cache ? (j0 == 0 ? 1 : 2) : 0;
         if (launch_explain_shared_chunk(p, words, sm_count, max_smem, stream, info) != cudaSuccess) return 0;

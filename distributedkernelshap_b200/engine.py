@@ -198,9 +198,8 @@ class GpuKernelExplainer:
                 "set); the CUDA engine runs the selection for instances whose groups all vary only -- pass l1_reg=False")
         if self.plan_mode != "shared":
             raise NotImplementedError("l1 feature selection runs with plan_mode='shared' only")
-        if self.spec.act_code != _cabi.ACT_BINARY_LOGISTIC or not np.allclose(self.data.weights, self.data.weights[0]):
-            raise NotImplementedError("l1 feature selection needs the binary-logistic head and uniform background weights "
-                                      "(the shared-plan path)")
+        if self.spec.act_code != _cabi.ACT_BINARY_LOGISTIC:
+            raise NotImplementedError("l1 feature selection needs the binary-logistic head (the shared-plan path)")
         mode, k = explicit if explicit is not None else (1, 0)
         return (mode, k, 1 if len(present) > 1 else 0)
 
@@ -559,15 +558,17 @@ class GpuKernelExplainer:
         'smem' | 'regs'), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
-        are reported as unsupported, not computed) and ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
-        row-group slices at one warp each, or fewer slices shared by several warps each)."""
-        out = np.zeros(10, dtype=np.int32)
+        are reported as unsupported, not computed), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
+        row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
+        'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
+        the weighted one)."""
+        out = np.zeros(11, dtype=np.int32)
         _cabi.check(self.lib.dks_last_path(self._ctx, _cabi.ptr(out), len(out)))
         names = self._PATH_NAMES
         return {"shared": names["shared"][out[0]], "chunks": int(out[1]), "warps": int(out[2]), "grid": int(out[3]),
                 "fused_B": int(out[4]), "fused_NI": int(out[5]), "solve": names["solve"][out[6]],
                 "pmat_kpad": int(out[7]), "general": names["general"][out[8]],
-                "cta_warps": int(out[9])}
+                "cta_warps": int(out[9]), "bg_weights": ("uniform", "weighted")[out[10]]}
 
     def debug_scores(self, X, instance, nsamples="auto"):
         """Raw accumulator tile of the tensor-core kernel for one instance: float32 [S_cap, Npad] of scaled masked scores

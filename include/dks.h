@@ -220,7 +220,9 @@ int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by th
 #define DKS_PATH_FUSED_CTA_WARPS 9 /* fused kernel: warps per CTA it runs.  DKS_PATH_WARPS is the row-group slices a CTA
                                     * holds with one warp per slice (what decides fused or not); when fewer slices cover the
                                     * plan, several warps share each slice and this is larger */
-#define DKS_PATH_FIELDS 10
+#define DKS_PATH_BG_WEIGHTS 10   /* shared-plan kernels: 0 = uniform-background instantiations, 1 = the weighted ones
+                                  * (background weights not all equal) */
+#define DKS_PATH_FIELDS 11
 #define DKS_SHARED_NONE 0
 #define DKS_SHARED_FUSED 1       /* explain_shared_fused_kernel: link + projection solve inside */
 #define DKS_SHARED_SMEM 2        /* explain_shared_smem_kernel (Dm rows in shared memory) */
