@@ -288,7 +288,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     }
     const bool fused = fast && !l1 && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
                        dks::shared_path::fused_config(ctx->N, G, pg.S_pad, ctx->sm_count, ctx->max_smem_optin,
-                                                      ctx->opt_fused_ni, ctx->opt_fused_warps, ctx->opt_fused_B, &fcfg,
+                                                      ctx->opt_fused_warps, ctx->opt_fused_B, &fcfg,
                                                       wn != nullptr);
     ctx->last_fused = fused;
     if (fused) {
@@ -319,7 +319,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         CUDA_TRY(dks::shared_path::launch_explain_fused(fp, fcfg, ctx->sm_count, ctx->stream));
         ctx->launches += 1;
         path[DKS_PATH_SHARED] = DKS_SHARED_FUSED; path[DKS_PATH_CHUNKS] = 1; path[DKS_PATH_WARPS] = fcfg.warps;
-        path[DKS_PATH_GRID] = ctx->sm_count; path[DKS_PATH_FUSED_B] = fcfg.B; path[DKS_PATH_FUSED_NI] = fcfg.ni;
+        path[DKS_PATH_GRID] = ctx->sm_count; path[DKS_PATH_FUSED_B] = fcfg.B; path[DKS_PATH_FUSED_NI] = 1;
         path[DKS_PATH_SOLVE] = DKS_SOLVE_FUSED; path[DKS_PATH_FUSED_CTA_WARPS] = fcfg.slices * fcfg.kw;
         CUDA_TRY(cudaGetLastError());
         p.list = ctx->d_idx_other;
@@ -549,7 +549,6 @@ int dks_create(dks_ctx** out, int device) {
     {
         auto env_int = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
         ctx->opt_fused = env_int("DKS_FUSED", 1);
-        ctx->opt_fused_ni = env_int("DKS_FUSED_NI", 0);
         ctx->opt_fused_warps = env_int("DKS_FUSED_WARPS", 0);
         ctx->opt_fused_B = env_int("DKS_FUSED_B", 0);
         ctx->push_in_kernel = env_int("DKS_PUSH_IN_KERNEL", 0) != 0;
@@ -1375,7 +1374,6 @@ int dks_set_option(dks_ctx* ctx, const char* name, int value) {
     REQUIRE(ctx && name, "dks_set_option: bad arguments");
     const std::string key(name);
     if (key == "fused") ctx->opt_fused = value;
-    else if (key == "fused_ni") ctx->opt_fused_ni = value;
     else if (key == "fused_warps") ctx->opt_fused_warps = value;
     else if (key == "fused_batch") ctx->opt_fused_B = value;
     else if (key == "push_in_kernel") ctx->push_in_kernel = value != 0;

@@ -225,8 +225,8 @@ struct dks_ctx {
     unsigned long long* d_step = nullptr;          // device-side step counter of the flag exchange
     bool push_in_kernel = false;                   // 1: the fused kernel's epilogue stores phi into the peers' buffers itself
                                                    // (measured slower than the separate coalesced push kernel: DESIGN.md §7)
-    // tuning knobs (dks_set_option; defaults from the environment at dks_create: DKS_FUSED, DKS_FUSED_NI, ...)
-    int opt_fused = 1, opt_fused_ni = 0, opt_fused_warps = 0, opt_fused_B = 0;
+    // tuning knobs (dks_set_option; defaults from the environment at dks_create: DKS_FUSED, DKS_FUSED_WARPS, ...)
+    int opt_fused = 1, opt_fused_warps = 0, opt_fused_B = 0;
     bool opt_graph_timing = false;   // keep the timing event records inside a captured graph (dks_last_timings after replays)
     bool timing_valid = false, last_was_graph = false;
     bool last_fused = false;                       // the last explain ran the fused shared-plan kernel

@@ -17,8 +17,7 @@
 // A CTA holds `slices` row groups: each slice is the group's 32 rows of Dm (pair sums and pair products, as in
 // explain_shared_smem_kernel) and of P.  kw warps share a slice and stream disjoint subsets of the instances through it,
 // each with its own staging tile.  kw = 1 is one slice per warp, which fits the most row groups into a CTA (the largest
-// plans); kw > 1 runs more warps per SM than slices of their own would fit.  NI = 1 or 2 instances share one pass over the
-// slice (one load feeds both).
+// plans); kw > 1 runs more warps per SM than slices of their own would fit.
 #pragma once
 
 #include "dks_shared.cuh"
@@ -120,11 +119,23 @@ inline size_t fused_smem_bytes(int slices, int kw, int kpad, int B, int N, bool 
            (weighted ? sizeof(float2) * (size_t)dm_quads_w(N) : 0);
 }
 
+// one slice per CTA with the flat split of the kernel below: a second slice of Dm and P (no second set of staging tiles)
+inline size_t fused_flat_smem_bytes(int kw, int kpad, int B, int N, bool weighted = false) {
+    return fused_smem_bytes(1, kw, kpad, B, N, weighted) + (weighted ? dm_slice_bytes_w(N) : dm_slice_bytes(N)) +
+           (size_t)32 * kpad * sizeof(double);
+}
+
 // NCT: background rows at compile time (0 = run-time p.N): with NCT the chunk loop unrolls completely (static shared-memory
 // offsets, no loop control, the tail folded).  B (instances parked per warp) is a power of two.  Warp w of a CTA works on
 // slice w / kw; warps from slices * kw on idle.  WT: weighted background (quad_acc_w, dks_shared.cuh).
-template <int NCT, int KPAD, int NWARPS, int NI, bool WT = false>
-__global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(FusedParams p, int slices, int kw) {
+// flat (one slice per CTA, at least as many CTAs as row groups): instead of whole replicas of a row group, CTA c takes the
+// c-th of gridDim.x equal contiguous ranges of the (row group, instance ordinal) pairs, row group major, and its kw warps
+// split that range into equal contiguous pieces.  A range spans at most two row groups, so the CTA holds two slices of Dm
+// and P; every CTA of the grid works, however the row groups divide into the SMs.  Each (instance, row group) pair is
+// still delivered exactly once.
+template <int NCT, int KPAD, int NWARPS, bool WT = false>
+__global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(FusedParams p, int slices, int kw, int flat) {
+    constexpr int NI = 1;                                // instances per pass over the slice
     extern __shared__ __align__(16) unsigned char fsm[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int slice = warp / kw, sub = warp - slice * kw;
@@ -132,9 +143,10 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
     const int nq = dm_quads(NCT ? NCT : p.N);
     const int nqw = dm_quads_w(NCT ? NCT : p.N);                                 // weighted: quads of the slice (even)
     const int sq4 = WT ? 2 * nqw : nq;                                           // float4 per lane and slice
-    float4* sDm = reinterpret_cast<float4*>(fsm);                                // [slices][sq4][32]
-    double* sP = reinterpret_cast<double*>(sDm + (size_t)slices * sq4 * 32);     // [slices][32][KPAD]
-    double* sY = sP + (size_t)slices * 32 * KPAD;                                // [slices * kw][32][B + 1]
+    const int nsl = flat ? 2 : slices;                                            // slices of Dm and P held
+    float4* sDm = reinterpret_cast<float4*>(fsm);                                // [nsl][sq4][32]
+    double* sP = reinterpret_cast<double*>(sDm + (size_t)nsl * sq4 * 32);        // [nsl][32][KPAD]
+    double* sY = sP + (size_t)nsl * 32 * KPAD;                                   // [slices * kw][32][B + 1]
     LogTabEntry* s_logtab = reinterpret_cast<LogTabEntry*>(sY + (size_t)slices * kw * 32 * ystride);
     float2* sW2 = reinterpret_cast<float2*>(s_logtab + DKS_LOGTAB_SIZE);         // weighted: [nqw]
     if (threadIdx.x >= 64 && threadIdx.x < 64 + DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x - 64);
@@ -149,13 +161,21 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
     const int n_rg = p.S_pad / 32;                       // row groups
     const int nparts = gridDim.x * slices / n_rg;        // replicas of every row group (>= 1: checked by the host)
     const int gs = blockIdx.x * slices + slice;
-    const bool active = slice < slices && gs < nparts * n_rg;
-    const int rg = active ? gs % n_rg : 0, part = active ? gs / n_rg : 0;
-    const int s = rg * 32 + lane;
-    double* sPw = sP + (size_t)slice * 32 * KPAD;
+    const bool active = slice < slices && (flat || gs < nparts * n_rg);
     double* sYw = sY + (size_t)warp * 32 * ystride;
-    float4* sl = sDm + (size_t)slice * sq4 * 32;         // this warp's slice
-    if (active) {
+    // flat: the CTA's pairs [c0, c1) and this warp's [u0, u1); row groups rg_lo .. rg_lo + 1 in slices 0 and 1
+    const int cnt_f = flat ? *p.count : 0;
+    const long long U = (long long)n_rg * cnt_f;
+    const long long c0 = U * blockIdx.x / gridDim.x, c1 = U * (blockIdx.x + 1) / gridDim.x;
+    const long long u0 = c0 + (c1 - c0) * sub / kw, u1 = c0 + (c1 - c0) * (sub + 1) / kw;
+    const int rg_lo = cnt_f > 0 ? (int)(c0 / cnt_f) : 0;
+    const int nfill = flat ? (c1 > c0 ? (int)((c1 - 1) / cnt_f) - rg_lo + 1 : 0) : 1;
+    for (int f = 0; active && f < nfill; ++f) {
+        const int fs = flat ? f : slice;
+        const int rg = flat ? rg_lo + f : gs % n_rg;
+        const int s = rg * 32 + lane;
+        double* sPw = sP + (size_t)fs * 32 * KPAD;
+        float4* sl = sDm + (size_t)fs * sq4 * 32;
         // ---- the slice's 32 rows of P and of Dm, split over its kw warps; Dm as pair sums and pair products per quad of
         // columns (0,2) (1,3)
         const double* src = p.pmat64 + (size_t)rg * 32 * KPAD;     // the slice's 32 rows are contiguous
@@ -195,205 +215,216 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
         const int cnt = *p.count;
         const int G = p.G, nA = G - 1;
         const int nq_t = ntail >> 2, rem_t = ntail & 3;
-        const double es = p.dme[s];
-        const uint64_t zz = s < p.S ? p.z[s] : 0ull;
-        const int ntab = (G + 3) / 4;                     // <= 4 (the host sends wider problems down the unfused path)
-        const f32x2 one2 = f2_pack(1.f, 1.f), two2 = f2_pack(2.f, 2.f);
-        const double yf = p.link == DKS_LINK_LOGIT ? p.linkfnull[1] : p.fnull[1], inv_n = 1.0 / (double)N;   // link(fnull)
-        const size_t slab = (size_t)p.n * G;
-        // instances of this warp: ordinals first, first + stride, ... of the list (the part's instances dealt round-robin
-        // over the slice's kw warps)
-        const int first = part + sub * nparts, stride = nparts * kw;
-        const int my_n = first < cnt ? (cnt - first + stride - 1) / stride : 0;
-        const bool row_ok = s < p.S;
-        const int bmask = B - 1;
+        // segments of this warp's work: one row group each, instance ordinals first, first + stride, ...; flat: up to two
+        // row groups, contiguous ordinals; otherwise the part's instances dealt round-robin over the slice's kw warps
+        const long long seg_end = flat && u0 < u1 ? ((u0 / cnt) + 1) * cnt : 0;
+        const int nseg = flat ? (u0 < u1 ? (u1 > seg_end ? 2 : 1) : 0) : 1;
+        for (int seg = 0; seg < nseg; ++seg) {
+            const int rg = flat ? (int)(u0 / cnt) + seg : gs % n_rg;
+            const int s = rg * 32 + lane;
+            const int fs = flat ? rg - rg_lo : slice;
+            const double* sPw = sP + (size_t)fs * 32 * KPAD;
+            const float4* sl = sDm + (size_t)fs * sq4 * 32;
+            const int first = flat ? (seg == 0 ? (int)(u0 % cnt) : 0) : gs / n_rg + sub * nparts;
+            const int stride = flat ? 1 : nparts * kw;
+            const int my_n = flat ? (int)(seg == 0 ? (u1 < seg_end ? u1 : seg_end) - u0 : u1 - seg_end)
+                                  : (first < cnt ? (cnt - first + stride - 1) / stride : 0);
+            const double es = p.dme[s];
+            const uint64_t zz = s < p.S ? p.z[s] : 0ull;
+            const int ntab = (G + 3) / 4;                     // <= 4 (the host sends wider problems down the unfused path)
+            const f32x2 one2 = f2_pack(1.f, 1.f), two2 = f2_pack(2.f, 2.f);
+            const double yf = p.link == DKS_LINK_LOGIT ? p.linkfnull[1] : p.fnull[1], inv_n = 1.0 / (double)N;   // link(fnull)
+            const size_t slab = (size_t)p.n * G;
+            const bool row_ok = s < p.S;
+            const int bmask = B - 1;
 
-        // ---- the turn-around: four lanes per instance of the batch (eight instances per round), lane q of an instance owns
-        // coefficients q, q + 4, ...; each sums the warp's 32 rows in order sr = 0 .. 31
-        auto flush = [&](int bstart, int bcount) {
-            constexpr int KPL = KPAD / 4;
-            const int q = lane & 3;
-            for (int b0 = 0; b0 < bcount; b0 += 8) {
-                const int b = b0 + (lane >> 2);
-                const bool mine = b < bcount;
-                int i = 0;
-                int fin_i = -1;             // instance this lane finished in this round (its phi is complete in local memory)
-                if (mine) {
-                    double beta[KPL];
+            // ---- the turn-around: four lanes per instance of the batch (eight instances per round), lane q of an instance owns
+            // coefficients q, q + 4, ...; each sums the warp's 32 rows in order sr = 0 .. 31
+            auto flush = [&](int bstart, int bcount) {
+                constexpr int KPL = KPAD / 4;
+                const int q = lane & 3;
+                for (int b0 = 0; b0 < bcount; b0 += 8) {
+                    const int b = b0 + (lane >> 2);
+                    const bool mine = b < bcount;
+                    int i = 0;
+                    int fin_i = -1;             // instance this lane finished in this round (its phi is complete in local memory)
+                    if (mine) {
+                        double beta[KPL];
 #pragma unroll
-                    for (int j = 0; j < KPL; ++j) beta[j] = 0.0;
+                        for (int j = 0; j < KPL; ++j) beta[j] = 0.0;
 #pragma unroll 4
-                    for (int sr = 0; sr < 32; ++sr) {
-                        const double y = sYw[sr * ystride + b];
+                        for (int sr = 0; sr < 32; ++sr) {
+                            const double y = sYw[sr * ystride + b];
 #pragma unroll
-                        for (int j = 0; j < KPL; ++j) beta[j] = fma(sPw[sr * KPAD + q + 4 * j], y, beta[j]);
+                            for (int j = 0; j < KPL; ++j) beta[j] = fma(sPw[sr * KPAD + q + 4 * j], y, beta[j]);
+                        }
+                        i = p.list[first + (bstart + b) * stride];
+                        long long* acc = p.acc + (size_t)i * KPAD;
+#pragma unroll
+                        for (int j = 0; j < KPL; ++j)
+                            if (q + 4 * j < nA)
+                                asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(acc + q + 4 * j),
+                                             "l"((unsigned long long)to_fix(beta[j])) : "memory");
                     }
-                    i = p.list[first + (bstart + b) * stride];
-                    long long* acc = p.acc + (size_t)i * KPAD;
-#pragma unroll
-                    for (int j = 0; j < KPL; ++j)
-                        if (q + 4 * j < nA)
-                            asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(acc + q + 4 * j),
-                                         "l"((unsigned long long)to_fix(beta[j])) : "memory");
-                }
-                __syncwarp();               // the instance's four lanes have added: its first lane publishes the delivery
-                if (mine && q == 0) {
-                    int old;
-                    asm volatile("atom.release.gpu.global.add.s32 %0, [%1], 1;" : "=r"(old) : "l"(p.done + i) : "memory");
-                    if (old == n_rg - 1) {
-                        // every row group has delivered: finish the instance
-                        asm volatile("fence.acq_rel.gpu;" ::: "memory");
-                        finish_instance<KPAD>(p, i, nA, slab);
-                        fin_i = i;
+                    __syncwarp();               // the instance's four lanes have added: its first lane publishes the delivery
+                    if (mine && q == 0) {
+                        int old;
+                        asm volatile("atom.release.gpu.global.add.s32 %0, [%1], 1;" : "=r"(old) : "l"(p.done + i) : "memory");
+                        if (old == n_rg - 1) {
+                            // every row group has delivered: finish the instance
+                            asm volatile("fence.acq_rel.gpu;" ::: "memory");
+                            finish_instance<KPAD>(p, i, nA, slab);
+                            fin_i = i;
+                        }
                     }
+                    if (p.npeers > 0) peer_push_finished(p.phi, p.peer_phi, p.npeers, fin_i, lane, G, slab);     // multi-GPU only (kept out of line: no registers here)
                 }
-                if (p.npeers > 0) peer_push_finished(p.phi, p.peer_phi, p.npeers, fin_i, lane, G, slab);     // multi-GPU only (kept out of line: no registers here)
-            }
-        };
+            };
 
-        // a(i, s) = sum over the row's nibbles of one table entry each; the entries of the NEXT instance are loaded one
-        // iteration ahead (the offsets depend on the row only), the instance index two ahead.  No branches: tables the
-        // problem does not have point at entry [0][0] (the empty subset: exactly 0.0), and past the last instance the
-        // loads repeat the last one.
-        const size_t xstride = (size_t)ntab * 16;
-        const double* xb0 = p.XT + (int)(zz & 15ull);
-        const double* xb1 = p.XT + (ntab > 1 ? 16 + (int)((zz >> 4) & 15ull) : 0);
-        const double* xb2 = p.XT + (ntab > 2 ? 32 + (int)((zz >> 8) & 15ull) : 0);
-        const double* xb3 = p.XT + (ntab > 3 ? 48 + (int)((zz >> 12) & 15ull) : 0);
-        const int last_it = my_n > 0 ? my_n - 1 : 0;
-        // NI instances share one pass over the warp's rows of Dm: instance ordinals it .. it + NI - 1
-        int i_nx[NI];
-        double nx[NI][4];
-#pragma unroll
-        for (int u = 0; u < NI; ++u) {
-            const int o0 = u < last_it ? u : last_it, o1 = NI + u < last_it ? NI + u : last_it;
-            i_nx[u] = my_n > 0 ? p.list[first + o1 * stride] : 0;
-            nx[u][0] = nx[u][1] = nx[u][2] = nx[u][3] = 0.0;
-            if (my_n > 0) {
-                const size_t o = (size_t)p.list[first + o0 * stride] * xstride;
-                nx[u][0] = __ldg(xb0 + o); nx[u][1] = __ldg(xb1 + o); nx[u][2] = __ldg(xb2 + o); nx[u][3] = __ldg(xb3 + o);
-            }
-        }
-
-        for (int it = 0; it < my_n; it += NI) {
-            float A[NI];
-            bool risky_l = false;
+            // a(i, s) = sum over the row's nibbles of one table entry each; the entries of the NEXT instance are loaded one
+            // iteration ahead (the offsets depend on the row only), the instance index two ahead.  No branches: tables the
+            // problem does not have point at entry [0][0] (the empty subset: exactly 0.0), and past the last instance the
+            // loads repeat the last one.
+            const size_t xstride = (size_t)ntab * 16;
+            const double* xb0 = p.XT + (int)(zz & 15ull);
+            const double* xb1 = p.XT + (ntab > 1 ? 16 + (int)((zz >> 4) & 15ull) : 0);
+            const double* xb2 = p.XT + (ntab > 2 ? 32 + (int)((zz >> 8) & 15ull) : 0);
+            const double* xb3 = p.XT + (ntab > 3 ? 48 + (int)((zz >> 12) & 15ull) : 0);
+            const int last_it = my_n > 0 ? my_n - 1 : 0;
+            // NI instances share one pass over the warp's rows of Dm: instance ordinals it .. it + NI - 1
+            int i_nx[NI];
+            double nx[NI][4];
 #pragma unroll
             for (int u = 0; u < NI; ++u) {
-                const double a = ((nx[u][0] + nx[u][1]) + (nx[u][2] + nx[u][3])) + es;
-                {
-                    const size_t o = (size_t)i_nx[u] * xstride;
+                const int o0 = u < last_it ? u : last_it, o1 = NI + u < last_it ? NI + u : last_it;
+                i_nx[u] = my_n > 0 ? p.list[first + o1 * stride] : 0;
+                nx[u][0] = nx[u][1] = nx[u][2] = nx[u][3] = 0.0;
+                if (my_n > 0) {
+                    const size_t o = (size_t)p.list[first + o0 * stride] * xstride;
                     nx[u][0] = __ldg(xb0 + o); nx[u][1] = __ldg(xb1 + o); nx[u][2] = __ldg(xb2 + o); nx[u][3] = __ldg(xb3 + o);
-                    const int it2 = it + 2 * NI + u < last_it ? it + 2 * NI + u : last_it;
-                    i_nx[u] = p.list[first + it2 * stride];
                 }
-                // A = 2^a = 2^n 2^f, n = rint(a) through the 1.5 * 2^52 trick (no conversion instructions), |f| <= 1/2; the
-                // exponent is clamped to [-120, 120] (saturated scores; the clamped scalar path below takes A > 1e18)
-                const double tm = a + 6755399441055744.0;
-                int an_i = __double2loint(tm);
-                an_i = an_i < -120 ? -120 : (an_i > 120 ? 120 : an_i);
-                A[u] = ex2_approx((float)(a - (tm - 6755399441055744.0))) * __int_as_float((127 + an_i) << 23);
-                risky_l = risky_l || A[u] > 1.0e18f;
             }
-            float s1[NI], s0[NI];
-            if constexpr (WT) {
-                if (__any_sync(0xffffffffu, risky_l)) {
+
+            for (int it = 0; it < my_n; it += NI) {
+                float A[NI];
+                bool risky_l = false;
 #pragma unroll
-                    for (int u = 0; u < NI; ++u) row_sums_clamped_w(p.DmT, p.wn, N, p.S_pad, s, A[u], s1[u], s0[u]);
+                for (int u = 0; u < NI; ++u) {
+                    const double a = ((nx[u][0] + nx[u][1]) + (nx[u][2] + nx[u][3])) + es;
+                    {
+                        const size_t o = (size_t)i_nx[u] * xstride;
+                        nx[u][0] = __ldg(xb0 + o); nx[u][1] = __ldg(xb1 + o); nx[u][2] = __ldg(xb2 + o); nx[u][3] = __ldg(xb3 + o);
+                        const int it2 = it + 2 * NI + u < last_it ? it + 2 * NI + u : last_it;
+                        i_nx[u] = p.list[first + it2 * stride];
+                    }
+                    // A = 2^a = 2^n 2^f, n = rint(a) through the 1.5 * 2^52 trick (no conversion instructions), |f| <= 1/2; the
+                    // exponent is clamped to [-120, 120] (saturated scores; the clamped scalar path below takes A > 1e18)
+                    const double tm = a + 6755399441055744.0;
+                    int an_i = __double2loint(tm);
+                    an_i = an_i < -120 ? -120 : (an_i > 120 ? 120 : an_i);
+                    A[u] = ex2_approx((float)(a - (tm - 6755399441055744.0))) * __int_as_float((127 + an_i) << 23);
+                    risky_l = risky_l || A[u] > 1.0e18f;
+                }
+                float s1[NI], s0[NI];
+                if constexpr (WT) {
+                    if (__any_sync(0xffffffffu, risky_l)) {
+#pragma unroll
+                        for (int u = 0; u < NI; ++u) row_sums_clamped_w(p.DmT, p.wn, N, p.S_pad, s, A[u], s1[u], s0[u]);
+                    } else {
+                        // every quad of the slice (all columns compiled in with NCT), two accumulator chains per instance
+                        f32x2 A2[NI], AA2[NI], acc1[NI][2], acc0[NI][2];
+#pragma unroll
+                        for (int u = 0; u < NI; ++u) {
+                            const float AA = A[u] * A[u];
+                            A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA);
+                            acc1[u][0] = acc1[u][1] = acc0[u][0] = acc0[u][1] = f2_pack(0.f, 0.f);
+                        }
+                        // quad q on accumulator chain h (a constant after unrolling: the accumulators stay in registers)
+                        auto quad = [&](int q, int h) {
+                            const float4 sq = sl[(2 * q) * 32 + lane], xy = sl[(2 * q + 1) * 32 + lane];
+                            const float2 w2 = sW2[q];
+#pragma unroll
+                            for (int u = 0; u < NI; ++u) quad_acc_w(A2[u], AA2[u], sq, xy, w2, one2, acc1[u][h], acc0[u][h]);
+                        };
+                        if (NCT) {
+#pragma unroll
+                            for (int q = 0; q < dm_quads(NCT); ++q) quad(q, q & 1);
+                        } else {
+                            // run-time N: the slice's even number of quads in pairs (a zero quad past an odd count adds 0)
+#pragma unroll 2
+                            for (int q = 0; q < nqw; q += 2) { quad(q, 0); quad(q + 1, 1); }
+                        }
+#pragma unroll
+                        for (int u = 0; u < NI; ++u) {
+                            float q0, q1, q2, q3;
+                            f2_unpack(f2_add(acc1[u][0], acc1[u][1]), q0, q1);
+                            f2_unpack(f2_add(acc0[u][0], acc0[u][1]), q2, q3);
+                            s1[u] = q0 + q1;
+                            s0[u] = q2 + q3;
+                        }
+                    }
+                } else if (__any_sync(0xffffffffu, risky_l)) {
+                    // A^2 would leave the fp32 range: clamped scalar path on the raw row from global memory (saturated scores)
+#pragma unroll
+                    for (int u = 0; u < NI; ++u) {
+                        float r1 = 0.f, r0 = 0.f;
+                        for (int j = 0; j + 1 < N; j += 2)
+                            pair_acc<true>(A[u], p.DmT[(size_t)j * p.S_pad + s], p.DmT[(size_t)(j + 1) * p.S_pad + s], r1, r0);
+                        if (N & 1) single_acc(A[u], p.DmT[(size_t)(N - 1) * p.S_pad + s], r1, r0);
+                        s1[u] = r1; s0[u] = r0;
+                    }
                 } else {
-                    // every quad of the slice (all columns compiled in with NCT), two accumulator chains per instance
-                    f32x2 A2[NI], AA2[NI], acc1[NI][2], acc0[NI][2];
+                    f32x2 A2[NI], AA2[NI], AA2x2[NI];
+                    f32x2 acc1[NI][2], acc0[NI][2];
+                    float t1s[NI], t0s[NI];
 #pragma unroll
                     for (int u = 0; u < NI; ++u) {
                         const float AA = A[u] * A[u];
-                        A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA);
+                        A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA); AA2x2[u] = f2_pack(2.f * AA, 2.f * AA);
                         acc1[u][0] = acc1[u][1] = acc0[u][0] = acc0[u][1] = f2_pack(0.f, 0.f);
+                        t1s[u] = t0s[u] = 0.f;
                     }
-                    // quad q on accumulator chain h (a constant after unrolling: the accumulators stay in registers)
-                    auto quad = [&](int q, int h) {
-                        const float4 sq = sl[(2 * q) * 32 + lane], xy = sl[(2 * q + 1) * 32 + lane];
-                        const float2 w2 = sW2[q];
+                    float v[2][16];
+                    dm_ld16(sl, 0, nq, lane, v[0]);
 #pragma unroll
-                        for (int u = 0; u < NI; ++u) quad_acc_w(A2[u], AA2[u], sq, xy, w2, one2, acc1[u][h], acc0[u][h]);
-                    };
-                    if (NCT) {
+                    for (int c = 0; c < MAXCH; ++c) {
+                        if (c < nch) {
+                            if (c + 1 < nch) dm_ld16(sl, c + 1, nq, lane, v[(c + 1) & 1]);
 #pragma unroll
-                        for (int q = 0; q < dm_quads(NCT); ++q) quad(q, q & 1);
-                    } else {
-                        // run-time N: the slice's even number of quads in pairs (a zero quad past an odd count adds 0)
-#pragma unroll 2
-                        for (int q = 0; q < nqw; q += 2) { quad(q, 0); quad(q + 1, 1); }
+                            for (int u = 0; u < NI; ++u) {
+                                if (c < nfull) chunk_sums<16>(v[c & 1], A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
+                                else chunk_sums_rt(v[c & 1], nq_t, rem_t, A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
+                            }
+                        }
                     }
 #pragma unroll
                     for (int u = 0; u < NI; ++u) {
                         float q0, q1, q2, q3;
                         f2_unpack(f2_add(acc1[u][0], acc1[u][1]), q0, q1);
                         f2_unpack(f2_add(acc0[u][0], acc0[u][1]), q2, q3);
-                        s1[u] = q0 + q1;
-                        s0[u] = q2 + q3;
+                        s1[u] = (q0 + q1) + t1s[u];
+                        s0[u] = (q2 + q3) + t0s[u];
                     }
                 }
-            } else if (__any_sync(0xffffffffu, risky_l)) {
-                // A^2 would leave the fp32 range: clamped scalar path on the raw row from global memory (saturated scores)
+                // ---- link in place, rows parked for the turn-around (B is a multiple of NI: a pass never straddles a batch)
 #pragma unroll
                 for (int u = 0; u < NI; ++u) {
-                    float r1 = 0.f, r0 = 0.f;
-                    for (int j = 0; j + 1 < N; j += 2)
-                        pair_acc<true>(A[u], p.DmT[(size_t)j * p.S_pad + s], p.DmT[(size_t)(j + 1) * p.S_pad + s], r1, r0);
-                    if (N & 1) single_acc(A[u], p.DmT[(size_t)(N - 1) * p.S_pad + s], r1, r0);
-                    s1[u] = r1; s0[u] = r0;
-                }
-            } else {
-                f32x2 A2[NI], AA2[NI], AA2x2[NI];
-                f32x2 acc1[NI][2], acc0[NI][2];
-                float t1s[NI], t0s[NI];
-#pragma unroll
-                for (int u = 0; u < NI; ++u) {
-                    const float AA = A[u] * A[u];
-                    A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA); AA2x2[u] = f2_pack(2.f * AA, 2.f * AA);
-                    acc1[u][0] = acc1[u][1] = acc0[u][0] = acc0[u][1] = f2_pack(0.f, 0.f);
-                    t1s[u] = t0s[u] = 0.f;
-                }
-                float v[2][16];
-                dm_ld16(sl, 0, nq, lane, v[0]);
-#pragma unroll
-                for (int c = 0; c < MAXCH; ++c) {
-                    if (c < nch) {
-                        if (c + 1 < nch) dm_ld16(sl, c + 1, nq, lane, v[(c + 1) & 1]);
-#pragma unroll
-                        for (int u = 0; u < NI; ++u) {
-                            if (c < nfull) chunk_sums<16>(v[c & 1], A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
-                            else chunk_sums_rt(v[c & 1], nq_t, rem_t, A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
+                    if (it + u < my_n) {
+                        double y = 0.0;
+                        if (row_ok) {
+                            if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(s1[u], s0[u], s_logtab) - yf;
+                            else y = (double)s1[u] * inv_n - yf;
                         }
+                        sYw[lane * ystride + ((it + u) & bmask)] = y;
                     }
                 }
-#pragma unroll
-                for (int u = 0; u < NI; ++u) {
-                    float q0, q1, q2, q3;
-                    f2_unpack(f2_add(acc1[u][0], acc1[u][1]), q0, q1);
-                    f2_unpack(f2_add(acc0[u][0], acc0[u][1]), q2, q3);
-                    s1[u] = (q0 + q1) + t1s[u];
-                    s0[u] = (q2 + q3) + t0s[u];
+                const int last_done = it + NI - 1 < last_it ? it + NI - 1 : last_it;      // last ordinal this pass completed
+                const int slot = last_done & bmask;
+                if (slot == bmask || last_done == last_it) {
+                    __syncwarp();
+                    flush(last_done - slot, slot + 1);
+                    __syncwarp();
                 }
-            }
-            // ---- link in place, rows parked for the turn-around (B is a multiple of NI: a pass never straddles a batch)
-#pragma unroll
-            for (int u = 0; u < NI; ++u) {
-                if (it + u < my_n) {
-                    double y = 0.0;
-                    if (row_ok) {
-                        if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(s1[u], s0[u], s_logtab) - yf;
-                        else y = (double)s1[u] * inv_n - yf;
-                    }
-                    sYw[lane * ystride + ((it + u) & bmask)] = y;
-                }
-            }
-            const int last_done = it + NI - 1 < last_it ? it + NI - 1 : last_it;      // last ordinal this pass completed
-            const int slot = last_done & bmask;
-            if (slot == bmask || last_done == last_it) {
-                __syncwarp();
-                flush(last_done - slot, slot + 1);
-                __syncwarp();
             }
         }
     }
@@ -436,22 +467,21 @@ inline int fused_kpad(int G) { return G - 1 <= 12 ? 12 : 16; }
 
 // slices: row groups per CTA; kw: warps per slice; warps: the slices a CTA holds at kw = 1 (the most row groups the fused
 // kernel covers per CTA: the fused / unfused boundary is S_pad / 32 <= sm_count * warps)
-struct FusedConfig { int ni, warps, slices, kw, B; size_t smem; };
+struct FusedConfig { int warps, slices, kw, B, flat; size_t smem; };
 
-// warps per CTA with kw > 1.  24 warps of 32 lanes fill the SM's register file at 80 registers per thread, which the
-// kernel fits without spilling only with the background size compiled in (NCT = 100, or 128 with 12 coefficients) and one
-// instance per pass; the other shapes take at most 16 warps (up to 128 registers)
-// Weighted backgrounds (one instance per pass only) take at most 20 warps with NCT = 100 / 128 and 16 elsewhere: at 24
-// warps (80 registers) the weighted kernel spills, at 20 (up to 102) it does not; their kw = 1 layouts hold at most 16
-// slices.
-inline int fused_max_cta_warps(int N, int kpad, int ni, bool weighted = false) {
+// warps per CTA with kw > 1: at most 20 (up to 96 registers per thread) with the background size compiled in (NCT = 100,
+// or 128 with 12 coefficients; weighted: NCT = 100 or 128), 16 (up to 128) elsewhere.  24 warps fit the register file
+// at 80 registers without spilling for the uniform NCT = 100 kernel, but with the flat split the 20-warp build is the
+// faster one (DESIGN.md 5.0.1); the weighted kernel spills at 80.  The kw = 1 layouts of weighted backgrounds hold at
+// most 16 slices.
+inline int fused_max_cta_warps(int N, int kpad, bool weighted = false) {
     if (weighted) return N == 100 || N == 128 ? 20 : 16;
-    return ni == 1 && (N == 100 || (N == 128 && kpad == 12)) ? 24 : 16;
+    return N == 100 || (N == 128 && kpad == 12) ? 20 : 16;
 }
 
 // picks the layout (slices, warps per slice) and the batch for a shape; returns false when the fused kernel does not apply.
 // want_warps (warps per CTA) / want_B: 0 = default (tuning knobs, dks_set_option)
-inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, int want_ni, int want_warps, int want_B,
+inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, int want_warps, int want_B,
                          FusedConfig* cfg, bool weighted = false) {
     if (G < 2 || G > 16 || N > MAXN) return false;                        // at most four nibble tables, 15 coefficients
     const int kpad = fused_kpad(G);
@@ -470,11 +500,17 @@ inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, in
     if (warps < 1) return false;
     const int n_rg = S_pad / 32;
     if ((long long)sm_count * warps < n_rg) return false;                // every row group needs a slice
-    const int ni = (want_ni == 2 && kpad == 12 && !weighted) ? 2 : 1;   // two instances per pass over Dm (tuning knob)
     // kw > 1: R slices of floor(cap / R) warps each, where that keeps more warps streaming than kw = 1 does (replicas of
-    // every row group: floor(sm_count * R / n_rg); the slices beyond them idle)
-    auto busy = [&](int R, int K) { return (long long)K * ((long long)sm_count * R / n_rg) * n_rg; };
-    const int max_cta = fused_max_cta_warps(N, kpad, ni, weighted);
+    // every row group: floor(sm_count * R / n_rg); the slices beyond them idle).  One slice per CTA takes the flat split
+    // where its two slices fit: every CTA streams.
+    auto flat_fits = [&](int R, int K) {
+        return R == 1 && fused_flat_smem_bytes(K, kpad, B, N, weighted) + 1024 <= (size_t)max_smem;
+    };
+    auto busy = [&](int R, int K) {
+        if (K > 1 && flat_fits(R, K)) return (long long)K * sm_count;
+        return (long long)K * ((long long)sm_count * R / n_rg) * n_rg;
+    };
+    const int max_cta = fused_max_cta_warps(N, kpad, weighted);
     const int cap = want_warps > 0 && want_warps < max_cta ? want_warps : max_cta;
     int slices = warps, kw = 1;
     for (int R = 1; R <= warps && cap / R >= 2; ++R) {
@@ -482,34 +518,34 @@ inline bool fused_config(int N, int G, int S_pad, int sm_count, int max_smem, in
         if ((long long)sm_count * R < n_rg || fused_smem_bytes(R, K, kpad, B, N, weighted) + 1024 > (size_t)max_smem) continue;
         if (busy(R, K) > busy(slices, kw)) { slices = R; kw = K; }
     }
-    cfg->ni = ni;
     cfg->warps = warps; cfg->slices = slices; cfg->kw = kw; cfg->B = B;
-    cfg->smem = fused_smem_bytes(slices, kw, kpad, B, N, weighted);
+    cfg->flat = kw > 1 && flat_fits(slices, kw) ? 1 : 0;
+    cfg->smem = cfg->flat ? fused_flat_smem_bytes(kw, kpad, B, N, weighted) : fused_smem_bytes(slices, kw, kpad, B, N, weighted);
     return true;
 }
 
 inline cudaError_t launch_explain_fused(const FusedParams& p, const FusedConfig& cfg, int grid, cudaStream_t stream) {
     const int kpad = fused_kpad(p.G);
     cudaError_t err = cudaSuccess;
-#define DKS_FUSED_LAUNCH(NCT, KP, NW, NI)                                                                             \
+#define DKS_FUSED_LAUNCH(NCT, KP, NW)                                                                                 \
     do {                                                                                                              \
-        err = cudaFuncSetAttribute(explain_shared_fused_kernel<NCT, KP, NW, NI>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+        err = cudaFuncSetAttribute(explain_shared_fused_kernel<NCT, KP, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                    (int)cfg.smem);                                                                    \
         if (err == cudaSuccess)                                                                                       \
-            explain_shared_fused_kernel<NCT, KP, NW, NI><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.slices, cfg.kw); \
+            explain_shared_fused_kernel<NCT, KP, NW><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.slices, cfg.kw, cfg.flat); \
     } while (0)
     // background sizes with a compile-time specialisation (the chunk loop unrolls completely); everything else takes the
-    // run-time version.  Block size: the smallest of 12 / 16 / 20 / 24 warps that holds slices x kw (24 only where
+    // run-time version.  Block size: the smallest of 12 / 16 / 20 warps that holds slices x kw (20 only where
     // fused_max_cta_warps allows it).
     const int cta_warps = cfg.slices * cfg.kw;
     if (p.wn != nullptr) {
-        // weighted background: one instance per pass, 12 / 16 / 20 warps (20 only where fused_max_cta_warps allows it)
+        // weighted background: 12 / 16 / 20 warps (20 only where fused_max_cta_warps allows it)
 #define DKS_FUSED_LAUNCH_WT(NCT, KP, NW)                                                                              \
     do {                                                                                                              \
-        err = cudaFuncSetAttribute(explain_shared_fused_kernel<NCT, KP, NW, 1, true>,                                 \
+        err = cudaFuncSetAttribute(explain_shared_fused_kernel<NCT, KP, NW, true>,                                 \
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.smem);                       \
         if (err == cudaSuccess)                                                                                       \
-            explain_shared_fused_kernel<NCT, KP, NW, 1, true><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.slices, cfg.kw); \
+            explain_shared_fused_kernel<NCT, KP, NW, true><<<grid, 32 * NW, cfg.smem, stream>>>(p, cfg.slices, cfg.kw, cfg.flat); \
     } while (0)
 #define DKS_FUSED_WT(NCT, KP)                                                                                         \
     do {                                                                                                              \
@@ -536,31 +572,22 @@ inline cudaError_t launch_explain_fused(const FusedParams& p, const FusedConfig&
 #undef DKS_FUSED_LAUNCH_WT
         return err;
     }
-    const int nw = cta_warps > 20 ? 24 : (cta_warps > 16 ? 20 : (cta_warps > 12 ? 16 : 12));
-#define DKS_FUSED_NW(NCT, KP, NI)                                                                                     \
+    const int nw = cta_warps > 16 ? 20 : (cta_warps > 12 ? 16 : 12);
+#define DKS_FUSED_NW(NCT, KP)                                                                                         \
     do {                                                                                                              \
-        if (nw == 12) DKS_FUSED_LAUNCH(NCT, KP, 12, NI);                                                              \
-        else if (nw == 16) DKS_FUSED_LAUNCH(NCT, KP, 16, NI);                                                         \
-        else DKS_FUSED_LAUNCH(NCT, KP, 20, NI);                                                                       \
+        if (nw == 12) DKS_FUSED_LAUNCH(NCT, KP, 12);                                                                  \
+        else if (nw == 16) DKS_FUSED_LAUNCH(NCT, KP, 16);                                                             \
+        else DKS_FUSED_LAUNCH(NCT, KP, 20);                                                                           \
     } while (0)
-#define DKS_FUSED_NW24(NCT, KP, NI)                                                                                   \
-    do {                                                                                                              \
-        if (nw == 24) DKS_FUSED_LAUNCH(NCT, KP, 24, NI);                                                              \
-        else DKS_FUSED_NW(NCT, KP, NI);                                                                               \
-    } while (0)
-    if (kpad == 12 && cfg.ni == 2) {
-        if (p.N == 100) DKS_FUSED_NW(100, 12, 2);
-        else DKS_FUSED_NW(0, 12, 2);
-    } else if (kpad == 12) {
-        if (p.N == 100) DKS_FUSED_NW24(100, 12, 1);
-        else if (p.N == 128) DKS_FUSED_NW24(128, 12, 1);
-        else if (p.N == 64) DKS_FUSED_NW(64, 12, 1);
-        else DKS_FUSED_NW(0, 12, 1);
+    if (kpad == 12) {
+        if (p.N == 100) DKS_FUSED_NW(100, 12);
+        else if (p.N == 128) DKS_FUSED_NW(128, 12);
+        else if (p.N == 64) DKS_FUSED_NW(64, 12);
+        else DKS_FUSED_NW(0, 12);
     } else {
-        if (p.N == 100) DKS_FUSED_NW24(100, 16, 1);
-        else DKS_FUSED_NW(0, 16, 1);
+        if (p.N == 100) DKS_FUSED_NW(100, 16);
+        else DKS_FUSED_NW(0, 16);
     }
-#undef DKS_FUSED_NW24
 #undef DKS_FUSED_NW
 #undef DKS_FUSED_LAUNCH
     return err;

@@ -146,7 +146,7 @@ class GpuKernelExplainer:
         self.kernel = kernel
 
     def set_option(self, name, value):
-        """Tuning knob of the C library (``dks_set_option``): 'fused', 'fused_ni', 'fused_warps', 'fused_batch',
+        """Tuning knob of the C library (``dks_set_option``): 'fused', 'fused_warps', 'fused_batch',
         'push_in_kernel', 'graph', 'graph_timing', 'wide_gemm', 'wide_acache'."""
         _cabi.check(self.lib.dks_set_option(self._ctx, str(name).encode(), int(value)))
 

@@ -193,8 +193,7 @@ int dks_summarise_host(dks_ctx* ctx, int n, const int32_t* seg_offsets_host, int
 /* ---- knobs / introspection ---------------------------------------------------------------------- */
 int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
 /* tuning knobs, all optional (defaults are the measured best): "fused" 0/1 -- link + projection solve inside the shared-plan
- * coalition kernel (default 1; 0 = separate (sum p1, sum p0) buffer + solve kernel); "fused_ni" 1/2 instances per pass over
- * a warp's rows; "fused_warps" caps the warps per CTA (default: as many as fit, at most 24); "fused_batch" instances
+ * coalition kernel (default 1; 0 = separate (sum p1, sum p0) buffer + solve kernel); "fused_warps" caps the warps per CTA (default: as many as fit, at most 20); "fused_batch" instances
  * parked per warp before the turn-around;
  * "push_in_kernel" 0/1 -- multi-GPU: the fused kernel's epilogue stores phi into the peers' buffers itself instead of the
  * separate push kernel (default 0: measured slower, it stalls the finishing warps); "graph" 0/1 (CUDA-graph
@@ -213,7 +212,7 @@ int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by th
 #define DKS_PATH_WARPS 2         /* warps per CTA the coalition kernel uses (the fewest over the chunks) */
 #define DKS_PATH_GRID 3          /* CTAs of the coalition kernel (the largest over the chunks) */
 #define DKS_PATH_FUSED_B 4       /* fused kernel: instances parked per warp before the turn-around */
-#define DKS_PATH_FUSED_NI 5      /* fused kernel: instances per pass over a warp's rows */
+#define DKS_PATH_FUSED_NI 5      /* fused kernel: instances per pass over a warp's rows (1) */
 #define DKS_PATH_SOLVE 6         /* DKS_SOLVE_* */
 #define DKS_PATH_PMAT_KPAD 7     /* projection solve (DKS_SOLVE_PMAT): coefficient rows of P, padded */
 #define DKS_PATH_GENERAL 8       /* DKS_GENERAL_*: the kernel of the instances the shared-plan path does not take */

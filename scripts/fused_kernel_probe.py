@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Time the fused shared-plan coalition kernel on its own, on the bench.py workload, and sweep its warps per CTA.
+"""Time the fused shared-plan coalition kernel on its own, on the bench.py workload, and sweep its warps per CTA and
+the number of instances.
 
-  python scripts/fused_kernel_probe.py [--launches 200] [--steps 50] [--warps 4,6,8,10,12] [--out FILE]
+  python scripts/fused_kernel_probe.py [--launches 200] [--steps 50] [--warps 4,6,8,10,12] [--n 64,256,2560] [--out FILE]
 
 The workload is bench.py's: 2560 Adult-shaped instances, 12 groups, 100 background rows, nsamples = 2048, shared plans.
 For the engine's default configuration and for every ``fused_warps`` value of the sweep it reports
@@ -12,6 +13,9 @@ For the engine's default configuration and for every ``fused_warps`` value of th
   step_ms     a whole device-resident step (CUDA graph replay, as bench.py's ``value`` times it), mean over ``--steps``,
               L2 flushed before each;
   path        what the engine reports it launched (``last_path()``).
+
+The ``--n`` sweep explains the first n instances of the workload with the default configuration (few instances leave
+most of the streaming warps with one or two instances each).
 
 One JSON line on stdout, with the GPU name, its power limit and the SM clock sampled while the kernels ran.
 """
@@ -67,6 +71,7 @@ def main():
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warps", default="4,6,8,10,12", help="fused_warps values to sweep (comma separated)")
+    ap.add_argument("--n", default="64,256,2560", help="instance counts of the mapping sweep (comma separated)")
     ap.add_argument("--out", default=None, help="also write the JSON line to this file")
     args = ap.parse_args()
 
@@ -100,13 +105,19 @@ def main():
         sweep[str(w)] = measure(engine, X_dev, n, phi_dev, flush, stream, args.launches, args.steps)
         sweep[str(w)]["phi_equal_to_default"] = bool(np.array_equal(phi_dev.cpu().numpy(), phi_default))
     engine.set_option("fused_warps", 0)
+    by_n = {}
+    for m in [int(v) for v in args.n.split(",") if v]:
+        m = min(m, n)
+        phi_m = torch.empty((C, m, G), dtype=torch.float64, device="cuda")
+        by_n[str(m)] = measure(engine, X_dev[:m], m, phi_m, flush, stream, args.launches, args.steps)
+        by_n[str(m)]["phi_equal_to_default"] = bool(np.array_equal(phi_m.cpu().numpy(), phi_default[:, :m]))
     clocks = sampler.stop()
     engine.close()
 
     props = torch.cuda.get_device_properties(0)
     line = {"probe": "fused shared-plan kernel", "workload": "bench.py: 2560 Adult-shaped instances, G = 12, N = 100, "
             "nsamples = 2048, shared plans", "launches": args.launches, "steps": args.steps,
-            "default": default, "fused_warps_sweep": sweep,
+            "default": default, "fused_warps_sweep": sweep, "n_sweep": by_n,
             "clocks": {"sm_mhz": clocks["sm_mhz"], "sm_max_mhz": clocks["sm_max_mhz"], "reasons": clocks["reasons"],
                        "samples": clocks["samples"]},
             "gpu": {"name": props.name, "sm_count": props.multi_processor_count, "power_limit_w": bench._power_limit_w(0)}}
