@@ -9,6 +9,7 @@
 #include "dks_shared.cuh"
 #include "dks_fused.cuh"
 #include "dks_l1.cuh"
+#include "dks_multi.cuh"
 #include "dks_wide.cuh"
 #include "dks_sampler.cuh"
 
@@ -88,7 +89,7 @@ int ensure_workspace(dks_ctx* ctx, int n) {
     if (n <= ctx->cap_n) return DKS_OK;
     const int G = ctx->G, R = ctx->R, C = ctx->C;
     TRY(dev_alloc(&ctx->d_XW, (size_t)n * G * R));
-    TRY(dev_alloc(&ctx->d_XT, (size_t)n * ((G + 3) / 4) * 16));
+    TRY(dev_alloc(&ctx->d_XT, (size_t)n * R * ((G + 3) / 4) * 16));
     TRY(dev_alloc(&ctx->d_vflag, (size_t)n * G));
     TRY(dev_alloc(&ctx->d_vmask, (size_t)n));
     TRY(dev_alloc(&ctx->d_M, (size_t)n));
@@ -127,18 +128,73 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D);
     auto kern = stage ? dks::prep_kernel<true> : dks::prep_kernel<false>;
+    // nibble tables: the binary head's scaled contributions; the softmax head's per class (log2 e XW) and the identity
+    // head's XW - Bbar, up to 128 groups (what the shared-plan path of those heads covers)
+    double* xt = nullptr;
+    if (ctx->act == DKS_ACT_BINARY_LOGISTIC && ctx->R == 1) xt = ctx->d_XT;
+    else if ((ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_IDENTITY) && G <= 128 && ctx->plan_mode == 0) xt = ctx->d_XT;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
         X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
         ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
         ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-        (ctx->act == DKS_ACT_BINARY_LOGISTIC && ctx->R == 1) ? ctx->d_XT : nullptr, ctx->scale);
+        xt, ctx->scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
     ctx->cur_n = n;
     ctx->cur_X = X_dev;
     ctx->prepared = true;
+    return DKS_OK;
+}
+
+// upstream's l1 branch on the shared plan of G groups: moments of y per (instance, output), then the LARS path + criterion +
+// restricted WLS, one warp each.  nout = 1: the binary head (y from the (sum p1, sum p0) buffer); nout = C: the softmax and
+// identity heads (y from src).
+int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, int nout, const dks::shared_path::HeadSource& src, double* phi_dev) {
+    const int G = ctx->G, S = pg.S, S_pad = pg.S_pad;
+    const dks_ctx::L1Dev& lt = ctx->h_l1[G];
+    const size_t need_m = (size_t)n * nout * (2 * G + 4);
+    if (need_m > ctx->cap_mom) { TRY(dev_alloc(&ctx->d_mom, need_m)); ctx->cap_mom = need_m; ctx->epoch++; }
+    dks::l1::Params lp;
+    memset(&lp, 0, sizeof(lp));
+    lp.n = n; lp.N = ctx->N; lp.G = G; lp.C = ctx->C; lp.S = S; lp.S_pad = S_pad; lp.link = ctx->link;
+    lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.nout = nout; lp.src = src; lp.sums = ctx->d_sums; lp.z = pg.z; lp.w = pg.w;
+    lp.t.gram_raw = lt.gram_raw; lp.t.gram_norm = lt.gram_norm; lp.t.colsum = lt.colsum; lp.t.scale = lt.scale;
+    lp.t.bz = lt.bz; lp.t.gram_w = lt.gram_w; lp.t.b = lt.b; lp.t.sqab = lt.sqab; lp.t.sum_b = lt.sum_b;
+    lp.t.sum_sqb = lt.sum_sqb; lp.t.n_aug = lt.n_aug;
+    lp.dlink = ctx->d_dlink; lp.linkfnull = ctx->d_linkfnull; lp.fnull = ctx->d_fnull; lp.list = ctx->d_idx_full;
+    lp.count = ctx->d_counts; lp.mom = ctx->d_mom; lp.phi = phi_dev; lp.status = ctx->d_status;
+    const size_t msm = sizeof(double) * (size_t)S;
+    if (msm + 8192 > (size_t)ctx->max_smem_optin)
+        return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: %d coalitions per plan exceed the shared-memory staging", S);
+    const int tasks = n * nout;
+    const int mgrid = tasks < ctx->sm_count * 2 ? tasks : ctx->sm_count * 2;
+#define DKS_MOM(W, MULTI)                                                                                                 \
+    CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_moments_kernel<W, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm)); \
+    dks::l1::l1_moments_kernel<W, MULTI><<<mgrid, dks::l1::MOM_THREADS, msm, ctx->stream>>>(lp);
+    if (nout == 1) {
+        if (pg.W == 1) { DKS_MOM(1, false) } else { DKS_MOM(2, false) }
+    } else {
+        if (pg.W == 1) { DKS_MOM(1, true) } else { DKS_MOM(2, true) }
+    }
+#undef DKS_MOM
+    const size_t per_warp = dks::l1::lars_smem_per_warp(G);
+    const size_t gram_bytes = sizeof(double) * (size_t)G * G;
+    const size_t budget = (size_t)ctx->max_smem_optin - 2048;
+    // the Gram matrix of the path goes to shared memory when at least four warps still fit next to it
+    const int stage_gram = (gram_bytes + 4 * per_warp <= budget) ? 1 : 0;
+    int wpc = (int)((budget - (stage_gram ? gram_bytes : 0)) / per_warp);
+    if (wpc < 1) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory", G, G);
+    if (wpc > 8) wpc = 8;
+    const size_t lsm = per_warp * wpc + (stage_gram ? gram_bytes : 0);
+    int per_sm = (int)((size_t)ctx->max_smem_optin / (lsm + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 4) per_sm = 4;
+    int lgrid = (tasks + wpc - 1) / wpc;
+    if (lgrid > ctx->sm_count * per_sm) lgrid = ctx->sm_count * per_sm;
+    CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_lars_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm));
+    dks::l1::l1_lars_kernel<<<lgrid, 32 * wpc, lsm, ctx->stream>>>(lp, wpc, stage_gram);
     return DKS_OK;
 }
 
@@ -249,6 +305,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     }
 
     int kernel = ctx->kernel_choice;
+    const int kernel_req = kernel;
     CUDA_TRY(record_ev(ctx, 2));
 
     // ---- shared-plan fast path: instances whose varying set is all G groups, evaluated against the plan's Dm table
@@ -257,14 +314,21 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     const bool fast = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
                       ctx->act == DKS_ACT_BINARY_LOGISTIC && G >= 2 && pg.dmT != nullptr &&
                       pg.S == dks_effective_S(G, ctx->nsamples_req) && (pg.W <= 2 || pg.ptw != nullptr);
-    if (kernel == DKS_KERNEL_SHARED && !fast && ext_z == nullptr && pg.z != nullptr)
-        return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head");
+    // softmax and identity heads, up to 128 groups: per-class sums of the softmax coalition kernel (dks_multi.cuh) or the
+    // identity head's tables, then a solve per (instance, output)
+    const bool sfm = ctx->act == DKS_ACT_SOFTMAX;
+    const bool multi = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
+                       (sfm || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128 && ctx->plan_mode == 0 &&
+                       pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) && (!sfm || ctx->h_smx[G].dm != nullptr);
+    if (kernel == DKS_KERNEL_SHARED && !fast && !multi && ext_z == nullptr && pg.z != nullptr)
+        return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head, or the softmax / identity head "
+                    "with at most 128 groups");
     // non-uniform background weights: the weighted instantiations of the shared-plan kernels (dks_shared.cuh)
     const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn;
-    if (fast) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
+    if (fast || multi) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
     // the general kernel below (instances that are not on the shared-plan path) forks off here and joins at the end
     cudaStream_t gstream = ctx->stream;
-    if (fast && ctx->side_stream != nullptr) {
+    if ((fast || multi) && ctx->side_stream != nullptr) {
         CUDA_TRY(cudaEventRecord(ctx->ev_fork, ctx->stream));
         CUDA_TRY(cudaStreamWaitEvent(ctx->side_stream, ctx->ev_fork, 0));
         gstream = ctx->side_stream;
@@ -282,9 +346,9 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
         if (pg.W > 2)
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
-        if (!fast || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic head) and the "
-                        "l1 tables of the M=%d plan (dks_set_l1_tables)", G);
+        if (!(fast || multi) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S)
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax or "
+                        "identity head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
     }
     const bool fused = fast && !l1 && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
                        dks::shared_path::fused_config(ctx->N, G, pg.S_pad, ctx->sm_count, ctx->max_smem_optin,
@@ -349,46 +413,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         wp.linkfnull = ctx->d_linkfnull; wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts;
         wp.phi = phi_dev;
         if (l1) {
-            // upstream's l1 branch: moments of y per instance, then the LARS path + criterion + restricted WLS, one warp each
-            const dks_ctx::L1Dev& lt = ctx->h_l1[G];
-            const size_t need_m = (size_t)n * (2 * G + 4);
-            if (need_m > ctx->cap_mom) { TRY(dev_alloc(&ctx->d_mom, need_m)); ctx->cap_mom = need_m; ctx->epoch++; }
-            dks::l1::Params lp;
-            memset(&lp, 0, sizeof(lp));
-            lp.n = n; lp.N = ctx->N; lp.G = G; lp.C = ctx->C; lp.S = S; lp.S_pad = S_pad; lp.link = ctx->link;
-            lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.sums = ctx->d_sums; lp.z = pg.z; lp.w = pg.w;
-            lp.t.gram_raw = lt.gram_raw; lp.t.gram_norm = lt.gram_norm; lp.t.colsum = lt.colsum; lp.t.scale = lt.scale;
-            lp.t.bz = lt.bz; lp.t.gram_w = lt.gram_w; lp.t.b = lt.b; lp.t.sqab = lt.sqab; lp.t.sum_b = lt.sum_b;
-            lp.t.sum_sqb = lt.sum_sqb; lp.t.n_aug = lt.n_aug;
-            lp.dlink = ctx->d_dlink; lp.linkfnull = ctx->d_linkfnull; lp.fnull = ctx->d_fnull; lp.list = ctx->d_idx_full;
-            lp.count = ctx->d_counts; lp.mom = ctx->d_mom; lp.phi = phi_dev; lp.status = ctx->d_status;
-            const size_t msm = sizeof(double) * (size_t)S;
-            if (msm + 8192 > (size_t)ctx->max_smem_optin)
-                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: %d coalitions per plan exceed the shared-memory staging", S);
-            const int mgrid = n < ctx->sm_count * 2 ? n : ctx->sm_count * 2;
-            if (pg.W == 1) {
-                CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_moments_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm));
-                dks::l1::l1_moments_kernel<1><<<mgrid, dks::l1::MOM_THREADS, msm, ctx->stream>>>(lp);
-            } else {
-                CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_moments_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm));
-                dks::l1::l1_moments_kernel<2><<<mgrid, dks::l1::MOM_THREADS, msm, ctx->stream>>>(lp);
-            }
-            const size_t per_warp = dks::l1::lars_smem_per_warp(G);
-            const size_t gram_bytes = sizeof(double) * (size_t)G * G;
-            const size_t budget = (size_t)ctx->max_smem_optin - 2048;
-            // the Gram matrix of the path goes to shared memory when at least four warps still fit next to it
-            const int stage_gram = (gram_bytes + 4 * per_warp <= budget) ? 1 : 0;
-            int wpc = (int)((budget - (stage_gram ? gram_bytes : 0)) / per_warp);
-            if (wpc < 1) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory", G, G);
-            if (wpc > 8) wpc = 8;
-            const size_t lsm = per_warp * wpc + (stage_gram ? gram_bytes : 0);
-            int per_sm = (int)((size_t)ctx->max_smem_optin / (lsm + 1024));
-            if (per_sm < 1) per_sm = 1;
-            if (per_sm > 4) per_sm = 4;
-            int lgrid = (n + wpc - 1) / wpc;
-            if (lgrid > ctx->sm_count * per_sm) lgrid = ctx->sm_count * per_sm;
-            CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_lars_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm));
-            dks::l1::l1_lars_kernel<<<lgrid, 32 * wpc, lsm, ctx->stream>>>(lp, wpc, stage_gram);
+            TRY(launch_l1(ctx, pg, n, 1, dks::shared_path::HeadSource{}, phi_dev));
             path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
         } else if (pg.W > 2) {
             // more than 128 groups: link, float64 product with the host-supplied projection, remainder (dks_wide.cuh)
@@ -434,6 +459,59 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         CUDA_TRY(cudaGetLastError());
         p.list = ctx->d_idx_other;      // the general kernel below takes the remaining instances
         p.count = ctx->d_counts + 1;
+    } else if (multi) {
+        const int S = pg.S, S_pad = pg.S_pad, C = ctx->C;
+        dks::shared_path::HeadSource src;
+        src.act = ctx->act; src.ntab = (G + 3) / 4; src.msums = nullptr; src.XT = ctx->d_XT;
+        if (sfm) {
+            // the workspace is C n S_pad floats: the engine explains these heads in row blocks of 2 / C the binary path's
+            const size_t need = (size_t)n * C * S_pad;
+            if (need > ctx->cap_msums) { TRY(dev_alloc(&ctx->d_msums, need)); ctx->cap_msums = need; ctx->epoch++; }
+            dks::multi::SoftmaxParams mp;
+            memset(&mp, 0, sizeof(mp));
+            mp.n = n; mp.N = ctx->N; mp.G = G; mp.S = S; mp.S_pad = S_pad; mp.ntab = src.ntab; mp.scale = ctx->scale;
+            mp.dm = ctx->h_smx[G].dm; mp.lo = ctx->h_smx[G].lo; mp.wn = ctx->d_wn; mp.z = pg.z; mp.XT = ctx->d_XT; mp.BW = ctx->d_BW;
+            mp.scores = ctx->d_scores; mp.list = ctx->d_idx_full; mp.count = ctx->d_counts; mp.sums = ctx->d_msums;
+            int grid = 0;
+            const int nl = dks::multi::launch_explain_softmax(mp, C, pg.W, n, ctx->sm_count, ctx->max_smem_optin, ctx->stream,
+                                                              &grid);
+            if (nl == 0) return fail(DKS_ERR_CUDA, "softmax coalition kernel: %s", cudaGetErrorString(cudaGetLastError()));
+            ctx->launches += nl;
+            path[DKS_PATH_SHARED] = DKS_SHARED_SOFTMAX; path[DKS_PATH_CHUNKS] = nl;
+            path[DKS_PATH_WARPS] = dks::multi::MC_WARPS; path[DKS_PATH_GRID] = grid;
+            src.msums = ctx->d_msums;
+        } else {
+            path[DKS_PATH_SHARED] = DKS_SHARED_AFFINE;       // y straight from the tables: no coalition kernel
+        }
+        if (l1) {
+            TRY(launch_l1(ctx, pg, n, C, src, phi_dev));
+            ctx->launches += 2;
+            path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
+        } else {
+            dks::shared_path::WlsSharedParams wp;
+            memset(&wp, 0, sizeof(wp));
+            wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link; wp.uniform_w = 1;
+            wp.src = src; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink; wp.linkfnull = ctx->d_linkfnull;
+            wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts; wp.phi = phi_dev;
+            const size_t wsm = dks::shared_path::wls_shared_smem(G);
+            int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 24 * 1024));
+            if (per_sm > 4) per_sm = 4;
+            if (per_sm < 1) per_sm = 1;
+            const int tasks = n * C;
+            const int wgrid = tasks < ctx->sm_count * per_sm ? tasks : ctx->sm_count * per_sm;
+            if (pg.W == 1) {
+                CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
+                dks::shared_path::wls_shared_kernel<1, true><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
+            } else {
+                CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
+                dks::shared_path::wls_shared_kernel<2, true><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
+            }
+            ctx->launches += 1;
+            path[DKS_PATH_SOLVE] = DKS_SOLVE_WLS_SHARED;
+        }
+        CUDA_TRY(cudaGetLastError());
+        p.list = ctx->d_idx_other;
+        p.count = ctx->d_counts + 1;
     }
     if (l1 && !ctx->l1_others_plain) {
         // instances with a partial varying set would need their own selection: reported, not computed
@@ -451,9 +529,9 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
             return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
         }
-        if (!fast)
-            return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, kernel "
-                        "'auto' or 'shared', shared plan of M=%d uploaded)", G);
+        if (!fast && !multi)
+            return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, or the "
+                        "softmax / identity head up to 128 groups; kernel 'auto' or 'shared', shared plan of M=%d uploaded)", G);
         dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 1;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
@@ -471,9 +549,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         TRY(dks::tc_launch(ctx, p, gstream));
         path[DKS_PATH_GENERAL] = DKS_GENERAL_TC;
     } else {
-        const bool sfm = ctx->act == DKS_ACT_SOFTMAX;
         size_t smem = dks::simt_smem_bytes(S_cap, ctx->N, ctx->G, sfm ? ctx->R : 1, sfm ? ctx->C : 1);
-        if ((long long)smem > (long long)ctx->max_smem_optin && fast) {
+        if ((long long)smem > (long long)ctx->max_smem_optin && (fast || multi)) {
             // the shared-plan path took the instances whose groups all vary; the general kernel is sized for the largest
             // plan set and cannot hold it.  The instances left for it (often none) are reported, not computed.
             dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
@@ -483,6 +560,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             CUDA_TRY(join());
             CUDA_TRY(record_ev(ctx, 3));
             return DKS_OK;
+        }
+        if ((long long)smem > (long long)ctx->max_smem_optin && !multi && pg.z == nullptr &&
+            (kernel_req == DKS_KERNEL_AUTO || kernel_req == DKS_KERNEL_SHARED) && ext_z == nullptr && ctx->plan_mode == 0 &&
+            (sfm || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128) {
+            // the softmax / identity head's shared-plan path takes these instances once the plan of G groups is uploaded
+            ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
+            return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
         }
         if ((long long)smem > (long long)ctx->max_smem_optin)
             return fail(DKS_ERR_UNSUPPORTED, "SIMT kernel needs %zu B of shared memory (> %d): N*G or nsamples too large",
@@ -585,7 +669,7 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_fnull); dev_free(&ctx->d_linkfnull); dev_free(&ctx->d_BWs); dev_free(&ctx->d_bases);
     dev_free(&ctx->d_wbf); dev_free(&ctx->d_wn); dev_free(&ctx->d_plans); dev_free(&ctx->d_X); dev_free(&ctx->d_XW); dev_free(&ctx->d_XT);
     dev_free(&ctx->d_vflag); dev_free(&ctx->d_vmask); dev_free(&ctx->d_M); dev_free(&ctx->d_dlink);
-    dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_sums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
+    dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_sums); dev_free(&ctx->d_msums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
     dev_free(&ctx->d_status); ctx->d_hist = nullptr; ctx->d_counts = nullptr; dev_free(&ctx->d_yw); dev_free(&ctx->d_betaw); dev_free(&ctx->d_acache); dev_free(&ctx->d_phi); if (ctx->h_phi_pin) { cudaFreeHost(ctx->h_phi_pin); ctx->h_phi_pin = nullptr; } dev_free(&ctx->d_genz); dev_free(&ctx->d_genw); dev_free(&ctx->d_genchol); dev_free(&ctx->d_genainv); dev_free(&ctx->d_afix); dev_free(&ctx->d_sinfo); dev_free(&ctx->d_extz);
     dev_free(&ctx->d_extw);
     dev_free(&ctx->dbg_T);
@@ -758,6 +842,7 @@ int dks_fit(dks_ctx* ctx) {
         free_plan_allocs(ctx, -1);
         memset(ctx->h_plans, 0, sizeof(ctx->h_plans));
         memset(ctx->h_l1, 0, sizeof(ctx->h_l1));
+        memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
         ctx->max_plan_S = 0;
         CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));
     }
@@ -825,6 +910,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
         free_plan_allocs(ctx, M);
         memset(&ctx->h_plans[M], 0, sizeof(PlanDev));
         memset(&ctx->h_l1[M], 0, sizeof(ctx->h_l1[M]));
+        memset(&ctx->h_smx[M], 0, sizeof(ctx->h_smx[M]));
         ctx->h_afix[M] = nullptr;
         ctx->epoch++;
     }
@@ -914,6 +1000,24 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
             pd.pmat64 = pm64; pd.dvec64 = dv64; pd.kpad = kpad;
         }
     }
+    if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_SOFTMAX && W <= 2) {
+        // softmax head: per-class Dm table and row bounds for the full varying set (dks_multi.cuh)
+        const int C = ctx->C;
+        float* sd = nullptr; float* sl = nullptr;
+        CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)C * ctx->N * pd.S_pad));
+        ctx->plan_allocs[M].push_back(sd);
+        CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)C * pd.S_pad));
+        ctx->plan_allocs[M].push_back(sl);
+        if (W == 1)
+            dks::multi::plan_softmax_kernel<1><<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW,
+                ctx->d_scores, ctx->N, M, C, ctx->scale, sd, sl);
+        else
+            dks::multi::plan_softmax_kernel<2><<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW,
+                ctx->d_scores, ctx->N, M, C, ctx->scale, sd, sl);
+        ctx->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        ctx->h_smx[M].dm = sd; ctx->h_smx[M].lo = sl;
+    }
     ctx->h_plans[M] = pd;
     ctx->epoch++;
     ctx->h_afix[M] = nullptr;                       // sampling info of a replaced plan is stale
@@ -931,6 +1035,7 @@ int dks_clear_plans(dks_ctx* ctx) {
     ctx->epoch++;
     memset(ctx->h_plans, 0, sizeof(ctx->h_plans));
     memset(ctx->h_l1, 0, sizeof(ctx->h_l1));
+    memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
     memset(ctx->h_afix, 0, sizeof(ctx->h_afix));
     memset(ctx->h_sinfo, 0, sizeof(ctx->h_sinfo));
     ctx->max_plan_S = 0;

@@ -139,7 +139,11 @@ struct dks_ctx {
     };
     L1Dev h_l1[DKS_MAX_GROUPS + 1] = {};
     int l1_mode = 0, l1_k = 0, l1_others_plain = 0;
-    double* d_mom = nullptr;     // [n][2G + 4] per-instance moments of y
+    // softmax head, full varying set (M == G): per-class Dm [C][N][S_pad] = 2^(d_c(s, j) - max_c d_c(s, j)) and row bounds
+    // lo [C][S_pad] = min_j log2 Dm_c(s, j) (dks_multi.cuh); owned by plan_allocs[M], cleared with the plan
+    struct SmxDev { const float* dm; const float* lo; };
+    SmxDev h_smx[DKS_MAX_GROUPS + 1] = {};
+    double* d_mom = nullptr;     // [n][outputs solved][2G + 4] per-instance moments of y
     size_t cap_mom = 0;
     double* d_yw = nullptr;      // [n][S_pad] link-space y of the wide (more than 128 groups) solve
     double* d_betaw = nullptr;   // [n][kpw] its coefficients before the delta term
@@ -170,7 +174,10 @@ struct dks_ctx {
     size_t cap_X = 0;
     const double* cur_X = nullptr;
     double* d_XW = nullptr;
-    double* d_XT = nullptr;      // [n][ceil(G/4)][16] nibble tables of the scaled grouped contributions (binary head)
+    double* d_XT = nullptr;      // [n][R][ceil(G/4)][16] nibble tables of the scaled grouped contributions (binary head:
+                                 // R = 1; softmax: log2 e XW; identity head: XW - Bbar)
+    float* d_msums = nullptr;    // [n][C][S_pad] per-class sums of the softmax coalition kernel
+    size_t cap_msums = 0;
     unsigned char* d_vflag = nullptr;
     uint64_t* d_vmask = nullptr;
     int* d_M = nullptr;

@@ -208,7 +208,7 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
                             double kappa, int link, int ipb, double* __restrict__ XW, uint64_t* __restrict__ vmask,
                             int* __restrict__ Mcnt, double* __restrict__ dlink, int* __restrict__ hist,
                             int* __restrict__ counts, int* __restrict__ idx_full, int* __restrict__ idx_other,
-                            double* __restrict__ XT, double xt_scale) {
+                            double* __restrict__ XT, double xt_scale, const double* __restrict__ xt_sub) {
     extern __shared__ __align__(16) unsigned char prep_smem[];
     double* sXW = reinterpret_cast<double*>(prep_smem);                        // [ipb][G][R]
     double* sX = sXW + (size_t)ipb * G * R;                                    // STAGE: [ipb][D]
@@ -259,18 +259,23 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
     }
     __syncthreads();
     if (XT != nullptr) {
-        // XT[i][t][x] = xt_scale * sum_{b<4} bit_b(x) XW[i][4t+b]: the shared-plan kernel adds one table entry per nibble
-        // of a coalition row instead of one term per group (R == 1)
+        // XT[i][r][t][x] = xt_scale * sum_{b<4} bit_b(x) (XW[i][4t+b][r] - xt_sub[4t+b][r]): the shared-plan kernels add
+        // one table entry per nibble of a coalition row instead of one term per group (xt_sub: the identity head's Bbar)
         const int ntab = (G + 3) / 4;
-        for (int idx = threadIdx.x; idx < ipb * ntab * 16; idx += blockDim.x) {
-            const int li = idx / (ntab * 16), rem = idx - li * ntab * 16, t = rem >> 4, x = rem & 15;
+        for (int idx = threadIdx.x; idx < ipb * R * ntab * 16; idx += blockDim.x) {
+            const int li = idx / (R * ntab * 16), rem = idx - li * R * ntab * 16, r = rem / (ntab * 16);
+            const int t = (rem >> 4) - r * ntab, x = rem & 15;
             const int i = i0 + li;
             if (i >= n) continue;
             double acc = 0.0;
 #pragma unroll
             for (int b = 0; b < 4; ++b)
-                if (((x >> b) & 1) && 4 * t + b < G) acc += sXW[(size_t)li * G + 4 * t + b];
-            XT[((size_t)i * ntab + t) * 16 + x] = xt_scale * acc;
+                if (((x >> b) & 1) && 4 * t + b < G) {
+                    const int k = 4 * t + b;
+                    acc += xt_sub != nullptr ? sXW[((size_t)li * G + k) * R + r] - xt_sub[(size_t)k * R + r]
+                                             : sXW[((size_t)li * G + k) * R + r];
+                }
+            XT[(((size_t)i * R + r) * ntab + t) * 16 + x] = xt_scale * acc;
         }
     }
     for (int li = threadIdx.x; li < ipb; li += blockDim.x) {

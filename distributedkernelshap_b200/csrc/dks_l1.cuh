@@ -41,6 +41,8 @@ struct Tables {              // per plan (M == G), device pointers
 
 struct Params {
     int n, N, G, C, S, S_pad, link, mode, kfeat;
+    int nout;                // outputs solved per instance: 1 (binary head: class 1, class 0 its negation) or C
+    shared_path::HeadSource src;   // softmax / identity heads (nout == C)
     const float2* sums;      // [n][S_pad]
     const uint64_t* z;       // [S][W]
     const double* w;         // [S]
@@ -50,40 +52,74 @@ struct Params {
     const double* fnull;
     const int* list;
     const int* count;
-    double* mom;             // [n][2G + 4]: c, u, T1, Qw, R
+    double* mom;             // [n][nout][2G + 4]: c, u, T1, Qw, R
     double* phi;             // [C][n][G]
     int* status;
 };
 
 // ---- moments of y over the plan rows: c_k, u_k (k < G) and T1 = sum b y, Qw = sum w y^2, R = sum (sqrt a + sqrt b) y
+// MULTI: the softmax and identity heads, one task per (instance, output) with y from p.src; the fixed point is scaled per
+// task (shared_path::fix_exponent; Qw, quadratic in y, by its own even exponent) and the moments are stored unscaled, so the
+// LARS path compares them with its absolute thresholds in the units of y.
 constexpr int MOM_THREADS = 256;
-template <int W>
+template <int W, bool MULTI = false>
 __global__ void __launch_bounds__(MOM_THREADS) l1_moments_kernel(Params p) {
     extern __shared__ double s_y[];                       // [S]
     __shared__ long long s_part[MOM_THREADS / 32][32];
     __shared__ LogTabEntry s_logtab[DKS_LOGTAB_SIZE];
+    __shared__ double s_bound[MOM_THREADS / 32][2];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int G = p.G;
-    const int cnt = *p.count;
+    const int nout = MULTI ? p.nout : 1;
+    const int cnt = *p.count * nout;
     if ((int)blockIdx.x >= cnt) return;
     if (threadIdx.x < DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x);
     __syncthreads();
     const double lf1 = p.linkfnull[1], f1 = p.fnull[1], inv_n = 1.0 / (double)p.N;
     for (int m = blockIdx.x; m < cnt; m += gridDim.x) {
-        const int i = p.list[m];
+        const int i = p.list[MULTI ? m / nout : m];
+        const int cls = MULTI ? m % nout : 1;
         const float2* sums = p.sums + (size_t)i * p.S_pad;
-        double* mom = p.mom + (size_t)i * (2 * G + 4);
+        double* mom = p.mom + ((size_t)i * nout + (MULTI ? cls : 0)) * (2 * G + 4);
         // pass 0: y into shared memory + the three scalars
         long long t1 = 0, qw = 0, rr = 0;
-        for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
-            const float2 a = sums[s];
-            double y;
-            if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(a.x, a.y, s_logtab) - lf1;
-            else y = (double)a.x * inv_n - f1;
-            s_y[s] = y;
-            t1 += to_fix(p.t.b[s] * y);
-            qw += to_fix(p.w[s] * y * y);
-            rr += to_fix(p.t.sqab[s] * y);
+        double sc = 1.0, isc = 1.0, sq = 1.0, isq = 1.0;
+        if constexpr (MULTI) {
+            const double fnc = p.fnull[cls], lfc = p.linkfnull[cls];
+            double b1 = 0.0, b2 = 0.0;        // bounds of the linear moments and of Qw
+            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
+                const double y = shared_path::head_y<W>(p.src, i, cls, p.C, s, p.S_pad, p.z + (size_t)s * W, p.link, inv_n,
+                                                        fnc, lfc);
+                s_y[s] = y;
+                b1 += (p.w[s] + p.t.b[s] + p.t.sqab[s]) * fabs(y);
+                b2 += p.w[s] * y * y;
+            }
+            b1 = warp_sum(b1); b2 = warp_sum(b2);
+            if (lane == 0) { s_bound[wib][0] = b1; s_bound[wib][1] = b2; }
+            __syncthreads();
+            double t1b = 0.0, t2b = 0.0;
+#pragma unroll
+            for (int wq = 0; wq < MOM_THREADS / 32; ++wq) { t1b += s_bound[wq][0]; t2b += s_bound[wq][1]; }
+            const int e1 = shared_path::fix_exponent(t1b), e2 = shared_path::fix_exponent(t2b) >> 1;
+            sc = ldexp(1.0, e1); isc = ldexp(1.0, -e1);
+            sq = ldexp(1.0, e2); isq = ldexp(1.0, -2 * e2);
+            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
+                const double y = s_y[s];
+                t1 += to_fix(p.t.b[s] * y * sc);
+                qw += to_fix(p.w[s] * (y * sq) * (y * sq));
+                rr += to_fix(p.t.sqab[s] * y * sc);
+            }
+        } else {
+            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
+                const float2 a = sums[s];
+                double y;
+                if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(a.x, a.y, s_logtab) - lf1;
+                else y = (double)a.x * inv_n - f1;
+                s_y[s] = y;
+                t1 += to_fix(p.t.b[s] * y);
+                qw += to_fix(p.w[s] * y * y);
+                rr += to_fix(p.t.sqab[s] * y);
+            }
         }
         t1 = warp_sum_ll(t1); qw = warp_sum_ll(qw); rr = warp_sum_ll(rr);
         if (lane == 0) { s_part[wib][0] = t1; s_part[wib][1] = qw; s_part[wib][2] = rr; }
@@ -91,7 +127,7 @@ __global__ void __launch_bounds__(MOM_THREADS) l1_moments_kernel(Params p) {
         if (threadIdx.x < 3) {
             long long acc = 0;
             for (int wq = 0; wq < MOM_THREADS / 32; ++wq) acc += s_part[wq][threadIdx.x];
-            mom[2 * G + threadIdx.x] = from_fix(acc);
+            mom[2 * G + threadIdx.x] = MULTI ? from_fix(acc) * (threadIdx.x == 1 ? isq : isc) : from_fix(acc);
         }
         __syncthreads();
         // sixteen coefficients of c and u per pass over the rows
@@ -101,7 +137,7 @@ __global__ void __launch_bounds__(MOM_THREADS) l1_moments_kernel(Params p) {
             for (int k = 0; k < 16; ++k) { Ck[k] = 0; Uk[k] = 0; }
 #pragma unroll 2
             for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
-                const double y = s_y[s];
+                const double y = MULTI ? s_y[s] * sc : s_y[s];
                 const long long vc = to_fix(p.w[s] * y), vu = to_fix(p.t.b[s] * y);
                 const uint32_t zb = (uint32_t)(p.z[(size_t)s * W + (k0 >> 6)] >> (k0 & 63));
 #pragma unroll
@@ -118,7 +154,7 @@ __global__ void __launch_bounds__(MOM_THREADS) l1_moments_kernel(Params p) {
                 long long acc = 0;
                 for (int wq = 0; wq < MOM_THREADS / 32; ++wq) acc += s_part[wq][threadIdx.x];
                 const int k = k0 + (threadIdx.x & 15);
-                if (k < G) mom[(threadIdx.x < 16 ? 0 : G) + k] = from_fix(acc);
+                if (k < G) mom[(threadIdx.x < 16 ? 0 : G) + k] = MULTI ? from_fix(acc) * isc : from_fix(acc);
             }
             __syncthreads();
         }
@@ -208,10 +244,13 @@ __global__ void l1_lars_kernel(Params p, int warps_per_cta, int stage_gram) {
     const int max_iter = lasso ? 500 : p.kfeat;
     const size_t slab = (size_t)p.n * M;
 
-    for (int m = blockIdx.x * warps_per_cta + wib; m < cnt; m += gridDim.x * warps_per_cta) {
-        const int i = p.list[m];
-        const double* mom = p.mom + (size_t)i * (2 * M + 4);
-        const double delta = p.dlink[(size_t)i * C + 1];
+    const int nout = p.nout;
+    for (int m = blockIdx.x * warps_per_cta + wib; m < cnt * nout; m += gridDim.x * warps_per_cta) {
+        // one warp per (instance, output): upstream's solve runs the selection for each output on its own
+        const int i = p.list[m / nout];
+        const int cls = nout == 1 ? 1 : m % nout;
+        const double* mom = p.mom + ((size_t)i * nout + (nout == 1 ? 0 : cls)) * (2 * M + 4);
+        const double delta = p.dlink[(size_t)i * C + cls];
         const double T1 = mom[2 * M], Qw = mom[2 * M + 1], R = mom[2 * M + 2];
         const double ybar = lasso ? (R - delta * p.t.sum_sqb) / nsamp : 0.0;
         const double yy = (double)M * Qw - 2.0 * delta * T1 + delta * delta * p.t.sum_b - nsamp * ybar * ybar;
@@ -395,12 +434,13 @@ __global__ void l1_lars_kernel(Params p, int warps_per_cta, int stage_gram) {
             if (on) { if (lane == 0) perm[q] = v; ++q; }
         }
         __syncwarp();
-        double* phi1 = p.phi + slab + (size_t)i * M;
-        double* phi0 = p.phi + (size_t)i * M;
-        for (int v = lane; v < M; v += 32) { phi1[v] = 0.0; phi0[v] = 0.0; }
+        double* phi1 = p.phi + (size_t)cls * slab + (size_t)i * M;
+        double* phi0 = p.phi + (size_t)i * M;       // binary head only: class 0 is the negation of class 1
+        const bool anti = nout == 1;
+        for (int v = lane; v < M; v += 32) { phi1[v] = 0.0; if (anti) phi0[v] = 0.0; }
         __syncwarp();
         if (q == 1) {
-            if (lane == 0) { double val = fabs(delta) < 1e-10 ? 0.0 : delta; phi1[perm[0]] = val; phi0[perm[0]] = val == 0.0 ? 0.0 : -val; }
+            if (lane == 0) { double val = fabs(delta) < 1e-10 ? 0.0 : delta; phi1[perm[0]] = val; if (anti) phi0[perm[0]] = val == 0.0 ? 0.0 : -val; }
         } else if (q >= 2) {
             const int nA = q - 1, Lv = perm[q - 1];
             const double* gw = p.t.gram_w;
@@ -438,14 +478,14 @@ __global__ void l1_lars_kernel(Params p, int warps_per_cta, int stage_gram) {
                 sum += val;
                 if (fabs(val) < 1e-10) val = 0.0;
                 phi1[perm[r]] = val;
-                phi0[perm[r]] = val == 0.0 ? 0.0 : -val;
+                if (anti) phi0[perm[r]] = val == 0.0 ? 0.0 : -val;
             }
             sum = wsum(sum);
             if (lane == 0) {
                 double last = delta - sum;
                 if (fabs(last) < 1e-10) last = 0.0;
                 phi1[Lv] = last;
-                phi0[Lv] = last == 0.0 ? 0.0 : -last;
+                if (anti) phi0[Lv] = last == 0.0 ? 0.0 : -last;
             }
         }
         __syncwarp();

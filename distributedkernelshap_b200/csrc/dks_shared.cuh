@@ -681,8 +681,51 @@ inline int launch_explain_shared(SharedParams p, int words, int sm_count, int ma
     return launches;
 }
 
+// Where the softmax and identity heads' y(i, c, s) comes from on the shared-plan path: the per-class sums of the softmax
+// coalition kernel (dks_multi.cuh), or the identity head's float64 nibble tables of XW - Bbar (prep_kernel), for which
+// ey_c(s) = fnull_c + sum_k z_sk (XW_i[k][c] - Bbar[k][c]) needs no coalition kernel at all.
+struct HeadSource {
+    int act;                 // DKS_ACT_SOFTMAX or DKS_ACT_IDENTITY
+    int ntab;                // nibble tables per class: ceil(G / 4)
+    const float* msums;      // [n][C][S_pad] sum_j w'_j p_c(s, j), w'_j = N w_j
+    const double* XT;        // [n][C][ntab][16]
+};
+template <int W>
+__device__ __forceinline__ double head_y(const HeadSource& h, int i, int c, int C, int s, int S_pad, const uint64_t* zrow,
+                                         int link, double inv_n, double fn, double lf) {
+    if (h.act == DKS_ACT_SOFTMAX) {
+        const float* ms = h.msums + (size_t)i * C * S_pad + s;
+        const double e = (double)ms[(size_t)c * S_pad];
+        if (link == DKS_LINK_LOGIT) {
+            double rest = 0.0;                   // 1 - ey_c as the sum of the other classes: no cancellation
+            for (int c2 = 0; c2 < C; ++c2) if (c2 != c) rest += (double)ms[(size_t)c2 * S_pad];
+            return log(e / rest) - lf;
+        }
+        return e * inv_n - fn;
+    }
+    const double* xt = h.XT + ((size_t)i * C + c) * h.ntab * 16;
+    double a0 = 0.0, a1 = 0.0;
+    for (int t = 0; t < h.ntab; t += 2) {
+        a0 += __ldg(xt + t * 16 + (int)((zrow[t >> 4] >> (4 * (t & 15))) & 15ull));
+        if (t + 1 < h.ntab) a1 += __ldg(xt + (t + 1) * 16 + (int)((zrow[(t + 1) >> 4] >> (4 * ((t + 1) & 15))) & 15ull));
+    }
+    return link_f(fn + (a0 + a1), link) - lf;
+}
+
+// The 2^-40 fixed point holds |values| < 8e6.  Regression outputs have no such bound and small ones would lose relative
+// precision, so the multi-output solves scale each (instance, output) by 2^e, exact, chosen so that `bound` (a bound of
+// every fixed-point sum) becomes at most 2^22; the scale is undone before any absolute threshold.
+__device__ __forceinline__ int fix_exponent(double bound) {
+    if (!(bound > 0.0) || !isfinite(bound)) return 0;
+    int ex;
+    frexp(bound, &ex);                           // bound < 2^ex
+    const int e = 22 - ex;
+    return e < -1000 ? -1000 : (e > 1000 ? 1000 : e);
+}
+
 struct WlsSharedParams {
     int n, N, G, C, S, S_pad, link, uniform_w;
+    HeadSource src;          // softmax / identity heads (the MULTI instantiation)
     const float2* sums;      // [n][S_pad]
     const uint64_t* z;
     const double* w;
@@ -859,17 +902,21 @@ inline bool launch_wls_pmat(const WlsPmatParams& p, int n, int sm_count, int max
 
 // Persistent CTAs of 8 warps, each looping over instances: y = link(ey) - link(fnull) per coalition, E^T W y in 2^-40
 // fixed point (integer adds: exact, order-independent), beta = inv(E^T W E) (E^T W y), phi.
+// MULTI: the softmax and identity heads -- one task per (instance, output), y from p.src, each output's phi written on its
+// own (no antisymmetry), the fixed point scaled per task (fix_exponent).
 constexpr int WLS_THREADS = 256;
 inline size_t wls_shared_smem(int G) { return sizeof(double) * (size_t)(G - 1) * (G - 1); }
-template <int W>
+template <int W, bool MULTI = false>
 __global__ void __launch_bounds__(WLS_THREADS) wls_shared_kernel(WlsSharedParams p) {
     extern __shared__ double s_ainv[];                   // [(G-1)][(G-1)]
     __shared__ long long s_part[WLS_THREADS / 32][64 * W];
     __shared__ double s_rhs[64 * W];
     __shared__ LogTabEntry s_logtab[DKS_LOGTAB_SIZE];
+    __shared__ double s_bound[WLS_THREADS / 32];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int G = p.G, nA = G - 1, L = G - 1;
-    const int cnt = *p.count;
+    const int nout = MULTI ? p.C : 1;
+    const int cnt = *p.count * nout;
     if ((int)blockIdx.x >= cnt) return;
     if (threadIdx.x < DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x);
     for (int idx = threadIdx.x; idx < nA * nA; idx += blockDim.x) s_ainv[idx] = p.ainv[idx];
@@ -877,9 +924,29 @@ __global__ void __launch_bounds__(WLS_THREADS) wls_shared_kernel(WlsSharedParams
     const double lf1 = p.linkfnull[1], f1 = p.fnull[1], inv_n = 1.0 / (double)p.N;
     const size_t slab = (size_t)p.n * G;
     for (int m = blockIdx.x; m < cnt; m += gridDim.x) {
-        const int i = p.list[m];
-        const double delta = p.dlink[(size_t)i * p.C + 1];
+        const int i = p.list[MULTI ? m / nout : m];
+        const int cls = MULTI ? m % nout : 1;
+        const double delta = p.dlink[(size_t)i * p.C + cls];
         const float2* sums = p.sums + (size_t)i * p.S_pad;
+        const double fnc = p.fnull[cls], lfc = p.linkfnull[cls];
+        double sc = 1.0, isc = 1.0;
+        if constexpr (MULTI) {
+            double b = 0.0;                              // sum_s |w_s (y_s - z_sL delta)| bounds every coefficient's sum
+            for (int s = threadIdx.x; s < p.S; s += WLS_THREADS) {
+                const uint64_t* zrow = p.z + (size_t)s * W;
+                const bool zl = (zrow[L >> 6] >> (L & 63)) & 1ull;
+                const double y = head_y<W>(p.src, i, cls, p.C, s, p.S_pad, zrow, p.link, inv_n, fnc, lfc);
+                b += fabs(p.w[s] * (y - (zl ? delta : 0.0)));
+            }
+            b = warp_sum(b);
+            if (lane == 0) s_bound[wib] = b;
+            __syncthreads();
+            double tot = 0.0;
+#pragma unroll
+            for (int wq = 0; wq < WLS_THREADS / 32; ++wq) tot += s_bound[wq];     // fixed order: the same e every run
+            const int e = fix_exponent(tot);
+            sc = ldexp(1.0, e); isc = ldexp(1.0, -e);
+        }
         // thread handles coalitions tid, tid+256, ...; sixteen coefficients of E^T W y per pass over the rows
         for (int k0 = 0; k0 < nA; k0 += 16) {
             long long Tk[16];
@@ -887,13 +954,17 @@ __global__ void __launch_bounds__(WLS_THREADS) wls_shared_kernel(WlsSharedParams
             for (int k = 0; k < 16; ++k) Tk[k] = 0;
 #pragma unroll 2
             for (int s = threadIdx.x; s < p.S; s += WLS_THREADS) {
-                const float2 a = sums[s];
                 double y;
-                if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(a.x, a.y, s_logtab) - lf1;
-                else y = (p.uniform_w ? (double)a.x * inv_n : (double)a.x) - f1;
                 const uint64_t* zrow = p.z + (size_t)s * W;
+                if constexpr (MULTI) {
+                    y = head_y<W>(p.src, i, cls, p.C, s, p.S_pad, zrow, p.link, inv_n, fnc, lfc);
+                } else {
+                    const float2 a = sums[s];
+                    if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(a.x, a.y, s_logtab) - lf1;
+                    else y = (p.uniform_w ? (double)a.x * inv_n : (double)a.x) - f1;
+                }
                 const bool zl = (zrow[L >> 6] >> (L & 63)) & 1ull;
-                const double v = p.w[s] * (y - (zl ? delta : 0.0));
+                const double v = MULTI ? p.w[s] * (y - (zl ? delta : 0.0)) * sc : p.w[s] * (y - (zl ? delta : 0.0));
                 const uint64_t zw = zrow[k0 >> 6];               // a 16-bit window never straddles two words
                 const uint32_t zb = (uint32_t)((zl ? ~zw : zw) >> (k0 & 63));
                 const long long vi = zl ? -to_fix(v) : to_fix(v);
@@ -914,7 +985,7 @@ __global__ void __launch_bounds__(WLS_THREADS) wls_shared_kernel(WlsSharedParams
             long long acc = 0;
 #pragma unroll
             for (int wq = 0; wq < WLS_THREADS / 32; ++wq) acc += s_part[wq][threadIdx.x];
-            s_rhs[threadIdx.x] = from_fix(acc);
+            s_rhs[threadIdx.x] = MULTI ? from_fix(acc) * isc : from_fix(acc);
         }
         __syncthreads();
         if (wib == 0) {
@@ -944,12 +1015,12 @@ __global__ void __launch_bounds__(WLS_THREADS) wls_shared_kernel(WlsSharedParams
                 if (k < G) {
                     double val = k < nA ? beta[h] : delta - sum;       // the eliminated (last) group takes the remainder
                     if (fabs(val) < 1e-10) val = 0.0;
-                    p.phi[slab + (size_t)i * G + k] = val;
-                    p.phi[(size_t)i * G + k] = (val == 0.0) ? 0.0 : -val;
+                    p.phi[(size_t)cls * slab + (size_t)i * G + k] = val;
+                    if (!MULTI) p.phi[(size_t)i * G + k] = (val == 0.0) ? 0.0 : -val;
                 }
             }
         }
-        // s_part / s_rhs are rewritten only after the next instance's row loop, which ends with __syncthreads
+        // s_part / s_rhs / s_bound are rewritten only after the next task's row loop, which ends with __syncthreads
     }
 }
 

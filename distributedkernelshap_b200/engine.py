@@ -161,8 +161,8 @@ class GpuKernelExplainer:
         """Upstream's ``solve`` runs an l1 feature selection before the constrained WLS when ``l1_reg`` is 'aic' / 'bic' /
         'num_features(k)', or under 'auto' when fewer than 20% of the coalition space is evaluated.  Without ``hist``:
         whether the M histogram is needed to decide.  With it: ``(mode, k, others_plain)`` for ``dks_set_l1`` -- the
-        selection runs on the shared-plan path (csrc/dks_l1.cuh) for the instances whose groups all vary; what that path
-        does not cover is refused, never silently solved without the selection."""
+        selection runs on the shared-plan path (csrc/dks_l1.cuh) for the instances whose groups all vary (per output for the
+        softmax and identity heads); what that path does not cover is refused, never silently solved without the selection."""
         if l1_reg in (False, 0):
             return False if hist is None else (0, 0, 0)
         G = self.data.groups_size
@@ -198,8 +198,6 @@ class GpuKernelExplainer:
                 "set); the CUDA engine runs the selection for instances whose groups all vary only -- pass l1_reg=False")
         if self.plan_mode != "shared":
             raise NotImplementedError("l1 feature selection runs with plan_mode='shared' only")
-        if self.spec.act_code != _cabi.ACT_BINARY_LOGISTIC:
-            raise NotImplementedError("l1 feature selection needs the binary-logistic head (the shared-plan path)")
         mode, k = explicit if explicit is not None else (1, 0)
         return (mode, k, 1 if len(present) > 1 else 0)
 
@@ -318,10 +316,11 @@ class GpuKernelExplainer:
         self._set_nsamples(nsamples)
         need_hist = self._l1_guard(l1_reg, nsamples)
 
-        if n > MAX_ROWS_PER_CALL:     # large inputs go through in row chunks (results are independent per row)
+        rows = self._rows_per_call()
+        if n > rows:                  # large inputs go through in row chunks (results are independent per row)
             parts, fx_parts = [], []
-            for lo in range(0, n, MAX_ROWS_PER_CALL):
-                hi = min(n, lo + MAX_ROWS_PER_CALL)
+            for lo in range(0, n, rows):
+                hi = min(n, lo + rows)
                 sub = dict(nsamples=nsamples, l1_reg=l1_reg, row_offset=row_offset + lo)
                 if plans is not None:
                     sub["plans"] = plans[lo:hi]
@@ -372,6 +371,13 @@ class GpuKernelExplainer:
         if single:
             return [phi[c, 0] for c in range(self.D)]
         return [phi[c] for c in range(self.D)]
+
+    def _rows_per_call(self):
+        """Rows per C-ABI call.  The softmax head's shared-plan path keeps C per-class sums per coalition where the binary
+        head keeps two: its row blocks are 2 / C as long, so that the per-call workspace stays the binary path's."""
+        if self.spec.act_code == _cabi.ACT_SOFTMAX and self.D > 2:
+            return MAX_ROWS_PER_CALL * 2 // self.D
+        return MAX_ROWS_PER_CALL
 
     def link_predictions(self):
         """``link(f(x))`` of the rows of the last ``shap_values`` call, ``[n, C]`` (``[n]`` for scalar-output models):
@@ -547,7 +553,7 @@ class GpuKernelExplainer:
         return {"prepare": float(out[0]), "coalitions": float(out[1]), "total": float(out[2])}
 
     _PATH_NAMES = {
-        "shared": ("none", "fused", "smem", "regs"),
+        "shared": ("none", "fused", "smem", "regs", "softmax", "affine"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
         "general": ("none", "tc", "simt", "flagged"),
     }
@@ -555,7 +561,7 @@ class GpuKernelExplainer:
     def last_path(self):
         """Which kernels the last explain call launched (``dks_last_path``), recorded when the call was enqueued (a
         replayed CUDA graph reports the call it captured): ``shared`` (shared-plan coalition kernel: 'none' | 'fused' |
-        'smem' | 'regs'), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
+        'smem' | 'regs' | 'softmax', or 'affine' for the identity head, whose y needs no coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
         are reported as unsupported, not computed), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``

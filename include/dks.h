@@ -226,6 +226,8 @@ int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by th
 #define DKS_SHARED_FUSED 1       /* explain_shared_fused_kernel: link + projection solve inside */
 #define DKS_SHARED_SMEM 2        /* explain_shared_smem_kernel (Dm rows in shared memory) */
 #define DKS_SHARED_REGS 3        /* explain_shared_kernel (Dm rows in registers; DKS_SHARED_DM=regs) */
+#define DKS_SHARED_SOFTMAX 4     /* explain_softmax_kernel: per-class sums of the softmax head (C = R classes) */
+#define DKS_SHARED_AFFINE 5      /* identity head: y read from per-class tables, no coalition kernel */
 #define DKS_SOLVE_NONE 0
 #define DKS_SOLVE_FUSED 1
 #define DKS_SOLVE_PMAT 2         /* wls_pmat_kernel */
