@@ -1,5 +1,7 @@
 // libdks.so -- host side of the C ABI declared in include/dks.h.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC (see build.py)
+#include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -364,6 +366,10 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         fp.count = ctx->d_counts; fp.pmat64 = pg.pmat64; fp.dvec = pg.dvec64; fp.dlink = ctx->d_dlink;
         fp.linkfnull = ctx->d_linkfnull; fp.fnull = ctx->d_fnull; fp.acc = ctx->d_acc; fp.done = ctx->d_done; fp.phi = phi_dev;
         fp.wn = wn;
+        const bool table = ctx->opt_fused_table && pg.ltab != nullptr;
+        if (table) {
+            fp.ltab = pg.ltab; fp.ltab_rows = pg.ltab_rows; fp.ltab_inv_h = pg.ltab_inv_h; fp.ltab_fb = ctx->d_ltab_fb;
+        }
         if (ctx->peer_world > 1 && ctx->push_in_kernel) {
             double* slabs[16];
             int np = 0;
@@ -385,6 +391,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         path[DKS_PATH_SHARED] = DKS_SHARED_FUSED; path[DKS_PATH_CHUNKS] = 1; path[DKS_PATH_WARPS] = fcfg.warps;
         path[DKS_PATH_GRID] = ctx->sm_count; path[DKS_PATH_FUSED_B] = fcfg.B; path[DKS_PATH_FUSED_NI] = 1;
         path[DKS_PATH_SOLVE] = DKS_SOLVE_FUSED; path[DKS_PATH_FUSED_CTA_WARPS] = fcfg.slices * fcfg.kw;
+        path[DKS_PATH_FUSED_TABLE] = table ? 1 : 0;
         CUDA_TRY(cudaGetLastError());
         p.list = ctx->d_idx_other;
         p.count = ctx->d_counts + 1;
@@ -597,6 +604,95 @@ int check_status(dks_ctx* ctx) {
     return fail(ctx->h_status[0], "explain kernel reported status %d (detail %d)", ctx->h_status[0], ctx->h_status[1]);
 }
 
+// Chebyshev nodes of [0, 1] and the inverse of their Vandermonde matrix (Gauss-Jordan, partial pivoting)
+dks::shared_path::LinkTabFit make_link_tab_fit() {
+    constexpr int K = dks::shared_path::LTAB_NODES;
+    dks::shared_path::LinkTabFit f;
+    double a[K][2 * K];
+    for (int m = 0; m < K; ++m) {
+        f.t[m] = 0.5 - 0.5 * cos((2 * m + 1) * 3.14159265358979323846 / (2 * K));
+        for (int c = 0; c < K; ++c) { a[m][c] = pow(f.t[m], c); a[m][K + c] = m == c ? 1.0 : 0.0; }
+    }
+    for (int c = 0; c < K; ++c) {
+        int piv = c;
+        for (int r = c + 1; r < K; ++r) if (fabs(a[r][c]) > fabs(a[piv][c])) piv = r;
+        for (int k = 0; k < 2 * K; ++k) std::swap(a[c][k], a[piv][k]);
+        const double d = a[c][c];
+        for (int k = 0; k < 2 * K; ++k) a[c][k] /= d;
+        for (int r = 0; r < K; ++r) {
+            if (r == c) continue;
+            const double m = a[r][c];
+            for (int k = 0; k < 2 * K; ++k) a[r][k] -= m * a[c][k];
+        }
+    }
+    for (int r = 0; r < K; ++r) for (int c = 0; c < K; ++c) f.vinv[r * K + c] = a[r][K + c];
+    return f;
+}
+
+// The fused kernel's link table of a plan (dks_fused.cuh) at h = 1/4, refined once to h = 1/8.  pd.ltab stays NULL (the
+// plan keeps the exact loop) when both miss LTAB_TOL or the table would pass LTAB_BUDGET.
+int build_link_table(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz) {
+    using namespace dks::shared_path;
+    static const LinkTabFit fit = make_link_tab_fit();
+    const int N = ctx->N, S_pad = pd.S_pad;
+    cudaStream_t st = ctx->stream;
+    struct Scratch {
+        std::vector<void*> p;
+        ~Scratch() { for (void* q : p) cudaFree(q); }
+    } scratch;
+    double* ld = nullptr; double* wd = nullptr; LinkTabRow* rows = nullptr; unsigned long long* merr = nullptr;
+    CUDA_TRY(cudaMalloc((void**)&ld, sizeof(double) * (size_t)N * S_pad)); scratch.p.push_back(ld);
+    CUDA_TRY(cudaMalloc((void**)&rows, sizeof(LinkTabRow) * (size_t)S_pad)); scratch.p.push_back(rows);
+    CUDA_TRY(cudaMalloc((void**)&merr, sizeof(unsigned long long))); scratch.p.push_back(merr);
+    if (!ctx->uniform_w) {
+        std::vector<double> w(N);
+        for (int j = 0; j < N; ++j) w[j] = (double)N * ctx->h_wbg[j];
+        CUDA_TRY(cudaMalloc((void**)&wd, sizeof(double) * N)); scratch.p.push_back(wd);
+        CUDA_TRY(cudaMemcpy(wd, w.data(), sizeof(double) * N, cudaMemcpyHostToDevice));
+    }
+    if (ctx->d_ltab_fb == nullptr) {
+        TRY(dev_alloc(&ctx->d_ltab_fb, 1));
+        CUDA_TRY(cudaMemset(ctx->d_ltab_fb, 0, sizeof(unsigned long long)));
+    }
+    std::vector<LinkTabRow> hr(S_pad);
+    for (double h : {0.25, 0.125}) {
+        plan_ltab_rows_kernel<<<cdiv(S_pad, 128), 128, 0, st>>>(dz, pd.S, S_pad, ctx->d_BW, ctx->d_scores, N, ctx->G, ctx->scale,
+                                                                pd.dme, wd, h, ld, rows);
+        ctx->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(hr.data(), rows, sizeof(LinkTabRow) * S_pad, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        long long total = 0;
+        int maxn = 0;
+        for (LinkTabRow& r : hr) { r.off = (int)(total < (1LL << 30) ? total : 0); total += r.nint; maxn = std::max(maxn, r.nint); }
+        const size_t bytes = sizeof(LinkTabEntry) * (size_t)total + sizeof(LinkTabRow) * (size_t)S_pad;
+        if (bytes > LTAB_BUDGET || maxn > 65535 * 128) return DKS_OK;     // a finer grid only makes it larger
+        LinkTabEntry* tab = nullptr;
+        CUDA_TRY(cudaMalloc((void**)&tab, sizeof(LinkTabEntry) * (size_t)std::max(total, 1LL))); scratch.p.push_back(tab);
+        CUDA_TRY(cudaMemcpyAsync(rows, hr.data(), sizeof(LinkTabRow) * S_pad, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemsetAsync(merr, 0, sizeof(unsigned long long), st));
+        const dim3 grid(S_pad, cdiv(maxn, 128));
+        if (maxn > 0) {
+            plan_ltab_fit_kernel<<<grid, 128, 0, st>>>(fit, rows, ld, S_pad, wd, N, ctx->link, h, tab, merr);
+            ctx->launches += 1;
+            CUDA_TRY(cudaGetLastError());
+        }
+        unsigned long long bits = 0;
+        CUDA_TRY(cudaMemcpyAsync(&bits, merr, sizeof(bits), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        double err;
+        memcpy(&err, &bits, sizeof(err));
+        if (err <= LTAB_TOL) {
+            scratch.p.pop_back();                                    // tab and rows now belong to the plan
+            scratch.p.erase(std::find(scratch.p.begin(), scratch.p.end(), (void*)rows));
+            ctx->plan_allocs[M].push_back(tab); ctx->plan_allocs[M].push_back(rows);
+            pd.ltab = tab; pd.ltab_rows = rows; pd.ltab_inv_h = 1.0 / h; pd.ltab_bytes = (long long)bytes;
+            return DKS_OK;
+        }
+    }
+    return DKS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -669,7 +765,7 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_fnull); dev_free(&ctx->d_linkfnull); dev_free(&ctx->d_BWs); dev_free(&ctx->d_bases);
     dev_free(&ctx->d_wbf); dev_free(&ctx->d_wn); dev_free(&ctx->d_plans); dev_free(&ctx->d_X); dev_free(&ctx->d_XW); dev_free(&ctx->d_XT);
     dev_free(&ctx->d_vflag); dev_free(&ctx->d_vmask); dev_free(&ctx->d_M); dev_free(&ctx->d_dlink);
-    dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_sums); dev_free(&ctx->d_msums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
+    dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_sums); dev_free(&ctx->d_msums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_ltab_fb); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
     dev_free(&ctx->d_status); ctx->d_hist = nullptr; ctx->d_counts = nullptr; dev_free(&ctx->d_yw); dev_free(&ctx->d_betaw); dev_free(&ctx->d_acache); dev_free(&ctx->d_phi); if (ctx->h_phi_pin) { cudaFreeHost(ctx->h_phi_pin); ctx->h_phi_pin = nullptr; } dev_free(&ctx->d_genz); dev_free(&ctx->d_genw); dev_free(&ctx->d_genchol); dev_free(&ctx->d_genainv); dev_free(&ctx->d_afix); dev_free(&ctx->d_sinfo); dev_free(&ctx->d_extz);
     dev_free(&ctx->d_extw);
     dev_free(&ctx->dbg_T);
@@ -998,6 +1094,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
             ctx->launches += 2;
             CUDA_TRY(cudaGetLastError());
             pd.pmat64 = pm64; pd.dvec64 = dv64; pd.kpad = kpad;
+            if (ctx->N <= dks::shared_path::MAXN) TRY(build_link_table(ctx, pd, M, dz));
         }
     }
     if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_SOFTMAX && W <= 2) {
@@ -1481,6 +1578,7 @@ int dks_set_option(dks_ctx* ctx, const char* name, int value) {
     if (key == "fused") ctx->opt_fused = value;
     else if (key == "fused_warps") ctx->opt_fused_warps = value;
     else if (key == "fused_batch") ctx->opt_fused_B = value;
+    else if (key == "fused_table") ctx->opt_fused_table = value != 0;
     else if (key == "push_in_kernel") ctx->push_in_kernel = value != 0;
     else if (key == "graph") ctx->graph_enabled = value != 0;
     else if (key == "graph_timing") ctx->opt_graph_timing = value != 0;
@@ -1518,6 +1616,19 @@ int dks_last_timings(dks_ctx* ctx, float* ms3) {
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n) {
     REQUIRE(ctx && out && n >= 0, "dks_last_path: bad arguments");
     for (int k = 0; k < n; ++k) out[k] = k < DKS_PATH_FIELDS ? ctx->last_path[k] : 0;
+    return DKS_OK;
+}
+
+int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fallback_passes) {
+    BIND(ctx);
+    REQUIRE(M >= 0 && M <= DKS_MAX_GROUPS && table_bytes && fallback_passes, "dks_fused_table_info: bad arguments");
+    *table_bytes = ctx->h_plans[M].ltab != nullptr ? ctx->h_plans[M].ltab_bytes : 0;
+    unsigned long long fb = 0;
+    if (ctx->d_ltab_fb != nullptr) {
+        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+        CUDA_TRY(cudaMemcpy(&fb, ctx->d_ltab_fb, sizeof(fb), cudaMemcpyDeviceToHost));
+    }
+    *fallback_passes = (int64_t)fb;
     return DKS_OK;
 }
 

@@ -16,6 +16,8 @@
 // 64-bit words per coalition row of a plan over M groups: the kernels exist for rows of 1, 2 and 16 words
 __host__ __device__ __forceinline__ int dks_plan_words(int M) { return M <= 64 ? 1 : (M <= 128 ? 2 : 16); }
 
+namespace dks { namespace shared_path { struct LinkTabEntry; struct LinkTabRow; } }   // dks_fused.cuh
+
 // ---- device-visible plan table entry: one shared coalition plan per number of varying groups M ----------
 struct PlanDev {
     const uint64_t* z;   // [S][W] coalition bits in upstream row order (W = dks_plan_words(M))
@@ -30,6 +32,10 @@ struct PlanDev {
     const double* dvec64;  // [kpad] P z_L with the float64 P
     const double* ptw;     // [S_pad][kpw] float64 P^T supplied by the host for plans of more than 128 groups (dks_wide.cuh)
     const double* dvecw;   // [kpw] P z_L
+    const dks::shared_path::LinkTabEntry* ltab;      // per-row link table of the fused kernel, NULL if not built
+    const dks::shared_path::LinkTabRow* ltab_rows;   // [S_pad]
+    double ltab_inv_h;                               // 1 / its grid step
+    long long ltab_bytes;                            // table and row headers
     int kpw;
     int kpad;
     int S;
@@ -234,6 +240,8 @@ struct dks_ctx {
                                                    // (measured slower than the separate coalesced push kernel: DESIGN.md §7)
     // tuning knobs (dks_set_option; defaults from the environment at dks_create: DKS_FUSED, DKS_FUSED_WARPS, ...)
     int opt_fused = 1, opt_fused_warps = 0, opt_fused_B = 0;
+    int opt_fused_table = 1;                       // 0: the fused kernel ignores the plans' link tables (exact loop only)
+    unsigned long long* d_ltab_fb = nullptr;       // fused passes that fell back from the link table to the exact loop
     bool opt_graph_timing = false;   // keep the timing event records inside a captured graph (dks_last_timings after replays)
     bool timing_valid = false, last_was_graph = false;
     bool last_fused = false;                       // the last explain ran the fused shared-plan kernel

@@ -27,6 +27,102 @@ namespace shared_path {
 
 constexpr int FUSED_MAX_PEERS = 16;
 
+// ---- per-row link table ----------------------------------------------------------------------------------------------
+// With a shared plan and all groups varying, an instance enters coalition row s only through one scalar, x = a(i, s) + dme[s]:
+//     y(i, s) + link(fnull) = L_s(x) = ln sum_j w'_j / (1 + 2^x Dm(s, j)) - ln sum_j w'_j 2^x Dm(s, j) / (1 + 2^x Dm(s, j))
+// (identity link: sum_j w'_j / (1 + 2^x Dm(s, j)) / N), with w'_j = N w_j.  L_s depends on the plan and the background only,
+// so dks_set_shared_plan tabulates it per row in float64 (DESIGN.md 5.0.1), and the fused kernel reads y from the table in a
+// constant number of operations instead of summing N sigmoids.  Row s covers [x_lo, x_lo + nint h): x_lo is
+// -LTAB_MARGIN - max_j log2 Dm(s, j) rounded down to the grid, the end is at or past LTAB_MARGIN - min_j log2 Dm(s, j) (columns
+// of zero weight excluded).  Beyond either end every 2^x Dm is below 2^-33 or above 2^33; the kernel takes the exact loop
+// there.  Interval k holds the degree-5 polynomial in t = (x - x_lo) / h - k in [0, 1) through L_s at six Chebyshev nodes:
+// c0, c1 in float64, c2 .. c5 (at most ~1e-2) in float32, 32 bytes.  The build evaluates every interval against float64
+// L_s at t = 0, t = 1 and midway between consecutive nodes, exactly as the kernel evaluates it; a plan that misses LTAB_TOL
+// at h = 1/4 is rebuilt at h = 1/8, and one that misses it again, or whose table would pass LTAB_BUDGET bytes, has no table.
+constexpr double LTAB_MARGIN = 33.0;
+constexpr double LTAB_TOL = 1e-9;
+constexpr size_t LTAB_BUDGET = (size_t)256 << 20;
+constexpr int LTAB_NODES = 6;
+
+struct __align__(16) LinkTabEntry { double c0, c1; float c2, c3, c4, c5; };
+struct __align__(16) LinkTabRow { double x_lo; int off, nint; };       // nint = 0: padding row
+static_assert(sizeof(LinkTabEntry) == 32, "one interval is 32 bytes");
+
+// the fitting nodes in [0, 1] and the inverse of their Vandermonde matrix (monomial coefficients from node values)
+struct LinkTabFit { double t[LTAB_NODES]; double vinv[LTAB_NODES * LTAB_NODES]; };
+
+__host__ __device__ __forceinline__ double ltab_poly(const LinkTabEntry& e, double t) {
+    const float tf = (float)t;
+    const float q = fmaf(tf, fmaf(tf, fmaf(tf, e.c5, e.c4), e.c3), e.c2);
+    return fma(t, fma(t, (double)q, e.c1), e.c0);
+}
+
+// float64 L_s(x) from the row's log2 Dm (ld, stride S_pad); wd = w'_j, NULL for a uniform background.  With u = 2^z, z = x +
+// log2 Dm: p1 = 1 / (1 + u) and p0 = 1 / (1 + 1 / u) from e = 2^-|z| (no overflow, no cancellation)
+__device__ double ltab_exact(double x, const double* __restrict__ ld, int S_pad, const double* __restrict__ wd, int N, int link) {
+    double s1 = 0.0, s0 = 0.0;
+    for (int j = 0; j < N; ++j) {
+        const double w = wd ? wd[j] : 1.0;
+        const double z = x + ld[(size_t)j * S_pad];
+        const double e = exp2(-fabs(z));
+        const double r = w / (1.0 + e);
+        if (z > 0.0) { s1 += e * r; s0 += r; }
+        else { s1 += r; s0 += e * r; }
+    }
+    return link == DKS_LINK_LOGIT ? log(s1) - log(s0) : s1 / (double)N;
+}
+
+// per row: log2 Dm in float64 (the exponents plan_dm_kernel rounds to float32) and the row's domain at step h
+__global__ void plan_ltab_rows_kernel(const uint64_t* __restrict__ z, int S, int S_pad, const double* __restrict__ BW,
+                                      const double* __restrict__ scores, int N, int G, double scale,
+                                      const double* __restrict__ dme, const double* __restrict__ wd, double h,
+                                      double* __restrict__ ld, LinkTabRow* __restrict__ rows) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= S_pad) return;
+    LinkTabRow r;
+    r.x_lo = 0.0; r.off = 0; r.nint = 0;
+    if (s < S) {
+        double lmin = 1.0e300, lmax = -1.0e300;
+        for (int j = 0; j < N; ++j) {
+            const double v = plan_d(z + s, BW, scores, j, G, scale) - dme[s];
+            ld[(size_t)j * S_pad + s] = v;
+            if (wd == nullptr || wd[j] > 0.0) { lmin = fmin(lmin, v); lmax = fmax(lmax, v); }
+        }
+        r.x_lo = floor((-LTAB_MARGIN - lmax) / h) * h;
+        const double n = ceil((LTAB_MARGIN - lmin - r.x_lo) / h);
+        r.nint = n < 1.0e9 ? (int)n : 1000000000;         // the host's budget check turns such a plan down
+    }
+    rows[s] = r;
+}
+
+// one thread per interval (blockIdx.x = row): fit, store, and the largest error against float64 L_s (as ordered bits)
+__global__ void plan_ltab_fit_kernel(LinkTabFit f, const LinkTabRow* __restrict__ rows, const double* __restrict__ ld, int S_pad,
+                                     const double* __restrict__ wd, int N, int link, double h, LinkTabEntry* __restrict__ tab,
+                                     unsigned long long* __restrict__ maxerr) {
+    const int s = blockIdx.x, k = blockIdx.y * blockDim.x + threadIdx.x;
+    const LinkTabRow r = rows[s];
+    if (k >= r.nint) return;
+    const double x0 = r.x_lo + (double)k * h;
+    const double* lds = ld + s;
+    double fv[LTAB_NODES], c[LTAB_NODES];
+    for (int m = 0; m < LTAB_NODES; ++m) fv[m] = ltab_exact(x0 + h * f.t[m], lds, S_pad, wd, N, link);
+    for (int a = 0; a < LTAB_NODES; ++a) {
+        double v = 0.0;
+        for (int m = 0; m < LTAB_NODES; ++m) v = fma(f.vinv[a * LTAB_NODES + m], fv[m], v);
+        c[a] = v;
+    }
+    LinkTabEntry e;
+    e.c0 = c[0]; e.c1 = c[1]; e.c2 = (float)c[2]; e.c3 = (float)c[3]; e.c4 = (float)c[4]; e.c5 = (float)c[5];
+    double err = 0.0;
+    for (int q = 0; q <= LTAB_NODES; ++q) {
+        const double t = q == 0 ? 0.0 : (q == LTAB_NODES ? 1.0 : 0.5 * (f.t[q - 1] + f.t[q]));
+        err = fmax(err, fabs(ltab_poly(e, t) - ltab_exact(x0 + h * t, lds, S_pad, wd, N, link)));
+    }
+    if (!(err <= 1.0)) err = 1.0;                          // NaN or worse: the plan fails verification
+    atomicMax(maxerr, (unsigned long long)__double_as_longlong(err));
+    tab[(size_t)r.off + k] = e;
+}
+
 struct FusedParams {
     int n, N, G, C, S, S_pad, link, B;
     double scale;
@@ -47,6 +143,10 @@ struct FusedParams {
     int npeers;              // multi-GPU push: phi of every finished instance also goes to these buffers ([C][n][G] each)
     double* const* peer_phi; // [npeers] device array of the peers' slab addresses (NULL on one GPU)
     const float* wn;         // [N] weighted backgrounds: N w_j (the weighted instantiations only; dks_shared.cuh)
+    const LinkTabEntry* ltab;        // the plan's link table (below), NULL: every pass takes the exact loop
+    const LinkTabRow* ltab_rows;     // [S_pad]
+    double ltab_inv_h;               // 1 / grid step
+    unsigned long long* ltab_fb;     // passes that left the table's domain and took the exact loop (cumulative)
 };
 
 // one 16-column chunk whose valid columns are a run-time count: nq full quads (pair sums / products), then rem < 4 raw
@@ -306,118 +406,150 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
             }
 
             for (int it = 0; it < my_n; it += NI) {
-                float A[NI];
-                bool risky_l = false;
+                double a[NI], v[NI], y[NI];
+                bool in_tab = true;
+                // the row's domain in the link table (a padding row has none and needs none: its y is 0), reloaded per
+                // pass (an L1 hit) so that it holds no registers through the exact loop
+                LinkTabRow trow;
+                trow.x_lo = 0.0; trow.off = 0; trow.nint = 0;
+                if (p.ltab != nullptr && row_ok) trow = p.ltab_rows[s];
 #pragma unroll
                 for (int u = 0; u < NI; ++u) {
-                    const double a = ((nx[u][0] + nx[u][1]) + (nx[u][2] + nx[u][3])) + es;
+                    a[u] = ((nx[u][0] + nx[u][1]) + (nx[u][2] + nx[u][3])) + es;
                     {
                         const size_t o = (size_t)i_nx[u] * xstride;
                         nx[u][0] = __ldg(xb0 + o); nx[u][1] = __ldg(xb1 + o); nx[u][2] = __ldg(xb2 + o); nx[u][3] = __ldg(xb3 + o);
                         const int it2 = it + 2 * NI + u < last_it ? it + 2 * NI + u : last_it;
                         i_nx[u] = p.list[first + it2 * stride];
                     }
-                    // A = 2^a = 2^n 2^f, n = rint(a) through the 1.5 * 2^52 trick (no conversion instructions), |f| <= 1/2; the
-                    // exponent is clamped to [-120, 120] (saturated scores; the clamped scalar path below takes A > 1e18)
-                    const double tm = a + 6755399441055744.0;
-                    int an_i = __double2loint(tm);
-                    an_i = an_i < -120 ? -120 : (an_i > 120 ? 120 : an_i);
-                    A[u] = ex2_approx((float)(a - (tm - 6755399441055744.0))) * __int_as_float((127 + an_i) << 23);
-                    risky_l = risky_l || A[u] > 1.0e18f;
+                    v[u] = (a[u] - trow.x_lo) * p.ltab_inv_h;
+                    in_tab = in_tab && (!row_ok || (v[u] >= 0.0 && v[u] < (double)trow.nint));
                 }
-                float s1[NI], s0[NI];
-                if constexpr (WT) {
-                    if (__any_sync(0xffffffffu, risky_l)) {
+                if (p.ltab != nullptr && __all_sync(0xffffffffu, in_tab)) {
+                    // y from the row's table: one 32-byte interval and a Horner evaluation
 #pragma unroll
-                        for (int u = 0; u < NI; ++u) row_sums_clamped_w(p.DmT, p.wn, N, p.S_pad, s, A[u], s1[u], s0[u]);
+                    for (int u = 0; u < NI; ++u) {
+                        y[u] = 0.0;
+                        if (row_ok) {
+                            const int k = (int)v[u];
+                            const LinkTabEntry* ep = p.ltab + (size_t)trow.off + k;
+                            const double2 c01 = __ldg(reinterpret_cast<const double2*>(ep));
+                            const float4 c25 = __ldg(reinterpret_cast<const float4*>(ep) + 1);
+                            LinkTabEntry e;
+                            e.c0 = c01.x; e.c1 = c01.y; e.c2 = c25.x; e.c3 = c25.y; e.c4 = c25.z; e.c5 = c25.w;
+                            y[u] = ltab_poly(e, v[u] - (double)k) - yf;
+                        }
+                    }
+                } else {
+                    // a lane's x is outside its row's table (or the plan has none): the exact loop over the background
+                    if (p.ltab != nullptr && lane == 0) atomicAdd(p.ltab_fb, 1ull);
+                    float A[NI];
+                    bool risky_l = false;
+#pragma unroll
+                    for (int u = 0; u < NI; ++u) {
+                        // A = 2^a = 2^n 2^f, n = rint(a) through the 1.5 * 2^52 trick (no conversion instructions), |f| <= 1/2; the
+                        // exponent is clamped to [-120, 120] (saturated scores; the clamped scalar path below takes A > 1e18)
+                        const double tm = a[u] + 6755399441055744.0;
+                        int an_i = __double2loint(tm);
+                        an_i = an_i < -120 ? -120 : (an_i > 120 ? 120 : an_i);
+                        A[u] = ex2_approx((float)(a[u] - (tm - 6755399441055744.0))) * __int_as_float((127 + an_i) << 23);
+                        risky_l = risky_l || A[u] > 1.0e18f;
+                    }
+                    float s1[NI], s0[NI];
+                    if constexpr (WT) {
+                        if (__any_sync(0xffffffffu, risky_l)) {
+#pragma unroll
+                            for (int u = 0; u < NI; ++u) row_sums_clamped_w(p.DmT, p.wn, N, p.S_pad, s, A[u], s1[u], s0[u]);
+                        } else {
+                            // every quad of the slice (all columns compiled in with NCT), two accumulator chains per instance
+                            f32x2 A2[NI], AA2[NI], acc1[NI][2], acc0[NI][2];
+#pragma unroll
+                            for (int u = 0; u < NI; ++u) {
+                                const float AA = A[u] * A[u];
+                                A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA);
+                                acc1[u][0] = acc1[u][1] = acc0[u][0] = acc0[u][1] = f2_pack(0.f, 0.f);
+                            }
+                            // quad q on accumulator chain h (a constant after unrolling: the accumulators stay in registers)
+                            auto quad = [&](int q, int h) {
+                                const float4 sq = sl[(2 * q) * 32 + lane], xy = sl[(2 * q + 1) * 32 + lane];
+                                const float2 w2 = sW2[q];
+#pragma unroll
+                                for (int u = 0; u < NI; ++u) quad_acc_w(A2[u], AA2[u], sq, xy, w2, one2, acc1[u][h], acc0[u][h]);
+                            };
+                            if (NCT) {
+#pragma unroll
+                                for (int q = 0; q < dm_quads(NCT); ++q) quad(q, q & 1);
+                            } else {
+                                // run-time N: the slice's even number of quads in pairs (a zero quad past an odd count adds 0)
+#pragma unroll 2
+                                for (int q = 0; q < nqw; q += 2) { quad(q, 0); quad(q + 1, 1); }
+                            }
+#pragma unroll
+                            for (int u = 0; u < NI; ++u) {
+                                float q0, q1, q2, q3;
+                                f2_unpack(f2_add(acc1[u][0], acc1[u][1]), q0, q1);
+                                f2_unpack(f2_add(acc0[u][0], acc0[u][1]), q2, q3);
+                                s1[u] = q0 + q1;
+                                s0[u] = q2 + q3;
+                            }
+                        }
+                    } else if (__any_sync(0xffffffffu, risky_l)) {
+                        // A^2 would leave the fp32 range: clamped scalar path on the raw row from global memory (saturated scores)
+#pragma unroll
+                        for (int u = 0; u < NI; ++u) {
+                            float r1 = 0.f, r0 = 0.f;
+                            for (int j = 0; j + 1 < N; j += 2)
+                                pair_acc<true>(A[u], p.DmT[(size_t)j * p.S_pad + s], p.DmT[(size_t)(j + 1) * p.S_pad + s], r1, r0);
+                            if (N & 1) single_acc(A[u], p.DmT[(size_t)(N - 1) * p.S_pad + s], r1, r0);
+                            s1[u] = r1; s0[u] = r0;
+                        }
                     } else {
-                        // every quad of the slice (all columns compiled in with NCT), two accumulator chains per instance
-                        f32x2 A2[NI], AA2[NI], acc1[NI][2], acc0[NI][2];
+                        f32x2 A2[NI], AA2[NI], AA2x2[NI];
+                        f32x2 acc1[NI][2], acc0[NI][2];
+                        float t1s[NI], t0s[NI];
 #pragma unroll
                         for (int u = 0; u < NI; ++u) {
                             const float AA = A[u] * A[u];
-                            A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA);
+                            A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA); AA2x2[u] = f2_pack(2.f * AA, 2.f * AA);
                             acc1[u][0] = acc1[u][1] = acc0[u][0] = acc0[u][1] = f2_pack(0.f, 0.f);
+                            t1s[u] = t0s[u] = 0.f;
                         }
-                        // quad q on accumulator chain h (a constant after unrolling: the accumulators stay in registers)
-                        auto quad = [&](int q, int h) {
-                            const float4 sq = sl[(2 * q) * 32 + lane], xy = sl[(2 * q + 1) * 32 + lane];
-                            const float2 w2 = sW2[q];
+                        float v[2][16];
+                        dm_ld16(sl, 0, nq, lane, v[0]);
 #pragma unroll
-                            for (int u = 0; u < NI; ++u) quad_acc_w(A2[u], AA2[u], sq, xy, w2, one2, acc1[u][h], acc0[u][h]);
-                        };
-                        if (NCT) {
+                        for (int c = 0; c < MAXCH; ++c) {
+                            if (c < nch) {
+                                if (c + 1 < nch) dm_ld16(sl, c + 1, nq, lane, v[(c + 1) & 1]);
 #pragma unroll
-                            for (int q = 0; q < dm_quads(NCT); ++q) quad(q, q & 1);
-                        } else {
-                            // run-time N: the slice's even number of quads in pairs (a zero quad past an odd count adds 0)
-#pragma unroll 2
-                            for (int q = 0; q < nqw; q += 2) { quad(q, 0); quad(q + 1, 1); }
+                                for (int u = 0; u < NI; ++u) {
+                                    if (c < nfull) chunk_sums<16>(v[c & 1], A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
+                                    else chunk_sums_rt(v[c & 1], nq_t, rem_t, A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
+                                }
+                            }
                         }
 #pragma unroll
                         for (int u = 0; u < NI; ++u) {
                             float q0, q1, q2, q3;
                             f2_unpack(f2_add(acc1[u][0], acc1[u][1]), q0, q1);
                             f2_unpack(f2_add(acc0[u][0], acc0[u][1]), q2, q3);
-                            s1[u] = q0 + q1;
-                            s0[u] = q2 + q3;
+                            s1[u] = (q0 + q1) + t1s[u];
+                            s0[u] = (q2 + q3) + t0s[u];
                         }
                     }
-                } else if (__any_sync(0xffffffffu, risky_l)) {
-                    // A^2 would leave the fp32 range: clamped scalar path on the raw row from global memory (saturated scores)
+                    // ---- link in place
 #pragma unroll
                     for (int u = 0; u < NI; ++u) {
-                        float r1 = 0.f, r0 = 0.f;
-                        for (int j = 0; j + 1 < N; j += 2)
-                            pair_acc<true>(A[u], p.DmT[(size_t)j * p.S_pad + s], p.DmT[(size_t)(j + 1) * p.S_pad + s], r1, r0);
-                        if (N & 1) single_acc(A[u], p.DmT[(size_t)(N - 1) * p.S_pad + s], r1, r0);
-                        s1[u] = r1; s0[u] = r0;
-                    }
-                } else {
-                    f32x2 A2[NI], AA2[NI], AA2x2[NI];
-                    f32x2 acc1[NI][2], acc0[NI][2];
-                    float t1s[NI], t0s[NI];
-#pragma unroll
-                    for (int u = 0; u < NI; ++u) {
-                        const float AA = A[u] * A[u];
-                        A2[u] = f2_pack(A[u], A[u]); AA2[u] = f2_pack(AA, AA); AA2x2[u] = f2_pack(2.f * AA, 2.f * AA);
-                        acc1[u][0] = acc1[u][1] = acc0[u][0] = acc0[u][1] = f2_pack(0.f, 0.f);
-                        t1s[u] = t0s[u] = 0.f;
-                    }
-                    float v[2][16];
-                    dm_ld16(sl, 0, nq, lane, v[0]);
-#pragma unroll
-                    for (int c = 0; c < MAXCH; ++c) {
-                        if (c < nch) {
-                            if (c + 1 < nch) dm_ld16(sl, c + 1, nq, lane, v[(c + 1) & 1]);
-#pragma unroll
-                            for (int u = 0; u < NI; ++u) {
-                                if (c < nfull) chunk_sums<16>(v[c & 1], A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
-                                else chunk_sums_rt(v[c & 1], nq_t, rem_t, A[u], A2[u], AA2[u], AA2x2[u], one2, two2, acc1[u], acc0[u], t1s[u], t0s[u]);
-                            }
-                        }
-                    }
-#pragma unroll
-                    for (int u = 0; u < NI; ++u) {
-                        float q0, q1, q2, q3;
-                        f2_unpack(f2_add(acc1[u][0], acc1[u][1]), q0, q1);
-                        f2_unpack(f2_add(acc0[u][0], acc0[u][1]), q2, q3);
-                        s1[u] = (q0 + q1) + t1s[u];
-                        s0[u] = (q2 + q3) + t0s[u];
-                    }
-                }
-                // ---- link in place, rows parked for the turn-around (B is a multiple of NI: a pass never straddles a batch)
-#pragma unroll
-                for (int u = 0; u < NI; ++u) {
-                    if (it + u < my_n) {
-                        double y = 0.0;
+                        y[u] = 0.0;
                         if (row_ok) {
-                            if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(s1[u], s0[u], s_logtab) - yf;
-                            else y = (double)s1[u] * inv_n - yf;
+                            if (p.link == DKS_LINK_LOGIT) y[u] = fast_log_ratio(s1[u], s0[u], s_logtab) - yf;
+                            else y[u] = (double)s1[u] * inv_n - yf;
                         }
-                        sYw[lane * ystride + ((it + u) & bmask)] = y;
                     }
                 }
+                // ---- rows parked for the turn-around (B is a multiple of NI: a pass never straddles a batch)
+#pragma unroll
+                for (int u = 0; u < NI; ++u)
+                    if (it + u < my_n) sYw[lane * ystride + ((it + u) & bmask)] = y[u];
                 const int last_done = it + NI - 1 < last_it ? it + NI - 1 : last_it;      // last ordinal this pass completed
                 const int slot = last_done & bmask;
                 if (slot == bmask || last_done == last_it) {

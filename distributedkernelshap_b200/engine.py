@@ -567,14 +567,23 @@ class GpuKernelExplainer:
         are reported as unsupported, not computed), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
-        the weighted one)."""
-        out = np.zeros(11, dtype=np.int32)
+        the weighted one) and ``fused_table`` (1: the fused kernel read y from the plan's link table, passes outside its
+        domain excepted; 0: the exact loop over the background throughout)."""
+        out = np.zeros(12, dtype=np.int32)
         _cabi.check(self.lib.dks_last_path(self._ctx, _cabi.ptr(out), len(out)))
         names = self._PATH_NAMES
         return {"shared": names["shared"][out[0]], "chunks": int(out[1]), "warps": int(out[2]), "grid": int(out[3]),
                 "fused_B": int(out[4]), "fused_NI": int(out[5]), "solve": names["solve"][out[6]],
                 "pmat_kpad": int(out[7]), "general": names["general"][out[8]],
-                "cta_warps": int(out[9]), "bg_weights": ("uniform", "weighted")[out[10]]}
+                "cta_warps": int(out[9]), "bg_weights": ("uniform", "weighted")[out[10]], "fused_table": int(out[11])}
+
+    def fused_table_info(self, M):
+        """The fused kernel's link table of the plan over M groups: ``bytes`` (0: no table, the exact loop runs) and
+        ``fallback_passes``, the passes of this engine's fused launches so far that left a table's domain and took the
+        exact loop."""
+        nbytes, fb = C.c_int64(0), C.c_int64(0)
+        _cabi.check(self.lib.dks_fused_table_info(self._ctx, int(M), C.byref(nbytes), C.byref(fb)))
+        return {"bytes": int(nbytes.value), "fallback_passes": int(fb.value)}
 
     def debug_scores(self, X, instance, nsamples="auto"):
         """Raw accumulator tile of the tensor-core kernel for one instance: float32 [S_cap, Npad] of scaled masked scores

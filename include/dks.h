@@ -194,7 +194,8 @@ int dks_summarise_host(dks_ctx* ctx, int n, const int32_t* seg_offsets_host, int
 int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
 /* tuning knobs, all optional (defaults are the measured best): "fused" 0/1 -- link + projection solve inside the shared-plan
  * coalition kernel (default 1; 0 = separate (sum p1, sum p0) buffer + solve kernel); "fused_warps" caps the warps per CTA (default: as many as fit, at most 20); "fused_batch" instances
- * parked per warp before the turn-around;
+ * parked per warp before the turn-around; "fused_table" 0/1 -- the fused kernel reads y from the plan's link table
+ * (default 1; 0 = the exact loop over the background for every pass);
  * "push_in_kernel" 0/1 -- multi-GPU: the fused kernel's epilogue stores phi into the peers' buffers itself instead of the
  * separate push kernel (default 0: measured slower, it stalls the finishing warps); "graph" 0/1 (CUDA-graph
  * replay of dks_run_dev); "graph_timing" 0/1 -- keep the timing event records inside the graph (default 0: a replayed graph
@@ -204,6 +205,9 @@ int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
  * chunk's launch only (default 1).  Both give identical bits either way. */
 int dks_set_option(dks_ctx* ctx, const char* name, int value);
 int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by this ctx so far */
+/* The fused kernel's link table of the plan over M groups: its bytes (0 = the plan has none and the kernel runs the exact
+ * loop), and the passes of this ctx's fused launches so far that left a table's domain and took the exact loop. */
+int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fallback_passes);
 /* Which kernels the last explain call launched (dks_explain_* / dks_run_dev), recorded on the host while the launch
  * sequence is enqueued: a CUDA-graph replay keeps the record of the call it captured.  out[0 .. n) receives the first n
  * of the DKS_PATH_FIELDS entries indexed by DKS_PATH_*; n may be smaller (older callers) or larger (zero-filled). */
@@ -221,7 +225,9 @@ int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by th
                                     * plan, several warps share each slice and this is larger */
 #define DKS_PATH_BG_WEIGHTS 10   /* shared-plan kernels: 0 = uniform-background instantiations, 1 = the weighted ones
                                   * (background weights not all equal) */
-#define DKS_PATH_FIELDS 11
+#define DKS_PATH_FUSED_TABLE 11  /* fused kernel: 1 = y read from the plan's per-row link table (passes outside its domain
+                                  * take the exact loop), 0 = exact loop only ("fused_table" 0, or the plan has no table) */
+#define DKS_PATH_FIELDS 12
 #define DKS_SHARED_NONE 0
 #define DKS_SHARED_FUSED 1       /* explain_shared_fused_kernel: link + projection solve inside */
 #define DKS_SHARED_SMEM 2        /* explain_shared_smem_kernel (Dm rows in shared memory) */

@@ -2,7 +2,8 @@
 """Time the fused shared-plan coalition kernel on its own, on the bench.py workload, and sweep its warps per CTA and
 the number of instances.
 
-  python scripts/fused_kernel_probe.py [--launches 200] [--steps 50] [--warps 4,6,8,10,12] [--n 64,256,2560] [--out FILE]
+  python scripts/fused_kernel_probe.py [--launches 200] [--steps 50] [--warps 4,6,8,10,12] [--n 64,256,2560]
+                                      [--fused-table 1] [--out FILE]
 
 The workload is bench.py's: 2560 Adult-shaped instances, 12 groups, 100 background rows, nsamples = 2048, shared plans.
 For the engine's default configuration and for every ``fused_warps`` value of the sweep it reports
@@ -16,6 +17,8 @@ For the engine's default configuration and for every ``fused_warps`` value of th
 
 The ``--n`` sweep explains the first n instances of the workload with the default configuration (few instances leave
 most of the streaming warps with one or two instances each).
+
+``--fused-table 0`` runs everything on the exact loop over the background instead of the plan's link table.
 
 One JSON line on stdout, with the GPU name, its power limit and the SM clock sampled while the kernels ran.
 """
@@ -63,7 +66,8 @@ def measure(engine, X_dev, n, phi_dev, flush, stream, launches, steps, warmup=5)
     return {"kernel_ms": statistics.mean(kernel), "kernel_ms_min": min(kernel), "kernel_ms_max": max(kernel),
             "step_ms": statistics.mean(step), "kernel_share_of_step": statistics.mean(kernel) / statistics.mean(step),
             "path": {k: path[k] for k in ("shared", "warps", "grid", "fused_B", "fused_NI")} |
-                    ({"cta_warps": path["cta_warps"]} if "cta_warps" in path else {})}
+                    ({"cta_warps": path["cta_warps"]} if "cta_warps" in path else {}) |
+                    ({"fused_table": path["fused_table"]} if "fused_table" in path else {})}
 
 
 def main():
@@ -72,6 +76,7 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warps", default="4,6,8,10,12", help="fused_warps values to sweep (comma separated)")
     ap.add_argument("--n", default="64,256,2560", help="instance counts of the mapping sweep (comma separated)")
+    ap.add_argument("--fused-table", type=int, default=1, help="the engine's fused_table option (0: exact loop only)")
     ap.add_argument("--out", default=None, help="also write the JSON line to this file")
     args = ap.parse_args()
 
@@ -91,6 +96,7 @@ def main():
     stream = torch.cuda.Stream()
     torch.cuda.set_stream(stream)
     engine.set_stream(stream.cuda_stream)
+    engine.set_option("fused_table", args.fused_table)
     X_dev = torch.from_numpy(X).cuda()
     phi_dev = torch.empty((C, n, G), dtype=torch.float64, device="cuda")
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
@@ -115,7 +121,7 @@ def main():
     engine.close()
 
     props = torch.cuda.get_device_properties(0)
-    line = {"probe": "fused shared-plan kernel", "workload": "bench.py: 2560 Adult-shaped instances, G = 12, N = 100, "
+    line = {"probe": "fused shared-plan kernel", "fused_table": args.fused_table, "workload": "bench.py: 2560 Adult-shaped instances, G = 12, N = 100, "
             "nsamples = 2048, shared plans", "launches": args.launches, "steps": args.steps,
             "default": default, "fused_warps_sweep": sweep, "n_sweep": by_n,
             "clocks": {"sm_mhz": clocks["sm_mhz"], "sm_max_mhz": clocks["sm_max_mhz"], "reasons": clocks["reasons"],
