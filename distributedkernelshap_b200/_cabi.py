@@ -25,6 +25,7 @@ DKS_ERR_NUMERIC = 5
 ACT_IDENTITY = 0
 ACT_BINARY_LOGISTIC = 1
 ACT_SOFTMAX = 2
+ACT_OVR = 3
 LINK_IDENTITY = 0
 LINK_LOGIT = 1
 KERNEL_AUTO = 0

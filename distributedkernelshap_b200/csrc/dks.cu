@@ -130,11 +130,12 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D);
     auto kern = stage ? dks::prep_kernel<true> : dks::prep_kernel<false>;
-    // nibble tables: the binary head's scaled contributions; the softmax head's per class (log2 e XW) and the identity
-    // head's XW - Bbar, up to 128 groups (what the shared-plan path of those heads covers)
+    // nibble tables: the binary head's scaled contributions; the softmax and one-vs-rest heads' per class (log2 e XW) and
+    // the identity head's XW - Bbar, up to 128 groups (what the shared-plan path of those heads covers)
     double* xt = nullptr;
     if (ctx->act == DKS_ACT_BINARY_LOGISTIC && ctx->R == 1) xt = ctx->d_XT;
-    else if ((ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_IDENTITY) && G <= 128 && ctx->plan_mode == 0) xt = ctx->d_XT;
+    else if ((ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_IDENTITY) && G <= 128 &&
+             ctx->plan_mode == 0) xt = ctx->d_XT;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
         X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
@@ -151,8 +152,8 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
 }
 
 // upstream's l1 branch on the shared plan of G groups: moments of y per (instance, output), then the LARS path + criterion +
-// restricted WLS, one warp each.  nout = 1: the binary head (y from the (sum p1, sum p0) buffer); nout = C: the softmax and
-// identity heads (y from src).
+// restricted WLS, one warp each.  nout = 1: the binary head (y from the (sum p1, sum p0) buffer); nout = C: the softmax,
+// one-vs-rest and identity heads (y from src).
 int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, int nout, const dks::shared_path::HeadSource& src, double* phi_dev) {
     const int G = ctx->G, S = pg.S, S_pad = pg.S_pad;
     const dks_ctx::L1Dev& lt = ctx->h_l1[G];
@@ -316,15 +317,16 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     const bool fast = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
                       ctx->act == DKS_ACT_BINARY_LOGISTIC && G >= 2 && pg.dmT != nullptr &&
                       pg.S == dks_effective_S(G, ctx->nsamples_req) && (pg.W <= 2 || pg.ptw != nullptr);
-    // softmax and identity heads, up to 128 groups: per-class sums of the softmax coalition kernel (dks_multi.cuh) or the
-    // identity head's tables, then a solve per (instance, output)
-    const bool sfm = ctx->act == DKS_ACT_SOFTMAX;
+    // softmax, one-vs-rest and identity heads, up to 128 groups: per-class sums of the class-sum coalition kernels
+    // (dks_multi.cuh) or the identity head's tables, then a solve per (instance, output)
+    const bool sfm = ctx->act == DKS_ACT_SOFTMAX, ovr = ctx->act == DKS_ACT_OVR;
+    const bool mc = sfm || ovr;          // heads with per-class sums
     const bool multi = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
-                       (sfm || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128 && ctx->plan_mode == 0 &&
-                       pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) && (!sfm || ctx->h_smx[G].dm != nullptr);
+                       (mc || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128 && ctx->plan_mode == 0 &&
+                       pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) && (!mc || ctx->h_smx[G].dm != nullptr);
     if (kernel == DKS_KERNEL_SHARED && !fast && !multi && ext_z == nullptr && pg.z != nullptr)
-        return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head, or the softmax / identity head "
-                    "with at most 128 groups");
+        return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head, or the softmax / one-vs-rest / "
+                    "identity head with at most 128 groups");
     // non-uniform background weights: the weighted instantiations of the shared-plan kernels (dks_shared.cuh)
     const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn;
     if (fast || multi) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
@@ -349,8 +351,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if (pg.W > 2)
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
         if (!(fast || multi) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax or "
-                        "identity head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax, "
+                        "one-vs-rest or identity head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
     }
     const bool fused = fast && !l1 && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
                        dks::shared_path::fused_config(ctx->N, G, pg.S_pad, ctx->sm_count, ctx->max_smem_optin,
@@ -470,7 +472,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         const int S = pg.S, S_pad = pg.S_pad, C = ctx->C;
         dks::shared_path::HeadSource src;
         src.act = ctx->act; src.ntab = (G + 3) / 4; src.msums = nullptr; src.XT = ctx->d_XT;
-        if (sfm) {
+        if (mc) {
             // the workspace is C n S_pad floats: the engine explains these heads in row blocks of 2 / C the binary path's
             const size_t need = (size_t)n * C * S_pad;
             if (need > ctx->cap_msums) { TRY(dev_alloc(&ctx->d_msums, need)); ctx->cap_msums = need; ctx->epoch++; }
@@ -480,11 +482,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             mp.dm = ctx->h_smx[G].dm; mp.lo = ctx->h_smx[G].lo; mp.wn = ctx->d_wn; mp.z = pg.z; mp.XT = ctx->d_XT; mp.BW = ctx->d_BW;
             mp.scores = ctx->d_scores; mp.list = ctx->d_idx_full; mp.count = ctx->d_counts; mp.sums = ctx->d_msums;
             int grid = 0;
-            const int nl = dks::multi::launch_explain_softmax(mp, C, pg.W, n, ctx->sm_count, ctx->max_smem_optin, ctx->stream,
-                                                              &grid);
-            if (nl == 0) return fail(DKS_ERR_CUDA, "softmax coalition kernel: %s", cudaGetErrorString(cudaGetLastError()));
+            const int nl = dks::multi::launch_class_sums(mp, ovr, C, pg.W, n, ctx->sm_count, ctx->max_smem_optin, ctx->stream,
+                                                         &grid);
+            if (nl == 0)
+                return fail(DKS_ERR_CUDA, "%s coalition kernel: %s", ovr ? "one-vs-rest" : "softmax",
+                            cudaGetErrorString(cudaGetLastError()));
             ctx->launches += nl;
-            path[DKS_PATH_SHARED] = DKS_SHARED_SOFTMAX; path[DKS_PATH_CHUNKS] = nl;
+            path[DKS_PATH_SHARED] = ovr ? DKS_SHARED_OVR : DKS_SHARED_SOFTMAX; path[DKS_PATH_CHUNKS] = nl;
             path[DKS_PATH_WARPS] = dks::multi::MC_WARPS; path[DKS_PATH_GRID] = grid;
             src.msums = ctx->d_msums;
         } else {
@@ -538,7 +542,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         }
         if (!fast && !multi)
             return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, or the "
-                        "softmax / identity head up to 128 groups; kernel 'auto' or 'shared', shared plan of M=%d uploaded)", G);
+                        "softmax / one-vs-rest / identity head up to 128 groups; kernel 'auto' or 'shared', shared plan of "
+                        "M=%d uploaded)", G);
         dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 1;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
@@ -556,7 +561,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         TRY(dks::tc_launch(ctx, p, gstream));
         path[DKS_PATH_GENERAL] = DKS_GENERAL_TC;
     } else {
-        size_t smem = dks::simt_smem_bytes(S_cap, ctx->N, ctx->G, sfm ? ctx->R : 1, sfm ? ctx->C : 1);
+        size_t smem = dks::simt_smem_bytes(S_cap, ctx->N, ctx->G, mc ? ctx->R : 1, mc ? ctx->C : 1);
         if ((long long)smem > (long long)ctx->max_smem_optin && (fast || multi)) {
             // the shared-plan path took the instances whose groups all vary; the general kernel is sized for the largest
             // plan set and cannot hold it.  The instances left for it (often none) are reported, not computed.
@@ -570,8 +575,9 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         }
         if ((long long)smem > (long long)ctx->max_smem_optin && !multi && pg.z == nullptr &&
             (kernel_req == DKS_KERNEL_AUTO || kernel_req == DKS_KERNEL_SHARED) && ext_z == nullptr && ctx->plan_mode == 0 &&
-            (sfm || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128) {
-            // the softmax / identity head's shared-plan path takes these instances once the plan of G groups is uploaded
+            (mc || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128) {
+            // the softmax / one-vs-rest / identity head's shared-plan path takes these instances once the plan of G groups
+            // is uploaded
             ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
             return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
         }
@@ -843,6 +849,10 @@ int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int 
     } else if (activation == DKS_ACT_SOFTMAX) {
         REQUIRE(R >= 2, "softmax head needs at least two score rows (got %d)", R);
         ctx->C = R;
+    } else if (activation == DKS_ACT_OVR) {
+        REQUIRE(R >= 3, "one-vs-rest head needs at least three score rows (got %d)", R);
+        REQUIRE(kappa == 1.0, "one-vs-rest head needs kappa == 1 (got %g)", kappa);
+        ctx->C = R;
     } else {
         return fail(DKS_ERR_INVALID, "dks_set_model: unknown activation %d", activation);
     }
@@ -916,7 +926,7 @@ int dks_fit(dks_ctx* ctx) {
     CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
 
     ctx->scale = (ctx->act == DKS_ACT_BINARY_LOGISTIC) ? -ctx->kappa * 1.4426950408889634
-               : (ctx->act == DKS_ACT_SOFTMAX) ? 1.4426950408889634 : 1.0;
+               : (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR) ? 1.4426950408889634 : 1.0;
     dks::fit_bw_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D,
                                                                            G, R, ctx->d_BW);
     dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
@@ -1097,20 +1107,19 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
             if (ctx->N <= dks::shared_path::MAXN) TRY(build_link_table(ctx, pd, M, dz));
         }
     }
-    if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_SOFTMAX && W <= 2) {
-        // softmax head: per-class Dm table and row bounds for the full varying set (dks_multi.cuh)
-        const int C = ctx->C;
+    if (M == ctx->G && ctx->fitted && (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR) && W <= 2) {
+        // softmax / one-vs-rest head: per-class Dm table and row bounds for the full varying set (dks_multi.cuh); the
+        // one-vs-rest head keeps one more slot of each (nd per element, hi per row)
+        const int C = ctx->C, CS = ctx->act == DKS_ACT_OVR ? C + 1 : C;
         float* sd = nullptr; float* sl = nullptr;
-        CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)C * ctx->N * pd.S_pad));
+        CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)CS * ctx->N * pd.S_pad));
         ctx->plan_allocs[M].push_back(sd);
-        CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)C * pd.S_pad));
+        CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)CS * pd.S_pad));
         ctx->plan_allocs[M].push_back(sl);
-        if (W == 1)
-            dks::multi::plan_softmax_kernel<1><<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW,
-                ctx->d_scores, ctx->N, M, C, ctx->scale, sd, sl);
-        else
-            dks::multi::plan_softmax_kernel<2><<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW,
-                ctx->d_scores, ctx->N, M, C, ctx->scale, sd, sl);
+        auto kern = ctx->act == DKS_ACT_OVR ? (W == 1 ? dks::multi::plan_ovr_kernel<1> : dks::multi::plan_ovr_kernel<2>)
+                                            : (W == 1 ? dks::multi::plan_softmax_kernel<1> : dks::multi::plan_softmax_kernel<2>);
+        kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW, ctx->d_scores, ctx->N, M, C,
+                                                          ctx->scale, sd, sl);
         ctx->launches += 1;
         CUDA_TRY(cudaGetLastError());
         ctx->h_smx[M].dm = sd; ctx->h_smx[M].lo = sl;

@@ -146,7 +146,8 @@ struct dks_ctx {
     L1Dev h_l1[DKS_MAX_GROUPS + 1] = {};
     int l1_mode = 0, l1_k = 0, l1_others_plain = 0;
     // softmax head, full varying set (M == G): per-class Dm [C][N][S_pad] = 2^(d_c(s, j) - max_c d_c(s, j)) and row bounds
-    // lo [C][S_pad] = min_j log2 Dm_c(s, j) (dks_multi.cuh); owned by plan_allocs[M], cleared with the plan
+    // lo [C][S_pad] = min_j log2 Dm_c(s, j) (dks_multi.cuh); the one-vs-rest head's tables have one more slot each (nd per
+    // element, hi per row) and Dm relative to nd; owned by plan_allocs[M], cleared with the plan
     struct SmxDev { const float* dm; const float* lo; };
     SmxDev h_smx[DKS_MAX_GROUPS + 1] = {};
     double* d_mom = nullptr;     // [n][outputs solved][2G + 4] per-instance moments of y

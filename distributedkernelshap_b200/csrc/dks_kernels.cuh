@@ -74,6 +74,16 @@ __device__ inline void head_f64(const double* z, int R, int act, double kappa, d
         double sum = 0;
         for (int r = 0; r < R; ++r) { out[r] = exp(z[r] - m); sum += out[r]; }
         for (int r = 0; r < R; ++r) out[r] /= sum;
+    } else if (act == DKS_ACT_OVR) {
+        // one-vs-rest: sigmoid(z_r) / sum_r' sigmoid(z_r'), formed from log sigmoid so that no class underflows to 0/0
+        double m = -INFINITY;
+        for (int r = 0; r < R; ++r) {
+            out[r] = fmin(z[r], 0.0) - log1p(exp(-fabs(z[r])));
+            m = fmax(m, out[r]);
+        }
+        double sum = 0;
+        for (int r = 0; r < R; ++r) { out[r] = exp(out[r] - m); sum += out[r]; }
+        for (int r = 0; r < R; ++r) out[r] /= sum;
     } else {
         for (int r = 0; r < R; ++r) out[r] = z[r];
     }
@@ -658,7 +668,8 @@ __host__ __device__ inline size_t simt_smem_bytes(int S_cap, int N, int Mmax, in
 
 __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const bool softmax = p.act == DKS_ACT_SOFTMAX;
+    const bool ovr = p.act == DKS_ACT_OVR;
+    const bool softmax = p.act == DKS_ACT_SOFTMAX || ovr;     // C score rows and C y buffers
     SimtSmem sm = simt_carve(smem_raw, p.S_cap, softmax ? p.R : 1, softmax ? p.C : 1);
     const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C;
@@ -766,8 +777,9 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
                 const double* phi1 = p.phi + slab + (size_t)i * G;
                 for (int k = 0; k < M; ++k) { double v = phi1[sm.vi[k]]; phi0[sm.vi[k]] = (v == 0.0) ? 0.0 : -v; }
             }
-        } else if (p.act == DKS_ACT_SOFTMAX) {
-            // ---- general softmax head: R = C score rows, outputs softmax(scores); scale = log2(e) ----
+        } else if (softmax) {
+            // ---- general softmax and one-vs-rest heads: R = C score rows, outputs softmax(scores) or the normalised
+            // sigmoids of the scores; scale = log2(e) ----
             const int R = p.R;
             float* basesR = Bs + (size_t)R * M * N;      // [R][N]
             float* wbR = basesR + (size_t)R * N;         // [N]
@@ -801,7 +813,14 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
                         mx = fmaxf(mx, t[r]);
                     }
                     float den = 0.f;
-                    for (int r = 0; r < R; ++r) { t[r] = ex2_approx(t[r] - mx); den += t[r]; }
+                    if (ovr) {
+                        // 2^-h sigmoid_r = 1 / (2^h + 2^(h - t_r)) with h = min(max_r t_r, 0): the leading class is at
+                        // least 1/2, so den >= 1/2; classes 2^-128 below it overflow to 1 / inf = 0
+                        const float h = fminf(mx, 0.f), eh = ex2_approx(h);
+                        for (int r = 0; r < R; ++r) { t[r] = rcp_approx(eh + ex2_approx(h - t[r])); den += t[r]; }
+                    } else {
+                        for (int r = 0; r < R; ++r) { t[r] = ex2_approx(t[r] - mx); den += t[r]; }
+                    }
                     const float inv = wbR[j] * rcp_approx(den);
                     for (int r = 0; r < R; ++r) acc[r] = fmaf(t[r], inv, acc[r]);
                 }

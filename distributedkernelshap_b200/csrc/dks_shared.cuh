@@ -681,11 +681,11 @@ inline int launch_explain_shared(SharedParams p, int words, int sm_count, int ma
     return launches;
 }
 
-// Where the softmax and identity heads' y(i, c, s) comes from on the shared-plan path: the per-class sums of the softmax
-// coalition kernel (dks_multi.cuh), or the identity head's float64 nibble tables of XW - Bbar (prep_kernel), for which
-// ey_c(s) = fnull_c + sum_k z_sk (XW_i[k][c] - Bbar[k][c]) needs no coalition kernel at all.
+// Where the softmax, one-vs-rest and identity heads' y(i, c, s) comes from on the shared-plan path: the per-class sums of
+// the class-sum coalition kernels (dks_multi.cuh), or the identity head's float64 nibble tables of XW - Bbar (prep_kernel),
+// for which ey_c(s) = fnull_c + sum_k z_sk (XW_i[k][c] - Bbar[k][c]) needs no coalition kernel at all.
 struct HeadSource {
-    int act;                 // DKS_ACT_SOFTMAX or DKS_ACT_IDENTITY
+    int act;                 // DKS_ACT_SOFTMAX, DKS_ACT_OVR or DKS_ACT_IDENTITY
     int ntab;                // nibble tables per class: ceil(G / 4)
     const float* msums;      // [n][C][S_pad] sum_j w'_j p_c(s, j), w'_j = N w_j
     const double* XT;        // [n][C][ntab][16]
@@ -693,7 +693,7 @@ struct HeadSource {
 template <int W>
 __device__ __forceinline__ double head_y(const HeadSource& h, int i, int c, int C, int s, int S_pad, const uint64_t* zrow,
                                          int link, double inv_n, double fn, double lf) {
-    if (h.act == DKS_ACT_SOFTMAX) {
+    if (h.act != DKS_ACT_IDENTITY) {
         const float* ms = h.msums + (size_t)i * C * S_pad + s;
         const double e = (double)ms[(size_t)c * S_pad];
         if (link == DKS_LINK_LOGIT) {

@@ -373,9 +373,10 @@ class GpuKernelExplainer:
         return [phi[c] for c in range(self.D)]
 
     def _rows_per_call(self):
-        """Rows per C-ABI call.  The softmax head's shared-plan path keeps C per-class sums per coalition where the binary
-        head keeps two: its row blocks are 2 / C as long, so that the per-call workspace stays the binary path's."""
-        if self.spec.act_code == _cabi.ACT_SOFTMAX and self.D > 2:
+        """Rows per C-ABI call.  The softmax and one-vs-rest heads' shared-plan path keeps C per-class sums per coalition
+        where the binary head keeps two: their row blocks are 2 / C as long, so that the per-call workspace stays the
+        binary path's."""
+        if self.spec.act_code in (_cabi.ACT_SOFTMAX, _cabi.ACT_OVR) and self.D > 2:
             return MAX_ROWS_PER_CALL * 2 // self.D
         return MAX_ROWS_PER_CALL
 
@@ -553,7 +554,7 @@ class GpuKernelExplainer:
         return {"prepare": float(out[0]), "coalitions": float(out[1]), "total": float(out[2])}
 
     _PATH_NAMES = {
-        "shared": ("none", "fused", "smem", "regs", "softmax", "affine"),
+        "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
         "general": ("none", "tc", "simt", "flagged"),
     }
@@ -561,7 +562,7 @@ class GpuKernelExplainer:
     def last_path(self):
         """Which kernels the last explain call launched (``dks_last_path``), recorded when the call was enqueued (a
         replayed CUDA graph reports the call it captured): ``shared`` (shared-plan coalition kernel: 'none' | 'fused' |
-        'smem' | 'regs' | 'softmax', or 'affine' for the identity head, whose y needs no coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
+        'smem' | 'regs' | 'softmax' | 'ovr', or 'affine' for the identity head, whose y needs no coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
         are reported as unsupported, not computed), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``

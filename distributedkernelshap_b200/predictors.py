@@ -14,17 +14,21 @@ class LinearModelSpec:
     """``z = X W^T + b`` then a head.  ``W`` is [R, D], ``b`` [R].
 
     activation: 'identity' (outputs z), 'binary_logistic' (R == 1; outputs [1 - s, s], s = sigmoid(kappa z)),
-    'softmax' (outputs softmax(z), R = C >= 2).  ``scalar_out``: the callable returns a 1-D array."""
+    'softmax' (outputs softmax(z), R = C >= 2), 'ovr' (one-vs-rest, R = C >= 3: s_c = sigmoid(z_c), outputs
+    s_c / sum_c' s_c', scikit-learn's ``_predict_proba_lr``; kappa 1).  ``scalar_out``: the callable returns a 1-D
+    array."""
 
     def __init__(self, W, b, activation, kappa=1.0, scalar_out=False):
         self.W = np.ascontiguousarray(np.atleast_2d(np.asarray(W, dtype=np.float64)))
         self.b = np.ascontiguousarray(np.atleast_1d(np.asarray(b, dtype=np.float64)))
         if self.W.shape[0] != self.b.shape[0]:
             raise ValueError(f"W has {self.W.shape[0]} rows but b has {self.b.shape[0]} entries")
-        if activation not in ("identity", "binary_logistic", "softmax"):
+        if activation not in ("identity", "binary_logistic", "softmax", "ovr"):
             raise ValueError(f"unknown activation {activation!r}")
         if activation == "binary_logistic" and self.W.shape[0] != 1:
             raise ValueError("binary_logistic needs a single score row")
+        if activation == "ovr" and (self.W.shape[0] < 3 or float(kappa) != 1.0):
+            raise ValueError("the one-vs-rest head needs at least three score rows and kappa = 1")
         self.activation = activation
         self.kappa = float(kappa)
         self.scalar_out = bool(scalar_out)
@@ -32,7 +36,7 @@ class LinearModelSpec:
     @property
     def act_code(self):
         return {"identity": _cabi.ACT_IDENTITY, "binary_logistic": _cabi.ACT_BINARY_LOGISTIC,
-                "softmax": _cabi.ACT_SOFTMAX}[self.activation]
+                "softmax": _cabi.ACT_SOFTMAX, "ovr": _cabi.ACT_OVR}[self.activation]
 
     @property
     def n_outputs(self):
@@ -49,6 +53,10 @@ class LinearModelSpec:
         if self.activation == "binary_logistic":
             t = self.kappa * z[:, 0]
             scores = np.c_[-t / 2.0, t / 2.0]
+        elif self.activation == "ovr":
+            # _predict_proba_lr (scikit-learn 0.23.2): expit of each score, then each row divided by its sum
+            p = np.exp(-np.logaddexp(0.0, -z))
+            return p / p.sum(axis=1, keepdims=True)
         else:
             scores = z
         scores = scores - scores.max(axis=1, keepdims=True)
@@ -59,7 +67,8 @@ class LinearModelSpec:
 class LinearSoftmaxClassifier:
     """Minimal stand-in for the fitted scikit-learn 0.23 ``LogisticRegression(multi_class='multinomial')`` the
     reference pickles (scripts/fit_adult_model.py:27-32): ``coef_`` [1, D] / ``intercept_`` [1] for two classes
-    with ``predict_proba = softmax([-z, z])`` (so p1 = sigmoid(2 z)), or [C, D] / [C] with a plain softmax."""
+    with ``predict_proba = softmax([-z, z])`` (so p1 = sigmoid(2 z)), or [C, D] / [C] with a plain softmax.
+    ``multi_class='ovr'`` with C >= 3 classes: the one-vs-rest head (normalised per-class sigmoids)."""
 
     def __init__(self, coef, intercept, multi_class="multinomial"):
         self.coef_ = np.atleast_2d(np.asarray(coef, dtype=np.float64))
@@ -71,8 +80,10 @@ class LinearSoftmaxClassifier:
         if self.coef_.shape[0] == 1:
             return LinearModelSpec(self.coef_, self.intercept_, "binary_logistic",
                                    kappa=2.0 if self.multi_class == "multinomial" else 1.0)
+        if self.multi_class == "ovr":
+            return LinearModelSpec(self.coef_, self.intercept_, "ovr")
         if self.multi_class != "multinomial":
-            raise NotImplementedError("one-vs-rest multi-class heads are not supported")
+            raise NotImplementedError(f"multi_class={self.multi_class!r} is not supported")
         return LinearModelSpec(self.coef_, self.intercept_, "softmax")
 
     def decision_function(self, X):
@@ -90,7 +101,8 @@ def extract_linear_spec(predictor):
     """Recover ``LinearModelSpec`` from what the reference hands to ``KernelShap`` (a callable).
 
     Accepts: a ``LinearModelSpec``; any object/bound method whose owner offers ``dks_linear_spec()``; bound
-    ``predict_proba`` / ``decision_function`` / ``predict`` of scikit-learn linear models (``coef_``/``intercept_``).
+    ``predict_proba`` / ``decision_function`` / ``predict`` of scikit-learn linear models (``coef_``/``intercept_``);
+    bound ``predict_proba`` of a single-label ``OneVsRestClassifier`` over at least three binary linear models.
     Raises ``TypeError`` for everything else."""
     if isinstance(predictor, LinearModelSpec):
         return predictor
@@ -103,6 +115,8 @@ def extract_linear_spec(predictor):
                         "LinearModelSpec: the CUDA engine cannot call an opaque Python function and has no CPU fallback")
     if hasattr(owner, "dks_linear_spec") and method == "predict_proba":
         return owner.dks_linear_spec()
+    if hasattr(owner, "estimators_") and not hasattr(owner, "coef_"):
+        return _one_vs_rest_spec(owner, method)
     if not (hasattr(owner, "coef_") and hasattr(owner, "intercept_")):
         raise TypeError(f"{type(owner).__name__} exposes no coef_/intercept_: only linear models are supported")
     coef = np.atleast_2d(np.asarray(owner.coef_, dtype=np.float64))
@@ -113,11 +127,42 @@ def extract_linear_spec(predictor):
             # scikit-learn >= 1.5 binary problems: sigmoid(z); 0.23 'multinomial' binary: softmax([-z, z])
             kappa = 2.0 if mc == "multinomial" else 1.0
             return LinearModelSpec(coef, intercept, "binary_logistic", kappa=kappa)
-        if getattr(owner, "multi_class", "multinomial") == "ovr":
-            raise NotImplementedError("one-vs-rest multi-class heads are not supported")
+        if _is_ovr_rule(owner):
+            return LinearModelSpec(coef, intercept, "ovr")
         return LinearModelSpec(coef, intercept, "softmax")
     if method in ("decision_function", "predict", "_decision_function"):
         if method == "predict" and hasattr(owner, "classes_"):
             raise TypeError("classifier.predict returns labels, which KernelSHAP cannot explain; pass predict_proba")
         return LinearModelSpec(coef, intercept, "identity", scalar_out=coef.shape[0] == 1)
     raise TypeError(f"unsupported predictor method {method!r}")
+
+
+def _is_ovr_rule(owner):
+    """scikit-learn 0.23.2 ``LogisticRegression.predict_proba`` with C >= 3 classes is one-vs-rest (``_predict_proba_lr``)
+    when ``multi_class`` is 'ovr' or 'warn', or 'auto' with the liblinear solver; otherwise a softmax."""
+    mc = getattr(owner, "multi_class", "multinomial")
+    return mc in ("ovr", "warn") or (mc == "auto" and getattr(owner, "solver", None) == "liblinear")
+
+
+def _one_vs_rest_spec(owner, method):
+    """``OneVsRestClassifier.predict_proba`` over C >= 3 binary linear models: ``p_c = predict_proba_c[:, 1]`` normalised
+    per row.  Each estimator's ``predict_proba[:, 1]`` must be ``sigmoid(coef_ x + intercept_)`` -- the fit-time check
+    against the callable holds the stacked model to that."""
+    if method != "predict_proba":
+        raise TypeError(f"{type(owner).__name__}.{method} is not supported: pass predict_proba")
+    if getattr(owner, "multilabel_", False):
+        raise NotImplementedError("multilabel one-vs-rest outputs are not normalised per row: not supported")
+    ests = list(owner.estimators_)
+    if len(ests) < 3:
+        raise NotImplementedError(f"one-vs-rest over {len(ests)} estimator(s): the one-vs-rest head needs at least three "
+                                  "classes")
+    rows, bias = [], []
+    for e in ests:
+        if not (hasattr(e, "coef_") and hasattr(e, "intercept_")):
+            raise TypeError(f"{type(e).__name__} exposes no coef_/intercept_: only linear models are supported")
+        coef = np.atleast_2d(np.asarray(e.coef_, dtype=np.float64))
+        if coef.shape[0] != 1 or getattr(e, "multi_class", "auto") == "multinomial":
+            raise NotImplementedError("one-vs-rest estimators must be binary models with predict_proba = sigmoid(z)")
+        rows.append(coef[0])
+        bias.append(float(np.atleast_1d(np.asarray(e.intercept_, dtype=np.float64))[0]))
+    return LinearModelSpec(np.stack(rows), np.asarray(bias), "ovr")

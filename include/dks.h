@@ -40,6 +40,9 @@ extern "C" {
 #define DKS_ACT_BINARY_LOGISTIC 1 /* R = 1, outputs [1 - s, s], s = sigmoid(kappa * z): kappa = 1 is the
                                    * binary sigmoid, kappa = 2 the 2-class multinomial softmax([-z, z]) */
 #define DKS_ACT_SOFTMAX 2       /* R = C >= 2 scores, outputs softmax(z)                              */
+#define DKS_ACT_OVR 3           /* R = C in 3..8 scores, one-vs-rest: s_c = sigmoid(z_c), outputs s_c / sum_c' s_c'
+                                 * (scikit-learn's _predict_proba_lr: liblinear / multi_class='ovr' LogisticRegression,
+                                 * OneVsRestClassifier over binary linear models); kappa must be 1 */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -74,7 +77,8 @@ int dks_set_background(dks_ctx* ctx, const double* bg_host, int N, int D, const 
  * Every column must belong to exactly one group (DenseData asserts the sizes add up to D). */
 int dks_set_groups(dks_ctx* ctx, const int32_t* group_offsets, const int32_t* group_cols, int G);
 /* linear scores z = W x + b with W [R x D] row-major, b [R]; head per DKS_ACT_*; kappa used by
- * DKS_ACT_BINARY_LOGISTIC only.  scalar_out != 0 marks a predictor returning a 1-D array (vector_out False). */
+ * DKS_ACT_BINARY_LOGISTIC (DKS_ACT_OVR requires kappa == 1 and R >= 3).  scalar_out != 0 marks a predictor returning a
+ * 1-D array (vector_out False). */
 int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int R, int activation, double kappa,
                   int scalar_out);
 int dks_set_link(dks_ctx* ctx, int link);
@@ -234,6 +238,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_SHARED_REGS 3        /* explain_shared_kernel (Dm rows in registers; DKS_SHARED_DM=regs) */
 #define DKS_SHARED_SOFTMAX 4     /* explain_softmax_kernel: per-class sums of the softmax head (C = R classes) */
 #define DKS_SHARED_AFFINE 5      /* identity head: y read from per-class tables, no coalition kernel */
+#define DKS_SHARED_OVR 6         /* explain_ovr_kernel: per-class sums of the one-vs-rest head (C = R classes) */
 #define DKS_SOLVE_NONE 0
 #define DKS_SOLVE_FUSED 1
 #define DKS_SOLVE_PMAT 2         /* wls_pmat_kernel */
