@@ -56,7 +56,7 @@ SIGNATURES = {
     "dks_set_plan_projection": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "dks_clear_plans": (C.c_int, [C.c_void_p]),
     "dks_has_shared_plan": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int)]),
-    "dks_set_l1": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
+    "dks_set_l1": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_uint64]),
     "dks_set_l1_tables": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 8 + [C.c_double, C.c_double, C.c_int]),
     "dks_set_plan_sampling": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_double]),
     "dks_set_plan_mode": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
@@ -82,6 +82,7 @@ SIGNATURES = {
     "dks_kernel_launches": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "dks_fused_table_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "dks_last_timings": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "dks_last_general_l1_timings": (C.c_int, [C.c_void_p, C.c_void_p]),
     "dks_last_path": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "dks_debug_score_dump": (C.c_int, [C.c_void_p, C.c_int]),
     "dks_debug_get_timeline": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -98,6 +98,8 @@ int ensure_workspace(dks_ctx* ctx, int n) {
     TRY(dev_alloc(&ctx->d_dlink, (size_t)n * C));
     TRY(dev_alloc(&ctx->d_idx_full, (size_t)n));
     TRY(dev_alloc(&ctx->d_idx_other, (size_t)n));
+    TRY(dev_alloc(&ctx->d_idx_sel, (size_t)n));
+    TRY(dev_alloc(&ctx->d_idx_plain, (size_t)n));
     TRY(dev_alloc(&ctx->d_acc, (size_t)n * 16));
     TRY(dev_alloc(&ctx->d_done, (size_t)n));
     CUDA_TRY(cudaMemsetAsync(ctx->d_acc, 0, sizeof(long long) * (size_t)n * 16, ctx->stream));   // the fused kernel leaves
@@ -151,44 +153,29 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     return DKS_OK;
 }
 
-// upstream's l1 branch on the shared plan of G groups: moments of y per (instance, output), then the LARS path + criterion +
-// restricted WLS, one warp each.  nout = 1: the binary head (y from the (sum p1, sum p0) buffer); nout = C: the softmax,
-// one-vs-rest and identity heads (y from src).
-int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, int nout, const dks::shared_path::HeadSource& src, double* phi_dev) {
-    const int G = ctx->G, S = pg.S, S_pad = pg.S_pad;
-    const dks_ctx::L1Dev& lt = ctx->h_l1[G];
-    const size_t need_m = (size_t)n * nout * (2 * G + 4);
-    if (need_m > ctx->cap_mom) { TRY(dev_alloc(&ctx->d_mom, need_m)); ctx->cap_mom = need_m; ctx->epoch++; }
+// what the l1 kernels of both instance lists share
+dks::l1::Params l1_params(dks_ctx* ctx, int n, int nout, double* phi_dev) {
     dks::l1::Params lp;
     memset(&lp, 0, sizeof(lp));
-    lp.n = n; lp.N = ctx->N; lp.G = G; lp.C = ctx->C; lp.S = S; lp.S_pad = S_pad; lp.link = ctx->link;
-    lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.nout = nout; lp.src = src; lp.sums = ctx->d_sums; lp.z = pg.z; lp.w = pg.w;
-    lp.t.gram_raw = lt.gram_raw; lp.t.gram_norm = lt.gram_norm; lp.t.colsum = lt.colsum; lp.t.scale = lt.scale;
-    lp.t.bz = lt.bz; lp.t.gram_w = lt.gram_w; lp.t.b = lt.b; lp.t.sqab = lt.sqab; lp.t.sum_b = lt.sum_b;
-    lp.t.sum_sqb = lt.sum_sqb; lp.t.n_aug = lt.n_aug;
-    lp.dlink = ctx->d_dlink; lp.linkfnull = ctx->d_linkfnull; lp.fnull = ctx->d_fnull; lp.list = ctx->d_idx_full;
-    lp.count = ctx->d_counts; lp.mom = ctx->d_mom; lp.phi = phi_dev; lp.status = ctx->d_status;
-    const size_t msm = sizeof(double) * (size_t)S;
-    if (msm + 8192 > (size_t)ctx->max_smem_optin)
-        return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: %d coalitions per plan exceed the shared-memory staging", S);
-    const int tasks = n * nout;
-    const int mgrid = tasks < ctx->sm_count * 2 ? tasks : ctx->sm_count * 2;
-#define DKS_MOM(W, MULTI)                                                                                                 \
-    CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_moments_kernel<W, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm)); \
-    dks::l1::l1_moments_kernel<W, MULTI><<<mgrid, dks::l1::MOM_THREADS, msm, ctx->stream>>>(lp);
-    if (nout == 1) {
-        if (pg.W == 1) { DKS_MOM(1, false) } else { DKS_MOM(2, false) }
-    } else {
-        if (pg.W == 1) { DKS_MOM(1, true) } else { DKS_MOM(2, true) }
-    }
-#undef DKS_MOM
-    const size_t per_warp = dks::l1::lars_smem_per_warp(G);
-    const size_t gram_bytes = sizeof(double) * (size_t)G * G;
+    lp.n = n; lp.N = ctx->N; lp.G = ctx->G; lp.C = ctx->C; lp.link = ctx->link;
+    lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.nout = nout; lp.tabs = ctx->d_l1;
+    lp.binary = ctx->act == DKS_ACT_BINARY_LOGISTIC;
+    lp.dlink = ctx->d_dlink; lp.linkfnull = ctx->d_linkfnull; lp.fnull = ctx->d_fnull;
+    lp.mom = ctx->d_mom; lp.phi = phi_dev; lp.status = ctx->d_status;
+    return lp;
+}
+
+// the LARS path + criterion + restricted WLS, one warp per task (at most `tasks`); warps sized for lp.Mmax.  stage: every
+// task has M = lp.Mmax, whose Gram matrix may then be staged in shared memory.
+int launch_lars(dks_ctx* ctx, const dks::l1::Params& lp, int tasks, bool stage, cudaStream_t stream) {
+    const int M = lp.Mmax;
+    const size_t per_warp = dks::l1::lars_smem_per_warp(M);
+    const size_t gram_bytes = sizeof(double) * (size_t)M * M;
     const size_t budget = (size_t)ctx->max_smem_optin - 2048;
     // the Gram matrix of the path goes to shared memory when at least four warps still fit next to it
-    const int stage_gram = (gram_bytes + 4 * per_warp <= budget) ? 1 : 0;
+    const int stage_gram = (stage && gram_bytes + 4 * per_warp <= budget) ? 1 : 0;
     int wpc = (int)((budget - (stage_gram ? gram_bytes : 0)) / per_warp);
-    if (wpc < 1) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory", G, G);
+    if (wpc < 1) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory", M, M);
     if (wpc > 8) wpc = 8;
     const size_t lsm = per_warp * wpc + (stage_gram ? gram_bytes : 0);
     int per_sm = (int)((size_t)ctx->max_smem_optin / (lsm + 1024));
@@ -197,7 +184,40 @@ int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, int nout, const dks::share
     int lgrid = (tasks + wpc - 1) / wpc;
     if (lgrid > ctx->sm_count * per_sm) lgrid = ctx->sm_count * per_sm;
     CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_lars_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm));
-    dks::l1::l1_lars_kernel<<<lgrid, 32 * wpc, lsm, ctx->stream>>>(lp, wpc, stage_gram);
+    dks::l1::l1_lars_kernel<<<lgrid, 32 * wpc, lsm, stream>>>(lp, wpc, stage_gram);
+    return DKS_OK;
+}
+
+// upstream's l1 branch on the shared plan of G groups: moments of y per (instance, output), then the LARS path + criterion +
+// restricted WLS, one warp each.  The binary head: nout = 1, y from the (sum p1, sum p0) buffer; the softmax, one-vs-rest
+// and identity heads: nout = C (1 for a single regression output), y from src.
+int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, int nout, const dks::shared_path::HeadSource& src, double* phi_dev) {
+    const int G = ctx->G, S = pg.S, S_pad = pg.S_pad;
+    dks::l1::Params lp = l1_params(ctx, n, nout, phi_dev);
+    lp.S = S; lp.S_pad = S_pad; lp.Mmax = G; lp.src = src; lp.sums = ctx->d_sums; lp.z = pg.z; lp.w = pg.w;
+    lp.list = ctx->d_idx_full; lp.count = ctx->d_counts;
+    const size_t msm = sizeof(double) * (size_t)S;
+    if (msm + 8192 > (size_t)ctx->max_smem_optin)
+        return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: %d coalitions per plan exceed the shared-memory staging", S);
+    const int tasks = n * nout;
+    const int mgrid = tasks < ctx->sm_count * 2 ? tasks : ctx->sm_count * 2;
+#define DKS_MOM(W, MULTI)                                                                                                 \
+    CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_moments_kernel<W, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm)); \
+    dks::l1::l1_moments_kernel<W, MULTI><<<mgrid, dks::l1::MOM_THREADS, msm, ctx->stream>>>(lp);
+    if (lp.binary) {
+        if (pg.W == 1) { DKS_MOM(1, false) } else { DKS_MOM(2, false) }
+    } else {
+        if (pg.W == 1) { DKS_MOM(1, true) } else { DKS_MOM(2, true) }
+    }
+#undef DKS_MOM
+    return launch_lars(ctx, lp, tasks, true, ctx->stream);
+}
+
+// the device copy of the l1 table set (dks::l1::Params::tabs), after any change of h_l1
+int sync_l1_tables(dks_ctx* ctx) {
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_l1, ctx->h_l1, sizeof(dks::l1::Tables) * (DKS_L1_MAX_GROUPS + 1), cudaMemcpyHostToDevice,
+                             ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return DKS_OK;
 }
 
@@ -327,6 +347,46 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     if (kernel == DKS_KERNEL_SHARED && !fast && !multi && ext_z == nullptr && pg.z != nullptr)
         return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head, or the softmax / one-vs-rest / "
                     "identity head with at most 128 groups");
+    // l1 feature selection: on the shared-plan path when M = G selects, and on the general list (CUDA-core kernel for the
+    // moments, then l1_lars_kernel) for the instances with a partial varying set whose M selects
+    const bool l1 = ctx->l1_mode != 0;
+    auto selects = [&](int M) {
+        return l1 && M >= 1 && M <= DKS_L1_MAX_GROUPS && ((ctx->l1_sel[(M - 1) >> 6] >> ((M - 1) & 63)) & 1ull) != 0;
+    };
+    const bool l1_full = selects(G);
+    int l1_Mmax = 0;                     // largest M < G that selects
+    for (int M = 2; M < G && M <= DKS_L1_MAX_GROUPS; ++M) if (selects(M)) l1_Mmax = M;
+    const bool l1_gen = l1_Mmax > 0;
+    const int l1_nout = (mc || ctx->act == DKS_ACT_IDENTITY) ? ctx->C : 1;
+    size_t l1_smem = 0;
+    ctx->l1_timing_valid = false;
+    if (l1) {
+        if (ext_z != nullptr || ctx->plan_mode == 1)
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
+        if (l1_full && pg.W > 2)
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
+        if (l1_full && (!(fast || multi) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S))
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax, "
+                        "one-vs-rest or identity head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
+        if (l1_gen) {
+            if (G > 64)
+                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection for partial varying sets covers at most 64 groups (G=%d)", G);
+            if (kernel_req != DKS_KERNEL_AUTO && kernel_req != DKS_KERNEL_SHARED)
+                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs kernel 'auto' or 'shared' (the CUDA-core kernel "
+                            "forms the moments of instances with a partial varying set)");
+            for (int M = 2; M <= l1_Mmax; ++M)
+                if (selects(M) && (ctx->h_l1[M].gram_raw == nullptr || ctx->h_l1[M].S != dks_effective_S(M, ctx->nsamples_req) ||
+                                   ctx->h_plans[M].z == nullptr || ctx->h_plans[M].S != ctx->h_l1[M].S))
+                    return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared plan of M=%d and its l1 tables "
+                                "(dks_set_l1_tables)", M);
+            l1_smem = dks::simt_smem_bytes(S_cap, ctx->N, l1_Mmax, mc ? ctx->R : 1, mc ? ctx->C : 1);
+            if ((long long)l1_smem > (long long)ctx->max_smem_optin)
+                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the CUDA-core kernel's staging of instances with up to "
+                            "%d varying groups needs %zu B of shared memory (> %d)", l1_Mmax, l1_smem, ctx->max_smem_optin);
+        }
+        const size_t need_m = (size_t)n * l1_nout * (2 * G + 4);
+        if (need_m > ctx->cap_mom) { TRY(dev_alloc(&ctx->d_mom, need_m)); ctx->cap_mom = need_m; ctx->epoch++; }
+    }
     // non-uniform background weights: the weighted instantiations of the shared-plan kernels (dks_shared.cuh)
     const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn;
     if (fast || multi) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
@@ -344,17 +404,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         return e;
     };
     dks::shared_path::FusedConfig fcfg;
-    const bool l1 = ctx->l1_mode != 0;
-    if (l1) {
-        if (ext_z != nullptr || ctx->plan_mode == 1)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
-        if (pg.W > 2)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
-        if (!(fast || multi) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax, "
-                        "one-vs-rest or identity head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
-    }
-    const bool fused = fast && !l1 && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
+    const bool fused = fast && !l1_full && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
                        dks::shared_path::fused_config(ctx->N, G, pg.S_pad, ctx->sm_count, ctx->max_smem_optin,
                                                       ctx->opt_fused_warps, ctx->opt_fused_B, &fcfg,
                                                       wn != nullptr);
@@ -421,7 +471,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         wp.uniform_w = 1; wp.sums = ctx->d_sums; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink;
         wp.linkfnull = ctx->d_linkfnull; wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts;
         wp.phi = phi_dev;
-        if (l1) {
+        if (l1_full) {
             TRY(launch_l1(ctx, pg, n, 1, dks::shared_path::HeadSource{}, phi_dev));
             path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
         } else if (pg.W > 2) {
@@ -494,7 +544,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         } else {
             path[DKS_PATH_SHARED] = DKS_SHARED_AFFINE;       // y straight from the tables: no coalition kernel
         }
-        if (l1) {
+        if (l1_full) {
             TRY(launch_l1(ctx, pg, n, C, src, phi_dev));
             ctx->launches += 2;
             path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
@@ -524,15 +574,36 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         p.list = ctx->d_idx_other;
         p.count = ctx->d_counts + 1;
     }
-    if (l1 && !ctx->l1_others_plain) {
-        // instances with a partial varying set would need their own selection: reported, not computed
-        dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
-        ctx->launches += 1;
-        path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
+    if (l1_gen) {
+        // the general list splits into the instances whose M selects -- the CUDA-core kernel stores their moments and
+        // l1_lars_kernel selects and solves on the shared plan of each one's M -- and the rest, which keep the kernel below
+        CUDA_TRY(cudaMemsetAsync(ctx->d_l1_counts, 0, 2 * sizeof(int), gstream));
+        int pgrid = cdiv(n, 256);
+        if (pgrid > ctx->sm_count * 4) pgrid = ctx->sm_count * 4;
+        dks::l1::l1_partition_kernel<<<pgrid, 256, 0, gstream>>>(p.list, p.count, n, ctx->d_M, ctx->l1_sel[0], ctx->l1_sel[1],
+                                                                 ctx->d_idx_sel, ctx->d_idx_plain, ctx->d_l1_counts);
+        ExplainParams ps = p;
+        ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
+        CUDA_TRY(cudaFuncSetAttribute(dks::explain_simt_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l1_smem));
+        int per_sm = (int)((size_t)ctx->max_smem_optin / (l1_smem + 1024));
+        if (per_sm < 1) per_sm = 1;
+        if (per_sm > 8) per_sm = 8;
+        int grid = ctx->sm_count * per_sm;
+        if (grid > n) grid = n;
+        const bool timed = !ctx->capturing;
+        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
+        dks::explain_simt_kernel<true><<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom});
+        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[1], gstream));
+        dks::l1::Params lp = l1_params(ctx, n, l1_nout, phi_dev);
+        lp.Mmax = l1_Mmax; lp.Mcnt = ctx->d_M; lp.vmask = ctx->d_vmask; lp.list = ctx->d_idx_sel; lp.count = ctx->d_l1_counts;
+        TRY(launch_lars(ctx, lp, n * l1_nout, false, gstream));
+        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[2], gstream));
+        ctx->l1_timing_valid = timed;
+        ctx->launches += 3;
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(join());
-        CUDA_TRY(record_ev(ctx, 3));
-        return DKS_OK;
+        path[DKS_PATH_GENERAL_L1] = 1;
+        p.list = ctx->d_idx_plain;
+        p.count = ctx->d_l1_counts + 1;
     }
     if (G > 64) {
         // two-word coalition rows exist on the shared-plan path only: anything left over is reported, not computed
@@ -565,7 +636,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if ((long long)smem > (long long)ctx->max_smem_optin && (fast || multi)) {
             // the shared-plan path took the instances whose groups all vary; the general kernel is sized for the largest
             // plan set and cannot hold it.  The instances left for it (often none) are reported, not computed.
-            dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
+            dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(p.count, G, ctx->d_status);
             ctx->launches += 1;
             path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
             CUDA_TRY(cudaGetLastError());
@@ -584,13 +655,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if ((long long)smem > (long long)ctx->max_smem_optin)
             return fail(DKS_ERR_UNSUPPORTED, "SIMT kernel needs %zu B of shared memory (> %d): N*G or nsamples too large",
                         smem, ctx->max_smem_optin);
-        CUDA_TRY(cudaFuncSetAttribute(dks::explain_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(dks::explain_simt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int per_sm = (int)((size_t)ctx->max_smem_optin / (smem + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 8) per_sm = 8;
         int grid = ctx->sm_count * per_sm;
         if (grid > n) grid = n;
-        dks::explain_simt_kernel<<<grid, 256, smem, gstream>>>(p);
+        dks::explain_simt_kernel<false><<<grid, 256, smem, gstream>>>(p, dks::SimtL1{});
         ctx->launches += 1;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT;
     }
@@ -747,6 +818,7 @@ int dks_create(dks_ctx** out, int device) {
     CUDA_TRY(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
     ctx->own_stream = true;
     for (int i = 0; i < 4; ++i) CUDA_TRY(cudaEventCreate(&ctx->ev[i]));
+    for (int i = 0; i < 3; ++i) CUDA_TRY(cudaEventCreate(&ctx->ev_l1[i]));
     CUDA_TRY(cudaStreamCreateWithFlags(&ctx->side_stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
     CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
@@ -756,6 +828,9 @@ int dks_create(dks_ctx** out, int device) {
     ctx->d_counts = ctx->d_status + 2;
     ctx->d_hist = ctx->d_status + 4;
     CUDA_TRY(cudaMemset(ctx->d_status, 0, sizeof(int) * (4 + DKS_MAX_GROUPS + 1)));
+    CUDA_TRY(cudaMalloc((void**)&ctx->d_l1, sizeof(dks::l1::Tables) * (DKS_L1_MAX_GROUPS + 1)));
+    CUDA_TRY(cudaMemset(ctx->d_l1, 0, sizeof(dks::l1::Tables) * (DKS_L1_MAX_GROUPS + 1)));
+    CUDA_TRY(cudaMalloc((void**)&ctx->d_l1_counts, sizeof(int) * 2));
     *out = ctx;
     return DKS_OK;
 }
@@ -771,13 +846,14 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_fnull); dev_free(&ctx->d_linkfnull); dev_free(&ctx->d_BWs); dev_free(&ctx->d_bases);
     dev_free(&ctx->d_wbf); dev_free(&ctx->d_wn); dev_free(&ctx->d_plans); dev_free(&ctx->d_X); dev_free(&ctx->d_XW); dev_free(&ctx->d_XT);
     dev_free(&ctx->d_vflag); dev_free(&ctx->d_vmask); dev_free(&ctx->d_M); dev_free(&ctx->d_dlink);
-    dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_sums); dev_free(&ctx->d_msums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_ltab_fb); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
+    dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_idx_sel); dev_free(&ctx->d_idx_plain); dev_free(&ctx->d_l1_counts); dev_free(&ctx->d_l1); dev_free(&ctx->d_sums); dev_free(&ctx->d_msums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_ltab_fb); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
     dev_free(&ctx->d_status); ctx->d_hist = nullptr; ctx->d_counts = nullptr; dev_free(&ctx->d_yw); dev_free(&ctx->d_betaw); dev_free(&ctx->d_acache); dev_free(&ctx->d_phi); if (ctx->h_phi_pin) { cudaFreeHost(ctx->h_phi_pin); ctx->h_phi_pin = nullptr; } dev_free(&ctx->d_genz); dev_free(&ctx->d_genw); dev_free(&ctx->d_genchol); dev_free(&ctx->d_genainv); dev_free(&ctx->d_afix); dev_free(&ctx->d_sinfo); dev_free(&ctx->d_extz);
     dev_free(&ctx->d_extw);
     dev_free(&ctx->dbg_T);
     dev_free(&ctx->dbg_time);
     free_plan_allocs(ctx, -1);
     for (int i = 0; i < 4; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
+    for (int i = 0; i < 3; ++i) if (ctx->ev_l1[i]) cudaEventDestroy(ctx->ev_l1[i]);
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
     if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
     if (ctx->side_stream) cudaStreamDestroy(ctx->side_stream);
@@ -951,6 +1027,7 @@ int dks_fit(dks_ctx* ctx) {
         memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
         ctx->max_plan_S = 0;
         CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));
+        TRY(sync_l1_tables(ctx));
     }
     ctx->fitted = true;
     ctx->epoch++;
@@ -1019,6 +1096,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
         memset(&ctx->h_smx[M], 0, sizeof(ctx->h_smx[M]));
         ctx->h_afix[M] = nullptr;
         ctx->epoch++;
+        TRY(sync_l1_tables(ctx));
     }
     const int W = dks_plan_words(M);                        // 64-bit words per coalition row
     const size_t S_even = ((size_t)S + 1) & ~(size_t)1;     // TMA bulk copies move 16-byte multiples
@@ -1146,6 +1224,7 @@ int dks_clear_plans(dks_ctx* ctx) {
     memset(ctx->h_sinfo, 0, sizeof(ctx->h_sinfo));
     ctx->max_plan_S = 0;
     CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));
+    TRY(sync_l1_tables(ctx));
     return DKS_OK;
 }
 
@@ -1183,11 +1262,12 @@ int dks_set_plan_projection(dks_ctx* ctx, int M, const double* pt_host, const do
     return DKS_OK;
 }
 
-int dks_set_l1(dks_ctx* ctx, int mode, int k, int others_plain) {
+int dks_set_l1(dks_ctx* ctx, int mode, int k, uint64_t sel_lo, uint64_t sel_hi) {
     REQUIRE(ctx && mode >= 0 && mode <= 3, "dks_set_l1: mode must be 0 (off), 1 (aic), 2 (bic) or 3 (num_features)");
     REQUIRE(mode != 3 || k >= 1, "dks_set_l1: num_features needs k >= 1");
-    if (mode != ctx->l1_mode || k != ctx->l1_k || others_plain != ctx->l1_others_plain) ctx->epoch++;
-    ctx->l1_mode = mode; ctx->l1_k = k; ctx->l1_others_plain = others_plain;
+    REQUIRE((sel_lo & 1ull) == 0, "dks_set_l1: M = 1 has nothing to select");
+    if (mode != ctx->l1_mode || k != ctx->l1_k || sel_lo != ctx->l1_sel[0] || sel_hi != ctx->l1_sel[1]) ctx->epoch++;
+    ctx->l1_mode = mode; ctx->l1_k = k; ctx->l1_sel[0] = sel_lo; ctx->l1_sel[1] = sel_hi;
     return DKS_OK;
 }
 
@@ -1195,7 +1275,8 @@ int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double*
                       const double* scale, const double* bz, const double* gram_w, const double* b_rows,
                       const double* sqab_rows, double sum_b, double sum_sqb, int n_aug) {
     BIND(ctx);
-    REQUIRE(M >= 2 && M <= DKS_MAX_GROUPS, "dks_set_l1_tables: M out of range");
+    REQUIRE(M >= 2 && M <= DKS_L1_MAX_GROUPS, "dks_set_l1_tables: M out of range (the selection covers at most %d groups)",
+            DKS_L1_MAX_GROUPS);
     REQUIRE(gram_raw && gram_norm && colsum && scale && bz && gram_w && b_rows && sqab_rows, "dks_set_l1_tables: NULL table");
     const PlanDev& pd = ctx->h_plans[M];
     REQUIRE(pd.z != nullptr && n_aug == 2 * pd.S, "dks_set_l1_tables: set the shared plan of M=%d first (n_aug = 2 S)", M);
@@ -1204,7 +1285,7 @@ int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double*
     double* base = nullptr;
     CUDA_TRY(cudaMalloc((void**)&base, sizeof(double) * total));
     ctx->plan_allocs[M].push_back(base);
-    dks_ctx::L1Dev d;
+    dks::l1::Tables d;
     memset(&d, 0, sizeof(d));
     double* q = base;
     auto put = [&](const double* src, size_t cnt, const double** dst) -> cudaError_t {
@@ -1220,7 +1301,7 @@ int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double*
     d.sum_b = sum_b; d.sum_sqb = sum_sqb; d.n_aug = n_aug; d.S = pd.S;
     ctx->h_l1[M] = d;
     ctx->epoch++;
-    return DKS_OK;
+    return sync_l1_tables(ctx);
 }
 
 int dks_set_plan_sampling(dks_ctx* ctx, int M, int nfixed, int n_full, int n_paired, int ncdf, const double* cdf_host,
@@ -1619,6 +1700,16 @@ int dks_last_timings(dks_ctx* ctx, float* ms3) {
     CUDA_TRY(cudaEventElapsedTime(&ms3[0], ctx->ev[0], ctx->ev[1]));
     CUDA_TRY(cudaEventElapsedTime(&ms3[1], ctx->ev[2], ctx->ev[3]));
     CUDA_TRY(cudaEventElapsedTime(&ms3[2], ctx->ev[0], ctx->ev[3]));
+    return DKS_OK;
+}
+
+int dks_last_general_l1_timings(dks_ctx* ctx, float* ms2) {
+    BIND(ctx);
+    REQUIRE(ms2 && ctx->l1_timing_valid, "dks_last_general_l1_timings: the last explain ran no general-list l1 selection "
+            "outside a graph capture");
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    CUDA_TRY(cudaEventElapsedTime(&ms2[0], ctx->ev_l1[0], ctx->ev_l1[1]));
+    CUDA_TRY(cudaEventElapsedTime(&ms2[1], ctx->ev_l1[1], ctx->ev_l1[2]));
     return DKS_OK;
 }
 

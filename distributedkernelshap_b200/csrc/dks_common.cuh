@@ -43,6 +43,23 @@ struct PlanDev {
     int W;               // 64-bit words per row
 };
 
+// ---- l1 feature selection: what plan.py:l1_tables computes for the shared plan of M groups (dks_set_l1_tables) -------
+#define DKS_L1_MAX_GROUPS 128
+namespace dks { namespace l1 {
+struct Tables {              // device pointers
+    const double* gram_raw;  // [M][M]
+    const double* gram_norm; // [M][M]
+    const double* colsum;    // [M]
+    const double* scale;     // [M]
+    const double* bz;        // [M]
+    const double* gram_w;    // [M][M] sum_s w_s z_sk z_sl
+    const double* b;         // [S] w_s |z_s|
+    const double* sqab;      // [S] sqrt(a_s) + sqrt(b_s)
+    double sum_b, sum_sqb;
+    int n_aug, S;
+};
+} }
+
 // What the device-side sampler needs to continue a plan past its enumerated prefix (per M; plan.py: sampling_info)
 struct DksSamplingInfo {
     int nfixed;           // enumerated rows
@@ -137,14 +154,17 @@ struct dks_ctx {
     PlanDev* d_plans = nullptr;
     std::vector<void*> plan_allocs[DKS_MAX_GROUPS + 1];   // device buffers owned by the plan of each M (freed on replace)
     int max_plan_S = 0;
-    // l1 feature selection (dks_set_l1 / dks_set_l1_tables): per-M tables on the device
-    struct L1Dev {
-        const double *gram_raw, *gram_norm, *colsum, *scale, *bz, *gram_w, *b, *sqab;
-        double sum_b, sum_sqb;
-        int n_aug, S;
-    };
-    L1Dev h_l1[DKS_MAX_GROUPS + 1] = {};
-    int l1_mode = 0, l1_k = 0, l1_others_plain = 0;
+    // l1 feature selection (dks_set_l1 / dks_set_l1_tables): per-M tables on the device, and a device copy of the table
+    // set (the general list's LARS reads each task's own M)
+    dks::l1::Tables h_l1[DKS_MAX_GROUPS + 1] = {};
+    dks::l1::Tables* d_l1 = nullptr;             // [DKS_L1_MAX_GROUPS + 1]
+    int l1_mode = 0, l1_k = 0;
+    uint64_t l1_sel[2] = {0, 0};                 // bit M - 1: instances with M varying groups select
+    int* d_idx_sel = nullptr;                    // [n] general-list instances whose M selects ...
+    int* d_idx_plain = nullptr;                  // [n] ... and the rest
+    int* d_l1_counts = nullptr;                  // [2] their counts
+    cudaEvent_t ev_l1[3] = {nullptr, nullptr, nullptr};   // around the general list's moments kernel and LARS
+    bool l1_timing_valid = false;
     // softmax head, full varying set (M == G): per-class Dm [C][N][S_pad] = 2^(d_c(s, j) - max_c d_c(s, j)) and row bounds
     // lo [C][S_pad] = min_j log2 Dm_c(s, j) (dks_multi.cuh); the one-vs-rest head's tables have one more slot each (nd per
     // element, hi per row) and Dm relative to nd; owned by plan_allocs[M], cleared with the plan

@@ -666,7 +666,23 @@ __host__ __device__ inline size_t simt_smem_bytes(int S_cap, int N, int Mmax, in
            sizeof(float) * ((size_t)Mmax * N * R + (size_t)N * R + (size_t)N);
 }
 
-__global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
+namespace l1 {   // dks_l1.cuh
+constexpr int MOM_THREADS = 256;
+template <int W, bool SCALED>
+__device__ void block_moments(const double* ys, int S, int M, const uint64_t* __restrict__ z, const double* __restrict__ w,
+                              const double* __restrict__ b, const double* __restrict__ sqab, double* mom,
+                              long long (*part)[32], double (*bound)[2]);
+}
+
+// l1 feature selection on this kernel (instantiation L1): for the instances of its list it stores the moment vectors of y
+// of every output instead of solving the WLS, and l1_lars_kernel selects and solves from them
+struct SimtL1 {
+    const l1::Tables* tabs;  // [DKS_L1_MAX_GROUPS + 1] tables of the shared plan of each M
+    double* mom;             // [n][outputs][2G + 4]
+};
+
+template <bool L1>
+__global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, SimtL1 q) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const bool ovr = p.act == DKS_ACT_OVR;
     const bool softmax = p.act == DKS_ACT_SOFTMAX || ovr;     // C score rows and C y buffers
@@ -674,6 +690,10 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
     const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C;
     const size_t slab = (size_t)p.n * G;
+    // L1: the moments' reduction scratch lives where the WLS keeps its normal matrix
+    long long (*part)[32] = reinterpret_cast<long long (*)[32]>(sm.A);
+    double (*bound)[2] = reinterpret_cast<double (*)[2]>(sm.A + l1::MOM_THREADS);
+    const size_t mstride = 2 * (size_t)G + 4;
 
     const int ninst = dks_inst_count(p);
     for (int qi = blockIdx.x; qi < ninst; qi += gridDim.x) {
@@ -754,6 +774,11 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
                 sm.ys[s] = y;
             }
             __syncthreads();
+            if constexpr (L1) {
+                const l1::Tables& t = q.tabs[M];
+                l1::block_moments<1, false>(sm.ys, S, M, zp, wp, t.b, t.sqab, q.mom + (size_t)i * mstride, part, bound);
+                continue;
+            }
 
             // WLS for output 1; output 0 is its exact negation (p0 = 1 - p1 row-wise)
             const double* Lf;
@@ -837,6 +862,13 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
                 }
             }
             __syncthreads();
+            if constexpr (L1) {
+                const l1::Tables& t = q.tabs[M];
+                for (int c = 0; c < C; ++c)
+                    l1::block_moments<1, true>(sm.ys + (size_t)c * p.S_cap, S, M, zp, wp, t.b, t.sqab,
+                                               q.mom + ((size_t)i * C + c) * mstride, part, bound);
+                continue;
+            }
             if (chol != nullptr) {
                 for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
             } else {
@@ -858,14 +890,16 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
             // identity head: the background average commutes with the head, so
             // ey_r(s) = fnull_r + sum_k z_sk (XW_i[k][r] - Bbar[k][r])   -- float64 throughout
             const double* Lf;
-            if (chol != nullptr) {
-                for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
-            } else {
-                wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
-                __syncthreads();
-                if (tid < 32) {
-                    bool ok = wls_cholesky_warp(sm.A, M - 1);
-                    if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
+            if constexpr (!L1) {
+                if (chol != nullptr) {
+                    for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
+                } else {
+                    wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
+                    __syncthreads();
+                    if (tid < 32) {
+                        bool ok = wls_cholesky_warp(sm.A, M - 1);
+                        if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
+                    }
                 }
             }
             Lf = sm.A;
@@ -884,6 +918,12 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p) {
                     sm.ys[s] = link_f(a, p.link) - lfn;
                 }
                 __syncthreads();
+                if constexpr (L1) {
+                    const l1::Tables& t = q.tabs[M];
+                    l1::block_moments<1, true>(sm.ys, S, M, zp, wp, t.b, t.sqab, q.mom + ((size_t)i * C + r) * mstride,
+                                               part, bound);
+                    continue;
+                }
                 const double delta = p.dlink[(size_t)i * C + r];
                 wls_build_rhs(zp, wp, sm.ys, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
                 __syncthreads();

@@ -14,6 +14,10 @@
 // l1_moments_kernel forms them from the (sum p1, sum p0) buffer of the coalition kernel (fixed-point accumulation: exact,
 // order-independent); l1_lars_kernel runs the path, the criterion (residual sums of squares as quadratic forms in the Gram
 // matrix), and the restricted WLS, one warp per instance, float64, the Cholesky factor of the active block in shared memory.
+//
+// Instances with a partial varying set (M < G, up to 64 groups) select on the shared plan of their own M: the CUDA-core
+// kernel (explain_simt_kernel<true>) forms their moments with the same block_moments, and l1_lars_kernel reads each task's
+// M, its tables and its varying groups.
 #pragma once
 
 #include "dks_shared.cuh"
@@ -26,89 +30,135 @@ constexpr double TINY32 = 1.17549435082228750797e-38;     // np.finfo(np.float32
 constexpr double EQ_TOL = 1.1920928955078125e-07;         // np.finfo(np.float32).eps
 constexpr double EPS64 = 2.220446049250313e-16;
 
-struct Tables {              // per plan (M == G), device pointers
-    const double* gram_raw;  // [M][M]
-    const double* gram_norm; // [M][M]
-    const double* colsum;    // [M]
-    const double* scale;     // [M]
-    const double* bz;        // [M]
-    const double* gram_w;    // [M][M] sum_s w_s z_sk z_sl
-    const double* b;         // [S] w_s |z_s|
-    const double* sqab;      // [S] sqrt(a_s) + sqrt(b_s)
-    double sum_b, sum_sqb;
-    int n_aug;
-};
-
 struct Params {
     int n, N, G, C, S, S_pad, link, mode, kfeat;
     int nout;                // outputs solved per instance: 1 (binary head: class 1, class 0 its negation) or C
+    int binary;              // the binary head (nout 1 is also the identity head with one output, which has no class 0)
+    int Mmax;                // largest M of the tasks (sizes each warp's shared-memory area)
     shared_path::HeadSource src;   // softmax / identity heads (nout == C)
     const float2* sums;      // [n][S_pad]
     const uint64_t* z;       // [S][W]
     const double* w;         // [S]
-    Tables t;
+    const Tables* tabs;      // [DKS_L1_MAX_GROUPS + 1] tables of the shared plan of each M
+    const int* Mcnt;         // [n] M per instance; NULL: every task has M = G (the shared-plan path)
+    const uint64_t* vmask;   // [n] varying groups per instance (with Mcnt; M <= 64)
     const double* dlink;     // [n][C]
     const double* linkfnull;
     const double* fnull;
     const int* list;
     const int* count;
-    double* mom;             // [n][nout][2G + 4]: c, u, T1, Qw, R
+    double* mom;             // [n][nout][2G + 4]: c [M], u [M], T1, Qw, R
     double* phi;             // [C][n][G]
     int* status;
 };
 
-// ---- moments of y over the plan rows: c_k, u_k (k < G) and T1 = sum b y, Qw = sum w y^2, R = sum (sqrt a + sqrt b) y
-// MULTI: the softmax and identity heads, one task per (instance, output) with y from p.src; the fixed point is scaled per
-// task (shared_path::fix_exponent; Qw, quadratic in y, by its own even exponent) and the moments are stored unscaled, so the
-// LARS path compares them with its absolute thresholds in the units of y.
-constexpr int MOM_THREADS = 256;
+// ---- moments of y over the rows of a plan of M groups: c_k = sum_s w_s z_sk y_s and u_k = sum_s b_s z_sk y_s (k < M) into
+// mom[k] and mom[M + k]; T1 = sum b y, Qw = sum w y^2, R = sum (sqrt a + sqrt b) y into mom[2M .. 2M + 2].  By a block of
+// MOM_THREADS threads; y (ys[s], s < S) is in shared memory, written before a __syncthreads.  2^-40 fixed point: exact and
+// order-independent.  SCALED (the multi-output heads): the fixed point is scaled per task by an exact power of two
+// (shared_path::fix_exponent; Qw, quadratic in y, by its own even exponent) and the moments are stored unscaled, so the LARS
+// path compares them with its absolute thresholds in the units of y.  part / bound: shared scratch.
+template <int W, bool SCALED>
+__device__ void block_moments(const double* ys, int S, int M, const uint64_t* __restrict__ z, const double* __restrict__ w,
+                              const double* __restrict__ b, const double* __restrict__ sqab, double* mom,
+                              long long (*part)[32], double (*bound)[2]) {
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    long long t1 = 0, qw = 0, rr = 0;
+    double sc = 1.0, isc = 1.0, sq = 1.0, isq = 1.0;
+    if constexpr (SCALED) {
+        double b1 = 0.0, b2 = 0.0;        // bounds of the linear moments and of Qw
+        for (int s = threadIdx.x; s < S; s += MOM_THREADS) {
+            const double y = ys[s];
+            b1 += (w[s] + b[s] + sqab[s]) * fabs(y);
+            b2 += w[s] * y * y;
+        }
+        b1 = warp_sum(b1); b2 = warp_sum(b2);
+        if (lane == 0) { bound[wib][0] = b1; bound[wib][1] = b2; }
+        __syncthreads();
+        double t1b = 0.0, t2b = 0.0;
+#pragma unroll
+        for (int wq = 0; wq < MOM_THREADS / 32; ++wq) { t1b += bound[wq][0]; t2b += bound[wq][1]; }
+        const int e1 = shared_path::fix_exponent(t1b), e2 = shared_path::fix_exponent(t2b) >> 1;
+        sc = ldexp(1.0, e1); isc = ldexp(1.0, -e1);
+        sq = ldexp(1.0, e2); isq = ldexp(1.0, -2 * e2);
+        for (int s = threadIdx.x; s < S; s += MOM_THREADS) {
+            const double y = ys[s];
+            t1 += to_fix(b[s] * y * sc);
+            qw += to_fix(w[s] * (y * sq) * (y * sq));
+            rr += to_fix(sqab[s] * y * sc);
+        }
+    } else {
+        for (int s = threadIdx.x; s < S; s += MOM_THREADS) {
+            const double y = ys[s];
+            t1 += to_fix(b[s] * y);
+            qw += to_fix(w[s] * y * y);
+            rr += to_fix(sqab[s] * y);
+        }
+    }
+    t1 = warp_sum_ll(t1); qw = warp_sum_ll(qw); rr = warp_sum_ll(rr);
+    if (lane == 0) { part[wib][0] = t1; part[wib][1] = qw; part[wib][2] = rr; }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+        long long acc = 0;
+        for (int wq = 0; wq < MOM_THREADS / 32; ++wq) acc += part[wq][threadIdx.x];
+        mom[2 * M + threadIdx.x] = SCALED ? from_fix(acc) * (threadIdx.x == 1 ? isq : isc) : from_fix(acc);
+    }
+    __syncthreads();
+    // sixteen coefficients of c and u per pass over the rows
+    for (int k0 = 0; k0 < M; k0 += 16) {
+        long long Ck[16], Uk[16];
+#pragma unroll
+        for (int k = 0; k < 16; ++k) { Ck[k] = 0; Uk[k] = 0; }
+#pragma unroll 2
+        for (int s = threadIdx.x; s < S; s += MOM_THREADS) {
+            const double y = SCALED ? ys[s] * sc : ys[s];
+            const long long vc = to_fix(w[s] * y), vu = to_fix(b[s] * y);
+            const uint32_t zb = (uint32_t)(z[(size_t)s * W + (k0 >> 6)] >> (k0 & 63));
+#pragma unroll
+            for (int k = 0; k < 16; ++k)
+                if ((zb >> k) & 1u) { Ck[k] += vc; Uk[k] += vu; }
+        }
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            const long long rc = warp_sum_ll(Ck[k]), ru = warp_sum_ll(Uk[k]);
+            if (lane == 0) { part[wib][k] = rc; part[wib][16 + k] = ru; }
+        }
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            long long acc = 0;
+            for (int wq = 0; wq < MOM_THREADS / 32; ++wq) acc += part[wq][threadIdx.x];
+            const int k = k0 + (threadIdx.x & 15);
+            if (k < M) mom[(threadIdx.x < 16 ? 0 : M) + k] = SCALED ? from_fix(acc) * isc : from_fix(acc);
+        }
+        __syncthreads();
+    }
+}
+
+// ---- moments of the shared-plan path's instances (M = G): y from the (sum p1, sum p0) buffer, or (MULTI: the softmax,
+// one-vs-rest and identity heads, one task per (instance, output)) from p.src
 template <int W, bool MULTI = false>
 __global__ void __launch_bounds__(MOM_THREADS) l1_moments_kernel(Params p) {
     extern __shared__ double s_y[];                       // [S]
     __shared__ long long s_part[MOM_THREADS / 32][32];
     __shared__ LogTabEntry s_logtab[DKS_LOGTAB_SIZE];
     __shared__ double s_bound[MOM_THREADS / 32][2];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int G = p.G;
     const int nout = MULTI ? p.nout : 1;
     const int cnt = *p.count * nout;
     if ((int)blockIdx.x >= cnt) return;
     if (threadIdx.x < DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x);
     __syncthreads();
+    const Tables& t = p.tabs[G];
     const double lf1 = p.linkfnull[1], f1 = p.fnull[1], inv_n = 1.0 / (double)p.N;
     for (int m = blockIdx.x; m < cnt; m += gridDim.x) {
         const int i = p.list[MULTI ? m / nout : m];
         const int cls = MULTI ? m % nout : 1;
         const float2* sums = p.sums + (size_t)i * p.S_pad;
         double* mom = p.mom + ((size_t)i * nout + (MULTI ? cls : 0)) * (2 * G + 4);
-        // pass 0: y into shared memory + the three scalars
-        long long t1 = 0, qw = 0, rr = 0;
-        double sc = 1.0, isc = 1.0, sq = 1.0, isq = 1.0;
         if constexpr (MULTI) {
             const double fnc = p.fnull[cls], lfc = p.linkfnull[cls];
-            double b1 = 0.0, b2 = 0.0;        // bounds of the linear moments and of Qw
-            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
-                const double y = shared_path::head_y<W>(p.src, i, cls, p.C, s, p.S_pad, p.z + (size_t)s * W, p.link, inv_n,
-                                                        fnc, lfc);
-                s_y[s] = y;
-                b1 += (p.w[s] + p.t.b[s] + p.t.sqab[s]) * fabs(y);
-                b2 += p.w[s] * y * y;
-            }
-            b1 = warp_sum(b1); b2 = warp_sum(b2);
-            if (lane == 0) { s_bound[wib][0] = b1; s_bound[wib][1] = b2; }
-            __syncthreads();
-            double t1b = 0.0, t2b = 0.0;
-#pragma unroll
-            for (int wq = 0; wq < MOM_THREADS / 32; ++wq) { t1b += s_bound[wq][0]; t2b += s_bound[wq][1]; }
-            const int e1 = shared_path::fix_exponent(t1b), e2 = shared_path::fix_exponent(t2b) >> 1;
-            sc = ldexp(1.0, e1); isc = ldexp(1.0, -e1);
-            sq = ldexp(1.0, e2); isq = ldexp(1.0, -2 * e2);
-            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
-                const double y = s_y[s];
-                t1 += to_fix(p.t.b[s] * y * sc);
-                qw += to_fix(p.w[s] * (y * sq) * (y * sq));
-                rr += to_fix(p.t.sqab[s] * y * sc);
-            }
+            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS)
+                s_y[s] = shared_path::head_y<W>(p.src, i, cls, p.C, s, p.S_pad, p.z + (size_t)s * W, p.link, inv_n, fnc, lfc);
         } else {
             for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
                 const float2 a = sums[s];
@@ -116,48 +166,25 @@ __global__ void __launch_bounds__(MOM_THREADS) l1_moments_kernel(Params p) {
                 if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(a.x, a.y, s_logtab) - lf1;
                 else y = (double)a.x * inv_n - f1;
                 s_y[s] = y;
-                t1 += to_fix(p.t.b[s] * y);
-                qw += to_fix(p.w[s] * y * y);
-                rr += to_fix(p.t.sqab[s] * y);
             }
-        }
-        t1 = warp_sum_ll(t1); qw = warp_sum_ll(qw); rr = warp_sum_ll(rr);
-        if (lane == 0) { s_part[wib][0] = t1; s_part[wib][1] = qw; s_part[wib][2] = rr; }
-        __syncthreads();
-        if (threadIdx.x < 3) {
-            long long acc = 0;
-            for (int wq = 0; wq < MOM_THREADS / 32; ++wq) acc += s_part[wq][threadIdx.x];
-            mom[2 * G + threadIdx.x] = MULTI ? from_fix(acc) * (threadIdx.x == 1 ? isq : isc) : from_fix(acc);
         }
         __syncthreads();
-        // sixteen coefficients of c and u per pass over the rows
-        for (int k0 = 0; k0 < G; k0 += 16) {
-            long long Ck[16], Uk[16];
-#pragma unroll
-            for (int k = 0; k < 16; ++k) { Ck[k] = 0; Uk[k] = 0; }
-#pragma unroll 2
-            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
-                const double y = MULTI ? s_y[s] * sc : s_y[s];
-                const long long vc = to_fix(p.w[s] * y), vu = to_fix(p.t.b[s] * y);
-                const uint32_t zb = (uint32_t)(p.z[(size_t)s * W + (k0 >> 6)] >> (k0 & 63));
-#pragma unroll
-                for (int k = 0; k < 16; ++k)
-                    if ((zb >> k) & 1u) { Ck[k] += vc; Uk[k] += vu; }
-            }
-#pragma unroll
-            for (int k = 0; k < 16; ++k) {
-                const long long rc = warp_sum_ll(Ck[k]), ru = warp_sum_ll(Uk[k]);
-                if (lane == 0) { s_part[wib][k] = rc; s_part[wib][16 + k] = ru; }
-            }
-            __syncthreads();
-            if (threadIdx.x < 32) {
-                long long acc = 0;
-                for (int wq = 0; wq < MOM_THREADS / 32; ++wq) acc += s_part[wq][threadIdx.x];
-                const int k = k0 + (threadIdx.x & 15);
-                if (k < G) mom[(threadIdx.x < 16 ? 0 : G) + k] = MULTI ? from_fix(acc) * isc : from_fix(acc);
-            }
-            __syncthreads();
-        }
+        block_moments<W, MULTI>(s_y, p.S, G, p.z, p.w, t.b, t.sqab, mom, s_part, s_bound);
+    }
+}
+
+// splits the general kernels' instance list (all n instances when list is NULL) into those whose M selects (bit M - 1 of
+// sel) and the rest; counts [2] are zero on entry
+__global__ void l1_partition_kernel(const int* __restrict__ list, const int* __restrict__ count, int n,
+                                    const int* __restrict__ Mcnt, uint64_t sel_lo, uint64_t sel_hi, int* __restrict__ out_sel,
+                                    int* __restrict__ out_plain, int* __restrict__ counts) {
+    const int cnt = list != nullptr ? *count : n;
+    for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < cnt; q += gridDim.x * blockDim.x) {
+        const int i = list != nullptr ? list[q] : q;
+        const int M = Mcnt[i];
+        const bool sel = M >= 1 && M <= 128 && (((M <= 64 ? sel_lo >> (M - 1) : sel_hi >> (M - 65)) & 1ull) != 0);
+        if (sel) out_sel[atomicAdd(&counts[0], 1)] = i;
+        else out_plain[atomicAdd(&counts[1], 1)] = i;
     }
 }
 
@@ -208,56 +235,69 @@ __device__ inline void chol_solve(const double* L, double* x, int k, int lane) {
     __syncwarp();
 }
 
+// a warp's area ends with M ints: rounded up to whole doubles, so that the next warp's area (and the staged Gram matrix
+// behind the last one) stays 8-byte aligned for odd M
 __host__ __device__ inline size_t lars_smem_per_warp(int M) {
-    return sizeof(double) * ((size_t)M * (M + 1) / 2 + 8 * (size_t)M) + sizeof(int) * (size_t)M;
+    const size_t bytes = sizeof(double) * ((size_t)M * (M + 1) / 2 + 8 * (size_t)M) + sizeof(int) * (size_t)M;
+    return (bytes + sizeof(double) - 1) / sizeof(double) * sizeof(double);
 }
 
-// one warp per instance
+// group of the v-th varying position (the v-th set bit of vm)
+__device__ __forceinline__ int nth_set_bit(uint64_t vm, int v) {
+    for (int r = 0; r < v; ++r) vm &= vm - 1;
+    return __ffsll((long long)vm) - 1;
+}
+
+// one warp per (instance, output).  stage_gram: every task has M = p.Mmax (the shared-plan path's launch), whose Gram matrix
+// the CTA stages in shared memory; tasks of mixed M (the general list) read theirs through L2.
 __global__ void l1_lars_kernel(Params p, int warps_per_cta, int stage_gram) {
     extern __shared__ __align__(16) unsigned char l1_smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const int M = p.G, C = p.C;
+    const int G = p.G, C = p.C;
     const int cnt = *p.count;
-    const size_t per_warp = lars_smem_per_warp(M);
-    const bool lasso_mode = p.mode != MODE_NUM_FEATURES;
+    const size_t per_warp = lars_smem_per_warp(p.Mmax);
+    const bool lasso = p.mode != MODE_NUM_FEATURES;
+    double* sg = reinterpret_cast<double*>(l1_smem + (size_t)warps_per_cta * per_warp);
     if (stage_gram) {
         // the Gram matrix of the path (read k (M - k) times per step) shared by the warps of the CTA, behind their private areas
-        double* sg = reinterpret_cast<double*>(l1_smem + (size_t)warps_per_cta * per_warp);
-        const double* src = lasso_mode ? p.t.gram_norm : p.t.gram_raw;
-        for (int idx = threadIdx.x; idx < M * M; idx += blockDim.x) sg[idx] = src[idx];
+        const Tables& t = p.tabs[p.Mmax];
+        const double* src = lasso ? t.gram_norm : t.gram_raw;
+        for (int idx = threadIdx.x; idx < p.Mmax * p.Mmax; idx += blockDim.x) sg[idx] = src[idx];
         __syncthreads();
     }
-    double* L = reinterpret_cast<double*>(l1_smem + (size_t)wib * per_warp);    // packed lower triangle
-    double* cov = L + (size_t)M * (M + 1) / 2;      // by variable
-    double* cov0 = cov + M;
-    double* coef = cov0 + M;                        // by variable
-    double* ls = coef + M;                          // by active position
-    double* corr = ls + M;                          // by variable
-    double* sgn = corr + M;                         // by active position
-    double* xrow = sgn + M;                         // scratch
-    double* cm = xrow + M;                          // c moments (by variable)
-    int* perm = reinterpret_cast<int*>(cm + M);     // position -> variable
-    const bool lasso = lasso_mode;
-    const double* gram = stage_gram ? reinterpret_cast<const double*>(l1_smem + (size_t)warps_per_cta * per_warp)
-                                    : (lasso ? p.t.gram_norm : p.t.gram_raw);
-    const double nsamp = (double)p.t.n_aug;
+    unsigned char* warea = l1_smem + (size_t)wib * per_warp;
     const int max_iter = lasso ? 500 : p.kfeat;
-    const size_t slab = (size_t)p.n * M;
+    const size_t slab = (size_t)p.n * G;
 
     const int nout = p.nout;
     for (int m = blockIdx.x * warps_per_cta + wib; m < cnt * nout; m += gridDim.x * warps_per_cta) {
         // one warp per (instance, output): upstream's solve runs the selection for each output on its own
         const int i = p.list[m / nout];
-        const int cls = nout == 1 ? 1 : m % nout;
-        const double* mom = p.mom + ((size_t)i * nout + (nout == 1 ? 0 : cls)) * (2 * M + 4);
+        const int cls = p.binary ? 1 : m % nout;
+        const int M = p.Mcnt != nullptr ? p.Mcnt[i] : G;
+        const Tables* t = p.tabs + M;
+        double* L = reinterpret_cast<double*>(warea);  // packed lower triangle
+        double* cov = L + (size_t)M * (M + 1) / 2;      // by variable
+        double* cov0 = cov + M;
+        double* coef = cov0 + M;                        // by variable
+        double* ls = coef + M;                          // by active position
+        double* corr = ls + M;                          // by variable
+        double* sgn = corr + M;                         // by active position
+        double* xrow = sgn + M;                         // scratch
+        double* cm = xrow + M;                          // c moments (by variable)
+        int* perm = reinterpret_cast<int*>(cm + M);     // position -> variable
+        const double* gram = stage_gram ? sg : (lasso ? t->gram_norm : t->gram_raw);
+        const double nsamp = (double)t->n_aug;
+        const double sum_b = t->sum_b;
+        const double* mom = p.mom + ((size_t)i * nout + (p.binary ? 0 : cls)) * (2 * G + 4);
         const double delta = p.dlink[(size_t)i * C + cls];
         const double T1 = mom[2 * M], Qw = mom[2 * M + 1], R = mom[2 * M + 2];
-        const double ybar = lasso ? (R - delta * p.t.sum_sqb) / nsamp : 0.0;
-        const double yy = (double)M * Qw - 2.0 * delta * T1 + delta * delta * p.t.sum_b - nsamp * ybar * ybar;
+        const double ybar = lasso ? (R - delta * t->sum_sqb) / nsamp : 0.0;
+        const double yy = (double)M * Qw - 2.0 * delta * T1 + delta * delta * sum_b - nsamp * ybar * ybar;
         for (int v = lane; v < M; v += 32) {
             const double c = mom[v], u = mom[M + v];
-            double xty = ((double)M * c - u) - ((T1 - u) - delta * (p.t.sum_b - p.t.bz[v]));
-            if (lasso) xty = (xty - p.t.colsum[v] * ybar) / p.t.scale[v];
+            double xty = ((double)M * c - u) - ((T1 - u) - delta * (sum_b - t->bz[v]));
+            if (lasso) xty = (xty - t->colsum[v] * ybar) / t->scale[v];
             cov[v] = xty; cov0[v] = xty; coef[v] = 0.0; corr[v] = 0.0; cm[v] = c; perm[v] = v;
         }
         __syncwarp();
@@ -434,16 +474,19 @@ __global__ void l1_lars_kernel(Params p, int warps_per_cta, int stage_gram) {
             if (on) { if (lane == 0) perm[q] = v; ++q; }
         }
         __syncwarp();
-        double* phi1 = p.phi + (size_t)cls * slab + (size_t)i * M;
-        double* phi0 = p.phi + (size_t)i * M;       // binary head only: class 0 is the negation of class 1
-        const bool anti = nout == 1;
-        for (int v = lane; v < M; v += 32) { phi1[v] = 0.0; if (anti) phi0[v] = 0.0; }
+        double* phi1 = p.phi + (size_t)cls * slab + (size_t)i * G;
+        double* phi0 = p.phi + (size_t)i * G;       // binary head only: class 0 is the negation of class 1
+        const bool anti = p.binary != 0;
+        // variable v is the group of the v-th varying position; the groups that do not vary keep zeros
+        const uint64_t vm = p.Mcnt != nullptr ? p.vmask[i] : 0ull;
+        auto grp = [&](int v) { return p.Mcnt != nullptr ? nth_set_bit(vm, v) : v; };
+        for (int g = lane; g < G; g += 32) { phi1[g] = 0.0; if (anti) phi0[g] = 0.0; }
         __syncwarp();
         if (q == 1) {
-            if (lane == 0) { double val = fabs(delta) < 1e-10 ? 0.0 : delta; phi1[perm[0]] = val; if (anti) phi0[perm[0]] = val == 0.0 ? 0.0 : -val; }
+            if (lane == 0) { double val = fabs(delta) < 1e-10 ? 0.0 : delta; const int g = grp(perm[0]); phi1[g] = val; if (anti) phi0[g] = val == 0.0 ? 0.0 : -val; }
         } else if (q >= 2) {
             const int nA = q - 1, Lv = perm[q - 1];
-            const double* gw = p.t.gram_w;
+            const double* gw = t->gram_w;
             const double gLL = gw[(size_t)Lv * M + Lv];
             for (int r = lane; r < nA; r += 32) {
                 const int vr = perm[r];
@@ -477,15 +520,17 @@ __global__ void l1_lars_kernel(Params p, int warps_per_cta, int stage_gram) {
                 double val = xrow[r];
                 sum += val;
                 if (fabs(val) < 1e-10) val = 0.0;
-                phi1[perm[r]] = val;
-                if (anti) phi0[perm[r]] = val == 0.0 ? 0.0 : -val;
+                const int g = grp(perm[r]);
+                phi1[g] = val;
+                if (anti) phi0[g] = val == 0.0 ? 0.0 : -val;
             }
             sum = wsum(sum);
             if (lane == 0) {
                 double last = delta - sum;
                 if (fabs(last) < 1e-10) last = 0.0;
-                phi1[Lv] = last;
-                if (anti) phi0[Lv] = last == 0.0 ? 0.0 : -last;
+                const int g = grp(Lv);
+                phi1[g] = last;
+                if (anti) phi0[g] = last == 0.0 ? 0.0 : -last;
             }
         }
         __syncwarp();

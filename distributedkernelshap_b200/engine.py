@@ -38,6 +38,54 @@ def refuse_partial_sets_beyond_64_groups(G, hist):
             "needs every group to vary (unsupported otherwise)")
 
 
+def _explicit_l1(l1_reg):
+    """``(mode, k)`` of ``dks_set_l1`` for an ``l1_reg`` that selects whatever the sampled fraction ('aic', 'bic',
+    'num_features(k)'), None for 'auto'; a fixed Lasso strength is refused."""
+    if l1_reg in ("aic", "bic"):
+        return (1 if l1_reg == "aic" else 2, 0)
+    if isinstance(l1_reg, str) and l1_reg.startswith("num_features("):
+        return (3, int(l1_reg[len("num_features("):-1]))
+    if l1_reg != "auto":
+        raise NotImplementedError(f"l1_reg={l1_reg!r}: a fixed Lasso strength is not implemented in the CUDA engine; "
+                                  "use 'auto', 'aic', 'bic', 'num_features(k)' or False")
+    return None
+
+
+def _auto_selects(M, nsamples):
+    """l1_reg='auto': upstream selects when less than 20% of the coalition space of M groups is evaluated."""
+    S, max_s = resolve_nsamples(M, nsamples)
+    return S / max_s < 0.2
+
+
+def l1_selecting_sizes(l1_reg, nsamples, G, hist):
+    """Which instances run upstream's l1 feature selection before the constrained WLS (``solve``): all of them under
+    'aic' / 'bic' / 'num_features(k)', and under 'auto' those whose coalition plan covers less than 20% of the coalition
+    space -- a property of their number M of varying groups.  ``hist[M]`` = instances with M varying groups.  Returns
+    ``(mode, k, sizes)``: the ``dks_set_l1`` mode and k, and the sorted M (>= 2, present in ``hist``) that select; mode 0
+    and no sizes when none does.  Raises for what the engine does not cover: a fixed Lasso strength, more than 128 groups
+    selecting, and partial varying sets selecting beyond 64 groups."""
+    if l1_reg in (False, 0):
+        return 0, 0, []
+    explicit = _explicit_l1(l1_reg)
+
+    sizes = [M for M in range(2, G + 1) if hist[M] > 0 and (explicit is not None or _auto_selects(M, nsamples))]
+    if not sizes:
+        return 0, 0, []
+    if max(sizes) > 128:
+        raise NotImplementedError(
+            f"l1_reg={l1_reg!r} selects features among {max(sizes)} varying groups; the CUDA engine's LARS path covers at "
+            "most 128 groups -- pass l1_reg=False for the plain constrained WLS (or 'num_features(k)' on a narrower "
+            "grouping)")
+    partial = [M for M in sizes if M != G]
+    if partial and G > 64:
+        raise NotImplementedError(
+            f"l1_reg={l1_reg!r} selects features for instances with M in {partial[:8]} varying groups of {G} (a partial "
+            "varying set): beyond 64 groups the CUDA engine selects for instances whose groups all vary only -- pass "
+            "l1_reg=False")
+    mode, k = explicit if explicit is not None else (1, 0)
+    return mode, k, sizes
+
+
 class GpuKernelExplainer:
     """CUDA KernelSHAP explainer with the interface of ``shap.KernelExplainer`` / ``KernelExplainerWrapper``.
 
@@ -115,7 +163,8 @@ class GpuKernelExplainer:
         self._nsamples_req = None
         self._plan_cache = {}
         self._l1_uploaded = {}
-        self._l1_state = (0, 0, 0)
+        self._l1_state = (0, 0, 0, 0)
+        self._l1_general_all_select = False
         self._link_fx_parts = []
         self._last_rows = 0
         self._check_model_against_callable(bg)
@@ -157,68 +206,40 @@ class GpuKernelExplainer:
             _cabi.check(self.lib.dks_set_nsamples(self._ctx, req))
             self._nsamples_req = req
 
-    def _l1_guard(self, l1_reg, nsamples, hist=None):
-        """Upstream's ``solve`` runs an l1 feature selection before the constrained WLS when ``l1_reg`` is 'aic' / 'bic' /
-        'num_features(k)', or under 'auto' when fewer than 20% of the coalition space is evaluated.  Without ``hist``:
-        whether the M histogram is needed to decide.  With it: ``(mode, k, others_plain)`` for ``dks_set_l1`` -- the
-        selection runs on the shared-plan path (csrc/dks_l1.cuh) for the instances whose groups all vary (per output for the
-        softmax and identity heads); what that path does not cover is refused, never silently solved without the selection."""
+    def _l1_guard(self, l1_reg, nsamples):
+        """Whether the call needs the M histogram to decide which instances run upstream's l1 feature selection
+        (``l1_selecting_sizes``); a fixed Lasso strength is refused here, before any work."""
         if l1_reg in (False, 0):
-            return False if hist is None else (0, 0, 0)
-        G = self.data.groups_size
-        explicit = None
-        if l1_reg in ("aic", "bic"):
-            explicit = (1 if l1_reg == "aic" else 2, 0)
-        elif isinstance(l1_reg, str) and l1_reg.startswith("num_features("):
-            explicit = (3, int(l1_reg[len("num_features("):-1]))
-        elif l1_reg != "auto":
-            raise NotImplementedError(f"l1_reg={l1_reg!r}: a fixed Lasso strength is not implemented in the CUDA engine; "
-                                      "use 'auto', 'aic', 'bic', 'num_features(k)' or False")
-
-        def needs(M):
-            if explicit is not None:
-                return True
-            S, max_s = resolve_nsamples(M, nsamples)
-            return S / max_s < 0.2
-        if hist is None:
-            return explicit is not None or any(needs(M) for M in range(2, G + 1))
-        present = [M for M in range(2, G + 1) if hist[M] > 0]
-        wanting = [M for M in present if needs(M)]
-        if not wanting:
-            return (0, 0, 0)
-        if max(wanting) > 128:
-            raise NotImplementedError(
-                f"l1_reg={l1_reg!r} selects features among {max(wanting)} varying groups; the CUDA engine's LARS path covers at "
-                "most 128 groups -- pass l1_reg=False for the plain constrained WLS (or 'num_features(k)' on a narrower "
-                "grouping)")
-        partial = [M for M in wanting if M != G]
-        if partial:
-            raise NotImplementedError(
-                f"l1_reg={l1_reg!r} selects features for instances with M in {partial} varying groups (a partial varying "
-                "set); the CUDA engine runs the selection for instances whose groups all vary only -- pass l1_reg=False")
-        if self.plan_mode != "shared":
-            raise NotImplementedError("l1 feature selection runs with plan_mode='shared' only")
-        mode, k = explicit if explicit is not None else (1, 0)
-        return (mode, k, 1 if len(present) > 1 else 0)
+            return False
+        return _explicit_l1(l1_reg) is not None or any(_auto_selects(M, nsamples)
+                                                       for M in range(2, self.data.groups_size + 1))
 
     def _apply_l1(self, l1_reg, nsamples, hist):
-        """Uploads the l1 tables of the G-group plan when the call needs them and tells the library the mode."""
-        mode, k, others_plain = (0, 0, 0) if l1_reg in (False, 0) else self._l1_guard(l1_reg, nsamples, hist)
-        if mode:
-            G = self.data.groups_size
-            S, _ = resolve_nsamples(G, nsamples)
-            if self._l1_uploaded.get(G) != S:
+        """Tells the library which M select (``l1_selecting_sizes``) and uploads the l1 tables of their shared plans,
+        cached per (M, S).  The selection runs on the shared plans only, never solved without it: what the library does
+        not cover raises."""
+        G = self.data.groups_size
+        mode, k, sizes = (0, 0, []) if l1_reg in (False, 0) else l1_selecting_sizes(l1_reg, nsamples, G, hist)
+        if sizes and self.plan_mode != "shared":
+            raise NotImplementedError("l1 feature selection runs with plan_mode='shared' only")
+        for M in sizes:
+            S, _ = resolve_nsamples(M, nsamples)
+            if self._l1_uploaded.get(M) != S:
                 self._ensure_shared_plans(hist, nsamples)
-                t = l1_tables(self.shared_plan(G, nsamples))
+                t = l1_tables(self.shared_plan(M, nsamples))
                 sqab = np.ascontiguousarray(t["sqa"] + t["sqb"])
                 _cabi.check(self.lib.dks_set_l1_tables(
-                    self._ctx, G, _cabi.ptr(t["gram_raw"]), _cabi.ptr(t["gram_norm"]), _cabi.ptr(t["colsum"]),
+                    self._ctx, M, _cabi.ptr(t["gram_raw"]), _cabi.ptr(t["gram_norm"]), _cabi.ptr(t["colsum"]),
                     _cabi.ptr(t["scale"]), _cabi.ptr(t["bz"]), _cabi.ptr(t["gram_w"]), _cabi.ptr(t["b"]), _cabi.ptr(sqab),
                     t["sum_b"], t["sum_sqb"], t["n_aug"]))
-                self._l1_uploaded[G] = S
-        if (mode, k, others_plain) != self._l1_state:
-            _cabi.check(self.lib.dks_set_l1(self._ctx, mode, k, others_plain))
-            self._l1_state = (mode, k, others_plain)
+                self._l1_uploaded[M] = S
+        sel_lo = sum(1 << (M - 1) for M in sizes if M <= 64)
+        sel_hi = sum(1 << (M - 65) for M in sizes if M > 64)
+        # the general list (instances with M < G) runs the selection for some; does it hold any that do not select?
+        self._l1_general_all_select = bool(sizes) and not any(hist[M] > 0 for M in range(G) if M not in sizes)
+        if (mode, k, sel_lo, sel_hi) != self._l1_state:
+            _cabi.check(self.lib.dks_set_l1(self._ctx, mode, k, sel_lo, sel_hi))
+            self._l1_state = (mode, k, sel_lo, sel_hi)
 
     def shared_plan(self, M, nsamples="auto"):
         """The coalition plan every instance with ``M`` varying groups shares under ``plan_mode='shared'`` (also the
@@ -344,7 +365,7 @@ class GpuKernelExplainer:
             zb, w, stride = self._pack_external_plans(plans, n, nsamples)
             if need_hist:
                 _cabi.check(self.lib.dks_prepare_host(self._ctx, _cabi.ptr(X), n))
-                if self._l1_guard(l1_reg, nsamples, self.m_histogram())[0]:
+                if l1_selecting_sizes(l1_reg, nsamples, G, self.m_histogram())[2]:
                     raise NotImplementedError("l1 feature selection runs on the engine's shared plans, not on "
                                               "caller-supplied per-instance plans -- pass l1_reg=False")
             self._apply_l1(False, nsamples, None)
@@ -568,15 +589,28 @@ class GpuKernelExplainer:
         are reported as unsupported, not computed), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
-        the weighted one) and ``fused_table`` (1: the fused kernel read y from the plan's link table, passes outside its
-        domain excepted; 0: the exact loop over the background throughout)."""
-        out = np.zeros(12, dtype=np.int32)
+        the weighted one), ``fused_table`` (1: the fused kernel read y from the plan's link table, passes outside its
+        domain excepted; 0: the exact loop over the background throughout) and ``general_l1`` (1: the general list's
+        instances whose M selects ran the l1 selection -- moments on the CUDA-core kernel, then the LARS kernel; ``general``
+        then names the kernel of the others, or 'simt' when every instance of the general list selected)."""
+        out = np.zeros(13, dtype=np.int32)
         _cabi.check(self.lib.dks_last_path(self._ctx, _cabi.ptr(out), len(out)))
         names = self._PATH_NAMES
+        general = names["general"][out[8]]
+        if out[12] and self._l1_general_all_select:
+            general = "simt"
         return {"shared": names["shared"][out[0]], "chunks": int(out[1]), "warps": int(out[2]), "grid": int(out[3]),
                 "fused_B": int(out[4]), "fused_NI": int(out[5]), "solve": names["solve"][out[6]],
-                "pmat_kpad": int(out[7]), "general": names["general"][out[8]],
-                "cta_warps": int(out[9]), "bg_weights": ("uniform", "weighted")[out[10]], "fused_table": int(out[11])}
+                "pmat_kpad": int(out[7]), "general": general,
+                "cta_warps": int(out[9]), "bg_weights": ("uniform", "weighted")[out[10]], "fused_table": int(out[11]),
+                "general_l1": int(out[12])}
+
+    def general_l1_timings_ms(self):
+        """Device time of the last explain's l1 selection on the general list (``last_path()["general_l1"]``), from the
+        engine's CUDA events: ``general`` (the CUDA-core kernel forming the moments) and ``lars`` (the LARS kernel)."""
+        out = np.zeros(2, dtype=np.float32)
+        _cabi.check(self.lib.dks_last_general_l1_timings(self._ctx, _cabi.ptr(out)))
+        return {"general": float(out[0]), "lars": float(out[1])}
 
     def fused_table_info(self, M):
         """The fused kernel's link table of the plan over M groups: ``bytes`` (0: no table, the exact loop runs) and

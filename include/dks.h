@@ -111,12 +111,16 @@ int dks_has_shared_plan(dks_ctx* ctx, int M, int* present);
 /* ---- l1 feature selection: the l1_reg branch of KernelExplainer.solve (kwargs path kernel_shap.py:836-845, :880) --------
  * mode 0 = off (plain constrained WLS), 1 = LassoLarsIC 'aic' (what l1_reg='auto' means when under 20% of the coalition
  * space is sampled), 2 = 'bic', 3 = 'num_features(k)' (lars_path with max_iter = k); scikit-learn 0.23.2 semantics (the
- * reference's pin).  Runs on the shared-plan path for instances whose groups all vary; others_plain != 0 lets the remaining
- * instances take the plain WLS (the caller has checked that upstream would not select features for them), 0 reports them
- * as DKS_ERR_UNSUPPORTED.  dks_set_l1_tables uploads what plan.py:l1_tables computes for the shared plan of M groups (after
- * dks_set_shared_plan): Gram matrices of the augmented system [M x M], column sums / norms / b-weighted column sums [M], the
- * w-weighted Gram of the plain rows [M x M], per-row b_s and sqrt(a_s) + sqrt(b_s) [S], and three scalars. */
-int dks_set_l1(dks_ctx* ctx, int mode, int k, int others_plain);
+ * reference's pin).  Upstream decides per instance whether to select (under 'auto' from its own M); the caller makes that
+ * decision per M and passes the 128-bit set of the M that select: bit M - 1 of (sel_lo, sel_hi), M = 2..128.  Instances
+ * whose M is not in the set take the plain constrained WLS.  Those whose groups all vary select on the shared-plan path;
+ * those with a partial varying set (at most 64 groups, kernel auto or shared) on the CUDA-core kernel, which forms their
+ * moments of y, and the same LARS kernel, on the shared plan of their own M.  A selecting instance no kernel covers is
+ * reported as DKS_ERR_UNSUPPORTED, never solved without the selection.  dks_set_l1_tables uploads what plan.py:l1_tables
+ * computes for the shared plan of M <= 128 groups (after dks_set_shared_plan), for every M in the set: Gram matrices of the
+ * augmented system [M x M], column sums / norms / b-weighted column sums [M], the w-weighted Gram of the plain rows [M x M],
+ * per-row b_s and sqrt(a_s) + sqrt(b_s) [S], and three scalars. */
+int dks_set_l1(dks_ctx* ctx, int mode, int k, uint64_t sel_lo, uint64_t sel_hi);
 int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double* gram_norm, const double* colsum,
                       const double* scale, const double* bz, const double* gram_w, const double* b_rows,
                       const double* sqab_rows, double sum_b, double sum_sqb, int n_aug);
@@ -231,7 +235,9 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
                                   * (background weights not all equal) */
 #define DKS_PATH_FUSED_TABLE 11  /* fused kernel: 1 = y read from the plan's per-row link table (passes outside its domain
                                   * take the exact loop), 0 = exact loop only ("fused_table" 0, or the plan has no table) */
-#define DKS_PATH_FIELDS 12
+#define DKS_PATH_GENERAL_L1 12   /* 1: the general list's instances whose M selects ran the l1 selection (moments on the
+                                  * CUDA-core kernel, then the LARS kernel); DKS_PATH_GENERAL names the rest's kernel */
+#define DKS_PATH_FIELDS 13
 #define DKS_SHARED_NONE 0
 #define DKS_SHARED_FUSED 1       /* explain_shared_fused_kernel: link + projection solve inside */
 #define DKS_SHARED_SMEM 2        /* explain_shared_smem_kernel (Dm rows in shared memory) */
@@ -253,6 +259,9 @@ int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
 int dks_last_timings(dks_ctx* ctx, float* ms3);
+/* device-time in ms of the last explain's general-list l1 selection (DKS_PATH_GENERAL_L1): [0] the CUDA-core kernel that
+ * forms the moments, [1] the LARS kernel; an error when that call ran none (or was captured into a graph); synchronises. */
+int dks_last_general_l1_timings(dks_ctx* ctx, float* ms2);
 
 /* ---- debugging aid for the tensor-core kernel (tests only) ---------------------------------------------------
  * dks_debug_score_dump(ctx, i): the next explains also write the raw accumulator tile of instance i (scaled masked
