@@ -62,6 +62,8 @@ SIGNATURES = {
     "dks_set_plan_mode": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
     "dks_set_row_offset": (C.c_int, [C.c_void_p, C.c_int64]),
     "dks_get_instance_plans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "dks_get_instance_plans_w": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                           C.POINTER(C.c_int)]),
     "dks_prepare_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "dks_prepare_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "dks_get_m_histogram": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -14,6 +14,7 @@
 #include "dks_multi.cuh"
 #include "dks_wide.cuh"
 #include "dks_sampler.cuh"
+#include "dks_instance_wide.cuh"
 
 namespace {
 
@@ -230,24 +231,41 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     const double* ext_chol = nullptr;
     const double* ext_ainv = nullptr;
     int ext_fstride = 0;
-    if (ctx->G > 64 && (ext_z != nullptr || ctx->plan_mode == 1))
-        return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups: only shared plans are supported (no per-instance plans)");
+    if (ctx->G > 64 && ext_z != nullptr)
+        return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups: caller-supplied per-instance plans are not supported");
+    // per-instance plans of 65..128 groups (two-word rows): binary-logistic or identity head, CUDA-core kernel
+    const bool wide_pi = ctx->G > 64 && ctx->plan_mode == 1;
+    if (wide_pi) {
+        if (ctx->G > 128)
+            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans cover at most 128 groups (G=%d); use shared plans", ctx->G);
+        if (ctx->act != DKS_ACT_BINARY_LOGISTIC && ctx->act != DKS_ACT_IDENTITY)
+            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans of more than 64 groups: binary-logistic or identity head only");
+        if (ctx->kernel_choice != DKS_KERNEL_AUTO && ctx->kernel_choice != DKS_KERNEL_SIMT)
+            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans of more than 64 groups run on the CUDA-core kernel (kernel "
+                        "'auto' or 'simt')");
+        if (ctx->l1_mode != 0)
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
+    }
     if (ctx->plan_mode == 1 && ext_z == nullptr) {
         // every instance draws its own plan on the device; the explain kernels then read it like a caller-supplied one
         if (ctx->max_plan_S < 2)
             return fail(DKS_ERR_PLAN_MISSING, "per-instance plans need the shared plans of the M values present (their "
                         "enumerated prefix); none is set");
         const int stride = (ctx->max_plan_S + 1) & ~1;
+        const int W = wide_pi ? 2 : 1;                     // 64-bit words per coalition row
         const size_t need = (size_t)n * stride;
-        if (need > ctx->cap_gen) {
-            TRY(dev_alloc(&ctx->d_genz, need)); TRY(dev_alloc(&ctx->d_genw, need));
-            ctx->cap_gen = need; ctx->epoch++;
+        if (need > ctx->cap_gen || W != ctx->gen_words) {
+            TRY(dev_alloc(&ctx->d_genz, need * W)); TRY(dev_alloc(&ctx->d_genw, need));
+            ctx->cap_gen = need; ctx->gen_words = W; ctx->epoch++;
         }
         const int nAmax = ctx->G > 1 ? ctx->G - 1 : 1;
         const int fstride = nAmax * nAmax;
         const size_t needf = (size_t)n * fstride;
-        if (needf > ctx->cap_genf) {
-            TRY(dev_alloc(&ctx->d_genchol, needf)); TRY(dev_alloc(&ctx->d_genainv, needf));
+        if (needf > ctx->cap_genf || (!wide_pi && ctx->d_genainv == nullptr)) {
+            // two-word rows keep one matrix per instance (inverted in place); one-word rows its factor and its inverse
+            TRY(dev_alloc(&ctx->d_genchol, needf));
+            if (wide_pi) dev_free(&ctx->d_genainv);
+            else TRY(dev_alloc(&ctx->d_genainv, needf));
             ctx->cap_genf = needf; ctx->epoch++;
         }
         REQUIRE(ctx->d_sinfo && ctx->d_afix, "per-instance plans: dks_set_plan_sampling has not been called");
@@ -271,16 +289,25 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         sp.afix = ctx->d_afix;
         sp.out_z = ctx->d_genz; sp.out_w = ctx->d_genw; sp.out_chol = ctx->d_genchol; sp.out_ainv = ctx->d_genainv;
         sp.status = ctx->d_status;
-        const size_t ssm = dks::sampler::smem_bytes(cap, max_left, ctx->G);
+        const size_t ssm = dks::sampler::smem_bytes(cap, max_left, ctx->G, W);
         if (ssm + 2048 > (size_t)ctx->max_smem_optin)
             return fail(DKS_ERR_UNSUPPORTED, "per-instance plan sampler needs %zu B of shared memory", ssm);
-        CUDA_TRY(cudaFuncSetAttribute(dks::sampler::sample_plans_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
+        auto skern = W == 1 ? dks::sampler::sample_plans_kernel<1> : dks::sampler::sample_plans_kernel<2>;
+        CUDA_TRY(cudaFuncSetAttribute(skern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
         int per_sm = (int)((size_t)ctx->max_smem_optin / (ssm + 2048));
         if (per_sm > 6) per_sm = 6;
         if (per_sm < 1) per_sm = 1;
         const int sgrid = n < ctx->sm_count * per_sm ? n : ctx->sm_count * per_sm;
-        dks::sampler::sample_plans_kernel<<<sgrid, dks::sampler::THREADS, ssm, ctx->stream>>>(sp);
-        {
+        skern<<<sgrid, dks::sampler::THREADS, ssm, ctx->stream>>>(sp);
+        if (wide_pi) {
+            // one CTA per instance inverts its normal matrix in place
+            const size_t fsm = dks::sampler::wide_factor_smem(nAmax);
+            CUDA_TRY(cudaFuncSetAttribute(dks::sampler::factor_wide_plans_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)fsm));
+            const int fgrid = n < ctx->sm_count * 2 ? n : ctx->sm_count * 2;
+            dks::sampler::factor_wide_plans_kernel<<<fgrid, dks::sampler::WIDE_FACTOR_THREADS, fsm, ctx->stream>>>(
+                n, ctx->d_M, ctx->G, fstride, ctx->d_genchol, ctx->d_status);
+        } else {
             const size_t per_warp = (size_t)2 * nAmax * nAmax * sizeof(double);
             int fw = (int)((size_t)ctx->max_smem_optin / per_warp);
             if (fw > dks::sampler::FACTOR_WARPS) fw = dks::sampler::FACTOR_WARPS;
@@ -294,9 +321,10 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         }
         ctx->launches += 2;
         CUDA_TRY(cudaGetLastError());
-        ctx->gen_stride = stride; ctx->gen_n = n;
+        ctx->gen_stride = stride; ctx->gen_n = n; ctx->gen_plan_words = W;
         ext_z = ctx->d_genz; ext_w = ctx->d_genw; ext_stride = stride;
-        ext_chol = ctx->d_genchol; ext_ainv = ctx->d_genainv; ext_fstride = fstride;
+        ext_chol = wide_pi ? nullptr : ctx->d_genchol; ext_ainv = wide_pi ? ctx->d_genchol : ctx->d_genainv;
+        ext_fstride = fstride;
     }
     ExplainParams p;
     memset(&p, 0, sizeof(p));
@@ -604,6 +632,30 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         path[DKS_PATH_GENERAL_L1] = 1;
         p.list = ctx->d_idx_plain;
         p.count = ctx->d_l1_counts + 1;
+    }
+    if (wide_pi) {
+        // per-instance two-word plans: the instances whose groups all vary run the CUDA-core two-word kernel; a partial
+        // varying set is reported, not computed
+        p.list = ctx->d_idx_full; p.count = ctx->d_counts;
+        const size_t wsm = dks::iwide::smem_bytes(S_cap);
+        if ((long long)wsm > (long long)ctx->max_smem_optin)
+            return fail(DKS_ERR_UNSUPPORTED, "two-word per-instance kernel needs %zu B of shared memory (> %d): nsamples too "
+                        "large", wsm, ctx->max_smem_optin);
+        CUDA_TRY(cudaFuncSetAttribute(dks::iwide::explain_wide_instance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)wsm));
+        int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 1024));
+        if (per_sm < 1) per_sm = 1;
+        if (per_sm > 4) per_sm = 4;
+        int grid = ctx->sm_count * per_sm;
+        if (grid > n) grid = n;
+        dks::iwide::explain_wide_instance_kernel<<<grid, dks::iwide::THREADS, wsm, gstream>>>(p);
+        dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
+        ctx->launches += 2;
+        path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT_WIDE;
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(join());
+        CUDA_TRY(record_ev(ctx, 3));
+        return DKS_OK;
     }
     if (G > 64) {
         // two-word coalition rows exist on the shared-plan path only: anything left over is reported, not computed
@@ -1307,7 +1359,9 @@ int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double*
 int dks_set_plan_sampling(dks_ctx* ctx, int M, int nfixed, int n_full, int n_paired, int ncdf, const double* cdf_host,
                           double weight_left) {
     REQUIRE(ctx && M >= 2 && M <= DKS_MAX_GROUPS, "dks_set_plan_sampling: M out of range");
-    REQUIRE(ncdf >= 0 && ncdf <= 32 && (ncdf == 0 || cdf_host), "dks_set_plan_sampling: at most 32 sampled subset sizes");
+    REQUIRE(ncdf >= 0 && ncdf <= dks::sampler::MAX_SIZES && (ncdf == 0 || cdf_host),
+            "dks_set_plan_sampling: at most 64 sampled subset sizes");
+    if (M > 128) return fail(DKS_ERR_UNSUPPORTED, "dks_set_plan_sampling: per-instance plans cover at most 128 groups");
     REQUIRE(nfixed >= 0 && n_full >= 0 && n_paired >= 0, "dks_set_plan_sampling: bad arguments");
     DksSamplingInfo& inf = ctx->h_sinfo[M];
     memset(&inf, 0, sizeof(inf));
@@ -1320,7 +1374,8 @@ int dks_set_plan_sampling(dks_ctx* ctx, int M, int nfixed, int n_full, int n_pai
     double* af = nullptr;
     CUDA_TRY(cudaMalloc((void**)&af, sizeof(double) * (M - 1) * (M - 1)));
     ctx->plan_allocs[M].push_back(af);
-    dks::plan_prefix_normal_kernel<<<1, 256, sizeof(double) * (M - 1) * (M - 1), ctx->stream>>>(pd.z, pd.w, nfixed, M, af);
+    if (M <= 64) dks::plan_prefix_normal_kernel<<<1, 256, sizeof(double) * (M - 1) * (M - 1), ctx->stream>>>(pd.z, pd.w, nfixed, M, af);
+    else dks::plan_prefix_normal_wide_kernel<<<1, 1024, 0, ctx->stream>>>(pd.z, pd.w, nfixed, M, af);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     ctx->h_afix[M] = af;
@@ -1351,9 +1406,26 @@ int dks_get_instance_plans(dks_ctx* ctx, uint64_t* zbits_host, double* w_host, i
     BIND(ctx);
     REQUIRE(n_out && stride_out, "dks_get_instance_plans: bad arguments");
     *n_out = ctx->gen_n; *stride_out = ctx->gen_stride;
+    REQUIRE(!(zbits_host && w_host && ctx->gen_n > 0 && ctx->gen_plan_words != 1),
+            "dks_get_instance_plans: the last plans have two-word rows; use dks_get_instance_plans_w");
     if (zbits_host && w_host && ctx->gen_n > 0) {
         const size_t cnt = (size_t)ctx->gen_n * ctx->gen_stride;
         CUDA_TRY(cudaMemcpyAsync(zbits_host, ctx->d_genz, sizeof(uint64_t) * cnt, cudaMemcpyDeviceToHost, ctx->stream));
+        CUDA_TRY(cudaMemcpyAsync(w_host, ctx->d_genw, sizeof(double) * cnt, cudaMemcpyDeviceToHost, ctx->stream));
+        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    }
+    return DKS_OK;
+}
+
+int dks_get_instance_plans_w(dks_ctx* ctx, uint64_t* zbits_host, double* w_host, int* n_out, int* stride_out,
+                             int* words_out) {
+    BIND(ctx);
+    REQUIRE(n_out && stride_out && words_out, "dks_get_instance_plans_w: bad arguments");
+    *n_out = ctx->gen_n; *stride_out = ctx->gen_stride; *words_out = ctx->gen_plan_words;
+    if (zbits_host && w_host && ctx->gen_n > 0) {
+        const size_t cnt = (size_t)ctx->gen_n * ctx->gen_stride;
+        CUDA_TRY(cudaMemcpyAsync(zbits_host, ctx->d_genz, sizeof(uint64_t) * cnt * ctx->gen_plan_words,
+                                 cudaMemcpyDeviceToHost, ctx->stream));
         CUDA_TRY(cudaMemcpyAsync(w_host, ctx->d_genw, sizeof(double) * cnt, cudaMemcpyDeviceToHost, ctx->stream));
         CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     }

@@ -67,7 +67,7 @@ struct DksSamplingInfo {
     int n_paired;         // sizes whose complement has a different size
     int ncdf;             // sizes left to sample (0: the plan is fully enumerated)
     double weight_left;   // kernel mass of the sampled sizes
-    double cdf[32];       // cumulative probabilities of the sampled sizes (last = 1)
+    double cdf[64];       // cumulative probabilities of the sampled sizes (last = 1); M <= 128 has at most 63
 };
 
 // nsamples resolution of KernelExplainer.explain: 'auto' (req <= 0) = 2M + 2^11; capped at 2^M - 2 for M <= 30
@@ -185,11 +185,13 @@ struct dks_ctx {
     long long row_offset = 0;
     DksSamplingInfo h_sinfo[DKS_MAX_GROUPS + 1];
     DksSamplingInfo* d_sinfo = nullptr;
-    uint64_t* d_genz = nullptr;
+    uint64_t* d_genz = nullptr;  // [n][stride][gen_words]
     double* d_genw = nullptr;
     double* d_genchol = nullptr;
     double* d_genainv = nullptr;
     size_t cap_gen = 0, cap_genf = 0;
+    int gen_words = 1;           // words per row d_genz is laid out for
+    int gen_plan_words = 1;      // words per row of the last call's plans (dks_get_instance_plans_w)
     const double* h_afix[DKS_MAX_GROUPS + 1] = {};   // per M: normal matrix of the enumerated prefix (device pointers)
     const double** d_afix = nullptr;
     int gen_stride = 0, gen_n = 0;

@@ -459,13 +459,8 @@ __global__ void plan_factor_kernel(const uint64_t* __restrict__ z, const double*
 // ---- plans of 65..128 groups (two words per row) -----------------------------------------------------------------
 __device__ __forceinline__ bool zbit2(const uint64_t* __restrict__ row, int k) { return (row[k >> 6] >> (k & 63)) & 1ull; }
 
-// Same factorisation for two-word plans: the matrix (up to 127 x 127) lives in shared memory, the columns of the inverse
-// are solved in a global scratch buffer [nA][nA].
-__global__ void plan_factor_wide_kernel(const uint64_t* __restrict__ z, const double* __restrict__ w, int S, int M,
-                                        double* __restrict__ chol, double* __restrict__ ainv, double* __restrict__ scratch,
-                                        int* __restrict__ status) {
-    extern __shared__ double sm_d[];
-    double* A = sm_d;
+// E^T W E of the first S rows of a two-word plan, warp-per-entry (A in shared or global memory)
+__device__ inline void wls_build_normal2(const uint64_t* __restrict__ z, const double* __restrict__ w, int S, int M, double* A) {
     const int nA = M - 1, L = M - 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     const int npairs = nA * (nA + 1) / 2;
@@ -483,6 +478,17 @@ __global__ void plan_factor_wide_kernel(const uint64_t* __restrict__ z, const do
         acc = warp_sum(acc);
         if (lane == 0) { A[k * nA + l] = acc; A[l * nA + k] = acc; }
     }
+}
+
+// Same factorisation for two-word plans: the matrix (up to 127 x 127) lives in shared memory, the columns of the inverse
+// are solved in a global scratch buffer [nA][nA].
+__global__ void plan_factor_wide_kernel(const uint64_t* __restrict__ z, const double* __restrict__ w, int S, int M,
+                                        double* __restrict__ chol, double* __restrict__ ainv, double* __restrict__ scratch,
+                                        int* __restrict__ status) {
+    extern __shared__ double sm_d[];
+    double* A = sm_d;
+    const int nA = M - 1;
+    wls_build_normal2(z, w, S, M, A);
     __syncthreads();
     __shared__ int s_ok;
     if (threadIdx.x == 0) s_ok = 1;
@@ -634,6 +640,11 @@ __global__ void plan_prefix_normal_kernel(const uint64_t* __restrict__ z, const 
     wls_build_normal(z, w, rows, M, sm_d, threadIdx.x >> 5, blockDim.x >> 5);
     __syncthreads();
     for (int idx = threadIdx.x; idx < nA * nA; idx += blockDim.x) afix[idx] = sm_d[idx];
+}
+// the same for two-word plans, written straight to global memory (a 127 x 127 float64 matrix is 126 KB)
+__global__ void plan_prefix_normal_wide_kernel(const uint64_t* __restrict__ z, const double* __restrict__ w, int rows, int M,
+                                               double* __restrict__ afix) {
+    wls_build_normal2(z, w, rows, M, afix);
 }
 
 // ------------------------------------------------------------------------------------------------------

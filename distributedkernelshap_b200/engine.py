@@ -21,6 +21,36 @@ logger = logging.getLogger(__name__)
 
 MODEL_CHECK_RTOL = 1e-9
 MAX_ROWS_PER_CALL = 65536     # rows per C-ABI call: bounds the engine's per-call workspace (n x S x 8 B on the fast path)
+# per-instance plans of 65..128 groups keep, per row, the plan (S x 16 B words + S x 8 B weights) and the inverse of its
+# (M-1) x (M-1) normal matrix: about 222 KB at M = 128, S = 4096.  Row blocks of 4096 bound that workspace by ~0.9 GB.
+MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE = 4096
+MAX_SAMPLED_SIZES = 64        # subset sizes the device sampler draws from (csrc/dks_sampler.cuh, MAX_SIZES)
+
+
+def per_instance_workspace_bytes(M, S):
+    """Device workspace one row of ``plan_mode='per_instance'`` holds for a plan of S rows over M groups: the plan's
+    words and weights and one (M-1) x (M-1) float64 matrix (two of them, factor and inverse, up to 64 groups)."""
+    words = 1 if M <= 64 else 2
+    mats = 2 if M <= 64 else 1
+    return S * (8 * words + 8) + mats * 8 * (M - 1) ** 2
+
+
+def device_sampling_supported(M, n_sizes):
+    """Whether the device sampler draws the per-instance plans of M groups whose sampled part has ``n_sizes`` subset
+    sizes: up to 128 groups (one- and two-word rows) and 64 sizes (M <= 128 has at most 63)."""
+    return M <= 128 and n_sizes <= MAX_SAMPLED_SIZES
+
+
+def rows_per_call(act_code, n_outputs, plan_mode, G):
+    """Rows per C-ABI call.  The softmax and one-vs-rest heads' shared-plan path keeps C per-class sums per coalition
+    where the binary head keeps two: their row blocks are 2 / C as long, so that the per-call workspace stays the binary
+    path's.  Per-instance plans of more than 64 groups: ``MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE`` (plans are keyed by the
+    global row, so results do not depend on the block size)."""
+    if act_code in (_cabi.ACT_SOFTMAX, _cabi.ACT_OVR) and n_outputs > 2:
+        return MAX_ROWS_PER_CALL * 2 // n_outputs
+    if plan_mode == "per_instance" and G > 64:
+        return MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE
+    return MAX_ROWS_PER_CALL
 
 
 def refuse_partial_sets_beyond_64_groups(G, hist):
@@ -274,10 +304,13 @@ class GpuKernelExplainer:
                 pt, dvec = projection(plan)
                 _cabi.check(self.lib.dks_set_plan_projection(self._ctx, M, _cabi.ptr(pt), _cabi.ptr(dvec)))
             nfixed, n_full, n_paired, cdf, weight_left = sampling_info(plan)
-            if len(cdf) > 32:
+            if not device_sampling_supported(M, len(cdf)):
                 if self.plan_mode == "per_instance":
-                    raise NotImplementedError(f"per-instance device plans support at most 32 sampled subset sizes (M={M})")
+                    raise NotImplementedError(f"per-instance device plans support at most 128 groups and "
+                                              f"{MAX_SAMPLED_SIZES} sampled subset sizes (M={M})")
                 continue
+            if M > 64 and self.plan_mode != "per_instance":
+                continue                        # two-word rows are drawn per instance only
             _cabi.check(self.lib.dks_set_plan_sampling(self._ctx, M, nfixed, n_full, n_paired, len(cdf),
                                                        _cabi.ptr(cdf) if len(cdf) else None, weight_left))
 
@@ -394,12 +427,8 @@ class GpuKernelExplainer:
         return [phi[c] for c in range(self.D)]
 
     def _rows_per_call(self):
-        """Rows per C-ABI call.  The softmax and one-vs-rest heads' shared-plan path keeps C per-class sums per coalition
-        where the binary head keeps two: their row blocks are 2 / C as long, so that the per-call workspace stays the
-        binary path's."""
-        if self.spec.act_code in (_cabi.ACT_SOFTMAX, _cabi.ACT_OVR) and self.D > 2:
-            return MAX_ROWS_PER_CALL * 2 // self.D
-        return MAX_ROWS_PER_CALL
+        """Rows per C-ABI call (``rows_per_call``)."""
+        return rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size)
 
     def link_predictions(self):
         """``link(f(x))`` of the rows of the last ``shap_values`` call, ``[n, C]`` (``[n]`` for scalar-output models):
@@ -441,13 +470,17 @@ class GpuKernelExplainer:
 
     def instance_plans(self):
         """Plans the device drew in the last ``plan_mode='per_instance'`` call: ``(zbits uint64[n, stride],
-        w float64[n, stride])`` -- rows past an instance's S are zero.  For audits and tests."""
-        n, stride = C.c_int(0), C.c_int(0)
-        _cabi.check(self.lib.dks_get_instance_plans(self._ctx, None, None, C.byref(n), C.byref(stride)))
-        zb = np.zeros((n.value, stride.value), dtype=np.uint64)
+        w float64[n, stride])`` -- rows past an instance's S are zero; beyond 64 groups the rows have two words and
+        ``zbits`` is ``uint64[n, stride, 2]`` (little-endian: bit k of the row is bit k % 64 of word k // 64).  For audits
+        and tests."""
+        n, stride, words = C.c_int(0), C.c_int(0), C.c_int(0)
+        _cabi.check(self.lib.dks_get_instance_plans_w(self._ctx, None, None, C.byref(n), C.byref(stride), C.byref(words)))
+        shape = (n.value, stride.value) if words.value <= 1 else (n.value, stride.value, words.value)
+        zb = np.zeros(shape, dtype=np.uint64)
         w = np.zeros((n.value, stride.value), dtype=np.float64)
         if n.value:
-            _cabi.check(self.lib.dks_get_instance_plans(self._ctx, _cabi.ptr(zb), _cabi.ptr(w), C.byref(n), C.byref(stride)))
+            _cabi.check(self.lib.dks_get_instance_plans_w(self._ctx, _cabi.ptr(zb), _cabi.ptr(w), C.byref(n),
+                                                          C.byref(stride), C.byref(words)))
         return zb, w
 
     def _pack_external_plans(self, plans, n, nsamples):
@@ -577,7 +610,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide"),
     }
 
     def last_path(self):
@@ -586,7 +619,7 @@ class GpuKernelExplainer:
         'smem' | 'regs' | 'softmax' | 'ovr', or 'affine' for the identity head, whose y needs no coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
-        are reported as unsupported, not computed), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
+        are reported as unsupported, not computed, or 'simt_wide': per-instance plans of 65..128 groups), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
         the weighted one), ``fused_table`` (1: the fused kernel read y from the plan's link table, passes outside its

@@ -131,13 +131,21 @@ int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double*
  * shared plan of the instance's M, the sampled rows from Philox4x32-10 keyed by `seed` with counter (draw, global row),
  * with upstream's duplicate / complement / truncation / rescaling rules.  Plans depend on the global row index only
  * (dks_set_row_offset gives the index of row 0 of the next call), never on batching or the number of GPUs.
- * dks_set_plan_sampling uploads what the sampler needs for one M (plan.py: sampling_info); cdf has ncdf <= 32 entries. */
+ * Up to 64 groups every instance draws a one-word plan; from 65 to 128 groups (two-word rows) the instances whose groups
+ * all vary do, with the binary-logistic or identity head and kernel auto or simt (DKS_GENERAL_SIMT_WIDE).  A partial varying
+ * set, another head, kernel tcgen05 / shared, l1 selection or more than 128 groups is reported as DKS_ERR_UNSUPPORTED there.
+ * dks_set_plan_sampling uploads what the sampler needs for one M <= 128 (plan.py: sampling_info); cdf has ncdf <= 64
+ * entries (M <= 128 has at most 63 sampled sizes). */
 int dks_set_plan_sampling(dks_ctx* ctx, int M, int nfixed, int n_full, int n_paired, int ncdf, const double* cdf_host,
                           double weight_left);
 int dks_set_plan_mode(dks_ctx* ctx, int mode /* 0 shared per M, 1 per instance */, uint64_t seed);
 int dks_set_row_offset(dks_ctx* ctx, int64_t offset);
-/* plans of the last mode-1 explain call ([n][stride] each; pass NULL buffers to query n and stride); tests / audit. */
+/* plans of the last mode-1 explain call ([n][stride] each; pass NULL buffers to query n and stride); tests / audit.
+ * One-word rows only: when the last plans have two-word rows (65..128 groups) copying them is DKS_ERR_INVALID. */
 int dks_get_instance_plans(dks_ctx* ctx, uint64_t* zbits_host, double* w_host, int* n_out, int* stride_out);
+/* the same for any row width: zbits [n][stride][words], w [n][stride]; *words_out = 1 (up to 64 groups) or 2. */
+int dks_get_instance_plans_w(dks_ctx* ctx, uint64_t* zbits_host, double* w_host, int* n_out, int* stride_out,
+                             int* words_out);
 
 /* ---- explain: KernelExplainer.shap_values (reached from kernel_shap.py:250/253) ---------------------
  * Stage 1 (dks_prepare_*): per instance, grouped contributions W_g x_g, f(x), link(f(x)) - link(fnull),
@@ -255,6 +263,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_GENERAL_TC 1         /* explain_wgmma_kernel */
 #define DKS_GENERAL_SIMT 2       /* explain_simt_kernel */
 #define DKS_GENERAL_FLAGGED 3    /* not computed: instances left for it are reported as DKS_ERR_UNSUPPORTED */
+#define DKS_GENERAL_SIMT_WIDE 4  /* explain_wide_instance_kernel: per-instance plans of 65..128 groups (two-word rows) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
