@@ -26,6 +26,7 @@ ACT_IDENTITY = 0
 ACT_BINARY_LOGISTIC = 1
 ACT_SOFTMAX = 2
 ACT_OVR = 3
+ACT_EXP = 4
 LINK_IDENTITY = 0
 LINK_LOGIT = 1
 KERNEL_AUTO = 0

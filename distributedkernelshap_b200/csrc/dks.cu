@@ -133,18 +133,19 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D);
     auto kern = stage ? dks::prep_kernel<true> : dks::prep_kernel<false>;
-    // nibble tables: the binary head's scaled contributions; the softmax and one-vs-rest heads' per class (log2 e XW) and
-    // the identity head's XW - Bbar, up to 128 groups (what the shared-plan path of those heads covers)
+    // nibble tables: the binary head's scaled contributions; the softmax and one-vs-rest heads' per class (log2 e XW), the
+    // identity head's XW - Bbar and the exp head's log2 e XW, up to 128 groups (what the shared-plan path of those heads
+    // covers)
     double* xt = nullptr;
     if (ctx->act == DKS_ACT_BINARY_LOGISTIC && ctx->R == 1) xt = ctx->d_XT;
-    else if ((ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_IDENTITY) && G <= 128 &&
-             ctx->plan_mode == 0) xt = ctx->d_XT;
+    else if ((ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_IDENTITY ||
+              ctx->act == DKS_ACT_EXP) && G <= 128 && ctx->plan_mode == 0) xt = ctx->d_XT;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
         X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
         ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
         ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-        xt, ctx->scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr);
+        xt, ctx->scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr, ctx->d_status);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
@@ -161,6 +162,7 @@ dks::l1::Params l1_params(dks_ctx* ctx, int n, int nout, double* phi_dev) {
     lp.n = n; lp.N = ctx->N; lp.G = ctx->G; lp.C = ctx->C; lp.link = ctx->link;
     lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.nout = nout; lp.tabs = ctx->d_l1;
     lp.binary = ctx->act == DKS_ACT_BINARY_LOGISTIC;
+    lp.src.act = ctx->act;                           // the exp head's LARS skips tasks with non-finite moments
     lp.dlink = ctx->d_dlink; lp.linkfnull = ctx->d_linkfnull; lp.fnull = ctx->d_fnull;
     lp.mom = ctx->d_mom; lp.phi = phi_dev; lp.status = ctx->d_status;
     return lp;
@@ -233,13 +235,14 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     int ext_fstride = 0;
     if (ctx->G > 64 && ext_z != nullptr)
         return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups: caller-supplied per-instance plans are not supported");
-    // per-instance plans of 65..128 groups (two-word rows): binary-logistic or identity head, CUDA-core kernel
+    // per-instance plans of 65..128 groups (two-word rows): binary-logistic, identity or exp head, CUDA-core kernel
     const bool wide_pi = ctx->G > 64 && ctx->plan_mode == 1;
     if (wide_pi) {
         if (ctx->G > 128)
             return fail(DKS_ERR_UNSUPPORTED, "per-instance plans cover at most 128 groups (G=%d); use shared plans", ctx->G);
-        if (ctx->act != DKS_ACT_BINARY_LOGISTIC && ctx->act != DKS_ACT_IDENTITY)
-            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans of more than 64 groups: binary-logistic or identity head only");
+        if (ctx->act != DKS_ACT_BINARY_LOGISTIC && ctx->act != DKS_ACT_IDENTITY && ctx->act != DKS_ACT_EXP)
+            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans of more than 64 groups: binary-logistic, identity or exp head "
+                        "only");
         if (ctx->kernel_choice != DKS_KERNEL_AUTO && ctx->kernel_choice != DKS_KERNEL_SIMT)
             return fail(DKS_ERR_UNSUPPORTED, "per-instance plans of more than 64 groups run on the CUDA-core kernel (kernel "
                         "'auto' or 'simt')");
@@ -337,6 +340,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     p.plans = ctx->d_plans; p.ext_z = ext_z; p.ext_w = ext_w; p.ext_stride = ext_stride;
     p.ext_chol = ext_chol; p.ext_ainv = ext_ainv; p.ext_fstride = ext_fstride;
     p.phi = phi_dev; p.status = ctx->d_status;
+    const ExpBackground eb{ctx->d_BW, ctx->d_scores};
     // capacity of the per-CTA y buffer: the largest S any instance can need
     int S_cap = 0;
     if (ext_z) S_cap = ext_stride;
@@ -365,16 +369,18 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     const bool fast = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
                       ctx->act == DKS_ACT_BINARY_LOGISTIC && G >= 2 && pg.dmT != nullptr &&
                       pg.S == dks_effective_S(G, ctx->nsamples_req) && (pg.W <= 2 || pg.ptw != nullptr);
-    // softmax, one-vs-rest and identity heads, up to 128 groups: per-class sums of the class-sum coalition kernels
-    // (dks_multi.cuh) or the identity head's tables, then a solve per (instance, output)
-    const bool sfm = ctx->act == DKS_ACT_SOFTMAX, ovr = ctx->act == DKS_ACT_OVR;
+    // softmax, one-vs-rest, identity and exp heads, up to 128 groups: per-class sums of the class-sum coalition kernels
+    // (dks_multi.cuh) or the identity / exp head's tables, then a solve per (instance, output)
+    const bool sfm = ctx->act == DKS_ACT_SOFTMAX, ovr = ctx->act == DKS_ACT_OVR, expo = ctx->act == DKS_ACT_EXP;
     const bool mc = sfm || ovr;          // heads with per-class sums
+    const bool tabled = ctx->act == DKS_ACT_IDENTITY || expo;     // heads whose y comes from the instance's tables alone
     const bool multi = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
-                       (mc || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128 && ctx->plan_mode == 0 &&
-                       pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) && (!mc || ctx->h_smx[G].dm != nullptr);
+                       (mc || tabled) && G >= 2 && G <= 128 && ctx->plan_mode == 0 &&
+                       pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) && (!mc || ctx->h_smx[G].dm != nullptr) &&
+                       (!expo || ctx->h_expl[G] != nullptr);
     if (kernel == DKS_KERNEL_SHARED && !fast && !multi && ext_z == nullptr && pg.z != nullptr)
         return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head, or the softmax / one-vs-rest / "
-                    "identity head with at most 128 groups");
+                    "identity / exp head with at most 128 groups");
     // l1 feature selection: on the shared-plan path when M = G selects, and on the general list (CUDA-core kernel for the
     // moments, then l1_lars_kernel) for the instances with a partial varying set whose M selects
     const bool l1 = ctx->l1_mode != 0;
@@ -385,7 +391,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     int l1_Mmax = 0;                     // largest M < G that selects
     for (int M = 2; M < G && M <= DKS_L1_MAX_GROUPS; ++M) if (selects(M)) l1_Mmax = M;
     const bool l1_gen = l1_Mmax > 0;
-    const int l1_nout = (mc || ctx->act == DKS_ACT_IDENTITY) ? ctx->C : 1;
+    const int l1_nout = (mc || tabled) ? ctx->C : 1;
     size_t l1_smem = 0;
     ctx->l1_timing_valid = false;
     if (l1) {
@@ -395,7 +401,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
         if (l1_full && (!(fast || multi) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S))
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax, "
-                        "one-vs-rest or identity head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
+                        "one-vs-rest, identity or exp head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
         if (l1_gen) {
             if (G > 64)
                 return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection for partial varying sets covers at most 64 groups (G=%d)", G);
@@ -498,7 +504,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = ctx->C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link;
         wp.uniform_w = 1; wp.sums = ctx->d_sums; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink;
         wp.linkfnull = ctx->d_linkfnull; wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts;
-        wp.phi = phi_dev;
+        wp.phi = phi_dev; wp.status = ctx->d_status;
         if (l1_full) {
             TRY(launch_l1(ctx, pg, n, 1, dks::shared_path::HeadSource{}, phi_dev));
             path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
@@ -549,7 +555,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     } else if (multi) {
         const int S = pg.S, S_pad = pg.S_pad, C = ctx->C;
         dks::shared_path::HeadSource src;
-        src.act = ctx->act; src.ntab = (G + 3) / 4; src.msums = nullptr; src.XT = ctx->d_XT;
+        src.act = ctx->act; src.ntab = (G + 3) / 4; src.msums = nullptr; src.XT = ctx->d_XT; src.ell = ctx->h_expl[G];
         if (mc) {
             // the workspace is C n S_pad floats: the engine explains these heads in row blocks of 2 / C the binary path's
             const size_t need = (size_t)n * C * S_pad;
@@ -570,7 +576,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             path[DKS_PATH_WARPS] = dks::multi::MC_WARPS; path[DKS_PATH_GRID] = grid;
             src.msums = ctx->d_msums;
         } else {
-            path[DKS_PATH_SHARED] = DKS_SHARED_AFFINE;       // y straight from the tables: no coalition kernel
+            // y straight from the tables (and the plan's l(s) for the exp head): no coalition kernel
+            path[DKS_PATH_SHARED] = expo ? DKS_SHARED_EXP : DKS_SHARED_AFFINE;
         }
         if (l1_full) {
             TRY(launch_l1(ctx, pg, n, C, src, phi_dev));
@@ -582,6 +589,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link; wp.uniform_w = 1;
             wp.src = src; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink; wp.linkfnull = ctx->d_linkfnull;
             wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts; wp.phi = phi_dev;
+            wp.status = ctx->d_status;
             const size_t wsm = dks::shared_path::wls_shared_smem(G);
             int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 24 * 1024));
             if (per_sm > 4) per_sm = 4;
@@ -612,7 +620,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
                                                                  ctx->d_idx_sel, ctx->d_idx_plain, ctx->d_l1_counts);
         ExplainParams ps = p;
         ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
-        CUDA_TRY(cudaFuncSetAttribute(dks::explain_simt_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l1_smem));
+        auto l1kern = expo ? dks::explain_simt_kernel<true, true> : dks::explain_simt_kernel<true>;
+        CUDA_TRY(cudaFuncSetAttribute(l1kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l1_smem));
         int per_sm = (int)((size_t)ctx->max_smem_optin / (l1_smem + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 8) per_sm = 8;
@@ -620,7 +629,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if (grid > n) grid = n;
         const bool timed = !ctx->capturing;
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
-        dks::explain_simt_kernel<true><<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom});
+        l1kern<<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom}, eb);
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[1], gstream));
         dks::l1::Params lp = l1_params(ctx, n, l1_nout, phi_dev);
         lp.Mmax = l1_Mmax; lp.Mcnt = ctx->d_M; lp.vmask = ctx->d_vmask; lp.list = ctx->d_idx_sel; lp.count = ctx->d_l1_counts;
@@ -641,14 +650,14 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if ((long long)wsm > (long long)ctx->max_smem_optin)
             return fail(DKS_ERR_UNSUPPORTED, "two-word per-instance kernel needs %zu B of shared memory (> %d): nsamples too "
                         "large", wsm, ctx->max_smem_optin);
-        CUDA_TRY(cudaFuncSetAttribute(dks::iwide::explain_wide_instance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)wsm));
+        auto wkern = expo ? dks::iwide::explain_wide_instance_kernel<true> : dks::iwide::explain_wide_instance_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(wkern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
         int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 4) per_sm = 4;
         int grid = ctx->sm_count * per_sm;
         if (grid > n) grid = n;
-        dks::iwide::explain_wide_instance_kernel<<<grid, dks::iwide::THREADS, wsm, gstream>>>(p);
+        wkern<<<grid, dks::iwide::THREADS, wsm, gstream>>>(p, eb);
         dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 2;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT_WIDE;
@@ -665,8 +674,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         }
         if (!fast && !multi)
             return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, or the "
-                        "softmax / one-vs-rest / identity head up to 128 groups; kernel 'auto' or 'shared', shared plan of "
-                        "M=%d uploaded)", G);
+                        "softmax / one-vs-rest / identity head up to 128 groups, or the exp head up to 128 groups; kernel "
+                        "'auto' or 'shared', shared plan of M=%d uploaded)", G);
         dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 1;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
@@ -698,22 +707,23 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         }
         if ((long long)smem > (long long)ctx->max_smem_optin && !multi && pg.z == nullptr &&
             (kernel_req == DKS_KERNEL_AUTO || kernel_req == DKS_KERNEL_SHARED) && ext_z == nullptr && ctx->plan_mode == 0 &&
-            (mc || ctx->act == DKS_ACT_IDENTITY) && G >= 2 && G <= 128) {
-            // the softmax / one-vs-rest / identity head's shared-plan path takes these instances once the plan of G groups
-            // is uploaded
+            (mc || tabled) && G >= 2 && G <= 128) {
+            // the softmax / one-vs-rest / identity / exp head's shared-plan path takes these instances once the plan of G
+            // groups is uploaded
             ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
             return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
         }
         if ((long long)smem > (long long)ctx->max_smem_optin)
             return fail(DKS_ERR_UNSUPPORTED, "SIMT kernel needs %zu B of shared memory (> %d): N*G or nsamples too large",
                         smem, ctx->max_smem_optin);
-        CUDA_TRY(cudaFuncSetAttribute(dks::explain_simt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        auto skern = expo ? dks::explain_simt_kernel<false, true> : dks::explain_simt_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(skern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int per_sm = (int)((size_t)ctx->max_smem_optin / (smem + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 8) per_sm = 8;
         int grid = ctx->sm_count * per_sm;
         if (grid > n) grid = n;
-        dks::explain_simt_kernel<false><<<grid, 256, smem, gstream>>>(p, dks::SimtL1{});
+        skern<<<grid, 256, smem, gstream>>>(p, dks::SimtL1{}, eb);
         ctx->launches += 1;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT;
     }
@@ -729,7 +739,8 @@ int check_status(dks_ctx* ctx) {
     if (ctx->h_status[0] == DKS_ERR_PLAN_MISSING)
         return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", ctx->h_status[1]);
     if (ctx->h_status[0] == DKS_ERR_NUMERIC)
-        return fail(DKS_ERR_NUMERIC, "normal matrix not positive definite (instance/M %d)", ctx->h_status[1]);
+        return fail(DKS_ERR_NUMERIC, "normal matrix not positive definite, or (exp head) a model output that is not finite "
+                    "(instance/M %d)", ctx->h_status[1]);
     return fail(ctx->h_status[0], "explain kernel reported status %d (detail %d)", ctx->h_status[0], ctx->h_status[1]);
 }
 
@@ -981,6 +992,9 @@ int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int 
         REQUIRE(R >= 3, "one-vs-rest head needs at least three score rows (got %d)", R);
         REQUIRE(kappa == 1.0, "one-vs-rest head needs kappa == 1 (got %g)", kappa);
         ctx->C = R;
+    } else if (activation == DKS_ACT_EXP) {
+        REQUIRE(R == 1, "exp head needs R == 1 (got %d)", R);
+        ctx->C = 1;
     } else {
         return fail(DKS_ERR_INVALID, "dks_set_model: unknown activation %d", activation);
     }
@@ -1013,6 +1027,9 @@ int dks_fit(dks_ctx* ctx) {
         for (int c = 0; c < D; ++c) ctx->h_gcols[c] = c;
     }
     const int G = ctx->G;
+    if (ctx->act == DKS_ACT_EXP && ctx->link == DKS_LINK_LOGIT)
+        return fail(DKS_ERR_UNSUPPORTED, "exp head: the logit link is undefined wherever a predicted mean exceeds 1; use the "
+                    "identity link");
     {   // every column in exactly one group
         std::vector<int> seen(D, 0);
         REQUIRE((int)ctx->h_gcols.size() == D, "groups cover %d columns but the data has %d", (int)ctx->h_gcols.size(), D);
@@ -1054,7 +1071,7 @@ int dks_fit(dks_ctx* ctx) {
     CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
 
     ctx->scale = (ctx->act == DKS_ACT_BINARY_LOGISTIC) ? -ctx->kappa * 1.4426950408889634
-               : (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR) ? 1.4426950408889634 : 1.0;
+               : (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_EXP) ? 1.4426950408889634 : 1.0;
     dks::fit_bw_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D,
                                                                            G, R, ctx->d_BW);
     dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
@@ -1062,7 +1079,8 @@ int dks_fit(dks_ctx* ctx) {
     dks::fit_fnull_kernel<<<1, 256, 0, st>>>(ctx->d_scores, ctx->d_BW, ctx->d_wbg, N, G, R, C, ctx->act, ctx->kappa,
                                               ctx->link, ctx->d_fnull, ctx->d_linkfnull, ctx->d_Bbar);
     dks::fit_scale_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, G, R,
-                                                                              ctx->scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf);
+                                                                              ctx->scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf,
+                                                                              ctx->act == DKS_ACT_EXP ? 1 : 0);
     ctx->launches += 5;
     CUDA_TRY(cudaGetLastError());
     ctx->h_fnull.resize(C);
@@ -1070,6 +1088,9 @@ int dks_fit(dks_ctx* ctx) {
     CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
+    if (ctx->act == DKS_ACT_EXP && !std::isfinite(ctx->h_fnull[0]))
+        return fail(DKS_ERR_NUMERIC, "exp head: the background's predictions are not all finite in float64 (fnull = %g)",
+                    ctx->h_fnull[0]);
     ctx->cap_n = 0;  // workspace shapes depend on G, R, C
     ctx->prepared = false;
     if (any_plan_allocs(ctx)) {   // plans carry tables derived from the background/model: drop them
@@ -1077,6 +1098,7 @@ int dks_fit(dks_ctx* ctx) {
         memset(ctx->h_plans, 0, sizeof(ctx->h_plans));
         memset(ctx->h_l1, 0, sizeof(ctx->h_l1));
         memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
+        memset(ctx->h_expl, 0, sizeof(ctx->h_expl));
         ctx->max_plan_S = 0;
         CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));
         TRY(sync_l1_tables(ctx));
@@ -1146,6 +1168,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
         memset(&ctx->h_plans[M], 0, sizeof(PlanDev));
         memset(&ctx->h_l1[M], 0, sizeof(ctx->h_l1[M]));
         memset(&ctx->h_smx[M], 0, sizeof(ctx->h_smx[M]));
+        ctx->h_expl[M] = nullptr;
         ctx->h_afix[M] = nullptr;
         ctx->epoch++;
         TRY(sync_l1_tables(ctx));
@@ -1254,6 +1277,18 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
         CUDA_TRY(cudaGetLastError());
         ctx->h_smx[M].dm = sd; ctx->h_smx[M].lo = sl;
     }
+    if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_EXP && W <= 2) {
+        // exp head: l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) for the full varying set (head_y, dks_shared.cuh)
+        double* el = nullptr;
+        CUDA_TRY(cudaMalloc((void**)&el, sizeof(double) * (size_t)pd.S_pad));
+        ctx->plan_allocs[M].push_back(el);
+        auto kern = W == 1 ? dks::shared_path::plan_exp_kernel<1> : dks::shared_path::plan_exp_kernel<2>;
+        kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW, ctx->d_scores, ctx->d_wbg, ctx->N, M,
+                                                          ctx->scale, el);
+        ctx->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+        ctx->h_expl[M] = el;
+    }
     ctx->h_plans[M] = pd;
     ctx->epoch++;
     ctx->h_afix[M] = nullptr;                       // sampling info of a replaced plan is stale
@@ -1272,6 +1307,7 @@ int dks_clear_plans(dks_ctx* ctx) {
     memset(ctx->h_plans, 0, sizeof(ctx->h_plans));
     memset(ctx->h_l1, 0, sizeof(ctx->h_l1));
     memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
+    memset(ctx->h_expl, 0, sizeof(ctx->h_expl));
     memset(ctx->h_afix, 0, sizeof(ctx->h_afix));
     memset(ctx->h_sinfo, 0, sizeof(ctx->h_sinfo));
     ctx->max_plan_S = 0;

@@ -111,6 +111,18 @@ struct ExplainParams {
     const int* count;     // ... and how many (device memory)
 };
 
+// float64 background of the exp head's rows outside the range rule (a kernel parameter of its own: ExplainParams is
+// embedded in other kernels' parameter blocks, whose layout stays as it is)
+struct ExpBackground {
+    const double* BW;     // [N][G] grouped background contributions
+    const double* scores; // [N]    background scores
+};
+
+// exp head, CUDA-core kernels (DESIGN.md §5.0.8): a coalition row is summed in fp32 when the largest weighted background
+// exponent t'_j = log2 e d(s, j) + log2 w_j lies in [EXP_T_LO, EXP_T_HI]; other rows are evaluated in float64
+#define DKS_EXP_T_LO -60.f
+#define DKS_EXP_T_HI 100.f
+
 // number of instances a general kernel launch handles and the q-th of them
 __device__ __forceinline__ int dks_inst_count(const ExplainParams& p) { return p.list ? *p.count : p.n; }
 __device__ __forceinline__ int dks_inst_at(const ExplainParams& p, int q) { return p.list ? p.list[q] : q; }
@@ -170,6 +182,9 @@ struct dks_ctx {
     // element, hi per row) and Dm relative to nd; owned by plan_allocs[M], cleared with the plan
     struct SmxDev { const float* dm; const float* lo; };
     SmxDev h_smx[DKS_MAX_GROUPS + 1] = {};
+    // exp head, full varying set (M == G <= 128): l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) per row [S_pad] (plan_exp_kernel);
+    // owned by plan_allocs[M], cleared with the plan
+    const double* h_expl[DKS_MAX_GROUPS + 1] = {};
     double* d_mom = nullptr;     // [n][outputs solved][2G + 4] per-instance moments of y
     size_t cap_mom = 0;
     double* d_yw = nullptr;      // [n][S_pad] link-space y of the wide (more than 128 groups) solve

@@ -1,5 +1,5 @@
 // CUDA-core coalition kernel for per-instance plans of 65..128 groups (two 64-bit words per coalition row), for the
-// instances whose groups all vary (M = G, so varying position k is group k).  Binary-logistic and identity heads.
+// instances whose groups all vary (M = G, so varying position k is group k).  Binary-logistic, identity and exp heads.
 //
 // One CTA per instance (grid-stride over the instance list).  Binary head: the background is streamed in chunks of NC
 // rows; for each chunk the CTA builds nibble tables T[j][t][x] = sum_{b in x} BWs[4t + b][j] (scaled grouped background
@@ -74,7 +74,9 @@ __device__ inline void solve_write(const double* __restrict__ ainv, const double
     }
 }
 
-__global__ void __launch_bounds__(THREADS, 2) explain_wide_instance_kernel(ExplainParams p) {
+// EXP: the instantiation of the exp head, which compiles its branch only (the other heads' instantiation is unchanged)
+template <bool EXP = false>
+__global__ void __launch_bounds__(THREADS, 2) explain_wide_instance_kernel(ExplainParams p, ExpBackground eb) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double* ys = reinterpret_cast<double*>(smem_raw);                // [S_cap]
     float2* acc = reinterpret_cast<float2*>(ys);                      // [S_cap] (sum p1, sum p0): same bytes as ys[s]
@@ -107,7 +109,69 @@ __global__ void __launch_bounds__(THREADS, 2) explain_wide_instance_kernel(Expla
         const double* wp = p.ext_w + (size_t)i * p.ext_stride;
         const double* ainv = p.ext_ainv + (size_t)i * p.ext_fstride;
 
-        if (p.act == DKS_ACT_BINARY_LOGISTIC) {
+        if constexpr (EXP) {
+            // exp head (DESIGN.md §5.0.8): the binary head's chunk tables give the background part; per row acc[s] carries
+            // (sum_j 2^t'_j, max_j t'_j) across chunks, t'_j = bases_j - c (bases carry log2 w_j), and afs[s] is unused.
+            // ey = 2^a(s) sum with the instance part a(s) in float64; rows outside the range rule take exp_row_f64.
+            if (tid < M) xw[tid] = p.scale * p.XW[(size_t)i * G + tid];
+            for (int s = tid; s < S; s += THREADS) acc[s] = make_float2(0.f, -INFINITY);
+            const int tbase = (int)(reinterpret_cast<unsigned char*>(T) - smem_raw);
+            for (int j0 = 0; j0 < N; j0 += NC) {
+                const int nc = min(NC, N - j0);
+                __syncthreads();  // the previous chunk's tables are no longer read
+                // rows past the end of the background: zero tables and base -inf, so 2^t' = 0 and the maximum is unchanged
+                for (int idx = tid; idx < NC * NT * 16; idx += THREADS) {
+                    const int jj = idx / (NT * 16), t = (idx >> 4) & (NT - 1), x = idx & 15;
+                    float v = 0.f;
+#pragma unroll
+                    for (int b = 0; b < 4; ++b)
+                        if (jj < nc && ((x >> b) & 1) && 4 * t + b < M) v += p.BWs[(size_t)(4 * t + b) * N + j0 + jj];
+                    T[idx] = v;
+                }
+                if (tid < NC) bch[tid] = tid < nc ? p.bases[j0 + tid] : -INFINITY;
+                __syncthreads();
+                for (int s = tid; s < S; s += THREADS) {
+                    const uint64_t z0 = zp[2 * s], z1 = zp[2 * s + 1];
+                    int off[NT];
+#pragma unroll
+                    for (int t = 0; t < NT; ++t)
+                        off[t] = tbase + 4 * (t * 16 + (int)(((t < 16 ? z0 : z1) >> (4 * (t & 15))) & 15ull));
+                    float2 a2 = acc[s];
+                    float sum = a2.x, thi = a2.y;
+#pragma unroll
+                    for (int jj = 0; jj < NC; ++jj) {
+                        float c4[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+                        for (int t = 0; t < NT; ++t)
+                            c4[t & 3] += *reinterpret_cast<const float*>(smem_raw + off[t] + jj * (NT * 16 * 4));
+                        const float tt = bch[jj] - ((c4[0] + c4[1]) + (c4[2] + c4[3]));
+                        thi = fmaxf(thi, tt);
+                        sum += ex2_approx(tt);
+                    }
+                    acc[s] = make_float2(sum, thi);
+                }
+            }
+            __syncthreads();
+            const double fn = p.fnull[0], delta = p.dlink[i];
+            int bad = !isfinite(delta);
+            for (int s = tid; s < S; s += THREADS) {
+                const uint64_t z0 = zp[2 * s], z1 = zp[2 * s + 1];
+                double a = 0;
+                for (int k = 0; k < M; ++k) if (((k < 64 ? z0 : z1) >> (k & 63)) & 1ull) a += xw[k];
+                const float2 a2 = acc[s];
+                const double y = exp_row_ey(p, eb, i, a, a2.x, a2.y, z0, z1, M, nullptr) - fn;
+                bad |= !isfinite(y);
+                ys[s] = y;             // the same bytes as acc[s], read above by this thread only
+            }
+            if (__syncthreads_or(bad)) {
+                // a non-finite ey (or f(x)) is reported, never solved
+                if (tid == 0 && atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
+                continue;
+            }
+            build_rhs2(zp, wp, ys, S, M, delta, rhs);
+            __syncthreads();
+            solve_write(ainv, rhs, beta, M, delta, p.phi + (size_t)i * G, nullptr);
+        } else if (p.act == DKS_ACT_BINARY_LOGISTIC) {
             if (tid < M) xw[tid] = p.scale * p.XW[(size_t)i * G + tid];
             __syncthreads();
             for (int s = tid; s < S; s += THREADS) {

@@ -84,6 +84,8 @@ __device__ inline void head_f64(const double* z, int R, int act, double kappa, d
         double sum = 0;
         for (int r = 0; r < R; ++r) { out[r] = exp(out[r] - m); sum += out[r]; }
         for (int r = 0; r < R; ++r) out[r] /= sum;
+    } else if (act == DKS_ACT_EXP) {
+        out[0] = exp(z[0]);          // log-link GLM: predict = exp(z)
     } else {
         for (int r = 0; r < R; ++r) out[r] = z[r];
     }
@@ -155,9 +157,10 @@ __global__ void fit_fnull_kernel(const double* __restrict__ scores, const double
 }
 
 // scaled float copies consumed by the fused kernel: BWs[r][g][j] = scale*BW[j][g][r], bases[r][j] = scale*score
+// (fold_w, the exp head: bases[j] = scale*score + log2 w_j, so that 2^t carries the weight and a zero weight gives 2^-inf = 0)
 __global__ void fit_scale_kernel(const double* __restrict__ BW, const double* __restrict__ scores,
                                  const double* __restrict__ wbg, int N, int G, int R, double scale,
-                                 float* __restrict__ BWs, float* __restrict__ bases, float* __restrict__ wbf) {
+                                 float* __restrict__ BWs, float* __restrict__ bases, float* __restrict__ wbf, int fold_w) {
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx < N * G * R) {
         int j = idx % N, g = (idx / N) % G, r = idx / (N * G);
@@ -165,7 +168,8 @@ __global__ void fit_scale_kernel(const double* __restrict__ BW, const double* __
     }
     if (idx < N * R) {
         int j = idx % N, r = idx / N;
-        bases[idx] = (float)(scale * scores[(size_t)j * R + r]);
+        const double v = scale * scores[(size_t)j * R + r];
+        bases[idx] = (float)(fold_w ? v + log2(wbg[j]) : v);
     }
     if (idx < N) wbf[idx] = (float)wbg[idx];
 }
@@ -218,7 +222,8 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
                             double kappa, int link, int ipb, double* __restrict__ XW, uint64_t* __restrict__ vmask,
                             int* __restrict__ Mcnt, double* __restrict__ dlink, int* __restrict__ hist,
                             int* __restrict__ counts, int* __restrict__ idx_full, int* __restrict__ idx_other,
-                            double* __restrict__ XT, double xt_scale, const double* __restrict__ xt_sub) {
+                            double* __restrict__ XT, double xt_scale, const double* __restrict__ xt_sub,
+                            int* __restrict__ status) {
     extern __shared__ __align__(16) unsigned char prep_smem[];
     double* sXW = reinterpret_cast<double*>(prep_smem);                        // [ipb][G][R]
     double* sX = sXW + (size_t)ipb * G * R;                                    // STAGE: [ipb][D]
@@ -307,6 +312,8 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
         else idx_other[atomicAdd(&counts[1], 1)] = i;
         head_f64(z, R, act, kappa, o);
         for (int c = 0; c < C; ++c) dlink[(size_t)i * C + c] = link_f(o[c], link) - linkfnull[c];
+        // exp head: f(x) = exp(z) overflows for z > 709.78; the explain kernels then never write this instance's phi
+        if (act == DKS_ACT_EXP && !isfinite(o[0]) && atomicCAS(&status[0], 0, DKS_ERR_NUMERIC) == 0) status[1] = i;
     }
 }
 inline size_t prep_smem_bytes(bool stage, int ipb, int G, int R, int D) {
@@ -692,8 +699,45 @@ struct SimtL1 {
     double* mom;             // [n][outputs][2G + 4]
 };
 
-template <bool L1>
-__global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, SimtL1 q) {
+// exp head: ey(s) of one coalition row in float64, for the rows outside the fp32 range rule (DKS_EXP_T_LO / _HI):
+// exp(a + m + ln sum_j w_j e^(d_j - m)) with a = sum_{k in s} XW_i[k], d_j = score_j - sum_{k in s} BW[j][k] and m the
+// running maximum of d_j (one pass, the sum rescaled when m grows), zero-weight rows skipped.  Row bit k (k < M) is
+// varying position k, group vi[k] (vi NULL: group k); z1 holds bits 64..127.
+__device__ inline double exp_row_f64(const ExplainParams& p, const ExpBackground& eb, int i, uint64_t z0, uint64_t z1, int M,
+                                     const int* vi) {
+    const int G = p.G;
+    double a = 0.0;
+    for (int k = 0; k < M; ++k)
+        if (((k < 64 ? z0 : z1) >> (k & 63)) & 1ull) a += p.XW[(size_t)i * G + (vi ? vi[k] : k)];
+    double m = -INFINITY, e = 0.0;
+    for (int j = 0; j < p.N; ++j) {
+        const double wj = p.wbg[j];
+        if (!(wj > 0.0)) continue;
+        double c = 0.0;
+        for (int k = 0; k < M; ++k)
+            if (((k < 64 ? z0 : z1) >> (k & 63)) & 1ull) c += eb.BW[(size_t)j * G + (vi ? vi[k] : k)];
+        const double d = eb.scores[j] - c;
+        if (d > m) { e = e * exp(m - d) + wj; m = d; }
+        else e += wj * exp(d - m);
+    }
+    return exp(a + m + log(e));
+}
+
+// exp head: ey(s) from the fp32 sum of 2^t'_j (t'_j = log2 e d(s, j) + log2 w_j: bases carry log2 w_j) and its largest
+// exponent thi, times 2^a with a = log2 e sum_{k in s} XW_i[k] in float64.  Inside the range rule no term overflows and a
+// term that flushes to zero is below 2^-26 of the sum; other rows, and products that overflow, take exp_row_f64.
+__device__ __forceinline__ double exp_row_ey(const ExplainParams& p, const ExpBackground& eb, int i, double a, float sum,
+                                             float thi, uint64_t z0, uint64_t z1, int M, const int* vi) {
+    if (thi >= DKS_EXP_T_LO && thi <= DKS_EXP_T_HI) {
+        const double ey = exp2(a) * (double)sum;
+        if (isfinite(ey)) return ey;
+    }
+    return exp_row_f64(p, eb, i, z0, z1, M, vi);
+}
+
+// EXP: the instantiation of the exp head, which compiles its branch only (the other heads' instantiations are unchanged)
+template <bool L1, bool EXP = false>
+__global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, SimtL1 q, ExpBackground eb) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const bool ovr = p.act == DKS_ACT_OVR;
     const bool softmax = p.act == DKS_ACT_SOFTMAX || ovr;     // C score rows and C y buffers
@@ -715,7 +759,8 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
         for (int idx = tid; idx < C * G; idx += blockDim.x) p.phi[(size_t)(idx / G) * slab + (size_t)i * G + idx % G] = 0.0;
         if (M == 0) continue;
         if (M == 1) {
-            if (tid < C) {
+            // (exp head: a non-finite f(x) was reported by prep_kernel and is not written)
+            if (tid < C && (!EXP || isfinite(p.dlink[(size_t)i * C + tid]))) {
                 int g = __ffsll((long long)vm) - 1;
                 p.phi[(size_t)tid * slab + (size_t)i * G + g] = p.dlink[(size_t)i * C + tid];
             }
@@ -752,7 +797,61 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
         float* bases = Bs + (size_t)M * N;
         float* wb = bases + N;
 
-        if (p.act == DKS_ACT_BINARY_LOGISTIC) {
+        if constexpr (EXP) {
+            // ---- exp head (DESIGN.md §5.0.8): ey(s) = 2^a(s) sum_j 2^t'_j, the instance part a(s) factored out in float64,
+            // the background part t'_j = bases_j - sum_k z_sk BWs[k][j] summed in fp32; scale = log2(e) ----
+            for (int idx = tid; idx < M * N; idx += blockDim.x) {
+                int k = idx / N, j = idx - k * N;
+                Bs[idx] = p.BWs[(size_t)sm.vi[k] * N + j];
+            }
+            for (int j = tid; j < N; j += blockDim.x) bases[j] = p.bases[j];
+            if (tid < M) sm.xw[tid] = p.scale * p.XW[(size_t)i * G + sm.vi[tid]];
+            __syncthreads();
+            const double fn = p.fnull[0], delta = p.dlink[i];
+            int bad = !isfinite(delta);
+            for (int s = tid; s < S; s += blockDim.x) {
+                const uint64_t z = zp[s];
+                double a = 0;
+                for (int k = 0; k < M; ++k) if ((z >> k) & 1ull) a += sm.xw[k];
+                float sum = 0.f, thi = -INFINITY;
+                for (int j = 0; j < N; ++j) {
+                    float c = 0.f;
+                    for (int k = 0; k < M; ++k) if ((z >> k) & 1ull) c += Bs[k * N + j];
+                    const float t = bases[j] - c;
+                    thi = fmaxf(thi, t);
+                    sum += ex2_approx(t);
+                }
+                const double y = exp_row_ey(p, eb, i, a, sum, thi, z, 0ull, M, sm.vi) - fn;
+                bad |= !isfinite(y);
+                sm.ys[s] = y;
+            }
+            if (__syncthreads_or(bad)) {
+                // a non-finite ey (or f(x)) is reported, never solved: nothing of this instance reaches phi or the moments
+                if (tid == 0) {
+                    if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
+                    if constexpr (L1) q.mom[(size_t)i * mstride + 2 * M] = NAN;     // l1_lars_kernel skips the task
+                }
+                continue;
+            }
+            if constexpr (L1) {
+                const l1::Tables& t = q.tabs[M];
+                l1::block_moments<1, true>(sm.ys, S, M, zp, wp, t.b, t.sqab, q.mom + (size_t)i * mstride, part, bound);
+                continue;
+            }
+            if (chol != nullptr) {
+                for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
+            } else {
+                wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
+                __syncthreads();
+                if (tid < 32) {
+                    bool ok = wls_cholesky_warp(sm.A, M - 1);
+                    if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
+                }
+            }
+            wls_build_rhs(zp, wp, sm.ys, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
+            __syncthreads();
+            if (tid == 0) wls_solve_write(sm.A, sm.rhs, M, delta, sm.vi, p.phi + (size_t)i * G, 1.0);
+        } else if (p.act == DKS_ACT_BINARY_LOGISTIC) {
             // stage this instance's varying columns of the background table
             for (int idx = tid; idx < M * N; idx += blockDim.x) {
                 int k = idx / N, j = idx - k * N;

@@ -157,8 +157,21 @@ __global__ void __launch_bounds__(MOM_THREADS) l1_moments_kernel(Params p) {
         double* mom = p.mom + ((size_t)i * nout + (MULTI ? cls : 0)) * (2 * G + 4);
         if constexpr (MULTI) {
             const double fnc = p.fnull[cls], lfc = p.linkfnull[cls];
-            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS)
-                s_y[s] = shared_path::head_y<W>(p.src, i, cls, p.C, s, p.S_pad, p.z + (size_t)s * W, p.link, inv_n, fnc, lfc);
+            int bad = 0;
+            for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
+                const double y = shared_path::head_y<W>(p.src, i, cls, p.C, s, p.S_pad, p.z + (size_t)s * W, p.link, inv_n,
+                                                        fnc, lfc);
+                bad |= !isfinite(y);
+                s_y[s] = y;
+            }
+            // exp head: a non-finite y is reported and kept out of the fixed point; NaN moments make the LARS skip the task
+            if (__syncthreads_or(p.src.act == DKS_ACT_EXP && bad)) {
+                if (threadIdx.x == 0) {
+                    if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
+                    mom[2 * G] = NAN;
+                }
+                continue;
+            }
         } else {
             for (int s = threadIdx.x; s < p.S; s += MOM_THREADS) {
                 const float2 a = sums[s];
@@ -292,6 +305,11 @@ __global__ void l1_lars_kernel(Params p, int warps_per_cta, int stage_gram) {
         const double* mom = p.mom + ((size_t)i * nout + (p.binary ? 0 : cls)) * (2 * G + 4);
         const double delta = p.dlink[(size_t)i * C + cls];
         const double T1 = mom[2 * M], Qw = mom[2 * M + 1], R = mom[2 * M + 2];
+        if (p.src.act == DKS_ACT_EXP && !isfinite(T1 + delta)) {
+            // a task the moments kernel reported (non-finite y: NaN T1) or a non-finite f(x): nothing is written to phi
+            if (lane == 0 && atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
+            continue;
+        }
         const double ybar = lasso ? (R - delta * t->sum_sqb) / nsamp : 0.0;
         const double yy = (double)M * Qw - 2.0 * delta * T1 + delta * delta * sum_b - nsamp * ybar * ybar;
         for (int v = lane; v < M; v += 32) {

@@ -683,17 +683,47 @@ inline int launch_explain_shared(SharedParams p, int words, int sm_count, int ma
 
 // Where the softmax, one-vs-rest and identity heads' y(i, c, s) comes from on the shared-plan path: the per-class sums of
 // the class-sum coalition kernels (dks_multi.cuh), or the identity head's float64 nibble tables of XW - Bbar (prep_kernel),
-// for which ey_c(s) = fnull_c + sum_k z_sk (XW_i[k][c] - Bbar[k][c]) needs no coalition kernel at all.
+// for which ey_c(s) = fnull_c + sum_k z_sk (XW_i[k][c] - Bbar[k][c]) needs no coalition kernel at all.  The exp head
+// factorises the same way (DESIGN.md §3): ey(s) = 2^(a(s) + l(s)) with a(s) from the nibble tables of log2 e XW and
+// l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) from the plan (plan_exp_kernel) -- no coalition kernel either.
 struct HeadSource {
-    int act;                 // DKS_ACT_SOFTMAX, DKS_ACT_OVR or DKS_ACT_IDENTITY
+    int act;                 // DKS_ACT_SOFTMAX, DKS_ACT_OVR, DKS_ACT_IDENTITY or DKS_ACT_EXP
     int ntab;                // nibble tables per class: ceil(G / 4)
     const float* msums;      // [n][C][S_pad] sum_j w'_j p_c(s, j), w'_j = N w_j
     const double* XT;        // [n][C][ntab][16]
+    const double* ell;       // [S_pad] exp head: l(s)
 };
+
+// exp head, plan upload (M = G): l(s) = log2 e (m + ln sum_j w_j e^(d_j - m)) in float64, d_j = score_j - sum_{k in s} BW[j][k],
+// m = max_j d_j (running, the sum rescaled when it grows), zero-weight background rows skipped.  Padding rows get 0.
+template <int W>
+__global__ void plan_exp_kernel(const uint64_t* __restrict__ z, int S, int S_pad, const double* __restrict__ BW,
+                                const double* __restrict__ scores, const double* __restrict__ wbg, int N, int G, double scale,
+                                double* __restrict__ ell) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= S_pad) return;
+    if (s >= S) { ell[s] = 0.0; return; }
+    uint64_t zz[W];
+#pragma unroll
+    for (int q = 0; q < W; ++q) zz[q] = z[(size_t)s * W + q];
+    double m = -INFINITY, e = 0.0;
+    for (int j = 0; j < N; ++j) {
+        const double wj = wbg[j];
+        if (!(wj > 0.0)) continue;
+        double c = 0.0;
+        for (int k = 0; k < G; ++k)
+            if (((W == 1 || k < 64 ? zz[0] : zz[W - 1]) >> (k & 63)) & 1ull) c += BW[(size_t)j * G + k];
+        const double d = scores[j] - c;
+        if (d > m) { e = e * exp(m - d) + wj; m = d; }
+        else e += wj * exp(d - m);
+    }
+    ell[s] = scale * (m + log(e));
+}
+
 template <int W>
 __device__ __forceinline__ double head_y(const HeadSource& h, int i, int c, int C, int s, int S_pad, const uint64_t* zrow,
                                          int link, double inv_n, double fn, double lf) {
-    if (h.act != DKS_ACT_IDENTITY) {
+    if (h.act != DKS_ACT_IDENTITY && h.act != DKS_ACT_EXP) {
         const float* ms = h.msums + (size_t)i * C * S_pad + s;
         const double e = (double)ms[(size_t)c * S_pad];
         if (link == DKS_LINK_LOGIT) {
@@ -709,6 +739,7 @@ __device__ __forceinline__ double head_y(const HeadSource& h, int i, int c, int 
         a0 += __ldg(xt + t * 16 + (int)((zrow[t >> 4] >> (4 * (t & 15))) & 15ull));
         if (t + 1 < h.ntab) a1 += __ldg(xt + (t + 1) * 16 + (int)((zrow[(t + 1) >> 4] >> (4 * ((t + 1) & 15))) & 15ull));
     }
+    if (h.act == DKS_ACT_EXP) return link_f(exp2((a0 + a1) + __ldg(h.ell + s)), link) - lf;
     return link_f(fn + (a0 + a1), link) - lf;
 }
 
@@ -736,6 +767,7 @@ struct WlsSharedParams {
     const int* list;
     const int* count;
     double* phi;             // [C][n][G]
+    int* status;             // exp head (MULTI): a task whose y or delta is not finite is reported here, not solved
 };
 
 // ---- projection form of the solve for a shared plan ----------------------------------------------------------------
@@ -940,7 +972,12 @@ __global__ void __launch_bounds__(WLS_THREADS) wls_shared_kernel(WlsSharedParams
             }
             b = warp_sum(b);
             if (lane == 0) s_bound[wib] = b;
-            __syncthreads();
+            // exp head: any non-finite y or delta makes the bound non-finite; the task is reported and skipped (the barrier
+            // is the same for every thread, so is the decision)
+            if (__syncthreads_or(p.src.act == DKS_ACT_EXP && !isfinite(b))) {
+                if (threadIdx.x == 0 && atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
+                continue;
+            }
             double tot = 0.0;
 #pragma unroll
             for (int wq = 0; wq < WLS_THREADS / 32; ++wq) tot += s_bound[wq];     // fixed order: the same e every run

@@ -149,6 +149,9 @@ class GpuKernelExplainer:
         self.link = convert_to_link(link)
         self.model_callable = model
         self.spec = extract_linear_spec(model)
+        if self.spec.activation == "exp" and str(self.link) == "logit":
+            raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
+                                      "link log(ey / (1 - ey)) is undefined wherever a predicted mean exceeds 1")
         self.data = convert_to_data(data)
         if self.data.transposed:
             raise NotImplementedError("transposed DenseData (group sizes matching axis 0) is not supported")
@@ -608,7 +611,7 @@ class GpuKernelExplainer:
         return {"prepare": float(out[0]), "coalitions": float(out[1]), "total": float(out[2])}
 
     _PATH_NAMES = {
-        "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr"),
+        "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
         "general": ("none", "tc", "simt", "flagged", "simt_wide"),
     }
@@ -616,7 +619,8 @@ class GpuKernelExplainer:
     def last_path(self):
         """Which kernels the last explain call launched (``dks_last_path``), recorded when the call was enqueued (a
         replayed CUDA graph reports the call it captured): ``shared`` (shared-plan coalition kernel: 'none' | 'fused' |
-        'smem' | 'regs' | 'softmax' | 'ovr', or 'affine' for the identity head, whose y needs no coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
+        'smem' | 'regs' | 'softmax' | 'ovr', or 'affine' for the identity head and 'exp' for the exp head, whose y needs no
+        coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
         are reported as unsupported, not computed, or 'simt_wide': per-instance plans of 65..128 groups), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``

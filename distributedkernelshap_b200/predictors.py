@@ -15,18 +15,20 @@ class LinearModelSpec:
 
     activation: 'identity' (outputs z), 'binary_logistic' (R == 1; outputs [1 - s, s], s = sigmoid(kappa z)),
     'softmax' (outputs softmax(z), R = C >= 2), 'ovr' (one-vs-rest, R = C >= 3: s_c = sigmoid(z_c), outputs
-    s_c / sum_c' s_c', scikit-learn's ``_predict_proba_lr``; kappa 1).  ``scalar_out``: the callable returns a 1-D
-    array."""
+    s_c / sum_c' s_c', scikit-learn's ``_predict_proba_lr``; kappa 1), 'exp' (R = 1: outputs exp(z), the ``predict`` of
+    scikit-learn's log-link GLM regressors).  ``scalar_out``: the callable returns a 1-D array."""
 
     def __init__(self, W, b, activation, kappa=1.0, scalar_out=False):
         self.W = np.ascontiguousarray(np.atleast_2d(np.asarray(W, dtype=np.float64)))
         self.b = np.ascontiguousarray(np.atleast_1d(np.asarray(b, dtype=np.float64)))
         if self.W.shape[0] != self.b.shape[0]:
             raise ValueError(f"W has {self.W.shape[0]} rows but b has {self.b.shape[0]} entries")
-        if activation not in ("identity", "binary_logistic", "softmax", "ovr"):
+        if activation not in ("identity", "binary_logistic", "softmax", "ovr", "exp"):
             raise ValueError(f"unknown activation {activation!r}")
         if activation == "binary_logistic" and self.W.shape[0] != 1:
             raise ValueError("binary_logistic needs a single score row")
+        if activation == "exp" and self.W.shape[0] != 1:
+            raise ValueError("the exp head needs a single score row (log-link models with several outputs are not supported)")
         if activation == "ovr" and (self.W.shape[0] < 3 or float(kappa) != 1.0):
             raise ValueError("the one-vs-rest head needs at least three score rows and kappa = 1")
         self.activation = activation
@@ -36,7 +38,7 @@ class LinearModelSpec:
     @property
     def act_code(self):
         return {"identity": _cabi.ACT_IDENTITY, "binary_logistic": _cabi.ACT_BINARY_LOGISTIC,
-                "softmax": _cabi.ACT_SOFTMAX, "ovr": _cabi.ACT_OVR}[self.activation]
+                "softmax": _cabi.ACT_SOFTMAX, "ovr": _cabi.ACT_OVR, "exp": _cabi.ACT_EXP}[self.activation]
 
     @property
     def n_outputs(self):
@@ -50,6 +52,9 @@ class LinearModelSpec:
         z = X @ self.W.T + self.b
         if self.activation == "identity":
             return z[:, 0] if self.scalar_out else z
+        if self.activation == "exp":
+            e = np.exp(z)
+            return e[:, 0] if self.scalar_out else e
         if self.activation == "binary_logistic":
             t = self.kappa * z[:, 0]
             scores = np.c_[-t / 2.0, t / 2.0]
@@ -102,7 +107,8 @@ def extract_linear_spec(predictor):
 
     Accepts: a ``LinearModelSpec``; any object/bound method whose owner offers ``dks_linear_spec()``; bound
     ``predict_proba`` / ``decision_function`` / ``predict`` of scikit-learn linear models (``coef_``/``intercept_``);
-    bound ``predict_proba`` of a single-label ``OneVsRestClassifier`` over at least three binary linear models.
+    bound ``predict_proba`` of a single-label ``OneVsRestClassifier`` over at least three binary linear models; bound
+    ``predict`` of the log-link GLM regressors (``_is_log_link_glm``), whose head is 'exp'.
     Raises ``TypeError`` for everything else."""
     if isinstance(predictor, LinearModelSpec):
         return predictor
@@ -113,8 +119,9 @@ def extract_linear_spec(predictor):
     if owner is None:
         raise TypeError("predictor must be a bound method of a linear model (e.g. clf.predict_proba) or a "
                         "LinearModelSpec: the CUDA engine cannot call an opaque Python function and has no CPU fallback")
-    if hasattr(owner, "dks_linear_spec") and method == "predict_proba":
-        return owner.dks_linear_spec()
+    if hasattr(owner, "dks_linear_spec") and (method == "predict_proba" or
+                                              (method == "predict" and not hasattr(owner, "classes_"))):
+        return owner.dks_linear_spec()     # a regressor's predict (e.g. a log-link GLM stand-in) takes the hook too
     if hasattr(owner, "estimators_") and not hasattr(owner, "coef_"):
         return _one_vs_rest_spec(owner, method)
     if not (hasattr(owner, "coef_") and hasattr(owner, "intercept_")):
@@ -133,8 +140,24 @@ def extract_linear_spec(predictor):
     if method in ("decision_function", "predict", "_decision_function"):
         if method == "predict" and hasattr(owner, "classes_"):
             raise TypeError("classifier.predict returns labels, which KernelSHAP cannot explain; pass predict_proba")
+        if method == "predict" and _is_log_link_glm(owner):
+            return LinearModelSpec(coef, intercept, "exp", scalar_out=True)
         return LinearModelSpec(coef, intercept, "identity", scalar_out=coef.shape[0] == 1)
     raise TypeError(f"unsupported predictor method {method!r}")
+
+
+def _is_log_link_glm(owner):
+    """scikit-learn's GLM regressors (0.23 and later) whose ``predict`` is ``exp(X coef_ + intercept_)``:
+    ``PoissonRegressor``, ``GammaRegressor``, and ``TweedieRegressor`` with ``link='log'``, or ``link='auto'`` and
+    ``power > 0`` (``power <= 0`` picks the identity link).  Decided from the class and its public parameters; the
+    fit-time check against the callable has the last word."""
+    names = {c.__name__ for c in type(owner).__mro__ if c.__module__.startswith("sklearn.")}
+    if names & {"PoissonRegressor", "GammaRegressor"}:
+        return True
+    if "TweedieRegressor" in names:
+        link = getattr(owner, "link", "auto")
+        return link == "log" or (link == "auto" and float(getattr(owner, "power", 0.0)) > 0)
+    return False
 
 
 def _is_ovr_rule(owner):

@@ -32,7 +32,7 @@ extern "C" {
 #define DKS_ERR_CUDA 2          /* a CUDA runtime call failed (message has the CUDA error string) */
 #define DKS_ERR_UNSUPPORTED 3   /* valid request the engine does not implement (never a silent fallback) */
 #define DKS_ERR_PLAN_MISSING 4  /* an instance needs a coalition plan for an M that was not provided */
-#define DKS_ERR_NUMERIC 5       /* normal matrix not positive definite */
+#define DKS_ERR_NUMERIC 5       /* normal matrix not positive definite; exp head: a model output that is not finite */
 
 /* model head applied to the linear scores z = W x + b   (replaces the opaque `predictor` callable,
  * benchmarks/ray_pool.py:34; sklearn LogisticRegression.predict_proba per scripts/fit_adult_model.py:27) */
@@ -43,6 +43,16 @@ extern "C" {
 #define DKS_ACT_OVR 3           /* R = C in 3..8 scores, one-vs-rest: s_c = sigmoid(z_c), outputs s_c / sum_c' s_c'
                                  * (scikit-learn's _predict_proba_lr: liblinear / multi_class='ovr' LogisticRegression,
                                  * OneVsRestClassifier over binary linear models); kappa must be 1 */
+#define DKS_ACT_EXP 4           /* R = 1 score, output exp(z): the log-link GLM regressors (scikit-learn's PoissonRegressor,
+                                 * GammaRegressor, TweedieRegressor with a log link).  Link DKS_LINK_IDENTITY only (dks_fit
+                                 * refuses the logit link: a predicted mean above 1 has no logit).  dks_fit refuses a
+                                 * background whose prediction is not finite in float64; an instance whose f(x) or whose
+                                 * ey(s) = sum_j w_j exp(z(s, j)) is not finite is reported as DKS_ERR_NUMERIC and nothing
+                                 * non-finite is written into phi.  Shared plans with every group varying (G <= 128): y(s) =
+                                 * exp(a(s) + l(s)) - fnull in float64, a(s) from the instance's nibble tables and l(s) =
+                                 * ln sum_j w_j exp(d(s, j)) computed once per plan (DKS_SHARED_EXP); the CUDA-core kernels
+                                 * sum 2^t over the background in fp32 and send rows outside their range rule to float64
+                                 * (DESIGN.md §5.0.8); no tensor-core kernel */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -77,7 +87,7 @@ int dks_set_background(dks_ctx* ctx, const double* bg_host, int N, int D, const 
  * Every column must belong to exactly one group (DenseData asserts the sizes add up to D). */
 int dks_set_groups(dks_ctx* ctx, const int32_t* group_offsets, const int32_t* group_cols, int G);
 /* linear scores z = W x + b with W [R x D] row-major, b [R]; head per DKS_ACT_*; kappa used by
- * DKS_ACT_BINARY_LOGISTIC (DKS_ACT_OVR requires kappa == 1 and R >= 3).  scalar_out != 0 marks a predictor returning a
+ * DKS_ACT_BINARY_LOGISTIC (DKS_ACT_OVR requires kappa == 1 and R >= 3, DKS_ACT_EXP R == 1).  scalar_out != 0 marks a predictor returning a
  * 1-D array (vector_out False). */
 int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int R, int activation, double kappa,
                   int scalar_out);
@@ -132,7 +142,7 @@ int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double*
  * with upstream's duplicate / complement / truncation / rescaling rules.  Plans depend on the global row index only
  * (dks_set_row_offset gives the index of row 0 of the next call), never on batching or the number of GPUs.
  * Up to 64 groups every instance draws a one-word plan; from 65 to 128 groups (two-word rows) the instances whose groups
- * all vary do, with the binary-logistic or identity head and kernel auto or simt (DKS_GENERAL_SIMT_WIDE).  A partial varying
+ * all vary do, with the binary-logistic, identity or exp head and kernel auto or simt (DKS_GENERAL_SIMT_WIDE).  A partial varying
  * set, another head, kernel tcgen05 / shared, l1 selection or more than 128 groups is reported as DKS_ERR_UNSUPPORTED there.
  * dks_set_plan_sampling uploads what the sampler needs for one M <= 128 (plan.py: sampling_info); cdf has ncdf <= 64
  * entries (M <= 128 has at most 63 sampled sizes). */
@@ -253,6 +263,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_SHARED_SOFTMAX 4     /* explain_softmax_kernel: per-class sums of the softmax head (C = R classes) */
 #define DKS_SHARED_AFFINE 5      /* identity head: y read from per-class tables, no coalition kernel */
 #define DKS_SHARED_OVR 6         /* explain_ovr_kernel: per-class sums of the one-vs-rest head (C = R classes) */
+#define DKS_SHARED_EXP 7         /* exp head: y from the instance's tables and the plan's l(s), no coalition kernel */
 #define DKS_SOLVE_NONE 0
 #define DKS_SOLVE_FUSED 1
 #define DKS_SOLVE_PMAT 2         /* wls_pmat_kernel */
