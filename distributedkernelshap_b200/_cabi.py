@@ -21,6 +21,7 @@ DKS_ERR_CUDA = 2
 DKS_ERR_UNSUPPORTED = 3
 DKS_ERR_PLAN_MISSING = 4
 DKS_ERR_NUMERIC = 5
+DKS_ERR_DOMAIN = 6
 
 ACT_IDENTITY = 0
 ACT_BINARY_LOGISTIC = 1
@@ -46,6 +47,7 @@ SIGNATURES = {
     "dks_set_background": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "dks_set_groups": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "dks_set_model": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_int]),
+    "dks_set_column_maps": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "dks_set_link": (C.c_int, [C.c_void_p, C.c_int]),
     "dks_fit": (C.c_int, [C.c_void_p]),
     "dks_num_outputs": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
@@ -119,10 +121,14 @@ def load(build_if_needed=True):
     return lib
 
 
+class DksDomainError(DksError, ValueError):
+    """A raw value a column map refuses (``DKS_ERR_DOMAIN``): where scikit-learn's pipeline raises ``ValueError``."""
+
+
 def check(rc):
     if rc != DKS_OK:
         msg = load().dks_last_error()
-        raise DksError(rc, msg.decode() if msg else "")
+        raise (DksDomainError if rc == DKS_ERR_DOMAIN else DksError)(rc, msg.decode() if msg else "")
     return rc
 
 

@@ -130,9 +130,12 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     CUDA_TRY(record_ev(ctx, 0));
     int ipb = 256 / G;
     if (ipb < 1) ipb = 1;
-    const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D) <= (size_t)96 * 1024;
-    const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D);
-    auto kern = stage ? dks::prep_kernel<true> : dks::prep_kernel<false>;
+    const bool maps = ctx->cm.hdr != nullptr;
+    const size_t maps_doubles = maps ? (size_t)ctx->cm.n_keys + ctx->cm.n_vals : 0;
+    const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D, maps_doubles) <= (size_t)96 * 1024;
+    const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D, maps_doubles);
+    auto kern = maps ? (stage ? dks::prep_kernel<true, true> : dks::prep_kernel<false, true>)
+                     : (stage ? dks::prep_kernel<true, false> : dks::prep_kernel<false, false>);
     // nibble tables: the binary head's scaled contributions; the softmax and one-vs-rest heads' per class (log2 e XW), the
     // identity head's XW - Bbar and the exp head's log2 e XW, up to 128 groups (what the shared-plan path of those heads
     // covers)
@@ -145,7 +148,7 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
         X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
         ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
         ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-        xt, ctx->scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr, ctx->d_status);
+        xt, ctx->scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
@@ -738,6 +741,9 @@ int check_status(dks_ctx* ctx) {
     if (ctx->h_status[0] == 0) return DKS_OK;
     if (ctx->h_status[0] == DKS_ERR_PLAN_MISSING)
         return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", ctx->h_status[1]);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
+        return fail(DKS_ERR_DOMAIN, "instance %d holds a raw value its column map refuses (NaN, or a category unseen at "
+                    "fit time, where the pipeline raises)", ctx->h_status[1]);
     if (ctx->h_status[0] == DKS_ERR_NUMERIC)
         return fail(DKS_ERR_NUMERIC, "normal matrix not positive definite, or (exp head) a model output that is not finite "
                     "(instance/M %d)", ctx->h_status[1]);
@@ -904,6 +910,7 @@ int dks_destroy(dks_ctx* ctx) {
     cudaDeviceSynchronize();
     if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
     dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b);
+    if (ctx->cm.hdr) { cudaFree((void*)ctx->cm.hdr); cudaFree((void*)ctx->cm.keys); cudaFree((void*)ctx->cm.vals); }
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
     dev_free(&ctx->d_fnull); dev_free(&ctx->d_linkfnull); dev_free(&ctx->d_BWs); dev_free(&ctx->d_bases);
@@ -999,9 +1006,48 @@ int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int 
         return fail(DKS_ERR_INVALID, "dks_set_model: unknown activation %d", activation);
     }
     ctx->R = R; ctx->act = activation; ctx->kappa = kappa; ctx->scalar_out = scalar_out;
+    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();   // maps belong to one model
     ctx->h_W.assign(W_host, W_host + (size_t)R * ctx->D);
     ctx->h_b.assign(b_host, b_host + R);
     ctx->fitted = false;
+    return DKS_OK;
+}
+
+int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
+                        const double* vals_host, int n_vals) {
+    BIND(ctx);
+    ctx->fitted = false;
+    if (hdr_host == nullptr) {             // back to the scores W x + b
+        ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+        return DKS_OK;
+    }
+    REQUIRE(ctx->R > 0, "dks_set_column_maps: call dks_set_model first");
+    if (D != ctx->D || R != ctx->R)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: maps of %d columns x %d score rows, model has %d x %d", D, R,
+                    ctx->D, ctx->R);
+    if (n_keys < 0 || n_vals < 1 || (n_keys > 0 && !keys_host) || !vals_host)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: bad table sizes");
+    for (int c = 0; c < D; ++c) {
+        const int flags = hdr_host[4 * c], m = hdr_host[4 * c + 1], ko = hdr_host[4 * c + 2], vo = hdr_host[4 * c + 3];
+        const bool cat = flags & DKS_CM_CATEGORICAL;
+        const long long nk = cat ? m : (long long)m - 1;
+        const long long nv = (long long)R * (cat ? m + 2 : 2 * (long long)m + 1);
+        if ((flags & ~(DKS_CM_CATEGORICAL | DKS_CM_NAN_ERROR | DKS_CM_UNKNOWN_ERROR)) || (!cat && (flags & DKS_CM_UNKNOWN_ERROR)) ||
+            m < 1 || ko < 0 || vo < 0 || ko + nk > n_keys || vo + nv > n_vals)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: malformed header of column %d", c);
+        for (long long k = 0; k < nk; ++k) {
+            const double t = keys_host[ko + k];
+            if (!std::isfinite(t) || (k > 0 && !(keys_host[ko + k - 1] < t)))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: column %d: %s must be finite and strictly increasing",
+                            c, cat ? "keys" : "breakpoints");
+        }
+        for (long long k = 0; k < nv; ++k)
+            if (!std::isfinite(vals_host[vo + k]))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: column %d: values must be finite", c);
+    }
+    ctx->h_cm_hdr.assign(hdr_host, hdr_host + 4 * (size_t)D);
+    ctx->h_cm_keys.assign(keys_host, keys_host + n_keys);
+    ctx->h_cm_vals.assign(vals_host, vals_host + n_vals);
     return DKS_OK;
 }
 
@@ -1057,6 +1103,25 @@ int dks_fit(dks_ctx* ctx) {
     TRY(dev_alloc(&ctx->d_wbf, (size_t)N));
     TRY(dev_alloc(&ctx->d_wn, (size_t)N));
     cudaStream_t st = ctx->stream;
+    const bool maps = !ctx->h_cm_hdr.empty();
+    {
+        int* hdr = const_cast<int*>(ctx->cm.hdr);
+        double* keys = const_cast<double*>(ctx->cm.keys);
+        double* vals = const_cast<double*>(ctx->cm.vals);
+        dev_free(&hdr); dev_free(&keys); dev_free(&vals);
+        ctx->cm = ColumnMapsDev{};
+        if (maps) {
+            const size_t nk = ctx->h_cm_keys.size(), nv = ctx->h_cm_vals.size();
+            TRY(dev_alloc(&hdr, ctx->h_cm_hdr.size()));
+            TRY(dev_alloc(&keys, nk));
+            TRY(dev_alloc(&vals, nv));
+            CUDA_TRY(cudaMemcpy(hdr, ctx->h_cm_hdr.data(), sizeof(int) * ctx->h_cm_hdr.size(), cudaMemcpyHostToDevice));
+            if (nk) CUDA_TRY(cudaMemcpy(keys, ctx->h_cm_keys.data(), sizeof(double) * nk, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(vals, ctx->h_cm_vals.data(), sizeof(double) * nv, cudaMemcpyHostToDevice));
+            ctx->cm = ColumnMapsDev{hdr, keys, vals, (int)nk, (int)nv};
+        }
+    }
+    CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
     {
         // the weighted shared-plan kernels read w'_j = N w_j: their sums then have the magnitude of the uniform ones
         std::vector<float> wn(N);
@@ -1072,8 +1137,8 @@ int dks_fit(dks_ctx* ctx) {
 
     ctx->scale = (ctx->act == DKS_ACT_BINARY_LOGISTIC) ? -ctx->kappa * 1.4426950408889634
                : (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_EXP) ? 1.4426950408889634 : 1.0;
-    dks::fit_bw_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D,
-                                                                           G, R, ctx->d_BW);
+    (maps ? dks::fit_bw_kernel<true> : dks::fit_bw_kernel<false>)<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(
+        ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D, G, R, ctx->d_BW, ctx->cm, ctx->d_status);
     dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
     dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
     dks::fit_fnull_kernel<<<1, 256, 0, st>>>(ctx->d_scores, ctx->d_BW, ctx->d_wbg, N, G, R, C, ctx->act, ctx->kappa,
@@ -1087,7 +1152,11 @@ int dks_fit(dks_ctx* ctx) {
     ctx->h_linkfnull.resize(C);
     CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
+        return fail(DKS_ERR_DOMAIN, "background row %d holds a raw value its column map refuses (NaN, or a category unseen "
+                    "at fit time, where the pipeline raises)", ctx->h_status[1]);
     if (ctx->act == DKS_ACT_EXP && !std::isfinite(ctx->h_fnull[0]))
         return fail(DKS_ERR_NUMERIC, "exp head: the background's predictions are not all finite in float64 (fnull = %g)",
                     ctx->h_fnull[0]);
@@ -1133,13 +1202,18 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     TRY(dev_alloc(&dX, (size_t)n * ctx->D));
     TRY(dev_alloc(&dO, (size_t)n * ctx->C));
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
-    dks::predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act,
-                                                                ctx->kappa, dO);
+    CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
+    (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
+        dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(out_host, dO, sizeof(double) * n * ctx->C, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     cudaFree(dX); cudaFree(dO);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
+        return fail(DKS_ERR_DOMAIN, "row %d holds a raw value its column map refuses (NaN, or a category unseen at fit time, "
+                    "where the pipeline raises)", ctx->h_status[1]);
     return DKS_OK;
 }
 

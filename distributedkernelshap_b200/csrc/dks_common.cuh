@@ -111,6 +111,18 @@ struct ExplainParams {
     const int* count;     // ... and how many (device memory)
 };
 
+// column maps (dks_set_column_maps, DESIGN.md §5.0.9): per raw column, a piecewise affine or categorical function giving
+// that column's R score contributions -- a linear model behind per-column preprocessing, read in raw feature space
+#define DKS_CM_CATEGORICAL 1
+#define DKS_CM_NAN_ERROR 2
+#define DKS_CM_UNKNOWN_ERROR 4
+struct ColumnMapsDev {
+    const int* hdr;       // [D][4] {flags, m, key offset, value offset}
+    const double* keys;   // breakpoints (m - 1 per affine column) / keys (m per categorical column)
+    const double* vals;   // affine [m][2][R] + NaN row [R]; categorical [m][R] + unknown row [R] + NaN row [R]
+    int n_keys, n_vals;
+};
+
 // float64 background of the exp head's rows outside the range rule (a kernel parameter of its own: ExplainParams is
 // embedded in other kernels' parameter blocks, whose layout stays as it is)
 struct ExpBackground {
@@ -148,10 +160,13 @@ struct dks_ctx {
 
     // host copies
     std::vector<double> h_bg, h_wbg, h_W, h_b;
+    std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
+    std::vector<double> h_cm_keys, h_cm_vals;
     std::vector<int32_t> h_goff, h_gcols;
 
     // device, fit-time
     double *d_bg = nullptr, *d_wbg = nullptr, *d_W = nullptr, *d_b = nullptr;
+    ColumnMapsDev cm = {};                     // device copy of the column maps (cm.hdr == nullptr: none)
     int32_t *d_goff = nullptr, *d_gcols = nullptr;
     double *d_colmin = nullptr, *d_colmax = nullptr;
     int* d_colnan = nullptr;

@@ -91,16 +91,62 @@ __device__ inline void head_f64(const double* z, int R, int act, double kappa, d
     }
 }
 
+// column maps: adds f_col(x), the R score contributions of one raw value, to acc.  A binary search over the column's
+// breakpoints (numpy's searchsorted side='right': a value on a breakpoint takes the piece on its right) then R FMAs, or over
+// its keys (exact match, else the unknown row) then R loads.  Returns false, adding nothing, where the map's policy is
+// "error" (NaN, or a category unseen at fit time).
+__device__ __forceinline__ bool cm_add(const int* __restrict__ h, const double* __restrict__ keys,
+                                       const double* __restrict__ vals, double x, int R, double* acc) {
+    const int flags = h[0], m = h[1];
+    const double* t = keys + h[2];
+    const double* v = vals + h[3];
+    const double* row;
+    if (isnan(x)) {
+        if (flags & DKS_CM_NAN_ERROR) return false;
+        row = v + (size_t)((flags & DKS_CM_CATEGORICAL) ? m + 1 : 2 * m) * R;
+    } else if (flags & DKS_CM_CATEGORICAL) {
+        int lo = 0, hi = m;                       // first key >= x
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (t[mid] < x) lo = mid + 1; else hi = mid; }
+        if (lo < m && t[lo] == x) row = v + (size_t)lo * R;
+        else if (flags & DKS_CM_UNKNOWN_ERROR) return false;
+        else row = v + (size_t)m * R;
+    } else {
+        int lo = 0, hi = m - 1;                   // piece = breakpoints <= x
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (t[mid] <= x) lo = mid + 1; else hi = mid; }
+        const double* p = v + (size_t)2 * lo * R;
+        for (int r = 0; r < R; ++r) acc[r] += fma(p[r], x, p[R + r]);
+        return true;
+    }
+    for (int r = 0; r < R; ++r) acc[r] += row[r];
+    return true;
+}
+
+// reports the first instance / background row whose raw value a column map refuses
+__device__ __forceinline__ void cm_report(int* status, int row) {
+    if (atomicCAS(&status[0], 0, DKS_ERR_DOMAIN) == 0) status[1] = row;
+}
+
 // ------------------------------------------------------------------------------------------------------
 // K0: fit (DenseData + KernelExplainer.__init__)
 // ------------------------------------------------------------------------------------------------------
-// BW[j][g][r] = sum_{col in g} bg[j][col] * W[r][col]
+// BW[j][g][r] = sum_{col in g} bg[j][col] * W[r][col]; MAPS: sum_{col in g} f_{r,col}(bg[j][col]) (column maps)
+template <bool MAPS>
 __global__ void fit_bw_kernel(const double* __restrict__ bg, const double* __restrict__ W,
                               const int32_t* __restrict__ goff, const int32_t* __restrict__ gcols, int N, int D,
-                              int G, int R, double* __restrict__ BW) {
+                              int G, int R, double* __restrict__ BW, ColumnMapsDev cm, int* __restrict__ status) {
     int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= N * G * R) return;
     int r = idx % R, g = (idx / R) % G, j = idx / (R * G);
+    if (MAPS) {
+        double acc[8];
+        for (int q = 0; q < R; ++q) acc[q] = 0;
+        for (int c = goff[g]; c < goff[g + 1]; ++c) {
+            const int col = gcols[c];
+            if (!cm_add(cm.hdr + 4 * col, cm.keys, cm.vals, bg[(size_t)j * D + col], R, acc)) cm_report(status, j);
+        }
+        BW[idx] = acc[r];
+        return;
+    }
     double acc = 0;
     for (int c = goff[g]; c < goff[g + 1]; ++c) {
         int col = gcols[c];
@@ -174,17 +220,24 @@ __global__ void fit_scale_kernel(const double* __restrict__ BW, const double* __
     if (idx < N) wbf[idx] = (float)wbg[idx];
 }
 
-// f(X) for n rows, float64 (model check against the Python callable)
+// f(X) for n rows, float64 (model check against the Python callable); MAPS: the scores through the column maps
+template <bool MAPS>
 __global__ void predict_kernel(const double* __restrict__ X, const double* __restrict__ W,
                                const double* __restrict__ b, int n, int D, int R, int C, int act, double kappa,
-                               double* __restrict__ out) {
+                               double* __restrict__ out, ColumnMapsDev cm, int* __restrict__ status) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     double z[DKS_MAX_OUT], o[DKS_MAX_OUT];
-    for (int r = 0; r < R; ++r) {
-        double acc = b[r];
-        for (int c = 0; c < D; ++c) acc += X[(size_t)i * D + c] * W[(size_t)r * D + c];
-        z[r] = acc;
+    if (MAPS) {
+        for (int r = 0; r < R; ++r) z[r] = b[r];
+        for (int c = 0; c < D; ++c)
+            if (!cm_add(cm.hdr + 4 * c, cm.keys, cm.vals, X[(size_t)i * D + c], R, z)) cm_report(status, i);
+    } else {
+        for (int r = 0; r < R; ++r) {
+            double acc = b[r];
+            for (int c = 0; c < D; ++c) acc += X[(size_t)i * D + c] * W[(size_t)r * D + c];
+            z[r] = acc;
+        }
     }
     head_f64(z, R, act, kappa, o);
     for (int c = 0; c < C; ++c) out[(size_t)i * C + c] = o[c];
@@ -213,7 +266,10 @@ __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
 // (Measured on the Adult shape: 13.3 us per launch under ncu against 13.8 us unstaged -- the kernel is bound by launch +
 // one cold DRAM round trip + the serial per-instance tail, not by the column loop; kept because it is never slower.)
 // The host picks STAGE when the tables fit shared memory.
-template <bool STAGE>
+// MAPS: the contributions come from the column maps `cm` instead of W -- per column a binary search and R FMAs or loads
+// (cm_add); STAGE then stages the maps' tables where W would be.  A raw value a map refuses is reported as DKS_ERR_DOMAIN
+// with the instance index and contributes nothing.
+template <bool STAGE, bool MAPS>
 __global__ void prep_kernel(const double* __restrict__ X, const double* __restrict__ W, const double* __restrict__ b,
                             const double* __restrict__ bg, const int32_t* __restrict__ goff,
                             const int32_t* __restrict__ gcols, const double* __restrict__ colmin,
@@ -223,23 +279,30 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
                             int* __restrict__ Mcnt, double* __restrict__ dlink, int* __restrict__ hist,
                             int* __restrict__ counts, int* __restrict__ idx_full, int* __restrict__ idx_other,
                             double* __restrict__ XT, double xt_scale, const double* __restrict__ xt_sub,
-                            int* __restrict__ status) {
+                            int* __restrict__ status, ColumnMapsDev cm) {
     extern __shared__ __align__(16) unsigned char prep_smem[];
     double* sXW = reinterpret_cast<double*>(prep_smem);                        // [ipb][G][R]
     double* sX = sXW + (size_t)ipb * G * R;                                    // STAGE: [ipb][D]
-    double* sW = sX + (STAGE ? (size_t)ipb * D : 0);                           //        [R][D]
-    double* sMin = sW + (STAGE ? (size_t)R * D : 0);                           //        [D]
+    double* sW = sX + (STAGE ? (size_t)ipb * D : 0);                           //        [R][D] (MAPS: keys, values)
+    double* sMin = sW + (STAGE ? (MAPS ? (size_t)cm.n_keys + cm.n_vals : (size_t)R * D) : 0);   //        [D]
     double* sMax = sMin + (STAGE ? D : 0);                                     //        [D]
     int* sNan = reinterpret_cast<int*>(sMax + (STAGE ? D : 0));                //        [D]
     int* sCols = sNan + (STAGE ? D : 0);                                       //        [D]
     int* sOff = sCols + (STAGE ? D : 0);                                       //        [G + 1]
-    unsigned char* sflag = reinterpret_cast<unsigned char*>(sOff + (STAGE ? G + 1 : 0));   // [ipb][G]
+    int* sHdr = sOff + (STAGE ? G + 1 : 0);                                    // MAPS:  [D][4]
+    unsigned char* sflag = reinterpret_cast<unsigned char*>(sHdr + (STAGE && MAPS ? 4 * D : 0));   // [ipb][G]
     const int i0 = blockIdx.x * ipb;
     if (STAGE) {
         const int rows = min(ipb, n - i0);
         const double* Xb = X + (size_t)i0 * D;
         for (int idx = threadIdx.x; idx < rows * D; idx += blockDim.x) sX[idx] = Xb[idx];
-        for (int idx = threadIdx.x; idx < R * D; idx += blockDim.x) sW[idx] = W[idx];
+        if (MAPS) {
+            for (int idx = threadIdx.x; idx < cm.n_keys; idx += blockDim.x) sW[idx] = cm.keys[idx];
+            for (int idx = threadIdx.x; idx < cm.n_vals; idx += blockDim.x) sW[cm.n_keys + idx] = cm.vals[idx];
+            for (int idx = threadIdx.x; idx < 4 * D; idx += blockDim.x) sHdr[idx] = cm.hdr[idx];
+        } else {
+            for (int idx = threadIdx.x; idx < R * D; idx += blockDim.x) sW[idx] = W[idx];
+        }
         for (int idx = threadIdx.x; idx < D; idx += blockDim.x) {
             sMin[idx] = colmin[idx]; sMax[idx] = colmax[idx]; sNan[idx] = colnan[idx]; sCols[idx] = gcols[idx];
         }
@@ -256,7 +319,13 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
         for (int c = c0; c < c1; ++c) {
             const int col = STAGE ? sCols[c] : gcols[c];
             const double xv = STAGE ? sX[(size_t)li * D + col] : X[(size_t)i * D + col];
-            for (int r = 0; r < R; ++r) acc[r] += xv * (STAGE ? sW[(size_t)r * D + col] : W[(size_t)r * D + col]);
+            if (MAPS) {
+                if (!cm_add(STAGE ? sHdr + 4 * col : cm.hdr + 4 * col, STAGE ? sW : cm.keys,
+                            STAGE ? sW + cm.n_keys : cm.vals, xv, R, acc))
+                    cm_report(status, i);
+            } else {
+                for (int r = 0; r < R; ++r) acc[r] += xv * (STAGE ? sW[(size_t)r * D + col] : W[(size_t)r * D + col]);
+            }
             if ((STAGE ? sNan[col] : colnan[col]) || isnan(xv)) {
                 if (!varies)
                     for (int j = 0; j < N && !varies; ++j) varies = !np_isclose(xv, bg[(size_t)j * D + col]);
@@ -316,9 +385,13 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
         if (act == DKS_ACT_EXP && !isfinite(o[0]) && atomicCAS(&status[0], 0, DKS_ERR_NUMERIC) == 0) status[1] = i;
     }
 }
-inline size_t prep_smem_bytes(bool stage, int ipb, int G, int R, int D) {
+// maps_doubles: the column maps' keys + values staged in place of W (0: the W path); their headers add 4 D ints
+inline size_t prep_smem_bytes(bool stage, int ipb, int G, int R, int D, size_t maps_doubles = 0) {
     size_t b = sizeof(double) * (size_t)ipb * G * R + (size_t)ipb * G + 16;
-    if (stage) b += sizeof(double) * ((size_t)ipb * D + (size_t)R * D + 2 * (size_t)D) + sizeof(int) * (2 * (size_t)D + G + 1);
+    if (stage && maps_doubles)
+        b += sizeof(double) * ((size_t)ipb * D + maps_doubles + 2 * (size_t)D) + sizeof(int) * (6 * (size_t)D + G + 1);
+    else if (stage)
+        b += sizeof(double) * ((size_t)ipb * D + (size_t)R * D + 2 * (size_t)D) + sizeof(int) * (2 * (size_t)D + G + 1);
     return b;
 }
 

@@ -111,3 +111,44 @@ def wide_onehot(n, n_blocks=64, block_width=16, n_background=256, seed=0, single
         names = [f"var{b}" for b in range(n_blocks)]
     return {"predictor": predictor, "X_explain": both[n_background:], "background": both[:n_background],
             "groups": groups, "group_names": names}
+
+
+def decode_onehot_blocks(A, n_numeric, widths, drop_first):
+    """Raw columns of an encoded matrix: the ``n_numeric`` leading columns as they are, then one level code per one-hot
+    block of ``widths`` (``drop_first``: an all-zero block is level 0 and column k is level k + 1; else column k is level
+    k)."""
+    cols, start = [A[:, :n_numeric]], n_numeric
+    for w in widths:
+        block = A[:, start:start + w]
+        code = block.argmax(axis=1) + (1 if drop_first else 0)
+        if drop_first:
+            code = np.where(block.any(axis=1), code, 0)
+        cols.append(code[:, None].astype(np.float64))
+        start += w
+    return np.hstack(cols)
+
+
+def raw_space_pipeline(predictor, raw, n_numeric, widths, drop_first):
+    """A fitted scikit-learn ``Pipeline(ColumnTransformer(StandardScaler, OneHotEncoder(drop='first' | None)),
+    LogisticRegression)`` over the raw columns of ``decode_onehot_blocks`` that computes what the encoded two-class
+    ``predictor`` (``LinearSoftmaxClassifier``, p1 = sigmoid(2 z)) computes: its coefficients, with the scaler folded
+    back in.  This is how such a model ships (the reference's Adult model, scripts/process_adult_data.py)."""
+    from sklearn.compose import ColumnTransformer
+    from sklearn.linear_model import LogisticRegression
+    from sklearn.pipeline import Pipeline
+    from sklearn.preprocessing import OneHotEncoder, StandardScaler
+    num = list(range(n_numeric))
+    cats = [np.arange(w + (1.0 if drop_first else 0.0)) for w in widths]
+    parts = [("cat", OneHotEncoder(drop="first" if drop_first else None, categories=cats),
+              list(range(n_numeric, n_numeric + len(widths))))]
+    if n_numeric:
+        parts.insert(0, ("num", StandardScaler(), num))
+    ct = ColumnTransformer(parts).fit(raw)
+    lr = LogisticRegression().fit(ct.transform(raw)[:4], [0, 1, 0, 1])
+    coef, b = predictor.coef_[0], float(predictor.intercept_[0])
+    if n_numeric:
+        sc = ct.named_transformers_["num"]
+        coef = np.r_[coef[:n_numeric] * sc.scale_, coef[n_numeric:]]
+        b += float(predictor.coef_[0, :n_numeric] @ sc.mean_)
+    lr.coef_, lr.intercept_ = 2.0 * coef[None, :], np.array([2.0 * b])
+    return Pipeline([("prep", ct), ("clf", lr)])

@@ -123,7 +123,9 @@ class GpuKernelExplainer:
     ----------
     model
         What the reference passes as ``predictor``: a bound ``predict_proba`` / ``decision_function`` of a linear
-        model, or a ``LinearModelSpec`` (see ``predictors.extract_linear_spec``).
+        model or of a ``Pipeline`` of per-column preprocessing ending in one (explained in raw feature space), or a
+        ``LinearModelSpec`` (see ``predictors.extract_linear_spec``).  A raw value the pipeline would refuse (NaN, or an
+        unseen category under ``handle_unknown='error'``) raises ``ValueError``.
     data
         Background data: array, DataFrame or ``DenseData`` (groups and weights honoured).
     link
@@ -159,8 +161,8 @@ class GpuKernelExplainer:
         if bg.ndim != 2:
             raise TypeError("background data must be two-dimensional")
         self.N, self.P = bg.shape
-        if self.spec.W.shape[1] != self.P:
-            raise ValueError(f"model expects {self.spec.W.shape[1]} columns, background has {self.P}")
+        if self.spec.n_features != self.P:
+            raise ValueError(f"model expects {self.spec.n_features} columns, background has {self.P}")
         if self.N > 100:
             logger.warning("Using %d background data samples could cause slower run times. Consider using "
                            "shap.sample(data, K) or shap.kmeans(data, K) to summarize the background as K samples.",
@@ -178,8 +180,13 @@ class GpuKernelExplainer:
         offsets[1:] = np.cumsum([len(g) for g in self.data.groups])
         cols = np.ascontiguousarray(np.concatenate([np.asarray(g, dtype=np.int32) for g in self.data.groups]), dtype=np.int32)
         _cabi.check(self.lib.dks_set_groups(self._ctx, _cabi.ptr(offsets), _cabi.ptr(cols), self.data.groups_size))
-        _cabi.check(self.lib.dks_set_model(self._ctx, _cabi.ptr(self.spec.W), _cabi.ptr(self.spec.b), self.spec.W.shape[0],
+        maps = self.spec.maps
+        W = self.spec.W if maps is None else np.zeros((self.spec.R, self.P))    # not read once the maps are set
+        _cabi.check(self.lib.dks_set_model(self._ctx, _cabi.ptr(W), _cabi.ptr(self.spec.b), self.spec.R,
                                            self.spec.act_code, self.spec.kappa, int(self.spec.scalar_out)))
+        if maps is not None:
+            _cabi.check(self.lib.dks_set_column_maps(self._ctx, maps.D, maps.R, _cabi.ptr(maps.hdr), _cabi.ptr(maps.keys),
+                                                     len(maps.keys), _cabi.ptr(maps.vals), len(maps.vals)))
         link_code = _cabi.LINK_LOGIT if str(self.link) == "logit" else _cabi.LINK_IDENTITY
         _cabi.check(self.lib.dks_set_link(self._ctx, link_code))
         self.set_kernel(kernel)

@@ -11,29 +11,46 @@ from . import _cabi
 
 
 class LinearModelSpec:
-    """``z = X W^T + b`` then a head.  ``W`` is [R, D], ``b`` [R].
+    """``z = X W^T + b`` then a head.  ``W`` is [R, D], ``b`` [R].  With ``maps`` (a ``column_maps.ColumnMaps``; ``W`` is
+    then None) the scores are ``z = b + sum_col f_col(X[:, col])``: a linear model behind per-column preprocessing.
 
     activation: 'identity' (outputs z), 'binary_logistic' (R == 1; outputs [1 - s, s], s = sigmoid(kappa z)),
     'softmax' (outputs softmax(z), R = C >= 2), 'ovr' (one-vs-rest, R = C >= 3: s_c = sigmoid(z_c), outputs
     s_c / sum_c' s_c', scikit-learn's ``_predict_proba_lr``; kappa 1), 'exp' (R = 1: outputs exp(z), the ``predict`` of
     scikit-learn's log-link GLM regressors).  ``scalar_out``: the callable returns a 1-D array."""
 
-    def __init__(self, W, b, activation, kappa=1.0, scalar_out=False):
-        self.W = np.ascontiguousarray(np.atleast_2d(np.asarray(W, dtype=np.float64)))
+    def __init__(self, W, b, activation, kappa=1.0, scalar_out=False, maps=None):
         self.b = np.ascontiguousarray(np.atleast_1d(np.asarray(b, dtype=np.float64)))
-        if self.W.shape[0] != self.b.shape[0]:
-            raise ValueError(f"W has {self.W.shape[0]} rows but b has {self.b.shape[0]} entries")
+        self.maps = maps
+        if maps is None:
+            self.W = np.ascontiguousarray(np.atleast_2d(np.asarray(W, dtype=np.float64)))
+            R = self.W.shape[0]
+        else:
+            self.W = None           # the scores are b + maps.contributions(x) (column_maps.py)
+            R = maps.R
+        if R != self.b.shape[0]:
+            raise ValueError(f"W has {R} rows but b has {self.b.shape[0]} entries")
         if activation not in ("identity", "binary_logistic", "softmax", "ovr", "exp"):
             raise ValueError(f"unknown activation {activation!r}")
-        if activation == "binary_logistic" and self.W.shape[0] != 1:
+        if activation == "binary_logistic" and R != 1:
             raise ValueError("binary_logistic needs a single score row")
-        if activation == "exp" and self.W.shape[0] != 1:
+        if activation == "exp" and R != 1:
             raise ValueError("the exp head needs a single score row (log-link models with several outputs are not supported)")
-        if activation == "ovr" and (self.W.shape[0] < 3 or float(kappa) != 1.0):
+        if activation == "ovr" and (R < 3 or float(kappa) != 1.0):
             raise ValueError("the one-vs-rest head needs at least three score rows and kappa = 1")
         self.activation = activation
         self.kappa = float(kappa)
         self.scalar_out = bool(scalar_out)
+
+    @property
+    def R(self):
+        """Score rows."""
+        return self.b.shape[0]
+
+    @property
+    def n_features(self):
+        """Raw input columns the model reads."""
+        return self.maps.D if self.maps is not None else self.W.shape[1]
 
     @property
     def act_code(self):
@@ -42,14 +59,14 @@ class LinearModelSpec:
 
     @property
     def n_outputs(self):
-        return 2 if self.activation == "binary_logistic" else self.W.shape[0]
+        return 2 if self.activation == "binary_logistic" else self.R
 
     def __call__(self, X):
         """NumPy evaluation with scikit-learn's conventions (used on the host by build_explanation and tests)."""
         X = np.asarray(X, dtype=np.float64)
         if X.ndim == 1:
             X = X.reshape(1, -1)
-        z = X @ self.W.T + self.b
+        z = (self.maps.contributions(X) if self.maps is not None else X @ self.W.T) + self.b
         if self.activation == "identity":
             return z[:, 0] if self.scalar_out else z
         if self.activation == "exp":
@@ -108,7 +125,9 @@ def extract_linear_spec(predictor):
     Accepts: a ``LinearModelSpec``; any object/bound method whose owner offers ``dks_linear_spec()``; bound
     ``predict_proba`` / ``decision_function`` / ``predict`` of scikit-learn linear models (``coef_``/``intercept_``);
     bound ``predict_proba`` of a single-label ``OneVsRestClassifier`` over at least three binary linear models; bound
-    ``predict`` of the log-link GLM regressors (``_is_log_link_glm``), whose head is 'exp'.
+    ``predict`` of the log-link GLM regressors (``_is_log_link_glm``), whose head is 'exp'; the same methods of a fitted
+    scikit-learn ``Pipeline`` whose transformers act on one column at a time and whose final step is any of the above
+    (``_pipeline_spec``: the model is read in raw feature space through column maps).
     Raises ``TypeError`` for everything else."""
     if isinstance(predictor, LinearModelSpec):
         return predictor
@@ -119,6 +138,8 @@ def extract_linear_spec(predictor):
     if owner is None:
         raise TypeError("predictor must be a bound method of a linear model (e.g. clf.predict_proba) or a "
                         "LinearModelSpec: the CUDA engine cannot call an opaque Python function and has no CPU fallback")
+    if _is_sklearn_pipeline(owner):
+        return _pipeline_spec(owner, method)
     if hasattr(owner, "dks_linear_spec") and (method == "predict_proba" or
                                               (method == "predict" and not hasattr(owner, "classes_"))):
         return owner.dks_linear_spec()     # a regressor's predict (e.g. a log-link GLM stand-in) takes the hook too
@@ -144,6 +165,26 @@ def extract_linear_spec(predictor):
             return LinearModelSpec(coef, intercept, "exp", scalar_out=True)
         return LinearModelSpec(coef, intercept, "identity", scalar_out=coef.shape[0] == 1)
     raise TypeError(f"unsupported predictor method {method!r}")
+
+
+def _is_sklearn_pipeline(owner):
+    return any(c.__name__ == "Pipeline" and c.__module__.startswith("sklearn.") for c in type(owner).__mro__)
+
+
+def _pipeline_spec(pipe, method):
+    """A Pipeline's ``method`` as column maps over its raw columns (``column_maps.compile_maps``) followed by the head
+    its final estimator's ``method`` has.  The final estimator's intercept becomes ``b``."""
+    from .column_maps import compile_maps, pipeline_parts
+    pre, final = pipeline_parts(pipe)
+    bound = getattr(final, method, None)
+    if bound is None:
+        raise TypeError(f"{type(final).__name__} has no {method}")
+    inner = extract_linear_spec(bound)
+    n_raw = getattr(pipe, "n_features_in_", None)
+    if n_raw is None:
+        raise TypeError("the Pipeline is not fitted (no n_features_in_)")
+    maps = compile_maps(pre, int(n_raw), inner.W)
+    return LinearModelSpec(None, inner.b, inner.activation, kappa=inner.kappa, scalar_out=inner.scalar_out, maps=maps)
 
 
 def _is_log_link_glm(owner):

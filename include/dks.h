@@ -33,6 +33,8 @@ extern "C" {
 #define DKS_ERR_UNSUPPORTED 3   /* valid request the engine does not implement (never a silent fallback) */
 #define DKS_ERR_PLAN_MISSING 4  /* an instance needs a coalition plan for an M that was not provided */
 #define DKS_ERR_NUMERIC 5       /* normal matrix not positive definite; exp head: a model output that is not finite */
+#define DKS_ERR_DOMAIN 6        /* column maps: a raw value a map refuses (NaN or an unseen category under the policy
+                                 * "error"); the detail is the instance (or background row) index */
 
 /* model head applied to the linear scores z = W x + b   (replaces the opaque `predictor` callable,
  * benchmarks/ray_pool.py:34; sklearn LogisticRegression.predict_proba per scripts/fit_adult_model.py:27) */
@@ -91,6 +93,20 @@ int dks_set_groups(dks_ctx* ctx, const int32_t* group_offsets, const int32_t* gr
  * 1-D array (vector_out False). */
 int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int R, int activation, double kappa,
                   int scalar_out);
+/* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
+ * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
+ * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
+ *   piecewise affine (flags & 1 == 0): m pieces, m - 1 strictly increasing breakpoints t at keys_host[key offset ..]; piece
+ *     k = number of breakpoints <= x (numpy searchsorted side='right'), f_r(x) = a[k][r] x + c[k][r]; values [m][2][R] (the a
+ *     row then the c row of each piece) then the NaN row [R];
+ *   categorical (flags & 1): m strictly increasing keys; an exact match gives that key's row, no match the unknown row;
+ *     values [m][R], the unknown row [R], then the NaN row [R].
+ * flags & 2: NaN is refused; flags & 4 (categorical): an unknown value is refused.  A refused value is reported as
+ * DKS_ERR_DOMAIN (by dks_fit for a background row, by dks_predict_host and the explain calls for an instance); it is never
+ * evaluated.  Varying groups are still decided on the raw columns.  Malformed tables (shape, offsets, unsorted or
+ * non-finite keys, non-finite values) return DKS_ERR_UNSUPPORTED.  hdr_host == NULL clears the maps; dks_set_model does too. */
+int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
+                        const double* vals_host, int n_vals);
 int dks_set_link(dks_ctx* ctx, int link);
 /* runs the fit kernels (grouped background scores, fnull = sum_j w_j f(bg_j), link(fnull)); synchronises. */
 int dks_fit(dks_ctx* ctx);
