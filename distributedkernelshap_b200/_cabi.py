@@ -28,6 +28,7 @@ ACT_BINARY_LOGISTIC = 1
 ACT_SOFTMAX = 2
 ACT_OVR = 3
 ACT_EXP = 4
+ACT_MIX = 5
 LINK_IDENTITY = 0
 LINK_LOGIT = 1
 KERNEL_AUTO = 0
@@ -47,6 +48,7 @@ SIGNATURES = {
     "dks_set_background": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "dks_set_groups": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "dks_set_model": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_int]),
+    "dks_set_mixture": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "dks_set_column_maps": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "dks_set_link": (C.c_int, [C.c_void_p, C.c_int]),
     "dks_fit": (C.c_int, [C.c_void_p]),

@@ -11,6 +11,7 @@
 #include "dks_shared.cuh"
 #include "dks_fused.cuh"
 #include "dks_l1.cuh"
+#include "dks_mixture.cuh"
 #include "dks_multi.cuh"
 #include "dks_wide.cuh"
 #include "dks_sampler.cuh"
@@ -134,21 +135,26 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const size_t maps_doubles = maps ? (size_t)ctx->cm.n_keys + ctx->cm.n_vals : 0;
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D, maps_doubles) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D, maps_doubles);
-    auto kern = maps ? (stage ? dks::prep_kernel<true, true> : dks::prep_kernel<false, true>)
-                     : (stage ? dks::prep_kernel<true, false> : dks::prep_kernel<false, false>);
+    const bool mix = ctx->act == DKS_ACT_MIX;
+    auto kern = mix ? (maps ? (stage ? dks::prep_kernel<true, true, true> : dks::prep_kernel<false, true, true>)
+                            : (stage ? dks::prep_kernel<true, false, true> : dks::prep_kernel<false, false, true>))
+                    : maps ? (stage ? dks::prep_kernel<true, true> : dks::prep_kernel<false, true>)
+                           : (stage ? dks::prep_kernel<true, false> : dks::prep_kernel<false, false>);
     // nibble tables: the binary head's scaled contributions; the softmax and one-vs-rest heads' per class (log2 e XW), the
     // identity head's XW - Bbar and the exp head's log2 e XW, up to 128 groups (what the shared-plan path of those heads
     // covers)
     double* xt = nullptr;
     if (ctx->act == DKS_ACT_BINARY_LOGISTIC && ctx->R == 1) xt = ctx->d_XT;
     else if ((ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_IDENTITY ||
-              ctx->act == DKS_ACT_EXP) && G <= 128 && ctx->plan_mode == 0) xt = ctx->d_XT;
+              ctx->act == DKS_ACT_EXP || mix) && G <= 128 && ctx->plan_mode == 0) xt = ctx->d_XT;
+    // the mixture's tables are per member, member-major: -log2 e for binary members (the binary head's sign), log2 e else
+    const double xt_scale = mix ? (ctx->mix.mact == DKS_ACT_BINARY_LOGISTIC ? -DKS_LOG2E : DKS_LOG2E) : ctx->scale;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
         X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
         ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
         ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-        xt, ctx->scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm);
+        xt, xt_scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
@@ -158,13 +164,33 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     return DKS_OK;
 }
 
+// mixture of binary-logistic members: two outputs, class 0 the negation of class 1 (one solve, like the binary head)
+bool mix_binary(const dks_ctx* ctx) { return ctx->act == DKS_ACT_MIX && ctx->mix.mact == DKS_ACT_BINARY_LOGISTIC; }
+
+// the mixture's member buffer (one member's sums) for at least `need` floats
+int ensure_mixscr(dks_ctx* ctx, size_t need) {
+    if (need > ctx->cap_mixscr) { TRY(dev_alloc(&ctx->d_mixscr, need)); ctx->cap_mixscr = need; ctx->epoch++; }
+    return DKS_OK;
+}
+
+// dst (+)= pi_k x the member buffer, over the rows of the instances on the shared-plan path
+int launch_mix_axpy(dks_ctx* ctx, float* dst, float pi, bool first, int stride, int n) {
+    long long grid = cdiv((long long)n * stride, 256);
+    if (grid > (long long)ctx->sm_count * 8) grid = (long long)ctx->sm_count * 8;
+    if (grid < 1) grid = 1;
+    dks::mix::mix_axpy_kernel<<<(int)grid, 256, 0, ctx->stream>>>(ctx->d_mixscr, dst, pi, first ? 1 : 0, ctx->d_idx_full,
+                                                                   ctx->d_counts, stride);
+    CUDA_TRY(cudaGetLastError());
+    return DKS_OK;
+}
+
 // what the l1 kernels of both instance lists share
 dks::l1::Params l1_params(dks_ctx* ctx, int n, int nout, double* phi_dev) {
     dks::l1::Params lp;
     memset(&lp, 0, sizeof(lp));
     lp.n = n; lp.N = ctx->N; lp.G = ctx->G; lp.C = ctx->C; lp.link = ctx->link;
     lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.nout = nout; lp.tabs = ctx->d_l1;
-    lp.binary = ctx->act == DKS_ACT_BINARY_LOGISTIC;
+    lp.binary = ctx->act == DKS_ACT_BINARY_LOGISTIC || mix_binary(ctx);
     lp.src.act = ctx->act;                           // the exp head's LARS skips tasks with non-finite moments
     lp.dlink = ctx->d_dlink; lp.linkfnull = ctx->d_linkfnull; lp.fnull = ctx->d_fnull;
     lp.mom = ctx->d_mom; lp.phi = phi_dev; lp.status = ctx->d_status;
@@ -236,6 +262,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     const double* ext_chol = nullptr;
     const double* ext_ainv = nullptr;
     int ext_fstride = 0;
+    // the mixture head: one pass of the member head's shared-plan kernel per member for instances whose groups all vary (up
+    // to 128 groups), its CUDA-core kernel (dks_mixture.cuh) for the rest (up to 64 groups); no tensor-core kernel
+    const bool mixh = ctx->act == DKS_ACT_MIX;
+    if (mixh && ctx->G > 128)
+        return fail(DKS_ERR_UNSUPPORTED, "mixture head: %d groups; it covers at most 128", ctx->G);
+    if (mixh && ctx->kernel_choice == DKS_KERNEL_TCGEN05)
+        return fail(DKS_ERR_UNSUPPORTED, "mixture head: no tensor-core kernel (kernel 'auto', 'shared' or 'simt')");
     if (ctx->G > 64 && ext_z != nullptr)
         return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups: caller-supplied per-instance plans are not supported");
     // per-instance plans of 65..128 groups (two-word rows): binary-logistic, identity or exp head, CUDA-core kernel
@@ -381,7 +414,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
                        (mc || tabled) && G >= 2 && G <= 128 && ctx->plan_mode == 0 &&
                        pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) && (!mc || ctx->h_smx[G].dm != nullptr) &&
                        (!expo || ctx->h_expl[G] != nullptr);
-    if (kernel == DKS_KERNEL_SHARED && !fast && !multi && ext_z == nullptr && pg.z != nullptr)
+    // mixture head, up to 128 groups: one pass of the member head's coalition kernel per member, added times pi_k into one
+    // set of sums -- binary members the binary head's (sum p1, sum p0) and its solves, the others the per-class sums
+    const bool mixbin = mix_binary(ctx);
+    const bool mixs = mixh && (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr && G >= 2 &&
+                      G <= 128 && ctx->plan_mode == 0 && pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) &&
+                      ctx->mixp_M == G;
+    if (kernel == DKS_KERNEL_SHARED && !fast && !multi && !mixs && ext_z == nullptr && pg.z != nullptr)
         return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head, or the softmax / one-vs-rest / "
                     "identity / exp head with at most 128 groups");
     // l1 feature selection: on the shared-plan path when M = G selects, and on the general list (CUDA-core kernel for the
@@ -394,7 +433,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     int l1_Mmax = 0;                     // largest M < G that selects
     for (int M = 2; M < G && M <= DKS_L1_MAX_GROUPS; ++M) if (selects(M)) l1_Mmax = M;
     const bool l1_gen = l1_Mmax > 0;
-    const int l1_nout = (mc || tabled) ? ctx->C : 1;
+    const int l1_nout = (mc || tabled || (mixh && !mix_binary(ctx))) ? ctx->C : 1;
     size_t l1_smem = 0;
     ctx->l1_timing_valid = false;
     if (l1) {
@@ -402,9 +441,9 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
         if (l1_full && pg.W > 2)
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
-        if (l1_full && (!(fast || multi) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S))
+        if (l1_full && (!(fast || multi || mixs) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S))
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax, "
-                        "one-vs-rest, identity or exp head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
+                        "one-vs-rest, identity, exp or mixture head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
         if (l1_gen) {
             if (G > 64)
                 return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection for partial varying sets covers at most 64 groups (G=%d)", G);
@@ -416,7 +455,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
                                    ctx->h_plans[M].z == nullptr || ctx->h_plans[M].S != ctx->h_l1[M].S))
                     return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared plan of M=%d and its l1 tables "
                                 "(dks_set_l1_tables)", M);
-            l1_smem = dks::simt_smem_bytes(S_cap, ctx->N, l1_Mmax, mc ? ctx->R : 1, mc ? ctx->C : 1);
+            l1_smem = mixh ? dks::mix::smem_bytes(S_cap, ctx->N, l1_Mmax, ctx->mix, ctx->C)
+                           : dks::simt_smem_bytes(S_cap, ctx->N, l1_Mmax, mc ? ctx->R : 1, mc ? ctx->C : 1);
             if ((long long)l1_smem > (long long)ctx->max_smem_optin)
                 return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the CUDA-core kernel's staging of instances with up to "
                             "%d varying groups needs %zu B of shared memory (> %d)", l1_Mmax, l1_smem, ctx->max_smem_optin);
@@ -426,10 +466,10 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     }
     // non-uniform background weights: the weighted instantiations of the shared-plan kernels (dks_shared.cuh)
     const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn;
-    if (fast || multi) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
+    if (fast || multi || mixs) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
     // the general kernel below (instances that are not on the shared-plan path) forks off here and joins at the end
     cudaStream_t gstream = ctx->stream;
-    if ((fast || multi) && ctx->side_stream != nullptr) {
+    if ((fast || multi || mixs) && ctx->side_stream != nullptr) {
         CUDA_TRY(cudaEventRecord(ctx->ev_fork, ctx->stream));
         CUDA_TRY(cudaStreamWaitEvent(ctx->side_stream, ctx->ev_fork, 0));
         gstream = ctx->side_stream;
@@ -484,7 +524,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         CUDA_TRY(cudaGetLastError());
         p.list = ctx->d_idx_other;
         p.count = ctx->d_counts + 1;
-    } else if (fast) {
+    } else if (fast || (mixs && mixbin)) {
         const int S = pg.S, S_pad = pg.S_pad;
         size_t need = (size_t)n * S_pad;
         if (need > ctx->cap_sums) { TRY(dev_alloc(&ctx->d_sums, need)); ctx->cap_sums = need; ctx->epoch++; }
@@ -497,12 +537,34 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             if (need > ctx->cap_acache) { TRY(dev_alloc(&ctx->d_acache, need)); ctx->cap_acache = need; ctx->epoch++; }
             sp.acache = ctx->d_acache;
         }
-        dks::shared_path::SharedLaunch sl;
-        const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &sl);
-        if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
-        ctx->launches += nl - 1;
-        path[DKS_PATH_SHARED] = sl.regs ? DKS_SHARED_REGS : DKS_SHARED_SMEM; path[DKS_PATH_CHUNKS] = sl.chunks;
-        path[DKS_PATH_WARPS] = sl.warps; path[DKS_PATH_GRID] = sl.grid;
+        if (!mixs) {
+            dks::shared_path::SharedLaunch sl;
+            const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &sl);
+            if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
+            ctx->launches += nl - 1;
+            path[DKS_PATH_SHARED] = sl.regs ? DKS_SHARED_REGS : DKS_SHARED_SMEM; path[DKS_PATH_CHUNKS] = sl.chunks;
+            path[DKS_PATH_WARPS] = sl.warps; path[DKS_PATH_GRID] = sl.grid;
+        } else {
+            // binary members: the binary head's kernel per member, into the member buffer, then added times pi_k
+            const size_t stride = 2 * (size_t)S_pad;
+            TRY(ensure_mixscr(ctx, (size_t)n * stride));
+            const size_t xt_member = (size_t)n * ((G + 3) / 4) * 16;
+            sp.scale = -DKS_LOG2E; sp.sums = reinterpret_cast<float2*>(ctx->d_mixscr);
+            int chunks = 0, warps = 0, grid = 0;
+            for (int k = 0; k < ctx->mix.K; ++k) {
+                sp.DmT = ctx->mixp.dm[k]; sp.dme = ctx->mixp.dme[k]; sp.XT = ctx->d_XT + k * xt_member;
+                dks::shared_path::SharedLaunch sl;
+                const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream,
+                                                                       &sl);
+                if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
+                chunks += sl.chunks; warps = k == 0 ? sl.warps : std::min(warps, sl.warps); grid = std::max(grid, sl.grid);
+                TRY(launch_mix_axpy(ctx, reinterpret_cast<float*>(ctx->d_sums), ctx->mix.pif[k], k == 0, (int)stride, n));
+                ctx->launches += nl + 1;
+            }
+            ctx->launches -= 1;                      // the common tail below counts one coalition launch
+            path[DKS_PATH_SHARED] = DKS_SHARED_MIX; path[DKS_PATH_CHUNKS] = chunks;
+            path[DKS_PATH_WARPS] = warps; path[DKS_PATH_GRID] = grid;
+        }
         dks::shared_path::WlsSharedParams wp;
         wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = ctx->C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link;
         wp.uniform_w = 1; wp.sums = ctx->d_sums; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink;
@@ -555,11 +617,38 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         CUDA_TRY(cudaGetLastError());
         p.list = ctx->d_idx_other;      // the general kernel below takes the remaining instances
         p.count = ctx->d_counts + 1;
-    } else if (multi) {
+    } else if (multi || mixs) {
         const int S = pg.S, S_pad = pg.S_pad, C = ctx->C;
         dks::shared_path::HeadSource src;
         src.act = ctx->act; src.ntab = (G + 3) / 4; src.msums = nullptr; src.XT = ctx->d_XT; src.ell = ctx->h_expl[G];
-        if (mc) {
+        if (mixs) {
+            // softmax / one-vs-rest members: the class-sum kernel of the member head per member, into the member buffer,
+            // then added times pi_k into the per-class sums the solves read (HeadSource: the mixture's sums)
+            const MixHead& mh = ctx->mix;
+            const size_t need = (size_t)n * C * S_pad;
+            if (need > ctx->cap_msums) { TRY(dev_alloc(&ctx->d_msums, need)); ctx->cap_msums = need; ctx->epoch++; }
+            TRY(ensure_mixscr(ctx, need));
+            dks::multi::SoftmaxParams mp;
+            memset(&mp, 0, sizeof(mp));
+            mp.n = n; mp.N = ctx->N; mp.G = G; mp.S = S; mp.S_pad = S_pad; mp.ntab = src.ntab; mp.scale = DKS_LOG2E;
+            mp.wn = ctx->d_wn; mp.z = pg.z; mp.list = ctx->d_idx_full; mp.count = ctx->d_counts; mp.sums = ctx->d_mixscr;
+            const size_t xt_member = (size_t)n * mh.Rm * src.ntab * 16;
+            int chunks = 0, grid = 0;
+            for (int k = 0; k < mh.K; ++k) {
+                mp.dm = ctx->mixp.dm[k]; mp.lo = ctx->mixp.lo[k]; mp.XT = ctx->d_XT + k * xt_member;
+                mp.BW = ctx->d_mixBW + (size_t)k * ctx->N * G * mh.Rm; mp.scores = ctx->d_mixsc + (size_t)k * ctx->N * mh.Rm;
+                const int nl = dks::multi::launch_class_sums(mp, mh.mact == DKS_ACT_OVR, C, pg.W, n, ctx->sm_count,
+                                                             ctx->max_smem_optin, ctx->stream, &grid);
+                if (nl == 0)
+                    return fail(DKS_ERR_CUDA, "mixture member coalition kernel: %s", cudaGetErrorString(cudaGetLastError()));
+                chunks += nl;
+                TRY(launch_mix_axpy(ctx, ctx->d_msums, mh.pif[k], k == 0, C * S_pad, n));
+                ctx->launches += nl + 1;
+            }
+            path[DKS_PATH_SHARED] = DKS_SHARED_MIX; path[DKS_PATH_CHUNKS] = chunks;
+            path[DKS_PATH_WARPS] = dks::multi::MC_WARPS; path[DKS_PATH_GRID] = grid;
+            src.msums = ctx->d_msums;
+        } else if (mc) {
             // the workspace is C n S_pad floats: the engine explains these heads in row blocks of 2 / C the binary path's
             const size_t need = (size_t)n * C * S_pad;
             if (need > ctx->cap_msums) { TRY(dev_alloc(&ctx->d_msums, need)); ctx->cap_msums = need; ctx->epoch++; }
@@ -624,7 +713,8 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         ExplainParams ps = p;
         ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
         auto l1kern = expo ? dks::explain_simt_kernel<true, true> : dks::explain_simt_kernel<true>;
-        CUDA_TRY(cudaFuncSetAttribute(l1kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l1_smem));
+        CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<true> : (const void*)l1kern,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l1_smem));
         int per_sm = (int)((size_t)ctx->max_smem_optin / (l1_smem + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 8) per_sm = 8;
@@ -632,7 +722,11 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         if (grid > n) grid = n;
         const bool timed = !ctx->capturing;
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
-        l1kern<<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom}, eb);
+        if (mixh)
+            dks::mix::explain_simt_mix_kernel<true><<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
+                                                                                     ctx->mix);
+        else
+            l1kern<<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom}, eb);
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[1], gstream));
         dks::l1::Params lp = l1_params(ctx, n, l1_nout, phi_dev);
         lp.Mmax = l1_Mmax; lp.Mcnt = ctx->d_M; lp.vmask = ctx->d_vmask; lp.list = ctx->d_idx_sel; lp.count = ctx->d_l1_counts;
@@ -675,7 +769,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
             return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
         }
-        if (!fast && !multi)
+        if (!fast && !multi && !mixs)
             return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, or the "
                         "softmax / one-vs-rest / identity head up to 128 groups, or the exp head up to 128 groups; kernel "
                         "'auto' or 'shared', shared plan of M=%d uploaded)", G);
@@ -696,8 +790,9 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         TRY(dks::tc_launch(ctx, p, gstream));
         path[DKS_PATH_GENERAL] = DKS_GENERAL_TC;
     } else {
-        size_t smem = dks::simt_smem_bytes(S_cap, ctx->N, ctx->G, mc ? ctx->R : 1, mc ? ctx->C : 1);
-        if ((long long)smem > (long long)ctx->max_smem_optin && (fast || multi)) {
+        size_t smem = mixh ? dks::mix::smem_bytes(S_cap, ctx->N, ctx->G, ctx->mix, ctx->C)
+                           : dks::simt_smem_bytes(S_cap, ctx->N, ctx->G, mc ? ctx->R : 1, mc ? ctx->C : 1);
+        if ((long long)smem > (long long)ctx->max_smem_optin && (fast || multi || mixs)) {
             // the shared-plan path took the instances whose groups all vary; the general kernel is sized for the largest
             // plan set and cannot hold it.  The instances left for it (often none) are reported, not computed.
             dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(p.count, G, ctx->d_status);
@@ -710,7 +805,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         }
         if ((long long)smem > (long long)ctx->max_smem_optin && !multi && pg.z == nullptr &&
             (kernel_req == DKS_KERNEL_AUTO || kernel_req == DKS_KERNEL_SHARED) && ext_z == nullptr && ctx->plan_mode == 0 &&
-            (mc || tabled) && G >= 2 && G <= 128) {
+            (mc || tabled || mixh) && G >= 2 && G <= 128) {
             // the softmax / one-vs-rest / identity / exp head's shared-plan path takes these instances once the plan of G
             // groups is uploaded
             ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
@@ -720,13 +815,15 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
             return fail(DKS_ERR_UNSUPPORTED, "SIMT kernel needs %zu B of shared memory (> %d): N*G or nsamples too large",
                         smem, ctx->max_smem_optin);
         auto skern = expo ? dks::explain_simt_kernel<false, true> : dks::explain_simt_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(skern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<false> : (const void*)skern,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int per_sm = (int)((size_t)ctx->max_smem_optin / (smem + 1024));
         if (per_sm < 1) per_sm = 1;
         if (per_sm > 8) per_sm = 8;
         int grid = ctx->sm_count * per_sm;
         if (grid > n) grid = n;
-        skern<<<grid, 256, smem, gstream>>>(p, dks::SimtL1{}, eb);
+        if (mixh) dks::mix::explain_simt_mix_kernel<false><<<grid, 256, smem, gstream>>>(p, dks::SimtL1{}, ctx->mix);
+        else skern<<<grid, 256, smem, gstream>>>(p, dks::SimtL1{}, eb);
         ctx->launches += 1;
         path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT;
     }
@@ -748,6 +845,26 @@ int check_status(dks_ctx* ctx) {
         return fail(DKS_ERR_NUMERIC, "normal matrix not positive definite, or (exp head) a model output that is not finite "
                     "(instance/M %d)", ctx->h_status[1]);
     return fail(ctx->h_status[0], "explain kernel reported status %d (detail %d)", ctx->h_status[0], ctx->h_status[1]);
+}
+
+// projection form of the shared-plan solve of the binary head (and of binary mixtures): P = inv(E^T W E) E^T W and d = P z_L,
+// when it fits the solve kernel's staging
+int build_pmat(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz, const double* dw, const double* di) {
+    if (!(pd.W == 1 && M - 1 <= dks::shared_path::PMAT_MAXK &&
+          dks::shared_path::wls_pmat_smem(M, pd.S_pad, false) + 8192 <= (size_t)ctx->max_smem_optin))
+        return DKS_OK;
+    const int S = pd.S;
+    float* pm = nullptr; double* dv = nullptr;
+    CUDA_TRY(cudaMalloc((void**)&pm, sizeof(float) * (size_t)(M - 1) * pd.S_pad));
+    CUDA_TRY(cudaMalloc((void**)&dv, sizeof(double) * (M - 1)));
+    ctx->plan_allocs[M].push_back(pm); ctx->plan_allocs[M].push_back(dv);
+    long long tot = (long long)(M - 1) * pd.S_pad;
+    dks::shared_path::plan_pmat_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(dz, dw, di, S, pd.S_pad, M, pm);
+    dks::shared_path::plan_dvec_kernel<<<M - 1, 32, 0, ctx->stream>>>(dz, pm, S, pd.S_pad, M, dv);
+    ctx->launches += 2;
+    CUDA_TRY(cudaGetLastError());
+    pd.pmat = pm; pd.dvec = dv;
+    return DKS_OK;
 }
 
 // Chebyshev nodes of [0, 1] and the inverse of their Vandermonde matrix (Gauss-Jordan, partial pivoting)
@@ -909,7 +1026,8 @@ int dks_destroy(dks_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
-    dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b);
+    dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b); dev_free(&ctx->d_mix);
+    dev_free(&ctx->d_mixBW); dev_free(&ctx->d_mixsc); dev_free(&ctx->d_mixscr);
     if (ctx->cm.hdr) { cudaFree((void*)ctx->cm.hdr); cudaFree((void*)ctx->cm.keys); cudaFree((void*)ctx->cm.vals); }
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
@@ -986,6 +1104,7 @@ int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int 
     REQUIRE(ctx->D > 0, "dks_set_model: call dks_set_background first (D unknown)");
     REQUIRE(W_host && b_host && R > 0, "dks_set_model: need W, b, R > 0");
     if (R > 8) return fail(DKS_ERR_UNSUPPORTED, "dks_set_model: R=%d score rows; at most 8 supported", R);
+    if (activation == DKS_ACT_MIX) return fail(DKS_ERR_INVALID, "dks_set_model: the mixture head is set by dks_set_mixture");
     if (activation == DKS_ACT_BINARY_LOGISTIC) {
         REQUIRE(R == 1, "binary-logistic head needs R == 1 (got %d)", R);
         REQUIRE(kappa > 0, "binary-logistic head needs kappa > 0");
@@ -1007,6 +1126,43 @@ int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int 
     }
     ctx->R = R; ctx->act = activation; ctx->kappa = kappa; ctx->scalar_out = scalar_out;
     ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();   // maps belong to one model
+    ctx->h_W.assign(W_host, W_host + (size_t)R * ctx->D);
+    ctx->h_b.assign(b_host, b_host + R);
+    ctx->fitted = false;
+    return DKS_OK;
+}
+
+int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* W_host, const double* b_host,
+                    const double* pi_host, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_mixture: call dks_set_background first (D unknown)");
+    REQUIRE(W_host && b_host && pi_host, "dks_set_mixture: need W, b, pi");
+    REQUIRE(K >= 2, "dks_set_mixture: K=%d members; a single model is set by dks_set_model", K);
+    if (member_act == DKS_ACT_BINARY_LOGISTIC) {
+        REQUIRE(R_m == 1, "dks_set_mixture: binary-logistic members have one score row (got %d)", R_m);
+    } else if (member_act == DKS_ACT_SOFTMAX || member_act == DKS_ACT_OVR) {
+        if (R_m < 3 || R_m > 8)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_mixture: softmax / one-vs-rest members over %d classes; 3..8 supported", R_m);
+    } else {
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mixture: member head %d; binary-logistic, softmax or one-vs-rest only",
+                    member_act);
+    }
+    if ((long long)K * R_m > DKS_MIX_MAX_R)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mixture: %d members x %d score rows exceed %d rows", K, R_m, DKS_MIX_MAX_R);
+    double sum = 0.0;
+    for (int k = 0; k < K; ++k) {
+        REQUIRE(std::isfinite(pi_host[k]) && pi_host[k] > 0.0, "dks_set_mixture: pi[%d] = %g must be positive and finite", k,
+                pi_host[k]);
+        sum += pi_host[k];
+    }
+    const int R = K * R_m;
+    MixHead mh = {};
+    mh.K = K; mh.Rm = R_m; mh.mact = member_act;
+    for (int k = 0; k < K; ++k) { mh.pi[k] = pi_host[k] / sum; mh.pif[k] = (float)mh.pi[k]; }
+    ctx->mix = mh;
+    ctx->C = member_act == DKS_ACT_BINARY_LOGISTIC ? 2 : R_m;
+    ctx->R = R; ctx->act = DKS_ACT_MIX; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
+    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
     ctx->h_W.assign(W_host, W_host + (size_t)R * ctx->D);
     ctx->h_b.assign(b_host, b_host + R);
     ctx->fitted = false;
@@ -1102,7 +1258,9 @@ int dks_fit(dks_ctx* ctx) {
     TRY(dev_alloc(&ctx->d_bases, (size_t)N * R));
     TRY(dev_alloc(&ctx->d_wbf, (size_t)N));
     TRY(dev_alloc(&ctx->d_wn, (size_t)N));
+    TRY(dev_alloc(&ctx->d_mix, (size_t)1));
     cudaStream_t st = ctx->stream;
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_mix, &ctx->mix, sizeof(MixHead), cudaMemcpyHostToDevice, st));
     const bool maps = !ctx->h_cm_hdr.empty();
     {
         int* hdr = const_cast<int*>(ctx->cm.hdr);
@@ -1136,13 +1294,21 @@ int dks_fit(dks_ctx* ctx) {
     CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
 
     ctx->scale = (ctx->act == DKS_ACT_BINARY_LOGISTIC) ? -ctx->kappa * 1.4426950408889634
-               : (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_EXP) ? 1.4426950408889634 : 1.0;
-    (maps ? dks::fit_bw_kernel<true> : dks::fit_bw_kernel<false>)<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(
+               : (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_EXP || ctx->act == DKS_ACT_MIX)
+                   ? 1.4426950408889634 : 1.0;
+    (maps ? (R > 8 ? dks::fit_bw_kernel<true, true> : dks::fit_bw_kernel<true>) : dks::fit_bw_kernel<false>)<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(
         ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D, G, R, ctx->d_BW, ctx->cm, ctx->d_status);
     dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
+    if (ctx->act == DKS_ACT_MIX) {
+        TRY(dev_alloc(&ctx->d_mixBW, (size_t)N * G * R));
+        TRY(dev_alloc(&ctx->d_mixsc, (size_t)N * R));
+        dks::mix::mix_split_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, N, G, ctx->mix.K,
+                                                                                    ctx->mix.Rm, ctx->d_mixBW, ctx->d_mixsc);
+        ctx->launches += 1;
+    }
     dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
     dks::fit_fnull_kernel<<<1, 256, 0, st>>>(ctx->d_scores, ctx->d_BW, ctx->d_wbg, N, G, R, C, ctx->act, ctx->kappa,
-                                              ctx->link, ctx->d_fnull, ctx->d_linkfnull, ctx->d_Bbar);
+                                              ctx->link, ctx->d_fnull, ctx->d_linkfnull, ctx->d_Bbar, ctx->d_mix);
     dks::fit_scale_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, G, R,
                                                                               ctx->scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf,
                                                                               ctx->act == DKS_ACT_EXP ? 1 : 0);
@@ -1168,6 +1334,7 @@ int dks_fit(dks_ctx* ctx) {
         memset(ctx->h_l1, 0, sizeof(ctx->h_l1));
         memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
         memset(ctx->h_expl, 0, sizeof(ctx->h_expl));
+        ctx->mixp = {}; ctx->mixp_M = 0;
         ctx->max_plan_S = 0;
         CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));
         TRY(sync_l1_tables(ctx));
@@ -1204,7 +1371,7 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
     (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
-        dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status);
+        dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status, ctx->d_mix);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(out_host, dO, sizeof(double) * n * ctx->C, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1243,6 +1410,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
         memset(&ctx->h_l1[M], 0, sizeof(ctx->h_l1[M]));
         memset(&ctx->h_smx[M], 0, sizeof(ctx->h_smx[M]));
         ctx->h_expl[M] = nullptr;
+        if (ctx->mixp_M == M) { ctx->mixp = {}; ctx->mixp_M = 0; }
         ctx->h_afix[M] = nullptr;
         ctx->epoch++;
         TRY(sync_l1_tables(ctx));
@@ -1304,20 +1472,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
         CUDA_TRY(cudaGetLastError());
         pd.dme = dme;
         pd.dmT = dm;
-        // projection form of the solve: P = inv(E^T W E) E^T W and d = P z_L
-        if (W == 1 && M - 1 <= dks::shared_path::PMAT_MAXK &&
-            dks::shared_path::wls_pmat_smem(M, pd.S_pad, false) + 8192 <= (size_t)ctx->max_smem_optin) {
-            float* pm = nullptr; double* dv = nullptr;
-            CUDA_TRY(cudaMalloc((void**)&pm, sizeof(float) * (size_t)(M - 1) * pd.S_pad));
-            CUDA_TRY(cudaMalloc((void**)&dv, sizeof(double) * (M - 1)));
-            ctx->plan_allocs[M].push_back(pm); ctx->plan_allocs[M].push_back(dv);
-            long long tot = (long long)(M - 1) * pd.S_pad;
-            dks::shared_path::plan_pmat_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(dz, dw, di, S, pd.S_pad, M, pm);
-            dks::shared_path::plan_dvec_kernel<<<M - 1, 32, 0, ctx->stream>>>(dz, pm, S, pd.S_pad, M, dv);
-            ctx->launches += 2;
-            CUDA_TRY(cudaGetLastError());
-            pd.pmat = pm; pd.dvec = dv;
-        }
+        TRY(build_pmat(ctx, pd, M, dz, dw, di));
         // float64 P, row-major per coalition, for the fused kernel (link + solve inside the coalition kernel)
         if (W == 1 && M <= 16) {
             const int kpad = dks::shared_path::fused_kpad(M);
@@ -1333,6 +1488,45 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
             pd.pmat64 = pm64; pd.dvec64 = dv64; pd.kpad = kpad;
             if (ctx->N <= dks::shared_path::MAXN) TRY(build_link_table(ctx, pd, M, dz));
         }
+    }
+    if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_MIX && W <= 2) {
+        // mixture head: each member's tables from its own rows of the background (dks_fit split them per member) -- binary
+        // members the binary head's Dm / dme and projection, softmax / one-vs-rest members the class-sum tables
+        const MixHead& mh = ctx->mix;
+        const int N = ctx->N, Rm = mh.Rm, CS = mh.mact == DKS_ACT_OVR ? Rm + 1 : Rm;
+        const bool bin = mh.mact == DKS_ACT_BINARY_LOGISTIC;
+        dks_ctx::MixPlanDev mp = {};
+        for (int k = 0; k < mh.K; ++k) {
+            const double* BWk = ctx->d_mixBW + (size_t)k * N * M * Rm;
+            const double* sck = ctx->d_mixsc + (size_t)k * N * Rm;
+            if (bin) {
+                float* dm = nullptr; double* dme = nullptr;
+                CUDA_TRY(cudaMalloc((void**)&dm, sizeof(float) * (size_t)N * pd.S_pad));
+                CUDA_TRY(cudaMalloc((void**)&dme, sizeof(double) * (size_t)pd.S_pad));
+                ctx->plan_allocs[M].push_back(dm); ctx->plan_allocs[M].push_back(dme);
+                const long long total = (long long)N * pd.S_pad;
+                dks::shared_path::plan_dme_kernel<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, W, S, pd.S_pad, BWk, sck, N, M,
+                                                                                               -DKS_LOG2E, dme);
+                dks::shared_path::plan_dm_kernel<<<cdiv(total, 256), 256, 0, ctx->stream>>>(dz, W, S, pd.S_pad, BWk, sck, N, M,
+                                                                                              -DKS_LOG2E, dme, dm);
+                ctx->launches += 2;
+                mp.dm[k] = dm; mp.dme[k] = dme;
+            } else {
+                float* sd = nullptr; float* sl = nullptr;
+                CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)CS * N * pd.S_pad));
+                ctx->plan_allocs[M].push_back(sd);
+                CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)CS * pd.S_pad));
+                ctx->plan_allocs[M].push_back(sl);
+                auto kern = mh.mact == DKS_ACT_OVR ? (W == 1 ? dks::multi::plan_ovr_kernel<1> : dks::multi::plan_ovr_kernel<2>)
+                                                   : (W == 1 ? dks::multi::plan_softmax_kernel<1> : dks::multi::plan_softmax_kernel<2>);
+                kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, BWk, sck, N, M, Rm, DKS_LOG2E, sd, sl);
+                ctx->launches += 1;
+                mp.dm[k] = sd; mp.lo[k] = sl;
+            }
+            CUDA_TRY(cudaGetLastError());
+        }
+        if (bin) TRY(build_pmat(ctx, pd, M, dz, dw, di));
+        ctx->mixp = mp; ctx->mixp_M = M;
     }
     if (M == ctx->G && ctx->fitted && (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR) && W <= 2) {
         // softmax / one-vs-rest head: per-class Dm table and row bounds for the full varying set (dks_multi.cuh); the
@@ -1383,6 +1577,7 @@ int dks_clear_plans(dks_ctx* ctx) {
     memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
     memset(ctx->h_expl, 0, sizeof(ctx->h_expl));
     memset(ctx->h_afix, 0, sizeof(ctx->h_afix));
+    ctx->mixp = {}; ctx->mixp_M = 0;
     memset(ctx->h_sinfo, 0, sizeof(ctx->h_sinfo));
     ctx->max_plan_S = 0;
     CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));

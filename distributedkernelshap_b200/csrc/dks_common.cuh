@@ -130,6 +130,17 @@ struct ExpBackground {
     const double* scores; // [N]    background scores
 };
 
+// mixture head (dks_set_mixture, DESIGN.md §5.0.10): outputs sum_k pi_k h(z_k), K members of R_m score rows each, stacked
+// member-major (row k R_m + q), all with the member head h (binary-logistic with kappa folded into the scores, softmax or
+// one-vs-rest); K R_m <= DKS_MIX_MAX_R
+#define DKS_MIX_MAX_R 32
+#define DKS_LOG2E 1.4426950408889634
+struct MixHead {
+    int K, Rm, mact;             // members, score rows per member, member head (DKS_ACT_*)
+    float pif[DKS_MIX_MAX_R];    // pi_k in float (the CUDA-core kernel's fp32 sums)
+    double pi[DKS_MIX_MAX_R];    // pi_k > 0, sum 1
+};
+
 // exp head, CUDA-core kernels (DESIGN.md §5.0.8): a coalition row is summed in fp32 when the largest weighted background
 // exponent t'_j = log2 e d(s, j) + log2 w_j lies in [EXP_T_LO, EXP_T_HI]; other rows are evaluated in float64
 #define DKS_EXP_T_LO -60.f
@@ -159,6 +170,17 @@ struct dks_ctx {
     float* dbg_time = nullptr;  // [6][256] clock64 timeline of CTA 0 (debug kernel variant)
 
     // host copies
+    MixHead mix = {};           // mixture head (act == DKS_ACT_MIX): members and weights
+    MixHead* d_mix = nullptr;   // its device copy (stage 1 and the fit kernels evaluate f(x) in float64 from it)
+    double* d_mixBW = nullptr;  // [K][N][G][R_m] the background contributions split per member (plan tables of each member)
+    double* d_mixsc = nullptr;  // [K][N][R_m] the background scores split per member
+    // mixture head, full varying set (M == G <= 128): each member's shared-plan tables -- binary members the binary head's
+    // Dm / dme, softmax and one-vs-rest members the class-sum tables (SmxDev); owned by plan_allocs[mixp_M]
+    struct MixPlanDev { const float* dm[DKS_MIX_MAX_R]; const double* dme[DKS_MIX_MAX_R]; const float* lo[DKS_MIX_MAX_R]; };
+    MixPlanDev mixp = {};
+    int mixp_M = 0;             // the M the member tables belong to (0: none)
+    float* d_mixscr = nullptr;  // one member's sums before they are added, times pi_k, into the mixture's sums
+    size_t cap_mixscr = 0;
     std::vector<double> h_bg, h_wbg, h_W, h_b;
     std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
     std::vector<double> h_cm_keys, h_cm_vals;

@@ -91,6 +91,17 @@ __device__ inline void head_f64(const double* z, int R, int act, double kappa, d
     }
 }
 
+// mixture head in float64: sum_k pi_k h(z_k) over the members' score rows z[k R_m ..] (2 outputs for binary members, else R_m)
+__device__ inline void mix_head_f64(const double* z, const MixHead& mh, double* out) {
+    const int Co = mh.mact == DKS_ACT_BINARY_LOGISTIC ? 2 : mh.Rm;
+    for (int c = 0; c < Co; ++c) out[c] = 0.0;
+    for (int k = 0; k < mh.K; ++k) {
+        double o[8];
+        head_f64(z + (size_t)k * mh.Rm, mh.Rm, mh.mact, 1.0, o);
+        for (int c = 0; c < Co; ++c) out[c] = fma(mh.pi[k], o[c], out[c]);
+    }
+}
+
 // column maps: adds f_col(x), the R score contributions of one raw value, to acc.  A binary search over the column's
 // breakpoints (numpy's searchsorted side='right': a value on a breakpoint takes the piece on its right) then R FMAs, or over
 // its keys (exact match, else the unknown row) then R loads.  Returns false, adding nothing, where the map's policy is
@@ -130,7 +141,8 @@ __device__ __forceinline__ void cm_report(int* status, int row) {
 // K0: fit (DenseData + KernelExplainer.__init__)
 // ------------------------------------------------------------------------------------------------------
 // BW[j][g][r] = sum_{col in g} bg[j][col] * W[r][col]; MAPS: sum_{col in g} f_{r,col}(bg[j][col]) (column maps)
-template <bool MAPS>
+// WIDE: up to DKS_MIX_MAX_R score rows per column map (a pipeline ending in a mixture head); the other instantiation eight
+template <bool MAPS, bool WIDE = false>
 __global__ void fit_bw_kernel(const double* __restrict__ bg, const double* __restrict__ W,
                               const int32_t* __restrict__ goff, const int32_t* __restrict__ gcols, int N, int D,
                               int G, int R, double* __restrict__ BW, ColumnMapsDev cm, int* __restrict__ status) {
@@ -138,7 +150,7 @@ __global__ void fit_bw_kernel(const double* __restrict__ bg, const double* __res
     if (idx >= N * G * R) return;
     int r = idx % R, g = (idx / R) % G, j = idx / (R * G);
     if (MAPS) {
-        double acc[8];
+        double acc[WIDE ? DKS_MIX_MAX_R : 8];     // every score row of the column
         for (int q = 0; q < R; ++q) acc[q] = 0;
         for (int c = goff[g]; c < goff[g + 1]; ++c) {
             const int col = gcols[c];
@@ -183,13 +195,14 @@ __global__ void fit_colstats_kernel(const double* __restrict__ bg, int N, int D,
 __global__ void fit_fnull_kernel(const double* __restrict__ scores, const double* __restrict__ BW,
                                  const double* __restrict__ wbg, int N, int G, int R, int C, int act, double kappa,
                                  int link, double* __restrict__ fnull, double* __restrict__ linkfnull,
-                                 double* __restrict__ Bbar) {
+                                 double* __restrict__ Bbar, const MixHead* __restrict__ mix) {
     int t = threadIdx.x;
     if (t < C) {
         double acc = 0;
         for (int j = 0; j < N; ++j) {
             double out[DKS_MAX_OUT];
-            head_f64(scores + (size_t)j * R, R, act, kappa, out);
+            if (act == DKS_ACT_MIX) mix_head_f64(scores + (size_t)j * R, *mix, out);
+            else head_f64(scores + (size_t)j * R, R, act, kappa, out);
             acc += out[t] * wbg[j];
         }
         fnull[t] = acc;
@@ -224,7 +237,8 @@ __global__ void fit_scale_kernel(const double* __restrict__ BW, const double* __
 template <bool MAPS>
 __global__ void predict_kernel(const double* __restrict__ X, const double* __restrict__ W,
                                const double* __restrict__ b, int n, int D, int R, int C, int act, double kappa,
-                               double* __restrict__ out, ColumnMapsDev cm, int* __restrict__ status) {
+                               double* __restrict__ out, ColumnMapsDev cm, int* __restrict__ status,
+                               const MixHead* __restrict__ mix) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     double z[DKS_MAX_OUT], o[DKS_MAX_OUT];
@@ -239,7 +253,8 @@ __global__ void predict_kernel(const double* __restrict__ X, const double* __res
             z[r] = acc;
         }
     }
-    head_f64(z, R, act, kappa, o);
+    if (act == DKS_ACT_MIX) mix_head_f64(z, *mix, o);
+    else head_f64(z, R, act, kappa, o);
     for (int c = 0; c < C; ++c) out[(size_t)i * C + c] = o[c];
 }
 
@@ -269,7 +284,9 @@ __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
 // MAPS: the contributions come from the column maps `cm` instead of W -- per column a binary search and R FMAs or loads
 // (cm_add); STAGE then stages the maps' tables where W would be.  A raw value a map refuses is reported as DKS_ERR_DOMAIN
 // with the instance index and contributes nothing.
-template <bool STAGE, bool MAPS>
+// MIX: the mixture head (up to DKS_MIX_MAX_R score rows; f(x) = sum_k pi_k h(z_k) from `mix`).  The other instantiations
+// hold eight rows and never read `mix`.
+template <bool STAGE, bool MAPS, bool MIX = false>
 __global__ void prep_kernel(const double* __restrict__ X, const double* __restrict__ W, const double* __restrict__ b,
                             const double* __restrict__ bg, const int32_t* __restrict__ goff,
                             const int32_t* __restrict__ gcols, const double* __restrict__ colmin,
@@ -279,7 +296,8 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
                             int* __restrict__ Mcnt, double* __restrict__ dlink, int* __restrict__ hist,
                             int* __restrict__ counts, int* __restrict__ idx_full, int* __restrict__ idx_other,
                             double* __restrict__ XT, double xt_scale, const double* __restrict__ xt_sub,
-                            int* __restrict__ status, ColumnMapsDev cm) {
+                            int* __restrict__ status, ColumnMapsDev cm, const MixHead* __restrict__ mix) {
+    constexpr int RMAX = MIX ? DKS_MIX_MAX_R : 8;
     extern __shared__ __align__(16) unsigned char prep_smem[];
     double* sXW = reinterpret_cast<double*>(prep_smem);                        // [ipb][G][R]
     double* sX = sXW + (size_t)ipb * G * R;                                    // STAGE: [ipb][D]
@@ -313,7 +331,7 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
         const int li = idx / G, g = idx - li * G, i = i0 + li;
         if (i >= n) continue;
         bool varies = false;
-        double acc[8];
+        double acc[RMAX];
         for (int r = 0; r < R; ++r) acc[r] = 0;
         const int c0 = STAGE ? sOff[g] : goff[g], c1 = STAGE ? sOff[g + 1] : goff[g + 1];
         for (int c = c0; c < c1; ++c) {
@@ -359,7 +377,9 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
                     acc += xt_sub != nullptr ? sXW[((size_t)li * G + k) * R + r] - xt_sub[(size_t)k * R + r]
                                              : sXW[((size_t)li * G + k) * R + r];
                 }
-            XT[(((size_t)i * R + r) * ntab + t) * 16 + x] = xt_scale * acc;
+            // MIX: member-major [K][n][R_m][ntab][16], so that a member's tables are the layout of the single-model head
+            const size_t row = MIX ? ((size_t)(r / mix->Rm) * n + i) * mix->Rm + r % mix->Rm : (size_t)i * R + r;
+            XT[(row * ntab + t) * 16 + x] = xt_scale * acc;
         }
     }
     for (int li = threadIdx.x; li < ipb; li += blockDim.x) {
@@ -367,7 +387,7 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
         if (i >= n) continue;
         uint64_t m = 0;                       // varying bit-mask (groups 0..63; wider problems only use the count)
         int M = 0;
-        double z[8], o[DKS_MAX_OUT];
+        double z[RMAX], o[DKS_MAX_OUT];
         for (int r = 0; r < R; ++r) z[r] = b[r];
         for (int g = 0; g < G; ++g) {
             if (sflag[li * G + g]) { if (g < 64) m |= (1ull << g); ++M; }
@@ -379,7 +399,8 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
         // bucket: all groups vary (candidates for the shared-plan fast path) / everything else
         if (M == G && M >= 2) idx_full[atomicAdd(&counts[0], 1)] = i;
         else idx_other[atomicAdd(&counts[1], 1)] = i;
-        head_f64(z, R, act, kappa, o);
+        if constexpr (MIX) mix_head_f64(z, *mix, o);
+        else head_f64(z, R, act, kappa, o);
         for (int c = 0; c < C; ++c) dlink[(size_t)i * C + c] = link_f(o[c], link) - linkfnull[c];
         // exp head: f(x) = exp(z) overflows for z > 709.78; the explain kernels then never write this instance's phi
         if (act == DKS_ACT_EXP && !isfinite(o[0]) && atomicCAS(&status[0], 0, DKS_ERR_NUMERIC) == 0) status[1] = i;

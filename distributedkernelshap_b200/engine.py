@@ -41,11 +41,14 @@ def device_sampling_supported(M, n_sizes):
     return M <= 128 and n_sizes <= MAX_SAMPLED_SIZES
 
 
-def rows_per_call(act_code, n_outputs, plan_mode, G):
+def rows_per_call(act_code, n_outputs, plan_mode, G, score_rows=1):
     """Rows per C-ABI call.  The softmax and one-vs-rest heads' shared-plan path keeps C per-class sums per coalition
     where the binary head keeps two: their row blocks are 2 / C as long, so that the per-call workspace stays the binary
-    path's.  Per-instance plans of more than 64 groups: ``MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE`` (plans are keyed by the
-    global row, so results do not depend on the block size)."""
+    path's.  The mixture head keeps ``score_rows`` = K R_m nibble tables per instance and, on its shared-plan route, a
+    member's sums next to the mixture's: its blocks are 1 / (K R_m) as long.  Per-instance plans of more than 64 groups: ``MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE`` (plans
+    are keyed by the global row, so results do not depend on the block size)."""
+    if act_code == _cabi.ACT_MIX:
+        return MAX_ROWS_PER_CALL // max(1, score_rows)
     if act_code in (_cabi.ACT_SOFTMAX, _cabi.ACT_OVR) and n_outputs > 2:
         return MAX_ROWS_PER_CALL * 2 // n_outputs
     if plan_mode == "per_instance" and G > 64:
@@ -182,8 +185,14 @@ class GpuKernelExplainer:
         _cabi.check(self.lib.dks_set_groups(self._ctx, _cabi.ptr(offsets), _cabi.ptr(cols), self.data.groups_size))
         maps = self.spec.maps
         W = self.spec.W if maps is None else np.zeros((self.spec.R, self.P))    # not read once the maps are set
-        _cabi.check(self.lib.dks_set_model(self._ctx, _cabi.ptr(W), _cabi.ptr(self.spec.b), self.spec.R,
-                                           self.spec.act_code, self.spec.kappa, int(self.spec.scalar_out)))
+        if self.spec.activation == "mixture":
+            member = {"binary_logistic": _cabi.ACT_BINARY_LOGISTIC, "softmax": _cabi.ACT_SOFTMAX,
+                      "ovr": _cabi.ACT_OVR}[self.spec.member]
+            _cabi.check(self.lib.dks_set_mixture(self._ctx, self.spec.K, member, self.spec.R // self.spec.K, _cabi.ptr(W),
+                                                 _cabi.ptr(self.spec.b), _cabi.ptr(self.spec.pi), int(self.spec.scalar_out)))
+        else:
+            _cabi.check(self.lib.dks_set_model(self._ctx, _cabi.ptr(W), _cabi.ptr(self.spec.b), self.spec.R,
+                                               self.spec.act_code, self.spec.kappa, int(self.spec.scalar_out)))
         if maps is not None:
             _cabi.check(self.lib.dks_set_column_maps(self._ctx, maps.D, maps.R, _cabi.ptr(maps.hdr), _cabi.ptr(maps.keys),
                                                      len(maps.keys), _cabi.ptr(maps.vals), len(maps.vals)))
@@ -438,7 +447,7 @@ class GpuKernelExplainer:
 
     def _rows_per_call(self):
         """Rows per C-ABI call (``rows_per_call``)."""
-        return rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size)
+        return rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size, self.spec.R)
 
     def link_predictions(self):
         """``link(f(x))`` of the rows of the last ``shap_values`` call, ``[n, C]`` (``[n]`` for scalar-output models):
@@ -618,7 +627,7 @@ class GpuKernelExplainer:
         return {"prepare": float(out[0]), "coalitions": float(out[1]), "total": float(out[2])}
 
     _PATH_NAMES = {
-        "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp"),
+        "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp", "mixture"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
         "general": ("none", "tc", "simt", "flagged", "simt_wide"),
     }

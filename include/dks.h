@@ -55,6 +55,17 @@ extern "C" {
                                  * ln sum_j w_j exp(d(s, j)) computed once per plan (DKS_SHARED_EXP); the CUDA-core kernels
                                  * sum 2^t over the background in fp32 and send rows outside their range rule to float64
                                  * (DESIGN.md §5.0.8); no tensor-core kernel */
+#define DKS_ACT_MIX 5           /* mixture: outputs sum_k pi_k h(z_k) over K >= 2 members that share one member head h
+                                 * (binary-logistic, outputs [1 - p, p]; softmax or one-vs-rest over 3..8 classes), z_k = W_k x
+                                 * + b_k.  scikit-learn's CalibratedClassifierCV(method='sigmoid'), soft-voting and bagging
+                                 * ensembles of linear classifiers.  Set by dks_set_mixture only (dks_set_model refuses it).
+                                 * Shared plans with every group varying (G <= 128): one pass of the member head's
+                                 * coalition kernel per member, each member's sums added times pi_k into one set of sums,
+                                 * then the member head's solves and l1 selection (DKS_SHARED_MIX).  The rest (partial
+                                 * varying sets, per-instance or caller-supplied plans, kernel 'simt'; up to 64 groups): a
+                                 * CUDA-core kernel evaluating every member's head per element.  More than 128 groups, the
+                                 * tensor-core kernel and per-instance plans of 65..128 groups are DKS_ERR_UNSUPPORTED
+                                 * (DESIGN.md §5.0.10) */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -93,6 +104,13 @@ int dks_set_groups(dks_ctx* ctx, const int32_t* group_offsets, const int32_t* gr
  * 1-D array (vector_out False). */
 int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int R, int activation, double kappa,
                   int scalar_out);
+/* mixture head (DKS_ACT_MIX) in place of dks_set_model: K >= 2 members with the member head member_act (DKS_ACT_BINARY_LOGISTIC
+ * with R_m = 1 and kappa 1 -- fold kappa into W and b --, DKS_ACT_SOFTMAX or DKS_ACT_OVR with R_m = 3..8), K R_m <= 32 score
+ * rows.  W_host [K R_m x D] and b_host [K R_m], member-major (row k R_m + q is row q of member k); pi_host [K] positive
+ * finite weights, normalised to sum 1.  Outputs: 2 for binary members, R_m otherwise.  dks_set_column_maps may follow with
+ * R = K R_m. */
+int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* W_host, const double* b_host,
+                    const double* pi_host, int scalar_out);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
  * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
  * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
@@ -280,6 +298,9 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_SHARED_AFFINE 5      /* identity head: y read from per-class tables, no coalition kernel */
 #define DKS_SHARED_OVR 6         /* explain_ovr_kernel: per-class sums of the one-vs-rest head (C = R classes) */
 #define DKS_SHARED_EXP 7         /* exp head: y from the instance's tables and the plan's l(s), no coalition kernel */
+#define DKS_SHARED_MIX 8         /* mixture head: one pass of the member head's coalition kernel per member (binary members:
+                                  * explain_shared_smem_kernel, softmax / one-vs-rest members: the class-sum kernels), each
+                                  * added times pi_k into one set of sums; DKS_PATH_CHUNKS counts member x chunk launches */
 #define DKS_SOLVE_NONE 0
 #define DKS_SOLVE_FUSED 1
 #define DKS_SOLVE_PMAT 2         /* wls_pmat_kernel */
