@@ -58,17 +58,30 @@ void dev_free(T** p) {
 
 inline int cdiv(long long a, int b) { return (int)((a + b - 1) / b); }
 
-// frees the device buffers the plan of one M owns (all M when M < 0); the caller has synchronised the stream
-void free_plan_allocs(dks_ctx* ctx, int M) {
+// drops the plan of one M (every M when M < 0) with everything derived from it -- its l1 tables, sampling info and
+// full-set tables -- and brings the device copies the kernels read up to date
+int drop_plans(dks_ctx* ctx, int M) {
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));       // nothing in flight may still read the buffers
     for (int m = 0; m <= DKS_MAX_GROUPS; ++m) {
         if (M >= 0 && m != M) continue;
         for (void* q : ctx->plan_allocs[m]) cudaFree(q);
         ctx->plan_allocs[m].clear();
+        ctx->h_plans[m] = PlanDev{};
+        ctx->h_l1[m] = dks::l1::Tables{};
+        ctx->h_afix[m] = nullptr;
+        ctx->h_sinfo[m] = DksSamplingInfo{};
     }
-}
-bool any_plan_allocs(const dks_ctx* ctx) {
-    for (int m = 0; m <= DKS_MAX_GROUPS; ++m) if (!ctx->plan_allocs[m].empty()) return true;
-    return false;
+    if (M < 0 || ctx->full.M == M) ctx->full = FullSetTables{};
+    if (M < 0) ctx->max_plan_S = 0;
+    ctx->epoch++;
+    const cudaStream_t st = ctx->stream;
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_l1, ctx->h_l1, sizeof(dks::l1::Tables) * (DKS_L1_MAX_GROUPS + 1), cudaMemcpyHostToDevice,
+                             st));
+    if (ctx->d_sinfo) CUDA_TRY(cudaMemcpyAsync(ctx->d_sinfo, ctx->h_sinfo, sizeof(ctx->h_sinfo), cudaMemcpyHostToDevice, st));
+    if (ctx->d_afix) CUDA_TRY(cudaMemcpyAsync(ctx->d_afix, ctx->h_afix, sizeof(ctx->h_afix), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return DKS_OK;
 }
 
 int bind(dks_ctx* ctx) {
@@ -122,8 +135,62 @@ cudaError_t record_ev(dks_ctx* ctx, int k) {
     return cudaEventRecordWithFlags(ctx->ev[k], ctx->stream, ctx->capturing ? cudaEventRecordExternal : cudaEventRecordDefault);
 }
 
+// persistent CTAs: as many per SM as shared memory holds (each also reserving `reserve` bytes), at most `max_per_sm`, and
+// no more than there is work for
+int persistent_grid(const dks_ctx* ctx, size_t smem, size_t reserve, int max_per_sm, long long work) {
+    const int per_sm = std::min(std::max((int)((size_t)ctx->max_smem_optin / (smem + reserve)), 1), max_per_sm);
+    return (int)std::min((long long)ctx->sm_count * per_sm, work);
+}
+
+// grows a per-call workspace buffer to at least `need` elements; a move changes the epoch (a captured graph holds the old
+// address)
+template <typename T>
+int grow(dks_ctx* ctx, T** p, size_t* cap, size_t need) {
+    if (need <= *cap) return DKS_OK;
+    TRY(dev_alloc(p, need));
+    *cap = need;
+    ctx->epoch++;
+    return DKS_OK;
+}
+
+// the head's capabilities, read by every dispatch decision (dks_fit: the head is fixed until the next fit)
+HeadDesc describe_head(const dks_ctx* ctx) {
+    HeadDesc h;
+    switch (ctx->act) {
+    case DKS_ACT_BINARY_LOGISTIC:
+        h.shared = HEAD_SHARED_BINARY; h.shared_max_G = DKS_MAX_GROUPS; h.scale = -ctx->kappa * DKS_LOG2E;
+        h.xt_any = true; h.l1_binary = true; h.wide_pi = true; h.tc = true;
+        break;
+    case DKS_ACT_SOFTMAX:
+    case DKS_ACT_OVR:
+        h.shared = HEAD_SHARED_CLASS_SUMS; h.ovr = ctx->act == DKS_ACT_OVR; h.scale = DKS_LOG2E;
+        h.simt_R = ctx->R; h.simt_C = ctx->C;
+        break;
+    case DKS_ACT_IDENTITY:
+        h.shared = HEAD_SHARED_TABLES; h.xt_bbar = true; h.wide_pi = true;
+        break;
+    case DKS_ACT_EXP:
+        h.shared = HEAD_SHARED_TABLES; h.expo = true; h.scale = DKS_LOG2E; h.wide_pi = true;
+        break;
+    case DKS_ACT_MIX:
+        // the tables are per member, member-major: -log2 e for binary members (the binary head's sign), log2 e else
+        h.scale = DKS_LOG2E;
+        if (ctx->mix.mact == DKS_ACT_BINARY_LOGISTIC) {
+            h.shared = HEAD_SHARED_MIX_BINARY; h.l1_binary = true; h.xt_scale = -DKS_LOG2E;
+        } else {
+            h.shared = HEAD_SHARED_MIX_CLASS; h.ovr = ctx->mix.mact == DKS_ACT_OVR; h.xt_scale = DKS_LOG2E;
+        }
+        break;
+    }
+    if (h.shared != HEAD_SHARED_BINARY) h.shared_max_G = 128;
+    if (!h.mixture()) h.xt_scale = h.scale;
+    h.l1_nout = h.l1_binary ? 1 : ctx->C;
+    return h;
+}
+
 int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const int G = ctx->G;
+    const HeadDesc& h = ctx->head;
     TRY(ensure_workspace(ctx, n));
     // status word, list counters and the histogram of M are adjacent: one memset
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * (4 + G + 1), ctx->stream));
@@ -135,41 +202,25 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const size_t maps_doubles = maps ? (size_t)ctx->cm.n_keys + ctx->cm.n_vals : 0;
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D, maps_doubles) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D, maps_doubles);
-    const bool mix = ctx->act == DKS_ACT_MIX;
-    auto kern = mix ? (maps ? (stage ? dks::prep_kernel<true, true, true> : dks::prep_kernel<false, true, true>)
-                            : (stage ? dks::prep_kernel<true, false, true> : dks::prep_kernel<false, false, true>))
-                    : maps ? (stage ? dks::prep_kernel<true, true> : dks::prep_kernel<false, true>)
-                           : (stage ? dks::prep_kernel<true, false> : dks::prep_kernel<false, false>);
-    // nibble tables: the binary head's scaled contributions; the softmax and one-vs-rest heads' per class (log2 e XW), the
-    // identity head's XW - Bbar and the exp head's log2 e XW, up to 128 groups (what the shared-plan path of those heads
-    // covers)
-    double* xt = nullptr;
-    if (ctx->act == DKS_ACT_BINARY_LOGISTIC && ctx->R == 1) xt = ctx->d_XT;
-    else if ((ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_IDENTITY ||
-              ctx->act == DKS_ACT_EXP || mix) && G <= 128 && ctx->plan_mode == 0) xt = ctx->d_XT;
-    // the mixture's tables are per member, member-major: -log2 e for binary members (the binary head's sign), log2 e else
-    const double xt_scale = mix ? (ctx->mix.mact == DKS_ACT_BINARY_LOGISTIC ? -DKS_LOG2E : DKS_LOG2E) : ctx->scale;
+    auto kern = h.mixture() ? (maps ? (stage ? dks::prep_kernel<true, true, true> : dks::prep_kernel<false, true, true>)
+                                    : (stage ? dks::prep_kernel<true, false, true> : dks::prep_kernel<false, false, true>))
+                            : maps ? (stage ? dks::prep_kernel<true, true> : dks::prep_kernel<false, true>)
+                                   : (stage ? dks::prep_kernel<true, false> : dks::prep_kernel<false, false>);
+    // nibble tables for the shared-plan route: the binary head's at any G, the other heads' up to 128 groups (what their
+    // shared-plan route covers)
+    double* xt = (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
         X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
         ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
         ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-        xt, xt_scale, ctx->act == DKS_ACT_IDENTITY ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
+        xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
     ctx->cur_n = n;
     ctx->cur_X = X_dev;
     ctx->prepared = true;
-    return DKS_OK;
-}
-
-// mixture of binary-logistic members: two outputs, class 0 the negation of class 1 (one solve, like the binary head)
-bool mix_binary(const dks_ctx* ctx) { return ctx->act == DKS_ACT_MIX && ctx->mix.mact == DKS_ACT_BINARY_LOGISTIC; }
-
-// the mixture's member buffer (one member's sums) for at least `need` floats
-int ensure_mixscr(dks_ctx* ctx, size_t need) {
-    if (need > ctx->cap_mixscr) { TRY(dev_alloc(&ctx->d_mixscr, need)); ctx->cap_mixscr = need; ctx->epoch++; }
     return DKS_OK;
 }
 
@@ -180,25 +231,31 @@ int launch_mix_axpy(dks_ctx* ctx, float* dst, float pi, bool first, int stride, 
     if (grid < 1) grid = 1;
     dks::mix::mix_axpy_kernel<<<(int)grid, 256, 0, ctx->stream>>>(ctx->d_mixscr, dst, pi, first ? 1 : 0, ctx->d_idx_full,
                                                                    ctx->d_counts, stride);
+    ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     return DKS_OK;
 }
 
 // what the l1 kernels of both instance lists share
-dks::l1::Params l1_params(dks_ctx* ctx, int n, int nout, double* phi_dev) {
+dks::l1::Params l1_params(dks_ctx* ctx, int n, double* phi_dev) {
     dks::l1::Params lp;
     memset(&lp, 0, sizeof(lp));
     lp.n = n; lp.N = ctx->N; lp.G = ctx->G; lp.C = ctx->C; lp.link = ctx->link;
-    lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.nout = nout; lp.tabs = ctx->d_l1;
-    lp.binary = ctx->act == DKS_ACT_BINARY_LOGISTIC || mix_binary(ctx);
+    lp.mode = ctx->l1_mode; lp.kfeat = ctx->l1_k; lp.nout = ctx->head.l1_nout; lp.tabs = ctx->d_l1;
+    lp.binary = ctx->head.l1_binary;
     lp.src.act = ctx->act;                           // the exp head's LARS skips tasks with non-finite moments
     lp.dlink = ctx->d_dlink; lp.linkfnull = ctx->d_linkfnull; lp.fnull = ctx->d_fnull;
     lp.mom = ctx->d_mom; lp.phi = phi_dev; lp.status = ctx->d_status;
     return lp;
 }
 
-// the LARS path + criterion + restricted WLS, one warp per task (at most `tasks`); warps sized for lp.Mmax.  stage: every
-// task has M = lp.Mmax, whose Gram matrix may then be staged in shared memory.
+// does the LARS kernel hold one warp's workspace for M groups (its Gram matrix aside)?
+bool lars_fits(const dks_ctx* ctx, int M) {
+    return dks::l1::lars_smem_per_warp(M) <= (size_t)ctx->max_smem_optin - 2048;
+}
+
+// the LARS path + criterion + restricted WLS, one warp per task (at most `tasks`); warps sized for lp.Mmax (lars_fits).
+// stage: every task has M = lp.Mmax, whose Gram matrix may then be staged in shared memory.
 int launch_lars(dks_ctx* ctx, const dks::l1::Params& lp, int tasks, bool stage, cudaStream_t stream) {
     const int M = lp.Mmax;
     const size_t per_warp = dks::l1::lars_smem_per_warp(M);
@@ -206,32 +263,24 @@ int launch_lars(dks_ctx* ctx, const dks::l1::Params& lp, int tasks, bool stage, 
     const size_t budget = (size_t)ctx->max_smem_optin - 2048;
     // the Gram matrix of the path goes to shared memory when at least four warps still fit next to it
     const int stage_gram = (stage && gram_bytes + 4 * per_warp <= budget) ? 1 : 0;
-    int wpc = (int)((budget - (stage_gram ? gram_bytes : 0)) / per_warp);
-    if (wpc < 1) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory", M, M);
-    if (wpc > 8) wpc = 8;
+    const int wpc = std::min((int)((budget - (stage_gram ? gram_bytes : 0)) / per_warp), 8);
     const size_t lsm = per_warp * wpc + (stage_gram ? gram_bytes : 0);
-    int per_sm = (int)((size_t)ctx->max_smem_optin / (lsm + 1024));
-    if (per_sm < 1) per_sm = 1;
-    if (per_sm > 4) per_sm = 4;
-    int lgrid = (tasks + wpc - 1) / wpc;
-    if (lgrid > ctx->sm_count * per_sm) lgrid = ctx->sm_count * per_sm;
+    const int lgrid = persistent_grid(ctx, lsm, 1024, 4, (tasks + wpc - 1) / wpc);
     CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_lars_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lsm));
     dks::l1::l1_lars_kernel<<<lgrid, 32 * wpc, lsm, stream>>>(lp, wpc, stage_gram);
+    ctx->launches += 1;
     return DKS_OK;
 }
 
 // upstream's l1 branch on the shared plan of G groups: moments of y per (instance, output), then the LARS path + criterion +
-// restricted WLS, one warp each.  The binary head: nout = 1, y from the (sum p1, sum p0) buffer; the softmax, one-vs-rest
-// and identity heads: nout = C (1 for a single regression output), y from src.
-int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, int nout, const dks::shared_path::HeadSource& src, double* phi_dev) {
-    const int G = ctx->G, S = pg.S, S_pad = pg.S_pad;
-    dks::l1::Params lp = l1_params(ctx, n, nout, phi_dev);
-    lp.S = S; lp.S_pad = S_pad; lp.Mmax = G; lp.src = src; lp.sums = ctx->d_sums; lp.z = pg.z; lp.w = pg.w;
+// restricted WLS, one warp each.  The binary heads: one output, y from the (sum p1, sum p0) buffer; the others: C outputs,
+// y from src.
+int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, const dks::shared_path::HeadSource& src, double* phi_dev) {
+    dks::l1::Params lp = l1_params(ctx, n, phi_dev);
+    lp.S = pg.S; lp.S_pad = pg.S_pad; lp.Mmax = ctx->G; lp.src = src; lp.sums = ctx->d_sums; lp.z = pg.z; lp.w = pg.w;
     lp.list = ctx->d_idx_full; lp.count = ctx->d_counts;
-    const size_t msm = sizeof(double) * (size_t)S;
-    if (msm + 8192 > (size_t)ctx->max_smem_optin)
-        return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: %d coalitions per plan exceed the shared-memory staging", S);
-    const int tasks = n * nout;
+    const size_t msm = sizeof(double) * (size_t)pg.S;
+    const int tasks = n * lp.nout;
     const int mgrid = tasks < ctx->sm_count * 2 ? tasks : ctx->sm_count * 2;
 #define DKS_MOM(W, MULTI)                                                                                                 \
     CUDA_TRY(cudaFuncSetAttribute(dks::l1::l1_moments_kernel<W, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm)); \
@@ -242,6 +291,7 @@ int launch_l1(dks_ctx* ctx, const PlanDev& pg, int n, int nout, const dks::share
         if (pg.W == 1) { DKS_MOM(1, true) } else { DKS_MOM(2, true) }
     }
 #undef DKS_MOM
+    ctx->launches += 1;
     return launch_lars(ctx, lp, tasks, true, ctx->stream);
 }
 
@@ -253,245 +303,287 @@ int sync_l1_tables(dks_ctx* ctx) {
     return DKS_OK;
 }
 
-int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const double* ext_w, int ext_stride) {
-    REQUIRE(ctx->prepared, "dks_explain: call dks_prepare_* first");
-    REQUIRE((ext_z == nullptr) == (ext_w == nullptr), "ext_zbits and ext_w must both be given or both be NULL");
-    const int n = ctx->cur_n;
-    int32_t* path = ctx->last_path;                  // what this call launches (dks_last_path)
-    memset(path, 0, sizeof(ctx->last_path));
-    const double* ext_chol = nullptr;
-    const double* ext_ainv = nullptr;
-    int ext_fstride = 0;
+// ---- the explain dispatcher: choose_route decides every kernel of a call before the first one is enqueued --------------
+enum RouteShared {                      // the shared-plan route of the instances whose groups all vary
+    ROUTE_SHARED_NONE,
+    ROUTE_FUSED,                        // binary head: link + projection solve inside the coalition kernel
+    ROUTE_BINARY,                       // binary head: (sum p1, sum p0), then a solve
+    ROUTE_BINARY_MEMBERS,               // mixture of binary members: the binary head's kernel per member, then a solve
+    ROUTE_CLASS_SUMS,                   // softmax / one-vs-rest: per-class sums, then a solve per (instance, class)
+    ROUTE_CLASS_MEMBERS,                // mixture of softmax / one-vs-rest members: the class-sum kernel per member
+    ROUTE_TABLES,                       // identity / exp: y from the tables, no coalition kernel
+};
+
+// per-instance plans drawn on the device: their layout and the sampler's launch configuration
+struct SamplerConfig {
+    int stride, W, nAmax, fstride, max_left, cap, fw;
+    size_t ssm, fsm;
+};
+
+struct Route {
+    int shared = ROUTE_SHARED_NONE;
+    int solve = DKS_SOLVE_NONE;         // of the shared-plan route (DKS_SOLVE_*)
+    int general = DKS_GENERAL_NONE;     // the kernel of the other instances (DKS_GENERAL_*)
+    bool l1_full = false;               // the instances on the shared-plan route select (l1)
+    int l1_Mmax = 0;                    // largest M < G whose instances select on the general list (0: none)
+    bool wide_pi = false;               // per-instance plans of 65..128 groups (two-word rows)
+    bool draw = false;                  // per-instance plans are drawn on the device first (sc)
+    SamplerConfig sc = {};
+    int S_cap = 2;                      // the largest S any instance can need
+    size_t l1_smem = 0, smem = 0;       // staging of the general list's l1 kernel and of the general kernel
+    dks::shared_path::FusedConfig fcfg = {};
+};
+
+int sampler_config(const dks_ctx* ctx, bool wide_pi, SamplerConfig* sc) {
+    if (ctx->max_plan_S < 2)
+        return fail(DKS_ERR_PLAN_MISSING, "per-instance plans need the shared plans of the M values present (their "
+                    "enumerated prefix); none is set");
+    REQUIRE(ctx->d_sinfo && ctx->d_afix, "per-instance plans: dks_set_plan_sampling has not been called");
+    sc->stride = (ctx->max_plan_S + 1) & ~1;
+    sc->W = wide_pi ? 2 : 1;                            // 64-bit words per coalition row
+    sc->nAmax = ctx->G > 1 ? ctx->G - 1 : 1;
+    sc->fstride = sc->nAmax * sc->nAmax;
+    // table sized for the largest sampled part among the plans set (a plan's sampled rows <= its S)
+    int max_left = 32;
+    for (int M = 2; M <= ctx->G && M <= DKS_MAX_GROUPS; ++M)
+        if (ctx->h_plans[M].z && ctx->h_sinfo[M].ncdf > 0) max_left = std::max(max_left, ctx->h_plans[M].S - ctx->h_sinfo[M].nfixed);
+    sc->max_left = (max_left + 31) / 32 * 32;
+    if (sc->max_left > dks::sampler::MAX_SAMPLED)
+        return fail(DKS_ERR_UNSUPPORTED, "per-instance plans: %d sampled rows per plan exceed the sampler's limit of %d",
+                    sc->max_left, dks::sampler::MAX_SAMPLED);
+    int cap = 256;                           // hash slots; its arrays are reused for the bit-transposed plan and pair counts
+    while (cap < 2 * sc->max_left || cap < sc->nAmax * (sc->nAmax + 1) / 2) cap <<= 1;
+    sc->cap = cap;
+    sc->ssm = dks::sampler::smem_bytes(cap, sc->max_left, ctx->G, sc->W);
+    if (sc->ssm + 2048 > (size_t)ctx->max_smem_optin)
+        return fail(DKS_ERR_UNSUPPORTED, "per-instance plan sampler needs %zu B of shared memory", sc->ssm);
+    if (wide_pi) {
+        sc->fsm = dks::sampler::wide_factor_smem(sc->nAmax);     // one CTA per instance inverts its normal matrix in place
+    } else {
+        const size_t per_warp = (size_t)2 * sc->nAmax * sc->nAmax * sizeof(double);
+        sc->fw = std::min((int)((size_t)ctx->max_smem_optin / per_warp), dks::sampler::FACTOR_WARPS);
+        if (sc->fw < 1)
+            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans: normal-matrix workspace does not fit shared memory");
+        sc->fsm = (size_t)sc->fw * per_warp;
+    }
+    return DKS_OK;
+}
+
+int choose_route(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
+    const HeadDesc& h = ctx->head;
+    const int G = ctx->G, N = ctx->N, kernel = ctx->kernel_choice;
+    const bool auto_or_shared = kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED;
+    *rt = Route{};
     // the mixture head: one pass of the member head's shared-plan kernel per member for instances whose groups all vary (up
     // to 128 groups), its CUDA-core kernel (dks_mixture.cuh) for the rest (up to 64 groups); no tensor-core kernel
-    const bool mixh = ctx->act == DKS_ACT_MIX;
-    if (mixh && ctx->G > 128)
-        return fail(DKS_ERR_UNSUPPORTED, "mixture head: %d groups; it covers at most 128", ctx->G);
-    if (mixh && ctx->kernel_choice == DKS_KERNEL_TCGEN05)
+    if (h.mixture() && G > h.shared_max_G)
+        return fail(DKS_ERR_UNSUPPORTED, "mixture head: %d groups; it covers at most %d", G, h.shared_max_G);
+    if (h.mixture() && kernel == DKS_KERNEL_TCGEN05)
         return fail(DKS_ERR_UNSUPPORTED, "mixture head: no tensor-core kernel (kernel 'auto', 'shared' or 'simt')");
-    if (ctx->G > 64 && ext_z != nullptr)
+    if (G > 64 && ext_z != nullptr)
         return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups: caller-supplied per-instance plans are not supported");
     // per-instance plans of 65..128 groups (two-word rows): binary-logistic, identity or exp head, CUDA-core kernel
-    const bool wide_pi = ctx->G > 64 && ctx->plan_mode == 1;
-    if (wide_pi) {
-        if (ctx->G > 128)
-            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans cover at most 128 groups (G=%d); use shared plans", ctx->G);
-        if (ctx->act != DKS_ACT_BINARY_LOGISTIC && ctx->act != DKS_ACT_IDENTITY && ctx->act != DKS_ACT_EXP)
+    rt->wide_pi = G > 64 && ctx->plan_mode == 1;
+    if (rt->wide_pi) {
+        if (G > 128)
+            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans cover at most 128 groups (G=%d); use shared plans", G);
+        if (!h.wide_pi)
             return fail(DKS_ERR_UNSUPPORTED, "per-instance plans of more than 64 groups: binary-logistic, identity or exp head "
                         "only");
-        if (ctx->kernel_choice != DKS_KERNEL_AUTO && ctx->kernel_choice != DKS_KERNEL_SIMT)
+        if (kernel != DKS_KERNEL_AUTO && kernel != DKS_KERNEL_SIMT)
             return fail(DKS_ERR_UNSUPPORTED, "per-instance plans of more than 64 groups run on the CUDA-core kernel (kernel "
                         "'auto' or 'simt')");
-        if (ctx->l1_mode != 0)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
+        if (ctx->l1_mode != 0) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
     }
-    if (ctx->plan_mode == 1 && ext_z == nullptr) {
-        // every instance draws its own plan on the device; the explain kernels then read it like a caller-supplied one
-        if (ctx->max_plan_S < 2)
-            return fail(DKS_ERR_PLAN_MISSING, "per-instance plans need the shared plans of the M values present (their "
-                        "enumerated prefix); none is set");
-        const int stride = (ctx->max_plan_S + 1) & ~1;
-        const int W = wide_pi ? 2 : 1;                     // 64-bit words per coalition row
-        const size_t need = (size_t)n * stride;
-        if (need > ctx->cap_gen || W != ctx->gen_words) {
-            TRY(dev_alloc(&ctx->d_genz, need * W)); TRY(dev_alloc(&ctx->d_genw, need));
-            ctx->cap_gen = need; ctx->gen_words = W; ctx->epoch++;
-        }
-        const int nAmax = ctx->G > 1 ? ctx->G - 1 : 1;
-        const int fstride = nAmax * nAmax;
-        const size_t needf = (size_t)n * fstride;
-        if (needf > ctx->cap_genf || (!wide_pi && ctx->d_genainv == nullptr)) {
-            // two-word rows keep one matrix per instance (inverted in place); one-word rows its factor and its inverse
-            TRY(dev_alloc(&ctx->d_genchol, needf));
-            if (wide_pi) dev_free(&ctx->d_genainv);
-            else TRY(dev_alloc(&ctx->d_genainv, needf));
-            ctx->cap_genf = needf; ctx->epoch++;
-        }
-        REQUIRE(ctx->d_sinfo && ctx->d_afix, "per-instance plans: dks_set_plan_sampling has not been called");
-        // table sized for the largest sampled part among the plans set (a plan's sampled rows <= its S)
-        int max_left = 32;
-        for (int M = 2; M <= ctx->G && M <= DKS_MAX_GROUPS; ++M)
-            if (ctx->h_plans[M].z && ctx->h_sinfo[M].ncdf > 0) {
-                const int left = ctx->h_plans[M].S - ctx->h_sinfo[M].nfixed;
-                if (left > max_left) max_left = left;
-            }
-        max_left = (max_left + 31) / 32 * 32;
-        if (max_left > dks::sampler::MAX_SAMPLED)
-            return fail(DKS_ERR_UNSUPPORTED, "per-instance plans: %d sampled rows per plan exceed the sampler's limit of %d",
-                        max_left, dks::sampler::MAX_SAMPLED);
-        int cap = 256;                       // hash slots; its arrays are reused for the bit-transposed plan and pair counts
-        while (cap < 2 * max_left || cap < nAmax * (nAmax + 1) / 2) cap <<= 1;
-        dks::sampler::SamplerParams sp;
-        sp.n = n; sp.G = ctx->G; sp.S_req = ctx->nsamples_req; sp.stride = stride; sp.seed = ctx->sampler_seed;
-        sp.table_cap = cap; sp.max_left = max_left; sp.fstride = fstride;
-        sp.row_offset = ctx->row_offset; sp.Mcnt = ctx->d_M; sp.plans = ctx->d_plans; sp.info = ctx->d_sinfo;
-        sp.afix = ctx->d_afix;
-        sp.out_z = ctx->d_genz; sp.out_w = ctx->d_genw; sp.out_chol = ctx->d_genchol; sp.out_ainv = ctx->d_genainv;
-        sp.status = ctx->d_status;
-        const size_t ssm = dks::sampler::smem_bytes(cap, max_left, ctx->G, W);
-        if (ssm + 2048 > (size_t)ctx->max_smem_optin)
-            return fail(DKS_ERR_UNSUPPORTED, "per-instance plan sampler needs %zu B of shared memory", ssm);
-        auto skern = W == 1 ? dks::sampler::sample_plans_kernel<1> : dks::sampler::sample_plans_kernel<2>;
-        CUDA_TRY(cudaFuncSetAttribute(skern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssm));
-        int per_sm = (int)((size_t)ctx->max_smem_optin / (ssm + 2048));
-        if (per_sm > 6) per_sm = 6;
-        if (per_sm < 1) per_sm = 1;
-        const int sgrid = n < ctx->sm_count * per_sm ? n : ctx->sm_count * per_sm;
-        skern<<<sgrid, dks::sampler::THREADS, ssm, ctx->stream>>>(sp);
-        if (wide_pi) {
-            // one CTA per instance inverts its normal matrix in place
-            const size_t fsm = dks::sampler::wide_factor_smem(nAmax);
-            CUDA_TRY(cudaFuncSetAttribute(dks::sampler::factor_wide_plans_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)fsm));
-            const int fgrid = n < ctx->sm_count * 2 ? n : ctx->sm_count * 2;
-            dks::sampler::factor_wide_plans_kernel<<<fgrid, dks::sampler::WIDE_FACTOR_THREADS, fsm, ctx->stream>>>(
-                n, ctx->d_M, ctx->G, fstride, ctx->d_genchol, ctx->d_status);
-        } else {
-            const size_t per_warp = (size_t)2 * nAmax * nAmax * sizeof(double);
-            int fw = (int)((size_t)ctx->max_smem_optin / per_warp);
-            if (fw > dks::sampler::FACTOR_WARPS) fw = dks::sampler::FACTOR_WARPS;
-            if (fw < 1)
-                return fail(DKS_ERR_UNSUPPORTED, "per-instance plans: normal-matrix workspace does not fit shared memory");
-            const size_t fsm = (size_t)fw * per_warp;
-            CUDA_TRY(cudaFuncSetAttribute(dks::sampler::factor_plans_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsm));
-            int fgrid = (n + fw - 1) / fw;
-            dks::sampler::factor_plans_kernel<<<fgrid, fw * 32, fsm, ctx->stream>>>(n, ctx->d_M, fstride, ctx->d_genchol,
-                                                                                    ctx->d_genainv, nAmax, ctx->d_status);
-        }
-        ctx->launches += 2;
-        CUDA_TRY(cudaGetLastError());
-        ctx->gen_stride = stride; ctx->gen_n = n; ctx->gen_plan_words = W;
-        ext_z = ctx->d_genz; ext_w = ctx->d_genw; ext_stride = stride;
-        ext_chol = wide_pi ? nullptr : ctx->d_genchol; ext_ainv = wide_pi ? ctx->d_genchol : ctx->d_genainv;
-        ext_fstride = fstride;
-    }
-    ExplainParams p;
-    memset(&p, 0, sizeof(p));
-    p.n = n; p.N = ctx->N; p.G = ctx->G; p.R = ctx->R; p.C = ctx->C;
-    p.act = ctx->act; p.link = ctx->link; p.S_req = ctx->nsamples_req;
-    p.scale = ctx->scale;
-    p.BWs = ctx->d_BWs; p.bases = ctx->d_bases; p.wbf = ctx->d_wbf; p.wbg = ctx->d_wbg; p.Bbar = ctx->d_Bbar;
-    p.fnull = ctx->d_fnull; p.linkfnull = ctx->d_linkfnull;
-    p.XW = ctx->d_XW; p.vmask = ctx->d_vmask; p.Mcnt = ctx->d_M; p.dlink = ctx->d_dlink;
-    p.plans = ctx->d_plans; p.ext_z = ext_z; p.ext_w = ext_w; p.ext_stride = ext_stride;
-    p.ext_chol = ext_chol; p.ext_ainv = ext_ainv; p.ext_fstride = ext_fstride;
-    p.phi = phi_dev; p.status = ctx->d_status;
-    const ExpBackground eb{ctx->d_BW, ctx->d_scores};
-    // capacity of the per-CTA y buffer: the largest S any instance can need
-    int S_cap = 0;
-    if (ext_z) S_cap = ext_stride;
-    else S_cap = ctx->max_plan_S;
-    if (S_cap < 2) S_cap = 2;
-    p.S_cap = S_cap;
+    // every instance draws its own plan on the device; the explain kernels then read it like a caller-supplied one
+    rt->draw = ctx->plan_mode == 1 && ext_z == nullptr;
+    if (rt->draw) TRY(sampler_config(ctx, rt->wide_pi, &rt->sc));
+    const bool per_inst = ext_z != nullptr || rt->draw;
+    rt->S_cap = std::max(ext_z ? ext_stride : rt->draw ? rt->sc.stride : ctx->max_plan_S, 2);
 
-    if (ctx->dbg_i >= 0) {   // debug dump of one instance's accumulator tile (tensor-core kernel only)
-        int rows = S_cap, cols = dks::tc_npad(ctx->N);
-        if (rows != ctx->dbg_rows || cols != ctx->dbg_cols) {
-            TRY(dev_alloc(&ctx->dbg_T, (size_t)rows * cols));
-            ctx->dbg_rows = rows; ctx->dbg_cols = cols;
-        }
-        CUDA_TRY(cudaMemsetAsync(ctx->dbg_T, 0, sizeof(float) * rows * cols, ctx->stream));
-        if (!ctx->dbg_time) TRY(dev_alloc(&ctx->dbg_time, (size_t)6 * 256));
-        CUDA_TRY(cudaMemsetAsync(ctx->dbg_time, 0, sizeof(float) * 6 * 256, ctx->stream));
-    }
-
-    int kernel = ctx->kernel_choice;
-    const int kernel_req = kernel;
-    CUDA_TRY(record_ev(ctx, 2));
-
-    // ---- shared-plan fast path: instances whose varying set is all G groups, evaluated against the plan's Dm table
-    const int G = ctx->G;
+    // shared-plan route: the instances whose varying set is all G groups, on the plan of G groups and its tables
     const PlanDev& pg = ctx->h_plans[G <= DKS_MAX_GROUPS ? G : 0];
-    const bool fast = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
-                      ctx->act == DKS_ACT_BINARY_LOGISTIC && G >= 2 && pg.dmT != nullptr &&
-                      pg.S == dks_effective_S(G, ctx->nsamples_req) && (pg.W <= 2 || pg.ptw != nullptr);
-    // softmax, one-vs-rest, identity and exp heads, up to 128 groups: per-class sums of the class-sum coalition kernels
-    // (dks_multi.cuh) or the identity / exp head's tables, then a solve per (instance, output)
-    const bool sfm = ctx->act == DKS_ACT_SOFTMAX, ovr = ctx->act == DKS_ACT_OVR, expo = ctx->act == DKS_ACT_EXP;
-    const bool mc = sfm || ovr;          // heads with per-class sums
-    const bool tabled = ctx->act == DKS_ACT_IDENTITY || expo;     // heads whose y comes from the instance's tables alone
-    const bool multi = (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr &&
-                       (mc || tabled) && G >= 2 && G <= 128 && ctx->plan_mode == 0 &&
-                       pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) && (!mc || ctx->h_smx[G].dm != nullptr) &&
-                       (!expo || ctx->h_expl[G] != nullptr);
-    // mixture head, up to 128 groups: one pass of the member head's coalition kernel per member, added times pi_k into one
-    // set of sums -- binary members the binary head's (sum p1, sum p0) and its solves, the others the per-class sums
-    const bool mixbin = mix_binary(ctx);
-    const bool mixs = mixh && (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED) && ext_z == nullptr && G >= 2 &&
-                      G <= 128 && ctx->plan_mode == 0 && pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req) &&
-                      ctx->mixp_M == G;
-    if (kernel == DKS_KERNEL_SHARED && !fast && !multi && !mixs && ext_z == nullptr && pg.z != nullptr)
+    const bool plan_G = pg.z != nullptr && pg.S == dks_effective_S(G, ctx->nsamples_req);
+    bool shared = auto_or_shared && !per_inst && G >= 2 && G <= h.shared_max_G && plan_G;
+    if (h.shared == HEAD_SHARED_BINARY) shared = shared && pg.dmT != nullptr && (pg.W <= 2 || pg.ptw != nullptr);
+    else shared = shared && ctx->full.M == G;
+    if (kernel == DKS_KERNEL_SHARED && !shared && !per_inst && pg.z != nullptr)
         return fail(DKS_ERR_UNSUPPORTED, "shared-plan fast path needs the binary-logistic head, or the softmax / one-vs-rest / "
                     "identity / exp head with at most 128 groups");
-    // l1 feature selection: on the shared-plan path when M = G selects, and on the general list (CUDA-core kernel for the
+
+    // l1 feature selection: on the shared-plan route when M = G selects, and on the general list (CUDA-core kernel for the
     // moments, then l1_lars_kernel) for the instances with a partial varying set whose M selects
     const bool l1 = ctx->l1_mode != 0;
     auto selects = [&](int M) {
         return l1 && M >= 1 && M <= DKS_L1_MAX_GROUPS && ((ctx->l1_sel[(M - 1) >> 6] >> ((M - 1) & 63)) & 1ull) != 0;
     };
-    const bool l1_full = selects(G);
-    int l1_Mmax = 0;                     // largest M < G that selects
-    for (int M = 2; M < G && M <= DKS_L1_MAX_GROUPS; ++M) if (selects(M)) l1_Mmax = M;
-    const bool l1_gen = l1_Mmax > 0;
-    const int l1_nout = (mc || tabled || (mixh && !mix_binary(ctx))) ? ctx->C : 1;
-    size_t l1_smem = 0;
-    ctx->l1_timing_valid = false;
+    rt->l1_full = selects(G);
+    for (int M = 2; M < G && M <= DKS_L1_MAX_GROUPS; ++M) if (selects(M)) rt->l1_Mmax = M;
     if (l1) {
-        if (ext_z != nullptr || ctx->plan_mode == 1)
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
-        if (l1_full && pg.W > 2)
+        if (per_inst) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
+        if (rt->l1_full && pg.W > 2)
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection covers plans of at most 128 groups (M=%d)", G);
-        if (l1_full && (!(fast || multi || mixs) || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S))
+        if (rt->l1_full && (!shared || ctx->h_l1[G].gram_raw == nullptr || ctx->h_l1[G].S != pg.S))
             return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared-plan path (binary-logistic, softmax, "
                         "one-vs-rest, identity, exp or mixture head) and the l1 tables of the M=%d plan (dks_set_l1_tables)", G);
-        if (l1_gen) {
+        if (rt->l1_full && sizeof(double) * (size_t)pg.S + 8192 > (size_t)ctx->max_smem_optin)
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: %d coalitions per plan exceed the shared-memory staging",
+                        pg.S);
+        if (rt->l1_full && !lars_fits(ctx, G))
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory", G, G);
+        if (rt->l1_Mmax > 0) {
+            const int Mmax = rt->l1_Mmax;
             if (G > 64)
                 return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection for partial varying sets covers at most 64 groups (G=%d)", G);
-            if (kernel_req != DKS_KERNEL_AUTO && kernel_req != DKS_KERNEL_SHARED)
+            if (!auto_or_shared)
                 return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs kernel 'auto' or 'shared' (the CUDA-core kernel "
                             "forms the moments of instances with a partial varying set)");
-            for (int M = 2; M <= l1_Mmax; ++M)
+            for (int M = 2; M <= Mmax; ++M)
                 if (selects(M) && (ctx->h_l1[M].gram_raw == nullptr || ctx->h_l1[M].S != dks_effective_S(M, ctx->nsamples_req) ||
                                    ctx->h_plans[M].z == nullptr || ctx->h_plans[M].S != ctx->h_l1[M].S))
                     return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared plan of M=%d and its l1 tables "
                                 "(dks_set_l1_tables)", M);
-            l1_smem = mixh ? dks::mix::smem_bytes(S_cap, ctx->N, l1_Mmax, ctx->mix, ctx->C)
-                           : dks::simt_smem_bytes(S_cap, ctx->N, l1_Mmax, mc ? ctx->R : 1, mc ? ctx->C : 1);
-            if ((long long)l1_smem > (long long)ctx->max_smem_optin)
+            rt->l1_smem = h.mixture() ? dks::mix::smem_bytes(rt->S_cap, N, Mmax, ctx->mix, ctx->C)
+                                      : dks::simt_smem_bytes(rt->S_cap, N, Mmax, h.simt_R, h.simt_C);
+            if ((long long)rt->l1_smem > (long long)ctx->max_smem_optin)
                 return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the CUDA-core kernel's staging of instances with up to "
-                            "%d varying groups needs %zu B of shared memory (> %d)", l1_Mmax, l1_smem, ctx->max_smem_optin);
+                            "%d varying groups needs %zu B of shared memory (> %d)", Mmax, rt->l1_smem, ctx->max_smem_optin);
+            if (!lars_fits(ctx, Mmax))
+                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory",
+                            Mmax, Mmax);
         }
-        const size_t need_m = (size_t)n * l1_nout * (2 * G + 4);
-        if (need_m > ctx->cap_mom) { TRY(dev_alloc(&ctx->d_mom, need_m)); ctx->cap_mom = need_m; ctx->epoch++; }
     }
-    // non-uniform background weights: the weighted instantiations of the shared-plan kernels (dks_shared.cuh)
+
+    if (shared) {
+        switch (h.shared) {
+        case HEAD_SHARED_BINARY: {
+            const bool fused = !rt->l1_full && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
+                               dks::shared_path::fused_config(N, G, pg.S_pad, ctx->sm_count, ctx->max_smem_optin,
+                                                              ctx->opt_fused_warps, ctx->opt_fused_B, &rt->fcfg, !ctx->uniform_w);
+            rt->shared = fused ? ROUTE_FUSED : ROUTE_BINARY;
+            break;
+        }
+        case HEAD_SHARED_MIX_BINARY: rt->shared = ROUTE_BINARY_MEMBERS; break;
+        case HEAD_SHARED_CLASS_SUMS: rt->shared = ROUTE_CLASS_SUMS; break;
+        case HEAD_SHARED_MIX_CLASS: rt->shared = ROUTE_CLASS_MEMBERS; break;
+        default: rt->shared = ROUTE_TABLES; break;
+        }
+        const bool binary = rt->shared == ROUTE_BINARY || rt->shared == ROUTE_BINARY_MEMBERS;
+        if (rt->shared == ROUTE_FUSED) rt->solve = DKS_SOLVE_FUSED;
+        else if (rt->l1_full) rt->solve = DKS_SOLVE_L1;
+        else if (binary && pg.W > 2) rt->solve = DKS_SOLVE_WIDE;   // more than 128 groups: host-supplied projection
+        else if (binary && pg.pmat != nullptr) rt->solve = DKS_SOLVE_PMAT;
+        else rt->solve = DKS_SOLVE_WLS_SHARED;
+    }
+
+    // the kernel of the instances the shared-plan route does not take
+    if (rt->wide_pi) {
+        // per-instance two-word plans: the instances whose groups all vary run the CUDA-core two-word kernel; a partial
+        // varying set is reported, not computed
+        rt->smem = dks::iwide::smem_bytes(rt->S_cap);
+        if ((long long)rt->smem > (long long)ctx->max_smem_optin)
+            return fail(DKS_ERR_UNSUPPORTED, "two-word per-instance kernel needs %zu B of shared memory (> %d): nsamples too "
+                        "large", rt->smem, ctx->max_smem_optin);
+        rt->general = DKS_GENERAL_SIMT_WIDE;
+    } else if (G > 64) {
+        // two-word coalition rows exist on the shared-plan path only: anything left over is reported, not computed
+        if (!plan_G || (pg.W > 2 && pg.ptw == nullptr)) {
+            ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
+            return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
+        }
+        if (!shared)
+            return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, or the "
+                        "softmax / one-vs-rest / identity head up to 128 groups, or the exp head up to 128 groups; kernel "
+                        "'auto' or 'shared', shared plan of M=%d uploaded)", G);
+        rt->general = DKS_GENERAL_FLAGGED;
+    } else if (auto_or_shared ? dks::tc_supported(ctx, rt->S_cap) : kernel == DKS_KERNEL_TCGEN05) {
+        if (!dks::tc_supported(ctx, rt->S_cap))
+            return fail(DKS_ERR_UNSUPPORTED, "tensor-core kernel does not support this shape/head (N=%d G=%d act=%d)", N, G,
+                        ctx->act);
+        rt->general = DKS_GENERAL_TC;
+    } else {
+        rt->smem = h.mixture() ? dks::mix::smem_bytes(rt->S_cap, N, G, ctx->mix, ctx->C)
+                               : dks::simt_smem_bytes(rt->S_cap, N, G, h.simt_R, h.simt_C);
+        rt->general = DKS_GENERAL_SIMT;
+        if ((long long)rt->smem > (long long)ctx->max_smem_optin) {
+            // the shared-plan route took the instances whose groups all vary; the general kernel is sized for the largest
+            // plan set and cannot hold it.  The instances left for it (often none) are reported, not computed.
+            if (shared) {
+                rt->general = DKS_GENERAL_FLAGGED;
+            } else if (pg.z == nullptr && auto_or_shared && !per_inst && h.shared != HEAD_SHARED_BINARY && G >= 2 &&
+                       G <= h.shared_max_G) {
+                // these heads' shared-plan route takes these instances once the plan of G groups is uploaded
+                ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
+                return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
+            } else {
+                return fail(DKS_ERR_UNSUPPORTED, "SIMT kernel needs %zu B of shared memory (> %d): N*G or nsamples too large",
+                            rt->smem, ctx->max_smem_optin);
+            }
+        }
+    }
+    return DKS_OK;
+}
+
+// draws every instance's plan on the device and factors its normal matrix; p then reads the plans like caller-supplied ones
+int launch_sampler(dks_ctx* ctx, const Route& rt, ExplainParams* p) {
+    const SamplerConfig& sc = rt.sc;
+    const int n = ctx->cur_n;
+    const size_t need = (size_t)n * sc.stride;
+    if (need > ctx->cap_gen || sc.W != ctx->gen_words) {
+        TRY(dev_alloc(&ctx->d_genz, need * sc.W)); TRY(dev_alloc(&ctx->d_genw, need));
+        ctx->cap_gen = need; ctx->gen_words = sc.W; ctx->epoch++;
+    }
+    const size_t needf = (size_t)n * sc.fstride;
+    if (needf > ctx->cap_genf || (!rt.wide_pi && ctx->d_genainv == nullptr)) {
+        // two-word rows keep one matrix per instance (inverted in place); one-word rows its factor and its inverse
+        TRY(dev_alloc(&ctx->d_genchol, needf));
+        if (rt.wide_pi) dev_free(&ctx->d_genainv);
+        else TRY(dev_alloc(&ctx->d_genainv, needf));
+        ctx->cap_genf = needf; ctx->epoch++;
+    }
+    dks::sampler::SamplerParams sp;
+    sp.n = n; sp.G = ctx->G; sp.S_req = ctx->nsamples_req; sp.stride = sc.stride; sp.seed = ctx->sampler_seed;
+    sp.table_cap = sc.cap; sp.max_left = sc.max_left; sp.fstride = sc.fstride;
+    sp.row_offset = ctx->row_offset; sp.Mcnt = ctx->d_M; sp.plans = ctx->d_plans; sp.info = ctx->d_sinfo;
+    sp.afix = ctx->d_afix;
+    sp.out_z = ctx->d_genz; sp.out_w = ctx->d_genw; sp.out_chol = ctx->d_genchol; sp.out_ainv = ctx->d_genainv;
+    sp.status = ctx->d_status;
+    auto skern = sc.W == 1 ? dks::sampler::sample_plans_kernel<1> : dks::sampler::sample_plans_kernel<2>;
+    CUDA_TRY(cudaFuncSetAttribute(skern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.ssm));
+    skern<<<persistent_grid(ctx, sc.ssm, 2048, 6, n), dks::sampler::THREADS, sc.ssm, ctx->stream>>>(sp);
+    if (rt.wide_pi) {
+        CUDA_TRY(cudaFuncSetAttribute(dks::sampler::factor_wide_plans_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)sc.fsm));
+        const int fgrid = n < ctx->sm_count * 2 ? n : ctx->sm_count * 2;
+        dks::sampler::factor_wide_plans_kernel<<<fgrid, dks::sampler::WIDE_FACTOR_THREADS, sc.fsm, ctx->stream>>>(
+            n, ctx->d_M, ctx->G, sc.fstride, ctx->d_genchol, ctx->d_status);
+    } else {
+        CUDA_TRY(cudaFuncSetAttribute(dks::sampler::factor_plans_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.fsm));
+        dks::sampler::factor_plans_kernel<<<(n + sc.fw - 1) / sc.fw, sc.fw * 32, sc.fsm, ctx->stream>>>(
+            n, ctx->d_M, sc.fstride, ctx->d_genchol, ctx->d_genainv, sc.nAmax, ctx->d_status);
+    }
+    ctx->launches += 2;
+    CUDA_TRY(cudaGetLastError());
+    ctx->gen_stride = sc.stride; ctx->gen_n = n; ctx->gen_plan_words = sc.W;
+    p->ext_z = ctx->d_genz; p->ext_w = ctx->d_genw; p->ext_stride = sc.stride;
+    p->ext_chol = rt.wide_pi ? nullptr : ctx->d_genchol; p->ext_ainv = rt.wide_pi ? ctx->d_genchol : ctx->d_genainv;
+    p->ext_fstride = sc.fstride;
+    return DKS_OK;
+}
+
+// binary head on the shared-plan route: the fused kernel, or the coalition kernel into (sum p1, sum p0) -- per member, added
+// times pi_k, for a mixture of binary members
+int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, double* phi_dev) {
+    const int n = ctx->cur_n, G = ctx->G;
+    int32_t* path = ctx->last_path;
     const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn;
-    if (fast || multi || mixs) path[DKS_PATH_BG_WEIGHTS] = wn != nullptr ? 1 : 0;
-    // the general kernel below (instances that are not on the shared-plan path) forks off here and joins at the end
-    cudaStream_t gstream = ctx->stream;
-    if ((fast || multi || mixs) && ctx->side_stream != nullptr) {
-        CUDA_TRY(cudaEventRecord(ctx->ev_fork, ctx->stream));
-        CUDA_TRY(cudaStreamWaitEvent(ctx->side_stream, ctx->ev_fork, 0));
-        gstream = ctx->side_stream;
-    }
-    auto join = [&]() -> cudaError_t {
-        if (gstream == ctx->stream) return cudaSuccess;
-        cudaError_t e = cudaEventRecord(ctx->ev_join, gstream);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0);
-        return e;
-    };
-    dks::shared_path::FusedConfig fcfg;
-    const bool fused = fast && !l1_full && ctx->opt_fused && pg.pmat64 != nullptr && pg.W == 1 &&
-                       dks::shared_path::fused_config(ctx->N, G, pg.S_pad, ctx->sm_count, ctx->max_smem_optin,
-                                                      ctx->opt_fused_warps, ctx->opt_fused_B, &fcfg,
-                                                      wn != nullptr);
-    ctx->last_fused = fused;
-    if (fused) {
+    if (rt.shared == ROUTE_FUSED) {
         // link + projection solve inside the coalition kernel: no (sum p1, sum p0) buffer, no separate solve launch
+        const dks::shared_path::FusedConfig& fcfg = rt.fcfg;
         dks::shared_path::FusedParams fp;
         memset(&fp, 0, sizeof(fp));
         fp.n = n; fp.N = ctx->N; fp.G = G; fp.C = ctx->C; fp.S = pg.S; fp.S_pad = pg.S_pad; fp.link = ctx->link; fp.B = fcfg.B;
-        fp.scale = ctx->scale; fp.DmT = pg.dmT; fp.dme = pg.dme; fp.z = pg.z; fp.XT = ctx->d_XT; fp.list = ctx->d_idx_full;
+        fp.scale = ctx->head.scale; fp.DmT = pg.dmT; fp.dme = pg.dme; fp.z = pg.z; fp.XT = ctx->d_XT; fp.list = ctx->d_idx_full;
         fp.count = ctx->d_counts; fp.pmat64 = pg.pmat64; fp.dvec = pg.dvec64; fp.dlink = ctx->d_dlink;
         fp.linkfnull = ctx->d_linkfnull; fp.fnull = ctx->d_fnull; fp.acc = ctx->d_acc; fp.done = ctx->d_done; fp.phi = phi_dev;
         fp.wn = wn;
@@ -522,313 +614,317 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
         path[DKS_PATH_SOLVE] = DKS_SOLVE_FUSED; path[DKS_PATH_FUSED_CTA_WARPS] = fcfg.slices * fcfg.kw;
         path[DKS_PATH_FUSED_TABLE] = table ? 1 : 0;
         CUDA_TRY(cudaGetLastError());
-        p.list = ctx->d_idx_other;
-        p.count = ctx->d_counts + 1;
-    } else if (fast || (mixs && mixbin)) {
-        const int S = pg.S, S_pad = pg.S_pad;
-        size_t need = (size_t)n * S_pad;
-        if (need > ctx->cap_sums) { TRY(dev_alloc(&ctx->d_sums, need)); ctx->cap_sums = need; ctx->epoch++; }
-        dks::shared_path::SharedParams sp;
-        sp.n = n; sp.N = ctx->N; sp.G = G; sp.S = S; sp.S_pad = S_pad; sp.scale = ctx->scale;
-        sp.DmT = pg.dmT; sp.dme = pg.dme; sp.z = pg.z; sp.XT = ctx->d_XT; sp.list = ctx->d_idx_full; sp.count = ctx->d_counts; sp.sums = ctx->d_sums; sp.accumulate = 0;
-        sp.acache = nullptr; sp.acache_mode = 0; sp.wn = wn;
-        if (pg.W > 2 && ctx->opt_wide_acache && ctx->N > dks::shared_path::MAXN) {
-            // sixteen-word rows, several background chunks: A(i, s) is computed by the first chunk's launch only
-            if (need > ctx->cap_acache) { TRY(dev_alloc(&ctx->d_acache, need)); ctx->cap_acache = need; ctx->epoch++; }
-            sp.acache = ctx->d_acache;
-        }
-        if (!mixs) {
-            dks::shared_path::SharedLaunch sl;
-            const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &sl);
-            if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
-            ctx->launches += nl - 1;
-            path[DKS_PATH_SHARED] = sl.regs ? DKS_SHARED_REGS : DKS_SHARED_SMEM; path[DKS_PATH_CHUNKS] = sl.chunks;
-            path[DKS_PATH_WARPS] = sl.warps; path[DKS_PATH_GRID] = sl.grid;
-        } else {
-            // binary members: the binary head's kernel per member, into the member buffer, then added times pi_k
-            const size_t stride = 2 * (size_t)S_pad;
-            TRY(ensure_mixscr(ctx, (size_t)n * stride));
-            const size_t xt_member = (size_t)n * ((G + 3) / 4) * 16;
-            sp.scale = -DKS_LOG2E; sp.sums = reinterpret_cast<float2*>(ctx->d_mixscr);
-            int chunks = 0, warps = 0, grid = 0;
-            for (int k = 0; k < ctx->mix.K; ++k) {
-                sp.DmT = ctx->mixp.dm[k]; sp.dme = ctx->mixp.dme[k]; sp.XT = ctx->d_XT + k * xt_member;
-                dks::shared_path::SharedLaunch sl;
-                const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream,
-                                                                       &sl);
-                if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
-                chunks += sl.chunks; warps = k == 0 ? sl.warps : std::min(warps, sl.warps); grid = std::max(grid, sl.grid);
-                TRY(launch_mix_axpy(ctx, reinterpret_cast<float*>(ctx->d_sums), ctx->mix.pif[k], k == 0, (int)stride, n));
-                ctx->launches += nl + 1;
-            }
-            ctx->launches -= 1;                      // the common tail below counts one coalition launch
-            path[DKS_PATH_SHARED] = DKS_SHARED_MIX; path[DKS_PATH_CHUNKS] = chunks;
-            path[DKS_PATH_WARPS] = warps; path[DKS_PATH_GRID] = grid;
-        }
+        return DKS_OK;
+    }
+    const size_t need = (size_t)n * pg.S_pad;
+    TRY(grow(ctx, &ctx->d_sums, &ctx->cap_sums, need));
+    dks::shared_path::SharedParams sp;
+    sp.n = n; sp.N = ctx->N; sp.G = G; sp.S = pg.S; sp.S_pad = pg.S_pad; sp.scale = ctx->head.scale;
+    sp.DmT = pg.dmT; sp.dme = pg.dme; sp.z = pg.z; sp.XT = ctx->d_XT; sp.list = ctx->d_idx_full; sp.count = ctx->d_counts; sp.sums = ctx->d_sums; sp.accumulate = 0;
+    sp.acache = nullptr; sp.acache_mode = 0; sp.wn = wn;
+    if (pg.W > 2 && ctx->opt_wide_acache && ctx->N > dks::shared_path::MAXN) {
+        // sixteen-word rows, several background chunks: A(i, s) is computed by the first chunk's launch only
+        TRY(grow(ctx, &ctx->d_acache, &ctx->cap_acache, need));
+        sp.acache = ctx->d_acache;
+    }
+    if (rt.shared == ROUTE_BINARY) {
+        dks::shared_path::SharedLaunch sl;
+        const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &sl);
+        if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
+        ctx->launches += nl;
+        path[DKS_PATH_SHARED] = sl.regs ? DKS_SHARED_REGS : DKS_SHARED_SMEM; path[DKS_PATH_CHUNKS] = sl.chunks;
+        path[DKS_PATH_WARPS] = sl.warps; path[DKS_PATH_GRID] = sl.grid;
+        return DKS_OK;
+    }
+    // binary members: the binary head's kernel per member, into the member buffer, then added times pi_k
+    const size_t stride = 2 * (size_t)pg.S_pad;
+    TRY(grow(ctx, &ctx->d_mixscr, &ctx->cap_mixscr, (size_t)n * stride));
+    const size_t xt_member = (size_t)n * ((G + 3) / 4) * 16;
+    sp.scale = -DKS_LOG2E; sp.sums = reinterpret_cast<float2*>(ctx->d_mixscr);
+    int chunks = 0, warps = 0, grid = 0;
+    for (int k = 0; k < ctx->mix.K; ++k) {
+        sp.DmT = ctx->full.dm[k]; sp.dme = ctx->full.dme[k]; sp.XT = ctx->d_XT + k * xt_member;
+        dks::shared_path::SharedLaunch sl;
+        const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &sl);
+        if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
+        ctx->launches += nl;
+        chunks += sl.chunks; warps = k == 0 ? sl.warps : std::min(warps, sl.warps); grid = std::max(grid, sl.grid);
+        TRY(launch_mix_axpy(ctx, reinterpret_cast<float*>(ctx->d_sums), ctx->mix.pif[k], k == 0, (int)stride, n));
+    }
+    path[DKS_PATH_SHARED] = DKS_SHARED_MIX; path[DKS_PATH_CHUNKS] = chunks;
+    path[DKS_PATH_WARPS] = warps; path[DKS_PATH_GRID] = grid;
+    return DKS_OK;
+}
+
+// the solve of the binary heads' shared-plan route, from (sum p1, sum p0)
+int launch_binary_solve(dks_ctx* ctx, const Route& rt, const PlanDev& pg, double* phi_dev) {
+    const int n = ctx->cur_n, G = ctx->G, S = pg.S, S_pad = pg.S_pad;
+    if (rt.solve == DKS_SOLVE_L1) {
+        TRY(launch_l1(ctx, pg, n, dks::shared_path::HeadSource{}, phi_dev));
+    } else if (rt.solve == DKS_SOLVE_WIDE) {
+        // more than 128 groups: link, float64 product with the host-supplied projection, remainder (dks_wide.cuh)
+        TRY(grow(ctx, &ctx->d_yw, &ctx->cap_yw, (size_t)n * S_pad));
+        TRY(grow(ctx, &ctx->d_betaw, &ctx->cap_betaw, (size_t)n * pg.kpw));
+        dks::wide::WideParams qp;
+        memset(&qp, 0, sizeof(qp));
+        qp.n = n; qp.N = ctx->N; qp.G = G; qp.C = ctx->C; qp.S = S; qp.S_pad = S_pad; qp.KP = pg.kpw; qp.link = ctx->link;
+        qp.sums = ctx->d_sums; qp.PT = pg.ptw; qp.dvec = pg.dvecw; qp.dlink = ctx->d_dlink;
+        qp.linkfnull = ctx->d_linkfnull; qp.fnull = ctx->d_fnull; qp.list = ctx->d_idx_full; qp.count = ctx->d_counts;
+        qp.y = ctx->d_yw; qp.beta = ctx->d_betaw; qp.phi = phi_dev;
+        CUDA_TRY(dks::wide::launch_wide_solve(qp, n, ctx->sm_count, ctx->opt_wide_gemm, ctx->stream));
+        ctx->launches += 3;
+    } else if (rt.solve == DKS_SOLVE_PMAT) {
+        dks::shared_path::WlsPmatParams pp;
+        pp.n = n; pp.N = ctx->N; pp.G = G; pp.C = ctx->C; pp.S = S; pp.S_pad = S_pad; pp.link = ctx->link; pp.uniform_w = 1;
+        pp.sums = ctx->d_sums; pp.pmat = pg.pmat; pp.dvec = pg.dvec; pp.dlink = ctx->d_dlink;
+        pp.linkfnull = ctx->d_linkfnull; pp.fnull = ctx->d_fnull; pp.list = ctx->d_idx_full; pp.count = ctx->d_counts;
+        pp.phi = phi_dev;
+        cudaError_t perr = cudaSuccess;
+        if (!dks::shared_path::launch_wls_pmat(pp, n, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &perr))
+            return fail(DKS_ERR_UNSUPPORTED, "projection solve does not fit shared memory");
+        CUDA_TRY(perr);
+        ctx->launches += 1;
+        ctx->last_path[DKS_PATH_PMAT_KPAD] = dks::shared_path::wls_pmat_kpad(G);
+    } else {
         dks::shared_path::WlsSharedParams wp;
         wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = ctx->C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link;
         wp.uniform_w = 1; wp.sums = ctx->d_sums; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink;
         wp.linkfnull = ctx->d_linkfnull; wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts;
         wp.phi = phi_dev; wp.status = ctx->d_status;
-        if (l1_full) {
-            TRY(launch_l1(ctx, pg, n, 1, dks::shared_path::HeadSource{}, phi_dev));
-            path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
-        } else if (pg.W > 2) {
-            // more than 128 groups: link, float64 product with the host-supplied projection, remainder (dks_wide.cuh)
-            const size_t need_y = (size_t)n * S_pad, need_b = (size_t)n * pg.kpw;
-            if (need_y > ctx->cap_yw) { TRY(dev_alloc(&ctx->d_yw, need_y)); ctx->cap_yw = need_y; ctx->epoch++; }
-            if (need_b > ctx->cap_betaw) { TRY(dev_alloc(&ctx->d_betaw, need_b)); ctx->cap_betaw = need_b; ctx->epoch++; }
-            dks::wide::WideParams qp;
-            memset(&qp, 0, sizeof(qp));
-            qp.n = n; qp.N = ctx->N; qp.G = G; qp.C = ctx->C; qp.S = S; qp.S_pad = S_pad; qp.KP = pg.kpw; qp.link = ctx->link;
-            qp.sums = ctx->d_sums; qp.PT = pg.ptw; qp.dvec = pg.dvecw; qp.dlink = ctx->d_dlink;
-            qp.linkfnull = ctx->d_linkfnull; qp.fnull = ctx->d_fnull; qp.list = ctx->d_idx_full; qp.count = ctx->d_counts;
-            qp.y = ctx->d_yw; qp.beta = ctx->d_betaw; qp.phi = phi_dev;
-            CUDA_TRY(dks::wide::launch_wide_solve(qp, n, ctx->sm_count, ctx->opt_wide_gemm, ctx->stream));
-            ctx->launches += 2;                      // three launches; the common tail below counts one of them
-            path[DKS_PATH_SOLVE] = DKS_SOLVE_WIDE;
-        } else if (pg.pmat != nullptr) {
-            dks::shared_path::WlsPmatParams pp;
-            pp.n = n; pp.N = ctx->N; pp.G = G; pp.C = ctx->C; pp.S = S; pp.S_pad = S_pad; pp.link = ctx->link; pp.uniform_w = 1;
-            pp.sums = ctx->d_sums; pp.pmat = pg.pmat; pp.dvec = pg.dvec; pp.dlink = ctx->d_dlink;
-            pp.linkfnull = ctx->d_linkfnull; pp.fnull = ctx->d_fnull; pp.list = ctx->d_idx_full; pp.count = ctx->d_counts;
-            pp.phi = phi_dev;
-            cudaError_t perr = cudaSuccess;
-            if (!dks::shared_path::launch_wls_pmat(pp, n, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &perr))
-                return fail(DKS_ERR_UNSUPPORTED, "projection solve does not fit shared memory");
-            CUDA_TRY(perr);
-            path[DKS_PATH_SOLVE] = DKS_SOLVE_PMAT; path[DKS_PATH_PMAT_KPAD] = dks::shared_path::wls_pmat_kpad(G);
+        const size_t wsm = dks::shared_path::wls_shared_smem(G);
+        const int wgrid = persistent_grid(ctx, wsm, 24 * 1024, 4, n);   // persistent CTAs of 8 warps
+        if (pg.W == 1) {
+            CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
+            dks::shared_path::wls_shared_kernel<1><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
         } else {
-            const size_t wsm = dks::shared_path::wls_shared_smem(G);
-            int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 24 * 1024));
-            if (per_sm > 4) per_sm = 4;
-            if (per_sm < 1) per_sm = 1;
-            int wgrid = n < ctx->sm_count * per_sm ? n : ctx->sm_count * per_sm;   // persistent CTAs of 8 warps
-            if (pg.W == 1) {
-                CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-                dks::shared_path::wls_shared_kernel<1><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
-            } else {
-                CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-                dks::shared_path::wls_shared_kernel<2><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
-            }
-            path[DKS_PATH_SOLVE] = DKS_SOLVE_WLS_SHARED;
+            CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
+            dks::shared_path::wls_shared_kernel<2><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
         }
-        ctx->launches += 2;
-        CUDA_TRY(cudaGetLastError());
-        p.list = ctx->d_idx_other;      // the general kernel below takes the remaining instances
-        p.count = ctx->d_counts + 1;
-    } else if (multi || mixs) {
-        const int S = pg.S, S_pad = pg.S_pad, C = ctx->C;
-        dks::shared_path::HeadSource src;
-        src.act = ctx->act; src.ntab = (G + 3) / 4; src.msums = nullptr; src.XT = ctx->d_XT; src.ell = ctx->h_expl[G];
-        if (mixs) {
-            // softmax / one-vs-rest members: the class-sum kernel of the member head per member, into the member buffer,
-            // then added times pi_k into the per-class sums the solves read (HeadSource: the mixture's sums)
-            const MixHead& mh = ctx->mix;
-            const size_t need = (size_t)n * C * S_pad;
-            if (need > ctx->cap_msums) { TRY(dev_alloc(&ctx->d_msums, need)); ctx->cap_msums = need; ctx->epoch++; }
-            TRY(ensure_mixscr(ctx, need));
-            dks::multi::SoftmaxParams mp;
-            memset(&mp, 0, sizeof(mp));
-            mp.n = n; mp.N = ctx->N; mp.G = G; mp.S = S; mp.S_pad = S_pad; mp.ntab = src.ntab; mp.scale = DKS_LOG2E;
-            mp.wn = ctx->d_wn; mp.z = pg.z; mp.list = ctx->d_idx_full; mp.count = ctx->d_counts; mp.sums = ctx->d_mixscr;
-            const size_t xt_member = (size_t)n * mh.Rm * src.ntab * 16;
-            int chunks = 0, grid = 0;
-            for (int k = 0; k < mh.K; ++k) {
-                mp.dm = ctx->mixp.dm[k]; mp.lo = ctx->mixp.lo[k]; mp.XT = ctx->d_XT + k * xt_member;
-                mp.BW = ctx->d_mixBW + (size_t)k * ctx->N * G * mh.Rm; mp.scores = ctx->d_mixsc + (size_t)k * ctx->N * mh.Rm;
-                const int nl = dks::multi::launch_class_sums(mp, mh.mact == DKS_ACT_OVR, C, pg.W, n, ctx->sm_count,
-                                                             ctx->max_smem_optin, ctx->stream, &grid);
-                if (nl == 0)
-                    return fail(DKS_ERR_CUDA, "mixture member coalition kernel: %s", cudaGetErrorString(cudaGetLastError()));
-                chunks += nl;
-                TRY(launch_mix_axpy(ctx, ctx->d_msums, mh.pif[k], k == 0, C * S_pad, n));
-                ctx->launches += nl + 1;
-            }
-            path[DKS_PATH_SHARED] = DKS_SHARED_MIX; path[DKS_PATH_CHUNKS] = chunks;
-            path[DKS_PATH_WARPS] = dks::multi::MC_WARPS; path[DKS_PATH_GRID] = grid;
-            src.msums = ctx->d_msums;
-        } else if (mc) {
-            // the workspace is C n S_pad floats: the engine explains these heads in row blocks of 2 / C the binary path's
-            const size_t need = (size_t)n * C * S_pad;
-            if (need > ctx->cap_msums) { TRY(dev_alloc(&ctx->d_msums, need)); ctx->cap_msums = need; ctx->epoch++; }
-            dks::multi::SoftmaxParams mp;
-            memset(&mp, 0, sizeof(mp));
-            mp.n = n; mp.N = ctx->N; mp.G = G; mp.S = S; mp.S_pad = S_pad; mp.ntab = src.ntab; mp.scale = ctx->scale;
-            mp.dm = ctx->h_smx[G].dm; mp.lo = ctx->h_smx[G].lo; mp.wn = ctx->d_wn; mp.z = pg.z; mp.XT = ctx->d_XT; mp.BW = ctx->d_BW;
-            mp.scores = ctx->d_scores; mp.list = ctx->d_idx_full; mp.count = ctx->d_counts; mp.sums = ctx->d_msums;
-            int grid = 0;
-            const int nl = dks::multi::launch_class_sums(mp, ovr, C, pg.W, n, ctx->sm_count, ctx->max_smem_optin, ctx->stream,
-                                                         &grid);
-            if (nl == 0)
-                return fail(DKS_ERR_CUDA, "%s coalition kernel: %s", ovr ? "one-vs-rest" : "softmax",
-                            cudaGetErrorString(cudaGetLastError()));
-            ctx->launches += nl;
-            path[DKS_PATH_SHARED] = ovr ? DKS_SHARED_OVR : DKS_SHARED_SOFTMAX; path[DKS_PATH_CHUNKS] = nl;
-            path[DKS_PATH_WARPS] = dks::multi::MC_WARPS; path[DKS_PATH_GRID] = grid;
-            src.msums = ctx->d_msums;
-        } else {
-            // y straight from the tables (and the plan's l(s) for the exp head): no coalition kernel
-            path[DKS_PATH_SHARED] = expo ? DKS_SHARED_EXP : DKS_SHARED_AFFINE;
-        }
-        if (l1_full) {
-            TRY(launch_l1(ctx, pg, n, C, src, phi_dev));
-            ctx->launches += 2;
-            path[DKS_PATH_SOLVE] = DKS_SOLVE_L1;
-        } else {
-            dks::shared_path::WlsSharedParams wp;
-            memset(&wp, 0, sizeof(wp));
-            wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = C; wp.S = S; wp.S_pad = S_pad; wp.link = ctx->link; wp.uniform_w = 1;
-            wp.src = src; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink; wp.linkfnull = ctx->d_linkfnull;
-            wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts; wp.phi = phi_dev;
-            wp.status = ctx->d_status;
-            const size_t wsm = dks::shared_path::wls_shared_smem(G);
-            int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 24 * 1024));
-            if (per_sm > 4) per_sm = 4;
-            if (per_sm < 1) per_sm = 1;
-            const int tasks = n * C;
-            const int wgrid = tasks < ctx->sm_count * per_sm ? tasks : ctx->sm_count * per_sm;
-            if (pg.W == 1) {
-                CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-                dks::shared_path::wls_shared_kernel<1, true><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
-            } else {
-                CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-                dks::shared_path::wls_shared_kernel<2, true><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
-            }
-            ctx->launches += 1;
-            path[DKS_PATH_SOLVE] = DKS_SOLVE_WLS_SHARED;
-        }
-        CUDA_TRY(cudaGetLastError());
-        p.list = ctx->d_idx_other;
-        p.count = ctx->d_counts + 1;
-    }
-    if (l1_gen) {
-        // the general list splits into the instances whose M selects -- the CUDA-core kernel stores their moments and
-        // l1_lars_kernel selects and solves on the shared plan of each one's M -- and the rest, which keep the kernel below
-        CUDA_TRY(cudaMemsetAsync(ctx->d_l1_counts, 0, 2 * sizeof(int), gstream));
-        int pgrid = cdiv(n, 256);
-        if (pgrid > ctx->sm_count * 4) pgrid = ctx->sm_count * 4;
-        dks::l1::l1_partition_kernel<<<pgrid, 256, 0, gstream>>>(p.list, p.count, n, ctx->d_M, ctx->l1_sel[0], ctx->l1_sel[1],
-                                                                 ctx->d_idx_sel, ctx->d_idx_plain, ctx->d_l1_counts);
-        ExplainParams ps = p;
-        ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
-        auto l1kern = expo ? dks::explain_simt_kernel<true, true> : dks::explain_simt_kernel<true>;
-        CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<true> : (const void*)l1kern,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l1_smem));
-        int per_sm = (int)((size_t)ctx->max_smem_optin / (l1_smem + 1024));
-        if (per_sm < 1) per_sm = 1;
-        if (per_sm > 8) per_sm = 8;
-        int grid = ctx->sm_count * per_sm;
-        if (grid > n) grid = n;
-        const bool timed = !ctx->capturing;
-        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
-        if (mixh)
-            dks::mix::explain_simt_mix_kernel<true><<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
-                                                                                     ctx->mix);
-        else
-            l1kern<<<grid, 256, l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom}, eb);
-        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[1], gstream));
-        dks::l1::Params lp = l1_params(ctx, n, l1_nout, phi_dev);
-        lp.Mmax = l1_Mmax; lp.Mcnt = ctx->d_M; lp.vmask = ctx->d_vmask; lp.list = ctx->d_idx_sel; lp.count = ctx->d_l1_counts;
-        TRY(launch_lars(ctx, lp, n * l1_nout, false, gstream));
-        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[2], gstream));
-        ctx->l1_timing_valid = timed;
-        ctx->launches += 3;
-        CUDA_TRY(cudaGetLastError());
-        path[DKS_PATH_GENERAL_L1] = 1;
-        p.list = ctx->d_idx_plain;
-        p.count = ctx->d_l1_counts + 1;
-    }
-    if (wide_pi) {
-        // per-instance two-word plans: the instances whose groups all vary run the CUDA-core two-word kernel; a partial
-        // varying set is reported, not computed
-        p.list = ctx->d_idx_full; p.count = ctx->d_counts;
-        const size_t wsm = dks::iwide::smem_bytes(S_cap);
-        if ((long long)wsm > (long long)ctx->max_smem_optin)
-            return fail(DKS_ERR_UNSUPPORTED, "two-word per-instance kernel needs %zu B of shared memory (> %d): nsamples too "
-                        "large", wsm, ctx->max_smem_optin);
-        auto wkern = expo ? dks::iwide::explain_wide_instance_kernel<true> : dks::iwide::explain_wide_instance_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(wkern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
-        int per_sm = (int)((size_t)ctx->max_smem_optin / (wsm + 1024));
-        if (per_sm < 1) per_sm = 1;
-        if (per_sm > 4) per_sm = 4;
-        int grid = ctx->sm_count * per_sm;
-        if (grid > n) grid = n;
-        wkern<<<grid, dks::iwide::THREADS, wsm, gstream>>>(p, eb);
-        dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
-        ctx->launches += 2;
-        path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT_WIDE;
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(join());
-        CUDA_TRY(record_ev(ctx, 3));
-        return DKS_OK;
-    }
-    if (G > 64) {
-        // two-word coalition rows exist on the shared-plan path only: anything left over is reported, not computed
-        if (pg.z == nullptr || pg.S != dks_effective_S(G, ctx->nsamples_req) || (pg.W > 2 && pg.ptw == nullptr)) {
-            ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
-            return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
-        }
-        if (!fast && !multi && !mixs)
-            return fail(DKS_ERR_UNSUPPORTED, "more than 64 groups needs the shared-plan path (binary-logistic head, or the "
-                        "softmax / one-vs-rest / identity head up to 128 groups, or the exp head up to 128 groups; kernel "
-                        "'auto' or 'shared', shared plan of M=%d uploaded)", G);
-        dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
         ctx->launches += 1;
-        path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(join());
-        CUDA_TRY(record_ev(ctx, 3));
-        return DKS_OK;
     }
-    if (kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED)
-        kernel = dks::tc_supported(ctx, p) ? DKS_KERNEL_TCGEN05 : DKS_KERNEL_SIMT;
-    if (kernel == DKS_KERNEL_TCGEN05) {
-        if (!dks::tc_supported(ctx, p))
-            return fail(DKS_ERR_UNSUPPORTED, "tensor-core kernel does not support this shape/head (N=%d G=%d act=%d)", ctx->N,
-                        ctx->G, ctx->act);
-        TRY(dks::tc_launch(ctx, p, gstream));
-        path[DKS_PATH_GENERAL] = DKS_GENERAL_TC;
-    } else {
-        size_t smem = mixh ? dks::mix::smem_bytes(S_cap, ctx->N, ctx->G, ctx->mix, ctx->C)
-                           : dks::simt_smem_bytes(S_cap, ctx->N, ctx->G, mc ? ctx->R : 1, mc ? ctx->C : 1);
-        if ((long long)smem > (long long)ctx->max_smem_optin && (fast || multi || mixs)) {
-            // the shared-plan path took the instances whose groups all vary; the general kernel is sized for the largest
-            // plan set and cannot hold it.  The instances left for it (often none) are reported, not computed.
-            dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(p.count, G, ctx->d_status);
-            ctx->launches += 1;
-            path[DKS_PATH_GENERAL] = DKS_GENERAL_FLAGGED;
-            CUDA_TRY(cudaGetLastError());
-            CUDA_TRY(join());
-            CUDA_TRY(record_ev(ctx, 3));
-            return DKS_OK;
-        }
-        if ((long long)smem > (long long)ctx->max_smem_optin && !multi && pg.z == nullptr &&
-            (kernel_req == DKS_KERNEL_AUTO || kernel_req == DKS_KERNEL_SHARED) && ext_z == nullptr && ctx->plan_mode == 0 &&
-            (mc || tabled || mixh) && G >= 2 && G <= 128) {
-            // the softmax / one-vs-rest / identity / exp head's shared-plan path takes these instances once the plan of G
-            // groups is uploaded
-            ctx->h_status[0] = DKS_ERR_PLAN_MISSING; ctx->h_status[1] = G;
-            return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", G);
-        }
-        if ((long long)smem > (long long)ctx->max_smem_optin)
-            return fail(DKS_ERR_UNSUPPORTED, "SIMT kernel needs %zu B of shared memory (> %d): N*G or nsamples too large",
-                        smem, ctx->max_smem_optin);
-        auto skern = expo ? dks::explain_simt_kernel<false, true> : dks::explain_simt_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<false> : (const void*)skern,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = (int)((size_t)ctx->max_smem_optin / (smem + 1024));
-        if (per_sm < 1) per_sm = 1;
-        if (per_sm > 8) per_sm = 8;
-        int grid = ctx->sm_count * per_sm;
-        if (grid > n) grid = n;
-        if (mixh) dks::mix::explain_simt_mix_kernel<false><<<grid, 256, smem, gstream>>>(p, dks::SimtL1{}, ctx->mix);
-        else skern<<<grid, 256, smem, gstream>>>(p, dks::SimtL1{}, eb);
-        ctx->launches += 1;
-        path[DKS_PATH_GENERAL] = DKS_GENERAL_SIMT;
-    }
+    ctx->last_path[DKS_PATH_SOLVE] = rt.solve;
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(join());
+    return DKS_OK;
+}
+
+// softmax, one-vs-rest, identity, exp and class-member mixture heads on the shared-plan route: the per-class sums of the
+// class-sum coalition kernels (dks_multi.cuh; per member, added times pi_k, for a mixture) or the identity / exp head's
+// tables.  *src: where the solve reads y.
+int launch_class_sums(dks_ctx* ctx, const Route& rt, const PlanDev& pg, dks::shared_path::HeadSource* src) {
+    const int n = ctx->cur_n, G = ctx->G, C = ctx->C, S_pad = pg.S_pad;
+    int32_t* path = ctx->last_path;
+    src->act = ctx->act; src->ntab = (G + 3) / 4; src->msums = nullptr; src->XT = ctx->d_XT; src->ell = ctx->full.ell;
+    if (rt.shared == ROUTE_TABLES) {
+        // y straight from the tables (and the plan's l(s) for the exp head): no coalition kernel
+        path[DKS_PATH_SHARED] = ctx->head.expo ? DKS_SHARED_EXP : DKS_SHARED_AFFINE;
+        return DKS_OK;
+    }
+    // the workspace is C n S_pad floats: the engine explains these heads in row blocks of 2 / C the binary path's
+    const bool members = rt.shared == ROUTE_CLASS_MEMBERS;
+    const size_t need = (size_t)n * C * S_pad;
+    TRY(grow(ctx, &ctx->d_msums, &ctx->cap_msums, need));
+    if (members) TRY(grow(ctx, &ctx->d_mixscr, &ctx->cap_mixscr, need));
+    dks::multi::SoftmaxParams mp;
+    memset(&mp, 0, sizeof(mp));
+    mp.n = n; mp.N = ctx->N; mp.G = G; mp.S = pg.S; mp.S_pad = S_pad; mp.ntab = src->ntab; mp.scale = DKS_LOG2E;
+    mp.wn = ctx->d_wn; mp.z = pg.z; mp.list = ctx->d_idx_full; mp.count = ctx->d_counts;
+    mp.sums = members ? ctx->d_mixscr : ctx->d_msums;
+    const MixHead& mh = ctx->mix;
+    const int K = members ? mh.K : 1;
+    const size_t xt_member = (size_t)n * mh.Rm * src->ntab * 16;
+    int chunks = 0, grid = 0;
+    for (int k = 0; k < K; ++k) {
+        mp.dm = ctx->full.dm[k]; mp.lo = ctx->full.lo[k];
+        if (members) {
+            mp.XT = ctx->d_XT + k * xt_member;
+            mp.BW = ctx->d_mixBW + (size_t)k * ctx->N * G * mh.Rm; mp.scores = ctx->d_mixsc + (size_t)k * ctx->N * mh.Rm;
+        } else {
+            mp.XT = ctx->d_XT; mp.BW = ctx->d_BW; mp.scores = ctx->d_scores;
+        }
+        const int nl = dks::multi::launch_class_sums(mp, ctx->head.ovr, C, pg.W, n, ctx->sm_count, ctx->max_smem_optin,
+                                                     ctx->stream, &grid);
+        if (nl == 0)
+            return fail(DKS_ERR_CUDA, "%s coalition kernel: %s", members ? "mixture member" : ctx->head.ovr ? "one-vs-rest" : "softmax",
+                        cudaGetErrorString(cudaGetLastError()));
+        ctx->launches += nl;
+        chunks += nl;
+        if (members) TRY(launch_mix_axpy(ctx, ctx->d_msums, mh.pif[k], k == 0, C * S_pad, n));
+    }
+    path[DKS_PATH_SHARED] = members ? DKS_SHARED_MIX : ctx->head.ovr ? DKS_SHARED_OVR : DKS_SHARED_SOFTMAX;
+    path[DKS_PATH_CHUNKS] = chunks; path[DKS_PATH_WARPS] = dks::multi::MC_WARPS; path[DKS_PATH_GRID] = grid;
+    src->msums = ctx->d_msums;
+    return DKS_OK;
+}
+
+// the solve per (instance, output) of launch_class_sums' route
+int launch_class_solve(dks_ctx* ctx, const Route& rt, const PlanDev& pg, const dks::shared_path::HeadSource& src,
+                       double* phi_dev) {
+    const int n = ctx->cur_n, G = ctx->G, C = ctx->C;
+    if (rt.solve == DKS_SOLVE_L1) {
+        TRY(launch_l1(ctx, pg, n, src, phi_dev));
+    } else {
+        dks::shared_path::WlsSharedParams wp;
+        memset(&wp, 0, sizeof(wp));
+        wp.n = n; wp.N = ctx->N; wp.G = G; wp.C = C; wp.S = pg.S; wp.S_pad = pg.S_pad; wp.link = ctx->link; wp.uniform_w = 1;
+        wp.src = src; wp.z = pg.z; wp.w = pg.w; wp.ainv = pg.ainv; wp.dlink = ctx->d_dlink; wp.linkfnull = ctx->d_linkfnull;
+        wp.fnull = ctx->d_fnull; wp.list = ctx->d_idx_full; wp.count = ctx->d_counts; wp.phi = phi_dev;
+        wp.status = ctx->d_status;
+        const size_t wsm = dks::shared_path::wls_shared_smem(G);
+        const int wgrid = persistent_grid(ctx, wsm, 24 * 1024, 4, (long long)n * C);
+        if (pg.W == 1) {
+            CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
+            dks::shared_path::wls_shared_kernel<1, true><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
+        } else {
+            CUDA_TRY(cudaFuncSetAttribute(dks::shared_path::wls_shared_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsm));
+            dks::shared_path::wls_shared_kernel<2, true><<<wgrid, dks::shared_path::WLS_THREADS, wsm, ctx->stream>>>(wp);
+        }
+        ctx->launches += 1;
+    }
+    ctx->last_path[DKS_PATH_SOLVE] = rt.solve;
+    CUDA_TRY(cudaGetLastError());
+    return DKS_OK;
+}
+
+// the general list splits into the instances whose M selects -- the CUDA-core kernel stores their moments and
+// l1_lars_kernel selects and solves on the shared plan of each one's M -- and the rest, which p then lists
+int launch_general_l1(dks_ctx* ctx, const Route& rt, ExplainParams* p, double* phi_dev, cudaStream_t gstream) {
+    const int n = ctx->cur_n;
+    CUDA_TRY(cudaMemsetAsync(ctx->d_l1_counts, 0, 2 * sizeof(int), gstream));
+    int pgrid = cdiv(n, 256);
+    if (pgrid > ctx->sm_count * 4) pgrid = ctx->sm_count * 4;
+    dks::l1::l1_partition_kernel<<<pgrid, 256, 0, gstream>>>(p->list, p->count, n, ctx->d_M, ctx->l1_sel[0], ctx->l1_sel[1],
+                                                             ctx->d_idx_sel, ctx->d_idx_plain, ctx->d_l1_counts);
+    ExplainParams ps = *p;
+    ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
+    const bool mixh = ctx->head.mixture();
+    auto l1kern = ctx->head.expo ? dks::explain_simt_kernel<true, true> : dks::explain_simt_kernel<true>;
+    CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<true> : (const void*)l1kern,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rt.l1_smem));
+    const int grid = persistent_grid(ctx, rt.l1_smem, 1024, 8, n);
+    const bool timed = !ctx->capturing;
+    if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
+    if (mixh)
+        dks::mix::explain_simt_mix_kernel<true><<<grid, 256, rt.l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
+                                                                                   ctx->mix);
+    else
+        l1kern<<<grid, 256, rt.l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
+                                                   ExpBackground{ctx->d_BW, ctx->d_scores});
+    ctx->launches += 2;
+    if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[1], gstream));
+    dks::l1::Params lp = l1_params(ctx, n, phi_dev);
+    lp.Mmax = rt.l1_Mmax; lp.Mcnt = ctx->d_M; lp.vmask = ctx->d_vmask; lp.list = ctx->d_idx_sel; lp.count = ctx->d_l1_counts;
+    TRY(launch_lars(ctx, lp, n * lp.nout, false, gstream));
+    if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[2], gstream));
+    ctx->l1_timing_valid = timed;
+    CUDA_TRY(cudaGetLastError());
+    ctx->last_path[DKS_PATH_GENERAL_L1] = 1;
+    p->list = ctx->d_idx_plain;
+    p->count = ctx->d_l1_counts + 1;
+    return DKS_OK;
+}
+
+// the kernel of the instances the shared-plan route and the general list's l1 selection left (p.list)
+int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t gstream) {
+    const int n = ctx->cur_n, G = ctx->G;
+    const ExpBackground eb{ctx->d_BW, ctx->d_scores};
+    switch (rt.general) {
+    case DKS_GENERAL_SIMT_WIDE: {
+        p.list = ctx->d_idx_full; p.count = ctx->d_counts;
+        auto wkern = ctx->head.expo ? dks::iwide::explain_wide_instance_kernel<true> : dks::iwide::explain_wide_instance_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(wkern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rt.smem));
+        wkern<<<persistent_grid(ctx, rt.smem, 1024, 4, n), dks::iwide::THREADS, rt.smem, gstream>>>(p, eb);
+        dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(ctx->d_counts + 1, G, ctx->d_status);
+        ctx->launches += 2;
+        break;
+    }
+    case DKS_GENERAL_FLAGGED:
+        dks::flag_unsupported_kernel<<<1, 1, 0, gstream>>>(p.count, G, ctx->d_status);
+        ctx->launches += 1;
+        break;
+    case DKS_GENERAL_TC:
+        TRY(dks::tc_launch(ctx, p, gstream));
+        break;
+    default: {
+        const bool mixh = ctx->head.mixture();
+        auto skern = ctx->head.expo ? dks::explain_simt_kernel<false, true> : dks::explain_simt_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<false> : (const void*)skern,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rt.smem));
+        const int grid = persistent_grid(ctx, rt.smem, 1024, 8, n);
+        if (mixh) dks::mix::explain_simt_mix_kernel<false><<<grid, 256, rt.smem, gstream>>>(p, dks::SimtL1{}, ctx->mix);
+        else skern<<<grid, 256, rt.smem, gstream>>>(p, dks::SimtL1{}, eb);
+        ctx->launches += 1;
+        break;
+    }
+    }
+    ctx->last_path[DKS_PATH_GENERAL] = rt.general;
+    CUDA_TRY(cudaGetLastError());
+    return DKS_OK;
+}
+
+// debug dump of one instance's accumulator tile (tensor-core kernel only)
+int prepare_debug_dump(dks_ctx* ctx, int S_cap) {
+    const int rows = S_cap, cols = dks::tc_npad(ctx->N);
+    if (rows != ctx->dbg_rows || cols != ctx->dbg_cols) {
+        TRY(dev_alloc(&ctx->dbg_T, (size_t)rows * cols));
+        ctx->dbg_rows = rows; ctx->dbg_cols = cols;
+    }
+    CUDA_TRY(cudaMemsetAsync(ctx->dbg_T, 0, sizeof(float) * rows * cols, ctx->stream));
+    if (!ctx->dbg_time) TRY(dev_alloc(&ctx->dbg_time, (size_t)6 * 256));
+    CUDA_TRY(cudaMemsetAsync(ctx->dbg_time, 0, sizeof(float) * 6 * 256, ctx->stream));
+    return DKS_OK;
+}
+
+int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const double* ext_w, int ext_stride) {
+    REQUIRE(ctx->prepared, "dks_explain: call dks_prepare_* first");
+    REQUIRE((ext_z == nullptr) == (ext_w == nullptr), "ext_zbits and ext_w must both be given or both be NULL");
+    memset(ctx->last_path, 0, sizeof(ctx->last_path));   // what this call launches (dks_last_path)
+    Route rt;
+    TRY(choose_route(ctx, ext_z, ext_stride, &rt));
+    const int n = ctx->cur_n, G = ctx->G;
+    ExplainParams p;
+    memset(&p, 0, sizeof(p));
+    p.n = n; p.N = ctx->N; p.G = G; p.R = ctx->R; p.C = ctx->C;
+    p.act = ctx->act; p.link = ctx->link; p.S_req = ctx->nsamples_req;
+    p.scale = ctx->head.scale;
+    p.BWs = ctx->d_BWs; p.bases = ctx->d_bases; p.wbf = ctx->d_wbf; p.wbg = ctx->d_wbg; p.Bbar = ctx->d_Bbar;
+    p.fnull = ctx->d_fnull; p.linkfnull = ctx->d_linkfnull;
+    p.XW = ctx->d_XW; p.vmask = ctx->d_vmask; p.Mcnt = ctx->d_M; p.dlink = ctx->d_dlink;
+    p.plans = ctx->d_plans; p.ext_z = ext_z; p.ext_w = ext_w; p.ext_stride = ext_stride;
+    p.phi = phi_dev; p.status = ctx->d_status;
+    p.S_cap = rt.S_cap;
+    if (rt.draw) TRY(launch_sampler(ctx, rt, &p));
+    if (ctx->dbg_i >= 0) TRY(prepare_debug_dump(ctx, rt.S_cap));
+    CUDA_TRY(record_ev(ctx, 2));
+    ctx->l1_timing_valid = false;
+    if (ctx->l1_mode != 0) TRY(grow(ctx, &ctx->d_mom, &ctx->cap_mom, (size_t)n * ctx->head.l1_nout * (2 * G + 4)));
+    ctx->last_fused = rt.shared == ROUTE_FUSED;
+    // the general kernels (instances that are not on the shared-plan route) fork off here and join at the end
+    cudaStream_t gstream = ctx->stream;
+    if (rt.shared != ROUTE_SHARED_NONE) {
+        ctx->last_path[DKS_PATH_BG_WEIGHTS] = ctx->uniform_w ? 0 : 1;
+        if (ctx->side_stream != nullptr) {
+            CUDA_TRY(cudaEventRecord(ctx->ev_fork, ctx->stream));
+            CUDA_TRY(cudaStreamWaitEvent(ctx->side_stream, ctx->ev_fork, 0));
+            gstream = ctx->side_stream;
+        }
+        const PlanDev& pg = ctx->h_plans[G];
+        if (rt.shared == ROUTE_FUSED || rt.shared == ROUTE_BINARY || rt.shared == ROUTE_BINARY_MEMBERS) {
+            TRY(launch_shared_binary(ctx, rt, pg, phi_dev));
+            if (rt.shared != ROUTE_FUSED) TRY(launch_binary_solve(ctx, rt, pg, phi_dev));
+        } else {
+            dks::shared_path::HeadSource src;
+            TRY(launch_class_sums(ctx, rt, pg, &src));
+            TRY(launch_class_solve(ctx, rt, pg, src, phi_dev));
+        }
+        p.list = ctx->d_idx_other;      // the general kernels take the remaining instances
+        p.count = ctx->d_counts + 1;
+    }
+    if (rt.l1_Mmax > 0) TRY(launch_general_l1(ctx, rt, &p, phi_dev, gstream));
+    TRY(launch_general(ctx, rt, p, gstream));
+    if (gstream != ctx->stream) {
+        CUDA_TRY(cudaEventRecord(ctx->ev_join, gstream));
+        CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+    }
     CUDA_TRY(record_ev(ctx, 3));
     return DKS_OK;
 }
@@ -849,7 +945,7 @@ int check_status(dks_ctx* ctx) {
 
 // projection form of the shared-plan solve of the binary head (and of binary mixtures): P = inv(E^T W E) E^T W and d = P z_L,
 // when it fits the solve kernel's staging
-int build_pmat(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz, const double* dw, const double* di) {
+int build_pmat(dks_ctx* ctx, PlanDev& pd, int M) {
     if (!(pd.W == 1 && M - 1 <= dks::shared_path::PMAT_MAXK &&
           dks::shared_path::wls_pmat_smem(M, pd.S_pad, false) + 8192 <= (size_t)ctx->max_smem_optin))
         return DKS_OK;
@@ -859,8 +955,8 @@ int build_pmat(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz, const doubl
     CUDA_TRY(cudaMalloc((void**)&dv, sizeof(double) * (M - 1)));
     ctx->plan_allocs[M].push_back(pm); ctx->plan_allocs[M].push_back(dv);
     long long tot = (long long)(M - 1) * pd.S_pad;
-    dks::shared_path::plan_pmat_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(dz, dw, di, S, pd.S_pad, M, pm);
-    dks::shared_path::plan_dvec_kernel<<<M - 1, 32, 0, ctx->stream>>>(dz, pm, S, pd.S_pad, M, dv);
+    dks::shared_path::plan_pmat_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(pd.z, pd.w, pd.ainv, S, pd.S_pad, M, pm);
+    dks::shared_path::plan_dvec_kernel<<<M - 1, 32, 0, ctx->stream>>>(pd.z, pm, S, pd.S_pad, M, dv);
     ctx->launches += 2;
     CUDA_TRY(cudaGetLastError());
     pd.pmat = pm; pd.dvec = dv;
@@ -919,7 +1015,7 @@ int build_link_table(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz) {
     }
     std::vector<LinkTabRow> hr(S_pad);
     for (double h : {0.25, 0.125}) {
-        plan_ltab_rows_kernel<<<cdiv(S_pad, 128), 128, 0, st>>>(dz, pd.S, S_pad, ctx->d_BW, ctx->d_scores, N, ctx->G, ctx->scale,
+        plan_ltab_rows_kernel<<<cdiv(S_pad, 128), 128, 0, st>>>(dz, pd.S, S_pad, ctx->d_BW, ctx->d_scores, N, ctx->G, ctx->head.scale,
                                                                 pd.dme, wd, h, ld, rows);
         ctx->launches += 1;
         CUDA_TRY(cudaGetLastError());
@@ -1039,7 +1135,7 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_extw);
     dev_free(&ctx->dbg_T);
     dev_free(&ctx->dbg_time);
-    free_plan_allocs(ctx, -1);
+    for (auto& allocs : ctx->plan_allocs) for (void* q : allocs) cudaFree(q);
     for (int i = 0; i < 4; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
     for (int i = 0; i < 3; ++i) if (ctx->ev_l1[i]) cudaEventDestroy(ctx->ev_l1[i]);
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
@@ -1229,7 +1325,9 @@ int dks_fit(dks_ctx* ctx) {
         for (int c = 0; c < D; ++c) ctx->h_gcols[c] = c;
     }
     const int G = ctx->G;
-    if (ctx->act == DKS_ACT_EXP && ctx->link == DKS_LINK_LOGIT)
+    ctx->head = describe_head(ctx);
+    const HeadDesc& h = ctx->head;
+    if (h.expo && ctx->link == DKS_LINK_LOGIT)
         return fail(DKS_ERR_UNSUPPORTED, "exp head: the logit link is undefined wherever a predicted mean exceeds 1; use the "
                     "identity link");
     {   // every column in exactly one group
@@ -1293,13 +1391,10 @@ int dks_fit(dks_ctx* ctx) {
     CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
 
-    ctx->scale = (ctx->act == DKS_ACT_BINARY_LOGISTIC) ? -ctx->kappa * 1.4426950408889634
-               : (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR || ctx->act == DKS_ACT_EXP || ctx->act == DKS_ACT_MIX)
-                   ? 1.4426950408889634 : 1.0;
     (maps ? (R > 8 ? dks::fit_bw_kernel<true, true> : dks::fit_bw_kernel<true>) : dks::fit_bw_kernel<false>)<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(
         ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D, G, R, ctx->d_BW, ctx->cm, ctx->d_status);
     dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
-    if (ctx->act == DKS_ACT_MIX) {
+    if (h.mixture()) {
         TRY(dev_alloc(&ctx->d_mixBW, (size_t)N * G * R));
         TRY(dev_alloc(&ctx->d_mixsc, (size_t)N * R));
         dks::mix::mix_split_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, N, G, ctx->mix.K,
@@ -1310,8 +1405,8 @@ int dks_fit(dks_ctx* ctx) {
     dks::fit_fnull_kernel<<<1, 256, 0, st>>>(ctx->d_scores, ctx->d_BW, ctx->d_wbg, N, G, R, C, ctx->act, ctx->kappa,
                                               ctx->link, ctx->d_fnull, ctx->d_linkfnull, ctx->d_Bbar, ctx->d_mix);
     dks::fit_scale_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, G, R,
-                                                                              ctx->scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf,
-                                                                              ctx->act == DKS_ACT_EXP ? 1 : 0);
+                                                                              h.scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf,
+                                                                              h.expo ? 1 : 0);
     ctx->launches += 5;
     CUDA_TRY(cudaGetLastError());
     ctx->h_fnull.resize(C);
@@ -1323,22 +1418,14 @@ int dks_fit(dks_ctx* ctx) {
     if (ctx->h_status[0] == DKS_ERR_DOMAIN)
         return fail(DKS_ERR_DOMAIN, "background row %d holds a raw value its column map refuses (NaN, or a category unseen "
                     "at fit time, where the pipeline raises)", ctx->h_status[1]);
-    if (ctx->act == DKS_ACT_EXP && !std::isfinite(ctx->h_fnull[0]))
+    if (h.expo && !std::isfinite(ctx->h_fnull[0]))
         return fail(DKS_ERR_NUMERIC, "exp head: the background's predictions are not all finite in float64 (fnull = %g)",
                     ctx->h_fnull[0]);
     ctx->cap_n = 0;  // workspace shapes depend on G, R, C
     ctx->prepared = false;
-    if (any_plan_allocs(ctx)) {   // plans carry tables derived from the background/model: drop them
-        free_plan_allocs(ctx, -1);
-        memset(ctx->h_plans, 0, sizeof(ctx->h_plans));
-        memset(ctx->h_l1, 0, sizeof(ctx->h_l1));
-        memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
-        memset(ctx->h_expl, 0, sizeof(ctx->h_expl));
-        ctx->mixp = {}; ctx->mixp_M = 0;
-        ctx->max_plan_S = 0;
-        CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));
-        TRY(sync_l1_tables(ctx));
-    }
+    // plans carry tables derived from the background/model: drop them
+    for (const auto& allocs : ctx->plan_allocs)
+        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
     ctx->fitted = true;
     ctx->epoch++;
     return DKS_OK;
@@ -1397,24 +1484,10 @@ int dks_effective_nsamples(dks_ctx* ctx, int M, int* S) {
     return DKS_OK;
 }
 
-int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, const double* w_host) {
-    BIND(ctx);
-    REQUIRE(M >= 2 && M <= DKS_MAX_GROUPS, "dks_set_shared_plan: M=%d out of [2,%d]", M, DKS_MAX_GROUPS);
-    REQUIRE(S >= 1 && zbits_host && w_host, "dks_set_shared_plan: bad arguments");
+// uploads a plan of M groups and factors its normal matrix (plans of more than 128 groups: the host hands the projection
+// over with dks_set_plan_projection)
+static int upload_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, const double* w_host, PlanDev* out) {
     uint64_t* dz = nullptr; double* dw = nullptr; double* dc = nullptr; double* di = nullptr;
-    if (!ctx->plan_allocs[M].empty()) {
-        // replacing the plan of this M (another nsamples): nothing in flight may still read the old buffers
-        CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-        free_plan_allocs(ctx, M);
-        memset(&ctx->h_plans[M], 0, sizeof(PlanDev));
-        memset(&ctx->h_l1[M], 0, sizeof(ctx->h_l1[M]));
-        memset(&ctx->h_smx[M], 0, sizeof(ctx->h_smx[M]));
-        ctx->h_expl[M] = nullptr;
-        if (ctx->mixp_M == M) { ctx->mixp = {}; ctx->mixp_M = 0; }
-        ctx->h_afix[M] = nullptr;
-        ctx->epoch++;
-        TRY(sync_l1_tables(ctx));
-    }
     const int W = dks_plan_words(M);                        // 64-bit words per coalition row
     const size_t S_even = ((size_t)S + 1) & ~(size_t)1;     // TMA bulk copies move 16-byte multiples
     CUDA_TRY(cudaMalloc((void**)&dz, sizeof(uint64_t) * S_even * W));
@@ -1431,136 +1504,145 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
     CUDA_TRY(cudaMemcpyAsync(dz, zbits_host, sizeof(uint64_t) * S * W, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(dw, w_host, sizeof(double) * S, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
-    if (W > 2) {
-        // more than 128 groups: the (M-1) x (M-1) normal matrix is factored by the host, which hands the projection over
-        // with dks_set_plan_projection (the plan is not usable before)
-    } else if (W == 1) {
+    if (W == 1) {
         size_t smem = 2 * sizeof(double) * (size_t)(M - 1) * (M - 1);
         CUDA_TRY(cudaFuncSetAttribute(dks::plan_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         dks::plan_factor_kernel<<<1, 256, smem, ctx->stream>>>(dz, dw, S, M, dc, di, ctx->d_status);
-    } else {
+        ctx->launches += 1;
+    } else if (W == 2) {
         double* scratch = nullptr;
         CUDA_TRY(cudaMalloc((void**)&scratch, sizeof(double) * (M - 1) * (M - 1)));
         ctx->plan_allocs[M].push_back(scratch);
         size_t smem = sizeof(double) * (size_t)(M - 1) * (M - 1);
         CUDA_TRY(cudaFuncSetAttribute(dks::plan_factor_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         dks::plan_factor_wide_kernel<<<1, 1024, smem, ctx->stream>>>(dz, dw, S, M, dc, di, scratch, ctx->d_status);
+        ctx->launches += 1;
     }
-    if (W <= 2) ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (ctx->h_status[0] != 0)
         return fail(DKS_ERR_NUMERIC, "dks_set_shared_plan: normal matrix of the M=%d plan is not positive definite", M);
-    PlanDev pd;
+    PlanDev& pd = *out;
     memset(&pd, 0, sizeof(pd));
     pd.z = dz; pd.w = dw; pd.chol = dc; pd.ainv = di; pd.S = S; pd.W = W;
     pd.S_pad = (S + 31) / 32 * 32;
-    if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_BINARY_LOGISTIC) {
-        // shared-plan fast path: Dm table for the full varying set
-        float* dm = nullptr;
-        double* dme = nullptr;
-        CUDA_TRY(cudaMalloc((void**)&dm, sizeof(float) * (size_t)ctx->N * pd.S_pad));
-        CUDA_TRY(cudaMalloc((void**)&dme, sizeof(double) * (size_t)pd.S_pad));
-        ctx->plan_allocs[M].push_back(dm); ctx->plan_allocs[M].push_back(dme);
-        long long total = (long long)ctx->N * pd.S_pad;
-        dks::shared_path::plan_dme_kernel<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, W, S, pd.S_pad, ctx->d_BW, ctx->d_scores,
-                                                                                       ctx->N, ctx->G, ctx->scale, dme);
-        dks::shared_path::plan_dm_kernel<<<cdiv(total, 256), 256, 0, ctx->stream>>>(dz, W, S, pd.S_pad, ctx->d_BW, ctx->d_scores,
-                                                                                      ctx->N, ctx->G, ctx->scale, dme, dm);
-        ctx->launches += 2;
-        CUDA_TRY(cudaGetLastError());
-        pd.dme = dme;
-        pd.dmT = dm;
-        TRY(build_pmat(ctx, pd, M, dz, dw, di));
+    return DKS_OK;
+}
+
+// the binary head's Dm table and row exponents of a plan, from background contributions BW and scores (one member's for
+// a mixture)
+static int build_dm_tables(dks_ctx* ctx, const PlanDev& pd, int M, const double* BW, const double* scores, double scale,
+                           const float** dm_out, const double** dme_out) {
+    const int N = ctx->N;
+    float* dm = nullptr;
+    double* dme = nullptr;
+    CUDA_TRY(cudaMalloc((void**)&dm, sizeof(float) * (size_t)N * pd.S_pad));
+    CUDA_TRY(cudaMalloc((void**)&dme, sizeof(double) * (size_t)pd.S_pad));
+    ctx->plan_allocs[M].push_back(dm); ctx->plan_allocs[M].push_back(dme);
+    const long long total = (long long)N * pd.S_pad;
+    dks::shared_path::plan_dme_kernel<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(pd.z, pd.W, pd.S, pd.S_pad, BW, scores, N,
+                                                                                   M, scale, dme);
+    dks::shared_path::plan_dm_kernel<<<cdiv(total, 256), 256, 0, ctx->stream>>>(pd.z, pd.W, pd.S, pd.S_pad, BW, scores, N, M,
+                                                                                  scale, dme, dm);
+    ctx->launches += 2;
+    CUDA_TRY(cudaGetLastError());
+    *dm_out = dm; *dme_out = dme;
+    return DKS_OK;
+}
+
+// the softmax / one-vs-rest tables of a plan over C classes (dks_multi.cuh): per-class Dm [CS][N][S_pad] and row bounds
+// [CS][S_pad], the one-vs-rest head keeping one more slot of each (CS = C + 1: nd per element, hi per row)
+static int build_class_tables(dks_ctx* ctx, const PlanDev& pd, int M, const double* BW, const double* scores, int C,
+                              double scale, const float** dm_out, const float** lo_out) {
+    const bool ovr = ctx->head.ovr;
+    const int CS = ovr ? C + 1 : C;
+    float* sd = nullptr; float* sl = nullptr;
+    CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)CS * ctx->N * pd.S_pad));
+    ctx->plan_allocs[M].push_back(sd);
+    CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)CS * pd.S_pad));
+    ctx->plan_allocs[M].push_back(sl);
+    auto kern = ovr ? (pd.W == 1 ? dks::multi::plan_ovr_kernel<1> : dks::multi::plan_ovr_kernel<2>)
+                    : (pd.W == 1 ? dks::multi::plan_softmax_kernel<1> : dks::multi::plan_softmax_kernel<2>);
+    kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(pd.z, pd.S, pd.S_pad, BW, scores, ctx->N, M, C, scale, sd, sl);
+    ctx->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    *dm_out = sd; *lo_out = sl;
+    return DKS_OK;
+}
+
+// what the shared-plan route of the head reads besides the plan, for the full varying set (M == G)
+static int build_full_set_tables(dks_ctx* ctx, PlanDev& pd, int M) {
+    const HeadDesc& h = ctx->head;
+    FullSetTables& ft = ctx->full;
+    ft = FullSetTables{};
+    const MixHead& mh = ctx->mix;
+    const int N = ctx->N;
+    switch (h.shared) {
+    case HEAD_SHARED_BINARY:
+        TRY(build_dm_tables(ctx, pd, M, ctx->d_BW, ctx->d_scores, h.scale, &pd.dmT, &pd.dme));
+        TRY(build_pmat(ctx, pd, M));
         // float64 P, row-major per coalition, for the fused kernel (link + solve inside the coalition kernel)
-        if (W == 1 && M <= 16) {
+        if (pd.W == 1 && M <= 16) {
             const int kpad = dks::shared_path::fused_kpad(M);
             double* pm64 = nullptr; double* dv64 = nullptr;
             CUDA_TRY(cudaMalloc((void**)&pm64, sizeof(double) * (size_t)kpad * pd.S_pad));
             CUDA_TRY(cudaMalloc((void**)&dv64, sizeof(double) * kpad));
             ctx->plan_allocs[M].push_back(pm64); ctx->plan_allocs[M].push_back(dv64);
             long long tot = (long long)kpad * pd.S_pad;
-            dks::shared_path::plan_pmat64_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(dz, dw, di, S, pd.S_pad, M, kpad, pm64);
-            dks::shared_path::plan_dvec64_kernel<<<kpad, 32, 0, ctx->stream>>>(dz, pm64, S, M, kpad, dv64);
+            dks::shared_path::plan_pmat64_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(pd.z, pd.w, pd.ainv, pd.S, pd.S_pad, M,
+                                                                                          kpad, pm64);
+            dks::shared_path::plan_dvec64_kernel<<<kpad, 32, 0, ctx->stream>>>(pd.z, pm64, pd.S, M, kpad, dv64);
             ctx->launches += 2;
             CUDA_TRY(cudaGetLastError());
             pd.pmat64 = pm64; pd.dvec64 = dv64; pd.kpad = kpad;
-            if (ctx->N <= dks::shared_path::MAXN) TRY(build_link_table(ctx, pd, M, dz));
+            if (N <= dks::shared_path::MAXN) TRY(build_link_table(ctx, pd, M, pd.z));
         }
-    }
-    if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_MIX && W <= 2) {
-        // mixture head: each member's tables from its own rows of the background (dks_fit split them per member) -- binary
-        // members the binary head's Dm / dme and projection, softmax / one-vs-rest members the class-sum tables
-        const MixHead& mh = ctx->mix;
-        const int N = ctx->N, Rm = mh.Rm, CS = mh.mact == DKS_ACT_OVR ? Rm + 1 : Rm;
-        const bool bin = mh.mact == DKS_ACT_BINARY_LOGISTIC;
-        dks_ctx::MixPlanDev mp = {};
-        for (int k = 0; k < mh.K; ++k) {
-            const double* BWk = ctx->d_mixBW + (size_t)k * N * M * Rm;
-            const double* sck = ctx->d_mixsc + (size_t)k * N * Rm;
-            if (bin) {
-                float* dm = nullptr; double* dme = nullptr;
-                CUDA_TRY(cudaMalloc((void**)&dm, sizeof(float) * (size_t)N * pd.S_pad));
-                CUDA_TRY(cudaMalloc((void**)&dme, sizeof(double) * (size_t)pd.S_pad));
-                ctx->plan_allocs[M].push_back(dm); ctx->plan_allocs[M].push_back(dme);
-                const long long total = (long long)N * pd.S_pad;
-                dks::shared_path::plan_dme_kernel<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, W, S, pd.S_pad, BWk, sck, N, M,
-                                                                                               -DKS_LOG2E, dme);
-                dks::shared_path::plan_dm_kernel<<<cdiv(total, 256), 256, 0, ctx->stream>>>(dz, W, S, pd.S_pad, BWk, sck, N, M,
-                                                                                              -DKS_LOG2E, dme, dm);
-                ctx->launches += 2;
-                mp.dm[k] = dm; mp.dme[k] = dme;
-            } else {
-                float* sd = nullptr; float* sl = nullptr;
-                CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)CS * N * pd.S_pad));
-                ctx->plan_allocs[M].push_back(sd);
-                CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)CS * pd.S_pad));
-                ctx->plan_allocs[M].push_back(sl);
-                auto kern = mh.mact == DKS_ACT_OVR ? (W == 1 ? dks::multi::plan_ovr_kernel<1> : dks::multi::plan_ovr_kernel<2>)
-                                                   : (W == 1 ? dks::multi::plan_softmax_kernel<1> : dks::multi::plan_softmax_kernel<2>);
-                kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, BWk, sck, N, M, Rm, DKS_LOG2E, sd, sl);
-                ctx->launches += 1;
-                mp.dm[k] = sd; mp.lo[k] = sl;
-            }
+        break;
+    case HEAD_SHARED_MIX_BINARY:
+        // each member's tables from its own rows of the background (dks_fit split them per member)
+        for (int k = 0; k < mh.K; ++k)
+            TRY(build_dm_tables(ctx, pd, M, ctx->d_mixBW + (size_t)k * N * M * mh.Rm, ctx->d_mixsc + (size_t)k * N * mh.Rm,
+                                -DKS_LOG2E, &ft.dm[k], &ft.dme[k]));
+        TRY(build_pmat(ctx, pd, M));
+        break;
+    case HEAD_SHARED_CLASS_SUMS:
+        TRY(build_class_tables(ctx, pd, M, ctx->d_BW, ctx->d_scores, ctx->C, h.scale, &ft.dm[0], &ft.lo[0]));
+        break;
+    case HEAD_SHARED_MIX_CLASS:
+        for (int k = 0; k < mh.K; ++k)
+            TRY(build_class_tables(ctx, pd, M, ctx->d_mixBW + (size_t)k * N * M * mh.Rm, ctx->d_mixsc + (size_t)k * N * mh.Rm,
+                                   mh.Rm, DKS_LOG2E, &ft.dm[k], &ft.lo[k]));
+        break;
+    case HEAD_SHARED_TABLES:
+        if (h.expo) {
+            // exp head: l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) (head_y, dks_shared.cuh)
+            double* el = nullptr;
+            CUDA_TRY(cudaMalloc((void**)&el, sizeof(double) * (size_t)pd.S_pad));
+            ctx->plan_allocs[M].push_back(el);
+            auto kern = pd.W == 1 ? dks::shared_path::plan_exp_kernel<1> : dks::shared_path::plan_exp_kernel<2>;
+            kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(pd.z, pd.S, pd.S_pad, ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, M,
+                                                              h.scale, el);
+            ctx->launches += 1;
             CUDA_TRY(cudaGetLastError());
+            ft.ell = el;
         }
-        if (bin) TRY(build_pmat(ctx, pd, M, dz, dw, di));
-        ctx->mixp = mp; ctx->mixp_M = M;
+        break;
     }
-    if (M == ctx->G && ctx->fitted && (ctx->act == DKS_ACT_SOFTMAX || ctx->act == DKS_ACT_OVR) && W <= 2) {
-        // softmax / one-vs-rest head: per-class Dm table and row bounds for the full varying set (dks_multi.cuh); the
-        // one-vs-rest head keeps one more slot of each (nd per element, hi per row)
-        const int C = ctx->C, CS = ctx->act == DKS_ACT_OVR ? C + 1 : C;
-        float* sd = nullptr; float* sl = nullptr;
-        CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)CS * ctx->N * pd.S_pad));
-        ctx->plan_allocs[M].push_back(sd);
-        CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)CS * pd.S_pad));
-        ctx->plan_allocs[M].push_back(sl);
-        auto kern = ctx->act == DKS_ACT_OVR ? (W == 1 ? dks::multi::plan_ovr_kernel<1> : dks::multi::plan_ovr_kernel<2>)
-                                            : (W == 1 ? dks::multi::plan_softmax_kernel<1> : dks::multi::plan_softmax_kernel<2>);
-        kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW, ctx->d_scores, ctx->N, M, C,
-                                                          ctx->scale, sd, sl);
-        ctx->launches += 1;
-        CUDA_TRY(cudaGetLastError());
-        ctx->h_smx[M].dm = sd; ctx->h_smx[M].lo = sl;
-    }
-    if (M == ctx->G && ctx->fitted && ctx->act == DKS_ACT_EXP && W <= 2) {
-        // exp head: l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) for the full varying set (head_y, dks_shared.cuh)
-        double* el = nullptr;
-        CUDA_TRY(cudaMalloc((void**)&el, sizeof(double) * (size_t)pd.S_pad));
-        ctx->plan_allocs[M].push_back(el);
-        auto kern = W == 1 ? dks::shared_path::plan_exp_kernel<1> : dks::shared_path::plan_exp_kernel<2>;
-        kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(dz, S, pd.S_pad, ctx->d_BW, ctx->d_scores, ctx->d_wbg, ctx->N, M,
-                                                          ctx->scale, el);
-        ctx->launches += 1;
-        CUDA_TRY(cudaGetLastError());
-        ctx->h_expl[M] = el;
-    }
+    ft.M = M;
+    return DKS_OK;
+}
+
+int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, const double* w_host) {
+    BIND(ctx);
+    REQUIRE(M >= 2 && M <= DKS_MAX_GROUPS, "dks_set_shared_plan: M=%d out of [2,%d]", M, DKS_MAX_GROUPS);
+    REQUIRE(S >= 1 && zbits_host && w_host, "dks_set_shared_plan: bad arguments");
+    if (!ctx->plan_allocs[M].empty()) TRY(drop_plans(ctx, M));     // replacing the plan of this M (another nsamples)
+    PlanDev pd;
+    TRY(upload_plan(ctx, M, S, zbits_host, w_host, &pd));
+    if (M == ctx->G && ctx->fitted && M <= ctx->head.shared_max_G) TRY(build_full_set_tables(ctx, pd, M));
     ctx->h_plans[M] = pd;
     ctx->epoch++;
-    ctx->h_afix[M] = nullptr;                       // sampling info of a replaced plan is stale
-    memset(&ctx->h_sinfo[M], 0, sizeof(ctx->h_sinfo[M]));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (S > ctx->max_plan_S) ctx->max_plan_S = S;
@@ -1569,20 +1651,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
 
 int dks_clear_plans(dks_ctx* ctx) {
     BIND(ctx);
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    free_plan_allocs(ctx, -1);
-    ctx->epoch++;
-    memset(ctx->h_plans, 0, sizeof(ctx->h_plans));
-    memset(ctx->h_l1, 0, sizeof(ctx->h_l1));
-    memset(ctx->h_smx, 0, sizeof(ctx->h_smx));
-    memset(ctx->h_expl, 0, sizeof(ctx->h_expl));
-    memset(ctx->h_afix, 0, sizeof(ctx->h_afix));
-    ctx->mixp = {}; ctx->mixp_M = 0;
-    memset(ctx->h_sinfo, 0, sizeof(ctx->h_sinfo));
-    ctx->max_plan_S = 0;
-    CUDA_TRY(cudaMemcpy(ctx->d_plans, ctx->h_plans, sizeof(ctx->h_plans), cudaMemcpyHostToDevice));
-    TRY(sync_l1_tables(ctx));
-    return DKS_OK;
+    return drop_plans(ctx, -1);
 }
 
 int dks_has_shared_plan(dks_ctx* ctx, int M, int* present) {

@@ -146,6 +146,42 @@ struct MixHead {
 #define DKS_EXP_T_LO -60.f
 #define DKS_EXP_T_HI 100.f
 
+// ---- what the host dispatcher knows about the head: filled once per dks_fit (describe_head, dks.cu) ----------------
+enum HeadShared {               // what the shared-plan route of the full varying set evaluates
+    HEAD_SHARED_BINARY,         // the binary-logistic head's Dm tables
+    HEAD_SHARED_CLASS_SUMS,     // per-class sums of the softmax / one-vs-rest coalition kernels
+    HEAD_SHARED_TABLES,         // y from the instance's nibble tables alone (identity; exp with the plan's l(s))
+    HEAD_SHARED_MIX_BINARY,     // mixture of binary-logistic members: the binary head's kernel per member
+    HEAD_SHARED_MIX_CLASS,      // mixture of softmax / one-vs-rest members: the class-sum kernel per member
+};
+struct HeadDesc {
+    int shared = HEAD_SHARED_BINARY;
+    bool ovr = false;           // the class sums (of the head or of its members) are one-vs-rest ones
+    bool expo = false;          // exp head: the plan's l(s) and the exp instantiations of the CUDA-core kernels
+    int shared_max_G = 0;       // the most groups the shared-plan route covers
+    double scale = 1.0;         // applied to the grouped background contributions (fit) and the Dm tables
+    double xt_scale = 1.0;      // of the nibble tables stage 1 writes
+    bool xt_any = false;        // nibble tables for every G and plan mode (else up to 128 groups with shared plans)
+    bool xt_bbar = false;       // nibble tables of XW - Bbar (identity head)
+    int l1_nout = 1;            // outputs the l1 selection solves
+    bool l1_binary = false;     // ... from the binary head's (sum p1, sum p0)
+    int simt_R = 1, simt_C = 1; // score rows and outputs the CUDA-core kernel stages
+    bool wide_pi = false;       // per-instance plans of 65..128 groups
+    bool tc = false;            // tensor-core kernel
+    bool mixture() const { return shared == HEAD_SHARED_MIX_BINARY || shared == HEAD_SHARED_MIX_CLASS; }
+};
+
+// Tables derived from the plan of the full varying set (M == G) that PlanDev does not hold: the class-sum heads' per-class
+// Dm and row bounds (dks_multi.cuh), the exp head's l(s), the mixture members' tables.  Host-only; the buffers belong to
+// plan_allocs[M].
+struct FullSetTables {
+    int M;                              // the plan they were built for (0: none)
+    const float* dm[DKS_MIX_MAX_R];     // per member ([0]: the head itself): binary Dm, or per-class Dm
+    const double* dme[DKS_MIX_MAX_R];   // binary members: row exponents
+    const float* lo[DKS_MIX_MAX_R];     // class sums: row bounds
+    const double* ell;                  // exp head: l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) [S_pad]
+};
+
 // number of instances a general kernel launch handles and the q-th of them
 __device__ __forceinline__ int dks_inst_count(const ExplainParams& p) { return p.list ? *p.count : p.n; }
 __device__ __forceinline__ int dks_inst_at(const ExplainParams& p, int q) { return p.list ? p.list[q] : q; }
@@ -174,11 +210,6 @@ struct dks_ctx {
     MixHead* d_mix = nullptr;   // its device copy (stage 1 and the fit kernels evaluate f(x) in float64 from it)
     double* d_mixBW = nullptr;  // [K][N][G][R_m] the background contributions split per member (plan tables of each member)
     double* d_mixsc = nullptr;  // [K][N][R_m] the background scores split per member
-    // mixture head, full varying set (M == G <= 128): each member's shared-plan tables -- binary members the binary head's
-    // Dm / dme, softmax and one-vs-rest members the class-sum tables (SmxDev); owned by plan_allocs[mixp_M]
-    struct MixPlanDev { const float* dm[DKS_MIX_MAX_R]; const double* dme[DKS_MIX_MAX_R]; const float* lo[DKS_MIX_MAX_R]; };
-    MixPlanDev mixp = {};
-    int mixp_M = 0;             // the M the member tables belong to (0: none)
     float* d_mixscr = nullptr;  // one member's sums before they are added, times pi_k, into the mixture's sums
     size_t cap_mixscr = 0;
     std::vector<double> h_bg, h_wbg, h_W, h_b;
@@ -195,7 +226,7 @@ struct dks_ctx {
     double *d_BW = nullptr, *d_scores = nullptr, *d_Bbar = nullptr, *d_fnull = nullptr, *d_linkfnull = nullptr;
     float *d_BWs = nullptr, *d_bases = nullptr, *d_wbf = nullptr;
     float* d_wn = nullptr;      // [N] N w_j in float: the background weights the weighted shared-plan kernels read
-    double scale = 1.0;
+    HeadDesc head;
     std::vector<double> h_fnull, h_linkfnull;
 
     // plans
@@ -214,14 +245,7 @@ struct dks_ctx {
     int* d_l1_counts = nullptr;                  // [2] their counts
     cudaEvent_t ev_l1[3] = {nullptr, nullptr, nullptr};   // around the general list's moments kernel and LARS
     bool l1_timing_valid = false;
-    // softmax head, full varying set (M == G): per-class Dm [C][N][S_pad] = 2^(d_c(s, j) - max_c d_c(s, j)) and row bounds
-    // lo [C][S_pad] = min_j log2 Dm_c(s, j) (dks_multi.cuh); the one-vs-rest head's tables have one more slot each (nd per
-    // element, hi per row) and Dm relative to nd; owned by plan_allocs[M], cleared with the plan
-    struct SmxDev { const float* dm; const float* lo; };
-    SmxDev h_smx[DKS_MAX_GROUPS + 1] = {};
-    // exp head, full varying set (M == G <= 128): l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) per row [S_pad] (plan_exp_kernel);
-    // owned by plan_allocs[M], cleared with the plan
-    const double* h_expl[DKS_MAX_GROUPS + 1] = {};
+    FullSetTables full = {};     // tables of the plan of the full varying set, cleared with that plan
     double* d_mom = nullptr;     // [n][outputs solved][2G + 4] per-instance moments of y
     size_t cap_mom = 0;
     double* d_yw = nullptr;      // [n][S_pad] link-space y of the wide (more than 128 groups) solve

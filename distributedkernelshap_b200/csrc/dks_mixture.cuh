@@ -43,7 +43,7 @@ inline size_t smem_bytes(int S_cap, int N, int Mmax, const MixHead& mh, int C) {
 }
 
 // One CTA per instance (grid-stride), one thread per coalition row, any plan source (shared, per-instance, caller-supplied).
-// Scores are staged scaled by log2(e) (ctx->scale), so the exponent of member row r is t_r = log2(e) z_r(s, j).
+// Scores are staged scaled by log2(e) (the head's scale), so the exponent of member row r is t_r = log2(e) z_r(s, j).
 //   binary members (R_m = 1): u = 2^-t (t clamped to +-120), p1 = 1 / (1 + u), p0 = u p1 -- the binary head's pair, so
 //     that sum p0 carries no cancellation and the logit link reads log(sum p1 / sum p0);
 //   softmax members: 2^(t_q - max) / sum;  one-vs-rest members: the normalised sigmoids formed as in the one-vs-rest head.

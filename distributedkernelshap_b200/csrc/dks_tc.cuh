@@ -677,11 +677,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) explain_wgmma_kernel(TcParams tp)
 inline int tc_npad(int N) { return (N + 15) / 16 * 16; }
 inline int tc_nb(int N) { return (N + tc::NBLK - 1) / tc::NBLK * tc::NBLK; }
 
-inline bool tc_supported(const dks_ctx* ctx, const ExplainParams& p) {
-    if (ctx->act != DKS_ACT_BINARY_LOGISTIC || ctx->R != 1) return false;
+inline bool tc_supported(const dks_ctx* ctx, int S_cap) {
+    if (!ctx->head.tc) return false;
     if (ctx->G > tc::KP - 1) return false;            // M + constant column must fit one K = 16 step
     if (ctx->N > tc::MAX_NPAD) return false;          // one B operand holds the whole background
-    if ((long long)tc::smem_bytes(p.S_cap, tc_nb(ctx->N)) > (long long)ctx->max_smem_optin) return false;
+    if ((long long)tc::smem_bytes(S_cap, tc_nb(ctx->N)) > (long long)ctx->max_smem_optin) return false;
     return true;
 }
 
