@@ -16,6 +16,7 @@
 #include "dks_wide.cuh"
 #include "dks_sampler.cuh"
 #include "dks_instance_wide.cuh"
+#include "dks_trees.cuh"
 
 namespace {
 
@@ -181,8 +182,13 @@ HeadDesc describe_head(const dks_ctx* ctx) {
             h.shared = HEAD_SHARED_MIX_CLASS; h.ovr = ctx->mix.mact == DKS_ACT_OVR; h.xt_scale = DKS_LOG2E;
         }
         break;
+    case DKS_ACT_TREES:
+        // no shared-plan route: every instance runs the tree kernels; two outputs solve class 1 (class 0 its negation)
+        h.trees = true; h.l1_binary = ctx->C == 2;
+        h.expo = ctx->tree.head == DKS_TREE_HEAD_EXP;
+        break;
     }
-    if (h.shared != HEAD_SHARED_BINARY) h.shared_max_G = 128;
+    if (h.shared != HEAD_SHARED_BINARY && !h.trees) h.shared_max_G = 128;
     if (!h.mixture()) h.xt_scale = h.scale;
     h.l1_nout = h.l1_binary ? 1 : ctx->C;
     return h;
@@ -210,11 +216,25 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     // shared-plan route covers)
     double* xt = (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-    kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
-        X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
-        ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
-        ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-        xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
+    if (h.trees) {
+        // tree ensembles: prep_kernel decides the varying groups (its scores are those of a zero linear model, one identity
+        // output, and unused); the tree kernel then writes f(x) and link(f(x)) - link(fnull) of every output
+        kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
+            X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
+            ctx->d_linkfnull, n, ctx->N, ctx->D, G, 1, 1, DKS_ACT_IDENTITY, 1.0, ctx->link, ipb, ctx->d_XW,
+            ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
+            nullptr, 1.0, nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
+        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->tree, ctx->C, ctx->link,
+                                                                               ctx->d_linkfnull, nullptr, ctx->d_dlink,
+                                                                               ctx->d_status);
+        ctx->launches += 1;
+    } else {
+        kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
+            X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
+            ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
+            ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
+            xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
+    }
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
@@ -369,8 +389,155 @@ int sampler_config(const dks_ctx* ctx, bool wide_pi, SamplerConfig* sc) {
     return DKS_OK;
 }
 
+// tree ensembles: every instance on explain_tree_kernel (up to 64 groups, CUDA-core only), the instances whose M selects
+// through the general list's l1 route -- the kernel's moments, then l1_lars_kernel -- whatever their M, G included
+int choose_route_trees(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
+    const int G = ctx->G, kernel = ctx->kernel_choice;
+    if (kernel != DKS_KERNEL_AUTO && kernel != DKS_KERNEL_SIMT)
+        return fail(DKS_ERR_UNSUPPORTED, "tree ensembles run on the tree kernel only (kernel 'auto' or 'simt')");
+    if (G > 64) return fail(DKS_ERR_UNSUPPORTED, "tree ensembles: %d groups; the tree kernel covers at most 64", G);
+    rt->draw = ctx->plan_mode == 1 && ext_z == nullptr;
+    if (rt->draw) TRY(sampler_config(ctx, false, &rt->sc));
+    const bool per_inst = ext_z != nullptr || rt->draw;
+    rt->S_cap = std::max(ext_z ? ext_stride : rt->draw ? rt->sc.stride : ctx->max_plan_S, 2);
+    rt->smem = dks::trees::smem_bytes(rt->S_cap, ctx->C, ctx->tree.R, ctx->tree.T);
+    if ((long long)rt->smem > (long long)ctx->max_smem_optin)
+        return fail(DKS_ERR_UNSUPPORTED, "tree kernel needs %zu B of shared memory (> %d): nsamples, outputs or trees too many",
+                    rt->smem, ctx->max_smem_optin);
+    if (ctx->l1_mode != 0) {
+        if (per_inst) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
+        for (int M = 2; M <= G; ++M) {
+            if (!((ctx->l1_sel[0] >> (M - 1)) & 1ull)) continue;
+            if (ctx->h_l1[M].gram_raw == nullptr || ctx->h_l1[M].S != dks_effective_S(M, ctx->nsamples_req) ||
+                ctx->h_plans[M].z == nullptr || ctx->h_plans[M].S != ctx->h_l1[M].S)
+                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared plan of M=%d and its l1 tables "
+                            "(dks_set_l1_tables)", M);
+            rt->l1_Mmax = M;
+        }
+        if (rt->l1_Mmax > 0 && !lars_fits(ctx, rt->l1_Mmax))
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory",
+                        rt->l1_Mmax, rt->l1_Mmax);
+        rt->l1_smem = rt->smem;
+    }
+    rt->general = DKS_GENERAL_TREES;
+    return DKS_OK;
+}
+
+// the tree kernel over p.list (L1: its moments); its per-CTA node scratch is sized for the grid
+int launch_tree_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
+    const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
+    TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
+    auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, dks::trees::THREADS, smem, st>>>(p, l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{}, ctx->tree,
+                                                   ctx->cur_X, ctx->D);
+    ctx->launches += 1;
+    return DKS_OK;
+}
+
+// device copy of one tree array (replacing the previous one)
+template <typename T>
+int upload_tree_array(const T** dst, const T* src, size_t n, cudaStream_t st) {
+    T* p = nullptr;
+    TRY(dev_alloc(&p, n));
+    CUDA_TRY(cudaMemcpyAsync(p, src, sizeof(T) * n, cudaMemcpyHostToDevice, st));
+    if (*dst) cudaFree((void*)*dst);
+    *dst = p;
+    return DKS_OK;
+}
+
+void free_tree(dks_ctx* ctx) {
+    TreeDev& t = ctx->tree;
+    for (const void* q : {(const void*)t.feat, (const void*)t.thr, (const void*)t.left, (const void*)t.right, (const void*)t.miss,
+                          (const void*)t.val, (const void*)t.roots, (const void*)t.base, (const void*)t.colgrp,
+                          (const void*)t.bgdir, (const void*)t.xinfo})
+        if (q) cudaFree((void*)q);
+    t.feat = nullptr; t.thr = nullptr; t.left = nullptr; t.right = nullptr; t.miss = nullptr; t.val = nullptr;
+    t.roots = nullptr; t.base = nullptr; t.colgrp = nullptr; t.bgdir = nullptr; t.xinfo = nullptr;
+    ctx->cap_txinfo = 0;
+}
+
+// dks_fit of a tree ensemble: the node arrays, the group of every column, every background row's direction at every node,
+// the column statistics stage 1 decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the tree kernels
+int fit_trees(dks_ctx* ctx) {
+    const int N = ctx->N, D = ctx->D, G = ctx->G, C = ctx->C;
+    const cudaStream_t st = ctx->stream;
+    TreeDev& t = ctx->tree;
+    const size_t nodes = (size_t)t.nodes;
+    TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
+    TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
+    TRY(dev_alloc(&ctx->d_W, (size_t)D));
+    TRY(dev_alloc(&ctx->d_b, (size_t)1));
+    TRY(dev_alloc(&ctx->d_goff, (size_t)G + 1));
+    TRY(dev_alloc(&ctx->d_gcols, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colmin, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colmax, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colnan, (size_t)D));
+    TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
+    TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
+    {
+        int* hdr = const_cast<int*>(ctx->cm.hdr);
+        double* keys = const_cast<double*>(ctx->cm.keys);
+        double* vals = const_cast<double*>(ctx->cm.vals);
+        dev_free(&hdr); dev_free(&keys); dev_free(&vals);
+        ctx->cm = ColumnMapsDev{};
+    }
+    std::vector<int32_t> colgrp(D, 0);
+    for (int g = 0; g < G; ++g)
+        for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
+    free_tree(ctx);
+    TRY(upload_tree_array(&t.feat, ctx->h_tfeat.data(), nodes, st));
+    TRY(upload_tree_array(&t.thr, ctx->h_tthr.data(), nodes, st));
+    TRY(upload_tree_array(&t.left, ctx->h_tleft.data(), nodes, st));
+    TRY(upload_tree_array(&t.right, ctx->h_tright.data(), nodes, st));
+    TRY(upload_tree_array(&t.miss, ctx->h_tmiss.data(), nodes, st));
+    TRY(upload_tree_array(&t.val, ctx->h_tval.data(), nodes * t.R, st));
+    TRY(upload_tree_array(&t.roots, ctx->h_troots.data(), (size_t)t.T, st));
+    TRY(upload_tree_array(&t.base, ctx->h_tbase.data(), (size_t)t.R, st));
+    TRY(upload_tree_array(&t.colgrp, colgrp.data(), (size_t)D, st));
+    unsigned char* bgdir = nullptr;
+    TRY(dev_alloc(&bgdir, (size_t)N * nodes));
+    t.bgdir = bgdir;
+    double* pred = nullptr;
+    TRY(dev_alloc(&pred, (size_t)N * C));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_W, ctx->h_W.data(), sizeof(double) * D, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_b, ctx->h_b.data(), sizeof(double), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
+    dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
+    dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, st>>>(ctx->d_bg, N, D, t, bgdir);
+    dks::trees::tree_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(ctx->d_bg, N, D, t, C, ctx->link, nullptr, pred, nullptr,
+                                                                  nullptr);
+    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
+    ctx->launches += 4;
+    CUDA_TRY(cudaGetLastError());
+    ctx->h_fnull.resize(C);
+    ctx->h_linkfnull.resize(C);
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    cudaFree(pred);
+    for (int c = 0; c < C; ++c)
+        if (!std::isfinite(ctx->h_linkfnull[c]))
+            return fail(DKS_ERR_NUMERIC, "tree ensemble: link(fnull) of output %d is not finite (fnull = %g): the background's "
+                        "mean prediction is 0 or 1 under the logit link, or overflows", c, ctx->h_fnull[c]);
+    ctx->cap_n = 0;
+    ctx->prepared = false;
+    for (const auto& allocs : ctx->plan_allocs)
+        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
+    ctx->fitted = true;
+    ctx->epoch++;
+    return DKS_OK;
+}
+
 int choose_route(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
     const HeadDesc& h = ctx->head;
+    if (h.trees) {
+        *rt = Route{};
+        return choose_route_trees(ctx, ext_z, ext_stride, rt);
+    }
     const int G = ctx->G, N = ctx->N, kernel = ctx->kernel_choice;
     const bool auto_or_shared = kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED;
     *rt = Route{};
@@ -796,20 +963,26 @@ int launch_general_l1(dks_ctx* ctx, const Route& rt, ExplainParams* p, double* p
                                                              ctx->d_idx_sel, ctx->d_idx_plain, ctx->d_l1_counts);
     ExplainParams ps = *p;
     ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
-    const bool mixh = ctx->head.mixture();
-    auto l1kern = ctx->head.expo ? dks::explain_simt_kernel<true, true> : dks::explain_simt_kernel<true>;
-    CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<true> : (const void*)l1kern,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rt.l1_smem));
-    const int grid = persistent_grid(ctx, rt.l1_smem, 1024, 8, n);
     const bool timed = !ctx->capturing;
-    if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
-    if (mixh)
-        dks::mix::explain_simt_mix_kernel<true><<<grid, 256, rt.l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
-                                                                                   ctx->mix);
-    else
-        l1kern<<<grid, 256, rt.l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
-                                                   ExpBackground{ctx->d_BW, ctx->d_scores});
-    ctx->launches += 2;
+    if (ctx->head.trees) {
+        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
+        TRY(launch_tree_kernel(ctx, true, ps, rt.l1_smem, gstream));
+        ctx->launches += 1;
+    } else {
+        const bool mixh = ctx->head.mixture();
+        auto l1kern = ctx->head.expo ? dks::explain_simt_kernel<true, true> : dks::explain_simt_kernel<true>;
+        CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<true> : (const void*)l1kern,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rt.l1_smem));
+        const int grid = persistent_grid(ctx, rt.l1_smem, 1024, 8, n);
+        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
+        if (mixh)
+            dks::mix::explain_simt_mix_kernel<true><<<grid, 256, rt.l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
+                                                                                       ctx->mix);
+        else
+            l1kern<<<grid, 256, rt.l1_smem, gstream>>>(ps, dks::SimtL1{ctx->d_l1, ctx->d_mom},
+                                                       ExpBackground{ctx->d_BW, ctx->d_scores});
+        ctx->launches += 2;
+    }
     if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[1], gstream));
     dks::l1::Params lp = l1_params(ctx, n, phi_dev);
     lp.Mmax = rt.l1_Mmax; lp.Mcnt = ctx->d_M; lp.vmask = ctx->d_vmask; lp.list = ctx->d_idx_sel; lp.count = ctx->d_l1_counts;
@@ -843,6 +1016,9 @@ int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t 
         break;
     case DKS_GENERAL_TC:
         TRY(dks::tc_launch(ctx, p, gstream));
+        break;
+    case DKS_GENERAL_TREES:
+        TRY(launch_tree_kernel(ctx, false, p, rt.smem, gstream));
         break;
     default: {
         const bool mixh = ctx->head.mixture();
@@ -1124,6 +1300,7 @@ int dks_destroy(dks_ctx* ctx) {
     if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
     dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b); dev_free(&ctx->d_mix);
     dev_free(&ctx->d_mixBW); dev_free(&ctx->d_mixsc); dev_free(&ctx->d_mixscr);
+    free_tree(ctx);
     if (ctx->cm.hdr) { cudaFree((void*)ctx->cm.hdr); cudaFree((void*)ctx->cm.keys); cudaFree((void*)ctx->cm.vals); }
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
@@ -1265,6 +1442,60 @@ int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* 
     return DKS_OK;
 }
 
+int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const double* threshold, const int32_t* left,
+                       const int32_t* right, const uint8_t* missing_left, const double* value, int R, int n_trees,
+                       const int32_t* roots, const double* base, int head, int cmp, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_tree_model: call dks_set_background first (D unknown)");
+    REQUIRE(n_nodes > 0 && n_trees > 0 && feature && threshold && left && right && missing_left && value && roots && base,
+            "dks_set_tree_model: need the node arrays, roots and base");
+    if (R < 1 || R > DKS_TREE_MAX_R)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: R=%d raw scores; 1..%d supported", R, DKS_TREE_MAX_R);
+    if (cmp != DKS_TREE_CMP_F32 && cmp != DKS_TREE_CMP_F64)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: unknown comparison %d", cmp);
+    int C;
+    switch (head) {
+    case DKS_TREE_HEAD_IDENTITY: C = R; break;
+    case DKS_TREE_HEAD_SIGMOID: REQUIRE(R == 1, "sigmoid tree head needs R == 1 (got %d)", R); C = 2; break;
+    case DKS_TREE_HEAD_SOFTMAX: REQUIRE(R >= 2, "softmax tree head needs R >= 2 (got %d)", R); C = R; break;
+    case DKS_TREE_HEAD_EXP: REQUIRE(R == 1, "exp tree head needs R == 1 (got %d)", R); C = 1; break;
+    default: return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: unknown head %d", head);
+    }
+    for (int nd = 0; nd < n_nodes; ++nd) {
+        const int f = feature[nd];
+        if (f < 0) {
+            for (int q = 0; q < R; ++q)
+                if (!std::isfinite(value[(size_t)nd * R + q]))
+                    return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: leaf %d has a non-finite value", nd);
+            continue;
+        }
+        if (f >= ctx->D || std::isnan(threshold[nd]) || left[nd] <= nd || right[nd] <= nd || left[nd] >= n_nodes ||
+            right[nd] >= n_nodes)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: node %d is malformed (feature %d of %d, children %d / %d "
+                        "must follow it)", nd, f, ctx->D, left[nd], right[nd]);
+    }
+    for (int k = 0; k < n_trees; ++k)
+        if (roots[k] < 0 || roots[k] >= n_nodes) return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: root %d out of range", k);
+    for (int q = 0; q < R; ++q)
+        if (!std::isfinite(base[q])) return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: base must be finite");
+    ctx->h_tfeat.assign(feature, feature + n_nodes);
+    ctx->h_tthr.assign(threshold, threshold + n_nodes);
+    ctx->h_tleft.assign(left, left + n_nodes);
+    ctx->h_tright.assign(right, right + n_nodes);
+    ctx->h_tmiss.assign(missing_left, missing_left + n_nodes);
+    ctx->h_tval.assign(value, value + (size_t)n_nodes * R);
+    ctx->h_troots.assign(roots, roots + n_trees);
+    ctx->h_tbase.assign(base, base + R);
+    ctx->tree.nodes = n_nodes; ctx->tree.T = n_trees; ctx->tree.R = R; ctx->tree.head = head; ctx->tree.cmp = cmp;
+    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
+    ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_TREES; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
+    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+    ctx->h_W.assign((size_t)ctx->D, 0.0);
+    ctx->h_b.assign(1, 0.0);
+    ctx->fitted = false;
+    return DKS_OK;
+}
+
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
                         const double* vals_host, int n_vals) {
     BIND(ctx);
@@ -1274,6 +1505,7 @@ int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, con
         return DKS_OK;
     }
     REQUIRE(ctx->R > 0, "dks_set_column_maps: call dks_set_model first");
+    if (ctx->act == DKS_ACT_TREES) return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for tree ensembles");
     if (D != ctx->D || R != ctx->R)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: maps of %d columns x %d score rows, model has %d x %d", D, R,
                     ctx->D, ctx->R);
@@ -1338,6 +1570,7 @@ int dks_fit(dks_ctx* ctx) {
             REQUIRE(seen[c]++ == 0, "column %d appears in more than one group", c);
         }
     }
+    if (h.trees) return fit_trees(ctx);
     TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
     TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
     TRY(dev_alloc(&ctx->d_W, (size_t)R * D));
@@ -1457,8 +1690,12 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     TRY(dev_alloc(&dO, (size_t)n * ctx->C));
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
-    (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
-        dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status, ctx->d_mix);
+    if (ctx->head.trees)
+        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->tree, ctx->C, ctx->link,
+                                                                               nullptr, dO, nullptr, nullptr);
+    else
+        (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
+            dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status, ctx->d_mix);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(out_host, dO, sizeof(double) * n * ctx->C, cudaMemcpyDeviceToHost, ctx->stream));

@@ -141,6 +141,25 @@ struct MixHead {
     double pi[DKS_MIX_MAX_R];    // pi_k > 0, sum 1
 };
 
+// tree ensembles (dks_set_tree_model, DESIGN.md §5.0.11): every tree's nodes concatenated; raw scores r = base + sum over
+// trees of the leaf value [R], then the head DKS_TREE_HEAD_*.  A split sends x left when x <= thr (DKS_TREE_CMP_F32: the value
+// cast to float32 first, as sklearn.tree does), NaN where miss says.  Children have larger indices than their parent.
+#define DKS_TREE_MAX_R 8
+struct TreeDev {
+    const int* feat;             // [nodes] split column, -1 at a leaf
+    const double* thr;           // [nodes]
+    const int* left;             // [nodes] global node indices
+    const int* right;
+    const unsigned char* miss;   // [nodes] 1: NaN goes left
+    const double* val;           // [nodes][R] leaf values (learning rate / 1 over T folded in)
+    const int* roots;            // [T]
+    const double* base;          // [R]
+    const int* colgrp;           // [D] group of each column
+    const unsigned char* bgdir;  // [N][nodes] 1: background row j goes left at the node (internal nodes)
+    unsigned char* xinfo;        // [CTAs][nodes] explain kernel scratch: (x goes left) << 7 | varying position (127: none)
+    int nodes, T, R, head, cmp;
+};
+
 // exp head, CUDA-core kernels (DESIGN.md §5.0.8): a coalition row is summed in fp32 when the largest weighted background
 // exponent t'_j = log2 e d(s, j) + log2 w_j lies in [EXP_T_LO, EXP_T_HI]; other rows are evaluated in float64
 #define DKS_EXP_T_LO -60.f
@@ -168,6 +187,7 @@ struct HeadDesc {
     int simt_R = 1, simt_C = 1; // score rows and outputs the CUDA-core kernel stages
     bool wide_pi = false;       // per-instance plans of 65..128 groups
     bool tc = false;            // tensor-core kernel
+    bool trees = false;         // tree ensemble: the tree kernels only (dks_trees.cuh)
     bool mixture() const { return shared == HEAD_SHARED_MIX_BINARY || shared == HEAD_SHARED_MIX_CLASS; }
 };
 
@@ -212,6 +232,12 @@ struct dks_ctx {
     double* d_mixsc = nullptr;  // [K][N][R_m] the background scores split per member
     float* d_mixscr = nullptr;  // one member's sums before they are added, times pi_k, into the mixture's sums
     size_t cap_mixscr = 0;
+    // tree ensemble (act == DKS_ACT_TREES): host copies of the node arrays, and their device copies built by dks_fit
+    std::vector<int32_t> h_tfeat, h_tleft, h_tright, h_troots;
+    std::vector<double> h_tthr, h_tval, h_tbase;
+    std::vector<unsigned char> h_tmiss;
+    TreeDev tree = {};
+    size_t cap_txinfo = 0;
     std::vector<double> h_bg, h_wbg, h_W, h_b;
     std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
     std::vector<double> h_cm_keys, h_cm_vals;

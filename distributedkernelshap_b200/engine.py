@@ -16,6 +16,7 @@ from . import _cabi
 from .data import DenseData, convert_to_data, convert_to_link
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
 from .predictors import extract_linear_spec
+from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_tree_spec
 
 logger = logging.getLogger(__name__)
 
@@ -153,8 +154,9 @@ class GpuKernelExplainer:
         self.lib = _cabi.load()
         self.link = convert_to_link(link)
         self.model_callable = model
-        self.spec = extract_linear_spec(model)
-        if self.spec.activation == "exp" and str(self.link) == "logit":
+        tree_spec = extract_tree_spec(model)
+        self.spec = tree_spec if tree_spec is not None else extract_linear_spec(model)
+        if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
                                       "link log(ey / (1 - ey)) is undefined wherever a predicted mean exceeds 1")
         self.data = convert_to_data(data)
@@ -184,8 +186,17 @@ class GpuKernelExplainer:
         cols = np.ascontiguousarray(np.concatenate([np.asarray(g, dtype=np.int32) for g in self.data.groups]), dtype=np.int32)
         _cabi.check(self.lib.dks_set_groups(self._ctx, _cabi.ptr(offsets), _cabi.ptr(cols), self.data.groups_size))
         maps = self.spec.maps
-        W = self.spec.W if maps is None else np.zeros((self.spec.R, self.P))    # not read once the maps are set
-        if self.spec.activation == "mixture":
+        if tree_spec is not None and self.data.groups_size > TREE_MAX_GROUPS:
+            raise NotImplementedError(f"{self.data.groups_size} groups: tree ensembles are explained up to "
+                                      f"{TREE_MAX_GROUPS} groups")
+        W = None if tree_spec is not None else self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
+        if tree_spec is not None:
+            t = tree_spec
+            _cabi.check(self.lib.dks_set_tree_model(
+                self._ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
+                _cabi.ptr(t.missing_left), _cabi.ptr(t.value), t.R, t.n_trees, _cabi.ptr(t.roots), _cabi.ptr(t.base),
+                t.head_code, t.cmp, int(t.scalar_out)))
+        elif self.spec.activation == "mixture":
             member = {"binary_logistic": _cabi.ACT_BINARY_LOGISTIC, "softmax": _cabi.ACT_SOFTMAX,
                       "ovr": _cabi.ACT_OVR}[self.spec.member]
             _cabi.check(self.lib.dks_set_mixture(self._ctx, self.spec.K, member, self.spec.R // self.spec.K, _cabi.ptr(W),
@@ -629,7 +640,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp", "mixture"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees"),
     }
 
     def last_path(self):
@@ -639,7 +650,8 @@ class GpuKernelExplainer:
         coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
-        are reported as unsupported, not computed, or 'simt_wide': per-instance plans of 65..128 groups), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
+        are reported as unsupported, not computed, 'simt_wide': per-instance plans of 65..128 groups, or 'trees': the tree
+        kernel, which takes every instance of a tree ensemble), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
         the weighted one), ``fused_table`` (1: the fused kernel read y from the plan's link table, passes outside its

@@ -1,0 +1,299 @@
+"""Tree ensembles of scikit-learn read into flat node arrays (``TreeEnsembleSpec``) for the device's tree route.
+
+A spec is what ``dks_set_tree_model`` takes (include/dks.h): every tree's nodes concatenated, a raw score per model row
+``r = base + sum_t leaf_t(x)`` and a head applied to it:
+
+* ``DecisionTree*``, ``RandomForest*``, ``ExtraTrees*``: identity head over the mean of the trees' leaf outputs (class
+  fractions of ``tree_.value`` for classifiers, the leaf value for regressors); ``1/T`` is folded into the leaves.
+* ``GradientBoosting*``: the learning rate is folded into the leaves and ``base`` is the initial raw prediction
+  (``init_`` a ``DummyClassifier`` / ``DummyRegressor`` or ``'zero'``).  ``predict_proba``: ``[1 - expit(r), expit(r)]``
+  for two classes, a softmax over the K raw scores (K trees per stage) otherwise; ``decision_function`` / ``predict`` of
+  the regressor: identity.
+* ``HistGradientBoosting*``: as gradient boosting, ``base`` the baseline prediction; the regressor's ``predict`` is
+  ``exp(r)`` under a log-link loss (``'poisson'``, ``'gamma'``).
+
+A split sends x left when ``x <= threshold``: ``sklearn.tree`` compares the value cast to float32 (``DTYPE``), the
+histogram-based estimators compare float64 values.  NaN goes where the node's ``missing_go_to_left`` says.
+``TreeEnsembleSpec.__call__`` evaluates the same thing in NumPy.
+"""
+import numpy as np
+
+MAX_OUTPUTS = 8
+MAX_GROUPS = 64
+HEADS = ("identity", "sigmoid", "softmax", "exp")     # DKS_TREE_HEAD_* codes 0..3
+CMP_F32, CMP_F64 = 0, 1                               # DKS_TREE_CMP_*
+
+_SKTREE_FORESTS = {"DecisionTreeClassifier", "DecisionTreeRegressor", "ExtraTreeClassifier", "ExtraTreeRegressor",
+                   "RandomForestClassifier", "RandomForestRegressor", "ExtraTreesClassifier", "ExtraTreesRegressor"}
+_GB = {"GradientBoostingClassifier", "GradientBoostingRegressor"}
+_HGB = {"HistGradientBoostingClassifier", "HistGradientBoostingRegressor"}
+_TREE_MODELS = _SKTREE_FORESTS | _GB | _HGB
+# estimators that hold other estimators: a tree model inside one of them is refused by name
+_CONTAINERS = {"Pipeline", "VotingClassifier", "VotingRegressor", "BaggingClassifier", "BaggingRegressor",
+               "CalibratedClassifierCV", "StackingClassifier", "StackingRegressor", "OneVsRestClassifier",
+               "OneVsOneClassifier", "MultiOutputRegressor", "MultiOutputClassifier"}
+
+
+class TreeEnsembleSpec:
+    """Flat node arrays of a tree ensemble and its head.
+
+    feature [nodes] int32 (-1 at a leaf), threshold [nodes] float64, left / right [nodes] int32 (global node indices; -1 at
+    a leaf), missing_left [nodes] uint8, value [nodes, R] float64 (leaf outputs, scaled), roots [T] int32, base [R],
+    head in ``HEADS``, cmp ``CMP_F32`` / ``CMP_F64``."""
+
+    activation = "trees"
+    act_code = 6          # DKS_ACT_TREES
+    maps = None
+
+    def __init__(self, feature, threshold, left, right, missing_left, value, roots, base, head, cmp, n_features,
+                 scalar_out=False, n_outputs=None):
+        self.feature = np.ascontiguousarray(feature, dtype=np.int32)
+        self.threshold = np.ascontiguousarray(threshold, dtype=np.float64)
+        self.left = np.ascontiguousarray(left, dtype=np.int32)
+        self.right = np.ascontiguousarray(right, dtype=np.int32)
+        self.missing_left = np.ascontiguousarray(missing_left, dtype=np.uint8)
+        self.value = np.ascontiguousarray(np.atleast_2d(value), dtype=np.float64)
+        self.roots = np.ascontiguousarray(roots, dtype=np.int32)
+        self.base = np.ascontiguousarray(np.atleast_1d(base), dtype=np.float64)
+        self.head = head
+        self.cmp = int(cmp)
+        self.n_features = int(n_features)
+        self.scalar_out = bool(scalar_out)
+        self.R = self.value.shape[1]
+        self.n_outputs = int(n_outputs if n_outputs is not None else (2 if head == "sigmoid" else self.R))
+        if head not in HEADS:
+            raise ValueError(f"unknown tree head {head!r}")
+        if self.n_outputs > MAX_OUTPUTS:
+            raise NotImplementedError(f"{self.n_outputs} model outputs: the tree route covers at most {MAX_OUTPUTS}")
+
+    @property
+    def head_code(self):
+        return HEADS.index(self.head)
+
+    @property
+    def n_nodes(self):
+        return len(self.feature)
+
+    @property
+    def n_trees(self):
+        return len(self.roots)
+
+    def raw(self, X):
+        """r = base + sum over trees of the leaf value [n, R], trees added in order."""
+        X = np.atleast_2d(np.asarray(X, dtype=np.float64))
+        Xc = X.astype(np.float32).astype(np.float64) if self.cmp == CMP_F32 else X
+        n = X.shape[0]
+        out = np.tile(self.base, (n, 1))
+        rows = np.arange(n)
+        for root in self.roots:
+            node = np.full(n, root, dtype=np.int64)
+            while True:
+                f = self.feature[node]
+                inner = f >= 0
+                if not inner.any():
+                    break
+                v = Xc[rows[inner], f[inner]]
+                nd = node[inner]
+                go_left = np.where(np.isnan(v), self.missing_left[nd] != 0, v <= self.threshold[nd])
+                node[inner] = np.where(go_left, self.left[nd], self.right[nd])
+            out += self.value[node]
+        return out
+
+    def __call__(self, X):
+        """The scikit-learn method the spec was read from, in NumPy."""
+        r = self.raw(X)
+        if self.head == "sigmoid":
+            p1 = 1.0 / (1.0 + np.exp(-r[:, 0]))
+            out = np.stack([1.0 - p1, p1], axis=1)
+        elif self.head == "softmax":
+            e = np.exp(r - r.max(axis=1, keepdims=True))
+            out = e / e.sum(axis=1, keepdims=True)
+        elif self.head == "exp":
+            out = np.exp(r)
+        else:
+            out = r
+        return out[:, 0] if self.scalar_out else out
+
+
+def _names(obj):
+    return {c.__name__ for c in type(obj).__mro__ if c.__module__.startswith("sklearn.")}
+
+
+def _contains_tree(obj, depth=0):
+    if depth > 6 or obj is None:
+        return False
+    if _names(obj) & _TREE_MODELS:
+        return True
+    kids = []
+    for attr in ("steps", "estimators", "estimators_", "calibrated_classifiers_", "estimator", "base_estimator",
+                 "estimator_", "final_estimator_"):
+        v = getattr(obj, attr, None)
+        if v is None or isinstance(v, str):
+            continue
+        if isinstance(v, (list, tuple, np.ndarray)):
+            for e in np.ravel(np.asarray(v, dtype=object)) if isinstance(v, np.ndarray) else v:
+                kids.append(e[-1] if isinstance(e, tuple) else e)
+        else:
+            kids.append(v)
+    for k in kids:
+        if hasattr(k, "estimator") and not (_names(k) & (_CONTAINERS | _TREE_MODELS)):
+            k = k.estimator                 # calibrated classifier wrappers
+        if _contains_tree(k, depth + 1):
+            return True
+    return False
+
+
+def _flatten(trees, n_features):
+    """trees: list of (feature, threshold, left, right, missing_left, value [nodes, R]) with tree-local child indices."""
+    feats, thrs, lefts, rights, miss, vals, roots = [], [], [], [], [], [], []
+    off = 0
+    for f, t, l, r, m, v in trees:
+        f = np.asarray(f, dtype=np.int64)
+        leaf = f < 0
+        roots.append(off)
+        feats.append(np.where(leaf, -1, f))
+        thrs.append(np.where(leaf, 0.0, np.asarray(t, dtype=np.float64)))
+        lefts.append(np.where(leaf, -1, np.asarray(l, dtype=np.int64) + off))
+        rights.append(np.where(leaf, -1, np.asarray(r, dtype=np.int64) + off))
+        miss.append(np.asarray(m, dtype=np.uint8))
+        vals.append(np.where(leaf[:, None], np.asarray(v, dtype=np.float64), 0.0))
+        off += len(f)
+    if off >= 2 ** 31 - 1:
+        raise NotImplementedError("tree ensemble with more than 2^31 nodes")
+    out = [np.concatenate(a) for a in (feats, thrs, lefts, rights, miss, vals)]
+    if (out[0] >= n_features).any():
+        raise ValueError("a split refers to a feature the model does not have")
+    return out + [np.asarray(roots)]
+
+
+def _sk_tree(est, value):
+    t = est.tree_
+    feature = np.where(t.children_left < 0, -1, t.feature)
+    miss = getattr(t, "missing_go_to_left", np.zeros(t.node_count, dtype=np.uint8))
+    return feature, t.threshold, t.children_left, t.children_right, miss, value
+
+
+def _classifier_fractions(est, n_classes):
+    v = np.asarray(est.tree_.value[:, 0, :n_classes], dtype=np.float64)
+    s = v.sum(axis=1, keepdims=True)
+    s[s == 0.0] = 1.0
+    return v / s
+
+
+def _forest_spec(owner, method, names):
+    ests = list(getattr(owner, "estimators_", [owner]))
+    P = int(owner.n_features_in_)
+    if getattr(owner, "n_outputs_", 1) != 1:
+        raise NotImplementedError(f"{type(owner).__name__} with {owner.n_outputs_} outputs: multi-output trees are not "
+                                  "supported")
+    T = len(ests)
+    if hasattr(owner, "classes_"):
+        if method != "predict_proba":
+            raise TypeError(f"{type(owner).__name__}.{method} is not supported: pass predict_proba (predict returns labels)")
+        C = len(owner.classes_)
+        if C > MAX_OUTPUTS:
+            raise NotImplementedError(f"{C} classes: the tree route covers at most {MAX_OUTPUTS} outputs")
+        trees = [_sk_tree(e, _classifier_fractions(e, C) / T) for e in ests]
+        arrs = _flatten(trees, P)
+        return TreeEnsembleSpec(*arrs[:6], arrs[6], np.zeros(C), "identity", CMP_F32, P)
+    if method != "predict":
+        raise TypeError(f"{type(owner).__name__}.{method} is not supported: pass predict")
+    trees = [_sk_tree(e, np.asarray(e.tree_.value[:, 0, :1], dtype=np.float64) / T) for e in ests]
+    arrs = _flatten(trees, P)
+    return TreeEnsembleSpec(*arrs[:6], arrs[6], np.zeros(1), "identity", CMP_F32, P, scalar_out=True)
+
+
+def _gb_spec(owner, method, names):
+    P = int(owner.n_features_in_)
+    init = owner.init_
+    if not (isinstance(init, str) and init == "zero") and not (_names(init) & {"DummyClassifier", "DummyRegressor"}):
+        raise NotImplementedError(f"{type(owner).__name__} with init={type(init).__name__}: only the default "
+                                  "(DummyClassifier / DummyRegressor) or 'zero' initial estimator is supported")
+    stages = owner.estimators_            # [n_stages, K] DecisionTreeRegressor
+    K = stages.shape[1]
+    base = np.asarray(owner._raw_predict_init(np.zeros((1, P))), dtype=np.float64).reshape(-1)
+    lr = float(owner.learning_rate)
+    trees = []
+    for s in range(stages.shape[0]):
+        for k in range(K):
+            e = stages[s, k]
+            v = np.zeros((e.tree_.node_count, K))
+            v[:, k] = lr * e.tree_.value[:, 0, 0]
+            trees.append(_sk_tree(e, v))
+    arrs = _flatten(trees, P)
+    return _boosted_head(owner, method, arrs, base, K, CMP_F32, P)
+
+
+def _boosted_head(owner, method, arrs, base, K, cmp, P, link_exp=False):
+    name = type(owner).__name__
+    if hasattr(owner, "classes_"):
+        C = len(owner.classes_)
+        if C > MAX_OUTPUTS:
+            raise NotImplementedError(f"{C} classes: the tree route covers at most {MAX_OUTPUTS} outputs")
+        if method == "predict_proba":
+            return TreeEnsembleSpec(*arrs[:6], arrs[6], base, "sigmoid" if K == 1 else "softmax", cmp, P)
+        if method == "decision_function":
+            return TreeEnsembleSpec(*arrs[:6], arrs[6], base, "identity", cmp, P, scalar_out=K == 1)
+        raise TypeError(f"{name}.{method} is not supported: pass predict_proba or decision_function")
+    if method != "predict":
+        raise TypeError(f"{name}.{method} is not supported: pass predict")
+    if K != 1:
+        raise NotImplementedError(f"{name} with {K} outputs: multi-output regressors are not supported")
+    return TreeEnsembleSpec(*arrs[:6], arrs[6], base, "exp" if link_exp else "identity", cmp, P, scalar_out=True)
+
+
+def _hgb_spec(owner, method, names):
+    P = int(owner.n_features_in_)
+    if getattr(owner, "_preprocessor", None) is not None:
+        raise NotImplementedError(f"{type(owner).__name__} with categorical features (a fitted _preprocessor): "
+                                  "categorical splits are not supported")
+    cat = getattr(owner, "is_categorical_", None)
+    if cat is not None and np.any(cat):
+        raise NotImplementedError(f"{type(owner).__name__} with categorical features: categorical splits are not supported")
+    K = int(owner.n_trees_per_iteration_)
+    base = np.asarray(owner._baseline_prediction, dtype=np.float64).reshape(-1)
+    trees = []
+    for it in owner._predictors:
+        for k, pred in enumerate(it):
+            nd = pred.nodes
+            if np.any(nd["is_categorical"]):
+                raise NotImplementedError("categorical splits are not supported")
+            leaf = nd["is_leaf"].astype(bool)
+            v = np.zeros((len(nd), K))
+            v[:, k] = np.where(leaf, nd["value"], 0.0)
+            f = np.where(leaf, -1, nd["feature_idx"].astype(np.int64))
+            trees.append((f, nd["num_threshold"], nd["left"], nd["right"], nd["missing_go_to_left"], v))
+    arrs = _flatten(trees, P)
+    link_exp = False
+    if not hasattr(owner, "classes_"):
+        link = type(getattr(getattr(owner, "_loss", None), "link", None)).__name__
+        if link not in ("IdentityLink", "LogLink"):
+            raise NotImplementedError(f"{type(owner).__name__} with loss {owner.loss!r}: identity or log link only")
+        link_exp = link == "LogLink"
+    return _boosted_head(owner, method, arrs, base, K, CMP_F64, P, link_exp=link_exp)
+
+
+def extract_tree_spec(predictor):
+    """``TreeEnsembleSpec`` of a bound method of a fitted scikit-learn tree model, ``None`` for anything else (the engine
+    then reads a linear model).  A spec passes through.  Raises ``NotImplementedError`` / ``TypeError`` naming the reason
+    for tree models the route does not cover: categorical splits, custom boosting init estimators, multi-output
+    regressors, more than 8 outputs, trees inside a Pipeline or an ensemble, and unsupported methods."""
+    if isinstance(predictor, TreeEnsembleSpec):
+        return predictor
+    owner = getattr(predictor, "__self__", None)
+    method = getattr(predictor, "__name__", None)
+    if owner is None:
+        return None
+    names = _names(owner)
+    if names & _TREE_MODELS:
+        if not hasattr(owner, "n_features_in_"):
+            raise TypeError(f"{type(owner).__name__} is not fitted")
+        if names & _HGB:
+            return _hgb_spec(owner, method, names)
+        if names & _GB:
+            return _gb_spec(owner, method, names)
+        return _forest_spec(owner, method, names)
+    if names & _CONTAINERS and _contains_tree(owner):
+        raise NotImplementedError(f"{type(owner).__name__} holding a tree model: trees behind a Pipeline or inside an "
+                                  "ensemble are not supported; pass the tree model's own method")
+    return None

@@ -66,6 +66,16 @@ extern "C" {
                                  * CUDA-core kernel evaluating every member's head per element.  More than 128 groups, the
                                  * tensor-core kernel and per-instance plans of 65..128 groups are DKS_ERR_UNSUPPORTED
                                  * (DESIGN.md §5.0.10) */
+#define DKS_ACT_TREES 6         /* tree ensemble: set by dks_set_tree_model only (dks_set_model refuses it) */
+
+/* head of a tree ensemble on its raw scores r = base + sum_t leaf_t(x) (dks_set_tree_model) */
+#define DKS_TREE_HEAD_IDENTITY 0 /* outputs r (R outputs): forests' mean class fractions or values, decision_function, predict */
+#define DKS_TREE_HEAD_SIGMOID 1  /* R = 1, outputs [1 - expit(r), expit(r)]: binary gradient boosting predict_proba */
+#define DKS_TREE_HEAD_SOFTMAX 2  /* R = K >= 2 raw scores, outputs softmax(r): multi-class gradient boosting */
+#define DKS_TREE_HEAD_EXP 3      /* R = 1, output exp(r): histogram gradient boosting with a log-link loss; link identity only */
+/* split comparison: x goes left when x <= threshold */
+#define DKS_TREE_CMP_F32 0       /* (double)(float)x <= threshold: scikit-learn's sklearn.tree casts X to float32 */
+#define DKS_TREE_CMP_F64 1       /* x <= threshold in float64: the histogram gradient boosting estimators */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -111,6 +121,21 @@ int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int 
  * R = K R_m. */
 int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* W_host, const double* b_host,
                     const double* pi_host, int scalar_out);
+/* tree ensemble (DKS_ACT_TREES) in place of dks_set_model: n_trees trees whose nodes are concatenated into n_nodes entries.
+ * Per node: feature (the split column, -1 at a leaf), threshold, left / right (global indices of the children, each larger
+ * than the node's own; ignored at a leaf), missing_left (1: NaN goes left); value [n_nodes][R] row-major, read at leaves: the
+ * leaf's contribution to the R raw scores (the learning rate or 1 / n_trees folded in).  roots [n_trees]; base [R].
+ * r = base + sum over trees of the value of the leaf x reaches; outputs = head(r) per DKS_TREE_HEAD_*, compared per
+ * DKS_TREE_CMP_*.  R <= 8 and at most 8 outputs.  Malformed arrays (a child not after its parent, a feature out of range, a
+ * NaN threshold, a non-finite leaf value) are DKS_ERR_UNSUPPORTED.
+ * Every instance runs the tree kernels (DKS_GENERAL_TREES, DESIGN.md §5.0.11), up to 64 groups: shared plans (full and partial
+ * varying sets), per-instance device plans and caller-supplied plans, kernel 'auto' or 'simt' (tcgen05 / shared are
+ * DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route.  Float64 throughout; a link(ey) or link(f(x)) that
+ * is not finite (the logit of a probability of exactly 0 or 1) is DKS_ERR_NUMERIC, nothing non-finite is written into phi.
+ * A forest whose per-instance buffers do not fit shared memory is DKS_ERR_UNSUPPORTED. */
+int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const double* threshold, const int32_t* left,
+                       const int32_t* right, const uint8_t* missing_left, const double* value, int R, int n_trees,
+                       const int32_t* roots, const double* base, int head, int cmp, int scalar_out);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
  * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
  * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
@@ -312,6 +337,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_GENERAL_SIMT 2       /* explain_simt_kernel */
 #define DKS_GENERAL_FLAGGED 3    /* not computed: instances left for it are reported as DKS_ERR_UNSUPPORTED */
 #define DKS_GENERAL_SIMT_WIDE 4  /* explain_wide_instance_kernel: per-instance plans of 65..128 groups (two-word rows) */
+#define DKS_GENERAL_TREES 5      /* explain_tree_kernel: every instance of a tree ensemble (dks_set_tree_model) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
