@@ -405,14 +405,18 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                 }
             }
 
+            // the row's domain in the link table (a padding row has none and needs none: its y is 0).  With the background
+            // size compiled in it stays in registers for the whole segment; the run-time-N instantiations reload it every
+            // pass (an L1 hit), because holding it through their exact loop spills at 20 warps
+            LinkTabRow trow_seg;
+            trow_seg.x_lo = 0.0; trow_seg.off = 0; trow_seg.nint = 0;
+            if (NCT != 0 && p.ltab != nullptr && row_ok) trow_seg = p.ltab_rows[s];
+
             for (int it = 0; it < my_n; it += NI) {
                 double a[NI], v[NI], y[NI];
                 bool in_tab = true;
-                // the row's domain in the link table (a padding row has none and needs none: its y is 0), reloaded per
-                // pass (an L1 hit) so that it holds no registers through the exact loop
-                LinkTabRow trow;
-                trow.x_lo = 0.0; trow.off = 0; trow.nint = 0;
-                if (p.ltab != nullptr && row_ok) trow = p.ltab_rows[s];
+                LinkTabRow trow = trow_seg;
+                if (NCT == 0 && p.ltab != nullptr && row_ok) trow = p.ltab_rows[s];
 #pragma unroll
                 for (int u = 0; u < NI; ++u) {
                     a[u] = ((nx[u][0] + nx[u][1]) + (nx[u][2] + nx[u][3])) + es;
