@@ -145,7 +145,12 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
         for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
         if (M == 1) {
-            if (tid < C && !fx_bad) p.phi[(size_t)tid * slab + (size_t)i * G + (__ffsll((long long)vm) - 1)] = p.dlink[(size_t)i * C + tid];
+            // the one varying group takes link(f(x)) - link(fnull); two outputs: class 0 is the negation of class 1, as below
+            if (tid < C && !fx_bad) {
+                const double v = p.dlink[(size_t)i * C + (C == 2 ? 1 : tid)];
+                p.phi[(size_t)tid * slab + (size_t)i * G + (__ffsll((long long)vm) - 1)] =
+                    (C == 2 && tid == 0) ? ((v == 0.0) ? 0.0 : -v) : v;
+            }
             continue;
         }
         const int S = dks_effective_S(M, p.S_req);
