@@ -30,6 +30,7 @@ ACT_OVR = 3
 ACT_EXP = 4
 ACT_MIX = 5
 ACT_TREES = 6
+ACT_KMACH = 7
 LINK_IDENTITY = 0
 LINK_LOGIT = 1
 KERNEL_AUTO = 0
@@ -52,6 +53,8 @@ SIGNATURES = {
     "dks_set_mixture": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "dks_set_tree_model": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                                                                 C.c_int, C.c_int, C.c_int]),
+    "dks_set_kernel_machine": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 4 +
+                               [C.c_int, C.c_double, C.c_double, C.c_int] + [C.c_void_p] * 3 + [C.c_int]),
     "dks_set_column_maps": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "dks_set_link": (C.c_int, [C.c_void_p, C.c_int]),
     "dks_fit": (C.c_int, [C.c_void_p]),

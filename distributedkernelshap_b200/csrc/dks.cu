@@ -17,6 +17,7 @@
 #include "dks_sampler.cuh"
 #include "dks_instance_wide.cuh"
 #include "dks_trees.cuh"
+#include "dks_kmach.cuh"
 
 namespace {
 
@@ -187,8 +188,13 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         h.trees = true; h.l1_binary = ctx->C == 2;
         h.expo = ctx->tree.head == DKS_TREE_HEAD_EXP;
         break;
+    case DKS_ACT_KMACH:
+        // no shared-plan route: every instance runs the kernel-machine kernels; the calibrated head solves class 1 (class 0
+        // its negation)
+        h.kmach = true; h.l1_binary = ctx->km.head == DKS_KM_HEAD_CALIBRATED;
+        break;
     }
-    if (h.shared != HEAD_SHARED_BINARY && !h.trees) h.shared_max_G = 128;
+    if (h.shared != HEAD_SHARED_BINARY && !h.trees && !h.kmach) h.shared_max_G = 128;
     if (!h.mixture()) h.xt_scale = h.scale;
     h.l1_nout = h.l1_binary ? 1 : ctx->C;
     return h;
@@ -216,17 +222,23 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     // shared-plan route covers)
     double* xt = (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-    if (h.trees) {
-        // tree ensembles: prep_kernel decides the varying groups (its scores are those of a zero linear model, one identity
-        // output, and unused); the tree kernel then writes f(x) and link(f(x)) - link(fnull) of every output
+    if (h.trees || h.kmach) {
+        // tree ensembles and kernel machines: prep_kernel decides the varying groups (its scores are those of a zero linear
+        // model, one identity output, and unused); the model's predict kernel then writes f(x) and link(f(x)) - link(fnull)
+        // of every output
         kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
             X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
             ctx->d_linkfnull, n, ctx->N, ctx->D, G, 1, 1, DKS_ACT_IDENTITY, 1.0, ctx->link, ipb, ctx->d_XW,
             ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
             nullptr, 1.0, nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
-        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->tree, ctx->C, ctx->link,
-                                                                               ctx->d_linkfnull, nullptr, ctx->d_dlink,
-                                                                               ctx->d_status);
+        if (h.kmach)
+            dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->km, ctx->C, ctx->link,
+                                                                                 ctx->d_linkfnull, nullptr, ctx->d_dlink,
+                                                                                 ctx->d_status);
+        else
+            dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->tree, ctx->C,
+                                                                                   ctx->link, ctx->d_linkfnull, nullptr,
+                                                                                   ctx->d_dlink, ctx->d_status);
         ctx->launches += 1;
     } else {
         kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
@@ -532,11 +544,139 @@ int fit_trees(dks_ctx* ctx) {
     return DKS_OK;
 }
 
+// kernel machines: every instance on explain_kmach_kernel (up to 64 groups, CUDA-core only), the instances whose M selects
+// through the general list's l1 route -- the kernel's moments, then l1_lars_kernel -- whatever their M, G included
+int choose_route_kmach(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
+    const int G = ctx->G, kernel = ctx->kernel_choice;
+    if (kernel != DKS_KERNEL_AUTO && kernel != DKS_KERNEL_SIMT)
+        return fail(DKS_ERR_UNSUPPORTED, "kernel machines run on the kernel-machine kernel only (kernel 'auto' or 'simt')");
+    if (G > 64)
+        return fail(DKS_ERR_UNSUPPORTED, "kernel machines: %d groups; the kernel-machine kernel covers at most 64", G);
+    rt->draw = ctx->plan_mode == 1 && ext_z == nullptr;
+    if (rt->draw) TRY(sampler_config(ctx, false, &rt->sc));
+    const bool per_inst = ext_z != nullptr || rt->draw;
+    rt->S_cap = std::max(ext_z ? ext_stride : rt->draw ? rt->sc.stride : ctx->max_plan_S, 2);
+    rt->smem = dks::kmach::smem_bytes(rt->S_cap, ctx->C, ctx->km.R, G, ctx->km.head == DKS_KM_HEAD_CALIBRATED);
+    if ((long long)rt->smem > (long long)ctx->max_smem_optin)
+        return fail(DKS_ERR_UNSUPPORTED, "kernel-machine kernel needs %zu B of shared memory (> %d): nsamples, outputs or "
+                    "groups too many", rt->smem, ctx->max_smem_optin);
+    if (ctx->l1_mode != 0) {
+        if (per_inst) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
+        for (int M = 2; M <= G; ++M) {
+            if (!((ctx->l1_sel[0] >> (M - 1)) & 1ull)) continue;
+            if (ctx->h_l1[M].gram_raw == nullptr || ctx->h_l1[M].S != dks_effective_S(M, ctx->nsamples_req) ||
+                ctx->h_plans[M].z == nullptr || ctx->h_plans[M].S != ctx->h_l1[M].S)
+                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared plan of M=%d and its l1 tables "
+                            "(dks_set_l1_tables)", M);
+            rt->l1_Mmax = M;
+        }
+        if (rt->l1_Mmax > 0 && !lars_fits(ctx, rt->l1_Mmax))
+            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory",
+                        rt->l1_Mmax, rt->l1_Mmax);
+        rt->l1_smem = rt->smem;
+    }
+    rt->general = DKS_GENERAL_KMACH;
+    return DKS_OK;
+}
+
+// the kernel-machine kernel over p.list (L1: its moments)
+int launch_kmach_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
+    const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
+    auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{}, ctx->km,
+                                                   ctx->cur_X, ctx->d_bg, ctx->D, ctx->d_goff, ctx->d_gcols);
+    ctx->launches += 1;
+    return DKS_OK;
+}
+
+void free_kmach(dks_ctx* ctx) {
+    KmDev& k = ctx->km;
+    for (const void* q : {(const void*)k.sv, (const void*)k.dual, (const void*)k.colw, (const void*)k.colo, (const void*)k.Tbg})
+        if (q) cudaFree((void*)q);
+    k.sv = nullptr; k.dual = nullptr; k.colw = nullptr; k.colo = nullptr; k.Tbg = nullptr;
+}
+
+// dks_fit of a kernel machine: the arrays, T[j][v] of every background row and support vector, the column statistics stage 1
+// decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the kernel-machine kernels
+int fit_kmach(dks_ctx* ctx) {
+    const int N = ctx->N, D = ctx->D, G = ctx->G, C = ctx->C;
+    const cudaStream_t st = ctx->stream;
+    KmDev& k = ctx->km;
+    TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
+    TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
+    TRY(dev_alloc(&ctx->d_W, (size_t)D));
+    TRY(dev_alloc(&ctx->d_b, (size_t)1));
+    TRY(dev_alloc(&ctx->d_goff, (size_t)G + 1));
+    TRY(dev_alloc(&ctx->d_gcols, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colmin, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colmax, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colnan, (size_t)D));
+    TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
+    TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
+    {
+        int* hdr = const_cast<int*>(ctx->cm.hdr);
+        double* keys = const_cast<double*>(ctx->cm.keys);
+        double* vals = const_cast<double*>(ctx->cm.vals);
+        dev_free(&hdr); dev_free(&keys); dev_free(&vals);
+        ctx->cm = ColumnMapsDev{};
+    }
+    free_kmach(ctx);
+    TRY(upload_tree_array(&k.sv, ctx->h_ksv.data(), ctx->h_ksv.size(), st));
+    TRY(upload_tree_array(&k.dual, ctx->h_kdual.data(), ctx->h_kdual.size(), st));
+    TRY(upload_tree_array(&k.colw, ctx->h_kcolw.data(), ctx->h_kcolw.size(), st));
+    TRY(upload_tree_array(&k.colo, ctx->h_kcolo.data(), ctx->h_kcolo.size(), st));
+    double* Tbg = nullptr;
+    TRY(dev_alloc(&Tbg, (size_t)N * k.n_sv));
+    k.Tbg = Tbg;
+    double* pred = nullptr;
+    TRY(dev_alloc(&pred, (size_t)N * C));
+    CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_W, ctx->h_W.data(), sizeof(double) * D, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_b, ctx->h_b.data(), sizeof(double), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
+    dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
+    dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(ctx->d_bg, N, D, k, Tbg);
+    dks::kmach::km_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(ctx->d_bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
+                                                                ctx->d_status);
+    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
+    ctx->launches += 4;
+    CUDA_TRY(cudaGetLastError());
+    ctx->h_fnull.resize(C);
+    ctx->h_linkfnull.resize(C);
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    cudaFree(pred);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
+        return fail(DKS_ERR_DOMAIN, "background row %d holds NaN: kernel machines refuse it, as scikit-learn does",
+                    ctx->h_status[1]);
+    for (int c = 0; c < C; ++c)
+        if (!std::isfinite(ctx->h_linkfnull[c]))
+            return fail(DKS_ERR_NUMERIC, "kernel machine: link(fnull) of output %d is not finite (fnull = %g): the background's "
+                        "mean prediction is 0 or 1 under the logit link, or overflows", c, ctx->h_fnull[c]);
+    ctx->cap_n = 0;
+    ctx->prepared = false;
+    for (const auto& allocs : ctx->plan_allocs)
+        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
+    ctx->fitted = true;
+    ctx->epoch++;
+    return DKS_OK;
+}
+
 int choose_route(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
     const HeadDesc& h = ctx->head;
     if (h.trees) {
         *rt = Route{};
         return choose_route_trees(ctx, ext_z, ext_stride, rt);
+    }
+    if (h.kmach) {
+        *rt = Route{};
+        return choose_route_kmach(ctx, ext_z, ext_stride, rt);
     }
     const int G = ctx->G, N = ctx->N, kernel = ctx->kernel_choice;
     const bool auto_or_shared = kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED;
@@ -968,6 +1108,10 @@ int launch_general_l1(dks_ctx* ctx, const Route& rt, ExplainParams* p, double* p
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
         TRY(launch_tree_kernel(ctx, true, ps, rt.l1_smem, gstream));
         ctx->launches += 1;
+    } else if (ctx->head.kmach) {
+        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
+        TRY(launch_kmach_kernel(ctx, true, ps, rt.l1_smem, gstream));
+        ctx->launches += 1;
     } else {
         const bool mixh = ctx->head.mixture();
         auto l1kern = ctx->head.expo ? dks::explain_simt_kernel<true, true> : dks::explain_simt_kernel<true>;
@@ -1019,6 +1163,9 @@ int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t 
         break;
     case DKS_GENERAL_TREES:
         TRY(launch_tree_kernel(ctx, false, p, rt.smem, gstream));
+        break;
+    case DKS_GENERAL_KMACH:
+        TRY(launch_kmach_kernel(ctx, false, p, rt.smem, gstream));
         break;
     default: {
         const bool mixh = ctx->head.mixture();
@@ -1110,6 +1257,9 @@ int check_status(dks_ctx* ctx) {
     if (ctx->h_status[0] == 0) return DKS_OK;
     if (ctx->h_status[0] == DKS_ERR_PLAN_MISSING)
         return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", ctx->h_status[1]);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.kmach)
+        return fail(DKS_ERR_DOMAIN, "instance %d holds NaN: kernel machines refuse it, as scikit-learn does",
+                    ctx->h_status[1]);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN)
         return fail(DKS_ERR_DOMAIN, "instance %d holds a raw value its column map refuses (NaN, or a category unseen at "
                     "fit time, where the pipeline raises)", ctx->h_status[1]);
@@ -1301,6 +1451,7 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b); dev_free(&ctx->d_mix);
     dev_free(&ctx->d_mixBW); dev_free(&ctx->d_mixsc); dev_free(&ctx->d_mixscr);
     free_tree(ctx);
+    free_kmach(ctx);
     if (ctx->cm.hdr) { cudaFree((void*)ctx->cm.hdr); cudaFree((void*)ctx->cm.keys); cudaFree((void*)ctx->cm.vals); }
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
@@ -1496,6 +1647,83 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
     return DKS_OK;
 }
 
+int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const double* sv, const double* dual, int R,
+                           const double* intercept, const double* colw, const double* colo, const double* gamma, int kernel,
+                           double degree, double coef0, int head, const double* cal_a, const double* cal_b,
+                           const double* pi, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_kernel_machine: call dks_set_background first (D unknown)");
+    REQUIRE(sv_off && sv && dual && intercept && colw && colo && gamma,
+            "dks_set_kernel_machine: need the support vectors, dual coefficients, intercepts, column weights and gamma");
+    const int D = ctx->D;
+    auto finite = [](const double* a, size_t n) {
+        for (size_t e = 0; e < n; ++e) if (!std::isfinite(a[e])) return false;
+        return true;
+    };
+    if (K < 1 || K > DKS_KM_MAX_K)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: K=%d members; 1..%d supported", K, DKS_KM_MAX_K);
+    if (R < 1 || R > DKS_KM_MAX_R)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: R=%d outputs; 1..%d supported", R, DKS_KM_MAX_R);
+    if (kernel < DKS_KM_KERNEL_RBF || kernel > DKS_KM_KERNEL_SIGMOID)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: unknown kernel %d", kernel);
+    if (!std::isfinite(coef0) || !std::isfinite(degree) ||
+        (kernel == DKS_KM_KERNEL_POLY && (degree < 0 || degree != std::floor(degree))))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: degree %g / coef0 %g (degree: an integer >= 0)", degree, coef0);
+    int C;
+    if (head == DKS_KM_HEAD_IDENTITY) {
+        if (K != 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the identity head takes one member (K=%d)", K);
+        C = R;
+    } else if (head == DKS_KM_HEAD_CALIBRATED) {
+        if (R != 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the calibrated head needs R == 1 (got %d)", R);
+        if (!cal_a || !cal_b || !pi || !finite(cal_a, K) || !finite(cal_b, K))
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the calibrated head needs finite a, b and pi");
+        C = 2;
+    } else {
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: unknown head %d", head);
+    }
+    if (sv_off[0] != 0) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: sv_off[0] must be 0");
+    for (int m = 0; m < K; ++m)
+        if (sv_off[m + 1] < sv_off[m])
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: sv_off must not decrease (member %d)", m);
+    const int n_sv = sv_off[K];
+    if (n_sv < 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: no support vectors");
+    if (!finite(sv, (size_t)n_sv * D) || !finite(dual, (size_t)n_sv * R) || !finite(intercept, (size_t)K * R) ||
+        !finite(colw, (size_t)K * D) || !finite(colo, (size_t)K * D) || !finite(gamma, K))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the arrays must be finite");
+    for (size_t e = 0; e < (size_t)K * D; ++e)
+        if (!(colw[e] > 0)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: column weights must be positive");
+    double pisum = 0;
+    for (int m = 0; m < K; ++m) {
+        if (!(gamma[m] >= 0)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: gamma must be >= 0");
+        if (head == DKS_KM_HEAD_CALIBRATED) {
+            if (!(pi[m] > 0) || !std::isfinite(pi[m]))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: pi must be positive and finite");
+            pisum += pi[m];
+        }
+    }
+    KmDev& k = ctx->km;
+    for (int m = 0; m <= K; ++m) k.sv_off[m] = sv_off[m];
+    for (int m = 0; m < K; ++m) {
+        k.gamma[m] = gamma[m];
+        for (int q = 0; q < R; ++q) k.icpt[m * R + q] = intercept[m * R + q];
+        k.cal_a[m] = head == DKS_KM_HEAD_CALIBRATED ? cal_a[m] : 0.0;
+        k.cal_b[m] = head == DKS_KM_HEAD_CALIBRATED ? cal_b[m] : 0.0;
+        k.pi[m] = head == DKS_KM_HEAD_CALIBRATED ? pi[m] / pisum : 1.0;
+    }
+    k.degree = degree; k.coef0 = coef0; k.K = K; k.R = R; k.n_sv = n_sv; k.kernel = kernel; k.head = head;
+    ctx->h_ksv.assign(sv, sv + (size_t)n_sv * D);
+    ctx->h_kdual.assign(dual, dual + (size_t)n_sv * R);
+    ctx->h_kcolw.assign(colw, colw + (size_t)K * D);
+    ctx->h_kcolo.assign(colo, colo + (size_t)K * D);
+    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
+    ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_KMACH; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
+    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+    ctx->h_W.assign((size_t)D, 0.0);
+    ctx->h_b.assign(1, 0.0);
+    ctx->fitted = false;
+    return DKS_OK;
+}
+
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
                         const double* vals_host, int n_vals) {
     BIND(ctx);
@@ -1506,6 +1734,9 @@ int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, con
     }
     REQUIRE(ctx->R > 0, "dks_set_column_maps: call dks_set_model first");
     if (ctx->act == DKS_ACT_TREES) return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for tree ensembles");
+    if (ctx->act == DKS_ACT_KMACH)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for kernel machines (their scalers fold into the support "
+                    "vectors and column weights)");
     if (D != ctx->D || R != ctx->R)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: maps of %d columns x %d score rows, model has %d x %d", D, R,
                     ctx->D, ctx->R);
@@ -1571,6 +1802,7 @@ int dks_fit(dks_ctx* ctx) {
         }
     }
     if (h.trees) return fit_trees(ctx);
+    if (h.kmach) return fit_kmach(ctx);
     TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
     TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
     TRY(dev_alloc(&ctx->d_W, (size_t)R * D));
@@ -1693,6 +1925,9 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     if (ctx->head.trees)
         dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->tree, ctx->C, ctx->link,
                                                                                nullptr, dO, nullptr, nullptr);
+    else if (ctx->head.kmach)
+        dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->km, ctx->C, ctx->link,
+                                                                             nullptr, dO, nullptr, ctx->d_status);
     else
         (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
             dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status, ctx->d_mix);
@@ -1702,6 +1937,8 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     cudaFree(dX); cudaFree(dO);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.kmach)
+        return fail(DKS_ERR_DOMAIN, "row %d holds NaN: kernel machines refuse it, as scikit-learn does", ctx->h_status[1]);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN)
         return fail(DKS_ERR_DOMAIN, "row %d holds a raw value its column map refuses (NaN, or a category unseen at fit time, "
                     "where the pipeline raises)", ctx->h_status[1]);

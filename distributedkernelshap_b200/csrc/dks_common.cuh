@@ -160,6 +160,21 @@ struct TreeDev {
     int nodes, T, R, head, cmp;
 };
 
+// kernel machines (dks_set_kernel_machine, DESIGN.md §5.0.12): K members, member k owning support vectors sv_off[k] ..
+// sv_off[k + 1]; f_k = sum_v dual[v] phi(t) + icpt, t = sum_c h(x_c, sv_c) per DKS_KM_KERNEL_*, then the head
+// DKS_KM_HEAD_*.  Intercepts icpt[k R + q] (K R <= DKS_KM_MAX_K: one member of R <= 8 outputs, or K members of one).
+struct KmDev {
+    const double* sv;            // [n_sv][D] support vectors in raw feature space
+    const double* dual;          // [n_sv][R]
+    const double* colw;          // [K][D] column weights (the member's scalers folded in)
+    const double* colo;          // [K][D] column origins (dot-product kernels)
+    const double* Tbg;           // [N][n_sv] fit: t of background row j and support vector v
+    int sv_off[DKS_KM_MAX_K + 1];
+    double gamma[DKS_KM_MAX_K], icpt[DKS_KM_MAX_K], cal_a[DKS_KM_MAX_K], cal_b[DKS_KM_MAX_K], pi[DKS_KM_MAX_K];
+    double degree, coef0;
+    int K, R, n_sv, kernel, head;
+};
+
 // exp head, CUDA-core kernels (DESIGN.md §5.0.8): a coalition row is summed in fp32 when the largest weighted background
 // exponent t'_j = log2 e d(s, j) + log2 w_j lies in [EXP_T_LO, EXP_T_HI]; other rows are evaluated in float64
 #define DKS_EXP_T_LO -60.f
@@ -188,6 +203,7 @@ struct HeadDesc {
     bool wide_pi = false;       // per-instance plans of 65..128 groups
     bool tc = false;            // tensor-core kernel
     bool trees = false;         // tree ensemble: the tree kernels only (dks_trees.cuh)
+    bool kmach = false;         // kernel machine: the kernel-machine kernels only (dks_kmach.cuh)
     bool mixture() const { return shared == HEAD_SHARED_MIX_BINARY || shared == HEAD_SHARED_MIX_CLASS; }
 };
 
@@ -238,6 +254,9 @@ struct dks_ctx {
     std::vector<unsigned char> h_tmiss;
     TreeDev tree = {};
     size_t cap_txinfo = 0;
+    // kernel machine (act == DKS_ACT_KMACH): host copies of the arrays, and their device copies built by dks_fit
+    std::vector<double> h_ksv, h_kdual, h_kcolw, h_kcolo;
+    KmDev km = {};
     std::vector<double> h_bg, h_wbg, h_W, h_b;
     std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
     std::vector<double> h_cm_keys, h_cm_vals;

@@ -15,6 +15,7 @@ import numpy as np
 from . import _cabi
 from .data import DenseData, convert_to_data, convert_to_link
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
+from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, extract_kernel_machine_spec
 from .predictors import extract_linear_spec
 from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_tree_spec
 
@@ -155,7 +156,8 @@ class GpuKernelExplainer:
         self.link = convert_to_link(link)
         self.model_callable = model
         tree_spec = extract_tree_spec(model)
-        self.spec = tree_spec if tree_spec is not None else extract_linear_spec(model)
+        km_spec = extract_kernel_machine_spec(model) if tree_spec is None else None
+        self.spec = tree_spec if tree_spec is not None else km_spec if km_spec is not None else extract_linear_spec(model)
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
                                       "link log(ey / (1 - ey)) is undefined wherever a predicted mean exceeds 1")
@@ -189,8 +191,18 @@ class GpuKernelExplainer:
         if tree_spec is not None and self.data.groups_size > TREE_MAX_GROUPS:
             raise NotImplementedError(f"{self.data.groups_size} groups: tree ensembles are explained up to "
                                       f"{TREE_MAX_GROUPS} groups")
-        W = None if tree_spec is not None else self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
-        if tree_spec is not None:
+        if km_spec is not None and self.data.groups_size > KMACH_MAX_GROUPS:
+            raise NotImplementedError(f"{self.data.groups_size} groups: kernel machines are explained up to "
+                                      f"{KMACH_MAX_GROUPS} groups")
+        W = None if tree_spec is not None or km_spec is not None else \
+            self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
+        if km_spec is not None:
+            k = km_spec
+            _cabi.check(self.lib.dks_set_kernel_machine(
+                self._ctx, k.K, _cabi.ptr(k.sv_off), _cabi.ptr(k.sv), _cabi.ptr(k.dual), k.R, _cabi.ptr(k.intercept),
+                _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree, k.coef0, k.head_code,
+                _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
+        elif tree_spec is not None:
             t = tree_spec
             _cabi.check(self.lib.dks_set_tree_model(
                 self._ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
@@ -640,7 +652,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp", "mixture"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach"),
     }
 
     def last_path(self):
@@ -650,8 +662,9 @@ class GpuKernelExplainer:
         coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
-        are reported as unsupported, not computed, 'simt_wide': per-instance plans of 65..128 groups, or 'trees': the tree
-        kernel, which takes every instance of a tree ensemble), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
+        are reported as unsupported, not computed, 'simt_wide': per-instance plans of 65..128 groups, 'trees': the tree
+        kernel, which takes every instance of a tree ensemble, or 'kmach': the kernel-machine kernel, which takes every
+        instance of a kernel machine), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
         the weighted one), ``fused_table`` (1: the fused kernel read y from the plan's link table, passes outside its

@@ -76,6 +76,20 @@ extern "C" {
 /* split comparison: x goes left when x <= threshold */
 #define DKS_TREE_CMP_F32 0       /* (double)(float)x <= threshold: scikit-learn's sklearn.tree casts X to float32 */
 #define DKS_TREE_CMP_F64 1       /* x <= threshold in float64: the histogram gradient boosting estimators */
+#define DKS_ACT_KMACH 7         /* kernel machine: set by dks_set_kernel_machine only (dks_set_model refuses it) */
+
+/* kernel of a kernel machine (dks_set_kernel_machine): K(x, v) = phi(t), t = sum_c h(x_c, v_c) with the member's column
+ * weight w_c and origin o_c (its scalers folded in) */
+#define DKS_KM_KERNEL_RBF 0       /* h = w_c (x_c - v_c)^2,         phi = exp(-gamma t) */
+#define DKS_KM_KERNEL_LAPLACIAN 1 /* h = w_c |x_c - v_c|,           phi = exp(-gamma t) */
+#define DKS_KM_KERNEL_POLY 2      /* h = w_c (x_c - o_c)(v_c - o_c), phi = (gamma t + coef0)^degree, integer degree >= 0 */
+#define DKS_KM_KERNEL_SIGMOID 3   /* h = w_c (x_c - o_c)(v_c - o_c), phi = tanh(gamma t + coef0) */
+/* head of a kernel machine on the member scores f_k = sum_v dual[v] K(x, v) + intercept_k */
+#define DKS_KM_HEAD_IDENTITY 0    /* one member, R outputs f (SVC / NuSVC decision_function, SVR, NuSVR, KernelRidge) */
+#define DKS_KM_HEAD_CALIBRATED 1  /* R = 1, outputs [1 - p1, p1], p1 = sum_k pi_k expit(-(a_k f_k + b_k)): sigmoid
+                                   * CalibratedClassifierCV over a binary SVC / NuSVC */
+#define DKS_KM_MAX_R 8            /* outputs of the identity head */
+#define DKS_KM_MAX_K 16           /* members of the calibrated head */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -136,6 +150,23 @@ int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* 
 int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const double* threshold, const int32_t* left,
                        const int32_t* right, const uint8_t* missing_left, const double* value, int R, int n_trees,
                        const int32_t* roots, const double* base, int head, int cmp, int scalar_out);
+/* kernel machine (DKS_ACT_KMACH) in place of dks_set_model: K members, member k owning support vectors sv_off[k] ..
+ * sv_off[k + 1] (sv_off [K + 1], non-decreasing from 0, n_sv = sv_off[K] >= 1).  sv [n_sv][D] row-major in raw feature space,
+ * dual [n_sv][R], intercept [K][R]; per member colw [K][D] (> 0 at every column), colo [K][D] and gamma [K] (>= 0);
+ * kernel DKS_KM_KERNEL_*, degree (POLY: an integer >= 0) and coef0 shared by the members.  Member score
+ * f_k = sum_v dual[v] phi(sum_c h(x_c, sv[v][c])) + intercept_k; outputs per DKS_KM_HEAD_*: IDENTITY needs K = 1 and gives
+ * R <= 8 outputs; CALIBRATED needs R = 1 and reads cal_a, cal_b and pi [K] (pi > 0, normalised to sum 1), K <= 16.
+ * Non-finite values, bad offsets and unknown kernel or head codes are DKS_ERR_UNSUPPORTED.
+ * Every instance runs the kernel-machine kernel (DKS_GENERAL_KMACH, DESIGN.md §5.0.12), up to 64 groups: shared plans (full
+ * and partial varying sets), per-instance device plans and caller-supplied plans, kernel 'auto' or 'simt' (tcgen05 / shared
+ * are DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route.  Float64 throughout.  NaN in a background
+ * row (dks_fit) or an instance (dks_predict_host, the explain calls) is DKS_ERR_DOMAIN with the row; a link(ey) or
+ * link(f(x)) that is not finite is DKS_ERR_NUMERIC and nothing non-finite is written into phi.  Shapes whose per-instance
+ * buffers do not fit shared memory are DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused. */
+int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const double* sv, const double* dual, int R,
+                           const double* intercept, const double* colw, const double* colo, const double* gamma, int kernel,
+                           double degree, double coef0, int head, const double* cal_a, const double* cal_b,
+                           const double* pi, int scalar_out);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
  * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
  * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
@@ -338,6 +369,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_GENERAL_FLAGGED 3    /* not computed: instances left for it are reported as DKS_ERR_UNSUPPORTED */
 #define DKS_GENERAL_SIMT_WIDE 4  /* explain_wide_instance_kernel: per-instance plans of 65..128 groups (two-word rows) */
 #define DKS_GENERAL_TREES 5      /* explain_tree_kernel: every instance of a tree ensemble (dks_set_tree_model) */
+#define DKS_GENERAL_KMACH 6      /* explain_kmach_kernel: every instance of a kernel machine (dks_set_kernel_machine) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
