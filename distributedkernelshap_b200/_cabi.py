@@ -56,6 +56,9 @@ SIGNATURES = {
     "dks_set_kernel_machine": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 4 +
                                [C.c_int, C.c_double, C.c_double, C.c_int] + [C.c_void_p] * 3 + [C.c_int]),
     "dks_set_column_maps": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
+    "dks_set_column_encoding": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                          C.c_int]),
+    "dks_encode_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "dks_set_link": (C.c_int, [C.c_void_p, C.c_int]),
     "dks_fit": (C.c_int, [C.c_void_p]),
     "dks_num_outputs": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
@@ -130,7 +133,8 @@ def load(build_if_needed=True):
 
 
 class DksDomainError(DksError, ValueError):
-    """A raw value a column map refuses (``DKS_ERR_DOMAIN``): where scikit-learn's pipeline raises ``ValueError``."""
+    """A raw value a column map or column encoding refuses (``DKS_ERR_DOMAIN``): where scikit-learn's pipeline raises
+    ``ValueError``."""
 
 
 def check(rc):

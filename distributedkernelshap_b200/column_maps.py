@@ -27,7 +27,11 @@ Packed form (what ``dks_set_column_maps`` reads), ``R`` score rows, ``D`` raw co
 The tables are built by calling the fitted transformers themselves (on their own categories, bin representatives, one
 unseen value and NaN), so ``drop``, infrequent categories and unknown handling come from scikit-learn.  Scalers and
 imputers are folded analytically.  Anything that mixes columns or is not piecewise affine per column raises
-``TypeError`` naming the step."""
+``TypeError`` naming the step.
+
+The same walk also builds, per encoded column, an exact program of the steps' own arithmetic (``_Prog``): a tree model
+compares encoded values exactly, which folded maps cannot reproduce.  ``compile_encoding`` packs those programs
+(``ColumnEncoding``, what ``dks_set_column_encoding`` reads; DESIGN.md §5.0.13)."""
 import warnings
 
 import numpy as np
@@ -37,6 +41,9 @@ NAN_ERROR = 2
 UNKNOWN_ERROR = 4
 
 ERR = None          # a value for which the pipeline raises
+
+# ops of a column encoding (ColumnEncoding, dks_set_column_encoding): DKS_ENC_OP_* in include/dks.h
+OP_SUB, OP_DIV, OP_MUL, OP_ADD, OP_CLIP, OP_NANFILL, OP_ISNAN, OP_PIECES, OP_TABLE = range(9)
 
 
 class ColumnMaps:
@@ -101,10 +108,11 @@ class ColumnMaps:
 class _Affine:
     """Piecewise affine in the raw value; ``nan``: the value a raw NaN gives (float, NaN, or ERR)."""
 
-    def __init__(self, src, t, a, c, nan):
+    def __init__(self, src, t, a, c, nan, prog=None):
         self.src, self.t = src, np.asarray(t, dtype=np.float64)
         self.a, self.c = np.asarray(a, dtype=np.float64), np.asarray(c, dtype=np.float64)
         self.nan = nan
+        self.prog = prog if prog is not None else _Prog(src)
 
     def is_raw(self):
         return len(self.a) == 1 and self.a[0] == 1.0 and self.c[0] == 0.0
@@ -115,27 +123,106 @@ class _Affine:
     def values(self):
         return list(self.c) + [self.nan]
 
-    def map_values(self, g):
-        """Piecewise constant feature through the scalar function ``g`` (ERR in, ERR out)."""
-        return _Affine(self.src, self.t, np.zeros_like(self.c), [_apply(g, v) for v in self.c], _apply(g, self.nan))
+    def map_values(self, g, prog):
+        """Piecewise constant feature through the scalar function ``g`` (ERR in, ERR out); ``prog`` its exact program."""
+        return _Affine(self.src, self.t, np.zeros_like(self.c), [_apply(g, v) for v in self.c], _apply(g, self.nan), prog)
 
 
 class _Table:
     """Categorical in the raw value: ``vals[k]`` at ``keys[k]``, else ``unknown``; a raw NaN gives ``nan``."""
 
-    def __init__(self, src, keys, vals, unknown, nan):
+    def __init__(self, src, keys, vals, unknown, nan, prog):
         self.src, self.keys, self.vals = src, np.asarray(keys, dtype=np.float64), list(vals)
         self.unknown, self.nan = unknown, nan
+        self.prog = prog
 
     def values(self):
         return self.vals + [self.unknown, self.nan]
 
-    def map_values(self, g):
-        return _Table(self.src, self.keys, [_apply(g, v) for v in self.vals], _apply(g, self.unknown), _apply(g, self.nan))
+    def map_values(self, g, prog):
+        return _Table(self.src, self.keys, [_apply(g, v) for v in self.vals], _apply(g, self.unknown), _apply(g, self.nan),
+                      prog)
 
 
 def _apply(g, v):
     return ERR if v is ERR else g(float(v))
+
+
+# ---- exact programs: what pipe[:-1].transform does to one encoded column, op by op (ColumnEncoding) ------------------
+def _scalar(op, v):
+    """One scalar op on a float64 value, with the arithmetic of the scikit-learn step it stands for."""
+    code, c0, c1 = op
+    v = np.float64(v)
+    if code == OP_SUB:
+        return float(v - c0)
+    if code == OP_DIV:
+        return float(v / np.float64(c0))
+    if code == OP_MUL:
+        return float(v * c0)
+    if code == OP_ADD:
+        return float(v + c0)
+    if code == OP_CLIP:
+        return float(np.clip(v, c0, c1))
+    if code == OP_NANFILL:
+        return float(c0) if np.isnan(v) else float(v)
+    if code == OP_ISNAN:
+        return 1.0 if np.isnan(v) else 0.0
+    raise AssertionError(code)
+
+
+class _Lookup:
+    """The piecewise-constant end of a program: ``OP_PIECES`` (sorted edges, one output per bin, bin = numpy
+    searchsorted(edges, v, side='right')) or ``OP_TABLE`` (sorted keys, one output per key, ``unknown`` on no exact
+    match).  A NaN gives ``nan``.  Outputs may be ERR (the pipeline raises)."""
+
+    def __init__(self, code, keys, outs, unknown, nan):
+        self.code, self.keys, self.outs = code, np.asarray(keys, dtype=np.float64), list(outs)
+        self.unknown, self.nan = unknown, nan
+
+    def map(self, g):
+        return _Lookup(self.code, self.keys, [_apply(g, v) for v in self.outs],
+                       _apply(g, self.unknown) if self.code == OP_TABLE else None, _apply(g, self.nan))
+
+
+class _Prog:
+    """Exact program of one encoded column: scalar ops on raw column ``src``, optionally ending in a ``_Lookup``.  An op
+    that follows the lookup is folded into its outputs, so a program is always ``ops`` then at most one lookup."""
+
+    def __init__(self, src, ops=(), look=None):
+        self.src, self.ops, self.look = src, tuple(ops), look
+
+    def then(self, *ops):
+        p = self
+        for op in ops:
+            p = _Prog(p.src, p.ops + (op,)) if p.look is None else _Prog(p.src, p.ops, p.look.map(lambda v: _scalar(op, v)))
+        return p
+
+    def lookup(self, look):
+        """``look`` applied to this program's value (the program must not end in a lookup yet)."""
+        assert self.look is None
+        return _Prog(self.src, self.ops, look)
+
+    def values(self):
+        """``(sorted distinct finite values, whether NaN is one)`` of a piecewise-constant program: its lookup's outputs,
+        or what the ops after its last ``OP_ISNAN`` make of 0 and 1."""
+        if self.look is not None:
+            vs = self.look.outs + [self.look.unknown if self.look.code == OP_TABLE else ERR, self.look.nan]
+        else:
+            last = max(k for k, op in enumerate(self.ops) if op[0] == OP_ISNAN)
+            vs = []
+            for v in (0.0, 1.0):
+                for op in self.ops[last + 1:]:
+                    v = _scalar(op, v)
+                vs.append(v)
+        vs = [v for v in vs if v is not ERR]
+        return sorted({float(v) for v in vs if not np.isnan(v)}), any(np.isnan(v) for v in vs)
+
+    def compose(self, g, keys, has_nan):
+        """This program through ``g`` (a scalar function defined on the program's finite values ``keys`` and, with
+        ``has_nan``, on NaN): the lookup's outputs mapped, or a table over ``keys`` appended."""
+        if self.look is not None:
+            return _Prog(self.src, self.ops, self.look.map(g))
+        return self.lookup(_Lookup(OP_TABLE, keys, [g(k) for k in keys], ERR, g(np.nan) if has_nan else ERR))
 
 
 def _name(step):
@@ -143,30 +230,32 @@ def _name(step):
 
 
 # ---- per-step compilers -------------------------------------------------------------------------------------------
-def _affine_step(feats, mul, add, name, clip=None):
+def _affine_step(feats, mul, add, name, exact, clip=None):
     """y = x * mul + add per feature (add applied after mul), then optionally clipped to ``clip`` -- the order of the
-    scalers' own arithmetic, so that tables come out bit-identical to ``transform``."""
+    scalers' own arithmetic, so that tables come out bit-identical to ``transform``.  ``exact[i]``: the ops the step
+    itself performs on feature i (its program's continuation)."""
     out = []
-    for f, s, o in zip(feats, mul, add):
+    for f, s, o, ops in zip(feats, mul, add, exact):
         def g(v, s=s, o=o):
             y = v * s + o
             return float(np.clip(y, clip[0], clip[1])) if clip is not None else y
+        prog = f.prog.then(*ops)
         if isinstance(f, _Table) or f.is_constant():
-            out.append(f.map_values(g))
+            out.append(f.map_values(g, prog))
             continue
         a, c = f.a * s, f.c * s + o
         nan = _apply(g, f.nan)
         if clip is None:
-            out.append(_Affine(f.src, f.t, a, c, nan))
+            out.append(_Affine(f.src, f.t, a, c, nan, prog))
             continue
         if len(a) != 1:
             raise TypeError(f"{name}(clip=True) after a piecewise transformer is not supported")
         lo, hi = float(clip[0]), float(clip[1])
         x_lo, x_hi = (lo - c[0]) / a[0], (hi - c[0]) / a[0]
         if a[0] > 0:
-            out.append(_Affine(f.src, [x_lo, x_hi], [0.0, a[0], 0.0], [lo, c[0], hi], nan))
+            out.append(_Affine(f.src, [x_lo, x_hi], [0.0, a[0], 0.0], [lo, c[0], hi], nan, prog))
         else:
-            out.append(_Affine(f.src, [x_hi, x_lo], [0.0, a[0], 0.0], [hi, c[0], lo], nan))
+            out.append(_Affine(f.src, [x_hi, x_lo], [0.0, a[0], 0.0], [hi, c[0], lo], nan, prog))
     return out
 
 
@@ -174,24 +263,36 @@ def _scaler(step, feats):
     from sklearn import preprocessing as pp
     k = len(feats)
     one, zero = np.ones(k), np.zeros(k)
+
+    def ops(code, vals, on=True):
+        return [[(code, float(v), 0.0)] if on else [] for v in np.broadcast_to(np.asarray(vals, dtype=np.float64), (k,))]
     if isinstance(step, pp.StandardScaler):
-        mean = step.mean_ if step.with_mean and step.mean_ is not None else zero
+        with_mean = step.with_mean and step.mean_ is not None
+        mean = step.mean_ if with_mean else zero
         scale = step.scale_ if step.with_std and step.scale_ is not None else one
         # (x - mean) / scale
-        feats = _affine_step(feats, one, -np.asarray(mean, dtype=np.float64), "StandardScaler")
-        return _affine_step(feats, 1.0 / np.asarray(scale, dtype=np.float64), zero, "StandardScaler") \
-            if step.with_std else feats
+        feats = _affine_step(feats, one, -np.asarray(mean, dtype=np.float64), "StandardScaler",
+                             ops(OP_SUB, mean, with_mean))
+        return _affine_step(feats, 1.0 / np.asarray(scale, dtype=np.float64), zero, "StandardScaler",
+                            ops(OP_DIV, scale)) if step.with_std else feats
     if isinstance(step, pp.RobustScaler):
         if step.with_centering:
-            feats = _affine_step(feats, one, -np.asarray(step.center_, dtype=np.float64), "RobustScaler")
+            feats = _affine_step(feats, one, -np.asarray(step.center_, dtype=np.float64), "RobustScaler",
+                                 ops(OP_SUB, step.center_))
         if step.with_scaling:
-            feats = _affine_step(feats, 1.0 / np.asarray(step.scale_, dtype=np.float64), zero, "RobustScaler")
+            feats = _affine_step(feats, 1.0 / np.asarray(step.scale_, dtype=np.float64), zero, "RobustScaler",
+                                 ops(OP_DIV, step.scale_))
         return feats
     if isinstance(step, pp.MaxAbsScaler):
-        return _affine_step(feats, 1.0 / np.asarray(step.scale_, dtype=np.float64), zero, "MaxAbsScaler")
+        return _affine_step(feats, 1.0 / np.asarray(step.scale_, dtype=np.float64), zero, "MaxAbsScaler",
+                            ops(OP_DIV, step.scale_))
     if isinstance(step, pp.MinMaxScaler):
+        exact = [m + a for m, a in zip(ops(OP_MUL, step.scale_), ops(OP_ADD, step.min_))]
+        if step.clip:
+            lo, hi = (float(v) for v in step.feature_range)
+            exact = [e + [(OP_CLIP, lo, hi)] for e in exact]
         return _affine_step(feats, np.asarray(step.scale_, dtype=np.float64), np.asarray(step.min_, dtype=np.float64),
-                            "MinMaxScaler", clip=step.feature_range if step.clip else None)
+                            "MinMaxScaler", exact, clip=step.feature_range if step.clip else None)
     raise AssertionError
 
 
@@ -206,10 +307,11 @@ def _imputer(step, feats):
     for f, fill in zip(feats, stats):
         def g(v, fill=fill):
             return float(fill) if np.isnan(v) else v
+        prog = f.prog.then((OP_NANFILL, float(fill), 0.0))
         if isinstance(f, _Affine) and not f.is_constant():
-            out.append(_Affine(f.src, f.t, f.a, f.c, _apply(g, f.nan)))
+            out.append(_Affine(f.src, f.t, f.a, f.c, _apply(g, f.nan), prog))
         else:
-            out.append(f.map_values(g))
+            out.append(f.map_values(g, prog))
     ind = getattr(step, "indicator_", None)
     if step.add_indicator and ind is not None:
         for i in ind.features_:
@@ -217,10 +319,11 @@ def _imputer(step, feats):
 
             def h(v):
                 return 1.0 if np.isnan(v) else 0.0
+            prog = f.prog.then((OP_ISNAN, 0.0, 0.0))
             if isinstance(f, _Affine) and not f.is_constant():
-                out.append(_Affine(f.src, [], [0.0], [0.0], _apply(h, f.nan)))
+                out.append(_Affine(f.src, [], [0.0], [0.0], _apply(h, f.nan), prog))
             else:
-                out.append(f.map_values(h))
+                out.append(f.map_values(h, prog))
     return out
 
 
@@ -277,19 +380,26 @@ def _valuewise(step, feats):
                 res.append(ERR)
         return res
 
+    def col(o, j):
+        return ERR if o is ERR else float(o[j])
+
     out = []
     for i, f in enumerate(feats):
         n_out = int((owner == i).sum())
         if isinstance(f, _Affine) and f.is_raw():
             nan_out = probe(i, [f.nan])[0]
+            # the program replays the steps before this one, so its lookup sees what the step sees: a NaN only when no
+            # imputer filled it
+            nan_look = nan_out if f.nan is not ERR and np.isnan(f.nan) else probe(i, [np.nan])[0]
             if is_bins:
                 t = np.asarray(step.bin_edges_[i][1:-1], dtype=np.float64)
                 reps = [float(step.bin_edges_[i][0]) if len(t) == 0 else float(np.nextafter(t[0], -np.inf))]
                 reps += [float(v) for v in t]
                 outs = probe(i, reps)
                 for j in range(n_out):
+                    look = _Lookup(OP_PIECES, t, [col(o, j) for o in outs], None, col(nan_look, j))
                     out.append(_Affine(f.src, t, np.zeros(len(reps)), [o[j] for o in outs],
-                                       ERR if nan_out is ERR else nan_out[j]))
+                                       ERR if nan_out is ERR else nan_out[j], f.prog.lookup(look)))
             else:
                 cats = np.asarray(step.categories_[i], dtype=np.float64)
                 keys = np.unique(cats[~np.isnan(cats)])
@@ -297,18 +407,26 @@ def _valuewise(step, feats):
                 unseen = float(keys.max() + 1.0) if len(keys) else 0.0
                 unk = probe(i, [unseen])[0]
                 for j in range(n_out):
+                    look = _Lookup(OP_TABLE, keys, [col(o, j) for o in outs], col(unk, j), col(nan_look, j))
                     out.append(_Table(f.src, keys, [o[j] for o in outs], ERR if unk is ERR else unk[j],
-                                      ERR if nan_out is ERR else nan_out[j]))
+                                      ERR if nan_out is ERR else nan_out[j], f.prog.lookup(look)))
         elif isinstance(f, _Table) or f.is_constant():
             vals = sorted({float(v) for v in f.values() if v is not ERR and not np.isnan(v)})
             has_nan = any(v is not ERR and np.isnan(v) for v in f.values())
             outs = dict(zip(vals, probe(i, vals)))
             nan_out = probe(i, [np.nan])[0] if has_nan else ERR
+            # the program's own values (exact arithmetic; the folded ones above may differ in the last bit)
+            pvals, p_nan = f.prog.values()
+            pouts = dict(zip(pvals, probe(i, pvals)))
+            p_nan_out = probe(i, [np.nan])[0] if p_nan else ERR
             for j in range(n_out):
                 def g(v, j=j):
                     o = nan_out if np.isnan(v) else outs[v]
                     return ERR if o is ERR else float(o[j])
-                out.append(f.map_values(g))
+
+                def gp(v, j=j):
+                    return col(p_nan_out if np.isnan(v) else pouts[v], j)
+                out.append(f.map_values(g, f.prog.compose(gp, pvals, p_nan)))
         else:
             raise TypeError(f"{name} after a transformer that is not the identity or piecewise constant on its column "
                             "is not supported")
@@ -443,6 +561,135 @@ def compile_maps(steps, n_raw, W):
         nk += len(k)
         nv += len(v)
     return ColumnMaps(hdr, np.concatenate(keys), np.concatenate(vals), R)
+
+
+class ColumnEncoding:
+    """Packed exact programs of ``E`` encoded columns over ``D`` raw columns (what ``dks_set_column_encoding`` reads):
+    ``pipe[:-1].transform`` replayed column by column, bit for bit.
+
+    * ``hdr`` int32 [E][3] = {raw source column, first op, op count};
+    * ``ops`` int32 [n_ops][4] = {code ``OP_*``, flags ``NAN_ERROR`` | ``UNKNOWN_ERROR``, m, table offset};
+    * ``opvals`` float64 [n_ops][2]: the constants of the scalar ops (``OP_CLIP``: lo, hi);
+    * ``tab`` float64: per lookup, its m sorted edges (``OP_PIECES``) or keys (``OP_TABLE``), then its outputs -- m + 1
+      bins, or m keys and the unknown output --, then the NaN output: 2 m + 2 values.  Outputs under the policy "error"
+      are 0 and flagged instead.
+
+    A lookup can only end a program.  ``transform`` evaluates the encoding in NumPy."""
+
+    def __init__(self, D, hdr, ops, opvals, tab):
+        self.D = int(D)
+        self.hdr = np.ascontiguousarray(np.asarray(hdr, dtype=np.int32).reshape(-1, 3))
+        self.ops = np.ascontiguousarray(np.asarray(ops, dtype=np.int32).reshape(-1, 4))
+        self.opvals = np.ascontiguousarray(np.asarray(opvals, dtype=np.float64).reshape(-1, 2))
+        self.tab = np.ascontiguousarray(np.asarray(tab, dtype=np.float64).reshape(-1))
+        self.E = self.hdr.shape[0]
+
+    @property
+    def sources(self):
+        return self.hdr[:, 0].copy()
+
+    def column(self, e, x):
+        """Encoded column ``e`` [n] of the raw values ``x`` [n] of its source; raises ``ValueError`` naming the first row
+        whose value the pipeline refuses."""
+        v = np.array(x, dtype=np.float64)
+        _, first, count = (int(u) for u in self.hdr[e])
+        for k in range(first, first + count):
+            code, flags, m, off = (int(u) for u in self.ops[k])
+            c0, c1 = self.opvals[k]
+            if code == OP_SUB:
+                v = v - c0
+            elif code == OP_DIV:
+                v = v / c0
+            elif code == OP_MUL:
+                v = v * c0
+            elif code == OP_ADD:
+                v = v + c0
+            elif code == OP_CLIP:
+                v = np.clip(v, c0, c1)
+            elif code == OP_NANFILL:
+                v = np.where(np.isnan(v), c0, v)
+            elif code == OP_ISNAN:
+                v = np.isnan(v).astype(np.float64)
+            else:
+                keys = self.tab[off:off + m]
+                outs = self.tab[off + m:off + 2 * m + 1]
+                nan_out = self.tab[off + 2 * m + 1]
+                nan = np.isnan(v)
+                if code == OP_PIECES:
+                    idx = np.searchsorted(keys, v, side="right")
+                    bad = nan & bool(flags & NAN_ERROR)
+                else:
+                    pos = np.minimum(np.searchsorted(keys, v, side="left"), max(m - 1, 0))
+                    hit = (m > 0) & (keys[pos] == v) if m else np.zeros(v.shape, dtype=bool)
+                    idx = np.where(hit, pos, m)
+                    bad = (nan & bool(flags & NAN_ERROR)) | (~nan & ~hit & bool(flags & UNKNOWN_ERROR))
+                if bad.any():
+                    r = int(np.nonzero(bad)[0][0])
+                    raise ValueError(f"row {r}: raw column {int(self.hdr[e, 0])} holds {x[r]!r}, which the pipeline "
+                                     "refuses (NaN, or a category unseen at fit time)")
+                v = np.where(nan, nan_out, outs[np.minimum(idx, len(outs) - 1)])
+        return v
+
+    def transform(self, X):
+        """``pipe[:-1].transform(X)`` [n, E] float64, densified."""
+        X = np.atleast_2d(np.asarray(X, dtype=np.float64))
+        if X.shape[1] != self.D:
+            raise ValueError(f"X has {X.shape[1]} columns, the encoding {self.D}")
+        out = np.empty((X.shape[0], self.E))
+        for e in range(self.E):
+            out[:, e] = self.column(e, X[:, int(self.hdr[e, 0])])
+        return out
+
+
+def _encoders(step):
+    """Every encoder or KBinsDiscretizer inside a fitted transformer (Pipelines and ColumnTransformers walked)."""
+    from sklearn import compose, pipeline, preprocessing as pp
+    if isinstance(step, pipeline.Pipeline):
+        return [e for _, s in step.steps for e in _encoders(s)]
+    if isinstance(step, compose.ColumnTransformer):
+        return [e for _, t, _ in step.transformers_ for e in _encoders(t)]
+    return [step] if isinstance(step, (pp.OneHotEncoder, pp.OrdinalEncoder, pp.KBinsDiscretizer)) else []
+
+
+def compile_encoding(steps, n_raw, n_out):
+    """Exact per-column programs (``ColumnEncoding``) of the fitted transformer ``steps`` (applied in order) over
+    ``n_raw`` raw columns, for an estimator reading ``n_out`` encoded columns that compares their values (a tree
+    model).  Accepts what ``compile_maps`` accepts, less its rule that a raw column may not feed both an encoder and a
+    numeric transformer (a sum over columns needs it, a tree does not); refuses encoders whose output dtype is not
+    float64 (a tree would compare rounded values)."""
+    for enc in _encoders_of(steps):
+        dt = getattr(enc, "dtype", None)
+        if dt is not None and np.dtype(dt) != np.float64:
+            raise TypeError(f"{_name(enc)}(dtype={np.dtype(dt).name}): only float64 encoder output is supported behind a "
+                            "tree model")
+    feats = [_Affine(c, [], [1.0], [0.0], np.nan) for c in range(n_raw)]
+    for step in steps:
+        feats = _compile_step(step, feats)
+    if len(feats) != n_out:
+        raise TypeError(f"the preprocessing yields {len(feats)} columns but the estimator reads {n_out}")
+    hdr, ops, opvals, tab = [], [], [], []
+    for e, f in enumerate(feats):
+        p = f.prog
+        hdr.append((p.src, len(ops), len(p.ops) + (p.look is not None)))
+        for code, c0, c1 in p.ops:
+            ops.append((code, 0, 0, 0))
+            opvals.append((c0, c1))
+        if p.look is None:
+            continue
+        lk = p.look
+        outs = lk.outs + ([lk.unknown] if lk.code == OP_TABLE else [])
+        if any(v is ERR for v in lk.outs):
+            raise TypeError(f"encoded column {e}: a value known to one encoder is refused by a later step: not supported")
+        flags = (NAN_ERROR if lk.nan is ERR else 0) | (UNKNOWN_ERROR if lk.code == OP_TABLE and lk.unknown is ERR else 0)
+        ops.append((lk.code, flags, len(lk.keys), len(tab)))
+        opvals.append((0.0, 0.0))
+        tab.extend(float(k) for k in lk.keys)
+        tab.extend(0.0 if v is ERR else float(v) for v in outs + [lk.nan])
+    return ColumnEncoding(n_raw, hdr, ops, opvals, tab)
+
+
+def _encoders_of(steps):
+    return [e for s in steps for e in _encoders(s)]
 
 
 def pipeline_parts(pipe):

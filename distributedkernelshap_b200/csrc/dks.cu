@@ -17,6 +17,7 @@
 #include "dks_sampler.cuh"
 #include "dks_instance_wide.cuh"
 #include "dks_trees.cuh"
+#include "dks_encode.cuh"
 #include "dks_kmach.cuh"
 
 namespace {
@@ -200,6 +201,16 @@ HeadDesc describe_head(const dks_ctx* ctx) {
     return h;
 }
 
+// out [n][E] = the column encoding of the raw rows X_dev [n][D] (encode_kernel, grid-stride)
+int launch_encode(dks_ctx* ctx, const double* X_dev, int n, double* out) {
+    const long long total = (long long)n * ctx->enc.E;
+    const int grid = (int)std::min<long long>(cdiv(total, 256), (long long)ctx->sm_count * 8);
+    dks::enc::encode_kernel<<<grid, 256, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->enc, out, ctx->d_status);
+    ctx->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    return DKS_OK;
+}
+
 int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const int G = ctx->G;
     const HeadDesc& h = ctx->head;
@@ -222,6 +233,15 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     // shared-plan route covers)
     double* xt = (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
+    ctx->tree_X = X_dev;
+    ctx->tree_D = ctx->D;
+    if (h.trees && ctx->enc.E > 0) {
+        // a tree behind a column encoding: the tree kernels read the encoded rows (a refused value is reported here)
+        TRY(grow(ctx, &ctx->d_Xenc, &ctx->cap_Xenc, (size_t)n * ctx->enc.E));
+        TRY(launch_encode(ctx, X_dev, n, ctx->d_Xenc));
+        ctx->tree_X = ctx->d_Xenc;
+        ctx->tree_D = ctx->enc.E;
+    }
     if (h.trees || h.kmach) {
         // tree ensembles and kernel machines: prep_kernel decides the varying groups (its scores are those of a zero linear
         // model, one identity output, and unused); the model's predict kernel then writes f(x) and link(f(x)) - link(fnull)
@@ -236,9 +256,9 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
                                                                                  ctx->d_linkfnull, nullptr, ctx->d_dlink,
                                                                                  ctx->d_status);
         else
-            dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->tree, ctx->C,
-                                                                                   ctx->link, ctx->d_linkfnull, nullptr,
-                                                                                   ctx->d_dlink, ctx->d_status);
+            dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->tree_X, n, ctx->tree_D, ctx->tree,
+                                                                                   ctx->C, ctx->link, ctx->d_linkfnull,
+                                                                                   nullptr, ctx->d_dlink, ctx->d_status);
         ctx->launches += 1;
     } else {
         kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
@@ -442,7 +462,7 @@ int launch_tree_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t sme
     auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<grid, dks::trees::THREADS, smem, st>>>(p, l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{}, ctx->tree,
-                                                   ctx->cur_X, ctx->D);
+                                                   ctx->tree_X, ctx->tree_D);
     ctx->launches += 1;
     return DKS_OK;
 }
@@ -469,6 +489,14 @@ void free_tree(dks_ctx* ctx) {
     ctx->cap_txinfo = 0;
 }
 
+void free_encoding(dks_ctx* ctx) {
+    EncodingDev& e = ctx->enc;
+    for (const void* q : {(const void*)e.hdr, (const void*)e.ops, (const void*)e.opv, (const void*)e.tab})
+        if (q) cudaFree((void*)q);
+    e = EncodingDev{};
+    dev_free(&ctx->d_bg_enc);
+}
+
 // dks_fit of a tree ensemble: the node arrays, the group of every column, every background row's direction at every node,
 // the column statistics stage 1 decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the tree kernels
 int fit_trees(dks_ctx* ctx) {
@@ -476,6 +504,17 @@ int fit_trees(dks_ctx* ctx) {
     const cudaStream_t st = ctx->stream;
     TreeDev& t = ctx->tree;
     const size_t nodes = (size_t)t.nodes;
+    // a column encoding: the tree reads E encoded columns, each in the group of its raw source
+    const int E = ctx->h_ehdr.empty() ? 0 : (int)(ctx->h_ehdr.size() / 3);
+    const int width = E > 0 ? E : D;
+    for (int e = 0; e < E; ++e)
+        if (ctx->h_ehdr[3 * e] >= D)
+            return fail(DKS_ERR_UNSUPPORTED, "column encoding: encoded column %d reads raw column %d of %d", e,
+                        ctx->h_ehdr[3 * e], D);
+    for (int32_t f : ctx->h_tfeat)
+        if (f >= width)
+            return fail(DKS_ERR_UNSUPPORTED, "tree ensemble: a split reads column %d of %d %s", f, width,
+                        E > 0 ? "encoded columns" : "columns");
     TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
     TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
     TRY(dev_alloc(&ctx->d_W, (size_t)D));
@@ -497,7 +536,22 @@ int fit_trees(dks_ctx* ctx) {
     std::vector<int32_t> colgrp(D, 0);
     for (int g = 0; g < G; ++g)
         for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
+    if (E > 0) {
+        std::vector<int32_t> raw = colgrp;
+        colgrp.assign(E, 0);
+        for (int e = 0; e < E; ++e) colgrp[e] = raw[ctx->h_ehdr[3 * e]];
+    }
     free_tree(ctx);
+    free_encoding(ctx);
+    if (E > 0) {
+        EncodingDev& en = ctx->enc;
+        TRY(upload_tree_array(&en.hdr, ctx->h_ehdr.data(), ctx->h_ehdr.size(), st));
+        TRY(upload_tree_array(&en.ops, ctx->h_eops.data(), ctx->h_eops.size(), st));
+        TRY(upload_tree_array(&en.opv, ctx->h_eopv.data(), ctx->h_eopv.size(), st));
+        TRY(upload_tree_array(&en.tab, ctx->h_etab.data(), ctx->h_etab.size(), st));
+        en.E = E;
+        TRY(dev_alloc(&ctx->d_bg_enc, (size_t)N * E));
+    }
     TRY(upload_tree_array(&t.feat, ctx->h_tfeat.data(), nodes, st));
     TRY(upload_tree_array(&t.thr, ctx->h_tthr.data(), nodes, st));
     TRY(upload_tree_array(&t.left, ctx->h_tleft.data(), nodes, st));
@@ -506,7 +560,7 @@ int fit_trees(dks_ctx* ctx) {
     TRY(upload_tree_array(&t.val, ctx->h_tval.data(), nodes * t.R, st));
     TRY(upload_tree_array(&t.roots, ctx->h_troots.data(), (size_t)t.T, st));
     TRY(upload_tree_array(&t.base, ctx->h_tbase.data(), (size_t)t.R, st));
-    TRY(upload_tree_array(&t.colgrp, colgrp.data(), (size_t)D, st));
+    TRY(upload_tree_array(&t.colgrp, colgrp.data(), colgrp.size(), st));
     unsigned char* bgdir = nullptr;
     TRY(dev_alloc(&bgdir, (size_t)N * nodes));
     t.bgdir = bgdir;
@@ -518,9 +572,16 @@ int fit_trees(dks_ctx* ctx) {
     CUDA_TRY(cudaMemcpyAsync(ctx->d_b, ctx->h_b.data(), sizeof(double), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
+    // varying groups are decided on the raw columns; the tree kernels read the encoded background
     dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
-    dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, st>>>(ctx->d_bg, N, D, t, bgdir);
-    dks::trees::tree_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(ctx->d_bg, N, D, t, C, ctx->link, nullptr, pred, nullptr,
+    const double* tbg = ctx->d_bg;
+    if (E > 0) {
+        CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
+        TRY(launch_encode(ctx, ctx->d_bg, N, ctx->d_bg_enc));
+        tbg = ctx->d_bg_enc;
+    }
+    dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, st>>>(tbg, N, width, t, bgdir);
+    dks::trees::tree_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(tbg, N, width, t, C, ctx->link, nullptr, pred, nullptr,
                                                                   nullptr);
     dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
     ctx->launches += 4;
@@ -529,8 +590,12 @@ int fit_trees(dks_ctx* ctx) {
     ctx->h_linkfnull.resize(C);
     CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    if (E > 0) CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     cudaFree(pred);
+    if (E > 0 && ctx->h_status[0] == DKS_ERR_DOMAIN)
+        return fail(DKS_ERR_DOMAIN, "background row %d holds a raw value the column encoding refuses (NaN, or a category "
+                    "unseen at fit time, where the pipeline raises)", ctx->h_status[1]);
     for (int c = 0; c < C; ++c)
         if (!std::isfinite(ctx->h_linkfnull[c]))
             return fail(DKS_ERR_NUMERIC, "tree ensemble: link(fnull) of output %d is not finite (fnull = %g): the background's "
@@ -1260,6 +1325,9 @@ int check_status(dks_ctx* ctx) {
     if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.kmach)
         return fail(DKS_ERR_DOMAIN, "instance %d holds NaN: kernel machines refuse it, as scikit-learn does",
                     ctx->h_status[1]);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.trees)
+        return fail(DKS_ERR_DOMAIN, "instance %d holds a raw value the column encoding refuses (NaN, or a category unseen "
+                    "at fit time, where the pipeline raises)", ctx->h_status[1]);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN)
         return fail(DKS_ERR_DOMAIN, "instance %d holds a raw value its column map refuses (NaN, or a category unseen at "
                     "fit time, where the pipeline raises)", ctx->h_status[1]);
@@ -1451,6 +1519,8 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b); dev_free(&ctx->d_mix);
     dev_free(&ctx->d_mixBW); dev_free(&ctx->d_mixsc); dev_free(&ctx->d_mixscr);
     free_tree(ctx);
+    free_encoding(ctx);
+    dev_free(&ctx->d_Xenc);
     free_kmach(ctx);
     if (ctx->cm.hdr) { cudaFree((void*)ctx->cm.hdr); cudaFree((void*)ctx->cm.keys); cudaFree((void*)ctx->cm.vals); }
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
@@ -1550,6 +1620,7 @@ int dks_set_model(dks_ctx* ctx, const double* W_host, const double* b_host, int 
     }
     ctx->R = R; ctx->act = activation; ctx->kappa = kappa; ctx->scalar_out = scalar_out;
     ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();   // maps belong to one model
+    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();   // so does a column encoding
     ctx->h_W.assign(W_host, W_host + (size_t)R * ctx->D);
     ctx->h_b.assign(b_host, b_host + R);
     ctx->fitted = false;
@@ -1587,6 +1658,7 @@ int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* 
     ctx->C = member_act == DKS_ACT_BINARY_LOGISTIC ? 2 : R_m;
     ctx->R = R; ctx->act = DKS_ACT_MIX; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
     ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
     ctx->h_W.assign(W_host, W_host + (size_t)R * ctx->D);
     ctx->h_b.assign(b_host, b_host + R);
     ctx->fitted = false;
@@ -1612,6 +1684,7 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
     case DKS_TREE_HEAD_EXP: REQUIRE(R == 1, "exp tree head needs R == 1 (got %d)", R); C = 1; break;
     default: return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: unknown head %d", head);
     }
+    const int width = ctx->h_ehdr.empty() ? ctx->D : (int)(ctx->h_ehdr.size() / 3);   // encoded columns, if any
     for (int nd = 0; nd < n_nodes; ++nd) {
         const int f = feature[nd];
         if (f < 0) {
@@ -1620,10 +1693,10 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
                     return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: leaf %d has a non-finite value", nd);
             continue;
         }
-        if (f >= ctx->D || std::isnan(threshold[nd]) || left[nd] <= nd || right[nd] <= nd || left[nd] >= n_nodes ||
+        if (f >= width || std::isnan(threshold[nd]) || left[nd] <= nd || right[nd] <= nd || left[nd] >= n_nodes ||
             right[nd] >= n_nodes)
             return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: node %d is malformed (feature %d of %d, children %d / %d "
-                        "must follow it)", nd, f, ctx->D, left[nd], right[nd]);
+                        "must follow it)", nd, f, width, left[nd], right[nd]);
     }
     for (int k = 0; k < n_trees; ++k)
         if (roots[k] < 0 || roots[k] >= n_nodes) return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: root %d out of range", k);
@@ -1718,6 +1791,7 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
     // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
     ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_KMACH; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
     ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
     ctx->h_W.assign((size_t)D, 0.0);
     ctx->h_b.assign(1, 0.0);
     ctx->fitted = false;
@@ -1766,6 +1840,77 @@ int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, con
     return DKS_OK;
 }
 
+int dks_set_column_encoding(dks_ctx* ctx, int E, const int32_t* hdr_host, const int32_t* ops_host, const double* opvals_host,
+                            int n_ops, const double* tab_host, int n_tab) {
+    BIND(ctx);
+    ctx->fitted = false;
+    if (hdr_host == nullptr) {
+        ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
+        return DKS_OK;
+    }
+    REQUIRE(ctx->D > 0, "dks_set_column_encoding: call dks_set_background first (D unknown)");
+    if (ctx->act >= 0 && ctx->act != DKS_ACT_TREES)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: for tree ensembles only (linear models read their "
+                    "pipelines through dks_set_column_maps)");
+    if (E < 1 || n_ops < 0 || n_tab < 0 || (n_ops > 0 && (!ops_host || !opvals_host)) || (n_tab > 0 && !tab_host))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: bad sizes");
+    for (int e = 0; e < E; ++e) {
+        const int src = hdr_host[3 * e], first = hdr_host[3 * e + 1], count = hdr_host[3 * e + 2];
+        if (src < 0 || src >= ctx->D || first < 0 || count < 0 || (long long)first + count > n_ops)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: malformed header of encoded column %d (source %d of "
+                        "%d, ops %d + %d of %d)", e, src, ctx->D, first, count, n_ops);
+    }
+    for (int k = 0; k < n_ops; ++k) {
+        const int code = ops_host[4 * k], flags = ops_host[4 * k + 1], m = ops_host[4 * k + 2], off = ops_host[4 * k + 3];
+        const double c0 = opvals_host[2 * k], c1 = opvals_host[2 * k + 1];
+        if (code < DKS_ENC_OP_SUB || code > DKS_ENC_OP_TABLE)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: op %d: unknown code %d", k, code);
+        if (code < DKS_ENC_OP_PIECES) {
+            if (flags != 0 || !std::isfinite(c0) || (code == DKS_ENC_OP_CLIP && !(std::isfinite(c1) && c0 <= c1)))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: op %d: flags must be 0 and constants finite", k);
+            continue;
+        }
+        const int allowed = DKS_ENC_NAN_ERROR | (code == DKS_ENC_OP_TABLE ? DKS_ENC_UNKNOWN_ERROR : 0);
+        if ((flags & ~allowed) || m < 0 || off < 0 || (long long)off + 2 * (long long)m + 2 > n_tab)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: op %d: malformed lookup (flags %d, m %d, offset %d of "
+                        "%d)", k, flags, m, off, n_tab);
+        for (int q = 0; q < m; ++q) {
+            const double t = tab_host[off + q];
+            if (!std::isfinite(t) || (q > 0 && !(tab_host[off + q - 1] < t)))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: op %d: %s must be finite and strictly increasing",
+                            k, code == DKS_ENC_OP_PIECES ? "edges" : "keys");
+        }
+    }
+    ctx->h_ehdr.assign(hdr_host, hdr_host + 3 * (size_t)E);
+    ctx->h_eops.assign(ops_host, ops_host + 4 * (size_t)n_ops);
+    ctx->h_eopv.assign(opvals_host, opvals_host + 2 * (size_t)n_ops);
+    ctx->h_etab.assign(tab_host, tab_host + n_tab);
+    if (ctx->h_eops.empty()) ctx->h_eops.assign(4, 0), ctx->h_eopv.assign(2, 0.0);   // device copies are never empty
+    if (ctx->h_etab.empty()) ctx->h_etab.assign(1, 0.0);
+    return DKS_OK;
+}
+
+int dks_encode_host(dks_ctx* ctx, const double* X_host, int n, double* out_host) {
+    BIND(ctx);
+    REQUIRE(ctx->fitted && ctx->enc.E > 0, "dks_encode_host: call dks_fit with a column encoding set first");
+    REQUIRE(X_host && out_host && n > 0, "dks_encode_host: bad arguments");
+    const int E = ctx->enc.E;
+    double *dX = nullptr, *dO = nullptr;
+    TRY(dev_alloc(&dX, (size_t)n * ctx->D));
+    TRY(dev_alloc(&dO, (size_t)n * E));
+    CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
+    TRY(launch_encode(ctx, dX, n, dO));
+    CUDA_TRY(cudaMemcpyAsync(out_host, dO, sizeof(double) * n * E, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    cudaFree(dX); cudaFree(dO);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
+        return fail(DKS_ERR_DOMAIN, "row %d holds a raw value the column encoding refuses (NaN, or a category unseen at fit "
+                    "time, where the pipeline raises)", ctx->h_status[1]);
+    return DKS_OK;
+}
+
 int dks_set_link(dks_ctx* ctx, int link) {
     BIND(ctx);
     REQUIRE(link == DKS_LINK_IDENTITY || link == DKS_LINK_LOGIT, "dks_set_link: unknown link %d", link);
@@ -1801,6 +1946,8 @@ int dks_fit(dks_ctx* ctx) {
             REQUIRE(seen[c]++ == 0, "column %d appears in more than one group", c);
         }
     }
+    if (!h.trees && !ctx->h_ehdr.empty())
+        return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model is not a tree ensemble");
     if (h.trees) return fit_trees(ctx);
     if (h.kmach) return fit_kmach(ctx);
     TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
@@ -1922,9 +2069,15 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     TRY(dev_alloc(&dO, (size_t)n * ctx->C));
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
+    double* dXe = nullptr;
+    if (ctx->head.trees && ctx->enc.E > 0) {
+        TRY(dev_alloc(&dXe, (size_t)n * ctx->enc.E));
+        TRY(launch_encode(ctx, dX, n, dXe));
+    }
     if (ctx->head.trees)
-        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->tree, ctx->C, ctx->link,
-                                                                               nullptr, dO, nullptr, nullptr);
+        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dXe ? dXe : dX, n, dXe ? ctx->enc.E : ctx->D,
+                                                                               ctx->tree, ctx->C, ctx->link, nullptr, dO,
+                                                                               nullptr, nullptr);
     else if (ctx->head.kmach)
         dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->km, ctx->C, ctx->link,
                                                                              nullptr, dO, nullptr, ctx->d_status);
@@ -1937,8 +2090,12 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     cudaFree(dX); cudaFree(dO);
+    if (dXe) cudaFree(dXe);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.kmach)
         return fail(DKS_ERR_DOMAIN, "row %d holds NaN: kernel machines refuse it, as scikit-learn does", ctx->h_status[1]);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.trees)
+        return fail(DKS_ERR_DOMAIN, "row %d holds a raw value the column encoding refuses (NaN, or a category unseen at fit "
+                    "time, where the pipeline raises)", ctx->h_status[1]);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN)
         return fail(DKS_ERR_DOMAIN, "row %d holds a raw value its column map refuses (NaN, or a category unseen at fit time, "
                     "where the pipeline raises)", ctx->h_status[1]);

@@ -160,6 +160,16 @@ struct TreeDev {
     int nodes, T, R, head, cmp;
 };
 
+// column encoding of a tree ensemble (dks_set_column_encoding, DESIGN.md §5.0.13): E encoded columns, each a program of
+// DKS_ENC_OP_* over one raw column (dks_encode.cuh)
+struct EncodingDev {
+    const int* hdr;              // [E][3] {raw source column, first op, op count}
+    const int* ops;              // [n_ops][4] {code, flags, m, table offset}
+    const double* opv;           // [n_ops][2] constants
+    const double* tab;           // lookups: keys [m], outputs [m + 1], NaN output
+    int E;                       // 0: no encoding
+};
+
 // kernel machines (dks_set_kernel_machine, DESIGN.md §5.0.12): K members, member k owning support vectors sv_off[k] ..
 // sv_off[k + 1]; f_k = sum_v dual[v] phi(t) + icpt, t = sum_c h(x_c, sv_c) per DKS_KM_KERNEL_*, then the head
 // DKS_KM_HEAD_*.  Intercepts icpt[k R + q] (K R <= DKS_KM_MAX_K: one member of R <= 8 outputs, or K members of one).
@@ -254,6 +264,16 @@ struct dks_ctx {
     std::vector<unsigned char> h_tmiss;
     TreeDev tree = {};
     size_t cap_txinfo = 0;
+    // its column encoding (dks_set_column_encoding; empty h_ehdr: none), the device copy dks_fit builds, the encoded
+    // background and the encoded rows of the current call
+    std::vector<int32_t> h_ehdr, h_eops;
+    std::vector<double> h_eopv, h_etab;
+    EncodingDev enc = {};
+    double* d_bg_enc = nullptr;  // [N][E]
+    double* d_Xenc = nullptr;    // [n][E]
+    size_t cap_Xenc = 0;
+    const double* tree_X = nullptr;   // rows the tree kernels of the current call read (d_Xenc, or the raw rows) ...
+    int tree_D = 0;                   // ... and their width
     // kernel machine (act == DKS_ACT_KMACH): host copies of the arrays, and their device copies built by dks_fit
     std::vector<double> h_ksv, h_kdual, h_kcolw, h_kcolo;
     KmDev km = {};

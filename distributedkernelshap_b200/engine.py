@@ -17,7 +17,7 @@ from .data import DenseData, convert_to_data, convert_to_link
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
 from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, extract_kernel_machine_spec
 from .predictors import extract_linear_spec
-from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_tree_spec
+from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_tree_pipeline_spec, extract_tree_spec
 
 logger = logging.getLogger(__name__)
 
@@ -27,6 +27,8 @@ MAX_ROWS_PER_CALL = 65536     # rows per C-ABI call: bounds the engine's per-cal
 # (M-1) x (M-1) normal matrix: about 222 KB at M = 128, S = 4096.  Row blocks of 4096 bound that workspace by ~0.9 GB.
 MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE = 4096
 MAX_SAMPLED_SIZES = 64        # subset sizes the device sampler draws from (csrc/dks_sampler.cuh, MAX_SIZES)
+# a tree behind a column encoding keeps the encoded rows of a call on the device (n x E x 8 B): row blocks bound them
+MAX_ENCODED_BYTES_PER_CALL = 256 << 20
 
 
 def per_instance_workspace_bytes(M, S):
@@ -129,7 +131,8 @@ class GpuKernelExplainer:
     model
         What the reference passes as ``predictor``: a bound ``predict_proba`` / ``decision_function`` of a linear
         model or of a ``Pipeline`` of per-column preprocessing ending in one (explained in raw feature space), or a
-        ``LinearModelSpec`` (see ``predictors.extract_linear_spec``).  A raw value the pipeline would refuse (NaN, or an
+        ``LinearModelSpec`` (see ``predictors.extract_linear_spec``); a tree model, bare or behind such a ``Pipeline``
+        (``trees.extract_tree_pipeline_spec``: the device replays the steps bit for bit); a kernel machine.  A raw value the pipeline would refuse (NaN, or an
         unseen category under ``handle_unknown='error'``) raises ``ValueError``.
     data
         Background data: array, DataFrame or ``DenseData`` (groups and weights honoured).
@@ -155,7 +158,9 @@ class GpuKernelExplainer:
         self.lib = _cabi.load()
         self.link = convert_to_link(link)
         self.model_callable = model
-        tree_spec = extract_tree_spec(model)
+        pipe_spec = extract_tree_pipeline_spec(model)
+        # a tree behind per-column preprocessing: explained in raw feature space, the device replaying the steps
+        tree_spec, self.encoding = pipe_spec if pipe_spec is not None else (extract_tree_spec(model), None)
         km_spec = extract_kernel_machine_spec(model) if tree_spec is None else None
         self.spec = tree_spec if tree_spec is not None else km_spec if km_spec is not None else extract_linear_spec(model)
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
@@ -203,7 +208,10 @@ class GpuKernelExplainer:
                 _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree, k.coef0, k.head_code,
                 _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
         elif tree_spec is not None:
-            t = tree_spec
+            t, e = tree_spec, self.encoding
+            if e is not None:
+                _cabi.check(self.lib.dks_set_column_encoding(self._ctx, e.E, _cabi.ptr(e.hdr), _cabi.ptr(e.ops),
+                                                             _cabi.ptr(e.opvals), len(e.ops), _cabi.ptr(e.tab), len(e.tab)))
             _cabi.check(self.lib.dks_set_tree_model(
                 self._ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
                 _cabi.ptr(t.missing_left), _cabi.ptr(t.value), t.R, t.n_trees, _cabi.ptr(t.roots), _cabi.ptr(t.base),
@@ -239,9 +247,41 @@ class GpuKernelExplainer:
         self._l1_general_all_select = False
         self._link_fx_parts = []
         self._last_rows = 0
+        if self.encoding is not None:
+            self._check_encoding(bg)
         self._check_model_against_callable(bg)
 
     # ------------------------------------------------------------------------------------------------------
+    def encode(self, X):
+        """The encoded rows ``pipe[:-1].transform(X)`` [n, E] as the device computes them (``dks_encode_host``), for a
+        tree behind a column encoding."""
+        if self.encoding is None:
+            raise TypeError("the model has no column encoding (not a tree behind a Pipeline)")
+        X = np.ascontiguousarray(np.atleast_2d(np.asarray(X, dtype=np.float64)))
+        out = np.zeros((X.shape[0], self.encoding.E))
+        _cabi.check(self.lib.dks_encode_host(self._ctx, _cabi.ptr(X), X.shape[0], _cabi.ptr(out)))
+        return out
+
+    def _check_encoding(self, bg):
+        """The device's encoding of the background must be what the pipeline's own steps give, bit for bit."""
+        import warnings
+        from .column_maps import pipeline_parts
+        want = bg
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            for step in pipeline_parts(self.model_callable.__self__)[0]:
+                want = step.transform(want)
+        if hasattr(want, "toarray"):
+            want = want.toarray()
+        want = np.asarray(want, dtype=np.float64)
+        got = self.encode(bg)
+        if want.shape != got.shape or not np.array_equal(got, want, equal_nan=True):
+            bad = "shape mismatch" if want.shape != got.shape else \
+                f"{int((~((got == want) | (np.isnan(got) & np.isnan(want)))).sum())} entries differ"
+            raise ValueError("the column encoding compiled from the pipeline does not reproduce "
+                             f"pipeline[:-1].transform(background) bit for bit ({bad}): refusing to explain a different "
+                             "function")
+
     def _check_model_against_callable(self, bg):
         """The extracted linear model must reproduce the user's callable on the background rows."""
         if not callable(self.model_callable):
@@ -469,8 +509,13 @@ class GpuKernelExplainer:
         return [phi[c] for c in range(self.D)]
 
     def _rows_per_call(self):
-        """Rows per C-ABI call (``rows_per_call``)."""
-        return rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size, self.spec.R)
+        """Rows per C-ABI call (``rows_per_call``); a column encoding also bounds the encoded rows of a call by
+        ``MAX_ENCODED_BYTES_PER_CALL`` (results are per row and device plans keyed by the global row: the block size
+        does not change phi)."""
+        rows = rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size, self.spec.R)
+        if self.encoding is not None:
+            rows = min(rows, max(1, MAX_ENCODED_BYTES_PER_CALL // (8 * self.encoding.E)))
+        return rows
 
     def link_predictions(self):
         """``link(f(x))`` of the rows of the last ``shap_values`` call, ``[n, C]`` (``[n]`` for scalar-output models):

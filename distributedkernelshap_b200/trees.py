@@ -294,6 +294,29 @@ def extract_tree_spec(predictor):
             return _gb_spec(owner, method, names)
         return _forest_spec(owner, method, names)
     if names & _CONTAINERS and _contains_tree(owner):
-        raise NotImplementedError(f"{type(owner).__name__} holding a tree model: trees behind a Pipeline or inside an "
-                                  "ensemble are not supported; pass the tree model's own method")
+        raise NotImplementedError(f"{type(owner).__name__} holding a tree model: trees inside an ensemble are not "
+                                  "supported, and a Pipeline of per-column steps ending in a tree model is read by "
+                                  "extract_tree_pipeline_spec; pass the tree model's own method")
     return None
+
+
+def extract_tree_pipeline_spec(predictor):
+    """``(TreeEnsembleSpec, ColumnEncoding)`` of a bound method of a fitted ``Pipeline`` of per-column steps ending in a
+    tree model ``extract_tree_spec`` reads: the spec of the final estimator (its features index the encoded columns) and
+    the exact programs of ``pipe[:-1].transform`` (``column_maps.compile_encoding``).  ``None`` for anything else.  The
+    steps the column maps refuse raise ``TypeError`` naming the step; so do trees inside ensembles or calibrators behind
+    the pipeline, and the final estimator's own refusals raise as in ``extract_tree_spec``."""
+    from .column_maps import compile_encoding, pipeline_parts
+    owner = getattr(predictor, "__self__", None)
+    method = getattr(predictor, "__name__", None)
+    if owner is None or "Pipeline" not in _names(owner) or not hasattr(owner, "steps"):
+        return None
+    pre, final = pipeline_parts(owner)
+    if not (_names(final) & _TREE_MODELS):
+        return None
+    if not hasattr(owner, "n_features_in_") or not hasattr(final, "n_features_in_"):
+        raise TypeError("Pipeline is not fitted")
+    spec = extract_tree_spec(getattr(final, method))
+    enc = compile_encoding(pre, int(owner.n_features_in_), spec.n_features)
+    spec.n_features = enc.D
+    return spec, enc

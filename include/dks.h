@@ -76,7 +76,20 @@ extern "C" {
 /* split comparison: x goes left when x <= threshold */
 #define DKS_TREE_CMP_F32 0       /* (double)(float)x <= threshold: scikit-learn's sklearn.tree casts X to float32 */
 #define DKS_TREE_CMP_F64 1       /* x <= threshold in float64: the histogram gradient boosting estimators */
-#define DKS_ACT_KMACH 7         /* kernel machine: set by dks_set_kernel_machine only (dks_set_model refuses it) */
+/* ops of a column encoding (dks_set_column_encoding): each maps the float64 value v of one encoded column, in program order,
+ * rounding as scikit-learn's numpy arithmetic does (no fused multiply-add) */
+#define DKS_ENC_OP_SUB 0         /* v - c0 (StandardScaler, RobustScaler centring) */
+#define DKS_ENC_OP_DIV 1         /* v / c0 (StandardScaler, RobustScaler, MaxAbsScaler scaling) */
+#define DKS_ENC_OP_MUL 2         /* v * c0 (MinMaxScaler) */
+#define DKS_ENC_OP_ADD 3         /* v + c0 (MinMaxScaler) */
+#define DKS_ENC_OP_CLIP 4        /* np.clip(v, c0, c1): NaN stays NaN (MinMaxScaler(clip=True)) */
+#define DKS_ENC_OP_NANFILL 5     /* c0 where v is NaN (SimpleImputer) */
+#define DKS_ENC_OP_ISNAN 6       /* 1 where v is NaN, else 0 (SimpleImputer's missing indicator) */
+#define DKS_ENC_OP_PIECES 7      /* m sorted edges: output of bin numpy.searchsorted(edges, v, side='right') (KBinsDiscretizer) */
+#define DKS_ENC_OP_TABLE 8       /* m sorted keys: output of the exactly equal key, else the unknown output (encoders) */
+#define DKS_ENC_NAN_ERROR 2      /* op flag (PIECES, TABLE): a NaN is refused */
+#define DKS_ENC_UNKNOWN_ERROR 4  /* op flag (TABLE): a value matching no key is refused */
+#define DKS_ACT_KMACH 7        /* kernel machine: set by dks_set_kernel_machine only (dks_set_model refuses it) */
 
 /* kernel of a kernel machine (dks_set_kernel_machine): K(x, v) = phi(t), t = sum_c h(x_c, v_c) with the member's column
  * weight w_c and origin o_c (its scalers folded in) */
@@ -146,7 +159,8 @@ int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* 
  * varying sets), per-instance device plans and caller-supplied plans, kernel 'auto' or 'simt' (tcgen05 / shared are
  * DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route.  Float64 throughout; a link(ey) or link(f(x)) that
  * is not finite (the logit of a probability of exactly 0 or 1) is DKS_ERR_NUMERIC, nothing non-finite is written into phi.
- * A forest whose per-instance buffers do not fit shared memory is DKS_ERR_UNSUPPORTED. */
+ * A forest whose per-instance buffers do not fit shared memory is DKS_ERR_UNSUPPORTED.  With a column encoding set
+ * (dks_set_column_encoding) the split features index the E encoded columns, not the D raw ones. */
 int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const double* threshold, const int32_t* left,
                        const int32_t* right, const uint8_t* missing_left, const double* value, int R, int n_trees,
                        const int32_t* roots, const double* base, int head, int cmp, int scalar_out);
@@ -181,6 +195,23 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
  * non-finite keys, non-finite values) return DKS_ERR_UNSUPPORTED.  hdr_host == NULL clears the maps; dks_set_model does too. */
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
                         const double* vals_host, int n_vals);
+/* column encoding of a tree ensemble (call after dks_set_background / dks_set_groups, before dks_set_tree_model): the model
+ * reads E encoded columns, each an exact program over one raw column -- a scikit-learn Pipeline of per-column steps replayed
+ * bit for bit (DESIGN.md §5.0.13).  hdr_host [E][3] = {raw source column, first op, op count}; ops_host [n_ops][4] = {code
+ * DKS_ENC_OP_*, flags DKS_ENC_*_ERROR, m, table offset}; opvals_host [n_ops][2] = {c0, c1}; tab_host [n_tab]: per PIECES /
+ * TABLE op at its offset, the m strictly increasing finite edges / keys, the m + 1 outputs (bins; or keys then the unknown
+ * output), then the NaN output.  Varying groups and masking stay on the raw columns: encoded column e belongs to the group
+ * of its source, and every kernel of the tree route reads the encoded rows (encode_kernel, one thread per row and encoded
+ * column, runs first in dks_fit, stage 1 and dks_predict_host).  A refused value is DKS_ERR_DOMAIN (by dks_fit for a
+ * background row, by dks_predict_host and the explain calls for an instance).  Malformed input (a source out of range, an
+ * unknown op or flag, unsorted or non-finite keys or edges, non-finite constants, offsets out of range) is
+ * DKS_ERR_UNSUPPORTED; so is any model other than a tree ensemble (dks_set_model, dks_set_mixture and
+ * dks_set_kernel_machine clear the encoding).  hdr_host == NULL clears it. */
+int dks_set_column_encoding(dks_ctx* ctx, int E, const int32_t* hdr_host, const int32_t* ops_host, const double* opvals_host,
+                            int n_ops, const double* tab_host, int n_tab);
+/* the encoded rows [n x E] of host rows X_host [n x D], computed by the device's encode kernel (needs dks_fit with an
+ * encoding set); a refused value is DKS_ERR_DOMAIN with the row. */
+int dks_encode_host(dks_ctx* ctx, const double* X_host, int n, double* out_host);
 int dks_set_link(dks_ctx* ctx, int link);
 /* runs the fit kernels (grouped background scores, fnull = sum_j w_j f(bg_j), link(fnull)); synchronises. */
 int dks_fit(dks_ctx* ctx);
