@@ -211,6 +211,13 @@ int launch_encode(dks_ctx* ctx, const double* X_dev, int n, double* out) {
     return DKS_OK;
 }
 
+// stage 1's instantiation for R score rows: the compile-time bound 1 or 8 (a mixture: DKS_MIX_MAX_R)
+template <bool STAGE, bool MAPS>
+decltype(&dks::prep_kernel<STAGE, MAPS>) prep_kernel_for(bool mixture, int R) {
+    if (mixture) return dks::prep_kernel<STAGE, MAPS, true>;
+    return R == 1 ? dks::prep_kernel<STAGE, MAPS, false, 1> : dks::prep_kernel<STAGE, MAPS, false, 8>;
+}
+
 int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const int G = ctx->G;
     const HeadDesc& h = ctx->head;
@@ -225,10 +232,10 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const size_t maps_doubles = maps ? (size_t)ctx->cm.n_keys + ctx->cm.n_vals : 0;
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D, maps_doubles) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D, maps_doubles);
-    auto kern = h.mixture() ? (maps ? (stage ? dks::prep_kernel<true, true, true> : dks::prep_kernel<false, true, true>)
-                                    : (stage ? dks::prep_kernel<true, false, true> : dks::prep_kernel<false, false, true>))
-                            : maps ? (stage ? dks::prep_kernel<true, true> : dks::prep_kernel<false, true>)
-                                   : (stage ? dks::prep_kernel<true, false> : dks::prep_kernel<false, false>);
+    // the score rows stage 1 computes: one for trees and kernel machines (the scores of a zero linear model, unused)
+    const int R = h.trees || h.kmach ? 1 : ctx->R;
+    auto kern = stage ? (maps ? prep_kernel_for<true, true>(h.mixture(), R) : prep_kernel_for<true, false>(h.mixture(), R))
+                      : (maps ? prep_kernel_for<false, true>(h.mixture(), R) : prep_kernel_for<false, false>(h.mixture(), R));
     // nibble tables for the shared-plan route: the binary head's at any G, the other heads' up to 128 groups (what their
     // shared-plan route covers)
     double* xt = (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;

@@ -7,6 +7,8 @@
 // masked batch (S*N x D, KernelExplainer.allocate/addsample) is therefore never materialised.
 #pragma once
 
+#include <cuda_pipeline.h>
+
 #include "dks_common.cuh"
 #include "dks_linkmath.cuh"
 
@@ -59,8 +61,12 @@ __device__ __forceinline__ double link_f(double p, int link) {
     return link == DKS_LINK_LOGIT ? log(p / (1.0 - p)) : p;
 }
 
-// model head in float64 on R scores -> C outputs (C = 2 for the binary head, else R)
+// model head in float64 on R scores -> C outputs (C = 2 for the binary head, else R).
+// RB: a compile-time bound on R.  The loops then unroll over RB with r < R guards, so that a caller's z and out arrays
+// stay in registers; 0: the loops run to the run-time R.  The same operations in the same order either way.
+template <int RB = 0>
 __device__ inline void head_f64(const double* z, int R, int act, double kappa, double* out) {
+    constexpr bool fixed = RB > 0;
     if (act == DKS_ACT_BINARY_LOGISTIC) {
         // softmax([-kz/2, kz/2]) evaluated the numerically stable way sklearn does
         double t = kappa * z[0];
@@ -70,24 +76,32 @@ __device__ inline void head_f64(const double* z, int R, int act, double kappa, d
         out[0] = t >= 0 ? small : big;
     } else if (act == DKS_ACT_SOFTMAX) {
         double m = z[0];
-        for (int r = 1; r < R; ++r) m = fmax(m, z[r]);
+#pragma unroll
+        for (int r = 1; r < (fixed ? RB : R); ++r) if (!fixed || r < R) m = fmax(m, z[r]);
         double sum = 0;
-        for (int r = 0; r < R; ++r) { out[r] = exp(z[r] - m); sum += out[r]; }
-        for (int r = 0; r < R; ++r) out[r] /= sum;
+#pragma unroll
+        for (int r = 0; r < (fixed ? RB : R); ++r) if (!fixed || r < R) { out[r] = exp(z[r] - m); sum += out[r]; }
+#pragma unroll
+        for (int r = 0; r < (fixed ? RB : R); ++r) if (!fixed || r < R) out[r] /= sum;
     } else if (act == DKS_ACT_OVR) {
         // one-vs-rest: sigmoid(z_r) / sum_r' sigmoid(z_r'), formed from log sigmoid so that no class underflows to 0/0
         double m = -INFINITY;
-        for (int r = 0; r < R; ++r) {
+#pragma unroll
+        for (int r = 0; r < (fixed ? RB : R); ++r) {
+            if (fixed && r >= R) continue;
             out[r] = fmin(z[r], 0.0) - log1p(exp(-fabs(z[r])));
             m = fmax(m, out[r]);
         }
         double sum = 0;
-        for (int r = 0; r < R; ++r) { out[r] = exp(out[r] - m); sum += out[r]; }
-        for (int r = 0; r < R; ++r) out[r] /= sum;
+#pragma unroll
+        for (int r = 0; r < (fixed ? RB : R); ++r) if (!fixed || r < R) { out[r] = exp(out[r] - m); sum += out[r]; }
+#pragma unroll
+        for (int r = 0; r < (fixed ? RB : R); ++r) if (!fixed || r < R) out[r] /= sum;
     } else if (act == DKS_ACT_EXP) {
         out[0] = exp(z[0]);          // log-link GLM: predict = exp(z)
     } else {
-        for (int r = 0; r < R; ++r) out[r] = z[r];
+#pragma unroll
+        for (int r = 0; r < (fixed ? RB : R); ++r) if (!fixed || r < R) out[r] = z[r];
     }
 }
 
@@ -105,9 +119,11 @@ __device__ inline void mix_head_f64(const double* z, const MixHead& mh, double* 
 // column maps: adds f_col(x), the R score contributions of one raw value, to acc.  A binary search over the column's
 // breakpoints (numpy's searchsorted side='right': a value on a breakpoint takes the piece on its right) then R FMAs, or over
 // its keys (exact match, else the unknown row) then R loads.  Returns false, adding nothing, where the map's policy is
-// "error" (NaN, or a category unseen at fit time).
+// "error" (NaN, or a category unseen at fit time).  RB: a compile-time bound on R, as for head_f64.
+template <int RB = 0>
 __device__ __forceinline__ bool cm_add(const int* __restrict__ h, const double* __restrict__ keys,
                                        const double* __restrict__ vals, double x, int R, double* acc) {
+    constexpr bool fixed = RB > 0;
     const int flags = h[0], m = h[1];
     const double* t = keys + h[2];
     const double* v = vals + h[3];
@@ -125,10 +141,12 @@ __device__ __forceinline__ bool cm_add(const int* __restrict__ h, const double* 
         int lo = 0, hi = m - 1;                   // piece = breakpoints <= x
         while (lo < hi) { const int mid = (lo + hi) >> 1; if (t[mid] <= x) lo = mid + 1; else hi = mid; }
         const double* p = v + (size_t)2 * lo * R;
-        for (int r = 0; r < R; ++r) acc[r] += fma(p[r], x, p[R + r]);
+#pragma unroll
+        for (int r = 0; r < (fixed ? RB : R); ++r) if (!fixed || r < R) acc[r] += fma(p[r], x, p[R + r]);
         return true;
     }
-    for (int r = 0; r < R; ++r) acc[r] += row[r];
+#pragma unroll
+    for (int r = 0; r < (fixed ? RB : R); ++r) if (!fixed || r < R) acc[r] += row[r];
     return true;
 }
 
@@ -276,17 +294,22 @@ __device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
 // Fused preparation: a block handles `ipb` instances.  Phase 1, one thread per (instance, group): grouped
 // contribution XW[i][g][r] and the "group varies" flag (KernelExplainer.varying_groups); phase 2, one thread per
 // instance: varying bit-mask, M, histogram of M, f(x), link(f(x)) - link(fnull).
+// The two instance lists and the histogram are counted per block in shared memory first: one global atomic per block and
+// counter, and each instance takes the slot at its block's base plus its rank in the block.  The order of a list is
+// therefore unspecified (it already was with one atomic per instance); every consumer works per instance.
 // STAGE: the block first copies what phase 1 reads -- its instances' rows of X, W, the column statistics and the group
 // tables -- into shared memory with coalesced loads, so the per-(instance, group) loop runs without dependent global loads.
-// (Measured on the Adult shape: 13.3 us per launch under ncu against 13.8 us unstaged -- the kernel is bound by launch +
-// one cold DRAM round trip + the serial per-instance tail, not by the column loop; kept because it is never slower.)
-// The host picks STAGE when the tables fit shared memory.
+// The host picks STAGE when the tables fit shared memory.  (Measured on the Adult shape, 2560 instances: 7.5 us per launch
+// under torch.profiler on an H100 80GB HBM3 at 700 W, against 12.9 us with local-memory arrays, per-instance atomics and
+// synchronous staging; DESIGN.md 5.0.)
 // MAPS: the contributions come from the column maps `cm` instead of W -- per column a binary search and R FMAs or loads
 // (cm_add); STAGE then stages the maps' tables where W would be.  A raw value a map refuses is reported as DKS_ERR_DOMAIN
 // with the instance index and contributes nothing.
 // MIX: the mixture head (up to DKS_MIX_MAX_R score rows; f(x) = sum_k pi_k h(z_k) from `mix`).  The other instantiations
-// hold eight rows and never read `mix`.
-template <bool STAGE, bool MAPS, bool MIX = false>
+// never read `mix`.
+// RB: the compile-time bound on R (1 or 8; MIX: DKS_MIX_MAX_R).  The loops over score rows unroll over RB, so the per-thread
+// contributions and scores live in registers rather than in a local-memory stack frame.
+template <bool STAGE, bool MAPS, bool MIX = false, int RB = MIX ? DKS_MIX_MAX_R : 8>
 __global__ void prep_kernel(const double* __restrict__ X, const double* __restrict__ W, const double* __restrict__ b,
                             const double* __restrict__ bg, const int32_t* __restrict__ goff,
                             const int32_t* __restrict__ gcols, const double* __restrict__ colmin,
@@ -297,7 +320,7 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
                             int* __restrict__ counts, int* __restrict__ idx_full, int* __restrict__ idx_other,
                             double* __restrict__ XT, double xt_scale, const double* __restrict__ xt_sub,
                             int* __restrict__ status, ColumnMapsDev cm, const MixHead* __restrict__ mix) {
-    constexpr int RMAX = MIX ? DKS_MIX_MAX_R : 8;
+    constexpr int CB = MIX ? 8 : (RB == 1 ? 2 : RB);    // outputs: C = 2 (binary head) or R; mixtures at most 8
     extern __shared__ __align__(16) unsigned char prep_smem[];
     double* sXW = reinterpret_cast<double*>(prep_smem);                        // [ipb][G][R]
     double* sX = sXW + (size_t)ipb * G * R;                                    // STAGE: [ipb][D]
@@ -308,41 +331,58 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
     int* sCols = sNan + (STAGE ? D : 0);                                       //        [D]
     int* sOff = sCols + (STAGE ? D : 0);                                       //        [G + 1]
     int* sHdr = sOff + (STAGE ? G + 1 : 0);                                    // MAPS:  [D][4]
-    unsigned char* sflag = reinterpret_cast<unsigned char*>(sHdr + (STAGE && MAPS ? 4 * D : 0));   // [ipb][G]
+    int* sCnt = sHdr + (STAGE && MAPS ? 4 * D : 0);     // the block's counts of the two lists, their bases, hist [G + 1]
+    int* sHist = sCnt + 4;
+    unsigned char* sflag = reinterpret_cast<unsigned char*>(sHist + G + 1);   // [ipb][G]
+    for (int idx = threadIdx.x; idx < G + 5; idx += blockDim.x) sCnt[idx] = 0;
+    if (threadIdx.x == 0) {      // what only the tail reads: into L2 now, so that its loads do not wait on DRAM there
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(b));
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(linkfnull));
+    }
     const int i0 = blockIdx.x * ipb;
     if (STAGE) {
+        // asynchronous copies (cp.async), all issued before any is waited on: the staging costs one DRAM round trip rather
+        // than one per table
+        auto cp8 = [](double* d, const double* s) { __pipeline_memcpy_async(d, s, sizeof(double)); };
+        auto cp4 = [](int* d, const int* s) { __pipeline_memcpy_async(d, s, sizeof(int)); };
         const int rows = min(ipb, n - i0);
         const double* Xb = X + (size_t)i0 * D;
-        for (int idx = threadIdx.x; idx < rows * D; idx += blockDim.x) sX[idx] = Xb[idx];
+        for (int idx = threadIdx.x; idx < rows * D; idx += blockDim.x) cp8(sX + idx, Xb + idx);
         if (MAPS) {
-            for (int idx = threadIdx.x; idx < cm.n_keys; idx += blockDim.x) sW[idx] = cm.keys[idx];
-            for (int idx = threadIdx.x; idx < cm.n_vals; idx += blockDim.x) sW[cm.n_keys + idx] = cm.vals[idx];
-            for (int idx = threadIdx.x; idx < 4 * D; idx += blockDim.x) sHdr[idx] = cm.hdr[idx];
+            for (int idx = threadIdx.x; idx < cm.n_keys; idx += blockDim.x) cp8(sW + idx, cm.keys + idx);
+            for (int idx = threadIdx.x; idx < cm.n_vals; idx += blockDim.x) cp8(sW + cm.n_keys + idx, cm.vals + idx);
+            for (int idx = threadIdx.x; idx < 4 * D; idx += blockDim.x) cp4(sHdr + idx, cm.hdr + idx);
         } else {
-            for (int idx = threadIdx.x; idx < R * D; idx += blockDim.x) sW[idx] = W[idx];
+            for (int idx = threadIdx.x; idx < R * D; idx += blockDim.x) cp8(sW + idx, W + idx);
         }
         for (int idx = threadIdx.x; idx < D; idx += blockDim.x) {
-            sMin[idx] = colmin[idx]; sMax[idx] = colmax[idx]; sNan[idx] = colnan[idx]; sCols[idx] = gcols[idx];
+            cp8(sMin + idx, colmin + idx); cp8(sMax + idx, colmax + idx);
+            cp4(sNan + idx, colnan + idx); cp4(sCols + idx, gcols + idx);
         }
-        for (int idx = threadIdx.x; idx <= G; idx += blockDim.x) sOff[idx] = goff[idx];
+        for (int idx = threadIdx.x; idx <= G; idx += blockDim.x) cp4(sOff + idx, goff + idx);
+        __pipeline_commit();
+        __pipeline_wait_prior(0);
         __syncthreads();
     }
     for (int idx = threadIdx.x; idx < ipb * G; idx += blockDim.x) {
         const int li = idx / G, g = idx - li * G, i = i0 + li;
         if (i >= n) continue;
         bool varies = false;
-        double acc[RMAX];
-        for (int r = 0; r < R; ++r) acc[r] = 0;
+        double acc[RB];
+#pragma unroll
+        for (int r = 0; r < RB; ++r) acc[r] = 0;
         const int c0 = STAGE ? sOff[g] : goff[g], c1 = STAGE ? sOff[g + 1] : goff[g + 1];
         for (int c = c0; c < c1; ++c) {
             const int col = STAGE ? sCols[c] : gcols[c];
             const double xv = STAGE ? sX[(size_t)li * D + col] : X[(size_t)i * D + col];
             if (MAPS) {
-                if (!cm_add(STAGE ? sHdr + 4 * col : cm.hdr + 4 * col, STAGE ? sW : cm.keys,
-                            STAGE ? sW + cm.n_keys : cm.vals, xv, R, acc))
+                if (!cm_add<RB>(STAGE ? sHdr + 4 * col : cm.hdr + 4 * col, STAGE ? sW : cm.keys,
+                                STAGE ? sW + cm.n_keys : cm.vals, xv, R, acc))
                     cm_report(status, i);
             } else {
-                for (int r = 0; r < R; ++r) acc[r] += xv * (STAGE ? sW[(size_t)r * D + col] : W[(size_t)r * D + col]);
+#pragma unroll
+                for (int r = 0; r < RB; ++r)
+                    if (r < R) acc[r] += xv * (STAGE ? sW[(size_t)r * D + col] : W[(size_t)r * D + col]);
             }
             if ((STAGE ? sNan[col] : colnan[col]) || isnan(xv)) {
                 if (!varies)
@@ -353,7 +393,9 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
                 varies = varies || !np_isclose(xv, mn) || !np_isclose(xv, mx);
             }
         }
-        for (int r = 0; r < R; ++r) {
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+            if (r >= R) continue;
             sXW[(size_t)idx * R + r] = acc[r];
             XW[((size_t)i * G + g) * R + r] = acc[r];
         }
@@ -382,33 +424,46 @@ __global__ void prep_kernel(const double* __restrict__ X, const double* __restri
             XT[(row * ntab + t) * 16 + x] = xt_scale * acc;
         }
     }
-    for (int li = threadIdx.x; li < ipb; li += blockDim.x) {
-        const int i = i0 + li;
-        if (i >= n) continue;
+    // the per-instance tail, one thread per instance (ipb <= blockDim.x)
+    const int li = threadIdx.x, i = i0 + li;
+    const bool mine = li < ipb && i < n;
+    int list = 0, rank = 0;
+    if (mine) {
         uint64_t m = 0;                       // varying bit-mask (groups 0..63; wider problems only use the count)
         int M = 0;
-        double z[RMAX], o[DKS_MAX_OUT];
-        for (int r = 0; r < R; ++r) z[r] = b[r];
+        double z[RB], o[CB];
+#pragma unroll
+        for (int r = 0; r < RB; ++r) z[r] = r < R ? b[r] : 0.0;
         for (int g = 0; g < G; ++g) {
             if (sflag[li * G + g]) { if (g < 64) m |= (1ull << g); ++M; }
-            for (int r = 0; r < R; ++r) z[r] += sXW[((size_t)li * G + g) * R + r];
+#pragma unroll
+            for (int r = 0; r < RB; ++r) if (r < R) z[r] += sXW[((size_t)li * G + g) * R + r];
         }
         vmask[i] = m;
         Mcnt[i] = M;
-        atomicAdd(&hist[M], 1);
-        // bucket: all groups vary (candidates for the shared-plan fast path) / everything else
-        if (M == G && M >= 2) idx_full[atomicAdd(&counts[0], 1)] = i;
-        else idx_other[atomicAdd(&counts[1], 1)] = i;
+        atomicAdd(&sHist[M], 1);
+        // list: all groups vary (candidates for the shared-plan fast path) / everything else
+        list = M == G && M >= 2 ? 0 : 1;
+        rank = atomicAdd(&sCnt[list], 1);
         if constexpr (MIX) mix_head_f64(z, *mix, o);
-        else head_f64(z, R, act, kappa, o);
-        for (int c = 0; c < C; ++c) dlink[(size_t)i * C + c] = link_f(o[c], link) - linkfnull[c];
+        else head_f64<RB>(z, R, act, kappa, o);
+#pragma unroll
+        for (int c = 0; c < CB; ++c)
+            if (c < C) dlink[(size_t)i * C + c] = link_f(o[c], link) - linkfnull[c];
         // exp head: f(x) = exp(z) overflows for z > 709.78; the explain kernels then never write this instance's phi
         if (act == DKS_ACT_EXP && !isfinite(o[0]) && atomicCAS(&status[0], 0, DKS_ERR_NUMERIC) == 0) status[1] = i;
     }
+    __syncthreads();
+    if (threadIdx.x < 2 && sCnt[threadIdx.x] > 0) sCnt[2 + threadIdx.x] = atomicAdd(&counts[threadIdx.x], sCnt[threadIdx.x]);
+    for (int t = threadIdx.x; t <= G; t += blockDim.x)
+        if (sHist[t] > 0) atomicAdd(&hist[t], sHist[t]);
+    __syncthreads();
+    if (mine) (list == 0 ? idx_full : idx_other)[sCnt[2 + list] + rank] = i;
 }
-// maps_doubles: the column maps' keys + values staged in place of W (0: the W path); their headers add 4 D ints
+// maps_doubles: the column maps' keys + values staged in place of W (0: the W path); their headers add 4 D ints.
+// Every layout ends with the block's list counters and histogram (G + 5 ints) and the flags.
 inline size_t prep_smem_bytes(bool stage, int ipb, int G, int R, int D, size_t maps_doubles = 0) {
-    size_t b = sizeof(double) * (size_t)ipb * G * R + (size_t)ipb * G + 16;
+    size_t b = sizeof(double) * (size_t)ipb * G * R + sizeof(int) * ((size_t)G + 5) + (size_t)ipb * G + 16;
     if (stage && maps_doubles)
         b += sizeof(double) * ((size_t)ipb * D + maps_doubles + 2 * (size_t)D) + sizeof(int) * (6 * (size_t)D + G + 1);
     else if (stage)
