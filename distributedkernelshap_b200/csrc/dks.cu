@@ -428,21 +428,41 @@ int sampler_config(const dks_ctx* ctx, bool wide_pi, SamplerConfig* sc) {
     return DKS_OK;
 }
 
-// tree ensembles: every instance on explain_tree_kernel (up to 64 groups, CUDA-core only), the instances whose M selects
-// through the general list's l1 route -- the kernel's moments, then l1_lars_kernel -- whatever their M, G included
-int choose_route_trees(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
+// a model family with its own explain kernel (tree ensembles, kernel machines): the kernel's DKS_GENERAL_* value, the
+// wording of its route's messages and its shared memory at S_cap coalition rows
+struct OwnKernel {
+    int general;
+    const char* family;      // "<family> run on the <kernel> only", "<family>: %d groups"
+    const char* kernel;
+    const char* bound;       // "... nsamples, outputs or <bound> too many"
+    size_t (*smem)(const dks_ctx* ctx, int S_cap);
+};
+
+OwnKernel own_kernel(const dks_ctx* ctx) {
+    if (ctx->head.trees)
+        return {DKS_GENERAL_TREES, "tree ensembles", "tree kernel", "trees", [](const dks_ctx* c, int S_cap) {
+                    return dks::trees::smem_bytes(S_cap, c->C, c->tree.R, c->tree.T); }};
+    return {DKS_GENERAL_KMACH, "kernel machines", "kernel-machine kernel", "groups", [](const dks_ctx* c, int S_cap) {
+                return dks::kmach::smem_bytes(S_cap, c->C, c->km.R, c->G, c->km.head == DKS_KM_HEAD_CALIBRATED); }};
+}
+
+// tree ensembles and kernel machines: every instance on the family's own kernel (up to 64 groups, CUDA-core only), the
+// instances whose M selects through the general list's l1 route -- the kernel's moments, then l1_lars_kernel -- whatever
+// their M, G included
+int choose_route_own(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
+    const OwnKernel ok = own_kernel(ctx);
     const int G = ctx->G, kernel = ctx->kernel_choice;
     if (kernel != DKS_KERNEL_AUTO && kernel != DKS_KERNEL_SIMT)
-        return fail(DKS_ERR_UNSUPPORTED, "tree ensembles run on the tree kernel only (kernel 'auto' or 'simt')");
-    if (G > 64) return fail(DKS_ERR_UNSUPPORTED, "tree ensembles: %d groups; the tree kernel covers at most 64", G);
+        return fail(DKS_ERR_UNSUPPORTED, "%s run on the %s only (kernel 'auto' or 'simt')", ok.family, ok.kernel);
+    if (G > 64) return fail(DKS_ERR_UNSUPPORTED, "%s: %d groups; the %s covers at most 64", ok.family, G, ok.kernel);
     rt->draw = ctx->plan_mode == 1 && ext_z == nullptr;
     if (rt->draw) TRY(sampler_config(ctx, false, &rt->sc));
     const bool per_inst = ext_z != nullptr || rt->draw;
     rt->S_cap = std::max(ext_z ? ext_stride : rt->draw ? rt->sc.stride : ctx->max_plan_S, 2);
-    rt->smem = dks::trees::smem_bytes(rt->S_cap, ctx->C, ctx->tree.R, ctx->tree.T);
+    rt->smem = ok.smem(ctx, rt->S_cap);
     if ((long long)rt->smem > (long long)ctx->max_smem_optin)
-        return fail(DKS_ERR_UNSUPPORTED, "tree kernel needs %zu B of shared memory (> %d): nsamples, outputs or trees too many",
-                    rt->smem, ctx->max_smem_optin);
+        return fail(DKS_ERR_UNSUPPORTED, "%s needs %zu B of shared memory (> %d): nsamples, outputs or %s too many", ok.kernel,
+                    rt->smem, ctx->max_smem_optin, ok.bound);
     if (ctx->l1_mode != 0) {
         if (per_inst) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
         for (int M = 2; M <= G; ++M) {
@@ -458,19 +478,110 @@ int choose_route_trees(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Rout
                         rt->l1_Mmax, rt->l1_Mmax);
         rt->l1_smem = rt->smem;
     }
-    rt->general = DKS_GENERAL_TREES;
+    rt->general = ok.general;
     return DKS_OK;
 }
 
-// the tree kernel over p.list (L1: its moments); its per-CTA node scratch is sized for the grid
-int launch_tree_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
+// the family's own kernel over p.list (L1: its moments); the tree kernel's per-CTA node scratch is sized for the grid
+int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
     const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
-    TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
-    auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, dks::trees::THREADS, smem, st>>>(p, l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{}, ctx->tree,
-                                                   ctx->tree_X, ctx->tree_D);
+    const dks::SimtL1 q = l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{};
+    if (ctx->head.trees) {
+        TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
+        auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->tree_X, ctx->tree_D);
+    } else {
+        auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->cur_X, ctx->d_bg, ctx->D, ctx->d_goff, ctx->d_gcols);
+    }
     ctx->launches += 1;
+    return DKS_OK;
+}
+
+// DKS_ERR_DOMAIN: "<prefix> %d <phrase>", the phrase naming what refuses a raw value -- a kernel machine, a tree's column
+// encoding or a linear model's column maps
+const char* refusal_phrase(bool kmach, bool encoding) {
+    if (kmach) return "holds NaN: kernel machines refuse it, as scikit-learn does";
+    return encoding ? "holds a raw value the column encoding refuses (NaN, or a category unseen at fit time, where the "
+                      "pipeline raises)"
+                    : "holds a raw value its column map refuses (NaN, or a category unseen at fit time, where the pipeline "
+                      "raises)";
+}
+// the row named by the status word, refused by the model's family
+int fail_refused(const dks_ctx* ctx, const char* prefix) {
+    return fail(DKS_ERR_DOMAIN, "%s %d %s", prefix, ctx->h_status[1], refusal_phrase(ctx->head.kmach, ctx->head.trees));
+}
+
+void free_column_maps(dks_ctx* ctx) {
+    int* hdr = const_cast<int*>(ctx->cm.hdr);
+    double* keys = const_cast<double*>(ctx->cm.keys);
+    double* vals = const_cast<double*>(ctx->cm.vals);
+    dev_free(&hdr); dev_free(&keys); dev_free(&vals);
+    ctx->cm = ColumnMapsDev{};
+}
+
+// the start of dks_fit for every family: the background, its weights, the linear model's W and b, the groups and the
+// column statistics stage 1 decides the varying groups with on the device; fnull's buffers; no column maps; status cleared
+int fit_begin(dks_ctx* ctx) {
+    const int N = ctx->N, D = ctx->D, G = ctx->G, R = ctx->R, C = ctx->C;
+    const cudaStream_t st = ctx->stream;
+    TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
+    TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
+    TRY(dev_alloc(&ctx->d_W, (size_t)R * D));
+    TRY(dev_alloc(&ctx->d_b, (size_t)R));
+    TRY(dev_alloc(&ctx->d_goff, (size_t)G + 1));
+    TRY(dev_alloc(&ctx->d_gcols, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colmin, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colmax, (size_t)D));
+    TRY(dev_alloc(&ctx->d_colnan, (size_t)D));
+    TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
+    TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
+    free_column_maps(ctx);
+    CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_W, ctx->h_W.data(), sizeof(double) * R * D, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_b, ctx->h_b.data(), sizeof(double) * R, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
+    // varying groups are decided on the raw columns (a tree behind a column encoding reads the encoded background)
+    dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
+    ctx->launches += 1;
+    return DKS_OK;
+}
+
+// once the fit kernels are queued: fnull, link(fnull) and the status word back to the host.  A background row the model
+// refuses is DKS_ERR_DOMAIN; a family with its own kernel (`family` not NULL) refuses a non-finite link(fnull).
+int fit_readback(dks_ctx* ctx, const char* family) {
+    const int C = ctx->C;
+    const cudaStream_t st = ctx->stream;
+    CUDA_TRY(cudaGetLastError());
+    ctx->h_fnull.resize(C);
+    ctx->h_linkfnull.resize(C);
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN) return fail_refused(ctx, "background row");
+    if (family != nullptr)
+        for (int c = 0; c < C; ++c)
+            if (!std::isfinite(ctx->h_linkfnull[c]))
+                return fail(DKS_ERR_NUMERIC, "%s: link(fnull) of output %d is not finite (fnull = %g): the background's "
+                            "mean prediction is 0 or 1 under the logit link, or overflows", family, c, ctx->h_fnull[c]);
+    return DKS_OK;
+}
+
+// the end of a successful dks_fit: workspace shapes depend on G, R and C, and the plans carry tables derived from the
+// background and model: drop them
+int fit_done(dks_ctx* ctx) {
+    ctx->cap_n = 0;
+    ctx->prepared = false;
+    for (const auto& allocs : ctx->plan_allocs)
+        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
+    ctx->fitted = true;
+    ctx->epoch++;
     return DKS_OK;
 }
 
@@ -522,24 +633,7 @@ int fit_trees(dks_ctx* ctx) {
         if (f >= width)
             return fail(DKS_ERR_UNSUPPORTED, "tree ensemble: a split reads column %d of %d %s", f, width,
                         E > 0 ? "encoded columns" : "columns");
-    TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
-    TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
-    TRY(dev_alloc(&ctx->d_W, (size_t)D));
-    TRY(dev_alloc(&ctx->d_b, (size_t)1));
-    TRY(dev_alloc(&ctx->d_goff, (size_t)G + 1));
-    TRY(dev_alloc(&ctx->d_gcols, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmin, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmax, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colnan, (size_t)D));
-    TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
-    TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
-    {
-        int* hdr = const_cast<int*>(ctx->cm.hdr);
-        double* keys = const_cast<double*>(ctx->cm.keys);
-        double* vals = const_cast<double*>(ctx->cm.vals);
-        dev_free(&hdr); dev_free(&keys); dev_free(&vals);
-        ctx->cm = ColumnMapsDev{};
-    }
+    TRY(fit_begin(ctx));
     std::vector<int32_t> colgrp(D, 0);
     for (int g = 0; g < G; ++g)
         for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
@@ -573,17 +667,8 @@ int fit_trees(dks_ctx* ctx) {
     t.bgdir = bgdir;
     double* pred = nullptr;
     TRY(dev_alloc(&pred, (size_t)N * C));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_W, ctx->h_W.data(), sizeof(double) * D, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_b, ctx->h_b.data(), sizeof(double), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
-    // varying groups are decided on the raw columns; the tree kernels read the encoded background
-    dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
     const double* tbg = ctx->d_bg;
     if (E > 0) {
-        CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
         TRY(launch_encode(ctx, ctx->d_bg, N, ctx->d_bg_enc));
         tbg = ctx->d_bg_enc;
     }
@@ -591,75 +676,11 @@ int fit_trees(dks_ctx* ctx) {
     dks::trees::tree_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(tbg, N, width, t, C, ctx->link, nullptr, pred, nullptr,
                                                                   nullptr);
     dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
-    ctx->launches += 4;
-    CUDA_TRY(cudaGetLastError());
-    ctx->h_fnull.resize(C);
-    ctx->h_linkfnull.resize(C);
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
-    if (E > 0) CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    ctx->launches += 3;
+    const int rc = fit_readback(ctx, "tree ensemble");
     cudaFree(pred);
-    if (E > 0 && ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return fail(DKS_ERR_DOMAIN, "background row %d holds a raw value the column encoding refuses (NaN, or a category "
-                    "unseen at fit time, where the pipeline raises)", ctx->h_status[1]);
-    for (int c = 0; c < C; ++c)
-        if (!std::isfinite(ctx->h_linkfnull[c]))
-            return fail(DKS_ERR_NUMERIC, "tree ensemble: link(fnull) of output %d is not finite (fnull = %g): the background's "
-                        "mean prediction is 0 or 1 under the logit link, or overflows", c, ctx->h_fnull[c]);
-    ctx->cap_n = 0;
-    ctx->prepared = false;
-    for (const auto& allocs : ctx->plan_allocs)
-        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
-    ctx->fitted = true;
-    ctx->epoch++;
-    return DKS_OK;
-}
-
-// kernel machines: every instance on explain_kmach_kernel (up to 64 groups, CUDA-core only), the instances whose M selects
-// through the general list's l1 route -- the kernel's moments, then l1_lars_kernel -- whatever their M, G included
-int choose_route_kmach(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
-    const int G = ctx->G, kernel = ctx->kernel_choice;
-    if (kernel != DKS_KERNEL_AUTO && kernel != DKS_KERNEL_SIMT)
-        return fail(DKS_ERR_UNSUPPORTED, "kernel machines run on the kernel-machine kernel only (kernel 'auto' or 'simt')");
-    if (G > 64)
-        return fail(DKS_ERR_UNSUPPORTED, "kernel machines: %d groups; the kernel-machine kernel covers at most 64", G);
-    rt->draw = ctx->plan_mode == 1 && ext_z == nullptr;
-    if (rt->draw) TRY(sampler_config(ctx, false, &rt->sc));
-    const bool per_inst = ext_z != nullptr || rt->draw;
-    rt->S_cap = std::max(ext_z ? ext_stride : rt->draw ? rt->sc.stride : ctx->max_plan_S, 2);
-    rt->smem = dks::kmach::smem_bytes(rt->S_cap, ctx->C, ctx->km.R, G, ctx->km.head == DKS_KM_HEAD_CALIBRATED);
-    if ((long long)rt->smem > (long long)ctx->max_smem_optin)
-        return fail(DKS_ERR_UNSUPPORTED, "kernel-machine kernel needs %zu B of shared memory (> %d): nsamples, outputs or "
-                    "groups too many", rt->smem, ctx->max_smem_optin);
-    if (ctx->l1_mode != 0) {
-        if (per_inst) return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection runs on shared plans only");
-        for (int M = 2; M <= G; ++M) {
-            if (!((ctx->l1_sel[0] >> (M - 1)) & 1ull)) continue;
-            if (ctx->h_l1[M].gram_raw == nullptr || ctx->h_l1[M].S != dks_effective_S(M, ctx->nsamples_req) ||
-                ctx->h_plans[M].z == nullptr || ctx->h_plans[M].S != ctx->h_l1[M].S)
-                return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection needs the shared plan of M=%d and its l1 tables "
-                            "(dks_set_l1_tables)", M);
-            rt->l1_Mmax = M;
-        }
-        if (rt->l1_Mmax > 0 && !lars_fits(ctx, rt->l1_Mmax))
-            return fail(DKS_ERR_UNSUPPORTED, "l1 feature selection: the %d x %d Cholesky factor does not fit shared memory",
-                        rt->l1_Mmax, rt->l1_Mmax);
-        rt->l1_smem = rt->smem;
-    }
-    rt->general = DKS_GENERAL_KMACH;
-    return DKS_OK;
-}
-
-// the kernel-machine kernel over p.list (L1: its moments)
-int launch_kmach_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
-    const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
-    auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{}, ctx->km,
-                                                   ctx->cur_X, ctx->d_bg, ctx->D, ctx->d_goff, ctx->d_gcols);
-    ctx->launches += 1;
-    return DKS_OK;
+    TRY(rc);
+    return fit_done(ctx);
 }
 
 void free_kmach(dks_ctx* ctx) {
@@ -672,27 +693,10 @@ void free_kmach(dks_ctx* ctx) {
 // dks_fit of a kernel machine: the arrays, T[j][v] of every background row and support vector, the column statistics stage 1
 // decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the kernel-machine kernels
 int fit_kmach(dks_ctx* ctx) {
-    const int N = ctx->N, D = ctx->D, G = ctx->G, C = ctx->C;
+    const int N = ctx->N, D = ctx->D, C = ctx->C;
     const cudaStream_t st = ctx->stream;
     KmDev& k = ctx->km;
-    TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
-    TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
-    TRY(dev_alloc(&ctx->d_W, (size_t)D));
-    TRY(dev_alloc(&ctx->d_b, (size_t)1));
-    TRY(dev_alloc(&ctx->d_goff, (size_t)G + 1));
-    TRY(dev_alloc(&ctx->d_gcols, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmin, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmax, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colnan, (size_t)D));
-    TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
-    TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
-    {
-        int* hdr = const_cast<int*>(ctx->cm.hdr);
-        double* keys = const_cast<double*>(ctx->cm.keys);
-        double* vals = const_cast<double*>(ctx->cm.vals);
-        dev_free(&hdr); dev_free(&keys); dev_free(&vals);
-        ctx->cm = ColumnMapsDev{};
-    }
+    TRY(fit_begin(ctx));
     free_kmach(ctx);
     TRY(upload_tree_array(&k.sv, ctx->h_ksv.data(), ctx->h_ksv.size(), st));
     TRY(upload_tree_array(&k.dual, ctx->h_kdual.data(), ctx->h_kdual.size(), st));
@@ -703,52 +707,22 @@ int fit_kmach(dks_ctx* ctx) {
     k.Tbg = Tbg;
     double* pred = nullptr;
     TRY(dev_alloc(&pred, (size_t)N * C));
-    CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_W, ctx->h_W.data(), sizeof(double) * D, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_b, ctx->h_b.data(), sizeof(double), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
-    dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
     dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(ctx->d_bg, N, D, k, Tbg);
     dks::kmach::km_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(ctx->d_bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
                                                                 ctx->d_status);
     dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
-    ctx->launches += 4;
-    CUDA_TRY(cudaGetLastError());
-    ctx->h_fnull.resize(C);
-    ctx->h_linkfnull.resize(C);
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    ctx->launches += 3;
+    const int rc = fit_readback(ctx, "kernel machine");
     cudaFree(pred);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return fail(DKS_ERR_DOMAIN, "background row %d holds NaN: kernel machines refuse it, as scikit-learn does",
-                    ctx->h_status[1]);
-    for (int c = 0; c < C; ++c)
-        if (!std::isfinite(ctx->h_linkfnull[c]))
-            return fail(DKS_ERR_NUMERIC, "kernel machine: link(fnull) of output %d is not finite (fnull = %g): the background's "
-                        "mean prediction is 0 or 1 under the logit link, or overflows", c, ctx->h_fnull[c]);
-    ctx->cap_n = 0;
-    ctx->prepared = false;
-    for (const auto& allocs : ctx->plan_allocs)
-        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
-    ctx->fitted = true;
-    ctx->epoch++;
-    return DKS_OK;
+    TRY(rc);
+    return fit_done(ctx);
 }
 
 int choose_route(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
     const HeadDesc& h = ctx->head;
-    if (h.trees) {
+    if (h.trees || h.kmach) {
         *rt = Route{};
-        return choose_route_trees(ctx, ext_z, ext_stride, rt);
-    }
-    if (h.kmach) {
-        *rt = Route{};
-        return choose_route_kmach(ctx, ext_z, ext_stride, rt);
+        return choose_route_own(ctx, ext_z, ext_stride, rt);
     }
     const int G = ctx->G, N = ctx->N, kernel = ctx->kernel_choice;
     const bool auto_or_shared = kernel == DKS_KERNEL_AUTO || kernel == DKS_KERNEL_SHARED;
@@ -1176,13 +1150,9 @@ int launch_general_l1(dks_ctx* ctx, const Route& rt, ExplainParams* p, double* p
     ExplainParams ps = *p;
     ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
     const bool timed = !ctx->capturing;
-    if (ctx->head.trees) {
+    if (ctx->head.trees || ctx->head.kmach) {
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
-        TRY(launch_tree_kernel(ctx, true, ps, rt.l1_smem, gstream));
-        ctx->launches += 1;
-    } else if (ctx->head.kmach) {
-        if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
-        TRY(launch_kmach_kernel(ctx, true, ps, rt.l1_smem, gstream));
+        TRY(launch_own_kernel(ctx, true, ps, rt.l1_smem, gstream));
         ctx->launches += 1;
     } else {
         const bool mixh = ctx->head.mixture();
@@ -1234,10 +1204,8 @@ int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t 
         TRY(dks::tc_launch(ctx, p, gstream));
         break;
     case DKS_GENERAL_TREES:
-        TRY(launch_tree_kernel(ctx, false, p, rt.smem, gstream));
-        break;
     case DKS_GENERAL_KMACH:
-        TRY(launch_kmach_kernel(ctx, false, p, rt.smem, gstream));
+        TRY(launch_own_kernel(ctx, false, p, rt.smem, gstream));
         break;
     default: {
         const bool mixh = ctx->head.mixture();
@@ -1329,15 +1297,7 @@ int check_status(dks_ctx* ctx) {
     if (ctx->h_status[0] == 0) return DKS_OK;
     if (ctx->h_status[0] == DKS_ERR_PLAN_MISSING)
         return fail(DKS_ERR_PLAN_MISSING, "no shared plan for M=%d at the current nsamples", ctx->h_status[1]);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.kmach)
-        return fail(DKS_ERR_DOMAIN, "instance %d holds NaN: kernel machines refuse it, as scikit-learn does",
-                    ctx->h_status[1]);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.trees)
-        return fail(DKS_ERR_DOMAIN, "instance %d holds a raw value the column encoding refuses (NaN, or a category unseen "
-                    "at fit time, where the pipeline raises)", ctx->h_status[1]);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return fail(DKS_ERR_DOMAIN, "instance %d holds a raw value its column map refuses (NaN, or a category unseen at "
-                    "fit time, where the pipeline raises)", ctx->h_status[1]);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN) return fail_refused(ctx, "instance");
     if (ctx->h_status[0] == DKS_ERR_NUMERIC)
         return fail(DKS_ERR_NUMERIC, "normal matrix not positive definite, or (exp head) a model output that is not finite "
                     "(instance/M %d)", ctx->h_status[1]);
@@ -1529,7 +1489,7 @@ int dks_destroy(dks_ctx* ctx) {
     free_encoding(ctx);
     dev_free(&ctx->d_Xenc);
     free_kmach(ctx);
-    if (ctx->cm.hdr) { cudaFree((void*)ctx->cm.hdr); cudaFree((void*)ctx->cm.keys); cudaFree((void*)ctx->cm.vals); }
+    free_column_maps(ctx);
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
     dev_free(&ctx->d_fnull); dev_free(&ctx->d_linkfnull); dev_free(&ctx->d_BWs); dev_free(&ctx->d_bases);
@@ -1913,8 +1873,7 @@ int dks_encode_host(dks_ctx* ctx, const double* X_host, int n, double* out_host)
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     cudaFree(dX); cudaFree(dO);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return fail(DKS_ERR_DOMAIN, "row %d holds a raw value the column encoding refuses (NaN, or a category unseen at fit "
-                    "time, where the pipeline raises)", ctx->h_status[1]);
+        return fail(DKS_ERR_DOMAIN, "row %d %s", ctx->h_status[1], refusal_phrase(false, true));
     return DKS_OK;
 }
 
@@ -1957,20 +1916,10 @@ int dks_fit(dks_ctx* ctx) {
         return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model is not a tree ensemble");
     if (h.trees) return fit_trees(ctx);
     if (h.kmach) return fit_kmach(ctx);
-    TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
-    TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
-    TRY(dev_alloc(&ctx->d_W, (size_t)R * D));
-    TRY(dev_alloc(&ctx->d_b, (size_t)R));
-    TRY(dev_alloc(&ctx->d_goff, (size_t)G + 1));
-    TRY(dev_alloc(&ctx->d_gcols, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmin, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmax, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colnan, (size_t)D));
+    TRY(fit_begin(ctx));
     TRY(dev_alloc(&ctx->d_BW, (size_t)N * G * R));
     TRY(dev_alloc(&ctx->d_scores, (size_t)N * R));
     TRY(dev_alloc(&ctx->d_Bbar, (size_t)G * R));
-    TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
-    TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
     TRY(dev_alloc(&ctx->d_BWs, (size_t)N * G * R));
     TRY(dev_alloc(&ctx->d_bases, (size_t)N * R));
     TRY(dev_alloc(&ctx->d_wbf, (size_t)N));
@@ -1979,37 +1928,24 @@ int dks_fit(dks_ctx* ctx) {
     cudaStream_t st = ctx->stream;
     CUDA_TRY(cudaMemcpyAsync(ctx->d_mix, &ctx->mix, sizeof(MixHead), cudaMemcpyHostToDevice, st));
     const bool maps = !ctx->h_cm_hdr.empty();
-    {
-        int* hdr = const_cast<int*>(ctx->cm.hdr);
-        double* keys = const_cast<double*>(ctx->cm.keys);
-        double* vals = const_cast<double*>(ctx->cm.vals);
-        dev_free(&hdr); dev_free(&keys); dev_free(&vals);
-        ctx->cm = ColumnMapsDev{};
-        if (maps) {
-            const size_t nk = ctx->h_cm_keys.size(), nv = ctx->h_cm_vals.size();
-            TRY(dev_alloc(&hdr, ctx->h_cm_hdr.size()));
-            TRY(dev_alloc(&keys, nk));
-            TRY(dev_alloc(&vals, nv));
-            CUDA_TRY(cudaMemcpy(hdr, ctx->h_cm_hdr.data(), sizeof(int) * ctx->h_cm_hdr.size(), cudaMemcpyHostToDevice));
-            if (nk) CUDA_TRY(cudaMemcpy(keys, ctx->h_cm_keys.data(), sizeof(double) * nk, cudaMemcpyHostToDevice));
-            CUDA_TRY(cudaMemcpy(vals, ctx->h_cm_vals.data(), sizeof(double) * nv, cudaMemcpyHostToDevice));
-            ctx->cm = ColumnMapsDev{hdr, keys, vals, (int)nk, (int)nv};
-        }
+    if (maps) {
+        const size_t nk = ctx->h_cm_keys.size(), nv = ctx->h_cm_vals.size();
+        int* hdr = nullptr;
+        double *keys = nullptr, *vals = nullptr;
+        TRY(dev_alloc(&hdr, ctx->h_cm_hdr.size()));
+        TRY(dev_alloc(&keys, nk));
+        TRY(dev_alloc(&vals, nv));
+        CUDA_TRY(cudaMemcpy(hdr, ctx->h_cm_hdr.data(), sizeof(int) * ctx->h_cm_hdr.size(), cudaMemcpyHostToDevice));
+        if (nk) CUDA_TRY(cudaMemcpy(keys, ctx->h_cm_keys.data(), sizeof(double) * nk, cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(vals, ctx->h_cm_vals.data(), sizeof(double) * nv, cudaMemcpyHostToDevice));
+        ctx->cm = ColumnMapsDev{hdr, keys, vals, (int)nk, (int)nv};
     }
-    CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
     {
         // the weighted shared-plan kernels read w'_j = N w_j: their sums then have the magnitude of the uniform ones
         std::vector<float> wn(N);
         for (int j = 0; j < N; ++j) wn[j] = (float)((double)N * ctx->h_wbg[j]);
         CUDA_TRY(cudaMemcpy(ctx->d_wn, wn.data(), sizeof(float) * N, cudaMemcpyHostToDevice));
     }
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_W, ctx->h_W.data(), sizeof(double) * R * D, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_b, ctx->h_b.data(), sizeof(double) * R, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_goff, ctx->h_goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_gcols, ctx->h_gcols.data(), sizeof(int32_t) * D, cudaMemcpyHostToDevice, st));
-
     (maps ? (R > 8 ? dks::fit_bw_kernel<true, true> : dks::fit_bw_kernel<true>) : dks::fit_bw_kernel<false>)<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(
         ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D, G, R, ctx->d_BW, ctx->cm, ctx->d_status);
     dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
@@ -2020,34 +1956,17 @@ int dks_fit(dks_ctx* ctx) {
                                                                                     ctx->mix.Rm, ctx->d_mixBW, ctx->d_mixsc);
         ctx->launches += 1;
     }
-    dks::fit_colstats_kernel<<<cdiv(D, 128), 128, 0, st>>>(ctx->d_bg, N, D, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan);
     dks::fit_fnull_kernel<<<1, 256, 0, st>>>(ctx->d_scores, ctx->d_BW, ctx->d_wbg, N, G, R, C, ctx->act, ctx->kappa,
                                               ctx->link, ctx->d_fnull, ctx->d_linkfnull, ctx->d_Bbar, ctx->d_mix);
     dks::fit_scale_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, G, R,
                                                                               h.scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf,
                                                                               h.expo ? 1 : 0);
-    ctx->launches += 5;
-    CUDA_TRY(cudaGetLastError());
-    ctx->h_fnull.resize(C);
-    ctx->h_linkfnull.resize(C);
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_fnull.data(), ctx->d_fnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_linkfnull.data(), ctx->d_linkfnull, sizeof(double) * C, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return fail(DKS_ERR_DOMAIN, "background row %d holds a raw value its column map refuses (NaN, or a category unseen "
-                    "at fit time, where the pipeline raises)", ctx->h_status[1]);
+    ctx->launches += 4;
+    TRY(fit_readback(ctx, nullptr));
     if (h.expo && !std::isfinite(ctx->h_fnull[0]))
         return fail(DKS_ERR_NUMERIC, "exp head: the background's predictions are not all finite in float64 (fnull = %g)",
                     ctx->h_fnull[0]);
-    ctx->cap_n = 0;  // workspace shapes depend on G, R, C
-    ctx->prepared = false;
-    // plans carry tables derived from the background/model: drop them
-    for (const auto& allocs : ctx->plan_allocs)
-        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
-    ctx->fitted = true;
-    ctx->epoch++;
-    return DKS_OK;
+    return fit_done(ctx);
 }
 
 int dks_num_outputs(dks_ctx* ctx, int* C) {
@@ -2098,14 +2017,7 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     cudaFree(dX); cudaFree(dO);
     if (dXe) cudaFree(dXe);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.kmach)
-        return fail(DKS_ERR_DOMAIN, "row %d holds NaN: kernel machines refuse it, as scikit-learn does", ctx->h_status[1]);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN && ctx->head.trees)
-        return fail(DKS_ERR_DOMAIN, "row %d holds a raw value the column encoding refuses (NaN, or a category unseen at fit "
-                    "time, where the pipeline raises)", ctx->h_status[1]);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return fail(DKS_ERR_DOMAIN, "row %d holds a raw value its column map refuses (NaN, or a category unseen at fit time, "
-                    "where the pipeline raises)", ctx->h_status[1]);
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN) return fail_refused(ctx, "row");
     return DKS_OK;
 }
 

@@ -566,6 +566,103 @@ __device__ inline void wls_solve_write(const double* Lf, double* rhs, int M, dou
     phi_row[vi[nA]] = sign * last;
 }
 
+// ---- the edges of the per-instance CUDA-core kernels (one CTA per instance): plan lookup, the varying positions and the
+// solve of the instance's outputs.  What the kernels compute between them is their own. ----
+__device__ __forceinline__ void report_status(int* status, int code, int detail) {
+    if (atomicCAS(&status[0], 0, code) == 0) status[1] = detail;
+}
+
+// instance i's phi rows of every output start at zero: only the varying groups are written
+__device__ __forceinline__ void zero_phi_rows(const ExplainParams& p, int i) {
+    const size_t slab = (size_t)p.n * p.G;
+    for (int idx = threadIdx.x; idx < p.C * p.G; idx += blockDim.x)
+        p.phi[(size_t)(idx / p.G) * slab + (size_t)i * p.G + idx % p.G] = 0.0;
+}
+
+// the coalition plan of instance i (M >= 2 varying groups)
+struct InstPlan {
+    const uint64_t* z;
+    const double* w;
+    const double* chol;   // its factored normal matrix, NULL if not factored
+    int S;
+};
+
+// caller or sampler rows (ext_*), else the shared plan of M.  Returns false, the instance skipped, when the shared plan is
+// missing (DKS_ERR_PLAN_MISSING, detail M) or S exceeds the kernel's staging (DKS_ERR_INVALID, detail i).
+__device__ __forceinline__ bool inst_plan(const ExplainParams& p, int i, int M, InstPlan& pl) {
+    pl.S = dks_effective_S(M, p.S_req);
+    pl.chol = nullptr;
+    if (p.ext_z != nullptr) {
+        pl.z = p.ext_z + (size_t)i * p.ext_stride;
+        pl.w = p.ext_w + (size_t)i * p.ext_stride;
+        if (p.ext_chol != nullptr) pl.chol = p.ext_chol + (size_t)i * p.ext_fstride;   // factored with the plan
+    } else {
+        const PlanDev pd = p.plans[M];
+        if (pd.z == nullptr || pd.S != pl.S) {
+            if (threadIdx.x == 0) report_status(p.status, DKS_ERR_PLAN_MISSING, M);
+            return false;
+        }
+        pl.z = pd.z; pl.w = pd.w; pl.chol = pd.chol;
+    }
+    if (pl.S > p.S_cap) {
+        if (threadIdx.x == 0) report_status(p.status, DKS_ERR_INVALID, i);
+        return false;
+    }
+    return true;
+}
+
+// vi[k] = group of varying position k (thread 0; the caller's barrier publishes it)
+__device__ __forceinline__ void varying_positions(uint64_t vm, int G, int* vi) {
+    if (threadIdx.x == 0) {
+        int k = 0;
+        for (int g = 0; g < G; ++g) if ((vm >> g) & 1ull) vi[k++] = g;
+    }
+}
+
+// the plan's Cholesky factor into A: copied, or built and factored by warp 0 (not positive definite: DKS_ERR_NUMERIC,
+// detail i).  No barrier after it: wls_build_rhs does not read A, and the solve follows a barrier.
+__device__ __forceinline__ void block_normal(const InstPlan& pl, int M, double* A, int i, int* status) {
+    const int tid = threadIdx.x;
+    if (pl.chol != nullptr) {
+        for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) A[idx] = pl.chol[idx];
+    } else {
+        wls_build_normal(pl.z, pl.w, pl.S, M, A, tid >> 5, blockDim.x >> 5);
+        __syncthreads();
+        if (tid < 32) {
+            const bool ok = wls_cholesky_warp(A, M - 1);
+            if (!ok && tid == 0) report_status(status, DKS_ERR_NUMERIC, i);
+        }
+    }
+}
+
+// two outputs: class 0 is the exact negation of class 1 (p0 = 1 - p1 row-wise); thread 0, after class 1's solve
+__device__ __forceinline__ void write_class0_negation(double* phi0, const double* phi1, int M, const int* vi) {
+    for (int k = 0; k < M; ++k) { const double v = phi1[vi[k]]; phi0[vi[k]] = (v == 0.0) ? 0.0 : -v; }
+}
+
+// one output: rhs from its y row, then thread 0 solves with the factor in A and writes phi_row
+__device__ __forceinline__ void block_solve_one(const InstPlan& pl, int M, const double* ys, double delta, const double* A,
+                                                double* rhs, const int* vi, double* phi_row) {
+    wls_build_rhs(pl.z, pl.w, ys, pl.S, M, delta, rhs, threadIdx.x >> 5, blockDim.x >> 5);
+    __syncthreads();
+    if (threadIdx.x == 0) wls_solve_write(A, rhs, M, delta, vi, phi_row, 1.0);
+}
+
+// every solved output of instance i: output u's y row at ys + u * ystride, solved for class c = u, or (neg: two outputs,
+// one solved) for class 1 with class 0 its negation.  A barrier before each output: the previous solve still reads rhs.
+__device__ __forceinline__ void block_solve(const ExplainParams& p, int i, const InstPlan& pl, int M, const double* ys,
+                                            size_t ystride, int nsolve, bool neg, const double* A, double* rhs,
+                                            const int* vi) {
+    const size_t slab = (size_t)p.n * p.G;
+    for (int u = 0; u < nsolve; ++u) {
+        const int c = neg ? 1 : u;
+        __syncthreads();
+        block_solve_one(pl, M, ys + (size_t)u * ystride, p.dlink[(size_t)i * p.C + c], A, rhs, vi,
+                        p.phi + (size_t)c * slab + (size_t)i * p.G);
+    }
+    if (neg && threadIdx.x == 0) write_class0_negation(p.phi + (size_t)i * p.G, p.phi + slab + (size_t)i * p.G, M, vi);
+}
+
 // Block-level: Cholesky factor and inverse of the nA x nA matrix in A (shared memory, row-major; A must be followed by
 // nA*nA doubles of scratch).  Needs blockDim.x >= max(32, nA).  Returns (in every thread) whether A was positive definite.
 __device__ inline bool wls_factor_invert(double* A, int nA, double* __restrict__ chol, double* __restrict__ ainv) {
@@ -848,6 +945,25 @@ struct SimtL1 {
     double* mom;             // [n][outputs][2G + 4]
 };
 
+// instead of the solve: the moments of y of nsolve outputs (output u's y row at ys + u * ystride) into moment rows
+// row0 + u (instance i's outputs are rows i * outputs ...).  The reduction scratch lives where the solve keeps its
+// normal matrix, A.
+template <bool SCALED>
+__device__ __forceinline__ void block_moments_all(const SimtL1& q, int G, const InstPlan& pl, int M, const double* ys,
+                                                  size_t ystride, int nsolve, size_t row0, double* A) {
+    const l1::Tables& t = q.tabs[M];
+    const size_t mstride = 2 * (size_t)G + 4;
+    for (int u = 0; u < nsolve; ++u)
+        l1::block_moments<1, SCALED>(ys + (size_t)u * ystride, pl.S, M, pl.z, pl.w, t.b, t.sqab, q.mom + (row0 + u) * mstride,
+                                     reinterpret_cast<long long (*)[32]>(A),
+                                     reinterpret_cast<double (*)[2]>(A + l1::MOM_THREADS));
+}
+
+// moment rows row0 .. row0 + nsolve - 1 of an instance that is not solved: NaN at entry 2M, which l1_lars_kernel skips
+__device__ __forceinline__ void moments_skip(const SimtL1& q, int G, int M, int nsolve, size_t row0) {
+    if ((int)threadIdx.x < nsolve) q.mom[(row0 + threadIdx.x) * (2 * (size_t)G + 4) + 2 * M] = NAN;
+}
+
 // exp head: ey(s) of one coalition row in float64, for the rows outside the fp32 range rule (DKS_EXP_T_LO / _HI):
 // exp(a + m + ln sum_j w_j e^(d_j - m)) with a = sum_{k in s} XW_i[k], d_j = score_j - sum_{k in s} BW[j][k] and m the
 // running maximum of d_j (one pass, the sum rescaled when m grows), zero-weight rows skipped.  Row bit k (k < M) is
@@ -894,10 +1010,6 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
     const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C;
     const size_t slab = (size_t)p.n * G;
-    // L1: the moments' reduction scratch lives where the WLS keeps its normal matrix
-    long long (*part)[32] = reinterpret_cast<long long (*)[32]>(sm.A);
-    double (*bound)[2] = reinterpret_cast<double (*)[2]>(sm.A + l1::MOM_THREADS);
-    const size_t mstride = 2 * (size_t)G + 4;
 
     const int ninst = dks_inst_count(p);
     for (int qi = blockIdx.x; qi < ninst; qi += gridDim.x) {
@@ -905,7 +1017,7 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
         const int M = p.Mcnt[i];
         const uint64_t vm = p.vmask[i];
         __syncthreads();  // previous instance done with shared memory
-        for (int idx = tid; idx < C * G; idx += blockDim.x) p.phi[(size_t)(idx / G) * slab + (size_t)i * G + idx % G] = 0.0;
+        zero_phi_rows(p, i);
         if (M == 0) continue;
         if (M == 1) {
             // (exp head: a non-finite f(x) was reported by prep_kernel and is not written)
@@ -915,31 +1027,11 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
             }
             continue;
         }
-        const int S = dks_effective_S(M, p.S_req);
-        const uint64_t* zp;
-        const double* wp;
-        const double* chol = nullptr;
-        if (p.ext_z != nullptr) {
-            zp = p.ext_z + (size_t)i * p.ext_stride;
-            wp = p.ext_w + (size_t)i * p.ext_stride;
-            if (p.ext_chol != nullptr) chol = p.ext_chol + (size_t)i * p.ext_fstride;   // factored with the plan
-        } else {
-            PlanDev pd = p.plans[M];
-            if (pd.z == nullptr || pd.S != S) {
-                if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_PLAN_MISSING) == 0) p.status[1] = M; }
-                continue;
-            }
-            zp = pd.z; wp = pd.w; chol = pd.chol;
-        }
-        if (S > p.S_cap) {
-            if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_INVALID) == 0) p.status[1] = i; }
-            continue;
-        }
-
-        if (tid == 0) {
-            int k = 0;
-            for (int g = 0; g < G; ++g) if ((vm >> g) & 1ull) sm.vi[k++] = g;
-        }
+        InstPlan pl;
+        if (!inst_plan(p, i, M, pl)) continue;
+        const int S = pl.S;
+        const uint64_t* zp = pl.z;
+        varying_positions(vm, G, sm.vi);
         __syncthreads();
 
         float* Bs = sm.Bs;
@@ -976,30 +1068,16 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
             }
             if (__syncthreads_or(bad)) {
                 // a non-finite ey (or f(x)) is reported, never solved: nothing of this instance reaches phi or the moments
-                if (tid == 0) {
-                    if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
-                    if constexpr (L1) q.mom[(size_t)i * mstride + 2 * M] = NAN;     // l1_lars_kernel skips the task
-                }
+                if (tid == 0) report_status(p.status, DKS_ERR_NUMERIC, i);
+                if constexpr (L1) moments_skip(q, G, M, 1, i);
                 continue;
             }
             if constexpr (L1) {
-                const l1::Tables& t = q.tabs[M];
-                l1::block_moments<1, true>(sm.ys, S, M, zp, wp, t.b, t.sqab, q.mom + (size_t)i * mstride, part, bound);
+                block_moments_all<true>(q, G, pl, M, sm.ys, 0, 1, i, sm.A);
                 continue;
             }
-            if (chol != nullptr) {
-                for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
-            } else {
-                wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
-                __syncthreads();
-                if (tid < 32) {
-                    bool ok = wls_cholesky_warp(sm.A, M - 1);
-                    if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
-                }
-            }
-            wls_build_rhs(zp, wp, sm.ys, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
-            __syncthreads();
-            if (tid == 0) wls_solve_write(sm.A, sm.rhs, M, delta, sm.vi, p.phi + (size_t)i * G, 1.0);
+            block_normal(pl, M, sm.A, i, p.status);
+            block_solve_one(pl, M, sm.ys, delta, sm.A, sm.rhs, sm.vi, p.phi + (size_t)i * G);
         } else if (p.act == DKS_ACT_BINARY_LOGISTIC) {
             // stage this instance's varying columns of the background table
             for (int idx = tid; idx < M * N; idx += blockDim.x) {
@@ -1034,33 +1112,14 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
             }
             __syncthreads();
             if constexpr (L1) {
-                const l1::Tables& t = q.tabs[M];
-                l1::block_moments<1, false>(sm.ys, S, M, zp, wp, t.b, t.sqab, q.mom + (size_t)i * mstride, part, bound);
+                block_moments_all<false>(q, G, pl, M, sm.ys, 0, 1, i, sm.A);
                 continue;
             }
 
             // WLS for output 1; output 0 is its exact negation (p0 = 1 - p1 row-wise)
-            const double* Lf;
-            if (chol != nullptr) {
-                for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
-            } else {
-                wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
-                __syncthreads();
-                if (tid < 32) {
-                    bool ok = wls_cholesky_warp(sm.A, M - 1);
-                    if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
-                }
-            }
-            Lf = sm.A;
-            const double delta = p.dlink[(size_t)i * C + 1];
-            wls_build_rhs(zp, wp, sm.ys, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
-            __syncthreads();
-            if (tid == 0) {
-                wls_solve_write(Lf, sm.rhs, M, delta, sm.vi, p.phi + slab + (size_t)i * G, 1.0);
-                double* phi0 = p.phi + (size_t)i * G;
-                const double* phi1 = p.phi + slab + (size_t)i * G;
-                for (int k = 0; k < M; ++k) { double v = phi1[sm.vi[k]]; phi0[sm.vi[k]] = (v == 0.0) ? 0.0 : -v; }
-            }
+            block_normal(pl, M, sm.A, i, p.status);
+            block_solve_one(pl, M, sm.ys, p.dlink[(size_t)i * C + 1], sm.A, sm.rhs, sm.vi, p.phi + slab + (size_t)i * G);
+            if (tid == 0) write_class0_negation(p.phi + (size_t)i * G, p.phi + slab + (size_t)i * G, M, sm.vi);
         } else if (softmax) {
             // ---- general softmax and one-vs-rest heads: R = C score rows, outputs softmax(scores) or the normalised
             // sigmoids of the scores; scale = log2(e) ----
@@ -1122,46 +1181,15 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
             }
             __syncthreads();
             if constexpr (L1) {
-                const l1::Tables& t = q.tabs[M];
-                for (int c = 0; c < C; ++c)
-                    l1::block_moments<1, true>(sm.ys + (size_t)c * p.S_cap, S, M, zp, wp, t.b, t.sqab,
-                                               q.mom + ((size_t)i * C + c) * mstride, part, bound);
+                block_moments_all<true>(q, G, pl, M, sm.ys, p.S_cap, C, (size_t)i * C, sm.A);
                 continue;
             }
-            if (chol != nullptr) {
-                for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
-            } else {
-                wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
-                __syncthreads();
-                if (tid < 32) {
-                    bool ok = wls_cholesky_warp(sm.A, M - 1);
-                    if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
-                }
-            }
-            for (int c = 0; c < C; ++c) {
-                __syncthreads();
-                const double delta = p.dlink[(size_t)i * C + c];
-                wls_build_rhs(zp, wp, sm.ys + (size_t)c * p.S_cap, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
-                __syncthreads();
-                if (tid == 0) wls_solve_write(sm.A, sm.rhs, M, delta, sm.vi, p.phi + (size_t)c * slab + (size_t)i * G, 1.0);
-            }
+            block_normal(pl, M, sm.A, i, p.status);
+            block_solve(p, i, pl, M, sm.ys, p.S_cap, C, false, sm.A, sm.rhs, sm.vi);
         } else if (p.act == DKS_ACT_IDENTITY) {
             // identity head: the background average commutes with the head, so
             // ey_r(s) = fnull_r + sum_k z_sk (XW_i[k][r] - Bbar[k][r])   -- float64 throughout
-            const double* Lf;
-            if constexpr (!L1) {
-                if (chol != nullptr) {
-                    for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
-                } else {
-                    wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
-                    __syncthreads();
-                    if (tid < 32) {
-                        bool ok = wls_cholesky_warp(sm.A, M - 1);
-                        if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
-                    }
-                }
-            }
-            Lf = sm.A;
+            if constexpr (!L1) block_normal(pl, M, sm.A, i, p.status);
             for (int r = 0; r < p.R; ++r) {
                 __syncthreads();
                 if (tid < M) {
@@ -1178,15 +1206,11 @@ __global__ void __launch_bounds__(256) explain_simt_kernel(ExplainParams p, Simt
                 }
                 __syncthreads();
                 if constexpr (L1) {
-                    const l1::Tables& t = q.tabs[M];
-                    l1::block_moments<1, true>(sm.ys, S, M, zp, wp, t.b, t.sqab, q.mom + ((size_t)i * C + r) * mstride,
-                                               part, bound);
+                    block_moments_all<true>(q, G, pl, M, sm.ys, 0, 1, (size_t)i * C + r, sm.A);
                     continue;
                 }
-                const double delta = p.dlink[(size_t)i * C + r];
-                wls_build_rhs(zp, wp, sm.ys, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
-                __syncthreads();
-                if (tid == 0) wls_solve_write(Lf, sm.rhs, M, delta, sm.vi, p.phi + (size_t)r * slab + (size_t)i * G, 1.0);
+                block_solve_one(pl, M, sm.ys, p.dlink[(size_t)i * C + r], sm.A, sm.rhs, sm.vi,
+                                p.phi + (size_t)r * slab + (size_t)i * G);
             }
         }
     }

@@ -143,7 +143,7 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
                                                                 int D, const int* __restrict__ goff,
                                                                 const int* __restrict__ gcols) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C, R = k.R;
     const bool cal = k.head == DKS_KM_HEAD_CALIBRATED;
     double* acc = reinterpret_cast<double*>(smem_raw);          // [C][S_cap]
@@ -157,9 +157,7 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
     double* dl = du + TILE * R;                                 // [G][TILE]
     double* tb = dl + (size_t)G * TILE;                         // [ceil(G/4)][TILE][16]
     int* vi = reinterpret_cast<int*>(region + (tab > solve ? tab : solve));   // [64]
-    long long (*part)[32] = reinterpret_cast<long long (*)[32]>(A);
-    double (*bound)[2] = reinterpret_cast<double (*)[2]>(A + l1::MOM_THREADS);
-    const size_t slab = (size_t)p.n * G, mstride = 2 * (size_t)G + 4;
+    const size_t slab = (size_t)p.n * G;
     const int nsolve = cal ? 1 : C;                             // calibrated: class 0 is the negation of class 1
 
     const int ninst = dks_inst_count(p);
@@ -168,7 +166,7 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
         const int M = p.Mcnt[i];
         const uint64_t vm = p.vmask[i];
         __syncthreads();  // previous instance done with shared memory
-        for (int idx = tid; idx < C * G; idx += blockDim.x) p.phi[(size_t)(idx / G) * slab + (size_t)i * G + idx % G] = 0.0;
+        zero_phi_rows(p, i);
         bool fx_bad = false;                                    // stage 1 reported a NaN row or a non-finite link(f(x))
         for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
@@ -181,34 +179,15 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
             }
             continue;
         }
-        const int S = dks_effective_S(M, p.S_req);
-        const uint64_t* zp;
-        const double* wp;
-        const double* chol = nullptr;
-        if (p.ext_z != nullptr) {
-            zp = p.ext_z + (size_t)i * p.ext_stride;
-            wp = p.ext_w + (size_t)i * p.ext_stride;
-            if (p.ext_chol != nullptr) chol = p.ext_chol + (size_t)i * p.ext_fstride;
-        } else {
-            PlanDev pd = p.plans[M];
-            if (pd.z == nullptr || pd.S != S) {
-                if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_PLAN_MISSING) == 0) p.status[1] = M; }
-                continue;
-            }
-            zp = pd.z; wp = pd.w; chol = pd.chol;
-        }
-        if (S > p.S_cap) {
-            if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_INVALID) == 0) p.status[1] = i; }
-            continue;
-        }
+        InstPlan pl;
+        if (!inst_plan(p, i, M, pl)) continue;
         if (fx_bad) {
-            if (L1 && tid < nsolve) q.mom[((size_t)i * nsolve + tid) * mstride + 2 * M] = NAN;
+            if (L1) moments_skip(q, G, M, nsolve, (size_t)i * nsolve);
             continue;
         }
-        if (tid == 0) {
-            int c = 0;
-            for (int g = 0; g < G; ++g) if ((vm >> g) & 1ull) vi[c++] = g;
-        }
+        const int S = pl.S;
+        const uint64_t* zp = pl.z;
+        varying_positions(vm, G, vi);
         for (int idx = tid; idx < C * S; idx += blockDim.x) acc[(size_t)(idx / S) * p.S_cap + idx % S] = 0.0;
         if (cal) for (int s = tid; s < S; s += blockDim.x) fsc[s] = 0.0;
         __syncthreads();
@@ -306,40 +285,16 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
             for (int u = 0; u < nsolve; ++u) acc[(size_t)u * p.S_cap + s] = y[u];
         }
         if (__syncthreads_or(bad)) {
-            if (tid == 0 && atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
-            if (L1 && tid < nsolve) q.mom[((size_t)i * nsolve + tid) * mstride + 2 * M] = NAN;
+            if (tid == 0) report_status(p.status, DKS_ERR_NUMERIC, i);
+            if (L1) moments_skip(q, G, M, nsolve, (size_t)i * nsolve);
             continue;
         }
         if constexpr (L1) {
-            const l1::Tables& tbl = q.tabs[M];
-            for (int u = 0; u < nsolve; ++u)
-                l1::block_moments<1, true>(acc + (size_t)u * p.S_cap, S, M, zp, wp, tbl.b, tbl.sqab,
-                                           q.mom + ((size_t)i * nsolve + u) * mstride, part, bound);
+            block_moments_all<true>(q, G, pl, M, acc, p.S_cap, nsolve, (size_t)i * nsolve, A);
             continue;
         }
-        if (chol != nullptr) {
-            for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) A[idx] = chol[idx];
-        } else {
-            wls_build_normal(zp, wp, S, M, A, warp, blockDim.x >> 5);
-            __syncthreads();
-            if (tid < 32) {
-                const bool ok = wls_cholesky_warp(A, M - 1);
-                if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
-            }
-        }
-        for (int u = 0; u < nsolve; ++u) {
-            const int c = cal ? 1 : u;
-            __syncthreads();
-            const double delta = p.dlink[(size_t)i * C + c];
-            wls_build_rhs(zp, wp, acc + (size_t)u * p.S_cap, S, M, delta, rhs, warp, blockDim.x >> 5);
-            __syncthreads();
-            if (tid == 0) wls_solve_write(A, rhs, M, delta, vi, p.phi + (size_t)c * slab + (size_t)i * G, 1.0);
-        }
-        if (cal && tid == 0) {
-            double* phi0 = p.phi + (size_t)i * G;
-            const double* phi1 = p.phi + slab + (size_t)i * G;
-            for (int e = 0; e < M; ++e) { const double v = phi1[vi[e]]; phi0[vi[e]] = (v == 0.0) ? 0.0 : -v; }
-        }
+        block_normal(pl, M, A, i, p.status);
+        block_solve(p, i, pl, M, acc, p.S_cap, nsolve, cal, A, rhs, vi);
     }
 }
 

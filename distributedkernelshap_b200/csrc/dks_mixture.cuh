@@ -57,9 +57,6 @@ __global__ void __launch_bounds__(256, L1 ? 1 : 2) explain_simt_mix_kernel(Expla
     const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C;
     const size_t slab = (size_t)p.n * G;
-    long long (*part)[32] = reinterpret_cast<long long (*)[32]>(sm.A);
-    double (*bound)[2] = reinterpret_cast<double (*)[2]>(sm.A + l1::MOM_THREADS);
-    const size_t mstride = 2 * (size_t)G + 4;
 
     const int ninst = dks_inst_count(p);
     for (int qi = blockIdx.x; qi < ninst; qi += gridDim.x) {
@@ -67,7 +64,7 @@ __global__ void __launch_bounds__(256, L1 ? 1 : 2) explain_simt_mix_kernel(Expla
         const int M = p.Mcnt[i];
         const uint64_t vm = p.vmask[i];
         __syncthreads();  // previous instance done with shared memory
-        for (int idx = tid; idx < C * G; idx += blockDim.x) p.phi[(size_t)(idx / G) * slab + (size_t)i * G + idx % G] = 0.0;
+        zero_phi_rows(p, i);
         if (M == 0) continue;
         if (M == 1) {
             if (tid < C) {
@@ -76,30 +73,11 @@ __global__ void __launch_bounds__(256, L1 ? 1 : 2) explain_simt_mix_kernel(Expla
             }
             continue;
         }
-        const int S = dks_effective_S(M, p.S_req);
-        const uint64_t* zp;
-        const double* wp;
-        const double* chol = nullptr;
-        if (p.ext_z != nullptr) {
-            zp = p.ext_z + (size_t)i * p.ext_stride;
-            wp = p.ext_w + (size_t)i * p.ext_stride;
-            if (p.ext_chol != nullptr) chol = p.ext_chol + (size_t)i * p.ext_fstride;
-        } else {
-            PlanDev pd = p.plans[M];
-            if (pd.z == nullptr || pd.S != S) {
-                if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_PLAN_MISSING) == 0) p.status[1] = M; }
-                continue;
-            }
-            zp = pd.z; wp = pd.w; chol = pd.chol;
-        }
-        if (S > p.S_cap) {
-            if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_INVALID) == 0) p.status[1] = i; }
-            continue;
-        }
-        if (tid == 0) {
-            int k = 0;
-            for (int g = 0; g < G; ++g) if ((vm >> g) & 1ull) sm.vi[k++] = g;
-        }
+        InstPlan pl;
+        if (!inst_plan(p, i, M, pl)) continue;
+        const int S = pl.S;
+        const uint64_t* zp = pl.z;
+        varying_positions(vm, G, sm.vi);
         __syncthreads();
 
         float* Bs = sm.Bs;                              // [R][M][N] scaled background contributions of the varying groups
@@ -178,39 +156,20 @@ __global__ void __launch_bounds__(256, L1 ? 1 : 2) explain_simt_mix_kernel(Expla
         __syncthreads();
         const int nsolve = binary ? 1 : C;             // binary members: class 0 is the negation of class 1
         if constexpr (L1) {
-            const l1::Tables& t = q.tabs[M];
-            if (binary) {
-                l1::block_moments<1, false>(sm.ys, S, M, zp, wp, t.b, t.sqab, q.mom + (size_t)i * mstride, part, bound);
-            } else {
-                for (int c = 0; c < C; ++c)
-                    l1::block_moments<1, true>(sm.ys + (size_t)c * p.S_cap, S, M, zp, wp, t.b, t.sqab,
-                                               q.mom + ((size_t)i * C + c) * mstride, part, bound);
-            }
+            if (binary) block_moments_all<false>(q, G, pl, M, sm.ys, p.S_cap, 1, i, sm.A);
+            else block_moments_all<true>(q, G, pl, M, sm.ys, p.S_cap, C, (size_t)i * C, sm.A);
             continue;
         }
-        if (chol != nullptr) {
-            for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) sm.A[idx] = chol[idx];
-        } else {
-            wls_build_normal(zp, wp, S, M, sm.A, threadIdx.x >> 5, blockDim.x >> 5);
-            __syncthreads();
-            if (tid < 32) {
-                bool ok = wls_cholesky_warp(sm.A, M - 1);
-                if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
-            }
-        }
+        block_normal(pl, M, sm.A, i, p.status);
         for (int u = 0; u < nsolve; ++u) {
             const int c = binary ? 1 : u;
             __syncthreads();
             const double delta = p.dlink[(size_t)i * C + c];
-            wls_build_rhs(zp, wp, sm.ys + (size_t)u * p.S_cap, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
+            wls_build_rhs(pl.z, pl.w, sm.ys + (size_t)u * p.S_cap, S, M, delta, sm.rhs, threadIdx.x >> 5, blockDim.x >> 5);
             __syncthreads();
             if (tid == 0) wls_solve_write(sm.A, sm.rhs, M, delta, sm.vi, p.phi + (size_t)c * slab + (size_t)i * G, 1.0);
         }
-        if (binary && tid == 0) {
-            double* phi0 = p.phi + (size_t)i * G;
-            const double* phi1 = p.phi + slab + (size_t)i * G;
-            for (int k = 0; k < M; ++k) { double v = phi1[sm.vi[k]]; phi0[sm.vi[k]] = (v == 0.0) ? 0.0 : -v; }
-        }
+        if (binary && tid == 0) write_class0_negation(p.phi + (size_t)i * G, p.phi + slab + (size_t)i * G, M, sm.vi);
     }
 }
 

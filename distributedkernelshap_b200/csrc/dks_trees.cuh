@@ -128,9 +128,7 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
     int* dlist = reinterpret_cast<int*>(cj + 8);                // [T]
     int* wcnt = dlist + T;                                      // [8]
     int* vi = wcnt + 8;                                         // [64]
-    long long (*part)[32] = reinterpret_cast<long long (*)[32]>(A);
-    double (*bound)[2] = reinterpret_cast<double (*)[2]>(A + l1::MOM_THREADS);
-    const size_t slab = (size_t)p.n * G, mstride = 2 * (size_t)G + 4;
+    const size_t slab = (size_t)p.n * G;
     const int nsolve = C == 2 ? 1 : C;                          // two outputs: class 0 is the negation of class 1
     unsigned char* xi = t.xinfo + (size_t)blockIdx.x * nodes;
 
@@ -140,7 +138,7 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
         const int M = p.Mcnt[i];
         const uint64_t vm = p.vmask[i];
         __syncthreads();  // previous instance done with shared memory and xi
-        for (int idx = tid; idx < C * G; idx += blockDim.x) p.phi[(size_t)(idx / G) * slab + (size_t)i * G + idx % G] = 0.0;
+        zero_phi_rows(p, i);
         bool fx_bad = false;                                    // stage 1 reported a non-finite link(f(x))
         for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
@@ -153,34 +151,15 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
             }
             continue;
         }
-        const int S = dks_effective_S(M, p.S_req);
-        const uint64_t* zp;
-        const double* wp;
-        const double* chol = nullptr;
-        if (p.ext_z != nullptr) {
-            zp = p.ext_z + (size_t)i * p.ext_stride;
-            wp = p.ext_w + (size_t)i * p.ext_stride;
-            if (p.ext_chol != nullptr) chol = p.ext_chol + (size_t)i * p.ext_fstride;
-        } else {
-            PlanDev pd = p.plans[M];
-            if (pd.z == nullptr || pd.S != S) {
-                if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_PLAN_MISSING) == 0) p.status[1] = M; }
-                continue;
-            }
-            zp = pd.z; wp = pd.w; chol = pd.chol;
-        }
-        if (S > p.S_cap) {
-            if (tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_INVALID) == 0) p.status[1] = i; }
-            continue;
-        }
+        InstPlan pl;
+        if (!inst_plan(p, i, M, pl)) continue;
         if (fx_bad) {
-            if (L1 && tid < nsolve) q.mom[((size_t)i * nsolve + tid) * mstride + 2 * M] = NAN;
+            if (L1) moments_skip(q, G, M, nsolve, (size_t)i * nsolve);
             continue;
         }
-        if (tid == 0) {
-            int k = 0;
-            for (int g = 0; g < G; ++g) if ((vm >> g) & 1ull) vi[k++] = g;
-        }
+        const int S = pl.S;
+        const uint64_t* zp = pl.z;
+        varying_positions(vm, G, vi);
         // x's way at every internal node and the coalition bit of its group (NO_POS: the group does not vary)
         for (int nd = tid; nd < nodes; nd += blockDim.x) {
             const int f = t.feat[nd];
@@ -273,40 +252,22 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
             for (int u = 0; u < nsolve; ++u) acc[(size_t)u * p.S_cap + s] = y[u];
         }
         if (__syncthreads_or(bad)) {
-            if (tid == 0 && atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i;
-            if (L1 && tid < nsolve) q.mom[((size_t)i * nsolve + tid) * mstride + 2 * M] = NAN;
+            if (tid == 0) report_status(p.status, DKS_ERR_NUMERIC, i);
+            if (L1) moments_skip(q, G, M, nsolve, (size_t)i * nsolve);
             continue;
         }
         if constexpr (L1) {
-            const l1::Tables& tb = q.tabs[M];
-            for (int u = 0; u < nsolve; ++u)
-                l1::block_moments<1, true>(acc + (size_t)u * p.S_cap, S, M, zp, wp, tb.b, tb.sqab,
-                                           q.mom + ((size_t)i * nsolve + u) * mstride, part, bound);
+            block_moments_all<true>(q, G, pl, M, acc, p.S_cap, nsolve, (size_t)i * nsolve, A);
             continue;
         }
-        if (chol != nullptr) {
-            for (int idx = tid; idx < (M - 1) * (M - 1); idx += blockDim.x) A[idx] = chol[idx];
-        } else {
-            wls_build_normal(zp, wp, S, M, A, warp, blockDim.x >> 5);
-            __syncthreads();
-            if (tid < 32) {
-                const bool ok = wls_cholesky_warp(A, M - 1);
-                if (!ok && tid == 0) { if (atomicCAS(&p.status[0], 0, DKS_ERR_NUMERIC) == 0) p.status[1] = i; }
-            }
-        }
+        block_normal(pl, M, A, i, p.status);
         for (int u = 0; u < nsolve; ++u) {
             const int c = C == 2 ? 1 : u;
             __syncthreads();
-            const double delta = p.dlink[(size_t)i * C + c];
-            wls_build_rhs(zp, wp, acc + (size_t)u * p.S_cap, S, M, delta, rhs, warp, blockDim.x >> 5);
-            __syncthreads();
-            if (tid == 0) wls_solve_write(A, rhs, M, delta, vi, p.phi + (size_t)c * slab + (size_t)i * G, 1.0);
+            block_solve_one(pl, M, acc + (size_t)u * p.S_cap, p.dlink[(size_t)i * C + c], A, rhs, vi,
+                            p.phi + (size_t)c * slab + (size_t)i * G);
         }
-        if (C == 2 && tid == 0) {
-            double* phi0 = p.phi + (size_t)i * G;
-            const double* phi1 = p.phi + slab + (size_t)i * G;
-            for (int k = 0; k < M; ++k) { const double v = phi1[vi[k]]; phi0[vi[k]] = (v == 0.0) ? 0.0 : -v; }
-        }
+        if (C == 2 && tid == 0) write_class0_negation(p.phi + (size_t)i * G, p.phi + slab + (size_t)i * G, M, vi);
     }
 }
 
