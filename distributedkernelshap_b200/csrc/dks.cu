@@ -19,6 +19,7 @@
 #include "dks_trees.cuh"
 #include "dks_encode.cuh"
 #include "dks_kmach.cuh"
+#include "dks_mlp.cuh"
 
 namespace {
 
@@ -194,8 +195,12 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         // its negation)
         h.kmach = true; h.l1_binary = ctx->km.head == DKS_KM_HEAD_CALIBRATED;
         break;
+    case DKS_ACT_MLP:
+        // no shared-plan route: every instance runs the MLP kernels; the sigmoid head solves class 1 (class 0 its negation)
+        h.mlp = true; h.l1_binary = ctx->mlp.head == DKS_MLP_HEAD_SIGMOID;
+        break;
     }
-    if (h.shared != HEAD_SHARED_BINARY && !h.trees && !h.kmach) h.shared_max_G = 128;
+    if (h.shared != HEAD_SHARED_BINARY && !h.trees && !h.kmach && !h.mlp) h.shared_max_G = 128;
     if (!h.mixture()) h.xt_scale = h.scale;
     h.l1_nout = h.l1_binary ? 1 : ctx->C;
     return h;
@@ -210,6 +215,9 @@ int launch_encode(dks_ctx* ctx, const double* X_dev, int n, double* out) {
     CUDA_TRY(cudaGetLastError());
     return DKS_OK;
 }
+
+// CTAs of mlp_predict_kernel over n rows (one row per CTA, grid-stride)
+int mlp_predict_grid(const dks_ctx* ctx, int n) { return std::max(1, std::min(n, ctx->sm_count * 8)); }
 
 // stage 1's instantiation for R score rows: the compile-time bound 1 or 8 (a mixture: DKS_MIX_MAX_R)
 template <bool STAGE, bool MAPS>
@@ -232,8 +240,8 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const size_t maps_doubles = maps ? (size_t)ctx->cm.n_keys + ctx->cm.n_vals : 0;
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D, maps_doubles) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D, maps_doubles);
-    // the score rows stage 1 computes: one for trees and kernel machines (the scores of a zero linear model, unused)
-    const int R = h.trees || h.kmach ? 1 : ctx->R;
+    // the score rows stage 1 computes: one for trees, kernel machines and MLPs (the scores of a zero linear model, unused)
+    const int R = h.trees || h.kmach || h.mlp ? 1 : ctx->R;
     auto kern = stage ? (maps ? prep_kernel_for<true, true>(h.mixture(), R) : prep_kernel_for<true, false>(h.mixture(), R))
                       : (maps ? prep_kernel_for<false, true>(h.mixture(), R) : prep_kernel_for<false, false>(h.mixture(), R));
     // nibble tables for the shared-plan route: the binary head's at any G, the other heads' up to 128 groups (what their
@@ -249,8 +257,8 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
         ctx->tree_X = ctx->d_Xenc;
         ctx->tree_D = ctx->enc.E;
     }
-    if (h.trees || h.kmach) {
-        // tree ensembles and kernel machines: prep_kernel decides the varying groups (its scores are those of a zero linear
+    if (h.trees || h.kmach || h.mlp) {
+        // tree ensembles, kernel machines and MLPs: prep_kernel decides the varying groups (its scores are those of a zero linear
         // model, one identity output, and unused); the model's predict kernel then writes f(x) and link(f(x)) - link(fnull)
         // of every output
         kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
@@ -262,6 +270,9 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
             dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->km, ctx->C, ctx->link,
                                                                                  ctx->d_linkfnull, nullptr, ctx->d_dlink,
                                                                                  ctx->d_status);
+        else if (h.mlp)
+            dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
+                X_dev, n, ctx->D, ctx->mlp, ctx->C, ctx->link, ctx->d_linkfnull, nullptr, ctx->d_dlink, ctx->d_status);
         else
             dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->tree_X, n, ctx->tree_D, ctx->tree,
                                                                                    ctx->C, ctx->link, ctx->d_linkfnull,
@@ -438,10 +449,20 @@ struct OwnKernel {
     size_t (*smem)(const dks_ctx* ctx, int S_cap);
 };
 
+// warps of explain_mlp_kernel that evaluate coalitions at S_cap rows: as many (up to 8) as shared memory holds, at least 1
+int mlp_warps(const dks_ctx* ctx, int S_cap) {
+    int nw = dks::mlp::WARPS;
+    while (nw > 1 && dks::mlp::smem_bytes(S_cap, ctx->C, ctx->G, ctx->mlp, nw) > (size_t)ctx->max_smem_optin) --nw;
+    return nw;
+}
+
 OwnKernel own_kernel(const dks_ctx* ctx) {
     if (ctx->head.trees)
         return {DKS_GENERAL_TREES, "tree ensembles", "tree kernel", "trees", [](const dks_ctx* c, int S_cap) {
                     return dks::trees::smem_bytes(S_cap, c->C, c->tree.R, c->tree.T); }};
+    if (ctx->head.mlp)
+        return {DKS_GENERAL_MLP, "MLPs", "MLP kernel", "hidden units", [](const dks_ctx* c, int S_cap) {
+                    return dks::mlp::smem_bytes(S_cap, c->C, c->G, c->mlp, mlp_warps(c, S_cap)); }};
     return {DKS_GENERAL_KMACH, "kernel machines", "kernel-machine kernel", "groups", [](const dks_ctx* c, int S_cap) {
                 return dks::kmach::smem_bytes(S_cap, c->C, c->km.R, c->G, c->km.head == DKS_KM_HEAD_CALIBRATED); }};
 }
@@ -491,6 +512,11 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->tree_X, ctx->tree_D);
+    } else if (ctx->head.mlp) {
+        auto kern = l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->cur_X, ctx->d_bg, ctx->D,
+                                                    ctx->d_goff, ctx->d_gcols);
     } else {
         auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -511,6 +537,9 @@ const char* refusal_phrase(bool kmach, bool encoding) {
 }
 // the row named by the status word, refused by the model's family
 int fail_refused(const dks_ctx* ctx, const char* prefix) {
+    if (ctx->head.mlp)
+        return fail(DKS_ERR_DOMAIN, "%s %d holds NaN or an infinity: MLPs refuse it, as scikit-learn does", prefix,
+                    ctx->h_status[1]);
     return fail(DKS_ERR_DOMAIN, "%s %d %s", prefix, ctx->h_status[1], refusal_phrase(ctx->head.kmach, ctx->head.trees));
 }
 
@@ -718,9 +747,44 @@ int fit_kmach(dks_ctx* ctx) {
     return fit_done(ctx);
 }
 
+void free_mlp(dks_ctx* ctx) {
+    MlpDev& m = ctx->mlp;
+    for (const void* q : {(const void*)m.W, (const void*)m.b, (const void*)m.Wf, (const void*)m.bp, (const void*)m.Bbg})
+        if (q) cudaFree((void*)q);
+    m.W = nullptr; m.b = nullptr; m.Wf = nullptr; m.bp = nullptr; m.Bbg = nullptr;
+}
+
+// dks_fit of an MLP: the layers, B[j] = b_0 + bg_j W_0 of every background row, the column statistics stage 1 decides the
+// varying groups with, and fnull = sum_j w_j f(bg_j) from the MLP kernels
+int fit_mlp(dks_ctx* ctx) {
+    const int N = ctx->N, D = ctx->D, C = ctx->C;
+    const cudaStream_t st = ctx->stream;
+    MlpDev& m = ctx->mlp;
+    TRY(fit_begin(ctx));
+    free_mlp(ctx);
+    TRY(upload_tree_array(&m.W, ctx->h_mw.data(), ctx->h_mw.size(), st));
+    TRY(upload_tree_array(&m.b, ctx->h_mb.data(), ctx->h_mb.size(), st));
+    TRY(upload_tree_array(&m.Wf, ctx->h_mwf.data(), ctx->h_mwf.size(), st));
+    TRY(upload_tree_array(&m.bp, ctx->h_mbp.data(), ctx->h_mbp.size(), st));
+    double* Bbg = nullptr;
+    TRY(dev_alloc(&Bbg, (size_t)N * m.width[1]));
+    m.Bbg = Bbg;
+    double* pred = nullptr;
+    TRY(dev_alloc(&pred, (size_t)N * C));
+    dks::mlp::mlp_fit_table_kernel<<<cdiv((long long)N * m.width[1], 256), 256, 0, st>>>(ctx->d_bg, N, D, m, Bbg);
+    dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, N), dks::mlp::THREADS, 0, st>>>(ctx->d_bg, N, D, m, C, ctx->link,
+                                                                                       nullptr, pred, nullptr, ctx->d_status);
+    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
+    ctx->launches += 3;
+    const int rc = fit_readback(ctx, "MLP");
+    cudaFree(pred);
+    TRY(rc);
+    return fit_done(ctx);
+}
+
 int choose_route(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
     const HeadDesc& h = ctx->head;
-    if (h.trees || h.kmach) {
+    if (h.trees || h.kmach || h.mlp) {
         *rt = Route{};
         return choose_route_own(ctx, ext_z, ext_stride, rt);
     }
@@ -1150,7 +1214,7 @@ int launch_general_l1(dks_ctx* ctx, const Route& rt, ExplainParams* p, double* p
     ExplainParams ps = *p;
     ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
     const bool timed = !ctx->capturing;
-    if (ctx->head.trees || ctx->head.kmach) {
+    if (ctx->head.trees || ctx->head.kmach || ctx->head.mlp) {
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
         TRY(launch_own_kernel(ctx, true, ps, rt.l1_smem, gstream));
         ctx->launches += 1;
@@ -1205,6 +1269,7 @@ int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t 
         break;
     case DKS_GENERAL_TREES:
     case DKS_GENERAL_KMACH:
+    case DKS_GENERAL_MLP:
         TRY(launch_own_kernel(ctx, false, p, rt.smem, gstream));
         break;
     default: {
@@ -1489,6 +1554,7 @@ int dks_destroy(dks_ctx* ctx) {
     free_encoding(ctx);
     dev_free(&ctx->d_Xenc);
     free_kmach(ctx);
+    free_mlp(ctx);
     free_column_maps(ctx);
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
@@ -1765,6 +1831,90 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
     return DKS_OK;
 }
 
+int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double* W_host, const double* b_host, int activation,
+                int head, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_mlp: call dks_set_background first (D unknown)");
+    REQUIRE(widths && W_host && b_host, "dks_set_mlp: need the widths, weights and biases");
+    const int D = ctx->D;
+    if (n_hidden < 1 || n_hidden > DKS_MLP_MAX_HIDDEN)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: %d hidden layers; 1..%d supported", n_hidden, DKS_MLP_MAX_HIDDEN);
+    const int L = n_hidden + 1, R = widths[L];
+    if (widths[0] != D)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the first layer reads %d columns, the background has %d", widths[0], D);
+    for (int l = 1; l < L; ++l)
+        if (widths[l] < 1 || widths[l] > DKS_MLP_MAX_WIDTH)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: hidden layer %d has %d units; 1..%d supported", l, widths[l],
+                        DKS_MLP_MAX_WIDTH);
+    if (R < 1 || R > DKS_MLP_MAX_OUT)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: %d output units; 1..%d supported", R, DKS_MLP_MAX_OUT);
+    if (activation < DKS_MLP_ACT_IDENTITY || activation > DKS_MLP_ACT_RELU)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: unknown activation %d", activation);
+    int C;
+    switch (head) {
+    case DKS_MLP_HEAD_IDENTITY: C = R; break;
+    case DKS_MLP_HEAD_SIGMOID:
+        if (R != 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the sigmoid head needs one output unit (got %d)", R);
+        C = 2;
+        break;
+    case DKS_MLP_HEAD_SOFTMAX:
+        if (R < 2) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the softmax head needs at least two output units (got %d)", R);
+        C = R;
+        break;
+    default: return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: unknown head %d", head);
+    }
+    MlpDev m = {};
+    m.L = L; m.act = activation; m.head = head; m.R = R;
+    size_t nw = 0, nb = 0, nwf = 0, nbp = 0;
+    for (int l = 0; l <= L; ++l) {
+        m.width[l] = widths[l];
+        m.pad[l] = l == 0 ? D : l == L ? 8 : dks::mlp::pad16(widths[l]);
+    }
+    for (int l = 0; l < L; ++l) {
+        m.woff[l] = (int)nw; m.boff[l] = (int)nb; m.wfoff[l] = (int)nwf; m.bpoff[l] = (int)nbp;
+        nw += (size_t)widths[l] * widths[l + 1];
+        nb += (size_t)widths[l + 1];
+        if (l > 0) nwf += (size_t)m.pad[l] * m.pad[l + 1];
+        nbp += (size_t)m.pad[l + 1];
+    }
+    if (nw > (size_t)INT32_MAX) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: %zu weights are too many", nw);
+    for (size_t e = 0; e < nw; ++e)
+        if (!std::isfinite(W_host[e])) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the weights must be finite");
+    for (size_t e = 0; e < nb; ++e)
+        if (!std::isfinite(b_host[e])) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the biases must be finite");
+    m.nbuf = n_hidden >= 2 ? 2 : 1;
+    m.hmax = 16;
+    for (int l = 1; l < L; ++l) m.hmax = std::max(m.hmax, m.pad[l]);
+    // layers 1 .. L - 1 in B-fragment order: element (k, n) of layer l at ((k / 16) * (pad / 8) + n / 8) * 32 + lane, lane =
+    // (n % 8) * 4 + k % 4, entry (k % 16) / 4; zero rows and columns pad it.  Every layer's biases zero-padded.
+    ctx->h_mwf.assign(nwf, 0.0);
+    ctx->h_mbp.assign(nbp, 0.0);
+    for (int l = 0; l < L; ++l) {
+        const int K = widths[l], H = widths[l + 1], NT = m.pad[l + 1] / 8;
+        for (int n = 0; n < H; ++n) ctx->h_mbp[m.bpoff[l] + n] = b_host[m.boff[l] + n];
+        if (l == 0) continue;
+        for (int k = 0; k < K; ++k)
+            for (int n = 0; n < H; ++n) {
+                const int kk = k & 15;
+                const size_t at = (((size_t)(k >> 4) * NT + (n >> 3)) * 32 + (n & 7) * 4 + (kk & 3)) * 4 + (kk >> 2);
+                ctx->h_mwf[m.wfoff[l] + at] = W_host[m.woff[l] + (size_t)k * H + n];
+            }
+    }
+    ctx->h_mw.assign(W_host, W_host + nw);
+    ctx->h_mb.assign(b_host, b_host + nb);
+    // the previous device copies stay owned until dks_fit replaces them
+    m.W = ctx->mlp.W; m.b = ctx->mlp.b; m.Wf = ctx->mlp.Wf; m.bp = ctx->mlp.bp; m.Bbg = ctx->mlp.Bbg;
+    ctx->mlp = m;
+    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
+    ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_MLP; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
+    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
+    ctx->h_W.assign((size_t)D, 0.0);
+    ctx->h_b.assign(1, 0.0);
+    ctx->fitted = false;
+    return DKS_OK;
+}
+
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
                         const double* vals_host, int n_vals) {
     BIND(ctx);
@@ -1778,6 +1928,8 @@ int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, con
     if (ctx->act == DKS_ACT_KMACH)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for kernel machines (their scalers fold into the support "
                     "vectors and column weights)");
+    if (ctx->act == DKS_ACT_MLP)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for MLPs (their scalers fold into the first layer)");
     if (D != ctx->D || R != ctx->R)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: maps of %d columns x %d score rows, model has %d x %d", D, R,
                     ctx->D, ctx->R);
@@ -1916,6 +2068,7 @@ int dks_fit(dks_ctx* ctx) {
         return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model is not a tree ensemble");
     if (h.trees) return fit_trees(ctx);
     if (h.kmach) return fit_kmach(ctx);
+    if (h.mlp) return fit_mlp(ctx);
     TRY(fit_begin(ctx));
     TRY(dev_alloc(&ctx->d_BW, (size_t)N * G * R));
     TRY(dev_alloc(&ctx->d_scores, (size_t)N * R));
@@ -2007,6 +2160,9 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     else if (ctx->head.kmach)
         dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->km, ctx->C, ctx->link,
                                                                              nullptr, dO, nullptr, ctx->d_status);
+    else if (ctx->head.mlp)
+        dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
+            dX, n, ctx->D, ctx->mlp, ctx->C, ctx->link, nullptr, dO, nullptr, ctx->d_status);
     else
         (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
             dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status, ctx->d_mix);

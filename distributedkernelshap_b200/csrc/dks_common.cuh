@@ -185,6 +185,22 @@ struct KmDev {
     int K, R, n_sv, kernel, head;
 };
 
+// multi-layer perceptrons (dks_set_mlp, DESIGN.md §5.0.14): L = hidden + 1 weight layers, layer l mapping width[l] units to
+// width[l + 1] (width[0] = D raw columns, width[L] = R outputs).  The explain kernel reads layers 1 .. L - 1 in the FP64 mma
+// B-fragment order, zero-padded to pad[l] x pad[l + 1] (hidden widths to a multiple of 16, the output layer to 8): padding
+// is zero weights, never zero activations.
+struct MlpDev {
+    const double* W;             // layer l: [width[l]][width[l + 1]] row-major at woff[l] (layer 0: the scalers folded in)
+    const double* b;             // layer l: [width[l + 1]] at boff[l]
+    const double* Wf;            // layers 1 .. L - 1: [pad[l] / 16][pad[l + 1] / 8][32 lanes][4] at wfoff[l]
+    const double* bp;            // every layer's biases zero-padded to pad[l + 1], at bpoff[l]
+    const double* Bbg;           // [N][width[1]] fit: b_0 + bg_j W_0
+    int woff[DKS_MLP_MAX_HIDDEN + 1], boff[DKS_MLP_MAX_HIDDEN + 1], wfoff[DKS_MLP_MAX_HIDDEN + 1], bpoff[DKS_MLP_MAX_HIDDEN + 1];
+    int width[DKS_MLP_MAX_HIDDEN + 2], pad[DKS_MLP_MAX_HIDDEN + 2];
+    int L, act, head, R;
+    int nbuf, hmax;              // activation buffers per warp (2 with two or more hidden layers) and the widest padded layer
+};
+
 // exp head, CUDA-core kernels (DESIGN.md §5.0.8): a coalition row is summed in fp32 when the largest weighted background
 // exponent t'_j = log2 e d(s, j) + log2 w_j lies in [EXP_T_LO, EXP_T_HI]; other rows are evaluated in float64
 #define DKS_EXP_T_LO -60.f
@@ -214,6 +230,7 @@ struct HeadDesc {
     bool tc = false;            // tensor-core kernel
     bool trees = false;         // tree ensemble: the tree kernels only (dks_trees.cuh)
     bool kmach = false;         // kernel machine: the kernel-machine kernels only (dks_kmach.cuh)
+    bool mlp = false;           // multi-layer perceptron: the MLP kernels only (dks_mlp.cuh)
     bool mixture() const { return shared == HEAD_SHARED_MIX_BINARY || shared == HEAD_SHARED_MIX_CLASS; }
 };
 
@@ -277,6 +294,10 @@ struct dks_ctx {
     // kernel machine (act == DKS_ACT_KMACH): host copies of the arrays, and their device copies built by dks_fit
     std::vector<double> h_ksv, h_kdual, h_kcolw, h_kcolo;
     KmDev km = {};
+    // multi-layer perceptron (act == DKS_ACT_MLP): host copies of the layers (natural, fragment-ordered, padded biases), and
+    // their device copies built by dks_fit
+    std::vector<double> h_mw, h_mb, h_mwf, h_mbp;
+    MlpDev mlp = {};
     std::vector<double> h_bg, h_wbg, h_W, h_b;
     std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
     std::vector<double> h_cm_keys, h_cm_vals;

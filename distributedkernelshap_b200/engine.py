@@ -16,6 +16,7 @@ from . import _cabi
 from .data import DenseData, convert_to_data, convert_to_link
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
 from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, extract_kernel_machine_spec
+from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, extract_mlp_spec
 from .predictors import extract_linear_spec
 from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_tree_pipeline_spec, extract_tree_spec
 
@@ -49,7 +50,9 @@ def rows_per_call(act_code, n_outputs, plan_mode, G, score_rows=1):
     """Rows per C-ABI call.  The softmax and one-vs-rest heads' shared-plan path keeps C per-class sums per coalition
     where the binary head keeps two: their row blocks are 2 / C as long, so that the per-call workspace stays the binary
     path's.  The mixture head keeps ``score_rows`` = K R_m nibble tables per instance and, on its shared-plan route, a
-    member's sums next to the mixture's: its blocks are 1 / (K R_m) as long.  Per-instance plans of more than 64 groups: ``MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE`` (plans
+    member's sums next to the mixture's: its blocks are 1 / (K R_m) as long.  Tree ensembles, kernel machines and MLPs keep
+    no per-instance workspace beyond phi and f(x) (their kernels hold an instance's coalitions in shared memory): full
+    blocks.  Per-instance plans of more than 64 groups: ``MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE`` (plans
     are keyed by the global row, so results do not depend on the block size)."""
     if act_code == _cabi.ACT_MIX:
         return MAX_ROWS_PER_CALL // max(1, score_rows)
@@ -132,7 +135,8 @@ class GpuKernelExplainer:
         What the reference passes as ``predictor``: a bound ``predict_proba`` / ``decision_function`` of a linear
         model or of a ``Pipeline`` of per-column preprocessing ending in one (explained in raw feature space), or a
         ``LinearModelSpec`` (see ``predictors.extract_linear_spec``); a tree model, bare or behind such a ``Pipeline``
-        (``trees.extract_tree_pipeline_spec``: the device replays the steps bit for bit); a kernel machine.  A raw value the pipeline would refuse (NaN, or an
+        (``trees.extract_tree_pipeline_spec``: the device replays the steps bit for bit); a kernel machine; a
+        scikit-learn MLP (``mlp.extract_mlp_spec``).  A raw value the pipeline would refuse (NaN, or an
         unseen category under ``handle_unknown='error'``) raises ``ValueError``.
     data
         Background data: array, DataFrame or ``DenseData`` (groups and weights honoured).
@@ -162,7 +166,9 @@ class GpuKernelExplainer:
         # a tree behind per-column preprocessing: explained in raw feature space, the device replaying the steps
         tree_spec, self.encoding = pipe_spec if pipe_spec is not None else (extract_tree_spec(model), None)
         km_spec = extract_kernel_machine_spec(model) if tree_spec is None else None
-        self.spec = tree_spec if tree_spec is not None else km_spec if km_spec is not None else extract_linear_spec(model)
+        mlp_spec = extract_mlp_spec(model) if tree_spec is None and km_spec is None else None
+        own = next((s for s in (tree_spec, km_spec, mlp_spec) if s is not None), None)   # a model with its own kernel
+        self.spec = own if own is not None else extract_linear_spec(model)
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
                                       "link log(ey / (1 - ey)) is undefined wherever a predicted mean exceeds 1")
@@ -199,9 +205,15 @@ class GpuKernelExplainer:
         if km_spec is not None and self.data.groups_size > KMACH_MAX_GROUPS:
             raise NotImplementedError(f"{self.data.groups_size} groups: kernel machines are explained up to "
                                       f"{KMACH_MAX_GROUPS} groups")
-        W = None if tree_spec is not None or km_spec is not None else \
+        if mlp_spec is not None and self.data.groups_size > MLP_MAX_GROUPS:
+            raise NotImplementedError(f"{self.data.groups_size} groups: MLPs are explained up to {MLP_MAX_GROUPS} groups")
+        W = None if own is not None else \
             self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
-        if km_spec is not None:
+        if mlp_spec is not None:
+            widths, Wm, bm = mlp_spec.flat()
+            _cabi.check(self.lib.dks_set_mlp(self._ctx, mlp_spec.n_hidden, _cabi.ptr(widths), _cabi.ptr(Wm), _cabi.ptr(bm),
+                                             mlp_spec.act_code_hidden, mlp_spec.head_code, int(mlp_spec.scalar_out)))
+        elif km_spec is not None:
             k = km_spec
             _cabi.check(self.lib.dks_set_kernel_machine(
                 self._ctx, k.K, _cabi.ptr(k.sv_off), _cabi.ptr(k.sv), _cabi.ptr(k.dual), k.R, _cabi.ptr(k.intercept),
@@ -697,7 +709,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp", "mixture"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp"),
     }
 
     def last_path(self):
@@ -708,8 +720,9 @@ class GpuKernelExplainer:
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
         are reported as unsupported, not computed, 'simt_wide': per-instance plans of 65..128 groups, 'trees': the tree
-        kernel, which takes every instance of a tree ensemble, or 'kmach': the kernel-machine kernel, which takes every
-        instance of a kernel machine), ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
+        kernel, which takes every instance of a tree ensemble, 'kmach': the kernel-machine kernel, which takes every
+        instance of a kernel machine, or 'mlp': the MLP kernel, which takes every instance of a multi-layer perceptron),
+        ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
         the weighted one), ``fused_table`` (1: the fused kernel read y from the plan's link table, passes outside its

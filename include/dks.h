@@ -103,6 +103,20 @@ extern "C" {
                                    * CalibratedClassifierCV over a binary SVC / NuSVC */
 #define DKS_KM_MAX_R 8            /* outputs of the identity head */
 #define DKS_KM_MAX_K 16           /* members of the calibrated head */
+#define DKS_ACT_MLP 8          /* multi-layer perceptron: set by dks_set_mlp only (dks_set_model refuses it) */
+
+/* hidden activation of a multi-layer perceptron (dks_set_mlp), scikit-learn's ACTIVATIONS */
+#define DKS_MLP_ACT_IDENTITY 0    /* h = a */
+#define DKS_MLP_ACT_LOGISTIC 1    /* h = 1 / (1 + exp(-a)) */
+#define DKS_MLP_ACT_TANH 2        /* h = tanh(a) */
+#define DKS_MLP_ACT_RELU 3        /* h = max(a, 0) */
+/* output head of a multi-layer perceptron on the output layer's values z [R] */
+#define DKS_MLP_HEAD_IDENTITY 0   /* outputs z (MLPRegressor.predict, R <= 8) */
+#define DKS_MLP_HEAD_SIGMOID 1    /* R = 1, outputs [1 - expit(z), expit(z)] (binary MLPClassifier.predict_proba) */
+#define DKS_MLP_HEAD_SOFTMAX 2    /* R = 2..8, outputs softmax(z) (multi-class MLPClassifier.predict_proba) */
+#define DKS_MLP_MAX_HIDDEN 4      /* hidden layers */
+#define DKS_MLP_MAX_WIDTH 256     /* units per hidden layer */
+#define DKS_MLP_MAX_OUT 8         /* output units */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -181,6 +195,21 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
                            const double* intercept, const double* colw, const double* colo, const double* gamma, int kernel,
                            double degree, double coef0, int head, const double* cal_a, const double* cal_b,
                            const double* pi, int scalar_out);
+/* multi-layer perceptron (DKS_ACT_MLP) in place of dks_set_model: n_hidden (1..DKS_MLP_MAX_HIDDEN) hidden layers.
+ * widths [n_hidden + 2] = {D, H_1 .. H_n_hidden, R}: hidden widths 1..DKS_MLP_MAX_WIDTH, R outputs 1..DKS_MLP_MAX_OUT.
+ * W_host: the layers' weights concatenated, layer l [widths[l]][widths[l + 1]] row-major (scikit-learn's coefs_[l]; layer 0
+ * reads raw feature space, per-column scalers folded in); b_host: the biases concatenated, layer l [widths[l + 1]].
+ * a_l = act(a_{l-1} W_l + b_l) for the hidden layers (activation DKS_MLP_ACT_*), z = a_n W + b for the output layer, outputs
+ * per DKS_MLP_HEAD_*.  Non-finite weights, bad widths and unknown codes are DKS_ERR_UNSUPPORTED.
+ * Every instance runs the MLP kernel (DKS_GENERAL_MLP, DESIGN.md §5.0.14), up to 64 groups: shared plans (full and partial
+ * varying sets), per-instance device plans and caller-supplied plans, kernel 'auto' or 'simt' (tcgen05 / shared are
+ * DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route.  Float64 throughout, every product on the FP64
+ * tensor cores.  NaN or an infinity in a background row (dks_fit) or an instance (dks_predict_host, the explain calls) is
+ * DKS_ERR_DOMAIN with the row; a link(ey) or link(f(x)) that is not finite is DKS_ERR_NUMERIC and nothing non-finite is
+ * written into phi.  Shapes whose per-instance buffers do not fit shared memory are DKS_ERR_UNSUPPORTED.
+ * dks_set_column_maps is refused. */
+int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double* W_host, const double* b_host, int activation,
+                int head, int scalar_out);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
  * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
  * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
@@ -401,6 +430,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_GENERAL_SIMT_WIDE 4  /* explain_wide_instance_kernel: per-instance plans of 65..128 groups (two-word rows) */
 #define DKS_GENERAL_TREES 5      /* explain_tree_kernel: every instance of a tree ensemble (dks_set_tree_model) */
 #define DKS_GENERAL_KMACH 6      /* explain_kmach_kernel: every instance of a kernel machine (dks_set_kernel_machine) */
+#define DKS_GENERAL_MLP 7        /* explain_mlp_kernel: every instance of a multi-layer perceptron (dks_set_mlp) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
