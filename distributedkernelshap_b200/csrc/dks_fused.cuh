@@ -189,7 +189,8 @@ __device__ __noinline__ void peer_push_finished(const double* __restrict__ phi, 
 }
 
 // every row group has delivered instance i: phi of both classes from its accumulator (read from L2), then the accumulator
-// and the counter reset for the next launch
+// and the counter reset for the next launch.  One lane: the run-time-N instantiations, which have no registers to spare
+// for finish_instances at 20 warps
 template <int KPAD>
 __device__ __forceinline__ void finish_instance(const FusedParams& p, int i, int nA, size_t slab) {
     long long* acc = p.acc + (size_t)i * KPAD;
@@ -210,6 +211,50 @@ __device__ __forceinline__ void finish_instance(const FusedParams& p, int i, int
     phi1[nA] = last;
     phi0[nA] = (last == 0.0) ? 0.0 : -last;
     p.done[i] = 0;
+}
+
+// the same on the instance's four lanes (fin; i and fin are the same on the instance's four lanes q = 0 .. 3): phi of
+// both classes from its accumulator (read from L2), then the accumulator and the counter reset for the next launch.  Lane q
+// takes coefficients q, q + 4, ..., the ones it delivered, so its loads are independent and in flight together (one lane
+// looping over the coefficients waits for each load in turn: its phi and acc stores may alias the next load).  The
+// eliminated group's sum still runs k = 0 .. nA - 1 in order, on lane 0, over the values the quad parked in the instance's
+// column of the staging tile (ycol, row stride ystride), which the turn-around has finished reading.  Called by the whole
+// warp; returns true on lane 0 of a finishing quad.
+template <int KPAD>
+__device__ __forceinline__ bool finish_instances(const FusedParams& p, bool fin, int i, int q, int nA, size_t slab,
+                                                 double* ycol, int ystride) {
+    constexpr int KPL = KPAD / 4;
+    if (fin) {
+        long long* acc = p.acc + (size_t)i * KPAD;
+        double* phi1 = p.phi + slab + (size_t)i * p.G;
+        double* phi0 = p.phi + (size_t)i * p.G;
+        const double delta = p.dlink[(size_t)i * p.C + 1];
+        long long a[KPL];
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) a[j] = q + 4 * j < nA ? __ldcg(acc + q + 4 * j) : 0;
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) {
+            const int k = q + 4 * j;
+            if (k < nA) {
+                double val = from_fix(a[j]) - delta * p.dvec[k];
+                ycol[k * ystride] = val;
+                if (fabs(val) < 1e-10) val = 0.0;
+                phi1[k] = val;
+                phi0[k] = (val == 0.0) ? 0.0 : -val;
+                acc[k] = 0;
+            }
+        }
+    }
+    __syncwarp();
+    if (!fin || q != 0) return false;
+    double sum = 0.0;
+    for (int k = 0; k < nA; ++k) sum += ycol[k * ystride];
+    double last = p.dlink[(size_t)i * p.C + 1] - sum;     // the eliminated (last) group takes the remainder
+    if (fabs(last) < 1e-10) last = 0.0;
+    p.phi[slab + (size_t)i * p.G + nA] = last;
+    p.phi[(size_t)i * p.G + nA] = (last == 0.0) ? 0.0 : -last;
+    p.done[i] = 0;
+    return true;
 }
 
 // weighted: the weighted slice (twice the bytes) and the per-CTA W2 array of dks_shared.cuh
@@ -367,15 +412,25 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                                              "l"((unsigned long long)to_fix(beta[j])) : "memory");
                     }
                     __syncwarp();               // the instance's four lanes have added: its first lane publishes the delivery
+                    int old = 0;
                     if (mine && q == 0) {
-                        int old;
                         asm volatile("atom.release.gpu.global.add.s32 %0, [%1], 1;" : "=r"(old) : "l"(p.done + i) : "memory");
                         if (old == n_rg - 1) {
-                            // every row group has delivered: finish the instance
+                            // every row group has delivered: the acquire (with NCT ordered before the other three lanes'
+                            // reads by the __syncwarp below), then finish the instance
                             asm volatile("fence.acq_rel.gpu;" ::: "memory");
-                            finish_instance<KPAD>(p, i, nA, slab);
-                            fin_i = i;
+                            if constexpr (NCT == 0) {
+                                finish_instance<KPAD>(p, i, nA, slab);
+                                fin_i = i;
+                            }
                         }
+                    }
+                    if constexpr (NCT != 0) {
+                        __syncwarp();
+                        const int old_i = __shfl_sync(0xffffffffu, old, lane & ~3);
+                        const bool fin = mine && old_i == n_rg - 1;
+                        if (__any_sync(0xffffffffu, fin) && finish_instances<KPAD>(p, fin, i, q, nA, slab, sYw + b, ystride))
+                            fin_i = i;
                     }
                     if (p.npeers > 0) peer_push_finished(p.phi, p.peer_phi, p.npeers, fin_i, lane, G, slab);     // multi-GPU only (kept out of line: no registers here)
                 }
