@@ -20,6 +20,7 @@
 #include "dks_encode.cuh"
 #include "dks_kmach.cuh"
 #include "dks_mlp.cuh"
+#include "dks_knn.cuh"
 
 namespace {
 
@@ -199,8 +200,13 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         // no shared-plan route: every instance runs the MLP kernels; the sigmoid head solves class 1 (class 0 its negation)
         h.mlp = true; h.l1_binary = ctx->mlp.head == DKS_MLP_HEAD_SIGMOID;
         break;
+    case DKS_ACT_KNN:
+        // no shared-plan route: every instance runs the neighbour kernels; every output is solved on its own (count / k
+        // probabilities are not exact negations of each other in float64)
+        h.knn = true;
+        break;
     }
-    if (h.shared != HEAD_SHARED_BINARY && !h.trees && !h.kmach && !h.mlp) h.shared_max_G = 128;
+    if (h.shared != HEAD_SHARED_BINARY && !h.own()) h.shared_max_G = 128;
     if (!h.mixture()) h.xt_scale = h.scale;
     h.l1_nout = h.l1_binary ? 1 : ctx->C;
     return h;
@@ -240,8 +246,8 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const size_t maps_doubles = maps ? (size_t)ctx->cm.n_keys + ctx->cm.n_vals : 0;
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D, maps_doubles) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D, maps_doubles);
-    // the score rows stage 1 computes: one for trees, kernel machines and MLPs (the scores of a zero linear model, unused)
-    const int R = h.trees || h.kmach || h.mlp ? 1 : ctx->R;
+    // the score rows stage 1 computes: one for the families with their own kernel (the scores of a zero linear model, unused)
+    const int R = h.own() ? 1 : ctx->R;
     auto kern = stage ? (maps ? prep_kernel_for<true, true>(h.mixture(), R) : prep_kernel_for<true, false>(h.mixture(), R))
                       : (maps ? prep_kernel_for<false, true>(h.mixture(), R) : prep_kernel_for<false, false>(h.mixture(), R));
     // nibble tables for the shared-plan route: the binary head's at any G, the other heads' up to 128 groups (what their
@@ -257,8 +263,8 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
         ctx->tree_X = ctx->d_Xenc;
         ctx->tree_D = ctx->enc.E;
     }
-    if (h.trees || h.kmach || h.mlp) {
-        // tree ensembles, kernel machines and MLPs: prep_kernel decides the varying groups (its scores are those of a zero linear
+    if (h.own()) {
+        // tree ensembles, kernel machines, MLPs and neighbour models: prep_kernel decides the varying groups (its scores are those of a zero linear
         // model, one identity output, and unused); the model's predict kernel then writes f(x) and link(f(x)) - link(fnull)
         // of every output
         kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
@@ -273,6 +279,10 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
         else if (h.mlp)
             dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
                 X_dev, n, ctx->D, ctx->mlp, ctx->C, ctx->link, ctx->d_linkfnull, nullptr, ctx->d_dlink, ctx->d_status);
+        else if (h.knn)
+            dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->knn, ctx->C, ctx->link,
+                                                                               ctx->d_linkfnull, nullptr, ctx->d_dlink,
+                                                                               ctx->d_status);
         else
             dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->tree_X, n, ctx->tree_D, ctx->tree,
                                                                                    ctx->C, ctx->link, ctx->d_linkfnull,
@@ -456,6 +466,15 @@ int mlp_warps(const dks_ctx* ctx, int S_cap) {
     return nw;
 }
 
+// coalitions per chunk of explain_knn_kernel at S_cap rows: as many neighbour lists as the opt-in shared memory holds next
+// to the sums and the tables, at most S_cap and at least 1
+int knn_chunk(const dks_ctx* ctx, int S_cap) {
+    const size_t fixed = dks::knn::smem_bytes(S_cap, ctx->C, ctx->G, ctx->knn.k, 0);
+    const size_t per = (sizeof(double) + sizeof(int)) * (size_t)ctx->knn.k;
+    const long long room = (long long)ctx->max_smem_optin - (long long)fixed;
+    return (int)std::max(1LL, std::min((long long)S_cap, room / (long long)per));
+}
+
 OwnKernel own_kernel(const dks_ctx* ctx) {
     if (ctx->head.trees)
         return {DKS_GENERAL_TREES, "tree ensembles", "tree kernel", "trees", [](const dks_ctx* c, int S_cap) {
@@ -463,6 +482,9 @@ OwnKernel own_kernel(const dks_ctx* ctx) {
     if (ctx->head.mlp)
         return {DKS_GENERAL_MLP, "MLPs", "MLP kernel", "hidden units", [](const dks_ctx* c, int S_cap) {
                     return dks::mlp::smem_bytes(S_cap, c->C, c->G, c->mlp, mlp_warps(c, S_cap)); }};
+    if (ctx->head.knn)
+        return {DKS_GENERAL_KNN, "nearest-neighbour models", "neighbour kernel", "neighbours", [](const dks_ctx* c, int S_cap) {
+                    return dks::knn::smem_bytes(S_cap, c->C, c->G, c->knn.k, knn_chunk(c, S_cap)); }};
     return {DKS_GENERAL_KMACH, "kernel machines", "kernel-machine kernel", "groups", [](const dks_ctx* c, int S_cap) {
                 return dks::kmach::smem_bytes(S_cap, c->C, c->km.R, c->G, c->km.head == DKS_KM_HEAD_CALIBRATED); }};
 }
@@ -517,6 +539,11 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->cur_X, ctx->d_bg, ctx->D,
                                                     ctx->d_goff, ctx->d_gcols);
+    } else if (ctx->head.knn) {
+        auto kern = l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->cur_X, ctx->d_bg, ctx->D,
+                                                    ctx->d_goff, ctx->d_gcols);
     } else {
         auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -537,9 +564,9 @@ const char* refusal_phrase(bool kmach, bool encoding) {
 }
 // the row named by the status word, refused by the model's family
 int fail_refused(const dks_ctx* ctx, const char* prefix) {
-    if (ctx->head.mlp)
-        return fail(DKS_ERR_DOMAIN, "%s %d holds NaN or an infinity: MLPs refuse it, as scikit-learn does", prefix,
-                    ctx->h_status[1]);
+    if (ctx->head.mlp || ctx->head.knn)
+        return fail(DKS_ERR_DOMAIN, "%s %d holds NaN or an infinity: %s refuse it, as scikit-learn does", prefix,
+                    ctx->h_status[1], ctx->head.mlp ? "MLPs" : "nearest-neighbour models");
     return fail(DKS_ERR_DOMAIN, "%s %d %s", prefix, ctx->h_status[1], refusal_phrase(ctx->head.kmach, ctx->head.trees));
 }
 
@@ -782,9 +809,53 @@ int fit_mlp(dks_ctx* ctx) {
     return fit_done(ctx);
 }
 
+void free_knn(dks_ctx* ctx) {
+    KnnDev& k = ctx->knn;
+    for (const void* q : {(const void*)k.fitX, (const void*)k.colw, (const void*)k.colo, (const void*)k.y,
+                          (const void*)k.colgrp, (const void*)k.Tbg, (const void*)k.Ebg})
+        if (q) cudaFree((void*)q);
+    k.fitX = nullptr; k.colw = nullptr; k.colo = nullptr; k.y = nullptr; k.colgrp = nullptr; k.Tbg = nullptr; k.Ebg = nullptr;
+}
+
+// dks_fit of a nearest-neighbour model: the arrays, the group of every column, T[j][v] and the equality masks E[j][v] of
+// every background row and training row, the column statistics stage 1 decides the varying groups with, and
+// fnull = sum_j w_j f(bg_j) from the neighbour kernels
+int fit_knn(dks_ctx* ctx) {
+    const int N = ctx->N, D = ctx->D, G = ctx->G, C = ctx->C;
+    const cudaStream_t st = ctx->stream;
+    KnnDev& k = ctx->knn;
+    TRY(fit_begin(ctx));
+    std::vector<int32_t> colgrp(D, 0);
+    for (int g = 0; g < G; ++g)
+        for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
+    free_knn(ctx);
+    TRY(upload_tree_array(&k.fitX, ctx->h_nfitX.data(), ctx->h_nfitX.size(), st));
+    TRY(upload_tree_array(&k.colw, ctx->h_ncolw.data(), ctx->h_ncolw.size(), st));
+    TRY(upload_tree_array(&k.colo, ctx->h_ncolo.data(), ctx->h_ncolo.size(), st));
+    TRY(upload_tree_array(&k.y, ctx->h_ny.data(), ctx->h_ny.size(), st));
+    TRY(upload_tree_array(&k.colgrp, colgrp.data(), colgrp.size(), st));
+    double* Tbg = nullptr;
+    uint64_t* Ebg = nullptr;
+    TRY(dev_alloc(&Tbg, (size_t)N * k.n_fit));
+    k.Tbg = Tbg;
+    TRY(dev_alloc(&Ebg, (size_t)N * k.n_fit));
+    k.Ebg = Ebg;
+    double* pred = nullptr;
+    TRY(dev_alloc(&pred, (size_t)N * C));
+    dks::knn::knn_fit_table_kernel<<<cdiv((long long)N * k.n_fit, 256), 256, 0, st>>>(ctx->d_bg, N, D, G, k, Tbg, Ebg);
+    dks::knn::knn_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(ctx->d_bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
+                                                               ctx->d_status);
+    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
+    ctx->launches += 3;
+    const int rc = fit_readback(ctx, "nearest-neighbour model");
+    cudaFree(pred);
+    TRY(rc);
+    return fit_done(ctx);
+}
+
 int choose_route(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
     const HeadDesc& h = ctx->head;
-    if (h.trees || h.kmach || h.mlp) {
+    if (h.own()) {
         *rt = Route{};
         return choose_route_own(ctx, ext_z, ext_stride, rt);
     }
@@ -1214,7 +1285,7 @@ int launch_general_l1(dks_ctx* ctx, const Route& rt, ExplainParams* p, double* p
     ExplainParams ps = *p;
     ps.list = ctx->d_idx_sel; ps.count = ctx->d_l1_counts;
     const bool timed = !ctx->capturing;
-    if (ctx->head.trees || ctx->head.kmach || ctx->head.mlp) {
+    if (ctx->head.own()) {
         if (timed) CUDA_TRY(cudaEventRecord(ctx->ev_l1[0], gstream));
         TRY(launch_own_kernel(ctx, true, ps, rt.l1_smem, gstream));
         ctx->launches += 1;
@@ -1270,6 +1341,7 @@ int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t 
     case DKS_GENERAL_TREES:
     case DKS_GENERAL_KMACH:
     case DKS_GENERAL_MLP:
+    case DKS_GENERAL_KNN:
         TRY(launch_own_kernel(ctx, false, p, rt.smem, gstream));
         break;
     default: {
@@ -1555,6 +1627,7 @@ int dks_destroy(dks_ctx* ctx) {
     dev_free(&ctx->d_Xenc);
     free_kmach(ctx);
     free_mlp(ctx);
+    free_knn(ctx);
     free_column_maps(ctx);
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
@@ -1915,6 +1988,59 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
     return DKS_OK;
 }
 
+int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double* colw, const double* colo, int k, int metric,
+                      double p, int weights, int R, const double* labels_or_targets, int head, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_knn_model: call dks_set_background first (D unknown)");
+    REQUIRE(fitX && colw && colo && labels_or_targets, "dks_set_knn_model: need the training rows, column map and labels");
+    const int D = ctx->D;
+    auto finite = [](const double* a, size_t n) {
+        for (size_t e = 0; e < n; ++e) if (!std::isfinite(a[e])) return false;
+        return true;
+    };
+    if (k < 1 || k > DKS_KNN_MAX_K)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: k=%d neighbours; 1..%d supported", k, DKS_KNN_MAX_K);
+    if (n_fit < k)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: %d training rows for k=%d neighbours (need n_fit >= k)", n_fit, k);
+    if (metric < DKS_KNN_METRIC_EUCLIDEAN || metric > DKS_KNN_METRIC_SQEUCLIDEAN)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: unknown metric %d", metric);
+    if (metric == DKS_KNN_METRIC_MINKOWSKI && !(std::isfinite(p) && p >= 1))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: minkowski p=%g (a finite p >= 1)", p);
+    if (weights != DKS_KNN_WEIGHTS_UNIFORM && weights != DKS_KNN_WEIGHTS_DISTANCE)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: unknown weights %d", weights);
+    if (head != DKS_KNN_HEAD_CLASSIFY && head != DKS_KNN_HEAD_REGRESS)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: unknown head %d", head);
+    const int Rmin = head == DKS_KNN_HEAD_CLASSIFY ? 2 : 1;
+    if (R < Rmin || R > DKS_KNN_MAX_R)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: R=%d %s; %d..%d supported", R,
+                    head == DKS_KNN_HEAD_CLASSIFY ? "classes" : "targets", Rmin, DKS_KNN_MAX_R);
+    const size_t ny = head == DKS_KNN_HEAD_CLASSIFY ? (size_t)n_fit : (size_t)n_fit * R;
+    if (!finite(fitX, (size_t)n_fit * D) || !finite(colw, D) || !finite(colo, D) || !finite(labels_or_targets, ny))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: the arrays must be finite");
+    for (int c = 0; c < D; ++c)
+        if (colw[c] == 0) return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: column weights must be non-zero");
+    if (head == DKS_KNN_HEAD_CLASSIFY)
+        for (int v = 0; v < n_fit; ++v) {
+            const double l = labels_or_targets[v];
+            if (!(l >= 0 && l < R && l == std::floor(l)))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: the label of row %d is not a class index 0..%d", v, R - 1);
+        }
+    KnnDev& kd = ctx->knn;
+    kd.n_fit = n_fit; kd.k = k; kd.metric = metric; kd.p = p; kd.weights = weights; kd.R = R; kd.head = head;
+    ctx->h_nfitX.assign(fitX, fitX + (size_t)n_fit * D);
+    ctx->h_ncolw.assign(colw, colw + D);
+    ctx->h_ncolo.assign(colo, colo + D);
+    ctx->h_ny.assign(labels_or_targets, labels_or_targets + ny);
+    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
+    ctx->R = 1; ctx->C = R; ctx->act = DKS_ACT_KNN; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
+    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
+    ctx->h_W.assign((size_t)D, 0.0);
+    ctx->h_b.assign(1, 0.0);
+    ctx->fitted = false;
+    return DKS_OK;
+}
+
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
                         const double* vals_host, int n_vals) {
     BIND(ctx);
@@ -1930,6 +2056,9 @@ int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, con
                     "vectors and column weights)");
     if (ctx->act == DKS_ACT_MLP)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for MLPs (their scalers fold into the first layer)");
+    if (ctx->act == DKS_ACT_KNN)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for nearest-neighbour models (their scalers fold into the "
+                    "column weights and origins)");
     if (D != ctx->D || R != ctx->R)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: maps of %d columns x %d score rows, model has %d x %d", D, R,
                     ctx->D, ctx->R);
@@ -2069,6 +2198,7 @@ int dks_fit(dks_ctx* ctx) {
     if (h.trees) return fit_trees(ctx);
     if (h.kmach) return fit_kmach(ctx);
     if (h.mlp) return fit_mlp(ctx);
+    if (h.knn) return fit_knn(ctx);
     TRY(fit_begin(ctx));
     TRY(dev_alloc(&ctx->d_BW, (size_t)N * G * R));
     TRY(dev_alloc(&ctx->d_scores, (size_t)N * R));
@@ -2163,6 +2293,9 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     else if (ctx->head.mlp)
         dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
             dX, n, ctx->D, ctx->mlp, ctx->C, ctx->link, nullptr, dO, nullptr, ctx->d_status);
+    else if (ctx->head.knn)
+        dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->knn, ctx->C, ctx->link,
+                                                                           nullptr, dO, nullptr, ctx->d_status);
     else
         (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
             dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status, ctx->d_mix);

@@ -201,6 +201,20 @@ struct MlpDev {
     int nbuf, hmax;              // activation buffers per warp (2 with two or more hidden layers) and the widest padded layer
 };
 
+// k-nearest neighbours (dks_set_knn_model, DESIGN.md §5.0.15): t(x, v) = sum_c h((colw_c x_c + colo_c) - v_c) per
+// DKS_KNN_METRIC_*, the k smallest (t, index) over the training rows, then the vote or mean per DKS_KNN_HEAD_*
+struct KnnDev {
+    const double* fitX;          // [n_fit][D] training rows in the fitted space
+    const double* colw;          // [D] x' = colw x + colo (the scalers folded in)
+    const double* colo;          // [D]
+    const double* y;             // classify: [n_fit] class index; regress: [n_fit][R]
+    const int* colgrp;           // [D] group of every column
+    const double* Tbg;           // [N][n_fit] fit: t of background row j and training row v
+    const uint64_t* Ebg;         // [N][n_fit] fit: the groups on which background row j equals training row v exactly
+    double p;                    // Minkowski exponent
+    int n_fit, k, metric, weights, R, head;
+};
+
 // exp head, CUDA-core kernels (DESIGN.md §5.0.8): a coalition row is summed in fp32 when the largest weighted background
 // exponent t'_j = log2 e d(s, j) + log2 w_j lies in [EXP_T_LO, EXP_T_HI]; other rows are evaluated in float64
 #define DKS_EXP_T_LO -60.f
@@ -231,7 +245,9 @@ struct HeadDesc {
     bool trees = false;         // tree ensemble: the tree kernels only (dks_trees.cuh)
     bool kmach = false;         // kernel machine: the kernel-machine kernels only (dks_kmach.cuh)
     bool mlp = false;           // multi-layer perceptron: the MLP kernels only (dks_mlp.cuh)
+    bool knn = false;           // k-nearest neighbours: the neighbour kernels only (dks_knn.cuh)
     bool mixture() const { return shared == HEAD_SHARED_MIX_BINARY || shared == HEAD_SHARED_MIX_CLASS; }
+    bool own() const { return trees || kmach || mlp || knn; }   // a family whose every instance runs its own kernel
 };
 
 // Tables derived from the plan of the full varying set (M == G) that PlanDev does not hold: the class-sum heads' per-class
@@ -298,6 +314,9 @@ struct dks_ctx {
     // their device copies built by dks_fit
     std::vector<double> h_mw, h_mb, h_mwf, h_mbp;
     MlpDev mlp = {};
+    // k-nearest neighbours (act == DKS_ACT_KNN): host copies of the arrays, and their device copies built by dks_fit
+    std::vector<double> h_nfitX, h_ncolw, h_ncolo, h_ny;
+    KnnDev knn = {};
     std::vector<double> h_bg, h_wbg, h_W, h_b;
     std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
     std::vector<double> h_cm_keys, h_cm_vals;

@@ -17,6 +17,7 @@ from .data import DenseData, convert_to_data, convert_to_link
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
 from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, extract_kernel_machine_spec
 from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, extract_mlp_spec
+from .neighbors import MAX_GROUPS as KNN_MAX_GROUPS, extract_knn_spec
 from .predictors import extract_linear_spec
 from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_tree_pipeline_spec, extract_tree_spec
 
@@ -136,8 +137,9 @@ class GpuKernelExplainer:
         model or of a ``Pipeline`` of per-column preprocessing ending in one (explained in raw feature space), or a
         ``LinearModelSpec`` (see ``predictors.extract_linear_spec``); a tree model, bare or behind such a ``Pipeline``
         (``trees.extract_tree_pipeline_spec``: the device replays the steps bit for bit); a kernel machine; a
-        scikit-learn MLP (``mlp.extract_mlp_spec``).  A raw value the pipeline would refuse (NaN, or an
-        unseen category under ``handle_unknown='error'``) raises ``ValueError``.
+        scikit-learn MLP (``mlp.extract_mlp_spec``); a k-nearest-neighbour model (``neighbors.extract_knn_spec``).  A raw
+        value the pipeline would refuse (NaN, or an unseen category under ``handle_unknown='error'``) raises
+        ``ValueError``.
     data
         Background data: array, DataFrame or ``DenseData`` (groups and weights honoured).
     link
@@ -167,7 +169,8 @@ class GpuKernelExplainer:
         tree_spec, self.encoding = pipe_spec if pipe_spec is not None else (extract_tree_spec(model), None)
         km_spec = extract_kernel_machine_spec(model) if tree_spec is None else None
         mlp_spec = extract_mlp_spec(model) if tree_spec is None and km_spec is None else None
-        own = next((s for s in (tree_spec, km_spec, mlp_spec) if s is not None), None)   # a model with its own kernel
+        knn_spec = extract_knn_spec(model) if tree_spec is None and km_spec is None and mlp_spec is None else None
+        own = next((s for s in (tree_spec, km_spec, mlp_spec, knn_spec) if s is not None), None)   # its own kernel
         self.spec = own if own is not None else extract_linear_spec(model)
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
@@ -207,9 +210,17 @@ class GpuKernelExplainer:
                                       f"{KMACH_MAX_GROUPS} groups")
         if mlp_spec is not None and self.data.groups_size > MLP_MAX_GROUPS:
             raise NotImplementedError(f"{self.data.groups_size} groups: MLPs are explained up to {MLP_MAX_GROUPS} groups")
+        if knn_spec is not None and self.data.groups_size > KNN_MAX_GROUPS:
+            raise NotImplementedError(f"{self.data.groups_size} groups: nearest-neighbour models are explained up to "
+                                      f"{KNN_MAX_GROUPS} groups")
         W = None if own is not None else \
             self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
-        if mlp_spec is not None:
+        if knn_spec is not None:
+            k = knn_spec
+            _cabi.check(self.lib.dks_set_knn_model(
+                self._ctx, k.n_fit, _cabi.ptr(k.fitX), _cabi.ptr(k.colw), _cabi.ptr(k.colo), k.k, k.metric_code, k.p,
+                k.weights_code, k.R, _cabi.ptr(k.y), k.head_code, int(k.scalar_out)))
+        elif mlp_spec is not None:
             widths, Wm, bm = mlp_spec.flat()
             _cabi.check(self.lib.dks_set_mlp(self._ctx, mlp_spec.n_hidden, _cabi.ptr(widths), _cabi.ptr(Wm), _cabi.ptr(bm),
                                              mlp_spec.act_code_hidden, mlp_spec.head_code, int(mlp_spec.scalar_out)))
@@ -261,7 +272,7 @@ class GpuKernelExplainer:
         self._last_rows = 0
         if self.encoding is not None:
             self._check_encoding(bg)
-        self._check_model_against_callable(bg)
+        self._check_model_against_callable(bg, knn_spec)
 
     # ------------------------------------------------------------------------------------------------------
     def encode(self, X):
@@ -294,12 +305,27 @@ class GpuKernelExplainer:
                              f"pipeline[:-1].transform(background) bit for bit ({bad}): refusing to explain a different "
                              "function")
 
-    def _check_model_against_callable(self, bg):
-        """The extracted linear model must reproduce the user's callable on the background rows."""
+    def _check_model_against_callable(self, bg, knn_spec=None):
+        """The extracted model must reproduce the user's callable on the background rows.  A neighbour model is compared
+        on the rows whose k-th and (k + 1)-th nearest training rows are not equidistant; a row with such a boundary tie
+        is compared with the spec's own NumPy evaluation instead (which of equidistant rows is a neighbour is the
+        engine's rule, not scikit-learn's), and at least one row must be compared with the callable."""
         if not callable(self.model_callable):
             return
         want = np.asarray(self.model_callable(bg), dtype=np.float64).reshape(self.N, -1)
         got = self.predict(bg)
+        if knn_spec is not None and want.shape == got.shape:
+            tied = knn_spec.boundary_ties(bg)
+            if tied.all():
+                raise ValueError("every background row has a tie between its k-th and (k + 1)-th nearest training rows: "
+                                 "the neighbour model extracted from `predictor` cannot be checked against "
+                                 "predictor(background); refusing to explain a function that was not checked")
+            if tied.any():
+                logger.warning("%d of %d background rows have equidistant k-th and (k + 1)-th nearest training rows: "
+                               "they are checked against the engine's rule (the lower training index wins), not "
+                               "against `predictor`", int(tied.sum()), self.N)
+                want = want.copy()
+                want[tied] = np.asarray(knn_spec(bg[tied]), dtype=np.float64).reshape(int(tied.sum()), -1)
         if want.shape != got.shape or not np.allclose(got, want, rtol=1e-7, atol=1e-9, equal_nan=True):
             raise ValueError("the linear model extracted from `predictor` does not reproduce predictor(background): "
                              "refusing to explain a different function (max abs diff "
@@ -709,7 +735,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp", "mixture"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn"),
     }
 
     def last_path(self):
@@ -721,7 +747,8 @@ class GpuKernelExplainer:
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they
         are reported as unsupported, not computed, 'simt_wide': per-instance plans of 65..128 groups, 'trees': the tree
         kernel, which takes every instance of a tree ensemble, 'kmach': the kernel-machine kernel, which takes every
-        instance of a kernel machine, or 'mlp': the MLP kernel, which takes every instance of a multi-layer perceptron),
+        instance of a kernel machine, 'mlp': the MLP kernel, which takes every instance of a multi-layer perceptron, or
+        'knn': the neighbour kernel, which takes every instance of a k-nearest-neighbour model),
         ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take

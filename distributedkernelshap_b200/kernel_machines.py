@@ -153,8 +153,8 @@ def _is_kernel_machine(est):
     return bool(names & _KRR)
 
 
-def _affine(step):
-    """(a, b) of a fitted per-column affine scaler: x' = a x + b."""
+def _affine(step, family="kernel machine"):
+    """(a, b) of a fitted per-column affine scaler: x' = a x + b.  ``family`` names the model in refusals."""
     name = type(step).__name__
     P = int(step.n_features_in_)
     a, b = np.ones(P), np.zeros(P)
@@ -170,29 +170,30 @@ def _affine(step):
             b = -np.asarray(step.center_, dtype=np.float64) * a
     elif name == "MinMaxScaler":
         if step.clip:
-            raise NotImplementedError("MinMaxScaler(clip=True) is not affine: kernel machines fold affine scalers only")
+            raise NotImplementedError(f"MinMaxScaler(clip=True) is not affine: {family}s fold affine scalers only")
         a, b = np.asarray(step.scale_, dtype=np.float64), np.asarray(step.min_, dtype=np.float64)
     elif name == "MaxAbsScaler":
         a = 1.0 / np.asarray(step.scale_, dtype=np.float64)
     return a, b
 
 
-def _unwrap(est, P):
-    """(final estimator, a, b) with the pipeline's scalers composed into x' = a x + b."""
+def _unwrap(est, P, family="kernel machine", target="its support vectors"):
+    """(final estimator, a, b) with the pipeline's scalers composed into x' = a x + b.  ``family`` and ``target`` (what
+    the scalers fold into) name the model in refusals."""
     a, b = np.ones(P), np.zeros(P)
     while "Pipeline" in _names(est):
         for name, step in est.steps[:-1]:
             if step is None or step == "passthrough":
                 continue
             if type(step).__name__ not in _SCALERS:
-                raise NotImplementedError(f"Pipeline step {name!r} ({type(step).__name__}) in front of a kernel machine: "
+                raise NotImplementedError(f"Pipeline step {name!r} ({type(step).__name__}) in front of a {family}: "
                                           "only StandardScaler, MinMaxScaler, MaxAbsScaler and RobustScaler fold into "
-                                          "its support vectors")
-            sa, sb = _affine(step)
+                                          f"{target}")
+            sa, sb = _affine(step, family)
             a, b = sa * a, sa * b + sb
         est = est.steps[-1][1]
     if not (np.all(np.isfinite(a)) and np.all(np.isfinite(b)) and np.all(a != 0)):
-        raise NotImplementedError("a scaler with a zero or non-finite scale cannot be folded into a kernel machine")
+        raise NotImplementedError(f"a scaler with a zero or non-finite scale cannot be folded into a {family}")
     return est, a, b
 
 

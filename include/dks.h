@@ -117,6 +117,22 @@ extern "C" {
 #define DKS_MLP_MAX_HIDDEN 4      /* hidden layers */
 #define DKS_MLP_MAX_WIDTH 256     /* units per hidden layer */
 #define DKS_MLP_MAX_OUT 8         /* output units */
+#define DKS_ACT_KNN 9          /* k-nearest neighbours: set by dks_set_knn_model only (dks_set_model refuses it) */
+
+/* distance of a nearest-neighbour model (dks_set_knn_model): t = sum_c h(d_c) over the columns in order,
+ * d_c = (colw_c x_c + colo_c) - v_c for training row v */
+#define DKS_KNN_METRIC_EUCLIDEAN 0   /* h = d^2,   distance sqrt(t) */
+#define DKS_KNN_METRIC_MANHATTAN 1   /* h = |d|,   distance t */
+#define DKS_KNN_METRIC_MINKOWSKI 2   /* h = |d|^p, distance t^(1/p), finite p >= 1 */
+#define DKS_KNN_METRIC_SQEUCLIDEAN 3 /* h = d^2,   distance t */
+/* neighbour weights */
+#define DKS_KNN_WEIGHTS_UNIFORM 0    /* 1 */
+#define DKS_KNN_WEIGHTS_DISTANCE 1   /* 1 / distance; neighbours at distance 0 take 1 and the others 0 */
+/* output head */
+#define DKS_KNN_HEAD_CLASSIFY 0      /* R classes, outputs the per-class weight sums over their total (predict_proba) */
+#define DKS_KNN_HEAD_REGRESS 1       /* R targets, outputs the weighted mean of the neighbours' targets (predict) */
+#define DKS_KNN_MAX_K 32             /* neighbours */
+#define DKS_KNN_MAX_R 8              /* classes or targets */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -210,6 +226,24 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
  * dks_set_column_maps is refused. */
 int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double* W_host, const double* b_host, int activation,
                 int head, int scalar_out);
+/* k-nearest-neighbour model (DKS_ACT_KNN) in place of dks_set_model: n_fit >= k training rows fitX [n_fit][D] row-major in
+ * the space the model was fitted in; a row x is read as x'_c = colw_c x_c + colo_c (colw [D] non-zero, colo [D]: per-column
+ * scalers folded in).  k neighbours (1..DKS_KNN_MAX_K), metric DKS_KNN_METRIC_* (p: the Minkowski exponent, read for
+ * DKS_KNN_METRIC_MINKOWSKI), weights DKS_KNN_WEIGHTS_*.  head DKS_KNN_HEAD_CLASSIFY: R = 2..8 classes and
+ * labels_or_targets [n_fit] holds each row's class index 0..R-1; DKS_KNN_HEAD_REGRESS: R = 1..8 targets, labels_or_targets
+ * [n_fit][R].  The neighbours are the first k training rows ranked by (t, row index): of equidistant rows the lower index
+ * wins.  A row equal to a training row column for column (x'_c == v_c exactly) is at distance exactly 0 whatever the
+ * rounding of t; other distances are clamped at 0.  Non-finite arrays, bad sizes and unknown codes are
+ * DKS_ERR_UNSUPPORTED.
+ * Every instance runs the neighbour kernel (DKS_GENERAL_KNN, DESIGN.md §5.0.15), up to 64 groups: shared plans (full and
+ * partial varying sets), per-instance device plans and caller-supplied plans, kernel 'auto' or 'simt' (tcgen05 / shared are
+ * DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route; every output is solved on its own.  Float64
+ * throughout.  NaN or an infinity in a background row (dks_fit) or an instance (dks_predict_host, the explain calls) is
+ * DKS_ERR_DOMAIN with the row; a link(ey) or link(f(x)) that is not finite (the logit of a probability of exactly 0 or 1) is
+ * DKS_ERR_NUMERIC and nothing non-finite is written into phi.  Shapes whose per-instance buffers do not fit shared memory
+ * are DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused. */
+int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double* colw, const double* colo, int k, int metric,
+                      double p, int weights, int R, const double* labels_or_targets, int head, int scalar_out);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
  * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
  * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
@@ -431,6 +465,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_GENERAL_TREES 5      /* explain_tree_kernel: every instance of a tree ensemble (dks_set_tree_model) */
 #define DKS_GENERAL_KMACH 6      /* explain_kmach_kernel: every instance of a kernel machine (dks_set_kernel_machine) */
 #define DKS_GENERAL_MLP 7        /* explain_mlp_kernel: every instance of a multi-layer perceptron (dks_set_mlp) */
+#define DKS_GENERAL_KNN 8        /* explain_knn_kernel: every instance of a nearest-neighbour model (dks_set_knn_model) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
