@@ -651,17 +651,18 @@ def _encoders(step):
     return [step] if isinstance(step, (pp.OneHotEncoder, pp.OrdinalEncoder, pp.KBinsDiscretizer)) else []
 
 
-def compile_encoding(steps, n_raw, n_out):
+def compile_encoding(steps, n_raw, n_out, model="a tree model"):
     """Exact per-column programs (``ColumnEncoding``) of the fitted transformer ``steps`` (applied in order) over
-    ``n_raw`` raw columns, for an estimator reading ``n_out`` encoded columns that compares their values (a tree
-    model).  Accepts what ``compile_maps`` accepts, less its rule that a raw column may not feed both an encoder and a
-    numeric transformer (a sum over columns needs it, a tree does not); refuses encoders whose output dtype is not
-    float64 (a tree would compare rounded values)."""
+    ``n_raw`` raw columns, for an estimator (``model``, as refusals name it) reading ``n_out`` encoded columns: a tree
+    model, which compares their values, or a kernel machine, MLP or neighbour model, which sum over them.  Accepts what
+    ``compile_maps`` accepts, less its rule that a raw column may not feed both an encoder and a numeric transformer
+    (the linear maps need it: they fold every step into one function per raw column; an exact program per encoded
+    column does not); refuses encoders whose output dtype is not float64 (the estimator would read rounded values)."""
     for enc in _encoders_of(steps):
         dt = getattr(enc, "dtype", None)
         if dt is not None and np.dtype(dt) != np.float64:
-            raise TypeError(f"{_name(enc)}(dtype={np.dtype(dt).name}): only float64 encoder output is supported behind a "
-                            "tree model")
+            raise TypeError(f"{_name(enc)}(dtype={np.dtype(dt).name}): only float64 encoder output is supported behind "
+                            f"{model}")
     feats = [_Affine(c, [], [1.0], [0.0], np.nan) for c in range(n_raw)]
     for step in steps:
         feats = _compile_step(step, feats)
@@ -685,7 +686,9 @@ def compile_encoding(steps, n_raw, n_out):
         opvals.append((0.0, 0.0))
         tab.extend(float(k) for k in lk.keys)
         tab.extend(0.0 if v is ERR else float(v) for v in outs + [lk.nan])
-    return ColumnEncoding(n_raw, hdr, ops, opvals, tab)
+    enc = ColumnEncoding(n_raw, hdr, ops, opvals, tab)
+    enc.steps = list(steps)         # what the encoding replays: the engine checks it against their own transform
+    return enc
 
 
 def _encoders_of(steps):

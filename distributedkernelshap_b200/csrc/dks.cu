@@ -212,11 +212,13 @@ HeadDesc describe_head(const dks_ctx* ctx) {
     return h;
 }
 
-// out [n][E] = the column encoding of the raw rows X_dev [n][D] (encode_kernel, grid-stride)
+// out [n][E] = the column encoding of the raw rows X_dev [n][D] (grid-stride): encode_kernel for a tree ensemble,
+// encode_finite_kernel (raw infinities refused) for the families that sum over columns
 int launch_encode(dks_ctx* ctx, const double* X_dev, int n, double* out) {
     const long long total = (long long)n * ctx->enc.E;
     const int grid = (int)std::min<long long>(cdiv(total, 256), (long long)ctx->sm_count * 8);
-    dks::enc::encode_kernel<<<grid, 256, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->enc, out, ctx->d_status);
+    auto kern = ctx->head.trees ? dks::enc::encode_kernel : dks::enc::encode_finite_kernel;
+    kern<<<grid, 256, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->enc, out, ctx->d_status);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     return DKS_OK;
@@ -254,14 +256,21 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     // shared-plan route covers)
     double* xt = (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-    ctx->tree_X = X_dev;
-    ctx->tree_D = ctx->D;
-    if (h.trees && ctx->enc.E > 0) {
-        // a tree behind a column encoding: the tree kernels read the encoded rows (a refused value is reported here)
+    ctx->own_X = X_dev;
+    ctx->own_D = ctx->D;
+    ctx->own_bg = ctx->d_bg;
+    ctx->own_goff = ctx->d_goff;
+    ctx->own_gcols = ctx->d_gcols;
+    if (h.own() && ctx->enc.E > 0) {
+        // a model behind a column encoding: its kernels read the encoded rows, the encoded background and the encoded group
+        // CSR (a refused value is reported here); stage 1 decides the varying groups on the raw rows
         TRY(grow(ctx, &ctx->d_Xenc, &ctx->cap_Xenc, (size_t)n * ctx->enc.E));
         TRY(launch_encode(ctx, X_dev, n, ctx->d_Xenc));
-        ctx->tree_X = ctx->d_Xenc;
-        ctx->tree_D = ctx->enc.E;
+        ctx->own_X = ctx->d_Xenc;
+        ctx->own_D = ctx->enc.E;
+        ctx->own_bg = ctx->d_bg_enc;
+        ctx->own_goff = ctx->d_egoff;
+        ctx->own_gcols = ctx->d_egcols;
     }
     if (h.own()) {
         // tree ensembles, kernel machines, MLPs and neighbour models: prep_kernel decides the varying groups (its scores are those of a zero linear
@@ -272,21 +281,23 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
             ctx->d_linkfnull, n, ctx->N, ctx->D, G, 1, 1, DKS_ACT_IDENTITY, 1.0, ctx->link, ipb, ctx->d_XW,
             ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
             nullptr, 1.0, nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
+        const double* Xo = ctx->own_X;
+        const int Do = ctx->own_D;
         if (h.kmach)
-            dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->km, ctx->C, ctx->link,
+            dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->km, ctx->C, ctx->link,
                                                                                  ctx->d_linkfnull, nullptr, ctx->d_dlink,
                                                                                  ctx->d_status);
         else if (h.mlp)
             dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
-                X_dev, n, ctx->D, ctx->mlp, ctx->C, ctx->link, ctx->d_linkfnull, nullptr, ctx->d_dlink, ctx->d_status);
+                Xo, n, Do, ctx->mlp, ctx->C, ctx->link, ctx->d_linkfnull, nullptr, ctx->d_dlink, ctx->d_status);
         else if (h.knn)
-            dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->knn, ctx->C, ctx->link,
+            dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->knn, ctx->C, ctx->link,
                                                                                ctx->d_linkfnull, nullptr, ctx->d_dlink,
                                                                                ctx->d_status);
         else
-            dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(ctx->tree_X, n, ctx->tree_D, ctx->tree,
-                                                                                   ctx->C, ctx->link, ctx->d_linkfnull,
-                                                                                   nullptr, ctx->d_dlink, ctx->d_status);
+            dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->tree, ctx->C, ctx->link,
+                                                                                   ctx->d_linkfnull, nullptr, ctx->d_dlink,
+                                                                                   ctx->d_status);
         ctx->launches += 1;
     } else {
         kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
@@ -533,21 +544,22 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
         auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->tree_X, ctx->tree_D);
+        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->own_X, ctx->own_D);
     } else if (ctx->head.mlp) {
         auto kern = l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->cur_X, ctx->d_bg, ctx->D,
-                                                    ctx->d_goff, ctx->d_gcols);
+        kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
     } else if (ctx->head.knn) {
         auto kern = l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->cur_X, ctx->d_bg, ctx->D,
-                                                    ctx->d_goff, ctx->d_gcols);
+        kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
     } else {
         auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->cur_X, ctx->d_bg, ctx->D, ctx->d_goff, ctx->d_gcols);
+        kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->own_X, ctx->own_bg, ctx->own_D, ctx->own_goff,
+                                                      ctx->own_gcols);
     }
     ctx->launches += 1;
     return DKS_OK;
@@ -564,6 +576,9 @@ const char* refusal_phrase(bool kmach, bool encoding) {
 }
 // the row named by the status word, refused by the model's family
 int fail_refused(const dks_ctx* ctx, const char* prefix) {
+    if (ctx->enc.E > 0 && (ctx->head.kmach || ctx->head.mlp || ctx->head.knn))
+        return fail(DKS_ERR_DOMAIN, "%s %d holds a raw value the pipeline refuses (NaN where no imputer fills it, an "
+                    "infinity, or a category unseen at fit time), as scikit-learn does", prefix, ctx->h_status[1]);
     if (ctx->head.mlp || ctx->head.knn)
         return fail(DKS_ERR_DOMAIN, "%s %d holds NaN or an infinity: %s refuse it, as scikit-learn does", prefix,
                     ctx->h_status[1], ctx->head.mlp ? "MLPs" : "nearest-neighbour models");
@@ -669,46 +684,95 @@ void free_encoding(dks_ctx* ctx) {
         if (q) cudaFree((void*)q);
     e = EncodingDev{};
     dev_free(&ctx->d_bg_enc);
+    dev_free(&ctx->d_egoff);
+    dev_free(&ctx->d_egcols);
+}
+
+// encoded columns of the column encoding set by dks_set_column_encoding (0: none)
+int encoded_columns(const dks_ctx* ctx) { return (int)(ctx->h_ehdr.size() / 3); }
+// columns a model with its own kernel reads: the encoded ones behind a column encoding, else the raw ones
+int model_columns(const dks_ctx* ctx) { return encoded_columns(ctx) > 0 ? encoded_columns(ctx) : ctx->D; }
+
+// the group of every column the model reads: each raw column's, or behind a column encoding each encoded column's raw
+// source's
+std::vector<int32_t> column_groups(const dks_ctx* ctx) {
+    std::vector<int32_t> colgrp(ctx->D, 0);
+    for (int g = 0; g < ctx->G; ++g)
+        for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
+    const int E = encoded_columns(ctx);
+    if (E == 0) return colgrp;
+    std::vector<int32_t> enc(E);
+    for (int e = 0; e < E; ++e) enc[e] = colgrp[ctx->h_ehdr[3 * e]];
+    return enc;
+}
+
+// the sources of a column encoding are raw columns of the background (which dks_set_background may have changed since)
+int check_encoding_sources(const dks_ctx* ctx) {
+    for (int e = 0; e < encoded_columns(ctx); ++e)
+        if (ctx->h_ehdr[3 * e] >= ctx->D)
+            return fail(DKS_ERR_UNSUPPORTED, "column encoding: encoded column %d reads raw column %d of %d", e,
+                        ctx->h_ehdr[3 * e], ctx->D);
+    return DKS_OK;
+}
+
+// a kernel machine, MLP or neighbour model reads `width` columns: the encoded ones behind a column encoding, else the raw
+// ones
+int check_model_width(const dks_ctx* ctx, int width, const char* family) {
+    TRY(check_encoding_sources(ctx));
+    if (width != model_columns(ctx))
+        return fail(DKS_ERR_UNSUPPORTED, "%s: the model reads %d columns, %s %d", family, width,
+                    encoded_columns(ctx) > 0 ? "the column encoding gives" : "the background has", model_columns(ctx));
+    return DKS_OK;
+}
+
+// dks_fit's column encoding, after fit_begin: the device copy, the encoded background d_bg_enc and the encoded group CSR
+// (group g owns the encoded columns whose raw source is in g, in increasing encoded index).  Without an encoding the
+// previous one is dropped.
+int fit_encoding(dks_ctx* ctx) {
+    free_encoding(ctx);
+    const int E = encoded_columns(ctx), G = ctx->G;
+    if (E == 0) return DKS_OK;
+    const cudaStream_t st = ctx->stream;
+    EncodingDev& en = ctx->enc;
+    TRY(upload_tree_array(&en.hdr, ctx->h_ehdr.data(), ctx->h_ehdr.size(), st));
+    TRY(upload_tree_array(&en.ops, ctx->h_eops.data(), ctx->h_eops.size(), st));
+    TRY(upload_tree_array(&en.opv, ctx->h_eopv.data(), ctx->h_eopv.size(), st));
+    TRY(upload_tree_array(&en.tab, ctx->h_etab.data(), ctx->h_etab.size(), st));
+    en.E = E;
+    TRY(dev_alloc(&ctx->d_bg_enc, (size_t)ctx->N * E));
+    TRY(launch_encode(ctx, ctx->d_bg, ctx->N, ctx->d_bg_enc));
+    const std::vector<int32_t> colgrp = column_groups(ctx);
+    std::vector<int32_t> goff(G + 1, 0), gcols(E);
+    for (int e = 0; e < E; ++e) goff[colgrp[e] + 1] += 1;
+    for (int g = 0; g < G; ++g) goff[g + 1] += goff[g];
+    std::vector<int32_t> at(goff.begin(), goff.end() - 1);
+    for (int e = 0; e < E; ++e) gcols[at[colgrp[e]]++] = e;
+    TRY(dev_alloc(&ctx->d_egoff, (size_t)G + 1));
+    TRY(dev_alloc(&ctx->d_egcols, (size_t)E));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_egoff, goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_egcols, gcols.data(), sizeof(int32_t) * E, cudaMemcpyHostToDevice, st));
+    return DKS_OK;
 }
 
 // dks_fit of a tree ensemble: the node arrays, the group of every column, every background row's direction at every node,
 // the column statistics stage 1 decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the tree kernels
 int fit_trees(dks_ctx* ctx) {
-    const int N = ctx->N, D = ctx->D, G = ctx->G, C = ctx->C;
+    const int N = ctx->N, C = ctx->C;
     const cudaStream_t st = ctx->stream;
     TreeDev& t = ctx->tree;
     const size_t nodes = (size_t)t.nodes;
     // a column encoding: the tree reads E encoded columns, each in the group of its raw source
-    const int E = ctx->h_ehdr.empty() ? 0 : (int)(ctx->h_ehdr.size() / 3);
-    const int width = E > 0 ? E : D;
-    for (int e = 0; e < E; ++e)
-        if (ctx->h_ehdr[3 * e] >= D)
-            return fail(DKS_ERR_UNSUPPORTED, "column encoding: encoded column %d reads raw column %d of %d", e,
-                        ctx->h_ehdr[3 * e], D);
+    const int E = encoded_columns(ctx);
+    const int width = model_columns(ctx);
+    TRY(check_encoding_sources(ctx));
     for (int32_t f : ctx->h_tfeat)
         if (f >= width)
             return fail(DKS_ERR_UNSUPPORTED, "tree ensemble: a split reads column %d of %d %s", f, width,
                         E > 0 ? "encoded columns" : "columns");
     TRY(fit_begin(ctx));
-    std::vector<int32_t> colgrp(D, 0);
-    for (int g = 0; g < G; ++g)
-        for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
-    if (E > 0) {
-        std::vector<int32_t> raw = colgrp;
-        colgrp.assign(E, 0);
-        for (int e = 0; e < E; ++e) colgrp[e] = raw[ctx->h_ehdr[3 * e]];
-    }
+    const std::vector<int32_t> colgrp = column_groups(ctx);
     free_tree(ctx);
-    free_encoding(ctx);
-    if (E > 0) {
-        EncodingDev& en = ctx->enc;
-        TRY(upload_tree_array(&en.hdr, ctx->h_ehdr.data(), ctx->h_ehdr.size(), st));
-        TRY(upload_tree_array(&en.ops, ctx->h_eops.data(), ctx->h_eops.size(), st));
-        TRY(upload_tree_array(&en.opv, ctx->h_eopv.data(), ctx->h_eopv.size(), st));
-        TRY(upload_tree_array(&en.tab, ctx->h_etab.data(), ctx->h_etab.size(), st));
-        en.E = E;
-        TRY(dev_alloc(&ctx->d_bg_enc, (size_t)N * E));
-    }
+    TRY(fit_encoding(ctx));
     TRY(upload_tree_array(&t.feat, ctx->h_tfeat.data(), nodes, st));
     TRY(upload_tree_array(&t.thr, ctx->h_tthr.data(), nodes, st));
     TRY(upload_tree_array(&t.left, ctx->h_tleft.data(), nodes, st));
@@ -723,11 +787,7 @@ int fit_trees(dks_ctx* ctx) {
     t.bgdir = bgdir;
     double* pred = nullptr;
     TRY(dev_alloc(&pred, (size_t)N * C));
-    const double* tbg = ctx->d_bg;
-    if (E > 0) {
-        TRY(launch_encode(ctx, ctx->d_bg, N, ctx->d_bg_enc));
-        tbg = ctx->d_bg_enc;
-    }
+    const double* tbg = E > 0 ? ctx->d_bg_enc : ctx->d_bg;
     dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, st>>>(tbg, N, width, t, bgdir);
     dks::trees::tree_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(tbg, N, width, t, C, ctx->link, nullptr, pred, nullptr,
                                                                   nullptr);
@@ -749,10 +809,14 @@ void free_kmach(dks_ctx* ctx) {
 // dks_fit of a kernel machine: the arrays, T[j][v] of every background row and support vector, the column statistics stage 1
 // decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the kernel-machine kernels
 int fit_kmach(dks_ctx* ctx) {
-    const int N = ctx->N, D = ctx->D, C = ctx->C;
+    const int N = ctx->N, C = ctx->C;
     const cudaStream_t st = ctx->stream;
     KmDev& k = ctx->km;
+    const int D = (int)(ctx->h_kcolw.size() / k.K);   // the raw columns, or the encoded ones behind a column encoding
+    TRY(check_model_width(ctx, D, "kernel machine"));
     TRY(fit_begin(ctx));
+    TRY(fit_encoding(ctx));
+    const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
     free_kmach(ctx);
     TRY(upload_tree_array(&k.sv, ctx->h_ksv.data(), ctx->h_ksv.size(), st));
     TRY(upload_tree_array(&k.dual, ctx->h_kdual.data(), ctx->h_kdual.size(), st));
@@ -763,8 +827,8 @@ int fit_kmach(dks_ctx* ctx) {
     k.Tbg = Tbg;
     double* pred = nullptr;
     TRY(dev_alloc(&pred, (size_t)N * C));
-    dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(ctx->d_bg, N, D, k, Tbg);
-    dks::kmach::km_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(ctx->d_bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
+    dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(bg, N, D, k, Tbg);
+    dks::kmach::km_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
                                                                 ctx->d_status);
     dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
     ctx->launches += 3;
@@ -784,10 +848,14 @@ void free_mlp(dks_ctx* ctx) {
 // dks_fit of an MLP: the layers, B[j] = b_0 + bg_j W_0 of every background row, the column statistics stage 1 decides the
 // varying groups with, and fnull = sum_j w_j f(bg_j) from the MLP kernels
 int fit_mlp(dks_ctx* ctx) {
-    const int N = ctx->N, D = ctx->D, C = ctx->C;
+    const int N = ctx->N, C = ctx->C;
     const cudaStream_t st = ctx->stream;
     MlpDev& m = ctx->mlp;
+    const int D = m.width[0];                       // the raw columns, or the encoded ones behind a column encoding
+    TRY(check_model_width(ctx, D, "MLP"));
     TRY(fit_begin(ctx));
+    TRY(fit_encoding(ctx));
+    const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
     free_mlp(ctx);
     TRY(upload_tree_array(&m.W, ctx->h_mw.data(), ctx->h_mw.size(), st));
     TRY(upload_tree_array(&m.b, ctx->h_mb.data(), ctx->h_mb.size(), st));
@@ -798,9 +866,9 @@ int fit_mlp(dks_ctx* ctx) {
     m.Bbg = Bbg;
     double* pred = nullptr;
     TRY(dev_alloc(&pred, (size_t)N * C));
-    dks::mlp::mlp_fit_table_kernel<<<cdiv((long long)N * m.width[1], 256), 256, 0, st>>>(ctx->d_bg, N, D, m, Bbg);
-    dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, N), dks::mlp::THREADS, 0, st>>>(ctx->d_bg, N, D, m, C, ctx->link,
-                                                                                       nullptr, pred, nullptr, ctx->d_status);
+    dks::mlp::mlp_fit_table_kernel<<<cdiv((long long)N * m.width[1], 256), 256, 0, st>>>(bg, N, D, m, Bbg);
+    dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, N), dks::mlp::THREADS, 0, st>>>(bg, N, D, m, C, ctx->link, nullptr,
+                                                                                       pred, nullptr, ctx->d_status);
     dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
     ctx->launches += 3;
     const int rc = fit_readback(ctx, "MLP");
@@ -821,13 +889,15 @@ void free_knn(dks_ctx* ctx) {
 // every background row and training row, the column statistics stage 1 decides the varying groups with, and
 // fnull = sum_j w_j f(bg_j) from the neighbour kernels
 int fit_knn(dks_ctx* ctx) {
-    const int N = ctx->N, D = ctx->D, G = ctx->G, C = ctx->C;
+    const int N = ctx->N, G = ctx->G, C = ctx->C;
     const cudaStream_t st = ctx->stream;
     KnnDev& k = ctx->knn;
+    const int D = (int)ctx->h_ncolw.size();         // the raw columns, or the encoded ones behind a column encoding
+    TRY(check_model_width(ctx, D, "nearest-neighbour model"));
     TRY(fit_begin(ctx));
-    std::vector<int32_t> colgrp(D, 0);
-    for (int g = 0; g < G; ++g)
-        for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
+    TRY(fit_encoding(ctx));
+    const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
+    const std::vector<int32_t> colgrp = column_groups(ctx);
     free_knn(ctx);
     TRY(upload_tree_array(&k.fitX, ctx->h_nfitX.data(), ctx->h_nfitX.size(), st));
     TRY(upload_tree_array(&k.colw, ctx->h_ncolw.data(), ctx->h_ncolw.size(), st));
@@ -842,8 +912,8 @@ int fit_knn(dks_ctx* ctx) {
     k.Ebg = Ebg;
     double* pred = nullptr;
     TRY(dev_alloc(&pred, (size_t)N * C));
-    dks::knn::knn_fit_table_kernel<<<cdiv((long long)N * k.n_fit, 256), 256, 0, st>>>(ctx->d_bg, N, D, G, k, Tbg, Ebg);
-    dks::knn::knn_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(ctx->d_bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
+    dks::knn::knn_fit_table_kernel<<<cdiv((long long)N * k.n_fit, 256), 256, 0, st>>>(bg, N, D, G, k, Tbg, Ebg);
+    dks::knn::knn_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
                                                                ctx->d_status);
     dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
     ctx->launches += 3;
@@ -1790,7 +1860,7 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
     case DKS_TREE_HEAD_EXP: REQUIRE(R == 1, "exp tree head needs R == 1 (got %d)", R); C = 1; break;
     default: return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: unknown head %d", head);
     }
-    const int width = ctx->h_ehdr.empty() ? ctx->D : (int)(ctx->h_ehdr.size() / 3);   // encoded columns, if any
+    const int width = model_columns(ctx);
     for (int nd = 0; nd < n_nodes; ++nd) {
         const int f = feature[nd];
         if (f < 0) {
@@ -1834,7 +1904,7 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
     REQUIRE(ctx->D > 0, "dks_set_kernel_machine: call dks_set_background first (D unknown)");
     REQUIRE(sv_off && sv && dual && intercept && colw && colo && gamma,
             "dks_set_kernel_machine: need the support vectors, dual coefficients, intercepts, column weights and gamma");
-    const int D = ctx->D;
+    const int D = model_columns(ctx);
     auto finite = [](const double* a, size_t n) {
         for (size_t e = 0; e < n; ++e) if (!std::isfinite(a[e])) return false;
         return true;
@@ -1897,8 +1967,7 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
     // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
     ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_KMACH; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
     ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
-    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
-    ctx->h_W.assign((size_t)D, 0.0);
+    ctx->h_W.assign((size_t)ctx->D, 0.0);
     ctx->h_b.assign(1, 0.0);
     ctx->fitted = false;
     return DKS_OK;
@@ -1909,12 +1978,13 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
     BIND(ctx);
     REQUIRE(ctx->D > 0, "dks_set_mlp: call dks_set_background first (D unknown)");
     REQUIRE(widths && W_host && b_host, "dks_set_mlp: need the widths, weights and biases");
-    const int D = ctx->D;
+    const int E = encoded_columns(ctx), D = model_columns(ctx);
     if (n_hidden < 1 || n_hidden > DKS_MLP_MAX_HIDDEN)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: %d hidden layers; 1..%d supported", n_hidden, DKS_MLP_MAX_HIDDEN);
     const int L = n_hidden + 1, R = widths[L];
     if (widths[0] != D)
-        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the first layer reads %d columns, the background has %d", widths[0], D);
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the first layer reads %d columns, the %s has %d", widths[0],
+                    E > 0 ? "column encoding" : "background", D);
     for (int l = 1; l < L; ++l)
         if (widths[l] < 1 || widths[l] > DKS_MLP_MAX_WIDTH)
             return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: hidden layer %d has %d units; 1..%d supported", l, widths[l],
@@ -1981,8 +2051,7 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
     // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
     ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_MLP; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
     ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
-    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
-    ctx->h_W.assign((size_t)D, 0.0);
+    ctx->h_W.assign((size_t)ctx->D, 0.0);
     ctx->h_b.assign(1, 0.0);
     ctx->fitted = false;
     return DKS_OK;
@@ -1993,7 +2062,7 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
     BIND(ctx);
     REQUIRE(ctx->D > 0, "dks_set_knn_model: call dks_set_background first (D unknown)");
     REQUIRE(fitX && colw && colo && labels_or_targets, "dks_set_knn_model: need the training rows, column map and labels");
-    const int D = ctx->D;
+    const int D = model_columns(ctx);
     auto finite = [](const double* a, size_t n) {
         for (size_t e = 0; e < n; ++e) if (!std::isfinite(a[e])) return false;
         return true;
@@ -2034,8 +2103,7 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
     // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
     ctx->R = 1; ctx->C = R; ctx->act = DKS_ACT_KNN; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
     ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
-    ctx->h_ehdr.clear(); ctx->h_eops.clear(); ctx->h_eopv.clear(); ctx->h_etab.clear();
-    ctx->h_W.assign((size_t)D, 0.0);
+    ctx->h_W.assign((size_t)ctx->D, 0.0);
     ctx->h_b.assign(1, 0.0);
     ctx->fitted = false;
     return DKS_OK;
@@ -2097,7 +2165,8 @@ int dks_set_column_encoding(dks_ctx* ctx, int E, const int32_t* hdr_host, const 
         return DKS_OK;
     }
     REQUIRE(ctx->D > 0, "dks_set_column_encoding: call dks_set_background first (D unknown)");
-    if (ctx->act >= 0 && ctx->act != DKS_ACT_TREES)
+    if (ctx->act >= 0 && ctx->act != DKS_ACT_TREES && ctx->act != DKS_ACT_KMACH && ctx->act != DKS_ACT_MLP &&
+        ctx->act != DKS_ACT_KNN)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: for tree ensembles only (linear models read their "
                     "pipelines through dks_set_column_maps)");
     if (E < 1 || n_ops < 0 || n_tab < 0 || (n_ops > 0 && (!ops_host || !opvals_host)) || (n_tab > 0 && !tab_host))
@@ -2154,7 +2223,8 @@ int dks_encode_host(dks_ctx* ctx, const double* X_host, int n, double* out_host)
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     cudaFree(dX); cudaFree(dO);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return fail(DKS_ERR_DOMAIN, "row %d %s", ctx->h_status[1], refusal_phrase(false, true));
+        return ctx->head.own() ? fail_refused(ctx, "row")
+                               : fail(DKS_ERR_DOMAIN, "row %d %s", ctx->h_status[1], refusal_phrase(false, true));
     return DKS_OK;
 }
 
@@ -2193,7 +2263,7 @@ int dks_fit(dks_ctx* ctx) {
             REQUIRE(seen[c]++ == 0, "column %d appears in more than one group", c);
         }
     }
-    if (!h.trees && !ctx->h_ehdr.empty())
+    if (!h.own() && !ctx->h_ehdr.empty())
         return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model is not a tree ensemble");
     if (h.trees) return fit_trees(ctx);
     if (h.kmach) return fit_kmach(ctx);
@@ -2278,23 +2348,25 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     TRY(dev_alloc(&dO, (size_t)n * ctx->C));
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
+    // a model with its own kernel behind a column encoding reads the encoded rows
     double* dXe = nullptr;
-    if (ctx->head.trees && ctx->enc.E > 0) {
+    if (ctx->head.own() && ctx->enc.E > 0) {
         TRY(dev_alloc(&dXe, (size_t)n * ctx->enc.E));
         TRY(launch_encode(ctx, dX, n, dXe));
     }
+    const double* Xo = dXe ? dXe : dX;
+    const int Do = dXe ? ctx->enc.E : ctx->D;
     if (ctx->head.trees)
-        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dXe ? dXe : dX, n, dXe ? ctx->enc.E : ctx->D,
-                                                                               ctx->tree, ctx->C, ctx->link, nullptr, dO,
-                                                                               nullptr, nullptr);
+        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->tree, ctx->C, ctx->link,
+                                                                               nullptr, dO, nullptr, nullptr);
     else if (ctx->head.kmach)
-        dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->km, ctx->C, ctx->link,
+        dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->km, ctx->C, ctx->link,
                                                                              nullptr, dO, nullptr, ctx->d_status);
     else if (ctx->head.mlp)
         dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
-            dX, n, ctx->D, ctx->mlp, ctx->C, ctx->link, nullptr, dO, nullptr, ctx->d_status);
+            Xo, n, Do, ctx->mlp, ctx->C, ctx->link, nullptr, dO, nullptr, ctx->d_status);
     else if (ctx->head.knn)
-        dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(dX, n, ctx->D, ctx->knn, ctx->C, ctx->link,
+        dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->knn, ctx->C, ctx->link,
                                                                            nullptr, dO, nullptr, ctx->d_status);
     else
         (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(

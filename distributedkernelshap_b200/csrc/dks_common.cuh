@@ -160,8 +160,8 @@ struct TreeDev {
     int nodes, T, R, head, cmp;
 };
 
-// column encoding of a tree ensemble (dks_set_column_encoding, DESIGN.md §5.0.13): E encoded columns, each a program of
-// DKS_ENC_OP_* over one raw column (dks_encode.cuh)
+// column encoding of a model with its own kernel (dks_set_column_encoding, DESIGN.md §5.0.13, §5.0.16): E encoded columns,
+// each a program of DKS_ENC_OP_* over one raw column (dks_encode.cuh)
 struct EncodingDev {
     const int* hdr;              // [E][3] {raw source column, first op, op count}
     const int* ops;              // [n_ops][4] {code, flags, m, table offset}
@@ -297,16 +297,21 @@ struct dks_ctx {
     std::vector<unsigned char> h_tmiss;
     TreeDev tree = {};
     size_t cap_txinfo = 0;
-    // its column encoding (dks_set_column_encoding; empty h_ehdr: none), the device copy dks_fit builds, the encoded
-    // background and the encoded rows of the current call
+    // the column encoding of a model with its own kernel (dks_set_column_encoding; empty h_ehdr: none), the device copy
+    // dks_fit builds, the encoded background, the encoded group CSR and the encoded rows of the current call
     std::vector<int32_t> h_ehdr, h_eops;
     std::vector<double> h_eopv, h_etab;
     EncodingDev enc = {};
     double* d_bg_enc = nullptr;  // [N][E]
+    int32_t *d_egoff = nullptr, *d_egcols = nullptr;   // [G + 1], [E]: group g owns the encoded columns of its raw ones
     double* d_Xenc = nullptr;    // [n][E]
     size_t cap_Xenc = 0;
-    const double* tree_X = nullptr;   // rows the tree kernels of the current call read (d_Xenc, or the raw rows) ...
-    int tree_D = 0;                   // ... and their width
+    // what the family's own kernels of the current call read: the rows (d_Xenc, or the raw rows), their width, the
+    // background and the group CSR over those columns
+    const double* own_X = nullptr;
+    int own_D = 0;
+    const double* own_bg = nullptr;
+    const int32_t *own_goff = nullptr, *own_gcols = nullptr;
     // kernel machine (act == DKS_ACT_KMACH): host copies of the arrays, and their device copies built by dks_fit
     std::vector<double> h_ksv, h_kdual, h_kcolw, h_kcolo;
     KmDev km = {};

@@ -1,5 +1,5 @@
-// Column encodings (dks_set_column_encoding, DESIGN.md §5.0.13): a tree ensemble behind a scikit-learn Pipeline of
-// per-column steps reads encoded columns, each an exact program over one raw column.  encode_kernel replays the programs on
+// Column encodings (dks_set_column_encoding, DESIGN.md §5.0.13, §5.0.16): a tree ensemble, kernel machine, MLP or neighbour
+// model behind a scikit-learn Pipeline of per-column steps reads encoded columns, each an exact program over one raw column.  encode_kernel replays the programs on
 // raw rows, bit for bit what pipe[:-1].transform gives: the scalers' arithmetic is rounded op by op (__d*_rn: nvcc would
 // otherwise contract x * s + o into one fused multiply-add, which numpy does not), the clip keeps NaN as np.clip does, and
 // the lookups are exact binary searches over float64 keys.
@@ -94,6 +94,23 @@ __global__ void encode_kernel(const double* __restrict__ X, int n, int D, Encodi
         const int* h = e.hdr + 3 * (size_t)c;
         bool refused = false;
         Xe[idx] = encode_value(e, h[1], h[2], X[(size_t)i * D + h[0]], &refused);
+        if (refused && atomicCAS(&status[0], 0, DKS_ERR_DOMAIN) == 0) status[1] = i;
+    }
+}
+
+// encode_kernel for the models that sum over their columns (kernel machines, MLPs, neighbour models; DESIGN.md §5.0.16): a
+// raw infinity that any encoded column reads is refused as well.  Every scikit-learn transformer refuses one, and so do
+// these estimators when a column passes through to them.
+__global__ void encode_finite_kernel(const double* __restrict__ X, int n, int D, EncodingDev e, double* __restrict__ Xe,
+                                     int* __restrict__ status) {
+    const long long total = (long long)n * e.E;
+    for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int i = (int)(idx / e.E), c = (int)(idx - (long long)i * e.E);
+        const int* h = e.hdr + 3 * (size_t)c;
+        const double x = X[(size_t)i * D + h[0]];
+        bool refused = isinf(x);
+        Xe[idx] = encode_value(e, h[1], h[2], x, &refused);
         if (refused && atomicCAS(&status[0], 0, DKS_ERR_DOMAIN) == 0) status[1] = i;
     }
 }

@@ -19,7 +19,8 @@ from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, extract_kernel_mach
 from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, extract_mlp_spec
 from .neighbors import MAX_GROUPS as KNN_MAX_GROUPS, extract_knn_spec
 from .predictors import extract_linear_spec
-from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_tree_pipeline_spec, extract_tree_spec
+from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_encoded_pipeline_spec, extract_tree_pipeline_spec, \
+    extract_tree_spec
 
 logger = logging.getLogger(__name__)
 
@@ -29,7 +30,7 @@ MAX_ROWS_PER_CALL = 65536     # rows per C-ABI call: bounds the engine's per-cal
 # (M-1) x (M-1) normal matrix: about 222 KB at M = 128, S = 4096.  Row blocks of 4096 bound that workspace by ~0.9 GB.
 MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE = 4096
 MAX_SAMPLED_SIZES = 64        # subset sizes the device sampler draws from (csrc/dks_sampler.cuh, MAX_SIZES)
-# a tree behind a column encoding keeps the encoded rows of a call on the device (n x E x 8 B): row blocks bound them
+# a model behind a column encoding keeps the encoded rows of a call on the device (n x E x 8 B): row blocks bound them
 MAX_ENCODED_BYTES_PER_CALL = 256 << 20
 
 
@@ -137,9 +138,10 @@ class GpuKernelExplainer:
         model or of a ``Pipeline`` of per-column preprocessing ending in one (explained in raw feature space), or a
         ``LinearModelSpec`` (see ``predictors.extract_linear_spec``); a tree model, bare or behind such a ``Pipeline``
         (``trees.extract_tree_pipeline_spec``: the device replays the steps bit for bit); a kernel machine; a
-        scikit-learn MLP (``mlp.extract_mlp_spec``); a k-nearest-neighbour model (``neighbors.extract_knn_spec``).  A raw
-        value the pipeline would refuse (NaN, or an unseen category under ``handle_unknown='error'``) raises
-        ``ValueError``.
+        scikit-learn MLP (``mlp.extract_mlp_spec``); a k-nearest-neighbour model (``neighbors.extract_knn_spec``); each of
+        the last three bare, behind affine scalers (folded into the model) or behind such a ``Pipeline``
+        (``trees.extract_encoded_pipeline_spec``, replayed like a tree's).  A raw value the pipeline would refuse (NaN,
+        or an unseen category under ``handle_unknown='error'``) raises ``ValueError``.
     data
         Background data: array, DataFrame or ``DenseData`` (groups and weights honoured).
     link
@@ -165,11 +167,15 @@ class GpuKernelExplainer:
         self.link = convert_to_link(link)
         self.model_callable = model
         pipe_spec = extract_tree_pipeline_spec(model)
-        # a tree behind per-column preprocessing: explained in raw feature space, the device replaying the steps
-        tree_spec, self.encoding = pipe_spec if pipe_spec is not None else (extract_tree_spec(model), None)
-        km_spec = extract_kernel_machine_spec(model) if tree_spec is None else None
-        mlp_spec = extract_mlp_spec(model) if tree_spec is None and km_spec is None else None
-        knn_spec = extract_knn_spec(model) if tree_spec is None and km_spec is None and mlp_spec is None else None
+        if pipe_spec is None:
+            pipe_spec = extract_encoded_pipeline_spec(model)
+        # a model behind per-column preprocessing: explained in raw feature space, the device replaying the steps; the
+        # extractors below pass its spec through
+        target, self.encoding = pipe_spec if pipe_spec is not None else (model, None)
+        tree_spec = extract_tree_spec(target)
+        km_spec = extract_kernel_machine_spec(target) if tree_spec is None else None
+        mlp_spec = extract_mlp_spec(target) if tree_spec is None and km_spec is None else None
+        knn_spec = extract_knn_spec(target) if tree_spec is None and km_spec is None and mlp_spec is None else None
         own = next((s for s in (tree_spec, km_spec, mlp_spec, knn_spec) if s is not None), None)   # its own kernel
         self.spec = own if own is not None else extract_linear_spec(model)
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
@@ -215,6 +221,10 @@ class GpuKernelExplainer:
                                       f"{KNN_MAX_GROUPS} groups")
         W = None if own is not None else \
             self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
+        e = self.encoding
+        if e is not None:               # before the model: its columns are the encoded ones
+            _cabi.check(self.lib.dks_set_column_encoding(self._ctx, e.E, _cabi.ptr(e.hdr), _cabi.ptr(e.ops),
+                                                         _cabi.ptr(e.opvals), len(e.ops), _cabi.ptr(e.tab), len(e.tab)))
         if knn_spec is not None:
             k = knn_spec
             _cabi.check(self.lib.dks_set_knn_model(
@@ -231,10 +241,7 @@ class GpuKernelExplainer:
                 _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree, k.coef0, k.head_code,
                 _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
         elif tree_spec is not None:
-            t, e = tree_spec, self.encoding
-            if e is not None:
-                _cabi.check(self.lib.dks_set_column_encoding(self._ctx, e.E, _cabi.ptr(e.hdr), _cabi.ptr(e.ops),
-                                                             _cabi.ptr(e.opvals), len(e.ops), _cabi.ptr(e.tab), len(e.tab)))
+            t = tree_spec
             _cabi.check(self.lib.dks_set_tree_model(
                 self._ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
                 _cabi.ptr(t.missing_left), _cabi.ptr(t.value), t.R, t.n_trees, _cabi.ptr(t.roots), _cabi.ptr(t.base),
@@ -277,9 +284,9 @@ class GpuKernelExplainer:
     # ------------------------------------------------------------------------------------------------------
     def encode(self, X):
         """The encoded rows ``pipe[:-1].transform(X)`` [n, E] as the device computes them (``dks_encode_host``), for a
-        tree behind a column encoding."""
+        model behind a column encoding."""
         if self.encoding is None:
-            raise TypeError("the model has no column encoding (not a tree behind a Pipeline)")
+            raise TypeError("the model has no column encoding (not a model behind a Pipeline of per-column steps)")
         X = np.ascontiguousarray(np.atleast_2d(np.asarray(X, dtype=np.float64)))
         out = np.zeros((X.shape[0], self.encoding.E))
         _cabi.check(self.lib.dks_encode_host(self._ctx, _cabi.ptr(X), X.shape[0], _cabi.ptr(out)))
@@ -288,11 +295,10 @@ class GpuKernelExplainer:
     def _check_encoding(self, bg):
         """The device's encoding of the background must be what the pipeline's own steps give, bit for bit."""
         import warnings
-        from .column_maps import pipeline_parts
         want = bg
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
-            for step in pipeline_parts(self.model_callable.__self__)[0]:
+            for step in self.encoding.steps:
                 want = step.transform(want)
         if hasattr(want, "toarray"):
             want = want.toarray()
@@ -315,6 +321,8 @@ class GpuKernelExplainer:
         want = np.asarray(self.model_callable(bg), dtype=np.float64).reshape(self.N, -1)
         got = self.predict(bg)
         if knn_spec is not None and want.shape == got.shape:
+            if self.encoding is not None:
+                bg = self.encode(bg)    # the spec reads the encoded columns
             tied = knn_spec.boundary_ties(bg)
             if tied.all():
                 raise ValueError("every background row has a tie between its k-th and (k + 1)-th nearest training rows: "

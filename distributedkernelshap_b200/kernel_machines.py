@@ -265,7 +265,9 @@ def _svc_binary(est, what):
                                   "evaluates; only two classes are supported")
 
 
-def _calibrated_spec(owner, method, P):
+def _calibrated_spec(owner, method, P, bare=False):
+    """The calibrated head over the members' kernel machines; ``bare``: each member is read as its final estimator, its
+    pipeline's steps being replayed in front of it (``trees.extract_encoded_pipeline_spec``)."""
     if method != "predict_proba":
         raise TypeError(f"CalibratedClassifierCV.{method} is not supported: pass predict_proba")
     if len(owner.classes_) != 2:
@@ -280,7 +282,7 @@ def _calibrated_spec(owner, method, P):
             raise NotImplementedError(f"CalibratedClassifierCV over {type(_final(cc.estimator)).__name__}: the kernel-"
                                       "machine route calibrates SVC and NuSVC only")
         _svc_binary(cc.estimator, type(_final(cc.estimator)).__name__)
-        params, V, dual, icpt, colw, colo = _member(cc.estimator, P)
+        params, V, dual, icpt, colw, colo = _member(_final(cc.estimator) if bare else cc.estimator, P)
         cal = cc.calibrators[0]
         members.append((params, V, dual, icpt, colw, colo, float(cal.a_), float(cal.b_)))
     kinds = {m[0][0] for m in members}

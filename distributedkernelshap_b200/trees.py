@@ -320,3 +320,76 @@ def extract_tree_pipeline_spec(predictor):
     enc = compile_encoding(pre, int(owner.n_features_in_), spec.n_features)
     spec.n_features = enc.D
     return spec, enc
+
+
+def _foldable(step):
+    """A step ``kernel_machines._unwrap`` folds into the model: one of the four affine scalers (``MinMaxScaler``
+    without ``clip``), or no step."""
+    from .kernel_machines import _SCALERS
+    if step is None or isinstance(step, str):
+        return True
+    return type(step).__name__ in _SCALERS and not (type(step).__name__ == "MinMaxScaler" and step.clip)
+
+
+def extract_encoded_pipeline_spec(predictor):
+    """``(spec, ColumnEncoding)`` of a bound method of a fitted ``Pipeline`` of per-column steps ending in a kernel
+    machine (``extract_kernel_machine_spec``, the sigmoid-calibrated SVC included), an MLP (``extract_mlp_spec``) or a
+    k-nearest-neighbour model (``extract_knn_spec``), when some step is not one of the four affine scalers those
+    extractors fold: the spec of the bare final estimator (its columns are the encoded ones, ``colw = 1`` and
+    ``colo = 0``) and the exact programs of the steps (``column_maps.compile_encoding``).  A
+    ``CalibratedClassifierCV(ensemble=False)`` whose one fold is such a pipeline counts as one.  ``None`` for anything
+    else, scaler-only pipelines included (the extractors fold those).  Raises ``NotImplementedError`` naming the step
+    for steps the encoding refuses and for calibrated ensembles whose folds each hold their own fitted preprocessing; the
+    final estimator's own refusals raise as in its extractor."""
+    from .column_maps import compile_encoding, pipeline_parts
+    from .kernel_machines import _calibrated_spec, _final, _is_kernel_machine, extract_kernel_machine_spec
+    from .mlp import _MLPS, extract_mlp_spec
+    from .neighbors import _KNN, extract_knn_spec
+    owner = getattr(predictor, "__self__", None)
+    method = getattr(predictor, "__name__", None)
+    if owner is None:
+        return None
+    pre, final = pipeline_parts(owner) if "Pipeline" in _names(owner) and hasattr(owner, "steps") else ([], owner)
+    names = _names(final)
+    inner = False                   # the preprocessing of a single calibrated fold is compiled too
+    if "CalibratedClassifierCV" in names:
+        ccs = getattr(final, "calibrated_classifiers_", None)
+        if not ccs or not any(_is_kernel_machine(cc.estimator) for cc in ccs):
+            return None
+        family, extract = "a kernel machine", extract_kernel_machine_spec
+        folds = [pipeline_parts(cc.estimator)[0] if "Pipeline" in _names(cc.estimator) else [] for cc in ccs]
+        steps = [type(s).__name__ for s in folds[0] if not _foldable(s)]
+        if any(not _foldable(s) for f in folds for s in f):
+            if len(ccs) > 1:
+                raise NotImplementedError(
+                    f"CalibratedClassifierCV with {len(ccs)} folds, each with its own fitted preprocessing "
+                    f"({', '.join(steps)}): the device holds one column encoding; move the preprocessing in front of "
+                    "the calibrator (make_pipeline(preprocessing, CalibratedClassifierCV(...))) or pass ensemble=False")
+            pre, inner = pre + folds[0], True
+    elif _is_kernel_machine(final):
+        family, extract = "a kernel machine", extract_kernel_machine_spec
+    elif names & _MLPS:
+        family, extract = "an MLP", extract_mlp_spec
+    elif names & _KNN:
+        family, extract = "a neighbour model", extract_knn_spec
+    else:
+        return None
+    if all(_foldable(s) for s in pre):
+        return None
+    if not hasattr(owner, "n_features_in_"):
+        raise TypeError("Pipeline is not fitted")
+    if inner:
+        bare = _final(final.calibrated_classifiers_[0].estimator)
+        if not hasattr(bare, "n_features_in_"):
+            raise TypeError(f"{type(bare).__name__} is not fitted")
+        spec = _calibrated_spec(final, method, int(bare.n_features_in_), bare=True)
+    else:
+        spec = extract(getattr(final, method))
+    if spec is None:
+        return None
+    try:
+        enc = compile_encoding(pre, int(owner.n_features_in_), spec.n_features, model=family)
+    except TypeError as e:
+        raise NotImplementedError(f"Pipeline in front of {family}: {e}") from e
+    spec.n_features = enc.D
+    return spec, enc

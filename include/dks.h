@@ -206,7 +206,8 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
  * are DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route.  Float64 throughout.  NaN in a background
  * row (dks_fit) or an instance (dks_predict_host, the explain calls) is DKS_ERR_DOMAIN with the row; a link(ey) or
  * link(f(x)) that is not finite is DKS_ERR_NUMERIC and nothing non-finite is written into phi.  Shapes whose per-instance
- * buffers do not fit shared memory are DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused. */
+ * buffers do not fit shared memory are DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused.  With a column encoding set
+ * (dks_set_column_encoding) D is its E encoded columns. */
 int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const double* sv, const double* dual, int R,
                            const double* intercept, const double* colw, const double* colo, const double* gamma, int kernel,
                            double degree, double coef0, int head, const double* cal_a, const double* cal_b,
@@ -223,7 +224,7 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
  * tensor cores.  NaN or an infinity in a background row (dks_fit) or an instance (dks_predict_host, the explain calls) is
  * DKS_ERR_DOMAIN with the row; a link(ey) or link(f(x)) that is not finite is DKS_ERR_NUMERIC and nothing non-finite is
  * written into phi.  Shapes whose per-instance buffers do not fit shared memory are DKS_ERR_UNSUPPORTED.
- * dks_set_column_maps is refused. */
+ * dks_set_column_maps is refused.  With a column encoding set (dks_set_column_encoding) widths[0] is its E encoded columns. */
 int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double* W_host, const double* b_host, int activation,
                 int head, int scalar_out);
 /* k-nearest-neighbour model (DKS_ACT_KNN) in place of dks_set_model: n_fit >= k training rows fitX [n_fit][D] row-major in
@@ -241,7 +242,8 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
  * throughout.  NaN or an infinity in a background row (dks_fit) or an instance (dks_predict_host, the explain calls) is
  * DKS_ERR_DOMAIN with the row; a link(ey) or link(f(x)) that is not finite (the logit of a probability of exactly 0 or 1) is
  * DKS_ERR_NUMERIC and nothing non-finite is written into phi.  Shapes whose per-instance buffers do not fit shared memory
- * are DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused. */
+ * are DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused.  With a column encoding set (dks_set_column_encoding) D is its E
+ * encoded columns. */
 int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double* colw, const double* colo, int k, int metric,
                       double p, int weights, int R, const double* labels_or_targets, int head, int scalar_out);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
@@ -258,18 +260,21 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
  * non-finite keys, non-finite values) return DKS_ERR_UNSUPPORTED.  hdr_host == NULL clears the maps; dks_set_model does too. */
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
                         const double* vals_host, int n_vals);
-/* column encoding of a tree ensemble (call after dks_set_background / dks_set_groups, before dks_set_tree_model): the model
- * reads E encoded columns, each an exact program over one raw column -- a scikit-learn Pipeline of per-column steps replayed
- * bit for bit (DESIGN.md §5.0.13).  hdr_host [E][3] = {raw source column, first op, op count}; ops_host [n_ops][4] = {code
- * DKS_ENC_OP_*, flags DKS_ENC_*_ERROR, m, table offset}; opvals_host [n_ops][2] = {c0, c1}; tab_host [n_tab]: per PIECES /
- * TABLE op at its offset, the m strictly increasing finite edges / keys, the m + 1 outputs (bins; or keys then the unknown
- * output), then the NaN output.  Varying groups and masking stay on the raw columns: encoded column e belongs to the group
- * of its source, and every kernel of the tree route reads the encoded rows (encode_kernel, one thread per row and encoded
- * column, runs first in dks_fit, stage 1 and dks_predict_host).  A refused value is DKS_ERR_DOMAIN (by dks_fit for a
- * background row, by dks_predict_host and the explain calls for an instance).  Malformed input (a source out of range, an
- * unknown op or flag, unsorted or non-finite keys or edges, non-finite constants, offsets out of range) is
- * DKS_ERR_UNSUPPORTED; so is any model other than a tree ensemble (dks_set_model, dks_set_mixture and
- * dks_set_kernel_machine clear the encoding).  hdr_host == NULL clears it. */
+/* column encoding of a tree ensemble, kernel machine, MLP or neighbour model (call after dks_set_background /
+ * dks_set_groups, before dks_set_tree_model, dks_set_kernel_machine, dks_set_mlp or dks_set_knn_model, which then check the
+ * model's width against E): the model reads E encoded columns, each an exact program over one raw column -- a scikit-learn
+ * Pipeline of per-column steps replayed bit for bit (DESIGN.md §5.0.13, §5.0.16).  hdr_host [E][3] = {raw source column,
+ * first op, op count}; ops_host [n_ops][4] = {code DKS_ENC_OP_*, flags DKS_ENC_*_ERROR, m, table offset}; opvals_host
+ * [n_ops][2] = {c0, c1}; tab_host [n_tab]: per PIECES / TABLE op at its offset, the m strictly increasing finite edges /
+ * keys, the m + 1 outputs (bins; or keys then the unknown output), then the NaN output.  Varying groups stay on the raw
+ * columns: encoded column e belongs to the group of its source, and the model's kernels read the encoded rows, the
+ * encoded background and (kernel machines, MLPs, neighbour models) a group CSR over the encoded columns.  The encode kernel
+ * (one thread per row and encoded column) runs first in dks_fit, stage 1 and dks_predict_host; for kernel machines, MLPs
+ * and neighbour models it also refuses a raw +-inf that an encoded column reads.  A refused value is DKS_ERR_DOMAIN (by
+ * dks_fit for a background row, by dks_predict_host and the explain calls for an instance).  Malformed input (a source
+ * out of range, an unknown op or flag, unsorted or non-finite keys or edges, non-finite constants, offsets out of range)
+ * is DKS_ERR_UNSUPPORTED; so is any other model (dks_set_model and dks_set_mixture clear the encoding).  hdr_host == NULL
+ * clears it. */
 int dks_set_column_encoding(dks_ctx* ctx, int E, const int32_t* hdr_host, const int32_t* ops_host, const double* opvals_host,
                             int n_ops, const double* tab_host, int n_tab);
 /* the encoded rows [n x E] of host rows X_host [n x D], computed by the device's encode kernel (needs dks_fit with an
