@@ -188,22 +188,22 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         break;
     case DKS_ACT_TREES:
         // no shared-plan route: every instance runs the tree kernels; two outputs solve class 1 (class 0 its negation)
-        h.trees = true; h.l1_binary = ctx->C == 2;
+        h.family = DKS_GENERAL_TREES; h.l1_binary = ctx->C == 2;
         h.expo = ctx->tree.head == DKS_TREE_HEAD_EXP;
         break;
     case DKS_ACT_KMACH:
         // no shared-plan route: every instance runs the kernel-machine kernels; the calibrated head solves class 1 (class 0
         // its negation)
-        h.kmach = true; h.l1_binary = ctx->km.head == DKS_KM_HEAD_CALIBRATED;
+        h.family = DKS_GENERAL_KMACH; h.l1_binary = ctx->km.head == DKS_KM_HEAD_CALIBRATED;
         break;
     case DKS_ACT_MLP:
         // no shared-plan route: every instance runs the MLP kernels; the sigmoid head solves class 1 (class 0 its negation)
-        h.mlp = true; h.l1_binary = ctx->mlp.head == DKS_MLP_HEAD_SIGMOID;
+        h.family = DKS_GENERAL_MLP; h.l1_binary = ctx->mlp.head == DKS_MLP_HEAD_SIGMOID;
         break;
     case DKS_ACT_KNN:
         // no shared-plan route: every instance runs the neighbour kernels; every output is solved on its own (count / k
         // probabilities are not exact negations of each other in float64)
-        h.knn = true;
+        h.family = DKS_GENERAL_KNN;
         break;
     }
     if (h.shared != HEAD_SHARED_BINARY && !h.own()) h.shared_max_G = 128;
@@ -212,20 +212,310 @@ HeadDesc describe_head(const dks_ctx* ctx) {
     return h;
 }
 
-// out [n][E] = the column encoding of the raw rows X_dev [n][D] (grid-stride): encode_kernel for a tree ensemble,
-// encode_finite_kernel (raw infinities refused) for the families that sum over columns
+// ---- the model families with their own kernels (tree ensembles, kernel machines, MLPs, neighbour models): what differs
+// between them is here, keyed by HeadDesc::family.  Everything else treats them alike. --------------------------------
+
+enum OwnRefuses {                       // the raw values a family's predict and explain kernels refuse (DKS_ERR_DOMAIN)
+    REFUSES_NONE,                       // none: a tree sends NaN down the branch its node names
+    REFUSES_NAN,
+    REFUSES_NONFINITE,                  // NaN and the infinities
+};
+
+// a family (HeadDesc::family: its explain kernel's DKS_GENERAL_*) as the shared code sees it
+struct OwnKernel {
+    const char* family;      // "<family> run on the <kernel> only", "<family>: %d groups", "not for <family>"
+    const char* kernel;
+    const char* bound;       // "... nsamples, outputs or <bound> too many"
+    const char* model;       // "<model>: the model reads %d columns", "<model>: link(fnull) of output %d ..."
+    const char* maps_note;   // after "dks_set_column_maps: not for <family>"
+    int refuses;             // OwnRefuses
+    size_t (*smem)(const dks_ctx* ctx, int S_cap);   // the explain kernel's shared memory at S_cap coalition rows
+};
+
+// warps of explain_mlp_kernel that evaluate coalitions at S_cap rows: as many (up to 8) as shared memory holds, at least 1
+int mlp_warps(const dks_ctx* ctx, int S_cap) {
+    int nw = dks::mlp::WARPS;
+    while (nw > 1 && dks::mlp::smem_bytes(S_cap, ctx->C, ctx->G, ctx->mlp, nw) > (size_t)ctx->max_smem_optin) --nw;
+    return nw;
+}
+
+// coalitions per chunk of explain_knn_kernel at S_cap rows: as many neighbour lists as the opt-in shared memory holds next
+// to the sums and the tables, at most S_cap and at least 1
+int knn_chunk(const dks_ctx* ctx, int S_cap) {
+    const size_t fixed = dks::knn::smem_bytes(S_cap, ctx->C, ctx->G, ctx->knn.k, 0);
+    const size_t per = (sizeof(double) + sizeof(int)) * (size_t)ctx->knn.k;
+    const long long room = (long long)ctx->max_smem_optin - (long long)fixed;
+    return (int)std::max(1LL, std::min((long long)S_cap, room / (long long)per));
+}
+
+OwnKernel own_kernel(int family) {
+    switch (family) {
+    case DKS_GENERAL_TREES:
+        return {"tree ensembles", "tree kernel", "trees", "tree ensemble", "", REFUSES_NONE,
+                [](const dks_ctx* c, int S_cap) { return dks::trees::smem_bytes(S_cap, c->C, c->tree.R, c->tree.T); }};
+    case DKS_GENERAL_KMACH:
+        return {"kernel machines", "kernel-machine kernel", "groups", "kernel machine",
+                " (their scalers fold into the support vectors and column weights)", REFUSES_NAN,
+                [](const dks_ctx* c, int S_cap) {
+                    return dks::kmach::smem_bytes(S_cap, c->C, c->km.R, c->G, c->km.head == DKS_KM_HEAD_CALIBRATED); }};
+    case DKS_GENERAL_MLP:
+        return {"MLPs", "MLP kernel", "hidden units", "MLP", " (their scalers fold into the first layer)",
+                REFUSES_NONFINITE,
+                [](const dks_ctx* c, int S_cap) {
+                    return dks::mlp::smem_bytes(S_cap, c->C, c->G, c->mlp, mlp_warps(c, S_cap)); }};
+    case DKS_GENERAL_KNN:
+        return {"nearest-neighbour models", "neighbour kernel", "neighbours", "nearest-neighbour model",
+                " (their scalers fold into the column weights and origins)", REFUSES_NONFINITE,
+                [](const dks_ctx* c, int S_cap) {
+                    return dks::knn::smem_bytes(S_cap, c->C, c->G, c->knn.k, knn_chunk(c, S_cap)); }};
+    }
+    return {};                          // a linear head
+}
+
+// a device array of n elements owned by the fitted model (own_allocs)
+template <typename T>
+int own_alloc(dks_ctx* ctx, T** p, size_t n) {
+    *p = nullptr;
+    TRY(dev_alloc(p, n));
+    ctx->own_allocs.push_back((void*)*p);
+    return DKS_OK;
+}
+
+// the device copy of a host array, owned by the fitted model
+template <typename T>
+int own_upload(dks_ctx* ctx, const T** dst, const T* src, size_t n) {
+    T* p;
+    TRY(own_alloc(ctx, &p, n));
+    CUDA_TRY(cudaMemcpyAsync(p, src, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
+    *dst = p;
+    return DKS_OK;
+}
+
+// frees every device array of the fitted model, its column encoding included
+void free_own_model(dks_ctx* ctx) {
+    for (void* q : ctx->own_allocs) cudaFree(q);
+    ctx->own_allocs.clear();
+    ctx->enc = EncodingDev{};
+    ctx->fitted = false;
+    ctx->prepared = false;
+}
+
+// the end of a family's dks_set_*: its head, and the linear part stage 1 evaluates while it decides the varying groups --
+// one zero score row, no column maps
+int set_own_model(dks_ctx* ctx, int act, int C, int scalar_out) {
+    ctx->R = 1; ctx->C = C; ctx->act = act; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
+    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
+    ctx->h_W.assign((size_t)ctx->D, 0.0);
+    ctx->h_b.assign(1, 0.0);
+    ctx->fitted = false;
+    return DKS_OK;
+}
+
+bool all_finite(const double* a, size_t n) {
+    for (size_t e = 0; e < n; ++e)
+        if (!std::isfinite(a[e])) return false;
+    return true;
+}
+
+// encoded columns of the column encoding set by dks_set_column_encoding (0: none)
+int encoded_columns(const dks_ctx* ctx) { return (int)(ctx->h_ehdr.size() / 3); }
+// columns a model with its own kernel reads: the encoded ones behind a column encoding, else the raw ones
+int model_columns(const dks_ctx* ctx) { return encoded_columns(ctx) > 0 ? encoded_columns(ctx) : ctx->D; }
+
+// the group of every column the model reads: each raw column's, or behind a column encoding each encoded column's raw
+// source's
+std::vector<int32_t> column_groups(const dks_ctx* ctx) {
+    std::vector<int32_t> colgrp(ctx->D, 0);
+    for (int g = 0; g < ctx->G; ++g)
+        for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
+    const int E = encoded_columns(ctx);
+    if (E == 0) return colgrp;
+    std::vector<int32_t> enc(E);
+    for (int e = 0; e < E; ++e) enc[e] = colgrp[ctx->h_ehdr[3 * e]];
+    return enc;
+}
+
+// dks_fit: the columns the model reads against those the background gives (behind a column encoding: the encoded ones,
+// whose sources must be raw columns of the background, which dks_set_background may have changed since)
+int check_own_columns(const dks_ctx* ctx, const OwnKernel& ok) {
+    const int E = encoded_columns(ctx), width = model_columns(ctx);
+    for (int e = 0; e < E; ++e)
+        if (ctx->h_ehdr[3 * e] >= ctx->D)
+            return fail(DKS_ERR_UNSUPPORTED, "column encoding: encoded column %d reads raw column %d of %d", e,
+                        ctx->h_ehdr[3 * e], ctx->D);
+    int reads;
+    switch (ctx->head.family) {
+    case DKS_GENERAL_TREES:
+        for (int32_t f : ctx->h_tfeat)
+            if (f >= width)
+                return fail(DKS_ERR_UNSUPPORTED, "tree ensemble: a split reads column %d of %d %s", f, width,
+                            E > 0 ? "encoded columns" : "columns");
+        return DKS_OK;
+    case DKS_GENERAL_KMACH: reads = (int)(ctx->h_kcolw.size() / ctx->km.K); break;
+    case DKS_GENERAL_MLP: reads = ctx->mlp.width[0]; break;
+    default: reads = (int)ctx->h_ncolw.size(); break;
+    }
+    if (reads != width)
+        return fail(DKS_ERR_UNSUPPORTED, "%s: the model reads %d columns, %s %d", ok.model, reads,
+                    E > 0 ? "the column encoding gives" : "the background has", width);
+    return DKS_OK;
+}
+
+// dks_fit: the family's arrays on the device and its tables over the background bg [N][width] (encoded behind a column
+// encoding) -- a tree's node arrays and every background row's direction at every node; a kernel machine's T[j][v] of
+// every background row and support vector; an MLP's B[j] = b_0 + bg_j W_0; a neighbour model's T[j][v] and equality masks
+// E[j][v] of every background row and training row
+int own_fit_tables(dks_ctx* ctx, const double* bg, int width) {
+    const int N = ctx->N;
+    switch (ctx->head.family) {
+    case DKS_GENERAL_TREES: {
+        TreeDev& t = ctx->tree;
+        const size_t nodes = (size_t)t.nodes;
+        const std::vector<int32_t> colgrp = column_groups(ctx);
+        TRY(own_upload(ctx, &t.feat, ctx->h_tfeat.data(), nodes));
+        TRY(own_upload(ctx, &t.thr, ctx->h_tthr.data(), nodes));
+        TRY(own_upload(ctx, &t.left, ctx->h_tleft.data(), nodes));
+        TRY(own_upload(ctx, &t.right, ctx->h_tright.data(), nodes));
+        TRY(own_upload(ctx, &t.miss, ctx->h_tmiss.data(), nodes));
+        TRY(own_upload(ctx, &t.val, ctx->h_tval.data(), nodes * t.R));
+        TRY(own_upload(ctx, &t.roots, ctx->h_troots.data(), (size_t)t.T));
+        TRY(own_upload(ctx, &t.base, ctx->h_tbase.data(), (size_t)t.R));
+        TRY(own_upload(ctx, &t.colgrp, colgrp.data(), colgrp.size()));
+        unsigned char* bgdir;
+        TRY(own_alloc(ctx, &bgdir, (size_t)N * nodes));
+        t.bgdir = bgdir;
+        dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, ctx->stream>>>(bg, N, width, t, bgdir);
+        break;
+    }
+    case DKS_GENERAL_KMACH: {
+        KmDev& k = ctx->km;
+        TRY(own_upload(ctx, &k.sv, ctx->h_ksv.data(), ctx->h_ksv.size()));
+        TRY(own_upload(ctx, &k.dual, ctx->h_kdual.data(), ctx->h_kdual.size()));
+        TRY(own_upload(ctx, &k.colw, ctx->h_kcolw.data(), ctx->h_kcolw.size()));
+        TRY(own_upload(ctx, &k.colo, ctx->h_kcolo.data(), ctx->h_kcolo.size()));
+        double* Tbg;
+        TRY(own_alloc(ctx, &Tbg, (size_t)N * k.n_sv));
+        k.Tbg = Tbg;
+        dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, ctx->stream>>>(bg, N, width, k, Tbg);
+        break;
+    }
+    case DKS_GENERAL_MLP: {
+        MlpDev& m = ctx->mlp;
+        TRY(own_upload(ctx, &m.W, ctx->h_mw.data(), ctx->h_mw.size()));
+        TRY(own_upload(ctx, &m.b, ctx->h_mb.data(), ctx->h_mb.size()));
+        TRY(own_upload(ctx, &m.Wf, ctx->h_mwf.data(), ctx->h_mwf.size()));
+        TRY(own_upload(ctx, &m.bp, ctx->h_mbp.data(), ctx->h_mbp.size()));
+        double* Bbg;
+        TRY(own_alloc(ctx, &Bbg, (size_t)N * m.width[1]));
+        m.Bbg = Bbg;
+        dks::mlp::mlp_fit_table_kernel<<<cdiv((long long)N * m.width[1], 256), 256, 0, ctx->stream>>>(bg, N, width, m, Bbg);
+        break;
+    }
+    case DKS_GENERAL_KNN: {
+        KnnDev& k = ctx->knn;
+        const std::vector<int32_t> colgrp = column_groups(ctx);
+        TRY(own_upload(ctx, &k.fitX, ctx->h_nfitX.data(), ctx->h_nfitX.size()));
+        TRY(own_upload(ctx, &k.colw, ctx->h_ncolw.data(), ctx->h_ncolw.size()));
+        TRY(own_upload(ctx, &k.colo, ctx->h_ncolo.data(), ctx->h_ncolo.size()));
+        TRY(own_upload(ctx, &k.y, ctx->h_ny.data(), ctx->h_ny.size()));
+        TRY(own_upload(ctx, &k.colgrp, colgrp.data(), colgrp.size()));
+        double* Tbg;
+        uint64_t* Ebg;
+        TRY(own_alloc(ctx, &Tbg, (size_t)N * k.n_fit));
+        TRY(own_alloc(ctx, &Ebg, (size_t)N * k.n_fit));
+        k.Tbg = Tbg;
+        k.Ebg = Ebg;
+        dks::knn::knn_fit_table_kernel<<<cdiv((long long)N * k.n_fit, 256), 256, 0, ctx->stream>>>(bg, N, width, ctx->G, k,
+                                                                                                     Tbg, Ebg);
+        break;
+    }
+    }
+    ctx->launches += 1;
+    return DKS_OK;
+}
+
+// out [n][E] = the column encoding of the raw rows X_dev [n][D] (grid-stride): encode_kernel for a family that refuses no
+// raw value, encode_finite_kernel (raw infinities refused) for the others, which sum over columns
 int launch_encode(dks_ctx* ctx, const double* X_dev, int n, double* out) {
     const long long total = (long long)n * ctx->enc.E;
     const int grid = (int)std::min<long long>(cdiv(total, 256), (long long)ctx->sm_count * 8);
-    auto kern = ctx->head.trees ? dks::enc::encode_kernel : dks::enc::encode_finite_kernel;
+    auto kern = own_kernel(ctx->head.family).refuses == REFUSES_NONE ? dks::enc::encode_kernel : dks::enc::encode_finite_kernel;
     kern<<<grid, 256, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->enc, out, ctx->d_status);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     return DKS_OK;
 }
 
-// CTAs of mlp_predict_kernel over n rows (one row per CTA, grid-stride)
-int mlp_predict_grid(const dks_ctx* ctx, int n) { return std::max(1, std::min(n, ctx->sm_count * 8)); }
+// the family's predict kernel over n rows: out [n][C] = f(x) and dlink [n][C] = link(f(x)) - linkfnull, each when not NULL;
+// a refused row and a non-finite dlink are reported in the status word.  X holds the rows the model reads or, given Xenc,
+// raw rows [n][D] that the column encoding first writes to Xenc [n][E].
+int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const double* linkfnull, double* out,
+                       double* dlink) {
+    if (Xenc) {
+        TRY(launch_encode(ctx, X, n, Xenc));
+        X = Xenc;
+    }
+    const int D = ctx->enc.E > 0 ? ctx->enc.E : ctx->D, C = ctx->C, link = ctx->link;
+    const cudaStream_t st = ctx->stream;
+    switch (ctx->head.family) {
+    case DKS_GENERAL_TREES:
+        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->tree, C, link, linkfnull, out, dlink,
+                                                                      ctx->d_status);
+        break;
+    case DKS_GENERAL_KMACH:
+        dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->km, C, link, linkfnull, out, dlink,
+                                                                    ctx->d_status);
+        break;
+    case DKS_GENERAL_MLP:           // one row per CTA, grid-stride
+        dks::mlp::mlp_predict_kernel<<<std::max(1, std::min(n, ctx->sm_count * 8)), dks::mlp::THREADS, 0, st>>>(
+            X, n, D, ctx->mlp, C, link, linkfnull, out, dlink, ctx->d_status);
+        break;
+    case DKS_GENERAL_KNN:
+        dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->knn, C, link, linkfnull, out, dlink,
+                                                                   ctx->d_status);
+        break;
+    }
+    ctx->launches += 1;
+    return DKS_OK;
+}
+
+// the family's explain kernel over p.list (L1: its moments); the tree kernel's per-CTA node scratch is sized for the grid
+int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
+    const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
+    const dks::SimtL1 q = l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{};
+    switch (ctx->head.family) {
+    case DKS_GENERAL_TREES: {
+        TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
+        auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->own_X, ctx->own_D);
+        break;
+    }
+    case DKS_GENERAL_KMACH: {
+        auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->own_X, ctx->own_bg, ctx->own_D, ctx->own_goff,
+                                                      ctx->own_gcols);
+        break;
+    }
+    case DKS_GENERAL_MLP: {
+        auto kern = l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
+        break;
+    }
+    case DKS_GENERAL_KNN: {
+        auto kern = l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
+        break;
+    }
+    }
+    ctx->launches += 1;
+    return DKS_OK;
+}
 
 // stage 1's instantiation for R score rows: the compile-time bound 1 or 8 (a mixture: DKS_MIX_MAX_R)
 template <bool STAGE, bool MAPS>
@@ -248,64 +538,32 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
     const size_t maps_doubles = maps ? (size_t)ctx->cm.n_keys + ctx->cm.n_vals : 0;
     const bool stage = dks::prep_smem_bytes(true, ipb, G, ctx->R, ctx->D, maps_doubles) <= (size_t)96 * 1024;
     const size_t psm = dks::prep_smem_bytes(stage, ipb, G, ctx->R, ctx->D, maps_doubles);
-    // the score rows stage 1 computes: one for the families with their own kernel (the scores of a zero linear model, unused)
-    const int R = h.own() ? 1 : ctx->R;
+    // the families with their own kernel: stage 1 only decides the varying groups (its scores are those of a zero linear
+    // model, one identity output, and unused); the model's predict kernel then writes f(x) and link(f(x)) - link(fnull) of
+    // every output
+    const bool own = h.own();
+    const int R = own ? 1 : ctx->R;
     auto kern = stage ? (maps ? prep_kernel_for<true, true>(h.mixture(), R) : prep_kernel_for<true, false>(h.mixture(), R))
                       : (maps ? prep_kernel_for<false, true>(h.mixture(), R) : prep_kernel_for<false, false>(h.mixture(), R));
     // nibble tables for the shared-plan route: the binary head's at any G, the other heads' up to 128 groups (what their
     // shared-plan route covers)
-    double* xt = (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
+    double* xt = !own && (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
-    ctx->own_X = X_dev;
-    ctx->own_D = ctx->D;
-    ctx->own_bg = ctx->d_bg;
-    ctx->own_goff = ctx->d_goff;
-    ctx->own_gcols = ctx->d_gcols;
-    if (h.own() && ctx->enc.E > 0) {
-        // a model behind a column encoding: its kernels read the encoded rows, the encoded background and the encoded group
-        // CSR (a refused value is reported here); stage 1 decides the varying groups on the raw rows
-        TRY(grow(ctx, &ctx->d_Xenc, &ctx->cap_Xenc, (size_t)n * ctx->enc.E));
-        TRY(launch_encode(ctx, X_dev, n, ctx->d_Xenc));
-        ctx->own_X = ctx->d_Xenc;
-        ctx->own_D = ctx->enc.E;
-        ctx->own_bg = ctx->d_bg_enc;
-        ctx->own_goff = ctx->d_egoff;
-        ctx->own_gcols = ctx->d_egcols;
-    }
-    if (h.own()) {
-        // tree ensembles, kernel machines, MLPs and neighbour models: prep_kernel decides the varying groups (its scores are those of a zero linear
-        // model, one identity output, and unused); the model's predict kernel then writes f(x) and link(f(x)) - link(fnull)
-        // of every output
-        kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
-            X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
-            ctx->d_linkfnull, n, ctx->N, ctx->D, G, 1, 1, DKS_ACT_IDENTITY, 1.0, ctx->link, ipb, ctx->d_XW,
-            ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-            nullptr, 1.0, nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
-        const double* Xo = ctx->own_X;
-        const int Do = ctx->own_D;
-        if (h.kmach)
-            dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->km, ctx->C, ctx->link,
-                                                                                 ctx->d_linkfnull, nullptr, ctx->d_dlink,
-                                                                                 ctx->d_status);
-        else if (h.mlp)
-            dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
-                Xo, n, Do, ctx->mlp, ctx->C, ctx->link, ctx->d_linkfnull, nullptr, ctx->d_dlink, ctx->d_status);
-        else if (h.knn)
-            dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->knn, ctx->C, ctx->link,
-                                                                               ctx->d_linkfnull, nullptr, ctx->d_dlink,
-                                                                               ctx->d_status);
-        else
-            dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->tree, ctx->C, ctx->link,
-                                                                                   ctx->d_linkfnull, nullptr, ctx->d_dlink,
-                                                                                   ctx->d_status);
-        ctx->launches += 1;
-    } else {
-        kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
-            X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
-            ctx->d_linkfnull, n, ctx->N, ctx->D, G, ctx->R, ctx->C, ctx->act, ctx->kappa, ctx->link, ipb, ctx->d_XW,
-            ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full, ctx->d_idx_other,
-            xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
-    }
+    // a model behind a column encoding: its kernels read the encoded rows, the encoded background and the encoded group CSR
+    // (a refused value is reported by the encoding); stage 1 decides the varying groups on the raw rows
+    const bool enc = own && ctx->enc.E > 0;
+    if (enc) TRY(grow(ctx, &ctx->d_Xenc, &ctx->cap_Xenc, (size_t)n * ctx->enc.E));
+    ctx->own_X = enc ? ctx->d_Xenc : X_dev;
+    ctx->own_D = enc ? ctx->enc.E : ctx->D;
+    ctx->own_bg = enc ? ctx->d_bg_enc : ctx->d_bg;
+    ctx->own_goff = enc ? ctx->d_egoff : ctx->d_goff;
+    ctx->own_gcols = enc ? ctx->d_egcols : ctx->d_gcols;
+    kern<<<cdiv(n, ipb), 256, psm, ctx->stream>>>(
+        X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
+        ctx->d_linkfnull, n, ctx->N, ctx->D, G, R, own ? 1 : ctx->C, own ? DKS_ACT_IDENTITY : ctx->act, own ? 1.0 : ctx->kappa,
+        ctx->link, ipb, ctx->d_XW, ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full,
+        ctx->d_idx_other, xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
+    if (own) TRY(launch_own_predict(ctx, X_dev, n, enc ? ctx->d_Xenc : nullptr, ctx->d_linkfnull, nullptr, ctx->d_dlink));
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
@@ -460,51 +718,10 @@ int sampler_config(const dks_ctx* ctx, bool wide_pi, SamplerConfig* sc) {
     return DKS_OK;
 }
 
-// a model family with its own explain kernel (tree ensembles, kernel machines): the kernel's DKS_GENERAL_* value, the
-// wording of its route's messages and its shared memory at S_cap coalition rows
-struct OwnKernel {
-    int general;
-    const char* family;      // "<family> run on the <kernel> only", "<family>: %d groups"
-    const char* kernel;
-    const char* bound;       // "... nsamples, outputs or <bound> too many"
-    size_t (*smem)(const dks_ctx* ctx, int S_cap);
-};
-
-// warps of explain_mlp_kernel that evaluate coalitions at S_cap rows: as many (up to 8) as shared memory holds, at least 1
-int mlp_warps(const dks_ctx* ctx, int S_cap) {
-    int nw = dks::mlp::WARPS;
-    while (nw > 1 && dks::mlp::smem_bytes(S_cap, ctx->C, ctx->G, ctx->mlp, nw) > (size_t)ctx->max_smem_optin) --nw;
-    return nw;
-}
-
-// coalitions per chunk of explain_knn_kernel at S_cap rows: as many neighbour lists as the opt-in shared memory holds next
-// to the sums and the tables, at most S_cap and at least 1
-int knn_chunk(const dks_ctx* ctx, int S_cap) {
-    const size_t fixed = dks::knn::smem_bytes(S_cap, ctx->C, ctx->G, ctx->knn.k, 0);
-    const size_t per = (sizeof(double) + sizeof(int)) * (size_t)ctx->knn.k;
-    const long long room = (long long)ctx->max_smem_optin - (long long)fixed;
-    return (int)std::max(1LL, std::min((long long)S_cap, room / (long long)per));
-}
-
-OwnKernel own_kernel(const dks_ctx* ctx) {
-    if (ctx->head.trees)
-        return {DKS_GENERAL_TREES, "tree ensembles", "tree kernel", "trees", [](const dks_ctx* c, int S_cap) {
-                    return dks::trees::smem_bytes(S_cap, c->C, c->tree.R, c->tree.T); }};
-    if (ctx->head.mlp)
-        return {DKS_GENERAL_MLP, "MLPs", "MLP kernel", "hidden units", [](const dks_ctx* c, int S_cap) {
-                    return dks::mlp::smem_bytes(S_cap, c->C, c->G, c->mlp, mlp_warps(c, S_cap)); }};
-    if (ctx->head.knn)
-        return {DKS_GENERAL_KNN, "nearest-neighbour models", "neighbour kernel", "neighbours", [](const dks_ctx* c, int S_cap) {
-                    return dks::knn::smem_bytes(S_cap, c->C, c->G, c->knn.k, knn_chunk(c, S_cap)); }};
-    return {DKS_GENERAL_KMACH, "kernel machines", "kernel-machine kernel", "groups", [](const dks_ctx* c, int S_cap) {
-                return dks::kmach::smem_bytes(S_cap, c->C, c->km.R, c->G, c->km.head == DKS_KM_HEAD_CALIBRATED); }};
-}
-
-// tree ensembles and kernel machines: every instance on the family's own kernel (up to 64 groups, CUDA-core only), the
-// instances whose M selects through the general list's l1 route -- the kernel's moments, then l1_lars_kernel -- whatever
-// their M, G included
+// a family with its own kernel: every instance on that kernel (up to 64 groups, CUDA-core only), the instances whose M
+// selects through the general list's l1 route -- the kernel's moments, then l1_lars_kernel -- whatever their M, G included
 int choose_route_own(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route* rt) {
-    const OwnKernel ok = own_kernel(ctx);
+    const OwnKernel ok = own_kernel(ctx->head.family);
     const int G = ctx->G, kernel = ctx->kernel_choice;
     if (kernel != DKS_KERNEL_AUTO && kernel != DKS_KERNEL_SIMT)
         return fail(DKS_ERR_UNSUPPORTED, "%s run on the %s only (kernel 'auto' or 'simt')", ok.family, ok.kernel);
@@ -532,57 +749,23 @@ int choose_route_own(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route*
                         rt->l1_Mmax, rt->l1_Mmax);
         rt->l1_smem = rt->smem;
     }
-    rt->general = ok.general;
+    rt->general = ctx->head.family;
     return DKS_OK;
 }
 
-// the family's own kernel over p.list (L1: its moments); the tree kernel's per-CTA node scratch is sized for the grid
-int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
-    const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
-    const dks::SimtL1 q = l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{};
-    if (ctx->head.trees) {
-        TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
-        auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->own_X, ctx->own_D);
-    } else if (ctx->head.mlp) {
-        auto kern = l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
-                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
-    } else if (ctx->head.knn) {
-        auto kern = l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
-                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
-    } else {
-        auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->own_X, ctx->own_bg, ctx->own_D, ctx->own_goff,
-                                                      ctx->own_gcols);
-    }
-    ctx->launches += 1;
-    return DKS_OK;
-}
-
-// DKS_ERR_DOMAIN: "<prefix> %d <phrase>", the phrase naming what refuses a raw value -- a kernel machine, a tree's column
-// encoding or a linear model's column maps
-const char* refusal_phrase(bool kmach, bool encoding) {
-    if (kmach) return "holds NaN: kernel machines refuse it, as scikit-learn does";
-    return encoding ? "holds a raw value the column encoding refuses (NaN, or a category unseen at fit time, where the "
-                      "pipeline raises)"
-                    : "holds a raw value its column map refuses (NaN, or a category unseen at fit time, where the pipeline "
-                      "raises)";
-}
-// the row named by the status word, refused by the model's family
+// DKS_ERR_DOMAIN for the row the status word names, worded for what refused it: the family's kernels, or the pipeline in
+// front of them; a tree's column encoding; a linear model's column maps
 int fail_refused(const dks_ctx* ctx, const char* prefix) {
-    if (ctx->enc.E > 0 && (ctx->head.kmach || ctx->head.mlp || ctx->head.knn))
+    const OwnKernel ok = own_kernel(ctx->head.family);
+    const int row = ctx->h_status[1];
+    if (ok.refuses != REFUSES_NONE && ctx->enc.E > 0)
         return fail(DKS_ERR_DOMAIN, "%s %d holds a raw value the pipeline refuses (NaN where no imputer fills it, an "
-                    "infinity, or a category unseen at fit time), as scikit-learn does", prefix, ctx->h_status[1]);
-    if (ctx->head.mlp || ctx->head.knn)
-        return fail(DKS_ERR_DOMAIN, "%s %d holds NaN or an infinity: %s refuse it, as scikit-learn does", prefix,
-                    ctx->h_status[1], ctx->head.mlp ? "MLPs" : "nearest-neighbour models");
-    return fail(DKS_ERR_DOMAIN, "%s %d %s", prefix, ctx->h_status[1], refusal_phrase(ctx->head.kmach, ctx->head.trees));
+                    "infinity, or a category unseen at fit time), as scikit-learn does", prefix, row);
+    if (ok.refuses != REFUSES_NONE)
+        return fail(DKS_ERR_DOMAIN, "%s %d holds %s: %s refuse it, as scikit-learn does", prefix, row,
+                    ok.refuses == REFUSES_NAN ? "NaN" : "NaN or an infinity", ok.family);
+    return fail(DKS_ERR_DOMAIN, "%s %d holds a raw value %s refuses (NaN, or a category unseen at fit time, where the "
+                "pipeline raises)", prefix, row, ctx->head.own() ? "the column encoding" : "its column map");
 }
 
 void free_column_maps(dks_ctx* ctx) {
@@ -594,7 +777,8 @@ void free_column_maps(dks_ctx* ctx) {
 }
 
 // the start of dks_fit for every family: the background, its weights, the linear model's W and b, the groups and the
-// column statistics stage 1 decides the varying groups with on the device; fnull's buffers; no column maps; status cleared
+// column statistics stage 1 decides the varying groups with on the device; fnull's buffers; no column maps and none of the
+// previous fit's family arrays; status cleared
 int fit_begin(dks_ctx* ctx) {
     const int N = ctx->N, D = ctx->D, G = ctx->G, R = ctx->R, C = ctx->C;
     const cudaStream_t st = ctx->stream;
@@ -610,6 +794,7 @@ int fit_begin(dks_ctx* ctx) {
     TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
     TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
     free_column_maps(ctx);
+    free_own_model(ctx);
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
@@ -656,90 +841,19 @@ int fit_done(dks_ctx* ctx) {
     return DKS_OK;
 }
 
-// device copy of one tree array (replacing the previous one)
-template <typename T>
-int upload_tree_array(const T** dst, const T* src, size_t n, cudaStream_t st) {
-    T* p = nullptr;
-    TRY(dev_alloc(&p, n));
-    CUDA_TRY(cudaMemcpyAsync(p, src, sizeof(T) * n, cudaMemcpyHostToDevice, st));
-    if (*dst) cudaFree((void*)*dst);
-    *dst = p;
-    return DKS_OK;
-}
-
-void free_tree(dks_ctx* ctx) {
-    TreeDev& t = ctx->tree;
-    for (const void* q : {(const void*)t.feat, (const void*)t.thr, (const void*)t.left, (const void*)t.right, (const void*)t.miss,
-                          (const void*)t.val, (const void*)t.roots, (const void*)t.base, (const void*)t.colgrp,
-                          (const void*)t.bgdir, (const void*)t.xinfo})
-        if (q) cudaFree((void*)q);
-    t.feat = nullptr; t.thr = nullptr; t.left = nullptr; t.right = nullptr; t.miss = nullptr; t.val = nullptr;
-    t.roots = nullptr; t.base = nullptr; t.colgrp = nullptr; t.bgdir = nullptr; t.xinfo = nullptr;
-    ctx->cap_txinfo = 0;
-}
-
-void free_encoding(dks_ctx* ctx) {
-    EncodingDev& e = ctx->enc;
-    for (const void* q : {(const void*)e.hdr, (const void*)e.ops, (const void*)e.opv, (const void*)e.tab})
-        if (q) cudaFree((void*)q);
-    e = EncodingDev{};
-    dev_free(&ctx->d_bg_enc);
-    dev_free(&ctx->d_egoff);
-    dev_free(&ctx->d_egcols);
-}
-
-// encoded columns of the column encoding set by dks_set_column_encoding (0: none)
-int encoded_columns(const dks_ctx* ctx) { return (int)(ctx->h_ehdr.size() / 3); }
-// columns a model with its own kernel reads: the encoded ones behind a column encoding, else the raw ones
-int model_columns(const dks_ctx* ctx) { return encoded_columns(ctx) > 0 ? encoded_columns(ctx) : ctx->D; }
-
-// the group of every column the model reads: each raw column's, or behind a column encoding each encoded column's raw
-// source's
-std::vector<int32_t> column_groups(const dks_ctx* ctx) {
-    std::vector<int32_t> colgrp(ctx->D, 0);
-    for (int g = 0; g < ctx->G; ++g)
-        for (int c = ctx->h_goff[g]; c < ctx->h_goff[g + 1]; ++c) colgrp[ctx->h_gcols[c]] = g;
-    const int E = encoded_columns(ctx);
-    if (E == 0) return colgrp;
-    std::vector<int32_t> enc(E);
-    for (int e = 0; e < E; ++e) enc[e] = colgrp[ctx->h_ehdr[3 * e]];
-    return enc;
-}
-
-// the sources of a column encoding are raw columns of the background (which dks_set_background may have changed since)
-int check_encoding_sources(const dks_ctx* ctx) {
-    for (int e = 0; e < encoded_columns(ctx); ++e)
-        if (ctx->h_ehdr[3 * e] >= ctx->D)
-            return fail(DKS_ERR_UNSUPPORTED, "column encoding: encoded column %d reads raw column %d of %d", e,
-                        ctx->h_ehdr[3 * e], ctx->D);
-    return DKS_OK;
-}
-
-// a kernel machine, MLP or neighbour model reads `width` columns: the encoded ones behind a column encoding, else the raw
-// ones
-int check_model_width(const dks_ctx* ctx, int width, const char* family) {
-    TRY(check_encoding_sources(ctx));
-    if (width != model_columns(ctx))
-        return fail(DKS_ERR_UNSUPPORTED, "%s: the model reads %d columns, %s %d", family, width,
-                    encoded_columns(ctx) > 0 ? "the column encoding gives" : "the background has", model_columns(ctx));
-    return DKS_OK;
-}
-
 // dks_fit's column encoding, after fit_begin: the device copy, the encoded background d_bg_enc and the encoded group CSR
-// (group g owns the encoded columns whose raw source is in g, in increasing encoded index).  Without an encoding the
-// previous one is dropped.
+// (group g owns the encoded columns whose raw source is in g, in increasing encoded index)
 int fit_encoding(dks_ctx* ctx) {
-    free_encoding(ctx);
     const int E = encoded_columns(ctx), G = ctx->G;
     if (E == 0) return DKS_OK;
     const cudaStream_t st = ctx->stream;
     EncodingDev& en = ctx->enc;
-    TRY(upload_tree_array(&en.hdr, ctx->h_ehdr.data(), ctx->h_ehdr.size(), st));
-    TRY(upload_tree_array(&en.ops, ctx->h_eops.data(), ctx->h_eops.size(), st));
-    TRY(upload_tree_array(&en.opv, ctx->h_eopv.data(), ctx->h_eopv.size(), st));
-    TRY(upload_tree_array(&en.tab, ctx->h_etab.data(), ctx->h_etab.size(), st));
+    TRY(own_upload(ctx, &en.hdr, ctx->h_ehdr.data(), ctx->h_ehdr.size()));
+    TRY(own_upload(ctx, &en.ops, ctx->h_eops.data(), ctx->h_eops.size()));
+    TRY(own_upload(ctx, &en.opv, ctx->h_eopv.data(), ctx->h_eopv.size()));
+    TRY(own_upload(ctx, &en.tab, ctx->h_etab.data(), ctx->h_etab.size()));
     en.E = E;
-    TRY(dev_alloc(&ctx->d_bg_enc, (size_t)ctx->N * E));
+    TRY(own_alloc(ctx, &ctx->d_bg_enc, (size_t)ctx->N * E));
     TRY(launch_encode(ctx, ctx->d_bg, ctx->N, ctx->d_bg_enc));
     const std::vector<int32_t> colgrp = column_groups(ctx);
     std::vector<int32_t> goff(G + 1, 0), gcols(E);
@@ -747,177 +861,29 @@ int fit_encoding(dks_ctx* ctx) {
     for (int g = 0; g < G; ++g) goff[g + 1] += goff[g];
     std::vector<int32_t> at(goff.begin(), goff.end() - 1);
     for (int e = 0; e < E; ++e) gcols[at[colgrp[e]]++] = e;
-    TRY(dev_alloc(&ctx->d_egoff, (size_t)G + 1));
-    TRY(dev_alloc(&ctx->d_egcols, (size_t)E));
+    TRY(own_alloc(ctx, &ctx->d_egoff, (size_t)G + 1));
+    TRY(own_alloc(ctx, &ctx->d_egcols, (size_t)E));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_egoff, goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_egcols, gcols.data(), sizeof(int32_t) * E, cudaMemcpyHostToDevice, st));
     return DKS_OK;
 }
 
-// dks_fit of a tree ensemble: the node arrays, the group of every column, every background row's direction at every node,
-// the column statistics stage 1 decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the tree kernels
-int fit_trees(dks_ctx* ctx) {
+// dks_fit of a family with its own kernel: its column check, the common start, the column encoding, the family's arrays
+// and tables, and fnull = sum_j w_j f(bg_j) from its predict kernel
+int fit_own(dks_ctx* ctx) {
+    const OwnKernel ok = own_kernel(ctx->head.family);
     const int N = ctx->N, C = ctx->C;
-    const cudaStream_t st = ctx->stream;
-    TreeDev& t = ctx->tree;
-    const size_t nodes = (size_t)t.nodes;
-    // a column encoding: the tree reads E encoded columns, each in the group of its raw source
-    const int E = encoded_columns(ctx);
-    const int width = model_columns(ctx);
-    TRY(check_encoding_sources(ctx));
-    for (int32_t f : ctx->h_tfeat)
-        if (f >= width)
-            return fail(DKS_ERR_UNSUPPORTED, "tree ensemble: a split reads column %d of %d %s", f, width,
-                        E > 0 ? "encoded columns" : "columns");
-    TRY(fit_begin(ctx));
-    const std::vector<int32_t> colgrp = column_groups(ctx);
-    free_tree(ctx);
-    TRY(fit_encoding(ctx));
-    TRY(upload_tree_array(&t.feat, ctx->h_tfeat.data(), nodes, st));
-    TRY(upload_tree_array(&t.thr, ctx->h_tthr.data(), nodes, st));
-    TRY(upload_tree_array(&t.left, ctx->h_tleft.data(), nodes, st));
-    TRY(upload_tree_array(&t.right, ctx->h_tright.data(), nodes, st));
-    TRY(upload_tree_array(&t.miss, ctx->h_tmiss.data(), nodes, st));
-    TRY(upload_tree_array(&t.val, ctx->h_tval.data(), nodes * t.R, st));
-    TRY(upload_tree_array(&t.roots, ctx->h_troots.data(), (size_t)t.T, st));
-    TRY(upload_tree_array(&t.base, ctx->h_tbase.data(), (size_t)t.R, st));
-    TRY(upload_tree_array(&t.colgrp, colgrp.data(), colgrp.size(), st));
-    unsigned char* bgdir = nullptr;
-    TRY(dev_alloc(&bgdir, (size_t)N * nodes));
-    t.bgdir = bgdir;
-    double* pred = nullptr;
-    TRY(dev_alloc(&pred, (size_t)N * C));
-    const double* tbg = E > 0 ? ctx->d_bg_enc : ctx->d_bg;
-    dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, st>>>(tbg, N, width, t, bgdir);
-    dks::trees::tree_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(tbg, N, width, t, C, ctx->link, nullptr, pred, nullptr,
-                                                                  nullptr);
-    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
-    ctx->launches += 3;
-    const int rc = fit_readback(ctx, "tree ensemble");
-    cudaFree(pred);
-    TRY(rc);
-    return fit_done(ctx);
-}
-
-void free_kmach(dks_ctx* ctx) {
-    KmDev& k = ctx->km;
-    for (const void* q : {(const void*)k.sv, (const void*)k.dual, (const void*)k.colw, (const void*)k.colo, (const void*)k.Tbg})
-        if (q) cudaFree((void*)q);
-    k.sv = nullptr; k.dual = nullptr; k.colw = nullptr; k.colo = nullptr; k.Tbg = nullptr;
-}
-
-// dks_fit of a kernel machine: the arrays, T[j][v] of every background row and support vector, the column statistics stage 1
-// decides the varying groups with, and fnull = sum_j w_j f(bg_j) from the kernel-machine kernels
-int fit_kmach(dks_ctx* ctx) {
-    const int N = ctx->N, C = ctx->C;
-    const cudaStream_t st = ctx->stream;
-    KmDev& k = ctx->km;
-    const int D = (int)(ctx->h_kcolw.size() / k.K);   // the raw columns, or the encoded ones behind a column encoding
-    TRY(check_model_width(ctx, D, "kernel machine"));
+    TRY(check_own_columns(ctx, ok));
     TRY(fit_begin(ctx));
     TRY(fit_encoding(ctx));
     const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
-    free_kmach(ctx);
-    TRY(upload_tree_array(&k.sv, ctx->h_ksv.data(), ctx->h_ksv.size(), st));
-    TRY(upload_tree_array(&k.dual, ctx->h_kdual.data(), ctx->h_kdual.size(), st));
-    TRY(upload_tree_array(&k.colw, ctx->h_kcolw.data(), ctx->h_kcolw.size(), st));
-    TRY(upload_tree_array(&k.colo, ctx->h_kcolo.data(), ctx->h_kcolo.size(), st));
-    double* Tbg = nullptr;
-    TRY(dev_alloc(&Tbg, (size_t)N * k.n_sv));
-    k.Tbg = Tbg;
+    TRY(own_fit_tables(ctx, bg, model_columns(ctx)));
     double* pred = nullptr;
     TRY(dev_alloc(&pred, (size_t)N * C));
-    dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(bg, N, D, k, Tbg);
-    dks::kmach::km_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
-                                                                ctx->d_status);
-    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
-    ctx->launches += 3;
-    const int rc = fit_readback(ctx, "kernel machine");
-    cudaFree(pred);
-    TRY(rc);
-    return fit_done(ctx);
-}
-
-void free_mlp(dks_ctx* ctx) {
-    MlpDev& m = ctx->mlp;
-    for (const void* q : {(const void*)m.W, (const void*)m.b, (const void*)m.Wf, (const void*)m.bp, (const void*)m.Bbg})
-        if (q) cudaFree((void*)q);
-    m.W = nullptr; m.b = nullptr; m.Wf = nullptr; m.bp = nullptr; m.Bbg = nullptr;
-}
-
-// dks_fit of an MLP: the layers, B[j] = b_0 + bg_j W_0 of every background row, the column statistics stage 1 decides the
-// varying groups with, and fnull = sum_j w_j f(bg_j) from the MLP kernels
-int fit_mlp(dks_ctx* ctx) {
-    const int N = ctx->N, C = ctx->C;
-    const cudaStream_t st = ctx->stream;
-    MlpDev& m = ctx->mlp;
-    const int D = m.width[0];                       // the raw columns, or the encoded ones behind a column encoding
-    TRY(check_model_width(ctx, D, "MLP"));
-    TRY(fit_begin(ctx));
-    TRY(fit_encoding(ctx));
-    const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
-    free_mlp(ctx);
-    TRY(upload_tree_array(&m.W, ctx->h_mw.data(), ctx->h_mw.size(), st));
-    TRY(upload_tree_array(&m.b, ctx->h_mb.data(), ctx->h_mb.size(), st));
-    TRY(upload_tree_array(&m.Wf, ctx->h_mwf.data(), ctx->h_mwf.size(), st));
-    TRY(upload_tree_array(&m.bp, ctx->h_mbp.data(), ctx->h_mbp.size(), st));
-    double* Bbg = nullptr;
-    TRY(dev_alloc(&Bbg, (size_t)N * m.width[1]));
-    m.Bbg = Bbg;
-    double* pred = nullptr;
-    TRY(dev_alloc(&pred, (size_t)N * C));
-    dks::mlp::mlp_fit_table_kernel<<<cdiv((long long)N * m.width[1], 256), 256, 0, st>>>(bg, N, D, m, Bbg);
-    dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, N), dks::mlp::THREADS, 0, st>>>(bg, N, D, m, C, ctx->link, nullptr,
-                                                                                       pred, nullptr, ctx->d_status);
-    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
-    ctx->launches += 3;
-    const int rc = fit_readback(ctx, "MLP");
-    cudaFree(pred);
-    TRY(rc);
-    return fit_done(ctx);
-}
-
-void free_knn(dks_ctx* ctx) {
-    KnnDev& k = ctx->knn;
-    for (const void* q : {(const void*)k.fitX, (const void*)k.colw, (const void*)k.colo, (const void*)k.y,
-                          (const void*)k.colgrp, (const void*)k.Tbg, (const void*)k.Ebg})
-        if (q) cudaFree((void*)q);
-    k.fitX = nullptr; k.colw = nullptr; k.colo = nullptr; k.y = nullptr; k.colgrp = nullptr; k.Tbg = nullptr; k.Ebg = nullptr;
-}
-
-// dks_fit of a nearest-neighbour model: the arrays, the group of every column, T[j][v] and the equality masks E[j][v] of
-// every background row and training row, the column statistics stage 1 decides the varying groups with, and
-// fnull = sum_j w_j f(bg_j) from the neighbour kernels
-int fit_knn(dks_ctx* ctx) {
-    const int N = ctx->N, G = ctx->G, C = ctx->C;
-    const cudaStream_t st = ctx->stream;
-    KnnDev& k = ctx->knn;
-    const int D = (int)ctx->h_ncolw.size();         // the raw columns, or the encoded ones behind a column encoding
-    TRY(check_model_width(ctx, D, "nearest-neighbour model"));
-    TRY(fit_begin(ctx));
-    TRY(fit_encoding(ctx));
-    const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
-    const std::vector<int32_t> colgrp = column_groups(ctx);
-    free_knn(ctx);
-    TRY(upload_tree_array(&k.fitX, ctx->h_nfitX.data(), ctx->h_nfitX.size(), st));
-    TRY(upload_tree_array(&k.colw, ctx->h_ncolw.data(), ctx->h_ncolw.size(), st));
-    TRY(upload_tree_array(&k.colo, ctx->h_ncolo.data(), ctx->h_ncolo.size(), st));
-    TRY(upload_tree_array(&k.y, ctx->h_ny.data(), ctx->h_ny.size(), st));
-    TRY(upload_tree_array(&k.colgrp, colgrp.data(), colgrp.size(), st));
-    double* Tbg = nullptr;
-    uint64_t* Ebg = nullptr;
-    TRY(dev_alloc(&Tbg, (size_t)N * k.n_fit));
-    k.Tbg = Tbg;
-    TRY(dev_alloc(&Ebg, (size_t)N * k.n_fit));
-    k.Ebg = Ebg;
-    double* pred = nullptr;
-    TRY(dev_alloc(&pred, (size_t)N * C));
-    dks::knn::knn_fit_table_kernel<<<cdiv((long long)N * k.n_fit, 256), 256, 0, st>>>(bg, N, D, G, k, Tbg, Ebg);
-    dks::knn::knn_predict_kernel<<<cdiv(N, 128), 128, 0, st>>>(bg, N, D, k, C, ctx->link, nullptr, pred, nullptr,
-                                                               ctx->d_status);
-    dks::trees::tree_fnull_kernel<<<1, 32, 0, st>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
-    ctx->launches += 3;
-    const int rc = fit_readback(ctx, "nearest-neighbour model");
+    TRY(launch_own_predict(ctx, bg, N, nullptr, nullptr, pred, nullptr));
+    dks::fit_pred_fnull_kernel<<<1, 32, 0, ctx->stream>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
+    ctx->launches += 1;
+    const int rc = fit_readback(ctx, ok.model);
     cudaFree(pred);
     TRY(rc);
     return fit_done(ctx);
@@ -1408,13 +1374,11 @@ int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t 
     case DKS_GENERAL_TC:
         TRY(dks::tc_launch(ctx, p, gstream));
         break;
-    case DKS_GENERAL_TREES:
-    case DKS_GENERAL_KMACH:
-    case DKS_GENERAL_MLP:
-    case DKS_GENERAL_KNN:
-        TRY(launch_own_kernel(ctx, false, p, rt.smem, gstream));
-        break;
     default: {
+        if (ctx->head.own()) {
+            TRY(launch_own_kernel(ctx, false, p, rt.smem, gstream));
+            break;
+        }
         const bool mixh = ctx->head.mixture();
         auto skern = ctx->head.expo ? dks::explain_simt_kernel<false, true> : dks::explain_simt_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(mixh ? (const void*)dks::mix::explain_simt_mix_kernel<false> : (const void*)skern,
@@ -1692,12 +1656,9 @@ int dks_destroy(dks_ctx* ctx) {
     if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
     dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b); dev_free(&ctx->d_mix);
     dev_free(&ctx->d_mixBW); dev_free(&ctx->d_mixsc); dev_free(&ctx->d_mixscr);
-    free_tree(ctx);
-    free_encoding(ctx);
+    free_own_model(ctx);
+    dev_free(&ctx->tree.xinfo);
     dev_free(&ctx->d_Xenc);
-    free_kmach(ctx);
-    free_mlp(ctx);
-    free_knn(ctx);
     free_column_maps(ctx);
     dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
     dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
@@ -1887,13 +1848,7 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
     ctx->h_troots.assign(roots, roots + n_trees);
     ctx->h_tbase.assign(base, base + R);
     ctx->tree.nodes = n_nodes; ctx->tree.T = n_trees; ctx->tree.R = R; ctx->tree.head = head; ctx->tree.cmp = cmp;
-    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
-    ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_TREES; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
-    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
-    ctx->h_W.assign((size_t)ctx->D, 0.0);
-    ctx->h_b.assign(1, 0.0);
-    ctx->fitted = false;
-    return DKS_OK;
+    return set_own_model(ctx, DKS_ACT_TREES, C, scalar_out);
 }
 
 int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const double* sv, const double* dual, int R,
@@ -1905,10 +1860,6 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
     REQUIRE(sv_off && sv && dual && intercept && colw && colo && gamma,
             "dks_set_kernel_machine: need the support vectors, dual coefficients, intercepts, column weights and gamma");
     const int D = model_columns(ctx);
-    auto finite = [](const double* a, size_t n) {
-        for (size_t e = 0; e < n; ++e) if (!std::isfinite(a[e])) return false;
-        return true;
-    };
     if (K < 1 || K > DKS_KM_MAX_K)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: K=%d members; 1..%d supported", K, DKS_KM_MAX_K);
     if (R < 1 || R > DKS_KM_MAX_R)
@@ -1924,7 +1875,7 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
         C = R;
     } else if (head == DKS_KM_HEAD_CALIBRATED) {
         if (R != 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the calibrated head needs R == 1 (got %d)", R);
-        if (!cal_a || !cal_b || !pi || !finite(cal_a, K) || !finite(cal_b, K))
+        if (!cal_a || !cal_b || !pi || !all_finite(cal_a, K) || !all_finite(cal_b, K))
             return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the calibrated head needs finite a, b and pi");
         C = 2;
     } else {
@@ -1936,8 +1887,8 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
             return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: sv_off must not decrease (member %d)", m);
     const int n_sv = sv_off[K];
     if (n_sv < 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: no support vectors");
-    if (!finite(sv, (size_t)n_sv * D) || !finite(dual, (size_t)n_sv * R) || !finite(intercept, (size_t)K * R) ||
-        !finite(colw, (size_t)K * D) || !finite(colo, (size_t)K * D) || !finite(gamma, K))
+    if (!all_finite(sv, (size_t)n_sv * D) || !all_finite(dual, (size_t)n_sv * R) || !all_finite(intercept, (size_t)K * R) ||
+        !all_finite(colw, (size_t)K * D) || !all_finite(colo, (size_t)K * D) || !all_finite(gamma, K))
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the arrays must be finite");
     for (size_t e = 0; e < (size_t)K * D; ++e)
         if (!(colw[e] > 0)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: column weights must be positive");
@@ -1964,13 +1915,7 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
     ctx->h_kdual.assign(dual, dual + (size_t)n_sv * R);
     ctx->h_kcolw.assign(colw, colw + (size_t)K * D);
     ctx->h_kcolo.assign(colo, colo + (size_t)K * D);
-    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
-    ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_KMACH; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
-    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
-    ctx->h_W.assign((size_t)ctx->D, 0.0);
-    ctx->h_b.assign(1, 0.0);
-    ctx->fitted = false;
-    return DKS_OK;
+    return set_own_model(ctx, DKS_ACT_KMACH, C, scalar_out);
 }
 
 int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double* W_host, const double* b_host, int activation,
@@ -2021,10 +1966,8 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
         nbp += (size_t)m.pad[l + 1];
     }
     if (nw > (size_t)INT32_MAX) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: %zu weights are too many", nw);
-    for (size_t e = 0; e < nw; ++e)
-        if (!std::isfinite(W_host[e])) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the weights must be finite");
-    for (size_t e = 0; e < nb; ++e)
-        if (!std::isfinite(b_host[e])) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the biases must be finite");
+    if (!all_finite(W_host, nw)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the weights must be finite");
+    if (!all_finite(b_host, nb)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_mlp: the biases must be finite");
     m.nbuf = n_hidden >= 2 ? 2 : 1;
     m.hmax = 16;
     for (int l = 1; l < L; ++l) m.hmax = std::max(m.hmax, m.pad[l]);
@@ -2045,16 +1988,8 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
     }
     ctx->h_mw.assign(W_host, W_host + nw);
     ctx->h_mb.assign(b_host, b_host + nb);
-    // the previous device copies stay owned until dks_fit replaces them
-    m.W = ctx->mlp.W; m.b = ctx->mlp.b; m.Wf = ctx->mlp.Wf; m.bp = ctx->mlp.bp; m.Bbg = ctx->mlp.Bbg;
     ctx->mlp = m;
-    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
-    ctx->R = 1; ctx->C = C; ctx->act = DKS_ACT_MLP; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
-    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
-    ctx->h_W.assign((size_t)ctx->D, 0.0);
-    ctx->h_b.assign(1, 0.0);
-    ctx->fitted = false;
-    return DKS_OK;
+    return set_own_model(ctx, DKS_ACT_MLP, C, scalar_out);
 }
 
 int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double* colw, const double* colo, int k, int metric,
@@ -2063,10 +1998,6 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
     REQUIRE(ctx->D > 0, "dks_set_knn_model: call dks_set_background first (D unknown)");
     REQUIRE(fitX && colw && colo && labels_or_targets, "dks_set_knn_model: need the training rows, column map and labels");
     const int D = model_columns(ctx);
-    auto finite = [](const double* a, size_t n) {
-        for (size_t e = 0; e < n; ++e) if (!std::isfinite(a[e])) return false;
-        return true;
-    };
     if (k < 1 || k > DKS_KNN_MAX_K)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: k=%d neighbours; 1..%d supported", k, DKS_KNN_MAX_K);
     if (n_fit < k)
@@ -2084,7 +2015,7 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: R=%d %s; %d..%d supported", R,
                     head == DKS_KNN_HEAD_CLASSIFY ? "classes" : "targets", Rmin, DKS_KNN_MAX_R);
     const size_t ny = head == DKS_KNN_HEAD_CLASSIFY ? (size_t)n_fit : (size_t)n_fit * R;
-    if (!finite(fitX, (size_t)n_fit * D) || !finite(colw, D) || !finite(colo, D) || !finite(labels_or_targets, ny))
+    if (!all_finite(fitX, (size_t)n_fit * D) || !all_finite(colw, D) || !all_finite(colo, D) || !all_finite(labels_or_targets, ny))
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: the arrays must be finite");
     for (int c = 0; c < D; ++c)
         if (colw[c] == 0) return fail(DKS_ERR_UNSUPPORTED, "dks_set_knn_model: column weights must be non-zero");
@@ -2100,13 +2031,7 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
     ctx->h_ncolw.assign(colw, colw + D);
     ctx->h_ncolo.assign(colo, colo + D);
     ctx->h_ny.assign(labels_or_targets, labels_or_targets + ny);
-    // the linear part stage 1 evaluates while it decides the varying groups: one zero score row
-    ctx->R = 1; ctx->C = R; ctx->act = DKS_ACT_KNN; ctx->kappa = 1.0; ctx->scalar_out = scalar_out;
-    ctx->h_cm_hdr.clear(); ctx->h_cm_keys.clear(); ctx->h_cm_vals.clear();
-    ctx->h_W.assign((size_t)ctx->D, 0.0);
-    ctx->h_b.assign(1, 0.0);
-    ctx->fitted = false;
-    return DKS_OK;
+    return set_own_model(ctx, DKS_ACT_KNN, R, scalar_out);
 }
 
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
@@ -2118,15 +2043,8 @@ int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, con
         return DKS_OK;
     }
     REQUIRE(ctx->R > 0, "dks_set_column_maps: call dks_set_model first");
-    if (ctx->act == DKS_ACT_TREES) return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for tree ensembles");
-    if (ctx->act == DKS_ACT_KMACH)
-        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for kernel machines (their scalers fold into the support "
-                    "vectors and column weights)");
-    if (ctx->act == DKS_ACT_MLP)
-        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for MLPs (their scalers fold into the first layer)");
-    if (ctx->act == DKS_ACT_KNN)
-        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for nearest-neighbour models (their scalers fold into the "
-                    "column weights and origins)");
+    const OwnKernel ok = own_kernel(describe_head(ctx).family);
+    if (ok.family) return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: not for %s%s", ok.family, ok.maps_note);
     if (D != ctx->D || R != ctx->R)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_maps: maps of %d columns x %d score rows, model has %d x %d", D, R,
                     ctx->D, ctx->R);
@@ -2165,10 +2083,9 @@ int dks_set_column_encoding(dks_ctx* ctx, int E, const int32_t* hdr_host, const 
         return DKS_OK;
     }
     REQUIRE(ctx->D > 0, "dks_set_column_encoding: call dks_set_background first (D unknown)");
-    if (ctx->act >= 0 && ctx->act != DKS_ACT_TREES && ctx->act != DKS_ACT_KMACH && ctx->act != DKS_ACT_MLP &&
-        ctx->act != DKS_ACT_KNN)
-        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: for tree ensembles only (linear models read their "
-                    "pipelines through dks_set_column_maps)");
+    if (ctx->act >= 0 && !describe_head(ctx).own())
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: for models with their own kernels only (linear models read "
+                    "their pipelines through dks_set_column_maps)");
     if (E < 1 || n_ops < 0 || n_tab < 0 || (n_ops > 0 && (!ops_host || !opvals_host)) || (n_tab > 0 && !tab_host))
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_column_encoding: bad sizes");
     for (int e = 0; e < E; ++e) {
@@ -2222,9 +2139,7 @@ int dks_encode_host(dks_ctx* ctx, const double* X_host, int n, double* out_host)
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     cudaFree(dX); cudaFree(dO);
-    if (ctx->h_status[0] == DKS_ERR_DOMAIN)
-        return ctx->head.own() ? fail_refused(ctx, "row")
-                               : fail(DKS_ERR_DOMAIN, "row %d %s", ctx->h_status[1], refusal_phrase(false, true));
+    if (ctx->h_status[0] == DKS_ERR_DOMAIN) return fail_refused(ctx, "row");
     return DKS_OK;
 }
 
@@ -2263,12 +2178,10 @@ int dks_fit(dks_ctx* ctx) {
             REQUIRE(seen[c]++ == 0, "column %d appears in more than one group", c);
         }
     }
-    if (!h.own() && !ctx->h_ehdr.empty())
-        return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model is not a tree ensemble");
-    if (h.trees) return fit_trees(ctx);
-    if (h.kmach) return fit_kmach(ctx);
-    if (h.mlp) return fit_mlp(ctx);
-    if (h.knn) return fit_knn(ctx);
+    if (h.own()) return fit_own(ctx);
+    if (!ctx->h_ehdr.empty())
+        return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model has no kernel of its own (linear "
+                    "models read their pipelines through dks_set_column_maps)");
     TRY(fit_begin(ctx));
     TRY(dev_alloc(&ctx->d_BW, (size_t)N * G * R));
     TRY(dev_alloc(&ctx->d_scores, (size_t)N * R));
@@ -2348,30 +2261,15 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     TRY(dev_alloc(&dO, (size_t)n * ctx->C));
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
-    // a model with its own kernel behind a column encoding reads the encoded rows
-    double* dXe = nullptr;
-    if (ctx->head.own() && ctx->enc.E > 0) {
-        TRY(dev_alloc(&dXe, (size_t)n * ctx->enc.E));
-        TRY(launch_encode(ctx, dX, n, dXe));
-    }
-    const double* Xo = dXe ? dXe : dX;
-    const int Do = dXe ? ctx->enc.E : ctx->D;
-    if (ctx->head.trees)
-        dks::trees::tree_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->tree, ctx->C, ctx->link,
-                                                                               nullptr, dO, nullptr, nullptr);
-    else if (ctx->head.kmach)
-        dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->km, ctx->C, ctx->link,
-                                                                             nullptr, dO, nullptr, ctx->d_status);
-    else if (ctx->head.mlp)
-        dks::mlp::mlp_predict_kernel<<<mlp_predict_grid(ctx, n), dks::mlp::THREADS, 0, ctx->stream>>>(
-            Xo, n, Do, ctx->mlp, ctx->C, ctx->link, nullptr, dO, nullptr, ctx->d_status);
-    else if (ctx->head.knn)
-        dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, ctx->stream>>>(Xo, n, Do, ctx->knn, ctx->C, ctx->link,
-                                                                           nullptr, dO, nullptr, ctx->d_status);
-    else
+    double* dXe = nullptr;             // a model with its own kernel behind a column encoding reads the encoded rows
+    if (ctx->head.own()) {
+        if (ctx->enc.E > 0) TRY(dev_alloc(&dXe, (size_t)n * ctx->enc.E));
+        TRY(launch_own_predict(ctx, dX, n, dXe, nullptr, dO, nullptr));
+    } else {
         (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
             dX, ctx->d_W, ctx->d_b, n, ctx->D, ctx->R, ctx->C, ctx->act, ctx->kappa, dO, ctx->cm, ctx->d_status, ctx->d_mix);
-    ctx->launches += 1;
+        ctx->launches += 1;
+    }
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(out_host, dO, sizeof(double) * n * ctx->C, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));

@@ -242,12 +242,10 @@ struct HeadDesc {
     int simt_R = 1, simt_C = 1; // score rows and outputs the CUDA-core kernel stages
     bool wide_pi = false;       // per-instance plans of 65..128 groups
     bool tc = false;            // tensor-core kernel
-    bool trees = false;         // tree ensemble: the tree kernels only (dks_trees.cuh)
-    bool kmach = false;         // kernel machine: the kernel-machine kernels only (dks_kmach.cuh)
-    bool mlp = false;           // multi-layer perceptron: the MLP kernels only (dks_mlp.cuh)
-    bool knn = false;           // k-nearest neighbours: the neighbour kernels only (dks_knn.cuh)
+    int family = DKS_GENERAL_NONE;  // a model family whose every instance runs its own kernels: its DKS_GENERAL_* (tree
+                                    // ensembles, kernel machines, MLPs, neighbour models; own_kernel, dks.cu)
     bool mixture() const { return shared == HEAD_SHARED_MIX_BINARY || shared == HEAD_SHARED_MIX_CLASS; }
-    bool own() const { return trees || kmach || mlp || knn; }   // a family whose every instance runs its own kernel
+    bool own() const { return family != DKS_GENERAL_NONE; }
 };
 
 // Tables derived from the plan of the full varying set (M == G) that PlanDev does not hold: the class-sum heads' per-class
@@ -322,6 +320,10 @@ struct dks_ctx {
     // k-nearest neighbours (act == DKS_ACT_KNN): host copies of the arrays, and their device copies built by dks_fit
     std::vector<double> h_nfitX, h_ncolw, h_ncolo, h_ny;
     KnnDev knn = {};
+    // every device array dks_fit builds for a family with its own kernel (the pointers of tree, km, mlp, knn, enc, d_bg_enc,
+    // d_egoff, d_egcols), freed together by the next dks_fit or dks_destroy.  No kernel reads one after that: freeing
+    // clears fitted and prepared, and every launch needs them.
+    std::vector<void*> own_allocs;
     std::vector<double> h_bg, h_wbg, h_W, h_b;
     std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
     std::vector<double> h_cm_keys, h_cm_vals;

@@ -233,6 +233,18 @@ __global__ void fit_fnull_kernel(const double* __restrict__ scores, const double
     }
 }
 
+// fnull[c] = sum_j w_j pred[j][c] in row order and linkfnull = link(fnull), from the background's predictions of a model with
+// its own kernel; one block
+__global__ void fit_pred_fnull_kernel(const double* __restrict__ pred, const double* __restrict__ wbg, int N, int C, int link,
+                                      double* __restrict__ fnull, double* __restrict__ linkfnull) {
+    const int c = threadIdx.x;
+    if (c >= C) return;
+    double acc = 0;
+    for (int j = 0; j < N; ++j) acc += pred[(size_t)j * C + c] * wbg[j];
+    fnull[c] = acc;
+    linkfnull[c] = link_f(acc, link);
+}
+
 // scaled float copies consumed by the fused kernel: BWs[r][g][j] = scale*BW[j][g][r], bases[r][j] = scale*score
 // (fold_w, the exp head: bases[j] = scale*score + log2 w_j, so that 2^t carries the weight and a zero weight gives 2^-inf = 0)
 __global__ void fit_scale_kernel(const double* __restrict__ BW, const double* __restrict__ scores,
@@ -570,6 +582,23 @@ __device__ inline void wls_solve_write(const double* Lf, double* rhs, int M, dou
 // solve of the instance's outputs.  What the kernels compute between them is their own. ----
 __device__ __forceinline__ void report_status(int* status, int code, int detail) {
     if (atomicCAS(&status[0], 0, code) == 0) status[1] = detail;
+}
+
+// the end of a family's predict kernel for row i with outputs o[C]: out [i][C] = o and dlink [i][C] = link(o) - linkfnull,
+// each when not NULL.  A non-finite dlink is reported as DKS_ERR_NUMERIC with the instance unless the row was refused.
+__device__ __forceinline__ void predict_epilogue(const double* o, int C, int i, int link, const double* __restrict__ linkfnull,
+                                                 double* __restrict__ out, double* __restrict__ dlink, int* status,
+                                                 bool refused) {
+    bool bad = false;
+    for (int c = 0; c < C; ++c) {
+        if (out) out[(size_t)i * C + c] = o[c];
+        if (dlink) {
+            const double d = link_f(o[c], link) - linkfnull[c];
+            dlink[(size_t)i * C + c] = d;
+            bad |= !isfinite(d);
+        }
+    }
+    if (bad && !refused) report_status(status, DKS_ERR_NUMERIC, i);
 }
 
 // instance i's phi rows of every output start at zero: only the varying groups are written

@@ -81,20 +81,11 @@ __global__ void km_predict_kernel(const double* __restrict__ X, int n, int D, Km
     double o[DKS_KM_MAX_R];
     if (nan) {
         for (int c = 0; c < C; ++c) o[c] = NAN;
-        if (status && atomicCAS(&status[0], 0, DKS_ERR_DOMAIN) == 0) status[1] = i;
+        if (status) report_status(status, DKS_ERR_DOMAIN, i);
     } else {
         km_outputs(k, x, D, o);
     }
-    bool bad = false;
-    for (int c = 0; c < C; ++c) {
-        if (out) out[(size_t)i * C + c] = o[c];
-        if (dlink) {
-            const double d = link_f(o[c], link) - linkfnull[c];
-            dlink[(size_t)i * C + c] = d;
-            bad |= !isfinite(d);
-        }
-    }
-    if (bad && !nan && atomicCAS(&status[0], 0, DKS_ERR_NUMERIC) == 0) status[1] = i;
+    predict_epilogue(o, C, i, link, linkfnull, out, dlink, status, nan);
 }
 
 // fit: T[j][v] = sum_c h(bg_j,c, v_c) with the weights and origins of v's member, columns in order

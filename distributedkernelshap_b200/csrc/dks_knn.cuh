@@ -115,7 +115,7 @@ __global__ void knn_predict_kernel(const double* __restrict__ X, int n, int D, K
     double o[DKS_KNN_MAX_R];
     if (refused) {
         for (int c = 0; c < C; ++c) o[c] = NAN;
-        if (status && atomicCAS(&status[0], 0, DKS_ERR_DOMAIN) == 0) status[1] = i;
+        if (status) report_status(status, DKS_ERR_DOMAIN, i);
     } else {
         double lt[DKS_KNN_MAX_K];
         int li[DKS_KNN_MAX_K];
@@ -135,16 +135,7 @@ __global__ void knn_predict_kernel(const double* __restrict__ X, int n, int D, K
         }
         knn_outputs(k, lt, li, 1, o);
     }
-    bool bad = false;
-    for (int c = 0; c < C; ++c) {
-        if (out) out[(size_t)i * C + c] = o[c];
-        if (dlink) {
-            const double d = link_f(o[c], link) - linkfnull[c];
-            dlink[(size_t)i * C + c] = d;
-            bad |= !isfinite(d);
-        }
-    }
-    if (bad && !refused && atomicCAS(&status[0], 0, DKS_ERR_NUMERIC) == 0) status[1] = i;
+    predict_epilogue(o, C, i, link, linkfnull, out, dlink, status, refused);
 }
 
 // fit: T[j][v] = sum_c h(bg'_j,c - v_c), columns in order, and E[j][v] = the groups (bit g) on which bg'_j equals v exactly

@@ -85,16 +85,7 @@ __global__ void __launch_bounds__(THREADS) mlp_predict_kernel(const double* __re
             } else {
                 mlp_head(m.head, z, m.R, o);
             }
-            bool nonfinite = false;
-            for (int c = 0; c < C; ++c) {
-                if (out) out[(size_t)i * C + c] = o[c];
-                if (dlink) {
-                    const double d = link_f(o[c], link) - linkfnull[c];
-                    dlink[(size_t)i * C + c] = d;
-                    nonfinite |= !isfinite(d);
-                }
-            }
-            if (nonfinite && !refused) report_status(status, DKS_ERR_NUMERIC, i);
+            predict_epilogue(o, C, i, link, linkfnull, out, dlink, status, refused);
         }
     }
 }

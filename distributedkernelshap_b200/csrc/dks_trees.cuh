@@ -65,27 +65,7 @@ __global__ void tree_predict_kernel(const double* __restrict__ X, int n, int D, 
     double r[DKS_TREE_MAX_R], o[DKS_TREE_MAX_R];
     tree_raw(t, X + (size_t)i * D, r);
     tree_head(r, t.R, t.head, o);
-    bool bad = false;
-    for (int c = 0; c < C; ++c) {
-        if (out) out[(size_t)i * C + c] = o[c];
-        if (dlink) {
-            const double d = link_f(o[c], link) - linkfnull[c];
-            dlink[(size_t)i * C + c] = d;
-            bad |= !isfinite(d);
-        }
-    }
-    if (bad && atomicCAS(&status[0], 0, DKS_ERR_NUMERIC) == 0) status[1] = i;
-}
-
-// fnull[c] = sum_j w_j f(bg_j)[c] in row order, link(fnull); one block
-__global__ void tree_fnull_kernel(const double* __restrict__ pred, const double* __restrict__ wbg, int N, int C, int link,
-                                  double* __restrict__ fnull, double* __restrict__ linkfnull) {
-    const int c = threadIdx.x;
-    if (c >= C) return;
-    double acc = 0;
-    for (int j = 0; j < N; ++j) acc += pred[(size_t)j * C + c] * wbg[j];
-    fnull[c] = acc;
-    linkfnull[c] = link_f(acc, link);
+    predict_epilogue(o, C, i, link, linkfnull, out, dlink, status, false);
 }
 
 // fit: every background row's direction at every internal node, bgdir[j][node]

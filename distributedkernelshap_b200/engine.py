@@ -15,12 +15,12 @@ import numpy as np
 from . import _cabi
 from .data import DenseData, convert_to_data, convert_to_link
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
-from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, extract_kernel_machine_spec
-from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, extract_mlp_spec
-from .neighbors import MAX_GROUPS as KNN_MAX_GROUPS, extract_knn_spec
+from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, KernelMachineSpec, extract_kernel_machine_spec
+from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, MlpSpec, extract_mlp_spec
+from .neighbors import MAX_GROUPS as KNN_MAX_GROUPS, KnnSpec, extract_knn_spec
 from .predictors import extract_linear_spec
-from .trees import MAX_GROUPS as TREE_MAX_GROUPS, extract_encoded_pipeline_spec, extract_tree_pipeline_spec, \
-    extract_tree_spec
+from .trees import MAX_GROUPS as TREE_MAX_GROUPS, TreeEnsembleSpec, extract_encoded_pipeline_spec, \
+    extract_tree_pipeline_spec, extract_tree_spec
 
 logger = logging.getLogger(__name__)
 
@@ -172,11 +172,16 @@ class GpuKernelExplainer:
         # a model behind per-column preprocessing: explained in raw feature space, the device replaying the steps; the
         # extractors below pass its spec through
         target, self.encoding = pipe_spec if pipe_spec is not None else (model, None)
-        tree_spec = extract_tree_spec(target)
-        km_spec = extract_kernel_machine_spec(target) if tree_spec is None else None
-        mlp_spec = extract_mlp_spec(target) if tree_spec is None and km_spec is None else None
-        knn_spec = extract_knn_spec(target) if tree_spec is None and km_spec is None and mlp_spec is None else None
-        own = next((s for s in (tree_spec, km_spec, mlp_spec, knn_spec) if s is not None), None)   # its own kernel
+        # the model families with their own kernels: the first extractor that reads the model wins; the family's kernels
+        # cover at most max_groups groups.  Built per construction, so the module's extractors are looked up when it runs.
+        families = ((extract_tree_spec, TREE_MAX_GROUPS, "tree ensembles"),
+                    (extract_kernel_machine_spec, KMACH_MAX_GROUPS, "kernel machines"),
+                    (extract_mlp_spec, MLP_MAX_GROUPS, "MLPs"),
+                    (extract_knn_spec, KNN_MAX_GROUPS, "nearest-neighbour models"))
+        for extract, max_groups, family in families:
+            own = extract(target)
+            if own is not None:
+                break
         self.spec = own if own is not None else extract_linear_spec(model)
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
@@ -208,40 +213,31 @@ class GpuKernelExplainer:
         cols = np.ascontiguousarray(np.concatenate([np.asarray(g, dtype=np.int32) for g in self.data.groups]), dtype=np.int32)
         _cabi.check(self.lib.dks_set_groups(self._ctx, _cabi.ptr(offsets), _cabi.ptr(cols), self.data.groups_size))
         maps = self.spec.maps
-        if tree_spec is not None and self.data.groups_size > TREE_MAX_GROUPS:
-            raise NotImplementedError(f"{self.data.groups_size} groups: tree ensembles are explained up to "
-                                      f"{TREE_MAX_GROUPS} groups")
-        if km_spec is not None and self.data.groups_size > KMACH_MAX_GROUPS:
-            raise NotImplementedError(f"{self.data.groups_size} groups: kernel machines are explained up to "
-                                      f"{KMACH_MAX_GROUPS} groups")
-        if mlp_spec is not None and self.data.groups_size > MLP_MAX_GROUPS:
-            raise NotImplementedError(f"{self.data.groups_size} groups: MLPs are explained up to {MLP_MAX_GROUPS} groups")
-        if knn_spec is not None and self.data.groups_size > KNN_MAX_GROUPS:
-            raise NotImplementedError(f"{self.data.groups_size} groups: nearest-neighbour models are explained up to "
-                                      f"{KNN_MAX_GROUPS} groups")
+        if own is not None and self.data.groups_size > max_groups:
+            raise NotImplementedError(f"{self.data.groups_size} groups: {family} are explained up to {max_groups} groups")
         W = None if own is not None else \
             self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
         e = self.encoding
         if e is not None:               # before the model: its columns are the encoded ones
             _cabi.check(self.lib.dks_set_column_encoding(self._ctx, e.E, _cabi.ptr(e.hdr), _cabi.ptr(e.ops),
                                                          _cabi.ptr(e.opvals), len(e.ops), _cabi.ptr(e.tab), len(e.tab)))
-        if knn_spec is not None:
-            k = knn_spec
+        if isinstance(own, KnnSpec):
+            k = own
             _cabi.check(self.lib.dks_set_knn_model(
                 self._ctx, k.n_fit, _cabi.ptr(k.fitX), _cabi.ptr(k.colw), _cabi.ptr(k.colo), k.k, k.metric_code, k.p,
                 k.weights_code, k.R, _cabi.ptr(k.y), k.head_code, int(k.scalar_out)))
-        elif mlp_spec is not None:
-            widths, Wm, bm = mlp_spec.flat()
-            _cabi.check(self.lib.dks_set_mlp(self._ctx, mlp_spec.n_hidden, _cabi.ptr(widths), _cabi.ptr(Wm), _cabi.ptr(bm),
-                                             mlp_spec.act_code_hidden, mlp_spec.head_code, int(mlp_spec.scalar_out)))
-        elif km_spec is not None:
-            k = km_spec
+        elif isinstance(own, MlpSpec):
+            widths, Wm, bm = own.flat()
+            _cabi.check(self.lib.dks_set_mlp(self._ctx, own.n_hidden, _cabi.ptr(widths), _cabi.ptr(Wm), _cabi.ptr(bm),
+                                             own.act_code_hidden, own.head_code, int(own.scalar_out)))
+        elif isinstance(own, KernelMachineSpec):
+            k = own
             _cabi.check(self.lib.dks_set_kernel_machine(
                 self._ctx, k.K, _cabi.ptr(k.sv_off), _cabi.ptr(k.sv), _cabi.ptr(k.dual), k.R, _cabi.ptr(k.intercept),
                 _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree, k.coef0, k.head_code,
                 _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
-        elif tree_spec is not None:
-            t = tree_spec
+        elif isinstance(own, TreeEnsembleSpec):
+            t = own
             _cabi.check(self.lib.dks_set_tree_model(
                 self._ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
                 _cabi.ptr(t.missing_left), _cabi.ptr(t.value), t.R, t.n_trees, _cabi.ptr(t.roots), _cabi.ptr(t.base),
@@ -279,7 +275,7 @@ class GpuKernelExplainer:
         self._last_rows = 0
         if self.encoding is not None:
             self._check_encoding(bg)
-        self._check_model_against_callable(bg, knn_spec)
+        self._check_model_against_callable(bg, own if isinstance(own, KnnSpec) else None)
 
     # ------------------------------------------------------------------------------------------------------
     def encode(self, X):
