@@ -33,6 +33,7 @@ ACT_TREES = 6
 ACT_KMACH = 7
 ACT_MLP = 8
 ACT_KNN = 9
+ACT_ENSEMBLE = 10
 LINK_IDENTITY = 0
 LINK_LOGIT = 1
 KERNEL_AUTO = 0
@@ -60,6 +61,7 @@ SIGNATURES = {
     "dks_set_mlp": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "dks_set_knn_model": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int, C.c_double, C.c_int,
                                                                              C.c_int, C.c_void_p, C.c_int, C.c_int]),
+    "dks_set_ensemble": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "dks_set_column_maps": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "dks_set_column_encoding": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                           C.c_int]),

@@ -21,6 +21,7 @@
 #include "dks_kmach.cuh"
 #include "dks_mlp.cuh"
 #include "dks_knn.cuh"
+#include "dks_ensemble.cuh"
 
 namespace {
 
@@ -91,6 +92,8 @@ int drop_plans(dks_ctx* ctx, int M) {
 
 int bind(dks_ctx* ctx) {
     if (!ctx) return fail(DKS_ERR_INVALID, "null ctx");
+    if (ctx->ens_parent)
+        return fail(DKS_ERR_INVALID, "this context is a member of a soft-voting ensemble (dks_set_ensemble), which owns it");
     CUDA_TRY(cudaSetDevice(ctx->device));
     return DKS_OK;
 }
@@ -205,6 +208,11 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         // probabilities are not exact negations of each other in float64)
         h.family = DKS_GENERAL_KNN;
         break;
+    case DKS_ACT_ENSEMBLE:
+        // no shared-plan route: every instance runs the members' kernels and the ensemble's tail; every output is solved on
+        // its own
+        h.family = DKS_GENERAL_ENSEMBLE;
+        break;
     }
     if (h.shared != HEAD_SHARED_BINARY && !h.own()) h.shared_max_G = 128;
     if (!h.mixture()) h.xt_scale = h.scale;
@@ -248,6 +256,15 @@ int knn_chunk(const dks_ctx* ctx, int S_cap) {
     return (int)std::max(1LL, std::min((long long)S_cap, room / (long long)per));
 }
 
+OwnKernel own_kernel(int family);
+
+// shared memory of the widest launch of a soft-voting ensemble at S_cap rows: a member's explain kernel or the tail
+size_t ensemble_smem(const dks_ctx* ctx, int S_cap) {
+    size_t smem = dks::ens::tail_smem_bytes(S_cap, ctx->C);
+    for (const dks_ctx* m : ctx->ens) smem = std::max(smem, own_kernel(m->head.family).smem(m, S_cap));
+    return smem;
+}
+
 OwnKernel own_kernel(int family) {
     switch (family) {
     case DKS_GENERAL_TREES:
@@ -268,8 +285,35 @@ OwnKernel own_kernel(int family) {
                 " (their scalers fold into the column weights and origins)", REFUSES_NONFINITE,
                 [](const dks_ctx* c, int S_cap) {
                     return dks::knn::smem_bytes(S_cap, c->C, c->G, c->knn.k, knn_chunk(c, S_cap)); }};
+    case DKS_GENERAL_ENSEMBLE:          // refuses: what its members refuse (refusing_kernel)
+        return {"soft-voting ensembles", "ensemble kernels", "groups", "soft-voting ensemble",
+                " (put the preprocessing in front of the ensemble)", REFUSES_NONE, ensemble_smem};
     }
     return {};                          // a linear head
+}
+
+// the family whose refusal of raw values applies: the ensemble member that refuses the most (the first of them), else the
+// model's own
+OwnKernel refusing_kernel(const dks_ctx* ctx) {
+    OwnKernel ok = own_kernel(ctx->head.family);
+    if (ctx->head.family != DKS_GENERAL_ENSEMBLE) return ok;
+    for (const dks_ctx* m : ctx->ens) {
+        const OwnKernel mk = own_kernel(m->head.family);
+        if (mk.refuses > ok.refuses) ok = mk;
+    }
+    return ok;
+}
+
+// runs a launch function of ensemble member m: its kernel launches count as the ensemble's, and a workspace it moved changes
+// the ensemble's epoch (a captured graph holds the old address)
+template <typename F>
+int on_member(dks_ctx* ctx, dks_ctx* m, F&& launch) {
+    const int64_t launches = m->launches;
+    const unsigned epoch = m->epoch;
+    const int rc = launch();
+    ctx->launches += m->launches - launches;
+    if (m->epoch != epoch) ctx->epoch++;
+    return rc;
 }
 
 // a device array of n elements owned by the fitted model (own_allocs)
@@ -353,6 +397,7 @@ int check_own_columns(const dks_ctx* ctx, const OwnKernel& ok) {
         return DKS_OK;
     case DKS_GENERAL_KMACH: reads = (int)(ctx->h_kcolw.size() / ctx->km.K); break;
     case DKS_GENERAL_MLP: reads = ctx->mlp.width[0]; break;
+    case DKS_GENERAL_ENSEMBLE: return DKS_OK;         // each member checks its own (fit_members)
     default: reads = (int)ctx->h_ncolw.size(); break;
     }
     if (reads != width)
@@ -439,7 +484,7 @@ int own_fit_tables(dks_ctx* ctx, const double* bg, int width) {
 int launch_encode(dks_ctx* ctx, const double* X_dev, int n, double* out) {
     const long long total = (long long)n * ctx->enc.E;
     const int grid = (int)std::min<long long>(cdiv(total, 256), (long long)ctx->sm_count * 8);
-    auto kern = own_kernel(ctx->head.family).refuses == REFUSES_NONE ? dks::enc::encode_kernel : dks::enc::encode_finite_kernel;
+    auto kern = refusing_kernel(ctx).refuses == REFUSES_NONE ? dks::enc::encode_kernel : dks::enc::encode_finite_kernel;
     kern<<<grid, 256, 0, ctx->stream>>>(X_dev, n, ctx->D, ctx->enc, out, ctx->d_status);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
@@ -474,42 +519,79 @@ int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const
         dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->knn, C, link, linkfnull, out, dlink,
                                                                    ctx->d_status);
         break;
+    case DKS_GENERAL_ENSEMBLE: {    // every member's f_k(x) into d_ens_out [K][n][C], then f(x) = sum_k pi_k f_k(x)
+        const int K = (int)ctx->ens.size();
+        TRY(grow(ctx, &ctx->d_ens_out, &ctx->cap_ens_out, (size_t)K * n * C));
+        for (int k = 0; k < K; ++k) {
+            dks_ctx* m = ctx->ens[k];
+            double* outk = ctx->d_ens_out + (size_t)k * n * C;
+            TRY(on_member(ctx, m, [&] { return launch_own_predict(m, X, n, nullptr, nullptr, outk, nullptr); }));
+        }
+        dks::ens::ensemble_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(ctx->d_ens_out, K, ctx->d_ens_pi, n, C, link,
+                                                                        linkfnull, out, dlink, ctx->d_status);
+        break;
+    }
     }
     ctx->launches += 1;
     return DKS_OK;
 }
 
-// the family's explain kernel over p.list (L1: its moments); the tree kernel's per-CTA node scratch is sized for the grid
-int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st) {
+// the family's explain kernel over p.list (L1: its moments; ea.ey set: a soft-voting ensemble's member adding into its
+// workspace, the ACC instantiation); the tree kernel's per-CTA node scratch is sized for the grid.  A soft-voting ensemble:
+// its members in order, then its tail.
+int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st,
+                      const dks::EnsAcc& ea = dks::EnsAcc{}) {
     const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
     const dks::SimtL1 q = l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{};
+    const bool acc = ea.ey != nullptr;
     switch (ctx->head.family) {
     case DKS_GENERAL_TREES: {
         TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
-        auto kern = l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
+        auto kern = acc ? dks::trees::explain_tree_kernel<false, true>
+                        : l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->own_X, ctx->own_D);
+        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->own_X, ctx->own_D, ea);
         break;
     }
     case DKS_GENERAL_KMACH: {
-        auto kern = l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
+        auto kern = acc ? dks::kmach::explain_kmach_kernel<false, true>
+                        : l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->own_X, ctx->own_bg, ctx->own_D, ctx->own_goff,
-                                                      ctx->own_gcols);
+                                                      ctx->own_gcols, ea);
         break;
     }
     case DKS_GENERAL_MLP: {
-        auto kern = l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
+        auto kern = acc ? dks::mlp::explain_mlp_kernel<false, true>
+                        : l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
-                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols, ea);
         break;
     }
     case DKS_GENERAL_KNN: {
-        auto kern = l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
+        auto kern = acc ? dks::knn::explain_knn_kernel<false, true>
+                        : l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
-                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols);
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols, ea);
+        break;
+    }
+    case DKS_GENERAL_ENSEMBLE: {
+        TRY(grow(ctx, &ctx->d_ens_ey, &ctx->cap_ens_ey, (size_t)ctx->cur_n * ctx->C * p.S_cap));
+        for (size_t k = 0; k < ctx->ens.size(); ++k) {
+            dks_ctx* m = ctx->ens[k];
+            m->cur_n = ctx->cur_n;                  // the rows, background and group CSR of this call
+            m->own_X = ctx->own_X; m->own_D = ctx->own_D; m->own_bg = ctx->own_bg;
+            m->own_goff = ctx->own_goff; m->own_gcols = ctx->own_gcols;
+            const size_t msm = own_kernel(m->head.family).smem(m, p.S_cap);
+            const dks::EnsAcc mea{ctx->d_ens_ey, ctx->h_ens_pi[k], k == 0 ? 1 : 0};
+            TRY(on_member(ctx, m, [&] { return launch_own_kernel(m, false, p, msm, st, mea); }));
+        }
+        const size_t tsm = dks::ens::tail_smem_bytes(p.S_cap, ctx->C);
+        auto kern = l1 ? dks::ens::explain_ensemble_tail_kernel<true> : dks::ens::explain_ensemble_tail_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsm));
+        kern<<<persistent_grid(ctx, tsm, 1024, 8, ctx->cur_n), dks::ens::THREADS, tsm, st>>>(p, q, ctx->d_ens_ey);
         break;
     }
     }
@@ -756,7 +838,7 @@ int choose_route_own(dks_ctx* ctx, const uint64_t* ext_z, int ext_stride, Route*
 // DKS_ERR_DOMAIN for the row the status word names, worded for what refused it: the family's kernels, or the pipeline in
 // front of them; a tree's column encoding; a linear model's column maps
 int fail_refused(const dks_ctx* ctx, const char* prefix) {
-    const OwnKernel ok = own_kernel(ctx->head.family);
+    const OwnKernel ok = refusing_kernel(ctx);
     const int row = ctx->h_status[1];
     if (ok.refuses != REFUSES_NONE && ctx->enc.E > 0)
         return fail(DKS_ERR_DOMAIN, "%s %d holds a raw value the pipeline refuses (NaN where no imputer fills it, an "
@@ -868,6 +950,41 @@ int fit_encoding(dks_ctx* ctx) {
     return DKS_OK;
 }
 
+int fit_model(dks_ctx* ctx);
+
+// dks_fit of a soft-voting ensemble, after the common start: every member fitted, in order, on the ensemble's background,
+// weights, groups and column encoding (under the identity link: the ensemble takes its link of the weighted sum), then
+// fnull = sum_k pi_k fnull_k in member order and pi on the device
+int fit_members(dks_ctx* ctx, const OwnKernel& ok) {
+    const int C = ctx->C;
+    std::vector<double> fnull(C, 0.0), linkfnull(C);
+    for (size_t k = 0; k < ctx->ens.size(); ++k) {
+        dks_ctx* m = ctx->ens[k];
+        m->N = ctx->N; m->D = ctx->D; m->G = ctx->G;
+        m->h_bg = ctx->h_bg; m->h_wbg = ctx->h_wbg; m->uniform_w = ctx->uniform_w;
+        m->h_goff = ctx->h_goff; m->h_gcols = ctx->h_gcols;
+        m->h_ehdr = ctx->h_ehdr; m->h_eops = ctx->h_eops; m->h_eopv = ctx->h_eopv; m->h_etab = ctx->h_etab;
+        m->link = DKS_LINK_IDENTITY;
+        const int rc = on_member(ctx, m, [&] { return fit_model(m); });
+        if (rc != DKS_OK) return fail(rc, "soft-voting ensemble member %d: %s", (int)k, g_last_error.c_str());
+        for (int c = 0; c < C; ++c) fnull[c] += ctx->h_ens_pi[k] * m->h_fnull[c];
+    }
+    for (int c = 0; c < C; ++c) {
+        linkfnull[c] = ctx->link == DKS_LINK_LOGIT ? std::log(fnull[c] / (1.0 - fnull[c])) : fnull[c];
+        if (!std::isfinite(linkfnull[c]))
+            return fail(DKS_ERR_NUMERIC, "%s: link(fnull) of output %d is not finite (fnull = %g): the background's "
+                        "mean prediction is 0 or 1 under the logit link, or overflows", ok.model, c, fnull[c]);
+    }
+    const cudaStream_t st = ctx->stream;
+    TRY(own_upload(ctx, &ctx->d_ens_pi, ctx->h_ens_pi.data(), ctx->h_ens_pi.size()));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_fnull, fnull.data(), sizeof(double) * C, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_linkfnull, linkfnull.data(), sizeof(double) * C, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    ctx->h_fnull = fnull;
+    ctx->h_linkfnull = linkfnull;
+    return fit_done(ctx);
+}
+
 // dks_fit of a family with its own kernel: its column check, the common start, the column encoding, the family's arrays
 // and tables, and fnull = sum_j w_j f(bg_j) from its predict kernel
 int fit_own(dks_ctx* ctx) {
@@ -876,6 +993,7 @@ int fit_own(dks_ctx* ctx) {
     TRY(check_own_columns(ctx, ok));
     TRY(fit_begin(ctx));
     TRY(fit_encoding(ctx));
+    if (ctx->head.family == DKS_GENERAL_ENSEMBLE) return fit_members(ctx, ok);
     const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
     TRY(own_fit_tables(ctx, bg, model_columns(ctx)));
     double* pred = nullptr;
@@ -1584,6 +1702,101 @@ int build_link_table(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz) {
     return DKS_OK;
 }
 
+// dks_fit without the binding (a soft-voting ensemble fits its members through it)
+int fit_model(dks_ctx* ctx) {
+    REQUIRE(ctx->N > 0 && ctx->R > 0, "dks_fit: background and model must be set first");
+    const int N = ctx->N, D = ctx->D, R = ctx->R, C = ctx->C;
+    if (ctx->G == 0) {  // default: one singleton group per column (DenseData default)
+        if (D > DKS_MAX_GROUPS)
+            return fail(DKS_ERR_UNSUPPORTED, "D=%d ungrouped columns; this build handles at most %d groups", D, DKS_MAX_GROUPS);
+        ctx->G = D;
+        ctx->h_goff.resize(D + 1);
+        ctx->h_gcols.resize(D);
+        for (int c = 0; c <= D; ++c) ctx->h_goff[c] = c;
+        for (int c = 0; c < D; ++c) ctx->h_gcols[c] = c;
+    }
+    const int G = ctx->G;
+    ctx->head = describe_head(ctx);
+    const HeadDesc& h = ctx->head;
+    if (h.expo && ctx->link == DKS_LINK_LOGIT)
+        return fail(DKS_ERR_UNSUPPORTED, "exp head: the logit link is undefined wherever a predicted mean exceeds 1; use the "
+                    "identity link");
+    {   // every column in exactly one group
+        std::vector<int> seen(D, 0);
+        REQUIRE((int)ctx->h_gcols.size() == D, "groups cover %d columns but the data has %d", (int)ctx->h_gcols.size(), D);
+        for (int c : ctx->h_gcols) {
+            REQUIRE(c >= 0 && c < D, "group column %d out of range", c);
+            REQUIRE(seen[c]++ == 0, "column %d appears in more than one group", c);
+        }
+    }
+    if (h.own()) return fit_own(ctx);
+    if (!ctx->h_ehdr.empty())
+        return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model has no kernel of its own (linear "
+                    "models read their pipelines through dks_set_column_maps)");
+    TRY(fit_begin(ctx));
+    TRY(dev_alloc(&ctx->d_BW, (size_t)N * G * R));
+    TRY(dev_alloc(&ctx->d_scores, (size_t)N * R));
+    TRY(dev_alloc(&ctx->d_Bbar, (size_t)G * R));
+    TRY(dev_alloc(&ctx->d_BWs, (size_t)N * G * R));
+    TRY(dev_alloc(&ctx->d_bases, (size_t)N * R));
+    TRY(dev_alloc(&ctx->d_wbf, (size_t)N));
+    TRY(dev_alloc(&ctx->d_wn, (size_t)N));
+    TRY(dev_alloc(&ctx->d_mix, (size_t)1));
+    cudaStream_t st = ctx->stream;
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_mix, &ctx->mix, sizeof(MixHead), cudaMemcpyHostToDevice, st));
+    const bool maps = !ctx->h_cm_hdr.empty();
+    if (maps) {
+        const size_t nk = ctx->h_cm_keys.size(), nv = ctx->h_cm_vals.size();
+        int* hdr = nullptr;
+        double *keys = nullptr, *vals = nullptr;
+        TRY(dev_alloc(&hdr, ctx->h_cm_hdr.size()));
+        TRY(dev_alloc(&keys, nk));
+        TRY(dev_alloc(&vals, nv));
+        CUDA_TRY(cudaMemcpy(hdr, ctx->h_cm_hdr.data(), sizeof(int) * ctx->h_cm_hdr.size(), cudaMemcpyHostToDevice));
+        if (nk) CUDA_TRY(cudaMemcpy(keys, ctx->h_cm_keys.data(), sizeof(double) * nk, cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(vals, ctx->h_cm_vals.data(), sizeof(double) * nv, cudaMemcpyHostToDevice));
+        ctx->cm = ColumnMapsDev{hdr, keys, vals, (int)nk, (int)nv};
+    }
+    {
+        // the weighted shared-plan kernels read w'_j = N w_j: their sums then have the magnitude of the uniform ones
+        std::vector<float> wn(N);
+        for (int j = 0; j < N; ++j) wn[j] = (float)((double)N * ctx->h_wbg[j]);
+        CUDA_TRY(cudaMemcpy(ctx->d_wn, wn.data(), sizeof(float) * N, cudaMemcpyHostToDevice));
+    }
+    (maps ? (R > 8 ? dks::fit_bw_kernel<true, true> : dks::fit_bw_kernel<true>) : dks::fit_bw_kernel<false>)<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(
+        ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D, G, R, ctx->d_BW, ctx->cm, ctx->d_status);
+    dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
+    if (h.mixture()) {
+        TRY(dev_alloc(&ctx->d_mixBW, (size_t)N * G * R));
+        TRY(dev_alloc(&ctx->d_mixsc, (size_t)N * R));
+        dks::mix::mix_split_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, N, G, ctx->mix.K,
+                                                                                    ctx->mix.Rm, ctx->d_mixBW, ctx->d_mixsc);
+        ctx->launches += 1;
+    }
+    dks::fit_fnull_kernel<<<1, 256, 0, st>>>(ctx->d_scores, ctx->d_BW, ctx->d_wbg, N, G, R, C, ctx->act, ctx->kappa,
+                                              ctx->link, ctx->d_fnull, ctx->d_linkfnull, ctx->d_Bbar, ctx->d_mix);
+    dks::fit_scale_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, G, R,
+                                                                              h.scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf,
+                                                                              h.expo ? 1 : 0);
+    ctx->launches += 4;
+    TRY(fit_readback(ctx, nullptr));
+    if (h.expo && !std::isfinite(ctx->h_fnull[0]))
+        return fail(DKS_ERR_NUMERIC, "exp head: the background's predictions are not all finite in float64 (fnull = %g)",
+                    ctx->h_fnull[0]);
+    return fit_done(ctx);
+}
+
+// frees the members a soft-voting ensemble owns (their stream and status word are the ensemble's)
+void destroy_members(dks_ctx* ctx) {
+    for (dks_ctx* m : ctx->ens) {
+        m->ens_parent = nullptr;
+        m->d_status = nullptr; m->d_counts = nullptr; m->d_hist = nullptr;
+        dks_destroy(m);
+    }
+    ctx->ens.clear();
+    ctx->h_ens_pi.clear();
+}
+
 }  // namespace
 
 extern "C" {
@@ -1651,8 +1864,12 @@ int dks_create(dks_ctx** out, int device) {
 
 int dks_destroy(dks_ctx* ctx) {
     if (!ctx) return DKS_OK;
+    if (ctx->ens_parent)
+        return fail(DKS_ERR_INVALID, "dks_destroy: this context is a member of a soft-voting ensemble, which frees it");
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
+    destroy_members(ctx);
+    dev_free(&ctx->d_ens_out); dev_free(&ctx->d_ens_ey);
     if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
     dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b); dev_free(&ctx->d_mix);
     dev_free(&ctx->d_mixBW); dev_free(&ctx->d_mixsc); dev_free(&ctx->d_mixscr);
@@ -1689,6 +1906,7 @@ int dks_set_stream(dks_ctx* ctx, void* stream) {
     }
     ctx->stream = (cudaStream_t)stream;
     ctx->own_stream = false;
+    for (dks_ctx* m : ctx->ens) m->stream = ctx->stream;     // a soft-voting ensemble's members launch on its stream
     return DKS_OK;
 }
 
@@ -2034,6 +2252,53 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
     return set_own_model(ctx, DKS_ACT_KNN, R, scalar_out);
 }
 
+int dks_set_ensemble(dks_ctx* ctx, int K, dks_ctx* const* members, const double* weights, int C, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_ensemble: call dks_set_background first (D unknown)");
+    REQUIRE(members && weights, "dks_set_ensemble: need the members and their weights");
+    if (K < 1 || K > DKS_ENS_MAX_MEMBERS)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: K=%d members; 1..%d supported", K, DKS_ENS_MAX_MEMBERS);
+    if (C < 1 || C > DKS_ENS_MAX_OUT)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: C=%d outputs; 1..%d supported", C, DKS_ENS_MAX_OUT);
+    double wsum = 0;
+    for (int k = 0; k < K; ++k) {
+        if (!std::isfinite(weights[k]) || weights[k] < 0)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: weights must be finite and non-negative");
+        wsum += weights[k];
+    }
+    if (!(wsum > 0) || !std::isfinite(wsum))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: the weights must have a positive finite sum");
+    for (int k = 0; k < K; ++k) {
+        const dks_ctx* m = members[k];
+        REQUIRE(m && m != ctx && !m->ens_parent && m->ens.empty(),
+                "dks_set_ensemble: member %d must be a context of its own, not this one, another ensemble or its member", k);
+        for (int k2 = 0; k2 < k; ++k2) REQUIRE(members[k2] != m, "dks_set_ensemble: member %d appears twice", k);
+        REQUIRE(m->device == ctx->device, "dks_set_ensemble: member %d is on device %d, the ensemble on %d", k, m->device,
+                ctx->device);
+        if (m->act != DKS_ACT_TREES && m->act != DKS_ACT_KMACH && m->act != DKS_ACT_MLP && m->act != DKS_ACT_KNN)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: member %d is not a tree ensemble, kernel machine, MLP or "
+                        "neighbour model (dks_set_tree_model, dks_set_kernel_machine, dks_set_mlp, dks_set_knn_model)", k);
+        if (m->C != C)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: member %d gives %d outputs, the ensemble %d", k, m->C, C);
+    }
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    destroy_members(ctx);
+    for (int k = 0; k < K; ++k) {
+        dks_ctx* m = members[k];
+        CUDA_TRY(cudaStreamSynchronize(m->stream));
+        if (m->own_stream && m->stream) CUDA_TRY(cudaStreamDestroy(m->stream));
+        m->stream = ctx->stream;
+        m->own_stream = false;
+        dev_free(&m->d_status);
+        m->d_status = ctx->d_status; m->d_counts = ctx->d_counts; m->d_hist = ctx->d_hist;
+        m->head = describe_head(m);
+        m->ens_parent = ctx;
+        ctx->ens.push_back(m);
+        ctx->h_ens_pi.push_back(weights[k] / wsum);
+    }
+    return set_own_model(ctx, DKS_ACT_ENSEMBLE, C, scalar_out);
+}
+
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,
                         const double* vals_host, int n_vals) {
     BIND(ctx);
@@ -2153,88 +2418,8 @@ int dks_set_link(dks_ctx* ctx, int link) {
 
 int dks_fit(dks_ctx* ctx) {
     BIND(ctx);
-    REQUIRE(ctx->N > 0 && ctx->R > 0, "dks_fit: background and model must be set first");
-    const int N = ctx->N, D = ctx->D, R = ctx->R, C = ctx->C;
-    if (ctx->G == 0) {  // default: one singleton group per column (DenseData default)
-        if (D > DKS_MAX_GROUPS)
-            return fail(DKS_ERR_UNSUPPORTED, "D=%d ungrouped columns; this build handles at most %d groups", D, DKS_MAX_GROUPS);
-        ctx->G = D;
-        ctx->h_goff.resize(D + 1);
-        ctx->h_gcols.resize(D);
-        for (int c = 0; c <= D; ++c) ctx->h_goff[c] = c;
-        for (int c = 0; c < D; ++c) ctx->h_gcols[c] = c;
-    }
-    const int G = ctx->G;
-    ctx->head = describe_head(ctx);
-    const HeadDesc& h = ctx->head;
-    if (h.expo && ctx->link == DKS_LINK_LOGIT)
-        return fail(DKS_ERR_UNSUPPORTED, "exp head: the logit link is undefined wherever a predicted mean exceeds 1; use the "
-                    "identity link");
-    {   // every column in exactly one group
-        std::vector<int> seen(D, 0);
-        REQUIRE((int)ctx->h_gcols.size() == D, "groups cover %d columns but the data has %d", (int)ctx->h_gcols.size(), D);
-        for (int c : ctx->h_gcols) {
-            REQUIRE(c >= 0 && c < D, "group column %d out of range", c);
-            REQUIRE(seen[c]++ == 0, "column %d appears in more than one group", c);
-        }
-    }
-    if (h.own()) return fit_own(ctx);
-    if (!ctx->h_ehdr.empty())
-        return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model has no kernel of its own (linear "
-                    "models read their pipelines through dks_set_column_maps)");
-    TRY(fit_begin(ctx));
-    TRY(dev_alloc(&ctx->d_BW, (size_t)N * G * R));
-    TRY(dev_alloc(&ctx->d_scores, (size_t)N * R));
-    TRY(dev_alloc(&ctx->d_Bbar, (size_t)G * R));
-    TRY(dev_alloc(&ctx->d_BWs, (size_t)N * G * R));
-    TRY(dev_alloc(&ctx->d_bases, (size_t)N * R));
-    TRY(dev_alloc(&ctx->d_wbf, (size_t)N));
-    TRY(dev_alloc(&ctx->d_wn, (size_t)N));
-    TRY(dev_alloc(&ctx->d_mix, (size_t)1));
-    cudaStream_t st = ctx->stream;
-    CUDA_TRY(cudaMemcpyAsync(ctx->d_mix, &ctx->mix, sizeof(MixHead), cudaMemcpyHostToDevice, st));
-    const bool maps = !ctx->h_cm_hdr.empty();
-    if (maps) {
-        const size_t nk = ctx->h_cm_keys.size(), nv = ctx->h_cm_vals.size();
-        int* hdr = nullptr;
-        double *keys = nullptr, *vals = nullptr;
-        TRY(dev_alloc(&hdr, ctx->h_cm_hdr.size()));
-        TRY(dev_alloc(&keys, nk));
-        TRY(dev_alloc(&vals, nv));
-        CUDA_TRY(cudaMemcpy(hdr, ctx->h_cm_hdr.data(), sizeof(int) * ctx->h_cm_hdr.size(), cudaMemcpyHostToDevice));
-        if (nk) CUDA_TRY(cudaMemcpy(keys, ctx->h_cm_keys.data(), sizeof(double) * nk, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(vals, ctx->h_cm_vals.data(), sizeof(double) * nv, cudaMemcpyHostToDevice));
-        ctx->cm = ColumnMapsDev{hdr, keys, vals, (int)nk, (int)nv};
-    }
-    {
-        // the weighted shared-plan kernels read w'_j = N w_j: their sums then have the magnitude of the uniform ones
-        std::vector<float> wn(N);
-        for (int j = 0; j < N; ++j) wn[j] = (float)((double)N * ctx->h_wbg[j]);
-        CUDA_TRY(cudaMemcpy(ctx->d_wn, wn.data(), sizeof(float) * N, cudaMemcpyHostToDevice));
-    }
-    (maps ? (R > 8 ? dks::fit_bw_kernel<true, true> : dks::fit_bw_kernel<true>) : dks::fit_bw_kernel<false>)<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(
-        ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D, G, R, ctx->d_BW, ctx->cm, ctx->d_status);
-    dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
-    if (h.mixture()) {
-        TRY(dev_alloc(&ctx->d_mixBW, (size_t)N * G * R));
-        TRY(dev_alloc(&ctx->d_mixsc, (size_t)N * R));
-        dks::mix::mix_split_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, N, G, ctx->mix.K,
-                                                                                    ctx->mix.Rm, ctx->d_mixBW, ctx->d_mixsc);
-        ctx->launches += 1;
-    }
-    dks::fit_fnull_kernel<<<1, 256, 0, st>>>(ctx->d_scores, ctx->d_BW, ctx->d_wbg, N, G, R, C, ctx->act, ctx->kappa,
-                                              ctx->link, ctx->d_fnull, ctx->d_linkfnull, ctx->d_Bbar, ctx->d_mix);
-    dks::fit_scale_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, G, R,
-                                                                              h.scale, ctx->d_BWs, ctx->d_bases, ctx->d_wbf,
-                                                                              h.expo ? 1 : 0);
-    ctx->launches += 4;
-    TRY(fit_readback(ctx, nullptr));
-    if (h.expo && !std::isfinite(ctx->h_fnull[0]))
-        return fail(DKS_ERR_NUMERIC, "exp head: the background's predictions are not all finite in float64 (fnull = %g)",
-                    ctx->h_fnull[0]);
-    return fit_done(ctx);
+    return fit_model(ctx);
 }
-
 int dks_num_outputs(dks_ctx* ctx, int* C) {
     BIND(ctx);
     REQUIRE(C, "dks_num_outputs: NULL");

@@ -243,7 +243,8 @@ struct HeadDesc {
     bool wide_pi = false;       // per-instance plans of 65..128 groups
     bool tc = false;            // tensor-core kernel
     int family = DKS_GENERAL_NONE;  // a model family whose every instance runs its own kernels: its DKS_GENERAL_* (tree
-                                    // ensembles, kernel machines, MLPs, neighbour models; own_kernel, dks.cu)
+                                    // ensembles, kernel machines, MLPs, neighbour models, soft-voting ensembles of
+                                    // those; own_kernel, dks.cu)
     bool mixture() const { return shared == HEAD_SHARED_MIX_BINARY || shared == HEAD_SHARED_MIX_CLASS; }
     bool own() const { return family != DKS_GENERAL_NONE; }
 };
@@ -320,6 +321,15 @@ struct dks_ctx {
     // k-nearest neighbours (act == DKS_ACT_KNN): host copies of the arrays, and their device copies built by dks_fit
     std::vector<double> h_nfitX, h_ncolw, h_ncolo, h_ny;
     KnnDev knn = {};
+    // soft-voting ensemble (act == DKS_ACT_ENSEMBLE): the member contexts it owns, pi, its device copy (built by dks_fit), the
+    // members' predictions of a call [K][n][C] and their weighted background means [n][C][S_cap]; a member points at its
+    // ensemble, shares its stream and status word, and refuses every call of the C ABI
+    std::vector<dks_ctx*> ens;
+    std::vector<double> h_ens_pi;
+    const double* d_ens_pi = nullptr;
+    double *d_ens_out = nullptr, *d_ens_ey = nullptr;
+    size_t cap_ens_out = 0, cap_ens_ey = 0;
+    dks_ctx* ens_parent = nullptr;
     // every device array dks_fit builds for a family with its own kernel (the pointers of tree, km, mlp, knn, enc, d_bg_enc,
     // d_egoff, d_egcols), freed together by the next dks_fit or dks_destroy.  No kernel reads one after that: freeing
     // clears fitted and prepared, and every launch needs them.

@@ -993,6 +993,26 @@ __device__ __forceinline__ void moments_skip(const SimtL1& q, int G, int M, int 
     if ((int)threadIdx.x < nsolve) q.mom[(row0 + threadIdx.x) * (2 * (size_t)G + 4) + 2 * M] = NAN;
 }
 
+// a member of a soft-voting ensemble (instantiation ACC of the family explain kernels, DESIGN.md §5.0.17): in place of the
+// link and the solve, the member's background means of every output, times pi_k, are written (first member) or added to
+// the ensemble's workspace ey [n][C][S_cap]; explain_ensemble_tail_kernel solves from it
+struct EnsAcc {
+    double* ey;              // NULL: not a member
+    double pi;
+    int first;
+};
+
+// instance i's sums acc [C][S_cap] of S coalitions into ey; each thread handles the coalitions s = tid (mod blockDim.x)
+__device__ __forceinline__ void ens_accumulate(const EnsAcc& e, const ExplainParams& p, int i, int S, const double* acc) {
+    double* ey = e.ey + (size_t)i * p.C * p.S_cap;
+    for (int s = threadIdx.x; s < S; s += blockDim.x)
+        for (int c = 0; c < p.C; ++c) {
+            const size_t at = (size_t)c * p.S_cap + s;
+            const double v = e.pi * acc[at];
+            ey[at] = e.first ? v : ey[at] + v;
+        }
+}
+
 // exp head: ey(s) of one coalition row in float64, for the rows outside the fp32 range rule (DKS_EXP_T_LO / _HI):
 // exp(a + m + ln sum_j w_j e^(d_j - m)) with a = sum_{k in s} XW_i[k], d_j = score_j - sum_{k in s} BW[j][k] and m the
 // running maximum of d_j (one pass, the sum rescaled when m grows), zero-weight rows skipped.  Row bit k (k < M) is

@@ -217,11 +217,13 @@ __device__ __forceinline__ void forward_tile(const MlpDev& m, int KC1, uint64_t 
 // per solved output (sigmoid head: class 1, class 0 its negation) and the CUDA-core kernel's constrained WLS, or (L1) the
 // moments of y for l1_lars_kernel.  A non-finite y or f(x) is reported as DKS_ERR_NUMERIC and nothing of the instance is
 // written.
-template <bool L1>
+// ACC (a soft-voting ensemble's member): the sums of every output go into ea.ey instead (ens_accumulate); instances
+// with M <= 1 or a refused f(x) are left to explain_ensemble_tail_kernel.
+template <bool L1, bool ACC = false>
 __global__ void __launch_bounds__(THREADS) explain_mlp_kernel(ExplainParams p, SimtL1 q, MlpDev m, int nw,
                                                               const double* __restrict__ X, const double* __restrict__ bg,
                                                               int D, const int* __restrict__ goff,
-                                                              const int* __restrict__ gcols) {
+                                                              const int* __restrict__ gcols, EnsAcc ea) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int N = p.N, G = p.G, C = p.C;
@@ -247,13 +249,13 @@ __global__ void __launch_bounds__(THREADS) explain_mlp_kernel(ExplainParams p, S
         const int M = p.Mcnt[i];
         const uint64_t vm = p.vmask[i];
         __syncthreads();  // previous instance done with shared memory
-        zero_phi_rows(p, i);
+        if constexpr (!ACC) zero_phi_rows(p, i);
         bool fx_bad = false;                          // stage 1 reported a refused row or a non-finite link(f(x))
         for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
         if (M == 1) {
             // the one varying group takes link(f(x)) - link(fnull); sigmoid head: class 0 is the negation of class 1
-            if (tid < C && !fx_bad) {
+            if (!ACC && tid < C && !fx_bad) {
                 const double v = p.dlink[(size_t)i * C + (bin ? 1 : tid)];
                 p.phi[(size_t)tid * slab + (size_t)i * G + (__ffsll((long long)vm) - 1)] =
                     (bin && tid == 0) ? ((v == 0.0) ? 0.0 : -v) : v;
@@ -310,6 +312,10 @@ __global__ void __launch_bounds__(THREADS) explain_mlp_kernel(ExplainParams p, S
             }
         }
         __syncthreads();
+        if constexpr (ACC) {
+            ens_accumulate(ea, p, i, S, acc);
+            continue;
+        }
 
         // y = link(ey) - link(fnull) per solved output, written over the sums (row u of acc); under the logit link the
         // 1 - ey of a classifier is the sum of its other classes' sums (no cancellation)

@@ -93,10 +93,12 @@ __host__ __device__ inline size_t smem_bytes(int S_cap, int C, int R, int T) {
 //      bg_j's way elsewhere, add the constant, apply the head and accumulate w_j head(r) into the row's float64 sums.
 // Every sum runs in a fixed order: the result does not depend on the grid.  Then y = link(ey) - link(fnull) per solved output
 // (two outputs: class 1, class 0 its negation), and the CUDA-core kernel's constrained WLS, or (L1) the moments of y for
-// l1_lars_kernel.  A non-finite y or f(x) is reported as DKS_ERR_NUMERIC and nothing of the instance is written.
-template <bool L1>
+// l1_lars_kernel.  A non-finite y or f(x) is reported as DKS_ERR_NUMERIC and nothing of the instance is written.  ACC (a
+// soft-voting ensemble's member): the sums of every output go into ea.ey instead (ens_accumulate); instances with M <= 1
+// or a refused f(x) are left to explain_ensemble_tail_kernel.
+template <bool L1, bool ACC = false>
 __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, SimtL1 q, TreeDev t, const double* __restrict__ X,
-                                                               int D) {
+                                                               int D, EnsAcc ea) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int N = p.N, G = p.G, C = p.C, R = t.R, T = t.T, nodes = t.nodes;
@@ -118,13 +120,13 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
         const int M = p.Mcnt[i];
         const uint64_t vm = p.vmask[i];
         __syncthreads();  // previous instance done with shared memory and xi
-        zero_phi_rows(p, i);
+        if constexpr (!ACC) zero_phi_rows(p, i);
         bool fx_bad = false;                                    // stage 1 reported a non-finite link(f(x))
         for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
         if (M == 1) {
             // the one varying group takes link(f(x)) - link(fnull); two outputs: class 0 is the negation of class 1, as below
-            if (tid < C && !fx_bad) {
+            if (!ACC && tid < C && !fx_bad) {
                 const double v = p.dlink[(size_t)i * C + (C == 2 ? 1 : tid)];
                 p.phi[(size_t)tid * slab + (size_t)i * G + (__ffsll((long long)vm) - 1)] =
                     (C == 2 && tid == 0) ? ((v == 0.0) ? 0.0 : -v) : v;
@@ -209,6 +211,10 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
                 for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + s]);
             }
             __syncthreads();
+        }
+        if constexpr (ACC) {
+            ens_accumulate(ea, p, i, S, acc);
+            continue;
         }
 
         // y = link(ey) - link(fnull) per solved output, written over the sums (row u of acc); the logit's 1 - ey is the sum

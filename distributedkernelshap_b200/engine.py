@@ -14,6 +14,7 @@ import numpy as np
 
 from . import _cabi
 from .data import DenseData, convert_to_data, convert_to_link
+from .ensembles import MAX_GROUPS as ENSEMBLE_MAX_GROUPS, EnsembleSpec, extract_ensemble_spec
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
 from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, KernelMachineSpec, extract_kernel_machine_spec
 from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, MlpSpec, extract_mlp_spec
@@ -32,6 +33,9 @@ MAX_ROWS_PER_CALL_WIDE_PER_INSTANCE = 4096
 MAX_SAMPLED_SIZES = 64        # subset sizes the device sampler draws from (csrc/dks_sampler.cuh, MAX_SIZES)
 # a model behind a column encoding keeps the encoded rows of a call on the device (n x E x 8 B): row blocks bound them
 MAX_ENCODED_BYTES_PER_CALL = 256 << 20
+# a soft-voting ensemble keeps its members' weighted background means of a call on the device (n x C x S x 8 B): row
+# blocks bound them
+MAX_ENSEMBLE_BYTES_PER_CALL = 1 << 30
 
 
 def per_instance_workspace_bytes(M, S):
@@ -140,8 +144,10 @@ class GpuKernelExplainer:
         (``trees.extract_tree_pipeline_spec``: the device replays the steps bit for bit); a kernel machine; a
         scikit-learn MLP (``mlp.extract_mlp_spec``); a k-nearest-neighbour model (``neighbors.extract_knn_spec``); each of
         the last three bare, behind affine scalers (folded into the model) or behind such a ``Pipeline``
-        (``trees.extract_encoded_pipeline_spec``, replayed like a tree's).  A raw value the pipeline would refuse (NaN,
-        or an unseen category under ``handle_unknown='error'``) raises ``ValueError``.
+        (``trees.extract_encoded_pipeline_spec``, replayed like a tree's); a soft ``VotingClassifier`` or a
+        ``VotingRegressor`` mixing those families with linear members, bare or behind such a ``Pipeline``
+        (``ensembles.extract_ensemble_spec``).  A raw value the pipeline would refuse (NaN, or an unseen category under
+        ``handle_unknown='error'``) raises ``ValueError``.
     data
         Background data: array, DataFrame or ``DenseData`` (groups and weights honoured).
     link
@@ -166,15 +172,20 @@ class GpuKernelExplainer:
         self.lib = _cabi.load()
         self.link = convert_to_link(link)
         self.model_callable = model
-        pipe_spec = extract_tree_pipeline_spec(model)
-        if pipe_spec is None:
-            pipe_spec = extract_encoded_pipeline_spec(model)
+        # a soft-voting ensemble of the families below (bare: its spec; behind per-column preprocessing: with the encoding)
+        ens = extract_ensemble_spec(model)
+        pipe_spec = ens if isinstance(ens, tuple) else None
+        if ens is None:
+            pipe_spec = extract_tree_pipeline_spec(model)
+            if pipe_spec is None:
+                pipe_spec = extract_encoded_pipeline_spec(model)
         # a model behind per-column preprocessing: explained in raw feature space, the device replaying the steps; the
         # extractors below pass its spec through
-        target, self.encoding = pipe_spec if pipe_spec is not None else (model, None)
+        target, self.encoding = pipe_spec if pipe_spec is not None else (model if ens is None else ens, None)
         # the model families with their own kernels: the first extractor that reads the model wins; the family's kernels
         # cover at most max_groups groups.  Built per construction, so the module's extractors are looked up when it runs.
-        families = ((extract_tree_spec, TREE_MAX_GROUPS, "tree ensembles"),
+        families = ((lambda t: t if isinstance(t, EnsembleSpec) else None, ENSEMBLE_MAX_GROUPS, "soft-voting ensembles"),
+                    (extract_tree_spec, TREE_MAX_GROUPS, "tree ensembles"),
                     (extract_kernel_machine_spec, KMACH_MAX_GROUPS, "kernel machines"),
                     (extract_mlp_spec, MLP_MAX_GROUPS, "MLPs"),
                     (extract_knn_spec, KNN_MAX_GROUPS, "nearest-neighbour models"))
@@ -217,31 +228,11 @@ class GpuKernelExplainer:
             raise NotImplementedError(f"{self.data.groups_size} groups: {family} are explained up to {max_groups} groups")
         W = None if own is not None else \
             self.spec.W if maps is None else np.zeros((self.spec.R, self.P))
-        e = self.encoding
-        if e is not None:               # before the model: its columns are the encoded ones
-            _cabi.check(self.lib.dks_set_column_encoding(self._ctx, e.E, _cabi.ptr(e.hdr), _cabi.ptr(e.ops),
-                                                         _cabi.ptr(e.opvals), len(e.ops), _cabi.ptr(e.tab), len(e.tab)))
-        if isinstance(own, KnnSpec):
-            k = own
-            _cabi.check(self.lib.dks_set_knn_model(
-                self._ctx, k.n_fit, _cabi.ptr(k.fitX), _cabi.ptr(k.colw), _cabi.ptr(k.colo), k.k, k.metric_code, k.p,
-                k.weights_code, k.R, _cabi.ptr(k.y), k.head_code, int(k.scalar_out)))
-        elif isinstance(own, MlpSpec):
-            widths, Wm, bm = own.flat()
-            _cabi.check(self.lib.dks_set_mlp(self._ctx, own.n_hidden, _cabi.ptr(widths), _cabi.ptr(Wm), _cabi.ptr(bm),
-                                             own.act_code_hidden, own.head_code, int(own.scalar_out)))
-        elif isinstance(own, KernelMachineSpec):
-            k = own
-            _cabi.check(self.lib.dks_set_kernel_machine(
-                self._ctx, k.K, _cabi.ptr(k.sv_off), _cabi.ptr(k.sv), _cabi.ptr(k.dual), k.R, _cabi.ptr(k.intercept),
-                _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree, k.coef0, k.head_code,
-                _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
-        elif isinstance(own, TreeEnsembleSpec):
-            t = own
-            _cabi.check(self.lib.dks_set_tree_model(
-                self._ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
-                _cabi.ptr(t.missing_left), _cabi.ptr(t.value), t.R, t.n_trees, _cabi.ptr(t.roots), _cabi.ptr(t.base),
-                t.head_code, t.cmp, int(t.scalar_out)))
+        self._set_encoding(self._ctx)   # before the model: its columns are the encoded ones
+        if isinstance(own, EnsembleSpec):
+            self._set_ensemble(own, bg, weights)
+        elif own is not None:
+            self._set_own_model(self._ctx, own)
         elif self.spec.activation == "mixture":
             member = {"binary_logistic": _cabi.ACT_BINARY_LOGISTIC, "softmax": _cabi.ACT_SOFTMAX,
                       "ovr": _cabi.ACT_OVR}[self.spec.member]
@@ -275,7 +266,58 @@ class GpuKernelExplainer:
         self._last_rows = 0
         if self.encoding is not None:
             self._check_encoding(bg)
-        self._check_model_against_callable(bg, own if isinstance(own, KnnSpec) else None)
+        self._check_model_against_callable(bg, own if isinstance(own, (KnnSpec, EnsembleSpec)) else None)
+
+    def _set_encoding(self, ctx):
+        e = self.encoding
+        if e is not None:
+            _cabi.check(self.lib.dks_set_column_encoding(ctx, e.E, _cabi.ptr(e.hdr), _cabi.ptr(e.ops), _cabi.ptr(e.opvals),
+                                                         len(e.ops), _cabi.ptr(e.tab), len(e.tab)))
+
+    def _set_own_model(self, ctx, own):
+        """The family setter of the C ABI for a tree, kernel-machine, MLP or neighbour spec."""
+        if isinstance(own, KnnSpec):
+            k = own
+            _cabi.check(self.lib.dks_set_knn_model(
+                ctx, k.n_fit, _cabi.ptr(k.fitX), _cabi.ptr(k.colw), _cabi.ptr(k.colo), k.k, k.metric_code, k.p,
+                k.weights_code, k.R, _cabi.ptr(k.y), k.head_code, int(k.scalar_out)))
+        elif isinstance(own, MlpSpec):
+            widths, Wm, bm = own.flat()
+            _cabi.check(self.lib.dks_set_mlp(ctx, own.n_hidden, _cabi.ptr(widths), _cabi.ptr(Wm), _cabi.ptr(bm),
+                                             own.act_code_hidden, own.head_code, int(own.scalar_out)))
+        elif isinstance(own, KernelMachineSpec):
+            k = own
+            _cabi.check(self.lib.dks_set_kernel_machine(
+                ctx, k.K, _cabi.ptr(k.sv_off), _cabi.ptr(k.sv), _cabi.ptr(k.dual), k.R, _cabi.ptr(k.intercept),
+                _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree, k.coef0, k.head_code,
+                _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
+        else:
+            t = own
+            _cabi.check(self.lib.dks_set_tree_model(
+                ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
+                _cabi.ptr(t.missing_left), _cabi.ptr(t.value), t.R, t.n_trees, _cabi.ptr(t.roots), _cabi.ptr(t.base),
+                t.head_code, t.cmp, int(t.scalar_out)))
+
+    def _set_ensemble(self, spec, bg, weights):
+        """One context per member (its background and column encoding give the setter the model's width), handed to
+        ``dks_set_ensemble``, which owns them from then on."""
+        members = []
+        try:
+            for _, member in spec.members:
+                m = C.c_void_p()
+                _cabi.check(self.lib.dks_create(C.byref(m), self.device))
+                members.append(m)
+                _cabi.check(self.lib.dks_set_background(m, _cabi.ptr(bg), self.N, self.P, _cabi.ptr(weights)))
+                self._set_encoding(m)
+                self._set_own_model(m, member)
+            ptrs = (C.c_void_p * len(members))(*[m.value for m in members])
+            pi = np.ascontiguousarray(spec.weights, dtype=np.float64)
+            _cabi.check(self.lib.dks_set_ensemble(self._ctx, len(members), ptrs, _cabi.ptr(pi), spec.n_outputs,
+                                                  int(spec.scalar_out)))
+        except Exception:
+            for m in members:               # not handed over: still ours
+                self.lib.dks_destroy(m)
+            raise
 
     # ------------------------------------------------------------------------------------------------------
     def encode(self, X):
@@ -308,18 +350,23 @@ class GpuKernelExplainer:
                              "function")
 
     def _check_model_against_callable(self, bg, knn_spec=None):
-        """The extracted model must reproduce the user's callable on the background rows.  A neighbour model is compared
-        on the rows whose k-th and (k + 1)-th nearest training rows are not equidistant; a row with such a boundary tie
-        is compared with the spec's own NumPy evaluation instead (which of equidistant rows is a neighbour is the
-        engine's rule, not scikit-learn's), and at least one row must be compared with the callable."""
+        """The extracted model must reproduce the user's callable on the background rows.  A neighbour model (or a
+        soft-voting ensemble with neighbour members: ``knn_spec`` is then the ``EnsembleSpec``) is compared on the rows
+        whose k-th and (k + 1)-th nearest training rows are not equidistant in any neighbour model; a row with such a
+        boundary tie is compared with the spec's own NumPy evaluation instead (which of equidistant rows is a neighbour is
+        the engine's rule, not scikit-learn's), and at least one row must be compared with the callable."""
         if not callable(self.model_callable):
             return
         want = np.asarray(self.model_callable(bg), dtype=np.float64).reshape(self.N, -1)
         got = self.predict(bg)
-        if knn_spec is not None and want.shape == got.shape:
+        knns = [s for _, s in knn_spec.members if isinstance(s, KnnSpec)] if isinstance(knn_spec, EnsembleSpec) else \
+            [knn_spec] if knn_spec is not None else []
+        if knns and want.shape == got.shape:
             if self.encoding is not None:
                 bg = self.encode(bg)    # the spec reads the encoded columns
-            tied = knn_spec.boundary_ties(bg)
+            tied = np.zeros(self.N, dtype=bool)
+            for k in knns:
+                tied |= k.boundary_ties(bg)
             if tied.all():
                 raise ValueError("every background row has a tie between its k-th and (k + 1)-th nearest training rows: "
                                  "the neighbour model extracted from `predictor` cannot be checked against "
@@ -557,6 +604,10 @@ class GpuKernelExplainer:
         rows = rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size, self.spec.R)
         if self.encoding is not None:
             rows = min(rows, max(1, MAX_ENCODED_BYTES_PER_CALL // (8 * self.encoding.E)))
+        if isinstance(self.spec, EnsembleSpec):
+            # the members' weighted background means: C outputs x S rows per instance, S at most that of all G groups
+            S, _ = resolve_nsamples(self.data.groups_size, self._nsamples_req or "auto")
+            rows = min(rows, max(1, MAX_ENSEMBLE_BYTES_PER_CALL // (8 * self.D * (S + 2))))
         return rows
 
     def link_predictions(self):
@@ -739,7 +790,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp", "mixture"),
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble"),
     }
 
     def last_path(self):
@@ -752,7 +803,8 @@ class GpuKernelExplainer:
         are reported as unsupported, not computed, 'simt_wide': per-instance plans of 65..128 groups, 'trees': the tree
         kernel, which takes every instance of a tree ensemble, 'kmach': the kernel-machine kernel, which takes every
         instance of a kernel machine, 'mlp': the MLP kernel, which takes every instance of a multi-layer perceptron, or
-        'knn': the neighbour kernel, which takes every instance of a k-nearest-neighbour model),
+        'knn': the neighbour kernel, which takes every instance of a k-nearest-neighbour model, or 'ensemble': the
+        members' kernels and the ensemble's tail, which take every instance of a soft-voting ensemble),
         ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take

@@ -133,6 +133,9 @@ extern "C" {
 #define DKS_KNN_HEAD_REGRESS 1       /* R targets, outputs the weighted mean of the neighbours' targets (predict) */
 #define DKS_KNN_MAX_K 32             /* neighbours */
 #define DKS_KNN_MAX_R 8              /* classes or targets */
+#define DKS_ACT_ENSEMBLE 10    /* soft-voting ensemble of the four families above: set by dks_set_ensemble only */
+#define DKS_ENS_MAX_MEMBERS 16       /* members of a soft-voting ensemble */
+#define DKS_ENS_MAX_OUT 8            /* its outputs */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -246,6 +249,21 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
  * encoded columns. */
 int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double* colw, const double* colo, int k, int metric,
                       double p, int weights, int R, const double* labels_or_targets, int head, int scalar_out);
+/* soft-voting ensemble (DKS_ACT_ENSEMBLE) in place of dks_set_model: outputs f = sum_k pi_k f_k over K (1..DKS_ENS_MAX_MEMBERS)
+ * members, pi = weights / sum(weights) (finite, >= 0, positive sum), members in order.  members [K] are distinct contexts on
+ * the same device, each made by dks_create and one dks_set_tree_model / dks_set_kernel_machine / dks_set_mlp /
+ * dks_set_knn_model (with the dks_set_background and dks_set_column_encoding that setter needs to know the model's width),
+ * every one giving C (1..DKS_ENS_MAX_OUT) outputs.  The ensemble takes ownership: dks_destroy of the ensemble frees them,
+ * and every call on a member afterwards is DKS_ERR_INVALID.  dks_fit fits every member on the ensemble's background,
+ * weights, groups and column encoding; fnull = sum_k pi_k fnull_k.  All member launches go on the ensemble's stream.
+ * Every instance runs the members' explain kernels back to back (DKS_GENERAL_ENSEMBLE, DESIGN.md §5.0.17), each adding
+ * pi_k times its background means of every output into one workspace [n][C][S_cap], then explain_ensemble_tail_kernel takes
+ * the link and the solve, every output solved on its own: K + 1 launches per call (stage 1: K predict launches and one
+ * that forms f(x)).  Up to 64 groups, every plan source, kernel 'auto' or 'simt' (tcgen05 / shared are
+ * DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route.  A raw value any member refuses is
+ * DKS_ERR_DOMAIN with the row (NaN in an ensemble of trees only is explained); a link(ey) or link(f(x)) that is not finite
+ * is DKS_ERR_NUMERIC and nothing non-finite is written into phi. */
+int dks_set_ensemble(dks_ctx* ctx, int K, dks_ctx* const* members, const double* weights, int C, int scalar_out);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
  * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
  * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
@@ -471,6 +489,8 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_GENERAL_KMACH 6      /* explain_kmach_kernel: every instance of a kernel machine (dks_set_kernel_machine) */
 #define DKS_GENERAL_MLP 7        /* explain_mlp_kernel: every instance of a multi-layer perceptron (dks_set_mlp) */
 #define DKS_GENERAL_KNN 8        /* explain_knn_kernel: every instance of a nearest-neighbour model (dks_set_knn_model) */
+#define DKS_GENERAL_ENSEMBLE 9   /* the members' explain kernels, then explain_ensemble_tail_kernel: every instance of a
+                                  * soft-voting ensemble (dks_set_ensemble) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
