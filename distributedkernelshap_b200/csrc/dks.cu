@@ -1264,7 +1264,7 @@ int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, doubl
     sp.n = n; sp.N = ctx->N; sp.G = G; sp.S = pg.S; sp.S_pad = pg.S_pad; sp.scale = ctx->head.scale;
     sp.DmT = pg.dmT; sp.dme = pg.dme; sp.z = pg.z; sp.XT = ctx->d_XT; sp.list = ctx->d_idx_full; sp.count = ctx->d_counts; sp.sums = ctx->d_sums; sp.accumulate = 0;
     sp.acache = nullptr; sp.acache_mode = 0; sp.wn = wn;
-    if (pg.W > 2 && ctx->opt_wide_acache && ctx->N > dks::shared_path::MAXN) {
+    if (pg.W > 2 && ctx->N > dks::shared_path::MAXN) {
         // sixteen-word rows, several background chunks: A(i, s) is computed by the first chunk's launch only
         TRY(grow(ctx, &ctx->d_acache, &ctx->cap_acache, need));
         sp.acache = ctx->d_acache;
@@ -1274,7 +1274,7 @@ int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, doubl
         const int nl = dks::shared_path::launch_explain_shared(sp, pg.W, ctx->sm_count, ctx->max_smem_optin, ctx->stream, &sl);
         if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
         ctx->launches += nl;
-        path[DKS_PATH_SHARED] = sl.regs ? DKS_SHARED_REGS : DKS_SHARED_SMEM; path[DKS_PATH_CHUNKS] = sl.chunks;
+        path[DKS_PATH_SHARED] = DKS_SHARED_SMEM; path[DKS_PATH_CHUNKS] = sl.chunks;
         path[DKS_PATH_WARPS] = sl.warps; path[DKS_PATH_GRID] = sl.grid;
         return DKS_OK;
     }
@@ -1313,7 +1313,7 @@ int launch_binary_solve(dks_ctx* ctx, const Route& rt, const PlanDev& pg, double
         qp.sums = ctx->d_sums; qp.PT = pg.ptw; qp.dvec = pg.dvecw; qp.dlink = ctx->d_dlink;
         qp.linkfnull = ctx->d_linkfnull; qp.fnull = ctx->d_fnull; qp.list = ctx->d_idx_full; qp.count = ctx->d_counts;
         qp.y = ctx->d_yw; qp.beta = ctx->d_betaw; qp.phi = phi_dev;
-        CUDA_TRY(dks::wide::launch_wide_solve(qp, n, ctx->sm_count, ctx->opt_wide_gemm, ctx->stream));
+        CUDA_TRY(dks::wide::launch_wide_solve(qp, n, ctx->sm_count, ctx->stream));
         ctx->launches += 3;
     } else if (rt.solve == DKS_SOLVE_PMAT) {
         dks::shared_path::WlsPmatParams pp;
@@ -1597,7 +1597,7 @@ int check_status(dks_ctx* ctx) {
 // when it fits the solve kernel's staging
 int build_pmat(dks_ctx* ctx, PlanDev& pd, int M) {
     if (!(pd.W == 1 && M - 1 <= dks::shared_path::PMAT_MAXK &&
-          dks::shared_path::wls_pmat_smem(M, pd.S_pad, false) + 8192 <= (size_t)ctx->max_smem_optin))
+          dks::shared_path::wls_pmat_smem(M, pd.S_pad) + 8192 <= (size_t)ctx->max_smem_optin))
         return DKS_OK;
     const int S = pd.S;
     float* pm = nullptr; double* dv = nullptr;
@@ -1836,8 +1836,6 @@ int dks_create(dks_ctx** out, int device) {
         ctx->opt_fused_warps = env_int("DKS_FUSED_WARPS", 0);
         ctx->opt_fused_B = env_int("DKS_FUSED_B", 0);
         ctx->push_in_kernel = env_int("DKS_PUSH_IN_KERNEL", 0) != 0;
-        ctx->opt_wide_gemm = env_int("DKS_WIDE_GEMM", ctx->opt_wide_gemm) == 2 ? 2 : 1;
-        ctx->opt_wide_acache = env_int("DKS_WIDE_ACACHE", ctx->opt_wide_acache ? 1 : 0) != 0;
     }
     ctx->sm_count = prop.multiProcessorCount;
     ctx->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
@@ -3112,8 +3110,6 @@ int dks_set_option(dks_ctx* ctx, const char* name, int value) {
     else if (key == "push_in_kernel") ctx->push_in_kernel = value != 0;
     else if (key == "graph") ctx->graph_enabled = value != 0;
     else if (key == "graph_timing") ctx->opt_graph_timing = value != 0;
-    else if (key == "wide_gemm") ctx->opt_wide_gemm = value == 2 ? 2 : 1;
-    else if (key == "wide_acache") ctx->opt_wide_acache = value != 0;
     else return fail(DKS_ERR_INVALID, "dks_set_option: unknown option '%s'", name);
     ctx->epoch++;                      // a captured graph holds the old launch sequence
     return DKS_OK;

@@ -375,8 +375,6 @@ struct dks_ctx {
     size_t cap_yw = 0, cap_betaw = 0;
     float* d_acache = nullptr;   // [n][S_pad] A(i, s) of sixteen-word rows, shared by the launches of the background chunks
     size_t cap_acache = 0;
-    int opt_wide_gemm = 2;       // float64 product of the wide solve: 1 = first version, 2 = conflict-free 128 x 64 tiles
-    bool opt_wide_acache = true; // A(i, s) computed by the first background chunk's launch only (measured: DESIGN.md 5.5)
     // per-instance plans drawn on the device (plan_mode 1)
     int plan_mode = 0;
     uint64_t sampler_seed = 0;

@@ -6,10 +6,9 @@
 // so  2^t = A(i, s) * Dm(s, j)  with Dm = 2^d independent of the instance.  Dm (S x N floats, 0.8 MB for Adult) is
 // computed once per plan, row-normalised; a warp owns 32 coalition rows and streams the instances through them.  Two
 // elements share a reciprocal,  p1a + p1b = (2 + sm) / (1 + sm + q),  sm = A (Dma + Dmb),  q = A^2 (Dma Dmb),  so what the
-// kernel keeps per row are the pair sums and pair products of Dm -- in SHARED MEMORY (explain_shared_smem_kernel, the
-// default) or, in the first version kept for comparisons, the raw row in registers (explain_shared_kernel,
-// DKS_SHARED_DM=regs).  No GEMM, no EX2 per element: 3.5 fp32 ops + 0.5 MUFU.  Output: (sum p1, sum p0) per
-// (instance, coalition); wls_pmat_kernel / wls_shared_kernel apply the link and solve with what the plan precomputed.
+// kernel keeps per row are the pair sums and pair products of Dm, in shared memory (explain_shared_smem_kernel).  No
+// GEMM, no EX2 per element: 3.5 fp32 ops + 0.5 MUFU.  Output: (sum p1, sum p0) per (instance, coalition);
+// wls_pmat_kernel / wls_shared_kernel apply the link and solve with what the plan precomputed.
 // Instances with a partial varying set, per-instance plans and other heads go through the general kernels.
 #pragma once
 
@@ -18,8 +17,7 @@
 namespace dks {
 namespace shared_path {
 
-constexpr int MAXN = 128;            // background rows per launch (a warp's slice of shared memory / a lane's registers)
-constexpr int WARPS_PER_CTA = 12;
+constexpr int MAXN = 128;            // background rows per launch (a warp's slice of shared memory)
 constexpr float U_CLAMP = 1.152921504606846976e18f;   // 2^60: (1 + ua)(1 + ub) stays finite in fp32
 
 // d(s, j) = scale * (score_j - sum_k z_sk BW[j][k])  for the full varying set (k = group index), in log2 units.
@@ -92,145 +90,12 @@ __device__ __forceinline__ void single_acc(float A, float dma, float& a1, float&
     a0 = fmaf(ua, r, a0);
 }
 
-// Four sigmoids (two pairs, each sharing one reciprocal) in packed arithmetic: da = (dm0, dm1), db = (dm2, dm3) pair up as
-// (0,2) and (1,3).  10 packed ops + 2 MUFU per four elements (pair_acc: 11 + 1 per two).
-__device__ __forceinline__ void quad_acc(f32x2 A2, f32x2 da, f32x2 db, f32x2 one2, f32x2 two2, f32x2& a1, f32x2& a0) {
-    const f32x2 u = f2_mul(A2, da), v = f2_mul(A2, db);
-    const f32x2 q = f2_mul(u, v), sm = f2_add(u, v);
-    const f32x2 t1 = f2_add(sm, one2);
-    const f32x2 den = f2_add(q, t1);
-    float dlo, dhi;
-    f2_unpack(den, dlo, dhi);
-    const f32x2 r = f2_pack(rcp_approx(dlo), rcp_approx(dhi));
-    a1 = f2_fma(r, f2_add(t1, one2), a1);
-    a0 = f2_fma(r, f2_fma(two2, q, sm), a0);
-}
-
-// NTAIL = N % 16 (compile time): the last, partial chunk is straight-line code
-template <bool CLAMP, int NTAIL>
-__device__ __forceinline__ void row_sums(const float (&dm)[MAXN], float A, int nfull, float& s1, float& s0) {
-    float acc1[4] = {0.f, 0.f, 0.f, 0.f}, acc0[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int c = 0; c < MAXN / 16; ++c) {
-        if (c < nfull) {
-#pragma unroll
-            for (int jj = 0; jj < 16; jj += 2)
-                pair_acc<CLAMP>(A, dm[c * 16 + jj], dm[c * 16 + jj + 1], acc1[(jj >> 1) & 3], acc0[(jj >> 1) & 3]);
-        } else if (NTAIL > 0 && c == nfull) {
-#pragma unroll
-            for (int jj = 0; jj + 1 < NTAIL; jj += 2)
-                pair_acc<CLAMP>(A, dm[c * 16 + jj], dm[c * 16 + jj + 1], acc1[(jj >> 1) & 3], acc0[(jj >> 1) & 3]);
-            if (NTAIL & 1) single_acc(A, dm[c * 16 + NTAIL - 1], acc1[3], acc0[3]);   // odd number of background rows
-        }
-    }
-    s1 = (acc1[0] + acc1[1]) + (acc1[2] + acc1[3]);
-    s0 = (acc0[0] + acc0[1]) + (acc0[2] + acc0[3]);
-}
-
-// Same sums with packed arithmetic (the common case: no clamping needed).  dm[2j], dm[2j+1] travel as one 64-bit operand.
-template <int NTAIL>
-__device__ __forceinline__ void row_sums_packed(const float (&dm)[MAXN], float A, int nfull, float& s1, float& s0) {
-    const f32x2 A2 = f2_pack(A, A), one2 = f2_pack(1.f, 1.f), two2 = f2_pack(2.f, 2.f);
-    f32x2 acc1[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)}, acc0[2] = {f2_pack(0.f, 0.f), f2_pack(0.f, 0.f)};
-    float t1s = 0.f, t0s = 0.f;
-#pragma unroll
-    for (int c = 0; c < MAXN / 16; ++c) {
-        if (c < nfull) {
-#pragma unroll
-            for (int jj = 0; jj < 16; jj += 4)
-                quad_acc(A2, f2_pack(dm[c * 16 + jj], dm[c * 16 + jj + 1]), f2_pack(dm[c * 16 + jj + 2], dm[c * 16 + jj + 3]),
-                         one2, two2, acc1[(jj >> 2) & 1], acc0[(jj >> 2) & 1]);
-        } else if (NTAIL > 0 && c == nfull) {
-#pragma unroll
-            for (int jj = 0; jj + 3 < NTAIL; jj += 4)
-                quad_acc(A2, f2_pack(dm[c * 16 + jj], dm[c * 16 + jj + 1]), f2_pack(dm[c * 16 + jj + 2], dm[c * 16 + jj + 3]),
-                         one2, two2, acc1[(jj >> 2) & 1], acc0[(jj >> 2) & 1]);
-            constexpr int Q = NTAIL & ~3;                 // what the quads covered
-            if ((NTAIL & 3) >= 2) pair_acc<false>(A, dm[c * 16 + Q], dm[c * 16 + Q + 1], t1s, t0s);
-            if (NTAIL & 1) single_acc(A, dm[c * 16 + NTAIL - 1], t1s, t0s);
-        }
-    }
-    float a, b, c2, d;
-    f2_unpack(f2_add(acc1[0], acc1[1]), a, b);
-    f2_unpack(f2_add(acc0[0], acc0[1]), c2, d);
-    s1 = (a + b) + t1s;
-    s0 = (c2 + d) + t0s;
-}
-
-// one warp = 32 coalition rows (one per lane) x a strided subset of the instances
-// W = 64-bit words per coalition row (1: up to 64 groups, 2: up to 128; the shared-memory version below also 16: up to 1024)
-template <int NTAIL, int W>
-__global__ void __launch_bounds__(32 * WARPS_PER_CTA, 1) explain_shared_kernel(SharedParams p) {
-    const int lane = threadIdx.x & 31;
-    const int gw = blockIdx.x * WARPS_PER_CTA + (threadIdx.x >> 5);
-    const int n_rg = p.S_pad / 32;                       // row groups
-    const int total_warps = gridDim.x * WARPS_PER_CTA;
-    const int nparts = total_warps / n_rg;               // replicas of every row group
-    if (nparts == 0 || gw >= nparts * n_rg) return;
-    const int rg = gw % n_rg, part = gw / n_rg;
-    const int s = rg * 32 + lane;
-    const int cnt = *p.count;
-    const int N = p.N, G = p.G;
-
-    // this lane's row of Dm, in registers (chunks of 16 columns; unused chunks are never touched)
-    float dm[MAXN];
-    float dmax = 0.f;
-#pragma unroll
-    for (int c = 0; c < MAXN / 16; ++c) {
-        if (c * 16 < N) {
-#pragma unroll
-            for (int jj = 0; jj < 16; ++jj) {
-                const int j = c * 16 + jj;
-                dm[j] = j < N ? p.DmT[(size_t)j * p.S_pad + s] : 0.f;
-                dmax = fmaxf(dmax, dm[j]);
-            }
-        }
-    }
-    uint64_t zz[W];
-#pragma unroll
-    for (int w = 0; w < W; ++w) zz[w] = s < p.S ? p.z[(size_t)s * W + w] : 0ull;
-    const int nfull = N / 16;
-    const double es = p.dme[s];                          // exponent the row of Dm was normalised by
-
-    const int ntab = (G + 3) / 4;
-    for (int m = part; m < cnt; m += nparts) {
-        const int i = p.list[m];
-        // a = scale * sum_k z_k XW_i[k] in float64, one table entry per nibble of the row (prep_kernel built the tables);
-        // the loads are independent, two partial sums keep the add chain short.
-        // A = 2^a = 2^n * 2^f with n = rint(a), |f| <= 1/2 (f exact in fp32 to 3e-8, ex2.approx to ~1e-7 relative)
-        const double* xt = p.XT + (size_t)i * ntab * 16;
-        double a0 = 0.0, a1 = 0.0;
-#pragma unroll
-        for (int w = 0; w < W; ++w) {
-#pragma unroll 4
-            for (int t = 0; t < 16 && 16 * w + t < ntab; t += 2) {
-                a0 += __ldg(xt + (16 * w + t) * 16 + (int)((zz[w] >> (4 * t)) & 15ull));
-                if (16 * w + t + 1 < ntab) a1 += __ldg(xt + (16 * w + t + 1) * 16 + (int)((zz[w] >> (4 * t + 4)) & 15ull));
-            }
-        }
-        double a = (a0 + a1) + es;
-        a = fmin(fmax(a, -120.0), 120.0);
-        const double an = rint(a);
-        const float A = ex2_approx((float)(a - an)) * __int_as_float((127 + (int)an) << 23);
-        float s1, s0;
-        // with u <= 1e18 the product q = ua*ub and the reciprocal of (1+ua)(1+ub) stay normal fp32 numbers: no clamps needed
-        const bool risky = __any_sync(0xffffffffu, A * dmax > 1.0e18f);
-        if (risky) row_sums<true, NTAIL>(dm, A, nfull, s1, s0);
-        else row_sums_packed<NTAIL>(dm, A, nfull, s1, s0);
-        if (s < p.S) {
-            float2* dst = p.sums + (size_t)i * p.S_pad + s;
-            if (p.accumulate) { const float2 o = *dst; s1 += o.x; s0 += o.y; }
-            *dst = make_float2(s1, s0);
-        }
-    }
-}
-
-// ---- the same kernel with the Dm rows parked in SHARED MEMORY ------------------------------------------------------
-// The register version above keeps a lane's row of Dm (up to 128 floats) in registers: 168 registers per thread, 12
-// warps per SM, and the kernel is latency bound.  Here every warp parks its 32 rows in its own slice of shared memory
-// instead, one float4 per (quad of columns, lane): a lane reads back only what it wrote itself (no barrier), and the
-// 128-bit loads of one quad by a warp cover 512 consecutive bytes (no bank conflicts).  That frees ~100 registers per
-// thread; the number of warps per CTA follows from the shared memory a slice takes.
+// ---- the coalition kernel, the Dm rows parked in shared memory ------------------------------------------------------
+// A lane's row of Dm (up to 128 floats) held in registers costs 168 registers per thread, 12 warps per SM, and leaves
+// the kernel latency bound.  Instead every warp parks its 32 rows in its own slice of shared memory, one float4 per
+// (quad of columns, lane): a lane reads back only what it wrote itself (no barrier), and the 128-bit loads of one quad by
+// a warp cover 512 consecutive bytes (no bank conflicts).  The number of warps per CTA follows from the shared memory a
+// slice takes.
 constexpr int TM_MAX_WARPS = 20;
 __host__ __device__ inline int dm_quads(int N) { return (N + 3) / 4; }
 __host__ __device__ inline size_t dm_slice_bytes(int N) { return (size_t)dm_quads(N) * 32 * sizeof(float4); }
@@ -249,9 +114,9 @@ __device__ __forceinline__ void dm_ld16(const float4* sl, int c, int nq, int lan
     }
 }
 
-// The same four sigmoids from what the slice holds for a quad of columns (0,2) (1,3): ds = (dm0 + dm2, dm1 + dm3) and
-// dq = (dm0 dm2, dm1 dm3), both independent of the instance:  sm = A ds,  q = A^2 dq.  14 fp32 ops + 2 MUFU per four
-// elements (A2 = (A, A), AA2 = (A^2, A^2), AA2x2 = 2 AA2).
+// Four sigmoids (two pairs, each sharing one reciprocal) in packed arithmetic, from what the slice holds for a quad of
+// columns (0,2) (1,3): ds = (dm0 + dm2, dm1 + dm3) and dq = (dm0 dm2, dm1 dm3), both independent of the instance:
+// sm = A ds,  q = A^2 dq.  14 fp32 ops + 2 MUFU per four elements (A2 = (A, A), AA2 = (A^2, A^2), AA2x2 = 2 AA2).
 __device__ __forceinline__ void quad_acc_sq(f32x2 A2, f32x2 AA2, f32x2 AA2x2, f32x2 ds, f32x2 dq, f32x2 one2, f32x2 two2,
                                             f32x2& a1, f32x2& a0) {
     const f32x2 sm = f2_mul(A2, ds);
@@ -347,6 +212,9 @@ __device__ __forceinline__ void row_sums_clamped_w(const float* __restrict__ DmT
     s1 = r1; s0 = r0;
 }
 
+// one warp = 32 coalition rows (one per lane) x a strided subset of the instances
+// NTAIL = N % 16 (compile time): the last, partial chunk is straight-line code
+// W = 64-bit words per coalition row (1: up to 64 groups, 2: up to 128, 16: up to 1024)
 // WT: weighted background (the weighted slice and quad_acc_w above; NTAIL is unused and 0)
 template <int NTAIL, int W, bool WT = false>
 __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_smem_kernel(SharedParams p, int warps_used) {
@@ -568,19 +436,9 @@ __global__ void __launch_bounds__(32 * TM_MAX_WARPS, 1) explain_shared_smem_kern
     }
 }
 
-// 0: registers, 1: shared memory (default); DKS_SHARED_DM=regs selects the register version for comparisons
-inline bool shared_dm_in_smem() {
-    static int mode = -1;
-    if (mode < 0) {
-        const char* e = getenv("DKS_SHARED_DM");
-        mode = (e && e[0] == 'r') ? 0 : 1;
-    }
-    return mode == 1;
-}
-
 // What the launches of the unfused coalition kernel used (reported by dks_last_path): the fewest warps per CTA and the
 // largest grid over the background chunks.
-struct SharedLaunch { int regs, warps, grid, chunks; };
+struct SharedLaunch { int warps, grid, chunks; };
 
 // CTAs for n_rg row groups at `warps` warps per CTA: at least one per SM, and enough that every row group has a warp (a
 // warp without a row group does nothing, so a grid of fewer warps than row groups would leave sums unwritten).  The
@@ -600,7 +458,6 @@ inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words,
         if (warps_used > TM_MAX_WARPS) warps_used = TM_MAX_WARPS;
         const size_t smem = (size_t)warps_used * slice + w2;
         const int grid = shared_grid(n_rg, warps_used, sm_count);
-        info->regs = 0;
         if (info->warps == 0 || warps_used < info->warps) info->warps = warps_used;
         if (grid > info->grid) info->grid = grid;
         cudaError_t err = cudaSuccess;
@@ -613,17 +470,16 @@ inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words,
 #undef DKS_CASE_WT
         return err;
     }
-    if (shared_dm_in_smem() || words > 2) {                  // sixteen-word rows exist for the shared-memory kernel only
-        const size_t slice = dm_slice_bytes(p.N);
-        int warps_used = (int)(((size_t)max_smem - 1024) / slice);
-        if (warps_used > TM_MAX_WARPS) warps_used = TM_MAX_WARPS;
-        const size_t smem = (size_t)warps_used * slice;
-        const int grid = shared_grid(n_rg, warps_used, sm_count);
-        info->regs = 0;
-        if (info->warps == 0 || warps_used < info->warps) info->warps = warps_used;
-        if (grid > info->grid) info->grid = grid;
-        cudaError_t err = cudaSuccess;
-        switch (p.N % 16) {
+    // uniform background
+    const size_t slice = dm_slice_bytes(p.N);
+    int warps_used = (int)(((size_t)max_smem - 1024) / slice);
+    if (warps_used > TM_MAX_WARPS) warps_used = TM_MAX_WARPS;
+    const size_t smem = (size_t)warps_used * slice;
+    const int grid = shared_grid(n_rg, warps_used, sm_count);
+    if (info->warps == 0 || warps_used < info->warps) info->warps = warps_used;
+    if (grid > info->grid) info->grid = grid;
+    cudaError_t err = cudaSuccess;
+    switch (p.N % 16) {
 #define DKS_CASE_W(T, W)                                                                                                  \
     err = cudaFuncSetAttribute(explain_shared_smem_kernel<T, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
     if (err == cudaSuccess) explain_shared_smem_kernel<T, W><<<grid, 32 * TM_MAX_WARPS, smem, stream>>>(p, warps_used);
@@ -633,30 +489,12 @@ inline cudaError_t launch_explain_shared_chunk(const SharedParams& p, int words,
         else if (words == 2) { DKS_CASE_W(T, 2) }                                                            \
         else { DKS_CASE_W(T, 16) }                                                                           \
         break;
-            DKS_CASE(0) DKS_CASE(1) DKS_CASE(2) DKS_CASE(3) DKS_CASE(4) DKS_CASE(5) DKS_CASE(6) DKS_CASE(7)
-            DKS_CASE(8) DKS_CASE(9) DKS_CASE(10) DKS_CASE(11) DKS_CASE(12) DKS_CASE(13) DKS_CASE(14) DKS_CASE(15)
-#undef DKS_CASE
-#undef DKS_CASE_W
-        }
-        return err;
-    }
-
-    const int threads = 32 * WARPS_PER_CTA;
-    const int grid = shared_grid(n_rg, WARPS_PER_CTA, sm_count);
-    info->regs = 1;
-    info->warps = WARPS_PER_CTA;
-    if (grid > info->grid) info->grid = grid;
-    switch (p.N % 16) {
-#define DKS_CASE(T)                                                             \
-    case T:                                                                     \
-        if (words == 1) explain_shared_kernel<T, 1><<<grid, threads, 0, stream>>>(p); \
-        else explain_shared_kernel<T, 2><<<grid, threads, 0, stream>>>(p);      \
-        break;
         DKS_CASE(0) DKS_CASE(1) DKS_CASE(2) DKS_CASE(3) DKS_CASE(4) DKS_CASE(5) DKS_CASE(6) DKS_CASE(7)
         DKS_CASE(8) DKS_CASE(9) DKS_CASE(10) DKS_CASE(11) DKS_CASE(12) DKS_CASE(13) DKS_CASE(14) DKS_CASE(15)
 #undef DKS_CASE
+#undef DKS_CASE_W
     }
-    return cudaSuccess;
+    return err;
 }
 
 // Backgrounds larger than MAXN rows go through in chunks of MAXN columns of Dm (one launch each, sums accumulated; a
@@ -816,33 +654,32 @@ struct WlsPmatParams {
     double* phi;
 };
 constexpr int PMAT_MAXK = 24;        // coefficients held in registers per thread
+constexpr int PMAT_THREADS = 256;
 inline int wls_pmat_kpad(int G) { return (G - 1 + 3) / 4 * 4; }       // coefficient rows padded to a multiple of four
-inline size_t wls_pmat_smem(int G, int S_pad, bool as_double) {
-    return (size_t)wls_pmat_kpad(G) * S_pad * (as_double ? sizeof(double) : sizeof(float));
-}
+inline size_t wls_pmat_smem(int G, int S_pad) { return (size_t)wls_pmat_kpad(G) * S_pad * sizeof(float); }
 
 // Persistent CTAs; P resident in shared memory.  Per coalition row: y, then KPAD multiply-adds in float64.
 // KPAD (compile time) = coefficients rounded up to a multiple of four, the padding rows of P are zero: the inner loop has
-// no bounds checks (the checks were a fifth of the instructions).  PT = float by default; a float64 copy of the table
-// (no float -> double conversions in the loop, but half the CTAs per SM) measured slower.
-template <int KPAD, typename PT, int THREADS>
-__global__ void __launch_bounds__(THREADS) wls_pmat_kernel(WlsPmatParams p) {
+// no bounds checks (the checks were a fifth of the instructions).  P is staged as float32: a float64 copy (no float ->
+// double conversions in the loop, but half the CTAs per SM) measured slower.
+template <int KPAD>
+__global__ void __launch_bounds__(PMAT_THREADS) wls_pmat_kernel(WlsPmatParams p) {
     extern __shared__ __align__(16) unsigned char s_praw[];
-    PT* s_P = reinterpret_cast<PT*>(s_praw);                        // [KPAD][S_pad]
-    __shared__ double s_part[THREADS / 32][KPAD];
+    float* s_P = reinterpret_cast<float*>(s_praw);                  // [KPAD][S_pad]
+    __shared__ double s_part[PMAT_THREADS / 32][KPAD];
     __shared__ LogTabEntry s_logtab[DKS_LOGTAB_SIZE];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int G = p.G, nA = G - 1;
     const int cnt = *p.count;
     if ((int)blockIdx.x >= cnt) return;
     if (threadIdx.x < DKS_LOGTAB_SIZE) logtab_fill(s_logtab, threadIdx.x);
-    for (int idx = threadIdx.x; idx < KPAD * p.S_pad; idx += THREADS) s_P[idx] = idx < nA * p.S_pad ? (PT)p.pmat[idx] : (PT)0;
+    for (int idx = threadIdx.x; idx < KPAD * p.S_pad; idx += PMAT_THREADS) s_P[idx] = idx < nA * p.S_pad ? p.pmat[idx] : 0.f;
     __syncthreads();
     const double lf1 = p.linkfnull[1], f1 = p.fnull[1], inv_n = 1.0 / (double)p.N;
     const size_t slab = (size_t)p.n * G;
     int i_next = p.list[blockIdx.x];
     double delta_next = p.dlink[(size_t)i_next * p.C + 1];
-    constexpr int INFLIGHT = THREADS >= 512 ? 4 : 8;                  // independent loads in flight per thread
+    constexpr int INFLIGHT = 8;                                        // independent loads in flight per thread
     for (int m = blockIdx.x; m < cnt; m += gridDim.x) {
         const int i = i_next;
         const double delta = delta_next;
@@ -854,16 +691,16 @@ __global__ void __launch_bounds__(THREADS) wls_pmat_kernel(WlsPmatParams p) {
         double Tk[KPAD];
 #pragma unroll
         for (int k = 0; k < KPAD; ++k) Tk[k] = 0.0;
-        for (int s0 = 0; s0 < p.S; s0 += INFLIGHT * THREADS) {
+        for (int s0 = 0; s0 < p.S; s0 += INFLIGHT * PMAT_THREADS) {
             float2 a[INFLIGHT];
 #pragma unroll
             for (int r = 0; r < INFLIGHT; ++r) {
-                const int s = s0 + r * THREADS + threadIdx.x;
+                const int s = s0 + r * PMAT_THREADS + threadIdx.x;
                 a[r] = s < p.S ? sums[s] : make_float2(1.f, 1.f);
             }
 #pragma unroll
             for (int r = 0; r < INFLIGHT; ++r) {
-                const int s = s0 + r * THREADS + threadIdx.x;
+                const int s = s0 + r * PMAT_THREADS + threadIdx.x;
                 if (s < p.S) {
                     double y;
                     if (p.link == DKS_LINK_LOGIT) y = fast_log_ratio(a[r].x, a[r].y, s_logtab) - lf1;
@@ -883,7 +720,7 @@ __global__ void __launch_bounds__(THREADS) wls_pmat_kernel(WlsPmatParams p) {
             double beta = 0.0;
             if (lane < nA) {
 #pragma unroll
-                for (int wq = 0; wq < THREADS / 32; ++wq) beta += s_part[wq][lane];      // fixed order: reproducible
+                for (int wq = 0; wq < PMAT_THREADS / 32; ++wq) beta += s_part[wq][lane];      // fixed order: reproducible
                 beta -= delta * p.dvec[lane];
             }
             const double sum = warp_sum(beta);
@@ -898,33 +735,21 @@ __global__ void __launch_bounds__(THREADS) wls_pmat_kernel(WlsPmatParams p) {
     }
 }
 
-// picks the instantiation; returns false when no variant fits shared memory
+// picks the instantiation; returns false when P does not fit shared memory
 inline bool launch_wls_pmat(const WlsPmatParams& p, int n, int sm_count, int max_smem, cudaStream_t stream, cudaError_t* err) {
-    const int kpad = wls_pmat_kpad(p.G);
-    const size_t sm_d = wls_pmat_smem(p.G, p.S_pad, true), sm_f = wls_pmat_smem(p.G, p.S_pad, false);
-    // float32 table, 2 CTAs of 256 threads per SM by default; DKS_PMAT=double selects the float64 variant (1 CTA of 512
-    // threads) for comparisons.
-    static int want_double = -1;
-    if (want_double < 0) { const char* e = getenv("DKS_PMAT"); want_double = (e && e[0] == 'd') ? 1 : 0; }
-    const bool as_double = want_double && sm_d + 8192 <= (size_t)max_smem;
-    if (!as_double && sm_f + 8192 > (size_t)max_smem) return false;
-    const size_t smem = as_double ? sm_d : sm_f;
+    const size_t smem = wls_pmat_smem(p.G, p.S_pad);
+    if (smem + 8192 > (size_t)max_smem) return false;
     int per_sm = (int)((size_t)max_smem / (smem + 8192));
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 4) per_sm = 4;
     const int grid = n < sm_count * per_sm ? n : sm_count * per_sm;
     *err = cudaSuccess;
-#define DKS_PM(K)                                                                                                         \
-    case K:                                                                                                               \
-        if (as_double) {                                                                                                  \
-            *err = cudaFuncSetAttribute(wls_pmat_kernel<K, double, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (*err == cudaSuccess) wls_pmat_kernel<K, double, 512><<<grid, 512, smem, stream>>>(p);                     \
-        } else {                                                                                                          \
-            *err = cudaFuncSetAttribute(wls_pmat_kernel<K, float, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (*err == cudaSuccess) wls_pmat_kernel<K, float, 256><<<grid, 256, smem, stream>>>(p);                      \
-        }                                                                                                                 \
+#define DKS_PM(K)                                                                                                  \
+    case K:                                                                                                        \
+        *err = cudaFuncSetAttribute(wls_pmat_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   \
+        if (*err == cudaSuccess) wls_pmat_kernel<K><<<grid, PMAT_THREADS, smem, stream>>>(p);                      \
         break;
-    switch (kpad) {
+    switch (wls_pmat_kpad(p.G)) {
         DKS_PM(4) DKS_PM(8) DKS_PM(12) DKS_PM(16) DKS_PM(20) DKS_PM(24)
         default: return false;
     }

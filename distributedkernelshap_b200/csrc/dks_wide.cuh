@@ -7,7 +7,7 @@
 // in float64 (plan.py: projection(), np.linalg.inv like upstream's solve) and uploaded transposed, PT [S_pad][KP], with
 // dks_set_plan_projection.  Per batch of instances the solve is then
 //     Y  [cnt x S]  = link(ey) - link(fnull)                     wide_link_kernel
-//     B  [cnt x KP] = Y PT                                       wide_beta_kernel   (float64 GEMM, CUDA cores)
+//     B  [cnt x KP] = Y PT                                       wide_beta2_kernel  (float64 GEMM, CUDA cores)
 //     phi_k = B_k - delta d_k,  phi_last = delta - sum_k phi_k   wide_finish_kernel
 // All of it float64; every sum has a fixed order (no atomics), so results are reproducible run to run.
 // Work per instance at M = 1024, S = 8192: 8.4 M float64 multiply-adds, about the cost of the coalition stage.
@@ -24,8 +24,8 @@
 namespace dks {
 namespace wide {
 
-constexpr int BM = 64, BN = 64, BK = 16;     // tile of the Y PT product: 64 instances x 64 coefficients, 16 coalitions a step
-constexpr int THREADS = 256;                 // 16 x 16 threads, 4 x 4 outputs each
+constexpr int BN = 64, BK = 16;              // tile of the Y PT product: 64 coefficients, 16 coalitions a step
+constexpr int THREADS = 256;                 // 16 x 16 threads
 
 inline int kpad(int M) { return (M - 1 + BN - 1) / BN * BN; }
 
@@ -67,64 +67,11 @@ __global__ void __launch_bounds__(256) wide_link_kernel(WideParams p) {
     }
 }
 
-// beta[i][k] = sum_s y[i][s] PT[s][k]: classic shared-memory tiled product, coalition index ascending (fixed order)
-__global__ void __launch_bounds__(THREADS) wide_beta_kernel(WideParams p) {
-    __shared__ double As[BK][BM + 1];        // y tile, transposed: [coalition][instance]
-    __shared__ double Bs[BK][BN];            // PT tile: [coalition][coefficient]
-    __shared__ int s_inst[BM];
-    const int cnt = *p.count;
-    const int m0 = blockIdx.y * BM, k0 = blockIdx.x * BN;
-    if (m0 >= cnt) return;
-    const int t = threadIdx.x;
-    if (t < BM) s_inst[t] = m0 + t < cnt ? p.list[m0 + t] : -1;
-    __syncthreads();
-    // loader roles: y tile -- instance t / 4, four consecutive coalitions; PT tile -- coalition t / 16, four coefficients
-    const int la_m = t >> 2, la_k = (t & 3) * 4;
-    const int lb_k = t >> 4, lb_c = (t & 15) * 4;
-    const int inst = s_inst[la_m];
-    const double* yrow = inst >= 0 ? p.y + (size_t)inst * p.S_pad : nullptr;
-    const int ty = t >> 4, tx = t & 15;      // outputs: instances 4 ty .. +3, coefficients 4 tx .. +3
-    double acc[4][4];
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
-    for (int s0 = 0; s0 < p.S_pad; s0 += BK) {             // S_pad is a multiple of 32
-#pragma unroll
-        for (int q = 0; q < 4; ++q) As[la_k + q][la_m] = yrow ? yrow[s0 + la_k + q] : 0.0;
-        const double* prow = p.PT + (size_t)(s0 + lb_k) * p.KP + k0 + lb_c;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) Bs[lb_k][lb_c + q] = prow[q];
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < BK; ++kk) {
-            double a[4], b[4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r) a[r] = As[kk][4 * ty + r];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) b[c] = Bs[kk][4 * tx + c];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) acc[r][c] = fma(a[r], b[c], acc[r][c]);
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-        const int i = s_inst[4 * ty + r];
-        if (i < 0) continue;
-        double* out = p.beta + (size_t)i * p.KP + k0 + 4 * tx;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) out[c] = acc[r][c];
-    }
-}
-
-// Second version of the product (profiles/r2l_ncu_full_wide_path.csv showed the first one bound by shared-memory loads:
-// 2.9e8 bank conflicts, FP64 pipe 29 % active).  128 instances x 64 coefficients per CTA, 8 x 4 outputs per thread, every
-// shared-memory operand a 128-bit load: a thread's rows are 4 ty .. +3 and 64 + 4 ty .. +3 (a warp holds two values of ty:
-// broadcasts), its columns 2 tx, 2 tx + 1 and 32 + 2 tx, 32 + 2 tx + 1 (sixteen consecutive 16-byte pieces per load: no
-// conflicts).  Per coalition step 6 LDS.128 feed 32 DFMA.  Same fixed summation order as the first version: identical bits.
+// beta[i][k] = sum_s y[i][s] PT[s][k], coalition index ascending (fixed order).  A plain 64 x 64 tiling is bound by
+// shared-memory loads (bank conflicts; FP64 pipe under a third active), so: 128 instances x 64 coefficients per CTA, 8 x 4
+// outputs per thread, every shared-memory operand a 128-bit load: a thread's rows are 4 ty .. +3 and 64 + 4 ty .. +3 (a
+// warp holds two values of ty: broadcasts), its columns 2 tx, 2 tx + 1 and 32 + 2 tx, 32 + 2 tx + 1 (sixteen consecutive
+// 16-byte pieces per load: no conflicts).  Per coalition step 6 LDS.128 feed 32 DFMA.
 constexpr int BM2 = 128;
 __global__ void __launch_bounds__(THREADS) wide_beta2_kernel(WideParams p) {
     __shared__ __align__(16) double As[BK][BM2];     // y tile, transposed: [coalition][instance]
@@ -233,16 +180,14 @@ inline dim3 link_grid(int S_pad, int n, int sm_count) {
     const int gx = (S_pad + 255) / 256 < 8 ? (S_pad + 255) / 256 : 8;
     return dim3(gx, n < 4 * sm_count ? n : 4 * sm_count);
 }
-inline dim3 beta_grid(int KP, int n) { return dim3(KP / BN, (n + BM - 1) / BM); }
 inline dim3 beta2_grid(int KP, int n) { return dim3(KP / BN, (n + BM2 - 1) / BM2); }
 inline int finish_grid(int n, int sm_count) { return n < 8 * sm_count ? n : 8 * sm_count; }
 
 #ifndef DKS_HOST_EMULATION
 // three launches on `stream`; n = instances of the call (upper bound of the device-side count)
-inline cudaError_t launch_wide_solve(const WideParams& p, int n, int sm_count, int gemm_version, cudaStream_t stream) {
+inline cudaError_t launch_wide_solve(const WideParams& p, int n, int sm_count, cudaStream_t stream) {
     wide_link_kernel<<<link_grid(p.S_pad, n, sm_count), 256, 0, stream>>>(p);
-    if (gemm_version == 2) wide_beta2_kernel<<<beta2_grid(p.KP, n), THREADS, 0, stream>>>(p);
-    else wide_beta_kernel<<<beta_grid(p.KP, n), THREADS, 0, stream>>>(p);
+    wide_beta2_kernel<<<beta2_grid(p.KP, n), THREADS, 0, stream>>>(p);
     wide_finish_kernel<<<finish_grid(n, sm_count), 256, 0, stream>>>(p);
     return cudaGetLastError();
 }

@@ -396,8 +396,8 @@ class GpuKernelExplainer:
         self.kernel = kernel
 
     def set_option(self, name, value):
-        """Tuning knob of the C library (``dks_set_option``): 'fused', 'fused_warps', 'fused_batch',
-        'push_in_kernel', 'graph', 'graph_timing', 'wide_gemm', 'wide_acache'."""
+        """Tuning knob of the C library (``dks_set_option``): 'fused', 'fused_warps', 'fused_batch', 'fused_table',
+        'push_in_kernel', 'graph', 'graph_timing'."""
         _cabi.check(self.lib.dks_set_option(self._ctx, str(name).encode(), int(value)))
 
     # ------------------------------------------------------------------------------------------------------
@@ -788,7 +788,7 @@ class GpuKernelExplainer:
         return {"prepare": float(out[0]), "coalitions": float(out[1]), "total": float(out[2])}
 
     _PATH_NAMES = {
-        "shared": ("none", "fused", "smem", "regs", "softmax", "affine", "ovr", "exp", "mixture"),
+        "shared": ("none", "fused", "smem", None, "softmax", "affine", "ovr", "exp", "mixture"),   # 3: not used
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
         "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble"),
     }
@@ -796,7 +796,7 @@ class GpuKernelExplainer:
     def last_path(self):
         """Which kernels the last explain call launched (``dks_last_path``), recorded when the call was enqueued (a
         replayed CUDA graph reports the call it captured): ``shared`` (shared-plan coalition kernel: 'none' | 'fused' |
-        'smem' | 'regs' | 'softmax' | 'ovr', or 'affine' for the identity head and 'exp' for the exp head, whose y needs no
+        'smem' | 'softmax' | 'ovr', or 'affine' for the identity head and 'exp' for the exp head, whose y needs no
         coalition kernel), ``chunks`` (background chunks), ``warps`` / ``grid`` (warps per CTA and CTAs of that kernel),
         ``fused_B`` / ``fused_NI``, ``solve`` ('none' | 'fused' | 'pmat' | 'wls_shared' | 'wide' | 'l1'), ``pmat_kpad``,
         ``general`` (kernel of the remaining instances: 'none' | 'tc' | 'simt' | 'flagged', the last meaning they

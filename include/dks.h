@@ -432,10 +432,7 @@ int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
  * "push_in_kernel" 0/1 -- multi-GPU: the fused kernel's epilogue stores phi into the peers' buffers itself instead of the
  * separate push kernel (default 0: measured slower, it stalls the finishing warps); "graph" 0/1 (CUDA-graph
  * replay of dks_run_dev); "graph_timing" 0/1 -- keep the timing event records inside the graph (default 0: a replayed graph
- * carries no timing nodes and dks_last_timings reports an error after it); plans of more than 128 groups: "wide_gemm" 1/2 --
- * float64 product of the projection solve, 2 = 128 x 64 tiles with conflict-free 128-bit shared-memory operands (default),
- * 1 = the first 64 x 64 version; "wide_acache" 0/1 -- A(i, s) of sixteen-word rows computed by the first background
- * chunk's launch only (default 1).  Both give identical bits either way. */
+ * carries no timing nodes and dks_last_timings reports an error after it). */
 int dks_set_option(dks_ctx* ctx, const char* name, int value);
 int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by this ctx so far */
 /* The fused kernel's link table of the plan over M groups: its bytes (0 = the plan has none and the kernel runs the exact
@@ -466,7 +463,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_SHARED_NONE 0
 #define DKS_SHARED_FUSED 1       /* explain_shared_fused_kernel: link + projection solve inside */
 #define DKS_SHARED_SMEM 2        /* explain_shared_smem_kernel (Dm rows in shared memory) */
-#define DKS_SHARED_REGS 3        /* explain_shared_kernel (Dm rows in registers; DKS_SHARED_DM=regs) */
+/* 3 is not used: a retired kernel's code, kept free so that the other codes keep their meaning */
 #define DKS_SHARED_SOFTMAX 4     /* explain_softmax_kernel: per-class sums of the softmax head (C = R classes) */
 #define DKS_SHARED_AFFINE 5      /* identity head: y read from per-class tables, no coalition kernel */
 #define DKS_SHARED_OVR 6         /* explain_ovr_kernel: per-class sums of the one-vs-rest head (C = R classes) */

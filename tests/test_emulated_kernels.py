@@ -1,7 +1,8 @@
 """Runs the solve kernels of csrc/dks_wide.cuh (plans of more than 128 groups) on HOST threads: tests/emu/emu_shim.h maps
 the CUDA execution model (threads of a block, __syncthreads, __shared__, warp butterfly sums) onto std::thread +
-std::barrier, tests/emu/wide_emu.cpp compiles the very kernel source nvcc compiles and checks link, float64 product and
-finish step against a plain reference at shapes that hit every tile boundary.  The GPU parity tests of the same path are
+std::barrier, tests/emu/wide_emu.cpp compiles the very kernel source nvcc compiles and checks link and finish step
+against a plain reference, and the float64 product bit for bit against the host's ascending fma chain, at shapes that
+hit every tile boundary.  The GPU parity tests of the same path are
 tests/test_gpu_wide.py and the configs[3] singleton case of tests/test_gpu_baseline_shapes.py."""
 import os
 import shutil
@@ -13,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
 
 
-def test_wide_solve_kernels_on_host_threads(tmp_path):
+def test_wide_solve_kernels_on_host_threads_product_bit_exact(tmp_path):
     gxx = shutil.which("g++")
     if gxx is None:
         pytest.skip("no g++")
