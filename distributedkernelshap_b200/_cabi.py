@@ -103,6 +103,7 @@ SIGNATURES = {
     "dks_set_kernel": (C.c_int, [C.c_void_p, C.c_int]),
     "dks_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "dks_kernel_launches": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
+    "dks_live_allocations": (C.c_int, [C.POINTER(C.c_int64)]),
     "dks_fused_table_info": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "dks_last_timings": (C.c_int, [C.c_void_p, C.c_void_p]),
     "dks_last_general_l1_timings": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -5,6 +5,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 
 #include "dks_kernels.cuh"
 #include "dks_tc.cuh"
@@ -49,19 +50,6 @@ int fail(int code, const char* fmt, ...) {
         if (!(cond)) return fail(DKS_ERR_INVALID, __VA_ARGS__); \
     } while (0)
 
-template <typename T>
-int dev_alloc(T** p, size_t count) {
-    if (*p) { cudaFree(*p); *p = nullptr; }
-    if (count == 0) count = 1;
-    CUDA_TRY(cudaMalloc((void**)p, count * sizeof(T)));
-    return DKS_OK;
-}
-
-template <typename T>
-void dev_free(T** p) {
-    if (*p) { cudaFree(*p); *p = nullptr; }
-}
-
 inline int cdiv(long long a, int b) { return (int)((a + b - 1) / b); }
 
 // drops the plan of one M (every M when M < 0) with everything derived from it -- its l1 tables, sampling info and
@@ -70,8 +58,7 @@ int drop_plans(dks_ctx* ctx, int M) {
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));       // nothing in flight may still read the buffers
     for (int m = 0; m <= DKS_MAX_GROUPS; ++m) {
         if (M >= 0 && m != M) continue;
-        for (void* q : ctx->plan_allocs[m]) cudaFree(q);
-        ctx->plan_allocs[m].clear();
+        ctx->plan_pool[m].clear();
         ctx->h_plans[m] = PlanDev{};
         ctx->h_l1[m] = dks::l1::Tables{};
         ctx->h_afix[m] = nullptr;
@@ -111,23 +98,23 @@ int bind(dks_ctx* ctx) {
     } while (0)
 
 int ensure_workspace(dks_ctx* ctx, int n) {
-    if (n <= ctx->cap_n) return DKS_OK;
+    if (n <= ctx->ws_n) return DKS_OK;
     const int G = ctx->G, R = ctx->R, C = ctx->C;
-    TRY(dev_alloc(&ctx->d_XW, (size_t)n * G * R));
-    TRY(dev_alloc(&ctx->d_XT, (size_t)n * R * ((G + 3) / 4) * 16));
-    TRY(dev_alloc(&ctx->d_vflag, (size_t)n * G));
-    TRY(dev_alloc(&ctx->d_vmask, (size_t)n));
-    TRY(dev_alloc(&ctx->d_M, (size_t)n));
-    TRY(dev_alloc(&ctx->d_dlink, (size_t)n * C));
-    TRY(dev_alloc(&ctx->d_idx_full, (size_t)n));
-    TRY(dev_alloc(&ctx->d_idx_other, (size_t)n));
-    TRY(dev_alloc(&ctx->d_idx_sel, (size_t)n));
-    TRY(dev_alloc(&ctx->d_idx_plain, (size_t)n));
-    TRY(dev_alloc(&ctx->d_acc, (size_t)n * 16));
-    TRY(dev_alloc(&ctx->d_done, (size_t)n));
+    CUDA_TRY(ctx->d_XW.alloc((size_t)n * G * R));
+    CUDA_TRY(ctx->d_XT.alloc((size_t)n * R * ((G + 3) / 4) * 16));
+    CUDA_TRY(ctx->d_vflag.alloc((size_t)n * G));
+    CUDA_TRY(ctx->d_vmask.alloc((size_t)n));
+    CUDA_TRY(ctx->d_M.alloc((size_t)n));
+    CUDA_TRY(ctx->d_dlink.alloc((size_t)n * C));
+    CUDA_TRY(ctx->d_idx_full.alloc((size_t)n));
+    CUDA_TRY(ctx->d_idx_other.alloc((size_t)n));
+    CUDA_TRY(ctx->d_idx_sel.alloc((size_t)n));
+    CUDA_TRY(ctx->d_idx_plain.alloc((size_t)n));
+    CUDA_TRY(ctx->d_acc.alloc((size_t)n * 16));
+    CUDA_TRY(ctx->d_done.alloc((size_t)n));
     CUDA_TRY(cudaMemsetAsync(ctx->d_acc, 0, sizeof(long long) * (size_t)n * 16, ctx->stream));   // the fused kernel leaves
     CUDA_TRY(cudaMemsetAsync(ctx->d_done, 0, sizeof(int) * (size_t)n, ctx->stream));             // both zeroed behind it
-    ctx->cap_n = n;
+    ctx->ws_n = n;
     ctx->epoch++;            // buffers moved: a captured graph holds the old addresses
     return DKS_OK;
 }
@@ -153,10 +140,9 @@ int persistent_grid(const dks_ctx* ctx, size_t smem, size_t reserve, int max_per
 // grows a per-call workspace buffer to at least `need` elements; a move changes the epoch (a captured graph holds the old
 // address)
 template <typename T>
-int grow(dks_ctx* ctx, T** p, size_t* cap, size_t need) {
-    if (need <= *cap) return DKS_OK;
-    TRY(dev_alloc(p, need));
-    *cap = need;
+int grow(dks_ctx* ctx, DevBuf<T>& buf, size_t need) {
+    if (need <= buf.size()) return DKS_OK;
+    CUDA_TRY(buf.alloc(need));
     ctx->epoch++;
     return DKS_OK;
 }
@@ -316,34 +302,6 @@ int on_member(dks_ctx* ctx, dks_ctx* m, F&& launch) {
     return rc;
 }
 
-// a device array of n elements owned by the fitted model (own_allocs)
-template <typename T>
-int own_alloc(dks_ctx* ctx, T** p, size_t n) {
-    *p = nullptr;
-    TRY(dev_alloc(p, n));
-    ctx->own_allocs.push_back((void*)*p);
-    return DKS_OK;
-}
-
-// the device copy of a host array, owned by the fitted model
-template <typename T>
-int own_upload(dks_ctx* ctx, const T** dst, const T* src, size_t n) {
-    T* p;
-    TRY(own_alloc(ctx, &p, n));
-    CUDA_TRY(cudaMemcpyAsync(p, src, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
-    *dst = p;
-    return DKS_OK;
-}
-
-// frees every device array of the fitted model, its column encoding included
-void free_own_model(dks_ctx* ctx) {
-    for (void* q : ctx->own_allocs) cudaFree(q);
-    ctx->own_allocs.clear();
-    ctx->enc = EncodingDev{};
-    ctx->fitted = false;
-    ctx->prepared = false;
-}
-
 // the end of a family's dks_set_*: its head, and the linear part stage 1 evaluates while it decides the varying groups --
 // one zero score row, no column maps
 int set_own_model(dks_ctx* ctx, int act, int C, int scalar_out) {
@@ -412,62 +370,64 @@ int check_own_columns(const dks_ctx* ctx, const OwnKernel& ok) {
 // E[j][v] of every background row and training row
 int own_fit_tables(dks_ctx* ctx, const double* bg, int width) {
     const int N = ctx->N;
+    DevPool& pool = ctx->fit_pool;
+    const cudaStream_t st = ctx->stream;
     switch (ctx->head.family) {
     case DKS_GENERAL_TREES: {
         TreeDev& t = ctx->tree;
         const size_t nodes = (size_t)t.nodes;
         const std::vector<int32_t> colgrp = column_groups(ctx);
-        TRY(own_upload(ctx, &t.feat, ctx->h_tfeat.data(), nodes));
-        TRY(own_upload(ctx, &t.thr, ctx->h_tthr.data(), nodes));
-        TRY(own_upload(ctx, &t.left, ctx->h_tleft.data(), nodes));
-        TRY(own_upload(ctx, &t.right, ctx->h_tright.data(), nodes));
-        TRY(own_upload(ctx, &t.miss, ctx->h_tmiss.data(), nodes));
-        TRY(own_upload(ctx, &t.val, ctx->h_tval.data(), nodes * t.R));
-        TRY(own_upload(ctx, &t.roots, ctx->h_troots.data(), (size_t)t.T));
-        TRY(own_upload(ctx, &t.base, ctx->h_tbase.data(), (size_t)t.R));
-        TRY(own_upload(ctx, &t.colgrp, colgrp.data(), colgrp.size()));
+        CUDA_TRY(pool.upload(&t.feat, ctx->h_tfeat.data(), nodes, st));
+        CUDA_TRY(pool.upload(&t.thr, ctx->h_tthr.data(), nodes, st));
+        CUDA_TRY(pool.upload(&t.left, ctx->h_tleft.data(), nodes, st));
+        CUDA_TRY(pool.upload(&t.right, ctx->h_tright.data(), nodes, st));
+        CUDA_TRY(pool.upload(&t.miss, ctx->h_tmiss.data(), nodes, st));
+        CUDA_TRY(pool.upload(&t.val, ctx->h_tval.data(), nodes * t.R, st));
+        CUDA_TRY(pool.upload(&t.roots, ctx->h_troots.data(), (size_t)t.T, st));
+        CUDA_TRY(pool.upload(&t.base, ctx->h_tbase.data(), (size_t)t.R, st));
+        CUDA_TRY(pool.upload(&t.colgrp, colgrp.data(), colgrp.size(), st));
         unsigned char* bgdir;
-        TRY(own_alloc(ctx, &bgdir, (size_t)N * nodes));
+        CUDA_TRY(pool.alloc(&bgdir, (size_t)N * nodes));
         t.bgdir = bgdir;
-        dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, ctx->stream>>>(bg, N, width, t, bgdir);
+        dks::trees::tree_bgdir_kernel<<<cdiv((long long)N * nodes, 256), 256, 0, st>>>(bg, N, width, t, bgdir);
         break;
     }
     case DKS_GENERAL_KMACH: {
         KmDev& k = ctx->km;
-        TRY(own_upload(ctx, &k.sv, ctx->h_ksv.data(), ctx->h_ksv.size()));
-        TRY(own_upload(ctx, &k.dual, ctx->h_kdual.data(), ctx->h_kdual.size()));
-        TRY(own_upload(ctx, &k.colw, ctx->h_kcolw.data(), ctx->h_kcolw.size()));
-        TRY(own_upload(ctx, &k.colo, ctx->h_kcolo.data(), ctx->h_kcolo.size()));
+        CUDA_TRY(pool.upload(&k.sv, ctx->h_ksv.data(), ctx->h_ksv.size(), st));
+        CUDA_TRY(pool.upload(&k.dual, ctx->h_kdual.data(), ctx->h_kdual.size(), st));
+        CUDA_TRY(pool.upload(&k.colw, ctx->h_kcolw.data(), ctx->h_kcolw.size(), st));
+        CUDA_TRY(pool.upload(&k.colo, ctx->h_kcolo.data(), ctx->h_kcolo.size(), st));
         double* Tbg;
-        TRY(own_alloc(ctx, &Tbg, (size_t)N * k.n_sv));
+        CUDA_TRY(pool.alloc(&Tbg, (size_t)N * k.n_sv));
         k.Tbg = Tbg;
-        dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, ctx->stream>>>(bg, N, width, k, Tbg);
+        dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(bg, N, width, k, Tbg);
         break;
     }
     case DKS_GENERAL_MLP: {
         MlpDev& m = ctx->mlp;
-        TRY(own_upload(ctx, &m.W, ctx->h_mw.data(), ctx->h_mw.size()));
-        TRY(own_upload(ctx, &m.b, ctx->h_mb.data(), ctx->h_mb.size()));
-        TRY(own_upload(ctx, &m.Wf, ctx->h_mwf.data(), ctx->h_mwf.size()));
-        TRY(own_upload(ctx, &m.bp, ctx->h_mbp.data(), ctx->h_mbp.size()));
+        CUDA_TRY(pool.upload(&m.W, ctx->h_mw.data(), ctx->h_mw.size(), st));
+        CUDA_TRY(pool.upload(&m.b, ctx->h_mb.data(), ctx->h_mb.size(), st));
+        CUDA_TRY(pool.upload(&m.Wf, ctx->h_mwf.data(), ctx->h_mwf.size(), st));
+        CUDA_TRY(pool.upload(&m.bp, ctx->h_mbp.data(), ctx->h_mbp.size(), st));
         double* Bbg;
-        TRY(own_alloc(ctx, &Bbg, (size_t)N * m.width[1]));
+        CUDA_TRY(pool.alloc(&Bbg, (size_t)N * m.width[1]));
         m.Bbg = Bbg;
-        dks::mlp::mlp_fit_table_kernel<<<cdiv((long long)N * m.width[1], 256), 256, 0, ctx->stream>>>(bg, N, width, m, Bbg);
+        dks::mlp::mlp_fit_table_kernel<<<cdiv((long long)N * m.width[1], 256), 256, 0, st>>>(bg, N, width, m, Bbg);
         break;
     }
     case DKS_GENERAL_KNN: {
         KnnDev& k = ctx->knn;
         const std::vector<int32_t> colgrp = column_groups(ctx);
-        TRY(own_upload(ctx, &k.fitX, ctx->h_nfitX.data(), ctx->h_nfitX.size()));
-        TRY(own_upload(ctx, &k.colw, ctx->h_ncolw.data(), ctx->h_ncolw.size()));
-        TRY(own_upload(ctx, &k.colo, ctx->h_ncolo.data(), ctx->h_ncolo.size()));
-        TRY(own_upload(ctx, &k.y, ctx->h_ny.data(), ctx->h_ny.size()));
-        TRY(own_upload(ctx, &k.colgrp, colgrp.data(), colgrp.size()));
+        CUDA_TRY(pool.upload(&k.fitX, ctx->h_nfitX.data(), ctx->h_nfitX.size(), st));
+        CUDA_TRY(pool.upload(&k.colw, ctx->h_ncolw.data(), ctx->h_ncolw.size(), st));
+        CUDA_TRY(pool.upload(&k.colo, ctx->h_ncolo.data(), ctx->h_ncolo.size(), st));
+        CUDA_TRY(pool.upload(&k.y, ctx->h_ny.data(), ctx->h_ny.size(), st));
+        CUDA_TRY(pool.upload(&k.colgrp, colgrp.data(), colgrp.size(), st));
         double* Tbg;
         uint64_t* Ebg;
-        TRY(own_alloc(ctx, &Tbg, (size_t)N * k.n_fit));
-        TRY(own_alloc(ctx, &Ebg, (size_t)N * k.n_fit));
+        CUDA_TRY(pool.alloc(&Tbg, (size_t)N * k.n_fit));
+        CUDA_TRY(pool.alloc(&Ebg, (size_t)N * k.n_fit));
         k.Tbg = Tbg;
         k.Ebg = Ebg;
         dks::knn::knn_fit_table_kernel<<<cdiv((long long)N * k.n_fit, 256), 256, 0, ctx->stream>>>(bg, N, width, ctx->G, k,
@@ -521,7 +481,7 @@ int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const
         break;
     case DKS_GENERAL_ENSEMBLE: {    // every member's f_k(x) into d_ens_out [K][n][C], then f(x) = sum_k pi_k f_k(x)
         const int K = (int)ctx->ens.size();
-        TRY(grow(ctx, &ctx->d_ens_out, &ctx->cap_ens_out, (size_t)K * n * C));
+        TRY(grow(ctx, ctx->d_ens_out, (size_t)K * n * C));
         for (int k = 0; k < K; ++k) {
             dks_ctx* m = ctx->ens[k];
             double* outk = ctx->d_ens_out + (size_t)k * n * C;
@@ -546,7 +506,8 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
     const bool acc = ea.ey != nullptr;
     switch (ctx->head.family) {
     case DKS_GENERAL_TREES: {
-        TRY(grow(ctx, &ctx->tree.xinfo, &ctx->cap_txinfo, (size_t)grid * ctx->tree.nodes));
+        TRY(grow(ctx, ctx->txinfo, (size_t)grid * ctx->tree.nodes));
+        ctx->tree.xinfo = ctx->txinfo;
         auto kern = acc ? dks::trees::explain_tree_kernel<false, true>
                         : l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -578,7 +539,7 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         break;
     }
     case DKS_GENERAL_ENSEMBLE: {
-        TRY(grow(ctx, &ctx->d_ens_ey, &ctx->cap_ens_ey, (size_t)ctx->cur_n * ctx->C * p.S_cap));
+        TRY(grow(ctx, ctx->d_ens_ey, (size_t)ctx->cur_n * ctx->C * p.S_cap));
         for (size_t k = 0; k < ctx->ens.size(); ++k) {
             dks_ctx* m = ctx->ens[k];
             m->cur_n = ctx->cur_n;                  // the rows, background and group CSR of this call
@@ -629,12 +590,12 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
                       : (maps ? prep_kernel_for<false, true>(h.mixture(), R) : prep_kernel_for<false, false>(h.mixture(), R));
     // nibble tables for the shared-plan route: the binary head's at any G, the other heads' up to 128 groups (what their
     // shared-plan route covers)
-    double* xt = !own && (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT : nullptr;
+    double* xt = !own && (h.xt_any || (G <= 128 && ctx->plan_mode == 0)) ? ctx->d_XT.get() : nullptr;
     if (psm > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm));
     // a model behind a column encoding: its kernels read the encoded rows, the encoded background and the encoded group CSR
     // (a refused value is reported by the encoding); stage 1 decides the varying groups on the raw rows
     const bool enc = own && ctx->enc.E > 0;
-    if (enc) TRY(grow(ctx, &ctx->d_Xenc, &ctx->cap_Xenc, (size_t)n * ctx->enc.E));
+    if (enc) TRY(grow(ctx, ctx->d_Xenc, (size_t)n * ctx->enc.E));
     ctx->own_X = enc ? ctx->d_Xenc : X_dev;
     ctx->own_D = enc ? ctx->enc.E : ctx->D;
     ctx->own_bg = enc ? ctx->d_bg_enc : ctx->d_bg;
@@ -644,8 +605,8 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
         X_dev, ctx->d_W, ctx->d_b, ctx->d_bg, ctx->d_goff, ctx->d_gcols, ctx->d_colmin, ctx->d_colmax, ctx->d_colnan,
         ctx->d_linkfnull, n, ctx->N, ctx->D, G, R, own ? 1 : ctx->C, own ? DKS_ACT_IDENTITY : ctx->act, own ? 1.0 : ctx->kappa,
         ctx->link, ipb, ctx->d_XW, ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full,
-        ctx->d_idx_other, xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
-    if (own) TRY(launch_own_predict(ctx, X_dev, n, enc ? ctx->d_Xenc : nullptr, ctx->d_linkfnull, nullptr, ctx->d_dlink));
+        ctx->d_idx_other, xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar.get() : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
+    if (own) TRY(launch_own_predict(ctx, X_dev, n, enc ? ctx->d_Xenc.get() : nullptr, ctx->d_linkfnull, nullptr, ctx->d_dlink));
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
@@ -850,33 +811,27 @@ int fail_refused(const dks_ctx* ctx, const char* prefix) {
                 "pipeline raises)", prefix, row, ctx->head.own() ? "the column encoding" : "its column map");
 }
 
-void free_column_maps(dks_ctx* ctx) {
-    int* hdr = const_cast<int*>(ctx->cm.hdr);
-    double* keys = const_cast<double*>(ctx->cm.keys);
-    double* vals = const_cast<double*>(ctx->cm.vals);
-    dev_free(&hdr); dev_free(&keys); dev_free(&vals);
-    ctx->cm = ColumnMapsDev{};
-}
-
 // the start of dks_fit for every family: the background, its weights, the linear model's W and b, the groups and the
-// column statistics stage 1 decides the varying groups with on the device; fnull's buffers; no column maps and none of the
-// previous fit's family arrays; status cleared
+// column statistics stage 1 decides the varying groups with on the device; fnull's buffers; none of the previous fit's
+// arrays (column maps, column encoding, family arrays); status cleared
 int fit_begin(dks_ctx* ctx) {
     const int N = ctx->N, D = ctx->D, G = ctx->G, R = ctx->R, C = ctx->C;
     const cudaStream_t st = ctx->stream;
-    TRY(dev_alloc(&ctx->d_bg, (size_t)N * D));
-    TRY(dev_alloc(&ctx->d_wbg, (size_t)N));
-    TRY(dev_alloc(&ctx->d_W, (size_t)R * D));
-    TRY(dev_alloc(&ctx->d_b, (size_t)R));
-    TRY(dev_alloc(&ctx->d_goff, (size_t)G + 1));
-    TRY(dev_alloc(&ctx->d_gcols, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmin, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colmax, (size_t)D));
-    TRY(dev_alloc(&ctx->d_colnan, (size_t)D));
-    TRY(dev_alloc(&ctx->d_fnull, (size_t)C));
-    TRY(dev_alloc(&ctx->d_linkfnull, (size_t)C));
-    free_column_maps(ctx);
-    free_own_model(ctx);
+    CUDA_TRY(ctx->d_bg.alloc((size_t)N * D));
+    CUDA_TRY(ctx->d_wbg.alloc((size_t)N));
+    CUDA_TRY(ctx->d_W.alloc((size_t)R * D));
+    CUDA_TRY(ctx->d_b.alloc((size_t)R));
+    CUDA_TRY(ctx->d_goff.alloc((size_t)G + 1));
+    CUDA_TRY(ctx->d_gcols.alloc((size_t)D));
+    CUDA_TRY(ctx->d_colmin.alloc((size_t)D));
+    CUDA_TRY(ctx->d_colmax.alloc((size_t)D));
+    CUDA_TRY(ctx->d_colnan.alloc((size_t)D));
+    CUDA_TRY(ctx->d_fnull.alloc((size_t)C));
+    CUDA_TRY(ctx->d_linkfnull.alloc((size_t)C));
+    ctx->fit_pool.clear();
+    ctx->cm = ColumnMapsDev{}; ctx->enc = EncodingDev{};
+    ctx->fitted = false;
+    ctx->prepared = false;
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_bg, ctx->h_bg.data(), sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_wbg, ctx->h_wbg.data(), sizeof(double) * N, cudaMemcpyHostToDevice, st));
@@ -914,10 +869,10 @@ int fit_readback(dks_ctx* ctx, const char* family) {
 // the end of a successful dks_fit: workspace shapes depend on G, R and C, and the plans carry tables derived from the
 // background and model: drop them
 int fit_done(dks_ctx* ctx) {
-    ctx->cap_n = 0;
+    ctx->ws_n = 0;
     ctx->prepared = false;
-    for (const auto& allocs : ctx->plan_allocs)
-        if (!allocs.empty()) { TRY(drop_plans(ctx, -1)); break; }
+    for (const DevPool& pool : ctx->plan_pool)
+        if (!pool.empty()) { TRY(drop_plans(ctx, -1)); break; }
     ctx->fitted = true;
     ctx->epoch++;
     return DKS_OK;
@@ -930,12 +885,13 @@ int fit_encoding(dks_ctx* ctx) {
     if (E == 0) return DKS_OK;
     const cudaStream_t st = ctx->stream;
     EncodingDev& en = ctx->enc;
-    TRY(own_upload(ctx, &en.hdr, ctx->h_ehdr.data(), ctx->h_ehdr.size()));
-    TRY(own_upload(ctx, &en.ops, ctx->h_eops.data(), ctx->h_eops.size()));
-    TRY(own_upload(ctx, &en.opv, ctx->h_eopv.data(), ctx->h_eopv.size()));
-    TRY(own_upload(ctx, &en.tab, ctx->h_etab.data(), ctx->h_etab.size()));
+    DevPool& pool = ctx->fit_pool;
+    CUDA_TRY(pool.upload(&en.hdr, ctx->h_ehdr.data(), ctx->h_ehdr.size(), st));
+    CUDA_TRY(pool.upload(&en.ops, ctx->h_eops.data(), ctx->h_eops.size(), st));
+    CUDA_TRY(pool.upload(&en.opv, ctx->h_eopv.data(), ctx->h_eopv.size(), st));
+    CUDA_TRY(pool.upload(&en.tab, ctx->h_etab.data(), ctx->h_etab.size(), st));
     en.E = E;
-    TRY(own_alloc(ctx, &ctx->d_bg_enc, (size_t)ctx->N * E));
+    CUDA_TRY(pool.alloc(&ctx->d_bg_enc, (size_t)ctx->N * E));
     TRY(launch_encode(ctx, ctx->d_bg, ctx->N, ctx->d_bg_enc));
     const std::vector<int32_t> colgrp = column_groups(ctx);
     std::vector<int32_t> goff(G + 1, 0), gcols(E);
@@ -943,8 +899,8 @@ int fit_encoding(dks_ctx* ctx) {
     for (int g = 0; g < G; ++g) goff[g + 1] += goff[g];
     std::vector<int32_t> at(goff.begin(), goff.end() - 1);
     for (int e = 0; e < E; ++e) gcols[at[colgrp[e]]++] = e;
-    TRY(own_alloc(ctx, &ctx->d_egoff, (size_t)G + 1));
-    TRY(own_alloc(ctx, &ctx->d_egcols, (size_t)E));
+    CUDA_TRY(pool.alloc(&ctx->d_egoff, (size_t)G + 1));
+    CUDA_TRY(pool.alloc(&ctx->d_egcols, (size_t)E));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_egoff, goff.data(), sizeof(int32_t) * (G + 1), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_egcols, gcols.data(), sizeof(int32_t) * E, cudaMemcpyHostToDevice, st));
     return DKS_OK;
@@ -976,7 +932,7 @@ int fit_members(dks_ctx* ctx, const OwnKernel& ok) {
                         "mean prediction is 0 or 1 under the logit link, or overflows", ok.model, c, fnull[c]);
     }
     const cudaStream_t st = ctx->stream;
-    TRY(own_upload(ctx, &ctx->d_ens_pi, ctx->h_ens_pi.data(), ctx->h_ens_pi.size()));
+    CUDA_TRY(ctx->fit_pool.upload(&ctx->d_ens_pi, ctx->h_ens_pi.data(), ctx->h_ens_pi.size(), st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_fnull, fnull.data(), sizeof(double) * C, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_linkfnull, linkfnull.data(), sizeof(double) * C, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -996,14 +952,12 @@ int fit_own(dks_ctx* ctx) {
     if (ctx->head.family == DKS_GENERAL_ENSEMBLE) return fit_members(ctx, ok);
     const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
     TRY(own_fit_tables(ctx, bg, model_columns(ctx)));
-    double* pred = nullptr;
-    TRY(dev_alloc(&pred, (size_t)N * C));
+    DevBuf<double> pred;
+    CUDA_TRY(pred.alloc((size_t)N * C));
     TRY(launch_own_predict(ctx, bg, N, nullptr, nullptr, pred, nullptr));
     dks::fit_pred_fnull_kernel<<<1, 32, 0, ctx->stream>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
     ctx->launches += 1;
-    const int rc = fit_readback(ctx, ok.model);
-    cudaFree(pred);
-    TRY(rc);
+    TRY(fit_readback(ctx, ok.model));
     return fit_done(ctx);
 }
 
@@ -1171,17 +1125,17 @@ int launch_sampler(dks_ctx* ctx, const Route& rt, ExplainParams* p) {
     const SamplerConfig& sc = rt.sc;
     const int n = ctx->cur_n;
     const size_t need = (size_t)n * sc.stride;
-    if (need > ctx->cap_gen || sc.W != ctx->gen_words) {
-        TRY(dev_alloc(&ctx->d_genz, need * sc.W)); TRY(dev_alloc(&ctx->d_genw, need));
-        ctx->cap_gen = need; ctx->gen_words = sc.W; ctx->epoch++;
+    if (need > ctx->d_genw.size() || sc.W != ctx->gen_words) {
+        CUDA_TRY(ctx->d_genz.alloc(need * sc.W)); CUDA_TRY(ctx->d_genw.alloc(need));
+        ctx->gen_words = sc.W; ctx->epoch++;
     }
     const size_t needf = (size_t)n * sc.fstride;
-    if (needf > ctx->cap_genf || (!rt.wide_pi && ctx->d_genainv == nullptr)) {
+    if (needf > ctx->d_genchol.size() || (!rt.wide_pi && ctx->d_genainv == nullptr)) {
         // two-word rows keep one matrix per instance (inverted in place); one-word rows its factor and its inverse
-        TRY(dev_alloc(&ctx->d_genchol, needf));
-        if (rt.wide_pi) dev_free(&ctx->d_genainv);
-        else TRY(dev_alloc(&ctx->d_genainv, needf));
-        ctx->cap_genf = needf; ctx->epoch++;
+        CUDA_TRY(ctx->d_genchol.alloc(needf));
+        if (rt.wide_pi) ctx->d_genainv.reset();
+        else CUDA_TRY(ctx->d_genainv.alloc(needf));
+        ctx->epoch++;
     }
     dks::sampler::SamplerParams sp;
     sp.n = n; sp.G = ctx->G; sp.S_req = ctx->nsamples_req; sp.stride = sc.stride; sp.seed = ctx->sampler_seed;
@@ -1208,7 +1162,7 @@ int launch_sampler(dks_ctx* ctx, const Route& rt, ExplainParams* p) {
     CUDA_TRY(cudaGetLastError());
     ctx->gen_stride = sc.stride; ctx->gen_n = n; ctx->gen_plan_words = sc.W;
     p->ext_z = ctx->d_genz; p->ext_w = ctx->d_genw; p->ext_stride = sc.stride;
-    p->ext_chol = rt.wide_pi ? nullptr : ctx->d_genchol; p->ext_ainv = rt.wide_pi ? ctx->d_genchol : ctx->d_genainv;
+    p->ext_chol = rt.wide_pi ? nullptr : ctx->d_genchol.get(); p->ext_ainv = rt.wide_pi ? ctx->d_genchol : ctx->d_genainv;
     p->ext_fstride = sc.fstride;
     return DKS_OK;
 }
@@ -1218,7 +1172,7 @@ int launch_sampler(dks_ctx* ctx, const Route& rt, ExplainParams* p) {
 int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, double* phi_dev) {
     const int n = ctx->cur_n, G = ctx->G;
     int32_t* path = ctx->last_path;
-    const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn;
+    const float* wn = ctx->uniform_w ? nullptr : ctx->d_wn.get();
     if (rt.shared == ROUTE_FUSED) {
         // link + projection solve inside the coalition kernel: no (sum p1, sum p0) buffer, no separate solve launch
         const dks::shared_path::FusedConfig& fcfg = rt.fcfg;
@@ -1241,7 +1195,7 @@ int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, doubl
                 if (slab == phi_dev) continue;               // phi is written in place into the local slab
                 slabs[np++] = slab;
             }
-            if (!ctx->d_peer_list) TRY(dev_alloc(&ctx->d_peer_list, (size_t)16));
+            if (!ctx->d_peer_list) CUDA_TRY(ctx->d_peer_list.alloc(16));
             if (ctx->peer_list_for != phi_dev) {             // (never during a capture: the graph key holds the phi pointer)
                 CUDA_TRY(cudaMemcpy(ctx->d_peer_list, slabs, sizeof(double*) * np, cudaMemcpyHostToDevice));
                 ctx->peer_list_for = phi_dev;
@@ -1259,14 +1213,14 @@ int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, doubl
         return DKS_OK;
     }
     const size_t need = (size_t)n * pg.S_pad;
-    TRY(grow(ctx, &ctx->d_sums, &ctx->cap_sums, need));
+    TRY(grow(ctx, ctx->d_sums, need));
     dks::shared_path::SharedParams sp;
     sp.n = n; sp.N = ctx->N; sp.G = G; sp.S = pg.S; sp.S_pad = pg.S_pad; sp.scale = ctx->head.scale;
     sp.DmT = pg.dmT; sp.dme = pg.dme; sp.z = pg.z; sp.XT = ctx->d_XT; sp.list = ctx->d_idx_full; sp.count = ctx->d_counts; sp.sums = ctx->d_sums; sp.accumulate = 0;
     sp.acache = nullptr; sp.acache_mode = 0; sp.wn = wn;
     if (pg.W > 2 && ctx->N > dks::shared_path::MAXN) {
         // sixteen-word rows, several background chunks: A(i, s) is computed by the first chunk's launch only
-        TRY(grow(ctx, &ctx->d_acache, &ctx->cap_acache, need));
+        TRY(grow(ctx, ctx->d_acache, need));
         sp.acache = ctx->d_acache;
     }
     if (rt.shared == ROUTE_BINARY) {
@@ -1280,9 +1234,9 @@ int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, doubl
     }
     // binary members: the binary head's kernel per member, into the member buffer, then added times pi_k
     const size_t stride = 2 * (size_t)pg.S_pad;
-    TRY(grow(ctx, &ctx->d_mixscr, &ctx->cap_mixscr, (size_t)n * stride));
+    TRY(grow(ctx, ctx->d_mixscr, (size_t)n * stride));
     const size_t xt_member = (size_t)n * ((G + 3) / 4) * 16;
-    sp.scale = -DKS_LOG2E; sp.sums = reinterpret_cast<float2*>(ctx->d_mixscr);
+    sp.scale = -DKS_LOG2E; sp.sums = reinterpret_cast<float2*>(ctx->d_mixscr.get());
     int chunks = 0, warps = 0, grid = 0;
     for (int k = 0; k < ctx->mix.K; ++k) {
         sp.DmT = ctx->full.dm[k]; sp.dme = ctx->full.dme[k]; sp.XT = ctx->d_XT + k * xt_member;
@@ -1291,7 +1245,7 @@ int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, doubl
         if (nl == 0) return fail(DKS_ERR_CUDA, "shared-plan kernel: %s", cudaGetErrorString(cudaGetLastError()));
         ctx->launches += nl;
         chunks += sl.chunks; warps = k == 0 ? sl.warps : std::min(warps, sl.warps); grid = std::max(grid, sl.grid);
-        TRY(launch_mix_axpy(ctx, reinterpret_cast<float*>(ctx->d_sums), ctx->mix.pif[k], k == 0, (int)stride, n));
+        TRY(launch_mix_axpy(ctx, reinterpret_cast<float*>(ctx->d_sums.get()), ctx->mix.pif[k], k == 0, (int)stride, n));
     }
     path[DKS_PATH_SHARED] = DKS_SHARED_MIX; path[DKS_PATH_CHUNKS] = chunks;
     path[DKS_PATH_WARPS] = warps; path[DKS_PATH_GRID] = grid;
@@ -1305,8 +1259,8 @@ int launch_binary_solve(dks_ctx* ctx, const Route& rt, const PlanDev& pg, double
         TRY(launch_l1(ctx, pg, n, dks::shared_path::HeadSource{}, phi_dev));
     } else if (rt.solve == DKS_SOLVE_WIDE) {
         // more than 128 groups: link, float64 product with the host-supplied projection, remainder (dks_wide.cuh)
-        TRY(grow(ctx, &ctx->d_yw, &ctx->cap_yw, (size_t)n * S_pad));
-        TRY(grow(ctx, &ctx->d_betaw, &ctx->cap_betaw, (size_t)n * pg.kpw));
+        TRY(grow(ctx, ctx->d_yw, (size_t)n * S_pad));
+        TRY(grow(ctx, ctx->d_betaw, (size_t)n * pg.kpw));
         dks::wide::WideParams qp;
         memset(&qp, 0, sizeof(qp));
         qp.n = n; qp.N = ctx->N; qp.G = G; qp.C = ctx->C; qp.S = S; qp.S_pad = S_pad; qp.KP = pg.kpw; qp.link = ctx->link;
@@ -1364,8 +1318,8 @@ int launch_class_sums(dks_ctx* ctx, const Route& rt, const PlanDev& pg, dks::sha
     // the workspace is C n S_pad floats: the engine explains these heads in row blocks of 2 / C the binary path's
     const bool members = rt.shared == ROUTE_CLASS_MEMBERS;
     const size_t need = (size_t)n * C * S_pad;
-    TRY(grow(ctx, &ctx->d_msums, &ctx->cap_msums, need));
-    if (members) TRY(grow(ctx, &ctx->d_mixscr, &ctx->cap_mixscr, need));
+    TRY(grow(ctx, ctx->d_msums, need));
+    if (members) TRY(grow(ctx, ctx->d_mixscr, need));
     dks::multi::SoftmaxParams mp;
     memset(&mp, 0, sizeof(mp));
     mp.n = n; mp.N = ctx->N; mp.G = G; mp.S = pg.S; mp.S_pad = S_pad; mp.ntab = src->ntab; mp.scale = DKS_LOG2E;
@@ -1517,11 +1471,11 @@ int launch_general(dks_ctx* ctx, const Route& rt, ExplainParams p, cudaStream_t 
 int prepare_debug_dump(dks_ctx* ctx, int S_cap) {
     const int rows = S_cap, cols = dks::tc_npad(ctx->N);
     if (rows != ctx->dbg_rows || cols != ctx->dbg_cols) {
-        TRY(dev_alloc(&ctx->dbg_T, (size_t)rows * cols));
+        CUDA_TRY(ctx->dbg_T.alloc((size_t)rows * cols));
         ctx->dbg_rows = rows; ctx->dbg_cols = cols;
     }
     CUDA_TRY(cudaMemsetAsync(ctx->dbg_T, 0, sizeof(float) * rows * cols, ctx->stream));
-    if (!ctx->dbg_time) TRY(dev_alloc(&ctx->dbg_time, (size_t)6 * 256));
+    if (!ctx->dbg_time) CUDA_TRY(ctx->dbg_time.alloc(6 * 256));
     CUDA_TRY(cudaMemsetAsync(ctx->dbg_time, 0, sizeof(float) * 6 * 256, ctx->stream));
     return DKS_OK;
 }
@@ -1548,7 +1502,7 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     if (ctx->dbg_i >= 0) TRY(prepare_debug_dump(ctx, rt.S_cap));
     CUDA_TRY(record_ev(ctx, 2));
     ctx->l1_timing_valid = false;
-    if (ctx->l1_mode != 0) TRY(grow(ctx, &ctx->d_mom, &ctx->cap_mom, (size_t)n * ctx->head.l1_nout * (2 * G + 4)));
+    if (ctx->l1_mode != 0) TRY(grow(ctx, ctx->d_mom, (size_t)n * ctx->head.l1_nout * (2 * G + 4)));
     ctx->last_fused = rt.shared == ROUTE_FUSED;
     // the general kernels (instances that are not on the shared-plan route) fork off here and join at the end
     cudaStream_t gstream = ctx->stream;
@@ -1600,10 +1554,9 @@ int build_pmat(dks_ctx* ctx, PlanDev& pd, int M) {
           dks::shared_path::wls_pmat_smem(M, pd.S_pad) + 8192 <= (size_t)ctx->max_smem_optin))
         return DKS_OK;
     const int S = pd.S;
-    float* pm = nullptr; double* dv = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&pm, sizeof(float) * (size_t)(M - 1) * pd.S_pad));
-    CUDA_TRY(cudaMalloc((void**)&dv, sizeof(double) * (M - 1)));
-    ctx->plan_allocs[M].push_back(pm); ctx->plan_allocs[M].push_back(dv);
+    float* pm; double* dv;
+    CUDA_TRY(ctx->plan_pool[M].alloc(&pm, (size_t)(M - 1) * pd.S_pad));
+    CUDA_TRY(ctx->plan_pool[M].alloc(&dv, (size_t)(M - 1)));
     long long tot = (long long)(M - 1) * pd.S_pad;
     dks::shared_path::plan_pmat_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(pd.z, pd.w, pd.ainv, S, pd.S_pad, M, pm);
     dks::shared_path::plan_dvec_kernel<<<M - 1, 32, 0, ctx->stream>>>(pd.z, pm, S, pd.S_pad, M, dv);
@@ -1645,22 +1598,20 @@ int build_link_table(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz) {
     static const LinkTabFit fit = make_link_tab_fit();
     const int N = ctx->N, S_pad = pd.S_pad;
     cudaStream_t st = ctx->stream;
-    struct Scratch {
-        std::vector<void*> p;
-        ~Scratch() { for (void* q : p) cudaFree(q); }
-    } scratch;
-    double* ld = nullptr; double* wd = nullptr; LinkTabRow* rows = nullptr; unsigned long long* merr = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&ld, sizeof(double) * (size_t)N * S_pad)); scratch.p.push_back(ld);
-    CUDA_TRY(cudaMalloc((void**)&rows, sizeof(LinkTabRow) * (size_t)S_pad)); scratch.p.push_back(rows);
-    CUDA_TRY(cudaMalloc((void**)&merr, sizeof(unsigned long long))); scratch.p.push_back(merr);
+    DevBuf<double> ld, wd;
+    DevBuf<LinkTabRow> rows;
+    DevBuf<unsigned long long> merr;
+    CUDA_TRY(ld.alloc((size_t)N * S_pad));
+    CUDA_TRY(rows.alloc((size_t)S_pad));
+    CUDA_TRY(merr.alloc(1));
     if (!ctx->uniform_w) {
         std::vector<double> w(N);
         for (int j = 0; j < N; ++j) w[j] = (double)N * ctx->h_wbg[j];
-        CUDA_TRY(cudaMalloc((void**)&wd, sizeof(double) * N)); scratch.p.push_back(wd);
+        CUDA_TRY(wd.alloc((size_t)N));
         CUDA_TRY(cudaMemcpy(wd, w.data(), sizeof(double) * N, cudaMemcpyHostToDevice));
     }
     if (ctx->d_ltab_fb == nullptr) {
-        TRY(dev_alloc(&ctx->d_ltab_fb, 1));
+        CUDA_TRY(ctx->d_ltab_fb.alloc(1));
         CUDA_TRY(cudaMemset(ctx->d_ltab_fb, 0, sizeof(unsigned long long)));
     }
     std::vector<LinkTabRow> hr(S_pad);
@@ -1676,8 +1627,8 @@ int build_link_table(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz) {
         for (LinkTabRow& r : hr) { r.off = (int)(total < (1LL << 30) ? total : 0); total += r.nint; maxn = std::max(maxn, r.nint); }
         const size_t bytes = sizeof(LinkTabEntry) * (size_t)total + sizeof(LinkTabRow) * (size_t)S_pad;
         if (bytes > LTAB_BUDGET || maxn > 65535 * 128) return DKS_OK;     // a finer grid only makes it larger
-        LinkTabEntry* tab = nullptr;
-        CUDA_TRY(cudaMalloc((void**)&tab, sizeof(LinkTabEntry) * (size_t)std::max(total, 1LL))); scratch.p.push_back(tab);
+        DevBuf<LinkTabEntry> tab;
+        CUDA_TRY(tab.alloc((size_t)total));
         CUDA_TRY(cudaMemcpyAsync(rows, hr.data(), sizeof(LinkTabRow) * S_pad, cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaMemsetAsync(merr, 0, sizeof(unsigned long long), st));
         const dim3 grid(S_pad, cdiv(maxn, 128));
@@ -1692,10 +1643,9 @@ int build_link_table(dks_ctx* ctx, PlanDev& pd, int M, const uint64_t* dz) {
         double err;
         memcpy(&err, &bits, sizeof(err));
         if (err <= LTAB_TOL) {
-            scratch.p.pop_back();                                    // tab and rows now belong to the plan
-            scratch.p.erase(std::find(scratch.p.begin(), scratch.p.end(), (void*)rows));
-            ctx->plan_allocs[M].push_back(tab); ctx->plan_allocs[M].push_back(rows);
             pd.ltab = tab; pd.ltab_rows = rows; pd.ltab_inv_h = 1.0 / h; pd.ltab_bytes = (long long)bytes;
+            ctx->plan_pool[M].adopt(std::move(tab));                 // tab and rows now belong to the plan
+            ctx->plan_pool[M].adopt(std::move(rows));
             return DKS_OK;
         }
     }
@@ -1734,28 +1684,25 @@ int fit_model(dks_ctx* ctx) {
         return fail(DKS_ERR_UNSUPPORTED, "dks_fit: a column encoding is set, but the model has no kernel of its own (linear "
                     "models read their pipelines through dks_set_column_maps)");
     TRY(fit_begin(ctx));
-    TRY(dev_alloc(&ctx->d_BW, (size_t)N * G * R));
-    TRY(dev_alloc(&ctx->d_scores, (size_t)N * R));
-    TRY(dev_alloc(&ctx->d_Bbar, (size_t)G * R));
-    TRY(dev_alloc(&ctx->d_BWs, (size_t)N * G * R));
-    TRY(dev_alloc(&ctx->d_bases, (size_t)N * R));
-    TRY(dev_alloc(&ctx->d_wbf, (size_t)N));
-    TRY(dev_alloc(&ctx->d_wn, (size_t)N));
-    TRY(dev_alloc(&ctx->d_mix, (size_t)1));
+    CUDA_TRY(ctx->d_BW.alloc((size_t)N * G * R));
+    CUDA_TRY(ctx->d_scores.alloc((size_t)N * R));
+    CUDA_TRY(ctx->d_Bbar.alloc((size_t)G * R));
+    CUDA_TRY(ctx->d_BWs.alloc((size_t)N * G * R));
+    CUDA_TRY(ctx->d_bases.alloc((size_t)N * R));
+    CUDA_TRY(ctx->d_wbf.alloc((size_t)N));
+    CUDA_TRY(ctx->d_wn.alloc((size_t)N));
+    CUDA_TRY(ctx->d_mix.alloc(1));
     cudaStream_t st = ctx->stream;
     CUDA_TRY(cudaMemcpyAsync(ctx->d_mix, &ctx->mix, sizeof(MixHead), cudaMemcpyHostToDevice, st));
     const bool maps = !ctx->h_cm_hdr.empty();
     if (maps) {
-        const size_t nk = ctx->h_cm_keys.size(), nv = ctx->h_cm_vals.size();
-        int* hdr = nullptr;
-        double *keys = nullptr, *vals = nullptr;
-        TRY(dev_alloc(&hdr, ctx->h_cm_hdr.size()));
-        TRY(dev_alloc(&keys, nk));
-        TRY(dev_alloc(&vals, nv));
-        CUDA_TRY(cudaMemcpy(hdr, ctx->h_cm_hdr.data(), sizeof(int) * ctx->h_cm_hdr.size(), cudaMemcpyHostToDevice));
-        if (nk) CUDA_TRY(cudaMemcpy(keys, ctx->h_cm_keys.data(), sizeof(double) * nk, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(vals, ctx->h_cm_vals.data(), sizeof(double) * nv, cudaMemcpyHostToDevice));
-        ctx->cm = ColumnMapsDev{hdr, keys, vals, (int)nk, (int)nv};
+        ColumnMapsDev& cm = ctx->cm;
+        DevPool& pool = ctx->fit_pool;
+        CUDA_TRY(pool.upload(&cm.hdr, ctx->h_cm_hdr.data(), ctx->h_cm_hdr.size(), st));
+        CUDA_TRY(pool.upload(&cm.keys, ctx->h_cm_keys.data(), ctx->h_cm_keys.size(), st));
+        CUDA_TRY(pool.upload(&cm.vals, ctx->h_cm_vals.data(), ctx->h_cm_vals.size(), st));
+        cm.n_keys = (int)ctx->h_cm_keys.size();
+        cm.n_vals = (int)ctx->h_cm_vals.size();
     }
     {
         // the weighted shared-plan kernels read w'_j = N w_j: their sums then have the magnitude of the uniform ones
@@ -1767,8 +1714,8 @@ int fit_model(dks_ctx* ctx) {
         ctx->d_bg, ctx->d_W, ctx->d_goff, ctx->d_gcols, N, D, G, R, ctx->d_BW, ctx->cm, ctx->d_status);
     dks::fit_scores_kernel<<<cdiv((long long)N * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_b, N, G, R, ctx->d_scores);
     if (h.mixture()) {
-        TRY(dev_alloc(&ctx->d_mixBW, (size_t)N * G * R));
-        TRY(dev_alloc(&ctx->d_mixsc, (size_t)N * R));
+        CUDA_TRY(ctx->d_mixBW.alloc((size_t)N * G * R));
+        CUDA_TRY(ctx->d_mixsc.alloc((size_t)N * R));
         dks::mix::mix_split_kernel<<<cdiv((long long)N * G * R, 256), 256, 0, st>>>(ctx->d_BW, ctx->d_scores, N, G, ctx->mix.K,
                                                                                     ctx->mix.Rm, ctx->d_mixBW, ctx->d_mixsc);
         ctx->launches += 1;
@@ -1790,7 +1737,6 @@ int fit_model(dks_ctx* ctx) {
 void destroy_members(dks_ctx* ctx) {
     for (dks_ctx* m : ctx->ens) {
         m->ens_parent = nullptr;
-        m->d_status = nullptr; m->d_counts = nullptr; m->d_hist = nullptr;
         dks_destroy(m);
     }
     ctx->ens.clear();
@@ -1827,7 +1773,7 @@ int dks_create(dks_ctx** out, int device) {
     if (prop.major != 9 || prop.minor != 0)
         return fail(DKS_ERR_UNSUPPORTED, "dks_create: device %d is sm_%d%d; this library is built for sm_90a only", device,
                     prop.major, prop.minor);
-    dks_ctx* ctx = new dks_ctx();
+    std::unique_ptr<dks_ctx> ctx(new dks_ctx());   // freed with what it holds on any failure below
     ctx->device = device;
     { const char* e = getenv("DKS_GRAPH"); ctx->graph_enabled = !(e && e[0] == '0'); }
     {
@@ -1847,16 +1793,17 @@ int dks_create(dks_ctx** out, int device) {
     CUDA_TRY(cudaStreamCreateWithFlags(&ctx->side_stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
     CUDA_TRY(cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming));
-    CUDA_TRY(cudaMalloc((void**)&ctx->d_plans, sizeof(ctx->h_plans)));
+    CUDA_TRY(ctx->d_plans.alloc(DKS_MAX_GROUPS + 1));
     CUDA_TRY(cudaMemset(ctx->d_plans, 0, sizeof(ctx->h_plans)));
-    CUDA_TRY(cudaMalloc((void**)&ctx->d_status, sizeof(int) * (4 + DKS_MAX_GROUPS + 1)));   // status, list counts, histogram
+    CUDA_TRY(ctx->status.alloc(4 + DKS_MAX_GROUPS + 1));   // status, list counts, histogram
+    ctx->d_status = ctx->status;
     ctx->d_counts = ctx->d_status + 2;
     ctx->d_hist = ctx->d_status + 4;
     CUDA_TRY(cudaMemset(ctx->d_status, 0, sizeof(int) * (4 + DKS_MAX_GROUPS + 1)));
-    CUDA_TRY(cudaMalloc((void**)&ctx->d_l1, sizeof(dks::l1::Tables) * (DKS_L1_MAX_GROUPS + 1)));
+    CUDA_TRY(ctx->d_l1.alloc(DKS_L1_MAX_GROUPS + 1));
     CUDA_TRY(cudaMemset(ctx->d_l1, 0, sizeof(dks::l1::Tables) * (DKS_L1_MAX_GROUPS + 1)));
-    CUDA_TRY(cudaMalloc((void**)&ctx->d_l1_counts, sizeof(int) * 2));
-    *out = ctx;
+    CUDA_TRY(ctx->d_l1_counts.alloc(2));
+    *out = ctx.release();
     return DKS_OK;
 }
 
@@ -1867,31 +1814,6 @@ int dks_destroy(dks_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     destroy_members(ctx);
-    dev_free(&ctx->d_ens_out); dev_free(&ctx->d_ens_ey);
-    if (ctx->gexec) { cudaGraphExecDestroy(ctx->gexec); ctx->gexec = nullptr; }
-    dev_free(&ctx->d_bg); dev_free(&ctx->d_wbg); dev_free(&ctx->d_W); dev_free(&ctx->d_b); dev_free(&ctx->d_mix);
-    dev_free(&ctx->d_mixBW); dev_free(&ctx->d_mixsc); dev_free(&ctx->d_mixscr);
-    free_own_model(ctx);
-    dev_free(&ctx->tree.xinfo);
-    dev_free(&ctx->d_Xenc);
-    free_column_maps(ctx);
-    dev_free(&ctx->d_goff); dev_free(&ctx->d_gcols); dev_free(&ctx->d_colmin); dev_free(&ctx->d_colmax);
-    dev_free(&ctx->d_colnan); dev_free(&ctx->d_BW); dev_free(&ctx->d_scores); dev_free(&ctx->d_Bbar);
-    dev_free(&ctx->d_fnull); dev_free(&ctx->d_linkfnull); dev_free(&ctx->d_BWs); dev_free(&ctx->d_bases);
-    dev_free(&ctx->d_wbf); dev_free(&ctx->d_wn); dev_free(&ctx->d_plans); dev_free(&ctx->d_X); dev_free(&ctx->d_XW); dev_free(&ctx->d_XT);
-    dev_free(&ctx->d_vflag); dev_free(&ctx->d_vmask); dev_free(&ctx->d_M); dev_free(&ctx->d_dlink);
-    dev_free(&ctx->d_idx_full); dev_free(&ctx->d_idx_other); dev_free(&ctx->d_idx_sel); dev_free(&ctx->d_idx_plain); dev_free(&ctx->d_l1_counts); dev_free(&ctx->d_l1); dev_free(&ctx->d_sums); dev_free(&ctx->d_msums); dev_free(&ctx->d_acc); dev_free(&ctx->d_done); dev_free(&ctx->d_ltab_fb); dev_free(&ctx->d_mom); dev_free(&ctx->d_step); dev_free(&ctx->d_peer_list);
-    dev_free(&ctx->d_status); ctx->d_hist = nullptr; ctx->d_counts = nullptr; dev_free(&ctx->d_yw); dev_free(&ctx->d_betaw); dev_free(&ctx->d_acache); dev_free(&ctx->d_phi); if (ctx->h_phi_pin) { cudaFreeHost(ctx->h_phi_pin); ctx->h_phi_pin = nullptr; } dev_free(&ctx->d_genz); dev_free(&ctx->d_genw); dev_free(&ctx->d_genchol); dev_free(&ctx->d_genainv); dev_free(&ctx->d_afix); dev_free(&ctx->d_sinfo); dev_free(&ctx->d_extz);
-    dev_free(&ctx->d_extw);
-    dev_free(&ctx->dbg_T);
-    dev_free(&ctx->dbg_time);
-    for (auto& allocs : ctx->plan_allocs) for (void* q : allocs) cudaFree(q);
-    for (int i = 0; i < 4; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
-    for (int i = 0; i < 3; ++i) if (ctx->ev_l1[i]) cudaEventDestroy(ctx->ev_l1[i]);
-    if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-    if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
-    if (ctx->side_stream) cudaStreamDestroy(ctx->side_stream);
-    if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
     return DKS_OK;
 }
@@ -2287,7 +2209,7 @@ int dks_set_ensemble(dks_ctx* ctx, int K, dks_ctx* const* members, const double*
         if (m->own_stream && m->stream) CUDA_TRY(cudaStreamDestroy(m->stream));
         m->stream = ctx->stream;
         m->own_stream = false;
-        dev_free(&m->d_status);
+        m->status.reset();
         m->d_status = ctx->d_status; m->d_counts = ctx->d_counts; m->d_hist = ctx->d_hist;
         m->head = describe_head(m);
         m->ens_parent = ctx;
@@ -2392,16 +2314,15 @@ int dks_encode_host(dks_ctx* ctx, const double* X_host, int n, double* out_host)
     REQUIRE(ctx->fitted && ctx->enc.E > 0, "dks_encode_host: call dks_fit with a column encoding set first");
     REQUIRE(X_host && out_host && n > 0, "dks_encode_host: bad arguments");
     const int E = ctx->enc.E;
-    double *dX = nullptr, *dO = nullptr;
-    TRY(dev_alloc(&dX, (size_t)n * ctx->D));
-    TRY(dev_alloc(&dO, (size_t)n * E));
+    DevBuf<double> dX, dO;
+    CUDA_TRY(dX.alloc((size_t)n * ctx->D));
+    CUDA_TRY(dO.alloc((size_t)n * E));
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
     TRY(launch_encode(ctx, dX, n, dO));
     CUDA_TRY(cudaMemcpyAsync(out_host, dO, sizeof(double) * n * E, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    cudaFree(dX); cudaFree(dO);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN) return fail_refused(ctx, "row");
     return DKS_OK;
 }
@@ -2439,14 +2360,14 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     BIND(ctx);
     REQUIRE(ctx->fitted, "dks_predict_host: call dks_fit first");
     REQUIRE(X_host && out_host && n > 0, "dks_predict_host: bad arguments");
-    double *dX = nullptr, *dO = nullptr;
-    TRY(dev_alloc(&dX, (size_t)n * ctx->D));
-    TRY(dev_alloc(&dO, (size_t)n * ctx->C));
+    DevBuf<double> dX, dO;
+    CUDA_TRY(dX.alloc((size_t)n * ctx->D));
+    CUDA_TRY(dO.alloc((size_t)n * ctx->C));
     CUDA_TRY(cudaMemcpyAsync(dX, X_host, sizeof(double) * n * ctx->D, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(ctx->d_status, 0, sizeof(int) * 2, ctx->stream));
-    double* dXe = nullptr;             // a model with its own kernel behind a column encoding reads the encoded rows
+    DevBuf<double> dXe;                // a model with its own kernel behind a column encoding reads the encoded rows
     if (ctx->head.own()) {
-        if (ctx->enc.E > 0) TRY(dev_alloc(&dXe, (size_t)n * ctx->enc.E));
+        if (ctx->enc.E > 0) CUDA_TRY(dXe.alloc((size_t)n * ctx->enc.E));
         TRY(launch_own_predict(ctx, dX, n, dXe, nullptr, dO, nullptr));
     } else {
         (ctx->cm.hdr ? dks::predict_kernel<true> : dks::predict_kernel<false>)<<<cdiv(n, 128), 128, 0, ctx->stream>>>(
@@ -2457,8 +2378,6 @@ int dks_predict_host(dks_ctx* ctx, const double* X_host, int n, double* out_host
     CUDA_TRY(cudaMemcpyAsync(out_host, dO, sizeof(double) * n * ctx->C, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    cudaFree(dX); cudaFree(dO);
-    if (dXe) cudaFree(dXe);
     if (ctx->h_status[0] == DKS_ERR_DOMAIN) return fail_refused(ctx, "row");
     return DKS_OK;
 }
@@ -2479,19 +2398,17 @@ int dks_effective_nsamples(dks_ctx* ctx, int M, int* S) {
 // uploads a plan of M groups and factors its normal matrix (plans of more than 128 groups: the host hands the projection
 // over with dks_set_plan_projection)
 static int upload_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, const double* w_host, PlanDev* out) {
-    uint64_t* dz = nullptr; double* dw = nullptr; double* dc = nullptr; double* di = nullptr;
+    DevPool& pool = ctx->plan_pool[M];
+    uint64_t* dz; double* dw; double* dc = nullptr; double* di = nullptr;
     const int W = dks_plan_words(M);                        // 64-bit words per coalition row
     const size_t S_even = ((size_t)S + 1) & ~(size_t)1;     // TMA bulk copies move 16-byte multiples
-    CUDA_TRY(cudaMalloc((void**)&dz, sizeof(uint64_t) * S_even * W));
-    CUDA_TRY(cudaMalloc((void**)&dw, sizeof(double) * S_even));
-    ctx->plan_allocs[M].push_back(dz); ctx->plan_allocs[M].push_back(dw);
+    CUDA_TRY(pool.alloc(&dz, S_even * W));
+    CUDA_TRY(pool.alloc(&dw, S_even));
     CUDA_TRY(cudaMemsetAsync(dz, 0, sizeof(uint64_t) * S_even * W, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(dw, 0, sizeof(double) * S_even, ctx->stream));
     if (W <= 2) {
-        CUDA_TRY(cudaMalloc((void**)&dc, sizeof(double) * (M - 1) * (M - 1)));
-        ctx->plan_allocs[M].push_back(dc);
-        CUDA_TRY(cudaMalloc((void**)&di, sizeof(double) * (M - 1) * (M - 1)));
-        ctx->plan_allocs[M].push_back(di);
+        CUDA_TRY(pool.alloc(&dc, (size_t)(M - 1) * (M - 1)));
+        CUDA_TRY(pool.alloc(&di, (size_t)(M - 1) * (M - 1)));
     }
     CUDA_TRY(cudaMemcpyAsync(dz, zbits_host, sizeof(uint64_t) * S * W, cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(dw, w_host, sizeof(double) * S, cudaMemcpyHostToDevice, ctx->stream));
@@ -2502,9 +2419,8 @@ static int upload_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, c
         dks::plan_factor_kernel<<<1, 256, smem, ctx->stream>>>(dz, dw, S, M, dc, di, ctx->d_status);
         ctx->launches += 1;
     } else if (W == 2) {
-        double* scratch = nullptr;
-        CUDA_TRY(cudaMalloc((void**)&scratch, sizeof(double) * (M - 1) * (M - 1)));
-        ctx->plan_allocs[M].push_back(scratch);
+        double* scratch;
+        CUDA_TRY(pool.alloc(&scratch, (size_t)(M - 1) * (M - 1)));
         size_t smem = sizeof(double) * (size_t)(M - 1) * (M - 1);
         CUDA_TRY(cudaFuncSetAttribute(dks::plan_factor_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         dks::plan_factor_wide_kernel<<<1, 1024, smem, ctx->stream>>>(dz, dw, S, M, dc, di, scratch, ctx->d_status);
@@ -2527,11 +2443,10 @@ static int upload_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, c
 static int build_dm_tables(dks_ctx* ctx, const PlanDev& pd, int M, const double* BW, const double* scores, double scale,
                            const float** dm_out, const double** dme_out) {
     const int N = ctx->N;
-    float* dm = nullptr;
-    double* dme = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&dm, sizeof(float) * (size_t)N * pd.S_pad));
-    CUDA_TRY(cudaMalloc((void**)&dme, sizeof(double) * (size_t)pd.S_pad));
-    ctx->plan_allocs[M].push_back(dm); ctx->plan_allocs[M].push_back(dme);
+    float* dm;
+    double* dme;
+    CUDA_TRY(ctx->plan_pool[M].alloc(&dm, (size_t)N * pd.S_pad));
+    CUDA_TRY(ctx->plan_pool[M].alloc(&dme, (size_t)pd.S_pad));
     const long long total = (long long)N * pd.S_pad;
     dks::shared_path::plan_dme_kernel<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(pd.z, pd.W, pd.S, pd.S_pad, BW, scores, N,
                                                                                    M, scale, dme);
@@ -2549,11 +2464,9 @@ static int build_class_tables(dks_ctx* ctx, const PlanDev& pd, int M, const doub
                               double scale, const float** dm_out, const float** lo_out) {
     const bool ovr = ctx->head.ovr;
     const int CS = ovr ? C + 1 : C;
-    float* sd = nullptr; float* sl = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&sd, sizeof(float) * (size_t)CS * ctx->N * pd.S_pad));
-    ctx->plan_allocs[M].push_back(sd);
-    CUDA_TRY(cudaMalloc((void**)&sl, sizeof(float) * (size_t)CS * pd.S_pad));
-    ctx->plan_allocs[M].push_back(sl);
+    float* sd; float* sl;
+    CUDA_TRY(ctx->plan_pool[M].alloc(&sd, (size_t)CS * ctx->N * pd.S_pad));
+    CUDA_TRY(ctx->plan_pool[M].alloc(&sl, (size_t)CS * pd.S_pad));
     auto kern = ovr ? (pd.W == 1 ? dks::multi::plan_ovr_kernel<1> : dks::multi::plan_ovr_kernel<2>)
                     : (pd.W == 1 ? dks::multi::plan_softmax_kernel<1> : dks::multi::plan_softmax_kernel<2>);
     kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(pd.z, pd.S, pd.S_pad, BW, scores, ctx->N, M, C, scale, sd, sl);
@@ -2577,10 +2490,9 @@ static int build_full_set_tables(dks_ctx* ctx, PlanDev& pd, int M) {
         // float64 P, row-major per coalition, for the fused kernel (link + solve inside the coalition kernel)
         if (pd.W == 1 && M <= 16) {
             const int kpad = dks::shared_path::fused_kpad(M);
-            double* pm64 = nullptr; double* dv64 = nullptr;
-            CUDA_TRY(cudaMalloc((void**)&pm64, sizeof(double) * (size_t)kpad * pd.S_pad));
-            CUDA_TRY(cudaMalloc((void**)&dv64, sizeof(double) * kpad));
-            ctx->plan_allocs[M].push_back(pm64); ctx->plan_allocs[M].push_back(dv64);
+            double* pm64; double* dv64;
+            CUDA_TRY(ctx->plan_pool[M].alloc(&pm64, (size_t)kpad * pd.S_pad));
+            CUDA_TRY(ctx->plan_pool[M].alloc(&dv64, (size_t)kpad));
             long long tot = (long long)kpad * pd.S_pad;
             dks::shared_path::plan_pmat64_kernel<<<cdiv(tot, 256), 256, 0, ctx->stream>>>(pd.z, pd.w, pd.ainv, pd.S, pd.S_pad, M,
                                                                                           kpad, pm64);
@@ -2609,9 +2521,8 @@ static int build_full_set_tables(dks_ctx* ctx, PlanDev& pd, int M) {
     case HEAD_SHARED_TABLES:
         if (h.expo) {
             // exp head: l(s) = log2 sum_j w_j 2^(log2 e d(s, j)) (head_y, dks_shared.cuh)
-            double* el = nullptr;
-            CUDA_TRY(cudaMalloc((void**)&el, sizeof(double) * (size_t)pd.S_pad));
-            ctx->plan_allocs[M].push_back(el);
+            double* el;
+            CUDA_TRY(ctx->plan_pool[M].alloc(&el, (size_t)pd.S_pad));
             auto kern = pd.W == 1 ? dks::shared_path::plan_exp_kernel<1> : dks::shared_path::plan_exp_kernel<2>;
             kern<<<cdiv(pd.S_pad, 128), 128, 0, ctx->stream>>>(pd.z, pd.S, pd.S_pad, ctx->d_BW, ctx->d_scores, ctx->d_wbg, N, M,
                                                               h.scale, el);
@@ -2629,7 +2540,7 @@ int dks_set_shared_plan(dks_ctx* ctx, int M, int S, const uint64_t* zbits_host, 
     BIND(ctx);
     REQUIRE(M >= 2 && M <= DKS_MAX_GROUPS, "dks_set_shared_plan: M=%d out of [2,%d]", M, DKS_MAX_GROUPS);
     REQUIRE(S >= 1 && zbits_host && w_host, "dks_set_shared_plan: bad arguments");
-    if (!ctx->plan_allocs[M].empty()) TRY(drop_plans(ctx, M));     // replacing the plan of this M (another nsamples)
+    if (!ctx->plan_pool[M].empty()) TRY(drop_plans(ctx, M));     // replacing the plan of this M (another nsamples)
     PlanDev pd;
     TRY(upload_plan(ctx, M, S, zbits_host, w_host, &pd));
     if (M == ctx->G && ctx->fitted && M <= ctx->head.shared_max_G) TRY(build_full_set_tables(ctx, pd, M));
@@ -2662,11 +2573,9 @@ int dks_set_plan_projection(dks_ctx* ctx, int M, const double* pt_host, const do
     REQUIRE(pd.z != nullptr && pd.W > 2, "dks_set_plan_projection: set the shared plan of M=%d first", M);
     REQUIRE(pd.ptw == nullptr, "dks_set_plan_projection: the M=%d plan already has its projection (replace the plan first)", M);
     const int nA = M - 1, kp = dks::wide::kpad(M);
-    double* pt = nullptr; double* dv = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&pt, sizeof(double) * (size_t)pd.S_pad * kp));
-    ctx->plan_allocs[M].push_back(pt);
-    CUDA_TRY(cudaMalloc((void**)&dv, sizeof(double) * kp));
-    ctx->plan_allocs[M].push_back(dv);
+    double* pt; double* dv;
+    CUDA_TRY(ctx->plan_pool[M].alloc(&pt, (size_t)pd.S_pad * kp));
+    CUDA_TRY(ctx->plan_pool[M].alloc(&dv, (size_t)kp));
     CUDA_TRY(cudaMemsetAsync(pt, 0, sizeof(double) * (size_t)pd.S_pad * kp, ctx->stream));
     CUDA_TRY(cudaMemsetAsync(dv, 0, sizeof(double) * kp, ctx->stream));
     // host [S][M-1] -> device [S_pad][kp] (zero padded rows and columns)
@@ -2700,9 +2609,8 @@ int dks_set_l1_tables(dks_ctx* ctx, int M, const double* gram_raw, const double*
     REQUIRE(pd.z != nullptr && n_aug == 2 * pd.S, "dks_set_l1_tables: set the shared plan of M=%d first (n_aug = 2 S)", M);
     const size_t mm = (size_t)M * M, S = (size_t)pd.S;
     const size_t total = 3 * mm + 3 * (size_t)M + 2 * S;
-    double* base = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&base, sizeof(double) * total));
-    ctx->plan_allocs[M].push_back(base);
+    double* base;
+    CUDA_TRY(ctx->plan_pool[M].alloc(&base, total));
     dks::l1::Tables d;
     memset(&d, 0, sizeof(d));
     double* q = base;
@@ -2737,17 +2645,16 @@ int dks_set_plan_sampling(dks_ctx* ctx, int M, int nfixed, int n_full, int n_pai
     const PlanDev& pd = ctx->h_plans[M];
     REQUIRE(pd.z != nullptr && nfixed <= pd.S, "dks_set_plan_sampling: set the shared plan of M=%d first", M);
     BIND(ctx);
-    double* af = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&af, sizeof(double) * (M - 1) * (M - 1)));
-    ctx->plan_allocs[M].push_back(af);
+    double* af;
+    CUDA_TRY(ctx->plan_pool[M].alloc(&af, (size_t)(M - 1) * (M - 1)));
     if (M <= 64) dks::plan_prefix_normal_kernel<<<1, 256, sizeof(double) * (M - 1) * (M - 1), ctx->stream>>>(pd.z, pd.w, nfixed, M, af);
     else dks::plan_prefix_normal_wide_kernel<<<1, 1024, 0, ctx->stream>>>(pd.z, pd.w, nfixed, M, af);
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     ctx->h_afix[M] = af;
     // device copies of the tables the sampler reads (kept current here, not per explain call)
-    if (!ctx->d_sinfo) TRY(dev_alloc(&ctx->d_sinfo, (size_t)(DKS_MAX_GROUPS + 1)));
-    if (!ctx->d_afix) TRY(dev_alloc(&ctx->d_afix, (size_t)(DKS_MAX_GROUPS + 1)));
+    if (!ctx->d_sinfo) CUDA_TRY(ctx->d_sinfo.alloc(DKS_MAX_GROUPS + 1));
+    if (!ctx->d_afix) CUDA_TRY(ctx->d_afix.alloc(DKS_MAX_GROUPS + 1));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_sinfo, ctx->h_sinfo, sizeof(ctx->h_sinfo), cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_afix, ctx->h_afix, sizeof(ctx->h_afix), cudaMemcpyHostToDevice, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
@@ -2810,7 +2717,7 @@ int dks_prepare_host(dks_ctx* ctx, const double* X_host, int n) {
     REQUIRE(ctx->fitted, "dks_prepare: call dks_fit first");
     REQUIRE(X_host && n > 0, "dks_prepare: need X and n > 0");
     size_t need = (size_t)n * ctx->D;
-    if (need > ctx->cap_X) { TRY(dev_alloc(&ctx->d_X, need)); ctx->cap_X = need; }
+    if (need > ctx->d_X.size()) CUDA_TRY(ctx->d_X.alloc(need));
     CUDA_TRY(cudaMemcpyAsync(ctx->d_X, X_host, sizeof(double) * need, cudaMemcpyHostToDevice, ctx->stream));
     return launch_prepare(ctx, ctx->d_X, n);
 }
@@ -2984,7 +2891,7 @@ int dks_set_peer_flags(dks_ctx* ctx, const uint64_t* flag_ptrs_host) {
         ctx->peer_flags[r] = reinterpret_cast<unsigned long long*>(flag_ptrs_host[r]);
     }
     if (!ctx->d_step) {
-        TRY(dev_alloc(&ctx->d_step, (size_t)1));
+        CUDA_TRY(ctx->d_step.alloc(1));
         CUDA_TRY(cudaMemset(ctx->d_step, 0, sizeof(unsigned long long)));
     }
     ctx->peer_flags_set = true;
@@ -3004,12 +2911,12 @@ int dks_explain_host(dks_ctx* ctx, const double* X_host, int n, double* phi_host
     REQUIRE(X_host && phi_host && n > 0, "dks_explain_host: bad arguments");
     TRY(dks_prepare_host(ctx, X_host, n));
     size_t need_phi = (size_t)ctx->C * n * ctx->G;
-    if (need_phi > ctx->cap_phi) { TRY(dev_alloc(&ctx->d_phi, need_phi)); ctx->cap_phi = need_phi; }
+    if (need_phi > ctx->d_phi.size()) CUDA_TRY(ctx->d_phi.alloc(need_phi));
     const uint64_t* dz = nullptr; const double* dw = nullptr;
     if (ext_zbits_host) {
         REQUIRE(ext_w_host && ext_stride > 0, "dks_explain_host: ext_w / ext_stride missing");
         size_t need = (size_t)n * ext_stride;
-        if (need > ctx->cap_ext) { TRY(dev_alloc(&ctx->d_extz, need)); TRY(dev_alloc(&ctx->d_extw, need)); ctx->cap_ext = need; }
+        if (need > ctx->d_extw.size()) { CUDA_TRY(ctx->d_extz.alloc(need)); CUDA_TRY(ctx->d_extw.alloc(need)); }
         CUDA_TRY(cudaMemcpyAsync(ctx->d_extz, ext_zbits_host, sizeof(uint64_t) * need, cudaMemcpyHostToDevice, ctx->stream));
         CUDA_TRY(cudaMemcpyAsync(ctx->d_extw, ext_w_host, sizeof(double) * need, cudaMemcpyHostToDevice, ctx->stream));
         dz = ctx->d_extz; dw = ctx->d_extw;
@@ -3024,12 +2931,7 @@ int dks_explain_host(dks_ctx* ctx, const double* X_host, int n, double* phi_host
         if (cudaPointerGetAttributes(&attr, phi_host) == cudaSuccess) direct = attr.type == cudaMemoryTypeHost;
         else cudaGetLastError();
     }
-    if (!direct && need_phi > ctx->cap_phi_pin) {
-        if (ctx->h_phi_pin) cudaFreeHost(ctx->h_phi_pin);
-        ctx->h_phi_pin = nullptr; ctx->cap_phi_pin = 0;
-        CUDA_TRY(cudaHostAlloc((void**)&ctx->h_phi_pin, sizeof(double) * need_phi, cudaHostAllocDefault));
-        ctx->cap_phi_pin = need_phi;
-    }
+    if (!direct && need_phi > ctx->h_phi_pin.size()) CUDA_TRY(ctx->h_phi_pin.alloc(need_phi));
     CUDA_TRY(cudaMemcpyAsync(direct ? phi_host : ctx->h_phi_pin, ctx->d_phi, sizeof(double) * need_phi, cudaMemcpyDeviceToHost,
                              ctx->stream));
     CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
@@ -3051,16 +2953,17 @@ int dks_summarise_host(dks_ctx* ctx, int n, const int32_t* seg_offsets_host, int
     } else {
         REQUIRE(Gp == G, "dks_summarise_host: without segments Gp must equal the number of groups");
     }
-    int* d_seg = nullptr; double* d_sum = nullptr; unsigned long long* d_abs = nullptr; double* d_mean = nullptr; int* d_ord = nullptr;
-    int* d_arg = nullptr;
+    DevBuf<int> d_seg, d_ord, d_arg;
+    DevBuf<double> d_sum, d_mean;
+    DevBuf<unsigned long long> d_abs;
     const size_t cells = (size_t)C * Gp;
-    TRY(dev_alloc(&d_abs, cells)); TRY(dev_alloc(&d_mean, (size_t)(C + 1) * Gp)); TRY(dev_alloc(&d_ord, (size_t)(C + 1) * Gp));
-    TRY(dev_alloc(&d_arg, (size_t)n));
+    CUDA_TRY(d_abs.alloc(cells)); CUDA_TRY(d_mean.alloc((size_t)(C + 1) * Gp)); CUDA_TRY(d_ord.alloc((size_t)(C + 1) * Gp));
+    CUDA_TRY(d_arg.alloc((size_t)n));
     if (seg_offsets_host) {
-        TRY(dev_alloc(&d_seg, (size_t)Gp + 1));
+        CUDA_TRY(d_seg.alloc((size_t)Gp + 1));
         CUDA_TRY(cudaMemcpyAsync(d_seg, seg_offsets_host, sizeof(int) * (Gp + 1), cudaMemcpyHostToDevice, ctx->stream));
     }
-    if (phi_sum_host) TRY(dev_alloc(&d_sum, cells * n));
+    if (phi_sum_host) CUDA_TRY(d_sum.alloc(cells * n));
     CUDA_TRY(cudaMemsetAsync(d_abs, 0, sizeof(unsigned long long) * cells, ctx->stream));
     const long long total = (long long)cells * n;
     int grid = cdiv(total, 256);
@@ -3075,9 +2978,6 @@ int dks_summarise_host(dks_ctx* ctx, int n, const int32_t* seg_offsets_host, int
     if (order_host) CUDA_TRY(cudaMemcpyAsync(order_host, d_ord, sizeof(int) * (C + 1) * Gp, cudaMemcpyDeviceToHost, ctx->stream));
     if (argmax_host) CUDA_TRY(cudaMemcpyAsync(argmax_host, d_arg, sizeof(int) * n, cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    cudaFree(d_abs); cudaFree(d_mean); cudaFree(d_ord); cudaFree(d_arg);
-    if (d_seg) cudaFree(d_seg);
-    if (d_sum) cudaFree(d_sum);
     return DKS_OK;
 }
 
@@ -3124,6 +3024,12 @@ int dks_set_kernel(dks_ctx* ctx, int kernel) {
 int dks_kernel_launches(dks_ctx* ctx, int64_t* count) {
     REQUIRE(ctx && count, "dks_kernel_launches: bad arguments");
     *count = ctx->launches;
+    return DKS_OK;
+}
+
+int dks_live_allocations(int64_t* count) {
+    REQUIRE(count, "dks_live_allocations: NULL");
+    *count = dks::g_live_allocations.load();
     return DKS_OK;
 }
 

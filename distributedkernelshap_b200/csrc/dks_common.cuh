@@ -4,10 +4,102 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "dks.h"
+
+// ---- the memory the library holds for itself (host-only) --------------------------------------------------------------
+// Every device and pinned-host allocation of the library goes through this one pair, which counts what is live across the
+// process's contexts (dks_live_allocations).  The free is the synchronous one: its implicit device synchronisation is what
+// makes freeing a buffer that a kernel in flight still reads safe.
+namespace dks {
+inline std::atomic<int64_t> g_live_allocations{0};
+
+inline cudaError_t mem_alloc(void** p, size_t bytes, bool pinned) {
+    const cudaError_t e = pinned ? cudaHostAlloc(p, bytes, cudaHostAllocDefault) : cudaMalloc(p, bytes);
+    if (e == cudaSuccess) g_live_allocations++;
+    return e;
+}
+
+inline void mem_free(void* p, bool pinned) {
+    if (!p) return;
+    if (pinned) cudaFreeHost(p);
+    else cudaFree(p);
+    g_live_allocations--;
+}
+}  // namespace dks
+
+// an array of device (or pinned host) memory and its element count, freed when it is reset, reallocated or destroyed
+template <typename T, bool PINNED = false>
+class DksBuf {
+public:
+    DksBuf() = default;
+    DksBuf(DksBuf&& o) noexcept : p_(std::exchange(o.p_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+    DksBuf(const DksBuf&) = delete;
+    DksBuf& operator=(const DksBuf&) = delete;
+    ~DksBuf() { reset(); }
+
+    // frees what it holds, then holds `count` elements (at least one)
+    cudaError_t alloc(size_t count) {
+        reset();
+        if (count == 0) count = 1;
+        void* p;
+        const cudaError_t e = dks::mem_alloc(&p, count * sizeof(T), PINNED);
+        if (e == cudaSuccess) { p_ = static_cast<T*>(p); n_ = count; }
+        return e;
+    }
+    void reset() { dks::mem_free(std::exchange(p_, nullptr), PINNED); n_ = 0; }
+    T* release() { n_ = 0; return std::exchange(p_, nullptr); }     // the caller takes the memory over
+    size_t size() const { return n_; }
+    T* get() const { return p_; }
+    operator T*() const { return p_; }
+
+private:
+    T* p_ = nullptr;
+    size_t n_ = 0;
+};
+template <typename T> using DevBuf = DksBuf<T, false>;
+template <typename T> using PinnedBuf = DksBuf<T, true>;
+
+// device arrays whose pointers sit inside by-value kernel structs (TreeDev, PlanDev, ...): allocated through the pool that
+// owns them and freed together by clear() or the pool's destructor
+class DevPool {
+public:
+    DevPool() = default;
+    DevPool(const DevPool&) = delete;
+    ~DevPool() { clear(); }
+
+    template <typename T>
+    cudaError_t alloc(T** p, size_t count) {
+        DevBuf<T> b;
+        const cudaError_t e = b.alloc(count);
+        *p = b;
+        if (e == cudaSuccess) adopt(std::move(b));
+        return e;
+    }
+    // the device copy of a host array, ordered on `stream`
+    template <typename T>
+    cudaError_t upload(const T** dst, const T* src, size_t count, cudaStream_t stream) {
+        T* p;
+        const cudaError_t e = alloc(&p, count);
+        *dst = p;
+        if (e != cudaSuccess || count == 0) return e;
+        return cudaMemcpyAsync(p, src, sizeof(T) * count, cudaMemcpyHostToDevice, stream);
+    }
+    template <typename T>
+    void adopt(DevBuf<T>&& b) { bufs_.push_back(b.release()); }
+    void clear() {
+        for (void* q : bufs_) dks::mem_free(q, false);
+        bufs_.clear();
+    }
+    bool empty() const { return bufs_.empty(); }
+
+private:
+    std::vector<void*> bufs_;
+};
 
 #define DKS_MAX_GROUPS 1024 // coalition rows: one 64-bit word up to 64 groups; two words up to 128 and sixteen up to 1024 on
                             // the shared-plan path only
@@ -251,7 +343,7 @@ struct HeadDesc {
 
 // Tables derived from the plan of the full varying set (M == G) that PlanDev does not hold: the class-sum heads' per-class
 // Dm and row bounds (dks_multi.cuh), the exp head's l(s), the mixture members' tables.  Host-only; the buffers belong to
-// plan_allocs[M].
+// plan_pool[M].
 struct FullSetTables {
     int M;                              // the plan they were built for (0: none)
     const float* dm[DKS_MIX_MAX_R];     // per member ([0]: the head itself): binary Dm, or per-class Dm
@@ -264,7 +356,19 @@ struct FullSetTables {
 __device__ __forceinline__ int dks_inst_count(const ExplainParams& p) { return p.list ? *p.count : p.n; }
 __device__ __forceinline__ int dks_inst_at(const ExplainParams& p, int q) { return p.list ? p.list[q] : q; }
 
+// A context owns its device memory: DevBuf fields, fit_pool (what a dks_fit builds) and plan_pool[M] (the plan of M groups).
+// A raw pointer field never owns: it points into one of those, or an ensemble member's status word into its ensemble's.
 struct dks_ctx {
+    ~dks_ctx() {
+        if (gexec) cudaGraphExecDestroy(gexec);
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : ev_l1) if (e) cudaEventDestroy(e);
+        if (ev_fork) cudaEventDestroy(ev_fork);
+        if (ev_join) cudaEventDestroy(ev_join);
+        if (side_stream) cudaStreamDestroy(side_stream);
+        if (own_stream && stream) cudaStreamDestroy(stream);
+    }
+
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
@@ -279,32 +383,30 @@ struct dks_ctx {
     int kernel_choice = DKS_KERNEL_AUTO;
     int nsamples_req = 0;
     bool uniform_w = true;      // background weights all equal
-    float* dbg_T = nullptr;     // debug dump of the tensor-core score tile of instance dbg_i ([dbg_rows][dbg_cols])
+    DevBuf<float> dbg_T;        // debug dump of the tensor-core score tile of instance dbg_i ([dbg_rows][dbg_cols])
     int dbg_i = -1, dbg_rows = 0, dbg_cols = 0;
-    float* dbg_time = nullptr;  // [6][256] clock64 timeline of CTA 0 (debug kernel variant)
+    DevBuf<float> dbg_time;     // [6][256] clock64 timeline of CTA 0 (debug kernel variant)
 
     // host copies
     MixHead mix = {};           // mixture head (act == DKS_ACT_MIX): members and weights
-    MixHead* d_mix = nullptr;   // its device copy (stage 1 and the fit kernels evaluate f(x) in float64 from it)
-    double* d_mixBW = nullptr;  // [K][N][G][R_m] the background contributions split per member (plan tables of each member)
-    double* d_mixsc = nullptr;  // [K][N][R_m] the background scores split per member
-    float* d_mixscr = nullptr;  // one member's sums before they are added, times pi_k, into the mixture's sums
-    size_t cap_mixscr = 0;
+    DevBuf<MixHead> d_mix;      // its device copy (stage 1 and the fit kernels evaluate f(x) in float64 from it)
+    DevBuf<double> d_mixBW;     // [K][N][G][R_m] the background contributions split per member (plan tables of each member)
+    DevBuf<double> d_mixsc;     // [K][N][R_m] the background scores split per member
+    DevBuf<float> d_mixscr;     // one member's sums before they are added, times pi_k, into the mixture's sums
     // tree ensemble (act == DKS_ACT_TREES): host copies of the node arrays, and their device copies built by dks_fit
     std::vector<int32_t> h_tfeat, h_tleft, h_tright, h_troots;
     std::vector<double> h_tthr, h_tval, h_tbase;
     std::vector<unsigned char> h_tmiss;
     TreeDev tree = {};
-    size_t cap_txinfo = 0;
+    DevBuf<unsigned char> txinfo;   // the explain kernel's node scratch tree.xinfo points at
     // the column encoding of a model with its own kernel (dks_set_column_encoding; empty h_ehdr: none), the device copy
     // dks_fit builds, the encoded background, the encoded group CSR and the encoded rows of the current call
     std::vector<int32_t> h_ehdr, h_eops;
     std::vector<double> h_eopv, h_etab;
     EncodingDev enc = {};
-    double* d_bg_enc = nullptr;  // [N][E]
+    double* d_bg_enc = nullptr;  // [N][E] (fit_pool)
     int32_t *d_egoff = nullptr, *d_egcols = nullptr;   // [G + 1], [E]: group g owns the encoded columns of its raw ones
-    double* d_Xenc = nullptr;    // [n][E]
-    size_t cap_Xenc = 0;
+    DevBuf<double> d_Xenc;       // [n][E]
     // what the family's own kernels of the current call read: the rows (d_Xenc, or the raw rows), their width, the
     // background and the group CSR over those columns
     const double* own_X = nullptr;
@@ -327,103 +429,93 @@ struct dks_ctx {
     std::vector<dks_ctx*> ens;
     std::vector<double> h_ens_pi;
     const double* d_ens_pi = nullptr;
-    double *d_ens_out = nullptr, *d_ens_ey = nullptr;
-    size_t cap_ens_out = 0, cap_ens_ey = 0;
+    DevBuf<double> d_ens_out, d_ens_ey;
     dks_ctx* ens_parent = nullptr;
-    // every device array dks_fit builds for a family with its own kernel (the pointers of tree, km, mlp, knn, enc, d_bg_enc,
-    // d_egoff, d_egcols), freed together by the next dks_fit or dks_destroy.  No kernel reads one after that: freeing
-    // clears fitted and prepared, and every launch needs them.
-    std::vector<void*> own_allocs;
+    // every device array dks_fit builds that a by-value kernel struct points at (the pointers of tree, km, mlp, knn, enc, cm,
+    // d_bg_enc, d_egoff, d_egcols, d_ens_pi), freed together by the next dks_fit or with the context.  No kernel reads one
+    // after that: freeing clears fitted and prepared, and every launch needs them.
+    DevPool fit_pool;
     std::vector<double> h_bg, h_wbg, h_W, h_b;
     std::vector<int32_t> h_cm_hdr;             // column maps (dks_set_column_maps); empty: the scores are W x + b
     std::vector<double> h_cm_keys, h_cm_vals;
     std::vector<int32_t> h_goff, h_gcols;
 
     // device, fit-time
-    double *d_bg = nullptr, *d_wbg = nullptr, *d_W = nullptr, *d_b = nullptr;
-    ColumnMapsDev cm = {};                     // device copy of the column maps (cm.hdr == nullptr: none)
-    int32_t *d_goff = nullptr, *d_gcols = nullptr;
-    double *d_colmin = nullptr, *d_colmax = nullptr;
-    int* d_colnan = nullptr;
-    double *d_BW = nullptr, *d_scores = nullptr, *d_Bbar = nullptr, *d_fnull = nullptr, *d_linkfnull = nullptr;
-    float *d_BWs = nullptr, *d_bases = nullptr, *d_wbf = nullptr;
-    float* d_wn = nullptr;      // [N] N w_j in float: the background weights the weighted shared-plan kernels read
+    DevBuf<double> d_bg, d_wbg, d_W, d_b;
+    ColumnMapsDev cm = {};                     // device copy of the column maps (cm.hdr == nullptr: none; fit_pool)
+    DevBuf<int32_t> d_goff, d_gcols;
+    DevBuf<double> d_colmin, d_colmax;
+    DevBuf<int> d_colnan;
+    DevBuf<double> d_BW, d_scores, d_Bbar, d_fnull, d_linkfnull;
+    DevBuf<float> d_BWs, d_bases, d_wbf;
+    DevBuf<float> d_wn;         // [N] N w_j in float: the background weights the weighted shared-plan kernels read
     HeadDesc head;
     std::vector<double> h_fnull, h_linkfnull;
 
     // plans
     PlanDev h_plans[DKS_MAX_GROUPS + 1];
-    PlanDev* d_plans = nullptr;
-    std::vector<void*> plan_allocs[DKS_MAX_GROUPS + 1];   // device buffers owned by the plan of each M (freed on replace)
+    DevBuf<PlanDev> d_plans;
+    DevPool plan_pool[DKS_MAX_GROUPS + 1];       // device buffers owned by the plan of each M (freed on replace)
     int max_plan_S = 0;
     // l1 feature selection (dks_set_l1 / dks_set_l1_tables): per-M tables on the device, and a device copy of the table
     // set (the general list's LARS reads each task's own M)
     dks::l1::Tables h_l1[DKS_MAX_GROUPS + 1] = {};
-    dks::l1::Tables* d_l1 = nullptr;             // [DKS_L1_MAX_GROUPS + 1]
+    DevBuf<dks::l1::Tables> d_l1;                // [DKS_L1_MAX_GROUPS + 1]
     int l1_mode = 0, l1_k = 0;
     uint64_t l1_sel[2] = {0, 0};                 // bit M - 1: instances with M varying groups select
-    int* d_idx_sel = nullptr;                    // [n] general-list instances whose M selects ...
-    int* d_idx_plain = nullptr;                  // [n] ... and the rest
-    int* d_l1_counts = nullptr;                  // [2] their counts
+    DevBuf<int> d_idx_sel;                       // [n] general-list instances whose M selects ...
+    DevBuf<int> d_idx_plain;                     // [n] ... and the rest
+    DevBuf<int> d_l1_counts;                     // [2] their counts
     cudaEvent_t ev_l1[3] = {nullptr, nullptr, nullptr};   // around the general list's moments kernel and LARS
     bool l1_timing_valid = false;
     FullSetTables full = {};     // tables of the plan of the full varying set, cleared with that plan
-    double* d_mom = nullptr;     // [n][outputs solved][2G + 4] per-instance moments of y
-    size_t cap_mom = 0;
-    double* d_yw = nullptr;      // [n][S_pad] link-space y of the wide (more than 128 groups) solve
-    double* d_betaw = nullptr;   // [n][kpw] its coefficients before the delta term
-    size_t cap_yw = 0, cap_betaw = 0;
-    float* d_acache = nullptr;   // [n][S_pad] A(i, s) of sixteen-word rows, shared by the launches of the background chunks
-    size_t cap_acache = 0;
+    DevBuf<double> d_mom;        // [n][outputs solved][2G + 4] per-instance moments of y
+    DevBuf<double> d_yw;         // [n][S_pad] link-space y of the wide (more than 128 groups) solve
+    DevBuf<double> d_betaw;      // [n][kpw] its coefficients before the delta term
+    DevBuf<float> d_acache;      // [n][S_pad] A(i, s) of sixteen-word rows, shared by the launches of the background chunks
     // per-instance plans drawn on the device (plan_mode 1)
     int plan_mode = 0;
     uint64_t sampler_seed = 0;
     long long row_offset = 0;
     DksSamplingInfo h_sinfo[DKS_MAX_GROUPS + 1];
-    DksSamplingInfo* d_sinfo = nullptr;
-    uint64_t* d_genz = nullptr;  // [n][stride][gen_words]
-    double* d_genw = nullptr;
-    double* d_genchol = nullptr;
-    double* d_genainv = nullptr;
-    size_t cap_gen = 0, cap_genf = 0;
+    DevBuf<DksSamplingInfo> d_sinfo;
+    DevBuf<uint64_t> d_genz;     // [n][stride][gen_words]
+    DevBuf<double> d_genw;       // [n][stride]
+    DevBuf<double> d_genchol;
+    DevBuf<double> d_genainv;
     int gen_words = 1;           // words per row d_genz is laid out for
     int gen_plan_words = 1;      // words per row of the last call's plans (dks_get_instance_plans_w)
     const double* h_afix[DKS_MAX_GROUPS + 1] = {};   // per M: normal matrix of the enumerated prefix (device pointers)
-    const double** d_afix = nullptr;
+    DevBuf<const double*> d_afix;
     int gen_stride = 0, gen_n = 0;
 
     // per-call workspace
-    int cap_n = 0, cur_n = 0;
+    int ws_n = 0, cur_n = 0;     // instances the workspace is laid out for (0: lay it out at the next call), and this call's
     bool prepared = false;
-    double* d_X = nullptr;       // staging for host inputs
-    size_t cap_X = 0;
+    DevBuf<double> d_X;          // staging for host inputs
     const double* cur_X = nullptr;
-    double* d_XW = nullptr;
-    double* d_XT = nullptr;      // [n][R][ceil(G/4)][16] nibble tables of the scaled grouped contributions (binary head:
+    DevBuf<double> d_XW;
+    DevBuf<double> d_XT;         // [n][R][ceil(G/4)][16] nibble tables of the scaled grouped contributions (binary head:
                                  // R = 1; softmax: log2 e XW; identity head: XW - Bbar)
-    float* d_msums = nullptr;    // [n][C][S_pad] per-class sums of the softmax coalition kernel
-    size_t cap_msums = 0;
-    unsigned char* d_vflag = nullptr;
-    uint64_t* d_vmask = nullptr;
-    int* d_M = nullptr;
-    double* d_dlink = nullptr;
-    int* d_hist = nullptr;       // status[2], list counts[2], then the histogram of M [G + 1] (one allocation, one memset)
-    int* d_status = nullptr;
+    DevBuf<float> d_msums;       // [n][C][S_pad] per-class sums of the softmax coalition kernel
+    DevBuf<unsigned char> d_vflag;
+    DevBuf<uint64_t> d_vmask;
+    DevBuf<int> d_M;
+    DevBuf<double> d_dlink;
+    DevBuf<int> status;          // status[2], list counts[2], then the histogram of M [G + 1] (one allocation, one memset)
+    int* d_status = nullptr;     // status, or an ensemble member's view of its ensemble's
     int* d_counts = nullptr;     // [0] instances on the shared fast path, [1] the others
-    int* d_idx_full = nullptr;   // [n] instances whose varying set is all G groups
-    int* d_idx_other = nullptr;  // [n] the rest
-    float2* d_sums = nullptr;    // [n][S_pad] (sum p1, sum p0) of the shared fast path
-    size_t cap_sums = 0;
-    long long* d_acc = nullptr;  // [n][24] fixed-point partial beta of the fused kernel (zero between launches)
-    int* d_done = nullptr;       // [n] row groups delivered per instance (zero between launches)
-    double* d_phi = nullptr;
-    size_t cap_phi = 0;
+    int* d_hist = nullptr;
+    DevBuf<int> d_idx_full;      // [n] instances whose varying set is all G groups
+    DevBuf<int> d_idx_other;     // [n] the rest
+    DevBuf<float2> d_sums;       // [n][S_pad] (sum p1, sum p0) of the shared fast path
+    DevBuf<long long> d_acc;     // [n][24] fixed-point partial beta of the fused kernel (zero between launches)
+    DevBuf<int> d_done;          // [n] row groups delivered per instance (zero between launches)
+    DevBuf<double> d_phi;
     int phi_rows = 0;             // rows of the last dks_explain_host result held in d_phi
-    double* h_phi_pin = nullptr;  // pinned staging for results going to pageable host memory
-    size_t cap_phi_pin = 0;
-    uint64_t* d_extz = nullptr;
-    double* d_extw = nullptr;
-    size_t cap_ext = 0;
+    PinnedBuf<double> h_phi_pin;  // pinned staging for results going to pageable host memory
+    DevBuf<uint64_t> d_extz;
+    DevBuf<double> d_extw;
     int h_status[2] = {0, 0};
 
     // CUDA graph of the device-resident explain sequence (dks_run_dev): captured on the second identical call
@@ -452,15 +544,15 @@ struct dks_ctx {
     double* peer_base[16] = {};                    // device pointers to each rank's [world][slab] buffer
     unsigned long long* peer_flags[16] = {};       // rank r's flag array [world] (peer-mapped); [peer_rank] is this rank's own
     bool peer_flags_set = false;
-    double** d_peer_list = nullptr;                // device copy of the peers' slab addresses for the current phi buffer
+    DevBuf<double*> d_peer_list;                   // device copy of the peers' slab addresses for the current phi buffer
     double* peer_list_for = nullptr;               // the phi buffer d_peer_list was built for
-    unsigned long long* d_step = nullptr;          // device-side step counter of the flag exchange
+    DevBuf<unsigned long long> d_step;             // device-side step counter of the flag exchange
     bool push_in_kernel = false;                   // 1: the fused kernel's epilogue stores phi into the peers' buffers itself
                                                    // (measured slower than the separate coalesced push kernel: DESIGN.md §7)
     // tuning knobs (dks_set_option; defaults from the environment at dks_create: DKS_FUSED, DKS_FUSED_WARPS, ...)
     int opt_fused = 1, opt_fused_warps = 0, opt_fused_B = 0;
     int opt_fused_table = 1;                       // 0: the fused kernel ignores the plans' link tables (exact loop only)
-    unsigned long long* d_ltab_fb = nullptr;       // fused passes that fell back from the link table to the exact loop
+    DevBuf<unsigned long long> d_ltab_fb;          // fused passes that fell back from the link table to the exact loop
     bool opt_graph_timing = false;   // keep the timing event records inside a captured graph (dks_last_timings after replays)
     bool timing_valid = false, last_was_graph = false;
     bool last_fused = false;                       // the last explain ran the fused shared-plan kernel

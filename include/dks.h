@@ -435,6 +435,9 @@ int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
  * carries no timing nodes and dks_last_timings reports an error after it). */
 int dks_set_option(dks_ctx* ctx, const char* name, int value);
 int dks_kernel_launches(dks_ctx* ctx, int64_t* count); /* kernels launched by this ctx so far */
+/* device and pinned-host allocations the library holds for itself now, across every context of the process (memory from
+ * dks_host_alloc belongs to the caller and is not counted): a context that is destroyed gives back all it took */
+int dks_live_allocations(int64_t* count);
 /* The fused kernel's link table of the plan over M groups: its bytes (0 = the plan has none and the kernel runs the exact
  * loop), and the passes of this ctx's fused launches so far that left a table's domain and took the exact loop. */
 int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fallback_passes);

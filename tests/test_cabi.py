@@ -62,3 +62,33 @@ def test_product_does_not_import_the_oracle():
                 src = open(os.path.join(root, f)).read()
                 assert not re.search(r"^\s*(from|import)\s+oracle\b", src, flags=re.M), f"{f} imports the oracle"
                 assert "shap_kernel_oracle" not in src, f"{f} references the oracle module"
+
+
+def _body_span(src, head):
+    """(start, end) offsets of the first definition in src whose head (up to its opening brace) matches `head`."""
+    m = re.search(head + r"\s*\{", src)
+    assert m, f"{head} is not defined"
+    depth, at = 0, m.end() - 1
+    while True:
+        depth += {"{": 1, "}": -1}.get(src[at], 0)
+        if depth == 0:
+            return m.start(), at
+        at += 1
+
+
+def test_only_the_buffer_owner_allocates():
+    # every device and pinned-host allocation of the library goes through one allocate / free pair, which counts them
+    # (dks_live_allocations); dks_host_alloc / dks_host_free hand page-locked memory to the caller
+    csrc = os.path.join(REPO, "distributedkernelshap_b200", "csrc")
+    allowed = {"dks_common.cuh": ("mem_alloc", "mem_free"), "dks.cu": ("dks_host_alloc", "dks_host_free")}
+    calls = re.compile(r"\bcuda(Malloc\w*|Free\w*|HostAlloc|HostRegister)\b")
+    for f in sorted(os.listdir(csrc)):
+        src = open(os.path.join(csrc, f)).read()
+        src = re.sub(r"//[^\n]*", "", re.sub(r"/\*.*?\*/", "", src, flags=re.S))
+        spans = [_body_span(src, r"\b" + name + r"\([^;{]*\)") for name in allowed.get(f, ())]
+        for m in calls.finditer(src):
+            line = src.count("\n", 0, m.start()) + 1
+            assert any(a <= m.start() < b for a, b in spans), f"{f}:{line}: {m.group(0)} outside the buffer owner"
+    common = open(os.path.join(csrc, "dks_common.cuh")).read()
+    start, end = _body_span(common, r"\bstruct dks_ctx")
+    assert not re.search(r"\bcap_\w+", common[start:end]), "dks_ctx keeps a capacity beside a buffer"
