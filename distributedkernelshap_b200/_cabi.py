@@ -56,6 +56,7 @@ SIGNATURES = {
     "dks_set_mixture": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "dks_set_tree_model": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                                                                 C.c_int, C.c_int, C.c_int]),
+    "dks_set_tree_offset": (C.c_int, [C.c_void_p, C.c_double]),
     "dks_set_kernel_machine": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 4 +
                                [C.c_int, C.c_double, C.c_double, C.c_int] + [C.c_void_p] * 3 + [C.c_int]),
     "dks_set_mlp": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),

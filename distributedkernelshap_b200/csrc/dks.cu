@@ -1671,6 +1671,9 @@ int fit_model(dks_ctx* ctx) {
     if (h.expo && ctx->link == DKS_LINK_LOGIT)
         return fail(DKS_ERR_UNSUPPORTED, "exp head: the logit link is undefined wherever a predicted mean exceeds 1; use the "
                     "identity link");
+    if (h.family == DKS_GENERAL_TREES && ctx->tree.head == DKS_TREE_HEAD_IFOREST && ctx->link == DKS_LINK_LOGIT)
+        return fail(DKS_ERR_UNSUPPORTED, "anomaly head: an IsolationForest score is not a probability and has no logit; use "
+                    "the identity link");
     {   // every column in exactly one group
         std::vector<int> seen(D, 0);
         REQUIRE((int)ctx->h_gcols.size() == D, "groups cover %d columns but the data has %d", (int)ctx->h_gcols.size(), D);
@@ -1957,6 +1960,7 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
     case DKS_TREE_HEAD_SIGMOID: REQUIRE(R == 1, "sigmoid tree head needs R == 1 (got %d)", R); C = 2; break;
     case DKS_TREE_HEAD_SOFTMAX: REQUIRE(R >= 2, "softmax tree head needs R >= 2 (got %d)", R); C = R; break;
     case DKS_TREE_HEAD_EXP: REQUIRE(R == 1, "exp tree head needs R == 1 (got %d)", R); C = 1; break;
+    case DKS_TREE_HEAD_IFOREST: REQUIRE(R == 1, "anomaly tree head needs R == 1 (got %d)", R); C = 1; break;
     default: return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_model: unknown head %d", head);
     }
     const int width = model_columns(ctx);
@@ -1986,7 +1990,18 @@ int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const 
     ctx->h_troots.assign(roots, roots + n_trees);
     ctx->h_tbase.assign(base, base + R);
     ctx->tree.nodes = n_nodes; ctx->tree.T = n_trees; ctx->tree.R = R; ctx->tree.head = head; ctx->tree.cmp = cmp;
+    ctx->tree.offset = 0.0;
     return set_own_model(ctx, DKS_ACT_TREES, C, scalar_out);
+}
+
+int dks_set_tree_offset(dks_ctx* ctx, double offset) {
+    BIND(ctx);
+    REQUIRE(ctx->act == DKS_ACT_TREES && ctx->tree.head == DKS_TREE_HEAD_IFOREST,
+            "dks_set_tree_offset: needs a tree ensemble with the anomaly head (dks_set_tree_model, DKS_TREE_HEAD_IFOREST)");
+    if (!std::isfinite(offset)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_tree_offset: the offset must be finite");
+    ctx->tree.offset = offset;
+    ctx->fitted = false;
+    return DKS_OK;
 }
 
 int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const double* sv, const double* dual, int R,

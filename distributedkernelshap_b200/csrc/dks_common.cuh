@@ -250,6 +250,7 @@ struct TreeDev {
     const unsigned char* bgdir;  // [N][nodes] 1: background row j goes left at the node (internal nodes)
     unsigned char* xinfo;        // [CTAs][nodes] explain kernel scratch: (x goes left) << 7 | varying position (127: none)
     int nodes, T, R, head, cmp;
+    double offset;               // subtracted by the anomaly head (DKS_TREE_HEAD_IFOREST), dks_set_tree_offset
 };
 
 // column encoding of a model with its own kernel (dks_set_column_encoding, DESIGN.md §5.0.13, §5.0.16): E encoded columns,

@@ -1,5 +1,5 @@
-// Tree ensembles on the device (DESIGN.md §5.0.11): scikit-learn decision trees, random / extra-trees forests and gradient
-// boosting, read into flat node arrays (TreeDev, dks_set_tree_model).  KernelSHAP on a tree needs the real masked forward
+// Tree ensembles on the device (DESIGN.md §5.0.11, §5.0.18): scikit-learn decision trees, random / extra-trees forests,
+// gradient boosting, SAMME AdaBoost and isolation forests, read into flat node arrays (TreeDev, dks_set_tree_model).  KernelSHAP on a tree needs the real masked forward
 // pass of every (coalition s, background row j): x's value for the groups of s that vary, bg_j's for the rest.  A tree walk
 // is a few dependent loads and a compare per level, so this route evaluates all S N of them per instance, in float64.
 //
@@ -23,8 +23,8 @@ __device__ __forceinline__ bool goes_left(double x, double thr, unsigned char mi
     return v <= thr;
 }
 
-// outputs of the head on the raw scores r[R], float64 (C = 2 for the sigmoid head, else R)
-__device__ __forceinline__ void tree_head(const double* r, int R, int head, double* o) {
+// outputs of the head on the raw scores r[R], float64 (C = 2 for the sigmoid head, else R); offset: the anomaly head's
+__device__ __forceinline__ void tree_head(const double* r, int R, int head, double offset, double* o) {
     if (head == DKS_TREE_HEAD_SIGMOID) {
         // [1 - expit(r), expit(r)] with neither half formed by cancellation
         const double e = exp(-fabs(r[0]));
@@ -39,6 +39,9 @@ __device__ __forceinline__ void tree_head(const double* r, int R, int head, doub
         for (int q = 0; q < R; ++q) o[q] /= sum;
     } else if (head == DKS_TREE_HEAD_EXP) {
         o[0] = exp(r[0]);
+    } else if (head == DKS_TREE_HEAD_IFOREST) {
+        // IsolationForest: r = -(sum of the path lengths) / (T c(max_samples)), the score is -2^r
+        o[0] = -exp2(r[0]) - offset;
     } else {
         for (int q = 0; q < R; ++q) o[q] = r[q];
     }
@@ -64,7 +67,7 @@ __global__ void tree_predict_kernel(const double* __restrict__ X, int n, int D, 
     if (i >= n) return;
     double r[DKS_TREE_MAX_R], o[DKS_TREE_MAX_R];
     tree_raw(t, X + (size_t)i * D, r);
-    tree_head(r, t.R, t.head, o);
+    tree_head(r, t.R, t.head, t.offset, o);
     predict_epilogue(o, C, i, link, linkfnull, out, dlink, status, false);
 }
 
@@ -207,7 +210,7 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
                     }
                     for (int u = 0; u < R; ++u) r[u] += t.val[(size_t)nd * R + u];
                 }
-                tree_head(r, R, t.head, o);
+                tree_head(r, R, t.head, t.offset, o);
                 for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + s]);
             }
             __syncthreads();

@@ -140,7 +140,8 @@ class GpuKernelExplainer:
     model
         What the reference passes as ``predictor``: a bound ``predict_proba`` / ``decision_function`` of a linear
         model or of a ``Pipeline`` of per-column preprocessing ending in one (explained in raw feature space), or a
-        ``LinearModelSpec`` (see ``predictors.extract_linear_spec``); a tree model, bare or behind such a ``Pipeline``
+        ``LinearModelSpec`` (see ``predictors.extract_linear_spec``); a tree model (``trees.extract_tree_spec``:
+        ``IsolationForest`` and ``AdaBoostClassifier`` included), bare or behind such a ``Pipeline``
         (``trees.extract_tree_pipeline_spec``: the device replays the steps bit for bit); a kernel machine; a
         scikit-learn MLP (``mlp.extract_mlp_spec``); a k-nearest-neighbour model (``neighbors.extract_knn_spec``); each of
         the last three bare, behind affine scalers (folded into the model) or behind such a ``Pipeline``
@@ -197,6 +198,9 @@ class GpuKernelExplainer:
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
                                       "link log(ey / (1 - ey)) is undefined wherever a predicted mean exceeds 1")
+        if getattr(self.spec, "head", None) == "iforest" and str(self.link) == "logit":
+            raise NotImplementedError("the anomaly head (IsolationForest) supports link='identity' only: its scores are "
+                                      "negative and not probabilities, so they have no logit")
         self.data = convert_to_data(data)
         if self.data.transposed:
             raise NotImplementedError("transposed DenseData (group sizes matching axis 0) is not supported")
@@ -297,6 +301,8 @@ class GpuKernelExplainer:
                 ctx, t.n_nodes, _cabi.ptr(t.feature), _cabi.ptr(t.threshold), _cabi.ptr(t.left), _cabi.ptr(t.right),
                 _cabi.ptr(t.missing_left), _cabi.ptr(t.value), t.R, t.n_trees, _cabi.ptr(t.roots), _cabi.ptr(t.base),
                 t.head_code, t.cmp, int(t.scalar_out)))
+            if t.head == "iforest":
+                _cabi.check(self.lib.dks_set_tree_offset(ctx, t.offset))
 
     def _set_ensemble(self, spec, bg, weights):
         """One context per member (its background and column encoding give the setter the model's width), handed to

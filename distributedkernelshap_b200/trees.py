@@ -11,6 +11,15 @@ A spec is what ``dks_set_tree_model`` takes (include/dks.h): every tree's nodes 
   the regressor: identity.
 * ``HistGradientBoosting*``: as gradient boosting, ``base`` the baseline prediction; the regressor's ``predict`` is
   ``exp(r)`` under a log-link loss (``'poisson'``, ``'gamma'``).
+* ``AdaBoostClassifier`` (SAMME) over ``sklearn.tree`` classifiers: tree t votes ``w_t`` for the class its leaf predicts
+  (``argmax tree_.value``, the first class on a tie) and ``-w_t / (K - 1)`` for every other class; ``1 / sum w`` is folded
+  into the leaves.  ``decision_function``: identity head, for two classes one score ``dec[1] - dec[0]``;
+  ``predict_proba``: ``[1 - expit(r), expit(r)]`` on that score for two classes, a softmax of ``dec / (K - 1)`` (folded
+  into the leaves) otherwise.
+* ``IsolationForest``: tree t's leaf holds ``h = depth + c(n_node_samples) - 1`` (``compute_node_depths``, the root at 1;
+  ``c`` the average path length of an unsuccessful search), times ``-1 / d`` with ``d = T c(max_samples)``, so that
+  ``score_samples = -2^r`` (every score ``-0.5`` when ``d = 0``) and ``decision_function = -2^r - offset_``: the
+  ``"iforest"`` head.  A tree fitted on a feature subset has its split features mapped back to the original columns.
 
 A split sends x left when ``x <= threshold``: ``sklearn.tree`` compares the value cast to float32 (``DTYPE``), the
 histogram-based estimators compare float64 values.  NaN goes where the node's ``missing_go_to_left`` says.
@@ -20,14 +29,18 @@ import numpy as np
 
 MAX_OUTPUTS = 8
 MAX_GROUPS = 64
-HEADS = ("identity", "sigmoid", "softmax", "exp")     # DKS_TREE_HEAD_* codes 0..3
+HEADS = ("identity", "sigmoid", "softmax", "exp", "iforest")     # DKS_TREE_HEAD_* codes 0..4
 CMP_F32, CMP_F64 = 0, 1                               # DKS_TREE_CMP_*
 
 _SKTREE_FORESTS = {"DecisionTreeClassifier", "DecisionTreeRegressor", "ExtraTreeClassifier", "ExtraTreeRegressor",
                    "RandomForestClassifier", "RandomForestRegressor", "ExtraTreesClassifier", "ExtraTreesRegressor"}
 _GB = {"GradientBoostingClassifier", "GradientBoostingRegressor"}
 _HGB = {"HistGradientBoostingClassifier", "HistGradientBoostingRegressor"}
-_TREE_MODELS = _SKTREE_FORESTS | _GB | _HGB
+_ADABOOST = {"AdaBoostClassifier"}
+_IFOREST = {"IsolationForest"}
+_TREE_MODELS = _SKTREE_FORESTS | _GB | _HGB | _ADABOOST | _IFOREST
+# the base estimators an AdaBoostClassifier is read with
+_SKTREE_CLASSIFIERS = {"DecisionTreeClassifier", "ExtraTreeClassifier"}
 # estimators that hold other estimators: a tree model inside one of them is refused by name
 _CONTAINERS = {"Pipeline", "VotingClassifier", "VotingRegressor", "BaggingClassifier", "BaggingRegressor",
                "CalibratedClassifierCV", "StackingClassifier", "StackingRegressor", "OneVsRestClassifier",
@@ -39,14 +52,14 @@ class TreeEnsembleSpec:
 
     feature [nodes] int32 (-1 at a leaf), threshold [nodes] float64, left / right [nodes] int32 (global node indices; -1 at
     a leaf), missing_left [nodes] uint8, value [nodes, R] float64 (leaf outputs, scaled), roots [T] int32, base [R],
-    head in ``HEADS``, cmp ``CMP_F32`` / ``CMP_F64``."""
+    head in ``HEADS``, cmp ``CMP_F32`` / ``CMP_F64``; offset: what the ``"iforest"`` head subtracts."""
 
     activation = "trees"
     act_code = 6          # DKS_ACT_TREES
     maps = None
 
     def __init__(self, feature, threshold, left, right, missing_left, value, roots, base, head, cmp, n_features,
-                 scalar_out=False, n_outputs=None):
+                 scalar_out=False, n_outputs=None, offset=0.0):
         self.feature = np.ascontiguousarray(feature, dtype=np.int32)
         self.threshold = np.ascontiguousarray(threshold, dtype=np.float64)
         self.left = np.ascontiguousarray(left, dtype=np.int32)
@@ -59,6 +72,7 @@ class TreeEnsembleSpec:
         self.cmp = int(cmp)
         self.n_features = int(n_features)
         self.scalar_out = bool(scalar_out)
+        self.offset = float(offset)
         self.R = self.value.shape[1]
         self.n_outputs = int(n_outputs if n_outputs is not None else (2 if head == "sigmoid" else self.R))
         if head not in HEADS:
@@ -110,6 +124,8 @@ class TreeEnsembleSpec:
             out = e / e.sum(axis=1, keepdims=True)
         elif self.head == "exp":
             out = np.exp(r)
+        elif self.head == "iforest":
+            out = -np.exp2(r) - self.offset
         else:
             out = r
         return out[:, 0] if self.scalar_out else out
@@ -273,11 +289,84 @@ def _hgb_spec(owner, method, names):
     return _boosted_head(owner, method, arrs, base, K, CMP_F64, P, link_exp=link_exp)
 
 
+def _average_path_length(n):
+    """c(n) of ``sklearn.ensemble._iforest``: 0 for n <= 1, 1 for n = 2, else 2 (ln(n - 1) + gamma) - 2 (n - 1) / n."""
+    n = np.asarray(n, dtype=np.float64)
+    out = np.zeros(n.shape)
+    big = n > 2
+    out[n == 2] = 1.0
+    out[big] = 2.0 * (np.log(n[big] - 1.0) + np.euler_gamma) - 2.0 * (n[big] - 1.0) / n[big]
+    return out
+
+
+def _iforest_spec(owner, method, names):
+    if method not in ("score_samples", "decision_function"):
+        raise TypeError(f"IsolationForest.{method} is not supported: pass decision_function or score_samples "
+                        "(predict returns labels)")
+    P = int(owner.n_features_in_)
+    ests = list(owner.estimators_)
+    d = len(ests) * float(_average_path_length([owner.max_samples_])[0])
+    trees = []
+    for e, feats in zip(ests, owner.estimators_features_):
+        t = e.tree_
+        h = t.compute_node_depths() + _average_path_length(t.n_node_samples) - 1.0
+        feature, thr, left, right, miss, _ = _sk_tree(e, None)
+        if len(feats) != P:                     # a feature subset: scikit-learn reads X[:, feats]
+            feature = np.where(feature < 0, -1, np.asarray(feats)[np.maximum(feature, 0)])
+        # d = 0 (max_samples = 1): scikit-learn takes the ratio as 1, so r = base = -1 and every score is -2^-1
+        trees.append((feature, thr, left, right, miss, (-h / d if d != 0 else np.zeros_like(h))[:, None]))
+    arrs = _flatten(trees, P)
+    offset = float(owner.offset_) if method == "decision_function" else 0.0
+    return TreeEnsembleSpec(*arrs[:6], arrs[6], np.array([0.0 if d != 0 else -1.0]), "iforest", CMP_F32, P,
+                            scalar_out=True, offset=offset)
+
+
+def _adaboost_spec(owner, method, names):
+    name = type(owner).__name__
+    if method not in ("predict_proba", "decision_function"):
+        raise TypeError(f"{name}.{method} is not supported: pass predict_proba or decision_function (predict returns "
+                        "labels)")
+    P = int(owner.n_features_in_)
+    classes = np.asarray(owner.classes_)
+    K = len(classes)
+    if K < 2:
+        raise NotImplementedError(f"{name} with one class: its outputs are constant, there is nothing to explain")
+    if K > MAX_OUTPUTS:
+        raise NotImplementedError(f"{K} classes: the tree route covers at most {MAX_OUTPUTS} outputs")
+    ests = list(owner.estimators_)
+    for e in ests:
+        if not (_names(e) & _SKTREE_CLASSIFIERS):
+            raise NotImplementedError(f"{name} over {type(e).__name__}: only sklearn.tree classifiers "
+                                      "(DecisionTreeClassifier, ExtraTreeClassifier) are supported as base estimators")
+        if getattr(e, "n_outputs_", 1) != 1:
+            raise NotImplementedError(f"{name} over multi-output trees is not supported")
+    w = np.asarray(owner.estimator_weights_, dtype=np.float64)
+    wsum = float(w.sum())
+    # SAMME: K = 2 folds dec[1] - dec[0] into one score (+-2 w_t); more classes: K scores, over K - 1 for predict_proba
+    scale = 1.0 / wsum if K == 2 or method == "decision_function" else 1.0 / (wsum * (K - 1))
+    trees = []
+    for e, wt in zip(ests, w):              # an early stop leaves fewer estimators than weights; the rest are 0
+        pred = np.searchsorted(classes, e.classes_)[np.argmax(e.tree_.value[:, 0, :], axis=1)]    # ensemble indices
+        if K == 2:
+            v = np.where(pred == 1, 2.0 * wt, -2.0 * wt)[:, None] * scale
+        else:
+            v = np.full((e.tree_.node_count, K), -wt / (K - 1))
+            v[np.arange(len(pred)), pred] = wt
+            v *= scale
+        trees.append(_sk_tree(e, v))
+    arrs = _flatten(trees, P)
+    R = 1 if K == 2 else K
+    if method == "predict_proba":
+        return TreeEnsembleSpec(*arrs[:6], arrs[6], np.zeros(R), "sigmoid" if K == 2 else "softmax", CMP_F32, P)
+    return TreeEnsembleSpec(*arrs[:6], arrs[6], np.zeros(R), "identity", CMP_F32, P, scalar_out=K == 2)
+
+
 def extract_tree_spec(predictor):
     """``TreeEnsembleSpec`` of a bound method of a fitted scikit-learn tree model, ``None`` for anything else (the engine
     then reads a linear model).  A spec passes through.  Raises ``NotImplementedError`` / ``TypeError`` naming the reason
     for tree models the route does not cover: categorical splits, custom boosting init estimators, multi-output
-    regressors, more than 8 outputs, trees inside a Pipeline or an ensemble, and unsupported methods."""
+    regressors, more than 8 outputs, trees inside a Pipeline or an ensemble, ``AdaBoostRegressor``, AdaBoost over base
+    estimators that are not ``sklearn.tree`` classifiers or with one class, and unsupported methods."""
     if isinstance(predictor, TreeEnsembleSpec):
         return predictor
     owner = getattr(predictor, "__self__", None)
@@ -285,9 +374,16 @@ def extract_tree_spec(predictor):
     if owner is None:
         return None
     names = _names(owner)
+    if "AdaBoostRegressor" in names:
+        raise NotImplementedError("AdaBoostRegressor: its prediction is the weighted median of its trees' predictions, "
+                                  "not a sum of leaf values, so the tree route cannot read it")
     if names & _TREE_MODELS:
         if not hasattr(owner, "n_features_in_"):
             raise TypeError(f"{type(owner).__name__} is not fitted")
+        if names & _IFOREST:
+            return _iforest_spec(owner, method, names)
+        if names & _ADABOOST:
+            return _adaboost_spec(owner, method, names)
         if names & _HGB:
             return _hgb_spec(owner, method, names)
         if names & _GB:

@@ -73,6 +73,9 @@ extern "C" {
 #define DKS_TREE_HEAD_SIGMOID 1  /* R = 1, outputs [1 - expit(r), expit(r)]: binary gradient boosting predict_proba */
 #define DKS_TREE_HEAD_SOFTMAX 2  /* R = K >= 2 raw scores, outputs softmax(r): multi-class gradient boosting */
 #define DKS_TREE_HEAD_EXP 3      /* R = 1, output exp(r): histogram gradient boosting with a log-link loss; link identity only */
+#define DKS_TREE_HEAD_IFOREST 4  /* R = 1, output -2^r - offset (dks_set_tree_offset): IsolationForest score_samples /
+                                  * decision_function with -1 / (n_trees c(max_samples)) folded into the leaves; link
+                                  * identity only */
 /* split comparison: x goes left when x <= threshold */
 #define DKS_TREE_CMP_F32 0       /* (double)(float)x <= threshold: scikit-learn's sklearn.tree casts X to float32 */
 #define DKS_TREE_CMP_F64 1       /* x <= threshold in float64: the histogram gradient boosting estimators */
@@ -188,6 +191,11 @@ int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* 
  * r = base + sum over trees of the value of the leaf x reaches; outputs = head(r) per DKS_TREE_HEAD_*, compared per
  * DKS_TREE_CMP_*.  R <= 8 and at most 8 outputs.  Malformed arrays (a child not after its parent, a feature out of range, a
  * NaN threshold, a non-finite leaf value) are DKS_ERR_UNSUPPORTED.
+ * The models read this way (DESIGN.md §5.0.11, §5.0.18): decision trees, random / extra-trees forests (identity head over
+ * the mean class fractions or values), gradient boosting and histogram gradient boosting (identity, sigmoid, softmax or exp
+ * head on the raw scores), SAMME AdaBoostClassifier over sklearn.tree classifiers (each leaf holds its tree's weighted class
+ * vote, 1 / sum of the weights and, for predict_proba, 1 / (K - 1) folded in: identity, sigmoid or softmax head) and
+ * IsolationForest (each leaf holds -(depth + c(n_node_samples) - 1) / (n_trees c(max_samples)): the anomaly head).
  * Every instance runs the tree kernels (DKS_GENERAL_TREES, DESIGN.md §5.0.11), up to 64 groups: shared plans (full and partial
  * varying sets), per-instance device plans and caller-supplied plans, kernel 'auto' or 'simt' (tcgen05 / shared are
  * DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route.  Float64 throughout; a link(ey) or link(f(x)) that
@@ -197,6 +205,10 @@ int dks_set_mixture(dks_ctx* ctx, int K, int member_act, int R_m, const double* 
 int dks_set_tree_model(dks_ctx* ctx, int n_nodes, const int32_t* feature, const double* threshold, const int32_t* left,
                        const int32_t* right, const uint8_t* missing_left, const double* value, int R, int n_trees,
                        const int32_t* roots, const double* base, int head, int cmp, int scalar_out);
+/* the offset the anomaly head (DKS_TREE_HEAD_IFOREST) subtracts: IsolationForest.offset_ for decision_function, 0 for
+ * score_samples.  Call after dks_set_tree_model, which sets it to 0, and before dks_fit.  A context whose model is not a tree
+ * ensemble with the anomaly head is DKS_ERR_INVALID; a non-finite offset is DKS_ERR_UNSUPPORTED. */
+int dks_set_tree_offset(dks_ctx* ctx, double offset);
 /* kernel machine (DKS_ACT_KMACH) in place of dks_set_model: K members, member k owning support vectors sv_off[k] ..
  * sv_off[k + 1] (sv_off [K + 1], non-decreasing from 0, n_sv = sv_off[K] >= 1).  sv [n_sv][D] row-major in raw feature space,
  * dual [n_sv][R], intercept [K][R]; per member colw [K][D] (> 0 at every column), colo [K][D] and gamma [K] (>= 0);
