@@ -111,9 +111,8 @@ int ensure_workspace(dks_ctx* ctx, int n) {
     CUDA_TRY(ctx->d_idx_sel.alloc((size_t)n));
     CUDA_TRY(ctx->d_idx_plain.alloc((size_t)n));
     CUDA_TRY(ctx->d_acc.alloc((size_t)n * 16));
-    CUDA_TRY(ctx->d_done.alloc((size_t)n));
-    CUDA_TRY(cudaMemsetAsync(ctx->d_acc, 0, sizeof(long long) * (size_t)n * 16, ctx->stream));   // the fused kernel leaves
-    CUDA_TRY(cudaMemsetAsync(ctx->d_done, 0, sizeof(int) * (size_t)n, ctx->stream));             // both zeroed behind it
+    CUDA_TRY(cudaMemsetAsync(ctx->d_acc, 0, sizeof(long long) * (size_t)n * 16, ctx->stream));   // the fused route's finish
+                                                                                                  // kernel leaves it zeroed
     ctx->ws_n = n;
     ctx->epoch++;            // buffers moved: a captured graph holds the old addresses
     return DKS_OK;
@@ -1181,30 +1180,27 @@ int launch_shared_binary(dks_ctx* ctx, const Route& rt, const PlanDev& pg, doubl
         fp.n = n; fp.N = ctx->N; fp.G = G; fp.C = ctx->C; fp.S = pg.S; fp.S_pad = pg.S_pad; fp.link = ctx->link; fp.B = fcfg.B;
         fp.scale = ctx->head.scale; fp.DmT = pg.dmT; fp.dme = pg.dme; fp.z = pg.z; fp.XT = ctx->d_XT; fp.list = ctx->d_idx_full;
         fp.count = ctx->d_counts; fp.pmat64 = pg.pmat64; fp.dvec = pg.dvec64; fp.dlink = ctx->d_dlink;
-        fp.linkfnull = ctx->d_linkfnull; fp.fnull = ctx->d_fnull; fp.acc = ctx->d_acc; fp.done = ctx->d_done; fp.phi = phi_dev;
-        fp.wn = wn;
+        fp.linkfnull = ctx->d_linkfnull; fp.fnull = ctx->d_fnull; fp.acc = ctx->d_acc; fp.wn = wn;
         const bool table = ctx->opt_fused_table && pg.ltab != nullptr;
         if (table) {
             fp.ltab = pg.ltab; fp.ltab_rows = pg.ltab_rows; fp.ltab_inv_h = pg.ltab_inv_h; fp.ltab_fb = ctx->d_ltab_fb;
         }
+        CUDA_TRY(dks::shared_path::launch_explain_fused(fp, fcfg, ctx->sm_count, ctx->stream));
+        // phi from the accumulators the fused kernel filled, sixteen lanes per instance; with push_in_kernel it also
+        // stores the rows into the peers' gathered buffers
+        dks::PeerPush pp;
+        pp.npeers = 0;
         if (ctx->peer_world > 1 && ctx->push_in_kernel) {
-            double* slabs[16];
-            int np = 0;
             for (int r = 0; r < ctx->peer_world; ++r) {
                 double* slab = ctx->peer_base[r] + (long long)ctx->peer_rank * ctx->peer_slab;
                 if (slab == phi_dev) continue;               // phi is written in place into the local slab
-                slabs[np++] = slab;
+                pp.dst[pp.npeers++] = slab;
             }
-            if (!ctx->d_peer_list) CUDA_TRY(ctx->d_peer_list.alloc(16));
-            if (ctx->peer_list_for != phi_dev) {             // (never during a capture: the graph key holds the phi pointer)
-                CUDA_TRY(cudaMemcpy(ctx->d_peer_list, slabs, sizeof(double*) * np, cudaMemcpyHostToDevice));
-                ctx->peer_list_for = phi_dev;
-            }
-            fp.npeers = np;
-            fp.peer_phi = ctx->d_peer_list;
         }
-        CUDA_TRY(dks::shared_path::launch_explain_fused(fp, fcfg, ctx->sm_count, ctx->stream));
-        ctx->launches += 1;
+        dks::shared_path::finish_fused_kernel<<<cdiv(n, 16), 256, 0, ctx->stream>>>(
+            ctx->d_idx_full, ctx->d_counts, ctx->d_acc, dks::shared_path::fused_kpad(G), pg.dvec64, ctx->d_dlink, n, G, ctx->C,
+            phi_dev, pp);
+        ctx->launches += 1;          // the fused launch and its finish count as the route's one coalition launch
         path[DKS_PATH_SHARED] = DKS_SHARED_FUSED; path[DKS_PATH_CHUNKS] = 1; path[DKS_PATH_WARPS] = fcfg.warps;
         path[DKS_PATH_GRID] = ctx->sm_count; path[DKS_PATH_FUSED_B] = fcfg.B; path[DKS_PATH_FUSED_NI] = 1;
         path[DKS_PATH_SOLVE] = DKS_SOLVE_FUSED; path[DKS_PATH_FUSED_CTA_WARPS] = fcfg.slices * fcfg.kw;
@@ -2785,7 +2781,7 @@ static int launch_push(dks_ctx* ctx, const double* phi_dev) {
     }
     if (pp.npeers == 0) return DKS_OK;
     if (ctx->last_fused && ctx->push_in_kernel) {
-        // the fused kernel stored its instances into the peers' buffers as it finished them: only the general kernels' rows are left
+        // the fused route's finish kernel stored its instances into the peers' buffers: only the general kernels' rows are left
         dks::push_rows_kernel<<<8, 256, 0, ctx->stream>>>(phi_dev, pp, ctx->d_idx_other, ctx->d_counts + 1, ctx->cur_n, ctx->G, ctx->C);
         ctx->launches += 1;
         CUDA_TRY(cudaGetLastError());
@@ -2892,7 +2888,6 @@ int dks_set_peers(dks_ctx* ctx, int world, int rank, const uint64_t* gathered_pt
     }
     REQUIRE((slab_doubles & 1) == 0, "dks_set_peers: slab size must be even (128-bit stores)");
     ctx->peer_world = world; ctx->peer_rank = rank; ctx->peer_slab = slab_doubles;
-    ctx->peer_list_for = nullptr;
     return DKS_OK;
 }
 

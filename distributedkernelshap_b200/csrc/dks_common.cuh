@@ -511,7 +511,6 @@ struct dks_ctx {
     DevBuf<int> d_idx_other;     // [n] the rest
     DevBuf<float2> d_sums;       // [n][S_pad] (sum p1, sum p0) of the shared fast path
     DevBuf<long long> d_acc;     // [n][24] fixed-point partial beta of the fused kernel (zero between launches)
-    DevBuf<int> d_done;          // [n] row groups delivered per instance (zero between launches)
     DevBuf<double> d_phi;
     int phi_rows = 0;             // rows of the last dks_explain_host result held in d_phi
     PinnedBuf<double> h_phi_pin;  // pinned staging for results going to pageable host memory
@@ -545,11 +544,9 @@ struct dks_ctx {
     double* peer_base[16] = {};                    // device pointers to each rank's [world][slab] buffer
     unsigned long long* peer_flags[16] = {};       // rank r's flag array [world] (peer-mapped); [peer_rank] is this rank's own
     bool peer_flags_set = false;
-    DevBuf<double*> d_peer_list;                   // device copy of the peers' slab addresses for the current phi buffer
-    double* peer_list_for = nullptr;               // the phi buffer d_peer_list was built for
     DevBuf<unsigned long long> d_step;             // device-side step counter of the flag exchange
-    bool push_in_kernel = false;                   // 1: the fused kernel's epilogue stores phi into the peers' buffers itself
-                                                   // (measured slower than the separate coalesced push kernel: DESIGN.md §7)
+    bool push_in_kernel = false;                   // 1: the fused route's finish kernel stores its phi rows into the peers'
+                                                   // buffers itself (DESIGN.md §7)
     // tuning knobs (dks_set_option; defaults from the environment at dks_create: DKS_FUSED, DKS_FUSED_WARPS, ...)
     int opt_fused = 1, opt_fused_warps = 0, opt_fused_B = 0;
     int opt_fused_table = 1;                       // 0: the fused kernel ignores the plans' link tables (exact loop only)

@@ -9,10 +9,10 @@
 // rows with P broadcast from shared memory, four lanes per instance and KPAD / 4 coefficients per lane (every lane busy on
 // the otherwise idle FP64 pipe, no shuffles).  Each warp adds its partial beta to a per-instance accumulator in 2^-40 FIXED
 // POINT with relaxed 64-bit integer reductions (exact and order-independent: results are bit-reproducible whatever the
-// scheduling), then publishes the delivery with a release add on a per-instance counter; the warp that delivers the last of
-// the S/32 partials of an instance takes an acquire fence, applies the delta term, back-fills the eliminated group, snaps
-// |phi| < 1e-10 and writes phi for both classes (and, on a multi-GPU run, stores them into every peer's gathered buffer over
-// NVLink).  It also resets the accumulator and the counter, so the next launch needs no memset.
+// scheduling), and that is all it does with it: no counter, no fence.  The end of the kernel makes every reduction visible
+// to the next kernel on the stream, finish_fused_kernel, which applies the delta term, back-fills the eliminated group,
+// snaps |phi| < 1e-10 and writes phi for both classes (and, on a multi-GPU run with push_in_kernel, stores them into every
+// peer's gathered buffer over NVLink).  It also zeroes the accumulator, so the next launch needs no memset.
 //
 // A CTA holds `slices` row groups: each slice is the group's 32 rows of Dm (pair sums and pair products, as in
 // explain_shared_smem_kernel) and of P.  kw warps share a slice and stream disjoint subsets of the instances through it,
@@ -24,8 +24,6 @@
 
 namespace dks {
 namespace shared_path {
-
-constexpr int FUSED_MAX_PEERS = 16;
 
 // ---- per-row link table ----------------------------------------------------------------------------------------------
 // With a shared plan and all groups varying, an instance enters coalition row s only through one scalar, x = a(i, s) + dme[s]:
@@ -138,10 +136,6 @@ struct FusedParams {
     const double* linkfnull;
     const double* fnull;
     long long* acc;          // [n][KPAD] fixed-point partial beta (zero between launches)
-    int* done;               // [n] row groups that have delivered (zero between launches)
-    double* phi;             // [C][n][G]
-    int npeers;              // multi-GPU push: phi of every finished instance also goes to these buffers ([C][n][G] each)
-    double* const* peer_phi; // [npeers] device array of the peers' slab addresses (NULL on one GPU)
     const float* wn;         // [N] weighted backgrounds: N w_j (the weighted instantiations only; dks_shared.cuh)
     const LinkTabEntry* ltab;        // the plan's link table (below), NULL: every pass takes the exact loop
     const LinkTabRow* ltab_rows;     // [S_pad]
@@ -169,92 +163,40 @@ __device__ __forceinline__ void chunk_sums_rt(const float (&v)[16], int nq, int 
     }
 }
 
-// multi-GPU: the phi rows of the instances this warp just finished go to every peer's gathered buffer, stored by the whole warp
-// (lanes = groups: coalesced NVLink packets instead of one 8-byte store per value from the finishing lane).  Out of line so
-// that the single-GPU instantiation of the kernel does not pay registers for it.
-__device__ __noinline__ void peer_push_finished(const double* __restrict__ phi, double* const* __restrict__ peers, int npeers,
-                                                int fin_i, int lane, int G, size_t slab) {
-    unsigned fin = __ballot_sync(0xffffffffu, fin_i >= 0);
-    while (fin) {
-        const int src = __ffs(fin) - 1;
-        fin &= fin - 1;
-        const int i = __shfl_sync(0xffffffffu, fin_i, src);
-        __syncwarp();
-        for (int idx = lane; idx < 2 * G; idx += 32) {
-            const size_t off = (idx < G ? 0 : slab) + (size_t)i * G + (idx < G ? idx : idx - G);
-            const double v = __ldcg(phi + off);
-            for (int r = 0; r < npeers; ++r) peers[r][off] = v;
-        }
+// every row group has delivered: phi of both classes for the count[0] instances of `list`, from the fixed-point
+// accumulators explain_shared_fused_kernel left (its end made every reduction visible), then the accumulators zeroed for
+// the next launch.  Sixteen lanes per instance (G <= 16 on the fused path): lane k takes coefficient k, lane nA the
+// eliminated group, so each class's phi row is one contiguous store.  Every lane forms the eliminated group's sum over
+// k = 0 .. nA - 1 in order from shuffles, the operations and order of a one-lane loop.  peers: on a multi-GPU run with
+// push_in_kernel, the rows also go to every peer's gathered buffer (npeers = 0 otherwise).
+__global__ void __launch_bounds__(256) finish_fused_kernel(const int* __restrict__ list, const int* __restrict__ count,
+                                                           long long* __restrict__ acc, int kpad, const double* __restrict__ dvec,
+                                                           const double* __restrict__ dlink, int n, int G, int C,
+                                                           double* __restrict__ phi, PeerPush peers) {
+    const int t = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 4), k = threadIdx.x & 15;
+    if (t >= *count) return;                                   // the same on the instance's sixteen lanes
+    const unsigned half = 0xffffu << (threadIdx.x & 16);
+    const int i = list[t], nA = G - 1;
+    long long* a = acc + (size_t)i * kpad;
+    const double delta = dlink[(size_t)i * C + 1];
+    double val = 0.0;
+    if (k < nA) {
+        val = from_fix(a[k]) - delta * dvec[k];
+        a[k] = 0;
     }
-}
-
-// every row group has delivered instance i: phi of both classes from its accumulator (read from L2), then the accumulator
-// and the counter reset for the next launch.  One lane: the run-time-N instantiations, which have no registers to spare
-// for finish_instances at 20 warps
-template <int KPAD>
-__device__ __forceinline__ void finish_instance(const FusedParams& p, int i, int nA, size_t slab) {
-    long long* acc = p.acc + (size_t)i * KPAD;
-    const double delta = p.dlink[(size_t)i * p.C + 1];
     double sum = 0.0;
-    double* phi1 = p.phi + slab + (size_t)i * p.G;
-    double* phi0 = p.phi + (size_t)i * p.G;
-    for (int k = 0; k < nA; ++k) {
-        double val = from_fix(__ldcg(acc + k)) - delta * p.dvec[k];
-        sum += val;
-        if (fabs(val) < 1e-10) val = 0.0;
-        phi1[k] = val;
-        phi0[k] = (val == 0.0) ? 0.0 : -val;
-        acc[k] = 0;
+    for (int m = 0; m < nA; ++m) sum += __shfl_sync(half, val, m, 16);
+    if (k == nA) val = delta - sum;                            // the eliminated (last) group takes the remainder
+    if (k > nA) return;
+    if (fabs(val) < 1e-10) val = 0.0;
+    const double neg = (val == 0.0) ? 0.0 : -val;
+    const size_t slab = (size_t)n * G, off = (size_t)i * G + k;
+    phi[slab + off] = val;
+    phi[off] = neg;
+    for (int r = 0; r < peers.npeers; ++r) {
+        peers.dst[r][slab + off] = val;
+        peers.dst[r][off] = neg;
     }
-    double last = delta - sum;                  // the eliminated (last) group takes the remainder
-    if (fabs(last) < 1e-10) last = 0.0;
-    phi1[nA] = last;
-    phi0[nA] = (last == 0.0) ? 0.0 : -last;
-    p.done[i] = 0;
-}
-
-// the same on the instance's four lanes (fin; i and fin are the same on the instance's four lanes q = 0 .. 3): phi of
-// both classes from its accumulator (read from L2), then the accumulator and the counter reset for the next launch.  Lane q
-// takes coefficients q, q + 4, ..., the ones it delivered, so its loads are independent and in flight together (one lane
-// looping over the coefficients waits for each load in turn: its phi and acc stores may alias the next load).  The
-// eliminated group's sum still runs k = 0 .. nA - 1 in order, on lane 0, over the values the quad parked in the instance's
-// column of the staging tile (ycol, row stride ystride), which the turn-around has finished reading.  Called by the whole
-// warp; returns true on lane 0 of a finishing quad.
-template <int KPAD>
-__device__ __forceinline__ bool finish_instances(const FusedParams& p, bool fin, int i, int q, int nA, size_t slab,
-                                                 double* ycol, int ystride) {
-    constexpr int KPL = KPAD / 4;
-    if (fin) {
-        long long* acc = p.acc + (size_t)i * KPAD;
-        double* phi1 = p.phi + slab + (size_t)i * p.G;
-        double* phi0 = p.phi + (size_t)i * p.G;
-        const double delta = p.dlink[(size_t)i * p.C + 1];
-        long long a[KPL];
-#pragma unroll
-        for (int j = 0; j < KPL; ++j) a[j] = q + 4 * j < nA ? __ldcg(acc + q + 4 * j) : 0;
-#pragma unroll
-        for (int j = 0; j < KPL; ++j) {
-            const int k = q + 4 * j;
-            if (k < nA) {
-                double val = from_fix(a[j]) - delta * p.dvec[k];
-                ycol[k * ystride] = val;
-                if (fabs(val) < 1e-10) val = 0.0;
-                phi1[k] = val;
-                phi0[k] = (val == 0.0) ? 0.0 : -val;
-                acc[k] = 0;
-            }
-        }
-    }
-    __syncwarp();
-    if (!fin || q != 0) return false;
-    double sum = 0.0;
-    for (int k = 0; k < nA; ++k) sum += ycol[k * ystride];
-    double last = p.dlink[(size_t)i * p.C + 1] - sum;     // the eliminated (last) group takes the remainder
-    if (fabs(last) < 1e-10) last = 0.0;
-    p.phi[slab + (size_t)i * p.G + nA] = last;
-    p.phi[(size_t)i * p.G + nA] = (last == 0.0) ? 0.0 : -last;
-    p.done[i] = 0;
-    return true;
 }
 
 // weighted: the weighted slice (twice the bytes) and the per-CTA W2 array of dks_shared.cuh
@@ -364,46 +306,47 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
         // row groups, contiguous ordinals; otherwise the part's instances dealt round-robin over the slice's kw warps
         const long long seg_end = flat && u0 < u1 ? ((u0 / cnt) + 1) * cnt : 0;
         const int nseg = flat ? (u0 < u1 ? (u1 > seg_end ? 2 : 1) : 0) : 1;
+        // what the segments need of the flat range, formed once (the 64-bit bounds are not held through the passes)
+        const int rg0 = flat ? (u0 < u1 ? (int)(u0 / cnt) : 0) : gs % n_rg;
+        const int first0 = flat ? (u0 < u1 ? (int)(u0 % cnt) : 0) : gs / n_rg + sub * nparts;
+        const int my_n0 = flat ? (int)((u1 < seg_end ? u1 : seg_end) - u0) : 0, my_n1 = flat ? (int)(u1 - seg_end) : 0;
         for (int seg = 0; seg < nseg; ++seg) {
-            const int rg = flat ? (int)(u0 / cnt) + seg : gs % n_rg;
+            const int rg = rg0 + seg;
             const int s = rg * 32 + lane;
             const int fs = flat ? rg - rg_lo : slice;
             const double* sPw = sP + (size_t)fs * 32 * KPAD;
             const float4* sl = sDm + (size_t)fs * sq4 * 32;
-            const int first = flat ? (seg == 0 ? (int)(u0 % cnt) : 0) : gs / n_rg + sub * nparts;
+            const int first = seg == 0 ? first0 : 0;
             const int stride = flat ? 1 : nparts * kw;
-            const int my_n = flat ? (int)(seg == 0 ? (u1 < seg_end ? u1 : seg_end) - u0 : u1 - seg_end)
-                                  : (first < cnt ? (cnt - first + stride - 1) / stride : 0);
+            const int my_n = flat ? (seg == 0 ? my_n0 : my_n1) : (first < cnt ? (cnt - first + stride - 1) / stride : 0);
             const double es = p.dme[s];
             const uint64_t zz = s < p.S ? p.z[s] : 0ull;
             const int ntab = (G + 3) / 4;                     // <= 4 (the host sends wider problems down the unfused path)
             const f32x2 one2 = f2_pack(1.f, 1.f), two2 = f2_pack(2.f, 2.f);
             const double yf = p.link == DKS_LINK_LOGIT ? p.linkfnull[1] : p.fnull[1], inv_n = 1.0 / (double)N;   // link(fnull)
-            const size_t slab = (size_t)p.n * G;
             const bool row_ok = s < p.S;
             const int bmask = B - 1;
 
             // ---- the turn-around: four lanes per instance of the batch (eight instances per round), lane q of an instance owns
-            // coefficients q, q + 4, ...; each sums the warp's 32 rows in order sr = 0 .. 31
+            // coefficients q, q + 4, ...; each sums the warp's 32 rows in order sr = 0 .. 31 and adds the partial to the
+            // instance's accumulator (finish_fused_kernel reads the sums once the kernel has ended).  The run-time-N
+            // instantiations unroll the rows by two: by four they spill at 20 warps
             auto flush = [&](int bstart, int bcount) {
                 constexpr int KPL = KPAD / 4;
                 const int q = lane & 3;
                 for (int b0 = 0; b0 < bcount; b0 += 8) {
                     const int b = b0 + (lane >> 2);
-                    const bool mine = b < bcount;
-                    int i = 0;
-                    int fin_i = -1;             // instance this lane finished in this round (its phi is complete in local memory)
-                    if (mine) {
+                    if (b < bcount) {
                         double beta[KPL];
 #pragma unroll
                         for (int j = 0; j < KPL; ++j) beta[j] = 0.0;
-#pragma unroll 4
+#pragma unroll (NCT != 0 ? 4 : 2)
                         for (int sr = 0; sr < 32; ++sr) {
                             const double y = sYw[sr * ystride + b];
 #pragma unroll
                             for (int j = 0; j < KPL; ++j) beta[j] = fma(sPw[sr * KPAD + q + 4 * j], y, beta[j]);
                         }
-                        i = p.list[first + (bstart + b) * stride];
+                        const int i = p.list[first + (bstart + b) * stride];
                         long long* acc = p.acc + (size_t)i * KPAD;
 #pragma unroll
                         for (int j = 0; j < KPL; ++j)
@@ -411,28 +354,6 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
                                 asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(acc + q + 4 * j),
                                              "l"((unsigned long long)to_fix(beta[j])) : "memory");
                     }
-                    __syncwarp();               // the instance's four lanes have added: its first lane publishes the delivery
-                    int old = 0;
-                    if (mine && q == 0) {
-                        asm volatile("atom.release.gpu.global.add.s32 %0, [%1], 1;" : "=r"(old) : "l"(p.done + i) : "memory");
-                        if (old == n_rg - 1) {
-                            // every row group has delivered: the acquire (with NCT ordered before the other three lanes'
-                            // reads by the __syncwarp below), then finish the instance
-                            asm volatile("fence.acq_rel.gpu;" ::: "memory");
-                            if constexpr (NCT == 0) {
-                                finish_instance<KPAD>(p, i, nA, slab);
-                                fin_i = i;
-                            }
-                        }
-                    }
-                    if constexpr (NCT != 0) {
-                        __syncwarp();
-                        const int old_i = __shfl_sync(0xffffffffu, old, lane & ~3);
-                        const bool fin = mine && old_i == n_rg - 1;
-                        if (__any_sync(0xffffffffu, fin) && finish_instances<KPAD>(p, fin, i, q, nA, slab, sYw + b, ystride))
-                            fin_i = i;
-                    }
-                    if (p.npeers > 0) peer_push_finished(p.phi, p.peer_phi, p.npeers, fin_i, lane, G, slab);     // multi-GPU only (kept out of line: no registers here)
                 }
             };
 

@@ -807,7 +807,7 @@ __global__ void push_phi_kernel(const double* __restrict__ src, PeerPush pp, lon
     if ((n_doubles & 1) && blockIdx.x == 0 && threadIdx.x == 0) dst[n_doubles - 1] = src[n_doubles - 1];
 }
 
-// Same, for the rows of an instance list only (the fused shared-plan kernel has already stored its instances into the
+// Same, for the rows of an instance list only (the fused route's finish kernel has already stored its instances into the
 // peers' buffers; what the general kernels computed still has to travel).  phi is [C][n][G].
 __global__ void push_rows_kernel(const double* __restrict__ src, PeerPush pp, const int* __restrict__ list,
                                  const int* __restrict__ count, int n, int G, int C) {

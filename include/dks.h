@@ -441,8 +441,9 @@ int dks_set_kernel(dks_ctx* ctx, int kernel);       /* DKS_KERNEL_* */
  * coalition kernel (default 1; 0 = separate (sum p1, sum p0) buffer + solve kernel); "fused_warps" caps the warps per CTA (default: as many as fit, at most 20); "fused_batch" instances
  * parked per warp before the turn-around; "fused_table" 0/1 -- the fused kernel reads y from the plan's link table
  * (default 1; 0 = the exact loop over the background for every pass);
- * "push_in_kernel" 0/1 -- multi-GPU: the fused kernel's epilogue stores phi into the peers' buffers itself instead of the
- * separate push kernel (default 0: measured slower, it stalls the finishing warps); "graph" 0/1 (CUDA-graph
+ * "push_in_kernel" 0/1 -- multi-GPU: the fused route's finish kernel stores the phi rows of its instances into the peers'
+ * buffers as it writes them, and the push kernel after the solve moves only the other instances' rows (default 0: the
+ * push kernel moves every row); "graph" 0/1 (CUDA-graph
  * replay of dks_run_dev); "graph_timing" 0/1 -- keep the timing event records inside the graph (default 0: a replayed graph
  * carries no timing nodes and dks_last_timings reports an error after it). */
 int dks_set_option(dks_ctx* ctx, const char* name, int value);

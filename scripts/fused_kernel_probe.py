@@ -8,7 +8,7 @@ the number of instances.
 The workload is bench.py's: 2560 Adult-shaped instances, 12 groups, 100 background rows, nsamples = 2048, shared plans.
 For the engine's default configuration and for every ``fused_warps`` value of the sweep it reports
 
-  kernel_ms   the coalition stage (explain_shared_fused_kernel) timed by the engine's own CUDA events
+  kernel_ms   the coalition stage (explain_shared_fused_kernel and its finish_fused_kernel) timed by the engine's own CUDA events
               (``last_timings_ms()["coalitions"]``, plain launches: ``graph`` 0), mean / min / max over ``--launches``
               launches, L2 flushed before each;
   step_ms     a whole device-resident step (CUDA graph replay, as bench.py's ``value`` times it), mean over ``--steps``,

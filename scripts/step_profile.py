@@ -10,9 +10,11 @@ then ``--steps`` times under ``torch.profiler`` with CUDA activities (a run of i
 DIR/step_trace_n<n>.json).  From the trace, per step:
 
   nodes   the device time of every node of the replayed graph: the status/counter memset, stage 1 (``prep_kernel``), the
-          fused shared-plan kernel and the general kernel(s) of the remaining instances;
+          fused shared-plan kernel, its finish kernel (``finish_fused_kernel``) and the general kernel(s) of the
+          remaining instances;
   gaps    from the end of the memset to the start of stage 1, from the end of stage 1 to the start of the fused kernel,
-          and from the end of the fused kernel to the end of the step;
+          from the end of the fused kernel to the start of the finish kernel, and from the end of the fused kernel to
+          the end of the step;
   stage1_plus_gaps   memset end -> fused kernel start, what stage 1 costs the step;
   span    memset start -> the end of the last node.
 
@@ -34,7 +36,7 @@ import numpy as np  # noqa: E402
 
 import bench  # noqa: E402  (the workload and the NVML power limit of the benchmark)
 
-ROLES = (("prep", "prep_kernel"), ("fused", "explain_shared_fused_kernel"))
+ROLES = (("prep", "prep_kernel"), ("fused", "explain_shared_fused_kernel"), ("finish", "finish_fused_kernel"))
 
 
 def role_of(ev):
@@ -88,6 +90,8 @@ def attribute(step):
                        "fused->step_end": end - t["fused"][1]},
            "stage1_plus_gaps_us": t["fused"][0] - t["memset"][1],
            "span_us": end - t["memset"][0]}
+    if "finish" in t:
+        out["gaps_us"]["fused->finish"] = t["finish"][0] - t["fused"][1]
     if "general" in t:
         out["gaps_us"]["prep->general"] = t["general"][0] - t["prep"][1]
     return out
