@@ -5,14 +5,14 @@
 // the job: y = link(ey) - link(fnull) in place, then beta_k(i) = sum_s P[k][s] y(i, s) with P = inv(E^T W E) E^T W of the
 // shared plan (float64, the warp's 32 rows of it resident in shared memory).  The sum over s runs across the lanes of a warp
 // (lane = coalition row), so instead of shuffling per instance the warp parks y for a batch of B instances in shared
-// memory ([row][instance], conflict-free both ways) and then turns the tile around: lane = instance, loop over its 32
-// rows with P broadcast from shared memory, four lanes per instance and KPAD / 4 coefficients per lane (every lane busy on
-// the otherwise idle FP64 pipe, no shuffles).  Each warp adds its partial beta to a per-instance accumulator in 2^-40 FIXED
-// POINT with relaxed 64-bit integer reductions (exact and order-independent: results are bit-reproducible whatever the
-// scheduling), and that is all it does with it: no counter, no fence.  The end of the kernel makes every reduction visible
-// to the next kernel on the stream, finish_fused_kernel, which applies the delta term, back-fills the eliminated group,
-// snaps |phi| < 1e-10 and writes phi for both classes (and, on a multi-GPU run with push_in_kernel, stores them into every
-// peer's gathered buffer over NVLink).  It also zeroes the accumulator, so the next launch needs no memset.
+// memory ([row][instance], conflict-free both ways) and then turns the tile around on the FP64 tensor cores: eight
+// DMMA.16x8x4 per eight instances sum P y over the 32 rows (P from shared memory, no shuffles).  Each warp adds its
+// partial beta to a per-instance accumulator in 2^-40 FIXED POINT with relaxed 64-bit integer reductions (exact and
+// order-independent: results are bit-reproducible whatever the scheduling), and that is all it does with it: no
+// counter, no fence.  The end of the kernel makes every reduction visible to the next kernel on the stream,
+// finish_fused_kernel, which applies the delta term, back-fills the eliminated group, snaps |phi| < 1e-10 and writes
+// phi for both classes (and, on a multi-GPU run with push_in_kernel, stores them into every peer's gathered buffer over
+// NVLink).  It also zeroes the accumulator, so the next launch needs no memset.
 //
 // A CTA holds `slices` row groups: each slice is the group's 32 rows of Dm (pair sums and pair products, as in
 // explain_shared_smem_kernel) and of P.  kw warps share a slice and stream disjoint subsets of the instances through it,
@@ -327,32 +327,38 @@ __global__ void __launch_bounds__(32 * NWARPS, 1) explain_shared_fused_kernel(Fu
             const bool row_ok = s < p.S;
             const int bmask = B - 1;
 
-            // ---- the turn-around: four lanes per instance of the batch (eight instances per round), lane q of an instance owns
-            // coefficients q, q + 4, ...; each sums the warp's 32 rows in order sr = 0 .. 31 and adds the partial to the
-            // instance's accumulator (finish_fused_kernel reads the sums once the kernel has ended).  The run-time-N
-            // instantiations unroll the rows by two: by four they spill at 20 warps
+            // ---- the turn-around on the FP64 tensor cores: eight instances of the batch per round, beta = P y over the
+            // warp's 32 rows as eight mma.m16n8k4 k-steps (rows 4 kk .. 4 kk + 3, kk = 0 .. 7, in order).  Lane (tig =
+            // lane & 3, gid = lane >> 2) feeds P[gid][s] and P[gid + 8][s] (A) and y of instance gid (B) at row
+            // s = 4 kk + tig, and receives coefficients gid and gid + 8 of instances 2 tig and 2 tig + 1 (D).  A D column
+            // depends on its own B column only, so an instance's partial does not depend on the batch it shares; the
+            // partial goes to the instance's accumulator (finish_fused_kernel reads the sums once the kernel has ended)
             auto flush = [&](int bstart, int bcount) {
-                constexpr int KPL = KPAD / 4;
-                const int q = lane & 3;
+                const int tig = lane & 3, gid = lane >> 2;
                 for (int b0 = 0; b0 < bcount; b0 += 8) {
-                    const int b = b0 + (lane >> 2);
-                    if (b < bcount) {
-                        double beta[KPL];
+                    double d0 = 0.0, d1 = 0.0, d2 = 0.0, d3 = 0.0;
+                    // by two: fully unrolled, some instantiations spill at their register bound
+#pragma unroll 2
+                    for (int kk = 0; kk < 8; ++kk) {
+                        const int sr = 4 * kk + tig;
+                        const double a0 = sPw[sr * KPAD + gid], a1 = gid + 8 < KPAD ? sPw[sr * KPAD + gid + 8] : 0.0;
+                        const double y = sYw[sr * ystride + b0 + gid];      // columns past bcount: not delivered
+                        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, "
+                                     "{%0,%1,%2,%3};"
+                                     : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3) : "d"(a0), "d"(a1), "d"(y));
+                    }
 #pragma unroll
-                        for (int j = 0; j < KPL; ++j) beta[j] = 0.0;
-#pragma unroll (NCT != 0 ? 4 : 2)
-                        for (int sr = 0; sr < 32; ++sr) {
-                            const double y = sYw[sr * ystride + b];
-#pragma unroll
-                            for (int j = 0; j < KPL; ++j) beta[j] = fma(sPw[sr * KPAD + q + 4 * j], y, beta[j]);
+                    for (int h = 0; h < 2; ++h) {
+                        const int b = b0 + 2 * tig + h;
+                        if (b < bcount) {
+                            long long* acc = p.acc + (size_t)p.list[first + (bstart + b) * stride] * KPAD;
+                            if (gid < nA)
+                                asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(acc + gid),
+                                             "l"((unsigned long long)to_fix(h ? d1 : d0)) : "memory");
+                            if (gid + 8 < nA)
+                                asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(acc + gid + 8),
+                                             "l"((unsigned long long)to_fix(h ? d3 : d2)) : "memory");
                         }
-                        const int i = p.list[first + (bstart + b) * stride];
-                        long long* acc = p.acc + (size_t)i * KPAD;
-#pragma unroll
-                        for (int j = 0; j < KPL; ++j)
-                            if (q + 4 * j < nA)
-                                asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(acc + q + 4 * j),
-                                             "l"((unsigned long long)to_fix(beta[j])) : "memory");
                     }
                 }
             };
