@@ -34,6 +34,9 @@ ACT_KMACH = 7
 ACT_MLP = 8
 ACT_KNN = 9
 ACT_ENSEMBLE = 10
+ACT_EXTERNAL = 11
+EXTERNAL_FLOAT32 = 0
+EXTERNAL_FLOAT64 = 1
 LINK_IDENTITY = 0
 LINK_LOGIT = 1
 KERNEL_AUTO = 0
@@ -63,6 +66,13 @@ SIGNATURES = {
     "dks_set_knn_model": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int, C.c_double, C.c_int,
                                                                              C.c_int, C.c_void_p, C.c_int, C.c_int]),
     "dks_set_ensemble": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "dks_set_external_model": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
+    "dks_set_external_background": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+    "dks_external_prepare": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
+    "dks_external_begin": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int64)]),
+    "dks_external_mask": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    "dks_external_reduce": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int]),
+    "dks_external_finish": (C.c_int, [C.c_void_p, C.c_void_p]),
     "dks_set_column_maps": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     "dks_set_column_encoding": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                           C.c_int]),

@@ -23,6 +23,7 @@
 #include "dks_mlp.cuh"
 #include "dks_knn.cuh"
 #include "dks_ensemble.cuh"
+#include "dks_external.cuh"
 
 namespace {
 
@@ -198,6 +199,11 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         // its own
         h.family = DKS_GENERAL_ENSEMBLE;
         break;
+    case DKS_ACT_EXTERNAL:
+        // no shared-plan route: the caller's module evaluates the masked rows, every instance runs the ensemble's tail on
+        // their background means; every output is solved on its own
+        h.family = DKS_GENERAL_EXTERNAL;
+        break;
     }
     if (h.shared != HEAD_SHARED_BINARY && !h.own()) h.shared_max_G = 128;
     if (!h.mixture()) h.xt_scale = h.scale;
@@ -273,6 +279,9 @@ OwnKernel own_kernel(int family) {
     case DKS_GENERAL_ENSEMBLE:          // refuses: what its members refuse (refusing_kernel)
         return {"soft-voting ensembles", "ensemble kernels", "groups", "soft-voting ensemble",
                 " (put the preprocessing in front of the ensemble)", REFUSES_NONE, ensemble_smem};
+    case DKS_GENERAL_EXTERNAL:          // refuses: nothing (the module sees every raw value)
+        return {"modules", "module route", "nsamples", "module", " (put the preprocessing inside the module)", REFUSES_NONE,
+                [](const dks_ctx* c, int S_cap) { return dks::ens::tail_smem_bytes(S_cap, c->C); }};
     }
     return {};                          // a linear head
 }
@@ -355,6 +364,11 @@ int check_own_columns(const dks_ctx* ctx, const OwnKernel& ok) {
     case DKS_GENERAL_KMACH: reads = (int)(ctx->h_kcolw.size() / ctx->km.K); break;
     case DKS_GENERAL_MLP: reads = ctx->mlp.width[0]; break;
     case DKS_GENERAL_ENSEMBLE: return DKS_OK;         // each member checks its own (fit_members)
+    case DKS_GENERAL_EXTERNAL:                        // the module reads the raw rows: the caller checked its width
+        if (E > 0)
+            return fail(DKS_ERR_UNSUPPORTED, "module: a column encoding is not supported (put the preprocessing inside the "
+                        "module)");
+        return DKS_OK;
     default: reads = (int)ctx->h_ncolw.size(); break;
     }
     if (reads != width)
@@ -490,8 +504,26 @@ int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const
                                                                         linkfnull, out, dlink, ctx->d_status);
         break;
     }
+    case DKS_GENERAL_EXTERNAL:      // the module's outputs on these rows, which the caller handed to dks_external_prepare
+        if (ctx->ext_y == nullptr)
+            return fail(DKS_ERR_UNSUPPORTED, "module: the engine cannot run a module; run it on the rows and hand its outputs "
+                        "to dks_external_prepare, then explain with dks_external_begin / _mask / _reduce / _finish");
+        dks::ext::external_load_kernel<<<cdiv(n, 128), 128, 0, st>>>(ctx->ext_y, ctx->ext_y_f64, n, C, link, linkfnull, out,
+                                                                     dlink, ctx->d_status);
+        break;
     }
     ctx->launches += 1;
+    return DKS_OK;
+}
+
+// explain_ensemble_tail_kernel over p.list on the background means ey [n][C][S_cap] (L1: the moments of y; complement: the
+// logit's 1 - ey_c taken per output, for outputs that need not sum to one)
+int launch_tail(dks_ctx* ctx, bool l1, const ExplainParams& p, const dks::SimtL1& q, const double* ey, bool complement,
+                cudaStream_t st) {
+    const size_t tsm = dks::ens::tail_smem_bytes(p.S_cap, ctx->C);
+    auto kern = l1 ? dks::ens::explain_ensemble_tail_kernel<true> : dks::ens::explain_ensemble_tail_kernel<false>;
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsm));
+    kern<<<persistent_grid(ctx, tsm, 1024, 8, ctx->cur_n), dks::ens::THREADS, tsm, st>>>(p, q, ey, complement ? 1 : 0);
     return DKS_OK;
 }
 
@@ -548,12 +580,12 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
             const dks::EnsAcc mea{ctx->d_ens_ey, ctx->h_ens_pi[k], k == 0 ? 1 : 0};
             TRY(on_member(ctx, m, [&] { return launch_own_kernel(m, false, p, msm, st, mea); }));
         }
-        const size_t tsm = dks::ens::tail_smem_bytes(p.S_cap, ctx->C);
-        auto kern = l1 ? dks::ens::explain_ensemble_tail_kernel<true> : dks::ens::explain_ensemble_tail_kernel<false>;
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tsm));
-        kern<<<persistent_grid(ctx, tsm, 1024, 8, ctx->cur_n), dks::ens::THREADS, tsm, st>>>(p, q, ctx->d_ens_ey);
+        TRY(launch_tail(ctx, l1, p, q, ctx->d_ens_ey, false, st));
         break;
     }
+    case DKS_GENERAL_EXTERNAL:      // ey from dks_external_reduce; a module's outputs need not sum to one
+        TRY(launch_tail(ctx, l1, p, q, ctx->d_ens_ey, true, st));
+        break;
     }
     ctx->launches += 1;
     return DKS_OK;
@@ -567,6 +599,7 @@ decltype(&dks::prep_kernel<STAGE, MAPS>) prep_kernel_for(bool mixture, int R) {
 }
 
 int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
+    ctx->ext_coalitions = -1;           // stage 1 rewrites what a module's call laid out by dks_external_begin reads
     const int G = ctx->G;
     const HeadDesc& h = ctx->head;
     TRY(ensure_workspace(ctx, n));
@@ -816,6 +849,7 @@ int fail_refused(const dks_ctx* ctx, const char* prefix) {
 int fit_begin(dks_ctx* ctx) {
     const int N = ctx->N, D = ctx->D, G = ctx->G, R = ctx->R, C = ctx->C;
     const cudaStream_t st = ctx->stream;
+    ctx->ext_coalitions = -1;
     CUDA_TRY(ctx->d_bg.alloc((size_t)N * D));
     CUDA_TRY(ctx->d_wbg.alloc((size_t)N));
     CUDA_TRY(ctx->d_W.alloc((size_t)R * D));
@@ -949,12 +983,24 @@ int fit_own(dks_ctx* ctx) {
     TRY(fit_begin(ctx));
     TRY(fit_encoding(ctx));
     if (ctx->head.family == DKS_GENERAL_ENSEMBLE) return fit_members(ctx, ok);
-    const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
-    TRY(own_fit_tables(ctx, bg, model_columns(ctx)));
     DevBuf<double> pred;
-    CUDA_TRY(pred.alloc((size_t)N * C));
-    TRY(launch_own_predict(ctx, bg, N, nullptr, nullptr, pred, nullptr));
-    dks::fit_pred_fnull_kernel<<<1, 32, 0, ctx->stream>>>(pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull, ctx->d_linkfnull);
+    const double* bg_pred = pred;
+    if (ctx->head.family == DKS_GENERAL_EXTERNAL) {
+        // a module: its outputs on the background (dks_set_external_background), and the group of every column for the mask
+        REQUIRE(ctx->d_ext_bgy.size() == (size_t)N * C,
+                "dks_fit: a module needs its outputs on the %d background rows first (dks_set_external_background)", N);
+        const std::vector<int32_t> colgrp = column_groups(ctx);
+        CUDA_TRY(ctx->fit_pool.upload(&ctx->d_ext_colgrp, colgrp.data(), colgrp.size(), ctx->stream));
+        bg_pred = ctx->d_ext_bgy;
+    } else {
+        const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
+        TRY(own_fit_tables(ctx, bg, model_columns(ctx)));
+        CUDA_TRY(pred.alloc((size_t)N * C));
+        TRY(launch_own_predict(ctx, bg, N, nullptr, nullptr, pred, nullptr));
+        bg_pred = pred;
+    }
+    dks::fit_pred_fnull_kernel<<<1, 32, 0, ctx->stream>>>(bg_pred, ctx->d_wbg, N, C, ctx->link, ctx->d_fnull,
+                                                          ctx->d_linkfnull);
     ctx->launches += 1;
     TRY(fit_readback(ctx, ok.model));
     return fit_done(ctx);
@@ -1476,14 +1522,17 @@ int prepare_debug_dump(dks_ctx* ctx, int S_cap) {
     return DKS_OK;
 }
 
-int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const double* ext_w, int ext_stride) {
+// the start of an explain call: its route and the explain kernels' parameters, every instance's plan drawn first when the
+// device draws them
+int explain_setup(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const double* ext_w, int ext_stride, Route* rtp,
+                  ExplainParams* pp) {
     REQUIRE(ctx->prepared, "dks_explain: call dks_prepare_* first");
     REQUIRE((ext_z == nullptr) == (ext_w == nullptr), "ext_zbits and ext_w must both be given or both be NULL");
     memset(ctx->last_path, 0, sizeof(ctx->last_path));   // what this call launches (dks_last_path)
-    Route rt;
+    Route& rt = *rtp;
     TRY(choose_route(ctx, ext_z, ext_stride, &rt));
     const int n = ctx->cur_n, G = ctx->G;
-    ExplainParams p;
+    ExplainParams& p = *pp;
     memset(&p, 0, sizeof(p));
     p.n = n; p.N = ctx->N; p.G = G; p.R = ctx->R; p.C = ctx->C;
     p.act = ctx->act; p.link = ctx->link; p.S_req = ctx->nsamples_req;
@@ -1495,6 +1544,13 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     p.phi = phi_dev; p.status = ctx->d_status;
     p.S_cap = rt.S_cap;
     if (rt.draw) TRY(launch_sampler(ctx, rt, &p));
+    return DKS_OK;
+}
+
+// the explain kernels of a call explain_setup laid out, phi into p.phi
+int explain_launch(dks_ctx* ctx, const Route& rt, ExplainParams p) {
+    const int n = ctx->cur_n, G = ctx->G;
+    double* phi_dev = p.phi;
     if (ctx->dbg_i >= 0) TRY(prepare_debug_dump(ctx, rt.S_cap));
     CUDA_TRY(record_ev(ctx, 2));
     ctx->l1_timing_valid = false;
@@ -1529,6 +1585,16 @@ int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const d
     }
     CUDA_TRY(record_ev(ctx, 3));
     return DKS_OK;
+}
+
+int launch_explain(dks_ctx* ctx, double* phi_dev, const uint64_t* ext_z, const double* ext_w, int ext_stride) {
+    if (ctx->head.family == DKS_GENERAL_EXTERNAL)
+        return fail(DKS_ERR_UNSUPPORTED, "module: the caller runs the module between the engine's launches; explain with "
+                    "dks_external_begin / _mask / _reduce / _finish");
+    Route rt;
+    ExplainParams p;
+    TRY(explain_setup(ctx, phi_dev, ext_z, ext_w, ext_stride, &rt, &p));
+    return explain_launch(ctx, rt, p);
 }
 
 int check_status(dks_ctx* ctx) {
@@ -2914,24 +2980,23 @@ int dks_graph_launches(dks_ctx* ctx, int64_t* count) {
     return DKS_OK;
 }
 
-int dks_explain_host(dks_ctx* ctx, const double* X_host, int n, double* phi_host, const uint64_t* ext_zbits_host,
-                     const double* ext_w_host, int ext_stride) {
-    BIND(ctx);
-    REQUIRE(ctx->fitted, "dks_explain_host: call dks_fit first");
-    REQUIRE(X_host && phi_host && n > 0, "dks_explain_host: bad arguments");
-    TRY(dks_prepare_host(ctx, X_host, n));
-    size_t need_phi = (size_t)ctx->C * n * ctx->G;
-    if (need_phi > ctx->d_phi.size()) CUDA_TRY(ctx->d_phi.alloc(need_phi));
-    const uint64_t* dz = nullptr; const double* dw = nullptr;
-    if (ext_zbits_host) {
-        REQUIRE(ext_w_host && ext_stride > 0, "dks_explain_host: ext_w / ext_stride missing");
-        size_t need = (size_t)n * ext_stride;
-        if (need > ctx->d_extw.size()) { CUDA_TRY(ctx->d_extz.alloc(need)); CUDA_TRY(ctx->d_extw.alloc(need)); }
-        CUDA_TRY(cudaMemcpyAsync(ctx->d_extz, ext_zbits_host, sizeof(uint64_t) * need, cudaMemcpyHostToDevice, ctx->stream));
-        CUDA_TRY(cudaMemcpyAsync(ctx->d_extw, ext_w_host, sizeof(double) * need, cudaMemcpyHostToDevice, ctx->stream));
-        dz = ctx->d_extz; dw = ctx->d_extw;
-    }
-    TRY(launch_explain(ctx, ctx->d_phi, dz, dw, ext_stride));
+// caller-supplied plans [n][ext_stride] from host memory into the context's buffers (*dz, *dw; NULL without plans)
+static int stage_ext_plans(dks_ctx* ctx, int n, const uint64_t* ext_zbits_host, const double* ext_w_host, int ext_stride,
+                           const uint64_t** dz, const double** dw) {
+    *dz = nullptr; *dw = nullptr;
+    if (!ext_zbits_host) return DKS_OK;
+    REQUIRE(ext_w_host && ext_stride > 0, "dks_explain_host: ext_w / ext_stride missing");
+    size_t need = (size_t)n * ext_stride;
+    if (need > ctx->d_extw.size()) { CUDA_TRY(ctx->d_extz.alloc(need)); CUDA_TRY(ctx->d_extw.alloc(need)); }
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_extz, ext_zbits_host, sizeof(uint64_t) * need, cudaMemcpyHostToDevice, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(ctx->d_extw, ext_w_host, sizeof(double) * need, cudaMemcpyHostToDevice, ctx->stream));
+    *dz = ctx->d_extz; *dw = ctx->d_extw;
+    return DKS_OK;
+}
+
+// d_phi [C][n][G] of the call just enqueued into phi_host and the status word back; synchronises
+static int phi_to_host(dks_ctx* ctx, int n, double* phi_host) {
+    const size_t need_phi = (size_t)ctx->C * n * ctx->G;
     ctx->phi_rows = n;                      // dks_summarise_host works off this buffer
     // results travel through a pinned staging buffer: one asynchronous DMA + one host memcpy instead of the driver's
     // chunked pageable path (the caller's array is ordinary NumPy memory)
@@ -2948,6 +3013,183 @@ int dks_explain_host(dks_ctx* ctx, const double* X_host, int n, double* phi_host
     CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (!direct) memcpy(phi_host, ctx->h_phi_pin, sizeof(double) * need_phi);
     return check_status(ctx);
+}
+
+int dks_explain_host(dks_ctx* ctx, const double* X_host, int n, double* phi_host, const uint64_t* ext_zbits_host,
+                     const double* ext_w_host, int ext_stride) {
+    BIND(ctx);
+    REQUIRE(ctx->fitted, "dks_explain_host: call dks_fit first");
+    REQUIRE(X_host && phi_host && n > 0, "dks_explain_host: bad arguments");
+    TRY(dks_prepare_host(ctx, X_host, n));
+    size_t need_phi = (size_t)ctx->C * n * ctx->G;
+    if (need_phi > ctx->d_phi.size()) CUDA_TRY(ctx->d_phi.alloc(need_phi));
+    const uint64_t* dz; const double* dw;
+    TRY(stage_ext_plans(ctx, n, ext_zbits_host, ext_w_host, ext_stride, &dz, &dw));
+    TRY(launch_explain(ctx, ctx->d_phi, dz, dw, ext_stride));
+    return phi_to_host(ctx, n, phi_host);
+}
+
+// ---- a model the caller evaluates (DKS_ACT_EXTERNAL, dks_external.cuh) -------------------------------------------------
+static int external_dtype(int dtype, const char* what) {
+    if (dtype != DKS_EXTERNAL_FLOAT32 && dtype != DKS_EXTERNAL_FLOAT64)
+        return fail(DKS_ERR_UNSUPPORTED, "%s: dtype %d; DKS_EXTERNAL_FLOAT32 or DKS_EXTERNAL_FLOAT64 only", what, dtype);
+    return DKS_OK;
+}
+
+int dks_set_external_model(dks_ctx* ctx, int C, int scalar_out, int dtype) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_external_model: call dks_set_background first (D unknown)");
+    if (C < 1 || C > DKS_ENS_MAX_OUT)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_external_model: C=%d outputs; 1..%d supported", C, DKS_ENS_MAX_OUT);
+    REQUIRE(!scalar_out || C == 1, "dks_set_external_model: a scalar output is one output (C=%d)", C);
+    TRY(external_dtype(dtype, "dks_set_external_model"));
+    ctx->ext_in_f64 = dtype == DKS_EXTERNAL_FLOAT64;
+    ctx->d_ext_bgy.reset();
+    return set_own_model(ctx, DKS_ACT_EXTERNAL, C, scalar_out);
+}
+
+int dks_set_external_background(dks_ctx* ctx, const void* y_dev, int y_dtype) {
+    BIND(ctx);
+    REQUIRE(ctx->act == DKS_ACT_EXTERNAL, "dks_set_external_background: call dks_set_external_model first");
+    REQUIRE(y_dev, "dks_set_external_background: y is NULL");
+    TRY(external_dtype(y_dtype, "dks_set_external_background"));
+    const int N = ctx->N, C = ctx->C;
+    CUDA_TRY(ctx->d_ext_bgy.alloc((size_t)N * C));
+    dks::ext::external_load_kernel<<<cdiv(N, 128), 128, 0, ctx->stream>>>(y_dev, y_dtype == DKS_EXTERNAL_FLOAT64, N, C,
+                                                                         ctx->link, nullptr, ctx->d_ext_bgy, nullptr, nullptr);
+    ctx->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));       // the caller may free y_dev once this returns
+    ctx->fitted = false;
+    return DKS_OK;
+}
+
+// what an external call's steps after dks_external_begin depend on: the rows, the phi buffer, the options that decide the
+// route and plans, the epoch (fit, plans, l1 tables, buffers moved) and the stream
+static dks_ctx::GraphKey external_key(const dks_ctx* ctx) {
+    return {ctx->cur_X, ctx->d_phi.get(), ctx->cur_n, ctx->nsamples_req, ctx->kernel_choice, ctx->plan_mode,
+            ctx->row_offset, (unsigned long long)ctx->sampler_seed, ctx->epoch, ctx->stream};
+}
+
+// the call dks_external_begin laid out is still the one the context would run
+static int require_begun(dks_ctx* ctx, const char* what) {
+    REQUIRE(ctx->ext_coalitions >= 0 && ctx->prepared, "%s: call dks_external_begin first", what);
+    if (!(external_key(ctx) == ctx->ext_key)) {
+        ctx->ext_coalitions = -1;
+        return fail(DKS_ERR_INVALID, "%s: the rows, plans, options, stream or fit changed since dks_external_begin; "
+                    "prepare and begin the call again", what);
+    }
+    return DKS_OK;
+}
+
+static int require_external(dks_ctx* ctx, const char* what) {
+    REQUIRE(ctx->fitted && ctx->act == DKS_ACT_EXTERNAL, "%s: needs a fitted context with a module (dks_set_external_model, "
+            "dks_fit)", what);
+    return DKS_OK;
+}
+
+int dks_external_prepare(dks_ctx* ctx, const double* X_dev, int n, const void* fx_dev, int fx_dtype) {
+    BIND(ctx);
+    TRY(require_external(ctx, "dks_external_prepare"));
+    REQUIRE(X_dev && fx_dev && n > 0, "dks_external_prepare: need X, the module's outputs on it and n > 0");
+    TRY(external_dtype(fx_dtype, "dks_external_prepare"));
+    ctx->ext_coalitions = -1;
+    ctx->ext_y = fx_dev; ctx->ext_y_f64 = fx_dtype == DKS_EXTERNAL_FLOAT64;
+    const int rc = launch_prepare(ctx, X_dev, n);
+    ctx->ext_y = nullptr;                   // the caller's buffer: read by the launch just enqueued, not kept
+    return rc;
+}
+
+int dks_external_begin(dks_ctx* ctx, const uint64_t* ext_zbits_host, const double* ext_w_host, int ext_stride,
+                       int64_t* rows_total) {
+    BIND(ctx);
+    TRY(require_external(ctx, "dks_external_begin"));
+    REQUIRE(ctx->prepared && rows_total, "dks_external_begin: call dks_external_prepare first");
+    const int n = ctx->cur_n;
+    ctx->ext_coalitions = -1;
+    const size_t need_phi = (size_t)ctx->C * n * ctx->G;
+    if (need_phi > ctx->d_phi.size()) CUDA_TRY(ctx->d_phi.alloc(need_phi));
+    const uint64_t* dz; const double* dw;
+    TRY(stage_ext_plans(ctx, n, ext_zbits_host, ext_w_host, ext_stride, &dz, &dw));
+    Route rt;
+    ExplainParams p;
+    TRY(explain_setup(ctx, ctx->d_phi, dz, dw, ext_stride, &rt, &p));
+    TRY(grow(ctx, ctx->d_ens_ey, (size_t)n * ctx->C * p.S_cap));
+    TRY(grow(ctx, ctx->d_ext_soff, (size_t)n + 1));
+    dks::ext::external_offsets_kernel<<<1, dks::ext::SCAN_THREADS, 0, ctx->stream>>>(p, ctx->d_ext_soff);
+    ctx->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    long long total = 0;
+    CUDA_TRY(cudaMemcpyAsync(&total, ctx->d_ext_soff.get() + n, sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaMemcpyAsync(ctx->h_status, ctx->d_status, sizeof(int) * 2, cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    TRY(check_status(ctx));
+    ctx->ext_p = p;
+    ctx->ext_call_z = dz; ctx->ext_call_stride = ext_stride;
+    ctx->ext_coalitions = total;
+    ctx->ext_key = external_key(ctx);
+    *rows_total = (int64_t)total * ctx->N;
+    return DKS_OK;
+}
+
+// the coalitions [*q0, *q1) of rows row0 .. row0 + rows - 1 of the call dks_external_begin laid out
+static int external_rows(dks_ctx* ctx, const char* what, int64_t row0, int64_t rows, const void* buf, long long* q0,
+                         long long* q1) {
+    BIND(ctx);
+    TRY(require_external(ctx, what));
+    TRY(require_begun(ctx, what));
+    const int64_t N = ctx->N;
+    REQUIRE(buf && rows > 0 && row0 >= 0 && row0 % N == 0 && rows % N == 0 && row0 + rows <= ctx->ext_coalitions * N,
+            "%s: rows %lld .. %lld are not whole coalitions of N=%lld rows within the call's %lld rows", what,
+            (long long)row0, (long long)(row0 + rows), (long long)N, (long long)(ctx->ext_coalitions * N));
+    *q0 = row0 / N; *q1 = (row0 + rows) / N;
+    return DKS_OK;
+}
+
+int dks_external_mask(dks_ctx* ctx, int64_t row0, int64_t rows, void* out_dev) {
+    long long q0, q1;
+    TRY(external_rows(ctx, "dks_external_mask", row0, rows, out_dev, &q0, &q1));
+    const int grid = cdiv(q1 - q0, dks::ext::MASK_COALITIONS);
+    const cudaStream_t st = ctx->stream;
+    if (ctx->ext_in_f64)
+        dks::ext::external_mask_kernel<double><<<grid, dks::ext::MASK_THREADS, 0, st>>>(
+            ctx->ext_p, ctx->d_ext_soff, q0, q1, ctx->cur_X, ctx->d_bg, ctx->D, ctx->d_ext_colgrp, (double*)out_dev);
+    else
+        dks::ext::external_mask_kernel<float><<<grid, dks::ext::MASK_THREADS, 0, st>>>(
+            ctx->ext_p, ctx->d_ext_soff, q0, q1, ctx->cur_X, ctx->d_bg, ctx->D, ctx->d_ext_colgrp, (float*)out_dev);
+    ctx->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    return DKS_OK;
+}
+
+int dks_external_reduce(dks_ctx* ctx, int64_t row0, int64_t rows, const void* y_dev, int y_dtype) {
+    long long q0, q1;
+    TRY(external_rows(ctx, "dks_external_reduce", row0, rows, y_dev, &q0, &q1));
+    TRY(external_dtype(y_dtype, "dks_external_reduce"));
+    constexpr int wpc = dks::ext::REDUCE_THREADS / 32;
+    const int grid = (int)std::min<long long>(cdiv(q1 - q0, wpc), (long long)ctx->sm_count * 16);
+    const ExplainParams& p = ctx->ext_p;
+    if (y_dtype == DKS_EXTERNAL_FLOAT64)
+        dks::ext::external_reduce_kernel<double><<<grid, dks::ext::REDUCE_THREADS, 0, ctx->stream>>>(
+            ctx->d_ext_soff, p.n, ctx->N, ctx->C, p.S_cap, q0, q1, (const double*)y_dev, ctx->d_wbg, ctx->d_ens_ey);
+    else
+        dks::ext::external_reduce_kernel<float><<<grid, dks::ext::REDUCE_THREADS, 0, ctx->stream>>>(
+            ctx->d_ext_soff, p.n, ctx->N, ctx->C, p.S_cap, q0, q1, (const float*)y_dev, ctx->d_wbg, ctx->d_ens_ey);
+    ctx->launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    return DKS_OK;
+}
+
+int dks_external_finish(dks_ctx* ctx, double* phi_host) {
+    BIND(ctx);
+    TRY(require_external(ctx, "dks_external_finish"));
+    REQUIRE(phi_host, "dks_external_finish: phi is NULL");
+    TRY(require_begun(ctx, "dks_external_finish"));
+    ctx->ext_coalitions = -1;
+    Route rt;                               // the route begin chose (the same state decides it; nothing is launched)
+    TRY(choose_route(ctx, ctx->ext_call_z, ctx->ext_call_stride, &rt));
+    TRY(explain_launch(ctx, rt, ctx->ext_p));
+    return phi_to_host(ctx, ctx->cur_n, phi_host);
 }
 
 int dks_summarise_host(dks_ctx* ctx, int n, const int32_t* seg_offsets_host, int Gp, double* phi_sum_host,

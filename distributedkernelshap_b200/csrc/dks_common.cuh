@@ -432,6 +432,21 @@ struct dks_ctx {
     const double* d_ens_pi = nullptr;
     DevBuf<double> d_ens_out, d_ens_ey;
     dks_ctx* ens_parent = nullptr;
+    // a module the caller runs (act == DKS_ACT_EXTERNAL, dks_set_external_model): the dtype of its input rows, its outputs on
+    // the background in float64 (dks_set_external_background), the group of every column (d_ext_colgrp, fit_pool), the
+    // outputs stage 1 reads while dks_external_prepare runs (the caller's memory), and the call dks_external_begin laid
+    // out: its explain parameters, the plans it was given, the coalition offsets [n + 1] and their total (-1: none; also
+    // the next stage 1 and dks_fit drop it), and ext_key below.  The background means ey go to d_ens_ey.
+    int ext_in_f64 = 1;
+    DevBuf<double> d_ext_bgy;
+    const int32_t* d_ext_colgrp = nullptr;
+    const void* ext_y = nullptr;
+    int ext_y_f64 = 1;
+    ExplainParams ext_p = {};
+    const uint64_t* ext_call_z = nullptr;
+    int ext_call_stride = 0;
+    DevBuf<long long> d_ext_soff;
+    long long ext_coalitions = -1;
     // every device array dks_fit builds that a by-value kernel struct points at (the pointers of tree, km, mlp, knn, enc, cm,
     // d_bg_enc, d_egoff, d_egcols, d_ens_pi), freed together by the next dks_fit or with the context.  No kernel reads one
     // after that: freeing clears fitted and prepared, and every launch needs them.
@@ -532,6 +547,8 @@ struct dks_ctx {
     bool capturing = false;
     bool have_last_key = false;
     GraphKey last_key{}, graph_key{};
+    GraphKey ext_key{};           // the rows, plans, options, epoch and stream dks_external_begin laid its call out for: the
+                                  // steps after it refuse to run when anything of it changed since
     cudaGraphExec_t gexec = nullptr;
     unsigned epoch = 0;           // bumped by everything that changes what the sequence launches (fit, plans, ...)
     int64_t graph_launches = 0;

@@ -34,12 +34,14 @@ __host__ __device__ inline size_t tail_smem_bytes(int S_cap, int C) {
 }
 
 // One CTA per instance (grid-stride) over the list the members ran on.  M = 0 and M = 1 from the ensemble's dlink; else
-// y = link(ey) - link(fnull) for every output (each solved on its own, as shap does; under the logit 1 - ey_c is the sum of
-// the other outputs' ey, no cancellation), then the CUDA-core kernel's constrained WLS, or (L1) the moments of y for
-// l1_lars_kernel.  A non-finite y or f(x) is reported as DKS_ERR_NUMERIC and nothing of the instance is written.
+// y = link(ey) - link(fnull) for every output (each solved on its own, as shap does), then the CUDA-core kernel's
+// constrained WLS, or (L1) the moments of y for l1_lars_kernel.  Under the logit 1 - ey_c is, for a soft-voting ensemble
+// of probabilities that sum to one, the sum of the other outputs' ey (no cancellation); with `complement` (a model whose
+// outputs need not sum to one, dks_external.cuh) it is 1 - ey_c itself, the elementwise logit stage 1 and fnull take.  A
+// non-finite y or f(x) is reported as DKS_ERR_NUMERIC and nothing of the instance is written.
 template <bool L1>
 __global__ void __launch_bounds__(THREADS) explain_ensemble_tail_kernel(ExplainParams p, SimtL1 q,
-                                                                        const double* __restrict__ ey) {
+                                                                        const double* __restrict__ ey, int complement) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x;
     const int G = p.G, C = p.C;
@@ -81,7 +83,7 @@ __global__ void __launch_bounds__(THREADS) explain_ensemble_tail_kernel(ExplainP
                 double v;
                 if (p.link == DKS_LINK_LOGIT) {
                     double rest = 0.0;
-                    if (C == 1) rest = 1.0 - ec;
+                    if (C == 1 || complement) rest = 1.0 - ec;
                     else for (int c2 = 0; c2 < C; ++c2) if (c2 != c) rest += e[(size_t)c2 * p.S_cap + s];
                     v = log(ec / rest) - p.linkfnull[c];
                 } else {

@@ -20,6 +20,8 @@ from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, KernelMachineSpec, 
 from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, MlpSpec, extract_mlp_spec
 from .neighbors import MAX_GROUPS as KNN_MAX_GROUPS, KnnSpec, extract_knn_spec
 from .predictors import extract_linear_spec
+from . import torch_models
+from .torch_models import TorchModelSpec
 from .trees import MAX_GROUPS as TREE_MAX_GROUPS, TreeEnsembleSpec, extract_encoded_pipeline_spec, \
     extract_tree_pipeline_spec, extract_tree_spec
 
@@ -132,6 +134,12 @@ def l1_selecting_sizes(l1_reg, nsamples, G, hist):
     return mode, k, sizes
 
 
+def _dtype_code(t):
+    """``DKS_EXTERNAL_FLOAT32`` / ``_FLOAT64`` of a float32 / float64 tensor."""
+    import torch
+    return _cabi.EXTERNAL_FLOAT64 if t.dtype == torch.float64 else _cabi.EXTERNAL_FLOAT32
+
+
 class GpuKernelExplainer:
     """CUDA KernelSHAP explainer with the interface of ``shap.KernelExplainer`` / ``KernelExplainerWrapper``.
 
@@ -148,7 +156,10 @@ class GpuKernelExplainer:
         (``trees.extract_encoded_pipeline_spec``, replayed like a tree's); a soft ``VotingClassifier`` or a
         ``VotingRegressor`` mixing those families with linear members, bare or behind such a ``Pipeline``
         (``ensembles.extract_ensemble_spec``).  A raw value the pipeline would refuse (NaN, or an unseen category under
-        ``handle_unknown='error'``) raises ``ValueError``.
+        ``handle_unknown='error'``) raises ``ValueError``.  Or a ``torch.nn.Module`` in eval mode on one CUDA device,
+        float32 or float64, mapping [B, D] to [B] or [B, C <= 8] (``torch_models.TorchModelSpec``): the engine builds the
+        masked rows on the device, the module runs on them and the engine reduces its outputs and solves (up to 64
+        groups, no column encoding, no ``explain_device``).
     data
         Background data: array, DataFrame or ``DenseData`` (groups and weights honoured).
     link
@@ -157,10 +168,14 @@ class GpuKernelExplainer:
         As in ``KernelExplainerWrapper.__init__`` (kernel_shap.py:225-228): seeds the global legacy NumPy stream the
         sampled part of the coalition plans is drawn from.
     device
-        CUDA device ordinal (default: ``LOCAL_RANK`` under torchrun, else 0).
+        CUDA device ordinal (default: ``LOCAL_RANK`` under torchrun, else 0; a module's own device).
+    model_batch_rows
+        A module only: masked rows per module call (default 2^20), rounded down to whole coalitions of the background,
+        at least one.  The module's activation memory grows with it.
     """
 
-    def __init__(self, model, data, link="identity", seed=None, device=None, kernel="auto", plan_mode="shared", **kwargs):
+    def __init__(self, model, data, link="identity", seed=None, device=None, kernel="auto", plan_mode="shared",
+                 model_batch_rows=None, **kwargs):
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         if plan_mode not in ("shared", "per_instance"):
@@ -173,19 +188,30 @@ class GpuKernelExplainer:
         self.lib = _cabi.load()
         self.link = convert_to_link(link)
         self.model_callable = model
-        # a soft-voting ensemble of the families below (bare: its spec; behind per-column preprocessing: with the encoding)
-        ens = extract_ensemble_spec(model)
-        pipe_spec = ens if isinstance(ens, tuple) else None
-        if ens is None:
-            pipe_spec = extract_tree_pipeline_spec(model)
-            if pipe_spec is None:
-                pipe_spec = extract_encoded_pipeline_spec(model)
+        torch_models.refuse_module_in_pipeline(model)
+        if torch_models.is_torch_module(model):
+            # a module: recognised and checked here, run on the background below
+            if kernel not in ("auto", "simt"):
+                raise NotImplementedError(f"kernel={kernel!r}: a torch module runs on the module route (kernel 'auto' or "
+                                          "'simt')")
+            ens, pipe_spec = None, None
+        else:
+            # a soft-voting ensemble of the families below (bare: its spec; behind per-column preprocessing: with the
+            # encoding)
+            ens = extract_ensemble_spec(model)
+            pipe_spec = ens if isinstance(ens, tuple) else None
+            if ens is None:
+                pipe_spec = extract_tree_pipeline_spec(model)
+                if pipe_spec is None:
+                    pipe_spec = extract_encoded_pipeline_spec(model)
         # a model behind per-column preprocessing: explained in raw feature space, the device replaying the steps; the
         # extractors below pass its spec through
         target, self.encoding = pipe_spec if pipe_spec is not None else (model if ens is None else ens, None)
         # the model families with their own kernels: the first extractor that reads the model wins; the family's kernels
         # cover at most max_groups groups.  Built per construction, so the module's extractors are looked up when it runs.
-        families = ((lambda t: t if isinstance(t, EnsembleSpec) else None, ENSEMBLE_MAX_GROUPS, "soft-voting ensembles"),
+        families = ((lambda t: TorchModelSpec(t) if torch_models.is_torch_module(t) else None, torch_models.MAX_GROUPS,
+                     "torch modules"),
+                    (lambda t: t if isinstance(t, EnsembleSpec) else None, ENSEMBLE_MAX_GROUPS, "soft-voting ensembles"),
                     (extract_tree_spec, TREE_MAX_GROUPS, "tree ensembles"),
                     (extract_kernel_machine_spec, KMACH_MAX_GROUPS, "kernel machines"),
                     (extract_mlp_spec, MLP_MAX_GROUPS, "MLPs"),
@@ -208,6 +234,16 @@ class GpuKernelExplainer:
         if bg.ndim != 2:
             raise TypeError("background data must be two-dimensional")
         self.N, self.P = bg.shape
+        self._bg_outputs = None
+        if isinstance(own, TorchModelSpec):
+            if self.data.groups_size > max_groups:
+                raise NotImplementedError(f"{self.data.groups_size} groups: {family} are explained up to {max_groups} "
+                                          "groups")
+            if device is not None and int(device) != own.device:
+                raise ValueError(f"device={device}: the module is on cuda:{own.device}")
+            device = own.device
+            self._bg_outputs = own.bind_background(bg)
+            self.model_batch_rows = torch_models.model_batch_rows(model_batch_rows, self.N)
         if self.spec.n_features != self.P:
             raise ValueError(f"model expects {self.spec.n_features} columns, background has {self.P}")
         if self.N > 100:
@@ -221,6 +257,9 @@ class GpuKernelExplainer:
 
         self._ctx = C.c_void_p()
         _cabi.check(self.lib.dks_create(C.byref(self._ctx), self.device))
+        self._stream = None
+        if isinstance(own, TorchModelSpec):
+            self._bind_torch_stream()           # the background outputs are read on torch's stream
         weights = np.ascontiguousarray(self.data.weights, dtype=np.float64)
         _cabi.check(self.lib.dks_set_background(self._ctx, _cabi.ptr(bg), self.N, self.P, _cabi.ptr(weights)))
         offsets = np.zeros(self.data.groups_size + 1, dtype=np.int32)
@@ -235,6 +274,11 @@ class GpuKernelExplainer:
         self._set_encoding(self._ctx)   # before the model: its columns are the encoded ones
         if isinstance(own, EnsembleSpec):
             self._set_ensemble(own, bg, weights)
+        elif isinstance(own, TorchModelSpec):
+            _cabi.check(self.lib.dks_set_external_model(self._ctx, own.n_outputs, int(own.scalar_out), own.dtype_code))
+            y = self._bg_outputs
+            _cabi.check(self.lib.dks_set_external_background(self._ctx, C.c_void_p(y.data_ptr()), _dtype_code(y)))
+            self._bg_outputs = None
         elif own is not None:
             self._set_own_model(self._ctx, own)
         elif self.spec.activation == "mixture":
@@ -270,7 +314,17 @@ class GpuKernelExplainer:
         self._last_rows = 0
         if self.encoding is not None:
             self._check_encoding(bg)
-        self._check_model_against_callable(bg, own if isinstance(own, (KnnSpec, EnsembleSpec)) else None)
+        if not isinstance(own, TorchModelSpec):     # a module's outputs are the module's: nothing was extracted
+            self._check_model_against_callable(bg, own if isinstance(own, (KnnSpec, EnsembleSpec)) else None)
+
+    def _bind_torch_stream(self):
+        """A module: the engine enqueues on torch's current stream of the module's device, so the masked rows, the module
+        and the reduction run in order without host synchronisation."""
+        import torch
+        stream = torch.cuda.current_stream(torch.device("cuda", self.device)).cuda_stream
+        if stream != self._stream:
+            self.set_stream(stream)
+            self._stream = stream
 
     def _set_encoding(self, ctx):
         e = self.encoding
@@ -389,7 +443,9 @@ class GpuKernelExplainer:
                              f"{np.max(np.abs(got - want)) if want.shape == got.shape else 'shape mismatch'})")
 
     def predict(self, X):
-        """Model outputs [n, C] computed on the GPU in float64."""
+        """Model outputs [n, C] computed on the GPU in float64 (a module: its own outputs, in float64)."""
+        if isinstance(self.spec, TorchModelSpec):
+            return self.spec.predict(np.atleast_2d(np.asarray(X, dtype=np.float64)))
         X = np.ascontiguousarray(np.atleast_2d(np.asarray(X, dtype=np.float64)))
         out = np.zeros((X.shape[0], self.D))
         _cabi.check(self.lib.dks_predict_host(self._ctx, _cabi.ptr(X), X.shape[0], _cabi.ptr(out)))
@@ -568,7 +624,9 @@ class GpuKernelExplainer:
         if self.plan_mode == "per_instance":
             # the device draws each row's plan from (seed, global row index): tell it where this block starts
             _cabi.check(self.lib.dks_set_row_offset(self._ctx, row_offset))
-        if plans is not None:
+        if isinstance(self.spec, TorchModelSpec):
+            self._explain_module(X, phi, nsamples, l1_reg, plans, need_hist)
+        elif plans is not None:
             if G > 64:
                 raise NotImplementedError("caller-supplied per-instance plans need at most 64 groups (multi-word coalition "
                                           "rows exist on the shared-plan path only)")
@@ -603,6 +661,56 @@ class GpuKernelExplainer:
             return [phi[c, 0] for c in range(self.D)]
         return [phi[c] for c in range(self.D)]
 
+    def _explain_module(self, X, phi, nsamples, l1_reg, plans, need_hist):
+        """One block of rows through a module: stage 1 on the module's outputs, the plans (and the l1 decision), then
+        mask -> module -> reduce per block of ``model_batch_rows`` masked rows into one reused input tensor, then the
+        solve into ``phi``."""
+        import torch
+        n, G, spec = X.shape[0], self.data.groups_size, self.spec
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(dev), torch.inference_mode():
+            self._bind_torch_stream()
+            X_dev = torch.from_numpy(X).to(dev)             # read by every mask launch until finish returns
+            fx = spec.outputs(X_dev.to(spec.dtype))
+            _cabi.check(self.lib.dks_external_prepare(self._ctx, C.c_void_p(X_dev.data_ptr()), n,
+                                                      C.c_void_p(fx.data_ptr()), _dtype_code(fx)))
+            zb = w = None
+            stride = 0
+            if plans is not None:
+                zb, w, stride = self._pack_external_plans(plans, n, nsamples)
+                if need_hist and l1_selecting_sizes(l1_reg, nsamples, G, self.m_histogram())[2]:
+                    raise NotImplementedError("l1 feature selection runs on the engine's shared plans, not on "
+                                              "caller-supplied per-instance plans -- pass l1_reg=False")
+                self._apply_l1(False, nsamples, None)
+            elif need_hist:
+                hist = self.m_histogram()
+                self._ensure_shared_plans(hist, nsamples)
+                self._apply_l1(l1_reg, nsamples, hist)
+            else:
+                self._apply_l1(False, nsamples, None)
+            total = C.c_int64(0)
+            rc = self.lib.dks_external_begin(self._ctx, _cabi.ptr(zb), _cabi.ptr(w), stride, C.byref(total))
+            if rc == _cabi.DKS_ERR_PLAN_MISSING:
+                # first call (or a new M): build the missing plans from the M histogram and lay the call out again
+                self._ensure_shared_plans(self.m_histogram(), nsamples)
+                rc = self.lib.dks_external_begin(self._ctx, _cabi.ptr(zb), _cabi.ptr(w), stride, C.byref(total))
+            _cabi.check(rc)
+            blocks = torch_models.plan_blocks(total.value, self.N, self.model_batch_rows)
+            rows_in = torch.empty((blocks[0][1] if blocks else 0, self.P), dtype=spec.dtype, device=dev)
+            for row0, rows in blocks:
+                x = rows_in[:rows]
+                _cabi.check(self.lib.dks_external_mask(self._ctx, row0, rows, C.c_void_p(x.data_ptr())))
+                y = spec.outputs(x)
+                _cabi.check(self.lib.dks_external_reduce(self._ctx, row0, rows, C.c_void_p(y.data_ptr()),
+                                                         _dtype_code(y)))
+            _cabi.check(self.lib.dks_external_finish(self._ctx, _cabi.ptr(phi)))
+
+    def _refuse_module(self, what):
+        if isinstance(self.spec, TorchModelSpec):
+            raise NotImplementedError(f"{what}: a torch module runs between the engine's launches, so it cannot be "
+                                      "explained from device rows in one enqueued sequence or replayed as a CUDA graph; "
+                                      "use shap_values")
+
     def _rows_per_call(self):
         """Rows per C-ABI call (``rows_per_call``); a column encoding also bounds the encoded rows of a call by
         ``MAX_ENCODED_BYTES_PER_CALL`` (results are per row and device plans keyed by the global row: the block size
@@ -610,8 +718,9 @@ class GpuKernelExplainer:
         rows = rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size, self.spec.R)
         if self.encoding is not None:
             rows = min(rows, max(1, MAX_ENCODED_BYTES_PER_CALL // (8 * self.encoding.E)))
-        if isinstance(self.spec, EnsembleSpec):
-            # the members' weighted background means: C outputs x S rows per instance, S at most that of all G groups
+        if isinstance(self.spec, (EnsembleSpec, TorchModelSpec)):
+            # the members' weighted background means (or the module's): C outputs x S rows per instance, S at most that
+            # of all G groups
             S, _ = resolve_nsamples(self.data.groups_size, self._nsamples_req or "auto")
             rows = min(rows, max(1, MAX_ENSEMBLE_BYTES_PER_CALL // (8 * self.D * (S + 2))))
         return rows
@@ -694,6 +803,7 @@ class GpuKernelExplainer:
         """Asynchronously explain ``n`` rows resident in device memory (float64 [n, D] at ``X_dev_ptr``) into the device
         buffer ``phi_dev_ptr`` (float64 [C, n, G]) using the shared plans already on the device.  Call ``check_status()``
         after synchronising to learn about missing plans / numerical failures."""
+        self._refuse_module("explain_device")
         self._set_nsamples(nsamples)
         self._apply_l1(False, nsamples, None)             # the device-resident call is the plain constrained WLS
         _cabi.check(self.lib.dks_run_dev(self._ctx, C.c_void_p(int(X_dev_ptr)), int(n), C.c_void_p(int(phi_dev_ptr))))
@@ -702,6 +812,7 @@ class GpuKernelExplainer:
         """Explain host rows ``X`` and leave the shap values ON THE DEVICE: returns a float64 CUDA tensor ``[C, n, G]``
         (torch owns the buffers; the engine sees raw pointers).  Used by the SPMD path of ``DistributedExplainer`` so that
         the all-gather runs on what the solve wrote, without a host round trip.  Zero rows give an empty tensor."""
+        self._refuse_module("explain_block_to_device")
         import torch
         X = np.ascontiguousarray(np.atleast_2d(np.asarray(X, dtype=np.float64)))
         n, G = X.shape[0], self.data.groups_size
@@ -796,7 +907,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", None, "softmax", "affine", "ovr", "exp", "mixture"),   # 3: not used
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble", "torch"),
     }
 
     def last_path(self):
@@ -810,7 +921,8 @@ class GpuKernelExplainer:
         kernel, which takes every instance of a tree ensemble, 'kmach': the kernel-machine kernel, which takes every
         instance of a kernel machine, 'mlp': the MLP kernel, which takes every instance of a multi-layer perceptron, or
         'knn': the neighbour kernel, which takes every instance of a k-nearest-neighbour model, or 'ensemble': the
-        members' kernels and the ensemble's tail, which take every instance of a soft-voting ensemble),
+        members' kernels and the ensemble's tail, which take every instance of a soft-voting ensemble, or 'torch': the
+        ensemble's tail on the background means of a module's outputs, every instance of a module),
         ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take
@@ -822,7 +934,7 @@ class GpuKernelExplainer:
         _cabi.check(self.lib.dks_last_path(self._ctx, _cabi.ptr(out), len(out)))
         names = self._PATH_NAMES
         general = names["general"][out[8]]
-        if out[12] and self._l1_general_all_select:
+        if out[12] and self._l1_general_all_select and general != "torch":
             general = "simt"
         return {"shared": names["shared"][out[0]], "chunks": int(out[1]), "warps": int(out[2]), "grid": int(out[3]),
                 "fused_B": int(out[4]), "fused_NI": int(out[5]), "solve": names["solve"][out[6]],

@@ -22,6 +22,7 @@ from distributedkernelshap_b200 import data as shap_data
 from distributedkernelshap_b200.data import Data, DenseData, DenseDataWithIndex, convert_to_link
 from distributedkernelshap_b200.engine import GpuKernelExplainer
 from distributedkernelshap_b200.explainers.distributed import DistributedExplainer
+from distributedkernelshap_b200.torch_models import is_torch_module
 from distributedkernelshap_b200.explainers.interface import (DEFAULT_DATA_KERNEL_SHAP, DEFAULT_META_KERNEL_SHAP,
                                                               Explainer, Explanation, FitMixin)
 
@@ -148,7 +149,8 @@ class KernelShap(Explainer, FitMixin):
                  task: str = 'classification',
                  seed: int = None,
                  distributed_opts: Optional[Dict] = None,
-                 plan_mode: str = 'shared'):
+                 plan_mode: str = 'shared',
+                 model_batch_rows: Optional[int] = None):
         """KernelSHAP explainer with grouping of encoded categorical variables; see the reference docstring
         (kernel_shap.py:274-337) for parameter semantics -- they are unchanged.
 
@@ -158,7 +160,11 @@ class KernelShap(Explainer, FitMixin):
 
         ``plan_mode`` (not in the reference): ``'shared'`` evaluates one coalition plan per number of varying groups for
         all instances (drawn on the host from the seeded NumPy stream); ``'per_instance'`` draws a fresh plan for every
-        instance on the GPU, as shap does on the CPU, from a counter-based stream keyed by (seed, row index)."""
+        instance on the GPU, as shap does on the CPU, from a counter-based stream keyed by (seed, row index).
+
+        ``predictor`` may also be a ``torch.nn.Module`` on a CUDA device (see ``GpuKernelExplainer``); ``model_batch_rows``
+        (not in the reference) then caps the masked rows per module call.  A module is explained on one GPU: it cannot
+        be combined with ``distributed_opts``."""
         super().__init__(meta=copy.deepcopy(DEFAULT_META_KERNEL_SHAP))
 
         self.link = link
@@ -177,6 +183,11 @@ class KernelShap(Explainer, FitMixin):
         self.summarise_result = False      # sum shap values over encoded levels after the fact
         self.summarise_background = False  # background was subsampled / clustered
         self._fitted = False
+        self.model_batch_rows = model_batch_rows
+        if distributed_opts and is_torch_module(predictor):
+            raise NotImplementedError("distributed_opts with a torch.nn.Module: the pool replicates the explainer on "
+                                      "every GPU, and moving a module between devices is not supported; explain it on "
+                                      "its own device without distributed_opts")
         self.distributed_opts = copy.deepcopy(DISTRIBUTED_OPTS)
         if distributed_opts:
             self.distributed_opts.update(distributed_opts)
@@ -403,6 +414,8 @@ class KernelShap(Explainer, FitMixin):
         explainer_kwargs = {'link': self.link, 'seed': self.seed}
         if self.plan_mode != 'shared':
             explainer_kwargs.update(plan_mode=self.plan_mode)
+        if self.model_batch_rows is not None:
+            explainer_kwargs.update(model_batch_rows=self.model_batch_rows)
         if self.distribute:
             self._explainer = DistributedExplainer(
                 self.distributed_opts,
@@ -499,7 +512,9 @@ class KernelShap(Explainer, FitMixin):
         # interpreted per-element loop; both links are NumPy ufunc expressions, so they are applied to the array)
         raw_predictions = kwargs.get('link_predictions')
         if raw_predictions is None:
-            raw_predictions = convert_to_link(self.link).f(np.asarray(self.predictor(X), dtype=np.float64))
+            # a module takes device tensors, not the NumPy rows a callable predictor takes: the explainer runs it
+            predict = self._explainer.predict if is_torch_module(self.predictor) else self.predictor
+            raw_predictions = convert_to_link(self.link).f(np.asarray(predict(X), dtype=np.float64))
 
         if device_summary is not None and len(shap_values) + 1 == device_summary['mean_abs'].shape[0]:
             argmax_pred = device_summary['argmax'] if self.task != 'regression' else []

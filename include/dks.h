@@ -139,6 +139,10 @@ extern "C" {
 #define DKS_ACT_ENSEMBLE 10    /* soft-voting ensemble of the four families above: set by dks_set_ensemble only */
 #define DKS_ENS_MAX_MEMBERS 16       /* members of a soft-voting ensemble */
 #define DKS_ENS_MAX_OUT 8            /* its outputs */
+#define DKS_ACT_EXTERNAL 11    /* a model the caller evaluates (a torch.nn.Module on the device): set by dks_set_external_model
+                                * only, explained stepwise by dks_external_* */
+#define DKS_EXTERNAL_FLOAT32 0       /* dtypes of the module's input rows and outputs */
+#define DKS_EXTERNAL_FLOAT64 1
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -276,6 +280,39 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
  * DKS_ERR_DOMAIN with the row (NaN in an ensemble of trees only is explained); a link(ey) or link(f(x)) that is not finite
  * is DKS_ERR_NUMERIC and nothing non-finite is written into phi. */
 int dks_set_ensemble(dks_ctx* ctx, int K, dks_ctx* const* members, const double* weights, int C, int scalar_out);
+/* a model the engine cannot evaluate (DKS_ACT_EXTERNAL) in place of dks_set_model: C (1..DKS_ENS_MAX_OUT) outputs that the
+ * caller computes on the device from rows of `dtype` (DKS_EXTERNAL_FLOAT32 / _FLOAT64) -- a torch.nn.Module (DESIGN.md
+ * §5.0.19).  Before dks_fit, dks_set_external_background hands over the module's outputs on the N background rows, y_dev
+ * [N][C] of y_dtype in device memory, read on the context's stream before the call returns; fnull is their weighted mean.
+ * The engine never calls the module, so dks_predict_host, dks_prepare_*, dks_explain_* and dks_run_dev are
+ * DKS_ERR_UNSUPPORTED; a column encoding or column maps are refused.  An explain call is stepwise, all on the context's
+ * stream (dks_set_stream: the caller's, so that its module runs in order with the engine's kernels):
+ *   dks_external_prepare: stage 1 over the rows X_dev [n][D] (float64, device; kept by the caller until _finish returns)
+ *     with the module's outputs fx_dev [n][C] on them (read before the call returns): varying groups, the M histogram,
+ *     link(f(x)).  dks_get_m_histogram then decides the plans and the l1 selection as for any model.
+ *   dks_external_begin: the route (shared, caller-supplied or device-drawn plans; l1 selection) and the coalition offsets;
+ *     synchronises once and returns in *rows_total the masked rows of the call, sum over instances with M >= 2 of S_i N.
+ *     DKS_ERR_PLAN_MISSING when a shared plan is missing (upload it and call again).
+ *   dks_external_mask: masked rows row0 .. row0 + rows - 1 into out_dev [rows][D] of the module's dtype: row (i, s, j) =
+ *     z_s(group(d)) ? x_i[d] : bg_j[d], rows numbered instances in index order, then coalition s of the instance's plan, then
+ *     background row j; row0 and rows are whole coalitions (multiples of N).
+ *   dks_external_reduce: the module's outputs y_dev [rows][C] (y_dtype) on those rows into the background means
+ *     ey[i][c][s] = sum_j w_j y(i, s, j)_c, summed over j in a fixed order whatever the split into calls.
+ *   dks_external_finish: link + constrained WLS (with l1 selection: moments, LARS, restricted solve) of every instance,
+ *     phi_host [C][n][G] as dks_explain_host writes it (dks_summarise_host and dks_get_link_fx then apply); synchronises.
+ * After dks_external_begin, another stage 1, a dks_fit, a plan or l1 table upload, a change of nsamples, plan mode, row
+ * offset, kernel or stream makes _mask, _reduce and _finish DKS_ERR_INVALID until the call is prepared and begun again.
+ * Under DKS_LINK_LOGIT every output is taken as a probability of its own: y = log(ey_c / (1 - ey_c)) - link(fnull_c), as
+ * for f(x) and fnull, whether or not the outputs sum to one.
+ * Up to 64 groups, kernel 'auto' or 'simt'; a non-finite link(ey), link(f(x)) or link(fnull) is DKS_ERR_NUMERIC. */
+int dks_set_external_model(dks_ctx* ctx, int C, int scalar_out, int dtype);
+int dks_set_external_background(dks_ctx* ctx, const void* y_dev, int y_dtype);
+int dks_external_prepare(dks_ctx* ctx, const double* X_dev, int n, const void* fx_dev, int fx_dtype);
+int dks_external_begin(dks_ctx* ctx, const uint64_t* ext_zbits_host, const double* ext_w_host, int ext_stride,
+                       int64_t* rows_total);
+int dks_external_mask(dks_ctx* ctx, int64_t row0, int64_t rows, void* out_dev);
+int dks_external_reduce(dks_ctx* ctx, int64_t row0, int64_t rows, const void* y_dev, int y_dtype);
+int dks_external_finish(dks_ctx* ctx, double* phi_host);
 /* column maps (call after dks_set_model, before dks_fit): the scores become z_r = b_r + sum_col f_{r,col}(x_col), a linear
  * model behind per-column preprocessing (a scikit-learn Pipeline of scalers, encoders, binning and imputation) read in raw
  * feature space; W is then not read.  Per column, hdr_host[4 col ..] = {flags, m, key offset, value offset}:
@@ -504,6 +541,8 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
 #define DKS_GENERAL_KNN 8        /* explain_knn_kernel: every instance of a nearest-neighbour model (dks_set_knn_model) */
 #define DKS_GENERAL_ENSEMBLE 9   /* the members' explain kernels, then explain_ensemble_tail_kernel: every instance of a
                                   * soft-voting ensemble (dks_set_ensemble) */
+#define DKS_GENERAL_EXTERNAL 10  /* explain_ensemble_tail_kernel on the means dks_external_reduce formed: every instance of a
+                                  * module the caller runs (dks_set_external_model) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
