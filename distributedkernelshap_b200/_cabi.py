@@ -35,6 +35,7 @@ ACT_MLP = 8
 ACT_KNN = 9
 ACT_ENSEMBLE = 10
 ACT_EXTERNAL = 11
+ACT_STACKING = 12
 EXTERNAL_FLOAT32 = 0
 EXTERNAL_FLOAT64 = 1
 LINK_IDENTITY = 0
@@ -66,6 +67,8 @@ SIGNATURES = {
     "dks_set_knn_model": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int, C.c_double, C.c_int,
                                                                              C.c_int, C.c_void_p, C.c_int, C.c_int]),
     "dks_set_ensemble": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "dks_set_stacking": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                   C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64]),
     "dks_set_external_model": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "dks_set_external_background": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     "dks_external_prepare": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]),

@@ -24,6 +24,7 @@
 #include "dks_knn.cuh"
 #include "dks_ensemble.cuh"
 #include "dks_external.cuh"
+#include "dks_stacking.cuh"
 
 namespace {
 
@@ -199,6 +200,11 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         // its own
         h.family = DKS_GENERAL_ENSEMBLE;
         break;
+    case DKS_ACT_STACKING:
+        // no shared-plan route: every instance runs the members' kernels, the final estimator's reduction and the
+        // ensemble's tail; every output is solved on its own
+        h.family = DKS_GENERAL_STACKING;
+        break;
     case DKS_ACT_EXTERNAL:
         // no shared-plan route: the caller's module evaluates the masked rows, every instance runs the ensemble's tail on
         // their background means; every output is solved on its own
@@ -249,7 +255,8 @@ int knn_chunk(const dks_ctx* ctx, int S_cap) {
 
 OwnKernel own_kernel(int family);
 
-// shared memory of the widest launch of a soft-voting ensemble at S_cap rows: a member's explain kernel or the tail
+// shared memory of the widest launch of a soft-voting or stacking ensemble at S_cap rows: a member's explain kernel or the
+// tail (stacking_reduce_kernel's is static and smaller)
 size_t ensemble_smem(const dks_ctx* ctx, int S_cap) {
     size_t smem = dks::ens::tail_smem_bytes(S_cap, ctx->C);
     for (const dks_ctx* m : ctx->ens) smem = std::max(smem, own_kernel(m->head.family).smem(m, S_cap));
@@ -279,6 +286,9 @@ OwnKernel own_kernel(int family) {
     case DKS_GENERAL_ENSEMBLE:          // refuses: what its members refuse (refusing_kernel)
         return {"soft-voting ensembles", "ensemble kernels", "groups", "soft-voting ensemble",
                 " (put the preprocessing in front of the ensemble)", REFUSES_NONE, ensemble_smem};
+    case DKS_GENERAL_STACKING:          // refuses: what its members refuse (refusing_kernel)
+        return {"stacking ensembles", "stacking kernels", "groups", "stacking ensemble",
+                " (put the preprocessing in front of the ensemble)", REFUSES_NONE, ensemble_smem};
     case DKS_GENERAL_EXTERNAL:          // refuses: nothing (the module sees every raw value)
         return {"modules", "module route", "nsamples", "module", " (put the preprocessing inside the module)", REFUSES_NONE,
                 [](const dks_ctx* c, int S_cap) { return dks::ens::tail_smem_bytes(S_cap, c->C); }};
@@ -290,7 +300,7 @@ OwnKernel own_kernel(int family) {
 // model's own
 OwnKernel refusing_kernel(const dks_ctx* ctx) {
     OwnKernel ok = own_kernel(ctx->head.family);
-    if (ctx->head.family != DKS_GENERAL_ENSEMBLE) return ok;
+    if (ctx->head.family != DKS_GENERAL_ENSEMBLE && ctx->head.family != DKS_GENERAL_STACKING) return ok;
     for (const dks_ctx* m : ctx->ens) {
         const OwnKernel mk = own_kernel(m->head.family);
         if (mk.refuses > ok.refuses) ok = mk;
@@ -364,6 +374,12 @@ int check_own_columns(const dks_ctx* ctx, const OwnKernel& ok) {
     case DKS_GENERAL_KMACH: reads = (int)(ctx->h_kcolw.size() / ctx->km.K); break;
     case DKS_GENERAL_MLP: reads = ctx->mlp.width[0]; break;
     case DKS_GENERAL_ENSEMBLE: return DKS_OK;         // each member checks its own (fit_members)
+    case DKS_GENERAL_STACKING:                        // each member checks its own; the passthrough reads every column
+        if (!ctx->h_stk_Wp.empty() && ctx->h_stk_Wp.size() != (size_t)ctx->stk.R * width)
+            return fail(DKS_ERR_UNSUPPORTED, "%s: the passthrough reads %d columns, %s %d", ok.model,
+                        (int)(ctx->h_stk_Wp.size() / ctx->stk.R), E > 0 ? "the column encoding gives" : "the background has",
+                        width);
+        return DKS_OK;
     case DKS_GENERAL_EXTERNAL:                        // the module reads the raw rows: the caller checked its width
         if (E > 0)
             return fail(DKS_ERR_UNSUPPORTED, "module: a column encoding is not supported (put the preprocessing inside the "
@@ -504,6 +520,21 @@ int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const
                                                                         linkfnull, out, dlink, ctx->d_status);
         break;
     }
+    case DKS_GENERAL_STACKING: {    // every member's outputs into d_ens_out [K][n][C_k], then the final estimator
+        const int K = (int)ctx->ens.size();
+        size_t width = 0;
+        for (const dks_ctx* m : ctx->ens) width += (size_t)m->C;
+        TRY(grow(ctx, ctx->d_ens_out, width * n));
+        double* outk = ctx->d_ens_out;
+        for (int k = 0; k < K; ++k) {
+            dks_ctx* m = ctx->ens[k];
+            TRY(on_member(ctx, m, [&] { return launch_own_predict(m, X, n, nullptr, nullptr, outk, nullptr); }));
+            outk += (size_t)n * m->C;
+        }
+        dks::stack::stacking_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(ctx->d_ens_out, ctx->stk, X, n, link, linkfnull,
+                                                                          out, dlink, ctx->d_status);
+        break;
+    }
     case DKS_GENERAL_EXTERNAL:      // the module's outputs on these rows, which the caller handed to dks_external_prepare
         if (ctx->ext_y == nullptr)
             return fail(DKS_ERR_UNSUPPORTED, "module: the engine cannot run a module; run it on the rows and hand its outputs "
@@ -527,46 +558,53 @@ int launch_tail(dks_ctx* ctx, bool l1, const ExplainParams& p, const dks::SimtL1
     return DKS_OK;
 }
 
+int launch_stacking(dks_ctx* ctx, bool l1, const ExplainParams& p, cudaStream_t st);
+
 // the family's explain kernel over p.list (L1: its moments; ea.ey set: a soft-voting ensemble's member adding into its
-// workspace, the ACC instantiation); the tree kernel's per-CTA node scratch is sized for the grid.  A soft-voting ensemble:
-// its members in order, then its tail.
+// workspace, the ACC instantiation; er.ws set: a stacking ensemble's member storing its outputs of every masked row, the
+// ROWS instantiation); the tree kernel's per-CTA node scratch is sized for the grid.  A soft-voting ensemble: its members
+// in order, then its tail; a stacking ensemble: launch_stacking.
 int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem, cudaStream_t st,
-                      const dks::EnsAcc& ea = dks::EnsAcc{}) {
+                      const dks::EnsAcc& ea = dks::EnsAcc{}, const dks::EnsRows& er = dks::EnsRows{}) {
     const int grid = persistent_grid(ctx, smem, 1024, 8, ctx->cur_n);
     const dks::SimtL1 q = l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{};
-    const bool acc = ea.ey != nullptr;
+    const bool acc = ea.ey != nullptr, rows = er.ws != nullptr;
     switch (ctx->head.family) {
     case DKS_GENERAL_TREES: {
         TRY(grow(ctx, ctx->txinfo, (size_t)grid * ctx->tree.nodes));
         ctx->tree.xinfo = ctx->txinfo;
-        auto kern = acc ? dks::trees::explain_tree_kernel<false, true>
-                        : l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
+        auto kern = rows ? dks::trees::explain_tree_kernel<false, true, true>
+                    : acc ? dks::trees::explain_tree_kernel<false, true>
+                    : l1 ? dks::trees::explain_tree_kernel<true> : dks::trees::explain_tree_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->own_X, ctx->own_D, ea);
+        kern<<<grid, dks::trees::THREADS, smem, st>>>(p, q, ctx->tree, ctx->own_X, ctx->own_D, ea, er);
         break;
     }
     case DKS_GENERAL_KMACH: {
-        auto kern = acc ? dks::kmach::explain_kmach_kernel<false, true>
-                        : l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
+        auto kern = rows ? dks::kmach::explain_kmach_kernel<false, true, true>
+                    : acc ? dks::kmach::explain_kmach_kernel<false, true>
+                    : l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->own_X, ctx->own_bg, ctx->own_D, ctx->own_goff,
-                                                      ctx->own_gcols, ea);
+                                                      ctx->own_gcols, ea, er);
         break;
     }
     case DKS_GENERAL_MLP: {
-        auto kern = acc ? dks::mlp::explain_mlp_kernel<false, true>
-                        : l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
+        auto kern = rows ? dks::mlp::explain_mlp_kernel<false, true, true>
+                    : acc ? dks::mlp::explain_mlp_kernel<false, true>
+                    : l1 ? dks::mlp::explain_mlp_kernel<true> : dks::mlp::explain_mlp_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::mlp::THREADS, smem, st>>>(p, q, ctx->mlp, mlp_warps(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
-                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols, ea);
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols, ea, er);
         break;
     }
     case DKS_GENERAL_KNN: {
-        auto kern = acc ? dks::knn::explain_knn_kernel<false, true>
-                        : l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
+        auto kern = rows ? dks::knn::explain_knn_kernel<false, true, true>
+                    : acc ? dks::knn::explain_knn_kernel<false, true>
+                    : l1 ? dks::knn::explain_knn_kernel<true> : dks::knn::explain_knn_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
-                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols, ea);
+                                                    ctx->own_D, ctx->own_goff, ctx->own_gcols, ea, er);
         break;
     }
     case DKS_GENERAL_ENSEMBLE: {
@@ -583,12 +621,50 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         TRY(launch_tail(ctx, l1, p, q, ctx->d_ens_ey, false, st));
         break;
     }
+    case DKS_GENERAL_STACKING:
+        TRY(launch_stacking(ctx, l1, p, st));
+        break;
     case DKS_GENERAL_EXTERNAL:      // ey from dks_external_reduce; a module's outputs need not sum to one
         TRY(launch_tail(ctx, l1, p, q, ctx->d_ens_ey, true, st));
         break;
     }
     ctx->launches += 1;
     return DKS_OK;
+}
+
+// a stacking ensemble's explain over p.list: the background in the fewest chunks [j0, j1) whose members' outputs
+// [n][F][j1 - j0][S_cap] fit the workspace budget (at least one row each); per chunk the members' ROWS kernels in order and
+// stacking_reduce_kernel, whose chain of ey continues across chunks; then the tail (an identity head's outputs need not sum
+// to one: the logit's 1 - ey_c is taken per output).  chunks (K + 1) + 1 launches.
+int launch_stacking(dks_ctx* ctx, bool l1, const ExplainParams& p, cudaStream_t st) {
+    const int n = ctx->cur_n, N = ctx->N, F = ctx->stk.F;
+    const size_t per_row = sizeof(double) * (size_t)F * n * p.S_cap;
+    const int width = (int)std::max<long long>(1, std::min<long long>(N, ctx->stk_budget / (long long)per_row));
+    TRY(grow(ctx, ctx->d_stk_ws, (size_t)F * n * width * p.S_cap));
+    TRY(grow(ctx, ctx->d_ens_ey, (size_t)n * ctx->C * p.S_cap));
+    const double* XWg = ctx->stk.Wp != nullptr ? ctx->d_stk_XWg.get() : nullptr;
+    int chunks = 0;
+    for (int j0 = 0; j0 < N; j0 += width, ++chunks) {
+        const int j1 = std::min(N, j0 + width);
+        for (size_t k = 0, f0 = 0; k < ctx->ens.size(); f0 += ctx->stk.ccount[k], ++k) {
+            dks_ctx* m = ctx->ens[k];
+            m->cur_n = n;                           // the rows, background and group CSR of this call
+            m->own_X = ctx->own_X; m->own_D = ctx->own_D; m->own_bg = ctx->own_bg;
+            m->own_goff = ctx->own_goff; m->own_gcols = ctx->own_gcols;
+            ExplainParams pm = p;
+            pm.C = m->C;
+            const size_t msm = own_kernel(m->head.family).smem(m, p.S_cap);
+            const dks::EnsRows mer{ctx->d_stk_ws, p.dlink, ctx->C, F, (int)f0, ctx->stk.cfirst[k], ctx->stk.ccount[k], j0, j1};
+            TRY(on_member(ctx, m, [&] { return launch_own_kernel(m, false, pm, msm, st, dks::EnsAcc{}, mer); }));
+        }
+        dks::stack::stacking_reduce_kernel<<<std::max(1, std::min(n, ctx->sm_count * 8)), dks::stack::THREADS, 0, st>>>(
+            p, ctx->stk, ctx->d_stk_ws, j0, j1, XWg, ctx->d_stk_BWg, ctx->d_stk_BWtot, ctx->d_ens_ey, j0 == 0 ? 1 : 0);
+        ctx->launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    ctx->stk_chunks = chunks;
+    const dks::SimtL1 q = l1 ? dks::SimtL1{ctx->d_l1, ctx->d_mom} : dks::SimtL1{};
+    return launch_tail(ctx, l1, p, q, ctx->d_ens_ey, ctx->stk.head == DKS_STACK_HEAD_IDENTITY, st);
 }
 
 // stage 1's instantiation for R score rows: the compile-time bound 1 or 8 (a mixture: DKS_MIX_MAX_R)
@@ -639,6 +715,13 @@ int launch_prepare(dks_ctx* ctx, const double* X_dev, int n) {
         ctx->link, ipb, ctx->d_XW, ctx->d_vmask, ctx->d_M, ctx->d_dlink, ctx->d_hist, ctx->d_counts, ctx->d_idx_full,
         ctx->d_idx_other, xt, h.xt_scale, h.xt_bbar ? ctx->d_Bbar.get() : nullptr, ctx->d_status, ctx->cm, ctx->d_mix);
     if (own) TRY(launch_own_predict(ctx, X_dev, n, enc ? ctx->d_Xenc.get() : nullptr, ctx->d_linkfnull, nullptr, ctx->d_dlink));
+    if (h.family == DKS_GENERAL_STACKING && ctx->stk.Wp != nullptr) {
+        // the instances' passthrough per group, over the columns the members read
+        TRY(grow(ctx, ctx->d_stk_XWg, (size_t)n * G * ctx->stk.R));
+        dks::stack::stacking_pass_kernel<<<cdiv((long long)n * ctx->stk.R, 128), 128, 0, ctx->stream>>>(
+            ctx->own_X, n, G, ctx->own_goff, ctx->own_gcols, ctx->stk, ctx->d_stk_XWg, nullptr);
+        ctx->launches += 1;
+    }
     ctx->launches += 1;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(record_ev(ctx, 1));
@@ -941,12 +1024,9 @@ int fit_encoding(dks_ctx* ctx) {
 
 int fit_model(dks_ctx* ctx);
 
-// dks_fit of a soft-voting ensemble, after the common start: every member fitted, in order, on the ensemble's background,
-// weights, groups and column encoding (under the identity link: the ensemble takes its link of the weighted sum), then
-// fnull = sum_k pi_k fnull_k in member order and pi on the device
-int fit_members(dks_ctx* ctx, const OwnKernel& ok) {
-    const int C = ctx->C;
-    std::vector<double> fnull(C, 0.0), linkfnull(C);
+// dks_fit of a soft-voting or stacking ensemble's members: every member fitted, in order, on the ensemble's background,
+// weights, groups and column encoding, under the identity link (the ensemble takes its own link)
+int fit_member_contexts(dks_ctx* ctx) {
     for (size_t k = 0; k < ctx->ens.size(); ++k) {
         dks_ctx* m = ctx->ens[k];
         m->N = ctx->N; m->D = ctx->D; m->G = ctx->G;
@@ -955,9 +1035,20 @@ int fit_members(dks_ctx* ctx, const OwnKernel& ok) {
         m->h_ehdr = ctx->h_ehdr; m->h_eops = ctx->h_eops; m->h_eopv = ctx->h_eopv; m->h_etab = ctx->h_etab;
         m->link = DKS_LINK_IDENTITY;
         const int rc = on_member(ctx, m, [&] { return fit_model(m); });
-        if (rc != DKS_OK) return fail(rc, "soft-voting ensemble member %d: %s", (int)k, g_last_error.c_str());
-        for (int c = 0; c < C; ++c) fnull[c] += ctx->h_ens_pi[k] * m->h_fnull[c];
+        if (rc != DKS_OK)
+            return fail(rc, "%s member %d: %s", own_kernel(ctx->head.family).model, (int)k, g_last_error.c_str());
     }
+    return DKS_OK;
+}
+
+// dks_fit of a soft-voting ensemble, after the common start: its members (fit_member_contexts), then
+// fnull = sum_k pi_k fnull_k in member order and pi on the device
+int fit_members(dks_ctx* ctx, const OwnKernel& ok) {
+    const int C = ctx->C;
+    std::vector<double> fnull(C, 0.0), linkfnull(C);
+    TRY(fit_member_contexts(ctx));
+    for (size_t k = 0; k < ctx->ens.size(); ++k)
+        for (int c = 0; c < C; ++c) fnull[c] += ctx->h_ens_pi[k] * ctx->ens[k]->h_fnull[c];
     for (int c = 0; c < C; ++c) {
         linkfnull[c] = ctx->link == DKS_LINK_LOGIT ? std::log(fnull[c] / (1.0 - fnull[c])) : fnull[c];
         if (!std::isfinite(linkfnull[c]))
@@ -972,6 +1063,35 @@ int fit_members(dks_ctx* ctx, const OwnKernel& ok) {
     ctx->h_fnull = fnull;
     ctx->h_linkfnull = linkfnull;
     return fit_done(ctx);
+}
+
+// dks_fit of a stacking ensemble, after the common start and its column encoding: its members (fit_member_contexts), the
+// final estimator on the device and the background's passthrough tables over bg [N][width] (encoded behind a column
+// encoding)
+int fit_stacking(dks_ctx* ctx, const double* bg, int width) {
+    TRY(fit_member_contexts(ctx));
+    DevPool& pool = ctx->fit_pool;
+    const cudaStream_t st = ctx->stream;
+    StackDev& sd = ctx->stk;
+    CUDA_TRY(pool.upload(&sd.W, ctx->h_stk_W.data(), ctx->h_stk_W.size(), st));
+    CUDA_TRY(pool.upload(&sd.b, ctx->h_stk_b.data(), ctx->h_stk_b.size(), st));
+    sd.Wp = nullptr;
+    sd.D = width;
+    ctx->d_stk_BWg = ctx->d_stk_BWtot = nullptr;
+    if (!ctx->h_stk_Wp.empty()) {
+        CUDA_TRY(pool.upload(&sd.Wp, ctx->h_stk_Wp.data(), ctx->h_stk_Wp.size(), st));
+        double *BWg, *BWtot;
+        CUDA_TRY(pool.alloc(&BWg, (size_t)ctx->N * ctx->G * sd.R));
+        CUDA_TRY(pool.alloc(&BWtot, (size_t)ctx->N * sd.R));
+        const bool enc = ctx->enc.E > 0;
+        dks::stack::stacking_pass_kernel<<<cdiv((long long)ctx->N * sd.R, 128), 128, 0, st>>>(
+            bg, ctx->N, ctx->G, enc ? ctx->d_egoff : ctx->d_goff.get(), enc ? ctx->d_egcols : ctx->d_gcols.get(), sd, BWg,
+            BWtot);
+        ctx->launches += 1;
+        ctx->d_stk_BWg = BWg;
+        ctx->d_stk_BWtot = BWtot;
+    }
+    return DKS_OK;
 }
 
 // dks_fit of a family with its own kernel: its column check, the common start, the column encoding, the family's arrays
@@ -994,7 +1114,8 @@ int fit_own(dks_ctx* ctx) {
         bg_pred = ctx->d_ext_bgy;
     } else {
         const double* bg = ctx->enc.E > 0 ? ctx->d_bg_enc : ctx->d_bg;
-        TRY(own_fit_tables(ctx, bg, model_columns(ctx)));
+        if (ctx->head.family == DKS_GENERAL_STACKING) TRY(fit_stacking(ctx, bg, model_columns(ctx)));
+        else TRY(own_fit_tables(ctx, bg, model_columns(ctx)));
         CUDA_TRY(pred.alloc((size_t)N * C));
         TRY(launch_own_predict(ctx, bg, N, nullptr, nullptr, pred, nullptr));
         bg_pred = pred;
@@ -1808,6 +1929,45 @@ void destroy_members(dks_ctx* ctx) {
     ctx->h_ens_pi.clear();
 }
 
+// the members [K] a soft-voting or stacking ensemble (setter `fn`) is handed: distinct contexts of their own on its device,
+// each a tree ensemble, kernel machine, MLP or neighbour model, and (C > 0) each giving C outputs
+int check_members(const dks_ctx* ctx, int K, dks_ctx* const* members, const char* fn, int C) {
+    for (int k = 0; k < K; ++k) {
+        const dks_ctx* m = members[k];
+        REQUIRE(m && m != ctx && !m->ens_parent && m->ens.empty(),
+                "%s: member %d must be a context of its own, not this one, another ensemble or its member", fn, k);
+        for (int k2 = 0; k2 < k; ++k2) REQUIRE(members[k2] != m, "%s: member %d appears twice", fn, k);
+        REQUIRE(m->device == ctx->device, "%s: member %d is on device %d, the ensemble on %d", fn, k, m->device,
+                ctx->device);
+        if (m->act != DKS_ACT_TREES && m->act != DKS_ACT_KMACH && m->act != DKS_ACT_MLP && m->act != DKS_ACT_KNN)
+            return fail(DKS_ERR_UNSUPPORTED, "%s: member %d is not a tree ensemble, kernel machine, MLP or neighbour model "
+                        "(dks_set_tree_model, dks_set_kernel_machine, dks_set_mlp, dks_set_knn_model)", fn, k);
+        if (C > 0 && m->C != C)
+            return fail(DKS_ERR_UNSUPPORTED, "%s: member %d gives %d outputs, the ensemble %d", fn, k, m->C, C);
+    }
+    return DKS_OK;
+}
+
+// the ensemble takes the checked members over, in order, in place of any it held: they launch on its stream, report into
+// its status word and refuse the C ABI from then on
+int adopt_members(dks_ctx* ctx, int K, dks_ctx* const* members) {
+    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    destroy_members(ctx);
+    for (int k = 0; k < K; ++k) {
+        dks_ctx* m = members[k];
+        CUDA_TRY(cudaStreamSynchronize(m->stream));
+        if (m->own_stream && m->stream) CUDA_TRY(cudaStreamDestroy(m->stream));
+        m->stream = ctx->stream;
+        m->own_stream = false;
+        m->status.reset();
+        m->d_status = ctx->d_status; m->d_counts = ctx->d_counts; m->d_hist = ctx->d_hist;
+        m->head = describe_head(m);
+        m->ens_parent = ctx;
+        ctx->ens.push_back(m);
+    }
+    return DKS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2265,35 +2425,55 @@ int dks_set_ensemble(dks_ctx* ctx, int K, dks_ctx* const* members, const double*
     }
     if (!(wsum > 0) || !std::isfinite(wsum))
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: the weights must have a positive finite sum");
+    TRY(check_members(ctx, K, members, "dks_set_ensemble", C));
+    TRY(adopt_members(ctx, K, members));
+    for (int k = 0; k < K; ++k) ctx->h_ens_pi.push_back(weights[k] / wsum);
+    return set_own_model(ctx, DKS_ACT_ENSEMBLE, C, scalar_out);
+}
+
+int dks_set_stacking(dks_ctx* ctx, int K, dks_ctx* const* members, const int32_t* col_first, const int32_t* col_count,
+                     const double* W, const double* b, int R, int head, const double* W_pass, int C, int scalar_out,
+                     int64_t workspace_bytes) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_stacking: call dks_set_background first (D unknown)");
+    REQUIRE(members && col_first && col_count && W && b, "dks_set_stacking: need the members, their columns, W and b");
+    if (K < 1 || K > DKS_ENS_MAX_MEMBERS)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_stacking: K=%d members; 1..%d supported", K, DKS_ENS_MAX_MEMBERS);
+    if (C < 1 || C > DKS_ENS_MAX_OUT)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_stacking: C=%d outputs; 1..%d supported", C, DKS_ENS_MAX_OUT);
+    const bool heads_ok = (head == DKS_STACK_HEAD_IDENTITY && R == C) || (head == DKS_STACK_HEAD_SIGMOID && R == 1 && C == 2) ||
+                          (head == DKS_STACK_HEAD_SOFTMAX && R == C && R >= 2);
+    if (!heads_ok)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_stacking: head %d with R=%d scores and C=%d outputs (identity: R = C; "
+                    "sigmoid: R = 1, C = 2; softmax: R = C >= 2)", head, R, C);
+    REQUIRE(workspace_bytes > 0, "dks_set_stacking: the workspace budget must be positive");
+    int F = 0;
+    TRY(check_members(ctx, K, members, "dks_set_stacking", 0));
     for (int k = 0; k < K; ++k) {
         const dks_ctx* m = members[k];
-        REQUIRE(m && m != ctx && !m->ens_parent && m->ens.empty(),
-                "dks_set_ensemble: member %d must be a context of its own, not this one, another ensemble or its member", k);
-        for (int k2 = 0; k2 < k; ++k2) REQUIRE(members[k2] != m, "dks_set_ensemble: member %d appears twice", k);
-        REQUIRE(m->device == ctx->device, "dks_set_ensemble: member %d is on device %d, the ensemble on %d", k, m->device,
-                ctx->device);
-        if (m->act != DKS_ACT_TREES && m->act != DKS_ACT_KMACH && m->act != DKS_ACT_MLP && m->act != DKS_ACT_KNN)
-            return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: member %d is not a tree ensemble, kernel machine, MLP or "
-                        "neighbour model (dks_set_tree_model, dks_set_kernel_machine, dks_set_mlp, dks_set_knn_model)", k);
-        if (m->C != C)
-            return fail(DKS_ERR_UNSUPPORTED, "dks_set_ensemble: member %d gives %d outputs, the ensemble %d", k, m->C, C);
+        if (col_count[k] < 1 || col_first[k] < 0 || col_first[k] + col_count[k] > m->C)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_stacking: member %d keeps outputs %d..%d of its %d", k, col_first[k],
+                        col_first[k] + col_count[k] - 1, m->C);
+        F += col_count[k];
     }
-    CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    destroy_members(ctx);
+    if (F > DKS_STACK_MAX_F)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_stacking: F=%d meta columns; at most %d", F, DKS_STACK_MAX_F);
+    const int width = model_columns(ctx);
+    if (!all_finite(W, (size_t)R * F) || !all_finite(b, R) || (W_pass && !all_finite(W_pass, (size_t)R * width)))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_stacking: the final estimator's weights must be finite");
+    TRY(adopt_members(ctx, K, members));
+    StackDev& sd = ctx->stk;
+    sd = StackDev{};
+    sd.K = K; sd.F = F; sd.R = R; sd.C = C; sd.head = head; sd.D = width;
     for (int k = 0; k < K; ++k) {
-        dks_ctx* m = members[k];
-        CUDA_TRY(cudaStreamSynchronize(m->stream));
-        if (m->own_stream && m->stream) CUDA_TRY(cudaStreamDestroy(m->stream));
-        m->stream = ctx->stream;
-        m->own_stream = false;
-        m->status.reset();
-        m->d_status = ctx->d_status; m->d_counts = ctx->d_counts; m->d_hist = ctx->d_hist;
-        m->head = describe_head(m);
-        m->ens_parent = ctx;
-        ctx->ens.push_back(m);
-        ctx->h_ens_pi.push_back(weights[k] / wsum);
+        sd.ck[k] = members[k]->C; sd.cfirst[k] = col_first[k]; sd.ccount[k] = col_count[k];
     }
-    return set_own_model(ctx, DKS_ACT_ENSEMBLE, C, scalar_out);
+    ctx->h_stk_W.assign(W, W + (size_t)R * F);
+    ctx->h_stk_b.assign(b, b + R);
+    if (W_pass) ctx->h_stk_Wp.assign(W_pass, W_pass + (size_t)R * width);
+    else ctx->h_stk_Wp.clear();
+    ctx->stk_budget = workspace_bytes;
+    return set_own_model(ctx, DKS_ACT_STACKING, C, scalar_out);
 }
 
 int dks_set_column_maps(dks_ctx* ctx, int D, int R, const int32_t* hdr_host, const double* keys_host, int n_keys,

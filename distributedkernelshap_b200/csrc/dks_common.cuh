@@ -321,6 +321,18 @@ enum HeadShared {               // what the shared-plan route of the full varyin
     HEAD_SHARED_MIX_BINARY,     // mixture of binary-logistic members: the binary head's kernel per member
     HEAD_SHARED_MIX_CLASS,      // mixture of softmax / one-vs-rest members: the class-sum kernel per member
 };
+// stacking ensemble (dks_set_stacking, DESIGN.md §5.0.20): the final estimator and the member columns it reads (by value;
+// W, b and W_pass in device memory)
+struct StackDev {
+    const double* W;         // [R][F]
+    const double* b;         // [R]
+    const double* Wp;        // [R][D] passthrough weights over the columns the members read, or NULL
+    int K, F, R, C, head, D;
+    int ck[DKS_ENS_MAX_MEMBERS];        // outputs of member k
+    int cfirst[DKS_ENS_MAX_MEMBERS];    // its first output kept
+    int ccount[DKS_ENS_MAX_MEMBERS];    // outputs kept
+};
+
 struct HeadDesc {
     int shared = HEAD_SHARED_BINARY;
     bool ovr = false;           // the class sums (of the head or of its members) are one-vs-rest ones
@@ -432,6 +444,17 @@ struct dks_ctx {
     const double* d_ens_pi = nullptr;
     DevBuf<double> d_ens_out, d_ens_ey;
     dks_ctx* ens_parent = nullptr;
+    // stacking ensemble (act == DKS_ACT_STACKING): its members in `ens` (owned as above); the final estimator's host copies
+    // and its descriptor (stk.W / b / Wp built by dks_fit), the workspace budget of a call, the members' kept outputs of one
+    // background chunk [n][F][j1 - j0][S_cap], the instances' passthrough table XWg [n][G][R] (stage 1), the background's
+    // BWg [N][G][R] and BWtot [N][R] (dks_fit, fit_pool), and the chunks of the last call
+    std::vector<double> h_stk_W, h_stk_b, h_stk_Wp;
+    StackDev stk = {};
+    int64_t stk_budget = 0;
+    DevBuf<double> d_stk_ws, d_stk_XWg;
+    const double* d_stk_BWg = nullptr;
+    const double* d_stk_BWtot = nullptr;
+    int stk_chunks = 0;
     // a module the caller runs (act == DKS_ACT_EXTERNAL, dks_set_external_model): the dtype of its input rows, its outputs on
     // the background in float64 (dks_set_external_background), the group of every column (d_ext_colgrp, fit_pool), the
     // outputs stage 1 reads while dks_external_prepare runs (the caller's memory), and the call dks_external_begin laid

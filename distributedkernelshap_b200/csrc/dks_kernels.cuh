@@ -1013,6 +1013,39 @@ __device__ __forceinline__ void ens_accumulate(const EnsAcc& e, const ExplainPar
         }
 }
 
+// a member of a stacking ensemble (instantiation ROWS of the family explain kernels, DESIGN.md §5.0.20): in place of the
+// background mean, the member's outputs c0 .. c0 + nc - 1 on every masked row (s, j) of the chunk j0 <= j < j1 (rows with
+// w_j = 0 skipped) are stored to the stacking's workspace ws [n][F][j1 - j0][S_cap] at meta columns f0 .. f0 + nc - 1;
+// stacking_reduce_kernel applies the final estimator to them.  dlink [n][Cs] is the stacking's (its f(x) refused or not
+// finite: the instance is skipped, as the tail skips it).
+struct EnsRows {
+    double* ws;              // NULL: not a stacking member
+    const double* dlink;
+    int Cs, F, f0, c0, nc, j0, j1;
+};
+
+__device__ __forceinline__ bool rows_fx_bad(const EnsRows& r, int i) {
+    bool bad = false;
+    for (int c = 0; c < r.Cs; ++c) bad |= !isfinite(r.dlink[(size_t)i * r.Cs + c]);
+    return bad;
+}
+
+// coalition s of background row j: the kept outputs of o into the workspace (threads own consecutive s: coalesced).  NO > 0:
+// o [NO] is indexed at compile time only, for a kernel that keeps it in registers (the MLP's); NO = 0: at run time, for the
+// kernels whose o already lives in local memory (unrolling would only add live addresses there).
+template <int NO>
+__device__ __forceinline__ void rows_store(const EnsRows& r, int S_cap, int i, int j, int s, const double* o) {
+    const size_t nj = (size_t)(r.j1 - r.j0);
+    double* w = r.ws + (((size_t)i * r.F + r.f0) * nj + (size_t)(j - r.j0)) * S_cap + s;
+    if constexpr (NO > 0) {
+#pragma unroll
+        for (int c = 0; c < NO; ++c)
+            if (c >= r.c0 && c < r.c0 + r.nc) w[(size_t)(c - r.c0) * nj * S_cap] = o[c];
+    } else {
+        for (int c = 0; c < r.nc; ++c) w[(size_t)c * nj * S_cap] = o[r.c0 + c];
+    }
+}
+
 // exp head: ey(s) of one coalition row in float64, for the rows outside the fp32 range rule (DKS_EXP_T_LO / _HI):
 // exp(a + m + ln sum_j w_j e^(d_j - m)) with a = sum_{k in s} XW_i[k], d_j = score_j - sum_{k in s} BW[j][k] and m the
 // running maximum of d_j (one pass, the sum rescaled when m grows), zero-weight rows skipped.  Row bit k (k < M) is

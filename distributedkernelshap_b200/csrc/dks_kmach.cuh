@@ -130,11 +130,14 @@ __host__ __device__ inline size_t smem_bytes(int S_cap, int C, int R, int G, boo
 // DKS_ERR_NUMERIC and nothing of the instance is written.
 // ACC (a soft-voting ensemble's member): the sums of every output go into ea.ey instead (ens_accumulate); instances
 // with M <= 1 or a refused f(x) are left to explain_ensemble_tail_kernel.
-template <bool L1, bool ACC = false>
+// ROWS (a stacking ensemble's member, with ACC): per background row of the chunk the sums are formed at unit weight from
+// zero -- each coalition's outputs -- and go to er.ws (rows_store), each thread storing the coalitions it owns; nothing is
+// summed over the background.
+template <bool L1, bool ACC = false, bool ROWS = false>
 __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p, SimtL1 q, KmDev k,
                                                                 const double* __restrict__ X, const double* __restrict__ bg,
                                                                 int D, const int* __restrict__ goff,
-                                                                const int* __restrict__ gcols, EnsAcc ea) {
+                                                                const int* __restrict__ gcols, EnsAcc ea, EnsRows er) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C, R = k.R;
@@ -161,7 +164,8 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
         __syncthreads();  // previous instance done with shared memory
         if constexpr (!ACC) zero_phi_rows(p, i);
         bool fx_bad = false;                                    // stage 1 reported a NaN row or a non-finite link(f(x))
-        for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
+        if constexpr (ROWS) fx_bad = rows_fx_bad(er, i);
+        else for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
         if (M == 1) {
             // the one varying group takes link(f(x)) - link(fnull); calibrated: class 0 is the negation of class 1, as below
@@ -187,10 +191,14 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
 
         const double* x = X + (size_t)i * D;
         const int nib = (M + 3) >> 2;
-        for (int j = 0; j < N; ++j) {
-            const double wj = p.wbg[j];
-            if (wj == 0.0) continue;                            // block-uniform
+        for (int j = ROWS ? er.j0 : 0; j < (ROWS ? er.j1 : N); ++j) {
+            const double wb = p.wbg[j];
+            if (wb == 0.0) continue;                            // block-uniform
+            const double wj = ROWS ? 1.0 : wb;
             const double* b = bg + (size_t)j * D;
+            if constexpr (ROWS)
+                for (int s = tid; s < S; s += blockDim.x)
+                    for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = 0.0;
             if (!cal)
                 for (int s = tid; s < S; s += blockDim.x)
                     for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = fma(wj, k.icpt[c], acc[(size_t)c * p.S_cap + s]);
@@ -256,8 +264,15 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
                     }
                 }
             }
+            if constexpr (ROWS)
+                for (int s = tid; s < S; s += blockDim.x) {
+                    double o[DKS_KM_MAX_R];
+                    for (int c = 0; c < C; ++c) o[c] = acc[(size_t)c * p.S_cap + s];
+                    rows_store<0>(er, p.S_cap, i, j, s, o);
+                }
         }
         __syncthreads();
+        if constexpr (ROWS) continue;
         if constexpr (ACC) {
             ens_accumulate(ea, p, i, S, acc);
             continue;

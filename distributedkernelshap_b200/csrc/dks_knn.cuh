@@ -187,11 +187,13 @@ __host__ __device__ inline size_t smem_bytes(int S_cap, int C, int G, int k, int
 // is written.
 // ACC (a soft-voting ensemble's member): the sums of every output go into ea.ey instead (ens_accumulate); instances
 // with M <= 1 or a refused f(x) are left to explain_ensemble_tail_kernel.
-template <bool L1, bool ACC = false>
+// ROWS (a stacking ensemble's member, with ACC): each masked row's kept outputs go to er.ws instead (rows_store), for the
+// background rows of the chunk only; nothing is summed.
+template <bool L1, bool ACC = false, bool ROWS = false>
 __global__ void __launch_bounds__(THREADS) explain_knn_kernel(ExplainParams p, SimtL1 q, KnnDev k, int chunk,
                                                               const double* __restrict__ X, const double* __restrict__ bg,
                                                               int D, const int* __restrict__ goff,
-                                                              const int* __restrict__ gcols, EnsAcc ea) {
+                                                              const int* __restrict__ gcols, EnsAcc ea, EnsRows er) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C, K = k.k;
@@ -218,7 +220,8 @@ __global__ void __launch_bounds__(THREADS) explain_knn_kernel(ExplainParams p, S
         __syncthreads();  // previous instance done with shared memory
         if constexpr (!ACC) zero_phi_rows(p, i);
         bool fx_bad = false;                                    // stage 1 reported a refused row or a non-finite link(f(x))
-        for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
+        if constexpr (ROWS) fx_bad = rows_fx_bad(er, i);
+        else for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
         if (M == 1) {
             // the one varying group takes link(f(x)) - link(fnull) of every output
@@ -246,7 +249,7 @@ __global__ void __launch_bounds__(THREADS) explain_knn_kernel(ExplainParams p, S
         const uint64_t fixed = gall & ~vm;
         for (int c0 = 0; c0 < S; c0 += chunk) {
             const int nc = min(chunk, S - c0);
-            for (int j = 0; j < N; ++j) {
+            for (int j = ROWS ? er.j0 : 0; j < (ROWS ? er.j1 : N); ++j) {
                 const double wj = p.wbg[j];
                 if (wj == 0.0) continue;                        // block-uniform
                 const double* b = bg + (size_t)j * D;
@@ -314,12 +317,17 @@ __global__ void __launch_bounds__(THREADS) explain_knn_kernel(ExplainParams p, S
                 for (int s = tid; s < nc; s += blockDim.x) {
                     double o[DKS_KNN_MAX_R];
                     knn_outputs(k, lt + s, li + s, chunk, o);
-                    for (int c = 0; c < C; ++c)
-                        acc[(size_t)c * p.S_cap + c0 + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + c0 + s]);
+                    if constexpr (ROWS) {
+                        rows_store<0>(er, p.S_cap, i, j, c0 + s, o);
+                    } else {
+                        for (int c = 0; c < C; ++c)
+                            acc[(size_t)c * p.S_cap + c0 + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + c0 + s]);
+                    }
                 }
             }
         }
         __syncthreads();
+        if constexpr (ROWS) continue;
         if constexpr (ACC) {
             ens_accumulate(ea, p, i, S, acc);
             continue;

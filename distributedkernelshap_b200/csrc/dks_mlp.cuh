@@ -219,11 +219,13 @@ __device__ __forceinline__ void forward_tile(const MlpDev& m, int KC1, uint64_t 
 // written.
 // ACC (a soft-voting ensemble's member): the sums of every output go into ea.ey instead (ens_accumulate); instances
 // with M <= 1 or a refused f(x) are left to explain_ensemble_tail_kernel.
-template <bool L1, bool ACC = false>
+// ROWS (a stacking ensemble's member, with ACC): each masked row's kept outputs go to er.ws instead (rows_store), for the
+// background rows of the chunk only; nothing is summed.
+template <bool L1, bool ACC = false, bool ROWS = false>
 __global__ void __launch_bounds__(THREADS) explain_mlp_kernel(ExplainParams p, SimtL1 q, MlpDev m, int nw,
                                                               const double* __restrict__ X, const double* __restrict__ bg,
                                                               int D, const int* __restrict__ goff,
-                                                              const int* __restrict__ gcols, EnsAcc ea) {
+                                                              const int* __restrict__ gcols, EnsAcc ea, EnsRows er) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int N = p.N, G = p.G, C = p.C;
@@ -251,7 +253,8 @@ __global__ void __launch_bounds__(THREADS) explain_mlp_kernel(ExplainParams p, S
         __syncthreads();  // previous instance done with shared memory
         if constexpr (!ACC) zero_phi_rows(p, i);
         bool fx_bad = false;                          // stage 1 reported a refused row or a non-finite link(f(x))
-        for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
+        if constexpr (ROWS) fx_bad = rows_fx_bad(er, i);
+        else for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
         if (M == 1) {
             // the one varying group takes link(f(x)) - link(fnull); sigmoid head: class 0 is the negation of class 1
@@ -276,7 +279,7 @@ __global__ void __launch_bounds__(THREADS) explain_mlp_kernel(ExplainParams p, S
 
         const double* x = X + (size_t)i * D;
         const int MP = pad16(M), KC1 = MP >> 4;
-        for (int j = 0; j < N; ++j) {
+        for (int j = ROWS ? er.j0 : 0; j < (ROWS ? er.j1 : N); ++j) {
             const double wj = p.wbg[j];
             if (wj == 0.0) continue;                  // block-uniform
             const double* b = bg + (size_t)j * D;
@@ -306,12 +309,14 @@ __global__ void __launch_bounds__(THREADS) explain_mlp_kernel(ExplainParams p, S
                 if (lane < 16 && s < S) {
                     double o[DKS_MLP_MAX_OUT];
                     mlp_head(m.head, lg + lane * 8, m.R, o);
-                    for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + s]);
+                    if constexpr (ROWS) rows_store<DKS_MLP_MAX_OUT>(er, p.S_cap, i, j, s, o);
+                    else for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + s]);
                 }
                 __syncwarp();                         // lg is rewritten by the next tile
             }
         }
         __syncthreads();
+        if constexpr (ROWS) continue;
         if constexpr (ACC) {
             ens_accumulate(ea, p, i, S, acc);
             continue;

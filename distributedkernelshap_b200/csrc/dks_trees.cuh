@@ -99,9 +99,11 @@ __host__ __device__ inline size_t smem_bytes(int S_cap, int C, int R, int T) {
 // l1_lars_kernel.  A non-finite y or f(x) is reported as DKS_ERR_NUMERIC and nothing of the instance is written.  ACC (a
 // soft-voting ensemble's member): the sums of every output go into ea.ey instead (ens_accumulate); instances with M <= 1
 // or a refused f(x) are left to explain_ensemble_tail_kernel.
-template <bool L1, bool ACC = false>
+// ROWS (a stacking ensemble's member, with ACC): each masked row's kept outputs go to er.ws instead (rows_store), for the
+// background rows of the chunk only; nothing is summed.
+template <bool L1, bool ACC = false, bool ROWS = false>
 __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, SimtL1 q, TreeDev t, const double* __restrict__ X,
-                                                               int D, EnsAcc ea) {
+                                                               int D, EnsAcc ea, EnsRows er) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int N = p.N, G = p.G, C = p.C, R = t.R, T = t.T, nodes = t.nodes;
@@ -125,7 +127,8 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
         __syncthreads();  // previous instance done with shared memory and xi
         if constexpr (!ACC) zero_phi_rows(p, i);
         bool fx_bad = false;                                    // stage 1 reported a non-finite link(f(x))
-        for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
+        if constexpr (ROWS) fx_bad = rows_fx_bad(er, i);
+        else for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
         if (M == 0) continue;
         if (M == 1) {
             // the one varying group takes link(f(x)) - link(fnull); two outputs: class 0 is the negation of class 1, as below
@@ -159,7 +162,7 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
         for (int idx = tid; idx < C * S; idx += blockDim.x) acc[(size_t)(idx / S) * p.S_cap + idx % S] = 0.0;
         __syncthreads();
 
-        for (int j = 0; j < N; ++j) {
+        for (int j = ROWS ? er.j0 : 0; j < (ROWS ? er.j1 : N); ++j) {
             const double wj = p.wbg[j];
             if (wj == 0.0) continue;                            // block-uniform
             const unsigned char* bd = t.bgdir + (size_t)j * nodes;
@@ -211,10 +214,12 @@ __global__ void __launch_bounds__(THREADS) explain_tree_kernel(ExplainParams p, 
                     for (int u = 0; u < R; ++u) r[u] += t.val[(size_t)nd * R + u];
                 }
                 tree_head(r, R, t.head, t.offset, o);
-                for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + s]);
+                if constexpr (ROWS) rows_store<0>(er, p.S_cap, i, j, s, o);
+                else for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = fma(wj, o[c], acc[(size_t)c * p.S_cap + s]);
             }
             __syncthreads();
         }
+        if constexpr (ROWS) continue;
         if constexpr (ACC) {
             ens_accumulate(ea, p, i, S, acc);
             continue;

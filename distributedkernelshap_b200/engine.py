@@ -19,7 +19,8 @@ from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_ns
 from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, KernelMachineSpec, extract_kernel_machine_spec
 from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, MlpSpec, extract_mlp_spec
 from .neighbors import MAX_GROUPS as KNN_MAX_GROUPS, KnnSpec, extract_knn_spec
-from .predictors import extract_linear_spec
+from .predictors import LinearModelSpec, extract_linear_spec
+from .stacking import MAX_GROUPS as STACKING_MAX_GROUPS, StackingSpec, extract_stacking_spec
 from . import torch_models
 from .torch_models import TorchModelSpec
 from .trees import MAX_GROUPS as TREE_MAX_GROUPS, TreeEnsembleSpec, extract_encoded_pipeline_spec, \
@@ -38,6 +39,9 @@ MAX_ENCODED_BYTES_PER_CALL = 256 << 20
 # a soft-voting ensemble keeps its members' weighted background means of a call on the device (n x C x S x 8 B): row
 # blocks bound them
 MAX_ENSEMBLE_BYTES_PER_CALL = 1 << 30
+# a stacking ensemble keeps its members' outputs of every masked row of one background chunk on the device
+# (n x F x chunk x S x 8 B): the library splits the background into the fewest chunks within this budget
+MAX_STACKING_BYTES_PER_CALL = 1 << 30
 
 
 def per_instance_workspace_bytes(M, S):
@@ -155,7 +159,9 @@ class GpuKernelExplainer:
         the last three bare, behind affine scalers (folded into the model) or behind such a ``Pipeline``
         (``trees.extract_encoded_pipeline_spec``, replayed like a tree's); a soft ``VotingClassifier`` or a
         ``VotingRegressor`` mixing those families with linear members, bare or behind such a ``Pipeline``
-        (``ensembles.extract_ensemble_spec``).  A raw value the pipeline would refuse (NaN, or an unseen category under
+        (``ensembles.extract_ensemble_spec``); a ``StackingClassifier`` (``predict_proba``, ``decision_function``) or a
+        ``StackingRegressor`` over those families with a linear final estimator, bare or behind such a ``Pipeline``
+        (``stacking.extract_stacking_spec``).  A raw value the pipeline would refuse (NaN, or an unseen category under
         ``handle_unknown='error'``) raises ``ValueError``.  Or a ``torch.nn.Module`` in eval mode on one CUDA device,
         float32 or float64, mapping [B, D] to [B] or [B, C <= 8] (``torch_models.TorchModelSpec``): the engine builds the
         masked rows on the device, the module runs on them and the engine reduces its outputs and solves (up to 64
@@ -189,6 +195,7 @@ class GpuKernelExplainer:
         self.link = convert_to_link(link)
         self.model_callable = model
         torch_models.refuse_module_in_pipeline(model)
+        linear_target = model
         if torch_models.is_torch_module(model):
             # a module: recognised and checked here, run on the background below
             if kernel not in ("auto", "simt"):
@@ -196,9 +203,13 @@ class GpuKernelExplainer:
                                           "'simt')")
             ens, pipe_spec = None, None
         else:
-            # a soft-voting ensemble of the families below (bare: its spec; behind per-column preprocessing: with the
-            # encoding)
-            ens = extract_ensemble_spec(model)
+            # a stacking or soft-voting ensemble of the families below (bare: its spec; behind per-column preprocessing:
+            # with the encoding); an all-linear stacking regressor folds into one linear model
+            ens = extract_stacking_spec(model)
+            if isinstance(ens, LinearModelSpec):
+                linear_target, ens = ens, None
+            elif ens is None:
+                ens = extract_ensemble_spec(model)
             pipe_spec = ens if isinstance(ens, tuple) else None
             if ens is None:
                 pipe_spec = extract_tree_pipeline_spec(model)
@@ -206,12 +217,13 @@ class GpuKernelExplainer:
                     pipe_spec = extract_encoded_pipeline_spec(model)
         # a model behind per-column preprocessing: explained in raw feature space, the device replaying the steps; the
         # extractors below pass its spec through
-        target, self.encoding = pipe_spec if pipe_spec is not None else (model if ens is None else ens, None)
+        target, self.encoding = pipe_spec if pipe_spec is not None else (linear_target if ens is None else ens, None)
         # the model families with their own kernels: the first extractor that reads the model wins; the family's kernels
         # cover at most max_groups groups.  Built per construction, so the module's extractors are looked up when it runs.
         families = ((lambda t: TorchModelSpec(t) if torch_models.is_torch_module(t) else None, torch_models.MAX_GROUPS,
                      "torch modules"),
                     (lambda t: t if isinstance(t, EnsembleSpec) else None, ENSEMBLE_MAX_GROUPS, "soft-voting ensembles"),
+                    (lambda t: t if isinstance(t, StackingSpec) else None, STACKING_MAX_GROUPS, "stacking ensembles"),
                     (extract_tree_spec, TREE_MAX_GROUPS, "tree ensembles"),
                     (extract_kernel_machine_spec, KMACH_MAX_GROUPS, "kernel machines"),
                     (extract_mlp_spec, MLP_MAX_GROUPS, "MLPs"),
@@ -220,7 +232,7 @@ class GpuKernelExplainer:
             own = extract(target)
             if own is not None:
                 break
-        self.spec = own if own is not None else extract_linear_spec(model)
+        self.spec = own if own is not None else extract_linear_spec(linear_target)
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
                                       "link log(ey / (1 - ey)) is undefined wherever a predicted mean exceeds 1")
@@ -274,6 +286,8 @@ class GpuKernelExplainer:
         self._set_encoding(self._ctx)   # before the model: its columns are the encoded ones
         if isinstance(own, EnsembleSpec):
             self._set_ensemble(own, bg, weights)
+        elif isinstance(own, StackingSpec):
+            self._set_stacking(own, bg, weights)
         elif isinstance(own, TorchModelSpec):
             _cabi.check(self.lib.dks_set_external_model(self._ctx, own.n_outputs, int(own.scalar_out), own.dtype_code))
             y = self._bg_outputs
@@ -315,7 +329,7 @@ class GpuKernelExplainer:
         if self.encoding is not None:
             self._check_encoding(bg)
         if not isinstance(own, TorchModelSpec):     # a module's outputs are the module's: nothing was extracted
-            self._check_model_against_callable(bg, own if isinstance(own, (KnnSpec, EnsembleSpec)) else None)
+            self._check_model_against_callable(bg, own if isinstance(own, (KnnSpec, EnsembleSpec, StackingSpec)) else None)
 
     def _bind_torch_stream(self):
         """A module: the engine enqueues on torch's current stream of the module's device, so the masked rows, the module
@@ -358,22 +372,43 @@ class GpuKernelExplainer:
             if t.head == "iforest":
                 _cabi.check(self.lib.dks_set_tree_offset(ctx, t.offset))
 
+    def _member_contexts(self, spec, bg, weights, members):
+        """Appends to ``members`` one context per member of a soft-voting or stacking ensemble (its background and column
+        encoding give the setter the model's width)."""
+        for _, member in spec.members:
+            m = C.c_void_p()
+            _cabi.check(self.lib.dks_create(C.byref(m), self.device))
+            members.append(m)
+            _cabi.check(self.lib.dks_set_background(m, _cabi.ptr(bg), self.N, self.P, _cabi.ptr(weights)))
+            self._set_encoding(m)
+            self._set_own_model(m, member)
+
     def _set_ensemble(self, spec, bg, weights):
-        """One context per member (its background and column encoding give the setter the model's width), handed to
-        ``dks_set_ensemble``, which owns them from then on."""
+        """One context per member, handed to ``dks_set_ensemble``, which owns them from then on."""
         members = []
         try:
-            for _, member in spec.members:
-                m = C.c_void_p()
-                _cabi.check(self.lib.dks_create(C.byref(m), self.device))
-                members.append(m)
-                _cabi.check(self.lib.dks_set_background(m, _cabi.ptr(bg), self.N, self.P, _cabi.ptr(weights)))
-                self._set_encoding(m)
-                self._set_own_model(m, member)
+            self._member_contexts(spec, bg, weights, members)
             ptrs = (C.c_void_p * len(members))(*[m.value for m in members])
             pi = np.ascontiguousarray(spec.weights, dtype=np.float64)
             _cabi.check(self.lib.dks_set_ensemble(self._ctx, len(members), ptrs, _cabi.ptr(pi), spec.n_outputs,
                                                   int(spec.scalar_out)))
+        except Exception:
+            for m in members:               # not handed over: still ours
+                self.lib.dks_destroy(m)
+            raise
+
+    def _set_stacking(self, spec, bg, weights):
+        """One context per member, as for a soft-voting ensemble, handed to ``dks_set_stacking`` with the final
+        estimator and ``MAX_STACKING_BYTES_PER_CALL`` as the workspace budget of a call."""
+        members = []
+        try:
+            self._member_contexts(spec, bg, weights, members)
+            ptrs = (C.c_void_p * len(members))(*[m.value for m in members])
+            first, count = spec.col_first, spec.col_count
+            _cabi.check(self.lib.dks_set_stacking(self._ctx, len(members), ptrs, _cabi.ptr(first), _cabi.ptr(count),
+                                                  _cabi.ptr(spec.W), _cabi.ptr(spec.b), spec.W.shape[0], spec.head_code,
+                                                  _cabi.ptr(spec.W_pass), spec.n_outputs, int(spec.scalar_out),
+                                                  int(MAX_STACKING_BYTES_PER_CALL)))
         except Exception:
             for m in members:               # not handed over: still ours
                 self.lib.dks_destroy(m)
@@ -419,7 +454,8 @@ class GpuKernelExplainer:
             return
         want = np.asarray(self.model_callable(bg), dtype=np.float64).reshape(self.N, -1)
         got = self.predict(bg)
-        knns = [s for _, s in knn_spec.members if isinstance(s, KnnSpec)] if isinstance(knn_spec, EnsembleSpec) else \
+        knns = [s for _, s in knn_spec.members if isinstance(s, KnnSpec)] \
+            if isinstance(knn_spec, (EnsembleSpec, StackingSpec)) else \
             [knn_spec] if knn_spec is not None else []
         if knns and want.shape == got.shape:
             if self.encoding is not None:
@@ -718,7 +754,7 @@ class GpuKernelExplainer:
         rows = rows_per_call(self.spec.act_code, self.D, self.plan_mode, self.data.groups_size, self.spec.R)
         if self.encoding is not None:
             rows = min(rows, max(1, MAX_ENCODED_BYTES_PER_CALL // (8 * self.encoding.E)))
-        if isinstance(self.spec, (EnsembleSpec, TorchModelSpec)):
+        if isinstance(self.spec, (EnsembleSpec, StackingSpec, TorchModelSpec)):
             # the members' weighted background means (or the module's): C outputs x S rows per instance, S at most that
             # of all G groups
             S, _ = resolve_nsamples(self.data.groups_size, self._nsamples_req or "auto")
@@ -907,7 +943,7 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", None, "softmax", "affine", "ovr", "exp", "mixture"),   # 3: not used
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble", "torch"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble", "torch", "stacking"),
     }
 
     def last_path(self):
@@ -922,7 +958,9 @@ class GpuKernelExplainer:
         instance of a kernel machine, 'mlp': the MLP kernel, which takes every instance of a multi-layer perceptron, or
         'knn': the neighbour kernel, which takes every instance of a k-nearest-neighbour model, or 'ensemble': the
         members' kernels and the ensemble's tail, which take every instance of a soft-voting ensemble, or 'torch': the
-        ensemble's tail on the background means of a module's outputs, every instance of a module),
+        ensemble's tail on the background means of a module's outputs, every instance of a module, or 'stacking': per
+        background chunk the members' kernels and the final estimator's reduction, then the ensemble's tail, every
+        instance of a stacking ensemble),
         ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take

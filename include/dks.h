@@ -143,6 +143,12 @@ extern "C" {
                                 * only, explained stepwise by dks_external_* */
 #define DKS_EXTERNAL_FLOAT32 0       /* dtypes of the module's input rows and outputs */
 #define DKS_EXTERNAL_FLOAT64 1
+#define DKS_ACT_STACKING 12    /* stacking ensemble of the four families above: set by dks_set_stacking only */
+#define DKS_STACK_MAX_F 128          /* meta columns the final estimator reads: DKS_ENS_MAX_MEMBERS x DKS_ENS_MAX_OUT */
+/* head of a stacking ensemble's final estimator on its R scores r = W m + b (+ W_pass x) (dks_set_stacking) */
+#define DKS_STACK_HEAD_IDENTITY 0    /* outputs r (C = R): decision_function, a linear regressor's predict */
+#define DKS_STACK_HEAD_SIGMOID 1     /* R = 1, outputs [1 - expit(r), expit(r)] (C = 2): binary logistic predict_proba */
+#define DKS_STACK_HEAD_SOFTMAX 2     /* R = C >= 2, outputs softmax(r): multinomial logistic predict_proba */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -280,6 +286,22 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
  * DKS_ERR_DOMAIN with the row (NaN in an ensemble of trees only is explained); a link(ey) or link(f(x)) that is not finite
  * is DKS_ERR_NUMERIC and nothing non-finite is written into phi. */
 int dks_set_ensemble(dks_ctx* ctx, int K, dks_ctx* const* members, const double* weights, int C, int scalar_out);
+/* stacking ensemble (DKS_ACT_STACKING) in place of dks_set_model: outputs f(x) = head(W m(x) + b + W_pass x) of the final
+ * estimator (DKS_STACK_HEAD_*: R = C scores, or R = 1 and C = 2 under the sigmoid) over the meta columns m(x) [F]: outputs
+ * col_first[k] .. col_first[k] + col_count[k] - 1 of each of the K (1..DKS_ENS_MAX_MEMBERS) members in order, F = sum
+ * col_count <= DKS_STACK_MAX_F.  W [R][F], b [R] and W_pass [R][D] (passthrough over the columns the members read -- the
+ * encoded ones behind a column encoding -- or NULL) must be finite.  Members, ownership, stream, status word and dks_fit of
+ * the members follow dks_set_ensemble; fnull = sum_j w_j f(bg_j) in background order.  Every instance runs, per chunk
+ * j0 <= j < j1 of the background, the members' explain kernels (each storing its kept outputs of every masked row (s, j)
+ * into a workspace [n][F][j1 - j0][S_cap]) and stacking_reduce_kernel (the final estimator per row, ey(s) += w_j f), then
+ * explain_ensemble_tail_kernel (DKS_GENERAL_STACKING, DESIGN.md §5.0.20).  The chunks are the fewest whose workspace fits
+ * workspace_bytes (at least one background row each): chunks (K + 1) + 1 launches per call, phi bit-identical whatever the
+ * chunking.  Up to 64 groups, every plan source, kernel 'auto' or 'simt', l1 selection through the general list's LARS
+ * route; raw values and non-finite results are reported as for dks_set_ensemble.  Malformed input (non-finite weights,
+ * column ranges outside a member's outputs, F or R out of range, R not matching the head) is DKS_ERR_UNSUPPORTED. */
+int dks_set_stacking(dks_ctx* ctx, int K, dks_ctx* const* members, const int32_t* col_first, const int32_t* col_count,
+                     const double* W, const double* b, int R, int head, const double* W_pass, int C, int scalar_out,
+                     int64_t workspace_bytes);
 /* a model the engine cannot evaluate (DKS_ACT_EXTERNAL) in place of dks_set_model: C (1..DKS_ENS_MAX_OUT) outputs that the
  * caller computes on the device from rows of `dtype` (DKS_EXTERNAL_FLOAT32 / _FLOAT64) -- a torch.nn.Module (DESIGN.md
  * §5.0.19).  Before dks_fit, dks_set_external_background hands over the module's outputs on the N background rows, y_dev
@@ -543,6 +565,8 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
                                   * soft-voting ensemble (dks_set_ensemble) */
 #define DKS_GENERAL_EXTERNAL 10  /* explain_ensemble_tail_kernel on the means dks_external_reduce formed: every instance of a
                                   * module the caller runs (dks_set_external_model) */
+#define DKS_GENERAL_STACKING 11  /* per background chunk the members' explain kernels and stacking_reduce_kernel, then
+                                  * explain_ensemble_tail_kernel: every instance of a stacking ensemble (dks_set_stacking) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
