@@ -371,7 +371,15 @@ int check_own_columns(const dks_ctx* ctx, const OwnKernel& ok) {
                 return fail(DKS_ERR_UNSUPPORTED, "tree ensemble: a split reads column %d of %d %s", f, width,
                             E > 0 ? "encoded columns" : "columns");
         return DKS_OK;
-    case DKS_GENERAL_KMACH: reads = (int)(ctx->h_kcolw.size() / ctx->km.K); break;
+    case DKS_GENERAL_KMACH:
+        if (ctx->km.kernel == DKS_KM_KERNEL_PROGRAM) {
+            if (ctx->kprog.n == 0)
+                return fail(DKS_ERR_INVALID, "kernel machine: the program kernel needs dks_set_kernel_program before dks_fit");
+            reads = (int)(ctx->h_kpcolw.size() / ctx->kprog.L);
+            break;
+        }
+        reads = (int)(ctx->h_kcolw.size() / ctx->km.K);
+        break;
     case DKS_GENERAL_MLP: reads = ctx->mlp.width[0]; break;
     case DKS_GENERAL_ENSEMBLE: return DKS_OK;         // each member checks its own (fit_members)
     case DKS_GENERAL_STACKING:                        // each member checks its own; the passthrough reads every column
@@ -423,11 +431,21 @@ int own_fit_tables(dks_ctx* ctx, const double* bg, int width) {
     }
     case DKS_GENERAL_KMACH: {
         KmDev& k = ctx->km;
+        const bool prog = k.kernel == DKS_KM_KERNEL_PROGRAM;
         CUDA_TRY(pool.upload(&k.sv, ctx->h_ksv.data(), ctx->h_ksv.size(), st));
         CUDA_TRY(pool.upload(&k.dual, ctx->h_kdual.data(), ctx->h_kdual.size(), st));
-        CUDA_TRY(pool.upload(&k.colw, ctx->h_kcolw.data(), ctx->h_kcolw.size(), st));
-        CUDA_TRY(pool.upload(&k.colo, ctx->h_kcolo.data(), ctx->h_kcolo.size(), st));
+        const std::vector<double>& colw = prog ? ctx->h_kpcolw : ctx->h_kcolw;
+        const std::vector<double>& colo = prog ? ctx->h_kpcolo : ctx->h_kcolo;
+        CUDA_TRY(pool.upload(&k.colw, colw.data(), colw.size(), st));
+        CUDA_TRY(pool.upload(&k.colo, colo.data(), colo.size(), st));
         double* Tbg;
+        if (prog) {                 // T[j][v][l] of every statistic
+            const long long n = (long long)N * k.n_sv * ctx->kprog.L;
+            CUDA_TRY(pool.alloc(&Tbg, (size_t)n));
+            k.Tbg = Tbg;
+            dks::kmach::km_prog_fit_table_kernel<<<cdiv(n, 256), 256, 0, st>>>(bg, N, width, k, ctx->kprog, Tbg);
+            break;
+        }
         CUDA_TRY(pool.alloc(&Tbg, (size_t)N * k.n_sv));
         k.Tbg = Tbg;
         dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(bg, N, width, k, Tbg);
@@ -497,8 +515,12 @@ int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const
                                                                       ctx->d_status);
         break;
     case DKS_GENERAL_KMACH:
-        dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->km, C, link, linkfnull, out, dlink,
-                                                                    ctx->d_status);
+        if (ctx->km.kernel == DKS_KM_KERNEL_PROGRAM)
+            dks::kmach::km_prog_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->km, ctx->kprog, C, link,
+                                                                             linkfnull, out, dlink, ctx->d_status);
+        else
+            dks::kmach::km_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->km, C, link, linkfnull, out, dlink,
+                                                                        ctx->d_status);
         break;
     case DKS_GENERAL_MLP:           // one row per CTA, grid-stride
         dks::mlp::mlp_predict_kernel<<<std::max(1, std::min(n, ctx->sm_count * 8)), dks::mlp::THREADS, 0, st>>>(
@@ -581,12 +603,17 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         break;
     }
     case DKS_GENERAL_KMACH: {
-        auto kern = rows ? dks::kmach::explain_kmach_kernel<false, true, true>
+        auto kern = ctx->km.kernel == DKS_KM_KERNEL_PROGRAM
+                    ? (rows ? dks::kmach::explain_kmach_kernel<false, true, true, true>
+                       : acc ? dks::kmach::explain_kmach_kernel<false, true, false, true>
+                       : l1 ? dks::kmach::explain_kmach_kernel<true, false, false, true>
+                            : dks::kmach::explain_kmach_kernel<false, false, false, true>)
+                    : rows ? dks::kmach::explain_kmach_kernel<false, true, true>
                     : acc ? dks::kmach::explain_kmach_kernel<false, true>
                     : l1 ? dks::kmach::explain_kmach_kernel<true> : dks::kmach::explain_kmach_kernel<false>;
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->own_X, ctx->own_bg, ctx->own_D, ctx->own_goff,
-                                                      ctx->own_gcols, ea, er);
+                                                      ctx->own_gcols, ea, er, ctx->kprog);
         break;
     }
     case DKS_GENERAL_MLP: {
@@ -2239,8 +2266,10 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: K=%d members; 1..%d supported", K, DKS_KM_MAX_K);
     if (R < 1 || R > DKS_KM_MAX_R)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: R=%d outputs; 1..%d supported", R, DKS_KM_MAX_R);
-    if (kernel < DKS_KM_KERNEL_RBF || kernel > DKS_KM_KERNEL_SIGMOID)
+    if (kernel < DKS_KM_KERNEL_RBF || kernel > DKS_KM_KERNEL_PROGRAM)
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: unknown kernel %d", kernel);
+    if (kernel == DKS_KM_KERNEL_PROGRAM && (K != 1 || head != DKS_KM_HEAD_IDENTITY))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: the program kernel takes one member and the identity head");
     if (!std::isfinite(coef0) || !std::isfinite(degree) ||
         (kernel == DKS_KM_KERNEL_POLY && (degree < 0 || degree != std::floor(degree))))
         return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_machine: degree %g / coef0 %g (degree: an integer >= 0)", degree, coef0);
@@ -2290,7 +2319,66 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
     ctx->h_kdual.assign(dual, dual + (size_t)n_sv * R);
     ctx->h_kcolw.assign(colw, colw + (size_t)K * D);
     ctx->h_kcolo.assign(colo, colo + (size_t)K * D);
+    ctx->kprog = KmProg{};
+    ctx->h_kpcolw.clear(); ctx->h_kpcolo.clear();
     return set_own_model(ctx, DKS_ACT_KMACH, C, scalar_out);
+}
+
+int dks_set_kernel_program(dks_ctx* ctx, int L, const int32_t* kinds, const double* colw, const double* colo, int n_ops,
+                           const int32_t* ops, const int32_t* args, const double* a, const double* b) {
+    BIND(ctx);
+    REQUIRE(ctx->act == DKS_ACT_KMACH && ctx->km.kernel == DKS_KM_KERNEL_PROGRAM,
+            "dks_set_kernel_program: needs a kernel machine set with DKS_KM_KERNEL_PROGRAM (dks_set_kernel_machine)");
+    REQUIRE(kinds && colw && colo && ops && args && a && b,
+            "dks_set_kernel_program: need the statistic kinds, column weights and origins and the instructions");
+    const int D = model_columns(ctx);
+    if (L < 1 || L > DKS_KM_MAX_STATS)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: L=%d statistics; 1..%d supported", L, DKS_KM_MAX_STATS);
+    if (n_ops < 1 || n_ops > DKS_KM_MAX_OPS)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: %d instructions; 1..%d supported", n_ops, DKS_KM_MAX_OPS);
+    for (int l = 0; l < L; ++l)
+        if (kinds[l] != DKS_KM_STAT_SQDIST && kinds[l] != DKS_KM_STAT_DOT)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: unknown statistic kind %d", kinds[l]);
+    if (!all_finite(colw, (size_t)L * D) || !all_finite(colo, (size_t)L * D))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: the column weights and origins must be finite");
+    for (size_t e = 0; e < (size_t)L * D; ++e)
+        if (!(colw[e] > 0)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: column weights must be positive");
+    int depth = 0;
+    for (int i = 0; i < n_ops; ++i) {
+        const int op = ops[i];
+        if (op < DKS_KM_OP_CONST || op > DKS_KM_OP_MULC)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: unknown instruction %d at %d", op, i);
+        if (!std::isfinite(a[i]) || !std::isfinite(b[i]))
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: non-finite constant at instruction %d", i);
+        if (op == DKS_KM_OP_EXPSINE && (a[i] == 0.0 || b[i] == 0.0))
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: zero periodicity or length scale at instruction %d", i);
+        if (op >= DKS_KM_OP_CONST && op <= DKS_KM_OP_EXPSINE) {
+            if (op != DKS_KM_OP_CONST && (args[i] < 0 || args[i] >= L))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: statistic %d at instruction %d (L=%d)", args[i], i, L);
+            if (++depth > DKS_KM_MAX_STACK)
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: more than %d operands at instruction %d",
+                            DKS_KM_MAX_STACK, i);
+        } else if (op == DKS_KM_OP_ADD || op == DKS_KM_OP_MUL) {
+            if (--depth < 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: stack underflow at instruction %d", i);
+        } else if (depth < 1) {
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: stack underflow at instruction %d", i);
+        }
+    }
+    if (depth != 1)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_kernel_program: the expression leaves %d values (1 expected)", depth);
+    KmProg g = {};
+    g.L = L; g.n = n_ops;
+    for (int l = 0; l < L; ++l) g.kind[l] = kinds[l];
+    for (int i = 0; i < n_ops; ++i) {
+        g.op[i] = (signed char)ops[i];
+        g.arg[i] = (signed char)(ops[i] == DKS_KM_OP_CONST || ops[i] > DKS_KM_OP_EXPSINE ? 0 : args[i]);
+        g.a[i] = a[i]; g.b[i] = b[i];
+    }
+    ctx->kprog = g;
+    ctx->h_kpcolw.assign(colw, colw + (size_t)L * D);
+    ctx->h_kpcolo.assign(colo, colo + (size_t)L * D);
+    ctx->fitted = false;
+    return DKS_OK;
 }
 
 int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double* W_host, const double* b_host, int activation,

@@ -278,6 +278,16 @@ struct KmDev {
     int K, R, n_sv, kernel, head;
 };
 
+// the program kernel of a kernel machine (DKS_KM_KERNEL_PROGRAM, dks_set_kernel_program, DESIGN.md §5.0.21): L statistics of
+// kind kind[l] (DKS_KM_STAT_*), whose column weights and origins are KmDev's colw / colo rows l, and a postfix expression of
+// n instructions {op, arg, a, b} (DKS_KM_OP_*) over them.  KmDev's Tbg is then [N][n_sv][L].
+struct KmProg {
+    double a[DKS_KM_MAX_OPS], b[DKS_KM_MAX_OPS];
+    signed char op[DKS_KM_MAX_OPS], arg[DKS_KM_MAX_OPS];
+    int kind[DKS_KM_MAX_STATS];
+    int L, n;                    // n = 0: no program
+};
+
 // multi-layer perceptrons (dks_set_mlp, DESIGN.md §5.0.14): L = hidden + 1 weight layers, layer l mapping width[l] units to
 // width[l + 1] (width[0] = D raw columns, width[L] = R outputs).  The explain kernel reads layers 1 .. L - 1 in the FP64 mma
 // B-fragment order, zero-padded to pad[l] x pad[l + 1] (hidden widths to a multiple of 16, the output layer to 8): padding
@@ -428,7 +438,9 @@ struct dks_ctx {
     const int32_t *own_goff = nullptr, *own_gcols = nullptr;
     // kernel machine (act == DKS_ACT_KMACH): host copies of the arrays, and their device copies built by dks_fit
     std::vector<double> h_ksv, h_kdual, h_kcolw, h_kcolo;
+    std::vector<double> h_kpcolw, h_kpcolo;     // the program kernel's [L][D] column weights and origins
     KmDev km = {};
+    KmProg kprog = {};
     // multi-layer perceptron (act == DKS_ACT_MLP): host copies of the layers (natural, fragment-ordered, padded biases), and
     // their device copies built by dks_fit
     std::vector<double> h_mw, h_mb, h_mwf, h_mbp;

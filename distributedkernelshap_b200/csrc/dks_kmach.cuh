@@ -8,6 +8,8 @@
 //   Delta_j[p][v] = sum_{c in group p} h(x_c, v_c) - h(bg_j,c, v_c)                  (per instance and row).
 // Per (j, tile of support vectors) the Delta go into nibble tables (16 partial sums per 4 varying groups), so one masked
 // forward pass costs ceil(M / 4) table reads and one phi per support vector, whatever the number of columns.
+// The program kernel (DKS_KM_KERNEL_PROGRAM, KmProg, DESIGN.md §5.0.21) carries L <= 4 such statistics, each with its own
+// column weights and origins, and evaluates a postfix expression of them per support vector: L ceil(M / 4) table reads.
 #pragma once
 
 #include "dks_kernels.cuh"
@@ -39,6 +41,83 @@ __device__ __forceinline__ void cal_member(double z, double* p0, double* p1) {
     const double big = 1.0 / (1.0 + e), small = e / (1.0 + e);
     *p1 = z >= 0 ? small : big;
     *p0 = z >= 0 ? big : small;
+}
+
+// per-column term of a program statistic (DKS_KM_STAT_*): the rbf and dot-product terms above
+__device__ __forceinline__ double km_stat_term(int kind, double m, double v, double w, double o) {
+    return km_term(kind == DKS_KM_STAT_SQDIST ? DKS_KM_KERNEL_RBF : DKS_KM_KERNEL_POLY, m, v, w, o);
+}
+
+// K(x, v) of the program kernel from the statistics t[L].  The operand stack is four registers shifted on every push and
+// pop (indices known at compile time: nothing goes to local memory); t is read through unrolled selects for the same reason.
+// A squared distance formed from tables can come out a rounding below zero: the square roots clamp it.
+__device__ __forceinline__ double km_program(const KmProg& g, const double* t) {
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+    for (int pc = 0; pc < g.n; ++pc) {
+        const int op = g.op[pc];
+        const double a = g.a[pc];
+        if (op == DKS_KM_OP_ADD || op == DKS_KM_OP_MUL) {
+            s0 = op == DKS_KM_OP_ADD ? s1 + s0 : s1 * s0;
+            s1 = s2; s2 = s3;
+            continue;
+        }
+        if (op == DKS_KM_OP_POW) { s0 = pow(s0, a); continue; }
+        if (op == DKS_KM_OP_ADDC) { s0 = s0 + a; continue; }
+        if (op == DKS_KM_OP_MULC) { s0 = s0 * a; continue; }
+        const int l = g.arg[pc];
+        double tl = t[0];
+#pragma unroll
+        for (int q = 1; q < DKS_KM_MAX_STATS; ++q)
+            if (l == q) tl = t[q];
+        double v;
+        if (op == DKS_KM_OP_CONST) {
+            v = a;
+        } else if (op == DKS_KM_OP_STAT) {
+            v = tl;
+        } else if (op == DKS_KM_OP_EXP) {
+            v = exp(-a * tl);
+        } else if (op == DKS_KM_OP_RQ) {
+            v = pow(1.0 + tl, a);
+        } else {
+            const double r = sqrt(fmax(tl, 0.0));
+            if (op == DKS_KM_OP_MATERN05) {
+                v = exp(-r);
+            } else if (op == DKS_KM_OP_MATERN15) {
+                const double k = r * 1.7320508075688772;
+                v = (1.0 + k) * exp(-k);
+            } else if (op == DKS_KM_OP_MATERN25) {
+                const double k = r * 2.23606797749979;
+                v = (1.0 + k + k * k / 3.0) * exp(-k);
+            } else {
+                const double sn = sin(3.141592653589793 * r / a) / g.b[pc];
+                v = exp(-2.0 * (sn * sn));
+            }
+        }
+        s3 = s2; s2 = s1; s1 = s0; s0 = v;
+    }
+    return s0;
+}
+
+// outputs o[R] of one row under the program kernel (identity head, one member): t_l per statistic, columns in order
+__device__ inline void km_prog_outputs(const KmDev& k, const KmProg& g, const double* __restrict__ x, int D, double* o) {
+    double f[DKS_KM_MAX_R];
+    for (int q = 0; q < k.R; ++q) f[q] = 0.0;
+    for (int v = 0; v < k.n_sv; ++v) {
+        const double* sv = k.sv + (size_t)v * D;
+        double t[DKS_KM_MAX_STATS];
+#pragma unroll
+        for (int l = 0; l < DKS_KM_MAX_STATS; ++l) {
+            t[l] = 0.0;
+            if (l < g.L) {
+                const double* w = k.colw + (size_t)l * D;
+                const double* org = k.colo + (size_t)l * D;
+                for (int c = 0; c < D; ++c) t[l] += km_stat_term(g.kind[l], x[c], sv[c], w[c], org[c]);
+            }
+        }
+        const double kv = km_program(g, t);
+        for (int q = 0; q < k.R; ++q) f[q] = fma(k.dual[(size_t)v * k.R + q], kv, f[q]);
+    }
+    for (int q = 0; q < k.R; ++q) o[q] = f[q] + k.icpt[q];
 }
 
 // outputs o[C] of one row: member scores summed over support vectors in order, then the head
@@ -104,6 +183,42 @@ __global__ void km_fit_table_kernel(const double* __restrict__ bg, int N, int D,
     Tbg[idx] = t;
 }
 
+// km_predict_kernel under the program kernel
+__global__ void km_prog_predict_kernel(const double* __restrict__ X, int n, int D, KmDev k, KmProg g, int C, int link,
+                                       const double* __restrict__ linkfnull, double* __restrict__ out,
+                                       double* __restrict__ dlink, int* __restrict__ status) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double* x = X + (size_t)i * D;
+    bool nan = false;
+    for (int c = 0; c < D; ++c) nan |= isnan(x[c]);
+    double o[DKS_KM_MAX_R];
+    if (nan) {
+        for (int c = 0; c < C; ++c) o[c] = NAN;
+        if (status) report_status(status, DKS_ERR_DOMAIN, i);
+    } else {
+        km_prog_outputs(k, g, x, D, o);
+    }
+    predict_epilogue(o, C, i, link, linkfnull, out, dlink, status, nan);
+}
+
+// fit under the program kernel: T[j][v][l] = sum_c h_l(bg_j,c, v_c), columns in order
+__global__ void km_prog_fit_table_kernel(const double* __restrict__ bg, int N, int D, KmDev k, KmProg g,
+                                         double* __restrict__ Tbg) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)N * k.n_sv * g.L) return;
+    const long long jv = idx / g.L;
+    const int l = (int)(idx - jv * g.L);
+    const int j = (int)(jv / k.n_sv), v = (int)(jv - (long long)j * k.n_sv);
+    const double* w = k.colw + (size_t)l * D;
+    const double* org = k.colo + (size_t)l * D;
+    const double* sv = k.sv + (size_t)v * D;
+    const double* b = bg + (size_t)j * D;
+    double t = 0.0;
+    for (int c = 0; c < D; ++c) t += km_stat_term(g.kind[l], b[c], sv[c], w[c], org[c]);
+    Tbg[idx] = t;
+}
+
 // doubles of the per-tile tables: T_j [TILE], dual [TILE][R], Delta [G][TILE], nibble tables [ceil(G/4)][TILE][16]
 __host__ __device__ inline size_t tile_doubles(int R, int G) {
     return (size_t)TILE * (1 + R + G + 16 * ((G + 3) / 4));
@@ -133,11 +248,15 @@ __host__ __device__ inline size_t smem_bytes(int S_cap, int C, int R, int G, boo
 // ROWS (a stacking ensemble's member, with ACC): per background row of the chunk the sums are formed at unit weight from
 // zero -- each coalition's outputs -- and go to er.ws (rows_store), each thread storing the coalitions it owns; nothing is
 // summed over the background.
-template <bool L1, bool ACC = false, bool ROWS = false>
+// PROG (the program kernel, identity head): a tile holds TILE / L support vectors, and its T, Delta and nibble-table columns
+// are (statistic l, support vector v) at l nv + v, so the tables of L statistics fill the shared memory of one; per
+// coalition and support vector the L statistics are read from the tables and the expression gives the kernel value.
+template <bool L1, bool ACC = false, bool ROWS = false, bool PROG = false>
 __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p, SimtL1 q, KmDev k,
                                                                 const double* __restrict__ X, const double* __restrict__ bg,
                                                                 int D, const int* __restrict__ goff,
-                                                                const int* __restrict__ gcols, EnsAcc ea, EnsRows er) {
+                                                                const int* __restrict__ gcols, EnsAcc ea, EnsRows er,
+                                                                KmProg g) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int tid = threadIdx.x;
     const int N = p.N, G = p.G, C = p.C, R = k.R;
@@ -206,10 +325,34 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
                 const double gm = k.gamma[m];
                 const double* w = k.colw + (size_t)m * D;
                 const double* org = k.colo + (size_t)m * D;
-                for (int v0 = k.sv_off[m]; v0 < k.sv_off[m + 1]; v0 += TILE) {
-                    const int nv = min(TILE, k.sv_off[m + 1] - v0);
-                    for (int idx = tid; idx < nv; idx += blockDim.x) tj[idx] = k.Tbg[(size_t)j * k.n_sv + v0 + idx];
+                const int tw = PROG ? TILE / g.L : TILE;        // support vectors per tile
+                for (int v0 = k.sv_off[m]; v0 < k.sv_off[m + 1]; v0 += tw) {
+                    const int nv = min(tw, k.sv_off[m + 1] - v0);
+                    const int ncol = PROG ? g.L * nv : nv;      // table columns
+                    if constexpr (PROG) {
+                        for (int idx = tid; idx < ncol; idx += blockDim.x) {
+                            const int l = idx / nv, v = idx - l * nv;
+                            tj[idx] = k.Tbg[((size_t)j * k.n_sv + v0 + v) * g.L + l];
+                        }
+                    } else {
+                        for (int idx = tid; idx < nv; idx += blockDim.x) tj[idx] = k.Tbg[(size_t)j * k.n_sv + v0 + idx];
+                    }
                     for (int idx = tid; idx < nv * R; idx += blockDim.x) du[idx] = k.dual[(size_t)v0 * R + idx];
+                    if constexpr (PROG) {
+                        for (int idx = tid; idx < M * ncol; idx += blockDim.x) {
+                            const int pp = idx / ncol, col = idx - pp * ncol, l = col / nv, v = col - l * nv, g0 = vi[pp];
+                            const double* sv = k.sv + (size_t)(v0 + v) * D;
+                            const double* wl = k.colw + (size_t)l * D;
+                            const double* ol = k.colo + (size_t)l * D;
+                            const int kind = g.kind[l];
+                            double d = 0.0;
+                            for (int e = goff[g0]; e < goff[g0 + 1]; ++e) {
+                                const int c = gcols[e];
+                                d += km_stat_term(kind, x[c], sv[c], wl[c], ol[c]) - km_stat_term(kind, b[c], sv[c], wl[c], ol[c]);
+                            }
+                            dl[(size_t)pp * TILE + col] = d;
+                        }
+                    } else
                     for (int idx = tid; idx < M * nv; idx += blockDim.x) {
                         const int pp = idx / nv, v = idx - pp * nv, g = vi[pp];
                         const double* sv = k.sv + (size_t)(v0 + v) * D;
@@ -221,8 +364,8 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
                         dl[(size_t)pp * TILE + v] = d;
                     }
                     __syncthreads();
-                    for (int idx = tid; idx < nib * nv * 16; idx += blockDim.x) {
-                        const int qn = idx / (nv * 16), rem = idx - qn * nv * 16, v = rem >> 4, pat = rem & 15;
+                    for (int idx = tid; idx < nib * ncol * 16; idx += blockDim.x) {
+                        const int qn = idx / (ncol * 16), rem = idx - qn * ncol * 16, v = rem >> 4, pat = rem & 15;
                         double t = 0.0;
                         for (int bit = 0; bit < 4; ++bit)
                             if (((pat >> bit) & 1) && 4 * qn + bit < M) t += dl[(size_t)(4 * qn + bit) * TILE + v];
@@ -234,6 +377,25 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
                         double f[DKS_KM_MAX_R];
 #pragma unroll
                         for (int r = 0; r < DKS_KM_MAX_R; ++r) f[r] = 0.0;
+                        if constexpr (PROG) {
+                            for (int v = 0; v < nv; ++v) {
+                                double t[DKS_KM_MAX_STATS];
+#pragma unroll
+                                for (int l = 0; l < DKS_KM_MAX_STATS; ++l) {
+                                    t[l] = 0.0;
+                                    if (l < g.L) {
+                                        const int col = l * nv + v;
+                                        t[l] = tj[col];
+                                        for (int qn = 0; qn < nib; ++qn)
+                                            t[l] += tb[((size_t)qn * TILE + col) * 16 + ((z >> (4 * qn)) & 15)];
+                                    }
+                                }
+                                const double kv = km_program(g, t);
+#pragma unroll
+                                for (int r = 0; r < DKS_KM_MAX_R; ++r)
+                                    if (r < R) f[r] = fma(du[v * R + r], kv, f[r]);
+                            }
+                        } else
                         for (int v = 0; v < nv; ++v) {
                             double t = tj[v];
                             for (int qn = 0; qn < nib; ++qn) t += tb[((size_t)qn * TILE + v) * 16 + ((z >> (4 * qn)) & 15)];

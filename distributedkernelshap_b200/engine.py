@@ -363,6 +363,13 @@ class GpuKernelExplainer:
                 ctx, k.K, _cabi.ptr(k.sv_off), _cabi.ptr(k.sv), _cabi.ptr(k.dual), k.R, _cabi.ptr(k.intercept),
                 _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree, k.coef0, k.head_code,
                 _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
+            if k.program is not None:
+                g = k.program
+                ops, args, a, b = g.flat()
+                kinds = g.kind_codes
+                _cabi.check(self.lib.dks_set_kernel_program(ctx, g.L, _cabi.ptr(kinds), _cabi.ptr(g.colw),
+                                                            _cabi.ptr(g.colo), len(ops), _cabi.ptr(ops),
+                                                            _cabi.ptr(args), _cabi.ptr(a), _cabi.ptr(b)))
         else:
             t = own
             _cabi.check(self.lib.dks_set_tree_model(

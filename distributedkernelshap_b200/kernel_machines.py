@@ -21,6 +21,13 @@ Member score ``f_k = sum_v dual[v] phi(t(x, v)) + intercept_k``; heads:
 * calibrated: ``CalibratedClassifierCV(SVC | NuSVC, method='sigmoid')`` ``predict_proba`` over two classes,
   ``p1 = sum_k pi_k expit(-(a_k f_k + b_k))`` with ``pi_k = 1 / K``, outputs ``[1 - p1, p1]``.
 
+Gaussian-process regressors (``predict``: ``K(x, X_train_) alpha_``, un-normalised), ``KernelRidge`` with a scikit-learn
+``Kernel`` object and one-class SVMs (``decision_function``, ``score_samples``) share the identity head.  A one-class SVM
+with ``rbf`` / ``poly`` / ``sigmoid`` takes the kernels above; a ``Kernel`` object (scikit-learn's kernel algebra) is read
+into the ``program`` kernel: at most ``MAX_STATS`` additive statistics, each ``sqdist`` (``h = w_c (x_c - v_c)^2``) or
+``dot`` (``h = w_c (x_c - o_c)(v_c - o_c)``) with its own column weights and origins, and a short postfix expression over
+them (``KernelProgram``, ``dks_set_kernel_program``).
+
 ``KernelMachineSpec.__call__`` evaluates the same thing in NumPy.
 """
 import numpy as np
@@ -28,13 +35,120 @@ import numpy as np
 MAX_OUTPUTS = 8
 MAX_MEMBERS = 16
 MAX_GROUPS = 64
-KERNELS = ("rbf", "laplacian", "poly", "sigmoid")     # DKS_KM_KERNEL_* codes 0..3
+KERNELS = ("rbf", "laplacian", "poly", "sigmoid", "program")  # DKS_KM_KERNEL_* codes 0..4
 HEADS = ("identity", "calibrated")                    # DKS_KM_HEAD_* codes 0..1
+STATS = ("sqdist", "dot")                             # DKS_KM_STAT_* codes 0..1
+OPS = ("const", "stat", "exp", "matern05", "matern15", "matern25", "rq", "expsine", "add", "mul", "pow", "addc",
+       "mulc")                                        # DKS_KM_OP_* codes 0..12
+MAX_STATS = 4                                         # DKS_KM_MAX_STATS
+MAX_OPS = 32                                          # DKS_KM_MAX_OPS
+MAX_STACK = 4                                         # DKS_KM_MAX_STACK
 
 _SVM_CLASSIFIERS = {"SVC", "NuSVC"}
 _SVM_REGRESSORS = {"SVR", "NuSVR"}
 _KRR = {"KernelRidge"}
-_KERNEL_MACHINES = _SVM_CLASSIFIERS | _SVM_REGRESSORS | _KRR
+_GPR = {"GaussianProcessRegressor"}
+_OCSVM = {"OneClassSVM"}
+_KERNEL_MACHINES = _SVM_CLASSIFIERS | _SVM_REGRESSORS | _KRR | _GPR | _OCSVM
+# leaves and operators of scikit-learn's kernel algebra the program kernel reads
+_GP_KERNELS = {"RBF", "Matern", "RationalQuadratic", "ExpSineSquared", "DotProduct", "ConstantKernel", "WhiteKernel", "Sum",
+               "Product", "Exponentiation"}
+_MATERN_OPS = {0.5: "matern05", 1.5: "matern15", 2.5: "matern25"}
+
+
+class KernelProgram:
+    """The kernel of a ``Kernel`` object as L <= ``MAX_STATS`` additive statistics and a postfix expression over them.
+
+    kinds [L] in ``STATS``; colw / colo [L, D] (column weights and origins, scalers folded in); ops: a list of
+    ``(op, arg, a, b)`` with op in ``OPS``.  Leaves push a value: ``const`` a; ``stat`` t_arg; ``exp`` exp(-a t);
+    ``matern05/15/25`` scikit-learn's closed forms of r = sqrt(t); ``rq`` (1 + t)^a; ``expsine``
+    exp(-2 (sin(pi r / a) / b)^2).  ``add`` / ``mul`` pop two, ``pow`` / ``addc`` / ``mulc`` apply a to the top."""
+
+    def __init__(self, kinds, colw, colo, ops):
+        self.kinds = list(kinds)
+        self.colw = np.ascontiguousarray(np.asarray(colw, dtype=np.float64).reshape(len(self.kinds), -1))
+        self.colo = np.ascontiguousarray(np.asarray(colo, dtype=np.float64).reshape(len(self.kinds), -1))
+        self.ops = [(str(o), int(g), float(a), float(b)) for o, g, a, b in ops]
+        if not 1 <= self.L <= MAX_STATS:
+            raise NotImplementedError(f"a kernel of {self.L} statistics: the program kernel takes 1 to {MAX_STATS}")
+        if len(self.ops) > MAX_OPS:
+            raise NotImplementedError(f"a kernel expression of {len(self.ops)} operations: up to {MAX_OPS} are supported")
+        if self.depth() > MAX_STACK:
+            raise NotImplementedError(f"a kernel expression {self.depth()} operands deep: up to {MAX_STACK} are supported")
+
+    @property
+    def L(self):
+        return len(self.kinds)
+
+    def depth(self):
+        d = top = 0
+        for op, *_ in self.ops:
+            top += 1 if op in ("const", "stat", "exp", "matern05", "matern15", "matern25", "rq", "expsine") else (
+                -1 if op in ("add", "mul") else 0)
+            d = max(d, top)
+        return d
+
+    @property
+    def kind_codes(self):
+        return np.asarray([STATS.index(k) for k in self.kinds], dtype=np.int32)
+
+    def flat(self):
+        """(op codes [n], args [n] int32, a [n], b [n] float64) for ``dks_set_kernel_program``."""
+        return (np.asarray([OPS.index(o[0]) for o in self.ops], dtype=np.int32),
+                np.asarray([o[1] for o in self.ops], dtype=np.int32),
+                np.asarray([o[2] for o in self.ops], dtype=np.float64),
+                np.asarray([o[3] for o in self.ops], dtype=np.float64))
+
+    def statistics(self, X, V):
+        """t_l [n, n_v] of the rows of X against the rows V, per statistic."""
+        out = []
+        for kind, w, o in zip(self.kinds, self.colw, self.colo):
+            if kind == "sqdist":
+                out.append(((X[:, None, :] - V[None, :, :]) ** 2 * w).sum(axis=2))
+            else:
+                out.append(((X - o) * w) @ (V - o).T)
+        return out
+
+    def __call__(self, t):
+        """Kernel values of the statistics t (list of arrays), in the device's order."""
+        st = []
+        for op, g, a, b in self.ops:
+            if op == "const":
+                st.append(np.full(t[0].shape, a))
+            elif op == "stat":
+                st.append(t[g])
+            elif op == "exp":
+                st.append(np.exp(-a * t[g]))
+            elif op in ("matern05", "matern15", "matern25", "expsine"):
+                r = np.sqrt(np.maximum(t[g], 0.0))
+                if op == "matern05":
+                    st.append(np.exp(-r))
+                elif op == "matern15":
+                    k = r * np.sqrt(3.0)
+                    st.append((1.0 + k) * np.exp(-k))
+                elif op == "matern25":
+                    k = r * np.sqrt(5.0)
+                    st.append((1.0 + k + k * k / 3.0) * np.exp(-k))
+                else:
+                    st.append(np.exp(-2.0 * (np.sin(np.pi * r / a) / b) ** 2))
+            elif op == "rq":
+                st.append((1.0 + t[g]) ** a)
+            elif op in ("add", "mul"):
+                y = st.pop()
+                st[-1] = st[-1] + y if op == "add" else st[-1] * y
+            elif op == "pow":
+                st[-1] = st[-1] ** a
+            elif op == "addc":
+                st[-1] = st[-1] + a
+            else:
+                st[-1] = st[-1] * a
+        return st[0]
+
+    def folded(self, a, b):
+        """The program behind one more affine map x' = a x + b of its raw columns."""
+        return KernelProgram(self.kinds, self.colw * a * a,
+                             np.stack([(o - b) / a if k == "dot" else o for k, o in zip(self.kinds, self.colo)]),
+                             self.ops)
 _SCALERS = {"StandardScaler", "MinMaxScaler", "MaxAbsScaler", "RobustScaler"}
 
 
@@ -50,7 +164,7 @@ class KernelMachineSpec:
     maps = None
 
     def __init__(self, sv, sv_off, dual, intercept, colw, colo, gamma, kernel, degree, coef0, head, n_features,
-                 cal_a=None, cal_b=None, pi=None, scalar_out=False):
+                 cal_a=None, cal_b=None, pi=None, scalar_out=False, program=None):
         self.sv = np.ascontiguousarray(np.atleast_2d(sv), dtype=np.float64)
         self.sv_off = np.ascontiguousarray(sv_off, dtype=np.int32)
         self.dual = np.ascontiguousarray(np.asarray(dual, dtype=np.float64).reshape(self.sv.shape[0], -1))
@@ -66,8 +180,11 @@ class KernelMachineSpec:
         self.head = head
         self.n_features = int(n_features)
         self.scalar_out = bool(scalar_out)
+        self.program = program
         if kernel not in KERNELS:
             raise ValueError(f"unknown kernel {kernel!r}")
+        if (kernel == "program") != (program is not None) or (program is not None and (head != "identity" or self.K != 1)):
+            raise ValueError("the program kernel takes a KernelProgram, one member and the identity head")
         if head not in HEADS:
             raise ValueError(f"unknown kernel-machine head {head!r}")
         if head == "calibrated":
@@ -116,7 +233,10 @@ class KernelMachineSpec:
         X = np.atleast_2d(np.asarray(X, dtype=np.float64))
         out = np.empty((X.shape[0], self.K, self.R))
         for k in range(self.K):
-            Kv = self.kernel_values(self.statistic(X, k), k)
+            if self.program is not None:
+                Kv = self.program(self.program.statistics(X, self.sv[self.sv_off[k]:self.sv_off[k + 1]]))
+            else:
+                Kv = self.kernel_values(self.statistic(X, k), k)
             out[:, k, :] = Kv @ self.dual[self.sv_off[k]:self.sv_off[k + 1]] + self.intercept[k]
         return out
 
@@ -145,12 +265,135 @@ def _final(est):
 
 
 def _is_kernel_machine(est):
-    """A kernel machine with a non-linear kernel (linear SVMs stay on the linear route)."""
+    """A kernel machine with a non-linear kernel (linear SVMs stay on the linear route), a Gaussian process (classifiers
+    included: the extractor refuses them by name) or a one-class SVM."""
     est = _final(est)
     names = _names(est)
     if names & (_SVM_CLASSIFIERS | _SVM_REGRESSORS):
         return getattr(est, "kernel", None) != "linear"
-    return bool(names & _KRR)
+    return bool(names & (_KRR | _GPR | _OCSVM | {"GaussianProcessClassifier"}))
+
+
+def _is_kernel_object(k):
+    """A scikit-learn ``gaussian_process.kernels.Kernel`` (any subclass)."""
+    return any(c.__name__ == "Kernel" and c.__module__ == "sklearn.gaussian_process.kernels" for c in type(k).__mro__)
+
+
+def _kernel_tree(k, P, stats):
+    """Expression tree of a scikit-learn kernel object over the columns it reads; ``stats`` collects the statistics
+    ``(kind, colw)`` the leaves read (equal ones shared).  Constants fold."""
+    name = type(k).__name__
+    if type(k).__module__ != "sklearn.gaussian_process.kernels" or name not in _GP_KERNELS:
+        what = "a user-defined kernel" if type(k).__module__ != "sklearn.gaussian_process.kernels" else name
+        raise NotImplementedError(f"{what} ({name}) is not supported: the kernel-machine route reads "
+                                  f"{', '.join(sorted(_GP_KERNELS))}")
+
+    def stat(kind, w):
+        w = np.ascontiguousarray(np.broadcast_to(np.asarray(w, dtype=np.float64), (P,)))
+        for i, (kd, sw) in enumerate(stats):
+            if kd == kind and np.array_equal(sw, w):
+                return i
+        stats.append((kind, w))
+        return len(stats) - 1
+
+    def scales(ls):
+        ls = np.asarray(ls, dtype=np.float64)
+        if ls.ndim > 0 and ls.size != P:
+            raise NotImplementedError(f"{name} with {ls.size} length scales over {P} columns")
+        return ls
+
+    if name in ("Sum", "Product"):
+        x, y = _kernel_tree(k.k1, P, stats), _kernel_tree(k.k2, P, stats)
+        return _node_add(x, y) if name == "Sum" else _node_mul(x, y)
+    if name == "Exponentiation":
+        return _node_pow(_kernel_tree(k.kernel, P, stats), float(k.exponent))
+    if name == "ConstantKernel":
+        return ("c", float(k.constant_value))
+    if name == "WhiteKernel":
+        return ("c", 0.0)                               # k(X, Y) is zero whenever Y is given (every prediction)
+    if name == "DotProduct":
+        return _node_add(("leaf", "stat", stat("dot", 1.0), 0.0, 0.0), ("c", float(k.sigma_0) ** 2))
+    if name == "ExpSineSquared":
+        return ("leaf", "expsine", stat("sqdist", 1.0), float(k.periodicity), float(k.length_scale))
+    if name == "RationalQuadratic":
+        ls, al = float(k.length_scale), float(k.alpha)
+        return ("leaf", "rq", stat("sqdist", 1.0 / (2.0 * al * ls ** 2)), -al, 0.0)
+    ls = scales(k.length_scale)
+    if name == "RBF":
+        return ("leaf", "exp", stat("sqdist", 1.0 / ls ** 2), 0.5, 0.0)
+    nu = float(k.nu)                                    # Matern
+    if np.isinf(nu):
+        return ("leaf", "exp", stat("sqdist", 1.0 / ls ** 2), 0.5, 0.0)
+    if nu not in _MATERN_OPS:
+        raise NotImplementedError(f"Matern(nu={nu!r}) is not supported: nu 0.5, 1.5, 2.5 and inf have closed forms, "
+                                  "others need a Bessel function")
+    return ("leaf", _MATERN_OPS[nu], stat("sqdist", 1.0 / ls ** 2), 0.0, 0.0)
+
+
+def _node_add(x, y):
+    if x[0] == "c" and y[0] == "c":
+        return ("c", x[1] + y[1])
+    if x[0] == "c":
+        x, y = y, x
+    if y[0] == "c":
+        return x if y[1] == 0.0 else ("addc", x, y[1])
+    return ("add", x, y)
+
+
+def _node_mul(x, y):
+    if x[0] == "c" and y[0] == "c":
+        return ("c", x[1] * y[1])
+    if x[0] == "c":
+        x, y = y, x
+    if y[0] == "c":
+        return x if y[1] == 1.0 else (("c", 0.0) if y[1] == 0.0 else ("mulc", x, y[1]))
+    return ("mul", x, y)
+
+
+def _node_pow(x, e):
+    if x[0] == "c":
+        return ("c", x[1] ** e)
+    return x if e == 1.0 else ("pow", x, e)
+
+
+def _need(n):
+    """Stack slots the postfix form of node n needs (Sethi-Ullman: the deeper operand goes first)."""
+    if n[0] in ("c", "leaf"):
+        return 1
+    if n[0] in ("addc", "mulc", "pow"):
+        return _need(n[1])
+    a, b = _need(n[1]), _need(n[2])
+    return a + 1 if a == b else max(a, b)
+
+
+def _emit(n, out):
+    if n[0] == "c":
+        out.append(("const", 0, n[1], 0.0))
+    elif n[0] == "leaf":
+        out.append((n[1], n[2], n[3], n[4]))
+    elif n[0] in ("addc", "mulc", "pow"):
+        _emit(n[1], out)
+        out.append((n[0], 0, n[2], 0.0))
+    else:
+        x, y = (n[1], n[2]) if _need(n[1]) >= _need(n[2]) else (n[2], n[1])
+        _emit(x, out)
+        _emit(y, out)
+        out.append((n[0], 0, 0.0, 0.0))
+
+
+def _kernel_program(kernel, P):
+    """``KernelProgram`` of a scikit-learn kernel object over P columns (no scalers folded yet)."""
+    stats = []
+    tree = _kernel_tree(kernel, P, stats)
+    if tree[0] == "c":
+        raise NotImplementedError(f"the kernel {kernel!r} is constant on every prediction: the model does not depend on "
+                                  "its input")
+    if len(stats) > MAX_STATS:
+        raise NotImplementedError(f"the kernel {kernel!r} reads {len(stats)} statistics: the program kernel takes up to "
+                                  f"{MAX_STATS}")
+    ops = []
+    _emit(tree, ops)
+    return KernelProgram([kd for kd, _ in stats], np.stack([w for _, w in stats]), np.zeros((len(stats), P)), ops)
 
 
 def _affine(step, family="kernel machine"):
@@ -201,6 +444,15 @@ def _kernel_params(est, P):
     """(kernel, gamma, degree, coef0) resolved as scikit-learn evaluates them."""
     name = type(est).__name__
     kernel = est.kernel
+    if name in _KRR and _is_kernel_object(kernel):
+        if getattr(est, "kernel_params", None):
+            raise NotImplementedError("KernelRidge with kernel_params is not supported")
+        return "program", 0.0, 0.0, 0.0
+    if _is_kernel_object(kernel):
+        raise NotImplementedError(f"{name}(kernel={type(kernel).__name__}(...)) is not supported: kernel objects are read "
+                                  "for GaussianProcessRegressor and KernelRidge only")
+    if name in _OCSVM and kernel in ("linear", "precomputed"):
+        raise NotImplementedError(f"OneClassSVM(kernel={kernel!r}) is not supported: kernels 'rbf', 'poly' and 'sigmoid'")
     if callable(kernel) or kernel == "precomputed":
         raise NotImplementedError(f"{name}(kernel={'a callable' if callable(kernel) else repr(kernel)}) is not supported: "
                                   f"kernels {KERNELS[0]!r}, {KERNELS[2]!r}, {KERNELS[3]!r} (and 'laplacian' for "
@@ -229,32 +481,48 @@ def _dense(a):
 
 
 def _member(est, P):
-    """(kernel params, raw-space support vectors, dual [n_sv, R], intercept [R], colw, colo) of one fitted model behind
-    its scalers."""
+    """(kernel params, raw-space support vectors, dual [n_sv, R], intercept [R], colw, colo, program) of one fitted model
+    behind its scalers (``program``: the ``KernelProgram`` of a kernel object, else None)."""
     est, a, b = _unwrap(est, P)
     names = _names(est)
     if not (names & _KERNEL_MACHINES):
         raise NotImplementedError(f"{type(est).__name__} is not a kernel machine")
-    if not hasattr(est, "n_features_in_"):
-        raise TypeError(f"{type(est).__name__} is not fitted")
-    kernel, gamma, degree, coef0 = _kernel_params(est, P)
-    if names & _KRR:
-        Vt = _dense(est.X_fit_)
-        dual = np.asarray(est.dual_coef_, dtype=np.float64)
-        dual = dual.reshape(Vt.shape[0], -1)
-        intercept = np.zeros(dual.shape[1])
+    if names & _GPR:
+        if not hasattr(est, "X_train_"):
+            raise TypeError("GaussianProcessRegressor is not fitted (the prior mean is not explained)")
+        Vt = _dense(est.X_train_)
+        alpha = np.asarray(est.alpha_, dtype=np.float64).reshape(Vt.shape[0], -1)
+        R = alpha.shape[1]
+        std = np.broadcast_to(np.asarray(est._y_train_std, dtype=np.float64).reshape(-1), (R,))
+        dual = alpha * std                              # predict: std (K alpha) + mean, as scikit-learn un-normalises
+        intercept = np.broadcast_to(np.asarray(est._y_train_mean, dtype=np.float64).reshape(-1), (R,)).copy()
+        params, program = ("program", 0.0, 0.0, 0.0), _kernel_program(est.kernel_, P)
     else:
-        Vt = _dense(est.support_vectors_)
-        dual = _dense(est.dual_coef_).T.copy()
-        intercept = np.asarray(est.intercept_, dtype=np.float64).reshape(-1)
+        if not hasattr(est, "n_features_in_"):
+            raise TypeError(f"{type(est).__name__} is not fitted")
+        params = _kernel_params(est, P)
+        program = _kernel_program(est.kernel, P) if params[0] == "program" else None
+        if names & _KRR:
+            Vt = _dense(est.X_fit_)
+            dual = np.asarray(est.dual_coef_, dtype=np.float64)
+            dual = dual.reshape(Vt.shape[0], -1)
+            intercept = np.zeros(dual.shape[1])
+        else:
+            Vt = _dense(est.support_vectors_)
+            dual = _dense(est.dual_coef_).T.copy()
+            intercept = np.asarray(est.intercept_, dtype=np.float64).reshape(-1)
+    kernel = params[0]
     V = (Vt - b) / a
-    if kernel == "laplacian":
+    if program is not None:
+        program = program.folded(a, b)
+        colw, colo = np.ones(P), np.zeros(P)
+    elif kernel == "laplacian":
         colw, colo = np.abs(a), np.zeros(P)
     elif kernel == "rbf":
         colw, colo = a * a, np.zeros(P)
     else:
         colw, colo = a * a, -b / a
-    return (kernel, gamma, degree, coef0), V, dual, intercept, colw, colo
+    return params, V, dual, intercept, colw, colo, program
 
 
 def _svc_binary(est, what):
@@ -282,7 +550,7 @@ def _calibrated_spec(owner, method, P, bare=False):
             raise NotImplementedError(f"CalibratedClassifierCV over {type(_final(cc.estimator)).__name__}: the kernel-"
                                       "machine route calibrates SVC and NuSVC only")
         _svc_binary(cc.estimator, type(_final(cc.estimator)).__name__)
-        params, V, dual, icpt, colw, colo = _member(_final(cc.estimator) if bare else cc.estimator, P)
+        params, V, dual, icpt, colw, colo, _ = _member(_final(cc.estimator) if bare else cc.estimator, P)
         cal = cc.calibrators[0]
         members.append((params, V, dual, icpt, colw, colo, float(cal.a_), float(cal.b_)))
     kinds = {m[0][0] for m in members}
@@ -311,27 +579,39 @@ def _single_spec(owner, method, P):
         if method != "decision_function":
             raise TypeError(f"{name}.{method} is not supported: pass decision_function (predict returns labels)")
         _svc_binary(est, name)
+    elif names & _OCSVM:
+        if method not in ("decision_function", "score_samples"):
+            raise TypeError(f"{name}.{method} is not supported: pass decision_function or score_samples (predict returns "
+                            "labels)")
     elif method != "predict":
         raise TypeError(f"{name}.{method} is not supported: pass predict")
-    params, V, dual, icpt, colw, colo = _member(owner, P)
+    params, V, dual, icpt, colw, colo, program = _member(owner, P)
     if dual.shape[1] > MAX_OUTPUTS:
         raise NotImplementedError(f"{dual.shape[1]} targets: kernel machines are explained up to {MAX_OUTPUTS} outputs")
     scalar = True
     if names & _KRR:
         scalar = np.ndim(est.dual_coef_) == 1
+    elif names & _GPR:
+        scalar = dual.shape[1] == 1                     # predict squeezes one target
+    elif method == "score_samples":
+        icpt = icpt + float(np.ravel(est.offset_)[0])
     kernel, gamma, degree, coef0 = params
     return KernelMachineSpec(V, [0, V.shape[0]], dual, icpt[None, :], colw[None, :], colo[None, :], [gamma], kernel,
-                             degree, coef0, "identity", P, scalar_out=scalar)
+                             degree, coef0, "identity", P, scalar_out=scalar, program=program)
 
 
 def extract_kernel_machine_spec(predictor):
     """``KernelMachineSpec`` of a bound method of a fitted scikit-learn kernel machine -- ``SVC`` / ``NuSVC``
-    ``decision_function``, ``SVR`` / ``NuSVR`` / ``KernelRidge`` ``predict``, ``CalibratedClassifierCV(SVC | NuSVC,
-    method='sigmoid').predict_proba``, each possibly behind a ``Pipeline`` of per-column affine scalers -- and ``None``
-    for anything else (linear SVMs included: the engine then reads a linear model).  A spec passes through.  Raises
-    ``NotImplementedError`` / ``TypeError`` naming the reason for kernel machines the route does not cover: more than two
-    classes, ``SVC(probability=True).predict_proba``, precomputed, callable and chi2 kernels, a non-integer or negative
-    polynomial degree, pipeline steps other than the four affine scalers, calibration other than 'sigmoid'."""
+    ``decision_function``, ``SVR`` / ``NuSVR`` / ``KernelRidge`` (a ``Kernel`` object included) /
+    ``GaussianProcessRegressor`` ``predict``, ``OneClassSVM`` ``decision_function`` / ``score_samples``,
+    ``CalibratedClassifierCV(SVC | NuSVC, method='sigmoid').predict_proba``, each possibly behind a ``Pipeline`` of
+    per-column affine scalers -- and ``None`` for anything else (linear SVMs included: the engine then reads a linear
+    model).  A spec passes through.  Raises ``NotImplementedError`` / ``TypeError`` naming the reason for kernel machines
+    the route does not cover: more than two classes, ``SVC(probability=True).predict_proba``, precomputed, callable and
+    chi2 kernels, kernel objects on SVMs, kernel objects outside the program kernel (``Matern`` nu other than 0.5, 1.5,
+    2.5, inf, ``PairwiseKernel``, ``CompoundKernel``, user-defined kernels, more than ``MAX_STATS`` statistics),
+    ``GaussianProcessClassifier``, unfitted models, a non-integer or negative polynomial degree, pipeline steps other
+    than the four affine scalers, calibration other than 'sigmoid'."""
     if isinstance(predictor, KernelMachineSpec):
         return predictor
     owner = getattr(predictor, "__self__", None)
@@ -351,8 +631,15 @@ def extract_kernel_machine_spec(predictor):
         return spec
     if not _is_kernel_machine(owner):
         return None
-    if callable(outer.kernel) or outer.kernel == "precomputed":
-        _kernel_params(outer, 0)                        # raises, naming the kernel
+    if "GaussianProcessClassifier" in _names(outer):
+        raise NotImplementedError("GaussianProcessClassifier is not supported: its predict_proba needs the posterior "
+                                  "variance (a triangular solve against every training row per masked row)")
+    if not (_names(outer) & _GPR) and (callable(outer.kernel) or outer.kernel == "precomputed"):
+        _kernel_params(outer, 0)                        # raises, naming the kernel (kernel objects: KernelRidge reads them)
+    if (_names(outer) & _GPR) and not hasattr(outer, "X_train_"):
+        raise TypeError("GaussianProcessRegressor is not fitted (the prior mean is not explained)")
+    if (_names(outer) & _GPR) and not hasattr(owner, "n_features_in_"):
+        return _single_spec(owner, method, int(np.shape(owner.X_train_)[1]))     # kernels on non-vector input
     if not hasattr(outer, "n_features_in_"):
         raise TypeError(f"{type(outer).__name__} is not fitted")
     return _single_spec(owner, method, int(owner.n_features_in_))
@@ -360,6 +647,7 @@ def extract_kernel_machine_spec(predictor):
 
 def _fold_outer(spec, a, b):
     """The spec of the model behind one more affine map x' = a x + b of its raw columns."""
+    program = spec.program.folded(a, b) if spec.program is not None else None
     if spec.kernel == "laplacian":
         colw = spec.colw * np.abs(a)
     else:
@@ -367,4 +655,4 @@ def _fold_outer(spec, a, b):
     colo = (spec.colo - b) / a
     return KernelMachineSpec((spec.sv - b) / a, spec.sv_off, spec.dual, spec.intercept, colw, colo, spec.gamma,
                              spec.kernel, spec.degree, spec.coef0, spec.head, spec.n_features, cal_a=spec.cal_a,
-                             cal_b=spec.cal_b, pi=spec.pi, scalar_out=spec.scalar_out)
+                             cal_b=spec.cal_b, pi=spec.pi, scalar_out=spec.scalar_out, program=program)

@@ -100,6 +100,28 @@ extern "C" {
 #define DKS_KM_KERNEL_LAPLACIAN 1 /* h = w_c |x_c - v_c|,           phi = exp(-gamma t) */
 #define DKS_KM_KERNEL_POLY 2      /* h = w_c (x_c - o_c)(v_c - o_c), phi = (gamma t + coef0)^degree, integer degree >= 0 */
 #define DKS_KM_KERNEL_SIGMOID 3   /* h = w_c (x_c - o_c)(v_c - o_c), phi = tanh(gamma t + coef0) */
+#define DKS_KM_KERNEL_PROGRAM 4   /* up to DKS_KM_MAX_STATS statistics and an expression over them (dks_set_kernel_program):
+                                   * scikit-learn's kernel algebra (GaussianProcessRegressor, KernelRidge with a Kernel) */
+/* statistic of the program kernel: t_l = sum_c h(x_c, v_c) with the statistic's own column weights w and origins o */
+#define DKS_KM_STAT_SQDIST 0      /* h = w_c (x_c - v_c)^2 */
+#define DKS_KM_STAT_DOT 1         /* h = w_c (x_c - o_c)(v_c - o_c) */
+/* instructions of the program kernel's postfix expression {op, arg, a, b}; leaves push, operators pop */
+#define DKS_KM_OP_CONST 0         /* push a */
+#define DKS_KM_OP_STAT 1          /* push t_arg */
+#define DKS_KM_OP_EXP 2           /* push exp(-a t_arg) (RBF, Matern nu = inf: a = 1/2) */
+#define DKS_KM_OP_MATERN05 3      /* push exp(-r), r = sqrt(max(t_arg, 0)) */
+#define DKS_KM_OP_MATERN15 4      /* push (1 + k) exp(-k), k = sqrt(3) r */
+#define DKS_KM_OP_MATERN25 5      /* push (1 + k + k^2 / 3) exp(-k), k = sqrt(5) r */
+#define DKS_KM_OP_RQ 6            /* push (1 + t_arg)^a (RationalQuadratic: a = -alpha) */
+#define DKS_KM_OP_EXPSINE 7       /* push exp(-2 (sin(pi r / a) / b)^2) (ExpSineSquared: a periodicity, b length scale) */
+#define DKS_KM_OP_ADD 8           /* pop two, push their sum */
+#define DKS_KM_OP_MUL 9           /* pop two, push their product */
+#define DKS_KM_OP_POW 10          /* top = top^a */
+#define DKS_KM_OP_ADDC 11         /* top = top + a */
+#define DKS_KM_OP_MULC 12         /* top = top * a */
+#define DKS_KM_MAX_STATS 4        /* statistics of the program kernel */
+#define DKS_KM_MAX_OPS 32         /* instructions of the program kernel */
+#define DKS_KM_MAX_STACK 4        /* operands the program kernel's expression holds at once */
 /* head of a kernel machine on the member scores f_k = sum_v dual[v] K(x, v) + intercept_k */
 #define DKS_KM_HEAD_IDENTITY 0    /* one member, R outputs f (SVC / NuSVC decision_function, SVR, NuSVR, KernelRidge) */
 #define DKS_KM_HEAD_CALIBRATED 1  /* R = 1, outputs [1 - p1, p1], p1 = sum_k pi_k expit(-(a_k f_k + b_k)): sigmoid
@@ -232,11 +254,23 @@ int dks_set_tree_offset(dks_ctx* ctx, double offset);
  * row (dks_fit) or an instance (dks_predict_host, the explain calls) is DKS_ERR_DOMAIN with the row; a link(ey) or
  * link(f(x)) that is not finite is DKS_ERR_NUMERIC and nothing non-finite is written into phi.  Shapes whose per-instance
  * buffers do not fit shared memory are DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused.  With a column encoding set
- * (dks_set_column_encoding) D is its E encoded columns. */
+ * (dks_set_column_encoding) D is its E encoded columns.  kernel DKS_KM_KERNEL_PROGRAM needs K = 1, the identity head and
+ * dks_set_kernel_program before dks_fit (which is DKS_ERR_INVALID without it); gamma, degree, coef0, colw and colo are then
+ * unused (colw must still be positive). */
 int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const double* sv, const double* dual, int R,
                            const double* intercept, const double* colw, const double* colo, const double* gamma, int kernel,
                            double degree, double coef0, int head, const double* cal_a, const double* cal_b,
                            const double* pi, int scalar_out);
+/* the program kernel (DESIGN.md §5.0.21) of a kernel machine set with DKS_KM_KERNEL_PROGRAM: K(x, v) is a postfix expression
+ * of n_ops (1..DKS_KM_MAX_OPS) instructions ops / args / a / b (DKS_KM_OP_*) over L (1..DKS_KM_MAX_STATS) statistics
+ * t_l = sum_c h_l(x_c, v_c) of kind kinds[l] (DKS_KM_STAT_*) with column weights colw [L][D] (> 0) and origins colo [L][D].
+ * Leaves read statistic args[i] < L; the expression must leave exactly one value and hold at most DKS_KM_MAX_STACK at once.
+ * Unknown codes, out-of-range operands, a stack that under- or overflows, non-finite or zero-divisor constants are
+ * DKS_ERR_UNSUPPORTED; a context without a DKS_KM_KERNEL_PROGRAM kernel machine is DKS_ERR_INVALID.  Call before dks_fit.
+ * The explain kernel holds the tables of every statistic for 32 / L support vectors per tile, in the shared memory the
+ * other kernels use for 32: one masked row costs L ceil(M / 4) table reads and one expression per support vector. */
+int dks_set_kernel_program(dks_ctx* ctx, int L, const int32_t* kinds, const double* colw, const double* colo, int n_ops,
+                           const int32_t* ops, const int32_t* args, const double* a, const double* b);
 /* multi-layer perceptron (DKS_ACT_MLP) in place of dks_set_model: n_hidden (1..DKS_MLP_MAX_HIDDEN) hidden layers.
  * widths [n_hidden + 2] = {D, H_1 .. H_n_hidden, R}: hidden widths 1..DKS_MLP_MAX_WIDTH, R outputs 1..DKS_MLP_MAX_OUT.
  * W_host: the layers' weights concatenated, layer l [widths[l]][widths[l + 1]] row-major (scikit-learn's coefs_[l]; layer 0
