@@ -65,6 +65,8 @@ SIGNATURES = {
                                [C.c_int, C.c_double, C.c_double, C.c_int] + [C.c_void_p] * 3 + [C.c_int]),
     "dks_set_kernel_program": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] +
                                [C.c_void_p] * 4),
+    "dks_set_svc_multiclass": (C.c_int, [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 8 +
+                               [C.c_int, C.c_double, C.c_double, C.c_int] + [C.c_void_p] * 3 + [C.c_int]),
     "dks_set_mlp": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "dks_set_knn_model": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int, C.c_double, C.c_int,
                                                                              C.c_int, C.c_void_p, C.c_int, C.c_int]),

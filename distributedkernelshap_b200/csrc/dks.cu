@@ -272,6 +272,7 @@ OwnKernel own_kernel(int family) {
         return {"kernel machines", "kernel-machine kernel", "groups", "kernel machine",
                 " (their scalers fold into the support vectors and column weights)", REFUSES_NAN,
                 [](const dks_ctx* c, int S_cap) {
+                    if (c->km.head == DKS_KM_HEAD_OVO) return dks::kmach::ovo_smem_bytes(S_cap, c->C, c->km.R, c->G);
                     return dks::kmach::smem_bytes(S_cap, c->C, c->km.R, c->G, c->km.head == DKS_KM_HEAD_CALIBRATED); }};
     case DKS_GENERAL_MLP:
         return {"MLPs", "MLP kernel", "hidden units", "MLP", " (their scalers fold into the first layer)",
@@ -446,6 +447,13 @@ int own_fit_tables(dks_ctx* ctx, const double* bg, int width) {
             dks::kmach::km_prog_fit_table_kernel<<<cdiv(n, 256), 256, 0, st>>>(bg, N, width, k, ctx->kprog, Tbg);
             break;
         }
+        if (k.head == DKS_KM_HEAD_OVO) {   // the one-vs-one head's class blocks, pair intercepts and calibrations
+            KmOvo& ov = ctx->kovo;
+            CUDA_TRY(pool.upload(&ov.cls_off, ctx->h_kocls.data(), ctx->h_kocls.size(), st));
+            CUDA_TRY(pool.upload(&ov.icpt, ctx->h_koicpt.data(), ctx->h_koicpt.size(), st));
+            CUDA_TRY(pool.upload(&ov.cal_a, ctx->h_kocala.data(), ctx->h_kocala.size(), st));
+            CUDA_TRY(pool.upload(&ov.cal_b, ctx->h_kocalb.data(), ctx->h_kocalb.size(), st));
+        }
         CUDA_TRY(pool.alloc(&Tbg, (size_t)N * k.n_sv));
         k.Tbg = Tbg;
         dks::kmach::km_fit_table_kernel<<<cdiv((long long)N * k.n_sv, 256), 256, 0, st>>>(bg, N, width, k, Tbg);
@@ -515,7 +523,10 @@ int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const
                                                                       ctx->d_status);
         break;
     case DKS_GENERAL_KMACH:
-        if (ctx->km.kernel == DKS_KM_KERNEL_PROGRAM)
+        if (ctx->km.head == DKS_KM_HEAD_OVO)
+            dks::kmach::km_ovo_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->km, ctx->kovo, C, link, linkfnull,
+                                                                            out, dlink, ctx->d_status);
+        else if (ctx->km.kernel == DKS_KM_KERNEL_PROGRAM)
             dks::kmach::km_prog_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->km, ctx->kprog, C, link,
                                                                              linkfnull, out, dlink, ctx->d_status);
         else
@@ -603,6 +614,15 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         break;
     }
     case DKS_GENERAL_KMACH: {
+        if (ctx->km.head == DKS_KM_HEAD_OVO) {
+            auto kern = rows ? dks::kmach::explain_kmach_ovo_kernel<false, true, true>
+                        : acc ? dks::kmach::explain_kmach_ovo_kernel<false, true>
+                        : l1 ? dks::kmach::explain_kmach_ovo_kernel<true> : dks::kmach::explain_kmach_ovo_kernel<false>;
+            CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            kern<<<grid, dks::kmach::THREADS, smem, st>>>(p, q, ctx->km, ctx->kovo, ctx->own_X, ctx->own_bg, ctx->own_D,
+                                                          ctx->own_goff, ctx->own_gcols, ea, er);
+            break;
+        }
         auto kern = ctx->km.kernel == DKS_KM_KERNEL_PROGRAM
                     ? (rows ? dks::kmach::explain_kmach_kernel<false, true, true, true>
                        : acc ? dks::kmach::explain_kmach_kernel<false, true, false, true>
@@ -2379,6 +2399,99 @@ int dks_set_kernel_program(dks_ctx* ctx, int L, const int32_t* kinds, const doub
     ctx->h_kpcolo.assign(colo, colo + (size_t)L * D);
     ctx->fitted = false;
     return DKS_OK;
+}
+
+int dks_set_svc_multiclass(dks_ctx* ctx, int K, int classes, const int32_t* sv_off, const int32_t* cls_off, const double* sv,
+                           const double* dual, const double* intercept, const double* colw, const double* colo,
+                           const double* gamma, int kernel, double degree, double coef0, int mode, const double* cal_a,
+                           const double* cal_b, const double* pi, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_svc_multiclass: call dks_set_background first (D unknown)");
+    REQUIRE(sv_off && cls_off && sv && dual && intercept && colw && colo && gamma,
+            "dks_set_svc_multiclass: need the support vectors, class offsets, dual coefficients, intercepts, column weights "
+            "and gamma");
+    const int D = model_columns(ctx);
+    if (K < 1 || K > DKS_KM_MAX_K)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: K=%d members; 1..%d supported", K, DKS_KM_MAX_K);
+    if (classes < 3 || classes > DKS_KM_OVO_MAX_CLASSES)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: %d classes; 3..%d supported", classes,
+                    DKS_KM_OVO_MAX_CLASSES);
+    if (kernel != DKS_KM_KERNEL_RBF && kernel != DKS_KM_KERNEL_POLY && kernel != DKS_KM_KERNEL_SIGMOID)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: kernel %d; rbf, poly and sigmoid supported", kernel);
+    if (!std::isfinite(coef0) || !std::isfinite(degree) ||
+        (kernel == DKS_KM_KERNEL_POLY && (degree < 0 || degree != std::floor(degree))))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: degree %g / coef0 %g (degree: an integer >= 0)", degree,
+                    coef0);
+    const int P = classes * (classes - 1) / 2, R = classes - 1;
+    int C;
+    if (mode == DKS_KM_OVO_DECISION) {
+        if (K != 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: the pair values take one member (K=%d)", K);
+        if (P > DKS_KM_MAX_R)
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: %d pair values over %d classes; up to %d outputs", P,
+                        classes, DKS_KM_MAX_R);
+        C = P;
+    } else if (mode == DKS_KM_OVO_PROBA) {
+        if (!cal_a || !cal_b || !pi || !all_finite(cal_a, (size_t)K * classes) || !all_finite(cal_b, (size_t)K * classes))
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: the probabilities need finite a, b and pi");
+        C = classes;
+    } else {
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: unknown mode %d", mode);
+    }
+    if (sv_off[0] != 0) return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: sv_off[0] must be 0");
+    for (int m = 0; m < K; ++m) {
+        if (sv_off[m + 1] < sv_off[m])
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: sv_off must not decrease (member %d)", m);
+        const int32_t* co = cls_off + (size_t)m * (classes + 1);
+        if (co[0] != sv_off[m] || co[classes] != sv_off[m + 1])
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: the class blocks of member %d must span its support "
+                        "vectors", m);
+        for (int c = 0; c < classes; ++c)
+            if (co[c + 1] < co[c])
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: cls_off must not decrease (member %d, class %d)",
+                            m, c);
+    }
+    const int n_sv = sv_off[K];
+    if (n_sv < 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: no support vectors");
+    if (!all_finite(sv, (size_t)n_sv * D) || !all_finite(dual, (size_t)n_sv * R) || !all_finite(intercept, (size_t)K * P) ||
+        !all_finite(colw, (size_t)K * D) || !all_finite(colo, (size_t)K * D) || !all_finite(gamma, K))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: the arrays must be finite");
+    for (size_t e = 0; e < (size_t)K * D; ++e)
+        if (!(colw[e] > 0)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: column weights must be positive");
+    double pisum = 0;
+    for (int m = 0; m < K; ++m) {
+        if (!(gamma[m] >= 0)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: gamma must be >= 0");
+        if (mode == DKS_KM_OVO_PROBA) {
+            if (!(pi[m] > 0) || !std::isfinite(pi[m]))
+                return fail(DKS_ERR_UNSUPPORTED, "dks_set_svc_multiclass: pi must be positive and finite");
+            pisum += pi[m];
+        }
+    }
+    KmDev& k = ctx->km;
+    for (int m = 0; m <= K; ++m) k.sv_off[m] = sv_off[m];
+    for (int m = 0; m < K; ++m) {
+        k.gamma[m] = gamma[m];
+        k.icpt[m] = k.cal_a[m] = k.cal_b[m] = 0.0;      // the one-vs-one head reads its own (KmOvo)
+        k.pi[m] = mode == DKS_KM_OVO_PROBA ? pi[m] / pisum : 1.0;
+    }
+    k.degree = degree; k.coef0 = coef0; k.K = K; k.R = R; k.n_sv = n_sv; k.kernel = kernel; k.head = DKS_KM_HEAD_OVO;
+    ctx->h_ksv.assign(sv, sv + (size_t)n_sv * D);
+    ctx->h_kdual.assign(dual, dual + (size_t)n_sv * R);
+    ctx->h_kcolw.assign(colw, colw + (size_t)K * D);
+    ctx->h_kcolo.assign(colo, colo + (size_t)K * D);
+    ctx->kprog = KmProg{};
+    ctx->h_kpcolw.clear(); ctx->h_kpcolo.clear();
+    ctx->h_kocls.assign(cls_off, cls_off + (size_t)K * (classes + 1));
+    ctx->h_koicpt.assign(intercept, intercept + (size_t)K * P);
+    if (mode == DKS_KM_OVO_PROBA) {
+        ctx->h_kocala.assign(cal_a, cal_a + (size_t)K * classes);
+        ctx->h_kocalb.assign(cal_b, cal_b + (size_t)K * classes);
+    } else {
+        ctx->h_kocala.assign((size_t)K * classes, 0.0);
+        ctx->h_kocalb.assign((size_t)K * classes, 0.0);
+    }
+    ctx->kovo = KmOvo{};
+    ctx->kovo.classes = classes; ctx->kovo.P = P; ctx->kovo.mode = mode;
+    return set_own_model(ctx, DKS_ACT_KMACH, C, scalar_out);
 }
 
 int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double* W_host, const double* b_host, int activation,

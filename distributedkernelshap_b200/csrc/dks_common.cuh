@@ -288,6 +288,16 @@ struct KmProg {
     int L, n;                    // n = 0: no program
 };
 
+// the one-vs-one head of a multi-class SVM (DKS_KM_HEAD_OVO, dks_set_svc_multiclass, DESIGN.md §5.0.22): KmDev's members
+// hold their support vectors in class blocks, KmDev's dual is [n_sv][classes - 1] (R = classes - 1)
+struct KmOvo {
+    const int* cls_off;          // [K][classes + 1] absolute support-vector rows of each member's classes
+    const double* icpt;          // [K][P] pair intercepts
+    const double* cal_a;         // [K][classes] (DKS_KM_OVO_PROBA)
+    const double* cal_b;
+    int classes, P, mode;        // mode DKS_KM_OVO_*
+};
+
 // multi-layer perceptrons (dks_set_mlp, DESIGN.md §5.0.14): L = hidden + 1 weight layers, layer l mapping width[l] units to
 // width[l + 1] (width[0] = D raw columns, width[L] = R outputs).  The explain kernel reads layers 1 .. L - 1 in the FP64 mma
 // B-fragment order, zero-padded to pad[l] x pad[l + 1] (hidden widths to a multiple of 16, the output layer to 8): padding
@@ -441,6 +451,10 @@ struct dks_ctx {
     std::vector<double> h_kpcolw, h_kpcolo;     // the program kernel's [L][D] column weights and origins
     KmDev km = {};
     KmProg kprog = {};
+    // the one-vs-one head (km.head == DKS_KM_HEAD_OVO): host copies of its arrays, and the device copy dks_fit builds
+    std::vector<int32_t> h_kocls;
+    std::vector<double> h_koicpt, h_kocala, h_kocalb;
+    KmOvo kovo = {};
     // multi-layer perceptron (act == DKS_ACT_MLP): host copies of the layers (natural, fragment-ordered, padded biases), and
     // their device copies built by dks_fit
     std::vector<double> h_mw, h_mb, h_mwf, h_mbp;

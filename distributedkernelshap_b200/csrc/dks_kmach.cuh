@@ -472,5 +472,322 @@ __global__ void __launch_bounds__(THREADS) explain_kmach_kernel(ExplainParams p,
     }
 }
 
+// ---- multi-class SVMs: the one-vs-one head (DKS_KM_HEAD_OVO, KmOvo, DESIGN.md §5.0.22) ----------------------------------
+// A member's pair scores live in 28 registers d[] laid out for 8 classes (slot of pair (a, b) below); a multi-class SVM
+// with fewer classes leaves the slots of b >= classes at zero.  Every index into d, and into the per-class partials pt, is a
+// compile-time constant of an unrolled loop: nothing goes to local memory.
+
+constexpr int OVO_C = DKS_KM_OVO_MAX_CLASSES;
+constexpr int OVO_SLOTS = OVO_C * (OVO_C - 1) / 2;
+
+__host__ __device__ constexpr int ovo_slot(int a, int b) { return a * (2 * OVO_C - a - 1) / 2 + (b - a - 1); }
+
+// the partials pt[r] = sum_v dual[v][r] K(x, v) over support vectors of class c into the pair scores: dual row r of class c
+// belongs to pair (c, r + 1) for r >= c and to pair (r, c) for r < c (scikit-learn's dual_coef_ layout)
+__device__ __forceinline__ void ovo_scatter(int c, const double* pt, double* d) {
+#pragma unroll
+    for (int a = 0; a < OVO_C; ++a)
+#pragma unroll
+        for (int b = a + 1; b < OVO_C; ++b) {
+            if (c == a) d[ovo_slot(a, b)] += pt[b - 1];
+            else if (c == b) d[ovo_slot(a, b)] += pt[a];
+        }
+}
+
+// member m's head on its pair scores d (intercepts not yet added), handing each output to emit(row, value):
+// DKS_KM_OVO_DECISION dec_k = d + intercept for row k = 0 .. P - 1 in scikit-learn's pair order; DKS_KM_OVO_PROBA the
+// calibrated probabilities of the ovr-vote decision function f_c = votes_c + conf_c / (3 (|conf_c| + 1)) for row c (dec >= 0
+// votes for the first class of the pair, as libsvm decides it; conf summed in the pair order, as scikit-learn sums it),
+// e_c = expit(-(a_c f_c + b_c)), normalised by their sum (uniform 1 / classes for a zero sum), (1, 1 + 1e-5] clipped to 1
+template <typename Emit>
+__device__ __forceinline__ void ovo_head(const KmOvo& ov, int m, const double* d, Emit&& emit) {
+    const int nc = ov.classes;
+    const double* ic = ov.icpt + (size_t)m * ov.P;
+    double votes[OVO_C], conf[OVO_C];
+#pragma unroll
+    for (int c = 0; c < OVO_C; ++c) { votes[c] = 0.0; conf[c] = 0.0; }
+    int k = 0;
+#pragma unroll
+    for (int a = 0; a < OVO_C; ++a)
+#pragma unroll
+        for (int b = a + 1; b < OVO_C; ++b)
+            if (b < nc) {
+                const double dec = d[ovo_slot(a, b)] + ic[k];
+                if (ov.mode == DKS_KM_OVO_DECISION) {
+                    emit(k, dec);
+                } else {
+                    if (dec >= 0.0) votes[a] += 1.0; else votes[b] += 1.0;
+                    conf[a] += dec;
+                    conf[b] -= dec;
+                }
+                ++k;
+            }
+    if (ov.mode == DKS_KM_OVO_DECISION) return;
+    const double* ca = ov.cal_a + (size_t)m * nc;
+    const double* cb = ov.cal_b + (size_t)m * nc;
+    double e[OVO_C], sum = 0.0;
+#pragma unroll
+    for (int c = 0; c < OVO_C; ++c) {
+        e[c] = 0.0;
+        if (c < nc) {
+            const double f = votes[c] + conf[c] / (3.0 * (fabs(conf[c]) + 1.0));
+            double p0;
+            cal_member(fma(ca[c], f, cb[c]), &p0, &e[c]);
+            sum += e[c];
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < OVO_C; ++c)
+        if (c < nc) {
+            double pc = sum != 0.0 ? e[c] / sum : 1.0 / nc;
+            if (pc > 1.0 && pc <= 1.0 + 1e-5) pc = 1.0;
+            emit(c, pc);
+        }
+}
+
+// outputs o[C] of one row under the one-vs-one head: per member and class the partials over the class's support vectors
+// in order, then the head; members weighted by pi
+__device__ inline void km_ovo_outputs(const KmDev& k, const KmOvo& ov, const double* __restrict__ x, int D, double* o) {
+    const int C = ov.mode == DKS_KM_OVO_DECISION ? ov.P : ov.classes;
+    for (int c = 0; c < C; ++c) o[c] = 0.0;
+    for (int m = 0; m < k.K; ++m) {
+        double d[OVO_SLOTS];
+#pragma unroll
+        for (int e = 0; e < OVO_SLOTS; ++e) d[e] = 0.0;
+        const double* w = k.colw + (size_t)m * D;
+        const double* org = k.colo + (size_t)m * D;
+        const int* co = ov.cls_off + (size_t)m * (ov.classes + 1);
+        for (int c = 0; c < ov.classes; ++c) {
+            double pt[DKS_KM_MAX_R];
+#pragma unroll
+            for (int r = 0; r < DKS_KM_MAX_R; ++r) pt[r] = 0.0;
+            for (int v = co[c]; v < co[c + 1]; ++v) {
+                const double* sv = k.sv + (size_t)v * D;
+                double t = 0.0;
+                for (int cc = 0; cc < D; ++cc) t += km_term(k.kernel, x[cc], sv[cc], w[cc], org[cc]);
+                const double kv = km_phi(k, t, k.gamma[m]);
+#pragma unroll
+                for (int r = 0; r < DKS_KM_MAX_R; ++r)
+                    if (r < k.R) pt[r] = fma(k.dual[(size_t)v * k.R + r], kv, pt[r]);
+            }
+            ovo_scatter(c, pt, d);
+        }
+        const double pm = k.pi[m];
+        ovo_head(ov, m, d, [&](int r, double val) { o[r] = ov.mode == DKS_KM_OVO_DECISION ? val : fma(pm, val, o[r]); });
+    }
+}
+
+// km_predict_kernel under the one-vs-one head
+__global__ void km_ovo_predict_kernel(const double* __restrict__ X, int n, int D, KmDev k, KmOvo ov, int C, int link,
+                                      const double* __restrict__ linkfnull, double* __restrict__ out,
+                                      double* __restrict__ dlink, int* __restrict__ status) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double* x = X + (size_t)i * D;
+    bool nan = false;
+    for (int c = 0; c < D; ++c) nan |= isnan(x[c]);
+    double o[OVO_C];
+    if (nan) {
+        for (int c = 0; c < C; ++c) o[c] = NAN;
+        if (status) report_status(status, DKS_ERR_DOMAIN, i);
+    } else {
+        km_ovo_outputs(k, ov, x, D, o);
+    }
+    predict_epilogue(o, C, i, link, linkfnull, out, dlink, status, nan);
+}
+
+// shared memory of explain_kmach_ovo_kernel: [C][S_cap] float64 sums / y, then the tile-table / solve region and the varying
+// groups [64] as in explain_kmach_kernel (the pair scores live in registers)
+__host__ __device__ inline size_t ovo_smem_bytes(int S_cap, int C, int R, int G) {
+    const size_t tab = tile_doubles(R, G), solve = 63 * 63 + 64;
+    return sizeof(double) * ((size_t)C * S_cap + (tab > solve ? tab : solve)) + sizeof(int) * 64;
+}
+
+// explain_kmach_kernel for the one-vs-one head (one CTA per SM's worth of registers: the 28 pair scores stay in registers
+// without spilling): the same plans, tables, instantiations (L1, ACC, ROWS) and solve, in the
+// loop order the head needs.  Per background row j, coalitions go in chunks of blockDim.x, each thread owning one
+// coalition of the chunk; per member the thread keeps that coalition's pair scores in registers across the member's tiles.
+// Tiles follow the class blocks (class c is uniform within a tile): a support vector adds dual[v][r] K into the tile's
+// partials pt[r], which go into the pair scores when the tile is done (ovo_scatter).  When the member's classes are done,
+// its head adds w_j pi_m p_c (or w_j dec_k) into the sums.  The Delta and nibble tables are rebuilt per chunk; threads
+// without a coalition in the last chunk still build tables and reach every barrier.  Every sum runs in a fixed order: the
+// result does not depend on the grid.  Then y = link(ey) - link(fnull) for every output (logit: 1 - e_c is the sum of
+// the other classes), and the solve.
+template <bool L1, bool ACC = false, bool ROWS = false>
+__global__ void __launch_bounds__(THREADS, 1) explain_kmach_ovo_kernel(ExplainParams p, SimtL1 q, KmDev k, KmOvo ov,
+                                                                       const double* __restrict__ X,
+                                                                       const double* __restrict__ bg, int D,
+                                                                       const int* __restrict__ goff,
+                                                                       const int* __restrict__ gcols, EnsAcc ea,
+                                                                       EnsRows er) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int tid = threadIdx.x;
+    const int N = p.N, G = p.G, C = p.C, R = k.R;
+    const bool proba = ov.mode == DKS_KM_OVO_PROBA;
+    double* acc = reinterpret_cast<double*>(smem_raw);          // [C][S_cap]
+    double* region = acc + (size_t)C * p.S_cap;
+    const size_t tab = tile_doubles(R, G), solve = 63 * 63 + 64;
+    double* A = region;                                         // [63 * 63] (solve)
+    double* rhs = A + 63 * 63;                                  // [64]
+    double* tj = region;                                        // [TILE] (background loop)
+    double* du = tj + TILE;                                     // [TILE][R]
+    double* dl = du + TILE * R;                                 // [G][TILE]
+    double* tb = dl + (size_t)G * TILE;                         // [ceil(G/4)][TILE][16]
+    int* vi = reinterpret_cast<int*>(region + (tab > solve ? tab : solve));   // [64]
+    const size_t slab = (size_t)p.n * G;
+
+    const int ninst = dks_inst_count(p);
+    for (int qi = blockIdx.x; qi < ninst; qi += gridDim.x) {
+        const int i = dks_inst_at(p, qi);
+        const int M = p.Mcnt[i];
+        const uint64_t vm = p.vmask[i];
+        __syncthreads();  // previous instance done with shared memory
+        if constexpr (!ACC) zero_phi_rows(p, i);
+        bool fx_bad = false;                                    // stage 1 reported a NaN row or a non-finite link(f(x))
+        if constexpr (ROWS) fx_bad = rows_fx_bad(er, i);
+        else for (int c = 0; c < C; ++c) fx_bad |= !isfinite(p.dlink[(size_t)i * C + c]);
+        if (M == 0) continue;
+        if (M == 1) {
+            if (!ACC && tid < C && !fx_bad)
+                p.phi[(size_t)tid * slab + (size_t)i * G + (__ffsll((long long)vm) - 1)] = p.dlink[(size_t)i * C + tid];
+            continue;
+        }
+        InstPlan pl;
+        if (!inst_plan(p, i, M, pl)) continue;
+        if (fx_bad) {
+            if (L1) moments_skip(q, G, M, C, (size_t)i * C);
+            continue;
+        }
+        const int S = pl.S;
+        const uint64_t* zp = pl.z;
+        varying_positions(vm, G, vi);
+        for (int idx = tid; idx < C * S; idx += blockDim.x) acc[(size_t)(idx / S) * p.S_cap + idx % S] = 0.0;
+        __syncthreads();
+
+        const double* x = X + (size_t)i * D;
+        const int nib = (M + 3) >> 2;
+        for (int j = ROWS ? er.j0 : 0; j < (ROWS ? er.j1 : N); ++j) {
+            const double wb = p.wbg[j];
+            if (wb == 0.0) continue;                            // block-uniform
+            const double wj = ROWS ? 1.0 : wb;
+            const double* b = bg + (size_t)j * D;
+            for (int s0 = 0; s0 < S; s0 += blockDim.x) {
+                const int s = s0 + tid;
+                const bool live = s < S;
+                const uint64_t z = live ? zp[s] : 0;
+                if (ROWS && live)
+                    for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = 0.0;
+                for (int m = 0; m < k.K; ++m) {
+                    const double gm = k.gamma[m];
+                    const double* w = k.colw + (size_t)m * D;
+                    const double* org = k.colo + (size_t)m * D;
+                    const int* co = ov.cls_off + (size_t)m * (ov.classes + 1);
+                    double d[OVO_SLOTS];
+#pragma unroll
+                    for (int e = 0; e < OVO_SLOTS; ++e) d[e] = 0.0;
+                    for (int c = 0; c < ov.classes; ++c) {
+                        const int c1 = co[c + 1];
+                        for (int v0 = co[c]; v0 < c1; v0 += TILE) {
+                            const int nv = min(TILE, c1 - v0);
+                            for (int idx = tid; idx < nv; idx += blockDim.x) tj[idx] = k.Tbg[(size_t)j * k.n_sv + v0 + idx];
+                            for (int idx = tid; idx < nv * R; idx += blockDim.x) du[idx] = k.dual[(size_t)v0 * R + idx];
+                            for (int idx = tid; idx < M * nv; idx += blockDim.x) {
+                                const int pp = idx / nv, v = idx - pp * nv, g = vi[pp];
+                                const double* sv = k.sv + (size_t)(v0 + v) * D;
+                                double dd = 0.0;
+                                for (int e = goff[g]; e < goff[g + 1]; ++e) {
+                                    const int cc = gcols[e];
+                                    dd += km_term(k.kernel, x[cc], sv[cc], w[cc], org[cc]) -
+                                          km_term(k.kernel, b[cc], sv[cc], w[cc], org[cc]);
+                                }
+                                dl[(size_t)pp * TILE + v] = dd;
+                            }
+                            __syncthreads();
+                            for (int idx = tid; idx < nib * nv * 16; idx += blockDim.x) {
+                                const int qn = idx / (nv * 16), rem = idx - qn * nv * 16, v = rem >> 4, pat = rem & 15;
+                                double t = 0.0;
+                                for (int bit = 0; bit < 4; ++bit)
+                                    if (((pat >> bit) & 1) && 4 * qn + bit < M) t += dl[(size_t)(4 * qn + bit) * TILE + v];
+                                tb[((size_t)qn * TILE + v) * 16 + pat] = t;
+                            }
+                            __syncthreads();
+                            if (live) {
+                                double pt[DKS_KM_MAX_R];
+#pragma unroll
+                                for (int r = 0; r < DKS_KM_MAX_R; ++r) pt[r] = 0.0;
+                                for (int v = 0; v < nv; ++v) {
+                                    double t = tj[v];
+                                    for (int qn = 0; qn < nib; ++qn)
+                                        t += tb[((size_t)qn * TILE + v) * 16 + ((z >> (4 * qn)) & 15)];
+                                    const double kv = km_phi(k, t, gm);
+#pragma unroll
+                                    for (int r = 0; r < DKS_KM_MAX_R; ++r)
+                                        if (r < R) pt[r] = fma(du[v * R + r], kv, pt[r]);
+                                }
+                                ovo_scatter(c, pt, d);
+                            }
+                            __syncthreads();
+                        }
+                    }
+                    if (live) {
+                        const double wk = proba ? wj * k.pi[m] : wj;
+                        ovo_head(ov, m, d, [&](int r, double val) {
+                            double* a = acc + (size_t)r * p.S_cap + s;
+                            *a = fma(wk, val, *a);
+                        });
+                    }
+                }
+                if (ROWS && live) {
+                    double o[OVO_C];
+                    for (int c = 0; c < C; ++c) o[c] = acc[(size_t)c * p.S_cap + s];
+                    rows_store<0>(er, p.S_cap, i, j, s, o);
+                }
+            }
+        }
+        __syncthreads();
+        if constexpr (ROWS) continue;
+        if constexpr (ACC) {
+            ens_accumulate(ea, p, i, S, acc);
+            continue;
+        }
+
+        // y = link(ey) - link(fnull) per output, written over the sums: the probabilities' 1 - e_c is the sum of the other
+        // classes (no cancellation), the pair values' 1 - e as written.  Each thread reads and writes only the coalitions it
+        // owns.
+        int bad = 0;
+        for (int s = tid; s < S; s += blockDim.x) {
+            double y[OVO_C];
+            for (int c = 0; c < C; ++c) {
+                const double e = acc[(size_t)c * p.S_cap + s];
+                if (p.link == DKS_LINK_LOGIT) {
+                    double rest = 0.0;
+                    if (proba) {
+                        for (int c2 = 0; c2 < C; ++c2)
+                            if (c2 != c) rest += acc[(size_t)c2 * p.S_cap + s];
+                    } else {
+                        rest = 1.0 - e;
+                    }
+                    y[c] = log(e / rest) - p.linkfnull[c];
+                } else {
+                    y[c] = e - p.fnull[c];
+                }
+                bad |= !isfinite(y[c]);
+            }
+            for (int c = 0; c < C; ++c) acc[(size_t)c * p.S_cap + s] = y[c];
+        }
+        if (__syncthreads_or(bad)) {
+            if (tid == 0) report_status(p.status, DKS_ERR_NUMERIC, i);
+            if (L1) moments_skip(q, G, M, C, (size_t)i * C);
+            continue;
+        }
+        if constexpr (L1) {
+            block_moments_all<true>(q, G, pl, M, acc, p.S_cap, C, (size_t)i * C, A);
+            continue;
+        }
+        block_normal(pl, M, A, i, p.status);
+        block_solve(p, i, pl, M, acc, p.S_cap, C, false, A, rhs, vi);
+    }
+}
+
 }  // namespace kmach
 }  // namespace dks

@@ -16,7 +16,8 @@ from . import _cabi
 from .data import DenseData, convert_to_data, convert_to_link
 from .ensembles import MAX_GROUPS as ENSEMBLE_MAX_GROUPS, EnsembleSpec, extract_ensemble_spec
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
-from .kernel_machines import MAX_GROUPS as KMACH_MAX_GROUPS, KernelMachineSpec, extract_kernel_machine_spec
+from .kernel_machines import (MAX_GROUPS as KMACH_MAX_GROUPS, KernelMachineSpec, MulticlassSvmSpec,
+                              extract_kernel_machine_spec)
 from .mlp import MAX_GROUPS as MLP_MAX_GROUPS, MlpSpec, extract_mlp_spec
 from .neighbors import MAX_GROUPS as KNN_MAX_GROUPS, KnnSpec, extract_knn_spec
 from .predictors import LinearModelSpec, extract_linear_spec
@@ -357,6 +358,12 @@ class GpuKernelExplainer:
             widths, Wm, bm = own.flat()
             _cabi.check(self.lib.dks_set_mlp(ctx, own.n_hidden, _cabi.ptr(widths), _cabi.ptr(Wm), _cabi.ptr(bm),
                                              own.act_code_hidden, own.head_code, int(own.scalar_out)))
+        elif isinstance(own, MulticlassSvmSpec):
+            k = own
+            _cabi.check(self.lib.dks_set_svc_multiclass(
+                ctx, k.K, k.classes, _cabi.ptr(k.sv_off), _cabi.ptr(k.cls_off), _cabi.ptr(k.sv), _cabi.ptr(k.dual),
+                _cabi.ptr(k.intercept), _cabi.ptr(k.colw), _cabi.ptr(k.colo), _cabi.ptr(k.gamma), k.kernel_code, k.degree,
+                k.coef0, k.mode_code, _cabi.ptr(k.cal_a), _cabi.ptr(k.cal_b), _cabi.ptr(k.pi), int(k.scalar_out)))
         elif isinstance(own, KernelMachineSpec):
             k = own
             _cabi.check(self.lib.dks_set_kernel_machine(

@@ -28,6 +28,11 @@ into the ``program`` kernel: at most ``MAX_STATS`` additive statistics, each ``s
 ``dot`` (``h = w_c (x_c - o_c)(v_c - o_c)``) with its own column weights and origins, and a short postfix expression over
 them (``KernelProgram``, ``dks_set_kernel_program``).
 
+Multi-class ``SVC`` / ``NuSVC`` (3 to 8 classes) are read into ``MulticlassSvmSpec``, the one-vs-one head
+(``dks_set_svc_multiclass``): support vectors in class blocks, ``dual [n_sv, classes - 1]`` and one intercept per class
+pair.  Its outputs are the pair values of ``decision_function_shape='ovo'`` or the probabilities of
+``CalibratedClassifierCV(SVC | NuSVC, method='sigmoid')``, which calibrates the ovr-vote decision function per class.
+
 ``KernelMachineSpec.__call__`` evaluates the same thing in NumPy.
 """
 import numpy as np
@@ -43,6 +48,9 @@ OPS = ("const", "stat", "exp", "matern05", "matern15", "matern25", "rq", "expsin
 MAX_STATS = 4                                         # DKS_KM_MAX_STATS
 MAX_OPS = 32                                          # DKS_KM_MAX_OPS
 MAX_STACK = 4                                         # DKS_KM_MAX_STACK
+OVO_MODES = ("ovo", "ovo_proba")                      # DKS_KM_OVO_* codes 0..1
+OVO_HEAD = 2                                          # DKS_KM_HEAD_OVO
+MAX_CLASSES = 8                                       # DKS_KM_OVO_MAX_CLASSES
 
 _SVM_CLASSIFIERS = {"SVC", "NuSVC"}
 _SVM_REGRESSORS = {"SVR", "NuSVR"}
@@ -250,6 +258,112 @@ class KernelMachineSpec:
             out = np.stack([p0, p1], axis=1)
         else:
             out = f[:, 0, :]
+        return out[:, 0] if self.scalar_out else out
+
+
+class MulticlassSvmSpec(KernelMachineSpec):
+    """A multi-class SVC / NuSVC (3 to ``MAX_CLASSES`` classes) under the one-vs-one head, per member (calibration fold).
+
+    sv [n_sv, D], sv_off [K + 1]; cls_off [K, classes + 1] absolute rows of each member's class blocks; dual
+    [n_sv, classes - 1] (``dual_coef_`` transposed), intercept [K, P] with P = classes (classes - 1) / 2; colw / colo
+    [K, D], gamma [K], kernel ``rbf`` / ``poly`` / ``sigmoid``, degree, coef0.  head ``ovo``: one member, the P pair
+    values of ``decision_function_shape='ovo'``; ``ovo_proba``: cal_a / cal_b [K, classes] and pi [K], the calibrated
+    probabilities of ``CalibratedClassifierCV``."""
+
+    def __init__(self, sv, sv_off, cls_off, dual, intercept, colw, colo, gamma, kernel, degree, coef0, head, n_features,
+                 classes, cal_a=None, cal_b=None, pi=None, scalar_out=False):
+        self.classes = int(classes)
+        if not 3 <= self.classes <= MAX_CLASSES:
+            raise NotImplementedError(f"a multi-class SVM over {self.classes} classes: 3 to {MAX_CLASSES} are supported")
+        self.P = self.classes * (self.classes - 1) // 2
+        self.sv = np.ascontiguousarray(np.atleast_2d(sv), dtype=np.float64)
+        self.sv_off = np.ascontiguousarray(sv_off, dtype=np.int32)
+        self.K = len(self.sv_off) - 1
+        self.cls_off = np.ascontiguousarray(np.asarray(cls_off, dtype=np.int32).reshape(self.K, self.classes + 1))
+        self.R = self.classes - 1
+        self.dual = np.ascontiguousarray(np.asarray(dual, dtype=np.float64).reshape(self.sv.shape[0], self.R))
+        self.intercept = np.ascontiguousarray(np.asarray(intercept, dtype=np.float64).reshape(self.K, self.P))
+        self.colw = np.ascontiguousarray(np.asarray(colw, dtype=np.float64).reshape(self.K, -1))
+        self.colo = np.ascontiguousarray(np.asarray(colo, dtype=np.float64).reshape(self.K, -1))
+        self.gamma = np.ascontiguousarray(np.atleast_1d(gamma), dtype=np.float64)
+        self.kernel = kernel
+        self.degree = float(degree)
+        self.coef0 = float(coef0)
+        self.head = head
+        self.n_features = int(n_features)
+        self.scalar_out = bool(scalar_out)
+        self.program = None
+        if kernel not in ("rbf", "poly", "sigmoid"):
+            raise ValueError(f"kernel {kernel!r}: the one-vs-one head takes 'rbf', 'poly' and 'sigmoid'")
+        if head not in OVO_MODES:
+            raise ValueError(f"unknown one-vs-one head {head!r}")
+        if self.K > MAX_MEMBERS:
+            raise NotImplementedError(f"{self.K} calibrated members: kernel machines are explained up to {MAX_MEMBERS}")
+        if head == "ovo":
+            if self.K != 1:
+                raise ValueError("the pair values of decision_function_shape='ovo' take one member")
+            if self.P > MAX_OUTPUTS:
+                raise NotImplementedError(
+                    f"SVC(decision_function_shape='ovo').decision_function over {self.classes} classes gives {self.P} "
+                    f"pair values: up to {MAX_OUTPUTS} outputs (4 classes) are supported; explain "
+                    "CalibratedClassifierCV(SVC(), ensemble=False).predict_proba instead")
+            self.cal_a = self.cal_b = np.zeros((self.K, self.classes))
+            self.pi = np.ones(self.K)
+            self.n_outputs = self.P
+        else:
+            self.cal_a = np.ascontiguousarray(np.asarray(cal_a, dtype=np.float64).reshape(self.K, self.classes))
+            self.cal_b = np.ascontiguousarray(np.asarray(cal_b, dtype=np.float64).reshape(self.K, self.classes))
+            self.pi = np.ascontiguousarray(pi if pi is not None else np.full(self.K, 1.0 / self.K), dtype=np.float64)
+            self.n_outputs = self.classes
+
+    @property
+    def head_code(self):
+        return OVO_HEAD
+
+    @property
+    def mode_code(self):
+        return OVO_MODES.index(self.head)
+
+    def pairs(self):
+        """[(i, j)] of the class pairs in scikit-learn's order."""
+        return [(i, j) for i in range(self.classes) for j in range(i + 1, self.classes)]
+
+    def pair_values(self, X):
+        """dec [n, K, P] of every member, pairs in scikit-learn's order."""
+        X = np.atleast_2d(np.asarray(X, dtype=np.float64))
+        out = np.empty((X.shape[0], self.K, self.P))
+        for m in range(self.K):
+            Kv = self.kernel_values(self.statistic(X, m), m)
+            o = self.cls_off[m] - self.sv_off[m]
+            for k, (i, j) in enumerate(self.pairs()):
+                bi, bj = slice(o[i], o[i + 1]), slice(o[j], o[j + 1])
+                du = self.dual[self.sv_off[m]:self.sv_off[m + 1]]
+                out[:, m, k] = Kv[:, bi] @ du[bi, j - 1] + Kv[:, bj] @ du[bj, i] + self.intercept[m, k]
+        return out
+
+    def __call__(self, X):
+        """The scikit-learn method the spec was read from, in NumPy."""
+        dec = self.pair_values(X)
+        if self.head == "ovo":
+            out = dec[:, 0, :]
+        else:
+            out = np.zeros((dec.shape[0], self.classes))
+            for m in range(self.K):
+                votes = np.zeros_like(out)
+                conf = np.zeros_like(out)
+                for k, (i, j) in enumerate(self.pairs()):
+                    d = dec[:, m, k]
+                    votes[:, i] += d >= 0
+                    votes[:, j] += d < 0
+                    conf[:, i] += d
+                    conf[:, j] -= d
+                f = votes + conf / (3.0 * (np.abs(conf) + 1.0))
+                with np.errstate(over="ignore"):                # expit of a very negative argument is 0
+                    e = 1.0 / (1.0 + np.exp(self.cal_a[m] * f + self.cal_b[m]))
+                tot = e.sum(axis=1, keepdims=True)
+                p = np.divide(e, tot, out=np.full_like(e, 1.0 / self.classes), where=tot != 0)
+                p[(p > 1.0) & (p <= 1.0 + 1e-5)] = 1.0
+                out += self.pi[m] * p
         return out[:, 0] if self.scalar_out else out
 
 
@@ -525,12 +639,18 @@ def _member(est, P):
     return params, V, dual, intercept, colw, colo, program
 
 
-def _svc_binary(est, what):
-    clf = _final(est)
-    n = len(clf.classes_)
-    if n != 2:
-        raise NotImplementedError(f"{what} over {n} classes: its one-vs-one votes are not a head the kernel-machine route "
-                                  "evaluates; only two classes are supported")
+def _svc_classes(est, what):
+    """The classes of a fitted SVC / NuSVC: 2, or 3 to ``MAX_CLASSES`` for the one-vs-one head."""
+    n = len(_final(est).classes_)
+    if n > MAX_CLASSES:
+        raise NotImplementedError(f"{what} over {n} classes: the one-vs-one head of the kernel-machine route takes up to "
+                                  f"{MAX_CLASSES} classes ({MAX_CLASSES * (MAX_CLASSES - 1) // 2} pairs)")
+    return n
+
+
+def _class_blocks(est, off):
+    """cls_off [classes + 1] of a multi-class SVC whose support vectors start at row ``off``."""
+    return off + np.concatenate([[0], np.cumsum(np.asarray(_final(est).n_support_, dtype=np.int64))])
 
 
 def _calibrated_spec(owner, method, P, bare=False):
@@ -538,9 +658,12 @@ def _calibrated_spec(owner, method, P, bare=False):
     pipeline's steps being replayed in front of it (``trees.extract_encoded_pipeline_spec``)."""
     if method != "predict_proba":
         raise TypeError(f"CalibratedClassifierCV.{method} is not supported: pass predict_proba")
-    if len(owner.classes_) != 2:
-        raise NotImplementedError(f"CalibratedClassifierCV over {len(owner.classes_)} classes of a kernel machine: only "
-                                  "two classes are supported")
+    nc = len(owner.classes_)
+    if nc > MAX_CLASSES:
+        raise NotImplementedError(f"CalibratedClassifierCV over {nc} classes of a kernel machine: up to {MAX_CLASSES} "
+                                  "classes are supported")
+    if nc > 2:
+        return _calibrated_multiclass_spec(owner, P, bare)
     members = []
     for cc in owner.calibrated_classifiers_:
         if cc.method != "sigmoid":
@@ -549,7 +672,10 @@ def _calibrated_spec(owner, method, P, bare=False):
         if not (_names(_final(cc.estimator)) & _SVM_CLASSIFIERS):
             raise NotImplementedError(f"CalibratedClassifierCV over {type(_final(cc.estimator)).__name__}: the kernel-"
                                       "machine route calibrates SVC and NuSVC only")
-        _svc_binary(cc.estimator, type(_final(cc.estimator)).__name__)
+        n = len(_final(cc.estimator).classes_)
+        if n != 2:
+            raise NotImplementedError(f"{type(_final(cc.estimator)).__name__} over {n} classes in a calibration fold of "
+                                      "two classes: only folds that hold both classes are supported")
         params, V, dual, icpt, colw, colo, _ = _member(_final(cc.estimator) if bare else cc.estimator, P)
         cal = cc.calibrators[0]
         members.append((params, V, dual, icpt, colw, colo, float(cal.a_), float(cal.b_)))
@@ -567,6 +693,47 @@ def _calibrated_spec(owner, method, P, bare=False):
                              cal_a=[m[6] for m in members], cal_b=[m[7] for m in members], pi=np.full(K, 1.0 / K))
 
 
+def _calibrated_multiclass_spec(owner, P, bare):
+    """``_calibrated_spec`` over 3 to ``MAX_CLASSES`` classes: the one-vs-one head's calibrated probabilities."""
+    nc = len(owner.classes_)
+    members = []
+    off = 0
+    for cc in owner.calibrated_classifiers_:
+        if cc.method != "sigmoid":
+            raise NotImplementedError(f"CalibratedClassifierCV(method={cc.method!r}) over a kernel machine: only "
+                                      "method='sigmoid' is supported")
+        clf = _final(cc.estimator)
+        name = type(clf).__name__
+        if not (_names(clf) & _SVM_CLASSIFIERS):
+            raise NotImplementedError(f"CalibratedClassifierCV over {name}: the kernel-machine route calibrates SVC and "
+                                      "NuSVC only")
+        if len(clf.classes_) != nc:
+            raise NotImplementedError(f"CalibratedClassifierCV over {nc} classes with a fold whose {name} saw "
+                                      f"{len(clf.classes_)}: a fold missing classes is not supported (use folds that "
+                                      "hold every class)")
+        if getattr(clf, "decision_function_shape", "ovr") != "ovr":
+            raise NotImplementedError(f"CalibratedClassifierCV over {name}(decision_function_shape="
+                                      f"{clf.decision_function_shape!r}): the calibrated probabilities are read from the "
+                                      "default 'ovr' shape")
+        params, V, dual, icpt, colw, colo, _ = _member(clf if bare else cc.estimator, P)
+        cal_a = [float(c.a_) for c in cc.calibrators]
+        cal_b = [float(c.b_) for c in cc.calibrators]
+        members.append((params, V, dual, icpt, colw, colo, cal_a, cal_b, _class_blocks(clf, off)))
+        off += V.shape[0]
+    if len({m[0][0] for m in members}) != 1 or len({(m[0][2], m[0][3]) for m in members}) != 1:
+        raise NotImplementedError("calibrated members with different kernels, degrees or coef0")
+    K = len(members)
+    if K > MAX_MEMBERS:
+        raise NotImplementedError(f"{K} calibrated members: kernel machines are explained up to {MAX_MEMBERS}")
+    sv_off = np.concatenate([[0], np.cumsum([m[1].shape[0] for m in members])])
+    return MulticlassSvmSpec(np.concatenate([m[1] for m in members]), sv_off, np.stack([m[8] for m in members]),
+                             np.concatenate([m[2] for m in members]), np.stack([m[3] for m in members]),
+                             np.stack([m[4] for m in members]), np.stack([m[5] for m in members]),
+                             [m[0][1] for m in members], members[0][0][0], members[0][0][2], members[0][0][3],
+                             "ovo_proba", P, nc, cal_a=np.stack([m[6] for m in members]),
+                             cal_b=np.stack([m[7] for m in members]), pi=np.full(K, 1.0 / K))
+
+
 def _single_spec(owner, method, P):
     est = _final(owner)
     name = type(est).__name__
@@ -578,7 +745,18 @@ def _single_spec(owner, method, P):
                                       f"{name}(), ensemble=False).predict_proba instead")
         if method != "decision_function":
             raise TypeError(f"{name}.{method} is not supported: pass decision_function (predict returns labels)")
-        _svc_binary(est, name)
+        nc = _svc_classes(est, name)
+        if nc > 2 and est.decision_function_shape != "ovo":
+            raise NotImplementedError(
+                f"{name}.decision_function over {nc} classes with decision_function_shape='ovr': its integer part counts "
+                "one-vs-one votes, a label-like step function the kernel-machine route does not explain; pass "
+                f"{name}(decision_function_shape='ovo') for the pair values, or explain "
+                f"CalibratedClassifierCV({name}(), ensemble=False).predict_proba")
+        if nc > 2:
+            params, V, dual, icpt, colw, colo, _ = _member(owner, P)
+            kernel, gamma, degree, coef0 = params
+            return MulticlassSvmSpec(V, [0, V.shape[0]], _class_blocks(est, 0)[None, :], dual, icpt[None, :],
+                                     colw[None, :], colo[None, :], [gamma], kernel, degree, coef0, "ovo", P, nc)
     elif names & _OCSVM:
         if method not in ("decision_function", "score_samples"):
             raise TypeError(f"{name}.{method} is not supported: pass decision_function or score_samples (predict returns "
@@ -606,8 +784,12 @@ def extract_kernel_machine_spec(predictor):
     ``GaussianProcessRegressor`` ``predict``, ``OneClassSVM`` ``decision_function`` / ``score_samples``,
     ``CalibratedClassifierCV(SVC | NuSVC, method='sigmoid').predict_proba``, each possibly behind a ``Pipeline`` of
     per-column affine scalers -- and ``None`` for anything else (linear SVMs included: the engine then reads a linear
-    model).  A spec passes through.  Raises ``NotImplementedError`` / ``TypeError`` naming the reason for kernel machines
-    the route does not cover: more than two classes, ``SVC(probability=True).predict_proba``, precomputed, callable and
+    model).  Multi-class SVMs give a ``MulticlassSvmSpec`` (the one-vs-one head): ``SVC`` / ``NuSVC(decision_function_shape=
+    'ovo').decision_function`` over 3 or 4 classes (the pair values) and the calibrated ``predict_proba`` over 3 to 8
+    classes.  A spec passes through.  Raises ``NotImplementedError`` / ``TypeError`` naming the reason for kernel machines
+    the route does not cover: the default ``'ovr'`` ``decision_function`` of a multi-class SVM (a vote count), ``'ovo'``
+    with more than 8 pair values, more than 8 classes, a calibration fold that saw fewer classes than the calibrator,
+    ``SVC(probability=True).predict_proba``, precomputed, callable and
     chi2 kernels, kernel objects on SVMs, kernel objects outside the program kernel (``Matern`` nu other than 0.5, 1.5,
     2.5, inf, ``PairwiseKernel``, ``CompoundKernel``, user-defined kernels, more than ``MAX_STATS`` statistics),
     ``GaussianProcessClassifier``, unfitted models, a non-integer or negative polynomial degree, pipeline steps other
@@ -647,6 +829,11 @@ def extract_kernel_machine_spec(predictor):
 
 def _fold_outer(spec, a, b):
     """The spec of the model behind one more affine map x' = a x + b of its raw columns."""
+    if isinstance(spec, MulticlassSvmSpec):
+        return MulticlassSvmSpec((spec.sv - b) / a, spec.sv_off, spec.cls_off, spec.dual, spec.intercept,
+                                 spec.colw * a * a, (spec.colo - b) / a, spec.gamma, spec.kernel, spec.degree, spec.coef0,
+                                 spec.head, spec.n_features, spec.classes, cal_a=spec.cal_a, cal_b=spec.cal_b,
+                                 pi=spec.pi, scalar_out=spec.scalar_out)
     program = spec.program.folded(a, b) if spec.program is not None else None
     if spec.kernel == "laplacian":
         colw = spec.colw * np.abs(a)

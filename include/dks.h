@@ -126,8 +126,14 @@ extern "C" {
 #define DKS_KM_HEAD_IDENTITY 0    /* one member, R outputs f (SVC / NuSVC decision_function, SVR, NuSVR, KernelRidge) */
 #define DKS_KM_HEAD_CALIBRATED 1  /* R = 1, outputs [1 - p1, p1], p1 = sum_k pi_k expit(-(a_k f_k + b_k)): sigmoid
                                    * CalibratedClassifierCV over a binary SVC / NuSVC */
+#define DKS_KM_HEAD_OVO 2         /* multi-class SVC / NuSVC (dks_set_svc_multiclass): one-vs-one pair scores per member */
 #define DKS_KM_MAX_R 8            /* outputs of the identity head */
 #define DKS_KM_MAX_K 16           /* members of the calibrated head */
+/* output mode of the one-vs-one head (dks_set_svc_multiclass) */
+#define DKS_KM_OVO_DECISION 0     /* P = K (K - 1) / 2 pair values dec_k (decision_function_shape='ovo'), one member */
+#define DKS_KM_OVO_PROBA 1        /* K probabilities: per member the ovr-vote decision function, sigmoid-calibrated per
+                                   * class and normalised; members averaged with weights pi (CalibratedClassifierCV) */
+#define DKS_KM_OVO_MAX_CLASSES 8  /* classes of the one-vs-one head (28 pairs) */
 #define DKS_ACT_MLP 8          /* multi-layer perceptron: set by dks_set_mlp only (dks_set_model refuses it) */
 
 /* hidden activation of a multi-layer perceptron (dks_set_mlp), scikit-learn's ACTIVATIONS */
@@ -271,6 +277,27 @@ int dks_set_kernel_machine(dks_ctx* ctx, int K, const int32_t* sv_off, const dou
  * other kernels use for 32: one masked row costs L ceil(M / 4) table reads and one expression per support vector. */
 int dks_set_kernel_program(dks_ctx* ctx, int L, const int32_t* kinds, const double* colw, const double* colo, int n_ops,
                            const int32_t* ops, const int32_t* args, const double* a, const double* b);
+/* multi-class SVC / NuSVC (DKS_ACT_KMACH, head DKS_KM_HEAD_OVO, DESIGN.md §5.0.22) in place of dks_set_model: K members
+ * (1..DKS_KM_MAX_K calibration folds, or one SVM) over `classes` (3..DKS_KM_OVO_MAX_CLASSES) classes.  Member m owns support
+ * vectors sv_off[m] .. sv_off[m + 1] (sv_off [K + 1], non-decreasing from 0, n_sv = sv_off[K] >= 1), stored in class blocks:
+ * class c of member m owns cls_off[m (classes + 1) + c] .. cls_off[m (classes + 1) + c + 1] (absolute rows, from sv_off[m]
+ * to sv_off[m + 1], non-decreasing; a class may own none).  sv [n_sv][D] in raw feature space, dual [n_sv][classes - 1]
+ * (scikit-learn's dual_coef_ transposed), intercept [K][P] with P = classes (classes - 1) / 2; colw [K][D] (> 0), colo [K][D],
+ * gamma [K] (>= 0), kernel DKS_KM_KERNEL_RBF / _POLY / _SIGMOID, degree and coef0 as for dks_set_kernel_machine.  Pair
+ * k = (i, j), i < j, in the order i, then j:
+ *   dec_k = sum_{v in class i} dual[v][j - 1] K(x, v) + sum_{v in class j} dual[v][i] K(x, v) + intercept[m][k].
+ * mode DKS_KM_OVO_DECISION: one member, P <= 8 outputs dec (decision_function_shape='ovo').  mode DKS_KM_OVO_PROBA:
+ * `classes` outputs sum_m pi_m p_m (pi > 0, normalised to sum 1), p_m,c = e_c / sum e, e_c = expit(-(a f_c + b)) with
+ * a = cal_a[m][c], b = cal_b[m][c] [K][classes] and f the ovr-vote decision function votes_c + conf_c / (3 (|conf_c| + 1))
+ * (dec_k >= 0 votes for i, else for j; conf_i += dec_k, conf_j -= dec_k); a zero sum gives 1 / classes, and values in
+ * (1, 1 + 1e-5] become 1.  The device sums support vectors in its own fixed order, so a dec_k within rounding of 0 may vote
+ * otherwise than libsvm.  Non-finite values, bad offsets, unknown kernel or mode codes and out-of-range counts are
+ * DKS_ERR_UNSUPPORTED.  Everything else -- plans, groups, l1, NaN refusals, column encodings, ensembles -- is as for
+ * dks_set_kernel_machine; shapes whose per-instance buffers do not fit shared memory are DKS_ERR_UNSUPPORTED. */
+int dks_set_svc_multiclass(dks_ctx* ctx, int K, int classes, const int32_t* sv_off, const int32_t* cls_off, const double* sv,
+                           const double* dual, const double* intercept, const double* colw, const double* colo,
+                           const double* gamma, int kernel, double degree, double coef0, int mode, const double* cal_a,
+                           const double* cal_b, const double* pi, int scalar_out);
 /* multi-layer perceptron (DKS_ACT_MLP) in place of dks_set_model: n_hidden (1..DKS_MLP_MAX_HIDDEN) hidden layers.
  * widths [n_hidden + 2] = {D, H_1 .. H_n_hidden, R}: hidden widths 1..DKS_MLP_MAX_WIDTH, R outputs 1..DKS_MLP_MAX_OUT.
  * W_host: the layers' weights concatenated, layer l [widths[l]][widths[l + 1]] row-major (scikit-learn's coefs_[l]; layer 0
