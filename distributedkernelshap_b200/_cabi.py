@@ -36,6 +36,7 @@ ACT_KNN = 9
 ACT_ENSEMBLE = 10
 ACT_EXTERNAL = 11
 ACT_STACKING = 12
+ACT_GAUSS = 13
 EXTERNAL_FLOAT32 = 0
 EXTERNAL_FLOAT64 = 1
 LINK_IDENTITY = 0
@@ -70,6 +71,7 @@ SIGNATURES = {
     "dks_set_mlp": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]),
     "dks_set_knn_model": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int, C.c_double, C.c_int,
                                                                              C.c_int, C.c_void_p, C.c_int, C.c_int]),
+    "dks_set_gaussian_model": (C.c_int, [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int]),
     "dks_set_ensemble": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "dks_set_stacking": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                    C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64]),

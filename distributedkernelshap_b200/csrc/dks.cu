@@ -22,6 +22,7 @@
 #include "dks_kmach.cuh"
 #include "dks_mlp.cuh"
 #include "dks_knn.cuh"
+#include "dks_gauss.cuh"
 #include "dks_ensemble.cuh"
 #include "dks_external.cuh"
 #include "dks_stacking.cuh"
@@ -195,6 +196,10 @@ HeadDesc describe_head(const dks_ctx* ctx) {
         // probabilities are not exact negations of each other in float64)
         h.family = DKS_GENERAL_KNN;
         break;
+    case DKS_ACT_GAUSS:
+        // no shared-plan route: every instance runs the Gaussian kernel; every output is solved on its own
+        h.family = DKS_GENERAL_GAUSS;
+        break;
     case DKS_ACT_ENSEMBLE:
         // no shared-plan route: every instance runs the members' kernels and the ensemble's tail; every output is solved on
         // its own
@@ -284,6 +289,10 @@ OwnKernel own_kernel(int family) {
                 " (their scalers fold into the column weights and origins)", REFUSES_NONFINITE,
                 [](const dks_ctx* c, int S_cap) {
                     return dks::knn::smem_bytes(S_cap, c->C, c->G, c->knn.k, knn_chunk(c, S_cap)); }};
+    case DKS_GENERAL_GAUSS:
+        return {"Gaussian models", "Gaussian kernel", "components", "Gaussian model",
+                " (their scalers fold into the means and projections)", REFUSES_NONFINITE,
+                [](const dks_ctx* c, int S_cap) { return dks::gauss::smem_bytes(S_cap, c->C, c->G, c->gauss.K); }};
     case DKS_GENERAL_ENSEMBLE:          // refuses: what its members refuse (refusing_kernel)
         return {"soft-voting ensembles", "ensemble kernels", "groups", "soft-voting ensemble",
                 " (put the preprocessing in front of the ensemble)", REFUSES_NONE, ensemble_smem};
@@ -382,6 +391,7 @@ int check_own_columns(const dks_ctx* ctx, const OwnKernel& ok) {
         reads = (int)(ctx->h_kcolw.size() / ctx->km.K);
         break;
     case DKS_GENERAL_MLP: reads = ctx->mlp.width[0]; break;
+    case DKS_GENERAL_GAUSS: reads = (int)(ctx->h_gmu.size() / ctx->gauss.K); break;
     case DKS_GENERAL_ENSEMBLE: return DKS_OK;         // each member checks its own (fit_members)
     case DKS_GENERAL_STACKING:                        // each member checks its own; the passthrough reads every column
         if (!ctx->h_stk_Wp.empty() && ctx->h_stk_Wp.size() != (size_t)ctx->stk.R * width)
@@ -489,6 +499,21 @@ int own_fit_tables(dks_ctx* ctx, const double* bg, int width) {
                                                                                                      Tbg, Ebg);
         break;
     }
+    case DKS_GENERAL_GAUSS: {
+        GaussDev& g = ctx->gauss;
+        const bool enc = ctx->enc.E > 0;
+        CUDA_TRY(pool.upload(&g.mu, ctx->h_gmu.data(), ctx->h_gmu.size(), st));
+        CUDA_TRY(pool.upload(&g.L, ctx->h_gL.data(), ctx->h_gL.size(), st));
+        double *Abg, *alpha, *Pbg;
+        CUDA_TRY(pool.alloc(&Abg, (size_t)N * g.RT));
+        CUDA_TRY(pool.alloc(&alpha, (size_t)N * g.K));
+        CUDA_TRY(pool.alloc(&Pbg, (size_t)N * ctx->G * g.RT));
+        g.Abg = Abg; g.alpha = alpha; g.Pbg = Pbg;
+        dks::gauss::gauss_fit_tables_kernel<<<cdiv((long long)N * g.K, 128), 128, 0, st>>>(
+            bg, N, width, ctx->G, enc ? ctx->d_egoff : ctx->d_goff.get(), enc ? ctx->d_egcols : ctx->d_gcols.get(), g, Abg,
+            alpha, Pbg);
+        break;
+    }
     }
     ctx->launches += 1;
     return DKS_OK;
@@ -540,6 +565,10 @@ int launch_own_predict(dks_ctx* ctx, const double* X, int n, double* Xenc, const
     case DKS_GENERAL_KNN:
         dks::knn::knn_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->knn, C, link, linkfnull, out, dlink,
                                                                    ctx->d_status);
+        break;
+    case DKS_GENERAL_GAUSS:
+        dks::gauss::gauss_predict_kernel<<<cdiv(n, 128), 128, 0, st>>>(X, n, D, ctx->gauss, C, link, linkfnull, out, dlink,
+                                                                       ctx->d_status);
         break;
     case DKS_GENERAL_ENSEMBLE: {    // every member's f_k(x) into d_ens_out [K][n][C], then f(x) = sum_k pi_k f_k(x)
         const int K = (int)ctx->ens.size();
@@ -652,6 +681,15 @@ int launch_own_kernel(dks_ctx* ctx, bool l1, const ExplainParams& p, size_t smem
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, dks::knn::THREADS, smem, st>>>(p, q, ctx->knn, knn_chunk(ctx, p.S_cap), ctx->own_X, ctx->own_bg,
                                                     ctx->own_D, ctx->own_goff, ctx->own_gcols, ea, er);
+        break;
+    }
+    case DKS_GENERAL_GAUSS: {       // never an ensemble member (check_members)
+        TRY(grow(ctx, ctx->gxp, (size_t)grid * ctx->G * ctx->gauss.RT));
+        ctx->gauss.xp = ctx->gxp;
+        auto kern = l1 ? dks::gauss::explain_gauss_kernel<true> : dks::gauss::explain_gauss_kernel<false>;
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, dks::gauss::THREADS, smem, st>>>(p, q, ctx->gauss, ctx->own_X, ctx->own_D, ctx->own_goff,
+                                                      ctx->own_gcols);
         break;
     }
     case DKS_GENERAL_ENSEMBLE: {
@@ -2608,6 +2646,40 @@ int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double*
     ctx->h_ncolo.assign(colo, colo + D);
     ctx->h_ny.assign(labels_or_targets, labels_or_targets + ny);
     return set_own_model(ctx, DKS_ACT_KNN, R, scalar_out);
+}
+
+int dks_set_gaussian_model(dks_ctx* ctx, int K, int D, const int32_t* r_off, const double* mu, const double* L,
+                           const double* gamma, const double* c, int head, int scalar_out) {
+    BIND(ctx);
+    REQUIRE(ctx->D > 0, "dks_set_gaussian_model: call dks_set_background first (D unknown)");
+    REQUIRE(r_off && mu && L && gamma && c, "dks_set_gaussian_model: need r_off, mu, L, gamma and c");
+    if (K < 1 || K > DKS_GAUSS_MAX_K)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: K=%d components; 1..%d supported", K, DKS_GAUSS_MAX_K);
+    if (D < 1) return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: D=%d columns", D);
+    if (head < DKS_GAUSS_HEAD_SOFTMAX || head > DKS_GAUSS_HEAD_DIFF)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: unknown head %d", head);
+    if (head == DKS_GAUSS_HEAD_DIFF && K != 2)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: the difference head needs K = 2 (K=%d)", K);
+    if (r_off[0] != 0)
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: r_off must start at 0");
+    for (int k = 0; k < K; ++k)
+        if (r_off[k + 1] <= r_off[k])
+            return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: component %d has rank %d (at least 1)", k,
+                        r_off[k + 1] - r_off[k]);
+    const int RT = r_off[K];
+    if (!all_finite(mu, (size_t)K * D) || !all_finite(L, (size_t)RT * D) || !all_finite(gamma, K) || !all_finite(c, K))
+        return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: the arrays must be finite");
+    for (int k = 0; k < K; ++k)
+        if (!(gamma[k] > 0)) return fail(DKS_ERR_UNSUPPORTED, "dks_set_gaussian_model: gamma of component %d is not positive", k);
+    GaussDev& g = ctx->gauss;
+    g = GaussDev{};
+    g.K = K; g.RT = RT; g.head = head;
+    for (int k = 0; k <= K; ++k) g.r_off[k] = r_off[k];
+    for (int k = 0; k < K; ++k) { g.gamma[k] = gamma[k]; g.c[k] = c[k]; }
+    ctx->h_gmu.assign(mu, mu + (size_t)K * D);
+    ctx->h_gL.assign(L, L + (size_t)RT * D);
+    const int C = head == DKS_GAUSS_HEAD_SOFTMAX || head == DKS_GAUSS_HEAD_IDENTITY ? K : 1;
+    return set_own_model(ctx, DKS_ACT_GAUSS, C, scalar_out);
 }
 
 int dks_set_ensemble(dks_ctx* ctx, int K, dks_ctx* const* members, const double* weights, int C, int scalar_out) {

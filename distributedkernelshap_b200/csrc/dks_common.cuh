@@ -328,6 +328,20 @@ struct KnnDev {
     int n_fit, k, metric, weights, R, head;
 };
 
+// Gaussian generative models (dks_set_gaussian_model, DESIGN.md §5.0.23): l_k = c_k - gamma_k ||L_k^T (x - mu_k)||^2 for
+// K components, then the head DKS_GAUSS_HEAD_*.  RT = r_off[K] projection rows over all components.
+struct GaussDev {
+    const double* mu;            // [K][D]
+    const double* L;             // [RT][D]: row r_off[k] + t is column t of L_k
+    const double* Abg;           // [N][RT] fit: L_k^T (bg_j - mu_k)
+    const double* alpha;         // [N][K] fit: ||L_k^T (bg_j - mu_k)||^2
+    const double* Pbg;           // [N][G][RT] fit: L_k^T bg_j|_g
+    double* xp;                  // [CTAs][G][RT] explain kernel scratch: L_k^T x|_g of the CTA's instance
+    int r_off[DKS_GAUSS_MAX_K + 1];
+    double gamma[DKS_GAUSS_MAX_K], c[DKS_GAUSS_MAX_K];
+    int K, RT, head;
+};
+
 // exp head, CUDA-core kernels (DESIGN.md §5.0.8): a coalition row is summed in fp32 when the largest weighted background
 // exponent t'_j = log2 e d(s, j) + log2 w_j lies in [EXP_T_LO, EXP_T_HI]; other rows are evaluated in float64
 #define DKS_EXP_T_LO -60.f
@@ -462,6 +476,11 @@ struct dks_ctx {
     // k-nearest neighbours (act == DKS_ACT_KNN): host copies of the arrays, and their device copies built by dks_fit
     std::vector<double> h_nfitX, h_ncolw, h_ncolo, h_ny;
     KnnDev knn = {};
+    // Gaussian model (act == DKS_ACT_GAUSS): host copies of the arrays, their device copies built by dks_fit, and the
+    // explain kernel's per-CTA scratch gauss.xp points at
+    std::vector<double> h_gmu, h_gL;
+    GaussDev gauss = {};
+    DevBuf<double> gxp;
     // soft-voting ensemble (act == DKS_ACT_ENSEMBLE): the member contexts it owns, pi, its device copy (built by dks_fit), the
     // members' predictions of a call [K][n][C] and their weighted background means [n][C][S_cap]; a member points at its
     // ensemble, shares its stream and status word, and refuses every call of the C ABI

@@ -15,6 +15,8 @@ import numpy as np
 from . import _cabi
 from .data import DenseData, convert_to_data, convert_to_link
 from .ensembles import MAX_GROUPS as ENSEMBLE_MAX_GROUPS, EnsembleSpec, extract_ensemble_spec
+from .gaussian_models import (MAX_GROUPS as GAUSS_MAX_GROUPS, GaussianModelSpec, extract_gaussian_spec,
+                              refuse_gaussian_members)
 from .plan import build_plan, l1_tables, pack_dense_plan, projection, resolve_nsamples, sampling_info
 from .kernel_machines import (MAX_GROUPS as KMACH_MAX_GROUPS, KernelMachineSpec, MulticlassSvmSpec,
                               extract_kernel_machine_spec)
@@ -196,6 +198,7 @@ class GpuKernelExplainer:
         self.link = convert_to_link(link)
         self.model_callable = model
         torch_models.refuse_module_in_pipeline(model)
+        refuse_gaussian_members(model)
         linear_target = model
         if torch_models.is_torch_module(model):
             # a module: recognised and checked here, run on the background below
@@ -228,7 +231,8 @@ class GpuKernelExplainer:
                     (extract_tree_spec, TREE_MAX_GROUPS, "tree ensembles"),
                     (extract_kernel_machine_spec, KMACH_MAX_GROUPS, "kernel machines"),
                     (extract_mlp_spec, MLP_MAX_GROUPS, "MLPs"),
-                    (extract_knn_spec, KNN_MAX_GROUPS, "nearest-neighbour models"))
+                    (extract_knn_spec, KNN_MAX_GROUPS, "nearest-neighbour models"),
+                    (extract_gaussian_spec, GAUSS_MAX_GROUPS, "Gaussian models"))
         for extract, max_groups, family in families:
             own = extract(target)
             if own is not None:
@@ -237,6 +241,9 @@ class GpuKernelExplainer:
         if (self.spec.activation == "exp" or getattr(self.spec, "head", None) == "exp") and str(self.link) == "logit":
             raise NotImplementedError("the exp head (log-link GLM regressors) supports link='identity' only: the logit "
                                       "link log(ey / (1 - ey)) is undefined wherever a predicted mean exceeds 1")
+        if isinstance(self.spec, GaussianModelSpec) and self.spec.head != "softmax" and str(self.link) == "logit":
+            raise NotImplementedError("log densities, decision functions and Mahalanobis scores of Gaussian models are not "
+                                      "probabilities: they support link='identity' only (predict_proba takes 'logit')")
         if getattr(self.spec, "head", None) == "iforest" and str(self.link) == "logit":
             raise NotImplementedError("the anomaly head (IsolationForest) supports link='identity' only: its scores are "
                                       "negative and not probabilities, so they have no logit")
@@ -349,7 +356,12 @@ class GpuKernelExplainer:
 
     def _set_own_model(self, ctx, own):
         """The family setter of the C ABI for a tree, kernel-machine, MLP or neighbour spec."""
-        if isinstance(own, KnnSpec):
+        if isinstance(own, GaussianModelSpec):
+            r_off, L = own.flat()
+            _cabi.check(self.lib.dks_set_gaussian_model(
+                ctx, own.K, own.mu.shape[1], _cabi.ptr(r_off), _cabi.ptr(own.mu), _cabi.ptr(L), _cabi.ptr(own.gamma),
+                _cabi.ptr(own.c), own.head_code, int(own.scalar_out)))
+        elif isinstance(own, KnnSpec):
             k = own
             _cabi.check(self.lib.dks_set_knn_model(
                 ctx, k.n_fit, _cabi.ptr(k.fitX), _cabi.ptr(k.colw), _cabi.ptr(k.colo), k.k, k.metric_code, k.p,
@@ -957,7 +969,8 @@ class GpuKernelExplainer:
     _PATH_NAMES = {
         "shared": ("none", "fused", "smem", None, "softmax", "affine", "ovr", "exp", "mixture"),   # 3: not used
         "solve": ("none", "fused", "pmat", "wls_shared", "wide", "l1"),
-        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble", "torch", "stacking"),
+        "general": ("none", "tc", "simt", "flagged", "simt_wide", "trees", "kmach", "mlp", "knn", "ensemble", "torch",
+                    "stacking", "gauss"),
     }
 
     def last_path(self):
@@ -974,7 +987,8 @@ class GpuKernelExplainer:
         members' kernels and the ensemble's tail, which take every instance of a soft-voting ensemble, or 'torch': the
         ensemble's tail on the background means of a module's outputs, every instance of a module, or 'stacking': per
         background chunk the members' kernels and the final estimator's reduction, then the ensemble's tail, every
-        instance of a stacking ensemble),
+        instance of a stacking ensemble, or 'gauss': the Gaussian kernel, which takes every instance of a Gaussian
+        generative model),
         ``cta_warps`` (warps per CTA the fused kernel runs: ``warps``
         row-group slices at one warp each, or fewer slices shared by several warps each) and ``bg_weights`` ('uniform' |
         'weighted': which instantiation of the shared-plan kernels ran; background weights that are not all equal take

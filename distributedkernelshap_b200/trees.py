@@ -441,6 +441,7 @@ def extract_encoded_pipeline_spec(predictor):
     from .kernel_machines import _calibrated_spec, _final, _is_kernel_machine, extract_kernel_machine_spec
     from .mlp import _MLPS, extract_mlp_spec
     from .neighbors import _KNN, extract_knn_spec
+    from .gaussian_models import _GAUSSIAN, extract_gaussian_spec
     owner = getattr(predictor, "__self__", None)
     method = getattr(predictor, "__name__", None)
     if owner is None:
@@ -468,6 +469,8 @@ def extract_encoded_pipeline_spec(predictor):
         family, extract = "an MLP", extract_mlp_spec
     elif names & _KNN:
         family, extract = "a neighbour model", extract_knn_spec
+    elif names & _GAUSSIAN:
+        family, extract = "a Gaussian model", extract_gaussian_spec
     else:
         return None
     if all(_foldable(s) for s in pre):

@@ -177,6 +177,13 @@ extern "C" {
 #define DKS_STACK_HEAD_IDENTITY 0    /* outputs r (C = R): decision_function, a linear regressor's predict */
 #define DKS_STACK_HEAD_SIGMOID 1     /* R = 1, outputs [1 - expit(r), expit(r)] (C = 2): binary logistic predict_proba */
 #define DKS_STACK_HEAD_SOFTMAX 2     /* R = C >= 2, outputs softmax(r): multinomial logistic predict_proba */
+#define DKS_ACT_GAUSS 13       /* Gaussian generative model: set by dks_set_gaussian_model only */
+/* head of a Gaussian generative model over its K component scores l_k (dks_set_gaussian_model) */
+#define DKS_GAUSS_HEAD_SOFTMAX 0     /* K outputs softmax(l): QDA, GaussianNB, Gaussian mixtures predict_proba */
+#define DKS_GAUSS_HEAD_LOGSUMEXP 1   /* one output log sum_k exp(l_k): Gaussian mixtures score_samples */
+#define DKS_GAUSS_HEAD_IDENTITY 2    /* K outputs l: multi-class QDA decision_function, EllipticEnvelope (K = 1) */
+#define DKS_GAUSS_HEAD_DIFF 3        /* K = 2, one output l_1 - l_0: binary QDA decision_function */
+#define DKS_GAUSS_MAX_K 8            /* components or classes */
 
 /* link (shap.common.convert_to_link; reference call sites kernel_shap.py:775, :949) */
 #define DKS_LINK_IDENTITY 0
@@ -332,6 +339,22 @@ int dks_set_mlp(dks_ctx* ctx, int n_hidden, const int32_t* widths, const double*
  * encoded columns. */
 int dks_set_knn_model(dks_ctx* ctx, int n_fit, const double* fitX, const double* colw, const double* colo, int k, int metric,
                       double p, int weights, int R, const double* labels_or_targets, int head, int scalar_out);
+/* Gaussian generative model (DKS_ACT_GAUSS) in place of dks_set_model: K (1..DKS_GAUSS_MAX_K) component scores
+ *   l_k(x) = c_k - gamma_k ||L_k^T (x - mu_k)||^2
+ * over D columns (the model's width: the E encoded columns behind a column encoding), then the head DKS_GAUSS_HEAD_*.
+ * mu [K][D]; L_k is D x r_k (r_k >= 1), its columns stored as rows: row r_off[k] + t of L [r_off[K]][D] is column t of L_k
+ * (r_off [K + 1] increasing from 0); gamma [K] positive, c [K]; everything finite.  QDA, GaussianNB, GaussianMixture,
+ * BayesianGaussianMixture and EllipticEnvelope read this way (DESIGN.md §5.0.23), per-column scalers folded into mu and L.
+ * Malformed input is DKS_ERR_UNSUPPORTED.
+ * Every instance runs the Gaussian kernel (DKS_GENERAL_GAUSS), up to 64 groups: shared plans (full and partial varying
+ * sets), per-instance device plans and caller-supplied plans, kernel 'auto' or 'simt' (tcgen05 / shared are
+ * DKS_ERR_UNSUPPORTED), l1 selection through the general list's LARS route; every output is solved on its own.  Float64
+ * throughout.  NaN or an infinity in a background row (dks_fit) or an instance (dks_predict_host, the explain calls) is
+ * DKS_ERR_DOMAIN with the row; a link(ey) or link(f(x)) that is not finite is DKS_ERR_NUMERIC and nothing non-finite is
+ * written into phi.  The explain kernel holds K (G^2 + 1) doubles of tables in shared memory: shapes that do not fit are
+ * DKS_ERR_UNSUPPORTED.  dks_set_column_maps is refused; a Gaussian model is not an ensemble member. */
+int dks_set_gaussian_model(dks_ctx* ctx, int K, int D, const int32_t* r_off, const double* mu, const double* L,
+                           const double* gamma, const double* c, int head, int scalar_out);
 /* soft-voting ensemble (DKS_ACT_ENSEMBLE) in place of dks_set_model: outputs f = sum_k pi_k f_k over K (1..DKS_ENS_MAX_MEMBERS)
  * members, pi = weights / sum(weights) (finite, >= 0, positive sum), members in order.  members [K] are distinct contexts on
  * the same device, each made by dks_create and one dks_set_tree_model / dks_set_kernel_machine / dks_set_mlp /
@@ -628,6 +651,7 @@ int dks_fused_table_info(dks_ctx* ctx, int M, int64_t* table_bytes, int64_t* fal
                                   * module the caller runs (dks_set_external_model) */
 #define DKS_GENERAL_STACKING 11  /* per background chunk the members' explain kernels and stacking_reduce_kernel, then
                                   * explain_ensemble_tail_kernel: every instance of a stacking ensemble (dks_set_stacking) */
+#define DKS_GENERAL_GAUSS 12     /* explain_gauss_kernel: every instance of a Gaussian model (dks_set_gaussian_model) */
 int dks_last_path(dks_ctx* ctx, int32_t* out, int n);
 /* device-time of the last explain's stages in ms (CUDA events on the ctx stream): [0] prepare, [1] fused
  * coalition kernel, [2] total; synchronises. */
